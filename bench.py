@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the one hot path: FullSubNet+ / FullSubNet inference on synthetic 16 kHz clips.
 
-    python bench.py --gpus N --steps K --warmup W [--config 2|4|5]     # product arm (sm_100a kernels behind the C ABI)
+    python bench.py --gpus N --steps K --warmup W [--config 2|4|5] [--dump-outputs DIR]   # product arm (sm_90a kernels behind the C ABI)
     python bench.py --impl reference --gpus N --steps K ... [--config] # reference arm: the reference's own CPU PyTorch path
 
 Metric (BASELINE.json): frames/sec and real-time factor.  Workloads (BASELINE.json configs, 1-based like BASELINE.md):
@@ -18,9 +18,13 @@ Configs 2 / 5, what one "step" is (identical at every N, so the driver's scaling
   e2e       the same loop with HOST buffers: pinned host spectra -> H2D (copy stream) -> ... -> D2H of this rank's enhanced
             waveforms into pinned host memory, every step.
   extras    forward_only (plain fsn_model_forward loop, the round-1 `value`), e2e_cabi (fsn_model_forward_host_async loop: mask to
-            host, the round-1 `e2e`), cudnn_baseline (the reference model on the same B200 through stock PyTorch / cuDNN),
+            host, the round-1 `e2e`), cudnn_baseline (the reference model on the same GPU through stock PyTorch / cuDNN),
             cpu_baseline (+ .concurrent: as many B=1 workers as the host has cores for).
 Prints ONE JSON line on rank 0.
+
+--dump-outputs DIR (rank 0) writes what the timed path returned in its last timed step, so that two builds can be compared output for
+output on identical inputs (seeded clips, seeded weights): configs 2 / 5 `enhanced.npy` = the enhanced waveforms of the last batch of
+`value` [B, samples] float32; config 4 `mask.npy` = the mask frame returned by the last timed step [B, 2, F] float32.
 """
 import argparse
 import json
@@ -145,7 +149,7 @@ class ClockSampler:
 # ------------------------------------------------------------------------------------------------------------------
 def make_cpu_model(params, w):
     """Returns (callable forward(mag, real, imag) for ONE clip, kind).  kind = "reference": the unmodified reference class from
-    oracle/_ref (or /root/reference); "port": oracle/torch_port.py (same ATen op sequence) when the reference is absent or the
+    oracle/_ref (or FSN_REFERENCE_SRC); "port": oracle/torch_port.py (same ATen op sequence) when the reference is absent or the
     workload uses the additive num_layers knob the reference constructor does not have."""
     from oracle import ref_loader
     if ref_loader.available() and w["L"] == 2:
@@ -293,6 +297,19 @@ def reference_arm(args, w, state):
     print(json.dumps(line))
 
 
+def write_outputs(d, **arrays):
+    """--dump-outputs: each array as d/<name>.npy in float32 (64 MB in all at most: the workloads' outputs are 12 MB and less)."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    total = 0
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        total += a.nbytes
+        if total > 64 << 20:
+            raise SystemExit(f"--dump-outputs: {name} would exceed 64 MB")
+        np.save(os.path.join(d, name + ".npy"), a)
+
+
 # ------------------------------------------------------------------------------------------------------------------
 # product arm, configs 2 / 5
 # ------------------------------------------------------------------------------------------------------------------
@@ -353,12 +370,17 @@ def product_batched(args, w, model, state, rank, local_rank, world, make_model):
     lstm_impl = model.last_lstm_impl()
 
     # ---- value: pipelined enhancement, inputs resident in HBM, collective inside the timed region -------------------------
-    pipe = inf.EnhancePipeline(model, w["nsamp"], *stft_args, gather=True, to_host=False, keep_results=False)
+    dump = bool(args.dump_outputs) and rank == 0
+    pipe = inf.EnhancePipeline(model, w["nsamp"], *stft_args, gather=True, to_host=False, keep_results=dump)
+    flushed = []                                          # what the last flush returned: the results of the timed steps (with --dump-outputs)
     sampler = ClockSampler(local_rank) if rank == 0 else None
     if sampler:
         sampler.start()
         time.sleep(0.3)
-    ms_step, t0, t1 = timed(lambda i: pipe.push(Xs[i % NSETS]), K, max(W, pipe.NSLOT + 1), drain=pipe.flush)   # warm-up fills every ring slot (allocations)
+    ms_step, t0, t1 = timed(lambda i: pipe.push(Xs[i % NSETS]), K, max(W, pipe.NSLOT + 1), drain=lambda: flushed.append(pipe.flush()))   # warm-up fills every ring slot (allocations)
+    if dump:
+        write_outputs(args.dump_outputs, enhanced=flushed[-1][-1])
+    del flushed
     host_ms = timed.host_ms
     clocks = sampler.stop(t0, t1) if sampler else None
     lstm_ms = [x for x in model.lstm_ms_history(min(K, 32)) if x > 0]
@@ -376,8 +398,8 @@ def product_batched(args, w, model, state, rank, local_rank, world, make_model):
         k2 = [x for x in m2.lstm_ms_history(min(K, 32)) if x > 0]
         overlap = {"ms_per_step": ms2, "lstm_kernel_ms": statistics.mean(k2) if k2 else None,
                    "timeline_ms": {"columns": ["front_start", "front_end", "lstm_start", "lstm_end"], "last_steps": [[round(x, 3) for x in r] for r in m2.timeline(6)]},
-                   "note": "same loop with the front end of batch i+1 on a second stream / workspace lane while the LSTM of batch i runs on its 130 SMs: the front "
-                           "end lies inside the LSTM interval, and the LSTM kernel slows down by about the front end's stand-alone time (power-capped) -> off by default"}
+                   "note": "same loop with the front end of batch i+1 on a second stream / workspace lane while the LSTM of batch i runs (off by default: "
+                           "the LSTM occupies every SM, so the step does not get shorter)"}
         del pipe2, m2
 
     # ---- e2e: same loop, pinned host spectra in, this rank's enhanced waveforms out to pinned host memory --------------------
@@ -403,15 +425,12 @@ def product_batched(args, w, model, state, rank, local_rank, world, make_model):
         pk = json.load(open(peaks_path))
         peak, peak_burst, peak_src = pk["bf16_tflops_sustained"], pk["bf16_tflops"], "measured (MEASURED_PEAKS.json, sustained)"
     else:
-        peak, peak_burst, peak_src = 1400.0, 1590.0, "fallback (B200_PROFILING.md)"
-    traffic = None                                    # dram read+write bytes per launch from the committed ncu --set full capture
-    tpath = os.path.join(ROOT, "profiles", "lstm_traffic.json")
-    if os.path.exists(tpath) and lstm_impl == "tcgen05" and B == 64 and w["id"] == 2:
-        traffic = json.load(open(tpath)).get("dram_bytes_per_launch")
+        peak, peak_burst, peak_src = 989.0, 989.0, "H100 SXM data sheet, dense FP16 at 700 W (not measured)"
+    traffic = None
     k_ms = statistics.mean(lstm_ms) if lstm_ms else float("nan")
     k_ms_plain = statistics.mean(lstm_ms_plain) if lstm_ms_plain else float("nan")
     achieved = B * sb_flops / (k_ms * 1e-3) / 1e12
-    roofline = {"bound": "tensor", "kernel": f"sub-band LSTM ({lstm_impl}" + (", layer-wise: all layers incl. input-projection GEMMs" if w["L"] != 2 or cfg["sb_model_hidden_size"] > 384 else "") + ")",
+    roofline = {"bound": "tensor", "kernel": f"sub-band LSTM ({lstm_impl}" + (", layer-wise: all layers incl. input-projection GEMMs" if lstm_impl == "tcgen05" else "") + ")",
                 "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
                 "frac_of_burst_peak": achieved / peak_burst, "peak_source": peak_src,
                 "kernel_ms": k_ms, "kernel_ms_without_overlap": k_ms_plain, "kernel_share_of_step": k_ms / ms_step, "traffic": traffic,
@@ -467,7 +486,9 @@ def product_streaming(args, w, model, state, rank, local_rank, world):
     T = mag.shape[-1]
     frames = [mag[:, :, t].contiguous() for t in range(T)]
     hframes = [f.cpu().pin_memory() for f in frames]
-    K = T if args.steps <= 5 else min(T, args.steps)              # default: the whole 30 s clip
+    K = args.steps
+    if K > T:
+        raise SystemExit(f"--steps {K}: the streaming clip has {T} frames")
 
     def run(host):
         st = StreamingFullSubNet(model, batch_size=B, device=dev)
@@ -495,6 +516,7 @@ def product_streaming(args, w, model, state, rank, local_rank, world):
             lat.append((time.perf_counter() - t0) * 1e3)
         if not host:
             dev_ms = [a.elapsed_time(b) for a, b in evs]
+            run.last = y.clone() if y is not None else None          # what the last timed step returned
         st.close()
         return np.array(lat), np.array(dev_ms)
 
@@ -505,6 +527,8 @@ def product_streaming(args, w, model, state, rank, local_rank, world):
     t0 = time.time()
     lat, dev_ms = run(False)
     t1 = time.time()
+    if args.dump_outputs and rank == 0:
+        write_outputs(args.dump_outputs, mask=run.last)
     clocks = sampler.stop(t0, t1) if sampler else None
     lat_h, _ = run(True)
 
@@ -528,7 +552,7 @@ def product_streaming(args, w, model, state, rank, local_rank, world):
     if rank != 0:
         return None
     peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    hbm = json.load(open(peaks_path))["hbm_gbs"] if os.path.exists(peaks_path) else 6500.0
+    hbm = json.load(open(peaks_path))["hbm_gbs"] if os.path.exists(peaks_path) else 3350.0     # H100 SXM data sheet (not measured)
     # algorithmic bytes per frame: every weight once (sub-band LSTM fp16 images, full-band LSTM fp32 parameters) -- activations are negligible
     c = w["cfg"]
     Hs, Hf, I = c["sb_model_hidden_size"], c["fb_model_hidden_size"], 2 * c["sb_num_neighbors"] + 2
@@ -561,7 +585,7 @@ def product_streaming(args, w, model, state, rank, local_rank, world):
 # secondary baselines (N = 1, rank 0)
 # ------------------------------------------------------------------------------------------------------------------
 def cudnn_baseline(w, state, dev):
-    """The reference model on the SAME B200 through stock PyTorch / cuDNN (SURVEY.md 8d "secondary baseline"): (a) the unmodified
+    """The reference model on the SAME GPU through stock PyTorch / cuDNN (SURVEY.md 8d "secondary baseline"): (a) the unmodified
     reference class, one clip per call, fp32, as its inferencer issues it (inferencer.py:149-151) but with a real synchronize;
     (b) the torch port (same ATen ops, per-sample semantics at any batch size) at the full batch, fp32 and fp16 autocast."""
     import torch
@@ -649,6 +673,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-cudnn-baseline", action="store_true")
     ap.add_argument("--no-overlap-experiment", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
 
     import torch
@@ -671,7 +696,7 @@ def main():
 
     import torch.distributed as dist
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py (impl b200) needs a B200: there is no CPU fallback")
+        raise SystemExit("bench.py (impl b200) needs a CUDA GPU (H100): there is no CPU fallback")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:

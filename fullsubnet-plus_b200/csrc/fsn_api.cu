@@ -57,12 +57,11 @@ struct fsn_model {
     bool finalized = false;
     int Isb = 0;                                      // sub-band LSTM input size
     // packed LSTM weights
-    DevBuf sb_frag[4], sb_bias[4], sb_tc5_stream, sb_tc5_bias;
+    DevBuf sb_frag[4], sb_bias[4];
     DevBuf fb_frag[4], fb_bias[4];
-    bool tc5_ok = false;
-    // layer-wise tcgen05 path (k_lstm_tc5r.cu): per-layer recurrent streams, permuted input-projection matrices, biases
+    // layer-wise wgmma path (k_lstm_tc5r.cu): per-layer recurrent streams, permuted input-projection matrices, biases
     bool tc5r_ok = false;
-    DevBuf r_stream[4], r_wih[4], r_bias[4], r_gin, r_hseq;
+    DevBuf r_stream[4], r_wih[4], r_bias[4], r_gin, r_hseq;    // r_wih: input-projection matrices of the layers > 0
     // Front-end workspaces (everything the full-band stage writes and the sub-band LSTM reads), grow-only, keyed by the last
     // (B, T).  TWO lanes: the pipelined entry points (fsn_model_submit / fsn_model_forward_host_async) run the front end of
     // batch i+1 in lane (i+1)&1 on the front stream while the sub-band LSTM of batch i still reads lane i&1 on the LSTM stream.
@@ -70,23 +69,21 @@ struct fsn_model {
         int wsB = 0, wsT = 0;
         DevBuf fbin, fbout, xa, xb, y1, y2, stats, mu, ximg, magpad, fbx, hseq;
         DevBuf x0, xr;                                 // time-major fb input / relu'd last residual
-        DevBuf fbo;                                    // time-major full-band outputs [(branch, b, t), Cp] (fused-unfold path)
-        bool fbo_valid = false;                        // the last forward of this lane wrote fbo instead of fbout
         DevBuf tsse_scale, sb_rowsum;
         DevBuf xn, sigma;                              // pre-normalised inputs / sub-band std for the non-default norm types
         alignas(64) unsigned char mapX0[128], mapXa[128], mapXb[128], mapXr[128], mapY2[128];
         cudaEvent_t ev_front = nullptr, ev_lstm = nullptr;   // front end written / LSTM finished reading this lane
         bool used = false;                             // ev_lstm has been recorded (a pipelined batch ran / may still run in this lane)
         void release_all() {
-            DevBuf* all[] = {&fbin, &fbout, &xa, &xb, &y1, &y2, &stats, &mu, &ximg, &magpad, &fbx, &hseq, &x0, &xr, &fbo, &tsse_scale, &sb_rowsum, &xn, &sigma};
+            DevBuf* all[] = {&fbin, &fbout, &xa, &xb, &y1, &y2, &stats, &mu, &ximg, &magpad, &fbx, &hseq, &x0, &xr, &tsse_scale, &sb_rowsum, &xn, &sigma};
             for (auto* b : all) b->release();
         }
     } lane[2];
     int last_lane = 0;
     DevBuf cstate, mask_tmp, stage_in[3], stage_out;   // LSTM-side scratch (one LSTM runs at a time), host-entry staging
-    // tcgen05 TCN (FullSubNet+): folded / padded weights, per-block tensor maps, time-major activations
+    // wgmma TCN (FullSubNet+): folded / padded weights, per-block tensor maps, time-major activations
     bool tcn5 = false;
-    int Cp = 0, tcnNT = 0, tcnNtiles = 0, num_sms = 148;
+    int Cp = 0, tcnNT = 0, tcnNtiles = 0, num_sms = 132;
     DevBuf tW1, tW2, tWfc, tS1, tS2b, tBfc;            // [8][3][512][Cp], [8][3][Cp][512], [3][Cp][Cp], [8][3][Cp] x2, [3][Cp]
     DevBuf ws_h, ws_bar;                               // weight-stationary full-band LSTM: h exchange buffer, grid barrier
     alignas(64) unsigned char mapW1[8][128], mapW2[8][128], mapWfc[128];
@@ -95,14 +92,12 @@ struct fsn_model {
     // tuning knobs, read ONCE at fsn_model_create (never on the forward path): FSN_LSTM_IMPL overrides cfg.lstm_impl,
     // FSN_NO_WS=1 keeps the full-band LSTM of fullsubnet.Model off the weight-stationary kernel
     int env_impl = 0;
-    int env_split = 0;                                 // FSN_TC5_SPLIT: force the small-batch column split (1 / 2 / 4; 0 = auto)
     // FSN_FRONT_OVERLAP=1: the pipelined entry points run the front end of batch i+1 concurrently with the sub-band LSTM of batch i
-    // (two lanes, two streams).  Off by default: measured zero-sum on B200 -- the LSTM kernel runs at the board's power cap, and
-    // what the front end gains on the 18 idle SMs the LSTM loses in clock (profiles/r02_front_overlap.txt).
+    // (two lanes, two streams).  Off by default: no gain at the flagship size on the H100 (DESIGN.md §4), the LSTM occupies every SM.
     bool env_front_overlap = false;
     int env_pdl = -1;                                  // FSN_PDL: 0 / 1 / -1 (auto: small batches only)
-    double ws_cap_bytes = 48e9;                        // FSN_WS_CAP_GB: larger batches are run as sub-batches (plain forward entry points)
-    bool env_no_ws = false, env_no_xfuse = false;      // FSN_NO_XFUSE=1: packed sub-band images instead of the fused unfold (A/B only)
+    double ws_cap_bytes = 24e9;                        // FSN_WS_CAP_GB: larger batches are run as sub-batches (plain forward entry points)
+    bool env_no_ws = false;
     // pipelined execution: front-end stream, LSTM stream (higher priority), copy-in / copy-out streams, per-slot events
     cudaStream_t s_front = nullptr, s_lstm = nullptr, s_in = nullptr, s_out = nullptr;
     cudaEvent_t ev_in = nullptr, ev_plain = nullptr;   // caller's inputs ready / last plain forward finished
@@ -280,17 +275,16 @@ static float to_tf32(float x) {
     return y;
 }
 
-// FullSubNet+ TCN weights for the tcgen05 GEMMs (k_gemm_tc5.cu): channel dim padded to Cp (multiple of 32),
+// FullSubNet+ TCN weights for the wgmma GEMMs (k_gemm_tc5.cu): channel dim padded to Cp (multiple of 32),
 // the three branches stacked, gLN2 folded into the second 1x1 convolution:
 //   conv(W2, gLN(y)) = rstd * (W2 diag(gamma2)) y - mean * rstd * s1 + s2,  s1[n] = sum_c W2'[n,c],  s2[n] = sum_c W2[n,c] beta2[c]
 static int pack_tcn5(fsn_model* m) {
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs, Cp = (F + 31) / 32 * 32, Hd = 512;
     m->Cp = Cp;
-    int nt = 1;
-    for (; nt <= 64; ++nt) if (Cp % nt == 0 && (Cp / nt) % 16 == 0 && Cp / nt <= 256) break;
-    if (nt > 64) { m->tcn5 = false; return FSN_OK; }
-    m->tcnNtiles = nt; m->tcnNT = Cp / nt;
+    // N tile of the Cp-wide GEMMs: 64 or 128 columns (the last tile of a branch may overhang; those columns are not stored)
+    m->tcnNT = Cp <= 64 ? 64 : 128;
+    m->tcnNtiles = (Cp + m->tcnNT - 1) / m->tcnNT;
     cudaDeviceProp prop;
     int dev = 0;
     cudaGetDevice(&dev);
@@ -336,7 +330,7 @@ static int pack_tcn5(fsn_model* m) {
         upload(m->tS1, S1.data(), S1.size() * 4) || upload(m->tS2b, S2b.data(), S2b.size() * 4) || upload(m->tBfc, Bfc.data(), Bfc.size() * 4))
         return fail(FSN_ECUDA, "upload of the TCN weights failed");
     for (int blk = 0; blk < 8; ++blk) {
-        if (make_tmap_f32_2d(m->mapW1[blk], static_cast<float*>(m->tW1.p) + (size_t)blk * 3 * Hd * Cp, 3 * Hd, Cp, 256) ||
+        if (make_tmap_f32_2d(m->mapW1[blk], static_cast<float*>(m->tW1.p) + (size_t)blk * 3 * Hd * Cp, 3 * Hd, Cp, 128) ||
             make_tmap_f16_2d(m->mapW2[blk], static_cast<__half*>(m->tW2.p) + (size_t)blk * 3 * Cp * Hd, 3 * Cp, Hd, m->tcnNT))
             return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the TCN weights");
     }
@@ -378,13 +372,10 @@ extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
     m->cfg = c;
     { const char* e = getenv("FSN_LSTM_IMPL"); if (e && *e) m->env_impl = atoi(e); }
     { const char* e = getenv("FSN_NO_WS"); m->env_no_ws = e && atoi(e) != 0; }
-    { const char* e = getenv("FSN_NO_XFUSE"); m->env_no_xfuse = e && atoi(e) != 0; }
-    { const char* e = getenv("FSN_TC5_SPLIT"); if (e && *e) m->env_split = atoi(e); }
     { const char* e = getenv("FSN_FRONT_OVERLAP"); m->env_front_overlap = e && atoi(e) != 0; }
     // FSN_PDL: programmatic dependent launch of the ~30 kernels of the front-end chain.  0 = never, 1 = always, unset = only for small
-    // batches (the column-split regime, where the forward is launch-latency-bound: B = 1 3.21 -> 3.17 ms).  At B = 64 the chain itself gets
-    // 0.05 ms shorter but the pipelined step LOSES 0.1-0.4 ms: the denser front end no longer leaves gaps for the side stream's iSTFT
-    // kernels, which then run under the power-capped LSTM instead (same-box A/B, scripts/gpu_r2_w.sh).
+    // batches, where the forward is launch-latency-bound; for large batches a denser front end leaves no gaps for the side stream's
+    // iSTFT kernels of the pipelined entry points.
     { const char* e = getenv("FSN_PDL"); m->env_pdl = e ? (atoi(e) != 0 ? 1 : 0) : -1; }
     { const char* e = getenv("FSN_WS_CAP_GB"); if (e && atof(e) > 0) m->ws_cap_bytes = atof(e) * 1e9; }
     build_specs(m);
@@ -398,7 +389,7 @@ extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
 extern "C" void fsn_model_destroy(fsn_model* m) {
     if (!m) return;
     cudaDeviceSynchronize();
-    DevBuf* all[] = {&m->arena, &m->sb_tc5_stream, &m->sb_tc5_bias, &m->cstate, &m->mask_tmp, &m->stage_in[0], &m->stage_in[1], &m->stage_in[2],
+    DevBuf* all[] = {&m->arena, &m->cstate, &m->mask_tmp, &m->stage_in[0], &m->stage_in[1], &m->stage_in[2],
                      &m->stage_out, &m->tW1, &m->tW2, &m->tWfc, &m->tS1, &m->tS2b, &m->tBfc, &m->ws_h, &m->ws_bar};
     for (auto* b : all) b->release();
     for (auto& ln : m->lane) {
@@ -467,32 +458,7 @@ extern "C" int fsn_model_finalize(fsn_model* m) {
         const int Ipad = (c.num_freqs + 15) / 16 * 16;
         if (pack_lstm(m, "fb_model", c.num_freqs, Ipad, c.fb_hidden, c.num_layers, m->fb_frag, m->fb_bias)) return fail(FSN_ECUDA, "packing fb_model failed");
     }
-    m->tc5_ok = lstm_tc5_supported(c.num_layers, c.sb_hidden, m->Isb, c.output_size);
-    if (m->tc5_ok) {
-        const int H = c.sb_hidden;
-        const int64_t bytes = fsn_tc5_weight_stream_bytes(m->Isb, H);
-        std::vector<uint16_t> st((size_t)bytes / 2);
-        fsn_tc5_pack_weights(m->Isb, H, m->host["sb_model.sequence_model.weight_ih_l0"].data(),
-                             m->host["sb_model.sequence_model.weight_hh_l0"].data(),
-                             m->host["sb_model.sequence_model.weight_ih_l1"].data(),
-                             m->host["sb_model.sequence_model.weight_hh_l1"].data(), st.data());
-        if (upload(m->sb_tc5_stream, st.data(), (size_t)bytes)) return fail(FSN_ECUDA, "upload of tcgen05 weight stream failed");
-        std::vector<float> bp((size_t)2 * 4 * H);
-        for (int l = 0; l < 2; ++l) {
-            const auto& bi = m->host["sb_model.sequence_model.bias_ih_l" + std::to_string(l)];
-            const auto& bh = m->host["sb_model.sequence_model.bias_hh_l" + std::to_string(l)];
-            for (int j = 0; j < H / 32; ++j)
-                for (int n = 0; n < 128; ++n) {
-                    const int row = fsn_tc5_gate_row(H, j, n);
-                    // stored pre-scaled: the kernel evaluates exp2(-log2e * (acc + b)) as one FMA (tanh gate: -2 log2e)
-                    const int q = (n % 32) / 8;                        // gate position: i,f,g,o / GRU pseudo-gates r,z,n_x,n_h
-                    const float sc = (q == 2 || (q == 3 && c.rnn_type == FSN_RNN_GRU)) ? -2.8853900817779268f : -1.4426950408889634f;
-                    bp[(size_t)l * 4 * H + j * 128 + n] = sc * (bi[row] + bh[row]);
-                }
-        }
-        if (upload(m->sb_tc5_bias, bp.data(), bp.size() * 4)) return fail(FSN_ECUDA, "upload failed");
-    }
-    m->tc5r_ok = !m->tc5_ok && lstm_tc5r_supported(c.sb_hidden, c.output_size) && m->Isb <= 64;
+    m->tc5r_ok = lstm_tc5r_supported(c.sb_hidden, c.output_size) && m->Isb <= 64;
     if (m->tc5r_ok) {
         const int H = c.sb_hidden;
         for (int l = 0; l < c.num_layers; ++l) {
@@ -502,9 +468,15 @@ extern "C" int fsn_model_finalize(fsn_model* m) {
             std::vector<float> bp;
             lstm_tc5r_pack_layer(H, Kin, Kpad, m->host[q + "weight_ih_l" + sl].data(), m->host[q + "weight_hh_l" + sl].data(),
                                  m->host[q + "bias_ih_l" + sl].data(), m->host[q + "bias_hh_l" + sl].data(), c.rnn_type == FSN_RNN_GRU, st, wp, bp);
-            if (upload(m->r_stream[l], st.data(), st.size() * 2) || upload(m->r_wih[l], wp.data(), wp.size() * 2) ||
-                upload(m->r_bias[l], bp.data(), bp.size() * 4))
-                return fail(FSN_ECUDA, "upload of the layer-wise tcgen05 weights failed");
+            if (l == 0) {                                                   // first layer: [W_ih | W_hh] blocks, the input projection is in the recurrence
+                st.assign((size_t)(H / 32) * (1 + H / 64) * 8192, 0);
+                lstm_tc5_pack_first_layer(Kin, H, m->host[q + "weight_ih_l0"].data(), m->host[q + "weight_hh_l0"].data(), st.data());
+            } else {                                                        // deeper layers: W_hh blocks + the input-projection GEMM's matrix
+                lstm_tc5r_gin_order(H, Kpad, wp);
+                if (upload(m->r_wih[l], wp.data(), wp.size() * 2)) return fail(FSN_ECUDA, "upload of the layer-wise LSTM weights failed");
+            }
+            if (upload(m->r_stream[l], st.data(), st.size() * 2) || upload(m->r_bias[l], bp.data(), bp.size() * 4))
+                return fail(FSN_ECUDA, "upload of the layer-wise LSTM weights failed");
         }
     }
     if (c.model_kind == FSN_KIND_PLUS) {
@@ -528,21 +500,15 @@ static void fill_ws(fsn_model* m, LstmWsLaunch& w) {
     w.L = c.num_layers; w.H = c.fb_hidden; w.I = c.num_freqs; w.Ipad = (c.num_freqs + 15) / 16 * 16; w.fast = c.fast_math; w.gru = c.rnn_type == FSN_RNN_GRU;
 }
 
-// lstm_impl = auto: fused two-layer tcgen05 kernel when the geometry fits, else the layer-wise tcgen05 path (k_lstm_tc5r.cu), else
-// the generic mma.sync kernel; lstm_impl = mma forces the generic kernel.
+// lstm_impl = auto: the layer-wise wgmma path (input-projection GEMM + recurrent kernel per layer, k_lstm_tc5r.cu) when the geometry
+// fits (hidden % 64 == 0 and <= 512, output_size 2), else the generic mma.sync kernel; lstm_impl = mma forces the generic kernel.
+// (FSN_LSTM_TCGEN05 is the historical name of the tensor-core path.)
 static int pick_impl(const fsn_model* m) {
     int impl = m->env_impl ? m->env_impl : m->cfg.lstm_impl;
-    if (impl == FSN_LSTM_AUTO) impl = (m->tc5_ok || m->tc5r_ok) ? FSN_LSTM_TCGEN05 : FSN_LSTM_MMA;
+    if (impl == FSN_LSTM_AUTO) impl = m->tc5r_ok ? FSN_LSTM_TCGEN05 : FSN_LSTM_MMA;
     return impl;
 }
-// Fused unfold: the two-layer tcgen05 kernel builds its input tiles itself (k_lstm_tc5d.cu, x-tile builders) from the window source
-// and the full-band outputs -- for the per-utterance norms; the per-frame cumulative norms keep the packed images.
-static bool use_xfuse(const fsn_model* m) {
-    return pick_impl(m) == FSN_LSTM_TCGEN05 && m->tc5_ok && !m->env_no_xfuse &&
-           (m->cfg.norm_type == FSN_NORM_OFFLINE_LAPLACE || m->cfg.norm_type == FSN_NORM_OFFLINE_GAUSSIAN);
-}
-// tcgen05 requested, but the geometry is outside the fused two-layer kernel: run the layer-wise kernel (k_lstm_tc5r.cu)
-static bool use_layerwise(const fsn_model* m) { return pick_impl(m) == FSN_LSTM_TCGEN05 && !m->tc5_ok && m->tc5r_ok; }
+static bool use_layerwise(const fsn_model* m) { return pick_impl(m) == FSN_LSTM_TCGEN05 && m->tc5r_ok; }
 
 
 static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, cudaStream_t s, cudaStream_t sl) {
@@ -550,7 +516,7 @@ static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, cudaStream
     const int F = c.num_freqs, Tp = T + c.look_ahead, Pp = (Tp + 3) & ~3;
     const int nbr = (c.model_kind == FSN_KIND_PLUS) ? 3 : 1;
     const size_t act = (size_t)nbr * B * F * Pp * 4;
-    const int rows = B * F, ntiles = ((rows + 127) / 128 + 1) / 2 * 2;      // whole CTA pairs (k_lstm_tc5d.cu)
+    const int rows = B * F, ntiles = ((rows + 127) / 128 + 1) / 2 * 2;      // whole pairs of 128-row tiles (clusters of k_lstm_tc5r.cu)
     const bool regeo = (ln.wsB != B || ln.wsT != T);
     int e = 0;
     e |= ln.fbin.ensure(act, true, s);
@@ -563,16 +529,18 @@ static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, cudaStream
     // images are re-zeroed whenever the geometry changes (rows beyond B*F and k >= I must stay zero)
     const size_t img_bytes = (size_t)ntiles * Tp * 16384;
     if (regeo) { ln.ximg.release(); }
-    if (!use_xfuse(m)) e |= ln.ximg.ensure(img_bytes, true, s);
+    e |= ln.ximg.ensure(img_bytes, true, s);
     // LSTM-side scratch: shared by both lanes (LSTM launches are serialised on the LSTM stream)
     int ra = 0;
     size_t cs = lstm_mma_cstate_bytes(c.num_layers, rows, c.sb_hidden, &ra);
-    size_t cs5 = lstm_tc5_cstate_bytes(ntiles, c.sb_hidden);
+    size_t cs5 = 0;
     if (use_layerwise(m)) {
-        const size_t M = (size_t)ntiles * Tp * 128, csr = lstm_tc5r_cstate_bytes(ntiles, c.sb_hidden);
-        if (csr > cs5) cs5 = csr;
-        e |= m->r_gin.ensure(M * 4 * c.sb_hidden * 2, false, sl);
-        if (c.num_layers > 1) e |= m->r_hseq.ensure(M * c.sb_hidden * 2, false, sl);
+        const size_t M = (size_t)ntiles * Tp * 128;
+        cs5 = lstm_tc5r_cstate_bytes(ntiles, c.sb_hidden);
+        if (c.num_layers > 1) {                                          // Gin and the layer output of the deeper layers
+            e |= m->r_gin.ensure(M * 4 * c.sb_hidden * 2, false, sl);
+            e |= m->r_hseq.ensure(M * c.sb_hidden * 2, false, sl);
+        }
     }
     if (c.model_kind == FSN_KIND_FSN) {
         int ra2 = 0;
@@ -591,7 +559,6 @@ static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, cudaStream
         e |= ln.y1.ensure(trows * 512 * sizeof(__half), true, s);
         e |= ln.y2.ensure(trows * 512 * sizeof(__half), true, s);
         e |= ln.stats.ensure((size_t)8 * 2 * 3 * B * 2 * sizeof(double) + (size_t)8 * 3 * B * sizeof(float), true, s);   // gLN sums | per-block stream maxima
-        if (use_xfuse(m)) e |= ln.fbo.ensure(trows * m->Cp * 4, true, s);
         if (!e && regeo) {
             if (make_tmap_f32_2d(ln.mapX0, ln.x0.p, trows, m->Cp, 128) || make_tmap_f32_2d(ln.mapXa, ln.xa.p, trows, m->Cp, 128) ||
                 make_tmap_f32_2d(ln.mapXb, ln.xb.p, trows, m->Cp, 128) || make_tmap_f32_2d(ln.mapXr, ln.xr.p, trows, m->Cp, 128) ||
@@ -609,58 +576,46 @@ static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, cudaStream
     return FSN_OK;
 }
 
-// d_enh != null: write the enhanced spectrum (decompress_cIRM x noisy) instead of the mask -- fused into the epilogue of the tcgen05
-// kernels, a separate pass over a scratch mask for the generic kernel
-static int run_sb_lstm(fsn_model* m, fsn_model::Lane& ln, int B, int T, float* d_out, const XSrc& xs, const float* d_real, const float* d_imag,
+// d_enh != null: write the enhanced spectrum (decompress_cIRM x noisy) instead of the mask -- fused into the epilogue of the
+// layer-wise kernel's last layer, a separate pass over a scratch mask for the generic kernel
+static int run_sb_lstm(fsn_model* m, fsn_model::Lane& ln, int B, int T, float* d_out, const float* d_real, const float* d_imag,
                        float* d_enh, cudaStream_t s) {
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs, Tp = T + c.look_ahead, rows = B * F, ntiles = (rows + 127) / 128;
     const int impl = pick_impl(m);
     m->last_impl = impl;
     if (use_layerwise(m)) {
-        // one GEMM (input projection of every row and time step, k_gemm_f16.cu) + one recurrent launch per layer
+        // one recurrent launch per layer; the first one also projects its input (the packed images), each deeper one is preceded by
+        // one GEMM: the input projection of every row and time step (k_gemm_tc5.cu)
         const int H = c.sb_hidden, ntp = (ntiles + 1) / 2 * 2;
         const long long M = (long long)ntp * Tp * 128;
         for (int l = 0; l < c.num_layers; ++l) {
-            const int K = (l == 0) ? 64 : H;
-            const void* X = (l == 0) ? ln.ximg.p : m->r_hseq.p;
-            // row-major Gin[M, 4H] = X[M, K] * Wp[4H, K]^T, both operands K-major
-            GemmF16Launch g{M, 4 * H, K, static_cast<__half*>(m->r_gin.p), 4LL * H};
-            int ge = launch_gemm_f16(X, m->r_wih[l].p, g, m->num_sms, s);
-            if (ge) return fail(FSN_ECUDA, "input-projection GEMM launch failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)ge));
-            m->launches++;
+            if (l > 0) {
+                // row-major Gin[M, 4H] = X[M, H] * Wp[4H, H]^T, both operands K-major
+                GemmF16Launch g{M, 4 * H, H, static_cast<__half*>(m->r_gin.p), 4LL * H};
+                int ge = launch_gemm_f16(m->r_hseq.p, m->r_wih[l].p, g, m->num_sms, s);
+                if (ge) return fail(FSN_ECUDA, "input-projection GEMM launch failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)ge));
+                m->launches++;
+            }
             LstmTc5rLaunch a{};
             a.wstream = static_cast<const __half*>(m->r_stream[l].p);
             a.bias = static_cast<const float*>(m->r_bias[l].p);
             a.fc_w = P(m, "sb_model.fc_output_layer.weight");
             a.fc_b = P(m, "sb_model.fc_output_layer.bias");
             a.H = H; a.rows = rows; a.Tp = Tp; a.ntiles = ntiles;
-            a.gin = static_cast<const __half*>(m->r_gin.p);
+            if (l == 0) a.ximg = static_cast<const __half*>(ln.ximg.p);
+            else a.gin = static_cast<const __half*>(m->r_gin.p);
             a.hseq = static_cast<__half*>(m->r_hseq.p);
             a.cstate = static_cast<float*>(m->cstate.p);
             a.out = d_out; a.F = F; a.la = c.look_ahead;
             a.act = c.sb_act; a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU; a.last = (l == c.num_layers - 1);
             a.nreal = d_real; a.nimag = d_imag; a.enh = reinterpret_cast<float2*>(d_enh);
             int e = launch_lstm_tc5r(a, s);
-            if (e) return fail(FSN_ECUDA, "layer-wise tcgen05 LSTM launch failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)e));
+            if (e) return fail(FSN_ECUDA, "layer-wise LSTM launch failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)e));
             m->launches++;
         }
     } else if (impl == FSN_LSTM_TCGEN05) {
-        if (!m->tc5_ok) return fail(FSN_EINVAL, "tcgen05 LSTM needs hidden %% 64 == 0 and <= 512 (<= 384 for the fused two-layer kernel), input <= 64, output_size 2");
-        LstmTc5Launch a{};
-        a.wstream = static_cast<const __half*>(m->sb_tc5_stream.p);
-        a.bias = static_cast<const float*>(m->sb_tc5_bias.p);
-        a.fc_w = P(m, "sb_model.fc_output_layer.weight");
-        a.fc_b = P(m, "sb_model.fc_output_layer.bias");
-        a.H = c.sb_hidden; a.I = m->Isb; a.rows = rows; a.Tp = Tp;
-        a.img = static_cast<const __half*>(ln.ximg.p); a.ntiles = ntiles;
-        a.xs = xs;
-        a.split = m->env_split;
-        a.nreal = d_real; a.nimag = d_imag; a.enh = reinterpret_cast<float2*>(d_enh);
-        a.cstate = static_cast<float*>(m->cstate.p);
-        a.out = d_out; a.F = F; a.la = c.look_ahead; a.act = c.sb_act; a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU;
-        int e = launch_lstm_tc5_dbuf(a, s);
-        if (e) return fail(FSN_ECUDA, "tcgen05 LSTM launch failed: %s", cudaGetErrorString((cudaError_t)e));
+        return fail(FSN_EINVAL, "the tensor-core LSTM needs hidden %% 64 == 0 and <= 512, input <= 64, output_size 2");
     } else {
         LstmMmaLaunch a{};
         for (int l = 0; l < c.num_layers; ++l) {
@@ -702,7 +657,7 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
     if (c.model_kind == FSN_KIND_PLUS && (!d_real || !d_imag)) return fail(FSN_EINVAL, "FullSubNet_Plus.forward needs mag, real and imag");
     const int F = c.num_freqs, Tp = T + c.look_ahead, Pp = (Tp + 3) & ~3;
     // chained (programmatic dependent) launches of this thread's front-end kernels: see env_pdl; "small" = at most 16 row-tile pairs,
-    // the regime of the LSTM kernel's column split
+    // where the forward is launch-latency-bound
     fsn_chain_launch_set(m->env_pdl == 1 || (m->env_pdl < 0 && ((long long)B * F + 255) / 256 <= 16));
     if (c.model_kind == FSN_KIND_PLUS && c.channel_attention == FSN_ATTN_TSSE)
         for (int i = 0; i < 3; ++i)
@@ -714,9 +669,6 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
     const int evi = (int)(m->nfwd % fsn_model::NEV);
     cudaEventRecord(m->evf0[evi], s);
 
-    const bool xfuse = use_xfuse(m);
-    ln.fbo_valid = xfuse && c.model_kind == FSN_KIND_PLUS;
-    XSrc xs{};
     SbPackLaunch sp{};
     sp.B = B; sp.F = F; sp.Tp = Tp; sp.Ns = c.sb_num_neighbors; sp.Nf = c.fb_num_neighbors; sp.P = Pp;
     sp.mu = static_cast<float*>(ln.mu.p);
@@ -724,7 +676,6 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
     sp.rowsum = static_cast<float*>(ln.sb_rowsum.p);
     sp.norm_type = c.norm_type;
     sp.ximg = static_cast<__half*>(ln.ximg.p);
-    sp.plain = use_layerwise(m) ? 1 : 0;                              // the layer-wise path feeds the images to a GEMM as a plain matrix
     sp.ntiles = (B * F + 127) / 128;
 
     if (c.model_kind == FSN_KIND_PLUS) {
@@ -778,7 +729,7 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
                 double* st2 = stats + (size_t)(2 * blk + 1) * Z * 2;
                 auto key = [&](int b, const char* leaf) { return std::string("fb_model") + sfx[b] + ".sequence_model." + std::to_string(blk) + "." + leaf; };
                 GemmTc5Launch g1 = g;
-                g1.epi = EPI5_PRELU_STATS; g1.Kp = Cp; g1.NT = 256; g1.ntiles_n = 2; g1.Npad = 512;
+                g1.epi = EPI5_PRELU_STATS; g1.Kp = Cp; g1.NT = 128; g1.ntiles_n = 4; g1.Npad = 512;
                 for (int b = 0; b < 3; ++b) { g1.bias[b] = P(m, key(b, "conv1x1.bias")); g1.prelu[b] = P(m, key(b, "prelu1.weight")); }
                 g1.stats_out = st1; g1.Y16 = static_cast<__half*>(ln.y1.p); g1.ldY = 512; g1.amax_in = amax + (size_t)blk * Z;
                 int e = launch_gemm_tc5(curmap, m->mapW1[blk], g1, m->num_sms, s);
@@ -817,7 +768,6 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
             g3.epi = EPI5_OUT; g3.Kp = Cp; g3.NT = m->tcnNT; g3.ntiles_n = m->tcnNtiles; g3.Npad = Cp;
             for (int b = 0; b < 3; ++b) g3.bias[b] = static_cast<const float*>(m->tBfc.p) + (size_t)b * Cp;
             g3.out = static_cast<float*>(ln.fbout.p); g3.F = F; g3.P = Pp; g3.act = c.fb_act;
-            if (xfuse) { g3.out_tm = static_cast<float*>(ln.fbo.p); g3.ldY = Cp; }
             int e = launch_gemm_tc5(ln.mapXr, m->mapWfc, g3, m->num_sms, s);
             if (e) return fail(FSN_ECUDA, "TCN output GEMM launch failed: %s", cudaGetErrorString((cudaError_t)e));
             m->launches++;
@@ -826,14 +776,6 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
         sp.win = static_cast<const float*>(ln.fbin.p); sp.Pw = Pp;      // post-attention mag branch (fullsubnet_plus.py:182)
         sp.nfb = 3;
         for (int b = 0; b < 3; ++b) sp.fb[b] = static_cast<const float*>(ln.fbout.p) + (size_t)b * B * F * Pp;
-        if (xfuse) {                                                        // time-major views: window = x0 (branch 0), outputs = fbo
-            const long long rowsB = (long long)Tp * m->Cp;
-            for (int b = 0; b < 3; ++b) sp.fb[b] = static_cast<const float*>(ln.fbo.p) + (size_t)b * B * rowsB;
-            sp.fb_sb = rowsB; sp.fb_sf = 1; sp.fb_st = m->Cp;
-            xs.win = static_cast<const float*>(ln.x0.p); xs.win_sb = rowsB; xs.win_sf = 1; xs.win_st = m->Cp;
-            for (int b = 0; b < 3; ++b) xs.fb[b] = sp.fb[b];
-            xs.fb_sb = rowsB; xs.fb_sf = 1; xs.fb_st = m->Cp;
-        }
     } else {
         TsseLaunch ta{};
         ta.x[0] = d_mag; ta.nbranch = 1; ta.B = B; ta.F = F; ta.T = T; ta.Tp = Tp; ta.P = Pp; ta.attention = 0;
@@ -888,25 +830,16 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
         sp.win = static_cast<const float*>(ln.magpad.p); sp.Pw = Pp;    // raw padded magnitude (fullsubnet.py:94)
         sp.nfb = 1;
         sp.fb[0] = static_cast<const float*>(ln.fbout.p);
-        if (xfuse) {                                                        // frequency-major views of the padded magnitude / the full-band output
-            xs.win = sp.win; xs.win_sb = (long long)F * Pp; xs.win_sf = Pp; xs.win_st = 1;
-            xs.fb[0] = sp.fb[0]; xs.fb_sb = (long long)F * Pp; xs.fb_sf = Pp; xs.fb_st = 1;
-        }
     }
-    launch_sb_stats(sp, s); m->launches += (sp.fb_st > 1) ? 3 : 2;
-    if (xfuse) {
-        xs.nfb = sp.nfb; xs.Ns = sp.Ns; xs.Nf = sp.Nf; xs.mu = sp.mu; xs.sigma = sp.sigma;
-        xs.gauss = (c.norm_type == FSN_NORM_OFFLINE_GAUSSIAN) ? 1 : 0;
-    } else {
-        launch_sb_pack(sp, s); m->launches++;
-    }
+    launch_sb_stats(sp, s); m->launches += 2;
+    launch_sb_pack(sp, s); m->launches++;
     cudaEventRecord(m->evf1[evi], s);
     if (sl != s) {                                                      // pipelined: the LSTM stream picks the lane up when the front end is done
         CK(cudaEventRecord(ln.ev_front, s));
         CK(cudaStreamWaitEvent(sl, ln.ev_front, 0));
     }
     cudaEventRecord(m->ev0[evi], sl);
-    rc = run_sb_lstm(m, ln, B, T, d_out, xs, d_real, d_imag, d_enh, sl);
+    rc = run_sb_lstm(m, ln, B, T, d_out, d_real, d_imag, d_enh, sl);
     cudaEventRecord(m->ev1[evi], sl);
     if (rc) return rc;
     m->nfwd++;
@@ -922,7 +855,7 @@ static int ensure_pipeline(fsn_model* m) {
     int lo = 0, hi = 0;
     CK(cudaDeviceGetStreamPriorityRange(&lo, &hi));                     // hi = numerically lowest = highest priority
     CK(cudaStreamCreateWithPriority(&m->s_front, cudaStreamNonBlocking, lo));
-    CK(cudaStreamCreateWithPriority(&m->s_lstm, cudaStreamNonBlocking, hi));   // the LSTM's CTA pairs win the SMs when both are pending
+    CK(cudaStreamCreateWithPriority(&m->s_lstm, cudaStreamNonBlocking, hi));   // the LSTM's clusters win the SMs when both are pending
     CK(cudaEventCreateWithFlags(&m->ev_in, cudaEventDisableTiming));
     for (auto& ln : m->lane) {
         CK(cudaEventCreateWithFlags(&ln.ev_front, cudaEventDisableTiming));
@@ -960,11 +893,11 @@ static double ws_bytes_per_sample(const fsn_model* m, int T) {
     const fsn_config& c = m->cfg;
     const double F = c.num_freqs, Tp = T + c.look_ahead, rows = F;              // sequences per sample
     double b = 0;
-    if (c.model_kind == FSN_KIND_PLUS) b += 3 * F * Tp * 4 * 2 + 3 * Tp * (5.0 * m->Cp + 512) * 4;       // fb_in/out, X0/Xa/Xb/Xr/fbo (fp32), Y1/Y2 (fp16)
+    if (c.model_kind == FSN_KIND_PLUS) b += 3 * F * Tp * 4 * 2 + 3 * Tp * (4.0 * m->Cp + 512) * 4;       // fb_in/out, X0/Xa/Xb/Xr (fp32), Y1/Y2 (fp16)
     else b += F * Tp * 4 * 4 + Tp * (F + c.fb_hidden) * 4;
     b += rows * Tp * 128;                                                       // packed sub-band images (when used)
     b += rows * c.num_layers * c.sb_hidden * 4;                                  // cell state
-    if (use_layerwise(m)) b += rows * Tp * (4.0 * c.sb_hidden + c.sb_hidden) * 2;   // Gin + layer output sequence
+    if (use_layerwise(m) && c.num_layers > 1) b += rows * Tp * (4.0 * c.sb_hidden + c.sb_hidden) * 2;   // Gin + layer output sequence
     return b;
 }
 
@@ -976,7 +909,7 @@ static int forward_plain(fsn_model* m, const float* d_mag, const float* d_real, 
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     for (auto& ln : m->lane)                                             // batches still in flight in the pipeline share the scratch buffers
         if (ln.used) CK(cudaStreamWaitEvent(s, ln.ev_lstm, 0));
-    // Samples are independent, so a batch whose workspace would exceed the cap (FSN_WS_CAP_GB, default 48 of the 180 GB) is run as
+    // Samples are independent, so a batch whose workspace would exceed the cap (FSN_WS_CAP_GB, default 24 of the 80 GB) is run as
     // equal sub-batches one after the other on the same stream -- same results, bounded memory (e.g. 256 clips on the layer-wise path).
     const double per = ws_bytes_per_sample(m, T);
     int Bmax = (int)(m->ws_cap_bytes / (per > 1 ? per : 1));
@@ -1138,11 +1071,6 @@ extern "C" int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst,
     const std::string n(name);
     if (n == "fb_in" || n == "fb_out") {
         if (numel != (int64_t)nbr * B * F * Tp) return fail(FSN_EINVAL, "%s needs %lld elements", name, (long long)nbr * B * F * Tp);
-        if (n == "fb_out" && ln.fbo_valid) {                            // fused-unfold path: the outputs exist time-major only
-            launch_tm_to_fm(static_cast<const float*>(ln.fbo.p), d_dst, nbr * B, F, Tp, m->Cp, s);
-            CK(cudaGetLastError());
-            return FSN_OK;
-        }
         const void* src = (n == "fb_in") ? ln.fbin.p : ln.fbout.p;
         CK(cudaMemcpy2DAsync(d_dst, (size_t)Tp * 4, src, (size_t)Pp * 4, (size_t)Tp * 4, (size_t)nbr * B * F, cudaMemcpyDeviceToDevice, s));
         return FSN_OK;

@@ -1,4 +1,4 @@
-// Common device helpers for the fsnplus_b200 kernels (sm_100a only).
+// Common device helpers for the fsnplus_b200 kernels (sm_90a only: wgmma, TMA, mbarrier, clusters).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -7,8 +7,8 @@
 #include <cstdio>
 #endif
 
-#if defined(__CUDA_ARCH__) && !defined(__CUDA_ARCH_FEAT_SM100_ALL)
-#error "fsnplus_b200 kernels must be compiled with -gencode arch=compute_100a,code=sm_100a"
+#if defined(__CUDA_ARCH__) && !defined(__CUDA_ARCH_FEAT_SM90_ALL)
+#error "fsnplus_b200 kernels must be compiled with -gencode arch=compute_90a,code=sm_90a"
 #endif
 
 namespace fsn {
@@ -62,7 +62,7 @@ __device__ __forceinline__ float warp_sum(float v) {
 }
 // Programmatic dependent launch (front-end chain, ~30 short kernels per forward): a kernel launched with launch_chain() may start
 // while its predecessor in the stream is still draining -- its CTAs are placed as SMs free up and run their prologue (barrier
-// init, TMEM allocation) -- and MUST execute pdl_wait() before it touches anything the predecessor reads or writes; pdl_wait returns
+// init) -- and MUST execute pdl_wait() before it touches anything the predecessor reads or writes; pdl_wait returns
 // when the predecessor grid has completed and its memory is visible (a no-op for a normally launched kernel).  pdl_trigger() lets
 // the successor begin launching once every CTA of this grid has executed it.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -90,15 +90,15 @@ __host__ __device__ __forceinline__ int reflect_idx(int p, int F) {
     return p;
 }
 
-// Byte offset of element (row r, half k) inside a 128-row x 64-half K-major tile stored with the
-// 128-byte swizzle the tcgen05 shared-memory descriptor (SWIZZLE_128B) expects: rows at 128 B pitch,
+// Byte offset of element (row r, half k) inside a K-major tile of 64 halves (128 bytes) per row stored with the
+// 128-byte swizzle the wgmma shared-memory descriptor (SWIZZLE_128B) and TMA expect: rows at 128 B pitch,
 // 16-byte chunk index XORed with (row & 7).  Tile base must be 1024-byte aligned.
 __host__ __device__ __forceinline__ uint32_t sw128_offset(uint32_t r, uint32_t k) {
     return r * 128u + ((((k >> 3) ^ (r & 7u)) & 7u) << 4) + ((k & 7u) << 1);
 }
 
 // ----------------------------------------------------------------------------------------------
-// shared-memory / mbarrier / bulk-copy / tcgen05 PTX wrappers
+// shared-memory / mbarrier / bulk-copy / wgmma PTX wrappers
 // ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
@@ -127,7 +127,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 }
 // Bounded wait: a protocol bug must trap (-> launch error reported to the host), never hang the box.
 #ifndef FSN_MBAR_TIMEOUT_CYCLES
-#define FSN_MBAR_TIMEOUT_CYCLES 3000000000ll   // ~2 s at B200 clocks; no legitimate wait is longer than ms
+#define FSN_MBAR_TIMEOUT_CYCLES 3000000000ll   // ~1.6 s at H100 boost clock; no legitimate wait is longer than ms
 #endif
 #ifdef FSN_MBAR_DEBUG
 // debug builds (-DFSN_MBAR_DEBUG): a watchdog expiry reports WHICH wait of which role hung before trapping
@@ -160,130 +160,64 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                  : "memory");
 }
 
-// Same copy with an L2 eviction-priority hint: evict_first for data that is read exactly once (the per-step input images, 392 MB
-// per launch at B = 64, which otherwise push the 50 MB cell-state scratch out of L2), evict_last for the weight stream that every
-// CTA re-reads every step.
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-    return p;
-}
+// L2 eviction-priority hint for data every CTA re-reads (the weight streams of the recurrent kernel)
 __device__ __forceinline__ uint64_t l2_policy_evict_last() {
     uint64_t p;
     asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
     return p;
 }
-__device__ __forceinline__ void bulk_g2s_hint(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar, uint64_t policy) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
-                     smem_u32(smem_dst)),
-                 "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
-                 : "memory");
-}
 
-// plain global accesses with an L2 eviction-priority hint (same policies as the bulk copies above)
-__device__ __forceinline__ float ldg_hint(const float* p, uint64_t policy) {
-    float v;
-    asm volatile("ld.global.nc.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(policy));
-    return v;
-}
-__device__ __forceinline__ uint4 ldg_u4_hint(const uint4* p, uint64_t policy) {
-    uint4 v;
-    asm volatile("ld.global.nc.L2::cache_hint.v4.b32 {%0, %1, %2, %3}, [%4], %5;" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p), "l"(policy));
-    return v;
-}
-__device__ __forceinline__ float4 ld_f4_hint(const float4* p, uint64_t policy) {
-    float4 v;
-    asm volatile("ld.global.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p), "l"(policy) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_f4_hint(float4* p, float4 v, uint64_t policy) {
-    asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(policy) : "memory");
-}
-
-// One lane of a fully converged warp (elect.sync).  The tcgen05 issue loops must stay warp-uniform and predicate only
-// the instruction on this: an `if (lane == 0)` region forces every UTCHMMA operand through R2UR moves and serialises the
-// mbarrier polls with the issue -- measured 109 vs 64 cycles per M=128,N=128 MMA (fsn_probe_tcgen05, "probe4").
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-
-// ---- tcgen05 -------------------------------------------------------------------------------
-__device__ __forceinline__ void tc5_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc5_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-template <uint32_t NCOLS> __device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "n"(NCOLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t NCOLS> __device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-
-// Shared-memory matrix descriptor, K-major, SWIZZLE_128B, 64-half (128 B) rows, 8-row groups 1024 B
-// apart (field layout: cute/arch/mma_sm100_desc.hpp SmemDescriptor; version = 1 on sm_100).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// ---- wgmma (sm_90a warpgroup MMA) ---------------------------------------------------------
+// Shared-memory matrix descriptor, K-major, SWIZZLE_128B, 128-byte rows, 8-row groups 1024 B apart (the layout sw128_offset
+// describes and TMA writes with CU_TENSOR_MAP_SWIZZLE_128B).  Advancing K by 32 bytes inside the swizzle atom = start address + 2.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFFu);          // start address      [0,14)
     d |= (uint64_t)1u << 16;                              // leading byte off.  [16,30) (ignored for swizzled K-major)
     d |= (uint64_t)(1024u >> 4) << 32;                    // stride byte offset [32,46)
-    d |= (uint64_t)1u << 46;                              // version            [46,48)
-    d |= (uint64_t)2u << 61;                              // SWIZZLE_128B       [61,64)
+    d |= (uint64_t)1u << 62;                              // SWIZZLE_128B       [62,64)
     return d;
 }
-// Instruction descriptor kind::f16: D=f32, A=B=f16, both K-major (InstrDescriptor in the same header).
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t M, uint32_t N) {
-    return (1u << 4)                 // c_format = F32
-           | (0u << 7) | (0u << 10)  // a_format = b_format = F16
-           | (0u << 15) | (0u << 16) // a_major = b_major = K
-           | ((N >> 3) << 17) | ((M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of accumulator registers across an asynchronous wgmma
+template <int R> __device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-
-// D[tmem] (+)= A[smem] * B[smem]
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+// D[64 x N] (+)= A[64 x K-step] * B[N x K-step]^T, both operands K-major in shared memory.  Accumulator fragment of thread
+// (warp w of the warpgroup, lane l): d[4 j + 2 h + e] = D[16 w + l / 4 + 8 h][8 j + 2 (l % 4) + e].
+__device__ __forceinline__ void wgmma_f16_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(accumulate));
 }
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate));
 }
-// Make an mbarrier track completion of all tcgen05 ops issued so far by this thread
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32-bit, 16 consecutive columns: thread i of the warp <-> TMEM lane (lane_base + i).
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
+__device__ __forceinline__ void wgmma_tf32_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&v)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(v[0]), "r"(v[1]),
-                 "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-                 : "memory");
+__device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate));
 }
 
-// ---- CTA pairs (cta_group::2): one tcgen05.mma drives both SMs of a 2-CTA cluster; each CTA holds half of B ---------
+// ---- clusters ------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
@@ -292,88 +226,17 @@ __device__ __forceinline__ void cluster_sync_all() {
 __device__ __forceinline__ uint32_t mapa_u32(uint32_t smem_addr, uint32_t rank) {
     uint32_t r; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank)); return r;
 }
-// Remote arrive.  Relaxed on purpose: a cluster-scope RELEASE costs ~1K cycles per arrive (measured: 26 ms vs 12 ms
-// kernel), and nothing but the barrier state has to be published -- the payload it guards was written by the async
-// proxy (bulk copy -> shared memory) or lives in tensor memory (ordered by tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+// Arrive on an mbarrier of any CTA of the cluster.  CTA-scope release: it only has to order this thread's completed reads of a
+// ring slot (wgmma, retired by wgmma.wait_group) before the producer refills it; a cluster-scope release would also wait for every
+// outstanding global store of the thread.
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
-// cluster-scope variants for data handed over through distributed shared memory (column-split small-batch mode of k_lstm_tc5d.cu):
-// the writer stores into the remote CTA, fences at cluster scope and arrives; the reader's wait acquires at cluster scope
-__device__ __forceinline__ void fence_acq_rel_cluster() { asm volatile("fence.acq_rel.cluster;" ::: "memory"); }
-__device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.b32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-#ifdef FSN_MBAR_DEBUG
-#define mbar_wait_cluster(bar, parity) mbar_wait_cluster_dbg(bar, parity, __LINE__)
-__device__ __forceinline__ void mbar_wait_cluster_dbg(uint64_t* bar, uint32_t parity, int line) {
-    if (mbar_try_wait_cluster(bar, parity)) return;
-    const long long t0 = clock64();
-    while (!mbar_try_wait_cluster(bar, parity)) {
-        if (clock64() - t0 > FSN_MBAR_TIMEOUT_CYCLES) { mbar_report(line, parity); __nanosleep(2000000); __trap(); }
-    }
-}
-#else
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-    if (mbar_try_wait_cluster(bar, parity)) return;
-    const long long t0 = clock64();
-    while (!mbar_try_wait_cluster(bar, parity)) {
-        if (clock64() - t0 > FSN_MBAR_TIMEOUT_CYCLES) { __trap(); }
-    }
-}
-#endif
-__device__ __forceinline__ void st_cluster_v4(uint32_t cluster_addr, uint4 v) {
-    asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(cluster_addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-__device__ __forceinline__ void st_cluster_v2f(uint32_t cluster_addr, float a, float b) {
-    asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(cluster_addr), "f"(a), "f"(b) : "memory");
-}
-// remote store that carries its own completion: the 16 (8) bytes land in the destination CTA and its mbarrier's transaction count is
-// decremented by the same amount -- no fence, no separate arrive; a waiter that observes the phase sees the data
-__device__ __forceinline__ void st_async_v4(uint32_t cluster_addr, uint4 v, uint32_t cluster_mbar) {
-    asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1, %2, %3, %4}, [%5];" ::"r"(cluster_addr), "r"(v.x), "r"(v.y),
-                 "r"(v.z), "r"(v.w), "r"(cluster_mbar)
-                 : "memory");
-}
-__device__ __forceinline__ void st_async_v2f(uint32_t cluster_addr, float a, float b, uint32_t cluster_mbar) {
-    asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];" ::"r"(cluster_addr), "f"(a), "f"(b), "r"(cluster_mbar)
-                 : "memory");
-}
-template <uint32_t NCOLS> __device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_result) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "n"(NCOLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t NCOLS> __device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void umma2_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma2_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// completion of all prior cta_group::2 MMAs -> arrive on the barrier at the same offset in every CTA of `mask`
-__device__ __forceinline__ void umma2_commit_mc(uint64_t* bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-                 "h"(mask)
+// 1-D bulk copy global -> shared of every CTA in `mask` (same offset in each), completion on the mbarrier at the same offset in each
+__device__ __forceinline__ void bulk_g2s_multicast(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar, uint16_t mask, uint64_t policy) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint [%0], [%1], %2, [%3], %4, %5;" ::"r"(
+                     smem_u32(smem_dst)),
+                 "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "h"(mask), "l"(policy)
                  : "memory");
 }
 
@@ -426,13 +289,7 @@ __device__ __forceinline__ float gru_cell_plain(float gr, float gz, float gnx, f
     return fmaf(z, hprev - n, n);
 }
 
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, const uint32_t (&v)[4]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1,%2,%3,%4};" ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3])
-                 : "memory");
-}
-
-
-// ---- legacy tensor path (mma.sync) used by the generic kernels ------------------------------
+// ---- warp-level tensor path (mma.sync) used by the generic kernels ------------------------------
 __device__ __forceinline__ void mma_f16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
     asm volatile(
         "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"

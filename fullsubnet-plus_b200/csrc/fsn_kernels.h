@@ -46,7 +46,7 @@ struct TsseLaunch {
     float* rows;               // [nbranch, B, F, 35] row statistics handed from tsse_rowstats_kernel to the gate kernel (tsse_row_floats())
     int prenorm;               // 1: input is already normalised (input_norm_kernel), skip the utterance-mean division
     int sub;                   // subband_num (ECA, mag branch only): channels are groups of `sub` reflect-padded bins (fullsubnet_plus.py:146-153)
-    float* out_tm; int Cp;     // optional time-major copy [(branch, b, t), Cp] for the tcgen05 TCN (pad columns stay zero)
+    float* out_tm; int Cp;     // optional time-major copy [(branch, b, t), Cp] for the TCN GEMMs (pad columns stay zero)
 };
 inline size_t tsse_row_floats() { return 3 + 2 * 16; }
 void launch_tsse_norm(const TsseLaunch& a, cudaStream_t s);
@@ -70,14 +70,12 @@ struct SbPackLaunch {
     const float* fb[3];      // [B, F, P] full-band outputs (nfb of them)
     int nfb, P;
     int B, F, Tp, Ns, Nf;    // neighbours
-    long long fb_sb, fb_sf, fb_st;   // sb_stats only: element strides of fb[] (0, 0, 0 = the default [B, F, P] layout)
     float* mu;               // [B] utterance mean of the concatenated sub-band input
     float* sigma;            // [B] unbiased std (offline_gaussian_norm only)
     float* rowsum;           // [B, 1 + nfb, F, 2] scratch: row sums and sums of squares
     int norm_type;           // FSN_NORM_*
     __half* ximg;            // [ntiles, Tp, 128 rows, 64 halves] SWIZZLE_128B images
     int ntiles;
-    int plain;               // 1: rows are stored unswizzled (row-major [ntiles * Tp * 128, 64]): the A matrix of the layer-wise path's GEMM
 };
 void launch_sb_stats(const SbPackLaunch& a, cudaStream_t s);
 void launch_sb_pack(const SbPackLaunch& a, cudaStream_t s);
@@ -86,7 +84,6 @@ void launch_pad_copy(const float* x, float* y, int B, int F, int T, int P, cudaS
 // full-band LSTM input: [B, F, P] fp32 -> [Tp, Bpad, Ipad] fp16 (rows >= B and k >= F zero)
 void launch_fb_pack(const float* x, __half* y, int B, int F, int Tp, int P, int rows_pad, int Ipad, cudaStream_t s);
 
-void launch_tm_to_fm(const float* x, float* y, int Z, int F, int Tp, int ld, cudaStream_t s);
 void launch_apply_cirm(const float* crm, const float2* noisy, float2* enh, int B, int F, int T, cudaStream_t s);
 // same with the noisy spectrum as two planes [B, F, T] (the model's own real / imag inputs)
 void launch_apply_cirm_planar(const float* crm, const float* nreal, const float* nimag, float2* enh, int B, int F, int T, cudaStream_t s);
@@ -140,58 +137,24 @@ struct LstmWsLaunch {
 bool lstm_ws_supported(int L, int H, int Ipad, int rows, int num_sms);
 int launch_lstm_ws(const LstmWsLaunch& a, cudaStream_t s);
 
-// ---- k_lstm_tc5d.cu --------------------------------------------------------------------------
-// Where the sub-band LSTM's x-tile builders find the (never materialised) unfolded input: the window source and the full-band
-// outputs as strided [sample, frequency, frame] views, plus the per-sample normaliser.  reference: base_model.py:15-47 (unfold),
-// fullsubnet_plus.py:167-202 / fullsubnet.py:90-111 (concat + norm).
-struct XSrc {
-    const float* win;                      // null: the kernel streams pre-packed images (LstmTc5Launch::img) instead
-    long long win_sb, win_sf, win_st;      // element strides: sample, frequency bin, frame
-    const float* fb[3];
-    long long fb_sb, fb_sf, fb_st;
-    int nfb, Ns, Nf;
-    const float* mu;                       // [B] utterance mean of the concatenated input (sb_stats_kernel)
-    const float* sigma;                    // [B] unbiased std (offline_gaussian_norm), else unused
-    int gauss;                             // 0: x / (mu + 1e-5); 1: (x - mu) / (sigma + 1e-5)
-};
-struct LstmTc5Launch {
-    const __half* wstream;    // packed weight stream (fsn_tc5_pack_weights)
-    const float* bias;        // [2][4H] permuted to the stream's gate-column order
-    const float* fc_w;        // [O=2][H]
-    const float* fc_b;        // [2]
-    int H, I;
-    int rows, Tp;
-    const __half* img; int ntiles;   // [ntiles, Tp, 16 KB] pre-packed SW128 images (used when xs.win is null)
-    XSrc xs;                  // fused unfold + norm: the kernel builds the image of every step itself
-    float* cstate;            // [ntiles][2 layers][H/16 chunks][4][128][4] fp32
-    float* out; int F, la;
-    int act;                  // FSN_ACT_* applied to the Linear output (sb_output_activate_function, sequence_model.py:120-121)
-    int fast;
-    int gru;                  // 1: pseudo-gate GRU cell
-    int split;                // column split S for small batches: 0 = auto (4 / 2 / 1 by the number of row tiles), or forced 1 / 2 / 4
-    // fused post-processing (inferencer.py:152-157): when enh != null the epilogue decompresses the cIRM and multiplies it with the
-    // noisy spectrum (planes [B, F, T]) instead of writing the mask: enh [B, F, T] complex64 (interleaved re, im)
-    const float* nreal; const float* nimag; float2* enh;
-};
-size_t lstm_tc5_cstate_bytes(int ntiles, int H);
-bool lstm_tc5_supported(int L, int H, int I, int O);
-int lstm_tc5_split_for(int H, int ntiles, int forced);              // the column split launch_lstm_tc5_dbuf will use
-int launch_lstm_tc5_dbuf(const LstmTc5Launch& a, cudaStream_t s);   // k_lstm_tc5d.cu: CTA-pair kernel with two 64-column accumulators
-
-// ---- k_lstm_tc5r.cu: single-layer recurrent kernel (time-batched input projection) for stacks outside the fused kernel's envelope
+// ---- k_lstm_tc5r.cu: single-layer recurrent wgmma kernel, input projection time-batched by launch_gemm_f16 ------------------
 struct LstmTc5rLaunch {
-    const __half* wstream;    // this layer's recurrent weight stream (lstm_tc5r_pack_layer)
+    const __half* wstream;    // [H/32 chunks][k-blocks] of 16 KB: W_hh (lstm_tc5r_pack_layer), or [W_ih | W_hh] with ximg (lstm_tc5_pack_first_layer)
     const float* bias;        // [4H] pre-scaled, chunk column order
     const float* fc_w;        // [2][H]   (last layer)
     const float* fc_b;        // [2]
     int H, rows, Tp, ntiles;
-    const __half* gin;        // [ntiles_pad * Tp * 128, 4H] fp16 input projection X_l W_ih^T, chunk column order
+    const __half* gin;        // [ntiles_pad * Tp * 128, 4H] fp16 input projection X_l W_ih^T (lstm_tc5r_gin_order), or null with ximg
+    const __half* ximg;       // first layer: [ntiles_pad, Tp, 128 rows, 64 halves] SW128 input images; the input projection is then part
+                              // of the recurrence, with W_ih as one extra k-block in front of every chunk of the stream
     __half* hseq;             // [ntiles_pad * Tp * 128, H] fp16 output sequence (not the last layer)
-    float* cstate;            // [ntiles_pad][H/32][4][2][128][4] fp32
+    float* cstate;            // [2 ntiles_pad CTAs][H/32 chunks][4][128 threads] float4
     float* out; int F, la;    // last layer: mask [B, 2, F, Tp - la]
     int act;                  // FSN_ACT_* on the Linear output (last layer)
     int fast, gru, last;
-    const float* nreal; const float* nimag; float2* enh;   // fused post-processing, see LstmTc5Launch
+    // fused post-processing (inferencer.py:152-157): when enh != null the last layer decompresses the cIRM and multiplies it with the
+    // noisy spectrum (planes [B, F, T]) instead of writing the mask: enh [B, F, T] complex64 (interleaved re, im)
+    const float* nreal; const float* nimag; float2* enh;
 };
 bool lstm_tc5r_supported(int H, int O);
 size_t lstm_tc5r_cstate_bytes(int ntiles, int H);
@@ -199,17 +162,19 @@ int64_t lstm_tc5r_weight_stream_bytes(int H);
 int launch_lstm_tc5r(const LstmTc5rLaunch& a, cudaStream_t s);
 void lstm_tc5r_pack_layer(int H, int Kin, int Kpad, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, bool gru,
                           std::vector<uint16_t>& stream, std::vector<uint16_t>& wih_perm, std::vector<float>& bias);
+void lstm_tc5r_gin_order(int H, int Kpad, std::vector<uint16_t>& wih_perm);   // rows of wih_perm -> the Gin column order the kernel reads
+void lstm_tc5_pack_first_layer(int I, int H, const float* w_ih0, const float* w_hh0, uint16_t* dst);   // k_lstm_tc5d.cu: [x | hidden] blocks per chunk
 
-// ---- k_gemm_f16.cu: C[M, N] = A[M, K] B[N, K]^T, fp16 in / fp32 accumulate / fp16 out (input projection of the layer-wise path)
+// ---- k_gemm_tc5.cu (TCN on wgmma, time-major activations; the input projection of the layer-wise LSTM path) ----------------
+// C[M, N] = A[M, K] B[N, K]^T, fp16 in / fp32 accumulate / fp16 out (input projection of the layer-wise path)
 struct GemmF16Launch { long long M; int N, K; __half* C; long long ldc; };
 bool gemm_f16_supported(long long M, int N, int K);
 int launch_gemm_f16(const void* A, const void* B, const GemmF16Launch& a, int num_sms, cudaStream_t s);
 int make_tmap_f16_2d(void* out_map /*128 B, 64 B aligned*/, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows);   // box = 64 halves x box_rows, SWIZZLE_128B
 
-// ---- k_gemm_tc5.cu (TCN on tcgen05, time-major activations) ----------------------------------
-enum { EPI5_PRELU_STATS = 1, EPI5_GLN_RES = 2, EPI5_OUT = 3 };
+enum { EPI5_PRELU_STATS = 1, EPI5_GLN_RES = 2, EPI5_OUT = 3, EPI5_F16OUT = 4 };
 struct GemmTc5Launch {
-    int Kp, NT, nstage, ntiles_n, Npad;        // K (multiple of 32; GLN_RES: fp16 operands, multiple of 64), N tile, ring depth, N tiles and padded N per branch
+    int Kp, NT, nstage, ntiles_n, Npad;        // K (multiple of 32; GLN_RES: fp16 operands, multiple of 64), N tile (64 or 128), ring depth, N tiles and padded N per branch
     int rows_per_branch, tiles_m, nbranch, Tp, B;
     int epi;
     const float* bias[3];                      // PRELU_STATS / OUT: conv bias; GLN_RES: s2 + conv bias
@@ -218,12 +183,11 @@ struct GemmTc5Launch {
     double* stats_out;                         // [Z, 2]
     const double* stats_in; double count_in;
     float* Y; int ldY;                         // GLN_RES: new residual stream (fp32)
-    __half* Y16;                               // PRELU_STATS: the hidden activation, fp16 [rows, ldY], stored times fp16_store_scale(amax_in[z])
+    __half* Y16;                               // PRELU_STATS: the hidden activation, fp16 [rows, ldY], stored times fp16_store_scale(amax_in[z]); F16OUT: C
     const float* amax_in;                      // PRELU_STATS: [Z] max |x| of the block's input stream per sample
     float* amax_out;                           // GLN_RES: [Z] max |x| of the new stream per sample (atomicMax on the bit pattern; zeroed by the caller)
     const float* Xold; float* Xrelu;           // GLN_RES: residual input, optional relu'd copy
-    float* out; int F, P, act;                 // OUT: [Z, F, P] (frequency-major) ...
-    float* out_tm;                             // ... or, when set, time-major [(branch, b, t), ldY] (read by the LSTM's x-tile builders)
+    float* out; int F, P, act;                 // OUT: [Z, F, P] (frequency-major)
 };
 int make_tmap_f32_2d(void* out_map /*128 B, 64 B aligned*/, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows);
 int launch_gemm_tc5(const void* mapA, const void* mapB, GemmTc5Launch a, int num_sms, cudaStream_t s);

@@ -1,4 +1,4 @@
-// Full-band front end of the FullSubNet+/FullSubNet forward on sm_100a:
+// Full-band front end of the FullSubNet+/FullSubNet forward on sm_90a:
 //   * utterance Laplace norm + TSSE ("MulCA") channel attention     (K1 + K2 of SURVEY.md 2a)
 //   * the output Linear of fullsubnet.Model's full-band LSTM (the TCN of FullSubNet+ is in k_gemm_tc5.cu)  (K3)
 //   * utterance mean of the (never materialised) unfolded sub-band input and the fp16 packing of the
@@ -317,7 +317,7 @@ void launch_input_norm(const NormLaunch& a, cudaStream_t s) {
 // =============================================================================================
 // Output Linear of the full-band LSTM of fullsubnet.Model (fullsubnet.py:86, sequence_model.py:118-121):
 // Y[z] = act(W * X[z] + b) on the [Z, K, P] layout as a TF32 tensor-core GEMM (mma.sync m16n8k8), 64x64x32 tiles, 4 warps.
-// (The TCN's 1x1 convolutions run on tcgen05, k_gemm_tc5.cu; this small GEMM is latency-bound: Z <= 64, K = 512, M = 257.)
+// (The TCN's 1x1 convolutions run on wgmma, k_gemm_tc5.cu; this small GEMM is latency-bound: Z <= 64, K = 512, M = 257.)
 // =============================================================================================
 __global__ void __launch_bounds__(128) conv1x1_tf32_kernel(ConvLaunch a) {
     __shared__ uint32_t Ws[64][36];
@@ -416,23 +416,6 @@ __global__ void __launch_bounds__(256) sb_rowsum_kernel(SbPackLaunch a) {
     if (lane == 0) { a.rowsum[2 * (size_t)r] = acc; a.rowsum[2 * (size_t)r + 1] = acq; }
 }
 
-// window-source rows only, written into the [b][nsrc][f] slots of the full table (the full-band sources come from sb_colsum_kernel)
-__global__ void __launch_bounds__(256) sb_rowsum_strided_kernel(SbPackLaunch a, int nsrc) {
-    pdl_trigger();
-    pdl_wait();
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int F = a.F, Tp = a.Tp;
-    const int r0 = blockIdx.x * 8 + warp;                      // (b, f)
-    if (r0 >= a.B * F) return;
-    const int b = r0 / F, f = r0 % F;
-    const float* row = a.win + ((size_t)b * F + f) * a.Pw;
-    float acc = 0.f, acq = 0.f;
-    for (int t = lane; t < Tp; t += 32) { const float v = row[t]; acc += v; acq = fmaf(v, v, acq); }
-    acc = warp_sum(acc); acq = warp_sum(acq);
-    const size_t r = ((size_t)b * nsrc) * F + f;
-    if (lane == 0) { a.rowsum[2 * r] = acc; a.rowsum[2 * r + 1] = acq; }
-}
-
 __global__ void __launch_bounds__(256) sb_stats_kernel(SbPackLaunch a) {
     pdl_trigger();
     pdl_wait();
@@ -463,50 +446,8 @@ __global__ void __launch_bounds__(256) sb_stats_kernel(SbPackLaunch a) {
     }
 }
 
-// Same sums for full-band outputs stored TIME-major (fb_st > 1: element (b, f, t) at fb[q] + b fb_sb + f fb_sf + t fb_st with
-// fb_sf == 1): one CTA per (sample, source); threadIdx.x walks the bins (coalesced rows), threadIdx.y splits the frames into
-// blockDim.y interleaved slices, eight independent loads per thread in flight; the slices are added in a fixed order (deterministic).
-__global__ void __launch_bounds__(1024) sb_colsum_kernel(SbPackLaunch a) {
-    extern __shared__ float part[];                              // [blockDim.y][blockDim.x][2]
-    pdl_trigger();
-    pdl_wait();
-    const int b = blockIdx.x, q = blockIdx.y, F = a.F, Tp = a.Tp, nsrc = 1 + a.nfb;
-    const int ny = blockDim.y, ty = threadIdx.y;
-    const float* base = ((q == 0) ? a.fb[0] : (q == 1) ? a.fb[1] : a.fb[2]) + (size_t)b * a.fb_sb;
-    for (int f0 = 0; f0 < F; f0 += blockDim.x) {
-        const int f = f0 + threadIdx.x;
-        float acc = 0.f, acq = 0.f;
-        if (f < F) {
-            for (int t0 = ty; t0 < Tp; t0 += 8 * ny) {
-                float v[8];
-#pragma unroll
-                for (int u = 0; u < 8; ++u) { const int t = t0 + u * ny; v[u] = (t < Tp) ? __ldg(base + (size_t)t * a.fb_st + f) : 0.f; }
-#pragma unroll
-                for (int u = 0; u < 8; ++u) { acc += v[u]; acq = fmaf(v[u], v[u], acq); }
-            }
-        }
-        part[(ty * blockDim.x + threadIdx.x) * 2] = acc;
-        part[(ty * blockDim.x + threadIdx.x) * 2 + 1] = acq;
-        __syncthreads();
-        if (ty == 0 && f < F) {
-            for (int y = 1; y < ny; ++y) { acc += part[(y * blockDim.x + threadIdx.x) * 2]; acq += part[(y * blockDim.x + threadIdx.x) * 2 + 1]; }
-            const size_t r = ((size_t)b * nsrc + 1 + q) * F + f;
-            a.rowsum[2 * r] = acc; a.rowsum[2 * r + 1] = acq;
-        }
-        __syncthreads();
-    }
-}
-
 void launch_sb_stats(const SbPackLaunch& a, cudaStream_t s) {
-    if (a.fb_st > 1) {                                           // window source frequency-major, full-band outputs time-major
-        SbPackLaunch w = a;
-        w.nfb = 0;                                               // rows of the window source only ...
-        launch_chain(sb_rowsum_strided_kernel, dim3((a.B * a.F + 7) / 8), dim3(256), 0, s, w, 1 + a.nfb);
-        const int bx = (a.F + 31) / 32 * 32 < 512 ? (a.F + 31) / 32 * 32 : 512, by = 1024 / bx;
-        launch_chain(sb_colsum_kernel, dim3(a.B, a.nfb), dim3(bx, by), (size_t)bx * by * 2 * sizeof(float), s, a);    // ... the full-band outputs by columns
-    } else {
-        launch_chain(sb_rowsum_kernel, dim3((a.B * (1 + a.nfb) * a.F + 7) / 8), dim3(256), 0, s, a);
-    }
+    launch_chain(sb_rowsum_kernel, dim3((a.B * (1 + a.nfb) * a.F + 7) / 8), dim3(256), 0, s, a);
     launch_chain(sb_stats_kernel, dim3(a.B), dim3(256), 0, s, a);
 }
 
@@ -555,7 +496,7 @@ __global__ void __launch_bounds__(256) sb_pack_kernel(SbPackLaunch a) {
         u.z = pack_half2(val(c * 8 + 4, tt), val(c * 8 + 5, tt));
         u.w = pack_half2(val(c * 8 + 6, tt), val(c * 8 + 7, tt));
         char* img = reinterpret_cast<char*>(a.ximg) + ((size_t)tile * Tp + t0 + tt) * (128 * 128);
-        *reinterpret_cast<uint4*>(img + (a.plain ? (uint32_t)(r * 128 + c * 16) : sw128_offset(r, c * 8))) = u;
+        *reinterpret_cast<uint4*>(img + sw128_offset(r, c * 8)) = u;
     }
 }
 
@@ -606,7 +547,7 @@ __global__ void __launch_bounds__(128) sb_pack_cum_kernel(SbPackLaunch a) {
                 float w[8];
 #pragma unroll
                 for (int i = 0; i < 8; ++i) w[i] = (c * 8 + i < I) ? fminf(fmaxf(fmaf(v[c * 8 + i], sc, sh), -65504.f), 65504.f) : 0.f;
-                *reinterpret_cast<uint4*>(img + (a.plain ? (uint32_t)(r * 128 + c * 16) : sw128_offset(r, c * 8))) =
+                *reinterpret_cast<uint4*>(img + sw128_offset(r, c * 8)) =
                     make_uint4(pack_half2(w[0], w[1]), pack_half2(w[2], w[3]), pack_half2(w[4], w[5]), pack_half2(w[6], w[7]));
             }
         }
@@ -720,19 +661,6 @@ void launch_apply_cirm_planar(const float* crm, const float* nreal, const float*
 void launch_apply_cirm(const float* crm, const float2* noisy, float2* enh, int B, int F, int T, cudaStream_t s) {
     const size_t n = (size_t)B * F * T;
     apply_cirm_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(crm, noisy, enh, F * T, n);
-}
-
-// test hook: time-major [(z, t), ld] -> frequency-major [z, F, Tp]
-__global__ void tm_to_fm_kernel(const float* x, float* y, int Z, int F, int Tp, int ld) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= (size_t)Z * F * Tp) return;
-    const int t = (int)(i % Tp), f = (int)((i / Tp) % F);
-    const size_t z = i / ((size_t)Tp * F);
-    y[i] = x[(z * Tp + t) * ld + f];
-}
-void launch_tm_to_fm(const float* x, float* y, int Z, int F, int Tp, int ld, cudaStream_t s) {
-    const size_t n = (size_t)Z * F * Tp;
-    tm_to_fm_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(x, y, Z, F, Tp, ld);
 }
 
 __global__ void pad_copy_kernel(const float* x, float* y, int rows, int T, int P) {

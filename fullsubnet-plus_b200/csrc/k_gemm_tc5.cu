@@ -1,5 +1,6 @@
-// TCN full-band model (K3 of SURVEY.md 2a) on the 5th-generation tensor cores: the 1x1 convolutions of the eight
-// TCNBlocks and the output Linear as persistent tcgen05 GEMMs over time-major activations, plus the depth-wise convolution between them.
+// TCN full-band model (K3 of SURVEY.md 2a) on the Hopper tensor cores: the 1x1 convolutions of the eight TCNBlocks and the
+// output Linear as persistent wgmma GEMMs over time-major activations, plus the depth-wise convolution between them.  The same
+// GEMM kernel also computes the input projection of the layer-wise LSTM path (EPI5_F16OUT).
 //
 // reference: TCNBlock.forward (audio_zen/model/module/causal_conv.py:96-108) and SequenceModel.forward, TCN branch
 // (audio_zen/model/module/sequence_model.py:106-112).
@@ -7,19 +8,19 @@
 // Formulation.  Activations are stored time-major, rows = (branch, sample, frame), columns = channels (padded to a
 // multiple of 32 floats = one 128-byte swizzle atom), so every 1x1 convolution is  D[rows, C_out] = X[rows, C_in] *
 // W[C_out, C_in]^T  with BOTH operands K-major -- the layout PyTorch already stores W in.  Tiles of 128 rows x 128 bytes of k
-// (A) and N_TILE x 128 bytes of k (B) are fetched by TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B) into a shared-memory ring,
-// multiplied with tcgen05.mma (kind::tf32 on the fp32 residual stream, kind::f16 on the fp16 hidden activations) into double-
-// buffered TMEM accumulators, and finished by eight epilogue warps whose global loads / stores go through per-warp staging tiles
-// (g5_store_rows64: 8 rows x 64 contiguous bytes per instruction instead of 32 rows x 16 bytes):
+// (A) and NT x 128 bytes of k (B) are fetched by TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B) into a shared-memory ring by one
+// producer warp; two consumer warpgroups (64 rows each) multiply them with wgmma (tf32 on the fp32 residual stream, f16 on the
+// fp16 hidden activations) into register accumulators and run the epilogue on those registers while the producer already
+// fetches the next tile:
 //   EPI_PRELU_STATS : + bias, PReLU, per-sample sum / sum-of-squares for the following gLN, store as fp16 times a per-sample power of
 //                     two (fp16_store_scale: the hidden, 512-channel activations of a block live in fp16 -- the same 10 mantissa
 //                     bits the tf32 product consumed, half the bytes; the normalised real / imag streams reach 1e6 and beyond)
 //   EPI_GLN_RES     : gLN folded analytically -- conv(W, gLN(y)) = rstd * (W diag(gamma)) y - mean rstd s1 + s2 --
 //                     so the GEMM runs on the raw activation and the per-sample affine is applied here, + residual (fp32 stream),
 //                     + the running max |x| per sample of the new stream (the next block's store scale).
-//                     Its operands (hidden activation, folded weights) are fp16: kind::f16, 64-element k-blocks.
-//   EPI_OUT         : + bias, output activation, written time-major (the layout the sub-band LSTM's x-tile builders read) or,
-//                     for the packed path, transposed into [branch, B, F, T'].
+//                     Its operands (hidden activation, folded weights) are fp16: 64-element k-blocks.
+//   EPI_OUT         : + bias, output activation, transposed into [branch, B, F, T'].
+//   EPI_F16OUT      : fp16 result, row-major (Gin of the layer-wise LSTM, k_lstm_tc5r.cu).
 #include <cuda.h>
 
 #include "fsn_common.cuh"
@@ -28,104 +29,98 @@
 
 namespace fsn {
 
-constexpr int G5_EPI_WARPS = 8;       // two warps per TMEM lane quarter, each takes half of the 16-column chunks of a tile
-constexpr int G5_THREADS = (2 + G5_EPI_WARPS) * 32;   // warp 0 TMA producer, warp 1 MMA issuer + TMEM alloc, warps 2-9 epilogue
+constexpr int G5_CONS = 2;                                // consumer warpgroups, rows 64 wg .. 64 wg + 63 of a 128-row tile
+constexpr int G5_THREADS = (4 * G5_CONS + 1) * 32;        // + one TMA producer warp (warp 8)
 constexpr int G5_A_BYTES = 128 * 128;
 
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(uint32_t M, uint32_t N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);   // D=f32, A=B=tf32, K-major
-}
-__device__ __forceinline__ void umma_ss_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
                      smem_u32(smem_dst)),
                  "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
                  : "memory");
 }
-__device__ __forceinline__ float round_tf32(float x) { return __uint_as_float(f2tf32(x)); }
 
-// ---- coalesced epilogue I/O --------------------------------------------------------------------------------------------------
-// tcgen05.ld hands every epilogue thread ONE ROW of the tile (32x32b shape), so a direct global store touches 32 different 128-byte
-// lines per instruction with 16 bytes each: the L1 tag stage (one line per cycle) -- not HBM -- bounded these kernels (ncu, round 2:
-// 2.6 M store + 2.8 M load sector accesses in the second convolution = 20 us of its 48).  Each warp therefore owns a 2 KB staging tile
-// (32 rows x 64 bytes, 16-byte units XOR-swizzled): rows go in thread-per-row, come out with lane l <-> (row (l >> 2) + 8 i, unit l & 3),
-// i.e. 8 rows x 64 contiguous bytes per instruction (both views are bank-conflict free), and the same in reverse for the residual.
-constexpr int G5_STG_BYTES = 32 * 64;
-__device__ __forceinline__ uint4* g5_stg(uint8_t* t, int row, int unit) {
-    return reinterpret_cast<uint4*>(t + row * 64 + ((unit ^ ((row >> 1) & 3)) << 4));
+// one 32-byte k-step of the 64 x NT warpgroup tile: 16 fp16 or 8 tf32 elements
+template <int NT, bool AH>
+__device__ __forceinline__ void g5_mma(float (&acc)[NT / 2], uint64_t ad, uint64_t bd, uint32_t accumulate) {
+    if constexpr (NT == 128) { if constexpr (AH) wgmma_f16_n128(acc, ad, bd, accumulate); else wgmma_tf32_n128(acc, ad, bd, accumulate); }
+    else { static_assert(NT == 64, "NT is 64 or 128"); if constexpr (AH) wgmma_f16_n64(acc, ad, bd, accumulate); else wgmma_tf32_n64(acc, ad, bd, accumulate); }
 }
-// every lane holds the 64 bytes of its row; row r of the warp lives at gbase + r * pitch (bytes); rows >= nvalid are not written
-__device__ __forceinline__ void g5_store_rows64(uint8_t* t, int lane, const uint4 (&v)[4], uint8_t* gbase, size_t pitch, int nvalid) {
+
+// fp16 results (PRELU_STATS, F16OUT) leave through a per-warp staging tile: the accumulator fragment gives a lane 4 bytes of 8 rows
+// per store, so direct stores wrote 16-byte pieces of 8 lines per instruction; staged, a warp writes whole 512-byte row runs.
+// Tile = the warp's 16 rows x NT halves, 16-byte units XOR-swizzled by (row & 7) so both the fragment writes and the row reads are
+// free of bank conflicts.  hp[j][h] = the packed pair (columns 8 j + 2 (lane % 4), + 1) of row (lane / 4) + 8 h.
+template <int NT>
+__device__ __forceinline__ void g5_store_f16(uint8_t* stg, int lane, const uint32_t (&hp)[NT / 8][2], __half* gbase, size_t ld, int nvalid) {
+    constexpr int U = NT / 8;                                   // 16-byte units per row
 #pragma unroll
-    for (int q = 0; q < 4; ++q) *g5_stg(t, lane, q) = v[q];
+    for (int j = 0; j < U; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int r = (lane >> 2) + 8 * h;
+            *reinterpret_cast<uint32_t*>(stg + r * NT * 2 + ((j ^ (r & 7)) << 4) + (lane & 3) * 4) = hp[j][h];
+        }
     __syncwarp();
+    constexpr int RPI = 32 / U;                                 // rows per store instruction
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const int row = (lane >> 2) + 8 * i;
-        const uint4 u = *g5_stg(t, row, lane & 3);
-        if (row < nvalid) *reinterpret_cast<uint4*>(gbase + (size_t)row * pitch + (lane & 3) * 16) = u;
+    for (int i = 0; i < 16 / RPI; ++i) {
+        const int r = i * RPI + lane / U, u = lane % U;
+        const uint4 v = *reinterpret_cast<const uint4*>(stg + r * NT * 2 + ((u ^ (r & 7)) << 4));
+        if (r < nvalid) *reinterpret_cast<uint4*>(gbase + (size_t)r * ld + u * 8) = v;
     }
     __syncwarp();
 }
-__device__ __forceinline__ void g5_load_rows64_issue(int lane, const uint8_t* gbase, size_t pitch, int nvalid, uint4 (&g)[4]) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const int row = (lane >> 2) + 8 * i;
-        g[i] = (row < nvalid) ? *reinterpret_cast<const uint4*>(gbase + (size_t)row * pitch + (lane & 3) * 16) : make_uint4(0, 0, 0, 0);
+
+// sum (PRELU_STATS) or max (GLN_RES) of one value per lane into a per-sample slot: rows of a warp almost always belong to one
+// sample -- reduce in the warp, one atomic per warp; lanes whose row is invalid pass key -1
+__device__ __forceinline__ void g5_stats_add(int key, double s, double q, double* out) {
+    if (__match_any_sync(0xffffffffu, key) == 0xffffffffu) {
+        s = warp_sum_d(s); q = warp_sum_d(q);
+        if ((threadIdx.x & 31) == 0 && key >= 0) { atomicAdd(&out[2 * key], s); atomicAdd(&out[2 * key + 1], q); }
+    } else if (key >= 0) {
+        atomicAdd(&out[2 * key], s);
+        atomicAdd(&out[2 * key + 1], q);
     }
 }
-__device__ __forceinline__ void g5_load_rows64_commit(uint8_t* t, int lane, const uint4 (&g)[4], uint4 (&v)[4]) {
+__device__ __forceinline__ void g5_max_add(int key, float v, float* out) {
+    if (__match_any_sync(0xffffffffu, key) == 0xffffffffu) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i) *g5_stg(t, (lane >> 2) + 8 * i, lane & 3) = g[i];
-    __syncwarp();
-#pragma unroll
-    for (int q = 0; q < 4; ++q) v[q] = *g5_stg(t, lane, q);
-    __syncwarp();
+        for (int o = 16; o; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+        if ((threadIdx.x & 31) == 0 && key >= 0) atomicMax(reinterpret_cast<int*>(out + key), __float_as_int(v));
+    } else if (key >= 0) {
+        atomicMax(reinterpret_cast<int*>(out + key), __float_as_int(v));
+    }
 }
 
-template <int EPI>
+template <int EPI, int NT>
 __global__ void __launch_bounds__(G5_THREADS, 1)
 gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, GemmTc5Launch a) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    const int NT = a.NT, nstage = a.nstage, stage_bytes = G5_A_BYTES + NT * 128;
-    uint8_t* stg_all = smem + (size_t)nstage * stage_bytes;                  // [G5_EPI_WARPS][G5_STG_BYTES] epilogue staging tiles
-    uint64_t* bars = reinterpret_cast<uint64_t*>(stg_all + G5_EPI_WARPS * G5_STG_BYTES);
-    uint64_t* full = bars;
-    uint64_t* empty = full + nstage;
-    uint64_t* accfull = empty + nstage;
-    uint64_t* accempty = accfull + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accempty + 2);
+    const int nstage = a.nstage;
+    constexpr int stage_bytes = G5_A_BYTES + NT * 128;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    uint8_t* stg = smem + (size_t)nstage * stage_bytes + (warp & 7) * 16 * NT * 2;    // this consumer warp's fp16 staging tile
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)nstage * stage_bytes + 8 * 16 * NT * 2);
+    uint64_t* empty = full + nstage;
 
     if (tid == 0) {
-        for (int i = 0; i < nstage; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&accfull[i], 1); mbar_init(&accempty[i], G5_EPI_WARPS); }
+        for (int i = 0; i < nstage; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 4 * G5_CONS); }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc<512>(tmem_slot);
-    tc5_fence_before();
     __syncthreads();
-    tc5_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    // chained launch: barriers and tensor memory are set up while the previous kernel of the chain drains; nothing it wrote is read
-    // (and nothing it reads is overwritten) before this point
+    // chained launch: the barriers are set up while the previous kernel of the chain drains; nothing it wrote is read (and nothing it
+    // reads is overwritten) before this point
     pdl_trigger();
     pdl_wait();
-    constexpr bool AH = (EPI == EPI5_GLN_RES);             // fp16 operands: a 128-byte swizzle atom holds 64 k-elements instead of 32
+    constexpr bool AH = (EPI == EPI5_GLN_RES || EPI == EPI5_F16OUT);   // fp16 operands: a 128-byte swizzle atom holds 64 k-elements instead of 32
     constexpr int KBW = AH ? 64 : 32;
     const int nkb = a.Kp / KBW;
     const int tiles_per_branch = a.tiles_m * a.ntiles_n;
     const int total = a.nbranch * tiles_per_branch;
 
-    if (warp == 0) {
+    if (warp == 4 * G5_CONS) {
         if (lane == 0) {
             int slot = 0; uint32_t ph = 0;
             for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
@@ -142,208 +137,137 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                 }
             }
         }
-    } else if (warp == 1) {
-        {   // warp-uniform issue loop, instructions predicated on one elected lane (see elect_one)
-            const uint32_t idesc = AH ? umma_idesc_f16(128, NT) : umma_idesc_tf32(128, NT);
-            int slot = 0; uint32_t ph = 0, use[2] = {0, 0}, it = 0;
-            for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++it) {
-                const int buf = it & 1;
-                mbar_wait(&accempty[buf], (use[buf] & 1) ^ 1);
-                ++use[buf];
-                tc5_fence_after();
-                const uint32_t d = tmem + buf * 256;
-                for (int kb = 0; kb < nkb; ++kb) {
-                    mbar_wait(&full[slot], ph);
-                    tc5_fence_after();
-                    const uint32_t sa = smem_u32(smem + (size_t)slot * stage_bytes);
-                    const uint64_t adesc = umma_desc_sw128(sa), bdesc = umma_desc_sw128(sa + G5_A_BYTES);
-                    if (elect_one()) {
+        return;
+    }
+
+    const int wg = warp >> 2, wi = warp & 3;
+    float acc[NT / 2];
+    int slot = 0; uint32_t ph = 0;
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+        const int br = tile / tiles_per_branch, rem = tile % tiles_per_branch;
+        const int mt = rem / a.ntiles_n, nt = rem % a.ntiles_n;
+        // ---- main loop: one 128-byte k-block per ring slot, the slot is handed back as soon as its MMAs have retired ----
+        int prev = -1;
+        for (int kb = 0; kb < nkb; ++kb) {
+            mbar_wait(&full[slot], ph);
+            wgmma_fence();
+            const uint32_t sa = smem_u32(smem + (size_t)slot * stage_bytes);
+            const uint64_t adesc = wgmma_desc_sw128(sa + wg * 64 * 128), bdesc = wgmma_desc_sw128(sa + G5_A_BYTES);
 #pragma unroll
-                        for (int kk = 0; kk < 4; ++kk) {                  // 32 bytes of K per instruction: 8 tf32 or 16 fp16 elements
-                            if (AH) umma_ss(d, adesc + 2 * kk, bdesc + 2 * kk, idesc, (kb | kk) != 0);
-                            else umma_ss_tf32(d, adesc + 2 * kk, bdesc + 2 * kk, idesc, (kb | kk) != 0);
-                        }
-                        umma_commit(&empty[slot]);
-                        if (kb == nkb - 1) umma_commit(&accfull[buf]);
-                    }
-                    __syncwarp();
-                    if (++slot == nstage) { slot = 0; ph ^= 1; }
-                }
+            for (int kk = 0; kk < 4; ++kk) g5_mma<NT, AH>(acc, adesc + 2 * kk, bdesc + 2 * kk, (kb | kk) != 0);
+            wgmma_commit();
+            if (prev >= 0) {
+                wgmma_wait<1>();
+                if (lane == 0) mbar_arrive(&empty[prev]);
             }
+            prev = slot;
+            if (++slot == nstage) { slot = 0; ph ^= 1; }
         }
-    } else {
-        const int q = warp & 3, r = q * 32 + lane, half = (warp - 2) >> 2;
-        const uint32_t tl = tmem + ((uint32_t)(q * 32) << 16);
-        const int nchunk = NT / 16, cbeg = half ? (nchunk + 1) / 2 : 0, cend = half ? nchunk : (nchunk + 1) / 2;
-        uint32_t use[2] = {0, 0}, it = 0;
-        for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++it) {
-            const int br = tile / tiles_per_branch, rem = tile % tiles_per_branch;
-            const int mt = rem / a.ntiles_n, nt = rem % a.ntiles_n;
-            const int rib = mt * 128 + r;                              // row inside the branch
-            const bool valid = rib < a.rows_per_branch;
-            const int zb = rib / a.Tp, tt = rib % a.Tp;
-            const int z = br * a.B + zb;
-            const size_t grow = (size_t)br * a.rows_per_branch + rib;
-            const int buf = it & 1;
-            const int n0 = nt * NT;
-            float mean = 0.f, rstd = 1.f;
-            if (EPI == EPI5_GLN_RES && valid) {
-                const double su = a.stats_in[2 * z], sq = a.stats_in[2 * z + 1];
-                const double mu = su / a.count_in, var = sq / a.count_in - mu * mu;
-                mean = (float)mu;
-                rstd = (float)(1.0 / sqrt((var > 0 ? var : 0) + 1e-8));
-            }
-            const float slope = (EPI == EPI5_PRELU_STATS) ? __ldg(a.prelu[br]) : 0.f;
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(&empty[prev]);
+        wgmma_fence_regs(acc);
+
+        // ---- epilogue on the accumulator fragment: rows rl[h] of the tile, column pairs n0 + 8 j + 2 (lane % 4) ----
+        const int n0 = nt * NT, cq = 2 * (lane & 3);
+        int rib[2], z[2], tt[2];
+        bool valid[2];
+        size_t grow[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            rib[h] = mt * 128 + wg * 64 + wi * 16 + (lane >> 2) + 8 * h;         // row inside the branch
+            valid[h] = rib[h] < a.rows_per_branch;
+            z[h] = br * a.B + rib[h] / a.Tp;
+            tt[h] = rib[h] % a.Tp;
+            grow[h] = (size_t)br * a.rows_per_branch + rib[h];
+        }
+        // rows of this warp: rib0 .. rib0 + 15 of the branch, nvalid of them exist
+        const int rib0 = mt * 128 + wg * 64 + wi * 16;
+        const int nvalid = a.rows_per_branch - rib0;
+        __half* gbase = a.Y16 + ((size_t)br * a.rows_per_branch + rib0) * a.ldY + n0;
+        if constexpr (EPI == EPI5_F16OUT) {
+            uint32_t hp[NT / 8][2];
+#pragma unroll
+            for (int j = 0; j < NT / 8; ++j)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) hp[j][h] = pack_half2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+            g5_store_f16<NT>(stg, lane, hp, gbase, a.ldY, nvalid);
+        } else if constexpr (EPI == EPI5_PRELU_STATS) {
+            const float slope = __ldg(a.prelu[br]);
+            const float* bias = a.bias[br];
             // fp16 store scale of the hidden activation: a power of two from the absolute maximum of this sample's input stream (the
             // normalised real / imaginary branches reach 1e5 and beyond -- 1 / mean(real) is unbounded); undone exactly by the gLN that follows
-            const float ysc = (EPI == EPI5_PRELU_STATS && valid) ? fp16_store_scale(__ldg(a.amax_in + z)) : 1.f;
-            float rowmax = 0.f;
+            float ysc[2], ls[2] = {0.f, 0.f}, lq[2] = {0.f, 0.f};
+            uint32_t hp[NT / 8][2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) ysc[h] = valid[h] ? fp16_store_scale(__ldg(a.amax_in + z[h])) : 1.f;
+#pragma unroll
+            for (int j = 0; j < NT / 8; ++j) {
+                const int n = n0 + 8 * j + cq;
+                const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + n));
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    float y[2];
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        float t = acc[4 * j + 2 * h + e] + (e ? b2.y : b2.x);
+                        t = (t >= 0.f) ? t : slope * t;
+                        ls[h] += t; lq[h] = fmaf(t, t, lq[h]);
+                        y[e] = fminf(fmaxf(t * ysc[h], -65504.f), 65504.f);
+                    }
+                    hp[j][h] = pack_half2(y[0], y[1]);
+                }
+            }
+            g5_store_f16<NT>(stg, lane, hp, gbase, a.ldY, nvalid);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) g5_stats_add(valid[h] ? z[h] : -1, (double)ls[h], (double)lq[h], a.stats_out);
+        } else if constexpr (EPI == EPI5_GLN_RES) {
             const float* bias = a.bias[br];
             const float* s1 = a.s1[br];
-            double lsum = 0.0, lsq = 0.0;
-            // coalesced I/O of this warp's 32 rows (see g5_store_rows64): row 0 of the warp, rows valid, staging tile
-            uint8_t* stg = stg_all + (warp - 2) * G5_STG_BYTES;
-            const size_t wrow0 = (size_t)br * a.rows_per_branch + (size_t)mt * 128 + q * 32;
-            int nvalid = a.rows_per_branch - (mt * 128 + q * 32);
-            nvalid = nvalid < 0 ? 0 : (nvalid > 32 ? 32 : nvalid);
-            // GLN_RES: the residual of the first two chunks does not depend on the MMAs -- in flight while this warp waits for the accumulator
-            // (the loads miss to HBM; with one chunk ahead the 4-5 chunks of a warp were a chain of dependent DRAM round trips)
-            uint4 gA[4], gB[4];
-            const uint8_t* xbase = (EPI == EPI5_GLN_RES) ? reinterpret_cast<const uint8_t*>(a.Xold + wrow0 * a.ldY + n0) : nullptr;
-            if (EPI == EPI5_GLN_RES) {
-                if (cbeg < cend) g5_load_rows64_issue(lane, xbase + (size_t)cbeg * 64, (size_t)a.ldY * sizeof(float), nvalid, gA);
-                if (cbeg + 1 < cend) g5_load_rows64_issue(lane, xbase + (size_t)(cbeg + 1) * 64, (size_t)a.ldY * sizeof(float), nvalid, gB);
-            }
-            mbar_wait(&accfull[buf], use[buf] & 1);
-            ++use[buf];
-            tc5_fence_after();
-            if (EPI == EPI5_PRELU_STATS) {
-                // two 16-column chunks per pass: 32 fp16 values = 64 bytes per row
-                const size_t pitch = (size_t)a.ldY * sizeof(__half);
-                for (int c = cbeg; c < cend; c += 2) {
-                    uint32_t v[32];
-                    tmem_ld16(tl + buf * 256 + c * 16, *reinterpret_cast<uint32_t(*)[16]>(&v[0]));
-                    tmem_ld16(tl + buf * 256 + c * 16 + 16, *reinterpret_cast<uint32_t(*)[16]>(&v[16]));
-                    tmem_wait_ld();
-                    const int n = n0 + c * 16;
-                    float ls = 0.f, lq = 0.f;
-                    uint32_t hp[16];
+            float mean[2] = {0.f, 0.f}, rstd[2] = {1.f, 1.f}, rowmax[2] = {0.f, 0.f};
 #pragma unroll
-                    for (int i4 = 0; i4 < 8; ++i4) {
-                        const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias + n) + i4);
-                        const float bv[4] = {b4.x, b4.y, b4.z, b4.w};
-                        float y[4];
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            float t = __uint_as_float(v[4 * i4 + e]) + bv[e];
-                            t = (t >= 0.f) ? t : slope * t;
-                            ls += t; lq = fmaf(t, t, lq);
-                            y[e] = fminf(fmaxf(t * ysc, -65504.f), 65504.f);
-                        }
-                        hp[2 * i4] = pack_half2(y[0], y[1]);
-                        hp[2 * i4 + 1] = pack_half2(y[2], y[3]);
-                    }
-                    lsum += (double)ls; lsq += (double)lq;
-                    const uint4 ov[4] = {make_uint4(hp[0], hp[1], hp[2], hp[3]), make_uint4(hp[4], hp[5], hp[6], hp[7]),
-                                         make_uint4(hp[8], hp[9], hp[10], hp[11]), make_uint4(hp[12], hp[13], hp[14], hp[15])};
-                    g5_store_rows64(stg, lane, ov, reinterpret_cast<uint8_t*>(a.Y16 + wrow0 * a.ldY + n), pitch, nvalid);
+            for (int h = 0; h < 2; ++h)
+                if (valid[h]) {
+                    const double su = a.stats_in[2 * z[h]], sq = a.stats_in[2 * z[h] + 1];
+                    const double mu = su / a.count_in, var = sq / a.count_in - mu * mu;
+                    mean[h] = (float)mu;
+                    rstd[h] = (float)(1.0 / sqrt((var > 0 ? var : 0) + 1e-8));
                 }
-            } else if (EPI == EPI5_GLN_RES) {
-                const size_t pitch = (size_t)a.ldY * sizeof(float);
-                uint4 xcur[4];
-                if (cbeg < cend) g5_load_rows64_commit(stg, lane, gA, xcur);
-                auto chunk = [&](int c) {
-                    uint32_t v[16];
-                    tmem_ld16(tl + buf * 256 + c * 16, v);
-                    tmem_wait_ld();
-                    const int n = n0 + c * 16;
-                    uint4 ov[4], orl[4];
 #pragma unroll
-                    for (int i4 = 0; i4 < 4; ++i4) {
-                        const float xa[4] = {__uint_as_float(xcur[i4].x), __uint_as_float(xcur[i4].y), __uint_as_float(xcur[i4].z), __uint_as_float(xcur[i4].w)};
-                        const float4 s14 = __ldg(reinterpret_cast<const float4*>(s1 + n) + i4), b4 = __ldg(reinterpret_cast<const float4*>(bias + n) + i4);
-                        const float s1v[4] = {s14.x, s14.y, s14.z, s14.w}, bv[4] = {b4.x, b4.y, b4.z, b4.w};
-                        float o[4];
+            for (int j = 0; j < NT / 8; ++j) {
+                const int n = n0 + 8 * j + cq;
+                if (n >= a.Npad) continue;                            // past the channels of this branch (the tile overhangs)
+                const float2 s12 = __ldg(reinterpret_cast<const float2*>(s1 + n)), b2 = __ldg(reinterpret_cast<const float2*>(bias + n));
 #pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const float val = fmaf(rstd, __uint_as_float(v[i4 * 4 + e]), fmaf(-mean * rstd, s1v[e], bv[e]));
-                            o[e] = xa[e] + val;
-                            if (valid) rowmax = fmaxf(rowmax, fabsf(o[e]));
-                        }
-                        ov[i4] = make_uint4(__float_as_uint(o[0]), __float_as_uint(o[1]), __float_as_uint(o[2]), __float_as_uint(o[3]));
-                        orl[i4] = make_uint4(__float_as_uint(fmaxf(o[0], 0.f)), __float_as_uint(fmaxf(o[1], 0.f)), __float_as_uint(fmaxf(o[2], 0.f)),
-                                             __float_as_uint(fmaxf(o[3], 0.f)));
-                    }
-                    g5_store_rows64(stg, lane, ov, reinterpret_cast<uint8_t*>(a.Y + wrow0 * a.ldY + n), pitch, nvalid);
-                    if (a.Xrelu) g5_store_rows64(stg, lane, orl, reinterpret_cast<uint8_t*>(a.Xrelu + wrow0 * a.ldY + n), pitch, nvalid);
-                };
-                // chunks in pairs over two register buffers: every residual load is issued two chunk-times before it is needed
-                for (int c = cbeg; c < cend; c += 2) {
-                    if (c + 2 < cend) g5_load_rows64_issue(lane, xbase + (size_t)(c + 2) * 64, pitch, nvalid, gA);
-                    chunk(c);
-                    if (c + 1 < cend) {
-                        g5_load_rows64_commit(stg, lane, gB, xcur);
-                        if (c + 3 < cend) g5_load_rows64_issue(lane, xbase + (size_t)(c + 3) * 64, pitch, nvalid, gB);
-                        chunk(c + 1);
-                        if (c + 2 < cend) g5_load_rows64_commit(stg, lane, gA, xcur);
-                    }
-                }
-            } else {
-                for (int c = cbeg; c < cend; ++c) {
-                    uint32_t v[16];
-                    tmem_ld16(tl + buf * 256 + c * 16, v);
-                    tmem_wait_ld();
-                    const int n = n0 + c * 16;
-                    if (a.out_tm) {
-                        // time-major output [(branch, b, t), Npad]: the layout the sub-band LSTM's x-tile builders read (k_lstm_tc5d.cu)
-                        // (pad columns: zero weights, zero bias)
-                        uint4 ov[4];
-#pragma unroll
-                        for (int i4 = 0; i4 < 4; ++i4) {
-                            const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias + n) + i4);
-                            ov[i4] = make_uint4(__float_as_uint(apply_act(__uint_as_float(v[4 * i4]) + b4.x, a.act)), __float_as_uint(apply_act(__uint_as_float(v[4 * i4 + 1]) + b4.y, a.act)),
-                                                __float_as_uint(apply_act(__uint_as_float(v[4 * i4 + 2]) + b4.z, a.act)), __float_as_uint(apply_act(__uint_as_float(v[4 * i4 + 3]) + b4.w, a.act)));
-                        }
-                        g5_store_rows64(stg, lane, ov, reinterpret_cast<uint8_t*>(a.out_tm + wrow0 * a.ldY + n), (size_t)a.ldY * sizeof(float), nvalid);
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) {
-                            if (valid && n + i < a.F)
-                                a.out[((size_t)z * a.F + n + i) * a.P + tt] = apply_act(__uint_as_float(v[i]) + __ldg(bias + n + i), a.act);
-                        }
-                    }
+                for (int h = 0; h < 2; ++h) {
+                    if (!valid[h]) continue;
+                    const float2 x = *reinterpret_cast<const float2*>(a.Xold + grow[h] * a.ldY + n);
+                    float2 o;
+                    o.x = x.x + fmaf(rstd[h], acc[4 * j + 2 * h], fmaf(-mean[h] * rstd[h], s12.x, b2.x));
+                    o.y = x.y + fmaf(rstd[h], acc[4 * j + 2 * h + 1], fmaf(-mean[h] * rstd[h], s12.y, b2.y));
+                    rowmax[h] = fmaxf(rowmax[h], fmaxf(fabsf(o.x), fabsf(o.y)));
+                    *reinterpret_cast<float2*>(a.Y + grow[h] * a.ldY + n) = o;
+                    if (a.Xrelu) *reinterpret_cast<float2*>(a.Xrelu + grow[h] * a.ldY + n) = make_float2(fmaxf(o.x, 0.f), fmaxf(o.y, 0.f));
                 }
             }
-            tc5_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&accempty[buf]);
-            if (EPI == EPI5_GLN_RES && a.amax_out) {      // max |x| of the new stream per sample (max is order-independent: deterministic)
-                const int key = valid ? z : -1;
-                if (__match_any_sync(0xffffffffu, key) == 0xffffffffu) {
+            if (a.amax_out) {                                 // max |x| of the new stream per sample (max is order-independent: deterministic)
 #pragma unroll
-                    for (int o = 16; o; o >>= 1) rowmax = fmaxf(rowmax, __shfl_xor_sync(0xffffffffu, rowmax, o));
-                    if (lane == 0 && valid) atomicMax(reinterpret_cast<int*>(a.amax_out + z), __float_as_int(rowmax));
-                } else if (valid) {
-                    atomicMax(reinterpret_cast<int*>(a.amax_out + z), __float_as_int(rowmax));
-                }
+                for (int h = 0; h < 2; ++h) g5_max_add(valid[h] ? z[h] : -1, rowmax[h], a.amax_out);
             }
-            if (EPI == EPI5_PRELU_STATS) {
-                // rows of a warp almost always belong to one sample: reduce in the warp, one atomic pair per warp
-                const int key = valid ? z : -1;
-                if (__match_any_sync(0xffffffffu, key) == 0xffffffffu) {
-                    lsum = warp_sum_d(lsum); lsq = warp_sum_d(lsq);
-                    if (lane == 0 && valid) { atomicAdd(&a.stats_out[2 * z], lsum); atomicAdd(&a.stats_out[2 * z + 1], lsq); }
-                } else if (valid) {
-                    atomicAdd(&a.stats_out[2 * z], lsum);
-                    atomicAdd(&a.stats_out[2 * z + 1], lsq);
+        } else {
+            const float* bias = a.bias[br];
+#pragma unroll
+            for (int j = 0; j < NT / 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int n = n0 + 8 * j + cq + e;
+                    if (n >= a.F) continue;
+                    const float bv = __ldg(bias + n);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+                        if (valid[h]) a.out[((size_t)z[h] * a.F + n) * a.P + tt[h]] = apply_act(acc[4 * j + 2 * h + e] + bv, a.act);
                 }
-            }
         }
     }
-    tc5_fence_before();
-    __syncthreads();
-    tc5_fence_after();
-    if (warp == 1) tmem_dealloc<512>(tmem);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -353,7 +277,8 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-int make_tmap_f32_2d(void* out_map, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+// row-major [rows, cols] matrix, boxes of box_rows x 128 bytes (32 floats / 64 halves), SWIZZLE_128B
+static int make_tmap_2d(void* out_map, CUtensorMapDataType type, size_t esize, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
     static EncodeTiledFn fn = nullptr;
     if (!fn) {
         void* p = nullptr;
@@ -362,37 +287,66 @@ int make_tmap_f32_2d(void* out_map, const void* base, uint64_t rows, uint64_t co
         fn = reinterpret_cast<EncodeTiledFn>(p);
     }
     const cuuint64_t gdim[2] = {cols, rows};
-    const cuuint64_t gstride[1] = {cols * sizeof(float)};
-    const cuuint32_t box[2] = {32, box_rows};
+    const cuuint64_t gstride[1] = {cols * esize};
+    const cuuint32_t box[2] = {(cuuint32_t)(128 / esize), box_rows};
     const cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(reinterpret_cast<CUtensorMap*>(out_map), CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), gdim, gstride,
+    CUresult r = fn(reinterpret_cast<CUtensorMap*>(out_map), type, 2, const_cast<void*>(base), gdim, gstride,
                     box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS ? 0 : -(int)r;
 }
+int make_tmap_f32_2d(void* out_map, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+    return make_tmap_2d(out_map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, sizeof(float), base, rows, cols, box_rows);
+}
+int make_tmap_f16_2d(void* out_map, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+    return make_tmap_2d(out_map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, sizeof(__half), base, rows, cols, box_rows);
+}
 
-int launch_gemm_tc5(const void* mapA, const void* mapB, GemmTc5Launch a, int num_sms, cudaStream_t s) {
-    const int stage_bytes = G5_A_BYTES + a.NT * 128;
-    a.nstage = (227 * 1024 - 2048 - G5_EPI_WARPS * G5_STG_BYTES) / stage_bytes;
+template <int E, int NT>
+static int g5_launch(const CUtensorMap& mA, const CUtensorMap& mB, GemmTc5Launch a, int num_sms, cudaStream_t s) {
+    const int stage_bytes = G5_A_BYTES + NT * 128;
+    const int stg_bytes = 8 * 16 * NT * 2;                       // fp16 staging tiles of the eight consumer warps
+    a.nstage = (227 * 1024 - 1024 - 256 - stg_bytes) / stage_bytes;
     if (a.nstage > 8) a.nstage = 8;
-    if (a.nstage < 2 || a.NT % 16 || a.NT > 256 || a.Kp % (a.epi == EPI5_GLN_RES ? 64 : 32)) return (int)cudaErrorInvalidValue;
-    if (a.epi == EPI5_PRELU_STATS && a.NT % 64) return (int)cudaErrorInvalidValue;     // its epilogue takes 32 columns per pass and warp half
-    const size_t smem = (size_t)a.nstage * stage_bytes + G5_EPI_WARPS * G5_STG_BYTES + 1024 + 256;
+    const size_t smem = (size_t)a.nstage * stage_bytes + stg_bytes + 1024 + 256;
     const int total = a.nbranch * a.tiles_m * a.ntiles_n;
     const int grid = total < num_sms ? total : num_sms;
+    cudaError_t e = cudaFuncSetAttribute(gemm_tc5_kernel<E, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return (int)e;
+    e = launch_chain(gemm_tc5_kernel<E, NT>, dim3(grid), dim3(G5_THREADS), smem, s, mA, mB, a);
+    if (e != cudaSuccess) return (int)e;
+    return (int)cudaGetLastError();
+}
+
+int launch_gemm_tc5(const void* mapA, const void* mapB, GemmTc5Launch a, int num_sms, cudaStream_t s) {
+    if ((a.NT != 64 && a.NT != 128) || a.Kp % (a.epi == EPI5_GLN_RES ? 64 : 32) || a.Npad % 2) return (int)cudaErrorInvalidValue;
     const CUtensorMap& mA = *reinterpret_cast<const CUtensorMap*>(mapA);
     const CUtensorMap& mB = *reinterpret_cast<const CUtensorMap*>(mapB);
-    cudaError_t e;
-#define G5_LAUNCH(E)                                                                                              \
-    e = cudaFuncSetAttribute(gemm_tc5_kernel<E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);        \
-    if (e != cudaSuccess) return (int)e;                                                                          \
-    e = launch_chain(gemm_tc5_kernel<E>, dim3(grid), dim3(G5_THREADS), smem, s, mA, mB, a);                       \
-    if (e != cudaSuccess) return (int)e;
-    if (a.epi == EPI5_PRELU_STATS) { G5_LAUNCH(EPI5_PRELU_STATS) }
-    else if (a.epi == EPI5_GLN_RES) { G5_LAUNCH(EPI5_GLN_RES) }
-    else { G5_LAUNCH(EPI5_OUT) }
-#undef G5_LAUNCH
-    return (int)cudaGetLastError();
+    if (a.NT == 64) {
+        if (a.epi == EPI5_PRELU_STATS) return g5_launch<EPI5_PRELU_STATS, 64>(mA, mB, a, num_sms, s);
+        if (a.epi == EPI5_GLN_RES) return g5_launch<EPI5_GLN_RES, 64>(mA, mB, a, num_sms, s);
+        return g5_launch<EPI5_OUT, 64>(mA, mB, a, num_sms, s);
+    }
+    if (a.epi == EPI5_PRELU_STATS) return g5_launch<EPI5_PRELU_STATS, 128>(mA, mB, a, num_sms, s);
+    if (a.epi == EPI5_GLN_RES) return g5_launch<EPI5_GLN_RES, 128>(mA, mB, a, num_sms, s);
+    return g5_launch<EPI5_OUT, 128>(mA, mB, a, num_sms, s);
+}
+
+// Input projection of the layer-wise LSTM path: C[M, N] = A[M, K] B[N, K]^T, fp16 operands, fp32 accumulation, fp16 result.
+// reference: the W_ih x_t half of nn.LSTM / nn.GRU (audio_zen/model/module/sequence_model.py:31-46,113-119), batched over all
+// rows and time steps because it has no recurrence.  M = row tiles x frames x 128, N = 4H (a multiple of 256), K = 64 or H.
+bool gemm_f16_supported(long long M, int N, int K) { return M > 0 && M % 128 == 0 && M / 128 < (1LL << 31) / 128 && N % 128 == 0 && K % 64 == 0 && K >= 64; }
+
+int launch_gemm_f16(const void* A, const void* B, const GemmF16Launch& g, int num_sms, cudaStream_t s) {
+    if (!gemm_f16_supported(g.M, g.N, g.K) || g.ldc != g.N) return (int)cudaErrorInvalidValue;
+    alignas(64) CUtensorMap mA, mB;
+    if (make_tmap_f16_2d(&mA, A, (uint64_t)g.M, (uint64_t)g.K, 128) || make_tmap_f16_2d(&mB, B, (uint64_t)g.N, (uint64_t)g.K, 128))
+        return (int)cudaErrorInvalidValue;
+    GemmTc5Launch a{};
+    a.Kp = g.K; a.NT = 128; a.ntiles_n = g.N / 128; a.Npad = g.N;
+    a.rows_per_branch = (int)g.M; a.tiles_m = (int)(g.M / 128); a.nbranch = 1; a.Tp = 1; a.B = 1;
+    a.epi = EPI5_F16OUT; a.Y16 = g.C; a.ldY = g.N;
+    return g5_launch<EPI5_F16OUT, 128>(mA, mB, a, num_sms, s);
 }
 
 // gLN1 apply -> depth-wise conv (k=3, dilation d, zero padding in the normalised domain; causal or symmetric taps) -> PReLU2 + gLN2 statistics,
@@ -418,8 +372,8 @@ __global__ void __launch_bounds__(256) dwconv_tm_kernel(DwTmLaunch a) {
     const float unscale = 1.0f / fp16_store_scale(__ldg(a.amax + z));     // exact: a power of two
     const size_t base = (size_t)z * Tp * C + c0;
     const int cq = threadIdx.x & 15, tr = threadIdx.x >> 4;           // 16 columns of 4 channels x 16 frame rows per pass
-    // per-channel constants: staged once per CTA (64 channels x 6 values) -- as scalar loads per thread they were 85 % of the kernel's
-    // global load requests (ncu, round 2).  Four channels per thread keep the kernel at 4 CTAs per SM (48 registers).
+    // per-channel constants: staged once per CTA (64 channels x 6 values) instead of scalar loads per thread; four channels per thread
+    // keep the register count low enough for several CTAs per SM.
     __shared__ __align__(16) float cst[6][DW_CH];                     // gamma, beta, w0, w1, w2, bias
     if (threadIdx.x < DW_CH) {
         const int ch = c0 + threadIdx.x;

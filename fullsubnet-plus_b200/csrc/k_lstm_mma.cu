@@ -5,7 +5,8 @@
 // (L2 resident), weights are streamed from L2 in mma-fragment order.  Any hidden size that is a
 // multiple of 16 and up to 4 layers are supported, which makes this the kernel behind
 //   * the full-band LSTM of fullsubnet.Model           (reference fullsubnet.py:39-47,86-87)
-//   * sub-band LSTMs outside the tcgen05 kernel's envelope (hidden > 384, 3 layers, tiny test sizes)
+//   * sub-band LSTMs outside the layer-wise wgmma kernel's envelope (hidden not a multiple of 64 or > 512, output_size != 2),
+//     lstm_impl = "mma" and the streaming sub-band step
 // LSTM cell definition: nn.LSTM as used at audio_zen/model/module/sequence_model.py:32-38,118
 // (gate rows i,f,g,o; c = s(f)c + s(i)tanh(g); h = s(o)tanh(c); zero initial state).
 #include "fsn_common.cuh"

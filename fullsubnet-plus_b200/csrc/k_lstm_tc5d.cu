@@ -1,586 +1,14 @@
-// CTA-pair persistent tcgen05 LSTM with DOUBLE-BUFFERED accumulators: the sub-band kernel (its single-CTA and
-// single-accumulator predecessors live in the git history only).  reference: sequence_model.py:113-122, fullsubnet_plus.py:205-208.
-//
-// Why: TMEM is full (h0 192 + h1 192 + one 128-column accumulator = 512 columns), so the pair kernel serialises
-// "MMA chunk j -> drain chunk j -> MMA chunk j+1": ncu shows the tensor pipe 77 % active, the rest is 24 drain bubbles of
-// ~600 cycles per time step.  A 64-column cta_group::2 MMA runs at exactly half the time of a 128-column one when issued in
-// blocks of >= 8 (fsn_probe_tcgen05: 32.1 vs 64.1 cycles), so the 128 accumulator columns are split into TWO 64-column
-// accumulators: every 128-gate-column chunk is computed as two half-chunks, the epilogue warps are split into two sets
-// (set = column group & 1), and the MMAs of one half overlap the drain + cell update of the other.
-//   * half h of a chunk = column groups {h, h + 2}: CTA r of the pair contributes rows [32 h, 32 h + 32) of ITS 64-row
-//     half-tile, i.e. column group 2 r + h -- the packed weight stream is unchanged, only the copy order differs
-//     (per chunk: all k-blocks of half 0, then all k-blocks of half 1; 4 KB sub-blocks, ring slots of up to 4 sub-blocks);
-//   * accumulator h lives at columns [384 + 64 h, 448 + 64 h); column group cg reads accumulator cg & 1 at offset 32 (cg >> 1);
-//   * one accfull / accempty mbarrier pair per accumulator (8 epilogue warps per CTA arrive on each).
-// Everything else (producer / relay / leader-issuer roles, multicast commits, h parked in shared memory until the layer's
-// MMAs are done, cell state through L2, fused output Linear) is the pair kernel's protocol.
+// Host-side packing of the sub-band weight stream (128 gate columns x 64 k SWIZZLE_128B stages in consumption order) and the shared
+// swizzle helper, exposed through the C ABI (include/fsnplus_b200.h) so the packed layouts can be checked on a machine without a GPU.
 #include "fsn_common.cuh"
 #include "fsn_kernels.h"
 #include "../../include/fsnplus_b200.h"
 
 #include <cstring>
 
-namespace fsn {
-
-constexpr int D5_KB = 8192;         // one k-block of my half-tile in the packed stream: 64 of the 128 gate columns x 64 k x fp16
-constexpr int D5_SUB = 4096;        // the 32 gate columns of one half-chunk of it
-constexpr int D5_STAGE = 4 * D5_SUB; // a ring slot holds a GROUP of up to 4 sub-blocks: one mbarrier wait + one commit per 16 N=64 MMAs
-constexpr int D5_STAGE_FULL = 16384;
-constexpr int D5_XIMG = 16384;
-constexpr int D5_EPI_WARPS = 16;
-constexpr int D5_XB_WARPS = 2;                                  // x-tile builders (fused unfold + norm), 64 threads x 2 rows
-constexpr int D5_THREADS = (D5_EPI_WARPS + 2 + D5_XB_WARPS) * 32;
-constexpr int D5_MAX_SMEM = 227 * 1024;
-
-struct D5Plan { int nstage; size_t total; };
-bool lstm_tc5_supported(int L, int H, int I, int O) { return L == 2 && H % 64 == 0 && H >= 64 && H <= 384 && I <= 64 && O == 2; }
-size_t lstm_tc5_cstate_bytes(int ntiles, int H) { return (size_t)ntiles * 2 * H * 128 * sizeof(float); }
-
-static inline D5Plan d5_plan(int H, int S) {
-    D5Plan p;
-    const size_t fixed = D5_XIMG + (size_t)128 * H * 2 /*park*/ + (size_t)2 * 4 * H * 4 /*pre-scaled biases*/ + (size_t)S * 4 * 128 * 2 * 4 /*fc partials*/ + 64 * 8;
-    long avail = D5_MAX_SMEM - 1024 - (long)fixed;
-    p.nstage = (int)(avail / D5_STAGE);
-    if (p.nstage > 8) p.nstage = 8;
-    p.total = fixed + (size_t)p.nstage * D5_STAGE + 1024;
-    return p;
-}
-
-// S > 1: COLUMN-SPLIT mode for small batches (B*F rows fill fewer than half of the SMs).  A cluster holds S CTA pairs that all work on
-// the SAME 256 sequences; pair s computes the gate chunks [s NCH/S, (s+1) NCH/S) of every layer-step (1/S of the MMA stream, of the
-// weight traffic and of the cell updates), the new hidden values are exchanged through distributed shared memory (each epilogue
-// thread stores its 16 bytes into the `park` buffer of the S-1 other CTAs that own the same rows), and every CTA then refills its own
-// tensor-memory copy of h.  The latency of one layer-step drops from ~18 us to ~(18 / S + exchange) us: B = 1 (the only batch size
-// the reference's inferencer issues, base_inferencer.py:65-69) uses 16 SMs instead of 4.
-template <int H, bool FAST, bool GRU, int S>
-__global__ void __cluster_dims__(2 * S, 1, 1) __launch_bounds__(D5_THREADS, 1) lstm_tc5d_kernel(LstmTc5Launch a, int nstage) {
-    extern __shared__ uint8_t smem_raw[];
-    constexpr int NCH = H / 32, KBH = H / 64, hcols = H / 2, NCHS = NCH / S;
-    static_assert(NCH % S == 0, "the gate chunks must split evenly over the pairs of a cluster");
-    const int Tp = a.Tp;
-    const uint32_t crank = cluster_ctarank();
-    const uint32_t rank = crank & 1u, sidx = crank >> 1, lead = crank & ~1u;   // row half, column split, cluster rank of my pair's leader
-    const int tile = (blockIdx.x / (2 * S)) * 2 + (int)rank;
-    const int j0 = (int)sidx * NCHS;                                          // my pair's chunks: [j0, j0 + NCHS)
-    const uint16_t pairmask = (uint16_t)(3u << (2 * sidx));                    // multicast commits go to the two CTAs of my pair
-    const bool leader = (rank == 0);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* stages = smem;
-    uint8_t* ximg = stages + (size_t)nstage * D5_STAGE;
-    uint8_t* park = ximg + D5_XIMG;
-    float* bsm = reinterpret_cast<float*>(park + (size_t)128 * H * 2);       // [2][NCH][128] pre-scaled biases
-    float* fcpart = bsm + 2 * 4 * H;                                         // [S][4][128][2]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(fcpart + S * 4 * 128 * 2);
-    uint64_t* full = bars;
-    uint64_t* empty = full + nstage;
-    uint64_t* xfull = empty + nstage;
-    uint64_t* xempty = xfull + 1;
-    uint64_t* accfull = xempty + 1;                                          // [2]
-    uint64_t* accempty = accfull + 2;                                        // [2]
-    uint64_t* hready = accempty + 2;                                         // [2]: h of layer 0 / layer 1 is in TMEM
-    uint64_t* layerdone = hready + 2;
-    uint64_t* hall = layerdone + 1;                                          // S > 1: the other pairs' h chunks of this layer-step are parked here
-    uint64_t* pfree = hall + 1;                                              // S > 1: the other CTAs have consumed what I parked there last layer-step
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pfree + 1);
-
-    if (tid == 0) {
-        for (int i = 0; i < nstage; ++i) { mbar_init(&full[i], leader ? 2 : 1); mbar_init(&empty[i], 1); }
-        // x image of a step: either ONE bulk copy of a pre-packed image (producer's expect_tx arrive) or built in place by the
-        // D5_XB_WARPS builder warps (one arrive each); the leader additionally gets the peer's relay arrive
-        const uint32_t xarr = a.xs.win ? D5_XB_WARPS : 1;
-        mbar_init(xfull, leader ? xarr + 1 : xarr); mbar_init(xempty, 1);
-        for (int h = 0; h < 2; ++h) { mbar_init(&accfull[h], 1); mbar_init(&accempty[h], D5_EPI_WARPS); }   // 8 warps x 2 CTAs
-        mbar_init(&hready[0], 2 * D5_EPI_WARPS); mbar_init(&hready[1], 2 * D5_EPI_WARPS);
-        mbar_init(layerdone, 1);
-        // hall: a transaction-count barrier -- one local arming arrive per layer-step, completed by the bytes of the other pairs' st.async
-        if (S > 1) { mbar_init(hall, 1); mbar_init(pfree, (S - 1) * D5_EPI_WARPS); }
-        fence_barrier_init();
-    }
-    if (warp == D5_EPI_WARPS + 1) tmem_alloc_pair<512>(tmem_slot);
-    for (int i = tid; i < 2 * 4 * H; i += D5_THREADS) bsm[i] = a.bias[i];
-    tc5_fence_before();
-    __syncthreads();
-    cluster_sync_all();                                            // barriers of both CTAs are initialised
-    tc5_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const uint32_t acc_col = 2 * hcols;
-
-    if (warp == D5_EPI_WARPS) {
-        // ======================= bulk-copy producer (both CTAs, own half) ===================
-        if (lane == 0) {
-            const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.wstream) + (size_t)rank * D5_KB;
-            const uint8_t* xsrc = reinterpret_cast<const uint8_t*>(a.img) + (size_t)tile * Tp * D5_XIMG;
-            int slot = 0; uint32_t ph = 0;
-            const uint64_t pol_x = l2_policy_evict_first(), pol_w = l2_policy_evict_last();
-            const bool packed = (a.xs.win == nullptr);
-            if (packed) {
-                mbar_arrive_expect_tx(xfull, D5_XIMG);
-                bulk_g2s_hint(ximg, xsrc, D5_XIMG, xfull, pol_x);
-            }
-            constexpr int NKB0 = 1 + KBH, NKB1 = 2 * KBH;           // k-blocks per chunk: x | h0, h0 | h1
-            for (int t = 0; t < Tp; ++t) {
-                for (int layer = 0; layer < 2; ++layer) {
-                    const int nkb = layer == 0 ? NKB0 : NKB1;
-                    for (int j = j0; j < j0 + NCHS; ++j) {
-                        const int kb_base = layer == 0 ? j * NKB0 : NCH * NKB0 + j * NKB1;   // k-block index in the per-step stream
-                        for (int half = 0; half < 2; ++half) {
-                            if (packed && layer == 1 && j == j0 + NCHS / 2 && half == 0 && t + 1 < Tp) {     // x_{t+1}: layer 0 of step t is long done
-                                mbar_wait(xempty, t & 1);
-                                mbar_arrive_expect_tx(xfull, D5_XIMG);
-                                bulk_g2s_hint(ximg, xsrc + (size_t)(t + 1) * D5_XIMG, D5_XIMG, xfull, pol_x);
-                            }
-                            for (int kb0 = 0; kb0 < nkb; kb0 += 4) {
-                                const int nk = (nkb - kb0 < 4) ? nkb - kb0 : 4;
-                                mbar_wait(&empty[slot], ph ^ 1);
-                                mbar_arrive_expect_tx(&full[slot], nk * D5_SUB);
-                                for (int i = 0; i < nk; ++i) {
-                                    int kbs = kb0 + i;                      // layer 1: consumed recurrent part (stream k-blocks KBH..) first
-                                    if (layer == 1) kbs = (kbs < KBH) ? KBH + kbs : kbs - KBH;
-                                    bulk_g2s_hint(stages + (size_t)slot * D5_STAGE + i * D5_SUB,
-                                                  wsrc + (size_t)(kb_base + kbs) * D5_STAGE_FULL + half * D5_SUB, D5_SUB, &full[slot], pol_w);
-                                }
-                                if (++slot == nstage) { slot = 0; ph ^= 1; }
-                            }
-                        }
-                    }
-                }
-            }
-        }
-    } else if (warp == D5_EPI_WARPS + 1) {
-        if (leader) {
-            // ======================= MMA issuer for BOTH SMs ===============================
-            // Compile-time chunk / k-block structure, incremental descriptor words, one wait + one commit per group of
-            // up to 8 MMAs: the issue warp must stay below the tensor pipe's 64-74 cycles per instruction.
-            constexpr uint32_t IDESC = umma_idesc_f16(256, 64);
-            constexpr uint32_t DESC_HI = 0x40004040u;              // SBO = 1024 B, version 1, SWIZZLE_128B (umma_desc_sw128)
-            uint32_t d = tmem + acc_col;                           // accumulator of the current half-chunk
-            const uint32_t stage_lo0 = ((smem_u32(stages) >> 4) & 0x3FFFu) | (1u << 16);
-            const uint32_t x_lo = ((smem_u32(ximg) >> 4) & 0x3FFFu) | (1u << 16);
-            int slot = 0; uint32_t ph = 0, accuse = 0, ls = 0;
-            const int nkx = (a.I + 15) >> 4;
-            auto mma_ss = [&](uint32_t a_lo, uint32_t b_lo, uint32_t acc) {
-                asm volatile("{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, %4, 0;\n\tmov.b64 da, {%1, %5};\n\tmov.b64 db, {%2, %5};\n\t"
-                             "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %3, p;\n\t}" ::"r"(d), "r"(a_lo), "r"(b_lo), "r"(IDESC), "r"(acc), "r"(DESC_HI) : "memory");
-            };
-            auto mma_ts = [&](uint32_t a_col, uint32_t b_lo, uint32_t acc) {
-                asm volatile("{\n\t.reg .pred p;\n\t.reg .b64 db;\n\tsetp.ne.b32 p, %4, 0;\n\tmov.b64 db, {%2, %5};\n\t"
-                             "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], db, %3, p;\n\t}" ::"r"(d), "r"(tmem + a_col), "r"(b_lo), "r"(IDESC), "r"(acc), "r"(DESC_HI) : "memory");
-            };
-            // one k-block = 4 MMAs; kbi = index of the k-block inside its chunk (layer 0: 0 = x block, 1.. = h0(t-1); layer 1: h1(t-1)
-            // FIRST, then h0(t): the recurrent half does not depend on the layer-0 epilogue that is still finishing at the boundary)
-            auto kblock = [&](int layer, int kbi, uint32_t b_lo) {
-                if (layer == 0 && kbi == 0) {
-                    // x block: only ceil(I / 16) of the four K = 16 slices hold input columns (I = 34 -> 3); the rest is zero padding
-#pragma unroll
-                    for (int kk = 0; kk < 4; ++kk)
-                        if (kk < nkx) mma_ss(x_lo + 2 * kk, b_lo + 2 * kk, kk != 0);
-                } else {
-                    const uint32_t acol = (layer == 0) ? (kbi - 1) * 32 : (kbi < KBH ? hcols + kbi * 32 : (kbi - KBH) * 32);
-#pragma unroll
-                    for (int kk = 0; kk < 4; ++kk) mma_ts(acol + kk * 8, b_lo + 2 * kk, (kbi | kk) != 0);
-                }
-            };
-            // Dependencies across layer boundaries (one hready barrier per layer; phase 0 of both = the initial zeroing):
-            //   layer 0, step t  reads x(t), h0(t-1): h0(t-1) was awaited by layer 1 of step t-1 -> no wait, the MMAs start while
-            //                    the layer-1 epilogue of step t-1 is still running (it only writes h1 columns);
-            //   layer 1, step t  reads h1(t-1) [hready[1] phase t] from its first MMA and h0(t) [hready[0] phase t+1] from the
-            //                    first h0 k-block of its first half-chunk.
-            mbar_wait(&hready[0], 0);
-            tc5_fence_after();
-            for (int t = 0; t < Tp; ++t) {
-#pragma unroll
-                for (int layer = 0; layer < 2; ++layer, ++ls) {
-                    if (layer == 0) mbar_wait(xfull, t & 1);
-                    else mbar_wait(&hready[1], t & 1);
-                    if (NCHS == 1) {
-                        // One chunk per layer-step: each accumulator is used ONCE per layer-step, so nothing would stop this warp from
-                        // running a whole layer-step ahead of a slow epilogue warp -- `layerdone` would then complete two phases before
-                        // that warp tests the first one and its parity wait could never succeed (found on B200: H = 64 / 128 with S = 2 /
-                        // 4 hung in layer 1).  With >= 2 chunks per layer-step the second use of an accumulator already orders the issuer
-                        // behind every epilogue warp.  Here: do not start layer-step ls before the h of layer-step ls - 1 is in tensor
-                        // memory (all epilogue warps are past their layerdone wait then); the same phases are awaited again below.
-                        if (layer == 0) { if (t > 0) mbar_wait(&hready[1], t & 1); }
-                        else mbar_wait(&hready[0], (t + 1) & 1);
-                    }
-                    tc5_fence_after();
-                    constexpr int NKB0 = 1 + KBH, NKB1 = 2 * KBH;
-                    const int nkb = layer == 0 ? NKB0 : NKB1;
-                    for (int j = j0; j < j0 + NCHS; ++j) {
-#pragma unroll
-                        for (int half = 0; half < 2; ++half) {
-                            mbar_wait(&accempty[half], (accuse & 1) ^ 1);
-                            tc5_fence_after();
-                            d = tmem + acc_col + 64 * half;
-#pragma unroll
-                            for (int kb0 = 0; kb0 < NKB1; kb0 += 4) {
-                                if (kb0 < nkb) {
-                                    mbar_wait(&full[slot], ph);
-                                    tc5_fence_after();
-                                    const uint32_t b_lo = stage_lo0 + slot * (D5_STAGE >> 4);
-                                    if (elect_one()) {
-#pragma unroll
-                                        for (int i = 0; i < 4; ++i)
-                                            if (kb0 + i < nkb) {
-                                                if (layer == 1 && kb0 + i == KBH && j == j0 && half == 0) {   // h0(t) is needed from here on
-                                                    mbar_wait(&hready[0], (t + 1) & 1);
-                                                    tc5_fence_after();
-                                                }
-                                                kblock(layer, kb0 + i, b_lo + i * (D5_SUB >> 4));
-                                            }
-                                        umma2_commit_mc(&empty[slot], pairmask);
-                                        if (kb0 + 4 >= nkb) {
-                                            umma2_commit_mc(&accfull[half], pairmask);
-                                            if (j == j0 + NCHS - 1 && half == 1) {
-                                                if (layer == 0) umma2_commit_mc(xempty, pairmask);
-                                                umma2_commit_mc(layerdone, pairmask);
-                                            }
-                                        }
-                                    }
-                                    __syncwarp();
-                                    if (++slot == nstage) { slot = 0; ph ^= 1; }
-                                }
-                            }
-                        }
-                        ++accuse;
-                    }
-                }
-            }
-        } else {
-            // ======================= peer relay: my half-tiles have landed -> leader ========
-            if (lane == 0) {
-                const uint32_t r_xfull = mapa_u32(smem_u32(xfull), lead);
-                int slot = 0; uint32_t ph = 0;
-                constexpr int NG = 2 * NCHS * ((1 + KBH + 3) / 4 + (2 * KBH + 3) / 4);   // groups per time step (producer loop)
-                for (int t = 0; t < Tp; ++t) {
-                    mbar_wait(xfull, t & 1);
-                    mbar_arrive_remote(r_xfull);
-                    for (int g = 0; g < NG; ++g) {
-                        mbar_wait(&full[slot], ph);
-                        mbar_arrive_remote(mapa_u32(smem_u32(&full[slot]), lead));
-                        if (++slot == nstage) { slot = 0; ph ^= 1; }
-                    }
-                }
-            }
-        }
-    } else if (warp >= D5_EPI_WARPS + 2) {
-        // ======================= x-tile builders: fused BaseModel.unfold + concat + norm ====
-        // reference base_model.py:15-47, fullsubnet_plus.py:167-202 / fullsubnet.py:90-111.  Row (b, f) of step t is
-        //   [ win(b, reflect(f - Ns .. f + Ns), t) | fb_q(b, reflect(f - Nf .. f + Nf), t), q < nfb ] normalised per utterance,
-        // written as fp16 straight into the SWIZZLE_128B image the layer-0 MMAs read -- the 31x unfolded tensor (392 MB in
-        // fp16 at B = 64) is never written to or read from global memory.  Same arithmetic as sb_pack_kernel (k_front.cu).
-        if (a.xs.win) {
-            const XSrc& xs = a.xs;
-            const int rj = (warp - (D5_EPI_WARPS + 2)) * 32 + lane;    // rows rj and rj + 64: lanes <-> consecutive bins (coalesced loads)
-            const int nw = 2 * xs.Ns + 1, nf = 2 * xs.Nf + 1, I = nw + xs.nfb * nf, nchunk = (I + 7) >> 3;
-            const int F = a.F;
-            int rb[2], rf[2];
-            float inv[2], sub[2];
-            bool ok[2];
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                const int grow = tile * 128 + rj + 64 * i;
-                ok[i] = grow < a.rows;
-                rb[i] = ok[i] ? grow / F : 0; rf[i] = ok[i] ? grow % F : 0;
-                const float mu = __ldg(xs.mu + rb[i]);
-                inv[i] = xs.gauss ? 1.0f / (__ldg(xs.sigma + rb[i]) + 1e-5f) : 1.0f / (mu + 1e-5f);
-                sub[i] = xs.gauss ? mu : 0.f;
-                for (int c = 0; c < 8; ++c)                            // columns >= I and rows >= B*F stay zero for the whole launch
-                    *reinterpret_cast<uint4*>(ximg + sw128_offset(rj + 64 * i, c * 8)) = make_uint4(0u, 0u, 0u, 0u);
-            }
-            const uint64_t pol_x = l2_policy_evict_first();          // read (almost) once: must not push the cell-state scratch out of L2
-            auto src = [&](int i, int k, int t) -> const float* {
-                if (k < nw) return xs.win + rb[i] * xs.win_sb + reflect_idx(rf[i] + k - xs.Ns, F) * xs.win_sf + t * xs.win_st;
-                const int kk = k - nw, q = kk / nf, jn = kk - q * nf;
-                const float* base = (q == 0) ? xs.fb[0] : (q == 1) ? xs.fb[1] : xs.fb[2];
-                return base + rb[i] * xs.fb_sb + reflect_idx(rf[i] + jn - xs.Nf, F) * xs.fb_sf + t * xs.fb_st;
-            };
-            for (int t = 0; t < Tp; ++t) {
-                if (t > 0) mbar_wait(xempty, (t - 1) & 1);             // the layer-0 MMAs of step t-1 have read the image
-                for (int c = 0; c < nchunk; ++c) {
-                    float v[2][8];
-#pragma unroll
-                    for (int i = 0; i < 2; ++i)
-#pragma unroll
-                        for (int e = 0; e < 8; ++e) v[i][e] = (ok[i] && c * 8 + e < I) ? ldg_hint(src(i, c * 8 + e, t), pol_x) : 0.f;
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        if (!ok[i]) continue;
-                        float w[8];
-#pragma unroll
-                        for (int e = 0; e < 8; ++e) w[e] = (c * 8 + e < I) ? fminf(fmaxf((v[i][e] - sub[i]) * inv[i], -65504.f), 65504.f) : 0.f;
-                        *reinterpret_cast<uint4*>(ximg + sw128_offset(rj + 64 * i, c * 8)) =
-                            make_uint4(pack_half2(w[0], w[1]), pack_half2(w[2], w[3]), pack_half2(w[4], w[5]), pack_half2(w[6], w[7]));
-                    }
-                }
-                fence_proxy_async();                                   // generic-proxy stores -> visible to the tensor core's async-proxy reads
-                __syncwarp();
-                if (lane == 0) mbar_arrive(xfull);
-            }
-        }
-    } else {
-        // ======================= epilogue warps (both CTAs, own 128 sequences) ==============
-        const int cg = warp >> 2;
-        const int q = warp & 3;
-        const int r = q * 32 + lane;
-        const uint32_t tl = tmem + ((uint32_t)(q * 32) << 16);
-        const int set = cg & 1;                                     // which accumulator / half-chunk this warp serves
-        const uint32_t acc_my = acc_col + 64 * set + 32 * (cg >> 1);
-        uint64_t* my_accfull = &accfull[set];
-        uint64_t* my_accempty = &accempty[set];
-        const uint32_t r_accempty = mapa_u32(smem_u32(my_accempty), lead);
-        const uint32_t r_hready[2] = {mapa_u32(smem_u32(&hready[0]), lead), mapa_u32(smem_u32(&hready[1]), lead)};
-        {
-            const uint32_t z[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-            for (int c = cg; c < 2 * NCH * 2; c += 4) tmem_st8(tl + c * 8, z);
-            tmem_wait_st();
-            tc5_fence_before();
-            __syncwarp();
-            if (lane == 0)
-                for (int l = 0; l < 2; ++l) { if (leader) mbar_arrive(&hready[l]); else mbar_arrive_remote(r_hready[l]); }
-        }
-        uint32_t accn = 0, ls = 0;
-        const uint64_t pol_c = l2_policy_evict_last();               // the fp32 cell state lives in L2 for the whole launch
-        float4 cnext[2] = {make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)};   // t = 0: zero cell state
-        float* cbase = a.cstate + (size_t)tile * 2 * H * 128;
-        uint8_t* mypark = park + ((size_t)cg * NCH * 128 + r) * 16;
-        // S > 1: the same-row CTAs of the other pairs (cluster ranks 2 s' + rank): their park / fc-partial / barrier addresses
-        uint32_t r_park[S > 1 ? S - 1 : 1], r_hall[S > 1 ? S - 1 : 1], r_pfree[S > 1 ? S - 1 : 1];
-        uint32_t r_fcp = 0;
-        if (S > 1) {
-            int n = 0;
-            for (int sp = 0; sp < S; ++sp) {
-                if (sp == (int)sidx) continue;
-                const uint32_t cr = 2 * sp + rank;
-                r_park[n] = mapa_u32(smem_u32(mypark), cr);
-                r_hall[n] = mapa_u32(smem_u32(hall), cr);
-                r_pfree[n] = mapa_u32(smem_u32(pfree), cr);
-                ++n;
-            }
-            r_fcp = mapa_u32(smem_u32(fcpart + ((size_t)(sidx * 4 + cg) * 128 + r) * 2), rank);   // pair 0 (same rows) sums the fc partials
-        }
-        const uint32_t r_hall0 = (S > 1) ? mapa_u32(smem_u32(hall), rank) : 0;                   // pair 0's barrier (fc partials)
-        // bytes the other S - 1 same-row CTAs send me per layer-step: their h chunks (16 B x 128 rows x 4 column groups x NCHS chunks
-        // each), plus -- pair 0, layer 1 -- their Linear(H -> 2) partials (8 B x 128 rows x 4 column groups each)
-        constexpr uint32_t HALL_H = (S - 1) * NCHS * 128 * 4 * 16, HALL_FC = (S - 1) * 128 * 4 * 8;
-        const int grow = tile * 128 + r;
-        const int ob = grow / a.F, of = grow % a.F;
-        const int Tout = Tp - a.la;
-        const float fcb0 = __ldg(a.fc_b), fcb1 = __ldg(a.fc_b + 1);
-
-        for (int t = 0; t < Tp; ++t) {
-            for (int layer = 0; layer < 2; ++layer, ++ls) {
-                float fc0 = 0.f, fc1 = 0.f;
-                float2 nx = make_float2(0.f, 0.f);                 // noisy (re, im) of my output bin, in flight during the chunk loop
-                if (layer == 1 && a.enh && cg == 0 && t >= a.la && grow < a.rows) {
-                    const size_t ni = ((size_t)ob * a.F + of) * Tout + (t - a.la);
-                    nx = make_float2(__ldg(a.nreal + ni), __ldg(a.nimag + ni));
-                }
-                if (S > 1 && warp == 0 && lane == 0)                            // arm this layer-step's phase (the previous one is complete: I waited for it)
-                    mbar_arrive_expect_tx(hall, HALL_H + ((layer == 1 && sidx == 0) ? HALL_FC : 0u));
-                for (int j = j0; j < j0 + NCHS; ++j) {
-                    float4* cp = reinterpret_cast<float4*>(cbase + ((size_t)((layer * NCH + j) * 4 + cg) * 2) * 128 * 4) + r;
-                    const float4 c4[2] = {cnext[0], cnext[1]};     // prefetched during the previous chunk
-                    const float4* bj = reinterpret_cast<const float4*>(bsm + (size_t)(layer * NCH + j) * 128 + cg * 32);
-                    mbar_wait(my_accfull, accn & 1);
-                    ++accn;
-                    tc5_fence_after();
-                    uint32_t v[2][16];
-                    tmem_ld16(tl + acc_my, v[0]);
-                    tmem_ld16(tl + acc_my + 16, v[1]);
-                    tmem_wait_ld();
-                    tc5_fence_before();
-                    __syncwarp();
-                    if (lane == 0) { if (leader) mbar_arrive(my_accempty); else mbar_arrive_remote(r_accempty); }
-                    {   // cell state of the NEXT chunk in program order: (layer, j+1), else chunk 0 of the other layer (next step after layer 1)
-                        const int nj = (j + 1 < j0 + NCHS) ? j + 1 : j0;
-                        const int nl = (j + 1 < j0 + NCHS) ? layer : (layer ^ 1);
-                        const int nt = (j + 1 < j0 + NCHS || layer == 0) ? t : t + 1;
-                        const float4* np = reinterpret_cast<const float4*>(cbase + ((size_t)((nl * NCH + nj) * 4 + cg) * 2) * 128 * 4) + r;
-                        if (nt == 0 || nt >= Tp) { cnext[0] = make_float4(0.f, 0.f, 0.f, 0.f); cnext[1] = cnext[0]; }
-                        else { cnext[0] = ld_f4_hint(np, pol_c); cnext[1] = ld_f4_hint(np + 128, pol_c); }
-                    }
-
-                    const float L2E = 1.4426950408889634f;
-                    uint32_t hp[4];
-                    float cn[8];
-#pragma unroll
-                    for (int u4 = 0; u4 < 2; ++u4) {
-                        const float4 bi = bj[u4], bf = bj[2 + u4], bg = bj[4 + u4], bo = bj[6 + u4];
-                        const float bia[4] = {bi.x, bi.y, bi.z, bi.w}, bfa[4] = {bf.x, bf.y, bf.z, bf.w};
-                        const float bga[4] = {bg.x, bg.y, bg.z, bg.w}, boa[4] = {bo.x, bo.y, bo.z, bo.w};
-                        const float cpv[4] = {c4[u4].x, c4[u4].y, c4[u4].z, c4[u4].w};
-                        float hv[4];
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const int u = u4 * 4 + e;
-                            if (GRU) {
-                                gru_cell<FAST>(fmaf(__uint_as_float(v[0][u]), -L2E, bia[e]), fmaf(__uint_as_float(v[0][8 + u]), -L2E, bfa[e]),
-                                               fmaf(__uint_as_float(v[1][u]), -2.f * L2E, bga[e]), fmaf(__uint_as_float(v[1][8 + u]), -2.f * L2E, boa[e]),
-                                               cpv[e], hv[e]);
-                                cn[u] = hv[e];
-                            } else {
-                                lstm_cell<FAST>(fmaf(__uint_as_float(v[0][u]), -L2E, bia[e]), fmaf(__uint_as_float(v[0][8 + u]), -L2E, bfa[e]),
-                                                fmaf(__uint_as_float(v[1][u]), -2.f * L2E, bga[e]), fmaf(__uint_as_float(v[1][8 + u]), -L2E, boa[e]),
-                                                cpv[e], cn[u], hv[e]);
-                            }
-                        }
-                        if (layer == 1) {
-                            const float4 wa = __ldg(reinterpret_cast<const float4*>(a.fc_w + j * 32 + cg * 8) + u4);
-                            const float4 wb = __ldg(reinterpret_cast<const float4*>(a.fc_w + H + j * 32 + cg * 8) + u4);
-                            fc0 = fmaf(hv[0], wa.x, fmaf(hv[1], wa.y, fmaf(hv[2], wa.z, fmaf(hv[3], wa.w, fc0))));
-                            fc1 = fmaf(hv[0], wb.x, fmaf(hv[1], wb.y, fmaf(hv[2], wb.z, fmaf(hv[3], wb.w, fc1))));
-                        }
-                        hp[2 * u4] = pack_half2(hv[0], hv[1]);
-                        hp[2 * u4 + 1] = pack_half2(hv[2], hv[3]);
-                    }
-                    st_f4_hint(cp, make_float4(cn[0], cn[1], cn[2], cn[3]), pol_c);
-                    st_f4_hint(cp + 128, make_float4(cn[4], cn[5], cn[6], cn[7]), pol_c);
-                    // S > 1: what I parked remotely last layer-step must have been consumed before I overwrite it -- waited for as late as
-                    // possible (after the drain and the cell math of the first chunk), so the other pairs' tails overlap my epilogue
-                    if (S > 1 && ls > 0 && j == j0) mbar_wait_cluster(pfree, (ls - 1) & 1);
-                    *reinterpret_cast<uint4*>(mypark + (size_t)j * 128 * 16) = make_uint4(hp[0], hp[1], hp[2], hp[3]);
-                    if (S > 1) {
-#pragma unroll
-                        for (int n = 0; n < S - 1; ++n) st_async_v4(r_park[n] + (uint32_t)j * 128 * 16, make_uint4(hp[0], hp[1], hp[2], hp[3]), r_hall[n]);
-                    }
-                }
-                if (S > 1) {
-                    if (layer == 1) {                              // my pair's share of Linear(H -> 2): summed by pair 0 after the exchange
-                        if (sidx == 0) { fcpart[((size_t)cg * 128 + r) * 2] = fc0; fcpart[((size_t)cg * 128 + r) * 2 + 1] = fc1; }
-                        else st_async_v2f(r_fcp, fc0, fc1, r_hall0);
-                    }
-                }
-                mbar_wait(layerdone, ls & 1);
-                if (S > 1) mbar_wait_cluster(hall, ls & 1);        // every other pair's chunks of this layer-step are in my park buffer
-                tc5_fence_after();
-                for (int j = 0; j < NCH; ++j) {
-                    const uint4 p0 = *reinterpret_cast<const uint4*>(mypark + (size_t)j * 128 * 16);
-                    const uint32_t hv[4] = {p0.x, p0.y, p0.z, p0.w};
-                    tmem_st4(tl + layer * hcols + j * 16 + cg * 4, hv);
-                }
-                tmem_wait_st();
-                tc5_fence_before();
-                __syncwarp();
-                if (lane == 0) { if (leader) mbar_arrive(&hready[layer]); else mbar_arrive_remote(r_hready[layer]); }
-
-                if (layer == 1) {
-                    if (S == 1 && cg != 0) { fcpart[(cg * 128 + r) * 2] = fc0; fcpart[(cg * 128 + r) * 2 + 1] = fc1; }
-                    asm volatile("bar.sync 1, 512;" ::: "memory");
-                    if (cg == 0 && t >= a.la && grow < a.rows && sidx == 0) {
-                        float o0 = fcb0, o1 = fcb1;
-                        if (S == 1) {
-                            o0 += fc0 + fcpart[(128 + r) * 2] + fcpart[(256 + r) * 2] + fcpart[(384 + r) * 2];
-                            o1 += fc1 + fcpart[(128 + r) * 2 + 1] + fcpart[(256 + r) * 2 + 1] + fcpart[(384 + r) * 2 + 1];
-                        } else {
-#pragma unroll
-                            for (int i = 0; i < 4 * S; ++i) { o0 += fcpart[((size_t)i * 128 + r) * 2]; o1 += fcpart[((size_t)i * 128 + r) * 2 + 1]; }
-                        }
-                        if (a.enh) {                                   // fused decompress_cIRM x noisy spectrum (inferencer.py:152-157)
-                            const float m0 = decompress_cirm(apply_act(o0, a.act)), m1 = decompress_cirm(apply_act(o1, a.act));
-                            __stcs(a.enh + ((size_t)ob * a.F + of) * Tout + (t - a.la), make_float2(m0 * nx.x - m1 * nx.y, m1 * nx.x + m0 * nx.y));
-                        } else {
-                            __stcs(&a.out[(((size_t)ob * 2 + 0) * a.F + of) * Tout + (t - a.la)], apply_act(o0, a.act));   // streaming stores: written once
-                            __stcs(&a.out[(((size_t)ob * 2 + 1) * a.F + of) * Tout + (t - a.la)], apply_act(o1, a.act));
-                        }
-                    }
-                    asm volatile("bar.sync 2, 512;" ::: "memory");
-                }
-                if (S > 1) {                                       // park (and, after layer 1, the fc partials) of this layer-step are consumed
-                    __syncwarp();
-                    if (lane == 0) {
-#pragma unroll
-                        for (int n = 0; n < S - 1; ++n) mbar_arrive_remote(r_pfree[n]);
-                    }
-                }
-            }
-        }
-    }
-    tc5_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    tc5_fence_after();
-    if (warp == D5_EPI_WARPS + 1) tmem_dealloc_pair<512>(tmem);
-}
-
-// column split for small batches: S = 6 (12-CTA clusters, one per GPC) for up to 8 row-tile pairs, S = 4 (8-CTA clusters, two per GPC)
-// for up to 16, when S divides the chunk count; a.split forces a value (0 = auto)
-static int d5_pick_split(int H, int npairs, int forced) {
-    const int nch = H / 32;
-    if (forced == 1 || forced == 2 || forced == 4 || forced == 6) return (nch % forced == 0) ? forced : 1;
-    if (nch % 6 == 0 && npairs <= 8) return 6;           // 12-CTA clusters (non-portable size, one per GPC): B <= 7 at F = 257
-    if (nch % 4 == 0 && npairs <= 16) return 4;          // measured (B200, H = 384): 18.3 -> 10.3 us per layer-step; S = 2 does not pay
-    return 1;                                            // (19.9 us: the exchange costs as much as half the MMA stream saves)
-}
-
-template <int HH, bool FF, bool GG, int SS>
-static int d5_go(const LstmTc5Launch& a, int npairs, cudaStream_t s) {
-    const D5Plan p = d5_plan(HH, SS);
-    if (p.nstage < 2) return (int)cudaErrorInvalidValue;
-    cudaError_t e = cudaFuncSetAttribute(lstm_tc5d_kernel<HH, FF, GG, SS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.total);
-    if (e != cudaSuccess) return (int)e;
-    if (2 * SS > 8) {                                               // clusters of more than 8 CTAs are an opt-in on sm_100 (up to 16)
-        e = cudaFuncSetAttribute(lstm_tc5d_kernel<HH, FF, GG, SS>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-        if (e != cudaSuccess) { cudaGetLastError(); return -1; }
-        static int max_clusters = -1;                               // how many such clusters the device can hold at once (one CTA per SM)
-        if (max_clusters < 0) {
-            cudaLaunchConfig_t cfg = {};
-            cfg.gridDim = dim3(2 * SS, 1, 1); cfg.blockDim = dim3(D5_THREADS, 1, 1); cfg.dynamicSmemBytes = p.total;
-            cudaLaunchAttribute attr;
-            attr.id = cudaLaunchAttributeClusterDimension;
-            attr.val.clusterDim.x = 2 * SS; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
-            cfg.attrs = &attr; cfg.numAttrs = 1;
-            int n = 0;
-            if (cudaOccupancyMaxActiveClusters(&n, lstm_tc5d_kernel<HH, FF, GG, SS>, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
-            max_clusters = n;
-        }
-        if (max_clusters < npairs) return -1;                       // caller falls back to the next smaller split
-    }
-    lstm_tc5d_kernel<HH, FF, GG, SS><<<npairs * 2 * SS, D5_THREADS, p.total, s>>>(a, p.nstage);
-    return (int)cudaGetLastError();
-}
-template <int HH, int SS>
-static int d5_dispatch(const LstmTc5Launch& a, int npairs, cudaStream_t s) {
-    if (a.gru) return a.fast ? d5_go<HH, true, true, SS>(a, npairs, s) : d5_go<HH, false, true, SS>(a, npairs, s);
-    return a.fast ? d5_go<HH, true, false, SS>(a, npairs, s) : d5_go<HH, false, false, SS>(a, npairs, s);
-}
-template <int HH>
-static int d5_split(const LstmTc5Launch& a, int npairs, int S, cudaStream_t s) {
-    constexpr int nch = HH / 32;
-    if constexpr (nch % 6 == 0) {
-        if (S == 6) {
-            const int rc = d5_dispatch<HH, 6>(a, npairs, s);
-            if (rc != -1) return rc;                                // -1: the 12-CTA clusters do not fit this device / batch -> S = 4 or 1
-            S = (nch % 4 == 0 && npairs <= 16) ? 4 : 1;
-        }
-    }
-    if constexpr (nch % 4 == 0) { if (S == 4) return d5_dispatch<HH, 4>(a, npairs, s); }
-    if constexpr (nch % 2 == 0) { if (S == 2) return d5_dispatch<HH, 2>(a, npairs, s); }
-    return d5_dispatch<HH, 1>(a, npairs, s);
-}
-
-int launch_lstm_tc5_dbuf(const LstmTc5Launch& a, cudaStream_t s) {
-    if (!lstm_tc5_supported(2, a.H, a.I, 2)) return (int)cudaErrorInvalidValue;
-    const int npairs = (a.ntiles + 1) / 2;                          // whole pairs; the buffers cover the padded tile
-    const int S = d5_pick_split(a.H, npairs, a.split);
-    switch (a.H) {
-        case 64: return d5_split<64>(a, npairs, S, s);
-        case 128: return d5_split<128>(a, npairs, S, s);
-        case 192: return d5_split<192>(a, npairs, S, s);
-        case 256: return d5_split<256>(a, npairs, S, s);
-        case 320: return d5_split<320>(a, npairs, S, s);
-        case 384: return d5_split<384>(a, npairs, S, s);
-    }
-    return (int)cudaErrorInvalidValue;
-}
-
-int lstm_tc5_split_for(int H, int ntiles, int forced) { return d5_pick_split(H, (ntiles + 1) / 2, forced); }
-
-}  // namespace fsn
+static constexpr int kStage = 16384;      // one stage: 128 gate columns x 64 k x fp16
 
 // ---------------------------------------------------------------------------------------------
-// Host-side packing of the weight stream (exposed through the C ABI for CPU layout tests).
 // Stream order per time step: layer 0, chunk j = 0..H/32-1: [x block][H/64 hidden blocks];
 //                             layer 1, chunk j:              [H/64 blocks of W_ih1][H/64 blocks of W_hh1].
 // Stage = 128 gate columns (fsn_tc5_gate_row) x 64 k, K-major, SWIZZLE_128B.
@@ -595,35 +23,44 @@ static inline uint16_t d5_h_bits(float f) {
 extern "C" int64_t fsn_tc5_weight_stream_bytes(int32_t I, int32_t H) {
     if (H % 64 || I > 64) return -1;
     const int NCH = H / 32, KBH = H / 64;
-    return (int64_t)(NCH * (1 + KBH) + NCH * 2 * KBH) * fsn::D5_STAGE_FULL;
+    return (int64_t)(NCH * (1 + KBH) + NCH * 2 * KBH) * kStage;
 }
 
 // Gate column n (0..127) of chunk j <-> weight row: n = cg*32 + q*8 + u, q in (i,f,g,o), hidden unit 32 j + 8 cg + u.
 extern "C" int32_t fsn_tc5_gate_row(int32_t H, int32_t j, int32_t n) { return ((n % 32) / 8) * H + 32 * j + 8 * (n / 32) + (n % 8); }
 
+// one stage: 128 gate columns of chunk j x 64 k, getw(n, k)
+template <class G> static void pack_stage(uint16_t* dst, size_t s, G&& getw) {
+    uint8_t* img = reinterpret_cast<uint8_t*>(dst) + s * kStage;
+    for (int n = 0; n < 128; ++n)
+        for (int k = 0; k < 64; ++k) {
+            uint16_t b = d5_h_bits(getw(n, k));
+            std::memcpy(img + fsn::sw128_offset(n, k), &b, 2);
+        }
+}
+
+// Layer-0 section of the stream, [x block][H/64 hidden blocks] per chunk: also the weight stream of the layer-wise kernel's first
+// layer, whose input projection is part of the recurrence (k_lstm_tc5r.cu).
+void fsn::lstm_tc5_pack_first_layer(int I, int H, const float* w_ih0, const float* w_hh0, uint16_t* dst) {
+    const int NCH = H / 32, KBH = H / 64;
+    size_t s = 0;
+    for (int j = 0; j < NCH; ++j) {
+        auto row = [&](int n) { return fsn_tc5_gate_row(H, j, n); };
+        pack_stage(dst, s++, [&](int n, int k) { return k < I ? w_ih0[(size_t)row(n) * I + k] : 0.f; });
+        for (int kb = 0; kb < KBH; ++kb) pack_stage(dst, s++, [&](int n, int k) { return w_hh0[(size_t)row(n) * H + kb * 64 + k]; });
+    }
+}
+
 extern "C" int fsn_tc5_pack_weights(int32_t I, int32_t H, const float* w_ih0, const float* w_hh0, const float* w_ih1,
                                     const float* w_hh1, uint16_t* dst) {
     if (H % 64 || I > 64) return FSN_EINVAL;
     const int NCH = H / 32, KBH = H / 64;
-    size_t s = 0;
-    auto stage = [&](auto&& getw) {
-        uint8_t* img = reinterpret_cast<uint8_t*>(dst) + s * fsn::D5_STAGE_FULL;
-        for (int n = 0; n < 128; ++n)
-            for (int k = 0; k < 64; ++k) {
-                uint16_t b = d5_h_bits(getw(n, k));
-                std::memcpy(img + fsn::sw128_offset(n, k), &b, 2);
-            }
-        ++s;
-    };
+    fsn::lstm_tc5_pack_first_layer(I, H, w_ih0, w_hh0, dst);
+    size_t s = (size_t)NCH * (1 + KBH);
     for (int j = 0; j < NCH; ++j) {
         auto row = [&](int n) { return fsn_tc5_gate_row(H, j, n); };
-        stage([&](int n, int k) { return k < I ? w_ih0[(size_t)row(n) * I + k] : 0.f; });
-        for (int kb = 0; kb < KBH; ++kb) stage([&](int n, int k) { return w_hh0[(size_t)row(n) * H + kb * 64 + k]; });
-    }
-    for (int j = 0; j < NCH; ++j) {
-        auto row = [&](int n) { return fsn_tc5_gate_row(H, j, n); };
-        for (int kb = 0; kb < KBH; ++kb) stage([&](int n, int k) { return w_ih1[(size_t)row(n) * H + kb * 64 + k]; });
-        for (int kb = 0; kb < KBH; ++kb) stage([&](int n, int k) { return w_hh1[(size_t)row(n) * H + kb * 64 + k]; });
+        for (int kb = 0; kb < KBH; ++kb) pack_stage(dst, s++, [&](int n, int k) { return w_ih1[(size_t)row(n) * H + kb * 64 + k]; });
+        for (int kb = 0; kb < KBH; ++kb) pack_stage(dst, s++, [&](int n, int k) { return w_hh1[(size_t)row(n) * H + kb * 64 + k]; });
     }
     return FSN_OK;
 }

@@ -1,18 +1,25 @@
-// Single-layer recurrent tcgen05 kernel for stacked LSTMs / GRUs OUTSIDE the fused two-layer kernel's envelope
-// (k_lstm_tc5d.cu: exactly 2 layers, hidden <= 384 -- h of both layers plus the accumulators fill the 512 TMEM columns).
-// BASELINE config #5 (sub-band hidden 512, 3 layers; reference sequence_model.py:31-38,113-122) is the motivating case.
+// Single-layer recurrent LSTM / GRU kernel on the Hopper tensor cores (wgmma): the sub-band model of every stack the project
+// runs (reference sequence_model.py:31-46,113-122; BASELINE configs #1 and #5).
 //
 // Decomposition (the classic time-batched split, one layer at a time):
 //   gates_l(t) = W_ih_l x_l(t) + W_hh_l h_l(t-1) + b
-//   * the input projection has no recurrence: Gin_l = X_l W_ih_l^T is ONE plain GEMM over all rows and all time steps
-//     (cuBLAS, fp16 in / fp32 accumulate / fp16 out; fsn_api.cu), its gate columns pre-permuted to this kernel's chunk order;
-//   * this kernel runs the recurrence of one layer for all time steps: h_l in tensor memory (H/2 columns, packed fp16, the
-//     A operand of tcgen05.mma), W_hh_l streamed from L2 through a bulk-copy ring, four 64-column accumulators, the epilogue
-//     adds Gin_l(t) to the accumulator, does the cell update and either writes h_l(t) as the next layer's GEMM input
-//     (fp16, row-major) or, on the last layer, applies the output Linear(H -> 2) and writes the mask.
-// TMEM: H/2 + 256 <= 512 columns (four 64-column accumulators), i.e. H <= 512; h(t) is parked in shared memory until the step's MMAs are
-// done (parking it in its global output row instead, to deepen the weight ring from 5 to 12 slots, was tried: 4.34 -> 4.80 ms).  Roles, CTA pairs (cta_group::2), multicast commits, half-chunk double buffering and the relay protocol are those
-// of k_lstm_tc5d.cu; the per-step dependency (every MMA of step t reads h(t-1)) is inherent to a single layer.
+//   * the first layer's input is 64 wide: its projection is part of the recurrence -- every step the 64 x 64 input tile (the swizzled
+//     image of k_front.cu's packer) is one more k-block of the A operand, W_ih one more k-block in front of every gate chunk of the
+//     stream (lstm_tc5_pack_first_layer);
+//   * deeper layers' input projection has no recurrence: Gin_l = X_l W_ih_l^T is ONE GEMM over all rows and all time steps
+//     (launch_gemm_f16, k_gemm_tc5.cu: fp16 in / fp32 accumulate / fp16 out), its gate columns pre-permuted to the order this
+//     kernel's threads read them in (lstm_tc5r_gin_order);
+//   * this kernel runs the recurrence of one layer for all time steps.  A CTA owns 64 sequences: h(t-1) lives in shared memory
+//     (fp16, the swizzled K-major A operand of wgmma, double-buffered by step parity), W_hh streams from L2 through a ring of
+//     16 KB k-blocks (128 gate columns x 64 k).  The two CTAs of a cluster share the stream: each fetches half of every k-block
+//     and multicasts it to both, so the L2 reads W_hh once per 128 sequences.  Two consumer warpgroups take the 128-column
+//     gate chunks in turn (m64n128k16, accumulator in registers): while one runs its cell update the other's MMAs are in
+//     flight.  Each warpgroup has a ring of its own, consumed strictly in order (a shared ring would let one warpgroup wait on a
+//     slot two phases ahead, which an mbarrier parity wait cannot tell from the phase before).  The epilogue adds Gin_l(t), does
+//     the cell update and writes h_l(t) both into the next step's A buffer and, for all but the last layer, as the next layer's
+//     GEMM input (fp16, row-major); the last layer applies the output Linear(H -> 2) and writes the mask (or the enhanced spectrum).
+// Gate chunk j, column n = cg * 32 + q * 8 + u: gate q (i, f, g, o / GRU pseudo-gates r, z, n_x, n_h) of hidden unit
+// 32 j + 8 cg + u (fsn_tc5_gate_row), so every thread's accumulator fragment holds all four gates of its units.
 #include "fsn_common.cuh"
 #include "fsn_kernels.h"
 #include "../../include/fsnplus_b200.h"
@@ -22,307 +29,245 @@
 
 namespace fsn {
 
-constexpr int R5_KB = 8192;          // one k-block of my half-tile in the packed stream: 64 of the 128 gate columns x 64 k x fp16
-constexpr int R5_SUB = 4096;         // the 32 gate columns of one half-chunk of it
-constexpr int R5_STAGE = 4 * R5_SUB;  // ring slot: up to 4 sub-blocks = 16 N=64 MMAs per wait / commit
-constexpr int R5_STAGE_FULL = 16384;
-constexpr int R5_EPI_WARPS = 16;
-constexpr int R5_THREADS = (R5_EPI_WARPS + 2) * 32;
+constexpr int R5_STAGE = 16384;                 // one k-block of one chunk of the packed stream: 128 gate columns x 64 k x fp16
+constexpr int R5_CL = 2;                        // CTAs per cluster sharing the weight stream
+constexpr int R5_ROWS = 64;                     // sequences per CTA
+constexpr int R5_THREADS = 9 * 32;              // warps 0-7: two consumer warpgroups; warp 8: bulk-copy producer
 constexpr int R5_MAX_SMEM = 227 * 1024;
+constexpr int R5_XTILE = R5_ROWS * 128;         // one step's input tile of a CTA: 64 rows x 64 halves, SWIZZLE_128B
 
 struct R5Plan { int nstage; size_t total; };
 static inline R5Plan r5_plan(int H) {
     R5Plan p;
-    const size_t fixed = (size_t)128 * H * 2 /*park*/ + (size_t)4 * H * 4 /*pre-scaled biases*/ + 4 * 128 * 2 * 4 /*fc partials*/ + 64 * 8;
-    long avail = R5_MAX_SMEM - 1024 - (long)fixed;
-    p.nstage = (int)(avail / R5_STAGE);
+    const size_t fixed = (size_t)2 * R5_ROWS * H * 2 /*h, two step parities*/ + 2 * R5_XTILE /*input tiles*/ + 2 * 2 * R5_ROWS * 2 * 4 /*fc partials*/ +
+                         1024 /*align*/ + 256;
+    const long avail = R5_MAX_SMEM - (long)fixed;
+    p.nstage = (int)(avail / R5_STAGE) & ~1;                        // two rings of nstage / 2 slots, one per consumer warpgroup
     if (p.nstage > 8) p.nstage = 8;
-    p.total = fixed + (size_t)(p.nstage > 0 ? p.nstage : 0) * R5_STAGE + 1024;
+    p.total = fixed + (size_t)(p.nstage > 0 ? p.nstage : 0) * R5_STAGE;
     return p;
 }
 
 bool lstm_tc5r_supported(int H, int O) { return H % 64 == 0 && H >= 64 && H <= 512 && O == 2; }
 size_t lstm_tc5r_cstate_bytes(int ntiles, int H) { return (size_t)((ntiles + 1) / 2 * 2) * H * 128 * sizeof(float); }
-int64_t lstm_tc5r_weight_stream_bytes(int H) { return (int64_t)(H / 32) * (H / 64) * R5_STAGE_FULL; }
+int64_t lstm_tc5r_weight_stream_bytes(int H) { return (int64_t)(H / 32) * (H / 64) * R5_STAGE; }
 
 template <int H, bool FAST, bool GRU, bool LAST>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(R5_THREADS, 1) lstm_tc5r_kernel(LstmTc5rLaunch a, int nstage) {
+__global__ void __cluster_dims__(R5_CL, 1, 1) __launch_bounds__(R5_THREADS, 1) lstm_tc5r_kernel(LstmTc5rLaunch a, int nstage) {
     extern __shared__ uint8_t smem_raw[];
-    constexpr int NCH = H / 32, KBH = H / 64, hcols = H / 2;
-    constexpr int NG = (KBH + 3) / 4;                               // ring groups per half-chunk
+    constexpr int NCH = H / 32, KBH = H / 64, HBUF = KBH * R5_ROWS * 128;
     const int Tp = a.Tp;
-    const int tile = blockIdx.x;
+    const int cta = blockIdx.x;
     const uint32_t rank = cluster_ctarank();
-    const bool leader = (rank == 0);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* stages = smem;
-    uint8_t* park = stages + (size_t)nstage * R5_STAGE;
-    float* bsm = reinterpret_cast<float*>(park + (size_t)128 * H * 2);       // [NCH][128] pre-scaled biases
-    float* fcpart = bsm + 4 * H;                                             // [4][128][2]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(fcpart + 4 * 128 * 2);
-    uint64_t* full = bars;
+    uint8_t* hbuf = stages + (size_t)nstage * R5_STAGE;                     // [2][KBH][64 rows][128 B], SWIZZLE_128B
+    uint8_t* xbuf = hbuf + 2 * HBUF;                                       // [2 step parities][R5_XTILE] input tiles (first layer)
+    float* fcpart = reinterpret_cast<float*>(xbuf + 2 * R5_XTILE);         // [2 step parities][64 rows][2]
+    uint64_t* full = reinterpret_cast<uint64_t*>(fcpart + 2 * R5_ROWS * 2);   // [2 rings][nstage / 2]
     uint64_t* empty = full + nstage;
-    // FOUR 64-column accumulators (two per half-chunk, alternating with the chunk parity): TMEM has H/2 + 256 <= 512 columns to give, and
-    // with only two the issuer stalled whenever one epilogue set was late -- tensor pipe 43 % at H = 512 (profiles/r02_layerwise_c5_ncu.txt)
-    uint64_t* accfull = empty + nstage;                                      // [4]: index 2 * (chunk & 1) + half
-    uint64_t* accempty = accfull + 4;                                        // [4]
-    uint64_t* hready = accempty + 4;                                         // h(t) is in TMEM (phase 0: the initial zeroing)
-    uint64_t* stepdone = hready + 1;                                         // every MMA of the step has retired
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(stepdone + 1);
+    uint64_t* xfull = empty + nstage;                                      // [2]: input tile of the step parity landed
+    uint64_t* xempty = xfull + 2;                                          // [2]: every MMA of the step that read it has retired
+    const int KX = a.ximg ? 1 : 0, KT = KX + KBH;                          // k-blocks per gate chunk: [input][hidden]
 
     if (tid == 0) {
-        for (int i = 0; i < nstage; ++i) { mbar_init(&full[i], leader ? 2 : 1); mbar_init(&empty[i], 1); }
-        for (int h = 0; h < 4; ++h) { mbar_init(&accfull[h], 1); mbar_init(&accempty[h], R5_EPI_WARPS); }   // 8 warps x 2 CTAs
-        mbar_init(hready, 2 * R5_EPI_WARPS);
-        mbar_init(stepdone, 1);
+        for (int i = 0; i < nstage; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 4 * R5_CL); }
+        for (int i = 0; i < 2; ++i) { mbar_init(&xfull[i], 1); mbar_init(&xempty[i], 1); }
         fence_barrier_init();
     }
-    if (warp == R5_EPI_WARPS + 1) tmem_alloc_pair<512>(tmem_slot);
-    for (int i = tid; i < 4 * H; i += R5_THREADS) bsm[i] = a.bias[i];
-    tc5_fence_before();
+    for (int i = tid; i < HBUF / 16; i += R5_THREADS) reinterpret_cast<uint4*>(hbuf)[i] = make_uint4(0, 0, 0, 0);   // h(-1) = 0
+    fence_proxy_async();
     __syncthreads();
-    cluster_sync_all();                                            // barriers of both CTAs are initialised
-    tc5_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const uint32_t acc_col = hcols;
+    cluster_sync_all();                                                    // barriers of both CTAs are initialised
 
-    if (warp == R5_EPI_WARPS) {
-        // ======================= bulk-copy producer (both CTAs, own half of every weight tile) ===================
+    if (warp == 8) {
+        // ======================= producer: my half of every k-block, multicast to both CTAs ===================
         if (lane == 0) {
-            const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.wstream) + (size_t)rank * R5_KB;
-            int slot = 0; uint32_t ph = 0;
-            const uint64_t pol_w = l2_policy_evict_last();          // 2 MB of W_hh, re-read every step by every pair: must survive the Gin stream
-            for (int t = 0; t < Tp; ++t)
-                for (int j = 0; j < NCH; ++j)
-                    for (int half = 0; half < 2; ++half)
-                        for (int kb0 = 0; kb0 < KBH; kb0 += 4) {
-                            const int nk = (KBH - kb0 < 4) ? KBH - kb0 : 4;
-                            mbar_wait(&empty[slot], ph ^ 1);
-                            mbar_arrive_expect_tx(&full[slot], nk * R5_SUB);
-                            for (int i = 0; i < nk; ++i)
-                                bulk_g2s_hint(stages + (size_t)slot * R5_STAGE + i * R5_SUB,
-                                              wsrc + (size_t)(j * KBH + kb0 + i) * R5_STAGE_FULL + half * R5_SUB, R5_SUB, &full[slot], pol_w);
-                            if (++slot == nstage) { slot = 0; ph ^= 1; }
-                        }
-        }
-    } else if (warp == R5_EPI_WARPS + 1) {
-        if (leader) {
-            // ======================= MMA issuer for BOTH SMs ===============================
-            constexpr uint32_t IDESC = umma_idesc_f16(256, 64);
-            constexpr uint32_t DESC_HI = 0x40004040u;              // SBO = 1024 B, version 1, SWIZZLE_128B (umma_desc_sw128)
-            uint32_t d = tmem + acc_col;
-            const uint32_t stage_lo0 = ((smem_u32(stages) >> 4) & 0x3FFFu) | (1u << 16);
-            int slot = 0; uint32_t ph = 0, accuse = 0;               // accuse: chunks issued so far (each accumulator is used every second chunk)
-            auto mma_ts = [&](uint32_t a_col, uint32_t b_lo, uint32_t acc) {
-                asm volatile("{\n\t.reg .pred p;\n\t.reg .b64 db;\n\tsetp.ne.b32 p, %4, 0;\n\tmov.b64 db, {%2, %5};\n\t"
-                             "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], db, %3, p;\n\t}" ::"r"(d), "r"(tmem + a_col), "r"(b_lo), "r"(IDESC), "r"(acc), "r"(DESC_HI) : "memory");
-            };
+            constexpr uint32_t PART = R5_STAGE / R5_CL;
+            const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.wstream) + rank * PART;
+            const uint64_t pol_w = l2_policy_evict_last();          // the weights, re-read every step by every cluster: must survive the Gin stream
+            const int NS = nstage / 2;
+            int slot[2] = {0, 0}; uint32_t ph[2] = {0, 0};
             for (int t = 0; t < Tp; ++t) {
-                mbar_wait(hready, t & 1);                          // h(t-1) of both CTAs is in tensor memory
-                tc5_fence_after();
-                for (int j = 0; j < NCH; ++j) {
-#pragma unroll
-                    for (int half = 0; half < 2; ++half) {
-                        const int ai = 2 * (j & 1) + half;
-                        mbar_wait(&accempty[ai], ((accuse >> 1) & 1) ^ 1);
-                        tc5_fence_after();
-                        d = tmem + acc_col + 64 * ai;
-#pragma unroll
-                        for (int kb0 = 0; kb0 < KBH; kb0 += 4) {
-                            mbar_wait(&full[slot], ph);
-                            tc5_fence_after();
-                            const uint32_t b_lo = stage_lo0 + slot * (R5_STAGE >> 4);
-                            if (elect_one()) {
-#pragma unroll
-                                for (int i = 0; i < 4; ++i)
-                                    if (kb0 + i < KBH) {
-#pragma unroll
-                                        for (int kk = 0; kk < 4; ++kk)
-                                            mma_ts((kb0 + i) * 32 + kk * 8, b_lo + i * (R5_SUB >> 4) + 2 * kk, ((kb0 + i) | kk) != 0);
-                                    }
-                                umma2_commit_mc(&empty[slot], 3);
-                                if (kb0 + 4 >= KBH) {
-                                    umma2_commit_mc(&accfull[ai], 3);
-                                    if (j == NCH - 1 && half == 1) umma2_commit_mc(stepdone, 3);
-                                }
-                            }
-                            __syncwarp();
-                            if (++slot == nstage) { slot = 0; ph ^= 1; }
-                        }
-                    }
-                    ++accuse;
+                if (KX) {                                           // my 64 rows of the step's input image
+                    mbar_wait(&xempty[t & 1], ((t >> 1) & 1) ^ 1);
+                    mbar_arrive_expect_tx(&xfull[t & 1], R5_XTILE);
+                    bulk_g2s(xbuf + (t & 1) * R5_XTILE, reinterpret_cast<const uint8_t*>(a.ximg) + (((size_t)(cta >> 1) * Tp + t) * 128 + (cta & 1) * R5_ROWS) * 128,
+                             R5_XTILE, &xfull[t & 1]);
                 }
-            }
-        } else {
-            // ======================= peer relay: my half-tiles have landed -> leader ========
-            if (lane == 0) {
-                int slot = 0; uint32_t ph = 0;
-                const long total = (long)Tp * NCH * 2 * NG;
-                for (long g = 0; g < total; ++g) {
-                    mbar_wait(&full[slot], ph);
-                    mbar_arrive_remote(mapa_u32(smem_u32(&full[slot]), 0));
-                    if (++slot == nstage) { slot = 0; ph ^= 1; }
+                for (int j = 0; j < NCH; ++j) {
+                    const int r = j & 1, base = r * NS;             // chunk j goes to the ring of warpgroup j % 2
+                    for (int q = 0; q < KT; ++q) {
+                        const int i = base + slot[r];
+                        mbar_wait(&empty[i], ph[r] ^ 1);
+                        mbar_arrive_expect_tx(&full[i], R5_STAGE);
+                        bulk_g2s_multicast(stages + (size_t)i * R5_STAGE + rank * PART, wsrc + (size_t)(j * KT + q) * R5_STAGE, PART, &full[i],
+                                           (uint16_t)((1u << R5_CL) - 1), pol_w);
+                        if (++slot[r] == NS) { slot[r] = 0; ph[r] ^= 1; }
+                    }
                 }
             }
         }
     } else {
-        // ======================= epilogue warps (both CTAs, own 128 sequences) ==============
-        const int cg = warp >> 2;
-        const int q = warp & 3;
-        const int r = q * 32 + lane;
-        const uint32_t tl = tmem + ((uint32_t)(q * 32) << 16);
-        const int set = cg & 1;                                     // which accumulator / half-chunk this warp serves
-        const uint32_t acc_my0 = acc_col + 64 * set + 32 * (cg >> 1);          // + 128 for odd chunks
-        const uint32_t r_accempty0 = mapa_u32(smem_u32(&accempty[set]), 0), r_accempty1 = mapa_u32(smem_u32(&accempty[2 + set]), 0);
-        const uint32_t r_hready = mapa_u32(smem_u32(hready), 0);
-        {
-            const uint32_t z[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-            for (int c = cg; c < hcols / 8; c += 4) tmem_st8(tl + c * 8, z);
-            tmem_wait_st();
-            tc5_fence_before();
-            __syncwarp();
-            if (lane == 0) { if (leader) mbar_arrive(hready); else mbar_arrive_remote(r_hready); }
+        // ======================= consumers: warpgroup wg takes the chunks j = wg, wg + 2, ... =================
+        const int wg = warp >> 2, wi = warp & 3, wt = tid & 127, cq = 2 * (lane & 3);
+        int rl[2], grow[2];
+        size_t mrow0[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            rl[h] = wi * 16 + (lane >> 2) + 8 * h;
+            grow[h] = cta * R5_ROWS + rl[h];
+            mrow0[h] = (size_t)(cta >> 1) * Tp * 128 + (cta & 1) * R5_ROWS + rl[h];     // + t * 128: row of the (tile, t) block of Gin / hseq
         }
-        uint32_t accn = 0;
-        float4 cnext[2] = {make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)};   // t = 0: zero cell state
-        float* cbase = a.cstate + (size_t)tile * H * 128;
-        uint8_t* mypark = park + ((size_t)cg * NCH * 128 + r) * 16;
-        const int grow = tile * 128 + r;
-        const int ob = grow / a.F, of = grow % a.F;
         const int Tout = Tp - a.la;
-        const float fcb0 = LAST ? __ldg(a.fc_b) : 0.f, fcb1 = LAST ? __ldg(a.fc_b + 1) : 0.f;
-
-        // Gin of the NEXT chunk is loaded one chunk ahead (64 bytes per thread at a 4 KB row pitch: the loads take longer than one
-        // half-chunk of MMAs, so issuing them only before the accumulator wait left the epilogue waiting for memory)
-        // L2 policies: Gin (6.5 GB per layer at config #5) is read exactly once -> evict_first, so that it does not push the weight
-        // stream and the cell state (evict_last) out of L2
-        const uint64_t pol_g = l2_policy_evict_first(), pol_c = l2_policy_evict_last();
-        uint4 gn[4];
-        {
-            const uint4* g0p = reinterpret_cast<const uint4*>(a.gin + (((size_t)tile * Tp) * 128 + r) * (size_t)(4 * H) + cg * 32);
-            gn[0] = ldg_u4_hint(g0p, pol_g); gn[1] = ldg_u4_hint(g0p + 1, pol_g); gn[2] = ldg_u4_hint(g0p + 2, pol_g); gn[3] = ldg_u4_hint(g0p + 3, pol_g);
-        }
+        const float L2E = 1.4426950408889634f;
+        float* cbase = a.cstate + (size_t)cta * NCH * 4 * 128 * 4;
+        float acc[64];
+        const bool has_gin = a.gin != nullptr;
+        const int NS = nstage / 2;
+        int rslot = 0; uint32_t rph = 0;                            // position in this warpgroup's ring (slots wg * NS ..)
         for (int t = 0; t < Tp; ++t) {
-            const size_t mrow = ((size_t)tile * Tp + t) * 128 + r;  // my row of the (tile, t) block of Gin / hseq
-            const uint4* gsrc = reinterpret_cast<const uint4*>(a.gin + mrow * (size_t)(4 * H) + cg * 32);
-            float fc0 = 0.f, fc1 = 0.f;
-            float2 nx = make_float2(0.f, 0.f);                     // noisy (re, im) of my output bin, in flight during the chunk loop
-            if (LAST && a.enh && cg == 0 && t >= a.la && grow < a.rows) {
-                const size_t ni = ((size_t)ob * a.F + of) * Tout + (t - a.la);
-                nx = make_float2(__ldg(a.nreal + ni), __ldg(a.nimag + ni));
-            }
-            for (int j = 0; j < NCH; ++j) {
-                float4* cp = reinterpret_cast<float4*>(cbase + ((size_t)(j * 4 + cg) * 2) * 128 * 4) + r;
-                const float4 c4[2] = {cnext[0], cnext[1]};         // prefetched during the previous chunk
-                const float4* bj = reinterpret_cast<const float4*>(bsm + (size_t)j * 128 + cg * 32);
-                // input projection of this chunk: 32 halves = i(8) f(8) g(8) o(8) of my 8 hidden units; in flight during the wait below
-                const uint4 g0 = gn[0], g1 = gn[1], g2 = gn[2], g3 = gn[3];
-                {   // prefetch: chunk j + 1 of this step, or chunk 0 of the next step (one 128-row block further)
-                    const uint4* np = (j + 1 < NCH) ? gsrc + (j + 1) * 16 : gsrc + (size_t)128 * (4 * H) / 8;
-                    if (j + 1 < NCH || t + 1 < Tp) {
-                        gn[0] = ldg_u4_hint(np, pol_g); gn[1] = ldg_u4_hint(np + 1, pol_g); gn[2] = ldg_u4_hint(np + 2, pol_g); gn[3] = ldg_u4_hint(np + 3, pol_g);
+            const uint8_t* hA = hbuf + (size_t)(t & 1) * HBUF;
+            uint8_t* hN = hbuf + (size_t)((t + 1) & 1) * HBUF;
+            float fc0[2] = {0.f, 0.f}, fc1[2] = {0.f, 0.f};
+            for (int j = wg; j < NCH; j += 2) {
+                // input projection, cell state and biases of this chunk: in flight while the MMAs run
+                // (Gin columns of a chunk are in lane-quad order, lstm_tc5r_gin_order: the 32 values of my row are 64 contiguous bytes;
+                // word cg * 4 + q holds gate q of units cq, cq + 1 of column group cg)
+                uint32_t gw[2][16] = {};
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    if (!has_gin) break;
+                    const uint4* gp = reinterpret_cast<const uint4*>(a.gin + (mrow0[h] + (size_t)t * 128) * (size_t)(4 * H) + j * 128 + (lane & 3) * 32);
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        const uint4 v = __ldcs(gp + i);
+                        gw[h][4 * i] = v.x; gw[h][4 * i + 1] = v.y; gw[h][4 * i + 2] = v.z; gw[h][4 * i + 3] = v.w;
                     }
                 }
-                const int ai = 2 * (j & 1) + set;
-                const uint32_t acc_my = acc_my0 + 128 * (j & 1);
-                mbar_wait(&accfull[ai], (accn >> 1) & 1);
-                ++accn;
-                tc5_fence_after();
-                uint32_t v[2][16];
-                tmem_ld16(tl + acc_my, v[0]);
-                tmem_ld16(tl + acc_my + 16, v[1]);
-                tmem_wait_ld();
-                tc5_fence_before();
-                __syncwarp();
-                if (lane == 0) { if (leader) mbar_arrive(&accempty[ai]); else mbar_arrive_remote((j & 1) ? r_accempty1 : r_accempty0); }
-                {   // cell state of the next chunk in program order
-                    const int nj = (j + 1 < NCH) ? j + 1 : 0;
-                    const int nt = (j + 1 < NCH) ? t : t + 1;
-                    const float4* np = reinterpret_cast<const float4*>(cbase + ((size_t)(nj * 4 + cg) * 2) * 128 * 4) + r;
-                    if (nt == 0 || nt >= Tp) { cnext[0] = make_float4(0.f, 0.f, 0.f, 0.f); cnext[1] = cnext[0]; }
-                    else { cnext[0] = ld_f4_hint(np, pol_c); cnext[1] = ld_f4_hint(np + 128, pol_c); }
+                float4 c4[4];
+                float4* cp = reinterpret_cast<float4*>(cbase + (size_t)j * 4 * 128 * 4) + wt;
+#pragma unroll
+                for (int v = 0; v < 4; ++v) c4[v] = (t == 0) ? make_float4(0.f, 0.f, 0.f, 0.f) : __ldcg(cp + v * 128);
+
+                if (KX && j == wg) mbar_wait(&xfull[t & 1], (uint32_t)(t >> 1) & 1u);    // the step's input tile
+                int prev = -1;
+#pragma unroll 1
+                for (int kb = 0; kb < KT; ++kb) {
+                    const int slot = wg * NS + rslot;
+                    mbar_wait(&full[slot], rph);
+                    if (++rslot == NS) { rslot = 0; rph ^= 1; }
+                    wgmma_fence();
+                    const uint8_t* ablk = (kb < KX) ? xbuf + (t & 1) * R5_XTILE : hA + (kb - KX) * R5_ROWS * 128;
+                    const uint64_t adesc = wgmma_desc_sw128(smem_u32(ablk));
+                    const uint64_t bdesc = wgmma_desc_sw128(smem_u32(stages + (size_t)slot * R5_STAGE));
+#pragma unroll
+                    for (int kk = 0; kk < 4; ++kk) wgmma_f16_n128(acc, adesc + 2 * kk, bdesc + 2 * kk, (kb | kk) != 0);
+                    wgmma_commit();
+                    if (prev >= 0) {
+                        wgmma_wait<1>();
+                        if (lane == 0)
+                            for (uint32_t r = 0; r < R5_CL; ++r) mbar_arrive_cluster(mapa_u32(smem_u32(&empty[prev]), r));
+                    }
+                    prev = slot;
                 }
-                const uint32_t gw[16] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w, g2.x, g2.y, g2.z, g2.w, g3.x, g3.y, g3.z, g3.w};
-                const float L2E = 1.4426950408889634f;
-                uint32_t hp[4];
-                float cn[8];
+                wgmma_wait<0>();
+                if (lane == 0)
+                    for (uint32_t r = 0; r < R5_CL; ++r) mbar_arrive_cluster(mapa_u32(smem_u32(&empty[prev]), r));
+                wgmma_fence_regs(acc);
+
+                // cell update: thread holds rows rl[h], units 32 j + 8 cg + cq + e, all four gates (accumulator column block 4 cg + q)
+                float cn[16];
 #pragma unroll
-                for (int u4 = 0; u4 < 2; ++u4) {
-                    const float4 bi = bj[u4], bf = bj[2 + u4], bg = bj[4 + u4], bo = bj[6 + u4];
-                    const float bia[4] = {bi.x, bi.y, bi.z, bi.w}, bfa[4] = {bf.x, bf.y, bf.z, bf.w};
-                    const float bga[4] = {bg.x, bg.y, bg.z, bg.w}, boa[4] = {bo.x, bo.y, bo.z, bo.w};
-                    const float cpv[4] = {c4[u4].x, c4[u4].y, c4[u4].z, c4[u4].w};
-                    float hv[4];
+                for (int cg = 0; cg < 4; ++cg) {
+                    float bq[4][2];
 #pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const int u = u4 * 4 + e;
-                        // half u of gate q sits in word q * 4 + u / 2 of the 16 loaded words
-                        auto gin = [&](int qg) {
-                            const __half2 h2 = *reinterpret_cast<const __half2*>(&gw[qg * 4 + (u >> 1)]);
-                            return (u & 1) ? __high2float(h2) : __low2float(h2);
-                        };
-                        const float ai = __uint_as_float(v[0][u]) + gin(0), af = __uint_as_float(v[0][8 + u]) + gin(1);
-                        const float ag = __uint_as_float(v[1][u]) + gin(2), ao = __uint_as_float(v[1][8 + u]) + gin(3);
-                        if (GRU) {
-                            gru_cell<FAST>(fmaf(ai, -L2E, bia[e]), fmaf(af, -L2E, bfa[e]), fmaf(ag, -2.f * L2E, bga[e]), fmaf(ao, -2.f * L2E, boa[e]),
-                                           cpv[e], hv[e]);
-                            cn[u] = hv[e];
-                        } else {
-                            lstm_cell<FAST>(fmaf(ai, -L2E, bia[e]), fmaf(af, -L2E, bfa[e]), fmaf(ag, -2.f * L2E, bga[e]), fmaf(ao, -L2E, boa[e]),
-                                            cpv[e], cn[u], hv[e]);
+                    for (int q = 0; q < 4; ++q) {
+                        const float2 b2 = __ldg(reinterpret_cast<const float2*>(a.bias + j * 128 + cg * 32 + q * 8 + cq));
+                        bq[q][0] = b2.x; bq[q][1] = b2.y;
+                    }
+                    const int u0 = j * 32 + cg * 8 + cq;
+                    float hv[2][2];
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            auto pre = [&](int q) {
+                                const __half2 g2 = *reinterpret_cast<const __half2*>(&gw[h][cg * 4 + q]);
+                                return acc[4 * (4 * cg + q) + 2 * h + e] + (has_gin ? (e ? __high2float(g2) : __low2float(g2)) : 0.f);
+                            };
+                            const int v = h * 8 + cg * 2 + e;
+                            const float cprev = reinterpret_cast<const float*>(c4)[v];
+                            if (GRU) {
+                                gru_cell<FAST>(fmaf(pre(0), -L2E, bq[0][e]), fmaf(pre(1), -L2E, bq[1][e]), fmaf(pre(2), -2.f * L2E, bq[2][e]),
+                                               fmaf(pre(3), -2.f * L2E, bq[3][e]), cprev, hv[h][e]);
+                                cn[v] = hv[h][e];
+                            } else {
+                                lstm_cell<FAST>(fmaf(pre(0), -L2E, bq[0][e]), fmaf(pre(1), -L2E, bq[1][e]), fmaf(pre(2), -2.f * L2E, bq[2][e]),
+                                                fmaf(pre(3), -L2E, bq[3][e]), cprev, cn[v], hv[h][e]);
+                            }
+                        }
+                    float2 w0 = make_float2(0.f, 0.f), w1 = w0;
+                    if (LAST) {
+                        w0 = __ldg(reinterpret_cast<const float2*>(a.fc_w + u0));
+                        w1 = __ldg(reinterpret_cast<const float2*>(a.fc_w + H + u0));
+                    }
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const uint32_t hp = pack_half2(hv[h][0], hv[h][1]);
+                        *reinterpret_cast<uint32_t*>(hN + (u0 >> 6) * R5_ROWS * 128 + sw128_offset(rl[h], u0 & 63)) = hp;
+                        if (!LAST) *reinterpret_cast<uint32_t*>(a.hseq + (mrow0[h] + (size_t)t * 128) * H + u0) = hp;   // next layer's GEMM input
+                        if (LAST) {
+                            fc0[h] = fmaf(hv[h][0], w0.x, fmaf(hv[h][1], w0.y, fc0[h]));
+                            fc1[h] = fmaf(hv[h][0], w1.x, fmaf(hv[h][1], w1.y, fc1[h]));
                         }
                     }
-                    if (LAST) {
-                        const float4 wa = __ldg(reinterpret_cast<const float4*>(a.fc_w + j * 32 + cg * 8) + u4);
-                        const float4 wb = __ldg(reinterpret_cast<const float4*>(a.fc_w + H + j * 32 + cg * 8) + u4);
-                        fc0 = fmaf(hv[0], wa.x, fmaf(hv[1], wa.y, fmaf(hv[2], wa.z, fmaf(hv[3], wa.w, fc0))));
-                        fc1 = fmaf(hv[0], wb.x, fmaf(hv[1], wb.y, fmaf(hv[2], wb.z, fmaf(hv[3], wb.w, fc1))));
-                    }
-                    hp[2 * u4] = pack_half2(hv[0], hv[1]);
-                    hp[2 * u4 + 1] = pack_half2(hv[2], hv[3]);
                 }
-                st_f4_hint(cp, make_float4(cn[0], cn[1], cn[2], cn[3]), pol_c);
-                st_f4_hint(cp + 128, make_float4(cn[4], cn[5], cn[6], cn[7]), pol_c);
-                *reinterpret_cast<uint4*>(mypark + (size_t)j * 128 * 16) = make_uint4(hp[0], hp[1], hp[2], hp[3]);
+#pragma unroll
+                for (int v = 0; v < 4; ++v) __stcg(cp + v * 128, make_float4(cn[4 * v], cn[4 * v + 1], cn[4 * v + 2], cn[4 * v + 3]));
             }
-            mbar_wait(stepdone, t & 1);                            // every MMA that reads h(t-1) has retired: h(t) may replace it
-            tc5_fence_after();
-            for (int j = 0; j < NCH; ++j) {
-                const uint4 p0 = *reinterpret_cast<const uint4*>(mypark + (size_t)j * 128 * 16);
-                const uint32_t hv[4] = {p0.x, p0.y, p0.z, p0.w};
-                tmem_st4(tl + j * 16 + cg * 4, hv);
-                if (!LAST) __stcs(reinterpret_cast<uint4*>(a.hseq + mrow * (size_t)H + j * 32 + cg * 8), p0);   // next layer's GEMM input (streaming)
+            if (LAST) {                                             // the four lanes of a row hold disjoint units: reduce, then across the warpgroups
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int o = 1; o < 4; o <<= 1) {
+                        fc0[h] += __shfl_xor_sync(0xffffffffu, fc0[h], o);
+                        fc1[h] += __shfl_xor_sync(0xffffffffu, fc1[h], o);
+                    }
+                if (wg == 1 && (lane & 3) == 0)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        fcpart[((t & 1) * R5_ROWS + rl[h]) * 2] = fc0[h];
+                        fcpart[((t & 1) * R5_ROWS + rl[h]) * 2 + 1] = fc1[h];
+                    }
             }
-            tmem_wait_st();
-            tc5_fence_before();
-            __syncwarp();
-            if (lane == 0) { if (leader) mbar_arrive(hready); else mbar_arrive_remote(r_hready); }
-
-            if (LAST) {
-                if (cg != 0) { fcpart[(cg * 128 + r) * 2] = fc0; fcpart[(cg * 128 + r) * 2 + 1] = fc1; }
-                asm volatile("bar.sync 1, 512;" ::: "memory");
-                if (cg == 0 && t >= a.la && grow < a.rows) {
-                    const float o0 = fc0 + fcpart[(128 + r) * 2] + fcpart[(256 + r) * 2] + fcpart[(384 + r) * 2] + fcb0;
-                    const float o1 = fc1 + fcpart[(128 + r) * 2 + 1] + fcpart[(256 + r) * 2 + 1] + fcpart[(384 + r) * 2 + 1] + fcb1;
+            fence_proxy_async();                                    // h(t) (generic stores) -> the next step's wgmma (async proxy)
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            if (KX && tid == 0) mbar_arrive(&xempty[t & 1]);        // every MMA of step t has retired: the input tile may be replaced
+            if (LAST && wg == 0 && (lane & 3) == 0 && t >= a.la) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    if (grow[h] >= a.rows) continue;
+                    const int ob = grow[h] / a.F, of = grow[h] % a.F;
+                    const float o0 = apply_act(fc0[h] + fcpart[((t & 1) * R5_ROWS + rl[h]) * 2] + __ldg(a.fc_b), a.act);
+                    const float o1 = apply_act(fc1[h] + fcpart[((t & 1) * R5_ROWS + rl[h]) * 2 + 1] + __ldg(a.fc_b + 1), a.act);
+                    const size_t ni = ((size_t)ob * a.F + of) * Tout + (t - a.la);
                     if (a.enh) {                                       // fused decompress_cIRM x noisy spectrum (inferencer.py:152-157)
-                        const float m0 = decompress_cirm(apply_act(o0, a.act)), m1 = decompress_cirm(apply_act(o1, a.act));
-                        a.enh[((size_t)ob * a.F + of) * Tout + (t - a.la)] = make_float2(m0 * nx.x - m1 * nx.y, m1 * nx.x + m0 * nx.y);
+                        const float m0 = decompress_cirm(o0), m1 = decompress_cirm(o1);
+                        const float nr = __ldg(a.nreal + ni), nim = __ldg(a.nimag + ni);
+                        a.enh[ni] = make_float2(m0 * nr - m1 * nim, m1 * nr + m0 * nim);
                     } else {
-                        a.out[(((size_t)ob * 2 + 0) * a.F + of) * Tout + (t - a.la)] = apply_act(o0, a.act);
-                        a.out[(((size_t)ob * 2 + 1) * a.F + of) * Tout + (t - a.la)] = apply_act(o1, a.act);
+                        a.out[(((size_t)ob * 2 + 0) * a.F + of) * Tout + (t - a.la)] = o0;
+                        a.out[(((size_t)ob * 2 + 1) * a.F + of) * Tout + (t - a.la)] = o1;
                     }
                 }
-                asm volatile("bar.sync 2, 512;" ::: "memory");
             }
         }
     }
-    tc5_fence_before();
     __syncthreads();
-    cluster_sync_all();
-    tc5_fence_after();
-    if (warp == R5_EPI_WARPS + 1) tmem_dealloc_pair<512>(tmem);
+    cluster_sync_all();                                            // no CTA leaves while its peer may still arrive on its barriers
 }
 
 template <int HH, bool FF, bool GG, bool LL>
@@ -351,7 +296,7 @@ int launch_lstm_tc5r(const LstmTc5rLaunch& a, cudaStream_t s) {
     if (!lstm_tc5r_supported(a.H, 2)) return (int)cudaErrorInvalidValue;
     const R5Plan p = r5_plan(a.H);
     if (p.nstage < 2) return (int)cudaErrorInvalidValue;
-    const int grid = (a.ntiles + 1) / 2 * 2;                        // whole pairs; the buffers cover the padded tile
+    const int grid = (a.ntiles + 1) / 2 * 2 * (128 / R5_ROWS);    // whole clusters; the buffers cover the padded tile pair
     switch (a.H) {
         case 64: return r5_dispatch<64>(a, grid, p, s);
         case 128: return r5_dispatch<128>(a, grid, p, s);
@@ -371,21 +316,21 @@ int launch_lstm_tc5r(const LstmTc5rLaunch& a, cudaStream_t s) {
 //     SWIZZLE_128B -- the layer-0 "hidden block" format of fsn_tc5_pack_weights;
 //   * input-projection matrix for the GEMM: fp16 [4H, Kpad] row-major, row j * 128 + n = W_ih row fsn_tc5_gate_row(H, j, n),
 //     so that column j * 128 + cg * 32 + q * 8 + u of Gin is gate q of hidden unit 32 j + 8 cg + u;
-//   * biases: [4H] in the same column order, pre-scaled like fsn_api.cu does for the fused kernel.
+//   * biases: [4H] in the same column order, pre-scaled: the epilogue evaluates exp2(-log2(e) (acc + b)) as one FMA (tanh gates: -2 log2(e)).
 // ---------------------------------------------------------------------------------------------
 static inline uint16_t r5_h_bits(float f) { __half h = __float2half_rn(f); uint16_t b; std::memcpy(&b, &h, 2); return b; }
 
 void lstm_tc5r_pack_layer(int H, int Kin, int Kpad, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, bool gru,
                           std::vector<uint16_t>& stream, std::vector<uint16_t>& wih_perm, std::vector<float>& bias) {
     const int NCH = H / 32, KBH = H / 64;
-    stream.assign((size_t)NCH * KBH * (R5_STAGE_FULL / 2), 0);
+    stream.assign((size_t)NCH * KBH * (R5_STAGE / 2), 0);
     wih_perm.assign((size_t)4 * H * Kpad, 0);
     bias.assign((size_t)4 * H, 0.f);
     for (int j = 0; j < NCH; ++j)
         for (int n = 0; n < 128; ++n) {
             const int row = fsn_tc5_gate_row(H, j, n);
             for (int kb = 0; kb < KBH; ++kb) {
-                uint8_t* img = reinterpret_cast<uint8_t*>(stream.data()) + ((size_t)j * KBH + kb) * R5_STAGE_FULL;
+                uint8_t* img = reinterpret_cast<uint8_t*>(stream.data()) + ((size_t)j * KBH + kb) * R5_STAGE;
                 for (int k = 0; k < 64; ++k) {
                     const uint16_t b = r5_h_bits(w_hh[(size_t)row * H + kb * 64 + k]);
                     std::memcpy(img + sw128_offset(n, k), &b, 2);
@@ -395,6 +340,18 @@ void lstm_tc5r_pack_layer(int H, int Kin, int Kpad, const float* w_ih, const flo
             const int qg = (n % 32) / 8;
             const float sc = (qg == 2 || (qg == 3 && gru)) ? -2.8853900817779268f : -1.4426950408889634f;
             bias[(size_t)j * 128 + n] = sc * (b_ih[row] + b_hh[row]);
+        }
+}
+
+// Row order of the input-projection matrix the GEMM multiplies with, so that the Gin columns of chunk j come out in the order the
+// recurrent kernel reads them: column j * 128 + p * 32 + cg * 8 + q * 2 + e  <-  packed row j * 128 + (cg * 32 + q * 8 + 2 p + e).
+void lstm_tc5r_gin_order(int H, int Kpad, std::vector<uint16_t>& wih_perm) {
+    const std::vector<uint16_t> src(wih_perm);
+    for (int j = 0; j < H / 32; ++j)
+        for (int m = 0; m < 128; ++m) {
+            const int p = m / 32, cg = (m / 8) % 4, q = (m / 2) % 4, e = m % 2;
+            const int n = cg * 32 + q * 8 + 2 * p + e;
+            std::memcpy(&wih_perm[((size_t)j * 128 + m) * Kpad], &src[((size_t)j * 128 + n) * Kpad], (size_t)Kpad * 2);
         }
 }
 

@@ -1,4 +1,4 @@
-"""fsnplus_b200 -- B200-native FullSubNet+/FullSubNet inference forward (host-side mirror of the reference API).
+"""fsnplus_b200 -- H100-native (sm_90a) FullSubNet+/FullSubNet inference forward (host-side mirror of the reference API).
 
 Drop-in: point ``config[model].path`` of the reference's TOML at
 ``fsnplus_b200.model.FullSubNet_Plus`` (or ``fsnplus_b200.model.Model``) with this directory's parent

@@ -44,7 +44,7 @@ def load_library():
         return _LIB
     path = lib_path()
     if not os.path.exists(path):
-        raise FsnError(f"{path} not found: run `python __graft_entry__.py` (nvcc, sm_100a) first; "
+        raise FsnError(f"{path} not found: run `python __graft_entry__.py` (nvcc, sm_90a) first; "
                        "fsnplus_b200 has no CPU or PyTorch fallback")
     lib = C.CDLL(path)
     vp, i32, i64, fp = C.c_void_p, C.c_int32, C.c_int64, C.POINTER(C.c_float)

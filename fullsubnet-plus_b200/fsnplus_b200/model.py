@@ -4,7 +4,7 @@
 mirrors speech_enhance/fullsubnet/model/fullsubnet.py:12-118: same constructor keywords, same
 ``state_dict`` keys/shapes (so reference checkpoints load with ``strict=True``), same forward signature and
 ``[B, 2, F, T]`` float32 output.  The sub-modules below are *parameter containers only*: all arithmetic of
-``forward`` runs in the sm_100a CUDA library behind the C ABI of include/fsnplus_b200.h.  There is no
+``forward`` runs in the sm_90a CUDA library behind the C ABI of include/fsnplus_b200.h.  There is no
 PyTorch/CPU fallback -- CPU tensors, training mode or a missing library raise.
 """
 import ctypes as C
@@ -199,7 +199,7 @@ class _B200Model(nn.Module):
         if self.training:
             raise NotImplementedError("fsnplus_b200 implements the inference (eval) forward only; call .eval()")
         if not mag.is_cuda:
-            raise RuntimeError("fsnplus_b200 has no CPU fallback: move the model and its inputs to a B200 (cuda) device")
+            raise RuntimeError("fsnplus_b200 has no CPU fallback: move the model and its inputs to a CUDA (H100) device")
         if F != self._cfg.num_freqs:
             raise ValueError(f"expected {self._cfg.num_freqs} frequency bins, got {F}")
         ins = [x.detach().to(dtype=torch.float32).contiguous() if x is not None else None for x in (mag, real, imag)]
@@ -334,7 +334,7 @@ class FullSubNet_Plus(_B200Model):
         super().__init__()
         assert sequence_model in ("GRU", "LSTM", "TCN"), f"{self.__class__.__name__} only support GRU, LSTM and TCN."
         if sequence_model == "TCN":
-            raise NotImplementedError("a TCN sub-band model is not implemented on the B200 path (LSTM and GRU are)")
+            raise NotImplementedError("a TCN sub-band model is not implemented on the CUDA path (LSTM and GRU are)")
         if channel_attention_model not in _lib.ATTENTION:                                       # fullsubnet_plus.py:69-70
             raise NotImplementedError(f"Not implemented channel attention model {channel_attention_model}")
         # fullsubnet_plus.py:47-50.  With subband_num > 1 the reference builds all three attentions for F // subband_num + 1

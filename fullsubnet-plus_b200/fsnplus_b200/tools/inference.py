@@ -167,7 +167,7 @@ def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=pri
     # and start-up time scale with the batch, not with the dataset -- the reference streams one clip at a time)
     batches = bucket_by_length([wav_length(p, ds_sr) for p in files], batch_size)
     mine = [(bi, idx) for bi, idx in enumerate(batches) if bi % world == rank]
-    # Ragged real recordings make many small batches (a lone clip occupies 16 of 148 SMs in the column-split kernel): up to `streams`
+    # Ragged real recordings make many small batches (a lone clip fills a small fraction of the SMs): up to `streams`
     # batches are in flight at once, each on its own CUDA stream and its own model replica (own C handle and workspaces).
     nstream = max(1, min(streams, len(mine))) if (on_gpu and model_and_epoch is None) else 1
     models = [model] + [build_model(config["model"], Path(checkpoint_path).expanduser().absolute(), device, trust_checkpoint)[0]

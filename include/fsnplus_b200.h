@@ -1,5 +1,5 @@
 /*
- * fsnplus_b200 -- C ABI of the B200-native FullSubNet+/FullSubNet inference forward.
+ * fsnplus_b200 -- C ABI of the H100-native (sm_90a) FullSubNet+/FullSubNet inference forward.
  *
  * This is the drop-in boundary for ONE path of RookieJunChen/FullSubNet-plus: the model forward
  *   speech_enhance/fullsubnet_plus/model/fullsubnet_plus.py:122-209  (FullSubNet_Plus.forward)
@@ -58,7 +58,7 @@ extern "C" {
 /* lstm_impl */
 #define FSN_LSTM_AUTO 0
 #define FSN_LSTM_MMA 1     /* generic mma.sync kernel (any hidden size / layer count)               */
-#define FSN_LSTM_TCGEN05 2 /* persistent tcgen05/TMEM kernels: fused (2 layers, hidden <= 384) or layer-wise (hidden <= 512); input <= 64 */
+#define FSN_LSTM_TCGEN05 2 /* tensor-core path (historical name): layer-wise wgmma kernels, hidden % 64 == 0 and <= 512, input <= 64, output_size 2 */
 
 typedef struct fsn_config {
     int32_t model_kind;
@@ -109,7 +109,7 @@ int fsn_model_finalize(fsn_model* m);
  * Inputs: [B, 1, F, T] float32, contiguous, device.  Output: [B, output_size, F, T] float32, contiguous,
  * device, caller-owned.  Every sample is processed independently (the eval semantics of the reference
  * called with batch 1; the training-only drop_band of fullsubnet_plus.py:192-196 is never applied).  Because of that a
- * batch whose workspace would exceed FSN_WS_CAP_GB (default 48) is run as equal sub-batches on `stream`, with identical results. */
+ * batch whose workspace would exceed FSN_WS_CAP_GB (default 24) is run as equal sub-batches on `stream`, with identical results. */
 int fsn_model_forward(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
                       float* d_out, void* stream);
 /* The model call PLUS the two lines that follow it in the reference's inferencer methods (fullsubnet_plus/inferencer/inferencer.py:152-157,
@@ -127,8 +127,8 @@ int fsn_model_forward_host(fsn_model* m, const float* h_mag, const float* h_real
 /* Pipelined variants for STREAMS OF BATCHES (the reference's inferencer loop, base_inferencer.py:133-160, issues one forward
  * after the other; the outputs of a batch are only needed when its files are written).  The forward is split at the one point
  * where it changes character: the full-band front end (norm, attention, TCN / full-band LSTM, sub-band statistics + packing) is
- * bandwidth/latency-bound and occupies the whole GPU for a short time, the sub-band LSTM is tensor-bound and occupies 130 of the
- * 148 SMs for a long time.  Both entry points run the front end of batch i+1 on an internal stream, into the second of two
+ * bandwidth/latency-bound and occupies the whole GPU for a short time, the sub-band LSTM is tensor-bound and occupies the SMs for
+ * a long time.  Both entry points run the front end of batch i+1 on an internal stream, into the second of two
  * workspace lanes, WHILE the sub-band LSTM of batch i runs on another internal stream: the front end fills the idle SMs.
  *
  * fsn_model_submit: device buffers.  The inputs must be complete in `stream` order at the time of the call and stay untouched,
@@ -188,14 +188,14 @@ int fsn_model_last_lstm_impl(const fsn_model* m);
 /* Host-side packers exposed for CPU tests of the kernel layouts (no GPU needed). */
 /* 128-row x 64-half tile with the SWIZZLE_128B layout: byte offset of element (row, k). */
 uint32_t fsn_sw128_offset(uint32_t row, uint32_t k);
-/* Size in bytes and content of the tcgen05 weight stream for a 2-layer LSTM (see DESIGN.md 4.5). */
+/* Size in bytes and content of the packed two-layer weight stream (128 gate columns x 64 k SWIZZLE_128B stages, consumption order). */
 int64_t fsn_tc5_weight_stream_bytes(int32_t input_size, int32_t hidden);
 /* weight row (in [W_i; W_f; W_g; W_o] order) that gate column n (0..127) of 32-unit chunk j maps to */
 int32_t fsn_tc5_gate_row(int32_t hidden, int32_t chunk, int32_t n);
 int fsn_tc5_pack_weights(int32_t input_size, int32_t hidden, const float* w_ih0, const float* w_hh0, const float* w_ih1,
                          const float* w_hh1, uint16_t* h_dst /* fp16 bits */);
 
-/* Layer-wise tcgen05 path (DESIGN.md 4.7), one layer: recurrent stream (hidden/32 chunks x hidden/64 tiles of 16 KB), the
+/* Layer-wise wgmma path (DESIGN.md 3.3), one layer: recurrent stream (hidden/32 chunks x hidden/64 tiles of 16 KB), the
  * input-projection matrix for the GEMM ([4 hidden, k_pad] fp16, rows in chunk column order) and the pre-scaled biases
  * ([4 hidden] in the same order; gru != 0 scales pseudo-gate 3 like a tanh argument).  b_ih / b_hh in the nn.LSTM 4-block layout. */
 int64_t fsn_tc5r_weight_stream_bytes(int32_t hidden);

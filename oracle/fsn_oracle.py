@@ -5,7 +5,7 @@ tests/golden/*.npz, generated from the imported reference by
 tests/golden/make_golden.py.
 
 Every function cites the reference file:line it follows (paths relative to
-/root/reference/speech_enhance).  All arithmetic is plain numpy, float64 by
+speech_enhance/ of the reference).  All arithmetic is plain numpy, float64 by
 default (the "truth" the CUDA path is measured against, SURVEY.md 8c).
 
 The arithmetic of the reference lives in PyTorch (nn.LSTM, nn.Conv1d,

@@ -1,5 +1,5 @@
-"""Import the UNMODIFIED reference package (from /root/reference in the authoring container, else from the verbatim copy
-oracle/_ref/ made by oracle/make_ref.py) with the two stubs it needs in this image.
+"""Import the UNMODIFIED reference package (from its checkout, make_ref.SRC, else from the verbatim copy oracle/_ref/ made by
+oracle/make_ref.py) with the two stubs it needs in this image.
 
 TEST / BENCH INFRASTRUCTURE ONLY (see oracle/__init__.py).
 
@@ -17,7 +17,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 def reference_root():
-    for root in ("/root/reference", os.path.join(HERE, "_ref")):
+    from oracle.make_ref import SRC
+    for root in (SRC, os.path.join(HERE, "_ref")):
         if os.path.isdir(os.path.join(root, "speech_enhance", "fullsubnet_plus")):
             return root
     return None
@@ -51,8 +52,8 @@ def setup():
     """Put the reference on sys.path (both roots it imports from, SURVEY.md 8c) and install the stubs.  Returns the root."""
     root = reference_root()
     if root is None:
-        raise RuntimeError("the reference is not available: neither /root/reference nor oracle/_ref/ (run oracle/make_ref.py "
-                           "in the authoring container)")
+        raise RuntimeError("the reference is not available: neither its checkout (FSN_REFERENCE_SRC) nor oracle/_ref/ (run "
+                           "oracle/make_ref.py where the checkout exists)")
     os.environ.setdefault("PYTHONDONTWRITEBYTECODE", "1")
     sys.dont_write_bytecode = True
     _stubs()

@@ -1,12 +1,12 @@
 """PyTorch-CPU restatement of the reference forward, used ONLY as the timed CPU baseline.
 
 TEST/BENCH INFRASTRUCTURE ONLY (see oracle/__init__.py).  The reference is pure Python on top of PyTorch and
-cannot travel to the GPU box (/root/reference does not exist there), so bench.py's ``cpu_baseline`` leg and
+may be absent where the benchmark runs (oracle/_ref/ is only made from a checkout of it), so bench.py's ``cpu_baseline`` leg and
 ``--impl reference`` arm time this port instead: it issues the SAME ATen operators the reference issues
 (nn.LSTM, F.conv1d, F.group_norm, F.prelu, F.linear, F.pad(reflect) + F.unfold) in the same order, fp32,
 one sample per call (the only batch size the reference inference supports, base_inferencer.py:65-69), with all
 host threads.  Parity status: PINNED -- tests/test_oracle_golden.py checks it against the golden vectors
-generated from the unmodified reference.  Line references are to /root/reference/speech_enhance.
+generated from the unmodified reference.  Line references are to speech_enhance/ of the reference.
 """
 import torch
 import torch.nn as nn

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """BASELINE config #4: streaming/causal mode, look_ahead = 2 frames, one 30 s synthetic 16 kHz clip, per-frame latency
-p50/p99 on 1xB200.  Model: fullsubnet.Model (default hyper-parameters) + cumulative_laplace_norm, stepped frame by frame
+p50/p99 on one GPU.  Model: fullsubnet.Model (default hyper-parameters) + cumulative_laplace_norm, stepped frame by frame
 through the stateful C-ABI step API; every frame is synchronised (a real-time caller needs the mask before the next hop)."""
 import json
 import os

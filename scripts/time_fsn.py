@@ -18,20 +18,14 @@ with torch.no_grad():
     for B in (1, 8, 64):
         x = torch.rand(B, 1, 257, 188, device=dev)
         print(f"fullsubnet.Model B={B}: {timeit(lambda: m(x)):.2f} ms  (sub-band LSTM {m.last_lstm_ms():.2f} ms)")
-    # small batches: automatic column split (S CTA pairs per 256 sequences) against the unsplit kernel (FSN_TC5_SPLIT is read at model creation)
+    # FullSubNet+ from one clip to the flagship batch
     p = FullSubNet_Plus(**bench.default_cfg()).to(dev).eval()
-    os.environ["FSN_TC5_SPLIT"] = "1"
-    p1 = FullSubNet_Plus(**bench.default_cfg()).to(dev).eval()
-    p1.load_state_dict(p.state_dict())
-    x = torch.rand(1, 1, 257, 188, device=dev); p1(x, x - 0.5, x - 0.3)          # creates the handle while the knob is set
-    del os.environ["FSN_TC5_SPLIT"]
     for B in (1, 2, 4, 8, 16, 24, 32, 48, 64):
         x = torch.rand(B, 1, 257, 188, device=dev)
         ta = timeit(lambda: p(x, x - 0.5, x - 0.3)); la = p.last_lstm_ms()
-        t1 = timeit(lambda: p1(x, x - 0.5, x - 0.3)); l1 = p1.last_lstm_ms()
-        print(f"FullSubNet_Plus B={B:2d}: auto split {ta:6.2f} ms (sub-band LSTM {la:5.2f})   unsplit {t1:6.2f} ms (LSTM {l1:5.2f})   {ta / B:6.3f} ms/clip")
-    # other constructor values: GRU sub-band model (tcgen05 pair kernel with the GRU cell), SE attention, and BASELINE config #5
-    # (F = 513, H = 512, 3 layers, B = 32, T = 94: outside the tcgen05 kernel's TMEM envelope -> generic mma.sync kernel)
+        print(f"FullSubNet_Plus B={B:2d}: {ta:6.2f} ms (sub-band LSTM {la:5.2f})   {ta / B:6.3f} ms/clip")
+    # other constructor values: GRU sub-band model (tensor-core LSTM path with the GRU cell), SE attention, and BASELINE config #5
+    # (F = 513, H = 512, 3 layers, B = 32, T = 94)
     x = torch.rand(64, 1, 257, 188, device=dev)
     g = FullSubNet_Plus(**dict(bench.default_cfg(), sequence_model="GRU")).to(dev).eval()
     print(f"FullSubNet_Plus GRU B=64: {timeit(lambda: g(x, x - 0.5, x - 0.3)):.2f} ms  (sub-band GRU {g.last_lstm_ms():.2f} ms, {g.last_lstm_impl()})")

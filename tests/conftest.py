@@ -11,7 +11,7 @@ for p in (ROOT, PKG):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run by the driver with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA GPU (H100, sm_90a); select with -m gpu")
 
 
 @pytest.fixture(scope="session")
@@ -30,6 +30,10 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 def golden():
     import numpy as np
 
-    def load(name):
-        return dict(np.load(os.path.join(GOLDEN, name + ".npz")))
+    def load(name):                                     # name.npz plus its parts name.<part>.npz (fixtures are kept below 1 MB each)
+        d = dict(np.load(os.path.join(GOLDEN, name + ".npz")))
+        for f in sorted(os.listdir(GOLDEN)):
+            if f.startswith(name + ".") and f.endswith(".npz") and f != name + ".npz":
+                d.update(np.load(os.path.join(GOLDEN, f)))
+        return d
     return load

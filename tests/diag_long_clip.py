@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Where does the error of the 30 s / x3-weights case (tests/test_gpu_round2.py::test_config4_30s_clip_parity, 9.7e-4 against a bar of
 1e-3) come from?  Stage-wise: the full-band LSTM output (weight-stationary kernel) vs the CPU port, and the final mask when the sub-band
-stage is fed (a) its own full-band output, (b) nothing else changed -- run on a B200."""
+stage is fed (a) its own full-band output, (b) nothing else changed -- run on a GPU."""
 import os
 import sys
 

@@ -1,7 +1,6 @@
 """Generate the committed golden vectors from the UNMODIFIED reference.
 
-Run in the authoring container only (needs /root/reference, which does not
-exist on the GPU box):
+Needs the reference's checkout (oracle/make_ref.py: FSN_REFERENCE_SRC, by default /root/reference):
 
     PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
 
@@ -22,7 +21,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.modules.setdefault("librosa", types.ModuleType("librosa"))
-sys.path[:0] = ["/root/reference", "/root/reference/speech_enhance"]
+from oracle.make_ref import SRC as REF  # noqa: E402
+sys.path[:0] = [REF, os.path.join(REF, "speech_enhance")]
 
 import torch  # noqa: E402
 
@@ -101,11 +101,14 @@ def spectra(clips, n_fft=512, hop=256):
     return X.abs().numpy()[:, None], X.real.numpy()[:, None], X.imag.numpy()[:, None], X.numpy()
 
 
-def save(name, **kw):
-    path = os.path.join(HERE, name + ".npz")
-    np.savez_compressed(path, **{k: (v.astype(np.float32) if isinstance(v, np.ndarray) and v.dtype == np.float64 else v)
-                                 for k, v in kw.items()})
-    print(f"  wrote {name}.npz  {os.path.getsize(path) / 1e6:.2f} MB")
+def save(name, parts=None, **kw):
+    """name.npz; keys listed in ``parts`` ({suffix: keys}) go to name.<suffix>.npz instead (every fixture stays below 1 MB; the
+    golden fixture of tests/conftest.py merges the parts)."""
+    kw = {k: (v.astype(np.float32) if isinstance(v, np.ndarray) and v.dtype == np.float64 else v) for k, v in kw.items()}
+    for sfx, keys in [("", [k for k in kw if not any(k in ks for ks in (parts or {}).values())])] + list((parts or {}).items()):
+        path = os.path.join(HERE, name + (("." + sfx) if sfx else "") + ".npz")
+        np.savez_compressed(path, **{k: kw[k] for k in keys})
+        print(f"  wrote {os.path.basename(path)}  {os.path.getsize(path) / 1e6:.2f} MB")
 
 
 def small_plus_cfg():
@@ -152,8 +155,8 @@ def main():
                             length=clips.shape[1]).numpy()
             dref = ref_decompress(torch.from_numpy(out).permute(0, 2, 3, 1)).numpy()
             print("   decompress oracle-vs-ref:", O.rel_l2(O.decompress_cIRM(out).transpose(0, 2, 3, 1), dref))
-            save(tag, mag=mag, real=real, imag=imag, out=out, fb_in=fb_in, fb_out=fb_out, enhanced=enh,
-                 seed=0, lstm_scale=scale)
+            save(tag, parts={"fb": ["fb_in", "fb_out"], "enh": ["enhanced"]}, mag=mag, real=real, imag=imag, out=out, fb_in=fb_in,
+                 fb_out=fb_out, enhanced=enh, seed=0, lstm_scale=scale)
         else:
             save(tag, out=out, seed=0, lstm_scale=scale)
 

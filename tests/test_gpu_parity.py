@@ -95,7 +95,7 @@ def test_plus_small_other_attentions_golden(built_lib, golden, attn):
 
 @pytest.mark.parametrize("attn", ["SE", "ECA", "CBAM"])
 def test_plus_default_size_other_attentions_vs_oracle(built_lib, golden, attn):
-    """Default geometry (F=257, H=384, tcgen05 path), one clip, oracle as truth; for CBAM the mag branch has all-positive
+    """Default geometry (F=257, H=384, tensor-core LSTM path), one clip, oracle as truth; for CBAM the mag branch has all-positive
     rows and the real/imag branches a negative normaliser, which exercises the min/max selection of the squeeze."""
     gi = golden("plus_default")
     cfg = dict(O.default_plus_config(), channel_attention_model=attn)
@@ -161,7 +161,7 @@ def test_gru_plus_small_vs_oracle(built_lib, impl, H, fast):
 
 
 def test_gru_default_size_vs_oracle(built_lib, golden):
-    """Default geometry with a GRU sub-band model (tcgen05 pair kernel, H = 384) and the GRU fullsubnet.Model (H = 512 full
+    """Default geometry with a GRU sub-band model (tensor-core LSTM path, H = 384) and the GRU fullsubnet.Model (H = 512 full
     band on the weight-stationary kernel); one 3 s clip, oracle fp64 as truth; a parameter update must re-expand the gates."""
     gi = golden("plus_default")
     cfg = dict(O.default_plus_config(), sequence_model="GRU")
@@ -379,7 +379,7 @@ def test_config4_causal_fullsubnet_long_clip(built_lib):
 def test_config5_large_model(built_lib):
     """BASELINE config #5 geometry: num_freqs=513 (n_fft=1024, hop 512 -> T=94 for 3 s), sub-band hidden 512, 3-layer
     LSTMs (additive num_layers knob; oracle = SequenceModel(num_layers=3) semantics, pinned by tests/golden/lstm3_small).
-    Default = layer-wise tcgen05 path (k_lstm_tc5r.cu); lstm_impl="mma" = generic mma.sync kernel."""
+    Default = layer-wise wgmma path (k_lstm_tc5r.cu); lstm_impl="mma" = generic mma.sync kernel."""
     cfg = O.default_plus_config()
     cfg.update(num_freqs=513, sb_model_hidden_size=512, fb_model_hidden_size=512)
     params = O.make_params_plus(cfg, seed=31, num_layers=3)
@@ -445,7 +445,7 @@ def test_streaming_step_api_matches_offline(built_lib, norm, rnn):
 
 
 def test_large_batch_multiple_waves_and_long_sequence(built_lib):
-    """More CTA pairs than SMs (B*F = 167*33 rows... small F keeps the oracle cheap; 5511 rows = 44 tiles) is covered by
+    """More CTAs than SMs (B*F = 167*33 rows... small F keeps the oracle cheap; 5511 rows = 44 tiles) is covered by
     the full-size test; here: (a) odd tile count + a batch whose last pair is half empty, (b) a long sequence (T = 400) on
     FullSubNet+, both against the oracle."""
     cfg = small_cfg(64)
@@ -462,7 +462,7 @@ def test_large_batch_multiple_waves_and_long_sequence(built_lib):
 
 
 def test_default_config_batch_130(built_lib, golden):
-    """B = 130 clips at the default geometry: 33 410 rows = 262 tiles = 131 CTA pairs (> 74 resident pairs, two waves)."""
+    """B = 130 clips at the default geometry: 33 410 rows = 262 tiles = 524 CTAs of 64 rows (four waves on 132 SMs)."""
     g = golden("plus_default")
     cfg = O.default_plus_config()
     m = build_plus(cfg, O.make_params_plus(cfg, seed=0))
@@ -527,9 +527,9 @@ def test_command_line_tool_matches_reference_pipeline(built_lib, golden, tmp_pat
 
 @pytest.mark.parametrize("L,H,rnn", [(1, 64, "LSTM"), (3, 64, "LSTM"), (3, 128, "GRU"), (4, 64, "LSTM"), (3, 192, "LSTM"), (1, 448, "LSTM")])
 def test_layerwise_tcgen05_vs_oracle(built_lib, L, H, rnn):
-    """Layer-wise tcgen05 path (k_lstm_tc5r.cu: one cuBLAS input-projection GEMM + one recurrent launch per layer) for stacks
-    outside the fused kernel's envelope (default for hidden % 64 == 0, <= 512).  First / middle / last layer roles, LSTM and GRU cells,
-    more than one CTA pair (B*F = 5*33 = 165 rows -> 2 tiles) and a half-empty last tile."""
+    """Layer-wise wgmma path (k_lstm_tc5r.cu: one recurrent launch per layer, preceded by an input-projection GEMM for the deeper
+    layers; default for hidden % 64 == 0, <= 512).  First / middle / last layer roles, LSTM and GRU cells, more than one cluster
+    (B*F = 5*33 = 165 rows -> 2 tiles) and a half-empty last tile."""
     cfg = dict(small_cfg(H), sequence_model=rnn)
     params = O.make_params_plus(cfg, seed=40 + L, num_layers=L, lstm_scale=2.0)
     mag, real, imag = small_inputs(5, 33, 26, 12)
@@ -540,6 +540,6 @@ def test_layerwise_tcgen05_vs_oracle(built_lib, L, H, rnn):
         out2 = m(_t(mag), _t(real), _t(imag))
     assert m.last_lstm_impl() == "tcgen05"
     err = O.rel_l2(out.cpu().numpy(), ref)
-    print(f"\n[layer-wise tcgen05 L={L} H={H} {rnn}] cIRM {err:.3e}")
+    print(f"\n[layer-wise L={L} H={H} {rnn}] cIRM {err:.3e}")
     assert torch.equal(out, out2)
     assert err < MASK_TOL

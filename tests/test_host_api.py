@@ -200,7 +200,7 @@ def test_tc5_weight_stream_layout(built_lib):
 
 
 def test_tc5r_layer_packing(built_lib):
-    """Layer-wise tcgen05 path (k_lstm_tc5r.cu): recurrent stream tiles, permuted input-projection matrix and pre-scaled biases
+    """Layer-wise wgmma path (k_lstm_tc5r.cu): recurrent stream tiles, permuted input-projection matrix and pre-scaled biases
     of one layer follow the chunk column order n -> fsn_tc5_gate_row (gate q = (n % 32) // 8 of unit 32 j + 8 (n // 32) + n % 8)."""
     H, Kin, Kpad = 128, 34, 64
     rng = np.random.default_rng(1)

@@ -1,5 +1,5 @@
-"""The drop-in claim of INTEGRATION.md, executed: the reference's OWN loader and inferencer code (unmodified, imported from
-/root/reference here or from the verbatim copy oracle/_ref/ on the GPU box) driving ``fsnplus_b200.model.FullSubNet_Plus`` after
+"""The drop-in claim of INTEGRATION.md, executed: the reference's OWN loader and inferencer code (unmodified, imported from the
+checkout named by FSN_REFERENCE_SRC or from the verbatim copy oracle/_ref/) driving ``fsnplus_b200.model.FullSubNet_Plus`` after
 changing ONE string of config/inference.toml (``[model] path``).
 
   reference code on this path: audio_zen/utils.py:63-99 (initialize_module), audio_zen/inferencer/base_inferencer.py:22-60,97-110
@@ -7,7 +7,7 @@ changing ONE string of config/inference.toml (``[model] path``).
   sf.write) and fullsubnet_plus/inferencer/inferencer.py:140-165 (mag_complex_full_band_crm_mask).
 
 CPU test: everything up to the forward (construction from the shipped TOML's [model.args], strict checkpoint load, eval) and the
-documented error on CPU tensors.  GPU test: the whole reference inferencer loop with the model on the B200, its written int16
+documented error on CPU tensors.  GPU test: the whole reference inferencer loop with the model on the GPU, its written int16
 waveform compared with the golden waveform of the all-reference pipeline.
 """
 import os
@@ -21,7 +21,7 @@ from oracle import fsn_oracle as O
 from oracle import ref_loader
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-needs_ref = pytest.mark.skipif(not ref_loader.available(), reason="reference not available (neither /root/reference nor oracle/_ref)")
+needs_ref = pytest.mark.skipif(not ref_loader.available(), reason="reference not available (neither its checkout nor oracle/_ref)")
 
 
 def _config(tmp_path, clips):

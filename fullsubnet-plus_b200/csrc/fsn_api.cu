@@ -71,11 +71,12 @@ struct fsn_model {
         DevBuf x0, xr;                                 // time-major fb input / relu'd last residual
         DevBuf tsse_scale, sb_rowsum;
         DevBuf xn, sigma;                              // pre-normalised inputs / sub-band std for the non-default norm types
-        alignas(64) unsigned char mapX0[128], mapXa[128], mapXb[128], mapXr[128], mapY2[128];
+        DevBuf sbx;                                    // sub-band TCN: input [B*F*T', 64] fp32 time-major | max |x| per sequence [B*F]
+        alignas(64) unsigned char mapX0[128], mapXa[128], mapXb[128], mapXr[128], mapY2[128], mapSbx[128];
         cudaEvent_t ev_front = nullptr, ev_lstm = nullptr;   // front end written / LSTM finished reading this lane
         bool used = false;                             // ev_lstm has been recorded (a pipelined batch ran / may still run in this lane)
         void release_all() {
-            DevBuf* all[] = {&fbin, &fbout, &xa, &xb, &y1, &y2, &stats, &mu, &ximg, &magpad, &fbx, &hseq, &x0, &xr, &tsse_scale, &sb_rowsum, &xn, &sigma};
+            DevBuf* all[] = {&fbin, &fbout, &xa, &xb, &y1, &y2, &stats, &mu, &ximg, &magpad, &fbx, &hseq, &x0, &xr, &tsse_scale, &sb_rowsum, &xn, &sigma, &sbx};
             for (auto* b : all) b->release();
         }
     } lane[2];
@@ -87,6 +88,14 @@ struct fsn_model {
     DevBuf tW1, tW2, tWfc, tS1, tS2b, tBfc;            // [8][3][512][Cp], [8][3][Cp][512], [3][Cp][Cp], [8][3][Cp] x2, [3][Cp]
     DevBuf ws_h, ws_bar;                               // weight-stationary full-band LSTM: h exchange buffer, grid barrier
     alignas(64) unsigned char mapW1[8][128], mapW2[8][128], mapWfc[128];
+    // sub-band TCN (cfg.sb_tcn): the same block weights for one branch of Isb channels (Cp = 64, one 64-column N tile), the Linear
+    // head [O][64], and the scratch of the eight blocks -- shared by both lanes and ordered on the sub-band stream (like r_gin): two fp32
+    // streams, two fp16 hidden buffers, gLN sums and the stream maxima of blocks 1..7 (block 0's are written with the lane's input)
+    DevBuf sW1, sW2, sS1, sS2b, sFc;
+    alignas(64) unsigned char smapW1[8][128], smapW2[8][128];
+    DevBuf sb_xa, sb_xb, sb_y1, sb_y2, sb_stats;
+    long long sb_rows = 0;                             // rows of the tensor maps below
+    alignas(64) unsigned char mapSbXa[128], mapSbXb[128], mapSbY2[128];
     int64_t launches = 0;
     int last_impl = 0;
     // tuning knobs, read ONCE at fsn_model_create (never on the forward path): FSN_LSTM_IMPL overrides cfg.lstm_impl,
@@ -129,6 +138,27 @@ static void lstm_specs(std::vector<ParamSpec>& v, const std::string& pre, int I,
     add(v, pre + ".fc_output_layer.bias", O);
 }
 
+// SequenceModel(C, O, sequence_model="TCN"): 8 TCNBlock(C -> 512 -> C) + Linear(C -> O) (sequence_model.py:47-58,80-81)
+static void tcn_specs(std::vector<ParamSpec>& v, const std::string& pre, int C, int O) {
+    for (int i = 0; i < 8; ++i) {
+        const std::string q = pre + ".sequence_model." + std::to_string(i);
+        add(v, q + ".conv1x1.weight", (int64_t)512 * C);
+        add(v, q + ".conv1x1.bias", 512);
+        add(v, q + ".prelu1.weight", 1);
+        add(v, q + ".norm1.weight", 512);
+        add(v, q + ".norm1.bias", 512);
+        add(v, q + ".depthwise_conv.weight", 512 * 3);
+        add(v, q + ".depthwise_conv.bias", 512);
+        add(v, q + ".prelu2.weight", 1);
+        add(v, q + ".norm2.weight", 512);
+        add(v, q + ".norm2.bias", 512);
+        add(v, q + ".sconv.weight", (int64_t)C * 512);
+        add(v, q + ".sconv.bias", C);
+    }
+    add(v, pre + ".fc_output_layer.weight", (int64_t)O * C);
+    add(v, pre + ".fc_output_layer.bias", O);
+}
+
 static void build_specs(fsn_model* m) {
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs;
@@ -152,32 +182,14 @@ static void build_specs(fsn_model* m) {
             add(v, p + ".fc2.weight", (int64_t)F * (F / 2));
             add(v, p + ".fc2.bias", F);
         }
-        for (int b = 0; b < 3; ++b) {
-            const std::string p = std::string("fb_model") + sfx[b];
-            for (int i = 0; i < 8; ++i) {
-                const std::string q = p + ".sequence_model." + std::to_string(i);
-                add(v, q + ".conv1x1.weight", (int64_t)512 * F);
-                add(v, q + ".conv1x1.bias", 512);
-                add(v, q + ".prelu1.weight", 1);
-                add(v, q + ".norm1.weight", 512);
-                add(v, q + ".norm1.bias", 512);
-                add(v, q + ".depthwise_conv.weight", 512 * 3);
-                add(v, q + ".depthwise_conv.bias", 512);
-                add(v, q + ".prelu2.weight", 1);
-                add(v, q + ".norm2.weight", 512);
-                add(v, q + ".norm2.bias", 512);
-                add(v, q + ".sconv.weight", (int64_t)F * 512);
-                add(v, q + ".sconv.bias", F);
-            }
-            add(v, p + ".fc_output_layer.weight", (int64_t)F * F);
-            add(v, p + ".fc_output_layer.bias", F);
-        }
+        for (int b = 0; b < 3; ++b) tcn_specs(v, std::string("fb_model") + sfx[b], F, F);
         m->Isb = (2 * c.sb_num_neighbors + 1) + 3 * (2 * c.fb_num_neighbors + 1);
     } else {
         lstm_specs(v, "fb_model", F, c.fb_hidden, c.num_layers, F, c.rnn_type == FSN_RNN_GRU ? 3 : 4);
         m->Isb = (2 * c.sb_num_neighbors + 1) + (2 * c.fb_num_neighbors + 1);
     }
-    lstm_specs(v, "sb_model", m->Isb, c.sb_hidden, c.num_layers, c.output_size, c.rnn_type == FSN_RNN_GRU ? 3 : 4);
+    if (c.sb_tcn) tcn_specs(v, "sb_model", m->Isb, c.output_size);       // hidden width 512: sb_hidden and num_layers are unused
+    else lstm_specs(v, "sb_model", m->Isb, c.sb_hidden, c.num_layers, c.output_size, c.rnn_type == FSN_RNN_GRU ? 3 : 4);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -275,12 +287,57 @@ static float to_tf32(float x) {
     return y;
 }
 
-// FullSubNet+ TCN weights for the wgmma GEMMs (k_gemm_tc5.cu): channel dim padded to Cp (multiple of 32),
-// the three branches stacked, gLN2 folded into the second 1x1 convolution:
+// TCN block weights for the wgmma GEMMs (k_gemm_tc5.cu): channel dim C padded to Cp (multiple of 32), the branches (key prefixes
+// pre[b] = "<module>.sequence_model.") stacked, gLN2 folded into the second 1x1 convolution:
 //   conv(W2, gLN(y)) = rstd * (W2 diag(gamma2)) y - mean * rstd * s1 + s2,  s1[n] = sum_c W2'[n,c],  s2[n] = sum_c W2[n,c] beta2[c]
+// W1 [8][nbr][512][Cp] tf32, W2' [8][nbr][Cp][512] fp16, s1 / s2 + conv bias [8][nbr][Cp]; tensor maps per block: W1 in 128-row
+// boxes, W2' in NT-row boxes.
+static int pack_tcn_blocks(fsn_model* m, const std::vector<std::string>& pre, int C, int Cp, int NT, DevBuf& dW1, DevBuf& dW2, DevBuf& dS1,
+                           DevBuf& dS2b, unsigned char (*mapW1)[128], unsigned char (*mapW2)[128]) {
+    const int nbr = (int)pre.size(), Hd = 512;
+    std::vector<float> W1((size_t)8 * nbr * Hd * Cp, 0.f);
+    std::vector<__half> W2((size_t)8 * nbr * Cp * Hd, __float2half_rn(0.f));     // second 1x1 conv: fp16 operands (hidden activations are fp16)
+    std::vector<float> S1((size_t)8 * nbr * Cp, 0.f), S2b((size_t)8 * nbr * Cp, 0.f);
+    for (int blk = 0; blk < 8; ++blk)
+        for (int b = 0; b < nbr; ++b) {
+            const std::string q = pre[b] + std::to_string(blk) + ".";
+            const auto& w1 = m->host[q + "conv1x1.weight"];
+            const auto& w2 = m->host[q + "sconv.weight"];
+            const auto& b2 = m->host[q + "sconv.bias"];
+            const auto& g2 = m->host[q + "norm2.weight"];
+            const auto& be2 = m->host[q + "norm2.bias"];
+            float* d1 = &W1[((size_t)blk * nbr + b) * Hd * Cp];
+            for (int o = 0; o < Hd; ++o)
+                for (int k = 0; k < C; ++k) d1[(size_t)o * Cp + k] = to_tf32(w1[(size_t)o * C + k]);
+            __half* d2 = &W2[((size_t)blk * nbr + b) * Cp * Hd];
+            for (int n = 0; n < C; ++n) {
+                double s1 = 0, s2 = 0;
+                for (int k = 0; k < Hd; ++k) {
+                    const __half wh = __float2half_rn(w2[(size_t)n * Hd + k] * g2[k]);
+                    const float wf = __half2float(wh);
+                    d2[(size_t)n * Hd + k] = wh;
+                    s1 += (double)wf;
+                    s2 += (double)w2[(size_t)n * Hd + k] * (double)be2[k];
+                }
+                S1[((size_t)blk * nbr + b) * Cp + n] = (float)s1;
+                S2b[((size_t)blk * nbr + b) * Cp + n] = (float)(s2 + (double)b2[n]);
+            }
+        }
+    if (upload(dW1, W1.data(), W1.size() * 4) || upload(dW2, W2.data(), W2.size() * sizeof(__half)) ||
+        upload(dS1, S1.data(), S1.size() * 4) || upload(dS2b, S2b.data(), S2b.size() * 4))
+        return fail(FSN_ECUDA, "upload of the TCN weights failed");
+    for (int blk = 0; blk < 8; ++blk) {
+        if (make_tmap_f32_2d(mapW1[blk], static_cast<float*>(dW1.p) + (size_t)blk * nbr * Hd * Cp, nbr * Hd, Cp, 128) ||
+            make_tmap_f16_2d(mapW2[blk], static_cast<__half*>(dW2.p) + (size_t)blk * nbr * Cp * Hd, nbr * Cp, Hd, NT))
+            return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the TCN weights");
+    }
+    return FSN_OK;
+}
+
+// the three full-band TCNs of FullSubNet+ (F channels each) and their output Linear
 static int pack_tcn5(fsn_model* m) {
     const fsn_config& c = m->cfg;
-    const int F = c.num_freqs, Cp = (F + 31) / 32 * 32, Hd = 512;
+    const int F = c.num_freqs, Cp = (F + 31) / 32 * 32;
     m->Cp = Cp;
     // N tile of the Cp-wide GEMMs: 64 or 128 columns (the last tile of a branch may overhang; those columns are not stored)
     m->tcnNT = Cp <= 64 ? 64 : 128;
@@ -290,34 +347,11 @@ static int pack_tcn5(fsn_model* m) {
     cudaGetDevice(&dev);
     if (cudaGetDeviceProperties(&prop, dev) == cudaSuccess) m->num_sms = prop.multiProcessorCount;
     const char* sfx[3] = {"", "_real", "_imag"};
-    std::vector<float> W1((size_t)8 * 3 * Hd * Cp, 0.f), Wfc((size_t)3 * Cp * Cp, 0.f);
-    std::vector<__half> W2((size_t)8 * 3 * Cp * Hd, __float2half_rn(0.f));      // second 1x1 conv: fp16 operands (hidden activations are fp16)
-    std::vector<float> S1((size_t)8 * 3 * Cp, 0.f), S2b((size_t)8 * 3 * Cp, 0.f), Bfc((size_t)3 * Cp, 0.f);
-    for (int blk = 0; blk < 8; ++blk)
-        for (int b = 0; b < 3; ++b) {
-            const std::string q = std::string("fb_model") + sfx[b] + ".sequence_model." + std::to_string(blk) + ".";
-            const auto& w1 = m->host[q + "conv1x1.weight"];
-            const auto& w2 = m->host[q + "sconv.weight"];
-            const auto& b2 = m->host[q + "sconv.bias"];
-            const auto& g2 = m->host[q + "norm2.weight"];
-            const auto& be2 = m->host[q + "norm2.bias"];
-            float* d1 = &W1[((size_t)blk * 3 + b) * Hd * Cp];
-            for (int o = 0; o < Hd; ++o)
-                for (int k = 0; k < F; ++k) d1[(size_t)o * Cp + k] = to_tf32(w1[(size_t)o * F + k]);
-            __half* d2 = &W2[((size_t)blk * 3 + b) * Cp * Hd];
-            for (int n = 0; n < F; ++n) {
-                double s1 = 0, s2 = 0;
-                for (int k = 0; k < Hd; ++k) {
-                    const __half wh = __float2half_rn(w2[(size_t)n * Hd + k] * g2[k]);
-                    const float wf = __half2float(wh);
-                    d2[(size_t)n * Hd + k] = wh;
-                    s1 += (double)wf;
-                    s2 += (double)w2[(size_t)n * Hd + k] * (double)be2[k];
-                }
-                S1[((size_t)blk * 3 + b) * Cp + n] = (float)s1;
-                S2b[((size_t)blk * 3 + b) * Cp + n] = (float)(s2 + (double)b2[n]);
-            }
-        }
+    std::vector<std::string> pre;
+    for (int b = 0; b < 3; ++b) pre.push_back(std::string("fb_model") + sfx[b] + ".sequence_model.");
+    int rc = pack_tcn_blocks(m, pre, F, Cp, m->tcnNT, m->tW1, m->tW2, m->tS1, m->tS2b, m->mapW1, m->mapW2);
+    if (rc) return rc;
+    std::vector<float> Wfc((size_t)3 * Cp * Cp, 0.f), Bfc((size_t)3 * Cp, 0.f);
     for (int b = 0; b < 3; ++b) {
         const auto& w = m->host[std::string("fb_model") + sfx[b] + ".fc_output_layer.weight"];
         const auto& bb = m->host[std::string("fb_model") + sfx[b] + ".fc_output_layer.bias"];
@@ -326,16 +360,24 @@ static int pack_tcn5(fsn_model* m) {
             Bfc[(size_t)b * Cp + n] = bb[n];
         }
     }
-    if (upload(m->tW1, W1.data(), W1.size() * 4) || upload(m->tW2, W2.data(), W2.size() * sizeof(__half)) || upload(m->tWfc, Wfc.data(), Wfc.size() * 4) ||
-        upload(m->tS1, S1.data(), S1.size() * 4) || upload(m->tS2b, S2b.data(), S2b.size() * 4) || upload(m->tBfc, Bfc.data(), Bfc.size() * 4))
+    if (upload(m->tWfc, Wfc.data(), Wfc.size() * 4) || upload(m->tBfc, Bfc.data(), Bfc.size() * 4))
         return fail(FSN_ECUDA, "upload of the TCN weights failed");
-    for (int blk = 0; blk < 8; ++blk) {
-        if (make_tmap_f32_2d(m->mapW1[blk], static_cast<float*>(m->tW1.p) + (size_t)blk * 3 * Hd * Cp, 3 * Hd, Cp, 128) ||
-            make_tmap_f16_2d(m->mapW2[blk], static_cast<__half*>(m->tW2.p) + (size_t)blk * 3 * Cp * Hd, 3 * Cp, Hd, m->tcnNT))
-            return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the TCN weights");
-    }
     if (make_tmap_f32_2d(m->mapWfc, m->tWfc.p, 3 * Cp, Cp, m->tcnNT)) return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed (fc)");
     m->tcn5 = true;
+    return FSN_OK;
+}
+
+// the sub-band TCN (sequence_model = "TCN"): one branch of Isb <= 64 channels padded to 64, and its Linear(Isb -> O) as [O][64] fp32
+// (read by the GLN_HEAD epilogue)
+static int pack_sb_tcn(fsn_model* m) {
+    const int I = m->Isb, O = m->cfg.output_size;
+    int rc = pack_tcn_blocks(m, {"sb_model.sequence_model."}, I, 64, 64, m->sW1, m->sW2, m->sS1, m->sS2b, m->smapW1, m->smapW2);
+    if (rc) return rc;
+    std::vector<float> fc((size_t)O * 64, 0.f);
+    const auto& w = m->host["sb_model.fc_output_layer.weight"];
+    for (int o = 0; o < O; ++o)
+        for (int k = 0; k < I; ++k) fc[(size_t)o * 64 + k] = w[(size_t)o * I + k];
+    if (upload(m->sFc, fc.data(), fc.size() * 4)) return fail(FSN_ECUDA, "upload of the sub-band TCN head failed");
     return FSN_OK;
 }
 
@@ -352,8 +394,10 @@ extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
     if (c.num_freqs > 2048) return fail(FSN_EINVAL, "num_freqs > 2048 is not supported");
     if (c.num_freqs < 4 || c.look_ahead < 0 || c.sb_num_neighbors < 0 || c.fb_num_neighbors < 0) return fail(FSN_EINVAL, "bad geometry");
     if (c.sb_num_neighbors >= c.num_freqs || c.fb_num_neighbors >= c.num_freqs) return fail(FSN_EINVAL, "reflect padding needs neighbors < num_freqs");
+    if (c.sb_tcn != 0 && c.sb_tcn != 1) return fail(FSN_EINVAL, "sb_tcn must be 0 or 1");
+    if (c.sb_tcn && c.model_kind != FSN_KIND_PLUS) return fail(FSN_EINVAL, "a TCN sub-band model needs FullSubNet_Plus (fullsubnet.Model asserts GRU / LSTM)");
     if (c.num_layers < 1 || c.num_layers > 4) return fail(FSN_EINVAL, "num_layers must be 1..4");
-    if (c.sb_hidden % 16 || c.sb_hidden < 16) return fail(FSN_EINVAL, "sb_model_hidden_size must be a multiple of 16");
+    if (!c.sb_tcn && (c.sb_hidden % 16 || c.sb_hidden < 16)) return fail(FSN_EINVAL, "sb_model_hidden_size must be a multiple of 16");
     if (c.model_kind == FSN_KIND_FSN && (c.fb_hidden % 16 || c.fb_hidden < 16)) return fail(FSN_EINVAL, "fb_model_hidden_size must be a multiple of 16");
     if (c.output_size < 1 || c.output_size > 8) return fail(FSN_EINVAL, "output_size must be 1..8");
     if (c.rnn_type != FSN_RNN_LSTM && c.rnn_type != FSN_RNN_GRU) return fail(FSN_EINVAL, "unknown rnn_type %d", c.rnn_type);
@@ -366,6 +410,8 @@ extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
         for (int i = 0; i < 3; ++i)
             if (c.channel_attention == FSN_ATTN_TSSE && (c.kersize[i] < 1 || c.kersize[i] > 16)) return fail(FSN_EINVAL, "kersize must be in 1..16");
     }
+    const int isb = (2 * c.sb_num_neighbors + 1) + (c.model_kind == FSN_KIND_PLUS ? 3 : 1) * (2 * c.fb_num_neighbors + 1);
+    if (isb > 64) return fail(FSN_EINVAL, "sub-band input size %d > 64 not supported", isb);
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(FSN_ECUDA, "no CUDA device: fsnplus_b200 has no CPU fallback");
     fsn_model* m = new fsn_model();
@@ -381,7 +427,6 @@ extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
     build_specs(m);
     for (int i = 0; i < fsn_model::NEV; ++i) { cudaEventCreate(&m->ev0[i]); cudaEventCreate(&m->ev1[i]); cudaEventCreate(&m->evf0[i]); cudaEventCreate(&m->evf1[i]); }
     { cudaDeviceProp prop; int dev = 0; cudaGetDevice(&dev); if (cudaGetDeviceProperties(&prop, dev) == cudaSuccess) m->num_sms = prop.multiProcessorCount; }
-    if (m->Isb > 64) { delete m; return fail(FSN_EINVAL, "sub-band input size %d > 64 not supported", m->Isb); }
     *out = m;
     return FSN_OK;
 }
@@ -390,7 +435,8 @@ extern "C" void fsn_model_destroy(fsn_model* m) {
     if (!m) return;
     cudaDeviceSynchronize();
     DevBuf* all[] = {&m->arena, &m->cstate, &m->mask_tmp, &m->stage_in[0], &m->stage_in[1], &m->stage_in[2],
-                     &m->stage_out, &m->tW1, &m->tW2, &m->tWfc, &m->tS1, &m->tS2b, &m->tBfc, &m->ws_h, &m->ws_bar};
+                     &m->stage_out, &m->tW1, &m->tW2, &m->tWfc, &m->tS1, &m->tS2b, &m->tBfc, &m->ws_h, &m->ws_bar,
+                     &m->sW1, &m->sW2, &m->sS1, &m->sS2b, &m->sFc, &m->sb_xa, &m->sb_xb, &m->sb_y1, &m->sb_y2, &m->sb_stats};
     for (auto* b : all) b->release();
     for (auto& ln : m->lane) {
         ln.release_all();
@@ -439,7 +485,7 @@ extern "C" int fsn_model_finalize(fsn_model* m) {
     for (const auto& s : m->specs)
         if (!m->host.count(s.key)) return fail(FSN_ESTATE, "missing parameter %s", s.key.c_str());
     if (c.rnn_type == FSN_RNN_GRU) {
-        expand_gru(m, "sb_model", m->Isb, c.sb_hidden, c.num_layers);
+        if (!c.sb_tcn) expand_gru(m, "sb_model", m->Isb, c.sb_hidden, c.num_layers);
         if (c.model_kind == FSN_KIND_FSN) expand_gru(m, "fb_model", c.num_freqs, c.fb_hidden, c.num_layers);
     }
     size_t total = 0;
@@ -453,12 +499,12 @@ extern "C" int fsn_model_finalize(fsn_model* m) {
         m->dev[s.key] = d;
         off += (hv.size() * 4 + 255) & ~(size_t)255;
     }
-    if (pack_lstm(m, "sb_model", m->Isb, 64, c.sb_hidden, c.num_layers, m->sb_frag, m->sb_bias)) return fail(FSN_ECUDA, "packing sb_model failed");
+    if (!c.sb_tcn && pack_lstm(m, "sb_model", m->Isb, 64, c.sb_hidden, c.num_layers, m->sb_frag, m->sb_bias)) return fail(FSN_ECUDA, "packing sb_model failed");
     if (c.model_kind == FSN_KIND_FSN) {
         const int Ipad = (c.num_freqs + 15) / 16 * 16;
         if (pack_lstm(m, "fb_model", c.num_freqs, Ipad, c.fb_hidden, c.num_layers, m->fb_frag, m->fb_bias)) return fail(FSN_ECUDA, "packing fb_model failed");
     }
-    m->tc5r_ok = lstm_tc5r_supported(c.sb_hidden, c.output_size) && m->Isb <= 64;
+    m->tc5r_ok = !c.sb_tcn && lstm_tc5r_supported(c.sb_hidden, c.output_size) && m->Isb <= 64;
     if (m->tc5r_ok) {
         const int H = c.sb_hidden;
         for (int l = 0; l < c.num_layers; ++l) {
@@ -481,6 +527,10 @@ extern "C" int fsn_model_finalize(fsn_model* m) {
     }
     if (c.model_kind == FSN_KIND_PLUS) {
         int rc = pack_tcn5(m);
+        if (rc) return rc;
+    }
+    if (c.sb_tcn) {
+        int rc = pack_sb_tcn(m);
         if (rc) return rc;
     }
     m->finalized = true;
@@ -526,13 +576,35 @@ static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, cudaStream
     e |= ln.tsse_scale.ensure((size_t)nbr * B * F * 4 * (1 + tsse_row_floats()), true, s);      // per-row scale | row statistics
     e |= ln.sb_rowsum.ensure((size_t)B * 4 * F * 2 * 4, true, s);
     if (c.norm_type != FSN_NORM_OFFLINE_LAPLACE) e |= ln.xn.ensure((size_t)nbr * B * F * Tp * 4, true, s);
-    // images are re-zeroed whenever the geometry changes (rows beyond B*F and k >= I must stay zero)
-    const size_t img_bytes = (size_t)ntiles * Tp * 16384;
-    if (regeo) { ln.ximg.release(); }
-    e |= ln.ximg.ensure(img_bytes, true, s);
+    if (c.sb_tcn) {
+        // sub-band TCN: the lane's packed input (+ block 0's stream maxima), the shared scratch of the blocks (serialised on the sub-band
+        // stream like the LSTM scratch); every buffer is fully written before it is read (the pad columns by the packer / the epilogue)
+        const long long srows = (long long)B * F * Tp;
+        if (srows + 128 > 0x7fffffffLL) return fail(FSN_EINVAL, "B * num_freqs * (T + look_ahead) = %lld rows exceeds the sub-band TCN's 2^31 limit", srows);
+        if (regeo) ln.sbx.release();
+        e |= ln.sbx.ensure((size_t)srows * 64 * 4 + (size_t)B * F * 4, false, s);
+        e |= m->sb_xa.ensure((size_t)srows * 64 * 4, false, sl);
+        e |= m->sb_xb.ensure((size_t)srows * 64 * 4, false, sl);
+        e |= m->sb_y1.ensure((size_t)srows * 512 * sizeof(__half), false, sl);
+        e |= m->sb_y2.ensure((size_t)srows * 512 * sizeof(__half), false, sl);
+        e |= m->sb_stats.ensure((size_t)8 * 2 * B * F * 2 * sizeof(double) + (size_t)8 * B * F * sizeof(float), false, sl);
+        if (e) return fail(FSN_ECUDA, "workspace allocation failed for B=%d T=%d", B, T);
+        if (regeo && make_tmap_f32_2d(ln.mapSbx, ln.sbx.p, srows, 64, 128)) return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the sub-band input");
+        if (m->sb_rows != srows) {
+            if (make_tmap_f32_2d(m->mapSbXa, m->sb_xa.p, srows, 64, 128) || make_tmap_f32_2d(m->mapSbXb, m->sb_xb.p, srows, 64, 128) ||
+                make_tmap_f16_2d(m->mapSbY2, m->sb_y2.p, srows, 512, 128))
+                return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the sub-band TCN");
+            m->sb_rows = srows;
+        }
+    } else {
+        // images are re-zeroed whenever the geometry changes (rows beyond B*F and k >= I must stay zero)
+        const size_t img_bytes = (size_t)ntiles * Tp * 16384;
+        if (regeo) { ln.ximg.release(); }
+        e |= ln.ximg.ensure(img_bytes, true, s);
+    }
     // LSTM-side scratch: shared by both lanes (LSTM launches are serialised on the LSTM stream)
     int ra = 0;
-    size_t cs = lstm_mma_cstate_bytes(c.num_layers, rows, c.sb_hidden, &ra);
+    size_t cs = c.sb_tcn ? 0 : lstm_mma_cstate_bytes(c.num_layers, rows, c.sb_hidden, &ra);
     size_t cs5 = 0;
     if (use_layerwise(m)) {
         const size_t M = (size_t)ntiles * Tp * 128;
@@ -547,7 +619,7 @@ static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, cudaStream
         const size_t csf = lstm_mma_cstate_bytes(c.num_layers, B, c.fb_hidden, &ra2);
         if (csf > cs) cs = csf;
     }
-    e |= m->cstate.ensure(cs > cs5 ? cs : cs5, true, sl);
+    if (cs || cs5) e |= m->cstate.ensure(cs > cs5 ? cs : cs5, true, sl);
     if (c.model_kind == FSN_KIND_PLUS) {
         if (!m->tcn5) return fail(FSN_ESTATE, "the TCN weights were not packed");
         const size_t trows = (size_t)3 * B * Tp;
@@ -640,6 +712,69 @@ static int run_sb_lstm(fsn_model* m, fsn_model::Lane& ln, int B, int T, float* d
         if (d_enh) { launch_apply_cirm_planar(a.out, d_real, d_imag, reinterpret_cast<float2*>(d_enh), B, F, T, s); m->launches++; }
     }
     m->launches++;
+    return FSN_OK;
+}
+
+// The sub-band TCN (sequence_model = "TCN", fullsubnet_plus.py:102-110): the eight TCN blocks of the full band with one branch, the
+// B*F sequences of the sub-band input as the gLN groups and Isb (<= 64) channels in one 64-column N tile; the last block's second 1x1
+// convolution ends in ReLU + Linear + activation (EPI5_GLN_HEAD) and writes the mask -- or, with d_enh, the enhanced spectrum.
+static int run_sb_tcn(fsn_model* m, fsn_model::Lane& ln, int B, int T, float* d_out, const float* d_real, const float* d_imag, float* d_enh,
+                      cudaStream_t s) {
+    const fsn_config& c = m->cfg;
+    const int F = c.num_freqs, Tp = T + c.look_ahead, Z = B * F;
+    m->last_impl = FSN_LSTM_TCN;
+    double* stats = static_cast<double*>(m->sb_stats.p);
+    float* amax = reinterpret_cast<float*>(stats + (size_t)8 * 2 * Z * 2);              // [8][Z]: max |x| of the stream entering block k (k >= 1)
+    const float* amax0 = reinterpret_cast<const float*>(static_cast<float*>(ln.sbx.p) + (size_t)Z * Tp * 64);
+    CK(cudaMemsetAsync(stats, 0, (size_t)8 * 2 * Z * 2 * sizeof(double) + (size_t)8 * Z * sizeof(float), s));
+    static const int dil[8] = {1, 2, 5, 9, 1, 2, 5, 9};             // sequence_model.py:47-58
+    GemmTc5Launch g{};
+    g.rows_per_branch = Z * Tp; g.tiles_m = (Z * Tp + 127) / 128; g.nbranch = 1; g.Tp = Tp; g.B = Z;
+    const float* curp = static_cast<const float*>(ln.sbx.p);
+    const unsigned char* curmap = ln.mapSbx;
+    for (int blk = 0; blk < 8; ++blk) {
+        double* st1 = stats + (size_t)(2 * blk) * Z * 2;
+        double* st2 = stats + (size_t)(2 * blk + 1) * Z * 2;
+        const float* amax_in = blk ? amax + (size_t)blk * Z : amax0;
+        auto key = [&](const char* leaf) { return std::string("sb_model.sequence_model.") + std::to_string(blk) + "." + leaf; };
+        GemmTc5Launch g1 = g;
+        g1.epi = EPI5_PRELU_STATS; g1.Kp = 64; g1.NT = 128; g1.ntiles_n = 4; g1.Npad = 512;
+        g1.bias[0] = P(m, key("conv1x1.bias")); g1.prelu[0] = P(m, key("prelu1.weight"));
+        g1.stats_out = st1; g1.Y16 = static_cast<__half*>(m->sb_y1.p); g1.ldY = 512; g1.amax_in = amax_in;
+        int e = launch_gemm_tc5(curmap, m->smapW1[blk], g1, m->num_sms, s);
+        if (e) return fail(FSN_ECUDA, "sub-band TCN GEMM1 launch failed: %s", cudaGetErrorString((cudaError_t)e));
+        m->launches++;
+
+        DwTmLaunch dw{};
+        dw.X = static_cast<const __half*>(m->sb_y1.p); dw.Y = static_cast<__half*>(m->sb_y2.p);
+        dw.Z = Z; dw.B = Z; dw.C = 512; dw.Tp = Tp; dw.dilation = dil[blk]; dw.causal = 0;
+        dw.stats_in = st1; dw.stats_out = st2; dw.amax = amax_in;
+        dw.gamma[0] = P(m, key("norm1.weight")); dw.beta[0] = P(m, key("norm1.bias"));
+        dw.w[0] = P(m, key("depthwise_conv.weight")); dw.b[0] = P(m, key("depthwise_conv.bias")); dw.prelu[0] = P(m, key("prelu2.weight"));
+        e = launch_dwconv_tm(dw, s);
+        if (e) return fail(FSN_ECUDA, "sub-band TCN depth-wise conv launch failed: %s", cudaGetErrorString((cudaError_t)e));
+        m->launches++;
+
+        float* nxtp = (blk & 1) ? static_cast<float*>(m->sb_xb.p) : static_cast<float*>(m->sb_xa.p);
+        GemmTc5Launch g2 = g;
+        g2.epi = blk < 7 ? EPI5_GLN_RES : EPI5_GLN_HEAD; g2.Kp = 512; g2.NT = 64; g2.ntiles_n = 1; g2.Npad = 64;
+        g2.bias[0] = static_cast<const float*>(m->sS2b.p) + (size_t)blk * 64;
+        g2.s1[0] = static_cast<const float*>(m->sS1.p) + (size_t)blk * 64;
+        g2.stats_in = st2; g2.count_in = (double)512 * Tp;
+        g2.Xold = curp; g2.ldY = 64;
+        if (blk < 7) {
+            g2.Y = nxtp; g2.amax_out = amax + (size_t)(blk + 1) * Z;
+        } else {
+            g2.fc_w = static_cast<const float*>(m->sFc.p); g2.fc_b = P(m, "sb_model.fc_output_layer.bias");
+            g2.O = c.output_size; g2.la = c.look_ahead; g2.F = F; g2.act = c.sb_act;
+            g2.out = d_out; g2.nreal = d_real; g2.nimag = d_imag; g2.enh = reinterpret_cast<float2*>(d_enh);
+        }
+        e = launch_gemm_tc5(m->mapSbY2, m->smapW2[blk], g2, m->num_sms, s);
+        if (e) return fail(FSN_ECUDA, "sub-band TCN GEMM2 launch failed: %s", cudaGetErrorString((cudaError_t)e));
+        m->launches++;
+        curp = nxtp;
+        curmap = (blk & 1) ? m->mapSbXb : m->mapSbXa;
+    }
     return FSN_OK;
 }
 
@@ -832,14 +967,21 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
         sp.fb[0] = static_cast<const float*>(ln.fbout.p);
     }
     launch_sb_stats(sp, s); m->launches += 2;
-    launch_sb_pack(sp, s); m->launches++;
+    if (c.sb_tcn) {
+        sp.xtm = static_cast<float*>(ln.sbx.p);
+        sp.amax = sp.xtm + (size_t)B * F * Tp * 64;
+        launch_sb_pack_tm(sp, s);
+    } else {
+        launch_sb_pack(sp, s);
+    }
+    m->launches++;
     cudaEventRecord(m->evf1[evi], s);
     if (sl != s) {                                                      // pipelined: the LSTM stream picks the lane up when the front end is done
         CK(cudaEventRecord(ln.ev_front, s));
         CK(cudaStreamWaitEvent(sl, ln.ev_front, 0));
     }
     cudaEventRecord(m->ev0[evi], sl);
-    rc = run_sb_lstm(m, ln, B, T, d_out, d_real, d_imag, d_enh, sl);
+    rc = c.sb_tcn ? run_sb_tcn(m, ln, B, T, d_out, d_real, d_imag, d_enh, sl) : run_sb_lstm(m, ln, B, T, d_out, d_real, d_imag, d_enh, sl);
     cudaEventRecord(m->ev1[evi], sl);
     if (rc) return rc;
     m->nfwd++;
@@ -895,6 +1037,10 @@ static double ws_bytes_per_sample(const fsn_model* m, int T) {
     double b = 0;
     if (c.model_kind == FSN_KIND_PLUS) b += 3 * F * Tp * 4 * 2 + 3 * Tp * (4.0 * m->Cp + 512) * 4;       // fb_in/out, X0/Xa/Xb/Xr (fp32), Y1/Y2 (fp16)
     else b += F * Tp * 4 * 4 + Tp * (F + c.fb_hidden) * 4;
+    if (c.sb_tcn) {                                                             // input + two fp32 streams of 64 channels, two fp16 hidden
+        b += rows * Tp * (3 * 64 * 4 + 2 * 512 * 2) + rows * (8 * 2 * 2 * 8 + 9 * 4);   // buffers of 512; gLN sums and stream maxima
+        return b;
+    }
     b += rows * Tp * 128;                                                       // packed sub-band images (when used)
     b += rows * c.num_layers * c.sb_hidden * 4;                                  // cell state
     if (use_layerwise(m) && c.num_layers > 1) b += rows * Tp * (4.0 * c.sb_hidden + c.sb_hidden) * 2;   // Gin + layer output sequence
@@ -1073,6 +1219,13 @@ extern "C" int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst,
         if (numel != (int64_t)nbr * B * F * Tp) return fail(FSN_EINVAL, "%s needs %lld elements", name, (long long)nbr * B * F * Tp);
         const void* src = (n == "fb_in") ? ln.fbin.p : ln.fbout.p;
         CK(cudaMemcpy2DAsync(d_dst, (size_t)Tp * 4, src, (size_t)Pp * 4, (size_t)Tp * 4, (size_t)nbr * B * F, cudaMemcpyDeviceToDevice, s));
+        return FSN_OK;
+    }
+    if (n == "sb_in") {
+        if (!c.sb_tcn) return fail(FSN_EINVAL, "sb_in is kept only by the sub-band TCN (sequence_model = \"TCN\")");
+        if (numel != (int64_t)B * F * m->Isb * Tp) return fail(FSN_EINVAL, "sb_in needs %lld elements", (long long)B * F * m->Isb * Tp);
+        launch_tm_to_fm(static_cast<const float*>(ln.sbx.p), 64, d_dst, B * F, m->Isb, Tp, s);
+        CK(cudaGetLastError());
         return FSN_OK;
     }
     if (n == "sb_mu") {

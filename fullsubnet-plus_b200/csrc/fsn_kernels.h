@@ -76,9 +76,15 @@ struct SbPackLaunch {
     int norm_type;           // FSN_NORM_*
     __half* ximg;            // [ntiles, Tp, 128 rows, 64 halves] SWIZZLE_128B images
     int ntiles;
+    float* xtm;              // sub-band TCN input: fp32 time-major [B*F*Tp, 64], row (b*F + f)*Tp + t, columns >= I zero
+    float* amax;             // [B*F] max |x| of every sequence of xtm (zeroed by the launcher): block 0's fp16 store scale
 };
 void launch_sb_stats(const SbPackLaunch& a, cudaStream_t s);
 void launch_sb_pack(const SbPackLaunch& a, cudaStream_t s);
+// the same normalised values as launch_sb_pack, written to a.xtm / a.amax instead of the fp16 images
+void launch_sb_pack_tm(const SbPackLaunch& a, cudaStream_t s);
+// time-major [Z*Tp, ld] -> [Z, C, Tp] (test hook of the sub-band TCN input)
+void launch_tm_to_fm(const float* x, int ld, float* y, int Z, int C, int Tp, cudaStream_t s);
 // [B, F, T] fp32 (+ zero look-ahead pad) -> zero-padded copy [B, F, P]
 void launch_pad_copy(const float* x, float* y, int B, int F, int T, int P, cudaStream_t s);
 // full-band LSTM input: [B, F, P] fp32 -> [Tp, Bpad, Ipad] fp16 (rows >= B and k >= F zero)
@@ -172,7 +178,7 @@ bool gemm_f16_supported(long long M, int N, int K);
 int launch_gemm_f16(const void* A, const void* B, const GemmF16Launch& a, int num_sms, cudaStream_t s);
 int make_tmap_f16_2d(void* out_map /*128 B, 64 B aligned*/, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows);   // box = 64 halves x box_rows, SWIZZLE_128B
 
-enum { EPI5_PRELU_STATS = 1, EPI5_GLN_RES = 2, EPI5_OUT = 3, EPI5_F16OUT = 4 };
+enum { EPI5_PRELU_STATS = 1, EPI5_GLN_RES = 2, EPI5_OUT = 3, EPI5_F16OUT = 4, EPI5_GLN_HEAD = 5 };
 struct GemmTc5Launch {
     int Kp, NT, nstage, ntiles_n, Npad;        // K (multiple of 32; GLN_RES: fp16 operands, multiple of 64), N tile (64 or 128), ring depth, N tiles and padded N per branch
     int rows_per_branch, tiles_m, nbranch, Tp, B;
@@ -187,13 +193,18 @@ struct GemmTc5Launch {
     const float* amax_in;                      // PRELU_STATS: [Z] max |x| of the block's input stream per sample
     float* amax_out;                           // GLN_RES: [Z] max |x| of the new stream per sample (atomicMax on the bit pattern; zeroed by the caller)
     const float* Xold; float* Xrelu;           // GLN_RES: residual input, optional relu'd copy
-    float* out; int F, P, act;                 // OUT: [Z, F, P] (frequency-major)
+    float* out; int F, P, act;                 // OUT: [Z, F, P] (frequency-major); GLN_HEAD: mask [B, O, F, Tp - la]
+    // GLN_HEAD (last block of the sub-band TCN, one 64-column N tile): GLN_RES's new stream x, then act(Linear(relu(x))) per row;
+    // rows are (b * F + f) * Tp + t.  With enh != null: decompress_cIRM x the noisy planes [B, F, Tp - la] into enh instead of the mask
+    const float* fc_w; const float* fc_b;      // [O, 64] (columns >= I zero), [O]
+    int O, la;
+    const float* nreal; const float* nimag; float2* enh;
 };
 int make_tmap_f32_2d(void* out_map /*128 B, 64 B aligned*/, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows);
 int launch_gemm_tc5(const void* mapA, const void* mapB, GemmTc5Launch a, int num_sms, cudaStream_t s);
 struct DwTmLaunch {
     const __half* X; __half* Y;                // [Z * Tp, C] hidden activations, fp16
-    int Z, B, C, Tp, dilation;
+    int Z, B, C, Tp, dilation;                 // Z groups (sequences), branch of group z = z / B
     int causal;                                // 1: taps t-2d, t-d, t (TCNBlock(causal=True)); 0: t-d, t, t+d
     const double* stats_in; double* stats_out;
     const float* amax;                         // [Z]: X holds the activation times fp16_store_scale(amax[z]); the statistics are unscaled

@@ -451,10 +451,43 @@ void launch_sb_stats(const SbPackLaunch& a, cudaStream_t s) {
     launch_chain(sb_stats_kernel, dim3(a.B), dim3(256), 0, s, a);
 }
 
+// Stores of the normalised sub-band input.  Fp16Img: the SWIZZLE_128B images of the LSTM kernels (values clamped to the fp16
+// range).  Fp32Tm: the sub-band TCN's time-major fp32 rows of 64 channels, plus max |x| per sequence (block 0's fp16 store scale).
+// Both packers compute every value once and hand 8 consecutive channels k0 .. k0 + 7 of (sequence row, frame t) to store().
+struct Fp16Img {
+    static __device__ __forceinline__ void store(const SbPackLaunch& a, int row, int t, int k0, const float (&v)[8]) {
+        float w[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) w[i] = fminf(fmaxf(v[i], -65504.f), 65504.f);
+        char* img = reinterpret_cast<char*>(a.ximg) + ((size_t)(row >> 7) * a.Tp + t) * (128 * 128);
+        *reinterpret_cast<uint4*>(img + sw128_offset(row & 127, k0)) =
+            make_uint4(pack_half2(w[0], w[1]), pack_half2(w[2], w[3]), pack_half2(w[4], w[5]), pack_half2(w[6], w[7]));
+    }
+    static __device__ __forceinline__ void finish(const SbPackLaunch&, int, float, unsigned) {}
+};
+struct Fp32Tm {
+    static __device__ __forceinline__ void store(const SbPackLaunch& a, int row, int t, int k0, const float (&v)[8]) {
+        float4* dst = reinterpret_cast<float4*>(a.xtm + ((size_t)row * a.Tp + t) * 64 + k0);
+        dst[0] = make_float4(v[0], v[1], v[2], v[3]);
+        dst[1] = make_float4(v[4], v[5], v[6], v[7]);
+    }
+    // max over the lanes of `group` (lanes that share the sequence row), one atomic per group (values >= 0: int order = float order)
+    static __device__ __forceinline__ void finish(const SbPackLaunch& a, int row, float m, unsigned width) {
+        for (unsigned o = 1; o < width; o <<= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+        if ((threadIdx.x & (width - 1)) == 0 && row >= 0) atomicMax(reinterpret_cast<int*>(a.amax + row), __float_as_int(m));
+    }
+};
+__device__ __forceinline__ float vmax8(float m, const float (&v)[8]) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) m = fmaxf(m, fabsf(v[i]));
+    return m;
+}
+
 // One CTA = (sample, 32 consecutive bins, 32 frames).  The window source rows [f0 - Ns, f0 + 31 + Ns] (reflected) and the
-// full-band rows of the 32 bins are staged once in shared memory; work item = (bin, frame, 16-byte chunk of the 128-byte
-// image row), so 8 consecutive lanes write one full 128-byte line of the SWIZZLE_128B image.
+// full-band rows of the 32 bins are staged once in shared memory; work item = (bin, frame, 8 channels), so 8 consecutive lanes
+// write one whole row of 64 channels (one 128-byte line of the SWIZZLE_128B image).
 constexpr int SBP_F = 32, SBP_T = 32;
+template <class Store>
 __global__ void __launch_bounds__(256) sb_pack_kernel(SbPackLaunch a) {
     extern __shared__ float sm[];
     const int F = a.F, Tp = a.Tp, b = blockIdx.z, f0 = blockIdx.y * SBP_F, t0 = blockIdx.x * SBP_T;
@@ -481,36 +514,38 @@ __global__ void __launch_bounds__(256) sb_pack_kernel(SbPackLaunch a) {
     __syncthreads();
     const int c = threadIdx.x & 7, fr = threadIdx.x >> 3;          // chunk, bin inside the tile
     const int f = f0 + fr;
-    if (f >= F) return;
-    const int row = b * F + f, tile = row >> 7, r = row & 127;
+    const bool live = f < F;
+    const int row = b * F + f;
     auto val = [&](int k, int tt) -> float {
         float v = 0.f;
         if (k < nw) v = wsm[(fr + k) * (SBP_T + 1) + tt];
         else if (k < I) { const int kk = k - nw, q = kk / nf, j = kk % nf; v = fsm[(q * frows + fr + j) * (SBP_T + 1) + tt]; }
-        return (k < I) ? fminf(fmaxf((v - sub) * inv, -65504.f), 65504.f) : 0.f;
+        return (k < I) ? (v - sub) * inv : 0.f;
     };
-    for (int tt = 0; tt < SBP_T && t0 + tt < Tp; ++tt) {
-        uint4 u;
-        u.x = pack_half2(val(c * 8 + 0, tt), val(c * 8 + 1, tt));
-        u.y = pack_half2(val(c * 8 + 2, tt), val(c * 8 + 3, tt));
-        u.z = pack_half2(val(c * 8 + 4, tt), val(c * 8 + 5, tt));
-        u.w = pack_half2(val(c * 8 + 6, tt), val(c * 8 + 7, tt));
-        char* img = reinterpret_cast<char*>(a.ximg) + ((size_t)tile * Tp + t0 + tt) * (128 * 128);
-        *reinterpret_cast<uint4*>(img + sw128_offset(r, c * 8)) = u;
+    float m = 0.f;
+    for (int tt = 0; live && tt < SBP_T && t0 + tt < Tp; ++tt) {
+        float v[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] = val(c * 8 + i, tt);
+        m = vmax8(m, v);
+        Store::store(a, row, t0 + tt, c * 8, v);
     }
+    Store::finish(a, live ? row : -1, m, 8);
 }
 
 // Cumulative norms of the 4-D sub-band input (base_model.py:227-258 / :277-316 with dim 1 = F folded into the batch): every
 // sequence (b, f) is normalised by the running mean (and std) over its I channels.  One warp per sequence, lanes over
 // frames, warp scan with carry.
+template <class Store>
 __global__ void __launch_bounds__(128) sb_pack_cum_kernel(SbPackLaunch a) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int row = blockIdx.x * 4 + warp, F = a.F, Tp = a.Tp;
     if (row >= a.B * F) return;
-    const int b = row / F, f = row % F, tile = row >> 7, r = row & 127;
+    const int b = row / F, f = row % F;
     const int nw = 2 * a.Ns + 1, nf = 2 * a.Nf + 1, I = nw + a.nfb * nf;
     const double EPS = 1.1920928955078125e-07;
     double cs = 0.0, cq = 0.0;                                   // running sums carried across 32-frame chunks
+    float mx = 0.f;
     for (int t0 = 0; t0 < Tp; t0 += 32) {
         const int t = t0 + lane;
         float v[64];
@@ -541,28 +576,45 @@ __global__ void __launch_bounds__(128) sb_pack_cum_kernel(SbPackLaunch a) {
         else { const double cv = (dq - 2.0 * cm * ds) / cnt + cm * cm; const double inv = 1.0 / sqrt(cv + EPS); sc = (float)inv; sh = (float)(-cm * inv); }
         cs = __shfl_sync(0xffffffffu, ds, 31); cq = __shfl_sync(0xffffffffu, dq, 31);
         if (t < Tp) {
-            char* img = reinterpret_cast<char*>(a.ximg) + ((size_t)tile * Tp + t) * (128 * 128);
 #pragma unroll
             for (int c = 0; c < 8; ++c) {
                 float w[8];
 #pragma unroll
-                for (int i = 0; i < 8; ++i) w[i] = (c * 8 + i < I) ? fminf(fmaxf(fmaf(v[c * 8 + i], sc, sh), -65504.f), 65504.f) : 0.f;
-                *reinterpret_cast<uint4*>(img + sw128_offset(r, c * 8)) =
-                    make_uint4(pack_half2(w[0], w[1]), pack_half2(w[2], w[3]), pack_half2(w[4], w[5]), pack_half2(w[6], w[7]));
+                for (int i = 0; i < 8; ++i) w[i] = (c * 8 + i < I) ? fmaf(v[c * 8 + i], sc, sh) : 0.f;
+                mx = vmax8(mx, w);
+                Store::store(a, row, t, c * 8, w);
             }
         }
     }
+    Store::finish(a, row, mx, 32);
 }
 
-void launch_sb_pack(const SbPackLaunch& a, cudaStream_t s) {
+template <class Store>
+static void sb_pack_go(const SbPackLaunch& a, cudaStream_t s) {
     if (a.norm_type == FSN_NORM_CUMULATIVE_LAPLACE || a.norm_type == FSN_NORM_CUMULATIVE_LAYER)
-        sb_pack_cum_kernel<<<(a.B * a.F + 3) / 4, 128, 0, s>>>(a);
+        sb_pack_cum_kernel<Store><<<(a.B * a.F + 3) / 4, 128, 0, s>>>(a);
     else
     {
         const size_t smem = sizeof(float) * (SBP_T + 1) * ((SBP_F + 2 * a.Ns) + a.nfb * (SBP_F + 2 * a.Nf));
-        cudaFuncSetAttribute(sb_pack_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        sb_pack_kernel<<<dim3((a.Tp + SBP_T - 1) / SBP_T, (a.F + SBP_F - 1) / SBP_F, a.B), 256, smem, s>>>(a);
+        cudaFuncSetAttribute(sb_pack_kernel<Store>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        sb_pack_kernel<Store><<<dim3((a.Tp + SBP_T - 1) / SBP_T, (a.F + SBP_F - 1) / SBP_F, a.B), 256, smem, s>>>(a);
     }
+}
+void launch_sb_pack(const SbPackLaunch& a, cudaStream_t s) { sb_pack_go<Fp16Img>(a, s); }
+void launch_sb_pack_tm(const SbPackLaunch& a, cudaStream_t s) {
+    cudaMemsetAsync(a.amax, 0, (size_t)a.B * a.F * sizeof(float), s);
+    sb_pack_go<Fp32Tm>(a, s);
+}
+
+__global__ void tm_to_fm_kernel(const float* x, int ld, float* y, int Z, int C, int Tp) {
+    const size_t n = (size_t)Z * C * Tp;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t t = i % Tp, c = (i / Tp) % C, z = i / ((size_t)Tp * C);
+        y[i] = x[(z * Tp + t) * ld + c];
+    }
+}
+void launch_tm_to_fm(const float* x, int ld, float* y, int Z, int C, int Tp, cudaStream_t s) {
+    tm_to_fm_kernel<<<1024, 256, 0, s>>>(x, ld, y, Z, C, Tp);
 }
 
 

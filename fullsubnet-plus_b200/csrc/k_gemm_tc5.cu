@@ -1,6 +1,7 @@
 // TCN full-band model (K3 of SURVEY.md 2a) on the Hopper tensor cores: the 1x1 convolutions of the eight TCNBlocks and the
 // output Linear as persistent wgmma GEMMs over time-major activations, plus the depth-wise convolution between them.  The same
-// GEMM kernel also computes the input projection of the layer-wise LSTM path (EPI5_F16OUT).
+// kernels run the optional sub-band TCN (sequence_model = "TCN": one branch, the B*F sequences as the gLN groups, EPI5_GLN_HEAD
+// last), and the GEMM kernel also computes the input projection of the layer-wise LSTM path (EPI5_F16OUT).
 //
 // reference: TCNBlock.forward (audio_zen/model/module/causal_conv.py:96-108) and SequenceModel.forward, TCN branch
 // (audio_zen/model/module/sequence_model.py:106-112).
@@ -21,6 +22,9 @@
 //                     Its operands (hidden activation, folded weights) are fp16: 64-element k-blocks.
 //   EPI_OUT         : + bias, output activation, transposed into [branch, B, F, T'].
 //   EPI_F16OUT      : fp16 result, row-major (Gin of the layer-wise LSTM, k_lstm_tc5r.cu).
+//   EPI_GLN_HEAD    : last block of the sub-band TCN (one 64-column N tile, so a row's channels live in one lane quad): GLN_RES's
+//                     new stream, then ReLU, Linear(I -> O) reduced over the quad, the output activation, and the mask (or the
+//                     enhanced spectrum) of frames t >= look_ahead.  The final stream never goes to memory.
 #include <cuda.h>
 
 #include "fsn_common.cuh"
@@ -114,7 +118,7 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     // reads is overwritten) before this point
     pdl_trigger();
     pdl_wait();
-    constexpr bool AH = (EPI == EPI5_GLN_RES || EPI == EPI5_F16OUT);   // fp16 operands: a 128-byte swizzle atom holds 64 k-elements instead of 32
+    constexpr bool AH = (EPI == EPI5_GLN_RES || EPI == EPI5_F16OUT || EPI == EPI5_GLN_HEAD);   // fp16 operands: a 128-byte swizzle atom holds 64 k-elements instead of 32
     constexpr int KBW = AH ? 64 : 32;
     const int nkb = a.Kp / KBW;
     const int tiles_per_branch = a.tiles_m * a.ntiles_n;
@@ -253,6 +257,63 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
 #pragma unroll
                 for (int h = 0; h < 2; ++h) g5_max_add(valid[h] ? z[h] : -1, rowmax[h], a.amax_out);
             }
+        } else if constexpr (EPI == EPI5_GLN_HEAD) {
+            static_assert(NT == 64, "the head needs all channels of a row in one lane quad");
+            const float* bias = a.bias[br];
+            const float* s1 = a.s1[br];
+            float mean[2] = {0.f, 0.f}, rstd[2] = {1.f, 1.f}, fc[2][8];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                for (int q = 0; q < 8; ++q) fc[h][q] = 0.f;
+                if (valid[h]) {
+                    const double su = a.stats_in[2 * z[h]], sq = a.stats_in[2 * z[h] + 1];
+                    const double mu = su / a.count_in, var = sq / a.count_in - mu * mu;
+                    mean[h] = (float)mu;
+                    rstd[h] = (float)(1.0 / sqrt((var > 0 ? var : 0) + 1e-8));
+                }
+            }
+#pragma unroll
+            for (int j = 0; j < NT / 8; ++j) {
+                const int n = 8 * j + cq;
+                const float2 s12 = __ldg(reinterpret_cast<const float2*>(s1 + n)), b2 = __ldg(reinterpret_cast<const float2*>(bias + n));
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    if (!valid[h]) continue;
+                    const float2 x = *reinterpret_cast<const float2*>(a.Xold + grow[h] * a.ldY + n);
+                    const float o0 = fmaxf(x.x + fmaf(rstd[h], acc[4 * j + 2 * h], fmaf(-mean[h] * rstd[h], s12.x, b2.x)), 0.f);
+                    const float o1 = fmaxf(x.y + fmaf(rstd[h], acc[4 * j + 2 * h + 1], fmaf(-mean[h] * rstd[h], s12.y, b2.y)), 0.f);
+#pragma unroll
+                    for (int q = 0; q < 8; ++q)
+                        if (q < a.O) {
+                            const float2 w = __ldg(reinterpret_cast<const float2*>(a.fc_w + q * 64 + n));
+                            fc[h][q] = fmaf(o0, w.x, fmaf(o1, w.y, fc[h][q]));
+                        }
+                }
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int q = 0; q < 8; ++q)
+#pragma unroll
+                    for (int o = 1; o < 4; o <<= 1) fc[h][q] += __shfl_xor_sync(0xffffffffu, fc[h][q], o);
+            const int Tout = a.Tp - a.la;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                if (!valid[h] || (lane & 3) != 0 || tt[h] < a.la) continue;
+                const int ob = z[h] / a.F, of = z[h] % a.F;
+                const size_t ni = ((size_t)ob * a.F + of) * Tout + (tt[h] - a.la);
+                if (a.enh) {                                   // fused decompress_cIRM x noisy spectrum (inferencer.py:152-157), O = 2
+                    const float m0 = decompress_cirm(apply_act(fc[h][0] + __ldg(a.fc_b), a.act));
+                    const float m1 = decompress_cirm(apply_act(fc[h][1] + __ldg(a.fc_b + 1), a.act));
+                    const float nr = __ldg(a.nreal + ni), nim = __ldg(a.nimag + ni);
+                    a.enh[ni] = make_float2(m0 * nr - m1 * nim, m1 * nr + m0 * nim);
+                } else {
+#pragma unroll
+                    for (int q = 0; q < 8; ++q)
+                        if (q < a.O) a.out[(((size_t)ob * a.O + q) * a.F + of) * Tout + (tt[h] - a.la)] = apply_act(fc[h][q] + __ldg(a.fc_b + q), a.act);
+                }
+            }
         } else {
             const float* bias = a.bias[br];
 #pragma unroll
@@ -319,10 +380,14 @@ static int g5_launch(const CUtensorMap& mA, const CUtensorMap& mB, GemmTc5Launch
 }
 
 int launch_gemm_tc5(const void* mapA, const void* mapB, GemmTc5Launch a, int num_sms, cudaStream_t s) {
-    if ((a.NT != 64 && a.NT != 128) || a.Kp % (a.epi == EPI5_GLN_RES ? 64 : 32) || a.Npad % 2) return (int)cudaErrorInvalidValue;
+    const bool f16k = a.epi == EPI5_GLN_RES || a.epi == EPI5_GLN_HEAD;
+    if ((a.NT != 64 && a.NT != 128) || a.Kp % (f16k ? 64 : 32) || a.Npad % 2) return (int)cudaErrorInvalidValue;
+    if (a.epi == EPI5_GLN_HEAD && (a.NT != 64 || a.Npad != 64 || a.ntiles_n != 1 || a.nbranch != 1 || a.O < 1 || a.O > 8 || (a.enh && a.O != 2)))
+        return (int)cudaErrorInvalidValue;
     const CUtensorMap& mA = *reinterpret_cast<const CUtensorMap*>(mapA);
     const CUtensorMap& mB = *reinterpret_cast<const CUtensorMap*>(mapB);
     if (a.NT == 64) {
+        if (a.epi == EPI5_GLN_HEAD) return g5_launch<EPI5_GLN_HEAD, 64>(mA, mB, a, num_sms, s);
         if (a.epi == EPI5_PRELU_STATS) return g5_launch<EPI5_PRELU_STATS, 64>(mA, mB, a, num_sms, s);
         if (a.epi == EPI5_GLN_RES) return g5_launch<EPI5_GLN_RES, 64>(mA, mB, a, num_sms, s);
         return g5_launch<EPI5_OUT, 64>(mA, mB, a, num_sms, s);
@@ -360,7 +425,8 @@ __global__ void __launch_bounds__(256) dwconv_tm_kernel(DwTmLaunch a) {
     __shared__ double red[16];
     pdl_trigger();
     pdl_wait();
-    const int z = blockIdx.z, g = z / a.B, c0 = blockIdx.x * DW_CH;
+    // grid.x = Z * (C / 64): the group count (B * F sequences for the sub-band TCN) exceeds gridDim.z's 65535
+    const int ncb = a.C / DW_CH, z = blockIdx.x / ncb, g = z / a.B, c0 = (blockIdx.x % ncb) * DW_CH;
     const int C = a.C, Tp = a.Tp, d = a.dilation;
     const int t0 = blockIdx.y * DW_TCH, t1 = min(t0 + DW_TCH, Tp);
     const int lo = max(t0 - 2 * d, 0), hi = min(t1 + 2 * d, Tp);    // staged frames [lo, hi)
@@ -432,12 +498,13 @@ __global__ void __launch_bounds__(256) dwconv_tm_kernel(DwTmLaunch a) {
 }
 
 int launch_dwconv_tm(const DwTmLaunch& a, cudaStream_t s) {
-    if (a.C % DW_CH || 2 * a.dilation > DW_HALO) return (int)cudaErrorInvalidValue;
+    if (a.C % DW_CH || 2 * a.dilation > DW_HALO || (long long)a.Z * (a.C / DW_CH) > 0x7fffffffLL || (a.Tp + DW_TCH - 1) / DW_TCH > 65535)
+        return (int)cudaErrorInvalidValue;
     const int rows = (a.Tp < DW_TCH ? a.Tp : DW_TCH + 2 * DW_HALO);
     const size_t smem = (size_t)rows * DW_CH * sizeof(float);
     cudaError_t e = cudaFuncSetAttribute(dwconv_tm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
-    e = launch_chain(dwconv_tm_kernel, dim3(a.C / DW_CH, (a.Tp + DW_TCH - 1) / DW_TCH, a.Z), dim3(256), smem, s, a);
+    e = launch_chain(dwconv_tm_kernel, dim3(a.Z * (a.C / DW_CH), (a.Tp + DW_TCH - 1) / DW_TCH, 1), dim3(256), smem, s, a);
     if (e != cudaSuccess) return (int)e;
     return (int)cudaGetLastError();
 }

@@ -29,7 +29,8 @@ class FsnConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("model_kind", "num_freqs", "look_ahead", "sb_num_neighbors", "fb_num_neighbors",
                                           "fb_hidden", "sb_hidden", "num_layers", "output_size", "fb_act", "sb_act",
                                           "norm_type")] + [("kersize", C.c_int32 * 3), ("lstm_impl", C.c_int32),
-                                                           ("fast_math", C.c_int32), ("channel_attention", C.c_int32), ("rnn_type", C.c_int32), ("subband_num", C.c_int32), ("tcn_causal", C.c_int32)]
+                                                           ("fast_math", C.c_int32), ("channel_attention", C.c_int32), ("rnn_type", C.c_int32), ("subband_num", C.c_int32), ("tcn_causal", C.c_int32),
+                                                           ("sb_tcn", C.c_int32)]
 
 
 def lib_path():

@@ -118,7 +118,7 @@ class _B200Model(nn.Module):
 
     def _setup(self, num_freqs, look_ahead, sb_num_neighbors, fb_num_neighbors, fb_hidden, sb_hidden, num_layers,
                output_size, fb_act, sb_act, norm_type, kersize, lstm_impl, fast_math, channel_attention="TSSE",
-               rnn="LSTM", subband_num=1, tcn_causal=False):
+               rnn="LSTM", subband_num=1, tcn_causal=False, sb_tcn=False):
         if norm_type not in _lib.NORM:
             raise NotImplementedError("You must set up a type of Norm. e.g. offline_laplace_norm, "
                                       "cumulative_laplace_norm, forgetting_norm, etc.")       # base_model.py:328-329
@@ -137,6 +137,7 @@ class _B200Model(nn.Module):
         cfg.rnn_type = _lib.RNN[rnn]
         cfg.subband_num = int(subband_num)
         cfg.tcn_causal = int(bool(tcn_causal))
+        cfg.sb_tcn = int(bool(sb_tcn))
         self._cfg = cfg
         self._handle = None
         self._handle_device = None
@@ -293,7 +294,7 @@ class _B200Model(nn.Module):
 
     # -- introspection used by tests / bench -----------------------------------------------------
     def last_lstm_impl(self):
-        return {0: "none", 1: "mma", 2: "tcgen05"}[_lib.load_library().fsn_model_last_lstm_impl(self._handle)] if self._handle else "none"
+        return {0: "none", 1: "mma", 2: "tcgen05", 3: "tcn"}[_lib.load_library().fsn_model_last_lstm_impl(self._handle)] if self._handle else "none"
 
     def last_lstm_ms(self):
         return float(_lib.load_library().fsn_model_last_lstm_ms(self._handle)) if self._handle else -1.0
@@ -330,11 +331,11 @@ class FullSubNet_Plus(_B200Model):
                  output_size=2, subband_num=1, kersize=[3, 5, 10], weight_init=True,
                  num_layers=2, lstm_impl="auto", fast_math=True, causal_tcn=False):
         """Reference keywords (fullsubnet_plus.py:17-34) + additive ones: num_layers (LSTM depth), lstm_impl, fast_math,
-        causal_tcn (TCNBlock(causal=True) in the full-band models, causal_conv.py:74-75,104-105; parameters unchanged)."""
+        causal_tcn (TCNBlock(causal=True) in the full-band models, causal_conv.py:74-75,104-105; parameters unchanged).
+        With sequence_model="TCN" the sub-band model is the reference's 8-block TCN of hidden width 512: like the reference, it
+        ignores sb_model_hidden_size and num_layers, and lstm_impl / fast_math have no effect."""
         super().__init__()
         assert sequence_model in ("GRU", "LSTM", "TCN"), f"{self.__class__.__name__} only support GRU, LSTM and TCN."
-        if sequence_model == "TCN":
-            raise NotImplementedError("a TCN sub-band model is not implemented on the CUDA path (LSTM and GRU are)")
         if channel_attention_model not in _lib.ATTENTION:                                       # fullsubnet_plus.py:69-70
             raise NotImplementedError(f"Not implemented channel attention model {channel_attention_model}")
         # fullsubnet_plus.py:47-50.  With subband_num > 1 the reference builds all three attentions for F // subband_num + 1
@@ -360,7 +361,8 @@ class FullSubNet_Plus(_B200Model):
         self.output_size = output_size
         self._setup(num_freqs, look_ahead, sb_num_neighbors, fb_num_neighbors, fb_model_hidden_size, sb_model_hidden_size,
                     num_layers, output_size, fb_output_activate_function, sb_output_activate_function, norm_type, kersize,
-                    lstm_impl, fast_math, channel_attention_model, sequence_model, subband_num if self._subband_runs else 1, causal_tcn)
+                    lstm_impl, fast_math, channel_attention_model, "LSTM" if sequence_model == "TCN" else sequence_model,
+                    subband_num if self._subband_runs else 1, causal_tcn, sb_tcn=sequence_model == "TCN")
         self.causal_tcn = bool(causal_tcn)
         if weight_init:
             self.apply(_reference_weight_init)

@@ -59,6 +59,7 @@ extern "C" {
 #define FSN_LSTM_AUTO 0
 #define FSN_LSTM_MMA 1     /* generic mma.sync kernel (any hidden size / layer count)               */
 #define FSN_LSTM_TCGEN05 2 /* tensor-core path (historical name): layer-wise wgmma kernels, hidden % 64 == 0 and <= 512, input <= 64, output_size 2 */
+#define FSN_LSTM_TCN 3     /* reported by fsn_model_last_lstm_impl only: the sub-band model is the TCN (fsn_config.sb_tcn)   */
 
 typedef struct fsn_config {
     int32_t model_kind;
@@ -83,6 +84,9 @@ typedef struct fsn_config {
     int32_t tcn_causal;       /* 0: TCNBlock(causal=False), what SequenceModel("TCN") builds (sequence_model.py:47-58);
                                  1: TCNBlock(causal=True) in the three full-band models (causal_conv.py:74-75,104-105):
                                  depth-wise taps t-2d, t-d, t instead of t-d, t, t+d.  Additive knob (SURVEY.md 8f rank 2) */
+    int32_t sb_tcn;           /* 0: the sub-band model is the LSTM / GRU of rnn_type; 1: sequence_model = "TCN" of FullSubNet_Plus
+                                 (fullsubnet_plus.py:102-110): 8 non-causal TCNBlock(Isb -> 512 -> Isb) + ReLU + Linear(Isb -> output_size).
+                                 sb_hidden, num_layers, rnn_type, lstm_impl and fast_math do not apply to it */
 } fsn_config;
 
 typedef struct fsn_model fsn_model;
@@ -169,11 +173,12 @@ int fsn_apply_cirm(const float* d_crm, const float* d_noisy, float* d_enh, int32
 /* Test hooks: copy an intermediate of the LAST forward to a device buffer.
  *   "fb_in"  [nbranch, B, F, T+look_ahead]  post-norm (and post-attention) full-band inputs
  *   "fb_out" [nbranch, B, F, T+look_ahead]  full-band model outputs
- *   "sb_mu"  [B]                            utterance mean of the (un-normalised) sub-band input */
+ *   "sb_mu"  [B]                            utterance mean of the (un-normalised) sub-band input
+ *   "sb_in"  [B, F, Isb, T+look_ahead]       normalised sub-band input (sub-band TCN only) */
 int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst, int64_t numel, void* stream);
 /* Kernels launched by the last forward (bench.py reports it as gpu_launches). */
 int64_t fsn_model_last_launch_count(const fsn_model* m);
-/* Device time (ms, CUDA events on the forward's stream) of the sub-band LSTM kernel of the last forward;
+/* Device time (ms, CUDA events on the forward's stream) of the sub-band model (LSTM kernels or the TCN) of the last forward;
  * synchronises on the closing event.  < 0 if no forward has run. */
 float fsn_model_last_lstm_ms(fsn_model* m);
 /* Same for the last n forwards (n <= 32, oldest first); returns how many were written.  Synchronises. */
@@ -182,7 +187,7 @@ int fsn_model_lstm_ms_history(fsn_model* m, float* h_ms, int32_t n);
  * LSTM start, LSTM end in ms relative to the oldest one's front-end start (CUDA events on the streams the phases run on).  With
  * the pipelined entry points the front end of batch i+1 lies inside the LSTM interval of batch i.  Returns the count; synchronises. */
 int fsn_model_timeline(fsn_model* m, float* h_ms4, int32_t n);
-/* Which LSTM implementation the last forward used for the sub-band model (FSN_LSTM_MMA / _TCGEN05). */
+/* Which implementation the last forward used for the sub-band model (FSN_LSTM_MMA / _TCGEN05 / _TCN). */
 int fsn_model_last_lstm_impl(const fsn_model* m);
 
 /* Host-side packers exposed for CPU tests of the kernel layouts (no GPU needed). */

@@ -48,6 +48,32 @@ struct DevBuf {
 
 struct ParamSpec { std::string key; int64_t numel; };
 
+// The packed block weights of one TCN (pack_tcn_blocks): nbr branches (key prefixes pre[b] = "<module>.sequence_model.") of C channels
+// padded to Cp, gLN2 folded into the second 1x1 convolution; NT / ntiles = N tile and N tiles of its Cp-wide GEMMs.
+struct TcnWeights {
+    const char* name = "";                             // in error messages
+    std::vector<std::string> pre;
+    int nbr = 0, C = 0, Cp = 0, NT = 0, ntiles = 0;
+    DevBuf W1, W2, S1, S2b;                            // [8][nbr][512][Cp] tf32, [8][nbr][Cp][512] fp16, [8][nbr][Cp] x2
+    alignas(64) unsigned char mapW1[8][128], mapW2[8][128];
+    void release() { W1.release(); W2.release(); S1.release(); S2b.release(); }
+};
+
+// The scratch of the eight blocks of one TCN over `rows` time-major rows: two fp32 streams [rows, Cp] (ping-pong), the fp16 hidden
+// activations [rows, 512] before and after the depth-wise convolution, and the statistics (tcn_stats_bytes).
+struct TcnScratch {
+    DevBuf xa, xb, y1, y2, stats;
+    long long rows = 0;                                // rows the tensor maps were encoded for (0: none)
+    alignas(64) unsigned char mapXa[128], mapXb[128], mapY2[128];
+    void release() { xa.release(); xb.release(); y1.release(); y2.release(); stats.release(); rows = 0; }
+};
+
+// Statistics of a TCN with Z gLN groups: [8 blocks][gLN1, gLN2][Z][sum, sum of squares] doubles, then [8 blocks][Z] floats, the max |x|
+// per group of the stream entering each block (the fp16 store scale of its hidden activation).
+static size_t tcn_stats_bytes(size_t Z) { return 8 * 2 * Z * 2 * sizeof(double) + 8 * Z * sizeof(float); }
+static double* tcn_gln_sums(void* stats, size_t Z, int blk, int k) { return static_cast<double*>(stats) + (2 * blk + k) * Z * 2; }   // k = 0: gLN1, 1: gLN2
+static float* tcn_amax(void* stats, size_t Z, int blk) { return reinterpret_cast<float*>(static_cast<double*>(stats) + 8 * 2 * Z * 2) + blk * Z; }
+
 struct fsn_model {
     fsn_config cfg;
     std::vector<ParamSpec> specs;
@@ -67,35 +93,35 @@ struct fsn_model {
     // batch i+1 in lane (i+1)&1 on the front stream while the sub-band LSTM of batch i still reads lane i&1 on the LSTM stream.
     struct Lane {
         int wsB = 0, wsT = 0;
-        DevBuf fbin, fbout, xa, xb, y1, y2, stats, mu, ximg, magpad, fbx, hseq;
+        DevBuf fbin, fbout, mu, ximg, magpad, fbx, hseq;
         DevBuf x0, xr;                                 // time-major fb input / relu'd last residual
+        TcnScratch tcn;                                // the full-band TCN's blocks (written on the front stream)
         DevBuf tsse_scale, sb_rowsum;
         DevBuf xn, sigma;                              // pre-normalised inputs / sub-band std for the non-default norm types
         DevBuf sbx;                                    // sub-band TCN: input [B*F*T', 64] fp32 time-major | max |x| per sequence [B*F]
-        alignas(64) unsigned char mapX0[128], mapXa[128], mapXb[128], mapXr[128], mapY2[128], mapSbx[128];
+        alignas(64) unsigned char mapX0[128], mapXr[128], mapSbx[128];
         cudaEvent_t ev_front = nullptr, ev_lstm = nullptr;   // front end written / LSTM finished reading this lane
         bool used = false;                             // ev_lstm has been recorded (a pipelined batch ran / may still run in this lane)
         void release_all() {
-            DevBuf* all[] = {&fbin, &fbout, &xa, &xb, &y1, &y2, &stats, &mu, &ximg, &magpad, &fbx, &hseq, &x0, &xr, &tsse_scale, &sb_rowsum, &xn, &sigma, &sbx};
+            DevBuf* all[] = {&fbin, &fbout, &mu, &ximg, &magpad, &fbx, &hseq, &x0, &xr, &tsse_scale, &sb_rowsum, &xn, &sigma, &sbx};
             for (auto* b : all) b->release();
+            tcn.release();
         }
     } lane[2];
     int last_lane = 0;
     DevBuf cstate, mask_tmp, stage_in[3], stage_out;   // LSTM-side scratch (one LSTM runs at a time), host-entry staging
-    // wgmma TCN (FullSubNet+): folded / padded weights, per-block tensor maps, time-major activations
+    // wgmma TCN (FullSubNet+): the three full-band TCNs (branches of F channels) and their output Linear [3][Cp][Cp] tf32 + bias [3][Cp]
     bool tcn5 = false;
-    int Cp = 0, tcnNT = 0, tcnNtiles = 0, num_sms = 132;
-    DevBuf tW1, tW2, tWfc, tS1, tS2b, tBfc;            // [8][3][512][Cp], [8][3][Cp][512], [3][Cp][Cp], [8][3][Cp] x2, [3][Cp]
+    int num_sms = 132;
+    TcnWeights tcn_fb;
+    DevBuf fb_fc, fb_fc_b;
+    alignas(64) unsigned char map_fb_fc[128];
     DevBuf ws_h, ws_bar;                               // weight-stationary full-band LSTM: h exchange buffer, grid barrier
-    alignas(64) unsigned char mapW1[8][128], mapW2[8][128], mapWfc[128];
-    // sub-band TCN (cfg.sb_tcn): the same block weights for one branch of Isb channels (Cp = 64, one 64-column N tile), the Linear
-    // head [O][64], and the scratch of the eight blocks -- shared by both lanes and ordered on the sub-band stream (like r_gin): two fp32
-    // streams, two fp16 hidden buffers, gLN sums and the stream maxima of blocks 1..7 (block 0's are written with the lane's input)
-    DevBuf sW1, sW2, sS1, sS2b, sFc;
-    alignas(64) unsigned char smapW1[8][128], smapW2[8][128];
-    DevBuf sb_xa, sb_xb, sb_y1, sb_y2, sb_stats;
-    long long sb_rows = 0;                             // rows of the tensor maps below
-    alignas(64) unsigned char mapSbXa[128], mapSbXb[128], mapSbY2[128];
+    // sub-band TCN (cfg.sb_tcn): one branch of Isb channels, the Linear head [O][64], and the scratch of the eight blocks -- shared by
+    // both lanes and ordered on the sub-band stream (like r_gin); block 0's stream maxima are written with the lane's input (sbx)
+    TcnWeights tcn_sb;
+    DevBuf sb_fc;
+    TcnScratch sb_scratch;
     int64_t launches = 0;
     int last_impl = 0;
     // tuning knobs, read ONCE at fsn_model_create (never on the forward path): FSN_LSTM_IMPL overrides cfg.lstm_impl,
@@ -292,9 +318,12 @@ static float to_tf32(float x) {
 //   conv(W2, gLN(y)) = rstd * (W2 diag(gamma2)) y - mean * rstd * s1 + s2,  s1[n] = sum_c W2'[n,c],  s2[n] = sum_c W2[n,c] beta2[c]
 // W1 [8][nbr][512][Cp] tf32, W2' [8][nbr][Cp][512] fp16, s1 / s2 + conv bias [8][nbr][Cp]; tensor maps per block: W1 in 128-row
 // boxes, W2' in NT-row boxes.
-static int pack_tcn_blocks(fsn_model* m, const std::vector<std::string>& pre, int C, int Cp, int NT, DevBuf& dW1, DevBuf& dW2, DevBuf& dS1,
-                           DevBuf& dS2b, unsigned char (*mapW1)[128], unsigned char (*mapW2)[128]) {
+static int pack_tcn_blocks(fsn_model* m, TcnWeights& w, const char* name, const std::vector<std::string>& pre, int C, int Cp) {
     const int nbr = (int)pre.size(), Hd = 512;
+    w.name = name; w.pre = pre; w.nbr = nbr; w.C = C; w.Cp = Cp;
+    // N tile of the Cp-wide GEMMs: 64 or 128 columns (the last tile of a branch may overhang; those columns are not stored)
+    w.NT = Cp <= 64 ? 64 : 128;
+    w.ntiles = (Cp + w.NT - 1) / w.NT;
     std::vector<float> W1((size_t)8 * nbr * Hd * Cp, 0.f);
     std::vector<__half> W2((size_t)8 * nbr * Cp * Hd, __float2half_rn(0.f));     // second 1x1 conv: fp16 operands (hidden activations are fp16)
     std::vector<float> S1((size_t)8 * nbr * Cp, 0.f), S2b((size_t)8 * nbr * Cp, 0.f);
@@ -323,13 +352,13 @@ static int pack_tcn_blocks(fsn_model* m, const std::vector<std::string>& pre, in
                 S2b[((size_t)blk * nbr + b) * Cp + n] = (float)(s2 + (double)b2[n]);
             }
         }
-    if (upload(dW1, W1.data(), W1.size() * 4) || upload(dW2, W2.data(), W2.size() * sizeof(__half)) ||
-        upload(dS1, S1.data(), S1.size() * 4) || upload(dS2b, S2b.data(), S2b.size() * 4))
-        return fail(FSN_ECUDA, "upload of the TCN weights failed");
+    if (upload(w.W1, W1.data(), W1.size() * 4) || upload(w.W2, W2.data(), W2.size() * sizeof(__half)) ||
+        upload(w.S1, S1.data(), S1.size() * 4) || upload(w.S2b, S2b.data(), S2b.size() * 4))
+        return fail(FSN_ECUDA, "upload of the %s weights failed", name);
     for (int blk = 0; blk < 8; ++blk) {
-        if (make_tmap_f32_2d(mapW1[blk], static_cast<float*>(dW1.p) + (size_t)blk * nbr * Hd * Cp, nbr * Hd, Cp, 128) ||
-            make_tmap_f16_2d(mapW2[blk], static_cast<__half*>(dW2.p) + (size_t)blk * nbr * Cp * Hd, nbr * Cp, Hd, NT))
-            return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the TCN weights");
+        if (make_tmap_f32_2d(w.mapW1[blk], static_cast<float*>(w.W1.p) + (size_t)blk * nbr * Hd * Cp, nbr * Hd, Cp, 128) ||
+            make_tmap_f16_2d(w.mapW2[blk], static_cast<__half*>(w.W2.p) + (size_t)blk * nbr * Cp * Hd, nbr * Cp, Hd, w.NT))
+            return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the %s weights", name);
     }
     return FSN_OK;
 }
@@ -338,18 +367,10 @@ static int pack_tcn_blocks(fsn_model* m, const std::vector<std::string>& pre, in
 static int pack_tcn5(fsn_model* m) {
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs, Cp = (F + 31) / 32 * 32;
-    m->Cp = Cp;
-    // N tile of the Cp-wide GEMMs: 64 or 128 columns (the last tile of a branch may overhang; those columns are not stored)
-    m->tcnNT = Cp <= 64 ? 64 : 128;
-    m->tcnNtiles = (Cp + m->tcnNT - 1) / m->tcnNT;
-    cudaDeviceProp prop;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (cudaGetDeviceProperties(&prop, dev) == cudaSuccess) m->num_sms = prop.multiProcessorCount;
     const char* sfx[3] = {"", "_real", "_imag"};
     std::vector<std::string> pre;
     for (int b = 0; b < 3; ++b) pre.push_back(std::string("fb_model") + sfx[b] + ".sequence_model.");
-    int rc = pack_tcn_blocks(m, pre, F, Cp, m->tcnNT, m->tW1, m->tW2, m->tS1, m->tS2b, m->mapW1, m->mapW2);
+    int rc = pack_tcn_blocks(m, m->tcn_fb, "full-band TCN", pre, F, Cp);
     if (rc) return rc;
     std::vector<float> Wfc((size_t)3 * Cp * Cp, 0.f), Bfc((size_t)3 * Cp, 0.f);
     for (int b = 0; b < 3; ++b) {
@@ -360,24 +381,24 @@ static int pack_tcn5(fsn_model* m) {
             Bfc[(size_t)b * Cp + n] = bb[n];
         }
     }
-    if (upload(m->tWfc, Wfc.data(), Wfc.size() * 4) || upload(m->tBfc, Bfc.data(), Bfc.size() * 4))
+    if (upload(m->fb_fc, Wfc.data(), Wfc.size() * 4) || upload(m->fb_fc_b, Bfc.data(), Bfc.size() * 4))
         return fail(FSN_ECUDA, "upload of the TCN weights failed");
-    if (make_tmap_f32_2d(m->mapWfc, m->tWfc.p, 3 * Cp, Cp, m->tcnNT)) return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed (fc)");
+    if (make_tmap_f32_2d(m->map_fb_fc, m->fb_fc.p, 3 * Cp, Cp, m->tcn_fb.NT)) return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed (fc)");
     m->tcn5 = true;
     return FSN_OK;
 }
 
-// the sub-band TCN (sequence_model = "TCN"): one branch of Isb <= 64 channels padded to 64, and its Linear(Isb -> O) as [O][64] fp32
-// (read by the GLN_HEAD epilogue)
+// the sub-band TCN (sequence_model = "TCN"): one branch of Isb <= 64 channels padded to 64 -- the GLN_HEAD epilogue needs a row's
+// channels in one 64-column N tile -- and its Linear(Isb -> O) as [O][64] fp32 (read by that epilogue)
 static int pack_sb_tcn(fsn_model* m) {
     const int I = m->Isb, O = m->cfg.output_size;
-    int rc = pack_tcn_blocks(m, {"sb_model.sequence_model."}, I, 64, 64, m->sW1, m->sW2, m->sS1, m->sS2b, m->smapW1, m->smapW2);
+    int rc = pack_tcn_blocks(m, m->tcn_sb, "sub-band TCN", {"sb_model.sequence_model."}, I, 64);
     if (rc) return rc;
     std::vector<float> fc((size_t)O * 64, 0.f);
     const auto& w = m->host["sb_model.fc_output_layer.weight"];
     for (int o = 0; o < O; ++o)
         for (int k = 0; k < I; ++k) fc[(size_t)o * 64 + k] = w[(size_t)o * I + k];
-    if (upload(m->sFc, fc.data(), fc.size() * 4)) return fail(FSN_ECUDA, "upload of the sub-band TCN head failed");
+    if (upload(m->sb_fc, fc.data(), fc.size() * 4)) return fail(FSN_ECUDA, "upload of the sub-band TCN head failed");
     return FSN_OK;
 }
 
@@ -435,9 +456,9 @@ extern "C" void fsn_model_destroy(fsn_model* m) {
     if (!m) return;
     cudaDeviceSynchronize();
     DevBuf* all[] = {&m->arena, &m->cstate, &m->mask_tmp, &m->stage_in[0], &m->stage_in[1], &m->stage_in[2],
-                     &m->stage_out, &m->tW1, &m->tW2, &m->tWfc, &m->tS1, &m->tS2b, &m->tBfc, &m->ws_h, &m->ws_bar,
-                     &m->sW1, &m->sW2, &m->sS1, &m->sS2b, &m->sFc, &m->sb_xa, &m->sb_xb, &m->sb_y1, &m->sb_y2, &m->sb_stats};
+                     &m->stage_out, &m->fb_fc, &m->fb_fc_b, &m->ws_h, &m->ws_bar, &m->sb_fc};
     for (auto* b : all) b->release();
+    m->tcn_fb.release(); m->tcn_sb.release(); m->sb_scratch.release();
     for (auto& ln : m->lane) {
         ln.release_all();
         if (ln.ev_front) cudaEventDestroy(ln.ev_front);
@@ -561,6 +582,29 @@ static int pick_impl(const fsn_model* m) {
 static bool use_layerwise(const fsn_model* m) { return pick_impl(m) == FSN_LSTM_TCGEN05 && m->tc5r_ok; }
 
 
+// Grow the scratch of TCN w to `rows` rows and Z gLN groups (grow-only; zero: a new allocation is zero-filled on stream s) and encode its
+// tensor maps when the rows change.  The mapped buffers' sizes depend on the rows alone, so they are only reallocated with new rows, after
+// a release or after a failed allocation (rows = 0 in the last two cases).
+static int grow_tcn_scratch(TcnScratch& sc, const TcnWeights& w, long long rows, size_t Z, bool zero, cudaStream_t s) {
+    int e = 0;
+    e |= sc.xa.ensure((size_t)rows * w.Cp * 4, zero, s);
+    e |= sc.xb.ensure((size_t)rows * w.Cp * 4, zero, s);
+    e |= sc.y1.ensure((size_t)rows * 512 * sizeof(__half), zero, s);
+    e |= sc.y2.ensure((size_t)rows * 512 * sizeof(__half), zero, s);
+    e |= sc.stats.ensure(tcn_stats_bytes(Z), zero, s);
+    if (e) {
+        sc.rows = 0;
+        return fail(FSN_ECUDA, "workspace allocation failed for the %s (%lld rows)", w.name, rows);
+    }
+    if (sc.rows != rows) {
+        if (make_tmap_f32_2d(sc.mapXa, sc.xa.p, rows, w.Cp, 128) || make_tmap_f32_2d(sc.mapXb, sc.xb.p, rows, w.Cp, 128) ||
+            make_tmap_f16_2d(sc.mapY2, sc.y2.p, rows, 512, 128))
+            return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the %s", w.name);
+        sc.rows = rows;
+    }
+    return FSN_OK;
+}
+
 static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, cudaStream_t s, cudaStream_t sl) {
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs, Tp = T + c.look_ahead, Pp = (Tp + 3) & ~3;
@@ -583,19 +627,10 @@ static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, cudaStream
         if (srows + 128 > 0x7fffffffLL) return fail(FSN_EINVAL, "B * num_freqs * (T + look_ahead) = %lld rows exceeds the sub-band TCN's 2^31 limit", srows);
         if (regeo) ln.sbx.release();
         e |= ln.sbx.ensure((size_t)srows * 64 * 4 + (size_t)B * F * 4, false, s);
-        e |= m->sb_xa.ensure((size_t)srows * 64 * 4, false, sl);
-        e |= m->sb_xb.ensure((size_t)srows * 64 * 4, false, sl);
-        e |= m->sb_y1.ensure((size_t)srows * 512 * sizeof(__half), false, sl);
-        e |= m->sb_y2.ensure((size_t)srows * 512 * sizeof(__half), false, sl);
-        e |= m->sb_stats.ensure((size_t)8 * 2 * B * F * 2 * sizeof(double) + (size_t)8 * B * F * sizeof(float), false, sl);
         if (e) return fail(FSN_ECUDA, "workspace allocation failed for B=%d T=%d", B, T);
         if (regeo && make_tmap_f32_2d(ln.mapSbx, ln.sbx.p, srows, 64, 128)) return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the sub-band input");
-        if (m->sb_rows != srows) {
-            if (make_tmap_f32_2d(m->mapSbXa, m->sb_xa.p, srows, 64, 128) || make_tmap_f32_2d(m->mapSbXb, m->sb_xb.p, srows, 64, 128) ||
-                make_tmap_f16_2d(m->mapSbY2, m->sb_y2.p, srows, 512, 128))
-                return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the sub-band TCN");
-            m->sb_rows = srows;
-        }
+        int rc = grow_tcn_scratch(m->sb_scratch, m->tcn_sb, srows, (size_t)B * F, false, sl);
+        if (rc) return rc;
     } else {
         // images are re-zeroed whenever the geometry changes (rows beyond B*F and k >= I must stay zero)
         const size_t img_bytes = (size_t)ntiles * Tp * 16384;
@@ -622,21 +657,16 @@ static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, cudaStream
     if (cs || cs5) e |= m->cstate.ensure(cs > cs5 ? cs : cs5, true, sl);
     if (c.model_kind == FSN_KIND_PLUS) {
         if (!m->tcn5) return fail(FSN_ESTATE, "the TCN weights were not packed");
-        const size_t trows = (size_t)3 * B * Tp;
-        if (regeo) { ln.x0.release(); ln.xa.release(); ln.xb.release(); ln.xr.release(); ln.y1.release(); ln.y2.release(); }
-        e |= ln.x0.ensure(trows * m->Cp * 4, true, s);
-        e |= ln.xa.ensure(trows * m->Cp * 4, true, s);
-        e |= ln.xb.ensure(trows * m->Cp * 4, true, s);
-        e |= ln.xr.ensure(trows * m->Cp * 4, true, s);
-        e |= ln.y1.ensure(trows * 512 * sizeof(__half), true, s);
-        e |= ln.y2.ensure(trows * 512 * sizeof(__half), true, s);
-        e |= ln.stats.ensure((size_t)8 * 2 * 3 * B * 2 * sizeof(double) + (size_t)8 * 3 * B * sizeof(float), true, s);   // gLN sums | per-block stream maxima
-        if (!e && regeo) {
-            if (make_tmap_f32_2d(ln.mapX0, ln.x0.p, trows, m->Cp, 128) || make_tmap_f32_2d(ln.mapXa, ln.xa.p, trows, m->Cp, 128) ||
-                make_tmap_f32_2d(ln.mapXb, ln.xb.p, trows, m->Cp, 128) || make_tmap_f32_2d(ln.mapXr, ln.xr.p, trows, m->Cp, 128) ||
-                make_tmap_f16_2d(ln.mapY2, ln.y2.p, trows, 512, 128))
-                return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the activations");
-        }
+        // a new geometry gets fresh zero-filled buffers: the pad columns of x0 (and so of every stream) must be zero
+        const size_t trows = (size_t)3 * B * Tp, Cp = m->tcn_fb.Cp;
+        if (regeo) { ln.x0.release(); ln.xr.release(); ln.tcn.release(); }
+        e |= ln.x0.ensure(trows * Cp * 4, true, s);
+        e |= ln.xr.ensure(trows * Cp * 4, true, s);
+        if (e) return fail(FSN_ECUDA, "workspace allocation failed for B=%d T=%d", B, T);
+        if (regeo && (make_tmap_f32_2d(ln.mapX0, ln.x0.p, trows, Cp, 128) || make_tmap_f32_2d(ln.mapXr, ln.xr.p, trows, Cp, 128)))
+            return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the activations");
+        int rc = grow_tcn_scratch(ln.tcn, m->tcn_fb, (long long)trows, (size_t)3 * B, true, s);
+        if (rc) return rc;
     } else {
         const int Ipad = (F + 15) / 16 * 16, rows_pad = (B + 63) / 64 * 64;
         e |= ln.magpad.ensure((size_t)B * F * Pp * 4, true, s);
@@ -715,67 +745,85 @@ static int run_sb_lstm(fsn_model* m, fsn_model::Lane& ln, int B, int T, float* d
     return FSN_OK;
 }
 
-// The sub-band TCN (sequence_model = "TCN", fullsubnet_plus.py:102-110): the eight TCN blocks of the full band with one branch, the
-// B*F sequences of the sub-band input as the gLN groups and Isb (<= 64) channels in one 64-column N tile; the last block's second 1x1
-// convolution ends in ReLU + Linear + activation (EPI5_GLN_HEAD) and writes the mask -- or, with d_enh, the enhanced spectrum.
+// the M side of a GEMM over the time-major rows (branch, group, frame) of TCN w: G gLN groups per branch of Tp frames each
+static void set_tcn_rows(GemmTc5Launch& g, const TcnWeights& w, int G, int Tp) {
+    g.rows_per_branch = G * Tp; g.tiles_m = (G * Tp + 127) / 128; g.nbranch = w.nbr; g.Tp = Tp; g.B = G;
+}
+
+// The eight blocks of TCN w (SequenceModel TCN branch, sequence_model.py:47-58; TCNBlock, causal_conv.py:96-108) on stream s: per block
+// GEMM1 (1x1 conv + PReLU + gLN1 statistics), the depth-wise convolution, GEMM2 (folded gLN2 + residual), the stream ping-ponging between
+// sc.xa and sc.xb from the input x (tensor map xmap).  amax0: block 0's stream maxima [nbr * G], written with the input.  The last
+// GEMM2 ends as `last` says: its epilogue (EPI5_GLN_RES or EPI5_GLN_HEAD) and that epilogue's own outputs (Xrelu, or the head fields).
+static int run_tcn_blocks(fsn_model* m, const TcnWeights& w, TcnScratch& sc, const float* x, const unsigned char* xmap, const float* amax0,
+                          int G, int Tp, bool causal, const GemmTc5Launch& last, cudaStream_t s) {
+    static const int dil[8] = {1, 2, 5, 9, 1, 2, 5, 9};
+    const size_t Z = (size_t)w.nbr * G;
+    const float* curp = x;
+    const unsigned char* curmap = xmap;
+    for (int blk = 0; blk < 8; ++blk) {
+        double* st1 = tcn_gln_sums(sc.stats.p, Z, blk, 0);
+        double* st2 = tcn_gln_sums(sc.stats.p, Z, blk, 1);
+        const float* amax_in = blk ? tcn_amax(sc.stats.p, Z, blk) : amax0;
+        auto key = [&](int b, const char* leaf) { return w.pre[b] + std::to_string(blk) + "." + leaf; };
+        GemmTc5Launch g1{};
+        set_tcn_rows(g1, w, G, Tp);
+        g1.epi = EPI5_PRELU_STATS; g1.Kp = w.Cp; g1.NT = 128; g1.ntiles_n = 4; g1.Npad = 512;
+        for (int b = 0; b < w.nbr; ++b) { g1.bias[b] = P(m, key(b, "conv1x1.bias")); g1.prelu[b] = P(m, key(b, "prelu1.weight")); }
+        g1.stats_out = st1; g1.Y16 = static_cast<__half*>(sc.y1.p); g1.ldY = 512; g1.amax_in = amax_in;
+        int e = launch_gemm_tc5(curmap, w.mapW1[blk], g1, m->num_sms, s);
+        if (e) return fail(FSN_ECUDA, "%s GEMM1 launch failed: %s", w.name, cudaGetErrorString((cudaError_t)e));
+        m->launches++;
+
+        DwTmLaunch dw{};
+        dw.X = static_cast<const __half*>(sc.y1.p); dw.Y = static_cast<__half*>(sc.y2.p);
+        dw.Z = (int)Z; dw.B = G; dw.C = 512; dw.Tp = Tp; dw.dilation = dil[blk]; dw.causal = causal ? 1 : 0;
+        dw.stats_in = st1; dw.stats_out = st2; dw.amax = amax_in;
+        for (int b = 0; b < w.nbr; ++b) {
+            dw.gamma[b] = P(m, key(b, "norm1.weight")); dw.beta[b] = P(m, key(b, "norm1.bias"));
+            dw.w[b] = P(m, key(b, "depthwise_conv.weight")); dw.b[b] = P(m, key(b, "depthwise_conv.bias"));
+            dw.prelu[b] = P(m, key(b, "prelu2.weight"));
+        }
+        e = launch_dwconv_tm(dw, s);
+        if (e) return fail(FSN_ECUDA, "%s depth-wise conv launch failed: %s", w.name, cudaGetErrorString((cudaError_t)e));
+        m->launches++;
+
+        float* nxtp = static_cast<float*>((blk & 1) ? sc.xb.p : sc.xa.p);
+        GemmTc5Launch g2 = blk < 7 ? GemmTc5Launch{} : last;
+        if (blk < 7) { g2.epi = EPI5_GLN_RES; g2.amax_out = tcn_amax(sc.stats.p, Z, blk + 1); }
+        set_tcn_rows(g2, w, G, Tp);
+        g2.Kp = 512; g2.NT = w.NT; g2.ntiles_n = w.ntiles; g2.Npad = w.Cp;
+        for (int b = 0; b < w.nbr; ++b) {
+            g2.bias[b] = static_cast<const float*>(w.S2b.p) + ((size_t)blk * w.nbr + b) * w.Cp;
+            g2.s1[b] = static_cast<const float*>(w.S1.p) + ((size_t)blk * w.nbr + b) * w.Cp;
+        }
+        g2.stats_in = st2; g2.count_in = (double)512 * Tp;
+        g2.Xold = curp; g2.ldY = w.Cp;
+        if (g2.epi == EPI5_GLN_RES) g2.Y = nxtp;
+        e = launch_gemm_tc5(sc.mapY2, w.mapW2[blk], g2, m->num_sms, s);
+        if (e) return fail(FSN_ECUDA, "%s GEMM2 launch failed: %s", w.name, cudaGetErrorString((cudaError_t)e));
+        m->launches++;
+        curp = nxtp;
+        curmap = (blk & 1) ? sc.mapXb : sc.mapXa;
+    }
+    return FSN_OK;
+}
+
+// The sub-band TCN (sequence_model = "TCN", fullsubnet_plus.py:102-110): the TCN blocks with one branch, the B*F sequences of the sub-band
+// input as the gLN groups and Isb (<= 64) channels in one 64-column N tile; the last block's second 1x1 convolution ends in ReLU + Linear +
+// activation (EPI5_GLN_HEAD) and writes the mask -- or, with d_enh, the enhanced spectrum.
 static int run_sb_tcn(fsn_model* m, fsn_model::Lane& ln, int B, int T, float* d_out, const float* d_real, const float* d_imag, float* d_enh,
                       cudaStream_t s) {
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs, Tp = T + c.look_ahead, Z = B * F;
     m->last_impl = FSN_LSTM_TCN;
-    double* stats = static_cast<double*>(m->sb_stats.p);
-    float* amax = reinterpret_cast<float*>(stats + (size_t)8 * 2 * Z * 2);              // [8][Z]: max |x| of the stream entering block k (k >= 1)
-    const float* amax0 = reinterpret_cast<const float*>(static_cast<float*>(ln.sbx.p) + (size_t)Z * Tp * 64);
-    CK(cudaMemsetAsync(stats, 0, (size_t)8 * 2 * Z * 2 * sizeof(double) + (size_t)8 * Z * sizeof(float), s));
-    static const int dil[8] = {1, 2, 5, 9, 1, 2, 5, 9};             // sequence_model.py:47-58
-    GemmTc5Launch g{};
-    g.rows_per_branch = Z * Tp; g.tiles_m = (Z * Tp + 127) / 128; g.nbranch = 1; g.Tp = Tp; g.B = Z;
-    const float* curp = static_cast<const float*>(ln.sbx.p);
-    const unsigned char* curmap = ln.mapSbx;
-    for (int blk = 0; blk < 8; ++blk) {
-        double* st1 = stats + (size_t)(2 * blk) * Z * 2;
-        double* st2 = stats + (size_t)(2 * blk + 1) * Z * 2;
-        const float* amax_in = blk ? amax + (size_t)blk * Z : amax0;
-        auto key = [&](const char* leaf) { return std::string("sb_model.sequence_model.") + std::to_string(blk) + "." + leaf; };
-        GemmTc5Launch g1 = g;
-        g1.epi = EPI5_PRELU_STATS; g1.Kp = 64; g1.NT = 128; g1.ntiles_n = 4; g1.Npad = 512;
-        g1.bias[0] = P(m, key("conv1x1.bias")); g1.prelu[0] = P(m, key("prelu1.weight"));
-        g1.stats_out = st1; g1.Y16 = static_cast<__half*>(m->sb_y1.p); g1.ldY = 512; g1.amax_in = amax_in;
-        int e = launch_gemm_tc5(curmap, m->smapW1[blk], g1, m->num_sms, s);
-        if (e) return fail(FSN_ECUDA, "sub-band TCN GEMM1 launch failed: %s", cudaGetErrorString((cudaError_t)e));
-        m->launches++;
-
-        DwTmLaunch dw{};
-        dw.X = static_cast<const __half*>(m->sb_y1.p); dw.Y = static_cast<__half*>(m->sb_y2.p);
-        dw.Z = Z; dw.B = Z; dw.C = 512; dw.Tp = Tp; dw.dilation = dil[blk]; dw.causal = 0;
-        dw.stats_in = st1; dw.stats_out = st2; dw.amax = amax_in;
-        dw.gamma[0] = P(m, key("norm1.weight")); dw.beta[0] = P(m, key("norm1.bias"));
-        dw.w[0] = P(m, key("depthwise_conv.weight")); dw.b[0] = P(m, key("depthwise_conv.bias")); dw.prelu[0] = P(m, key("prelu2.weight"));
-        e = launch_dwconv_tm(dw, s);
-        if (e) return fail(FSN_ECUDA, "sub-band TCN depth-wise conv launch failed: %s", cudaGetErrorString((cudaError_t)e));
-        m->launches++;
-
-        float* nxtp = (blk & 1) ? static_cast<float*>(m->sb_xb.p) : static_cast<float*>(m->sb_xa.p);
-        GemmTc5Launch g2 = g;
-        g2.epi = blk < 7 ? EPI5_GLN_RES : EPI5_GLN_HEAD; g2.Kp = 512; g2.NT = 64; g2.ntiles_n = 1; g2.Npad = 64;
-        g2.bias[0] = static_cast<const float*>(m->sS2b.p) + (size_t)blk * 64;
-        g2.s1[0] = static_cast<const float*>(m->sS1.p) + (size_t)blk * 64;
-        g2.stats_in = st2; g2.count_in = (double)512 * Tp;
-        g2.Xold = curp; g2.ldY = 64;
-        if (blk < 7) {
-            g2.Y = nxtp; g2.amax_out = amax + (size_t)(blk + 1) * Z;
-        } else {
-            g2.fc_w = static_cast<const float*>(m->sFc.p); g2.fc_b = P(m, "sb_model.fc_output_layer.bias");
-            g2.O = c.output_size; g2.la = c.look_ahead; g2.F = F; g2.act = c.sb_act;
-            g2.out = d_out; g2.nreal = d_real; g2.nimag = d_imag; g2.enh = reinterpret_cast<float2*>(d_enh);
-        }
-        e = launch_gemm_tc5(m->mapSbY2, m->smapW2[blk], g2, m->num_sms, s);
-        if (e) return fail(FSN_ECUDA, "sub-band TCN GEMM2 launch failed: %s", cudaGetErrorString((cudaError_t)e));
-        m->launches++;
-        curp = nxtp;
-        curmap = (blk & 1) ? m->mapSbXb : m->mapSbXa;
-    }
-    return FSN_OK;
+    CK(cudaMemsetAsync(m->sb_scratch.stats.p, 0, tcn_stats_bytes(Z), s));
+    GemmTc5Launch head{};
+    head.epi = EPI5_GLN_HEAD;
+    head.fc_w = static_cast<const float*>(m->sb_fc.p); head.fc_b = P(m, "sb_model.fc_output_layer.bias");
+    head.O = c.output_size; head.la = c.look_ahead; head.F = F; head.act = c.sb_act;
+    head.out = d_out; head.nreal = d_real; head.nimag = d_imag; head.enh = reinterpret_cast<float2*>(d_enh);
+    const float* x = static_cast<const float*>(ln.sbx.p);
+    return run_tcn_blocks(m, m->tcn_sb, m->sb_scratch, x, ln.mapSbx, x + (size_t)Z * Tp * 64, Z, Tp, false, head, s);
 }
 
 // The whole forward.  Front end (norm, attention, full-band model, sub-band statistics + packing) on stream `s` into lane `ln`;
@@ -836,7 +884,7 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
         ta.out = static_cast<float*>(ln.fbin.p);
         ta.scale = static_cast<float*>(ln.tsse_scale.p);
         ta.rows = ta.scale + (size_t)ta.nbranch * B * F;
-        ta.out_tm = static_cast<float*>(ln.x0.p); ta.Cp = m->Cp;
+        ta.out_tm = static_cast<float*>(ln.x0.p); ta.Cp = m->tcn_fb.Cp;
         if (c.norm_type != FSN_NORM_OFFLINE_LAPLACE) {
             NormLaunch na{};
             na.x[0] = d_mag; na.x[1] = d_real; na.x[2] = d_imag; na.y = static_cast<float*>(ln.xn.p);
@@ -845,68 +893,23 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
             for (int b = 0; b < 3; ++b) ta.x[b] = static_cast<const float*>(ln.xn.p) + (size_t)b * B * F * Tp;
             ta.T = Tp; ta.prenorm = 1;                                  // padded frames are part of the normalised signal
         }
-        const int Z = 3 * B;
-        double* stats = static_cast<double*>(ln.stats.p);
-        float* amax = reinterpret_cast<float*>(stats + (size_t)8 * 2 * Z * 2);            // [8][Z]: max |x| of the stream entering block k, per sample
-        CK(cudaMemsetAsync(stats, 0, (size_t)8 * 2 * Z * 2 * sizeof(double) + (size_t)8 * Z * sizeof(float), s));
-        ta.amax = amax;                                                                    // block 0: written by the gate kernel
+        const TcnWeights& w = m->tcn_fb;
+        CK(cudaMemsetAsync(ln.tcn.stats.p, 0, tcn_stats_bytes(3 * B), s));
+        ta.amax = tcn_amax(ln.tcn.stats.p, 3 * B, 0);                  // block 0: written by the gate kernel
         launch_tsse_norm(ta, s); m->launches += 3;
 
-        static const int dil[8] = {1, 2, 5, 9, 1, 2, 5, 9};     // sequence_model.py:47-58
-        {
-            const int Cp = m->Cp;
-            GemmTc5Launch g{};
-            g.rows_per_branch = B * Tp; g.tiles_m = (B * Tp + 127) / 128; g.nbranch = 3; g.Tp = Tp; g.B = B;
-            const float* curp = static_cast<const float*>(ln.x0.p);
-            const unsigned char* curmap = ln.mapX0;
-            for (int blk = 0; blk < 8; ++blk) {
-                double* st1 = stats + (size_t)(2 * blk) * Z * 2;
-                double* st2 = stats + (size_t)(2 * blk + 1) * Z * 2;
-                auto key = [&](int b, const char* leaf) { return std::string("fb_model") + sfx[b] + ".sequence_model." + std::to_string(blk) + "." + leaf; };
-                GemmTc5Launch g1 = g;
-                g1.epi = EPI5_PRELU_STATS; g1.Kp = Cp; g1.NT = 128; g1.ntiles_n = 4; g1.Npad = 512;
-                for (int b = 0; b < 3; ++b) { g1.bias[b] = P(m, key(b, "conv1x1.bias")); g1.prelu[b] = P(m, key(b, "prelu1.weight")); }
-                g1.stats_out = st1; g1.Y16 = static_cast<__half*>(ln.y1.p); g1.ldY = 512; g1.amax_in = amax + (size_t)blk * Z;
-                int e = launch_gemm_tc5(curmap, m->mapW1[blk], g1, m->num_sms, s);
-                if (e) return fail(FSN_ECUDA, "TCN GEMM1 launch failed: %s", cudaGetErrorString((cudaError_t)e));
-                m->launches++;
-
-                DwTmLaunch dw{};
-                dw.X = static_cast<const __half*>(ln.y1.p); dw.Y = static_cast<__half*>(ln.y2.p);
-                dw.Z = Z; dw.B = B; dw.C = 512; dw.Tp = Tp; dw.dilation = dil[blk]; dw.causal = c.tcn_causal ? 1 : 0;
-                dw.stats_in = st1; dw.stats_out = st2; dw.amax = amax + (size_t)blk * Z;
-                for (int b = 0; b < 3; ++b) {
-                    dw.gamma[b] = P(m, key(b, "norm1.weight")); dw.beta[b] = P(m, key(b, "norm1.bias"));
-                    dw.w[b] = P(m, key(b, "depthwise_conv.weight")); dw.b[b] = P(m, key(b, "depthwise_conv.bias"));
-                    dw.prelu[b] = P(m, key(b, "prelu2.weight"));
-                }
-                e = launch_dwconv_tm(dw, s);
-                if (e) return fail(FSN_ECUDA, "TCN depth-wise conv launch failed: %s", cudaGetErrorString((cudaError_t)e));
-                m->launches++;
-
-                float* nxtp = (blk & 1) ? static_cast<float*>(ln.xb.p) : static_cast<float*>(ln.xa.p);
-                GemmTc5Launch g2 = g;
-                g2.epi = EPI5_GLN_RES; g2.Kp = 512; g2.NT = m->tcnNT; g2.ntiles_n = m->tcnNtiles; g2.Npad = Cp;
-                for (int b = 0; b < 3; ++b) {
-                    g2.bias[b] = static_cast<const float*>(m->tS2b.p) + ((size_t)blk * 3 + b) * Cp;
-                    g2.s1[b] = static_cast<const float*>(m->tS1.p) + ((size_t)blk * 3 + b) * Cp;
-                }
-                g2.stats_in = st2; g2.count_in = (double)512 * Tp;
-                g2.Xold = curp; g2.Y = nxtp; g2.ldY = Cp; g2.amax_out = (blk < 7) ? amax + (size_t)(blk + 1) * Z : nullptr; g2.Xrelu = (blk == 7) ? static_cast<float*>(ln.xr.p) : nullptr;
-                e = launch_gemm_tc5(ln.mapY2, m->mapW2[blk], g2, m->num_sms, s);
-                if (e) return fail(FSN_ECUDA, "TCN GEMM2 launch failed: %s", cudaGetErrorString((cudaError_t)e));
-                m->launches++;
-                curp = nxtp;
-                curmap = (blk & 1) ? ln.mapXb : ln.mapXa;
-            }
-            GemmTc5Launch g3 = g;
-            g3.epi = EPI5_OUT; g3.Kp = Cp; g3.NT = m->tcnNT; g3.ntiles_n = m->tcnNtiles; g3.Npad = Cp;
-            for (int b = 0; b < 3; ++b) g3.bias[b] = static_cast<const float*>(m->tBfc.p) + (size_t)b * Cp;
-            g3.out = static_cast<float*>(ln.fbout.p); g3.F = F; g3.P = Pp; g3.act = c.fb_act;
-            int e = launch_gemm_tc5(ln.mapXr, m->mapWfc, g3, m->num_sms, s);
-            if (e) return fail(FSN_ECUDA, "TCN output GEMM launch failed: %s", cudaGetErrorString((cudaError_t)e));
-            m->launches++;
-        }
+        GemmTc5Launch last{};                                           // the last block also writes relu(x) for the output Linear
+        last.epi = EPI5_GLN_RES; last.Xrelu = static_cast<float*>(ln.xr.p);
+        rc = run_tcn_blocks(m, w, ln.tcn, static_cast<const float*>(ln.x0.p), ln.mapX0, ta.amax, B, Tp, c.tcn_causal, last, s);
+        if (rc) return rc;
+        GemmTc5Launch g3{};
+        set_tcn_rows(g3, w, B, Tp);
+        g3.epi = EPI5_OUT; g3.Kp = w.Cp; g3.NT = w.NT; g3.ntiles_n = w.ntiles; g3.Npad = w.Cp;
+        for (int b = 0; b < 3; ++b) g3.bias[b] = static_cast<const float*>(m->fb_fc_b.p) + (size_t)b * w.Cp;
+        g3.out = static_cast<float*>(ln.fbout.p); g3.F = F; g3.P = Pp; g3.act = c.fb_act;
+        int e = launch_gemm_tc5(ln.mapXr, m->map_fb_fc, g3, m->num_sms, s);
+        if (e) return fail(FSN_ECUDA, "TCN output GEMM launch failed: %s", cudaGetErrorString((cudaError_t)e));
+        m->launches++;
 
         sp.win = static_cast<const float*>(ln.fbin.p); sp.Pw = Pp;      // post-attention mag branch (fullsubnet_plus.py:182)
         sp.nfb = 3;
@@ -1035,10 +1038,10 @@ static double ws_bytes_per_sample(const fsn_model* m, int T) {
     const fsn_config& c = m->cfg;
     const double F = c.num_freqs, Tp = T + c.look_ahead, rows = F;              // sequences per sample
     double b = 0;
-    if (c.model_kind == FSN_KIND_PLUS) b += 3 * F * Tp * 4 * 2 + 3 * Tp * (4.0 * m->Cp + 512) * 4;       // fb_in/out, X0/Xa/Xb/Xr (fp32), Y1/Y2 (fp16)
+    if (c.model_kind == FSN_KIND_PLUS) b += 3 * F * Tp * 4 * 2 + 3 * Tp * (4.0 * m->tcn_fb.Cp + 512) * 4;   // fb_in/out, X0/Xa/Xb/Xr (fp32), Y1/Y2 (fp16)
     else b += F * Tp * 4 * 4 + Tp * (F + c.fb_hidden) * 4;
     if (c.sb_tcn) {                                                             // input + two fp32 streams of 64 channels, two fp16 hidden
-        b += rows * Tp * (3 * 64 * 4 + 2 * 512 * 2) + rows * (8 * 2 * 2 * 8 + 9 * 4);   // buffers of 512; gLN sums and stream maxima
+        b += rows * Tp * (3 * 64 * 4 + 2 * 512 * 2) + rows * (tcn_stats_bytes(1) + 4);   // buffers of 512; statistics, the input's max |x|
         return b;
     }
     b += rows * Tp * 128;                                                       // packed sub-band images (when used)

@@ -97,6 +97,18 @@ __device__ __forceinline__ void g5_max_add(int key, float v, float* out) {
     }
 }
 
+// gLN of group z from its sum and sum of squares over `count` elements (stats[2z], stats[2z+1]): mean and 1 / sqrt(var + 1e-8)
+__device__ __forceinline__ void gln_mean_rstd(const double* stats, int z, double count, float& mean, float& rstd) {
+    const double mu = stats[2 * z] / count, var = stats[2 * z + 1] / count - mu * mu;
+    mean = (float)mu;
+    rstd = (float)(1.0 / sqrt((var > 0 ? var : 0) + 1e-8));
+}
+
+// one channel of the folded gLN + residual (EPI_GLN_RES): x + rstd * acc - mean * rstd * s1 + b
+__device__ __forceinline__ float gln_res(float x, float acc, float mean, float rstd, float s1, float b) {
+    return x + fmaf(rstd, acc, fmaf(-mean * rstd, s1, b));
+}
+
 template <int EPI, int NT>
 __global__ void __launch_bounds__(G5_THREADS, 1)
 gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, GemmTc5Launch a) {
@@ -230,12 +242,7 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             float mean[2] = {0.f, 0.f}, rstd[2] = {1.f, 1.f}, rowmax[2] = {0.f, 0.f};
 #pragma unroll
             for (int h = 0; h < 2; ++h)
-                if (valid[h]) {
-                    const double su = a.stats_in[2 * z[h]], sq = a.stats_in[2 * z[h] + 1];
-                    const double mu = su / a.count_in, var = sq / a.count_in - mu * mu;
-                    mean[h] = (float)mu;
-                    rstd[h] = (float)(1.0 / sqrt((var > 0 ? var : 0) + 1e-8));
-                }
+                if (valid[h]) gln_mean_rstd(a.stats_in, z[h], a.count_in, mean[h], rstd[h]);
 #pragma unroll
             for (int j = 0; j < NT / 8; ++j) {
                 const int n = n0 + 8 * j + cq;
@@ -246,8 +253,8 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                     if (!valid[h]) continue;
                     const float2 x = *reinterpret_cast<const float2*>(a.Xold + grow[h] * a.ldY + n);
                     float2 o;
-                    o.x = x.x + fmaf(rstd[h], acc[4 * j + 2 * h], fmaf(-mean[h] * rstd[h], s12.x, b2.x));
-                    o.y = x.y + fmaf(rstd[h], acc[4 * j + 2 * h + 1], fmaf(-mean[h] * rstd[h], s12.y, b2.y));
+                    o.x = gln_res(x.x, acc[4 * j + 2 * h], mean[h], rstd[h], s12.x, b2.x);
+                    o.y = gln_res(x.y, acc[4 * j + 2 * h + 1], mean[h], rstd[h], s12.y, b2.y);
                     rowmax[h] = fmaxf(rowmax[h], fmaxf(fabsf(o.x), fabsf(o.y)));
                     *reinterpret_cast<float2*>(a.Y + grow[h] * a.ldY + n) = o;
                     if (a.Xrelu) *reinterpret_cast<float2*>(a.Xrelu + grow[h] * a.ldY + n) = make_float2(fmaxf(o.x, 0.f), fmaxf(o.y, 0.f));
@@ -266,12 +273,7 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             for (int h = 0; h < 2; ++h) {
 #pragma unroll
                 for (int q = 0; q < 8; ++q) fc[h][q] = 0.f;
-                if (valid[h]) {
-                    const double su = a.stats_in[2 * z[h]], sq = a.stats_in[2 * z[h] + 1];
-                    const double mu = su / a.count_in, var = sq / a.count_in - mu * mu;
-                    mean[h] = (float)mu;
-                    rstd[h] = (float)(1.0 / sqrt((var > 0 ? var : 0) + 1e-8));
-                }
+                if (valid[h]) gln_mean_rstd(a.stats_in, z[h], a.count_in, mean[h], rstd[h]);
             }
 #pragma unroll
             for (int j = 0; j < NT / 8; ++j) {
@@ -281,8 +283,8 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                 for (int h = 0; h < 2; ++h) {
                     if (!valid[h]) continue;
                     const float2 x = *reinterpret_cast<const float2*>(a.Xold + grow[h] * a.ldY + n);
-                    const float o0 = fmaxf(x.x + fmaf(rstd[h], acc[4 * j + 2 * h], fmaf(-mean[h] * rstd[h], s12.x, b2.x)), 0.f);
-                    const float o1 = fmaxf(x.y + fmaf(rstd[h], acc[4 * j + 2 * h + 1], fmaf(-mean[h] * rstd[h], s12.y, b2.y)), 0.f);
+                    const float o0 = fmaxf(gln_res(x.x, acc[4 * j + 2 * h], mean[h], rstd[h], s12.x, b2.x), 0.f);
+                    const float o1 = fmaxf(gln_res(x.y, acc[4 * j + 2 * h + 1], mean[h], rstd[h], s12.y, b2.y), 0.f);
 #pragma unroll
                     for (int q = 0; q < 8; ++q)
                         if (q < a.O) {
@@ -430,10 +432,8 @@ __global__ void __launch_bounds__(256) dwconv_tm_kernel(DwTmLaunch a) {
     const int C = a.C, Tp = a.Tp, d = a.dilation;
     const int t0 = blockIdx.y * DW_TCH, t1 = min(t0 + DW_TCH, Tp);
     const int lo = max(t0 - 2 * d, 0), hi = min(t1 + 2 * d, Tp);    // staged frames [lo, hi)
-    const double cnt = (double)C * (double)Tp;
-    const double mu = a.stats_in[2 * z] / cnt;
-    const double var = a.stats_in[2 * z + 1] / cnt - mu * mu;
-    const float mean = (float)mu, rstd = (float)(1.0 / sqrt((var > 0 ? var : 0) + 1e-8));
+    float mean, rstd;
+    gln_mean_rstd(a.stats_in, z, (double)C * (double)Tp, mean, rstd);
     const float slope = __ldg(a.prelu[g]);
     const float unscale = 1.0f / fp16_store_scale(__ldg(a.amax + z));     // exact: a power of two
     const size_t base = (size_t)z * Tp * C + c0;

@@ -99,11 +99,12 @@ struct fsn_model {
         DevBuf tsse_scale, sb_rowsum;
         DevBuf xn, sigma;                              // pre-normalised inputs / sub-band std for the non-default norm types
         DevBuf sbx;                                    // sub-band TCN: input [B*F*T', 64] fp32 time-major | max |x| per sequence [B*F]
+        DevBuf tlen;                                   // ragged forwards: per-sample extent frames[b] + look_ahead as int32 [3][B] (clip_len)
         alignas(64) unsigned char mapX0[128], mapXr[128], mapSbx[128];
         cudaEvent_t ev_front = nullptr, ev_lstm = nullptr;   // front end written / LSTM finished reading this lane
         bool used = false;                             // ev_lstm has been recorded (a pipelined batch ran / may still run in this lane)
         void release_all() {
-            DevBuf* all[] = {&fbin, &fbout, &mu, &ximg, &magpad, &fbx, &hseq, &x0, &xr, &tsse_scale, &sb_rowsum, &xn, &sigma, &sbx};
+            DevBuf* all[] = {&fbin, &fbout, &mu, &ximg, &magpad, &fbx, &hseq, &x0, &xr, &tsse_scale, &sb_rowsum, &xn, &sigma, &sbx, &tlen};
             for (auto* b : all) b->release();
             tcn.release();
         }
@@ -145,6 +146,11 @@ struct fsn_model {
     cudaEvent_t ev0[NEV] = {}, ev1[NEV] = {};               // sub-band LSTM start / end
     cudaEvent_t evf0[NEV] = {}, evf1[NEV] = {};             // front end start / end (same ring index)
     int64_t nfwd = 0;                                 // forwards whose LSTM events were recorded
+    // ragged forwards: pinned staging slots of the per-sample extents.  A slot is refilled only after the event recorded behind its
+    // H2D copy has fired, so the caller's frames array is free when the call returns and no stream has to be synchronised.
+    static const int NLEN = 4;
+    struct LenSlot { int32_t* h = nullptr; size_t cap = 0; cudaEvent_t ev = nullptr; bool used = false; } len_slot[NLEN];
+    int64_t nlen = 0;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -477,6 +483,10 @@ extern "C" void fsn_model_destroy(fsn_model* m) {
         if (m->evf1[i]) cudaEventDestroy(m->evf1[i]);
     }
     for (int i = 0; i < 4; ++i) { m->sb_frag[i].release(); m->sb_bias[i].release(); m->fb_frag[i].release(); m->fb_bias[i].release(); }
+    for (auto& ls : m->len_slot) {
+        if (ls.h) cudaFreeHost(ls.h);
+        if (ls.ev) cudaEventDestroy(ls.ev);
+    }
     delete m;
 }
 
@@ -681,7 +691,7 @@ static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, cudaStream
 // d_enh != null: write the enhanced spectrum (decompress_cIRM x noisy) instead of the mask -- fused into the epilogue of the
 // layer-wise kernel's last layer, a separate pass over a scratch mask for the generic kernel
 static int run_sb_lstm(fsn_model* m, fsn_model::Lane& ln, int B, int T, float* d_out, const float* d_real, const float* d_imag,
-                       float* d_enh, cudaStream_t s) {
+                       float* d_enh, const int* tlen, cudaStream_t s) {
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs, Tp = T + c.look_ahead, rows = B * F, ntiles = (rows + 127) / 128;
     const int impl = pick_impl(m);
@@ -711,7 +721,7 @@ static int run_sb_lstm(fsn_model* m, fsn_model::Lane& ln, int B, int T, float* d
             a.cstate = static_cast<float*>(m->cstate.p);
             a.out = d_out; a.F = F; a.la = c.look_ahead;
             a.act = c.sb_act; a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU; a.last = (l == c.num_layers - 1);
-            a.nreal = d_real; a.nimag = d_imag; a.enh = reinterpret_cast<float2*>(d_enh);
+            a.nreal = d_real; a.nimag = d_imag; a.enh = reinterpret_cast<float2*>(d_enh); a.tlen = tlen;
             int e = launch_lstm_tc5r(a, s);
             if (e) return fail(FSN_ECUDA, "layer-wise LSTM launch failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)e));
             m->launches++;
@@ -732,14 +742,14 @@ static int run_sb_lstm(fsn_model* m, fsn_model::Lane& ln, int B, int T, float* d
         a.cstate = static_cast<float*>(m->cstate.p);
         lstm_mma_cstate_bytes(c.num_layers, rows, c.sb_hidden, &a.rows_alloc);
         a.out = d_out; a.O = c.output_size; a.F = F; a.la = c.look_ahead; a.act = c.sb_act;
-        a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU;
+        a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU; a.tlen = tlen;
         if (d_enh) {                                                    // generic kernel: mask into a scratch buffer, then one fused post-processing pass
             if (m->mask_tmp.ensure((size_t)B * 2 * F * T * 4, false, s)) return fail(FSN_ECUDA, "allocation failed");
             a.out = static_cast<float*>(m->mask_tmp.p);
         }
         int e = launch_lstm_mma(a, s);
         if (e) return fail(FSN_ECUDA, "mma LSTM launch failed: %s", cudaGetErrorString((cudaError_t)e));
-        if (d_enh) { launch_apply_cirm_planar(a.out, d_real, d_imag, reinterpret_cast<float2*>(d_enh), B, F, T, s); m->launches++; }
+        if (d_enh) { launch_apply_cirm_planar(a.out, d_real, d_imag, reinterpret_cast<float2*>(d_enh), B, F, T, tlen, c.look_ahead, s); m->launches++; }
     }
     m->launches++;
     return FSN_OK;
@@ -754,8 +764,9 @@ static void set_tcn_rows(GemmTc5Launch& g, const TcnWeights& w, int G, int Tp) {
 // GEMM1 (1x1 conv + PReLU + gLN1 statistics), the depth-wise convolution, GEMM2 (folded gLN2 + residual), the stream ping-ponging between
 // sc.xa and sc.xb from the input x (tensor map xmap).  amax0: block 0's stream maxima [nbr * G], written with the input.  The last
 // GEMM2 ends as `last` says: its epilogue (EPI5_GLN_RES or EPI5_GLN_HEAD) and that epilogue's own outputs (Xrelu, or the head fields).
+// tlen / zdiv: the per-sample extents of a ragged forward (GemmTc5Launch::tlen), or null.
 static int run_tcn_blocks(fsn_model* m, const TcnWeights& w, TcnScratch& sc, const float* x, const unsigned char* xmap, const float* amax0,
-                          int G, int Tp, bool causal, const GemmTc5Launch& last, cudaStream_t s) {
+                          int G, int Tp, bool causal, const GemmTc5Launch& last, const int* tlen, int zdiv, cudaStream_t s) {
     static const int dil[8] = {1, 2, 5, 9, 1, 2, 5, 9};
     const size_t Z = (size_t)w.nbr * G;
     const float* curp = x;
@@ -769,7 +780,7 @@ static int run_tcn_blocks(fsn_model* m, const TcnWeights& w, TcnScratch& sc, con
         set_tcn_rows(g1, w, G, Tp);
         g1.epi = EPI5_PRELU_STATS; g1.Kp = w.Cp; g1.NT = 128; g1.ntiles_n = 4; g1.Npad = 512;
         for (int b = 0; b < w.nbr; ++b) { g1.bias[b] = P(m, key(b, "conv1x1.bias")); g1.prelu[b] = P(m, key(b, "prelu1.weight")); }
-        g1.stats_out = st1; g1.Y16 = static_cast<__half*>(sc.y1.p); g1.ldY = 512; g1.amax_in = amax_in;
+        g1.stats_out = st1; g1.Y16 = static_cast<__half*>(sc.y1.p); g1.ldY = 512; g1.amax_in = amax_in; g1.tlen = tlen; g1.zdiv = zdiv;
         int e = launch_gemm_tc5(curmap, w.mapW1[blk], g1, m->num_sms, s);
         if (e) return fail(FSN_ECUDA, "%s GEMM1 launch failed: %s", w.name, cudaGetErrorString((cudaError_t)e));
         m->launches++;
@@ -777,7 +788,7 @@ static int run_tcn_blocks(fsn_model* m, const TcnWeights& w, TcnScratch& sc, con
         DwTmLaunch dw{};
         dw.X = static_cast<const __half*>(sc.y1.p); dw.Y = static_cast<__half*>(sc.y2.p);
         dw.Z = (int)Z; dw.B = G; dw.C = 512; dw.Tp = Tp; dw.dilation = dil[blk]; dw.causal = causal ? 1 : 0;
-        dw.stats_in = st1; dw.stats_out = st2; dw.amax = amax_in;
+        dw.stats_in = st1; dw.stats_out = st2; dw.amax = amax_in; dw.tlen = tlen; dw.zdiv = zdiv;
         for (int b = 0; b < w.nbr; ++b) {
             dw.gamma[b] = P(m, key(b, "norm1.weight")); dw.beta[b] = P(m, key(b, "norm1.bias"));
             dw.w[b] = P(m, key(b, "depthwise_conv.weight")); dw.b[b] = P(m, key(b, "depthwise_conv.bias"));
@@ -796,7 +807,7 @@ static int run_tcn_blocks(fsn_model* m, const TcnWeights& w, TcnScratch& sc, con
             g2.bias[b] = static_cast<const float*>(w.S2b.p) + ((size_t)blk * w.nbr + b) * w.Cp;
             g2.s1[b] = static_cast<const float*>(w.S1.p) + ((size_t)blk * w.nbr + b) * w.Cp;
         }
-        g2.stats_in = st2; g2.count_in = (double)512 * Tp;
+        g2.stats_in = st2; g2.count_row = 512; g2.tlen = tlen; g2.zdiv = zdiv;
         g2.Xold = curp; g2.ldY = w.Cp;
         if (g2.epi == EPI5_GLN_RES) g2.Y = nxtp;
         e = launch_gemm_tc5(sc.mapY2, w.mapW2[blk], g2, m->num_sms, s);
@@ -812,7 +823,7 @@ static int run_tcn_blocks(fsn_model* m, const TcnWeights& w, TcnScratch& sc, con
 // input as the gLN groups and Isb (<= 64) channels in one 64-column N tile; the last block's second 1x1 convolution ends in ReLU + Linear +
 // activation (EPI5_GLN_HEAD) and writes the mask -- or, with d_enh, the enhanced spectrum.
 static int run_sb_tcn(fsn_model* m, fsn_model::Lane& ln, int B, int T, float* d_out, const float* d_real, const float* d_imag, float* d_enh,
-                      cudaStream_t s) {
+                      const int* tlen, cudaStream_t s) {
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs, Tp = T + c.look_ahead, Z = B * F;
     m->last_impl = FSN_LSTM_TCN;
@@ -823,14 +834,37 @@ static int run_sb_tcn(fsn_model* m, fsn_model::Lane& ln, int B, int T, float* d_
     head.O = c.output_size; head.la = c.look_ahead; head.F = F; head.act = c.sb_act;
     head.out = d_out; head.nreal = d_real; head.nimag = d_imag; head.enh = reinterpret_cast<float2*>(d_enh);
     const float* x = static_cast<const float*>(ln.sbx.p);
-    return run_tcn_blocks(m, m->tcn_sb, m->sb_scratch, x, ln.mapSbx, x + (size_t)Z * Tp * 64, Z, Tp, false, head, s);
+    return run_tcn_blocks(m, m->tcn_sb, m->sb_scratch, x, ln.mapSbx, x + (size_t)Z * Tp * 64, Z, Tp, false, head, tlen, F, s);
 }
 
 // The whole forward.  Front end (norm, attention, full-band model, sub-band statistics + packing) on stream `s` into lane `ln`;
 // the sub-band LSTM on stream `sl` (== s for the plain entry point; the pipelined entry points pass the LSTM stream, ordered
 // after the front end by the lane's ev_front).
+// Copy the per-sample extents frames[b] + look_ahead of a ragged forward into the lane's device buffer ln.tlen ([3][B]: one row per
+// full-band branch, so a full-band gLN group z = branch * B + b indexes it directly) through the next pinned staging slot.
+static int stage_lengths(fsn_model* m, fsn_model::Lane& ln, const int32_t* h_frames, int B, cudaStream_t s) {
+    fsn_model::LenSlot& ls = m->len_slot[m->nlen++ % fsn_model::NLEN];
+    const size_t n = (size_t)3 * B;
+    if (!ls.ev) CK(cudaEventCreateWithFlags(&ls.ev, cudaEventDisableTiming));
+    if (ls.used) CK(cudaEventSynchronize(ls.ev));                        // the copy that last read this slot has completed
+    if (ls.cap < n) {
+        if (ls.h) CK(cudaFreeHost(ls.h));
+        ls.h = nullptr; ls.cap = 0;
+        CK(cudaHostAlloc(reinterpret_cast<void**>(&ls.h), n * sizeof(int32_t), cudaHostAllocDefault));
+        ls.cap = n;
+    }
+    for (int br = 0; br < 3; ++br)
+        for (int b = 0; b < B; ++b) ls.h[(size_t)br * B + b] = h_frames[b] + m->cfg.look_ahead;
+    if (ln.tlen.ensure(n * sizeof(int32_t), false, s)) return fail(FSN_ECUDA, "workspace allocation failed for the clip lengths");
+    CK(cudaMemcpyAsync(ln.tlen.p, ls.h, n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CK(cudaEventRecord(ls.ev, s));
+    ls.used = true;
+    return FSN_OK;
+}
+
+// h_frames: the frame count of every sample of a ragged batch (validated by the caller), or null when every sample spans T frames
 static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
-                        float* d_out, float* d_enh, cudaStream_t s, cudaStream_t sl) {
+                        const int32_t* h_frames, float* d_out, float* d_enh, cudaStream_t s, cudaStream_t sl) {
     if (!m || !d_mag || (!d_out && !d_enh)) return fail(FSN_EINVAL, "null argument");
     if (d_enh && (!d_real || !d_imag)) return fail(FSN_EINVAL, "the enhanced-spectrum output needs the noisy real and imaginary planes");
     if (d_enh && m->cfg.output_size != 2) return fail(FSN_EINVAL, "the enhanced-spectrum output needs output_size 2 (a complex mask)");
@@ -847,6 +881,12 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
             if (Tp < c.kersize[i]) return fail(FSN_EINVAL, "sequence shorter than the TSSE kernel size");
     int rc = ensure_ws(m, ln, B, T, s, sl);
     if (rc) return rc;
+    const int* tl = nullptr;                                            // per-sample extents on the device (null: all Tp)
+    if (h_frames) {
+        rc = stage_lengths(m, ln, h_frames, B, s);
+        if (rc) return rc;
+        tl = static_cast<const int*>(ln.tlen.p);
+    }
     m->launches = 0;
     m->last_lane = (int)(&ln - m->lane);
     const int evi = (int)(m->nfwd % fsn_model::NEV);
@@ -860,6 +900,7 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
     sp.norm_type = c.norm_type;
     sp.ximg = static_cast<__half*>(ln.ximg.p);
     sp.ntiles = (B * F + 127) / 128;
+    sp.tlen = tl;
 
     if (c.model_kind == FSN_KIND_PLUS) {
         const char* sfx[3] = {"", "_real", "_imag"};
@@ -885,10 +926,11 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
         ta.scale = static_cast<float*>(ln.tsse_scale.p);
         ta.rows = ta.scale + (size_t)ta.nbranch * B * F;
         ta.out_tm = static_cast<float*>(ln.x0.p); ta.Cp = m->tcn_fb.Cp;
+        ta.tlen = tl;
         if (c.norm_type != FSN_NORM_OFFLINE_LAPLACE) {
             NormLaunch na{};
             na.x[0] = d_mag; na.x[1] = d_real; na.x[2] = d_imag; na.y = static_cast<float*>(ln.xn.p);
-            na.nbranch = 3; na.B = B; na.F = F; na.T = T; na.Tp = Tp; na.type = c.norm_type;
+            na.nbranch = 3; na.B = B; na.F = F; na.T = T; na.Tp = Tp; na.type = c.norm_type; na.tlen = tl;
             launch_input_norm(na, s); m->launches++;
             for (int b = 0; b < 3; ++b) ta.x[b] = static_cast<const float*>(ln.xn.p) + (size_t)b * B * F * Tp;
             ta.T = Tp; ta.prenorm = 1;                                  // padded frames are part of the normalised signal
@@ -900,13 +942,13 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
 
         GemmTc5Launch last{};                                           // the last block also writes relu(x) for the output Linear
         last.epi = EPI5_GLN_RES; last.Xrelu = static_cast<float*>(ln.xr.p);
-        rc = run_tcn_blocks(m, w, ln.tcn, static_cast<const float*>(ln.x0.p), ln.mapX0, ta.amax, B, Tp, c.tcn_causal, last, s);
+        rc = run_tcn_blocks(m, w, ln.tcn, static_cast<const float*>(ln.x0.p), ln.mapX0, ta.amax, B, Tp, c.tcn_causal, last, tl, 1, s);
         if (rc) return rc;
         GemmTc5Launch g3{};
         set_tcn_rows(g3, w, B, Tp);
         g3.epi = EPI5_OUT; g3.Kp = w.Cp; g3.NT = w.NT; g3.ntiles_n = w.ntiles; g3.Npad = w.Cp;
         for (int b = 0; b < 3; ++b) g3.bias[b] = static_cast<const float*>(m->fb_fc_b.p) + (size_t)b * w.Cp;
-        g3.out = static_cast<float*>(ln.fbout.p); g3.F = F; g3.P = Pp; g3.act = c.fb_act;
+        g3.out = static_cast<float*>(ln.fbout.p); g3.F = F; g3.P = Pp; g3.act = c.fb_act;    // finite past each clip's end; the sub-band stages mask it
         int e = launch_gemm_tc5(ln.mapXr, m->map_fb_fc, g3, m->num_sms, s);
         if (e) return fail(FSN_ECUDA, "TCN output GEMM launch failed: %s", cudaGetErrorString((cudaError_t)e));
         m->launches++;
@@ -920,15 +962,18 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
         ta.out = static_cast<float*>(ln.fbin.p);
         ta.scale = static_cast<float*>(ln.tsse_scale.p);
         ta.rows = ta.scale + (size_t)ta.nbranch * B * F;
+        ta.tlen = tl;
         if (c.norm_type != FSN_NORM_OFFLINE_LAPLACE) {
             NormLaunch na{};
             na.x[0] = d_mag; na.y = static_cast<float*>(ln.xn.p);
-            na.nbranch = 1; na.B = B; na.F = F; na.T = T; na.Tp = Tp; na.type = c.norm_type;
+            na.nbranch = 1; na.B = B; na.F = F; na.T = T; na.Tp = Tp; na.type = c.norm_type; na.tlen = tl;
             launch_input_norm(na, s); m->launches++;
             ta.x[0] = static_cast<const float*>(ln.xn.p); ta.T = Tp; ta.prenorm = 1;
         }
         launch_tsse_norm(ta, s); m->launches += 3;
-        launch_pad_copy(d_mag, static_cast<float*>(ln.magpad.p), B, F, T, Pp, s); m->launches++;
+        launch_pad_copy(d_mag, static_cast<float*>(ln.magpad.p), B, F, T, Pp, tl, c.look_ahead, s); m->launches++;
+        // the full-band LSTM is causal, and its input (fb_in) is already zero past each clip's end: its outputs there are masked by the
+        // sub-band stages
         const int Ipad = (F + 15) / 16 * 16, rows_pad = (B + 63) / 64 * 64;
         launch_fb_pack(static_cast<const float*>(ln.fbin.p), static_cast<__half*>(ln.fbx.p), B, F, Tp, Pp, rows_pad, Ipad, s); m->launches++;
         if (lstm_ws_supported(c.num_layers, c.fb_hidden, Ipad, B, m->num_sms) && !m->env_no_ws) {
@@ -984,7 +1029,7 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
         CK(cudaStreamWaitEvent(sl, ln.ev_front, 0));
     }
     cudaEventRecord(m->ev0[evi], sl);
-    rc = c.sb_tcn ? run_sb_tcn(m, ln, B, T, d_out, d_real, d_imag, d_enh, sl) : run_sb_lstm(m, ln, B, T, d_out, d_real, d_imag, d_enh, sl);
+    rc = c.sb_tcn ? run_sb_tcn(m, ln, B, T, d_out, d_real, d_imag, d_enh, tl, sl) : run_sb_lstm(m, ln, B, T, d_out, d_real, d_imag, d_enh, tl, sl);
     cudaEventRecord(m->ev1[evi], sl);
     if (rc) return rc;
     m->nfwd++;
@@ -1023,7 +1068,7 @@ static int submit_impl(fsn_model* m, cudaEvent_t ready, const float* d_mag, cons
     if (ready) CK(cudaStreamWaitEvent(sf, ready, 0));
     if (m->plain_pending) { CK(cudaStreamWaitEvent(sf, m->ev_plain, 0)); CK(cudaStreamWaitEvent(m->s_lstm, m->ev_plain, 0)); }
     if (ln.used) CK(cudaStreamWaitEvent(sf, ln.ev_lstm, 0));              // the LSTM that read this lane has finished
-    rc = forward_impl(m, ln, d_mag, d_real, d_imag, B, T, d_out, d_enh, sf, m->s_lstm);
+    rc = forward_impl(m, ln, d_mag, d_real, d_imag, B, T, nullptr, d_out, d_enh, sf, m->s_lstm);
     if (rc) return rc;
     CK(cudaEventRecord(ln.ev_lstm, m->s_lstm));
     ln.used = true;
@@ -1051,7 +1096,7 @@ static double ws_bytes_per_sample(const fsn_model* m, int T) {
 }
 
 static int forward_plain(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
-                         float* d_out, float* d_enh, void* stream) {
+                         const int32_t* h_frames, float* d_out, float* d_enh, void* stream) {
     if (!m) return fail(FSN_EINVAL, "null argument");
     if (!m->finalized) return fail(FSN_ESTATE, "fsn_model_finalize has not been called");
     if (B < 1 || T < 1) return fail(FSN_EINVAL, "bad batch/frames");
@@ -1065,7 +1110,7 @@ static int forward_plain(fsn_model* m, const float* d_mag, const float* d_real, 
     if (Bmax < 1) Bmax = 1;
     int rc = FSN_OK;
     if (B <= Bmax) {
-        rc = forward_impl(m, m->lane[0], d_mag, d_real, d_imag, B, T, d_out, d_enh, s, s);
+        rc = forward_impl(m, m->lane[0], d_mag, d_real, d_imag, B, T, h_frames, d_out, d_enh, s, s);
     } else {
         const int nsplit = (B + Bmax - 1) / Bmax, Bs = (B + nsplit - 1) / nsplit;
         const size_t in_stride = (size_t)m->cfg.num_freqs * T, out_stride = (size_t)m->cfg.output_size * m->cfg.num_freqs * T;
@@ -1073,7 +1118,8 @@ static int forward_plain(fsn_model* m, const float* d_mag, const float* d_real, 
         for (int b0 = 0; b0 < B && rc == FSN_OK; b0 += Bs) {
             const int nb = (B - b0 < Bs) ? B - b0 : Bs;
             rc = forward_impl(m, m->lane[0], d_mag + b0 * in_stride, d_real ? d_real + b0 * in_stride : nullptr, d_imag ? d_imag + b0 * in_stride : nullptr,
-                              nb, T, d_out ? d_out + b0 * out_stride : nullptr, d_enh ? d_enh + b0 * in_stride * 2 : nullptr, s, s);
+                              nb, T, h_frames ? h_frames + b0 : nullptr, d_out ? d_out + b0 * out_stride : nullptr,
+                              d_enh ? d_enh + b0 * in_stride * 2 : nullptr, s, s);
             launches += m->launches;
         }
         m->launches = launches;
@@ -1097,12 +1143,51 @@ static int submit_plain(fsn_model* m, const float* d_mag, const float* d_real, c
 extern "C" int fsn_model_forward(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
                                  float* d_out, void* stream) {
     if (!d_out) return fail(FSN_EINVAL, "null argument");
-    return forward_plain(m, d_mag, d_real, d_imag, B, T, d_out, nullptr, stream);
+    return forward_plain(m, d_mag, d_real, d_imag, B, T, nullptr, d_out, nullptr, stream);
 }
 extern "C" int fsn_model_forward_enhance(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
                                          float* d_enh, void* stream) {
     if (!d_enh) return fail(FSN_EINVAL, "null argument");
-    return forward_plain(m, d_mag, d_real, d_imag, B, T, nullptr, d_enh, stream);
+    return forward_plain(m, d_mag, d_real, d_imag, B, T, nullptr, nullptr, d_enh, stream);
+}
+
+// The frame counts of a ragged batch: each in 1..T, and long enough for the TSSE convolutions.  Returns the array to pass on: null
+// when every clip spans all T frames, so that case runs exactly the unmasked forward.
+static int check_frames(const fsn_model* m, const int32_t* h_frames, int32_t B, int32_t T, const int32_t** use) {
+    *use = nullptr;
+    if (!h_frames) return FSN_OK;
+    if (!m) return fail(FSN_EINVAL, "null argument");
+    const fsn_config& c = m->cfg;
+    int kmax = 1;
+    if (c.model_kind == FSN_KIND_PLUS && c.channel_attention == FSN_ATTN_TSSE)
+        for (int i = 0; i < 3; ++i) kmax = c.kersize[i] > kmax ? c.kersize[i] : kmax;
+    bool all = true;
+    for (int b = 0; b < B; ++b) {
+        const int n = h_frames[b];
+        if (n < 1 || n > T) return fail(FSN_EINVAL, "frames[%d] = %d is outside 1..T = %d", b, n, T);
+        if (n + c.look_ahead < kmax)
+            return fail(FSN_EINVAL, "frames[%d] = %d: frames + look_ahead = %d is shorter than the TSSE kernel size %d", b, n, n + c.look_ahead, kmax);
+        all = all && n == T;
+    }
+    if (!all) *use = h_frames;
+    return FSN_OK;
+}
+
+extern "C" int fsn_model_forward_ragged(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
+                                        const int32_t* h_frames, float* d_out, void* stream) {
+    if (!d_out) return fail(FSN_EINVAL, "null argument");
+    if (B < 1 || T < 1) return fail(FSN_EINVAL, "bad batch/frames");
+    const int32_t* fr = nullptr;
+    int rc = check_frames(m, h_frames, B, T, &fr);
+    return rc ? rc : forward_plain(m, d_mag, d_real, d_imag, B, T, fr, d_out, nullptr, stream);
+}
+extern "C" int fsn_model_forward_enhance_ragged(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
+                                                const int32_t* h_frames, float* d_enh, void* stream) {
+    if (!d_enh) return fail(FSN_EINVAL, "null argument");
+    if (B < 1 || T < 1) return fail(FSN_EINVAL, "bad batch/frames");
+    const int32_t* fr = nullptr;
+    int rc = check_frames(m, h_frames, B, T, &fr);
+    return rc ? rc : forward_plain(m, d_mag, d_real, d_imag, B, T, fr, nullptr, d_enh, stream);
 }
 extern "C" int fsn_model_submit(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
                                 float* d_out, void* stream) {

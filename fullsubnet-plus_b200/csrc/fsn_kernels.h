@@ -47,11 +47,12 @@ struct TsseLaunch {
     int prenorm;               // 1: input is already normalised (input_norm_kernel), skip the utterance-mean division
     int sub;                   // subband_num (ECA, mag branch only): channels are groups of `sub` reflect-padded bins (fullsubnet_plus.py:146-153)
     float* out_tm; int Cp;     // optional time-major copy [(branch, b, t), Cp] for the TCN GEMMs (pad columns stay zero)
+    const int* tlen;           // optional [nbranch, B] per-sample extent frames[b] + look_ahead (clip_len); null: every sample spans Tp
 };
 inline size_t tsse_row_floats() { return 3 + 2 * 16; }
 void launch_tsse_norm(const TsseLaunch& a, cudaStream_t s);
 // norm types other than offline_laplace_norm (reference base_model.py:227-316): y[nbranch, B, F, Tp] = norm(pad(x))
-struct NormLaunch { const float* x[3]; float* y; int nbranch, B, F, T, Tp, type; };
+struct NormLaunch { const float* x[3]; float* y; int nbranch, B, F, T, Tp, type; const int* tlen; };   // tlen: as TsseLaunch
 void launch_input_norm(const NormLaunch& a, cudaStream_t s);
 
 struct ConvLaunch {          // Y[z] = act(W X[z] + b): output Linear of the full-band LSTM (fullsubnet.Model)
@@ -78,6 +79,7 @@ struct SbPackLaunch {
     int ntiles;
     float* xtm;              // sub-band TCN input: fp32 time-major [B*F*Tp, 64], row (b*F + f)*Tp + t, columns >= I zero
     float* amax;             // [B*F] max |x| of every sequence of xtm (zeroed by the launcher): block 0's fp16 store scale
+    const int* tlen;         // optional [B] per-sample extent in frames of Tp (rows past it are written as zero); null: Tp
 };
 void launch_sb_stats(const SbPackLaunch& a, cudaStream_t s);
 void launch_sb_pack(const SbPackLaunch& a, cudaStream_t s);
@@ -85,14 +87,16 @@ void launch_sb_pack(const SbPackLaunch& a, cudaStream_t s);
 void launch_sb_pack_tm(const SbPackLaunch& a, cudaStream_t s);
 // time-major [Z*Tp, ld] -> [Z, C, Tp] (test hook of the sub-band TCN input)
 void launch_tm_to_fm(const float* x, int ld, float* y, int Z, int C, int Tp, cudaStream_t s);
-// [B, F, T] fp32 (+ zero look-ahead pad) -> zero-padded copy [B, F, P]
-void launch_pad_copy(const float* x, float* y, int B, int F, int T, int P, cudaStream_t s);
+// [B, F, T] fp32 (+ zero look-ahead pad) -> zero-padded copy [B, F, P]; with tlen [B], sample b's input ends at tlen[b] - la
+void launch_pad_copy(const float* x, float* y, int B, int F, int T, int P, const int* tlen, int la, cudaStream_t s);
 // full-band LSTM input: [B, F, P] fp32 -> [Tp, Bpad, Ipad] fp16 (rows >= B and k >= F zero)
 void launch_fb_pack(const float* x, __half* y, int B, int F, int Tp, int P, int rows_pad, int Ipad, cudaStream_t s);
 
 void launch_apply_cirm(const float* crm, const float2* noisy, float2* enh, int B, int F, int T, cudaStream_t s);
-// same with the noisy spectrum as two planes [B, F, T] (the model's own real / imag inputs)
-void launch_apply_cirm_planar(const float* crm, const float* nreal, const float* nimag, float2* enh, int B, int F, int T, cudaStream_t s);
+// same with the noisy spectrum as two planes [B, F, T] (the model's own real / imag inputs); with tlen [B], frames
+// t >= tlen[b] - la are written as zero without reading the planes
+void launch_apply_cirm_planar(const float* crm, const float* nreal, const float* nimag, float2* enh, int B, int F, int T, const int* tlen,
+                              int la, cudaStream_t s);
 
 // streaming step kernels (k_front.cu): one frame of the cumulative norms with running sums carried in global memory
 struct StreamNormLaunch { const float* x; float* y; double* cum; int B, F, P, n, type; };       // x [B,F] -> y [B,F,P] (t = 0)
@@ -124,6 +128,7 @@ struct LstmMmaLaunch {
     int gru;                  // 1: pseudo-gate GRU cell (gru_cell), cstate carries h in fp32
     // streaming: hidden state carried across launches ([L, rows_alloc, H] fp16); resume = 1 continues from it
     __half* hstate; int resume;
+    const int* tlen;          // optional [B] per-sample extent in frames of Tp: output frames t - la >= tlen[b] - la are written as zero
 };
 size_t lstm_mma_cstate_bytes(int L, int rows, int H, int* rows_alloc);
 int launch_lstm_mma(const LstmMmaLaunch& a, cudaStream_t s);   // returns 0 or cudaError
@@ -161,6 +166,7 @@ struct LstmTc5rLaunch {
     // fused post-processing (inferencer.py:152-157): when enh != null the last layer decompresses the cIRM and multiplies it with the
     // noisy spectrum (planes [B, F, T]) instead of writing the mask: enh [B, F, T] complex64 (interleaved re, im)
     const float* nreal; const float* nimag; float2* enh;
+    const int* tlen;          // optional [B] per-sample extent in frames of Tp: output frames t - la >= tlen[b] - la are written as zero
 };
 bool lstm_tc5r_supported(int H, int O);
 size_t lstm_tc5r_cstate_bytes(int ntiles, int H);
@@ -187,7 +193,7 @@ struct GemmTc5Launch {
     const float* prelu[3];
     const float* s1[3];                        // GLN_RES: sum_c W'[n, c]
     double* stats_out;                         // [Z, 2]
-    const double* stats_in; double count_in;
+    const double* stats_in; double count_row;  // GLN_RES / GLN_HEAD: elements per row in stats_in (a group's count: count_row x its frames)
     float* Y; int ldY;                         // GLN_RES: new residual stream (fp32)
     __half* Y16;                               // PRELU_STATS: the hidden activation, fp16 [rows, ldY], stored times fp16_store_scale(amax_in[z]); F16OUT: C
     const float* amax_in;                      // PRELU_STATS: [Z] max |x| of the block's input stream per sample
@@ -199,6 +205,9 @@ struct GemmTc5Launch {
     const float* fc_w; const float* fc_b;      // [O, 64] (columns >= I zero), [O]
     int O, la;
     const float* nreal; const float* nimag; float2* enh;
+    // optional per-sample extent in frames of Tp, tlen[z / zdiv] for gLN group z (full band: z = branch * B + b, tlen [3][B], zdiv 1;
+    // sub band: z = b * F + f, zdiv F).  Rows t >= that extent are written as zero and left out of every statistic and maximum
+    const int* tlen; int zdiv;
 };
 int make_tmap_f32_2d(void* out_map /*128 B, 64 B aligned*/, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows);
 int launch_gemm_tc5(const void* mapA, const void* mapB, GemmTc5Launch a, int num_sms, cudaStream_t s);
@@ -209,6 +218,7 @@ struct DwTmLaunch {
     const double* stats_in; double* stats_out;
     const float* amax;                         // [Z]: X holds the activation times fp16_store_scale(amax[z]); the statistics are unscaled
     const float* gamma[3]; const float* beta[3]; const float* w[3]; const float* b[3]; const float* prelu[3];
+    const int* tlen; int zdiv;                 // as GemmTc5Launch: taps past the extent read zero, rows past it are written as zero
 };
 int launch_dwconv_tm(const DwTmLaunch& a, cudaStream_t s);
 

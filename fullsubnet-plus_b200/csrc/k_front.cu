@@ -29,11 +29,12 @@ __global__ void __launch_bounds__(256) tsse_rowstats_kernel(TsseLaunch a) {
     pdl_trigger();
     pdl_wait();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int F = a.F, T = a.T, Tp = a.Tp;
+    const int F = a.F;
     const int r = blockIdx.x * 8 + warp;                          // (branch, sample, bin)
     if (r >= a.nbranch * a.B * F) return;
     const int z = r / F, f = r % F, br = z / a.B, b = z % a.B;
-    const float* row = a.x[br] + ((size_t)b * F + f) * T;
+    const float* row = a.x[br] + ((size_t)b * F + f) * a.T;       // row pitch a.T; the sample's own extent T (input), Tp (padded)
+    const int Tp = a.tlen ? a.tlen[z] : a.Tp, T = Tp - (a.Tp - a.T);
     float acc = 0.f, mx = -INFINITY, mn = INFINITY;
     for (int t0 = 0; t0 < T; t0 += 256) {                         // eight independent loads per lane in flight
         float v[8];
@@ -67,7 +68,7 @@ __global__ void __launch_bounds__(1024) tsse_norm_kernel(TsseLaunch a) {
     pdl_trigger();
     pdl_wait();
     const int b = blockIdx.x, br = blockIdx.y;
-    const int F = a.F, T = a.T, Tp = a.Tp;
+    const int F = a.F, Tp = a.tlen ? a.tlen[br * a.B + b] : a.Tp, T = Tp - (a.Tp - a.T);   // this sample's extent
     float* S = sm;                                  // [F] row sums
     float* Pfx = S + F;                             // [F][KMAX]   Pfx[f][j] = sum_{t<j} x[f][t]
     float* Sfx = Pfx + F * TSSE_KMAX;               // [F][KMAX]   Sfx[f][m] = sum_{t>=Tp-m} x[f][t]
@@ -223,17 +224,18 @@ __global__ void __launch_bounds__(256) tsse_apply_kernel(TsseLaunch a) {
     __shared__ float tr[32][33];
     pdl_trigger();
     pdl_wait();
-    const int z = blockIdx.z, br = z / a.B, b = z % a.B, F = a.F, T = a.T, Tp = a.Tp;
+    const int z = blockIdx.z, br = z / a.B, b = z % a.B, F = a.F, Tp = a.Tp;
+    const int T = a.tlen ? a.tlen[z] - (a.Tp - a.T) : a.T;        // frames of this sample's input: zero from here on in both layouts
     const int f0 = blockIdx.y * 32, t0 = blockIdx.x * 32;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const float* x = a.x[br] + (size_t)b * F * T;
+    const float* x = a.x[br] + (size_t)b * F * a.T;
     float* out = a.out + (size_t)z * F * a.P;
     float* otm = a.out_tm ? a.out_tm + (size_t)z * Tp * a.Cp : nullptr;
     for (int rr = warp; rr < 32; rr += 8) {
         const int f = f0 + rr, t = t0 + lane;
         float v = 0.f;
         if (f < F && t < a.P) {
-            v = (t < T) ? x[(size_t)f * T + t] * a.scale[(size_t)z * F + f] : 0.f;
+            v = (t < T) ? x[(size_t)f * a.T + t] * a.scale[(size_t)z * F + f] : 0.f;
             out[(size_t)f * a.P + t] = v;
         }
         tr[rr][lane] = v;
@@ -264,6 +266,7 @@ void launch_tsse_norm(const TsseLaunch& a, cudaStream_t s) {
 __global__ void __launch_bounds__(256) input_norm_kernel(NormLaunch a) {
     extern __shared__ float sm[];
     const int b = blockIdx.x, br = blockIdx.y, F = a.F, T = a.T, Tp = a.Tp;
+    const int Tpe = a.tlen ? a.tlen[br * a.B + b] : Tp, Te = Tpe - (Tp - T);   // this sample's extent: padded, input
     float* cs = sm;             // [Tp] column sums
     float* cq = cs + Tp;        // [Tp] column sums of squares
     float* sa = cq + Tp;        // [Tp] scale
@@ -271,7 +274,7 @@ __global__ void __launch_bounds__(256) input_norm_kernel(NormLaunch a) {
     const float* x = a.x[br] + (size_t)b * F * T;
     for (int t = threadIdx.x; t < Tp; t += blockDim.x) {
         float s = 0.f, q = 0.f;
-        if (t < T)
+        if (t < Te)
             for (int f = 0; f < F; ++f) { const float v = x[(size_t)f * T + t]; s += v; q = fmaf(v, v, q); }
         cs[t] = s; cq[t] = q;
     }
@@ -280,14 +283,14 @@ __global__ void __launch_bounds__(256) input_norm_kernel(NormLaunch a) {
         const double EPS = 1.1920928955078125e-07;            // np.finfo(np.float32).eps (audio_zen/constant.py:8)
         if (a.type == FSN_NORM_OFFLINE_GAUSSIAN) {
             double s = 0, q = 0;
-            for (int t = 0; t < Tp; ++t) { s += cs[t]; q += cq[t]; }
-            const double n = (double)F * Tp, mu = s / n;
+            for (int t = 0; t < Tpe; ++t) { s += cs[t]; q += cq[t]; }
+            const double n = (double)F * Tpe, mu = s / n;
             const double var = (q - n * mu * mu) / (n - 1.0);  // torch.std: unbiased
             const double inv = 1.0 / (sqrt(var > 0 ? var : 0) + 1e-5);
-            for (int t = 0; t < Tp; ++t) { sa[t] = (float)inv; sb[t] = (float)(-mu * inv); }
+            for (int t = 0; t < Tpe; ++t) { sa[t] = (float)inv; sb[t] = (float)(-mu * inv); }
         } else {
             double s = 0, q = 0;
-            for (int t = 0; t < Tp; ++t) {
+            for (int t = 0; t < Tpe; ++t) {
                 s += cs[t]; q += cq[t];
                 const double cnt = (double)F * (t + 1), cm = s / cnt;
                 if (a.type == FSN_NORM_CUMULATIVE_LAPLACE) { sa[t] = (float)(1.0 / (cm + EPS)); sb[t] = 0.f; }
@@ -298,12 +301,13 @@ __global__ void __launch_bounds__(256) input_norm_kernel(NormLaunch a) {
                 }
             }
         }
+        for (int t = Tpe; t < Tp; ++t) { sa[t] = 0.f; sb[t] = 0.f; }      // past this sample's end: y = 0
     }
     __syncthreads();
     float* y = a.y + ((size_t)br * a.B + b) * F * Tp;
     for (int e = threadIdx.x; e < F * Tp; e += blockDim.x) {
         const int f = e / Tp, t = e % Tp;
-        const float v = (t < T) ? x[(size_t)f * T + t] : 0.f;
+        const float v = (t < Te) ? x[(size_t)f * T + t] : 0.f;
         y[e] = fmaf(v, sa[t], sb[t]);
     }
 }
@@ -404,10 +408,11 @@ __global__ void __launch_bounds__(256) sb_rowsum_kernel(SbPackLaunch a) {
     pdl_trigger();
     pdl_wait();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int F = a.F, Tp = a.Tp, nsrc = 1 + a.nfb;
+    const int F = a.F, nsrc = 1 + a.nfb;
     const int r = blockIdx.x * 8 + warp;                       // (b, which, f)
     if (r >= a.B * nsrc * F) return;
     const int b = r / (nsrc * F), which = (r / F) % nsrc, f = r % F;
+    const int Tp = a.tlen ? a.tlen[b] : a.Tp;
     const float* row = (which == 0) ? a.win + ((size_t)b * F + f) * a.Pw
                                     : ((which == 1) ? a.fb[0] : (which == 2) ? a.fb[1] : a.fb[2]) + ((size_t)b * F + f) * a.P;
     float acc = 0.f, acq = 0.f;
@@ -419,7 +424,7 @@ __global__ void __launch_bounds__(256) sb_rowsum_kernel(SbPackLaunch a) {
 __global__ void __launch_bounds__(256) sb_stats_kernel(SbPackLaunch a) {
     pdl_trigger();
     pdl_wait();
-    const int b = blockIdx.x, F = a.F, Tp = a.Tp, nsrc = 1 + a.nfb;
+    const int b = blockIdx.x, F = a.F, Tp = a.tlen ? a.tlen[b] : a.Tp, nsrc = 1 + a.nfb;
     __shared__ double red[16];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarp = blockDim.x >> 5;
     const float* S = a.rowsum + (size_t)b * nsrc * F * 2;        // [which][f][2]
@@ -491,6 +496,7 @@ template <class Store>
 __global__ void __launch_bounds__(256) sb_pack_kernel(SbPackLaunch a) {
     extern __shared__ float sm[];
     const int F = a.F, Tp = a.Tp, b = blockIdx.z, f0 = blockIdx.y * SBP_F, t0 = blockIdx.x * SBP_T;
+    const int Tpe = a.tlen ? a.tlen[b] : Tp;                       // frames t >= Tpe are past this sample's end: written as zero
     const int nw = 2 * a.Ns + 1, nf = 2 * a.Nf + 1, I = nw + a.nfb * nf;
     const int wrows = SBP_F + 2 * a.Ns, frows = SBP_F + 2 * a.Nf;
     float* wsm = sm;                                   // [wrows][SBP_T + 1]
@@ -501,14 +507,14 @@ __global__ void __launch_bounds__(256) sb_pack_kernel(SbPackLaunch a) {
     for (int e = threadIdx.x; e < wrows * SBP_T; e += blockDim.x) {
         const int rr = e / SBP_T, tt = e % SBP_T, t = t0 + tt;
         const int f = reflect_idx(min(f0 + rr - a.Ns, F - 1 + a.Ns), F);
-        wsm[rr * (SBP_T + 1) + tt] = (t < Tp) ? a.win[((size_t)b * F + f) * a.Pw + t] : 0.f;
+        wsm[rr * (SBP_T + 1) + tt] = (t < Tpe) ? a.win[((size_t)b * F + f) * a.Pw + t] : 0.f;
     }
     for (int q = 0; q < a.nfb; ++q) {
         const float* src = (q == 0) ? a.fb[0] : (q == 1) ? a.fb[1] : a.fb[2];
         for (int e = threadIdx.x; e < frows * SBP_T; e += blockDim.x) {
             const int rr = e / SBP_T, tt = e % SBP_T, t = t0 + tt;
             const int f = reflect_idx(min(f0 + rr - a.Nf, F - 1 + a.Nf), F);
-            fsm[(q * frows + rr) * (SBP_T + 1) + tt] = (t < Tp) ? src[((size_t)b * F + f) * a.P + t] : 0.f;
+            fsm[(q * frows + rr) * (SBP_T + 1) + tt] = (t < Tpe) ? src[((size_t)b * F + f) * a.P + t] : 0.f;
         }
     }
     __syncthreads();
@@ -520,7 +526,7 @@ __global__ void __launch_bounds__(256) sb_pack_kernel(SbPackLaunch a) {
         float v = 0.f;
         if (k < nw) v = wsm[(fr + k) * (SBP_T + 1) + tt];
         else if (k < I) { const int kk = k - nw, q = kk / nf, j = kk % nf; v = fsm[(q * frows + fr + j) * (SBP_T + 1) + tt]; }
-        return (k < I) ? (v - sub) * inv : 0.f;
+        return (k < I && t0 + tt < Tpe) ? (v - sub) * inv : 0.f;
     };
     float m = 0.f;
     for (int tt = 0; live && tt < SBP_T && t0 + tt < Tp; ++tt) {
@@ -542,6 +548,7 @@ __global__ void __launch_bounds__(128) sb_pack_cum_kernel(SbPackLaunch a) {
     const int row = blockIdx.x * 4 + warp, F = a.F, Tp = a.Tp;
     if (row >= a.B * F) return;
     const int b = row / F, f = row % F;
+    const int Tpe = a.tlen ? a.tlen[b] : Tp;                       // frames t >= Tpe are past this sample's end: written as zero
     const int nw = 2 * a.Ns + 1, nf = 2 * a.Nf + 1, I = nw + a.nfb * nf;
     const double EPS = 1.1920928955078125e-07;
     double cs = 0.0, cq = 0.0;                                   // running sums carried across 32-frame chunks
@@ -553,7 +560,7 @@ __global__ void __launch_bounds__(128) sb_pack_cum_kernel(SbPackLaunch a) {
 #pragma unroll
         for (int k = 0; k < 64; ++k) {
             float x = 0.f;
-            if (t < Tp && k < I) {
+            if (t < Tpe && k < I) {
                 if (k < nw) x = a.win[((size_t)b * F + reflect_idx(f + k - a.Ns, F)) * a.Pw + t];
                 else {
                     const int kk = k - nw, qq = kk / nf, j = kk % nf;
@@ -580,7 +587,7 @@ __global__ void __launch_bounds__(128) sb_pack_cum_kernel(SbPackLaunch a) {
             for (int c = 0; c < 8; ++c) {
                 float w[8];
 #pragma unroll
-                for (int i = 0; i < 8; ++i) w[i] = (c * 8 + i < I) ? fmaf(v[c * 8 + i], sc, sh) : 0.f;
+                for (int i = 0; i < 8; ++i) w[i] = (c * 8 + i < I && t < Tpe) ? fmaf(v[c * 8 + i], sc, sh) : 0.f;
                 mx = vmax8(mx, w);
                 Store::store(a, row, t, c * 8, w);
             }
@@ -698,33 +705,37 @@ __global__ void apply_cirm_kernel(const float* crm, const float2* noisy, float2*
     const float2 x = noisy[i];
     enh[i] = make_float2(m[0] * x.x - m[1] * x.y, m[1] * x.x + m[0] * x.y);
 }
-__global__ void apply_cirm_planar_kernel(const float* crm, const float* nreal, const float* nimag, float2* enh, int FT, size_t n) {
+__global__ void apply_cirm_planar_kernel(const float* crm, const float* nreal, const float* nimag, float2* enh, int T, int FT, size_t n,
+                                         const int* tlen, int la) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const size_t b = i / FT, e = i % FT;
+    if (tlen && (int)(e % T) >= tlen[b] - la) { enh[i] = make_float2(0.f, 0.f); return; }   // past the clip: the planes are not read
     const float m0 = decompress_cirm(crm[(b * 2 + 0) * FT + e]), m1 = decompress_cirm(crm[(b * 2 + 1) * FT + e]);
     const float xr = nreal[i], xi = nimag[i];
     enh[i] = make_float2(m0 * xr - m1 * xi, m1 * xr + m0 * xi);
 }
-void launch_apply_cirm_planar(const float* crm, const float* nreal, const float* nimag, float2* enh, int B, int F, int T, cudaStream_t s) {
+void launch_apply_cirm_planar(const float* crm, const float* nreal, const float* nimag, float2* enh, int B, int F, int T, const int* tlen,
+                              int la, cudaStream_t s) {
     const size_t n = (size_t)B * F * T;
-    apply_cirm_planar_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(crm, nreal, nimag, enh, F * T, n);
+    apply_cirm_planar_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(crm, nreal, nimag, enh, T, F * T, n, tlen, la);
 }
 void launch_apply_cirm(const float* crm, const float2* noisy, float2* enh, int B, int F, int T, cudaStream_t s) {
     const size_t n = (size_t)B * F * T;
     apply_cirm_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(crm, noisy, enh, F * T, n);
 }
 
-__global__ void pad_copy_kernel(const float* x, float* y, int rows, int T, int P) {
+__global__ void pad_copy_kernel(const float* x, float* y, int rows, int F, int T, int P, const int* tlen, int la) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (size_t)rows * P) return;
     int t = (int)(i % P);
     size_t r = i / P;
-    y[i] = (t < T) ? x[r * T + t] : 0.f;
+    const int Te = tlen ? tlen[r / F] - la : T;                   // frames of this sample's input
+    y[i] = (t < Te) ? x[r * T + t] : 0.f;
 }
-void launch_pad_copy(const float* x, float* y, int B, int F, int T, int P, cudaStream_t s) {
+void launch_pad_copy(const float* x, float* y, int B, int F, int T, int P, const int* tlen, int la, cudaStream_t s) {
     size_t n = (size_t)B * F * P;
-    pad_copy_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(x, y, B * F, T, P);
+    pad_copy_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(x, y, B * F, F, T, P, tlen, la);
 }
 
 __global__ void fb_pack_kernel(const float* x, __half* y, int B, int F, int Tp, int P, int rows_pad, int Ipad) {

@@ -185,8 +185,8 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
 
         // ---- epilogue on the accumulator fragment: rows rl[h] of the tile, column pairs n0 + 8 j + 2 (lane % 4) ----
         const int n0 = nt * NT, cq = 2 * (lane & 3);
-        int rib[2], z[2], tt[2];
-        bool valid[2];
+        int rib[2], z[2], tt[2], tz[2];
+        bool valid[2], live[2];
         size_t grow[2];
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -195,6 +195,8 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             z[h] = br * a.B + rib[h] / a.Tp;
             tt[h] = rib[h] % a.Tp;
             grow[h] = (size_t)br * a.rows_per_branch + rib[h];
+            tz[h] = (a.tlen && valid[h]) ? __ldg(a.tlen + z[h] / a.zdiv) : a.Tp;   // the frames of group z[h]
+            live[h] = valid[h] && tt[h] < tz[h];                                  // a row of the clip (not past its end)
         }
         // rows of this warp: rib0 .. rib0 + 15 of the branch, nvalid of them exist
         const int rib0 = mt * 128 + wg * 64 + wi * 16;
@@ -227,6 +229,7 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                     for (int e = 0; e < 2; ++e) {
                         float t = acc[4 * j + 2 * h + e] + (e ? b2.y : b2.x);
                         t = (t >= 0.f) ? t : slope * t;
+                        t = live[h] ? t : 0.f;                    // past the clip's end: zero, and nothing added to the statistics
                         ls[h] += t; lq[h] = fmaf(t, t, lq[h]);
                         y[e] = fminf(fmaxf(t * ysc[h], -65504.f), 65504.f);
                     }
@@ -242,7 +245,7 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             float mean[2] = {0.f, 0.f}, rstd[2] = {1.f, 1.f}, rowmax[2] = {0.f, 0.f};
 #pragma unroll
             for (int h = 0; h < 2; ++h)
-                if (valid[h]) gln_mean_rstd(a.stats_in, z[h], a.count_in, mean[h], rstd[h]);
+                if (valid[h]) gln_mean_rstd(a.stats_in, z[h], a.count_row * tz[h], mean[h], rstd[h]);
 #pragma unroll
             for (int j = 0; j < NT / 8; ++j) {
                 const int n = n0 + 8 * j + cq;
@@ -255,6 +258,7 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                     float2 o;
                     o.x = gln_res(x.x, acc[4 * j + 2 * h], mean[h], rstd[h], s12.x, b2.x);
                     o.y = gln_res(x.y, acc[4 * j + 2 * h + 1], mean[h], rstd[h], s12.y, b2.y);
+                    if (!live[h]) o = make_float2(0.f, 0.f);
                     rowmax[h] = fmaxf(rowmax[h], fmaxf(fabsf(o.x), fabsf(o.y)));
                     *reinterpret_cast<float2*>(a.Y + grow[h] * a.ldY + n) = o;
                     if (a.Xrelu) *reinterpret_cast<float2*>(a.Xrelu + grow[h] * a.ldY + n) = make_float2(fmaxf(o.x, 0.f), fmaxf(o.y, 0.f));
@@ -273,7 +277,7 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             for (int h = 0; h < 2; ++h) {
 #pragma unroll
                 for (int q = 0; q < 8; ++q) fc[h][q] = 0.f;
-                if (valid[h]) gln_mean_rstd(a.stats_in, z[h], a.count_in, mean[h], rstd[h]);
+                if (valid[h]) gln_mean_rstd(a.stats_in, z[h], a.count_row * tz[h], mean[h], rstd[h]);
             }
 #pragma unroll
             for (int j = 0; j < NT / 8; ++j) {
@@ -281,7 +285,7 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                 const float2 s12 = __ldg(reinterpret_cast<const float2*>(s1 + n)), b2 = __ldg(reinterpret_cast<const float2*>(bias + n));
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
-                    if (!valid[h]) continue;
+                    if (!live[h]) continue;
                     const float2 x = *reinterpret_cast<const float2*>(a.Xold + grow[h] * a.ldY + n);
                     const float o0 = fmaxf(gln_res(x.x, acc[4 * j + 2 * h], mean[h], rstd[h], s12.x, b2.x), 0.f);
                     const float o1 = fmaxf(gln_res(x.y, acc[4 * j + 2 * h + 1], mean[h], rstd[h], s12.y, b2.y), 0.f);
@@ -305,7 +309,11 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                 if (!valid[h] || (lane & 3) != 0 || tt[h] < a.la) continue;
                 const int ob = z[h] / a.F, of = z[h] % a.F;
                 const size_t ni = ((size_t)ob * a.F + of) * Tout + (tt[h] - a.la);
-                if (a.enh) {                                   // fused decompress_cIRM x noisy spectrum (inferencer.py:152-157), O = 2
+                if (!live[h]) {                                // past the clip's end: zeros, the noisy planes are not read
+                    if (a.enh) a.enh[ni] = make_float2(0.f, 0.f);
+                    else
+                        for (int q = 0; q < a.O; ++q) a.out[(((size_t)ob * a.O + q) * a.F + of) * Tout + (tt[h] - a.la)] = 0.f;
+                } else if (a.enh) {                            // fused decompress_cIRM x noisy spectrum (inferencer.py:152-157), O = 2
                     const float m0 = decompress_cirm(apply_act(fc[h][0] + __ldg(a.fc_b), a.act));
                     const float m1 = decompress_cirm(apply_act(fc[h][1] + __ldg(a.fc_b + 1), a.act));
                     const float nr = __ldg(a.nreal + ni), nim = __ldg(a.nimag + ni);
@@ -430,10 +438,11 @@ __global__ void __launch_bounds__(256) dwconv_tm_kernel(DwTmLaunch a) {
     // grid.x = Z * (C / 64): the group count (B * F sequences for the sub-band TCN) exceeds gridDim.z's 65535
     const int ncb = a.C / DW_CH, z = blockIdx.x / ncb, g = z / a.B, c0 = (blockIdx.x % ncb) * DW_CH;
     const int C = a.C, Tp = a.Tp, d = a.dilation;
+    const int Tz = a.tlen ? __ldg(a.tlen + z / a.zdiv) : Tp;          // frames of group z: taps past them read zero, rows past them are zero
     const int t0 = blockIdx.y * DW_TCH, t1 = min(t0 + DW_TCH, Tp);
-    const int lo = max(t0 - 2 * d, 0), hi = min(t1 + 2 * d, Tp);    // staged frames [lo, hi)
+    const int lo = max(t0 - 2 * d, 0), hi = min(t1 + 2 * d, Tz);    // staged frames [lo, hi)
     float mean, rstd;
-    gln_mean_rstd(a.stats_in, z, (double)C * (double)Tp, mean, rstd);
+    gln_mean_rstd(a.stats_in, z, (double)C * (double)Tz, mean, rstd);
     const float slope = __ldg(a.prelu[g]);
     const float unscale = 1.0f / fp16_store_scale(__ldg(a.amax + z));     // exact: a power of two
     const size_t base = (size_t)z * Tp * C + c0;
@@ -469,11 +478,12 @@ __global__ void __launch_bounds__(256) dwconv_tm_kernel(DwTmLaunch a) {
     float ls = 0.f, lq = 0.f;
     const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int t = t0 + tr; t < t1; t += 16) {
+        if (t >= Tz) { *reinterpret_cast<uint2*>(a.Y + base + (size_t)t * C + cq * 4) = make_uint2(0u, 0u); continue; }
         // taps (w0, w1, w2): non-causal (t-d, t, t+d); causal (t-2d, t-d, t) -- padding 2d + chomp, causal_conv.py:74-75,104-105
         const int tl = a.causal ? t - 2 * d : t - d, tm = a.causal ? t - d : t, tr2 = a.causal ? t : t + d;
         const float4 m = (tm >= 0) ? *reinterpret_cast<const float4*>(slab + (size_t)(tm - lo) * DW_CH + cq * 4) : zero;
         const float4 l = (tl >= 0) ? *reinterpret_cast<const float4*>(slab + (size_t)(tl - lo) * DW_CH + cq * 4) : zero;
-        const float4 r = (tr2 < Tp) ? *reinterpret_cast<const float4*>(slab + (size_t)(tr2 - lo) * DW_CH + cq * 4) : zero;
+        const float4 r = (tr2 < Tz) ? *reinterpret_cast<const float4*>(slab + (size_t)(tr2 - lo) * DW_CH + cq * 4) : zero;
         const float lv[4] = {l.x, l.y, l.z, l.w}, mv[4] = {m.x, m.y, m.z, m.w}, rv[4] = {r.x, r.y, r.z, r.w};
         float o[4];
 #pragma unroll

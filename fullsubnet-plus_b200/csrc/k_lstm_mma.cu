@@ -134,6 +134,8 @@ __global__ void __launch_bounds__(256, 1) lstm_mma_kernel(LstmMmaLaunch a) {
             for (int e = tid; e < R * a.O; e += blockDim.x) {
                 const int r = e / a.O, o = e % a.O, grow = row0 + r;
                 if (grow >= a.rows) continue;
+                const int b = grow / a.F, f = grow % a.F;
+                if (a.tlen && t >= a.tlen[b]) { a.out[(((size_t)b * a.O + o) * a.F + f) * (Tp - a.la) + (t - a.la)] = 0.f; continue; }   // past the clip's end
                 float acc = a.w.fc_b[o];
                 const __half2* hr = reinterpret_cast<const __half2*>(htop + (size_t)r * HS);
                 const float* w = fcw + (size_t)o * H;
@@ -145,7 +147,6 @@ __global__ void __launch_bounds__(256, 1) lstm_mma_kernel(LstmMmaLaunch a) {
                 if (a.act == FSN_ACT_RELU) acc = fmaxf(acc, 0.f);
                 else if (a.act == FSN_ACT_TANH) acc = tanhf(acc);
                 else if (a.act == FSN_ACT_RELU6) acc = fminf(fmaxf(acc, 0.f), 6.f);
-                const int b = grow / a.F, f = grow % a.F;
                 a.out[(((size_t)b * a.O + o) * a.F + f) * (Tp - a.la) + (t - a.la)] = acc;
             }
         }

@@ -251,6 +251,12 @@ __global__ void __cluster_dims__(R5_CL, 1, 1) __launch_bounds__(R5_THREADS, 1) l
                 for (int h = 0; h < 2; ++h) {
                     if (grow[h] >= a.rows) continue;
                     const int ob = grow[h] / a.F, of = grow[h] % a.F;
+                    if (a.tlen && t >= __ldg(a.tlen + ob)) {        // past the clip's end: zeros, the noisy planes are not read
+                        const size_t ni = ((size_t)ob * a.F + of) * Tout + (t - a.la);
+                        if (a.enh) a.enh[ni] = make_float2(0.f, 0.f);
+                        else { a.out[(((size_t)ob * 2 + 0) * a.F + of) * Tout + (t - a.la)] = 0.f; a.out[(((size_t)ob * 2 + 1) * a.F + of) * Tout + (t - a.la)] = 0.f; }
+                        continue;
+                    }
                     const float o0 = apply_act(fc0[h] + fcpart[((t & 1) * R5_ROWS + rl[h]) * 2] + __ldg(a.fc_b), a.act);
                     const float o1 = apply_act(fc1[h] + fcpart[((t & 1) * R5_ROWS + rl[h]) * 2 + 1] + __ldg(a.fc_b + 1), a.act);
                     const size_t ni = ((size_t)ob * a.F + of) * Tout + (t - a.la);

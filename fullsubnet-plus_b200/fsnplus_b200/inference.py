@@ -101,6 +101,42 @@ def enhance_batch(model, noisy, n_fft=512, hop_length=256, win_length=512, compl
     return istft(apply_cirm(crm, X), n_fft, hop_length, win_length, length=noisy.size(-1))
 
 
+@torch.no_grad()
+def enhance_ragged(model, clips, n_fft=512, hop_length=256, win_length=512, complex_inputs=True):
+    """Clips of different lengths in ONE model call: ``clips`` is a list of 1-D waveforms on one device; returns the list of
+    enhanced waveforms, each as long as its input and equal to what ``enhance_batch`` gives for that clip alone.
+
+    Each clip (or group of equal-length clips) gets its own centred STFT -- zero-padding the waveform instead would change its last
+    frames, whose windows reach past its end.  The spectra are scattered into a zero [B, F, T_max] batch and the model runs once with
+    ``frames`` = every clip's own frame count (the forward masks each clip at its own end).  The iSTFT runs per clip over the clip's
+    own frames only: a batched iSTFT over the padded spectra would put the padded frames into the window envelope
+    of the last hop."""
+    if len(clips) == 0:
+        return []
+    lengths = [int(c.numel()) for c in clips]
+    groups = {}
+    for i, n in enumerate(lengths):
+        groups.setdefault(n, []).append(i)
+    specs, frames = {}, [0] * len(clips)
+    for n, idx in groups.items():
+        specs[n] = stft(torch.stack([clips[i].reshape(-1) for i in idx]), n_fft, hop_length, win_length)
+        for i in idx:
+            frames[i] = specs[n].size(-1)
+    B, F, T = len(clips), specs[lengths[0]].size(1), max(frames)
+    X = torch.zeros((B, F, T), dtype=specs[lengths[0]].dtype, device=clips[0].device)
+    for n, idx in groups.items():
+        X[idx, :, :specs[n].size(-1)] = specs[n]
+    mag = X.abs().unsqueeze(1)
+    if hasattr(model, "enhance_spectrum") and X.is_cuda:
+        enh = model.enhance_spectrum(mag, X.real.unsqueeze(1).contiguous(), X.imag.unsqueeze(1).contiguous(), frames=frames)
+    else:
+        crm = (model(mag, X.real.unsqueeze(1).contiguous(), X.imag.unsqueeze(1).contiguous(), frames=frames) if complex_inputs
+               else model(mag, frames=frames))
+        enh = apply_cirm(crm, X)
+    # one iSTFT per clip: a batched one need not round like the per-clip call enhance_batch makes
+    return [istft(enh[b:b + 1, :, :frames[b]].contiguous(), n_fft, hop_length, win_length, length=lengths[b])[0] for b in range(B)]
+
+
 def shard_range(n_items, rank, world_size):
     """Contiguous shard [lo, hi) of rank; sizes differ by at most one (ragged batches are allowed)."""
     base, rem = divmod(n_items, world_size)

@@ -186,16 +186,31 @@ class _B200Model(nn.Module):
             pass
 
     # -- forward -------------------------------------------------------------------------------
-    def enhance_spectrum(self, noisy_mag, noisy_real, noisy_imag, pipelined=False, out=None, hold=True):
+    def enhance_spectrum(self, noisy_mag, noisy_real, noisy_imag, pipelined=False, out=None, hold=True, frames=None):
         """Model forward + decompress_cIRM + complex multiply with the noisy spectrum in ONE call (C ABI: fsn_model_forward_enhance /
         fsn_model_submit_enhance; reference inferencer.py:149-157): [B, 1, F, T] x3 -> enhanced spectrum complex64 [B, F, T], the
         argument of the inferencer's iSTFT.  The cIRM never goes to memory (fused into the sub-band LSTM's epilogue).
-        ``pipelined=True``: like ``submit()`` -- valid after ``wait()`` / ``wait_lane()``."""
-        return self._run(noisy_mag, noisy_real, noisy_imag, enhance=True, pipelined=pipelined, out=out, hold=hold)
+        ``pipelined=True``: like ``submit()`` -- valid after ``wait()`` / ``wait_lane()``.  ``frames``: as in ``forward()``."""
+        return self._run(noisy_mag, noisy_real, noisy_imag, enhance=True, pipelined=pipelined, out=out, hold=hold, frames=frames)
 
-    def _run(self, mag, real, imag, enhance=False, pipelined=False, out=None, hold=True):
+    @staticmethod
+    def _frames_arg(frames, B):
+        """``frames`` (a sequence of ints or a CPU integer tensor of length B) as a C int32 array."""
+        if isinstance(frames, torch.Tensor):
+            if frames.is_cuda or frames.is_floating_point() or frames.is_complex() or frames.dim() != 1:
+                raise ValueError("frames must be a 1-D CPU integer tensor or a sequence of ints")
+            frames = frames.tolist()
+        frames = [int(n) for n in frames]
+        if len(frames) != B:
+            raise ValueError(f"frames has {len(frames)} entries for a batch of {B}")
+        return (C.c_int32 * B)(*frames)
+
+    def _run(self, mag, real, imag, enhance=False, pipelined=False, out=None, hold=True, frames=None):
         assert mag.dim() == 4                                            # fullsubnet_plus.py:136
         B, Cn, F, T = mag.shape
+        if frames is not None and pipelined:
+            raise ValueError("frames (ragged batches) is not supported with pipelined=True / submit()")
+        hframes = self._frames_arg(frames, B) if frames is not None else None
         assert Cn == 1, f"{self.__class__.__name__} takes the mag feature as inputs."      # :141
         if self.training:
             raise NotImplementedError("fsnplus_b200 implements the inference (eval) forward only; call .eval()")
@@ -211,6 +226,10 @@ class _B200Model(nn.Module):
                        torch.empty((B, self._cfg.output_size, F, T), dtype=torch.float32, device=mag.device))
             ptr = lambda x: C.c_void_p(x.data_ptr()) if x is not None else C.c_void_p()
             stream = C.c_void_p(torch.cuda.current_stream(mag.device).cuda_stream)
+            if hframes is not None:
+                fn = lib.fsn_model_forward_enhance_ragged if enhance else lib.fsn_model_forward_ragged
+                _lib.check(fn(self._handle, ptr(ins[0]), ptr(ins[1]), ptr(ins[2]), B, T, hframes, ptr(out), stream))
+                return out
             fn = {(False, False): lib.fsn_model_forward, (True, False): lib.fsn_model_forward_enhance,
                   (False, True): lib.fsn_model_submit, (True, True): lib.fsn_model_submit_enhance}[(enhance, pipelined)]
             _lib.check(fn(self._handle, ptr(ins[0]), ptr(ins[1]), ptr(ins[2]), B, T, ptr(out), stream))
@@ -367,13 +386,16 @@ class FullSubNet_Plus(_B200Model):
         if weight_init:
             self.apply(_reference_weight_init)
 
-    def forward(self, noisy_mag, noisy_real, noisy_imag):
-        """[B, 1, F, T] x3 -> [B, 2, F, T] (reference fullsubnet_plus.py:122-209, eval semantics per sample)."""
+    def forward(self, noisy_mag, noisy_real, noisy_imag, *, frames=None):
+        """[B, 1, F, T] x3 -> [B, 2, F, T] (reference fullsubnet_plus.py:122-209, eval semantics per sample).
+        ``frames`` (additive, keyword-only): the frame count of every clip of a ragged batch, 1 <= frames[b] <= T.  Clip b is then
+        its first frames[b] frames; its output equals that clip's own forward there and is zero after (C ABI:
+        fsn_model_forward_ragged)."""
         if not self._subband_runs:
             raise RuntimeError(f"subband_num={self.subband_num}: the attention was built for {self.num_channels} channels but the "
                                "real/imag branches have num_freqs channels (the reference forward raises here too, "
                                "fullsubnet_plus.py:157-163); only channel_attention_model='ECA' runs with subband_num > 1")
-        return self._run(noisy_mag, noisy_real, noisy_imag)
+        return self._run(noisy_mag, noisy_real, noisy_imag, frames=frames)
 
 
 class Model(_B200Model):
@@ -401,6 +423,7 @@ class Model(_B200Model):
         if weight_init:
             self.apply(_reference_weight_init)
 
-    def forward(self, noisy_mag):
-        """[B, 1, F, T] -> [B, 2, F, T] (reference fullsubnet.py:68-118, eval semantics per sample)."""
-        return self._run(noisy_mag, None, None)
+    def forward(self, noisy_mag, *, frames=None):
+        """[B, 1, F, T] -> [B, 2, F, T] (reference fullsubnet.py:68-118, eval semantics per sample).  ``frames``: as in
+        FullSubNet_Plus.forward."""
+        return self._run(noisy_mag, None, None, frames=frames)

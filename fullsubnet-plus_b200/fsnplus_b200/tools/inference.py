@@ -13,7 +13,8 @@ strictly, every audio file under the dataset directories is enhanced with the ``
 What differs, by design: clips are enhanced in BATCHES.  The reference is hard-wired to batch 1
 (base_inferencer.py:65-69); here files are grouped by exact sample count (the forward is per-utterance -- offline norm,
 time pooling in the attention -- so padding a clip would change its result) and each group runs ``--batch_size`` clips per
-launch.  ``librosa`` / ``soundfile`` are not dependencies: WAV (PCM 8/16/24/32, float32/64) is read with scipy and written
+launch.  With ``--ragged`` files are instead sorted by sample count and cut into batches of ``--batch_size`` clips of different
+lengths, each enhanced by one ragged model call (every clip is masked at its own end, so its result is unchanged).  ``librosa`` / ``soundfile`` are not dependencies: WAV (PCM 8/16/24/32, float32/64) is read with scipy and written
 with the standard library; other containers are rejected with a clear error.
 """
 import argparse
@@ -126,6 +127,13 @@ def bucket_by_length(lengths, batch_size):
     return batches
 
 
+def batch_by_sorted_length(lengths, batch_size):
+    """Indices sorted by length (stable: ties keep the directory order), cut into runs of at most batch_size: neighbouring
+    clips have similar lengths, which keeps the padding of a ragged batch small."""
+    order = sorted(range(len(lengths)), key=lambda i: int(lengths[i]))
+    return [order[i:i + batch_size] for i in range(0, len(order), batch_size)]
+
+
 def build_model(model_config, checkpoint_path, device, trust_checkpoint=False):
     """base_inferencer.py:97-110 (_load_model).  The checkpoint is read with ``weights_only=True`` (tensors and plain containers
     only: the reference's ``{"model": state_dict, "epoch": int}`` loads); ``trust_checkpoint=True`` opts into full unpickling."""
@@ -144,10 +152,12 @@ def _rank_world():
 
 
 @torch.no_grad()
-def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=print, model_and_epoch=None, trust_checkpoint=False, streams=4):
+def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=print, model_and_epoch=None, trust_checkpoint=False, streams=4,
+        ragged=False):
     """Enhance every file of config["dataset"]["args"]["dataset_dir_list"].  Under torchrun each rank takes every
     world-size-th batch (files are independent: no collective).  Returns {name: path} of the files this rank wrote.
-    ``model_and_epoch`` (tests of the host logic) replaces the checkpoint load with a ready ``(callable, epoch)``."""
+    ``model_and_epoch`` (tests of the host logic) replaces the checkpoint load with a ready ``(callable, epoch)``.
+    ``ragged=True``: batches of clips of different lengths (length-sorted, ``batch_size`` clips each) through ``enhance_ragged``."""
     rank, world, local_rank = _rank_world()
     if device is None:
         device = f"cuda:{local_rank}"
@@ -165,7 +175,8 @@ def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=pri
 
     # bucket on the lengths from the WAV headers; a rank decodes only the files of ITS batches, one batch at a time (host memory
     # and start-up time scale with the batch, not with the dataset -- the reference streams one clip at a time)
-    batches = bucket_by_length([wav_length(p, ds_sr) for p in files], batch_size)
+    lengths = [wav_length(p, ds_sr) for p in files]
+    batches = batch_by_sorted_length(lengths, batch_size) if ragged else bucket_by_length(lengths, batch_size)
     mine = [(bi, idx) for bi, idx in enumerate(batches) if bi % world == rank]
     # Ragged real recordings make many small batches (a lone clip fills a small fraction of the SMs): up to `streams`
     # batches are in flight at once, each on its own CUDA stream and its own model replica (own C handle and workspaces).
@@ -180,7 +191,7 @@ def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=pri
         bi, idx, host, ev, n_samples = item
         if ev is not None:
             ev.synchronize()
-        enhanced = host.numpy()
+        enhanced = host.numpy() if torch.is_tensor(host) else [h.numpy() for h in host]
         log(f"[rank {rank}] batch {bi}: {len(idx)} x {n_samples} samples done")
         for j, i in enumerate(idx):
             y = enhanced[j]
@@ -191,11 +202,29 @@ def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=pri
             written[files[i].stem] = out
 
     for n, (bi, idx) in enumerate(mine):
-        noisy = torch.from_numpy(np.stack([read_wav(files[i], ds_sr) for i in idx]))
-        audio_s += len(idx) * noisy.size(1) / sr
         k = n % nstream
         if len(inflight) >= nstream:
             finish(inflight.pop(0))                                        # the batch that used this stream / replica last
+        if ragged:
+            clips = [torch.from_numpy(read_wav(files[i], ds_sr)) for i in idx]
+            audio_s += sum(c.numel() for c in clips) / sr
+            desc = f"{min(c.numel() for c in clips)}..{max(c.numel() for c in clips)}"
+            if on_gpu:
+                with torch.cuda.stream(cuda_streams[k]):
+                    enh = H.enhance_ragged(models[k], [c.pin_memory().to(device, non_blocking=True) for c in clips], n_fft, hop, win,
+                                           complex_inputs=INFERENCE_TYPES[itype])
+                    host = [torch.empty(tuple(e.shape), dtype=e.dtype).pin_memory() for e in enh]
+                    for h, e in zip(host, enh):
+                        h.copy_(e, non_blocking=True)
+                    ev = torch.cuda.Event()
+                    ev.record(cuda_streams[k])
+                inflight.append((bi, idx, host, ev, desc))
+            else:
+                enh = H.enhance_ragged(models[k], clips, n_fft, hop, win, complex_inputs=INFERENCE_TYPES[itype])
+                inflight.append((bi, idx, [e.cpu() for e in enh], None, desc))
+            continue
+        noisy = torch.from_numpy(np.stack([read_wav(files[i], ds_sr) for i in idx]))
+        audio_s += len(idx) * noisy.size(1) / sr
         if on_gpu:
             with torch.cuda.stream(cuda_streams[k]):
                 dev_noisy = noisy.pin_memory().to(device, non_blocking=True)
@@ -224,12 +253,15 @@ def main(argv=None):
     parser.add_argument("--batch_size", type=int, default=64, help="clips of equal length per launch (additive)")
     parser.add_argument("--trust_checkpoint", action="store_true", help="unpickle arbitrary objects from the checkpoint (default: tensors only)")
     parser.add_argument("--streams", type=int, default=4, help="batches in flight at once, each on its own CUDA stream and model replica (additive)")
+    parser.add_argument("--ragged", action="store_true",
+                        help="batch clips of different lengths (sorted by length, --batch_size per batch) in one ragged model call (additive)")
     args = parser.parse_args(argv)
     configuration = load_toml(args.configuration)
     if len(args.dataset_dir_list) > 0:
         print(f"use specified dataset_dir_list: {args.dataset_dir_list}, instead of in config")
         configuration["dataset"]["args"]["dataset_dir_list"] = args.dataset_dir_list
-    run(configuration, args.model_checkpoint_path, args.output_dir, batch_size=args.batch_size, trust_checkpoint=args.trust_checkpoint, streams=args.streams)
+    run(configuration, args.model_checkpoint_path, args.output_dir, batch_size=args.batch_size, trust_checkpoint=args.trust_checkpoint, streams=args.streams,
+        ragged=args.ragged)
 
 
 if __name__ == "__main__":

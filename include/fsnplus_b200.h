@@ -123,6 +123,18 @@ int fsn_model_forward(fsn_model* m, const float* d_mag, const float* d_real, con
  * the argument of the inferencer's iSTFT. */
 int fsn_model_forward_enhance(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
                               float* d_enh, void* stream);
+/* Ragged batches: fsn_model_forward / fsn_model_forward_enhance for clips of different lengths stored in one [B, 1, F, T] batch.
+ * h_frames: HOST array of B frame counts, 1 <= h_frames[b] <= T (with the TSSE attention also h_frames[b] + look_ahead >= every
+ * kersize), else FSN_EINVAL naming the sample.  Sample b is its first h_frames[b] frames followed by the look_ahead zero frames of
+ * the reference's right padding: every time reduction, norm and convolution tap of the forward stops at h_frames[b] + look_ahead.
+ * Inputs at t >= h_frames[b] are never read (they may hold anything, NaN included); outputs there are exact zeros, and
+ * out[b, ..., :h_frames[b]] equals the forward of that clip alone up to floating-point reordering.  h_frames may be reused as soon as
+ * the call returns (the counts go to the device through pinned staging slots; no stream is synchronised).  h_frames == NULL, or
+ * every count equal to T, runs the unragged forward unchanged. */
+int fsn_model_forward_ragged(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
+                             const int32_t* h_frames, float* d_out, void* stream);
+int fsn_model_forward_enhance_ragged(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
+                                     const int32_t* h_frames, float* d_enh, void* stream);
 /* Same call with HOST buffers (pinned or pageable): H2D copies, the forward and the D2H copy of the
  * mask are all enqueued on `stream` and the call returns after the result is in h_out. */
 int fsn_model_forward_host(fsn_model* m, const float* h_mag, const float* h_real, const float* h_imag, int32_t B, int32_t T,

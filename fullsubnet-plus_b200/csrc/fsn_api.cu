@@ -88,11 +88,12 @@ struct fsn_model {
     // layer-wise wgmma path (k_lstm_tc5r.cu): per-layer recurrent streams, permuted input-projection matrices, biases
     bool tc5r_ok = false;
     DevBuf r_stream[4], r_wih[4], r_bias[4], r_gin, r_hseq;    // r_wih: input-projection matrices of the layers > 0
+    DevBuf r_hstate, sb_cum;                           // windowed forwards: per-layer h at the window's end, the packer's cumulative sums
     // Front-end workspaces (everything the full-band stage writes and the sub-band LSTM reads), grow-only, keyed by the last
     // (B, T).  TWO lanes: the pipelined entry points (fsn_model_submit / fsn_model_forward_host_async) run the front end of
     // batch i+1 in lane (i+1)&1 on the front stream while the sub-band LSTM of batch i still reads lane i&1 on the LSTM stream.
     struct Lane {
-        int wsB = 0, wsT = 0;
+        int wsB = 0, wsT = 0, wsTw = 0;                // wsTw: sub-band window of the last geometry (0: whole clip)
         DevBuf fbin, fbout, mu, ximg, magpad, fbx, hseq;
         DevBuf x0, xr;                                 // time-major fb input / relu'd last residual
         TcnScratch tcn;                                // the full-band TCN's blocks (written on the front stream)
@@ -133,6 +134,8 @@ struct fsn_model {
     bool env_front_overlap = false;
     int env_pdl = -1;                                  // FSN_PDL: 0 / 1 / -1 (auto: small batches only)
     double ws_cap_bytes = 24e9;                        // FSN_WS_CAP_GB: larger batches are run as sub-batches (plain forward entry points)
+    int env_sb_window = 0;                             // FSN_SB_WINDOW: force a sub-band time window of this many frames (multiple of 32)
+    int plan_Bs = 0, plan_Tw = 0;                      // plan of the last plain forward (fsn_plan_forward): sub-batch, window (0: whole clip)
     bool env_no_ws = false;
     // pipelined execution: front-end stream, LSTM stream (higher priority), copy-in / copy-out streams, per-slot events
     cudaStream_t s_front = nullptr, s_lstm = nullptr, s_in = nullptr, s_out = nullptr;
@@ -439,10 +442,18 @@ extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
     }
     const int isb = (2 * c.sb_num_neighbors + 1) + (c.model_kind == FSN_KIND_PLUS ? 3 : 1) * (2 * c.fb_num_neighbors + 1);
     if (isb > 64) return fail(FSN_EINVAL, "sub-band input size %d > 64 not supported", isb);
+    int sb_window = 0;
+    if (const char* e = getenv("FSN_SB_WINDOW"); e && *e) {
+        char* end = nullptr;
+        const long w = strtol(e, &end, 10);
+        if (*end || w < 32 || w % 32 || w > (1L << 30)) return fail(FSN_EINVAL, "FSN_SB_WINDOW=%s: the window must be a positive multiple of 32 frames", e);
+        sb_window = (int)w;
+    }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(FSN_ECUDA, "no CUDA device: fsnplus_b200 has no CPU fallback");
     fsn_model* m = new fsn_model();
     m->cfg = c;
+    m->env_sb_window = sb_window;
     { const char* e = getenv("FSN_LSTM_IMPL"); if (e && *e) m->env_impl = atoi(e); }
     { const char* e = getenv("FSN_NO_WS"); m->env_no_ws = e && atoi(e) != 0; }
     { const char* e = getenv("FSN_FRONT_OVERLAP"); m->env_front_overlap = e && atoi(e) != 0; }
@@ -471,7 +482,7 @@ extern "C" void fsn_model_destroy(fsn_model* m) {
         if (ln.ev_lstm) cudaEventDestroy(ln.ev_lstm);
     }
     for (int i = 0; i < 4; ++i) { m->r_stream[i].release(); m->r_wih[i].release(); m->r_bias[i].release(); }
-    m->r_gin.release(); m->r_hseq.release();
+    m->r_gin.release(); m->r_hseq.release(); m->r_hstate.release(); m->sb_cum.release();
     if (m->s_front) { cudaStreamDestroy(m->s_front); cudaStreamDestroy(m->s_lstm); cudaEventDestroy(m->ev_in); }
     if (m->ev_plain) cudaEventDestroy(m->ev_plain);
     if (m->s_in) { cudaStreamDestroy(m->s_in); cudaStreamDestroy(m->s_out); for (int i = 0; i < 2; ++i) { cudaEventDestroy(m->ev_h2d[i]); cudaEventDestroy(m->ev_d2h[i]); cudaEventDestroy(m->ev_done[i]); } }
@@ -615,48 +626,58 @@ static int grow_tcn_scratch(TcnScratch& sc, const TcnWeights& w, long long rows,
     return FSN_OK;
 }
 
-static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, cudaStream_t s, cudaStream_t sl) {
-    const fsn_config& c = m->cfg;
-    const int F = c.num_freqs, Tp = T + c.look_ahead, Pp = (Tp + 3) & ~3;
-    const int nbr = (c.model_kind == FSN_KIND_PLUS) ? 3 : 1;
-    const size_t act = (size_t)nbr * B * F * Pp * 4;
-    const int rows = B * F, ntiles = ((rows + 127) / 128 + 1) / 2 * 2;      // whole pairs of 128-row tiles (clusters of k_lstm_tc5r.cu)
-    const bool regeo = (ln.wsB != B || ln.wsT != T);
-    int e = 0;
-    e |= ln.fbin.ensure(act, true, s);
-    e |= ln.fbout.ensure(act, true, s);
-    e |= ln.mu.ensure((size_t)B * 4, true, s);
-    e |= ln.sigma.ensure((size_t)B * 4, true, s);
-    e |= ln.tsse_scale.ensure((size_t)nbr * B * F * 4 * (1 + tsse_row_floats()), true, s);      // per-row scale | row statistics
-    e |= ln.sb_rowsum.ensure((size_t)B * 4 * F * 2 * 4, true, s);
-    if (c.norm_type != FSN_NORM_OFFLINE_LAPLACE) e |= ln.xn.ensure((size_t)nbr * B * F * Tp * 4, true, s);
-    if (c.sb_tcn) {
-        // sub-band TCN: the lane's packed input (+ block 0's stream maxima), the shared scratch of the blocks (serialised on the sub-band
-        // stream like the LSTM scratch); every buffer is fully written before it is read (the pad columns by the packer / the epilogue)
-        const long long srows = (long long)B * F * Tp;
-        if (srows + 128 > 0x7fffffffLL) return fail(FSN_EINVAL, "B * num_freqs * (T + look_ahead) = %lld rows exceeds the sub-band TCN's 2^31 limit", srows);
-        if (regeo) ln.sbx.release();
-        e |= ln.sbx.ensure((size_t)srows * 64 * 4 + (size_t)B * F * 4, false, s);
-        if (e) return fail(FSN_ECUDA, "workspace allocation failed for B=%d T=%d", B, T);
-        if (regeo && make_tmap_f32_2d(ln.mapSbx, ln.sbx.p, srows, 64, 128)) return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the sub-band input");
-        int rc = grow_tcn_scratch(m->sb_scratch, m->tcn_sb, srows, (size_t)B * F, false, sl);
-        if (rc) return rc;
-    } else {
-        // images are re-zeroed whenever the geometry changes (rows beyond B*F and k >= I must stay zero)
-        const size_t img_bytes = (size_t)ntiles * Tp * 16384;
-        if (regeo) { ln.ximg.release(); }
-        e |= ln.ximg.ensure(img_bytes, true, s);
+// lstm_impl = auto / tcgen05 on a geometry the layer-wise kernels take, from the configuration alone (env_impl: FSN_LSTM_IMPL or 0)
+static bool config_layerwise(const fsn_config& c, int env_impl) {
+    const int isb = (2 * c.sb_num_neighbors + 1) + (c.model_kind == FSN_KIND_PLUS ? 3 : 1) * (2 * c.fb_num_neighbors + 1);
+    const bool ok = !c.sb_tcn && lstm_tc5r_supported(c.sb_hidden, c.output_size) && isb <= 64;
+    const int impl = env_impl ? env_impl : c.lstm_impl;
+    return ok && (impl == FSN_LSTM_AUTO || impl == FSN_LSTM_TCGEN05);
+}
+
+// Bytes of every forward workspace buffer ensure_ws requests for a batch of B clips of T frames, the sub-band images and the layer-wise
+// path's Gin / layer output sized by the window Tw (0: the whole clip).  ensure_ws allocates exactly these sizes, so the planner's count
+// (fsn_plan_forward) is what a forward asks for.
+struct WsSizes {
+    size_t act = 0, mu = 0, tsse = 0, rowsum = 0, xn = 0;      // lane: fbin / fbout, mu / sigma, TSSE scale + row statistics, row sums, norms
+    size_t sbx = 0, ximg = 0;                                   // lane: sub-band TCN input, or the sub-band images
+    size_t x0 = 0, tcn_x = 0, tcn_y = 0, tcn_stats = 0;         // lane, FullSubNet+: x0 / xr, the TCN's two fp32 streams, two fp16 hidden, statistics
+    size_t magpad = 0, fbx = 0, fbhseq = 0;                     // lane, fullsubnet.Model
+    size_t cstate = 0, gin = 0, hseq = 0, hstate = 0, cum = 0;  // LSTM-side scratch
+    size_t sb_x = 0, sb_y = 0, sb_stats = 0;                    // sub-band TCN scratch
+    size_t tlen = 0, wsh = 0;                                   // ragged extents; fullsubnet.Model's weight-stationary h exchange + barrier
+    size_t total() const {
+        return 2 * act + 2 * mu + tsse + rowsum + xn + sbx + ximg + 2 * x0 + 2 * tcn_x + 2 * tcn_y + tcn_stats + magpad + fbx + fbhseq + cstate +
+               gin + hseq + hstate + cum + 2 * sb_x + 2 * sb_y + sb_stats + tlen + wsh;
     }
-    // LSTM-side scratch: shared by both lanes (LSTM launches are serialised on the LSTM stream)
+};
+static WsSizes ws_sizes(const fsn_config& c, bool layerwise, int B, int T, int Tw) {
+    WsSizes z;
+    const int F = c.num_freqs, Tp = T + c.look_ahead, Pp = (Tp + 3) & ~3, Ts = Tw ? Tw : Tp;
+    const int nbr = (c.model_kind == FSN_KIND_PLUS) ? 3 : 1;
+    const size_t rows = (size_t)B * F, ntiles = ((rows + 127) / 128 + 1) / 2 * 2;   // whole pairs of 128-row tiles (clusters of k_lstm_tc5r.cu)
+    z.act = (size_t)nbr * B * F * Pp * 4;
+    z.mu = (size_t)B * 4;
+    z.tsse = (size_t)nbr * B * F * 4 * (1 + tsse_row_floats());
+    z.rowsum = (size_t)B * 4 * F * 2 * 4;
+    z.tlen = (size_t)3 * B * sizeof(int32_t);                  // counted whether the forward is ragged or not
+    if (c.norm_type != FSN_NORM_OFFLINE_LAPLACE) z.xn = (size_t)nbr * B * F * Tp * 4;
+    if (c.sb_tcn) {
+        const size_t srows = rows * Tp;
+        z.sbx = srows * 64 * 4 + rows * 4;
+        z.sb_x = srows * 64 * 4; z.sb_y = srows * 512 * sizeof(__half); z.sb_stats = tcn_stats_bytes(rows);
+    } else {
+        z.ximg = ntiles * Ts * 16384;
+    }
     int ra = 0;
-    size_t cs = c.sb_tcn ? 0 : lstm_mma_cstate_bytes(c.num_layers, rows, c.sb_hidden, &ra);
-    size_t cs5 = 0;
-    if (use_layerwise(m)) {
-        const size_t M = (size_t)ntiles * Tp * 128;
-        cs5 = lstm_tc5r_cstate_bytes(ntiles, c.sb_hidden);
-        if (c.num_layers > 1) {                                          // Gin and the layer output of the deeper layers
-            e |= m->r_gin.ensure(M * 4 * c.sb_hidden * 2, false, sl);
-            e |= m->r_hseq.ensure(M * c.sb_hidden * 2, false, sl);
+    size_t cs = c.sb_tcn ? 0 : lstm_mma_cstate_bytes(c.num_layers, (int)rows, c.sb_hidden, &ra), cs5 = 0;
+    if (layerwise) {
+        const size_t M = ntiles * Ts * 128;
+        cs5 = lstm_tc5r_cstate_bytes((int)ntiles, c.sb_hidden);
+        if (c.num_layers > 1) { z.gin = M * 4 * c.sb_hidden * 2; z.hseq = M * c.sb_hidden * 2; }
+        if (Tw) {                                                       // windowed: c / h of every layer carried to the next window
+            cs5 *= c.num_layers;
+            z.hstate = (size_t)c.num_layers * ntiles * 128 * c.sb_hidden * 2;
+            if (c.norm_type == FSN_NORM_CUMULATIVE_LAPLACE || c.norm_type == FSN_NORM_CUMULATIVE_LAYER) z.cum = rows * 2 * sizeof(double);
         }
     }
     if (c.model_kind == FSN_KIND_FSN) {
@@ -664,68 +685,166 @@ static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, cudaStream
         const size_t csf = lstm_mma_cstate_bytes(c.num_layers, B, c.fb_hidden, &ra2);
         if (csf > cs) cs = csf;
     }
-    if (cs || cs5) e |= m->cstate.ensure(cs > cs5 ? cs : cs5, true, sl);
+    z.cstate = cs > cs5 ? cs : cs5;
+    if (c.model_kind == FSN_KIND_PLUS) {
+        const size_t trows = (size_t)3 * B * Tp, Cp = (size_t)(F + 31) / 32 * 32;   // pack_tcn5's Cp
+        z.x0 = trows * Cp * 4;
+        z.tcn_x = trows * Cp * 4; z.tcn_y = trows * 512 * sizeof(__half); z.tcn_stats = tcn_stats_bytes((size_t)3 * B);
+    } else {
+        const size_t Ipad = (F + 15) / 16 * 16, rows_pad = (B + 63) / 64 * 64;
+        z.magpad = (size_t)B * F * Pp * 4;
+        z.fbx = (size_t)Tp * rows_pad * Ipad * 2;
+        z.fbhseq = (size_t)B * c.fb_hidden * Pp * 4;
+        z.wsh = (size_t)c.num_layers * 2 * 64 * c.fb_hidden * 2 + 64;   // counted whether that kernel runs or not
+    }
+    return z;
+}
+
+// Length limits of one forward (B clips of T frames), from the 32-bit quantities of the kernels on every path: the depth-wise TCN
+// convolution's grid covers T' in blocks of 256 frames along gridDim.y (<= 65535); the cIRM passes index one clip's F x T' plane with
+// an int; the full-band TCN GEMMs address their 3 B T' time-major rows (+ one 128-row tile) with int row indices and int32 tensor-map
+// coordinates.  Every element offset beyond these is 64-bit.  The sub-band TCN's B F T' row limit is checked with its workspace.
+static const long long FSN_MAX_TP = 65535LL * 256;
+static long long max_clips_for_rows(const fsn_config& c, int T) {
+    return c.model_kind == FSN_KIND_PLUS ? (0x7fffffffLL - 128) / (3LL * (T + c.look_ahead)) : 0x7fffffffLL;
+}
+static int check_length(const fsn_config& c, int B, int T) {
+    const long long Tp = (long long)T + c.look_ahead;
+    if (Tp > FSN_MAX_TP) return fail(FSN_EINVAL, "T + look_ahead = %lld frames exceeds the limit of %lld (65535 x 256, the TCN convolution grid)", Tp, FSN_MAX_TP);
+    if ((long long)c.num_freqs * Tp > 0x7fffffffLL)
+        return fail(FSN_EINVAL, "num_freqs x (T + look_ahead) = %lld exceeds 2^31 - 1, the per-clip plane index limit", (long long)c.num_freqs * Tp);
+    if (B > max_clips_for_rows(c, T))
+        return fail(FSN_EINVAL, "3 x B x (T + look_ahead) = %lld rows exceeds the full-band TCN's 2^31 row limit", 3LL * B * Tp);
+    return FSN_OK;
+}
+
+static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, int Tw, cudaStream_t s, cudaStream_t sl) {
+    const fsn_config& c = m->cfg;
+    const int F = c.num_freqs, Tp = T + c.look_ahead;
+    const WsSizes z = ws_sizes(c, use_layerwise(m), B, T, Tw);
+    const bool regeo = (ln.wsB != B || ln.wsT != T || ln.wsTw != Tw);
+    if (Tw) {
+        // A windowed forward exists to bound the workspace: first give back what earlier, longer or unwindowed forwards grew beyond this
+        // one's need (the grow-only buffers of both lanes and the sub-band scratch), so the model then holds at most the plan's bytes.
+        // The buffers a new geometry releases anyway (images, x0 / xr, the TCN scratch) are left to that rule.
+        auto fit = [](DevBuf& b, size_t need) { if (b.bytes > need) b.release(); };
+        fit(ln.fbin, z.act); fit(ln.fbout, z.act); fit(ln.mu, z.mu); fit(ln.sigma, z.mu); fit(ln.tsse_scale, z.tsse);
+        fit(ln.sb_rowsum, z.rowsum); fit(ln.xn, z.xn); fit(ln.tlen, z.tlen); fit(ln.magpad, z.magpad); fit(ln.fbx, z.fbx); fit(ln.hseq, z.fbhseq);
+        fit(m->r_gin, z.gin); fit(m->r_hseq, z.hseq); fit(m->r_hstate, z.hstate); fit(m->sb_cum, z.cum); fit(m->cstate, z.cstate);
+        m->mask_tmp.release(); m->sb_scratch.release();
+        fsn_model::Lane& other = m->lane[&ln == &m->lane[0] ? 1 : 0];    // the pipelined entry points' second lane
+        other.release_all(); other.wsB = other.wsT = other.wsTw = 0;
+    }
+    int e = 0;
+    e |= ln.fbin.ensure(z.act, true, s);
+    e |= ln.fbout.ensure(z.act, true, s);
+    e |= ln.mu.ensure(z.mu, true, s);
+    e |= ln.sigma.ensure(z.mu, true, s);
+    e |= ln.tsse_scale.ensure(z.tsse, true, s);                          // per-row scale | row statistics
+    e |= ln.sb_rowsum.ensure(z.rowsum, true, s);
+    if (z.xn) e |= ln.xn.ensure(z.xn, true, s);
+    if (c.sb_tcn) {
+        // sub-band TCN: the lane's packed input (+ block 0's stream maxima), the shared scratch of the blocks (serialised on the sub-band
+        // stream like the LSTM scratch); every buffer is fully written before it is read (the pad columns by the packer / the epilogue)
+        const long long srows = (long long)B * F * Tp;
+        if (srows + 128 > 0x7fffffffLL) return fail(FSN_EINVAL, "B * num_freqs * (T + look_ahead) = %lld rows exceeds the sub-band TCN's 2^31 limit", srows);
+        if (regeo) ln.sbx.release();
+        e |= ln.sbx.ensure(z.sbx, false, s);
+        if (e) return fail(FSN_ECUDA, "workspace allocation failed for B=%d T=%d", B, T);
+        if (regeo && make_tmap_f32_2d(ln.mapSbx, ln.sbx.p, srows, 64, 128)) return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the sub-band input");
+        int rc = grow_tcn_scratch(m->sb_scratch, m->tcn_sb, srows, (size_t)B * F, false, sl);
+        if (rc) return rc;
+    } else {
+        // images are re-zeroed whenever the geometry changes (rows beyond B*F and k >= I must stay zero)
+        if (regeo) { ln.ximg.release(); }
+        e |= ln.ximg.ensure(z.ximg, true, s);
+    }
+    // LSTM-side scratch: shared by both lanes (LSTM launches are serialised on the LSTM stream)
+    if (Tw) {
+        e |= m->r_hstate.ensure(z.hstate, false, sl);
+        if (z.cum) e |= m->sb_cum.ensure(z.cum, false, sl);
+    }
+    if (z.gin) {                                                         // Gin and the layer output of the deeper layers
+        e |= m->r_gin.ensure(z.gin, false, sl);
+        e |= m->r_hseq.ensure(z.hseq, false, sl);
+    }
+    if (z.cstate) e |= m->cstate.ensure(z.cstate, true, sl);
     if (c.model_kind == FSN_KIND_PLUS) {
         if (!m->tcn5) return fail(FSN_ESTATE, "the TCN weights were not packed");
         // a new geometry gets fresh zero-filled buffers: the pad columns of x0 (and so of every stream) must be zero
         const size_t trows = (size_t)3 * B * Tp, Cp = m->tcn_fb.Cp;
         if (regeo) { ln.x0.release(); ln.xr.release(); ln.tcn.release(); }
-        e |= ln.x0.ensure(trows * Cp * 4, true, s);
-        e |= ln.xr.ensure(trows * Cp * 4, true, s);
+        e |= ln.x0.ensure(z.x0, true, s);
+        e |= ln.xr.ensure(z.x0, true, s);
         if (e) return fail(FSN_ECUDA, "workspace allocation failed for B=%d T=%d", B, T);
         if (regeo && (make_tmap_f32_2d(ln.mapX0, ln.x0.p, trows, Cp, 128) || make_tmap_f32_2d(ln.mapXr, ln.xr.p, trows, Cp, 128)))
             return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the activations");
         int rc = grow_tcn_scratch(ln.tcn, m->tcn_fb, (long long)trows, (size_t)3 * B, true, s);
         if (rc) return rc;
     } else {
-        const int Ipad = (F + 15) / 16 * 16, rows_pad = (B + 63) / 64 * 64;
-        e |= ln.magpad.ensure((size_t)B * F * Pp * 4, true, s);
-        e |= ln.fbx.ensure((size_t)Tp * rows_pad * Ipad * 2, true, s);
-        e |= ln.hseq.ensure((size_t)B * c.fb_hidden * Pp * 4, true, s);
+        e |= ln.magpad.ensure(z.magpad, true, s);
+        e |= ln.fbx.ensure(z.fbx, true, s);
+        e |= ln.hseq.ensure(z.fbhseq, true, s);
     }
     if (e) return fail(FSN_ECUDA, "workspace allocation failed for B=%d T=%d", B, T);
-    ln.wsB = B; ln.wsT = T;
+    ln.wsB = B; ln.wsT = T; ln.wsTw = Tw;
     return FSN_OK;
 }
 
 // d_enh != null: write the enhanced spectrum (decompress_cIRM x noisy) instead of the mask -- fused into the epilogue of the
 // layer-wise kernel's last layer, a separate pass over a scratch mask for the generic kernel
-static int run_sb_lstm(fsn_model* m, fsn_model::Lane& ln, int B, int T, float* d_out, const float* d_real, const float* d_imag,
-                       float* d_enh, const int* tlen, cudaStream_t s) {
+// Tw > 0: the sub-band stage runs in time windows of Tw frames (the last one shorter); for each window the images are packed (`sp`, the
+// front end's packer arguments) and every layer resumes from the h / c its previous window left (DESIGN.md §3.7).  Tw = 0: the images of
+// the whole clip are already packed and every layer runs once over all frames.
+static int run_sb_lstm(fsn_model* m, fsn_model::Lane& ln, int B, int T, int Tw, SbPackLaunch sp, float* d_out, const float* d_real,
+                       const float* d_imag, float* d_enh, const int* tlen, cudaStream_t s) {
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs, Tp = T + c.look_ahead, rows = B * F, ntiles = (rows + 127) / 128;
     const int impl = pick_impl(m);
     m->last_impl = impl;
     if (use_layerwise(m)) {
         // one recurrent launch per layer; the first one also projects its input (the packed images), each deeper one is preceded by
-        // one GEMM: the input projection of every row and time step (k_gemm_tc5.cu)
+        // one GEMM: the input projection of every row and time step of the window (k_gemm_tc5.cu)
         const int H = c.sb_hidden, ntp = (ntiles + 1) / 2 * 2;
-        const long long M = (long long)ntp * Tp * 128;
-        for (int l = 0; l < c.num_layers; ++l) {
-            if (l > 0) {
-                // row-major Gin[M, 4H] = X[M, H] * Wp[4H, H]^T, both operands K-major
-                GemmF16Launch g{M, 4 * H, H, static_cast<__half*>(m->r_gin.p), 4LL * H};
-                int ge = launch_gemm_f16(m->r_hseq.p, m->r_wih[l].p, g, m->num_sms, s);
-                if (ge) return fail(FSN_ECUDA, "input-projection GEMM launch failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)ge));
+        const size_t cs_layer = lstm_tc5r_cstate_bytes(ntiles, H) / sizeof(float), hs_layer = (size_t)ntp * 128 * H;
+        for (int w0 = 0; w0 < Tp; w0 += (Tw ? Tw : Tp)) {
+            const int tw = Tw ? (Tp - w0 < Tw ? Tp - w0 : Tw) : Tp;
+            if (Tw) {
+                sp.t0 = w0; sp.Tw = tw;
+                launch_sb_pack(sp, s);
                 m->launches++;
             }
-            LstmTc5rLaunch a{};
-            a.wstream = static_cast<const __half*>(m->r_stream[l].p);
-            a.bias = static_cast<const float*>(m->r_bias[l].p);
-            a.fc_w = P(m, "sb_model.fc_output_layer.weight");
-            a.fc_b = P(m, "sb_model.fc_output_layer.bias");
-            a.H = H; a.rows = rows; a.Tp = Tp; a.ntiles = ntiles;
-            if (l == 0) a.ximg = static_cast<const __half*>(ln.ximg.p);
-            else a.gin = static_cast<const __half*>(m->r_gin.p);
-            a.hseq = static_cast<__half*>(m->r_hseq.p);
-            a.cstate = static_cast<float*>(m->cstate.p);
-            a.out = d_out; a.F = F; a.la = c.look_ahead;
-            a.act = c.sb_act; a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU; a.last = (l == c.num_layers - 1);
-            a.nreal = d_real; a.nimag = d_imag; a.enh = reinterpret_cast<float2*>(d_enh); a.tlen = tlen;
-            int e = launch_lstm_tc5r(a, s);
-            if (e) return fail(FSN_ECUDA, "layer-wise LSTM launch failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)e));
-            m->launches++;
+            const long long M = (long long)ntp * tw * 128;
+            for (int l = 0; l < c.num_layers; ++l) {
+                if (l > 0) {
+                    // row-major Gin[M, 4H] = X[M, H] * Wp[4H, H]^T, both operands K-major
+                    GemmF16Launch g{M, 4 * H, H, static_cast<__half*>(m->r_gin.p), 4LL * H};
+                    int ge = launch_gemm_f16(m->r_hseq.p, m->r_wih[l].p, g, m->num_sms, s);
+                    if (ge) return fail(FSN_ECUDA, "input-projection GEMM launch failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)ge));
+                    m->launches++;
+                }
+                LstmTc5rLaunch a{};
+                a.wstream = static_cast<const __half*>(m->r_stream[l].p);
+                a.bias = static_cast<const float*>(m->r_bias[l].p);
+                a.fc_w = P(m, "sb_model.fc_output_layer.weight");
+                a.fc_b = P(m, "sb_model.fc_output_layer.bias");
+                a.H = H; a.rows = rows; a.Tp = Tp; a.ntiles = ntiles;
+                a.t0 = w0; a.Tw = tw;
+                if (l == 0) a.ximg = static_cast<const __half*>(ln.ximg.p);
+                else a.gin = static_cast<const __half*>(m->r_gin.p);
+                a.hseq = static_cast<__half*>(m->r_hseq.p);
+                a.cstate = static_cast<float*>(m->cstate.p) + (Tw ? l * cs_layer : 0);
+                if (Tw) a.hstate = static_cast<__half*>(m->r_hstate.p) + l * hs_layer;
+                a.out = d_out; a.F = F; a.la = c.look_ahead;
+                a.act = c.sb_act; a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU; a.last = (l == c.num_layers - 1);
+                a.nreal = d_real; a.nimag = d_imag; a.enh = reinterpret_cast<float2*>(d_enh); a.tlen = tlen;
+                int e = launch_lstm_tc5r(a, s);
+                if (e) return fail(FSN_ECUDA, "layer-wise LSTM launch failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)e));
+                m->launches++;
+            }
         }
+    } else if (Tw) {
+        return fail(FSN_EINVAL, "time windows of the sub-band stage need the layer-wise LSTM path");
     } else if (impl == FSN_LSTM_TCGEN05) {
         return fail(FSN_EINVAL, "the tensor-core LSTM needs hidden %% 64 == 0 and <= 512, input <= 64, output_size 2");
     } else {
@@ -863,8 +982,9 @@ static int stage_lengths(fsn_model* m, fsn_model::Lane& ln, const int32_t* h_fra
 }
 
 // h_frames: the frame count of every sample of a ragged batch (validated by the caller), or null when every sample spans T frames
+// Tw: time window of the sub-band stage (0: the whole clip; > 0 needs s == sl, the plain entry points)
 static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
-                        const int32_t* h_frames, float* d_out, float* d_enh, cudaStream_t s, cudaStream_t sl) {
+                        const int32_t* h_frames, float* d_out, float* d_enh, cudaStream_t s, cudaStream_t sl, int Tw = 0) {
     if (!m || !d_mag || (!d_out && !d_enh)) return fail(FSN_EINVAL, "null argument");
     if (d_enh && (!d_real || !d_imag)) return fail(FSN_EINVAL, "the enhanced-spectrum output needs the noisy real and imaginary planes");
     if (d_enh && m->cfg.output_size != 2) return fail(FSN_EINVAL, "the enhanced-spectrum output needs output_size 2 (a complex mask)");
@@ -879,7 +999,9 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
     if (c.model_kind == FSN_KIND_PLUS && c.channel_attention == FSN_ATTN_TSSE)
         for (int i = 0; i < 3; ++i)
             if (Tp < c.kersize[i]) return fail(FSN_EINVAL, "sequence shorter than the TSSE kernel size");
-    int rc = ensure_ws(m, ln, B, T, s, sl);
+    int rc = check_length(c, B, T);
+    if (rc) return rc;
+    rc = ensure_ws(m, ln, B, T, Tw, s, sl);
     if (rc) return rc;
     const int* tl = nullptr;                                            // per-sample extents on the device (null: all Tp)
     if (h_frames) {
@@ -900,6 +1022,8 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
     sp.norm_type = c.norm_type;
     sp.ximg = static_cast<__half*>(ln.ximg.p);
     sp.ntiles = (B * F + 127) / 128;
+    sp.t0 = 0; sp.Tw = Tp;
+    sp.cum = Tw ? static_cast<double*>(m->sb_cum.p) : nullptr;
     sp.tlen = tl;
 
     if (c.model_kind == FSN_KIND_PLUS) {
@@ -1019,17 +1143,18 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
         sp.xtm = static_cast<float*>(ln.sbx.p);
         sp.amax = sp.xtm + (size_t)B * F * Tp * 64;
         launch_sb_pack_tm(sp, s);
-    } else {
+        m->launches++;
+    } else if (!Tw) {                                                   // windowed: run_sb_lstm packs each window
         launch_sb_pack(sp, s);
+        m->launches++;
     }
-    m->launches++;
     cudaEventRecord(m->evf1[evi], s);
     if (sl != s) {                                                      // pipelined: the LSTM stream picks the lane up when the front end is done
         CK(cudaEventRecord(ln.ev_front, s));
         CK(cudaStreamWaitEvent(sl, ln.ev_front, 0));
     }
     cudaEventRecord(m->ev0[evi], sl);
-    rc = c.sb_tcn ? run_sb_tcn(m, ln, B, T, d_out, d_real, d_imag, d_enh, tl, sl) : run_sb_lstm(m, ln, B, T, d_out, d_real, d_imag, d_enh, tl, sl);
+    rc = c.sb_tcn ? run_sb_tcn(m, ln, B, T, d_out, d_real, d_imag, d_enh, tl, sl) : run_sb_lstm(m, ln, B, T, Tw, sp, d_out, d_real, d_imag, d_enh, tl, sl);
     cudaEventRecord(m->ev1[evi], sl);
     if (rc) return rc;
     m->nfwd++;
@@ -1079,11 +1204,12 @@ static int submit_impl(fsn_model* m, cudaEvent_t ready, const float* d_mag, cons
 
 // Workspace per sample (bytes) of a forward with T frames: the per-sample slices of every grow-only buffer of ensure_ws.  The
 // layer-wise path dominates: its time-batched input projection Gin takes 257 x T' x 4H x 2 bytes per sample (0.2 GB at config #5).
-static double ws_bytes_per_sample(const fsn_model* m, int T) {
-    const fsn_config& c = m->cfg;
+// This estimate picks the sub-batch of a batch that fits unwindowed (plan_forward); it counts F rows per sample where the layer-wise
+// buffers hold whole pairs of 128-row tiles, so plan_forward checks its choice against the exact count of ws_sizes.
+static double ws_bytes_per_sample(const fsn_config& c, bool layerwise, int T) {
     const double F = c.num_freqs, Tp = T + c.look_ahead, rows = F;              // sequences per sample
     double b = 0;
-    if (c.model_kind == FSN_KIND_PLUS) b += 3 * F * Tp * 4 * 2 + 3 * Tp * (4.0 * m->tcn_fb.Cp + 512) * 4;   // fb_in/out, X0/Xa/Xb/Xr (fp32), Y1/Y2 (fp16)
+    if (c.model_kind == FSN_KIND_PLUS) b += 3 * F * Tp * 4 * 2 + 3 * Tp * (4.0 * ((c.num_freqs + 31) / 32 * 32) + 512) * 4;   // fb_in/out, X0/Xa/Xb/Xr (fp32), Y1/Y2 (fp16)
     else b += F * Tp * 4 * 4 + Tp * (F + c.fb_hidden) * 4;
     if (c.sb_tcn) {                                                             // input + two fp32 streams of 64 channels, two fp16 hidden
         b += rows * Tp * (3 * 64 * 4 + 2 * 512 * 2) + rows * (tcn_stats_bytes(1) + 4);   // buffers of 512; statistics, the input's max |x|
@@ -1091,8 +1217,55 @@ static double ws_bytes_per_sample(const fsn_model* m, int T) {
     }
     b += rows * Tp * 128;                                                       // packed sub-band images (when used)
     b += rows * c.num_layers * c.sb_hidden * 4;                                  // cell state
-    if (use_layerwise(m) && c.num_layers > 1) b += rows * Tp * (4.0 * c.sb_hidden + c.sb_hidden) * 2;   // Gin + layer output sequence
+    if (layerwise && c.num_layers > 1) b += rows * Tp * (4.0 * c.sb_hidden + c.sb_hidden) * 2;   // Gin + layer output sequence
     return b;
+}
+
+// The plan of a plain forward (fsn_plan_forward): sub-batch Bs and sub-band window Tw (0: whole clip) so that the exact workspace
+// (ws_sizes) stays within cap.
+//   * the sub-batch of the per-sample estimate, if it fits unwindowed: the forward of every release before windows existed;
+//   * else (layer-wise path only) the largest sub-batch that fits with a window of 256 frames (32 if none does), then the longest window
+//     (a multiple of 32) that fits, evened out over the same number of windows; more sequences in flight keep more SMs busy;
+//   * nothing fits: one clip at a time with a 256-frame window, allocated anyway.
+// force > 0 (FSN_SB_WINDOW) windows every layer-wise forward with exactly that window.  Sub-batches are equal splits of B.
+static void plan_forward(const fsn_config& c, bool layerwise, int B, int T, double cap, int force, int* pBs, int* pTw, int64_t* pbytes) {
+    const int Tp = T + c.look_ahead, wmax = (Tp + 31) / 32 * 32;
+    const long long blim = max_clips_for_rows(c, T);             // sub-batches never exceed the full-band TCN's row limit
+    auto split = [&](int bmax) { if (bmax > blim) bmax = (int)blim; if (bmax < 1) bmax = 1; if (B <= bmax) return B; const int n = (B + bmax - 1) / bmax; return (B + n - 1) / n; };
+    auto bytes = [&](int bs, int tw) { return (double)ws_sizes(c, layerwise, bs, T, tw).total(); };
+    // largest equal split whose workspace with window tw fits (0 if even one clip does not)
+    auto max_split = [&](int tw) {
+        int lo = 0, hi = B;                                             // invariant: split(lo) fits or lo == 0; split(hi + 1) does not
+        while (lo < hi) { const int mid = (lo + hi + 1) / 2; if (bytes(split(mid), tw) <= cap) lo = mid; else hi = mid - 1; }
+        return lo ? split(lo) : 0;
+    };
+    const double per = ws_bytes_per_sample(c, layerwise, T);
+    const double bmax = cap / (per > 1 ? per : 1);
+    int Bs = split(bmax < B ? (int)bmax : B), Tw = 0;
+    if (layerwise && force > 0) {
+        Tw = force;
+        const int b = max_split(Tw);
+        Bs = b ? b : 1;
+    } else if (layerwise && bytes(Bs, 0) > cap) {
+        int b = 0, wmin = 0;
+        for (int w : {256, 32}) {
+            wmin = w < wmax ? w : wmax;
+            if ((b = max_split(wmin))) break;
+        }
+        if (!b) {
+            Bs = 1; Tw = 256 < wmax ? 256 : wmax;
+        } else if (bytes(b, 0) <= cap) {
+            Bs = b;                                                     // the smaller sub-batch fits unwindowed
+        } else {
+            Bs = b;
+            int lo = wmin / 32, hi = wmax / 32;                         // longest window (in 32-frame units) that fits
+            while (lo < hi) { const int mid = (lo + hi + 1) / 2; if (bytes(Bs, 32 * mid) <= cap) lo = mid; else hi = mid - 1; }
+            const int nwin = (Tp + 32 * lo - 1) / (32 * lo);
+            Tw = ((Tp + nwin - 1) / nwin + 31) / 32 * 32;
+        }
+    }
+    *pBs = Bs; *pTw = Tw;
+    if (pbytes) *pbytes = (int64_t)bytes(Bs, Tw);
 }
 
 static int forward_plain(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
@@ -1104,22 +1277,23 @@ static int forward_plain(fsn_model* m, const float* d_mag, const float* d_real, 
     for (auto& ln : m->lane)                                             // batches still in flight in the pipeline share the scratch buffers
         if (ln.used) CK(cudaStreamWaitEvent(s, ln.ev_lstm, 0));
     // Samples are independent, so a batch whose workspace would exceed the cap (FSN_WS_CAP_GB, default 24 of the 80 GB) is run as
-    // equal sub-batches one after the other on the same stream -- same results, bounded memory (e.g. 256 clips on the layer-wise path).
-    const double per = ws_bytes_per_sample(m, T);
-    int Bmax = (int)(m->ws_cap_bytes / (per > 1 ? per : 1));
-    if (Bmax < 1) Bmax = 1;
+    // equal sub-batches one after the other on the same stream -- same results, bounded memory (e.g. 256 clips on the layer-wise path);
+    // a clip too long for the cap runs its sub-band stage in time windows (plan_forward) -- same bits, O(window) sub-band memory.
+    if (int rc = check_length(m->cfg, 1, T)) return rc;
+    int Bs = B, Tw = 0;
+    plan_forward(m->cfg, use_layerwise(m), B, T, m->ws_cap_bytes, m->env_sb_window, &Bs, &Tw, nullptr);
+    m->plan_Bs = Bs; m->plan_Tw = Tw;
     int rc = FSN_OK;
-    if (B <= Bmax) {
-        rc = forward_impl(m, m->lane[0], d_mag, d_real, d_imag, B, T, h_frames, d_out, d_enh, s, s);
+    if (Bs >= B) {
+        rc = forward_impl(m, m->lane[0], d_mag, d_real, d_imag, B, T, h_frames, d_out, d_enh, s, s, Tw);
     } else {
-        const int nsplit = (B + Bmax - 1) / Bmax, Bs = (B + nsplit - 1) / nsplit;
         const size_t in_stride = (size_t)m->cfg.num_freqs * T, out_stride = (size_t)m->cfg.output_size * m->cfg.num_freqs * T;
         int64_t launches = 0;
         for (int b0 = 0; b0 < B && rc == FSN_OK; b0 += Bs) {
             const int nb = (B - b0 < Bs) ? B - b0 : Bs;
             rc = forward_impl(m, m->lane[0], d_mag + b0 * in_stride, d_real ? d_real + b0 * in_stride : nullptr, d_imag ? d_imag + b0 * in_stride : nullptr,
                               nb, T, h_frames ? h_frames + b0 : nullptr, d_out ? d_out + b0 * out_stride : nullptr,
-                              d_enh ? d_enh + b0 * in_stride * 2 : nullptr, s, s);
+                              d_enh ? d_enh + b0 * in_stride * 2 : nullptr, s, s, Tw);
             launches += m->launches;
         }
         m->launches = launches;
@@ -1473,3 +1647,54 @@ extern "C" float fsn_model_last_lstm_ms(fsn_model* m) {
     return fsn_model_lstm_ms_history(m, &ms, 1) == 1 ? ms : -1.f;
 }
 extern "C" int fsn_model_last_lstm_impl(const fsn_model* m) { return m ? m->last_impl : 0; }
+
+extern "C" int fsn_plan_forward(const fsn_config* cfg, int32_t B, int32_t T, double cap_bytes, int32_t force_window, int32_t* Bs, int32_t* Tw,
+                                int64_t* bytes) {
+    if (!cfg || !Bs || !Tw || B < 1 || T < 1 || !(cap_bytes > 0)) return fail(FSN_EINVAL, "bad argument");
+    if (force_window < 0 || force_window % 32) return fail(FSN_EINVAL, "force_window must be 0 or a positive multiple of 32");
+    if (cfg->num_freqs < 4 || cfg->num_layers < 1 || cfg->num_layers > 4 || cfg->look_ahead < 0) return fail(FSN_EINVAL, "bad configuration");
+    if (int rc = check_length(*cfg, 1, T)) return rc;
+    int bs = 0, tw = 0;
+    plan_forward(*cfg, config_layerwise(*cfg, 0), B, T, cap_bytes, force_window, &bs, &tw, bytes);
+    *Bs = bs; *Tw = tw;
+    return FSN_OK;
+}
+
+extern "C" int fsn_model_plan(const fsn_model* m, int32_t B, int32_t T, int32_t* Bs, int32_t* Tw, int64_t* bytes) {
+    if (!m || !Bs || !Tw || B < 1 || T < 1) return fail(FSN_EINVAL, "bad argument");
+    if (int rc = check_length(m->cfg, 1, T)) return rc;
+    int bs = 0, tw = 0;
+    plan_forward(m->cfg, config_layerwise(m->cfg, m->env_impl), B, T, m->ws_cap_bytes, m->env_sb_window, &bs, &tw, bytes);
+    *Bs = bs; *Tw = tw;
+    return FSN_OK;
+}
+
+extern "C" int fsn_model_release_workspace(fsn_model* m) {
+    if (!m) return fail(FSN_EINVAL, "null model");
+    CK(cudaDeviceSynchronize());                                         // nothing in flight may still read the buffers
+    for (auto& ln : m->lane) { ln.release_all(); ln.wsB = ln.wsT = ln.wsTw = 0; }
+    DevBuf* lstm[] = {&m->cstate, &m->mask_tmp, &m->r_gin, &m->r_hseq, &m->r_hstate, &m->sb_cum, &m->ws_h, &m->ws_bar};
+    for (auto* b : lstm) b->release();
+    m->sb_scratch.release();
+    return FSN_OK;
+}
+
+extern "C" int64_t fsn_model_workspace_bytes(const fsn_model* m) {
+    if (!m) return 0;
+    size_t n = 0;
+    for (const auto& ln : m->lane) {
+        const DevBuf* all[] = {&ln.fbin, &ln.fbout, &ln.mu, &ln.ximg, &ln.magpad, &ln.fbx, &ln.hseq, &ln.x0, &ln.xr, &ln.tsse_scale,
+                               &ln.sb_rowsum, &ln.xn, &ln.sigma, &ln.sbx, &ln.tlen, &ln.tcn.xa, &ln.tcn.xb, &ln.tcn.y1, &ln.tcn.y2, &ln.tcn.stats};
+        for (const auto* b : all) n += b->bytes;
+    }
+    const DevBuf* lstm[] = {&m->cstate, &m->mask_tmp, &m->r_gin, &m->r_hseq, &m->r_hstate, &m->sb_cum, &m->ws_h, &m->ws_bar,
+                            &m->sb_scratch.xa, &m->sb_scratch.xb, &m->sb_scratch.y1, &m->sb_scratch.y2, &m->sb_scratch.stats};
+    for (const auto* b : lstm) n += b->bytes;
+    return (int64_t)n;
+}
+
+extern "C" int fsn_model_last_plan(const fsn_model* m, int32_t* Bs, int32_t* Tw) {
+    if (!m || !Bs || !Tw) return fail(FSN_EINVAL, "null argument");
+    *Bs = m->plan_Bs; *Tw = m->plan_Tw;
+    return FSN_OK;
+}

@@ -75,8 +75,10 @@ struct SbPackLaunch {
     float* sigma;            // [B] unbiased std (offline_gaussian_norm only)
     float* rowsum;           // [B, 1 + nfb, F, 2] scratch: row sums and sums of squares
     int norm_type;           // FSN_NORM_*
-    __half* ximg;            // [ntiles, Tp, 128 rows, 64 halves] SWIZZLE_128B images
+    __half* ximg;            // [ntiles, Tw, 128 rows, 64 halves] SWIZZLE_128B images of frames t0 .. t0 + Tw - 1
     int ntiles;
+    int t0, Tw;              // frame window of the images (t0 = 0, Tw = Tp: the whole clip); Tw is a multiple of 32 except in the last window
+    double* cum;             // cumulative norms, windowed: running (sum, sum of squares) [B*F][2] at the window's end, reloaded when t0 > 0
     float* xtm;              // sub-band TCN input: fp32 time-major [B*F*Tp, 64], row (b*F + f)*Tp + t, columns >= I zero
     float* amax;             // [B*F] max |x| of every sequence of xtm (zeroed by the launcher): block 0's fp16 store scale
     const int* tlen;         // optional [B] per-sample extent in frames of Tp (rows past it are written as zero); null: Tp
@@ -154,12 +156,17 @@ struct LstmTc5rLaunch {
     const float* bias;        // [4H] pre-scaled, chunk column order
     const float* fc_w;        // [2][H]   (last layer)
     const float* fc_b;        // [2]
-    int H, rows, Tp, ntiles;
-    const __half* gin;        // [ntiles_pad * Tp * 128, 4H] fp16 input projection X_l W_ih^T (lstm_tc5r_gin_order), or null with ximg
-    const __half* ximg;       // first layer: [ntiles_pad, Tp, 128 rows, 64 halves] SW128 input images; the input projection is then part
+    int H, rows, Tp, ntiles;  // Tp: frames of the whole clip (T + look_ahead)
+    // time window of this launch: steps t0 .. t0 + Tw - 1 (t0 = 0, Tw = Tp: the whole clip).  gin / ximg / hseq hold the window only
+    // (window-local step index, stride Tw); the output index, the look-ahead test and tlen use the absolute step t0 + t
+    int t0, Tw;
+    const __half* gin;        // [ntiles_pad * Tw * 128, 4H] fp16 input projection X_l W_ih^T (lstm_tc5r_gin_order), or null with ximg
+    const __half* ximg;       // first layer: [ntiles_pad, Tw, 128 rows, 64 halves] SW128 input images; the input projection is then part
                               // of the recurrence, with W_ih as one extra k-block in front of every chunk of the stream
-    __half* hseq;             // [ntiles_pad * Tp * 128, H] fp16 output sequence (not the last layer)
-    float* cstate;            // [2 ntiles_pad CTAs][H/32 chunks][4][128 threads] float4
+    __half* hseq;             // [ntiles_pad * Tw * 128, H] fp16 output sequence (not the last layer)
+    float* cstate;            // [2 ntiles_pad CTAs][H/32 chunks][4][128 threads] float4: c (GRU: h in fp32), read back at t0 > 0
+    __half* hstate;           // windowed forwards: this layer's fp16 h [ntiles_pad * 128, H], loaded at entry when t0 > 0 (instead
+                              // of h = 0) and stored at exit; null: h starts at zero and is not kept
     float* out; int F, la;    // last layer: mask [B, 2, F, Tp - la]
     int act;                  // FSN_ACT_* on the Linear output (last layer)
     int fast, gru, last;

@@ -464,7 +464,7 @@ struct Fp16Img {
         float w[8];
 #pragma unroll
         for (int i = 0; i < 8; ++i) w[i] = fminf(fmaxf(v[i], -65504.f), 65504.f);
-        char* img = reinterpret_cast<char*>(a.ximg) + ((size_t)(row >> 7) * a.Tp + t) * (128 * 128);
+        char* img = reinterpret_cast<char*>(a.ximg) + ((size_t)(row >> 7) * a.Tw + (t - a.t0)) * (128 * 128);
         *reinterpret_cast<uint4*>(img + sw128_offset(row & 127, k0)) =
             make_uint4(pack_half2(w[0], w[1]), pack_half2(w[2], w[3]), pack_half2(w[4], w[5]), pack_half2(w[6], w[7]));
     }
@@ -495,7 +495,7 @@ constexpr int SBP_F = 32, SBP_T = 32;
 template <class Store>
 __global__ void __launch_bounds__(256) sb_pack_kernel(SbPackLaunch a) {
     extern __shared__ float sm[];
-    const int F = a.F, Tp = a.Tp, b = blockIdx.z, f0 = blockIdx.y * SBP_F, t0 = blockIdx.x * SBP_T;
+    const int F = a.F, Tp = a.t0 + a.Tw, b = blockIdx.z, f0 = blockIdx.y * SBP_F, t0 = a.t0 + blockIdx.x * SBP_T;   // Tp: the window's end
     const int Tpe = a.tlen ? a.tlen[b] : Tp;                       // frames t >= Tpe are past this sample's end: written as zero
     const int nw = 2 * a.Ns + 1, nf = 2 * a.Nf + 1, I = nw + a.nfb * nf;
     const int wrows = SBP_F + 2 * a.Ns, frows = SBP_F + 2 * a.Nf;
@@ -545,15 +545,16 @@ __global__ void __launch_bounds__(256) sb_pack_kernel(SbPackLaunch a) {
 template <class Store>
 __global__ void __launch_bounds__(128) sb_pack_cum_kernel(SbPackLaunch a) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int row = blockIdx.x * 4 + warp, F = a.F, Tp = a.Tp;
+    const int row = blockIdx.x * 4 + warp, F = a.F, Tp = a.t0 + a.Tw;   // Tp: the window's end
     if (row >= a.B * F) return;
     const int b = row / F, f = row % F;
-    const int Tpe = a.tlen ? a.tlen[b] : Tp;                       // frames t >= Tpe are past this sample's end: written as zero
+    const int Tpe = a.tlen ? a.tlen[b] : a.Tp;                     // frames t >= Tpe are past this sample's end: written as zero
     const int nw = 2 * a.Ns + 1, nf = 2 * a.Nf + 1, I = nw + a.nfb * nf;
     const double EPS = 1.1920928955078125e-07;
-    double cs = 0.0, cq = 0.0;                                   // running sums carried across 32-frame chunks
+    double cs = 0.0, cq = 0.0;                                   // running sums carried across 32-frame chunks (and windows: a.cum)
+    if (a.cum && a.t0 > 0) { cs = a.cum[2 * (size_t)row]; cq = a.cum[2 * (size_t)row + 1]; }
     float mx = 0.f;
-    for (int t0 = 0; t0 < Tp; t0 += 32) {
+    for (int t0 = a.t0; t0 < Tp; t0 += 32) {
         const int t = t0 + lane;
         float v[64];
         float s = 0.f, q = 0.f;
@@ -593,6 +594,7 @@ __global__ void __launch_bounds__(128) sb_pack_cum_kernel(SbPackLaunch a) {
             }
         }
     }
+    if (a.cum && lane == 0) { a.cum[2 * (size_t)row] = cs; a.cum[2 * (size_t)row + 1] = cq; }
     Store::finish(a, row, mx, 32);
 }
 
@@ -604,7 +606,7 @@ static void sb_pack_go(const SbPackLaunch& a, cudaStream_t s) {
     {
         const size_t smem = sizeof(float) * (SBP_T + 1) * ((SBP_F + 2 * a.Ns) + a.nfb * (SBP_F + 2 * a.Nf));
         cudaFuncSetAttribute(sb_pack_kernel<Store>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        sb_pack_kernel<Store><<<dim3((a.Tp + SBP_T - 1) / SBP_T, (a.F + SBP_F - 1) / SBP_F, a.B), 256, smem, s>>>(a);
+        sb_pack_kernel<Store><<<dim3((a.Tw + SBP_T - 1) / SBP_T, (a.F + SBP_F - 1) / SBP_F, a.B), 256, smem, s>>>(a);
     }
 }
 void launch_sb_pack(const SbPackLaunch& a, cudaStream_t s) { sb_pack_go<Fp16Img>(a, s); }

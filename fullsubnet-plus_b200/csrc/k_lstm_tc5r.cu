@@ -18,6 +18,8 @@
 //     slot two phases ahead, which an mbarrier parity wait cannot tell from the phase before).  The epilogue adds Gin_l(t), does
 //     the cell update and writes h_l(t) both into the next step's A buffer and, for all but the last layer, as the next layer's
 //     GEMM input (fp16, row-major); the last layer applies the output Linear(H -> 2) and writes the mask (or the enhanced spectrum).
+// Long clips run one launch per time window (LstmTc5rLaunch::t0 / Tw, DESIGN.md §3.7): h enters from and leaves to a per-layer fp16
+// state, c stays in the per-layer cstate, so a windowed layer computes exactly what one launch over all frames computes.
 // Gate chunk j, column n = cg * 32 + q * 8 + u: gate q (i, f, g, o / GRU pseudo-gates r, z, n_x, n_h) of hidden unit
 // 32 j + 8 cg + u (fsn_tc5_gate_row), so every thread's accumulator fragment holds all four gates of its units.
 #include "fsn_common.cuh"
@@ -56,7 +58,9 @@ template <int H, bool FAST, bool GRU, bool LAST>
 __global__ void __cluster_dims__(R5_CL, 1, 1) __launch_bounds__(R5_THREADS, 1) lstm_tc5r_kernel(LstmTc5rLaunch a, int nstage) {
     extern __shared__ uint8_t smem_raw[];
     constexpr int NCH = H / 32, KBH = H / 64, HBUF = KBH * R5_ROWS * 128;
-    const int Tp = a.Tp;
+    // steps t0 .. tend - 1 of the clip (the window); t is the absolute step throughout: the window-local buffers (images, Gin, hseq) are
+    // indexed with t - t0, and since t0 % 4 == 0 the step parities and the phases of the input-tile barriers match a launch from t = 0
+    const int t0 = a.t0, tend = a.t0 + a.Tw;
     const int cta = blockIdx.x;
     const uint32_t rank = cluster_ctarank();
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -77,7 +81,15 @@ __global__ void __cluster_dims__(R5_CL, 1, 1) __launch_bounds__(R5_THREADS, 1) l
         for (int i = 0; i < 2; ++i) { mbar_init(&xfull[i], 1); mbar_init(&xempty[i], 1); }
         fence_barrier_init();
     }
-    for (int i = tid; i < HBUF / 16; i += R5_THREADS) reinterpret_cast<uint4*>(hbuf)[i] = make_uint4(0, 0, 0, 0);   // h(-1) = 0
+    if (a.hstate && t0 > 0) {                                              // h(t0 - 1) of the previous window into parity t0 & 1 = 0
+        for (int i = tid; i < R5_ROWS * H / 8; i += R5_THREADS) {
+            const int r = i / (H / 8), u = (i % (H / 8)) * 8;
+            *reinterpret_cast<uint4*>(hbuf + (u >> 6) * R5_ROWS * 128 + sw128_offset(r, u & 63)) =
+                __ldcg(reinterpret_cast<const uint4*>(a.hstate + (size_t)(cta * R5_ROWS + r) * H + u));
+        }
+    } else {
+        for (int i = tid; i < HBUF / 16; i += R5_THREADS) reinterpret_cast<uint4*>(hbuf)[i] = make_uint4(0, 0, 0, 0);   // h(-1) = 0
+    }
     fence_proxy_async();
     __syncthreads();
     cluster_sync_all();                                                    // barriers of both CTAs are initialised
@@ -90,11 +102,11 @@ __global__ void __cluster_dims__(R5_CL, 1, 1) __launch_bounds__(R5_THREADS, 1) l
             const uint64_t pol_w = l2_policy_evict_last();          // the weights, re-read every step by every cluster: must survive the Gin stream
             const int NS = nstage / 2;
             int slot[2] = {0, 0}; uint32_t ph[2] = {0, 0};
-            for (int t = 0; t < Tp; ++t) {
+            for (int t = t0; t < tend; ++t) {
                 if (KX) {                                           // my 64 rows of the step's input image
                     mbar_wait(&xempty[t & 1], ((t >> 1) & 1) ^ 1);
                     mbar_arrive_expect_tx(&xfull[t & 1], R5_XTILE);
-                    bulk_g2s(xbuf + (t & 1) * R5_XTILE, reinterpret_cast<const uint8_t*>(a.ximg) + (((size_t)(cta >> 1) * Tp + t) * 128 + (cta & 1) * R5_ROWS) * 128,
+                    bulk_g2s(xbuf + (t & 1) * R5_XTILE, reinterpret_cast<const uint8_t*>(a.ximg) + (((size_t)(cta >> 1) * a.Tw + (t - t0)) * 128 + (cta & 1) * R5_ROWS) * 128,
                              R5_XTILE, &xfull[t & 1]);
                 }
                 for (int j = 0; j < NCH; ++j) {
@@ -119,16 +131,17 @@ __global__ void __cluster_dims__(R5_CL, 1, 1) __launch_bounds__(R5_THREADS, 1) l
         for (int h = 0; h < 2; ++h) {
             rl[h] = wi * 16 + (lane >> 2) + 8 * h;
             grow[h] = cta * R5_ROWS + rl[h];
-            mrow0[h] = (size_t)(cta >> 1) * Tp * 128 + (cta & 1) * R5_ROWS + rl[h];     // + t * 128: row of the (tile, t) block of Gin / hseq
+            // + t * 128: row of the (tile, t - t0) block of Gin / hseq (mod 2^64: the sum is the window-local row)
+            mrow0[h] = ((size_t)(cta >> 1) * a.Tw - t0) * 128 + (cta & 1) * R5_ROWS + rl[h];
         }
-        const int Tout = Tp - a.la;
+        const int Tout = a.Tp - a.la;
         const float L2E = 1.4426950408889634f;
         float* cbase = a.cstate + (size_t)cta * NCH * 4 * 128 * 4;
         float acc[64];
         const bool has_gin = a.gin != nullptr;
         const int NS = nstage / 2;
         int rslot = 0; uint32_t rph = 0;                            // position in this warpgroup's ring (slots wg * NS ..)
-        for (int t = 0; t < Tp; ++t) {
+        for (int t = t0; t < tend; ++t) {
             const uint8_t* hA = hbuf + (size_t)(t & 1) * HBUF;
             uint8_t* hN = hbuf + (size_t)((t + 1) & 1) * HBUF;
             float fc0[2] = {0.f, 0.f}, fc1[2] = {0.f, 0.f};
@@ -251,7 +264,7 @@ __global__ void __cluster_dims__(R5_CL, 1, 1) __launch_bounds__(R5_THREADS, 1) l
                 for (int h = 0; h < 2; ++h) {
                     if (grow[h] >= a.rows) continue;
                     const int ob = grow[h] / a.F, of = grow[h] % a.F;
-                    if (a.tlen && t >= __ldg(a.tlen + ob)) {        // past the clip's end: zeros, the noisy planes are not read
+                    if (a.tlen && t >= __ldg(a.tlen + ob)) {       // past the clip's end: zeros, the noisy planes are not read
                         const size_t ni = ((size_t)ob * a.F + of) * Tout + (t - a.la);
                         if (a.enh) a.enh[ni] = make_float2(0.f, 0.f);
                         else { a.out[(((size_t)ob * 2 + 0) * a.F + of) * Tout + (t - a.la)] = 0.f; a.out[(((size_t)ob * 2 + 1) * a.F + of) * Tout + (t - a.la)] = 0.f; }
@@ -273,6 +286,14 @@ __global__ void __cluster_dims__(R5_CL, 1, 1) __launch_bounds__(R5_THREADS, 1) l
         }
     }
     __syncthreads();
+    if (a.hstate) {                                                        // h(t0 + Tw - 1): the A buffer of step parity Tw
+        const uint8_t* hL = hbuf + (size_t)(tend & 1) * HBUF;
+        for (int i = tid; i < R5_ROWS * H / 8; i += R5_THREADS) {
+            const int r = i / (H / 8), u = (i % (H / 8)) * 8;
+            __stcg(reinterpret_cast<uint4*>(a.hstate + (size_t)(cta * R5_ROWS + r) * H + u),
+                   *reinterpret_cast<const uint4*>(hL + (u >> 6) * R5_ROWS * 128 + sw128_offset(r, u & 63)));
+        }
+    }
     cluster_sync_all();                                            // no CTA leaves while its peer may still arrive on its barriers
 }
 
@@ -299,7 +320,7 @@ static int r5_dispatch(const LstmTc5rLaunch& a, int grid, const R5Plan& p, cudaS
 }
 
 int launch_lstm_tc5r(const LstmTc5rLaunch& a, cudaStream_t s) {
-    if (!lstm_tc5r_supported(a.H, 2)) return (int)cudaErrorInvalidValue;
+    if (!lstm_tc5r_supported(a.H, 2) || a.Tw < 1 || a.t0 < 0 || a.t0 % 4 || a.t0 + a.Tw > a.Tp) return (int)cudaErrorInvalidValue;
     const R5Plan p = r5_plan(a.H);
     if (p.nstage < 2) return (int)cudaErrorInvalidValue;
     const int grid = (a.ntiles + 1) / 2 * 2 * (128 / R5_ROWS);    // whole clusters; the buffers cover the padded tile pair

@@ -17,6 +17,7 @@ SYMBOLS = [
     "fsn_version", "fsn_last_error", "fsn_model_create", "fsn_model_destroy", "fsn_model_set_param",
     "fsn_model_num_params", "fsn_model_param_info", "fsn_model_finalize", "fsn_model_forward",
     "fsn_model_forward_host", "fsn_model_forward_host_async", "fsn_model_sync_host", "fsn_model_submit", "fsn_model_wait", "fsn_model_forward_enhance", "fsn_model_submit_enhance", "fsn_model_forward_ragged", "fsn_model_forward_enhance_ragged", "fsn_model_last_lane", "fsn_model_wait_lane", "fsn_apply_cirm", "fsn_stream_create", "fsn_stream_step", "fsn_stream_destroy", "fsn_model_get_stage", "fsn_model_last_launch_count", "fsn_model_last_lstm_impl", "fsn_model_last_lstm_ms", "fsn_model_lstm_ms_history", "fsn_model_timeline",
+    "fsn_plan_forward", "fsn_model_workspace_bytes", "fsn_model_last_plan", "fsn_model_plan", "fsn_model_release_workspace",
     "fsn_sw128_offset", "fsn_tc5_weight_stream_bytes", "fsn_tc5_pack_weights", "fsn_tc5_gate_row", "fsn_tc5r_weight_stream_bytes", "fsn_tc5r_pack_layer",
 ]
 
@@ -83,6 +84,12 @@ def load_library():
     lib.fsn_model_last_lstm_ms.restype = C.c_float
     lib.fsn_model_lstm_ms_history.argtypes = [vp, fp, i32]
     lib.fsn_model_timeline.argtypes = [vp, fp, i32]
+    lib.fsn_plan_forward.argtypes = [C.POINTER(FsnConfig), i32, i32, C.c_double, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i64)]
+    lib.fsn_model_workspace_bytes.argtypes = [vp]
+    lib.fsn_model_workspace_bytes.restype = i64
+    lib.fsn_model_last_plan.argtypes = [vp, C.POINTER(i32), C.POINTER(i32)]
+    lib.fsn_model_plan.argtypes = [vp, i32, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i64)]
+    lib.fsn_model_release_workspace.argtypes = [vp]
     lib.fsn_sw128_offset.argtypes = [C.c_uint32, C.c_uint32]
     lib.fsn_sw128_offset.restype = C.c_uint32
     lib.fsn_tc5_weight_stream_bytes.argtypes = [i32, i32]
@@ -100,3 +107,25 @@ def load_library():
 def check(rc):
     if rc != 0:
         raise FsnError(f"fsnplus_b200 error {rc}: {load_library().fsn_last_error().decode()}")
+
+
+DEFAULT_WS_CAP = 24e9
+
+
+def ws_cap_bytes():
+    """The workspace cap of a model created now: FSN_WS_CAP_GB (GB, > 0) or the default 24 GB (read by fsn_model_create)."""
+    try:
+        v = float(os.environ.get("FSN_WS_CAP_GB", ""))
+    except ValueError:
+        return DEFAULT_WS_CAP
+    return v * 1e9 if v > 0 else DEFAULT_WS_CAP
+
+
+def plan_forward(cfg, B, T, cap_bytes=None, force_window=0):
+    """fsn_plan_forward: (clips per sub-batch, sub-band window in frames or 0, workspace bytes) of a plain forward of B clips of
+    T frames under the cap (default: ws_cap_bytes()).  Computed on the host from the configuration; needs no GPU."""
+    lib = load_library()
+    bs, tw, nb = C.c_int32(), C.c_int32(), C.c_int64()
+    cap = ws_cap_bytes() if cap_bytes is None else float(cap_bytes)
+    check(lib.fsn_plan_forward(C.byref(cfg), int(B), int(T), cap, int(force_window), C.byref(bs), C.byref(tw), C.byref(nb)))
+    return bs.value, tw.value, nb.value

@@ -332,6 +332,36 @@ class _B200Model(nn.Module):
     def last_launch_count(self):
         return int(_lib.load_library().fsn_model_last_launch_count(self._handle)) if self._handle else 0
 
+    def workspace_bytes(self):
+        """Bytes this model currently holds in forward workspaces (both lanes and the sub-band scratch; parameters excluded)."""
+        return int(_lib.load_library().fsn_model_workspace_bytes(self._handle)) if self._handle else 0
+
+    def last_plan(self):
+        """(clips per sub-batch, sub-band window in frames) of the last plain forward; window 0 = unwindowed."""
+        if not self._handle:
+            return (0, 0)
+        bs, tw = C.c_int32(), C.c_int32()
+        _lib.check(_lib.load_library().fsn_model_last_plan(self._handle, C.byref(bs), C.byref(tw)))
+        return (bs.value, tw.value)
+
+    def plan(self, B, T):
+        """(clips per sub-batch, sub-band window in frames or 0, workspace bytes) that this model's next plain forward of B clips of
+        T frames will use (C ABI: fsn_model_plan, with the FSN_* knobs the handle read at creation).  Creates the handle if needed, so
+        the model must be on its CUDA device; enqueues no GPU work."""
+        dev = next(self.parameters()).device
+        if dev.type != "cuda":
+            raise RuntimeError("plan() needs the model on its CUDA device (the plan is the handle's)")
+        with torch.cuda.device(dev):
+            lib = self._ensure_handle(dev)
+        bs, tw, nb = C.c_int32(), C.c_int32(), C.c_int64()
+        _lib.check(lib.fsn_model_plan(self._handle, int(B), int(T), C.byref(bs), C.byref(tw), C.byref(nb)))
+        return bs.value, tw.value, nb.value
+
+    def release_workspace(self):
+        """Free every forward workspace this model holds (synchronises the device); the next forward allocates again."""
+        if self._handle:
+            _lib.check(_lib.load_library().fsn_model_release_workspace(self._handle))
+
     def get_stage(self, name, shape, device):
         t = torch.empty(shape, dtype=torch.float32, device=device)
         stream = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)

@@ -115,23 +115,50 @@ def write_wav_int16(path, pcm, sr):
         w.writeframes(np.ascontiguousarray(pcm, dtype="<i2").tobytes())
 
 
-def bucket_by_length(lengths, batch_size):
-    """Indices grouped by identical length, each group cut into runs of at most batch_size; groups in order of first
-    appearance so the output order stays close to the directory order."""
+def _cut(idx, lengths, batch_size, max_samples):
+    """Runs of at most batch_size indices; with max_samples, a run is also cut before its total length would exceed
+    max_samples (a clip longer than that is a run of its own)."""
+    if max_samples is None:
+        return [idx[i:i + batch_size] for i in range(0, len(idx), batch_size)]
+    runs, cur, tot = [], [], 0
+    for i in idx:
+        n = int(lengths[i])
+        if cur and (len(cur) == batch_size or tot + n > max_samples):
+            runs.append(cur)
+            cur, tot = [], 0
+        cur.append(i)
+        tot += n
+    if cur:
+        runs.append(cur)
+    return runs
+
+
+def bucket_by_length(lengths, batch_size, max_samples=None):
+    """Indices grouped by identical length, each group cut into runs of at most batch_size (and, with max_samples, at most
+    max_samples samples of audio); groups in order of first appearance so the output order stays close to the directory order."""
     groups = {}
     for i, n in enumerate(lengths):
         groups.setdefault(int(n), []).append(i)
     batches = []
     for idx in groups.values():
-        batches += [idx[i:i + batch_size] for i in range(0, len(idx), batch_size)]
+        batches += _cut(idx, lengths, batch_size, max_samples)
     return batches
 
 
-def batch_by_sorted_length(lengths, batch_size):
-    """Indices sorted by length (stable: ties keep the directory order), cut into runs of at most batch_size: neighbouring
-    clips have similar lengths, which keeps the padding of a ragged batch small."""
+def batch_by_sorted_length(lengths, batch_size, max_samples=None):
+    """Indices sorted by length (stable: ties keep the directory order), cut into runs of at most batch_size (and, with
+    max_samples, at most max_samples samples of audio): neighbouring clips have similar lengths, which keeps the padding of a
+    ragged batch small."""
     order = sorted(range(len(lengths)), key=lambda i: int(lengths[i]))
-    return [order[i:i + batch_size] for i in range(0, len(order), batch_size)]
+    return _cut(order, lengths, batch_size, max_samples)
+
+
+def plan_is_windowed(model, batch, frames):
+    """True when the model's plain forward of `batch` clips of `frames` STFT frames will run its sub-band stage in time windows
+    (model.plan, the C ABI's fsn_plan_forward): such a forward takes the model's whole workspace cap.  Stand-in models without a
+    plan are never windowed."""
+    plan = getattr(model, "plan", None)
+    return plan is not None and plan(batch, frames)[1] > 0
 
 
 def build_model(model_config, checkpoint_path, device, trust_checkpoint=False):
@@ -153,11 +180,16 @@ def _rank_world():
 
 @torch.no_grad()
 def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=print, model_and_epoch=None, trust_checkpoint=False, streams=4,
-        ragged=False):
+        ragged=False, max_batch_seconds=None, replicas=None):
     """Enhance every file of config["dataset"]["args"]["dataset_dir_list"].  Under torchrun each rank takes every
     world-size-th batch (files are independent: no collective).  Returns {name: path} of the files this rank wrote.
     ``model_and_epoch`` (tests of the host logic) replaces the checkpoint load with a ready ``(callable, epoch)``.
-    ``ragged=True``: batches of clips of different lengths (length-sorted, ``batch_size`` clips each) through ``enhance_ragged``."""
+    ``ragged=True``: batches of clips of different lengths (length-sorted, ``batch_size`` clips each) through ``enhance_ragged``.
+    ``max_batch_seconds``: a batch is also cut before its total audio exceeds that many seconds (a longer clip goes alone).
+    A batch whose forward the model plans in time windows (a long clip: it uses the model's whole workspace cap) runs alone on the
+    first replica: every batch in flight is finished and every replica's workspaces are released first, and the first replica's
+    after it, so only one capped workspace exists at a time.
+    ``replicas`` (tests of the host logic, with ``model_and_epoch``): ready models for the replicas after the first."""
     rank, world, local_rank = _rank_world()
     if device is None:
         device = f"cuda:{local_rank}"
@@ -176,14 +208,25 @@ def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=pri
     # bucket on the lengths from the WAV headers; a rank decodes only the files of ITS batches, one batch at a time (host memory
     # and start-up time scale with the batch, not with the dataset -- the reference streams one clip at a time)
     lengths = [wav_length(p, ds_sr) for p in files]
-    batches = batch_by_sorted_length(lengths, batch_size) if ragged else bucket_by_length(lengths, batch_size)
+    max_samples = None if max_batch_seconds is None else max(1, int(max_batch_seconds * ds_sr))
+    batches = (batch_by_sorted_length(lengths, batch_size, max_samples=max_samples) if ragged
+               else bucket_by_length(lengths, batch_size, max_samples=max_samples))
     mine = [(bi, idx) for bi, idx in enumerate(batches) if bi % world == rank]
     # Ragged real recordings make many small batches (a lone clip fills a small fraction of the SMs): up to `streams`
     # batches are in flight at once, each on its own CUDA stream and its own model replica (own C handle and workspaces).
-    nstream = max(1, min(streams, len(mine))) if (on_gpu and model_and_epoch is None) else 1
-    models = [model] + [build_model(config["model"], Path(checkpoint_path).expanduser().absolute(), device, trust_checkpoint)[0]
-                        for _ in range(nstream - 1)]
-    cuda_streams = [torch.cuda.Stream(device) for _ in range(nstream)] if on_gpu else [None]
+    if replicas is not None:
+        nstream = max(1, min(streams, len(mine), 1 + len(replicas)))
+        models = [model] + list(replicas[:nstream - 1])
+    else:
+        nstream = max(1, min(streams, len(mine))) if (on_gpu and model_and_epoch is None) else 1
+        models = [model] + [build_model(config["model"], Path(checkpoint_path).expanduser().absolute(), device, trust_checkpoint)[0]
+                            for _ in range(nstream - 1)]
+    cuda_streams = [torch.cuda.Stream(device) for _ in range(nstream)] if on_gpu else [None] * nstream
+
+    def release_all(ms):
+        for m in ms:
+            if hasattr(m, "release_workspace"):
+                m.release_workspace()
     written, audio_s, inflight = {}, 0.0, []
     t_start = time.time()
 
@@ -202,9 +245,12 @@ def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=pri
             written[files[i].stem] = out
 
     for n, (bi, idx) in enumerate(mine):
-        k = n % nstream
-        if len(inflight) >= nstream:
+        alone = plan_is_windowed(models[0], len(idx), max(int(lengths[i]) for i in idx) // hop + 1)   # centred STFT frames
+        k = 0 if alone else n % nstream
+        while inflight and (alone or len(inflight) >= nstream):
             finish(inflight.pop(0))                                        # the batch that used this stream / replica last
+        if alone:
+            release_all(models)                                            # the windowed forward may take the whole cap
         if ragged:
             clips = [torch.from_numpy(read_wav(files[i], ds_sr)) for i in idx]
             audio_s += sum(c.numel() for c in clips) / sr
@@ -222,6 +268,9 @@ def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=pri
             else:
                 enh = H.enhance_ragged(models[k], clips, n_fft, hop, win, complex_inputs=INFERENCE_TYPES[itype])
                 inflight.append((bi, idx, [e.cpu() for e in enh], None, desc))
+            if alone:
+                finish(inflight.pop(0))
+                release_all(models[:1])
             continue
         noisy = torch.from_numpy(np.stack([read_wav(files[i], ds_sr) for i in idx]))
         audio_s += len(idx) * noisy.size(1) / sr
@@ -236,6 +285,9 @@ def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=pri
             inflight.append((bi, idx, host, ev, noisy.size(1)))
         else:
             inflight.append((bi, idx, H.enhance_batch(models[k], noisy, n_fft, hop, win, complex_inputs=INFERENCE_TYPES[itype]).cpu(), None, noisy.size(1)))
+        if alone:
+            finish(inflight.pop(0))                                        # nothing starts while the windowed batch holds its workspace
+            release_all(models[:1])
     while inflight:
         finish(inflight.pop(0))
     if audio_s > 0:
@@ -255,13 +307,15 @@ def main(argv=None):
     parser.add_argument("--streams", type=int, default=4, help="batches in flight at once, each on its own CUDA stream and model replica (additive)")
     parser.add_argument("--ragged", action="store_true",
                         help="batch clips of different lengths (sorted by length, --batch_size per batch) in one ragged model call (additive)")
+    parser.add_argument("--max_batch_seconds", type=float, default=None,
+                        help="also cut a batch before its total audio exceeds this many seconds; a longer clip goes alone (additive)")
     args = parser.parse_args(argv)
     configuration = load_toml(args.configuration)
     if len(args.dataset_dir_list) > 0:
         print(f"use specified dataset_dir_list: {args.dataset_dir_list}, instead of in config")
         configuration["dataset"]["args"]["dataset_dir_list"] = args.dataset_dir_list
     run(configuration, args.model_checkpoint_path, args.output_dir, batch_size=args.batch_size, trust_checkpoint=args.trust_checkpoint, streams=args.streams,
-        ragged=args.ragged)
+        ragged=args.ragged, max_batch_seconds=args.max_batch_seconds)
 
 
 if __name__ == "__main__":

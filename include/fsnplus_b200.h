@@ -202,6 +202,40 @@ int fsn_model_timeline(fsn_model* m, float* h_ms4, int32_t n);
 /* Which implementation the last forward used for the sub-band model (FSN_LSTM_MMA / _TCGEN05 / _TCN). */
 int fsn_model_last_lstm_impl(const fsn_model* m);
 
+/* Long clips (DESIGN.md §3.7).  The plain entry points (fsn_model_forward, _enhance, both _ragged ones, fsn_model_forward_host) plan
+ * every call so that its forward workspace stays within FSN_WS_CAP_GB (default 24): a batch that fits runs whole or as equal
+ * sub-batches, exactly as before; when one sub-batch would still exceed the cap, the layer-wise sub-band LSTM runs in time windows
+ * of Tw frames (a multiple of 32), carrying h and c exactly from one window to the next, so the result is bit-identical to the
+ * unwindowed forward and the sub-band memory is O(Tw).  Everything that needs the whole utterance (norms, attention pooling, the
+ * full-band model, the sub-band statistics) stays whole-clip at about 26 KB per frame (FullSubNet+) or 41 KB (fullsubnet.Model).
+ * FSN_SB_WINDOW=<frames> (a positive multiple of 32, read at fsn_model_create, else FSN_EINVAL) forces windows of that length.
+ * Windows apply to the layer-wise path only: the sub-band TCN, lstm_impl = FSN_LSTM_MMA and the pipelined entry points run unwindowed.
+ * Length limits (FSN_EINVAL naming the limit, from every forward entry point and fsn_plan_forward): T + look_ahead <= 16 776 960
+ * frames (65535 x 256, the TCN depth-wise convolution's grid), num_freqs x (T + look_ahead) <= 2^31 - 1 (the per-clip plane index), and
+ * for FullSubNet+ 3 x B x (T + look_ahead) + 128 <= 2^31 - 1 (the full-band TCN's rows; the planner keeps sub-batches below it).  At
+ * num_freqs = 257 that is 8 355 967 frames, about 37 hours at 16 kHz / hop 256.  Memory binds first: the whole-clip part, ~26 KB
+ * (FullSubNet+) / ~40 KB (fullsubnet.Model) per frame, leaves room in the 24 GB default cap for one clip of up to 4.0 / 2.6 hours
+ * (T = 915 689 / 599 084, windows then down to 32 frames); a longer clip runs with 256-frame windows and allocates past the cap.  A 2-hour
+ * clip (T = 450 000) plans 6016- / 2944-frame windows within the default cap; the sub-band TCN keeps its B * num_freqs * (T + look_ahead)
+ * < 2^31 row limit.
+ * After a windowed forward the model holds at most the plan's bytes: it first gives back whatever earlier forwards grew beyond them.
+ *
+ * fsn_plan_forward: the plan, from the configuration alone (its lstm_impl; no environment knob), for B clips of T frames under
+ * cap_bytes: *Bs clips per sub-batch, *Tw frames per window (0: unwindowed), *bytes (may be NULL) the workspace it requests.
+ * force_window: 0, or the FSN_SB_WINDOW value.  No GPU needed. */
+int fsn_plan_forward(const fsn_config* cfg, int32_t B, int32_t T, double cap_bytes, int32_t force_window, int32_t* Bs, int32_t* Tw,
+                     int64_t* bytes);
+/* Bytes the model currently holds in forward workspaces: both lanes plus the sub-band scratch (parameters and host-entry staging excluded). */
+int64_t fsn_model_workspace_bytes(const fsn_model* m);
+/* Plan of the last plain forward: sub-batch and window (Tw = 0: unwindowed). */
+int fsn_model_last_plan(const fsn_model* m, int32_t* Bs, int32_t* Tw);
+/* The plan the model's next plain forward of B clips of T frames will use: fsn_plan_forward with the knobs the model read at create
+ * (FSN_WS_CAP_GB, FSN_SB_WINDOW, FSN_LSTM_IMPL).  Host only; enqueues nothing. */
+int fsn_model_plan(const fsn_model* m, int32_t B, int32_t T, int32_t* Bs, int32_t* Tw, int64_t* bytes);
+/* Synchronises the device and frees every forward workspace of the model (fsn_model_workspace_bytes drops to 0); the next forward
+ * allocates what it needs again.  For callers that keep several models and run a capped (windowed) forward on one of them. */
+int fsn_model_release_workspace(fsn_model* m);
+
 /* Host-side packers exposed for CPU tests of the kernel layouts (no GPU needed). */
 /* 128-row x 64-half tile with the SWIZZLE_128B layout: byte offset of element (row, k). */
 uint32_t fsn_sw128_offset(uint32_t row, uint32_t k);

@@ -93,13 +93,13 @@ struct fsn_model {
     // (B, T).  TWO lanes: the pipelined entry points (fsn_model_submit / fsn_model_forward_host_async) run the front end of
     // batch i+1 in lane (i+1)&1 on the front stream while the sub-band LSTM of batch i still reads lane i&1 on the LSTM stream.
     struct Lane {
-        int wsB = 0, wsT = 0, wsTw = 0;                // wsTw: sub-band window of the last geometry (0: whole clip)
+        int wsB = 0, wsT = 0, wsTw = 0, wsFc = 0;      // wsTw / wsFc: sub-band window / bin chunk of the last geometry (0: whole clip / all bins)
         DevBuf fbin, fbout, mu, ximg, magpad, fbx, hseq;
         DevBuf x0, xr;                                 // time-major fb input / relu'd last residual
         TcnScratch tcn;                                // the full-band TCN's blocks (written on the front stream)
         DevBuf tsse_scale, sb_rowsum;
         DevBuf xn, sigma;                              // pre-normalised inputs / sub-band std for the non-default norm types
-        DevBuf sbx;                                    // sub-band TCN: input [B*F*T', 64] fp32 time-major | max |x| per sequence [B*F]
+        DevBuf sbx;                                    // sub-band TCN: input [B*Fc*T', 64] fp32 time-major | max |x| per sequence [B*Fc] (Fc = F unchunked)
         DevBuf tlen;                                   // ragged forwards: per-sample extent frames[b] + look_ahead as int32 [3][B] (clip_len)
         alignas(64) unsigned char mapX0[128], mapXr[128], mapSbx[128];
         cudaEvent_t ev_front = nullptr, ev_lstm = nullptr;   // front end written / LSTM finished reading this lane
@@ -135,7 +135,9 @@ struct fsn_model {
     int env_pdl = -1;                                  // FSN_PDL: 0 / 1 / -1 (auto: small batches only)
     double ws_cap_bytes = 24e9;                        // FSN_WS_CAP_GB: larger batches are run as sub-batches (plain forward entry points)
     int env_sb_window = 0;                             // FSN_SB_WINDOW: force a sub-band time window of this many frames (multiple of 32)
-    int plan_Bs = 0, plan_Tw = 0;                      // plan of the last plain forward (fsn_plan_forward): sub-batch, window (0: whole clip)
+    int env_sb_chunk = 0;                              // FSN_SB_CHUNK: run the sub-band TCN in chunks of this many bins (>= num_freqs: unchunked)
+    int plan_Bs = 0, plan_Tw = 0, plan_Fc = 0;         // plan of the last plain forward (fsn_plan_forward_bins): sub-batch, window (0: whole
+                                                       // clip), bin chunk (0: all bins)
     bool env_no_ws = false;
     // pipelined execution: front-end stream, LSTM stream (higher priority), copy-in / copy-out streams, per-slot events
     cudaStream_t s_front = nullptr, s_lstm = nullptr, s_in = nullptr, s_out = nullptr;
@@ -449,11 +451,19 @@ extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
         if (*end || w < 32 || w % 32 || w > (1L << 30)) return fail(FSN_EINVAL, "FSN_SB_WINDOW=%s: the window must be a positive multiple of 32 frames", e);
         sb_window = (int)w;
     }
+    int sb_chunk = 0;
+    if (const char* e = getenv("FSN_SB_CHUNK"); e && *e) {
+        char* end = nullptr;
+        const long w = strtol(e, &end, 10);
+        if (*end || w < 1) return fail(FSN_EINVAL, "FSN_SB_CHUNK=%s: the chunk must be a positive number of bins", e);
+        sb_chunk = w < c.num_freqs ? (int)w : c.num_freqs;
+    }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(FSN_ECUDA, "no CUDA device: fsnplus_b200 has no CPU fallback");
     fsn_model* m = new fsn_model();
     m->cfg = c;
     m->env_sb_window = sb_window;
+    m->env_sb_chunk = sb_chunk;
     { const char* e = getenv("FSN_LSTM_IMPL"); if (e && *e) m->env_impl = atoi(e); }
     { const char* e = getenv("FSN_NO_WS"); m->env_no_ws = e && atoi(e) != 0; }
     { const char* e = getenv("FSN_FRONT_OVERLAP"); m->env_front_overlap = e && atoi(e) != 0; }
@@ -635,8 +645,8 @@ static bool config_layerwise(const fsn_config& c, int env_impl) {
 }
 
 // Bytes of every forward workspace buffer ensure_ws requests for a batch of B clips of T frames, the sub-band images and the layer-wise
-// path's Gin / layer output sized by the window Tw (0: the whole clip).  ensure_ws allocates exactly these sizes, so the planner's count
-// (fsn_plan_forward) is what a forward asks for.
+// path's Gin / layer output sized by the window Tw (0: the whole clip), the sub-band TCN's input and scratch by the bin chunk Fc (0: all
+// bins).  ensure_ws allocates exactly these sizes, so the planner's count (fsn_plan_forward_bins) is what a forward asks for.
 struct WsSizes {
     size_t act = 0, mu = 0, tsse = 0, rowsum = 0, xn = 0;      // lane: fbin / fbout, mu / sigma, TSSE scale + row statistics, row sums, norms
     size_t sbx = 0, ximg = 0;                                   // lane: sub-band TCN input, or the sub-band images
@@ -650,7 +660,7 @@ struct WsSizes {
                gin + hseq + hstate + cum + 2 * sb_x + 2 * sb_y + sb_stats + tlen + wsh;
     }
 };
-static WsSizes ws_sizes(const fsn_config& c, bool layerwise, int B, int T, int Tw) {
+static WsSizes ws_sizes(const fsn_config& c, bool layerwise, int B, int T, int Tw, int Fc = 0) {
     WsSizes z;
     const int F = c.num_freqs, Tp = T + c.look_ahead, Pp = (Tp + 3) & ~3, Ts = Tw ? Tw : Tp;
     const int nbr = (c.model_kind == FSN_KIND_PLUS) ? 3 : 1;
@@ -662,9 +672,9 @@ static WsSizes ws_sizes(const fsn_config& c, bool layerwise, int B, int T, int T
     z.tlen = (size_t)3 * B * sizeof(int32_t);                  // counted whether the forward is ragged or not
     if (c.norm_type != FSN_NORM_OFFLINE_LAPLACE) z.xn = (size_t)nbr * B * F * Tp * 4;
     if (c.sb_tcn) {
-        const size_t srows = rows * Tp;
-        z.sbx = srows * 64 * 4 + rows * 4;
-        z.sb_x = srows * 64 * 4; z.sb_y = srows * 512 * sizeof(__half); z.sb_stats = tcn_stats_bytes(rows);
+        const size_t seqs = (size_t)B * (Fc ? Fc : F), srows = seqs * Tp;  // the sequences of one chunk run
+        z.sbx = srows * 64 * 4 + seqs * 4;
+        z.sb_x = srows * 64 * 4; z.sb_y = srows * 512 * sizeof(__half); z.sb_stats = tcn_stats_bytes(seqs);
     } else {
         z.ximg = ntiles * Ts * 16384;
     }
@@ -703,7 +713,9 @@ static WsSizes ws_sizes(const fsn_config& c, bool layerwise, int B, int T, int T
 // Length limits of one forward (B clips of T frames), from the 32-bit quantities of the kernels on every path: the depth-wise TCN
 // convolution's grid covers T' in blocks of 256 frames along gridDim.y (<= 65535); the cIRM passes index one clip's F x T' plane with
 // an int; the full-band TCN GEMMs address their 3 B T' time-major rows (+ one 128-row tile) with int row indices and int32 tensor-map
-// coordinates.  Every element offset beyond these is 64-bit.  The sub-band TCN's B F T' row limit is checked with its workspace.
+// coordinates.  Every element offset beyond these is 64-bit.  The sub-band TCN's B Fc T' row limit per chunk run (SB_MAX_ROWS) is kept by
+// the planner and checked with its workspace.
+static const long long SB_MAX_ROWS = 0x7fffffffLL - 128;
 static const long long FSN_MAX_TP = 65535LL * 256;
 static long long max_clips_for_rows(const fsn_config& c, int T) {
     return c.model_kind == FSN_KIND_PLUS ? (0x7fffffffLL - 128) / (3LL * (T + c.look_ahead)) : 0x7fffffffLL;
@@ -718,22 +730,26 @@ static int check_length(const fsn_config& c, int B, int T) {
     return FSN_OK;
 }
 
-static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, int Tw, cudaStream_t s, cudaStream_t sl) {
+static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, int Tw, int Fc, cudaStream_t s, cudaStream_t sl) {
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs, Tp = T + c.look_ahead;
-    const WsSizes z = ws_sizes(c, use_layerwise(m), B, T, Tw);
-    const bool regeo = (ln.wsB != B || ln.wsT != T || ln.wsTw != Tw);
-    if (Tw) {
-        // A windowed forward exists to bound the workspace: first give back what earlier, longer or unwindowed forwards grew beyond this
-        // one's need (the grow-only buffers of both lanes and the sub-band scratch), so the model then holds at most the plan's bytes.
+    const WsSizes z = ws_sizes(c, use_layerwise(m), B, T, Tw, Fc);
+    const bool regeo = (ln.wsB != B || ln.wsT != T || ln.wsTw != Tw || ln.wsFc != Fc);
+    if (Tw || Fc) {
+        // A windowed or bin-chunked forward exists to bound the workspace: first give back what earlier, longer, unwindowed or wider
+        // forwards grew beyond this one's need (the grow-only buffers of both lanes and the sub-band scratch), so the model then holds at
+        // most the plan's bytes.
         // The buffers a new geometry releases anyway (images, x0 / xr, the TCN scratch) are left to that rule.
         auto fit = [](DevBuf& b, size_t need) { if (b.bytes > need) b.release(); };
         fit(ln.fbin, z.act); fit(ln.fbout, z.act); fit(ln.mu, z.mu); fit(ln.sigma, z.mu); fit(ln.tsse_scale, z.tsse);
         fit(ln.sb_rowsum, z.rowsum); fit(ln.xn, z.xn); fit(ln.tlen, z.tlen); fit(ln.magpad, z.magpad); fit(ln.fbx, z.fbx); fit(ln.hseq, z.fbhseq);
         fit(m->r_gin, z.gin); fit(m->r_hseq, z.hseq); fit(m->r_hstate, z.hstate); fit(m->sb_cum, z.cum); fit(m->cstate, z.cstate);
-        m->mask_tmp.release(); m->sb_scratch.release();
+        m->mask_tmp.release();
+        const TcnScratch& sc = m->sb_scratch;                            // released whole: its tensor maps go with its buffers
+        if (sc.xa.bytes > z.sb_x || sc.xb.bytes > z.sb_x || sc.y1.bytes > z.sb_y || sc.y2.bytes > z.sb_y || sc.stats.bytes > z.sb_stats)
+            m->sb_scratch.release();
         fsn_model::Lane& other = m->lane[&ln == &m->lane[0] ? 1 : 0];    // the pipelined entry points' second lane
-        other.release_all(); other.wsB = other.wsT = other.wsTw = 0;
+        other.release_all(); other.wsB = other.wsT = other.wsTw = other.wsFc = 0;
     }
     int e = 0;
     e |= ln.fbin.ensure(z.act, true, s);
@@ -745,14 +761,16 @@ static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, int Tw, cu
     if (z.xn) e |= ln.xn.ensure(z.xn, true, s);
     if (c.sb_tcn) {
         // sub-band TCN: the lane's packed input (+ block 0's stream maxima), the shared scratch of the blocks (serialised on the sub-band
-        // stream like the LSTM scratch); every buffer is fully written before it is read (the pad columns by the packer / the epilogue)
-        const long long srows = (long long)B * F * Tp;
-        if (srows + 128 > 0x7fffffffLL) return fail(FSN_EINVAL, "B * num_freqs * (T + look_ahead) = %lld rows exceeds the sub-band TCN's 2^31 limit", srows);
+        // stream like the LSTM scratch); every buffer is fully written before it is read (the pad columns by the packer / the epilogue).
+        // A chunked forward sizes them for one chunk of Fc bins; a narrower last chunk leaves the rows past its own unread.
+        const long long seqs = (long long)B * (Fc ? Fc : F), srows = seqs * Tp;
+        if (srows > SB_MAX_ROWS)
+            return fail(FSN_EINVAL, "B * %s * (T + look_ahead) = %lld rows exceeds the sub-band TCN's 2^31 limit", Fc ? "bins per chunk" : "num_freqs", srows);
         if (regeo) ln.sbx.release();
         e |= ln.sbx.ensure(z.sbx, false, s);
         if (e) return fail(FSN_ECUDA, "workspace allocation failed for B=%d T=%d", B, T);
         if (regeo && make_tmap_f32_2d(ln.mapSbx, ln.sbx.p, srows, 64, 128)) return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the sub-band input");
-        int rc = grow_tcn_scratch(m->sb_scratch, m->tcn_sb, srows, (size_t)B * F, false, sl);
+        int rc = grow_tcn_scratch(m->sb_scratch, m->tcn_sb, srows, (size_t)seqs, false, sl);
         if (rc) return rc;
     } else {
         // images are re-zeroed whenever the geometry changes (rows beyond B*F and k >= I must stay zero)
@@ -787,7 +805,7 @@ static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, int Tw, cu
         e |= ln.hseq.ensure(z.fbhseq, true, s);
     }
     if (e) return fail(FSN_ECUDA, "workspace allocation failed for B=%d T=%d", B, T);
-    ln.wsB = B; ln.wsT = T; ln.wsTw = Tw;
+    ln.wsB = B; ln.wsT = T; ln.wsTw = Tw; ln.wsFc = Fc;
     return FSN_OK;
 }
 
@@ -941,19 +959,34 @@ static int run_tcn_blocks(fsn_model* m, const TcnWeights& w, TcnScratch& sc, con
 // The sub-band TCN (sequence_model = "TCN", fullsubnet_plus.py:102-110): the TCN blocks with one branch, the B*F sequences of the sub-band
 // input as the gLN groups and Isb (<= 64) channels in one 64-column N tile; the last block's second 1x1 convolution ends in ReLU + Linear +
 // activation (EPI5_GLN_HEAD) and writes the mask -- or, with d_enh, the enhanced spectrum.
-static int run_sb_tcn(fsn_model* m, fsn_model::Lane& ln, int B, int T, float* d_out, const float* d_real, const float* d_imag, float* d_enh,
-                      const int* tlen, cudaStream_t s) {
+// Fc > 0: the sequences run in chunks of Fc bins (the last one narrower), each packed here from the front end's whole-clip outputs (`sp`,
+// the front end's packer arguments) into the same buffers; every sequence is its own gLN group, so nothing carries from one chunk to the
+// next (DESIGN.md §3.8).  Fc = 0: the input of all bins is already packed and the blocks run once.
+static int run_sb_tcn(fsn_model* m, fsn_model::Lane& ln, int B, int T, int Fc, SbPackLaunch sp, float* d_out, const float* d_real,
+                      const float* d_imag, float* d_enh, const int* tlen, cudaStream_t s) {
     const fsn_config& c = m->cfg;
-    const int F = c.num_freqs, Tp = T + c.look_ahead, Z = B * F;
+    const int F = c.num_freqs, Tp = T + c.look_ahead, W = Fc ? Fc : F;
     m->last_impl = FSN_LSTM_TCN;
-    CK(cudaMemsetAsync(m->sb_scratch.stats.p, 0, tcn_stats_bytes(Z), s));
     GemmTc5Launch head{};
     head.epi = EPI5_GLN_HEAD;
     head.fc_w = static_cast<const float*>(m->sb_fc.p); head.fc_b = P(m, "sb_model.fc_output_layer.bias");
     head.O = c.output_size; head.la = c.look_ahead; head.F = F; head.act = c.sb_act;
     head.out = d_out; head.nreal = d_real; head.nimag = d_imag; head.enh = reinterpret_cast<float2*>(d_enh);
-    const float* x = static_cast<const float*>(ln.sbx.p);
-    return run_tcn_blocks(m, m->tcn_sb, m->sb_scratch, x, ln.mapSbx, x + (size_t)Z * Tp * 64, Z, Tp, false, head, tlen, F, s);
+    float* x = static_cast<float*>(ln.sbx.p);
+    float* amax0 = x + (size_t)B * W * Tp * 64;
+    for (int f0 = 0; f0 < F; f0 += W) {
+        const int fc = F - f0 < W ? F - f0 : W, Z = B * fc;
+        if (Fc) {
+            sp.xtm = x; sp.amax = amax0; sp.f0 = f0; sp.Fc = fc;
+            launch_sb_pack_tm(sp, s);
+            m->launches++;
+        }
+        CK(cudaMemsetAsync(m->sb_scratch.stats.p, 0, tcn_stats_bytes(Z), s));
+        head.Fg = fc; head.f0 = f0;
+        int rc = run_tcn_blocks(m, m->tcn_sb, m->sb_scratch, x, ln.mapSbx, amax0, Z, Tp, false, head, tlen, fc, s);
+        if (rc) return rc;
+    }
+    return FSN_OK;
 }
 
 // The whole forward.  Front end (norm, attention, full-band model, sub-band statistics + packing) on stream `s` into lane `ln`;
@@ -983,8 +1016,9 @@ static int stage_lengths(fsn_model* m, fsn_model::Lane& ln, const int32_t* h_fra
 
 // h_frames: the frame count of every sample of a ragged batch (validated by the caller), or null when every sample spans T frames
 // Tw: time window of the sub-band stage (0: the whole clip; > 0 needs s == sl, the plain entry points)
+// Fc: bin chunk of the sub-band TCN (0: all bins at once; > 0 needs s == sl, the plain entry points)
 static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
-                        const int32_t* h_frames, float* d_out, float* d_enh, cudaStream_t s, cudaStream_t sl, int Tw = 0) {
+                        const int32_t* h_frames, float* d_out, float* d_enh, cudaStream_t s, cudaStream_t sl, int Tw = 0, int Fc = 0) {
     if (!m || !d_mag || (!d_out && !d_enh)) return fail(FSN_EINVAL, "null argument");
     if (d_enh && (!d_real || !d_imag)) return fail(FSN_EINVAL, "the enhanced-spectrum output needs the noisy real and imaginary planes");
     if (d_enh && m->cfg.output_size != 2) return fail(FSN_EINVAL, "the enhanced-spectrum output needs output_size 2 (a complex mask)");
@@ -1001,7 +1035,7 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
             if (Tp < c.kersize[i]) return fail(FSN_EINVAL, "sequence shorter than the TSSE kernel size");
     int rc = check_length(c, B, T);
     if (rc) return rc;
-    rc = ensure_ws(m, ln, B, T, Tw, s, sl);
+    rc = ensure_ws(m, ln, B, T, Tw, Fc, s, sl);
     if (rc) return rc;
     const int* tl = nullptr;                                            // per-sample extents on the device (null: all Tp)
     if (h_frames) {
@@ -1025,6 +1059,7 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
     sp.t0 = 0; sp.Tw = Tp;
     sp.cum = Tw ? static_cast<double*>(m->sb_cum.p) : nullptr;
     sp.tlen = tl;
+    sp.f0 = 0; sp.Fc = F;
 
     if (c.model_kind == FSN_KIND_PLUS) {
         const char* sfx[3] = {"", "_real", "_imag"};
@@ -1140,10 +1175,12 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
     }
     launch_sb_stats(sp, s); m->launches += 2;
     if (c.sb_tcn) {
-        sp.xtm = static_cast<float*>(ln.sbx.p);
-        sp.amax = sp.xtm + (size_t)B * F * Tp * 64;
-        launch_sb_pack_tm(sp, s);
-        m->launches++;
+        if (!Fc) {                                                      // chunked: run_sb_tcn packs each chunk
+            sp.xtm = static_cast<float*>(ln.sbx.p);
+            sp.amax = sp.xtm + (size_t)B * F * Tp * 64;
+            launch_sb_pack_tm(sp, s);
+            m->launches++;
+        }
     } else if (!Tw) {                                                   // windowed: run_sb_lstm packs each window
         launch_sb_pack(sp, s);
         m->launches++;
@@ -1154,7 +1191,8 @@ static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, c
         CK(cudaStreamWaitEvent(sl, ln.ev_front, 0));
     }
     cudaEventRecord(m->ev0[evi], sl);
-    rc = c.sb_tcn ? run_sb_tcn(m, ln, B, T, d_out, d_real, d_imag, d_enh, tl, sl) : run_sb_lstm(m, ln, B, T, Tw, sp, d_out, d_real, d_imag, d_enh, tl, sl);
+    rc = c.sb_tcn ? run_sb_tcn(m, ln, B, T, Fc, sp, d_out, d_real, d_imag, d_enh, tl, sl)
+                  : run_sb_lstm(m, ln, B, T, Tw, sp, d_out, d_real, d_imag, d_enh, tl, sl);
     cudaEventRecord(m->ev1[evi], sl);
     if (rc) return rc;
     m->nfwd++;
@@ -1221,14 +1259,22 @@ static double ws_bytes_per_sample(const fsn_config& c, bool layerwise, int T) {
     return b;
 }
 
-// The plan of a plain forward (fsn_plan_forward): sub-batch Bs and sub-band window Tw (0: whole clip) so that the exact workspace
-// (ws_sizes) stays within cap.
+// The plan of a plain forward (fsn_plan_forward_bins): sub-batch Bs, sub-band window Tw (0: whole clip) and, for the sub-band TCN, bin
+// chunk Fc (0: all bins) so that the exact workspace (ws_sizes) stays within cap.
 //   * the sub-batch of the per-sample estimate, if it fits unwindowed: the forward of every release before windows existed;
 //   * else (layer-wise path only) the largest sub-batch that fits with a window of 256 frames (32 if none does), then the longest window
 //     (a multiple of 32) that fits, evened out over the same number of windows; more sequences in flight keep more SMs busy;
 //   * nothing fits: one clip at a time with a 256-frame window, allocated anyway.
 // force > 0 (FSN_SB_WINDOW) windows every layer-wise forward with exactly that window.  Sub-batches are equal splits of B.
-static void plan_forward(const fsn_config& c, bool layerwise, int B, int T, double cap, int force, int* pBs, int* pTw, int64_t* pbytes) {
+// The sub-band TCN is never windowed (every gLN spans a whole sequence) but runs in bin chunks (DESIGN.md §3.8):
+//   * the sub-batch of the per-sample estimate, if it fits unchunked: the forward before chunks existed;
+//   * else, over every equal split Bs, the widest chunk that fits, evened out over the same number of chunks; the plan with the fewest
+//     chunk runs ceil(B / Bs) * ceil(F / Fc) wins, ties to the larger Bs (Fc = F, unchunked, is a candidate);
+//   * nothing fits: one clip at a time in one-bin chunks, allocated anyway.
+// Every chunk run keeps Bs * Fc * T' <= SB_MAX_ROWS.  force_bins > 0 (FSN_SB_CHUNK) chunks every TCN forward with exactly that many bins
+// (>= F: unchunked) and the largest equal split that fits with them.
+static void plan_forward(const fsn_config& c, bool layerwise, int B, int T, double cap, int force, int force_bins, int* pBs, int* pTw,
+                         int* pFc, int64_t* pbytes) {
     const int Tp = T + c.look_ahead, wmax = (Tp + 31) / 32 * 32;
     const long long blim = max_clips_for_rows(c, T);             // sub-batches never exceed the full-band TCN's row limit
     auto split = [&](int bmax) { if (bmax > blim) bmax = (int)blim; if (bmax < 1) bmax = 1; if (B <= bmax) return B; const int n = (B + bmax - 1) / bmax; return (B + n - 1) / n; };
@@ -1241,8 +1287,40 @@ static void plan_forward(const fsn_config& c, bool layerwise, int B, int T, doub
     };
     const double per = ws_bytes_per_sample(c, layerwise, T);
     const double bmax = cap / (per > 1 ? per : 1);
-    int Bs = split(bmax < B ? (int)bmax : B), Tw = 0;
-    if (layerwise && force > 0) {
+    int Bs = split(bmax < B ? (int)bmax : B), Tw = 0, Fc = 0;
+    if (c.sb_tcn) {
+        const int F = c.num_freqs;
+        auto fits = [&](int bs, int fc) { return (long long)bs * fc * Tp <= SB_MAX_ROWS && ws_sizes(c, false, bs, T, 0, fc < F ? fc : 0).total() <= cap; };
+        const int fforce = force_bins > 0 ? (force_bins < F ? force_bins : F) : 0;
+        if (fforce < F && (fforce > 0 || !fits(Bs, F))) {
+            if (fforce) {
+                int lo = 0, hi = B;                                     // largest equal split that fits with fforce bins
+                while (lo < hi) { const int mid = (lo + hi + 1) / 2; if (fits(split(mid), fforce)) lo = mid; else hi = mid - 1; }
+                Bs = lo ? split(lo) : 1; Fc = fforce;
+            } else {
+                long long best = -1;
+                Bs = 1; Fc = 1;
+                for (int n = 1, prev = 0; n <= B; ++n) {                // the equal splits, largest first
+                    const int bs = (B + n - 1) / n;
+                    if (bs == prev || bs > blim) continue;
+                    prev = bs;
+                    int lo = 0, hi = F;                                 // widest chunk that fits
+                    while (lo < hi) { const int mid = (lo + hi + 1) / 2; if (fits(bs, mid)) lo = mid; else hi = mid - 1; }
+                    if (!lo) continue;
+                    const int nch = (F + lo - 1) / lo;
+                    const long long runs = (long long)((B + bs - 1) / bs) * nch;
+                    if (best < 0 || runs < best) { best = runs; Bs = bs; Fc = (F + nch - 1) / nch; }
+                }
+            }
+            if (Fc >= F) Fc = 0;
+        } else if (fforce == F) {
+            int lo = 0, hi = B;                                         // FSN_SB_CHUNK >= F: unchunked, largest equal split that fits
+            if (!fits(Bs, F)) {
+                while (lo < hi) { const int mid = (lo + hi + 1) / 2; if (fits(split(mid), F)) lo = mid; else hi = mid - 1; }
+                Bs = lo ? split(lo) : 1;
+            }
+        }
+    } else if (layerwise && force > 0) {
         Tw = force;
         const int b = max_split(Tw);
         Bs = b ? b : 1;
@@ -1264,8 +1342,8 @@ static void plan_forward(const fsn_config& c, bool layerwise, int B, int T, doub
             Tw = ((Tp + nwin - 1) / nwin + 31) / 32 * 32;
         }
     }
-    *pBs = Bs; *pTw = Tw;
-    if (pbytes) *pbytes = (int64_t)bytes(Bs, Tw);
+    *pBs = Bs; *pTw = Tw; *pFc = Fc;
+    if (pbytes) *pbytes = (int64_t)ws_sizes(c, layerwise, Bs, T, Tw, Fc).total();
 }
 
 static int forward_plain(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
@@ -1278,14 +1356,15 @@ static int forward_plain(fsn_model* m, const float* d_mag, const float* d_real, 
         if (ln.used) CK(cudaStreamWaitEvent(s, ln.ev_lstm, 0));
     // Samples are independent, so a batch whose workspace would exceed the cap (FSN_WS_CAP_GB, default 24 of the 80 GB) is run as
     // equal sub-batches one after the other on the same stream -- same results, bounded memory (e.g. 256 clips on the layer-wise path);
-    // a clip too long for the cap runs its sub-band stage in time windows (plan_forward) -- same bits, O(window) sub-band memory.
+    // a clip too long for the cap runs its sub-band stage in time windows (plan_forward) -- same bits, O(window) sub-band memory --
+    // or, with the sub-band TCN, in bin chunks -- O(chunk) sub-band memory.
     if (int rc = check_length(m->cfg, 1, T)) return rc;
-    int Bs = B, Tw = 0;
-    plan_forward(m->cfg, use_layerwise(m), B, T, m->ws_cap_bytes, m->env_sb_window, &Bs, &Tw, nullptr);
-    m->plan_Bs = Bs; m->plan_Tw = Tw;
+    int Bs = B, Tw = 0, Fc = 0;
+    plan_forward(m->cfg, use_layerwise(m), B, T, m->ws_cap_bytes, m->env_sb_window, m->env_sb_chunk, &Bs, &Tw, &Fc, nullptr);
+    m->plan_Bs = Bs; m->plan_Tw = Tw; m->plan_Fc = Fc;
     int rc = FSN_OK;
     if (Bs >= B) {
-        rc = forward_impl(m, m->lane[0], d_mag, d_real, d_imag, B, T, h_frames, d_out, d_enh, s, s, Tw);
+        rc = forward_impl(m, m->lane[0], d_mag, d_real, d_imag, B, T, h_frames, d_out, d_enh, s, s, Tw, Fc);
     } else {
         const size_t in_stride = (size_t)m->cfg.num_freqs * T, out_stride = (size_t)m->cfg.output_size * m->cfg.num_freqs * T;
         int64_t launches = 0;
@@ -1293,7 +1372,7 @@ static int forward_plain(fsn_model* m, const float* d_mag, const float* d_real, 
             const int nb = (B - b0 < Bs) ? B - b0 : Bs;
             rc = forward_impl(m, m->lane[0], d_mag + b0 * in_stride, d_real ? d_real + b0 * in_stride : nullptr, d_imag ? d_imag + b0 * in_stride : nullptr,
                               nb, T, h_frames ? h_frames + b0 : nullptr, d_out ? d_out + b0 * out_stride : nullptr,
-                              d_enh ? d_enh + b0 * in_stride * 2 : nullptr, s, s, Tw);
+                              d_enh ? d_enh + b0 * in_stride * 2 : nullptr, s, s, Tw, Fc);
             launches += m->launches;
         }
         m->launches = launches;
@@ -1485,6 +1564,7 @@ extern "C" int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst,
     }
     if (n == "sb_in") {
         if (!c.sb_tcn) return fail(FSN_EINVAL, "sb_in is kept only by the sub-band TCN (sequence_model = \"TCN\")");
+        if (ln.wsFc) return fail(FSN_ESTATE, "sb_in is not kept: the last forward was chunked over bins (%d per chunk), its buffer holds the last chunk only", ln.wsFc);
         if (numel != (int64_t)B * F * m->Isb * Tp) return fail(FSN_EINVAL, "sb_in needs %lld elements", (long long)B * F * m->Isb * Tp);
         launch_tm_to_fm(static_cast<const float*>(ln.sbx.p), 64, d_dst, B * F, m->Isb, Tp, s);
         CK(cudaGetLastError());
@@ -1648,31 +1728,43 @@ extern "C" float fsn_model_last_lstm_ms(fsn_model* m) {
 }
 extern "C" int fsn_model_last_lstm_impl(const fsn_model* m) { return m ? m->last_impl : 0; }
 
-extern "C" int fsn_plan_forward(const fsn_config* cfg, int32_t B, int32_t T, double cap_bytes, int32_t force_window, int32_t* Bs, int32_t* Tw,
-                                int64_t* bytes) {
-    if (!cfg || !Bs || !Tw || B < 1 || T < 1 || !(cap_bytes > 0)) return fail(FSN_EINVAL, "bad argument");
+extern "C" int fsn_plan_forward_bins(const fsn_config* cfg, int32_t B, int32_t T, double cap_bytes, int32_t force_window, int32_t force_bins,
+                                     int32_t* Bs, int32_t* Tw, int32_t* Fc, int64_t* bytes) {
+    if (!cfg || !Bs || !Tw || !Fc || B < 1 || T < 1 || !(cap_bytes > 0)) return fail(FSN_EINVAL, "bad argument");
     if (force_window < 0 || force_window % 32) return fail(FSN_EINVAL, "force_window must be 0 or a positive multiple of 32");
+    if (force_bins < 0) return fail(FSN_EINVAL, "force_bins must be 0 or a positive number of bins");
     if (cfg->num_freqs < 4 || cfg->num_layers < 1 || cfg->num_layers > 4 || cfg->look_ahead < 0) return fail(FSN_EINVAL, "bad configuration");
     if (int rc = check_length(*cfg, 1, T)) return rc;
-    int bs = 0, tw = 0;
-    plan_forward(*cfg, config_layerwise(*cfg, 0), B, T, cap_bytes, force_window, &bs, &tw, bytes);
-    *Bs = bs; *Tw = tw;
+    int bs = 0, tw = 0, fc = 0;
+    plan_forward(*cfg, config_layerwise(*cfg, 0), B, T, cap_bytes, force_window, force_bins, &bs, &tw, &fc, bytes);
+    *Bs = bs; *Tw = tw; *Fc = fc;
+    return FSN_OK;
+}
+
+extern "C" int fsn_plan_forward(const fsn_config* cfg, int32_t B, int32_t T, double cap_bytes, int32_t force_window, int32_t* Bs, int32_t* Tw,
+                                int64_t* bytes) {
+    int32_t fc = 0;
+    return fsn_plan_forward_bins(cfg, B, T, cap_bytes, force_window, 0, Bs, Tw, &fc, bytes);
+}
+
+extern "C" int fsn_model_plan_bins(const fsn_model* m, int32_t B, int32_t T, int32_t* Bs, int32_t* Tw, int32_t* Fc, int64_t* bytes) {
+    if (!m || !Bs || !Tw || !Fc || B < 1 || T < 1) return fail(FSN_EINVAL, "bad argument");
+    if (int rc = check_length(m->cfg, 1, T)) return rc;
+    int bs = 0, tw = 0, fc = 0;
+    plan_forward(m->cfg, config_layerwise(m->cfg, m->env_impl), B, T, m->ws_cap_bytes, m->env_sb_window, m->env_sb_chunk, &bs, &tw, &fc, bytes);
+    *Bs = bs; *Tw = tw; *Fc = fc;
     return FSN_OK;
 }
 
 extern "C" int fsn_model_plan(const fsn_model* m, int32_t B, int32_t T, int32_t* Bs, int32_t* Tw, int64_t* bytes) {
-    if (!m || !Bs || !Tw || B < 1 || T < 1) return fail(FSN_EINVAL, "bad argument");
-    if (int rc = check_length(m->cfg, 1, T)) return rc;
-    int bs = 0, tw = 0;
-    plan_forward(m->cfg, config_layerwise(m->cfg, m->env_impl), B, T, m->ws_cap_bytes, m->env_sb_window, &bs, &tw, bytes);
-    *Bs = bs; *Tw = tw;
-    return FSN_OK;
+    int32_t fc = 0;
+    return fsn_model_plan_bins(m, B, T, Bs, Tw, &fc, bytes);
 }
 
 extern "C" int fsn_model_release_workspace(fsn_model* m) {
     if (!m) return fail(FSN_EINVAL, "null model");
     CK(cudaDeviceSynchronize());                                         // nothing in flight may still read the buffers
-    for (auto& ln : m->lane) { ln.release_all(); ln.wsB = ln.wsT = ln.wsTw = 0; }
+    for (auto& ln : m->lane) { ln.release_all(); ln.wsB = ln.wsT = ln.wsTw = ln.wsFc = 0; }
     DevBuf* lstm[] = {&m->cstate, &m->mask_tmp, &m->r_gin, &m->r_hseq, &m->r_hstate, &m->sb_cum, &m->ws_h, &m->ws_bar};
     for (auto* b : lstm) b->release();
     m->sb_scratch.release();
@@ -1696,5 +1788,11 @@ extern "C" int64_t fsn_model_workspace_bytes(const fsn_model* m) {
 extern "C" int fsn_model_last_plan(const fsn_model* m, int32_t* Bs, int32_t* Tw) {
     if (!m || !Bs || !Tw) return fail(FSN_EINVAL, "null argument");
     *Bs = m->plan_Bs; *Tw = m->plan_Tw;
+    return FSN_OK;
+}
+
+extern "C" int fsn_model_last_plan_bins(const fsn_model* m, int32_t* Bs, int32_t* Tw, int32_t* Fc) {
+    if (!m || !Bs || !Tw || !Fc) return fail(FSN_EINVAL, "null argument");
+    *Bs = m->plan_Bs; *Tw = m->plan_Tw; *Fc = m->plan_Fc;
     return FSN_OK;
 }

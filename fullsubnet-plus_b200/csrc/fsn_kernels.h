@@ -79,9 +79,12 @@ struct SbPackLaunch {
     int ntiles;
     int t0, Tw;              // frame window of the images (t0 = 0, Tw = Tp: the whole clip); Tw is a multiple of 32 except in the last window
     double* cum;             // cumulative norms, windowed: running (sum, sum of squares) [B*F][2] at the window's end, reloaded when t0 > 0
-    float* xtm;              // sub-band TCN input: fp32 time-major [B*F*Tp, 64], row (b*F + f)*Tp + t, columns >= I zero
-    float* amax;             // [B*F] max |x| of every sequence of xtm (zeroed by the launcher): block 0's fp16 store scale
+    float* xtm;              // sub-band TCN input: fp32 time-major [B*Fc*Tp, 64], row (b*Fc + f - f0)*Tp + t, columns >= I zero
+    float* amax;             // [B*Fc] max |x| of every sequence of xtm (zeroed by the launcher): block 0's fp16 store scale
     const int* tlen;         // optional [B] per-sample extent in frames of Tp (rows past it are written as zero); null: Tp
+    // xtm only: the bins f0 .. f0 + Fc - 1 of every sample (a chunk of the sub-band TCN; f0 = 0, Fc = F: all of them).  Sequence
+    // (b, f) is row b * Fc + (f - f0) of xtm and amax; neighbours are still read from the absolute bins, reflected over the whole F
+    int f0, Fc;
 };
 void launch_sb_stats(const SbPackLaunch& a, cudaStream_t s);
 void launch_sb_pack(const SbPackLaunch& a, cudaStream_t s);
@@ -208,13 +211,16 @@ struct GemmTc5Launch {
     const float* Xold; float* Xrelu;           // GLN_RES: residual input, optional relu'd copy
     float* out; int F, P, act;                 // OUT: [Z, F, P] (frequency-major); GLN_HEAD: mask [B, O, F, Tp - la]
     // GLN_HEAD (last block of the sub-band TCN, one 64-column N tile): GLN_RES's new stream x, then act(Linear(relu(x))) per row;
-    // rows are (b * F + f) * Tp + t.  With enh != null: decompress_cIRM x the noisy planes [B, F, Tp - la] into enh instead of the mask
+    // rows are (b * Fg + f - f0) * Tp + t.  With enh != null: decompress_cIRM x the noisy planes [B, F, Tp - la] into enh instead of the mask
     const float* fc_w; const float* fc_b;      // [O, 64] (columns >= I zero), [O]
     int O, la;
     const float* nreal; const float* nimag; float2* enh;
     // optional per-sample extent in frames of Tp, tlen[z / zdiv] for gLN group z (full band: z = branch * B + b, tlen [3][B], zdiv 1;
     // sub band: z = b * F + f, zdiv F).  Rows t >= that extent are written as zero and left out of every statistic and maximum
     const int* tlen; int zdiv;
+    // GLN_HEAD: group z is bin f0 + z % Fg of clip z / Fg (a chunk of Fg bins from f0; Fg = F, f0 = 0: every bin).  F still sets the
+    // layout of the mask, the enhanced spectrum and the noisy planes
+    int Fg, f0;
 };
 int make_tmap_f32_2d(void* out_map /*128 B, 64 B aligned*/, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows);
 int launch_gemm_tc5(const void* mapA, const void* mapB, GemmTc5Launch a, int num_sms, cudaStream_t s);

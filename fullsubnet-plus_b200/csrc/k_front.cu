@@ -459,7 +459,9 @@ void launch_sb_stats(const SbPackLaunch& a, cudaStream_t s) {
 // Stores of the normalised sub-band input.  Fp16Img: the SWIZZLE_128B images of the LSTM kernels (values clamped to the fp16
 // range).  Fp32Tm: the sub-band TCN's time-major fp32 rows of 64 channels, plus max |x| per sequence (block 0's fp16 store scale).
 // Both packers compute every value once and hand 8 consecutive channels k0 .. k0 + 7 of (sequence row, frame t) to store().
+// kChunk: the store takes the bin range a.f0 .. a.f0 + a.Fc - 1 (rows b * Fc + f - f0); without it every bin, rows b * F + f.
 struct Fp16Img {
+    static constexpr bool kChunk = false;
     static __device__ __forceinline__ void store(const SbPackLaunch& a, int row, int t, int k0, const float (&v)[8]) {
         float w[8];
 #pragma unroll
@@ -471,6 +473,7 @@ struct Fp16Img {
     static __device__ __forceinline__ void finish(const SbPackLaunch&, int, float, unsigned) {}
 };
 struct Fp32Tm {
+    static constexpr bool kChunk = true;
     static __device__ __forceinline__ void store(const SbPackLaunch& a, int row, int t, int k0, const float (&v)[8]) {
         float4* dst = reinterpret_cast<float4*>(a.xtm + ((size_t)row * a.Tp + t) * 64 + k0);
         dst[0] = make_float4(v[0], v[1], v[2], v[3]);
@@ -488,14 +491,15 @@ __device__ __forceinline__ float vmax8(float m, const float (&v)[8]) {
     return m;
 }
 
-// One CTA = (sample, 32 consecutive bins, 32 frames).  The window source rows [f0 - Ns, f0 + 31 + Ns] (reflected) and the
+// One CTA = (sample, 32 consecutive bins of the range, 32 frames).  The window source rows [f0 - Ns, f0 + 31 + Ns] (reflected) and the
 // full-band rows of the 32 bins are staged once in shared memory; work item = (bin, frame, 8 channels), so 8 consecutive lanes
 // write one whole row of 64 channels (one 128-byte line of the SWIZZLE_128B image).
 constexpr int SBP_F = 32, SBP_T = 32;
 template <class Store>
 __global__ void __launch_bounds__(256) sb_pack_kernel(SbPackLaunch a) {
     extern __shared__ float sm[];
-    const int F = a.F, Tp = a.t0 + a.Tw, b = blockIdx.z, f0 = blockIdx.y * SBP_F, t0 = a.t0 + blockIdx.x * SBP_T;   // Tp: the window's end
+    const int fb = Store::kChunk ? a.f0 : 0, Fn = Store::kChunk ? a.Fc : a.F;   // bins fb .. fb + Fn - 1
+    const int F = a.F, Tp = a.t0 + a.Tw, b = blockIdx.z, f0 = fb + blockIdx.y * SBP_F, t0 = a.t0 + blockIdx.x * SBP_T;   // Tp: the window's end
     const int Tpe = a.tlen ? a.tlen[b] : Tp;                       // frames t >= Tpe are past this sample's end: written as zero
     const int nw = 2 * a.Ns + 1, nf = 2 * a.Nf + 1, I = nw + a.nfb * nf;
     const int wrows = SBP_F + 2 * a.Ns, frows = SBP_F + 2 * a.Nf;
@@ -520,8 +524,8 @@ __global__ void __launch_bounds__(256) sb_pack_kernel(SbPackLaunch a) {
     __syncthreads();
     const int c = threadIdx.x & 7, fr = threadIdx.x >> 3;          // chunk, bin inside the tile
     const int f = f0 + fr;
-    const bool live = f < F;
-    const int row = b * F + f;
+    const bool live = f < fb + Fn;
+    const int row = b * Fn + (f - fb);
     auto val = [&](int k, int tt) -> float {
         float v = 0.f;
         if (k < nw) v = wsm[(fr + k) * (SBP_T + 1) + tt];
@@ -545,9 +549,12 @@ __global__ void __launch_bounds__(256) sb_pack_kernel(SbPackLaunch a) {
 template <class Store>
 __global__ void __launch_bounds__(128) sb_pack_cum_kernel(SbPackLaunch a) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int fb = Store::kChunk ? a.f0 : 0, Fn = Store::kChunk ? a.Fc : a.F;   // bins fb .. fb + Fn - 1
     const int row = blockIdx.x * 4 + warp, F = a.F, Tp = a.t0 + a.Tw;   // Tp: the window's end
-    if (row >= a.B * F) return;
-    const int b = row / F, f = row % F;
+    if (row >= a.B * Fn) return;
+    // f < F always: the unsigned modulo changes no value, it tells the compiler f's range (without it, it keeps 64 neighbour addresses
+    // live across the frame loop and spills)
+    const int b = row / Fn, f = (int)((unsigned)(fb + row % Fn) % (unsigned)F);
     const int Tpe = a.tlen ? a.tlen[b] : a.Tp;                     // frames t >= Tpe are past this sample's end: written as zero
     const int nw = 2 * a.Ns + 1, nf = 2 * a.Nf + 1, I = nw + a.nfb * nf;
     const double EPS = 1.1920928955078125e-07;
@@ -600,18 +607,19 @@ __global__ void __launch_bounds__(128) sb_pack_cum_kernel(SbPackLaunch a) {
 
 template <class Store>
 static void sb_pack_go(const SbPackLaunch& a, cudaStream_t s) {
+    const int Fn = Store::kChunk ? a.Fc : a.F;
     if (a.norm_type == FSN_NORM_CUMULATIVE_LAPLACE || a.norm_type == FSN_NORM_CUMULATIVE_LAYER)
-        sb_pack_cum_kernel<Store><<<(a.B * a.F + 3) / 4, 128, 0, s>>>(a);
+        sb_pack_cum_kernel<Store><<<(a.B * Fn + 3) / 4, 128, 0, s>>>(a);
     else
     {
         const size_t smem = sizeof(float) * (SBP_T + 1) * ((SBP_F + 2 * a.Ns) + a.nfb * (SBP_F + 2 * a.Nf));
         cudaFuncSetAttribute(sb_pack_kernel<Store>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        sb_pack_kernel<Store><<<dim3((a.Tw + SBP_T - 1) / SBP_T, (a.F + SBP_F - 1) / SBP_F, a.B), 256, smem, s>>>(a);
+        sb_pack_kernel<Store><<<dim3((a.Tw + SBP_T - 1) / SBP_T, (Fn + SBP_F - 1) / SBP_F, a.B), 256, smem, s>>>(a);
     }
 }
 void launch_sb_pack(const SbPackLaunch& a, cudaStream_t s) { sb_pack_go<Fp16Img>(a, s); }
 void launch_sb_pack_tm(const SbPackLaunch& a, cudaStream_t s) {
-    cudaMemsetAsync(a.amax, 0, (size_t)a.B * a.F * sizeof(float), s);
+    cudaMemsetAsync(a.amax, 0, (size_t)a.B * a.Fc * sizeof(float), s);
     sb_pack_go<Fp32Tm>(a, s);
 }
 

@@ -307,7 +307,7 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 if (!valid[h] || (lane & 3) != 0 || tt[h] < a.la) continue;
-                const int ob = z[h] / a.F, of = z[h] % a.F;
+                const int ob = z[h] / a.Fg, of = a.f0 + z[h] % a.Fg;
                 const size_t ni = ((size_t)ob * a.F + of) * Tout + (tt[h] - a.la);
                 if (!live[h]) {                                // past the clip's end: zeros, the noisy planes are not read
                     if (a.enh) a.enh[ni] = make_float2(0.f, 0.f);

@@ -18,6 +18,7 @@ SYMBOLS = [
     "fsn_model_num_params", "fsn_model_param_info", "fsn_model_finalize", "fsn_model_forward",
     "fsn_model_forward_host", "fsn_model_forward_host_async", "fsn_model_sync_host", "fsn_model_submit", "fsn_model_wait", "fsn_model_forward_enhance", "fsn_model_submit_enhance", "fsn_model_forward_ragged", "fsn_model_forward_enhance_ragged", "fsn_model_last_lane", "fsn_model_wait_lane", "fsn_apply_cirm", "fsn_stream_create", "fsn_stream_step", "fsn_stream_destroy", "fsn_model_get_stage", "fsn_model_last_launch_count", "fsn_model_last_lstm_impl", "fsn_model_last_lstm_ms", "fsn_model_lstm_ms_history", "fsn_model_timeline",
     "fsn_plan_forward", "fsn_model_workspace_bytes", "fsn_model_last_plan", "fsn_model_plan", "fsn_model_release_workspace",
+    "fsn_plan_forward_bins", "fsn_model_plan_bins", "fsn_model_last_plan_bins",
     "fsn_sw128_offset", "fsn_tc5_weight_stream_bytes", "fsn_tc5_pack_weights", "fsn_tc5_gate_row", "fsn_tc5r_weight_stream_bytes", "fsn_tc5r_pack_layer",
 ]
 
@@ -90,6 +91,10 @@ def load_library():
     lib.fsn_model_last_plan.argtypes = [vp, C.POINTER(i32), C.POINTER(i32)]
     lib.fsn_model_plan.argtypes = [vp, i32, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i64)]
     lib.fsn_model_release_workspace.argtypes = [vp]
+    lib.fsn_plan_forward_bins.argtypes = [C.POINTER(FsnConfig), i32, i32, C.c_double, i32, i32, C.POINTER(i32), C.POINTER(i32),
+                                          C.POINTER(i32), C.POINTER(i64)]
+    lib.fsn_model_plan_bins.argtypes = [vp, i32, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i64)]
+    lib.fsn_model_last_plan_bins.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
     lib.fsn_sw128_offset.argtypes = [C.c_uint32, C.c_uint32]
     lib.fsn_sw128_offset.restype = C.c_uint32
     lib.fsn_tc5_weight_stream_bytes.argtypes = [i32, i32]
@@ -129,3 +134,14 @@ def plan_forward(cfg, B, T, cap_bytes=None, force_window=0):
     cap = ws_cap_bytes() if cap_bytes is None else float(cap_bytes)
     check(lib.fsn_plan_forward(C.byref(cfg), int(B), int(T), cap, int(force_window), C.byref(bs), C.byref(tw), C.byref(nb)))
     return bs.value, tw.value, nb.value
+
+
+def plan_forward_bins(cfg, B, T, cap_bytes=None, force_window=0, force_bins=0):
+    """fsn_plan_forward_bins: plan_forward's (clips per sub-batch, window, workspace bytes) with the sub-band TCN's bin chunk, as
+    (Bs, Tw, Fc, bytes); Fc = 0 means unchunked (always for LSTM / GRU).  force_bins: 0, or the FSN_SB_CHUNK value.  Needs no GPU."""
+    lib = load_library()
+    bs, tw, fc, nb = C.c_int32(), C.c_int32(), C.c_int32(), C.c_int64()
+    cap = ws_cap_bytes() if cap_bytes is None else float(cap_bytes)
+    check(lib.fsn_plan_forward_bins(C.byref(cfg), int(B), int(T), cap, int(force_window), int(force_bins), C.byref(bs), C.byref(tw),
+                                    C.byref(fc), C.byref(nb)))
+    return bs.value, tw.value, fc.value, nb.value

@@ -357,6 +357,28 @@ class _B200Model(nn.Module):
         _lib.check(lib.fsn_model_plan(self._handle, int(B), int(T), C.byref(bs), C.byref(tw), C.byref(nb)))
         return bs.value, tw.value, nb.value
 
+    def last_plan_bins(self):
+        """(clips per sub-batch, sub-band window in frames, sub-band TCN bins per chunk) of the last plain forward; 0 = unwindowed /
+        unchunked."""
+        if not self._handle:
+            return (0, 0, 0)
+        bs, tw, fc = C.c_int32(), C.c_int32(), C.c_int32()
+        _lib.check(_lib.load_library().fsn_model_last_plan_bins(self._handle, C.byref(bs), C.byref(tw), C.byref(fc)))
+        return (bs.value, tw.value, fc.value)
+
+    def plan_bins(self, B, T):
+        """plan() with the sub-band TCN's bin chunk: (clips per sub-batch, window or 0, bins per chunk or 0, workspace bytes) of this
+        model's next plain forward (C ABI: fsn_model_plan_bins, with the FSN_* knobs the handle read at creation, FSN_SB_CHUNK among
+        them).  Creates the handle if needed, so the model must be on its CUDA device; enqueues no GPU work."""
+        dev = next(self.parameters()).device
+        if dev.type != "cuda":
+            raise RuntimeError("plan_bins() needs the model on its CUDA device (the plan is the handle's)")
+        with torch.cuda.device(dev):
+            lib = self._ensure_handle(dev)
+        bs, tw, fc, nb = C.c_int32(), C.c_int32(), C.c_int32(), C.c_int64()
+        _lib.check(lib.fsn_model_plan_bins(self._handle, int(B), int(T), C.byref(bs), C.byref(tw), C.byref(fc), C.byref(nb)))
+        return bs.value, tw.value, fc.value, nb.value
+
     def release_workspace(self):
         """Free every forward workspace this model holds (synchronises the device); the next forward allocates again."""
         if self._handle:

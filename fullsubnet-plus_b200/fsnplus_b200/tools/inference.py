@@ -154,9 +154,13 @@ def batch_by_sorted_length(lengths, batch_size, max_samples=None):
 
 
 def plan_is_windowed(model, batch, frames):
-    """True when the model's plain forward of `batch` clips of `frames` STFT frames will run its sub-band stage in time windows
-    (model.plan, the C ABI's fsn_plan_forward): such a forward takes the model's whole workspace cap.  Stand-in models without a
-    plan are never windowed."""
+    """True when the model's plain forward of `batch` clips of `frames` STFT frames will run its sub-band stage in time windows or, for
+    the sub-band TCN, in bin chunks (model.plan_bins / model.plan, the C ABI's fsn_plan_forward_bins): such a forward takes the model's
+    whole workspace cap.  Stand-in models without a plan are never windowed."""
+    plan_bins = getattr(model, "plan_bins", None)
+    if plan_bins is not None:
+        _, tw, fc, _ = plan_bins(batch, frames)
+        return tw > 0 or fc > 0
     plan = getattr(model, "plan", None)
     return plan is not None and plan(batch, frames)[1] > 0
 
@@ -186,7 +190,7 @@ def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=pri
     ``model_and_epoch`` (tests of the host logic) replaces the checkpoint load with a ready ``(callable, epoch)``.
     ``ragged=True``: batches of clips of different lengths (length-sorted, ``batch_size`` clips each) through ``enhance_ragged``.
     ``max_batch_seconds``: a batch is also cut before its total audio exceeds that many seconds (a longer clip goes alone).
-    A batch whose forward the model plans in time windows (a long clip: it uses the model's whole workspace cap) runs alone on the
+    A batch whose forward the model plans in time windows or bin chunks (a long clip: it uses the model's whole workspace cap) runs alone on the
     first replica: every batch in flight is finished and every replica's workspaces are released first, and the first replica's
     after it, so only one capped workspace exists at a time.
     ``replicas`` (tests of the host logic, with ``model_and_epoch``): ready models for the replicas after the first."""
@@ -250,7 +254,7 @@ def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=pri
         while inflight and (alone or len(inflight) >= nstream):
             finish(inflight.pop(0))                                        # the batch that used this stream / replica last
         if alone:
-            release_all(models)                                            # the windowed forward may take the whole cap
+            release_all(models)                                            # the windowed / chunked forward may take the whole cap
         if ragged:
             clips = [torch.from_numpy(read_wav(files[i], ds_sr)) for i in idx]
             audio_s += sum(c.numel() for c in clips) / sr

@@ -209,29 +209,43 @@ int fsn_model_last_lstm_impl(const fsn_model* m);
  * unwindowed forward and the sub-band memory is O(Tw).  Everything that needs the whole utterance (norms, attention pooling, the
  * full-band model, the sub-band statistics) stays whole-clip at about 26 KB per frame (FullSubNet+) or 41 KB (fullsubnet.Model).
  * FSN_SB_WINDOW=<frames> (a positive multiple of 32, read at fsn_model_create, else FSN_EINVAL) forces windows of that length.
- * Windows apply to the layer-wise path only: the sub-band TCN, lstm_impl = FSN_LSTM_MMA and the pipelined entry points run unwindowed.
+ * Windows apply to the layer-wise path only: lstm_impl = FSN_LSTM_MMA and the pipelined entry points run unwindowed, and the sub-band
+ * TCN runs in bin chunks instead (DESIGN.md §3.8): when one sub-batch would exceed the cap, its B x num_freqs sequences run Fc bins at
+ * a time (the last chunk takes the remainder), each sequence with exactly its own arithmetic, so the sub-band memory is O(Fc x T').
+ * FSN_SB_CHUNK=<bins> (a positive integer, read at fsn_model_create, else FSN_EINVAL) forces chunks of that many bins on every plain
+ * forward of a sub-band TCN model (>= num_freqs: unchunked); LSTM / GRU models ignore it.  The pipelined entry points run unchunked.
  * Length limits (FSN_EINVAL naming the limit, from every forward entry point and fsn_plan_forward): T + look_ahead <= 16 776 960
  * frames (65535 x 256, the TCN depth-wise convolution's grid), num_freqs x (T + look_ahead) <= 2^31 - 1 (the per-clip plane index), and
  * for FullSubNet+ 3 x B x (T + look_ahead) + 128 <= 2^31 - 1 (the full-band TCN's rows; the planner keeps sub-batches below it).  At
  * num_freqs = 257 that is 8 355 967 frames, about 37 hours at 16 kHz / hop 256.  Memory binds first: the whole-clip part, ~26 KB
  * (FullSubNet+) / ~40 KB (fullsubnet.Model) per frame, leaves room in the 24 GB default cap for one clip of up to 4.0 / 2.6 hours
  * (T = 915 689 / 599 084, windows then down to 32 frames); a longer clip runs with 256-frame windows and allocates past the cap.  A 2-hour
- * clip (T = 450 000) plans 6016- / 2944-frame windows within the default cap; the sub-band TCN keeps its B * num_freqs * (T + look_ahead)
- * < 2^31 row limit.
- * After a windowed forward the model holds at most the plan's bytes: it first gives back whatever earlier forwards grew beyond them.
+ * clip (T = 450 000) plans 6016- / 2944-frame windows within the default cap; the planner keeps every sub-band TCN chunk run below its
+ * Bs * Fc * (T + look_ahead) + 128 < 2^31 row limit.
+ * After a windowed or chunked forward the model holds at most the plan's bytes: it first gives back whatever earlier forwards grew
+ * beyond them.
  *
  * fsn_plan_forward: the plan, from the configuration alone (its lstm_impl; no environment knob), for B clips of T frames under
  * cap_bytes: *Bs clips per sub-batch, *Tw frames per window (0: unwindowed), *bytes (may be NULL) the workspace it requests.
- * force_window: 0, or the FSN_SB_WINDOW value.  No GPU needed. */
+ * force_window: 0, or the FSN_SB_WINDOW value.  No GPU needed.  For a sub-band TCN configuration that chunks, *bytes is the chunked
+ * request (fsn_plan_forward_bins gives the chunk). */
 int fsn_plan_forward(const fsn_config* cfg, int32_t B, int32_t T, double cap_bytes, int32_t force_window, int32_t* Bs, int32_t* Tw,
                      int64_t* bytes);
+/* The same plan with the sub-band TCN's bin chunk: *Fc bins per chunk (0: unchunked; always 0 for LSTM / GRU).  force_bins: 0, or the
+ * FSN_SB_CHUNK value. */
+int fsn_plan_forward_bins(const fsn_config* cfg, int32_t B, int32_t T, double cap_bytes, int32_t force_window, int32_t force_bins,
+                          int32_t* Bs, int32_t* Tw, int32_t* Fc, int64_t* bytes);
 /* Bytes the model currently holds in forward workspaces: both lanes plus the sub-band scratch (parameters and host-entry staging excluded). */
 int64_t fsn_model_workspace_bytes(const fsn_model* m);
 /* Plan of the last plain forward: sub-batch and window (Tw = 0: unwindowed). */
 int fsn_model_last_plan(const fsn_model* m, int32_t* Bs, int32_t* Tw);
+/* The same with the bin chunk of the sub-band TCN (Fc = 0: unchunked). */
+int fsn_model_last_plan_bins(const fsn_model* m, int32_t* Bs, int32_t* Tw, int32_t* Fc);
 /* The plan the model's next plain forward of B clips of T frames will use: fsn_plan_forward with the knobs the model read at create
- * (FSN_WS_CAP_GB, FSN_SB_WINDOW, FSN_LSTM_IMPL).  Host only; enqueues nothing. */
+ * (FSN_WS_CAP_GB, FSN_SB_WINDOW, FSN_SB_CHUNK, FSN_LSTM_IMPL).  Host only; enqueues nothing. */
 int fsn_model_plan(const fsn_model* m, int32_t B, int32_t T, int32_t* Bs, int32_t* Tw, int64_t* bytes);
+/* The same with the bin chunk of the sub-band TCN (Fc = 0: unchunked). */
+int fsn_model_plan_bins(const fsn_model* m, int32_t B, int32_t T, int32_t* Bs, int32_t* Tw, int32_t* Fc, int64_t* bytes);
 /* Synchronises the device and frees every forward workspace of the model (fsn_model_workspace_bytes drops to 0); the next forward
  * allocates what it needs again.  For callers that keep several models and run a capped (windowed) forward on one of them. */
 int fsn_model_release_workspace(fsn_model* m);

@@ -139,6 +139,7 @@ struct fsn_model {
     int plan_Bs = 0, plan_Tw = 0, plan_Fc = 0;         // plan of the last plain forward (fsn_plan_forward_bins): sub-batch, window (0: whole
                                                        // clip), bin chunk (0: all bins)
     bool env_no_ws = false;
+    int env_gin_tile_n = 0;                            // FSN_GIN_GEMM=128: the input-projection GEMM on 128 x 128 tiles (GemmF16Launch::tile_n)
     // pipelined execution: front-end stream, LSTM stream (higher priority), copy-in / copy-out streams, per-slot events
     cudaStream_t s_front = nullptr, s_lstm = nullptr, s_in = nullptr, s_out = nullptr;
     cudaEvent_t ev_in = nullptr, ev_plain = nullptr;   // caller's inputs ready / last plain forward finished
@@ -458,10 +459,18 @@ extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
         if (*end || w < 1) return fail(FSN_EINVAL, "FSN_SB_CHUNK=%s: the chunk must be a positive number of bins", e);
         sb_chunk = w < c.num_freqs ? (int)w : c.num_freqs;
     }
+    // FSN_GIN_GEMM: N tile of the deeper layers' input-projection GEMM.  Unset or 256: 128 x 256 tiles on CTA pairs wherever the shape
+    // allows; 128: the 128 x 128 kernel everywhere (A/B runs in one process; both compute the same bits)
+    int gin_tile_n = 0;
+    if (const char* e = getenv("FSN_GIN_GEMM"); e && *e) {
+        if (strcmp(e, "128") && strcmp(e, "256")) return fail(FSN_EINVAL, "FSN_GIN_GEMM=%s: the N tile must be 128 or 256", e);
+        gin_tile_n = atoi(e);
+    }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(FSN_ECUDA, "no CUDA device: fsnplus_b200 has no CPU fallback");
     fsn_model* m = new fsn_model();
     m->cfg = c;
+    m->env_gin_tile_n = gin_tile_n;
     m->env_sb_window = sb_window;
     m->env_sb_chunk = sb_chunk;
     { const char* e = getenv("FSN_LSTM_IMPL"); if (e && *e) m->env_impl = atoi(e); }
@@ -836,7 +845,7 @@ static int run_sb_lstm(fsn_model* m, fsn_model::Lane& ln, int B, int T, int Tw, 
             for (int l = 0; l < c.num_layers; ++l) {
                 if (l > 0) {
                     // row-major Gin[M, 4H] = X[M, H] * Wp[4H, H]^T, both operands K-major
-                    GemmF16Launch g{M, 4 * H, H, static_cast<__half*>(m->r_gin.p), 4LL * H};
+                    GemmF16Launch g{M, 4 * H, H, static_cast<__half*>(m->r_gin.p), 4LL * H, m->env_gin_tile_n};
                     int ge = launch_gemm_f16(m->r_hseq.p, m->r_wih[l].p, g, m->num_sms, s);
                     if (ge) return fail(FSN_ECUDA, "input-projection GEMM launch failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)ge));
                     m->launches++;
@@ -1689,6 +1698,24 @@ extern "C" int fsn_apply_cirm(const float* d_crm, const float* d_noisy, float* d
     launch_apply_cirm(d_crm, reinterpret_cast<const float2*>(d_noisy), reinterpret_cast<float2*>(d_enh), B, F, T, static_cast<cudaStream_t>(stream));
     CK(cudaGetLastError());
     return FSN_OK;
+}
+
+extern "C" int fsn_gemm_f16(const void* d_a, const void* d_b, void* d_c, int64_t M, int32_t N, int32_t K, int32_t tile_n, void* stream) {
+    if (!d_a || !d_b || !d_c || !gemm_f16_supported(M, N, K) || (tile_n != 0 && tile_n != 128 && tile_n != 256))
+        return fail(FSN_EINVAL, "fsn_gemm_f16: M = %lld, N = %d, K = %d, tile_n = %d: needs M %% 128 == 0, N %% 128 == 0, K %% 64 == 0, tile_n 0 / 128 / 256",
+                    (long long)M, N, K, tile_n);
+    int dev = 0, sms = 0;
+    CK(cudaGetDevice(&dev));
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    GemmF16Launch g{M, N, K, static_cast<__half*>(d_c), N, tile_n};
+    const int e = launch_gemm_f16(d_a, d_b, g, sms, static_cast<cudaStream_t>(stream));
+    if (e) return fail(FSN_ECUDA, "fsn_gemm_f16 launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    return FSN_OK;
+}
+extern "C" int32_t fsn_gemm_f16_tile_n(int64_t M, int32_t N, int32_t K, int32_t tile_n) {
+    if (!gemm_f16_supported(M, N, K)) return fail(FSN_EINVAL, "fsn_gemm_f16_tile_n: unsupported shape");
+    GemmF16Launch g{M, N, K, nullptr, N, tile_n};
+    return gemm_f16_pair_tiles(g) ? 256 : 128;
 }
 
 extern "C" int64_t fsn_model_last_launch_count(const fsn_model* m) { return m ? m->launches : 0; }

@@ -188,9 +188,11 @@ void lstm_tc5r_gin_order(int H, int Kpad, std::vector<uint16_t>& wih_perm);   //
 void lstm_tc5_pack_first_layer(int I, int H, const float* w_ih0, const float* w_hh0, uint16_t* dst);   // k_lstm_tc5d.cu: [x | hidden] blocks per chunk
 
 // ---- k_gemm_tc5.cu (TCN on wgmma, time-major activations; the input projection of the layer-wise LSTM path) ----------------
-// C[M, N] = A[M, K] B[N, K]^T, fp16 in / fp32 accumulate / fp16 out (input projection of the layer-wise path)
-struct GemmF16Launch { long long M; int N, K; __half* C; long long ldc; };
+// C[M, N] = A[M, K] B[N, K]^T, fp16 in / fp32 accumulate / fp16 out (input projection of the layer-wise path).  tile_n: 0 or 256 =
+// 128 x 256 tiles on CTA pairs where the shape allows (gemm_f16_pair_tiles), else 128 x 128; 128 = always 128 x 128 (FSN_GIN_GEMM)
+struct GemmF16Launch { long long M; int N, K; __half* C; long long ldc; int tile_n; };
 bool gemm_f16_supported(long long M, int N, int K);
+bool gemm_f16_pair_tiles(const GemmF16Launch& g);
 int launch_gemm_f16(const void* A, const void* B, const GemmF16Launch& a, int num_sms, cudaStream_t s);
 int make_tmap_f16_2d(void* out_map /*128 B, 64 B aligned*/, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows);   // box = 64 halves x box_rows, SWIZZLE_128B
 

@@ -1,7 +1,8 @@
 // TCN full-band model (K3 of SURVEY.md 2a) on the Hopper tensor cores: the 1x1 convolutions of the eight TCNBlocks and the
 // output Linear as persistent wgmma GEMMs over time-major activations, plus the depth-wise convolution between them.  The same
 // kernels run the optional sub-band TCN (sequence_model = "TCN": one branch, the B*F sequences as the gLN groups, EPI5_GLN_HEAD
-// last), and the GEMM kernel also computes the input projection of the layer-wise LSTM path (EPI5_F16OUT).
+// last).  The input projection of the layer-wise LSTM path runs on gemm_f16_pair_kernel below (128 x 256 tiles on CTA pairs), or on
+// this GEMM kernel (EPI5_F16OUT) for shapes without tile pairs and under FSN_GIN_GEMM=128.
 //
 // reference: TCNBlock.forward (audio_zen/model/module/causal_conv.py:96-108) and SequenceModel.forward, TCN branch
 // (audio_zen/model/module/sequence_model.py:106-112).
@@ -43,6 +44,14 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
                  "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
                  : "memory");
 }
+// the same box written into the shared memory of every CTA in `mask` (same offset in each), completion on the mbarrier at the same
+// offset in each
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar, uint16_t mask) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%2, %3}], [%4], %5;" ::"r"(
+                     smem_u32(smem_dst)),
+                 "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar)), "h"(mask)
+                 : "memory");
+}
 
 // one 32-byte k-step of the 64 x NT warpgroup tile: 16 fp16 or 8 tf32 elements
 template <int NT, bool AH>
@@ -54,16 +63,16 @@ __device__ __forceinline__ void g5_mma(float (&acc)[NT / 2], uint64_t ad, uint64
 // fp16 results (PRELU_STATS, F16OUT) leave through a per-warp staging tile: the accumulator fragment gives a lane 4 bytes of 8 rows
 // per store, so direct stores wrote 16-byte pieces of 8 lines per instruction; staged, a warp writes whole 512-byte row runs.
 // Tile = the warp's 16 rows x NT halves, 16-byte units XOR-swizzled by (row & 7) so both the fragment writes and the row reads are
-// free of bank conflicts.  hp[j][h] = the packed pair (columns 8 j + 2 (lane % 4), + 1) of row (lane / 4) + 8 h.
-template <int NT>
-__device__ __forceinline__ void g5_store_f16(uint8_t* stg, int lane, const uint32_t (&hp)[NT / 8][2], __half* gbase, size_t ld, int nvalid) {
+// free of bank conflicts.  frag(j, h) = the packed pair (columns 8 j + 2 (lane % 4), + 1) of row (lane / 4) + 8 h.
+template <int NT, typename Frag>
+__device__ __forceinline__ void g5_store_f16_from(uint8_t* stg, int lane, Frag frag, __half* gbase, size_t ld, int nvalid) {
     constexpr int U = NT / 8;                                   // 16-byte units per row
 #pragma unroll
     for (int j = 0; j < U; ++j)
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int r = (lane >> 2) + 8 * h;
-            *reinterpret_cast<uint32_t*>(stg + r * NT * 2 + ((j ^ (r & 7)) << 4) + (lane & 3) * 4) = hp[j][h];
+            *reinterpret_cast<uint32_t*>(stg + r * NT * 2 + ((j ^ (r & 7)) << 4) + (lane & 3) * 4) = frag(j, h);
         }
     __syncwarp();
     constexpr int RPI = 32 / U;                                 // rows per store instruction
@@ -74,6 +83,10 @@ __device__ __forceinline__ void g5_store_f16(uint8_t* stg, int lane, const uint3
         if (r < nvalid) *reinterpret_cast<uint4*>(gbase + (size_t)r * ld + u * 8) = v;
     }
     __syncwarp();
+}
+template <int NT>
+__device__ __forceinline__ void g5_store_f16(uint8_t* stg, int lane, const uint32_t (&hp)[NT / 8][2], __half* gbase, size_t ld, int nvalid) {
+    g5_store_f16_from<NT>(stg, lane, [&](int j, int h) { return hp[j][h]; }, gbase, ld, nvalid);
 }
 
 // sum (PRELU_STATS) or max (GLN_RES) of one value per lane into a per-sample slot: rows of a warp almost always belong to one
@@ -407,13 +420,141 @@ int launch_gemm_tc5(const void* mapA, const void* mapB, GemmTc5Launch a, int num
     return g5_launch<EPI5_OUT, 128>(mA, mB, a, num_sms, s);
 }
 
+// ---------------------------------------------------------------------------------------------
+// Input projection of the layer-wise LSTM path on 128 x 256 tiles, the weight tile shared by a CTA pair (EPI5_F16OUT only).
+// On 128 x 128 tiles every byte brought from L2 into shared memory feeds 64 FLOP, and at K = 384 the kernel moves 58 GB per
+// flagship step that way -- bound by what the L2 delivers, not by HBM or the tensor cores.  Here the two CTAs of a cluster take
+// M tiles 2p and 2p + 1 of the same 256-column N tile: each TMA-loads its own 128-row A box and one 128-row half of the 256-row
+// B block, multicast to both, so per k-block a CTA pulls 16 KB of A and 16 KB of B for twice the MMAs (128 FLOP per byte).  Each
+// consumer warpgroup runs m64n256k16 into 128 accumulator registers; the 256 columns leave in two 128-column passes through the
+// staging tiles.  The k order (64-wide k-blocks, four 16-wide steps, fp32 accumulation) is the 128 x 128 kernel's: same bits.
+// An `empty` slot counts the consumer warps of BOTH CTAs (the peer's half of B lands in this CTA's slot too), and no CTA exits
+// while its peer may still arrive on its barriers.  The producer is a whole warpgroup (one thread issues the copies) so that the
+// register file can be moved to the consumers with setmaxnreg: 128 accumulators plus the epilogue do not fit the 168 registers
+// per thread that an even split of 288 or 384 threads leaves.
+// ---------------------------------------------------------------------------------------------
+constexpr int GP_CL = 2;                                  // CTAs per cluster: M tiles 2p, 2p + 1
+constexpr int GP_NT = 256;                                // N tile
+constexpr int GP_STAGE = G5_A_BYTES + GP_NT * 128;        // 16 KB of A + 32 KB of B per k-block
+constexpr int GP_STG = 8 * 16 * 128 * 2;                  // fp16 staging tiles of the eight consumer warps, one 128-column pass
+constexpr int GP_THREADS = 4 * (G5_CONS + 1) * 32;        // two consumer warpgroups + the producer warpgroup (warps 8-11)
+constexpr int GP_REG_CONS = 232, GP_REG_PROD = 40;        // 2 x 128 x 232 + 128 x 40 <= 64 K registers
+
+__global__ void __cluster_dims__(GP_CL, 1, 1) __launch_bounds__(GP_THREADS, 1)
+gemm_f16_pair_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, GemmTc5Launch a) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    const int nstage = a.nstage;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const uint32_t rank = cluster_ctarank();
+    uint8_t* stg = smem + (size_t)nstage * GP_STAGE + (warp & 7) * 16 * 128 * 2;   // this consumer warp's staging tile
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)nstage * GP_STAGE + GP_STG);
+    uint64_t* empty = full + nstage;
+
+    if (tid == 0) {
+        for (int i = 0; i < nstage; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 4 * G5_CONS * GP_CL); }
+        fence_barrier_init();
+    }
+    __syncthreads();
+    cluster_sync_all();                                   // the barriers of both CTAs are initialised before any multicast or remote arrive
+    pdl_trigger();
+    pdl_wait();
+    const int nkb = a.Kp / 64;
+    const int pairs = a.tiles_m / GP_CL * a.ntiles_n;     // (M tile pair, N tile), N inner: clusters in flight share their A rows in L2
+    const int cluster = blockIdx.x / GP_CL, nclusters = gridDim.x / GP_CL;
+
+    if (warp >= 4 * G5_CONS) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(GP_REG_PROD));
+        if (warp == 4 * G5_CONS && lane == 0) {
+            int slot = 0; uint32_t ph = 0;
+            for (int pt = cluster; pt < pairs; pt += nclusters) {
+                const int mt = pt / a.ntiles_n * GP_CL + (int)rank, nt = pt % a.ntiles_n;
+                for (int kb = 0; kb < nkb; ++kb) {
+                    mbar_wait(&empty[slot], ph ^ 1);
+                    uint8_t* st = smem + (size_t)slot * GP_STAGE;
+                    mbar_arrive_expect_tx(&full[slot], GP_STAGE);   // my A box + both halves of B (mine and the peer's)
+                    tma_load_2d(st, &mapA, kb * 64, mt * 128, &full[slot]);
+                    tma_load_2d_multicast(st + G5_A_BYTES + rank * 128 * 128, &mapB, kb * 64, nt * GP_NT + (int)rank * 128, &full[slot],
+                                          (uint16_t)((1u << GP_CL) - 1));
+                    if (++slot == nstage) { slot = 0; ph ^= 1; }
+                }
+            }
+        }
+        __syncwarp();
+    } else {
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(GP_REG_CONS));
+        const int wg = warp >> 2, wi = warp & 3;
+        float acc[GP_NT / 2];
+        int slot = 0; uint32_t ph = 0;
+        for (int pt = cluster; pt < pairs; pt += nclusters) {
+            const int mt = pt / a.ntiles_n * GP_CL + (int)rank, nt = pt % a.ntiles_n;
+            int prev = -1;
+            for (int kb = 0; kb < nkb; ++kb) {
+                mbar_wait(&full[slot], ph);
+                wgmma_fence();
+                const uint32_t sa = smem_u32(smem + (size_t)slot * GP_STAGE);
+                const uint64_t adesc = wgmma_desc_sw128(sa + wg * 64 * 128), bdesc = wgmma_desc_sw128(sa + G5_A_BYTES);
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk) wgmma_f16_n256(acc, adesc + 2 * kk, bdesc + 2 * kk, (kb | kk) != 0);
+                wgmma_commit();
+                if (prev >= 0) {
+                    wgmma_wait<1>();
+                    if (lane == 0)
+                        for (uint32_t r = 0; r < GP_CL; ++r) mbar_arrive_cluster(mapa_u32(smem_u32(&empty[prev]), r));
+                }
+                prev = slot;
+                if (++slot == nstage) { slot = 0; ph ^= 1; }
+            }
+            wgmma_wait<0>();
+            if (lane == 0)
+                for (uint32_t r = 0; r < GP_CL; ++r) mbar_arrive_cluster(mapa_u32(smem_u32(&empty[prev]), r));
+            wgmma_fence_regs(acc);
+
+            // rows rib0 .. rib0 + 15 of this warp, columns nt * 256 + 128 p .. + 127 in pass p (accumulator columns 8 j + 2 (lane % 4) of
+            // the 256 are acc[4 j + 2 h + e], j = 16 p .. 16 p + 15).  Pairs are packed as they are staged: next to 128 accumulators
+            // there is no room for a packed copy of a pass.
+            const int rib0 = mt * 128 + wg * 64 + wi * 16;
+            __half* gbase = a.Y16 + (size_t)rib0 * a.ldY + nt * GP_NT;
+#pragma unroll
+            for (int p = 0; p < 2; ++p)
+                g5_store_f16_from<128>(stg, lane, [&](int j, int h) { return pack_half2(acc[64 * p + 4 * j + 2 * h], acc[64 * p + 4 * j + 2 * h + 1]); },
+                                       gbase + p * 128, a.ldY, a.rows_per_branch - rib0);
+        }
+    }
+    cluster_sync_all();                                   // no CTA leaves while its peer may still arrive on its barriers
+}
+
+static int gp_launch(const CUtensorMap& mA, const CUtensorMap& mB, GemmTc5Launch a, cudaStream_t s) {
+    a.nstage = (227 * 1024 - 1024 - 256 - GP_STG) / GP_STAGE;      // 4 stages of 48 KB + 32 KB of staging tiles
+    const size_t smem = (size_t)a.nstage * GP_STAGE + GP_STG + 1024 + 256;
+    cudaError_t e = cudaFuncSetAttribute(gemm_f16_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return (int)e;
+    // persistent: as many clusters as can be resident at once, never more than the tile pairs
+    cudaLaunchConfig_t q{};
+    q.gridDim = dim3(GP_CL); q.blockDim = dim3(GP_THREADS); q.dynamicSmemBytes = smem;
+    int ncl = 0;
+    e = cudaOccupancyMaxActiveClusters(&ncl, gemm_f16_pair_kernel, &q);
+    if (e != cudaSuccess) return (int)e;
+    if (ncl < 1) return (int)cudaErrorInvalidConfiguration;
+    const int pairs = a.tiles_m / GP_CL * a.ntiles_n;
+    if (ncl > pairs) ncl = pairs;
+    e = launch_chain(gemm_f16_pair_kernel, dim3(GP_CL * ncl), dim3(GP_THREADS), smem, s, mA, mB, a);
+    if (e != cudaSuccess) return (int)e;
+    return (int)cudaGetLastError();
+}
+
 // Input projection of the layer-wise LSTM path: C[M, N] = A[M, K] B[N, K]^T, fp16 operands, fp32 accumulation, fp16 result.
 // reference: the W_ih x_t half of nn.LSTM / nn.GRU (audio_zen/model/module/sequence_model.py:31-46,113-119), batched over all
 // rows and time steps because it has no recurrence.  M = row tiles x frames x 128, N = 4H (a multiple of 256), K = 64 or H.
 bool gemm_f16_supported(long long M, int N, int K) { return M > 0 && M % 128 == 0 && M / 128 < (1LL << 31) / 128 && N % 128 == 0 && K % 64 == 0 && K >= 64; }
 
+// 128 x 256 pair tiles (gemm_f16_pair_kernel) when N is a multiple of 256 and the 128-row M tiles pair up -- every call of the
+// layer-wise path: M = ntp x frames x 128 with ntp even -- unless g.tile_n = 128 asks for the 128 x 128 kernel
+bool gemm_f16_pair_tiles(const GemmF16Launch& g) { return g.tile_n != 128 && g.N % GP_NT == 0 && (g.M / 128) % GP_CL == 0; }
+
 int launch_gemm_f16(const void* A, const void* B, const GemmF16Launch& g, int num_sms, cudaStream_t s) {
-    if (!gemm_f16_supported(g.M, g.N, g.K) || g.ldc != g.N) return (int)cudaErrorInvalidValue;
+    if (!gemm_f16_supported(g.M, g.N, g.K) || g.ldc != g.N || (g.tile_n != 0 && g.tile_n != 128 && g.tile_n != GP_NT))
+        return (int)cudaErrorInvalidValue;
     alignas(64) CUtensorMap mA, mB;
     if (make_tmap_f16_2d(&mA, A, (uint64_t)g.M, (uint64_t)g.K, 128) || make_tmap_f16_2d(&mB, B, (uint64_t)g.N, (uint64_t)g.K, 128))
         return (int)cudaErrorInvalidValue;
@@ -421,6 +562,10 @@ int launch_gemm_f16(const void* A, const void* B, const GemmF16Launch& g, int nu
     a.Kp = g.K; a.NT = 128; a.ntiles_n = g.N / 128; a.Npad = g.N;
     a.rows_per_branch = (int)g.M; a.tiles_m = (int)(g.M / 128); a.nbranch = 1; a.Tp = 1; a.B = 1;
     a.epi = EPI5_F16OUT; a.Y16 = g.C; a.ldY = g.N;
+    if (gemm_f16_pair_tiles(g)) {
+        a.NT = GP_NT; a.ntiles_n = g.N / GP_NT;
+        return gp_launch(mA, mB, a, s);
+    }
     return g5_launch<EPI5_F16OUT, 128>(mA, mB, a, num_sms, s);
 }
 

@@ -20,6 +20,7 @@ SYMBOLS = [
     "fsn_plan_forward", "fsn_model_workspace_bytes", "fsn_model_last_plan", "fsn_model_plan", "fsn_model_release_workspace",
     "fsn_plan_forward_bins", "fsn_model_plan_bins", "fsn_model_last_plan_bins",
     "fsn_sw128_offset", "fsn_tc5_weight_stream_bytes", "fsn_tc5_pack_weights", "fsn_tc5_gate_row", "fsn_tc5r_weight_stream_bytes", "fsn_tc5r_pack_layer",
+    "fsn_gemm_f16", "fsn_gemm_f16_tile_n",
 ]
 
 
@@ -105,6 +106,9 @@ def load_library():
     lib.fsn_tc5r_weight_stream_bytes.restype = i64
     lib.fsn_tc5r_pack_layer.argtypes = [i32, i32, i32, vp, vp, vp, vp, i32, vp, vp, vp]
     lib.fsn_tc5_gate_row.restype = i32
+    lib.fsn_gemm_f16.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp]
+    lib.fsn_gemm_f16_tile_n.argtypes = [i64, i32, i32, i32]
+    lib.fsn_gemm_f16_tile_n.restype = i32
     _LIB = lib
     return lib
 

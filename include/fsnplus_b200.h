@@ -267,6 +267,13 @@ int64_t fsn_tc5r_weight_stream_bytes(int32_t hidden);
 int fsn_tc5r_pack_layer(int32_t hidden, int32_t k_in, int32_t k_pad, const float* w_ih, const float* w_hh, const float* b_ih,
                         const float* b_hh, int32_t gru, uint16_t* h_stream, uint16_t* h_wih, float* h_bias);
 
+/* The layer-wise path's input-projection GEMM alone (test / bench hook): d_c[M, N] = d_a[M, K] d_b[N, K]^T, fp16 row-major device
+ * buffers, fp32 accumulation, enqueued on `stream`.  M % 128 == 0, N % 128 == 0, K % 64 == 0.  tile_n: 0 (or 256) = 128 x 256 tiles
+ * on CTA pairs where N % 256 == 0 and M / 128 is even, else 128 x 128; 128 = always 128 x 128 (what FSN_GIN_GEMM=128 selects). */
+int fsn_gemm_f16(const void* d_a, const void* d_b, void* d_c, int64_t M, int32_t N, int32_t K, int32_t tile_n, void* stream);
+/* The N tile (128 or 256) fsn_gemm_f16 runs that shape with, or FSN_EINVAL for a shape it rejects; host only. */
+int32_t fsn_gemm_f16_tile_n(int64_t M, int32_t N, int32_t K, int32_t tile_n);
+
 #ifdef __cplusplus
 }
 #endif

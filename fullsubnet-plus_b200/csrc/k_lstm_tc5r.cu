@@ -15,7 +15,8 @@
 //     and multicasts it to both, so the L2 reads W_hh once per 128 sequences.  Two consumer warpgroups take the 128-column
 //     gate chunks in turn (m64n128k16, accumulator in registers): while one runs its cell update the other's MMAs are in
 //     flight.  Each warpgroup has a ring of its own, consumed strictly in order (a shared ring would let one warpgroup wait on a
-//     slot two phases ahead, which an mbarrier parity wait cannot tell from the phase before).  The epilogue adds Gin_l(t), does
+//     slot two phases ahead, which an mbarrier parity wait cannot tell from the phase before), and each ring a producer warp of its
+//     own, so that one warpgroup's slow slot never holds back the other's stream.  The epilogue adds Gin_l(t), does
 //     the cell update and writes h_l(t) both into the next step's A buffer and, for all but the last layer, as the next layer's
 //     GEMM input (fp16, row-major); the last layer applies the output Linear(H -> 2) and writes the mask (or the enhanced spectrum).
 // Long clips run one launch per time window (LstmTc5rLaunch::t0 / Tw, DESIGN.md §3.7): h enters from and leaves to a per-layer fp16
@@ -34,21 +35,27 @@ namespace fsn {
 constexpr int R5_STAGE = 16384;                 // one k-block of one chunk of the packed stream: 128 gate columns x 64 k x fp16
 constexpr int R5_CL = 2;                        // CTAs per cluster sharing the weight stream
 constexpr int R5_ROWS = 64;                     // sequences per CTA
-constexpr int R5_THREADS = 9 * 32;              // warps 0-7: two consumer warpgroups; warp 8: bulk-copy producer
+constexpr int R5_THREADS = 10 * 32;             // warps 0-7: two consumer warpgroups; warps 8, 9: the bulk-copy producers of rings 0, 1
 constexpr int R5_MAX_SMEM = 227 * 1024;
 constexpr int R5_XTILE = R5_ROWS * 128;         // one step's input tile of a CTA: 64 rows x 64 halves, SWIZZLE_128B
+constexpr int R5_FCPART = 2 * R5_ROWS * 2 * 4;  // last layer: [2 step parities][64 rows][2] fp32 Linear partials of warpgroup 1
 
+// Shared memory of one layer: [stages][h: 2 parities][input tiles: first layer][fc partials: last layer][barriers].  Whatever the
+// fixed part leaves goes to the weight rings; ring 0 gets (nstage + 1) / 2 slots, ring 1 nstage / 2.
 struct R5Plan { int nstage; size_t total; };
-static inline R5Plan r5_plan(int H) {
+static inline R5Plan r5_plan(int H, bool kx, bool last) {
     R5Plan p;
-    const size_t fixed = (size_t)2 * R5_ROWS * H * 2 /*h, two step parities*/ + 2 * R5_XTILE /*input tiles*/ + 2 * 2 * R5_ROWS * 2 * 4 /*fc partials*/ +
-                         1024 /*align*/ + 256;
+    const size_t fixed = (size_t)2 * R5_ROWS * H * 2 + (kx ? 2 * R5_XTILE : 0) + (last ? R5_FCPART : 0) + 1024 /*align*/ + 4 * 8 /*xfull, xempty*/;
     const long avail = R5_MAX_SMEM - (long)fixed;
-    p.nstage = (int)(avail / R5_STAGE) & ~1;                        // two rings of nstage / 2 slots, one per consumer warpgroup
+    p.nstage = (int)(avail / (R5_STAGE + 2 * 8));                  // a slot and its full / empty barriers
     if (p.nstage > 8) p.nstage = 8;
-    p.total = fixed + (size_t)(p.nstage > 0 ? p.nstage : 0) * R5_STAGE;
+    if (p.nstage < 0) p.nstage = 0;
+    p.total = fixed + (size_t)p.nstage * (R5_STAGE + 2 * 8);
     return p;
 }
+// first slot and slot count of ring r (the ring of consumer warpgroup r) out of nstage
+__device__ __forceinline__ int r5_ring_base(int nstage, int r) { return r ? (nstage + 1) / 2 : 0; }
+__device__ __forceinline__ int r5_ring_slots(int nstage, int r) { return r ? nstage / 2 : (nstage + 1) / 2; }
 
 bool lstm_tc5r_supported(int H, int O) { return H % 64 == 0 && H >= 64 && H <= 512 && O == 2; }
 size_t lstm_tc5r_cstate_bytes(int ntiles, int H) { return (size_t)((ntiles + 1) / 2 * 2) * H * 128 * sizeof(float); }
@@ -68,13 +75,13 @@ __global__ void __cluster_dims__(R5_CL, 1, 1) __launch_bounds__(R5_THREADS, 1) l
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* stages = smem;
     uint8_t* hbuf = stages + (size_t)nstage * R5_STAGE;                     // [2][KBH][64 rows][128 B], SWIZZLE_128B
-    uint8_t* xbuf = hbuf + 2 * HBUF;                                       // [2 step parities][R5_XTILE] input tiles (first layer)
-    float* fcpart = reinterpret_cast<float*>(xbuf + 2 * R5_XTILE);         // [2 step parities][64 rows][2]
-    uint64_t* full = reinterpret_cast<uint64_t*>(fcpart + 2 * R5_ROWS * 2);   // [2 rings][nstage / 2]
+    const int KX = a.ximg ? 1 : 0, KT = KX + KBH;                          // k-blocks per gate chunk: [input][hidden]
+    uint8_t* xbuf = hbuf + 2 * HBUF;                                       // [2 step parities][R5_XTILE] input tiles (first layer only)
+    float* fcpart = reinterpret_cast<float*>(xbuf + KX * 2 * R5_XTILE);    // [2 step parities][64 rows][2] (last layer only)
+    uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(fcpart) + (LAST ? R5_FCPART : 0));   // [nstage]: ring 0, ring 1
     uint64_t* empty = full + nstage;
     uint64_t* xfull = empty + nstage;                                      // [2]: input tile of the step parity landed
     uint64_t* xempty = xfull + 2;                                          // [2]: every MMA of the step that read it has retired
-    const int KX = a.ximg ? 1 : 0, KT = KX + KBH;                          // k-blocks per gate chunk: [input][hidden]
 
     if (tid == 0) {
         for (int i = 0; i < nstage; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 4 * R5_CL); }
@@ -94,32 +101,32 @@ __global__ void __cluster_dims__(R5_CL, 1, 1) __launch_bounds__(R5_THREADS, 1) l
     __syncthreads();
     cluster_sync_all();                                                    // barriers of both CTAs are initialised
 
-    if (warp == 8) {
-        // ======================= producer: my half of every k-block, multicast to both CTAs ===================
+    if (warp >= 8) {
+        // ======================= producer of ring r: my half of every k-block of the chunks j = r, r + 2, ..., multicast to both CTAs
+        // (one producer per ring, so neither ring waits for the other warpgroup to free a slot; weights do not depend on h, so each
+        // producer runs ahead into the next step as far as its ring allows)
         if (lane == 0) {
             constexpr uint32_t PART = R5_STAGE / R5_CL;
+            const int r = warp - 8, base = r5_ring_base(nstage, r), NS = r5_ring_slots(nstage, r);
             const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.wstream) + rank * PART;
             const uint64_t pol_w = l2_policy_evict_last();          // the weights, re-read every step by every cluster: must survive the Gin stream
-            const int NS = nstage / 2;
-            int slot[2] = {0, 0}; uint32_t ph[2] = {0, 0};
+            int slot = 0; uint32_t ph = 0;
             for (int t = t0; t < tend; ++t) {
-                if (KX) {                                           // my 64 rows of the step's input image
+                if (KX && r == 0) {                                 // my 64 rows of the step's input image
                     mbar_wait(&xempty[t & 1], ((t >> 1) & 1) ^ 1);
                     mbar_arrive_expect_tx(&xfull[t & 1], R5_XTILE);
                     bulk_g2s(xbuf + (t & 1) * R5_XTILE, reinterpret_cast<const uint8_t*>(a.ximg) + (((size_t)(cta >> 1) * a.Tw + (t - t0)) * 128 + (cta & 1) * R5_ROWS) * 128,
                              R5_XTILE, &xfull[t & 1]);
                 }
-                for (int j = 0; j < NCH; ++j) {
-                    const int r = j & 1, base = r * NS;             // chunk j goes to the ring of warpgroup j % 2
+                for (int j = r; j < NCH; j += 2)
                     for (int q = 0; q < KT; ++q) {
-                        const int i = base + slot[r];
-                        mbar_wait(&empty[i], ph[r] ^ 1);
+                        const int i = base + slot;
+                        mbar_wait(&empty[i], ph ^ 1);
                         mbar_arrive_expect_tx(&full[i], R5_STAGE);
                         bulk_g2s_multicast(stages + (size_t)i * R5_STAGE + rank * PART, wsrc + (size_t)(j * KT + q) * R5_STAGE, PART, &full[i],
                                            (uint16_t)((1u << R5_CL) - 1), pol_w);
-                        if (++slot[r] == NS) { slot[r] = 0; ph[r] ^= 1; }
+                        if (++slot == NS) { slot = 0; ph ^= 1; }
                     }
-                }
             }
         }
     } else {
@@ -139,8 +146,8 @@ __global__ void __cluster_dims__(R5_CL, 1, 1) __launch_bounds__(R5_THREADS, 1) l
         float* cbase = a.cstate + (size_t)cta * NCH * 4 * 128 * 4;
         float acc[64];
         const bool has_gin = a.gin != nullptr;
-        const int NS = nstage / 2;
-        int rslot = 0; uint32_t rph = 0;                            // position in this warpgroup's ring (slots wg * NS ..)
+        const int rbase = r5_ring_base(nstage, wg), NS = r5_ring_slots(nstage, wg);
+        int rslot = 0; uint32_t rph = 0;                            // position in this warpgroup's ring (slots rbase ..)
         for (int t = t0; t < tend; ++t) {
             const uint8_t* hA = hbuf + (size_t)(t & 1) * HBUF;
             uint8_t* hN = hbuf + (size_t)((t + 1) & 1) * HBUF;
@@ -169,7 +176,7 @@ __global__ void __cluster_dims__(R5_CL, 1, 1) __launch_bounds__(R5_THREADS, 1) l
                 int prev = -1;
 #pragma unroll 1
                 for (int kb = 0; kb < KT; ++kb) {
-                    const int slot = wg * NS + rslot;
+                    const int slot = rbase + rslot;
                     mbar_wait(&full[slot], rph);
                     if (++rslot == NS) { rslot = 0; rph ^= 1; }
                     wgmma_fence();
@@ -321,7 +328,7 @@ static int r5_dispatch(const LstmTc5rLaunch& a, int grid, const R5Plan& p, cudaS
 
 int launch_lstm_tc5r(const LstmTc5rLaunch& a, cudaStream_t s) {
     if (!lstm_tc5r_supported(a.H, 2) || a.Tw < 1 || a.t0 < 0 || a.t0 % 4 || a.t0 + a.Tw > a.Tp) return (int)cudaErrorInvalidValue;
-    const R5Plan p = r5_plan(a.H);
+    const R5Plan p = r5_plan(a.H, a.ximg != nullptr, a.last != 0);
     if (p.nstage < 2) return (int)cudaErrorInvalidValue;
     const int grid = (a.ntiles + 1) / 2 * 2 * (128 / R5_ROWS);    // whole clusters; the buffers cover the padded tile pair
     switch (a.H) {

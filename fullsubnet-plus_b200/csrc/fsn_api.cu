@@ -63,10 +63,17 @@ struct TcnWeights {
 // activations [rows, 512] before and after the depth-wise convolution, and the statistics (tcn_stats_bytes).
 struct TcnScratch {
     DevBuf xa, xb, y1, y2, stats;
-    long long rows = 0;                                // rows the tensor maps were encoded for (0: none)
     alignas(64) unsigned char mapXa[128], mapXb[128], mapY2[128];
-    void release() { xa.release(); xb.release(); y1.release(); y2.release(); stats.release(); rows = 0; }
 };
+
+// The geometry a lane's workspaces were last sized for: B clips of T frames, window Tw, bin chunk Fc (0: whole clip / all bins); B = 0: none
+struct WsGeo {
+    int B = 0, T = 0, Tw = 0, Fc = 0;
+    bool operator!=(const WsGeo& o) const { return B != o.B || T != o.T || Tw != o.Tw || Fc != o.Fc; }
+};
+
+// The plan of a plain forward: sub-batch Bs, window Tw, bin chunk Fc (0: whole clip / all bins), workspace bytes (ws_sizes)
+struct Plan { int Bs = 0, Tw = 0, Fc = 0; int64_t bytes = 0; };
 
 // Statistics of a TCN with Z gLN groups: [8 blocks][gLN1, gLN2][Z][sum, sum of squares] doubles, then [8 blocks][Z] floats, the max |x|
 // per group of the stream entering each block (the fp16 store scale of its hidden activation).
@@ -86,14 +93,13 @@ struct fsn_model {
     DevBuf sb_frag[4], sb_bias[4];
     DevBuf fb_frag[4], fb_bias[4];
     // layer-wise wgmma path (k_lstm_tc5r.cu): per-layer recurrent streams, permuted input-projection matrices, biases
-    bool tc5r_ok = false;
     DevBuf r_stream[4], r_wih[4], r_bias[4], r_gin, r_hseq;    // r_wih: input-projection matrices of the layers > 0
     DevBuf r_hstate, sb_cum;                           // windowed forwards: per-layer h at the window's end, the packer's cumulative sums
     // Front-end workspaces (everything the full-band stage writes and the sub-band LSTM reads), grow-only, keyed by the last
-    // (B, T).  TWO lanes: the pipelined entry points (fsn_model_submit / fsn_model_forward_host_async) run the front end of
+    // geometry.  TWO lanes: the pipelined entry points (fsn_model_submit / fsn_model_forward_host_async) run the front end of
     // batch i+1 in lane (i+1)&1 on the front stream while the sub-band LSTM of batch i still reads lane i&1 on the LSTM stream.
     struct Lane {
-        int wsB = 0, wsT = 0, wsTw = 0, wsFc = 0;      // wsTw / wsFc: sub-band window / bin chunk of the last geometry (0: whole clip / all bins)
+        WsGeo geo;
         DevBuf fbin, fbout, mu, ximg, magpad, fbx, hseq;
         DevBuf x0, xr;                                 // time-major fb input / relu'd last residual
         TcnScratch tcn;                                // the full-band TCN's blocks (written on the front stream)
@@ -104,11 +110,6 @@ struct fsn_model {
         alignas(64) unsigned char mapX0[128], mapXr[128], mapSbx[128];
         cudaEvent_t ev_front = nullptr, ev_lstm = nullptr;   // front end written / LSTM finished reading this lane
         bool used = false;                             // ev_lstm has been recorded (a pipelined batch ran / may still run in this lane)
-        void release_all() {
-            DevBuf* all[] = {&fbin, &fbout, &mu, &ximg, &magpad, &fbx, &hseq, &x0, &xr, &tsse_scale, &sb_rowsum, &xn, &sigma, &sbx, &tlen};
-            for (auto* b : all) b->release();
-            tcn.release();
-        }
     } lane[2];
     int last_lane = 0;
     DevBuf cstate, mask_tmp, stage_in[3], stage_out;   // LSTM-side scratch (one LSTM runs at a time), host-entry staging
@@ -136,8 +137,7 @@ struct fsn_model {
     double ws_cap_bytes = 24e9;                        // FSN_WS_CAP_GB: larger batches are run as sub-batches (plain forward entry points)
     int env_sb_window = 0;                             // FSN_SB_WINDOW: force a sub-band time window of this many frames (multiple of 32)
     int env_sb_chunk = 0;                              // FSN_SB_CHUNK: run the sub-band TCN in chunks of this many bins (>= num_freqs: unchunked)
-    int plan_Bs = 0, plan_Tw = 0, plan_Fc = 0;         // plan of the last plain forward (fsn_plan_forward_bins): sub-batch, window (0: whole
-                                                       // clip), bin chunk (0: all bins)
+    Plan plan;                                         // plan of the last plain forward
     bool env_no_ws = false;
     int env_gin_tile_n = 0;                            // FSN_GIN_GEMM=128: the input-projection GEMM on 128 x 128 tiles (GemmF16Launch::tile_n)
     // pipelined execution: front-end stream, LSTM stream (higher priority), copy-in / copy-out streams, per-slot events
@@ -197,10 +197,28 @@ static void tcn_specs(std::vector<ParamSpec>& v, const std::string& pre, int C, 
     add(v, pre + ".fc_output_layer.bias", O);
 }
 
+// Channels of the sub-band input: a bin with 2 Ns neighbours of the magnitude, and with 2 Nf of each full-band output (3 in FullSubNet+)
+static int sb_input_size(const fsn_config& c) {
+    return (2 * c.sb_num_neighbors + 1) + (c.model_kind == FSN_KIND_PLUS ? 3 : 1) * (2 * c.fb_num_neighbors + 1);
+}
+
+// The layer-wise kernels (k_lstm_tc5r.cu) take this geometry (hidden % 64 == 0 and <= 512, output_size 2, input <= 64): their weights are packed
+static bool tc5r_ok(const fsn_config& c) {
+    return !c.sb_tcn && lstm_tc5r_supported(c.sb_hidden, c.output_size) && sb_input_size(c) <= 64;
+}
+
+// The sub-band LSTM runs layer-wise (else on the generic mma.sync kernel): lstm_impl = auto or tcgen05 (FSN_LSTM_TCGEN05, the historical
+// name of the tensor-core path) on a geometry those kernels take.  env_impl: FSN_LSTM_IMPL or 0.
+static bool runs_layerwise(const fsn_config& c, int env_impl) {
+    const int impl = env_impl ? env_impl : c.lstm_impl;
+    return tc5r_ok(c) && (impl == FSN_LSTM_AUTO || impl == FSN_LSTM_TCGEN05);
+}
+
 static void build_specs(fsn_model* m) {
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs;
     auto& v = m->specs;
+    m->Isb = sb_input_size(c);
     if (c.model_kind == FSN_KIND_PLUS) {
         const char* sfx[3] = {"", "_real", "_imag"};
         const char* cn[3] = {"smallConv1d", "middleConv1d", "largeConv1d"};
@@ -221,10 +239,8 @@ static void build_specs(fsn_model* m) {
             add(v, p + ".fc2.bias", F);
         }
         for (int b = 0; b < 3; ++b) tcn_specs(v, std::string("fb_model") + sfx[b], F, F);
-        m->Isb = (2 * c.sb_num_neighbors + 1) + 3 * (2 * c.fb_num_neighbors + 1);
     } else {
         lstm_specs(v, "fb_model", F, c.fb_hidden, c.num_layers, F, c.rnn_type == FSN_RNN_GRU ? 3 : 4);
-        m->Isb = (2 * c.sb_num_neighbors + 1) + (2 * c.fb_num_neighbors + 1);
     }
     if (c.sb_tcn) tcn_specs(v, "sb_model", m->Isb, c.output_size);       // hidden width 512: sb_hidden and num_layers are unused
     else lstm_specs(v, "sb_model", m->Isb, c.sb_hidden, c.num_layers, c.output_size, c.rnn_type == FSN_RNN_GRU ? 3 : 4);
@@ -443,7 +459,7 @@ extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
         for (int i = 0; i < 3; ++i)
             if (c.channel_attention == FSN_ATTN_TSSE && (c.kersize[i] < 1 || c.kersize[i] > 16)) return fail(FSN_EINVAL, "kersize must be in 1..16");
     }
-    const int isb = (2 * c.sb_num_neighbors + 1) + (c.model_kind == FSN_KIND_PLUS ? 3 : 1) * (2 * c.fb_num_neighbors + 1);
+    const int isb = sb_input_size(c);
     if (isb > 64) return fail(FSN_EINVAL, "sub-band input size %d > 64 not supported", isb);
     int sb_window = 0;
     if (const char* e = getenv("FSN_SB_WINDOW"); e && *e) {
@@ -488,20 +504,20 @@ extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
     return FSN_OK;
 }
 
+static void release_ws(fsn_model& m);
+
 extern "C" void fsn_model_destroy(fsn_model* m) {
     if (!m) return;
     cudaDeviceSynchronize();
-    DevBuf* all[] = {&m->arena, &m->cstate, &m->mask_tmp, &m->stage_in[0], &m->stage_in[1], &m->stage_in[2],
-                     &m->stage_out, &m->fb_fc, &m->fb_fc_b, &m->ws_h, &m->ws_bar, &m->sb_fc};
+    release_ws(*m);
+    DevBuf* all[] = {&m->arena, &m->stage_in[0], &m->stage_in[1], &m->stage_in[2], &m->stage_out, &m->fb_fc, &m->fb_fc_b, &m->sb_fc};
     for (auto* b : all) b->release();
-    m->tcn_fb.release(); m->tcn_sb.release(); m->sb_scratch.release();
+    m->tcn_fb.release(); m->tcn_sb.release();
     for (auto& ln : m->lane) {
-        ln.release_all();
         if (ln.ev_front) cudaEventDestroy(ln.ev_front);
         if (ln.ev_lstm) cudaEventDestroy(ln.ev_lstm);
     }
     for (int i = 0; i < 4; ++i) { m->r_stream[i].release(); m->r_wih[i].release(); m->r_bias[i].release(); }
-    m->r_gin.release(); m->r_hseq.release(); m->r_hstate.release(); m->sb_cum.release();
     if (m->s_front) { cudaStreamDestroy(m->s_front); cudaStreamDestroy(m->s_lstm); cudaEventDestroy(m->ev_in); }
     if (m->ev_plain) cudaEventDestroy(m->ev_plain);
     if (m->s_in) { cudaStreamDestroy(m->s_in); cudaStreamDestroy(m->s_out); for (int i = 0; i < 2; ++i) { cudaEventDestroy(m->ev_h2d[i]); cudaEventDestroy(m->ev_d2h[i]); cudaEventDestroy(m->ev_done[i]); } }
@@ -565,8 +581,7 @@ extern "C" int fsn_model_finalize(fsn_model* m) {
         const int Ipad = (c.num_freqs + 15) / 16 * 16;
         if (pack_lstm(m, "fb_model", c.num_freqs, Ipad, c.fb_hidden, c.num_layers, m->fb_frag, m->fb_bias)) return fail(FSN_ECUDA, "packing fb_model failed");
     }
-    m->tc5r_ok = !c.sb_tcn && lstm_tc5r_supported(c.sb_hidden, c.output_size) && m->Isb <= 64;
-    if (m->tc5r_ok) {
+    if (tc5r_ok(c)) {
         const int H = c.sb_hidden;
         for (int l = 0; l < c.num_layers; ++l) {
             const std::string q = "sb_model.sequence_model.", sl = std::to_string(l);
@@ -611,79 +626,49 @@ static void fill_ws(fsn_model* m, LstmWsLaunch& w) {
     w.L = c.num_layers; w.H = c.fb_hidden; w.I = c.num_freqs; w.Ipad = (c.num_freqs + 15) / 16 * 16; w.fast = c.fast_math; w.gru = c.rnn_type == FSN_RNN_GRU;
 }
 
-// lstm_impl = auto: the layer-wise wgmma path (input-projection GEMM + recurrent kernel per layer, k_lstm_tc5r.cu) when the geometry
-// fits (hidden % 64 == 0 and <= 512, output_size 2), else the generic mma.sync kernel; lstm_impl = mma forces the generic kernel.
-// (FSN_LSTM_TCGEN05 is the historical name of the tensor-core path.)
+// The implementation the sub-band LSTM reports (last_impl), and the one a forced lstm_impl names in its error
 static int pick_impl(const fsn_model* m) {
-    int impl = m->env_impl ? m->env_impl : m->cfg.lstm_impl;
-    if (impl == FSN_LSTM_AUTO) impl = m->tc5r_ok ? FSN_LSTM_TCGEN05 : FSN_LSTM_MMA;
-    return impl;
+    const int impl = m->env_impl ? m->env_impl : m->cfg.lstm_impl;
+    return runs_layerwise(m->cfg, m->env_impl) ? FSN_LSTM_TCGEN05 : impl == FSN_LSTM_AUTO ? FSN_LSTM_MMA : impl;
 }
-static bool use_layerwise(const fsn_model* m) { return pick_impl(m) == FSN_LSTM_TCGEN05 && m->tc5r_ok; }
 
-
-// Grow the scratch of TCN w to `rows` rows and Z gLN groups (grow-only; zero: a new allocation is zero-filled on stream s) and encode its
-// tensor maps when the rows change.  The mapped buffers' sizes depend on the rows alone, so they are only reallocated with new rows, after
-// a release or after a failed allocation (rows = 0 in the last two cases).
-static int grow_tcn_scratch(TcnScratch& sc, const TcnWeights& w, long long rows, size_t Z, bool zero, cudaStream_t s) {
-    int e = 0;
-    e |= sc.xa.ensure((size_t)rows * w.Cp * 4, zero, s);
-    e |= sc.xb.ensure((size_t)rows * w.Cp * 4, zero, s);
-    e |= sc.y1.ensure((size_t)rows * 512 * sizeof(__half), zero, s);
-    e |= sc.y2.ensure((size_t)rows * 512 * sizeof(__half), zero, s);
-    e |= sc.stats.ensure(tcn_stats_bytes(Z), zero, s);
-    if (e) {
-        sc.rows = 0;
-        return fail(FSN_ECUDA, "workspace allocation failed for the %s (%lld rows)", w.name, rows);
-    }
-    if (sc.rows != rows) {
-        if (make_tmap_f32_2d(sc.mapXa, sc.xa.p, rows, w.Cp, 128) || make_tmap_f32_2d(sc.mapXb, sc.xb.p, rows, w.Cp, 128) ||
-            make_tmap_f16_2d(sc.mapY2, sc.y2.p, rows, 512, 128))
-            return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the %s", w.name);
-        sc.rows = rows;
-    }
+// Encode the tensor maps of TCN w's scratch over `rows` rows
+static int map_tcn_scratch(TcnScratch& sc, const TcnWeights& w, long long rows) {
+    if (make_tmap_f32_2d(sc.mapXa, sc.xa.p, rows, w.Cp, 128) || make_tmap_f32_2d(sc.mapXb, sc.xb.p, rows, w.Cp, 128) ||
+        make_tmap_f16_2d(sc.mapY2, sc.y2.p, rows, 512, 128))
+        return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the %s", w.name);
     return FSN_OK;
 }
 
-// lstm_impl = auto / tcgen05 on a geometry the layer-wise kernels take, from the configuration alone (env_impl: FSN_LSTM_IMPL or 0)
-static bool config_layerwise(const fsn_config& c, int env_impl) {
-    const int isb = (2 * c.sb_num_neighbors + 1) + (c.model_kind == FSN_KIND_PLUS ? 3 : 1) * (2 * c.fb_num_neighbors + 1);
-    const bool ok = !c.sb_tcn && lstm_tc5r_supported(c.sb_hidden, c.output_size) && isb <= 64;
-    const int impl = env_impl ? env_impl : c.lstm_impl;
-    return ok && (impl == FSN_LSTM_AUTO || impl == FSN_LSTM_TCGEN05);
-}
-
-// Bytes of every forward workspace buffer ensure_ws requests for a batch of B clips of T frames, the sub-band images and the layer-wise
-// path's Gin / layer output sized by the window Tw (0: the whole clip), the sub-band TCN's input and scratch by the bin chunk Fc (0: all
-// bins).  ensure_ws allocates exactly these sizes, so the planner's count (fsn_plan_forward_bins) is what a forward asks for.
+// Bytes of every forward workspace buffer for a batch of B clips of T frames, the sub-band images and the layer-wise path's Gin / layer
+// output sized by the window Tw (0: the whole clip), the sub-band TCN's input and scratch by the bin chunk Fc (0: all bins).  One field
+// per entry of the table WS; ensure_ws allocates exactly these sizes, so the plan's count is what a forward holds.
 struct WsSizes {
-    size_t act = 0, mu = 0, tsse = 0, rowsum = 0, xn = 0;      // lane: fbin / fbout, mu / sigma, TSSE scale + row statistics, row sums, norms
-    size_t sbx = 0, ximg = 0;                                   // lane: sub-band TCN input, or the sub-band images
-    size_t x0 = 0, tcn_x = 0, tcn_y = 0, tcn_stats = 0;         // lane, FullSubNet+: x0 / xr, the TCN's two fp32 streams, two fp16 hidden, statistics
-    size_t magpad = 0, fbx = 0, fbhseq = 0;                     // lane, fullsubnet.Model
-    size_t cstate = 0, gin = 0, hseq = 0, hstate = 0, cum = 0;  // LSTM-side scratch
-    size_t sb_x = 0, sb_y = 0, sb_stats = 0;                    // sub-band TCN scratch
-    size_t tlen = 0, wsh = 0;                                   // ragged extents; fullsubnet.Model's weight-stationary h exchange + barrier
-    size_t total() const {
-        return 2 * act + 2 * mu + tsse + rowsum + xn + sbx + ximg + 2 * x0 + 2 * tcn_x + 2 * tcn_y + tcn_stats + magpad + fbx + fbhseq + cstate +
-               gin + hseq + hstate + cum + 2 * sb_x + 2 * sb_y + sb_stats + tlen + wsh;
-    }
+    size_t fbin = 0, fbout = 0, mu = 0, sigma = 0, tsse_scale = 0, sb_rowsum = 0, xn = 0, tlen = 0;       // lane: front end, ragged extents
+    size_t sbx = 0, ximg = 0;                                                   // lane: sub-band TCN input, or the sub-band images
+    size_t x0 = 0, xr = 0, tcn_xa = 0, tcn_xb = 0, tcn_y1 = 0, tcn_y2 = 0, tcn_stats = 0;   // lane, FullSubNet+: the full-band TCN
+    size_t magpad = 0, fbx = 0, hseq = 0;                                       // lane, fullsubnet.Model
+    size_t cstate = 0, r_gin = 0, r_hseq = 0, r_hstate = 0, sb_cum = 0;         // sub-band LSTM scratch
+    size_t sb_xa = 0, sb_xb = 0, sb_y1 = 0, sb_y2 = 0, sb_stats = 0;            // sub-band TCN scratch
+    size_t ws_h = 0, ws_bar = 0;                                                // fullsubnet.Model's weight-stationary h exchange, barrier
+    size_t mask_tmp = 0;                                                        // the generic kernel's scratch mask: not counted
+    size_t total() const;
 };
 static WsSizes ws_sizes(const fsn_config& c, bool layerwise, int B, int T, int Tw, int Fc = 0) {
     WsSizes z;
     const int F = c.num_freqs, Tp = T + c.look_ahead, Pp = (Tp + 3) & ~3, Ts = Tw ? Tw : Tp;
     const int nbr = (c.model_kind == FSN_KIND_PLUS) ? 3 : 1;
     const size_t rows = (size_t)B * F, ntiles = ((rows + 127) / 128 + 1) / 2 * 2;   // whole pairs of 128-row tiles (clusters of k_lstm_tc5r.cu)
-    z.act = (size_t)nbr * B * F * Pp * 4;
-    z.mu = (size_t)B * 4;
-    z.tsse = (size_t)nbr * B * F * 4 * (1 + tsse_row_floats());
-    z.rowsum = (size_t)B * 4 * F * 2 * 4;
-    z.tlen = (size_t)3 * B * sizeof(int32_t);                  // counted whether the forward is ragged or not
+    z.fbin = z.fbout = (size_t)nbr * B * F * Pp * 4;
+    z.mu = z.sigma = (size_t)B * 4;
+    z.tsse_scale = (size_t)nbr * B * F * 4 * (1 + tsse_row_floats());          // per-row scale | row statistics
+    z.sb_rowsum = (size_t)B * 4 * F * 2 * 4;
+    z.tlen = (size_t)3 * B * sizeof(int32_t);                                   // counted whether the forward is ragged or not
     if (c.norm_type != FSN_NORM_OFFLINE_LAPLACE) z.xn = (size_t)nbr * B * F * Tp * 4;
     if (c.sb_tcn) {
-        const size_t seqs = (size_t)B * (Fc ? Fc : F), srows = seqs * Tp;  // the sequences of one chunk run
-        z.sbx = srows * 64 * 4 + seqs * 4;
-        z.sb_x = srows * 64 * 4; z.sb_y = srows * 512 * sizeof(__half); z.sb_stats = tcn_stats_bytes(seqs);
+        const size_t seqs = (size_t)B * (Fc ? Fc : F), srows = seqs * Tp;      // the sequences of one chunk run
+        z.sbx = srows * 64 * 4 + seqs * 4;                                      // input | block 0's stream maxima
+        z.sb_xa = z.sb_xb = srows * 64 * 4; z.sb_y1 = z.sb_y2 = srows * 512 * sizeof(__half); z.sb_stats = tcn_stats_bytes(seqs);
     } else {
         z.ximg = ntiles * Ts * 16384;
     }
@@ -692,11 +677,11 @@ static WsSizes ws_sizes(const fsn_config& c, bool layerwise, int B, int T, int T
     if (layerwise) {
         const size_t M = ntiles * Ts * 128;
         cs5 = lstm_tc5r_cstate_bytes((int)ntiles, c.sb_hidden);
-        if (c.num_layers > 1) { z.gin = M * 4 * c.sb_hidden * 2; z.hseq = M * c.sb_hidden * 2; }
-        if (Tw) {                                                       // windowed: c / h of every layer carried to the next window
+        if (c.num_layers > 1) { z.r_gin = M * 4 * c.sb_hidden * 2; z.r_hseq = M * c.sb_hidden * 2; }
+        if (Tw) {                                                               // windowed: c / h of every layer carried to the next window
             cs5 *= c.num_layers;
-            z.hstate = (size_t)c.num_layers * ntiles * 128 * c.sb_hidden * 2;
-            if (c.norm_type == FSN_NORM_CUMULATIVE_LAPLACE || c.norm_type == FSN_NORM_CUMULATIVE_LAYER) z.cum = rows * 2 * sizeof(double);
+            z.r_hstate = (size_t)c.num_layers * ntiles * 128 * c.sb_hidden * 2;
+            if (c.norm_type == FSN_NORM_CUMULATIVE_LAPLACE || c.norm_type == FSN_NORM_CUMULATIVE_LAYER) z.sb_cum = rows * 2 * sizeof(double);
         }
     }
     if (c.model_kind == FSN_KIND_FSN) {
@@ -707,16 +692,86 @@ static WsSizes ws_sizes(const fsn_config& c, bool layerwise, int B, int T, int T
     z.cstate = cs > cs5 ? cs : cs5;
     if (c.model_kind == FSN_KIND_PLUS) {
         const size_t trows = (size_t)3 * B * Tp, Cp = (size_t)(F + 31) / 32 * 32;   // pack_tcn5's Cp
-        z.x0 = trows * Cp * 4;
-        z.tcn_x = trows * Cp * 4; z.tcn_y = trows * 512 * sizeof(__half); z.tcn_stats = tcn_stats_bytes((size_t)3 * B);
+        z.x0 = z.xr = trows * Cp * 4;
+        z.tcn_xa = z.tcn_xb = trows * Cp * 4; z.tcn_y1 = z.tcn_y2 = trows * 512 * sizeof(__half); z.tcn_stats = tcn_stats_bytes((size_t)3 * B);
     } else {
         const size_t Ipad = (F + 15) / 16 * 16, rows_pad = (B + 63) / 64 * 64;
         z.magpad = (size_t)B * F * Pp * 4;
         z.fbx = (size_t)Tp * rows_pad * Ipad * 2;
-        z.fbhseq = (size_t)B * c.fb_hidden * Pp * 4;
-        z.wsh = (size_t)c.num_layers * 2 * 64 * c.fb_hidden * 2 + 64;   // counted whether that kernel runs or not
+        z.hseq = (size_t)B * c.fb_hidden * Pp * 4;
+        z.ws_h = (size_t)c.num_layers * 2 * 64 * c.fb_hidden * 2; z.ws_bar = 64;   // counted whether that kernel runs or not
     }
     return z;
+}
+
+// The forward workspace: every buffer is one entry of WS.  ensure_ws sizes them (grows to the plan, gives back what exceeds it),
+// release_ws frees them, fsn_model_workspace_bytes and the plan (WsSizes::total) count them, all from this table.  ensure_ws
+// allocates in table order.
+using Lane = fsn_model::Lane;
+enum : unsigned {
+    WS_LANE = 1,        // one per lane (else one for the model, shared by both lanes: the sub-band stage runs one batch at a time)
+    WS_ZERO = 2,        // a fresh allocation is zero-filled, on the buffer's stream
+    WS_SL = 4,          // ordered on the sub-band stream sl (else the front stream s)
+    WS_REGEO = 8,       // a new geometry frees it first: the fresh zero-filled allocation keeps pad rows and columns zero
+    WS_ON_USE = 16,     // allocated where it is used, not by ensure_ws: ragged extents, weight-stationary LSTM, the scratch mask
+};
+struct WsBuf {
+    DevBuf& (*buf)(fsn_model&, Lane&);   // the buffer (a model's buffer ignores the lane)
+    size_t WsSizes::*need;               // its bytes in the plan
+    unsigned flags;
+};
+#define LANE_BUF(f) [](fsn_model&, Lane& ln) -> DevBuf& { return ln.f; }
+#define MODEL_BUF(f) [](fsn_model& m, Lane&) -> DevBuf& { return m.f; }
+static const WsBuf WS[] = {
+    {LANE_BUF(fbin), &WsSizes::fbin, WS_LANE | WS_ZERO},
+    {LANE_BUF(fbout), &WsSizes::fbout, WS_LANE | WS_ZERO},
+    {LANE_BUF(mu), &WsSizes::mu, WS_LANE | WS_ZERO},
+    {LANE_BUF(sigma), &WsSizes::sigma, WS_LANE | WS_ZERO},
+    {LANE_BUF(tsse_scale), &WsSizes::tsse_scale, WS_LANE | WS_ZERO},
+    {LANE_BUF(sb_rowsum), &WsSizes::sb_rowsum, WS_LANE | WS_ZERO},
+    {LANE_BUF(xn), &WsSizes::xn, WS_LANE | WS_ZERO},
+    {LANE_BUF(sbx), &WsSizes::sbx, WS_LANE | WS_REGEO},                            // fully written by the packer
+    // the sub-band TCN's scratch: every buffer is fully written before it is read (the pad columns by the packer / the epilogue)
+    {MODEL_BUF(sb_scratch.xa), &WsSizes::sb_xa, WS_SL},
+    {MODEL_BUF(sb_scratch.xb), &WsSizes::sb_xb, WS_SL},
+    {MODEL_BUF(sb_scratch.y1), &WsSizes::sb_y1, WS_SL},
+    {MODEL_BUF(sb_scratch.y2), &WsSizes::sb_y2, WS_SL},
+    {MODEL_BUF(sb_scratch.stats), &WsSizes::sb_stats, WS_SL},
+    {LANE_BUF(ximg), &WsSizes::ximg, WS_LANE | WS_ZERO | WS_REGEO},                // rows beyond B*F and k >= I stay zero
+    {MODEL_BUF(r_hstate), &WsSizes::r_hstate, WS_SL},
+    {MODEL_BUF(sb_cum), &WsSizes::sb_cum, WS_SL},
+    {MODEL_BUF(r_gin), &WsSizes::r_gin, WS_SL},
+    {MODEL_BUF(r_hseq), &WsSizes::r_hseq, WS_SL},
+    {MODEL_BUF(cstate), &WsSizes::cstate, WS_ZERO | WS_SL},
+    {LANE_BUF(x0), &WsSizes::x0, WS_LANE | WS_ZERO | WS_REGEO},                    // pad columns of x0 (and of every stream) stay zero
+    {LANE_BUF(xr), &WsSizes::xr, WS_LANE | WS_ZERO | WS_REGEO},
+    {LANE_BUF(tcn.xa), &WsSizes::tcn_xa, WS_LANE | WS_ZERO | WS_REGEO},
+    {LANE_BUF(tcn.xb), &WsSizes::tcn_xb, WS_LANE | WS_ZERO | WS_REGEO},
+    {LANE_BUF(tcn.y1), &WsSizes::tcn_y1, WS_LANE | WS_ZERO | WS_REGEO},
+    {LANE_BUF(tcn.y2), &WsSizes::tcn_y2, WS_LANE | WS_ZERO | WS_REGEO},
+    {LANE_BUF(tcn.stats), &WsSizes::tcn_stats, WS_LANE | WS_ZERO | WS_REGEO},
+    {LANE_BUF(magpad), &WsSizes::magpad, WS_LANE | WS_ZERO},
+    {LANE_BUF(fbx), &WsSizes::fbx, WS_LANE | WS_ZERO},
+    {LANE_BUF(hseq), &WsSizes::hseq, WS_LANE | WS_ZERO},
+    {LANE_BUF(tlen), &WsSizes::tlen, WS_LANE | WS_ON_USE},                         // stage_lengths
+    {MODEL_BUF(ws_h), &WsSizes::ws_h, WS_ON_USE},                                  // forward_impl
+    {MODEL_BUF(ws_bar), &WsSizes::ws_bar, WS_ON_USE},
+    {MODEL_BUF(mask_tmp), &WsSizes::mask_tmp, WS_ON_USE},                          // run_sb_lstm
+};
+
+size_t WsSizes::total() const {
+    size_t n = 0;
+    for (const WsBuf& e : WS) n += this->*e.need;
+    return n;
+}
+
+static void release_lane(fsn_model& m, Lane& ln) {
+    for (const WsBuf& e : WS) if (e.flags & WS_LANE) e.buf(m, ln).release();
+    ln.geo = WsGeo{};
+}
+static void release_ws(fsn_model& m) {
+    for (Lane& ln : m.lane) release_lane(m, ln);
+    for (const WsBuf& e : WS) if (!(e.flags & WS_LANE)) e.buf(m, m.lane[0]).release();
 }
 
 // Length limits of one forward (B clips of T frames), from the 32-bit quantities of the kernels on every path: the depth-wise TCN
@@ -739,82 +794,42 @@ static int check_length(const fsn_config& c, int B, int T) {
     return FSN_OK;
 }
 
-static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, int Tw, int Fc, cudaStream_t s, cudaStream_t sl) {
+// Size lane ln and the model's buffers for a forward of B clips of T frames with window Tw and bin chunk Fc (ws_sizes), each fresh
+// allocation zero-filled on its own stream (s: front end, sl: sub-band stage), and encode their tensor maps.
+static int ensure_ws(fsn_model* m, Lane& ln, int B, int T, int Tw, int Fc, cudaStream_t s, cudaStream_t sl) {
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs, Tp = T + c.look_ahead;
-    const WsSizes z = ws_sizes(c, use_layerwise(m), B, T, Tw, Fc);
-    const bool regeo = (ln.wsB != B || ln.wsT != T || ln.wsTw != Tw || ln.wsFc != Fc);
+    const long long srows = (long long)B * (Fc ? Fc : F) * Tp;          // sub-band TCN: the rows of one chunk run
+    if (c.sb_tcn && srows > SB_MAX_ROWS)
+        return fail(FSN_EINVAL, "B * %s * (T + look_ahead) = %lld rows exceeds the sub-band TCN's 2^31 limit", Fc ? "bins per chunk" : "num_freqs", srows);
+    if (c.model_kind == FSN_KIND_PLUS && !m->tcn5) return fail(FSN_ESTATE, "the TCN weights were not packed");
+    const WsSizes z = ws_sizes(c, runs_layerwise(c, m->env_impl), B, T, Tw, Fc);
+    const WsGeo geo{B, T, Tw, Fc};
+    const bool regeo = ln.geo != geo;
     if (Tw || Fc) {
-        // A windowed or bin-chunked forward exists to bound the workspace: first give back what earlier, longer, unwindowed or wider
-        // forwards grew beyond this one's need (the grow-only buffers of both lanes and the sub-band scratch), so the model then holds at
-        // most the plan's bytes.
-        // The buffers a new geometry releases anyway (images, x0 / xr, the TCN scratch) are left to that rule.
-        auto fit = [](DevBuf& b, size_t need) { if (b.bytes > need) b.release(); };
-        fit(ln.fbin, z.act); fit(ln.fbout, z.act); fit(ln.mu, z.mu); fit(ln.sigma, z.mu); fit(ln.tsse_scale, z.tsse);
-        fit(ln.sb_rowsum, z.rowsum); fit(ln.xn, z.xn); fit(ln.tlen, z.tlen); fit(ln.magpad, z.magpad); fit(ln.fbx, z.fbx); fit(ln.hseq, z.fbhseq);
-        fit(m->r_gin, z.gin); fit(m->r_hseq, z.hseq); fit(m->r_hstate, z.hstate); fit(m->sb_cum, z.cum); fit(m->cstate, z.cstate);
-        m->mask_tmp.release();
-        const TcnScratch& sc = m->sb_scratch;                            // released whole: its tensor maps go with its buffers
-        if (sc.xa.bytes > z.sb_x || sc.xb.bytes > z.sb_x || sc.y1.bytes > z.sb_y || sc.y2.bytes > z.sb_y || sc.stats.bytes > z.sb_stats)
-            m->sb_scratch.release();
-        fsn_model::Lane& other = m->lane[&ln == &m->lane[0] ? 1 : 0];    // the pipelined entry points' second lane
-        other.release_all(); other.wsB = other.wsT = other.wsTw = other.wsFc = 0;
+        // A windowed or bin-chunked forward exists to bound the workspace: first give back every buffer earlier forwards left larger than
+        // it needs, and the pipelined entry points' second lane, so that the model then holds at most the plan's bytes.
+        for (const WsBuf& e : WS) if (e.buf(*m, ln).bytes > z.*e.need) e.buf(*m, ln).release();
+        release_lane(*m, m->lane[&ln == &m->lane[0] ? 1 : 0]);
     }
-    int e = 0;
-    e |= ln.fbin.ensure(z.act, true, s);
-    e |= ln.fbout.ensure(z.act, true, s);
-    e |= ln.mu.ensure(z.mu, true, s);
-    e |= ln.sigma.ensure(z.mu, true, s);
-    e |= ln.tsse_scale.ensure(z.tsse, true, s);                          // per-row scale | row statistics
-    e |= ln.sb_rowsum.ensure(z.rowsum, true, s);
-    if (z.xn) e |= ln.xn.ensure(z.xn, true, s);
+    for (const WsBuf& e : WS) {
+        DevBuf& b = e.buf(*m, ln);
+        if (e.flags & WS_ON_USE) continue;
+        if (regeo && (e.flags & WS_REGEO)) b.release();
+        if (b.ensure(z.*e.need, e.flags & WS_ZERO, (e.flags & WS_SL) ? sl : s)) return fail(FSN_ECUDA, "workspace allocation failed for B=%d T=%d", B, T);
+    }
+    // every forward encodes the tensor maps on the buffers as they now are: none outlives the allocation it was encoded for
     if (c.sb_tcn) {
-        // sub-band TCN: the lane's packed input (+ block 0's stream maxima), the shared scratch of the blocks (serialised on the sub-band
-        // stream like the LSTM scratch); every buffer is fully written before it is read (the pad columns by the packer / the epilogue).
-        // A chunked forward sizes them for one chunk of Fc bins; a narrower last chunk leaves the rows past its own unread.
-        const long long seqs = (long long)B * (Fc ? Fc : F), srows = seqs * Tp;
-        if (srows > SB_MAX_ROWS)
-            return fail(FSN_EINVAL, "B * %s * (T + look_ahead) = %lld rows exceeds the sub-band TCN's 2^31 limit", Fc ? "bins per chunk" : "num_freqs", srows);
-        if (regeo) ln.sbx.release();
-        e |= ln.sbx.ensure(z.sbx, false, s);
-        if (e) return fail(FSN_ECUDA, "workspace allocation failed for B=%d T=%d", B, T);
-        if (regeo && make_tmap_f32_2d(ln.mapSbx, ln.sbx.p, srows, 64, 128)) return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the sub-band input");
-        int rc = grow_tcn_scratch(m->sb_scratch, m->tcn_sb, srows, (size_t)seqs, false, sl);
-        if (rc) return rc;
-    } else {
-        // images are re-zeroed whenever the geometry changes (rows beyond B*F and k >= I must stay zero)
-        if (regeo) { ln.ximg.release(); }
-        e |= ln.ximg.ensure(z.ximg, true, s);
+        if (make_tmap_f32_2d(ln.mapSbx, ln.sbx.p, srows, 64, 128)) return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the sub-band input");
+        if (int rc = map_tcn_scratch(m->sb_scratch, m->tcn_sb, srows)) return rc;
     }
-    // LSTM-side scratch: shared by both lanes (LSTM launches are serialised on the LSTM stream)
-    if (Tw) {
-        e |= m->r_hstate.ensure(z.hstate, false, sl);
-        if (z.cum) e |= m->sb_cum.ensure(z.cum, false, sl);
-    }
-    if (z.gin) {                                                         // Gin and the layer output of the deeper layers
-        e |= m->r_gin.ensure(z.gin, false, sl);
-        e |= m->r_hseq.ensure(z.hseq, false, sl);
-    }
-    if (z.cstate) e |= m->cstate.ensure(z.cstate, true, sl);
     if (c.model_kind == FSN_KIND_PLUS) {
-        if (!m->tcn5) return fail(FSN_ESTATE, "the TCN weights were not packed");
-        // a new geometry gets fresh zero-filled buffers: the pad columns of x0 (and so of every stream) must be zero
-        const size_t trows = (size_t)3 * B * Tp, Cp = m->tcn_fb.Cp;
-        if (regeo) { ln.x0.release(); ln.xr.release(); ln.tcn.release(); }
-        e |= ln.x0.ensure(z.x0, true, s);
-        e |= ln.xr.ensure(z.x0, true, s);
-        if (e) return fail(FSN_ECUDA, "workspace allocation failed for B=%d T=%d", B, T);
-        if (regeo && (make_tmap_f32_2d(ln.mapX0, ln.x0.p, trows, Cp, 128) || make_tmap_f32_2d(ln.mapXr, ln.xr.p, trows, Cp, 128)))
+        const long long trows = 3LL * B * Tp;
+        if (make_tmap_f32_2d(ln.mapX0, ln.x0.p, trows, m->tcn_fb.Cp, 128) || make_tmap_f32_2d(ln.mapXr, ln.xr.p, trows, m->tcn_fb.Cp, 128))
             return fail(FSN_ECUDA, "cuTensorMapEncodeTiled failed for the activations");
-        int rc = grow_tcn_scratch(ln.tcn, m->tcn_fb, (long long)trows, (size_t)3 * B, true, s);
-        if (rc) return rc;
-    } else {
-        e |= ln.magpad.ensure(z.magpad, true, s);
-        e |= ln.fbx.ensure(z.fbx, true, s);
-        e |= ln.hseq.ensure(z.fbhseq, true, s);
+        if (int rc = map_tcn_scratch(ln.tcn, m->tcn_fb, trows)) return rc;
     }
-    if (e) return fail(FSN_ECUDA, "workspace allocation failed for B=%d T=%d", B, T);
-    ln.wsB = B; ln.wsT = T; ln.wsTw = Tw; ln.wsFc = Fc;
+    ln.geo = geo;
     return FSN_OK;
 }
 
@@ -823,13 +838,13 @@ static int ensure_ws(fsn_model* m, fsn_model::Lane& ln, int B, int T, int Tw, in
 // Tw > 0: the sub-band stage runs in time windows of Tw frames (the last one shorter); for each window the images are packed (`sp`, the
 // front end's packer arguments) and every layer resumes from the h / c its previous window left (DESIGN.md §3.7).  Tw = 0: the images of
 // the whole clip are already packed and every layer runs once over all frames.
-static int run_sb_lstm(fsn_model* m, fsn_model::Lane& ln, int B, int T, int Tw, SbPackLaunch sp, float* d_out, const float* d_real,
+static int run_sb_lstm(fsn_model* m, Lane& ln, int B, int T, int Tw, SbPackLaunch sp, float* d_out, const float* d_real,
                        const float* d_imag, float* d_enh, const int* tlen, cudaStream_t s) {
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs, Tp = T + c.look_ahead, rows = B * F, ntiles = (rows + 127) / 128;
     const int impl = pick_impl(m);
     m->last_impl = impl;
-    if (use_layerwise(m)) {
+    if (runs_layerwise(c, m->env_impl)) {
         // one recurrent launch per layer; the first one also projects its input (the packed images), each deeper one is preceded by
         // one GEMM: the input projection of every row and time step of the window (k_gemm_tc5.cu)
         const int H = c.sb_hidden, ntp = (ntiles + 1) / 2 * 2;
@@ -971,7 +986,7 @@ static int run_tcn_blocks(fsn_model* m, const TcnWeights& w, TcnScratch& sc, con
 // Fc > 0: the sequences run in chunks of Fc bins (the last one narrower), each packed here from the front end's whole-clip outputs (`sp`,
 // the front end's packer arguments) into the same buffers; every sequence is its own gLN group, so nothing carries from one chunk to the
 // next (DESIGN.md §3.8).  Fc = 0: the input of all bins is already packed and the blocks run once.
-static int run_sb_tcn(fsn_model* m, fsn_model::Lane& ln, int B, int T, int Fc, SbPackLaunch sp, float* d_out, const float* d_real,
+static int run_sb_tcn(fsn_model* m, Lane& ln, int B, int T, int Fc, SbPackLaunch sp, float* d_out, const float* d_real,
                       const float* d_imag, float* d_enh, const int* tlen, cudaStream_t s) {
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs, Tp = T + c.look_ahead, W = Fc ? Fc : F;
@@ -1003,7 +1018,7 @@ static int run_sb_tcn(fsn_model* m, fsn_model::Lane& ln, int B, int T, int Fc, S
 // after the front end by the lane's ev_front).
 // Copy the per-sample extents frames[b] + look_ahead of a ragged forward into the lane's device buffer ln.tlen ([3][B]: one row per
 // full-band branch, so a full-band gLN group z = branch * B + b indexes it directly) through the next pinned staging slot.
-static int stage_lengths(fsn_model* m, fsn_model::Lane& ln, const int32_t* h_frames, int B, cudaStream_t s) {
+static int stage_lengths(fsn_model* m, Lane& ln, const int32_t* h_frames, int B, cudaStream_t s) {
     fsn_model::LenSlot& ls = m->len_slot[m->nlen++ % fsn_model::NLEN];
     const size_t n = (size_t)3 * B;
     if (!ls.ev) CK(cudaEventCreateWithFlags(&ls.ev, cudaEventDisableTiming));
@@ -1026,7 +1041,7 @@ static int stage_lengths(fsn_model* m, fsn_model::Lane& ln, const int32_t* h_fra
 // h_frames: the frame count of every sample of a ragged batch (validated by the caller), or null when every sample spans T frames
 // Tw: time window of the sub-band stage (0: the whole clip; > 0 needs s == sl, the plain entry points)
 // Fc: bin chunk of the sub-band TCN (0: all bins at once; > 0 needs s == sl, the plain entry points)
-static int forward_impl(fsn_model* m, fsn_model::Lane& ln, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
+static int forward_impl(fsn_model* m, Lane& ln, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
                         const int32_t* h_frames, float* d_out, float* d_enh, cudaStream_t s, cudaStream_t sl, int Tw = 0, int Fc = 0) {
     if (!m || !d_mag || (!d_out && !d_enh)) return fail(FSN_EINVAL, "null argument");
     if (d_enh && (!d_real || !d_imag)) return fail(FSN_EINVAL, "the enhanced-spectrum output needs the noisy real and imaginary planes");
@@ -1235,7 +1250,7 @@ static int submit_impl(fsn_model* m, cudaEvent_t ready, const float* d_mag, cons
     // shares the LSTM scratch): otherwise one lane, one stream -- the pipeline still overlaps copies and the caller's post-processing
     const bool overlap = m->env_front_overlap && (m->cfg.model_kind == FSN_KIND_PLUS);
     const int slot = overlap ? (int)(m->nsub & 1) : 0;
-    fsn_model::Lane& ln = m->lane[slot];
+    Lane& ln = m->lane[slot];
     cudaStream_t sf = overlap ? m->s_front : m->s_lstm;
     if (ready) CK(cudaStreamWaitEvent(sf, ready, 0));
     if (m->plain_pending) { CK(cudaStreamWaitEvent(sf, m->ev_plain, 0)); CK(cudaStreamWaitEvent(m->s_lstm, m->ev_plain, 0)); }
@@ -1268,6 +1283,12 @@ static double ws_bytes_per_sample(const fsn_config& c, bool layerwise, int T) {
     return b;
 }
 
+// The largest v in [lo, hi] with ok(v), or lo if there is none; ok(lo) is not asked.  ok must hold up to some v and fail after it.
+template <class Ok> static int largest(int lo, int hi, Ok ok) {
+    while (lo < hi) { const int mid = (lo + hi + 1) / 2; if (ok(mid)) lo = mid; else hi = mid - 1; }
+    return lo;
+}
+
 // The plan of a plain forward (fsn_plan_forward_bins): sub-batch Bs, sub-band window Tw (0: whole clip) and, for the sub-band TCN, bin
 // chunk Fc (0: all bins) so that the exact workspace (ws_sizes) stays within cap.
 //   * the sub-batch of the per-sample estimate, if it fits unwindowed: the forward of every release before windows existed;
@@ -1282,77 +1303,64 @@ static double ws_bytes_per_sample(const fsn_config& c, bool layerwise, int T) {
 //   * nothing fits: one clip at a time in one-bin chunks, allocated anyway.
 // Every chunk run keeps Bs * Fc * T' <= SB_MAX_ROWS.  force_bins > 0 (FSN_SB_CHUNK) chunks every TCN forward with exactly that many bins
 // (>= F: unchunked) and the largest equal split that fits with them.
-static void plan_forward(const fsn_config& c, bool layerwise, int B, int T, double cap, int force, int force_bins, int* pBs, int* pTw,
-                         int* pFc, int64_t* pbytes) {
+static Plan plan_forward(const fsn_config& c, bool layerwise, int B, int T, double cap, int force, int force_bins) {
     const int Tp = T + c.look_ahead, wmax = (Tp + 31) / 32 * 32;
     const long long blim = max_clips_for_rows(c, T);             // sub-batches never exceed the full-band TCN's row limit
     auto split = [&](int bmax) { if (bmax > blim) bmax = (int)blim; if (bmax < 1) bmax = 1; if (B <= bmax) return B; const int n = (B + bmax - 1) / bmax; return (B + n - 1) / n; };
     auto bytes = [&](int bs, int tw) { return (double)ws_sizes(c, layerwise, bs, T, tw).total(); };
-    // largest equal split whose workspace with window tw fits (0 if even one clip does not)
-    auto max_split = [&](int tw) {
-        int lo = 0, hi = B;                                             // invariant: split(lo) fits or lo == 0; split(hi + 1) does not
-        while (lo < hi) { const int mid = (lo + hi + 1) / 2; if (bytes(split(mid), tw) <= cap) lo = mid; else hi = mid - 1; }
-        return lo ? split(lo) : 0;
-    };
+    // largest equal split bs with fits(bs) (0 if even one clip does not fit)
+    auto max_split = [&](auto fits) { const int b = largest(0, B, [&](int v) { return fits(split(v)); }); return b ? split(b) : 0; };
     const double per = ws_bytes_per_sample(c, layerwise, T);
     const double bmax = cap / (per > 1 ? per : 1);
-    int Bs = split(bmax < B ? (int)bmax : B), Tw = 0, Fc = 0;
+    Plan p{split(bmax < B ? (int)bmax : B)};
     if (c.sb_tcn) {
         const int F = c.num_freqs;
         auto fits = [&](int bs, int fc) { return (long long)bs * fc * Tp <= SB_MAX_ROWS && ws_sizes(c, false, bs, T, 0, fc < F ? fc : 0).total() <= cap; };
         const int fforce = force_bins > 0 ? (force_bins < F ? force_bins : F) : 0;
-        if (fforce < F && (fforce > 0 || !fits(Bs, F))) {
-            if (fforce) {
-                int lo = 0, hi = B;                                     // largest equal split that fits with fforce bins
-                while (lo < hi) { const int mid = (lo + hi + 1) / 2; if (fits(split(mid), fforce)) lo = mid; else hi = mid - 1; }
-                Bs = lo ? split(lo) : 1; Fc = fforce;
-            } else {
-                long long best = -1;
-                Bs = 1; Fc = 1;
-                for (int n = 1, prev = 0; n <= B; ++n) {                // the equal splits, largest first
-                    const int bs = (B + n - 1) / n;
-                    if (bs == prev || bs > blim) continue;
-                    prev = bs;
-                    int lo = 0, hi = F;                                 // widest chunk that fits
-                    while (lo < hi) { const int mid = (lo + hi + 1) / 2; if (fits(bs, mid)) lo = mid; else hi = mid - 1; }
-                    if (!lo) continue;
-                    const int nch = (F + lo - 1) / lo;
-                    const long long runs = (long long)((B + bs - 1) / bs) * nch;
-                    if (best < 0 || runs < best) { best = runs; Bs = bs; Fc = (F + nch - 1) / nch; }
-                }
+        if (fforce) {                                                   // chunks of fforce bins (F: unchunked), the largest equal split that fits
+            if (fforce < F || !fits(p.Bs, F)) {
+                const int b = max_split([&](int bs) { return fits(bs, fforce); });
+                p.Bs = b ? b : 1;
             }
-            if (Fc >= F) Fc = 0;
-        } else if (fforce == F) {
-            int lo = 0, hi = B;                                         // FSN_SB_CHUNK >= F: unchunked, largest equal split that fits
-            if (!fits(Bs, F)) {
-                while (lo < hi) { const int mid = (lo + hi + 1) / 2; if (fits(split(mid), F)) lo = mid; else hi = mid - 1; }
-                Bs = lo ? split(lo) : 1;
+            p.Fc = fforce < F ? fforce : 0;
+        } else if (!fits(p.Bs, F)) {
+            long long best = -1;
+            p.Bs = 1; p.Fc = 1;
+            for (int n = 1, prev = 0; n <= B; ++n) {                    // the equal splits, largest first
+                const int bs = (B + n - 1) / n;
+                if (bs == prev || bs > blim) continue;
+                prev = bs;
+                const int fc = largest(0, F, [&](int v) { return fits(bs, v); });   // widest chunk that fits
+                if (!fc) continue;
+                const int nch = (F + fc - 1) / fc;
+                const long long runs = (long long)((B + bs - 1) / bs) * nch;
+                if (best < 0 || runs < best) { best = runs; p.Bs = bs; p.Fc = (F + nch - 1) / nch; }
             }
+            if (p.Fc >= F) p.Fc = 0;
         }
     } else if (layerwise && force > 0) {
-        Tw = force;
-        const int b = max_split(Tw);
-        Bs = b ? b : 1;
-    } else if (layerwise && bytes(Bs, 0) > cap) {
+        p.Tw = force;
+        const int b = max_split([&](int bs) { return bytes(bs, force) <= cap; });
+        p.Bs = b ? b : 1;
+    } else if (layerwise && bytes(p.Bs, 0) > cap) {
         int b = 0, wmin = 0;
         for (int w : {256, 32}) {
             wmin = w < wmax ? w : wmax;
-            if ((b = max_split(wmin))) break;
+            if ((b = max_split([&](int bs) { return bytes(bs, wmin) <= cap; }))) break;
         }
         if (!b) {
-            Bs = 1; Tw = 256 < wmax ? 256 : wmax;
+            p.Bs = 1; p.Tw = 256 < wmax ? 256 : wmax;
         } else if (bytes(b, 0) <= cap) {
-            Bs = b;                                                     // the smaller sub-batch fits unwindowed
+            p.Bs = b;                                                   // the smaller sub-batch fits unwindowed
         } else {
-            Bs = b;
-            int lo = wmin / 32, hi = wmax / 32;                         // longest window (in 32-frame units) that fits
-            while (lo < hi) { const int mid = (lo + hi + 1) / 2; if (bytes(Bs, 32 * mid) <= cap) lo = mid; else hi = mid - 1; }
-            const int nwin = (Tp + 32 * lo - 1) / (32 * lo);
-            Tw = ((Tp + nwin - 1) / nwin + 31) / 32 * 32;
+            p.Bs = b;
+            const int u = largest(wmin / 32, wmax / 32, [&](int v) { return bytes(b, 32 * v) <= cap; });   // longest window, in 32-frame units
+            const int nwin = (Tp + 32 * u - 1) / (32 * u);
+            p.Tw = ((Tp + nwin - 1) / nwin + 31) / 32 * 32;
         }
     }
-    *pBs = Bs; *pTw = Tw; *pFc = Fc;
-    if (pbytes) *pbytes = (int64_t)ws_sizes(c, layerwise, Bs, T, Tw, Fc).total();
+    p.bytes = (int64_t)ws_sizes(c, layerwise, p.Bs, T, p.Tw, p.Fc).total();
+    return p;
 }
 
 static int forward_plain(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
@@ -1368,9 +1376,8 @@ static int forward_plain(fsn_model* m, const float* d_mag, const float* d_real, 
     // a clip too long for the cap runs its sub-band stage in time windows (plan_forward) -- same bits, O(window) sub-band memory --
     // or, with the sub-band TCN, in bin chunks -- O(chunk) sub-band memory.
     if (int rc = check_length(m->cfg, 1, T)) return rc;
-    int Bs = B, Tw = 0, Fc = 0;
-    plan_forward(m->cfg, use_layerwise(m), B, T, m->ws_cap_bytes, m->env_sb_window, m->env_sb_chunk, &Bs, &Tw, &Fc, nullptr);
-    m->plan_Bs = Bs; m->plan_Tw = Tw; m->plan_Fc = Fc;
+    m->plan = plan_forward(m->cfg, runs_layerwise(m->cfg, m->env_impl), B, T, m->ws_cap_bytes, m->env_sb_window, m->env_sb_chunk);
+    const int Bs = m->plan.Bs, Tw = m->plan.Tw, Fc = m->plan.Fc;
     int rc = FSN_OK;
     if (Bs >= B) {
         rc = forward_impl(m, m->lane[0], d_mag, d_real, d_imag, B, T, h_frames, d_out, d_enh, s, s, Tw, Fc);
@@ -1558,10 +1565,10 @@ extern "C" int fsn_model_sync_host(fsn_model* m) {
 
 extern "C" int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst, int64_t numel, void* stream) {
     if (!m || !name || !d_dst) return fail(FSN_EINVAL, "null argument");
-    fsn_model::Lane& ln = m->lane[m->last_lane];
-    if (!ln.wsB) return fail(FSN_ESTATE, "no forward has run yet");
+    Lane& ln = m->lane[m->last_lane];
+    if (!ln.geo.B) return fail(FSN_ESTATE, "no forward has run yet");
     const fsn_config& c = m->cfg;
-    const int F = c.num_freqs, Tp = ln.wsT + c.look_ahead, Pp = (Tp + 3) & ~3, B = ln.wsB;
+    const int F = c.num_freqs, Tp = ln.geo.T + c.look_ahead, Pp = (Tp + 3) & ~3, B = ln.geo.B;
     const int nbr = (c.model_kind == FSN_KIND_PLUS) ? 3 : 1;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const std::string n(name);
@@ -1573,7 +1580,7 @@ extern "C" int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst,
     }
     if (n == "sb_in") {
         if (!c.sb_tcn) return fail(FSN_EINVAL, "sb_in is kept only by the sub-band TCN (sequence_model = \"TCN\")");
-        if (ln.wsFc) return fail(FSN_ESTATE, "sb_in is not kept: the last forward was chunked over bins (%d per chunk), its buffer holds the last chunk only", ln.wsFc);
+        if (ln.geo.Fc) return fail(FSN_ESTATE, "sb_in is not kept: the last forward was chunked over bins (%d per chunk), its buffer holds the last chunk only", ln.geo.Fc);
         if (numel != (int64_t)B * F * m->Isb * Tp) return fail(FSN_EINVAL, "sb_in needs %lld elements", (long long)B * F * m->Isb * Tp);
         launch_tm_to_fm(static_cast<const float*>(ln.sbx.p), 64, d_dst, B * F, m->Isb, Tp, s);
         CK(cudaGetLastError());
@@ -1755,6 +1762,12 @@ extern "C" float fsn_model_last_lstm_ms(fsn_model* m) {
 }
 extern "C" int fsn_model_last_lstm_impl(const fsn_model* m) { return m ? m->last_impl : 0; }
 
+static int put_plan(const Plan& p, int32_t* Bs, int32_t* Tw, int32_t* Fc, int64_t* bytes) {
+    *Bs = p.Bs; *Tw = p.Tw; *Fc = p.Fc;
+    if (bytes) *bytes = p.bytes;
+    return FSN_OK;
+}
+
 extern "C" int fsn_plan_forward_bins(const fsn_config* cfg, int32_t B, int32_t T, double cap_bytes, int32_t force_window, int32_t force_bins,
                                      int32_t* Bs, int32_t* Tw, int32_t* Fc, int64_t* bytes) {
     if (!cfg || !Bs || !Tw || !Fc || B < 1 || T < 1 || !(cap_bytes > 0)) return fail(FSN_EINVAL, "bad argument");
@@ -1762,10 +1775,7 @@ extern "C" int fsn_plan_forward_bins(const fsn_config* cfg, int32_t B, int32_t T
     if (force_bins < 0) return fail(FSN_EINVAL, "force_bins must be 0 or a positive number of bins");
     if (cfg->num_freqs < 4 || cfg->num_layers < 1 || cfg->num_layers > 4 || cfg->look_ahead < 0) return fail(FSN_EINVAL, "bad configuration");
     if (int rc = check_length(*cfg, 1, T)) return rc;
-    int bs = 0, tw = 0, fc = 0;
-    plan_forward(*cfg, config_layerwise(*cfg, 0), B, T, cap_bytes, force_window, force_bins, &bs, &tw, &fc, bytes);
-    *Bs = bs; *Tw = tw; *Fc = fc;
-    return FSN_OK;
+    return put_plan(plan_forward(*cfg, runs_layerwise(*cfg, 0), B, T, cap_bytes, force_window, force_bins), Bs, Tw, Fc, bytes);
 }
 
 extern "C" int fsn_plan_forward(const fsn_config* cfg, int32_t B, int32_t T, double cap_bytes, int32_t force_window, int32_t* Bs, int32_t* Tw,
@@ -1777,10 +1787,8 @@ extern "C" int fsn_plan_forward(const fsn_config* cfg, int32_t B, int32_t T, dou
 extern "C" int fsn_model_plan_bins(const fsn_model* m, int32_t B, int32_t T, int32_t* Bs, int32_t* Tw, int32_t* Fc, int64_t* bytes) {
     if (!m || !Bs || !Tw || !Fc || B < 1 || T < 1) return fail(FSN_EINVAL, "bad argument");
     if (int rc = check_length(m->cfg, 1, T)) return rc;
-    int bs = 0, tw = 0, fc = 0;
-    plan_forward(m->cfg, config_layerwise(m->cfg, m->env_impl), B, T, m->ws_cap_bytes, m->env_sb_window, m->env_sb_chunk, &bs, &tw, &fc, bytes);
-    *Bs = bs; *Tw = tw; *Fc = fc;
-    return FSN_OK;
+    return put_plan(plan_forward(m->cfg, runs_layerwise(m->cfg, m->env_impl), B, T, m->ws_cap_bytes, m->env_sb_window, m->env_sb_chunk),
+                    Bs, Tw, Fc, bytes);
 }
 
 extern "C" int fsn_model_plan(const fsn_model* m, int32_t B, int32_t T, int32_t* Bs, int32_t* Tw, int64_t* bytes) {
@@ -1791,35 +1799,26 @@ extern "C" int fsn_model_plan(const fsn_model* m, int32_t B, int32_t T, int32_t*
 extern "C" int fsn_model_release_workspace(fsn_model* m) {
     if (!m) return fail(FSN_EINVAL, "null model");
     CK(cudaDeviceSynchronize());                                         // nothing in flight may still read the buffers
-    for (auto& ln : m->lane) { ln.release_all(); ln.wsB = ln.wsT = ln.wsTw = ln.wsFc = 0; }
-    DevBuf* lstm[] = {&m->cstate, &m->mask_tmp, &m->r_gin, &m->r_hseq, &m->r_hstate, &m->sb_cum, &m->ws_h, &m->ws_bar};
-    for (auto* b : lstm) b->release();
-    m->sb_scratch.release();
+    release_ws(*m);
     return FSN_OK;
 }
 
 extern "C" int64_t fsn_model_workspace_bytes(const fsn_model* m) {
     if (!m) return 0;
+    fsn_model& mm = const_cast<fsn_model&>(*m);                          // the table's accessors are not const; nothing is changed
     size_t n = 0;
-    for (const auto& ln : m->lane) {
-        const DevBuf* all[] = {&ln.fbin, &ln.fbout, &ln.mu, &ln.ximg, &ln.magpad, &ln.fbx, &ln.hseq, &ln.x0, &ln.xr, &ln.tsse_scale,
-                               &ln.sb_rowsum, &ln.xn, &ln.sigma, &ln.sbx, &ln.tlen, &ln.tcn.xa, &ln.tcn.xb, &ln.tcn.y1, &ln.tcn.y2, &ln.tcn.stats};
-        for (const auto* b : all) n += b->bytes;
-    }
-    const DevBuf* lstm[] = {&m->cstate, &m->mask_tmp, &m->r_gin, &m->r_hseq, &m->r_hstate, &m->sb_cum, &m->ws_h, &m->ws_bar,
-                            &m->sb_scratch.xa, &m->sb_scratch.xb, &m->sb_scratch.y1, &m->sb_scratch.y2, &m->sb_scratch.stats};
-    for (const auto* b : lstm) n += b->bytes;
+    for (const WsBuf& e : WS)
+        for (int i = 0; i < ((e.flags & WS_LANE) ? 2 : 1); ++i) n += e.buf(mm, mm.lane[i]).bytes;
     return (int64_t)n;
 }
 
 extern "C" int fsn_model_last_plan(const fsn_model* m, int32_t* Bs, int32_t* Tw) {
     if (!m || !Bs || !Tw) return fail(FSN_EINVAL, "null argument");
-    *Bs = m->plan_Bs; *Tw = m->plan_Tw;
+    *Bs = m->plan.Bs; *Tw = m->plan.Tw;
     return FSN_OK;
 }
 
 extern "C" int fsn_model_last_plan_bins(const fsn_model* m, int32_t* Bs, int32_t* Tw, int32_t* Fc) {
     if (!m || !Bs || !Tw || !Fc) return fail(FSN_EINVAL, "null argument");
-    *Bs = m->plan_Bs; *Tw = m->plan_Tw; *Fc = m->plan_Fc;
-    return FSN_OK;
+    return put_plan(m->plan, Bs, Tw, Fc, nullptr);
 }

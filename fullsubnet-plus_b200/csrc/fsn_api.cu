@@ -1458,6 +1458,51 @@ extern "C" int fsn_model_forward_enhance_ragged(fsn_model* m, const float* d_mag
     int rc = check_frames(m, h_frames, B, T, &fr);
     return rc ? rc : forward_plain(m, d_mag, d_real, d_imag, B, T, fr, nullptr, d_enh, stream);
 }
+// Test hook: the sub-band stage alone on a given input, through the forward's own run_sb_lstm (its GEMM dispatch, per-layer state,
+// windows and epilogues); only the packer differs (SbPackLaunch::raw: the input as given instead of the normalised unfold)
+extern "C" int fsn_model_sb_forward(fsn_model* m, const float* d_x, int32_t B, int32_t T, int32_t Tw, const int32_t* h_frames,
+                                    float* d_out, const float* d_real, const float* d_imag, float* d_enh, void* stream) {
+    if (!m || !d_x || (!d_out && !d_enh)) return fail(FSN_EINVAL, "null argument");
+    if (!m->finalized) return fail(FSN_ESTATE, "fsn_model_finalize has not been called");
+    const fsn_config& c = m->cfg;
+    if (c.sb_tcn) return fail(FSN_EINVAL, "fsn_model_sb_forward runs the sub-band LSTM / GRU; this model's sub-band model is the TCN");
+    if (d_enh && (!d_real || !d_imag)) return fail(FSN_EINVAL, "the enhanced-spectrum output needs the noisy real and imaginary planes");
+    if (d_enh && c.output_size != 2) return fail(FSN_EINVAL, "the enhanced-spectrum output needs output_size 2 (a complex mask)");
+    if (B < 1 || T < 1) return fail(FSN_EINVAL, "bad batch/frames");
+    if (Tw < 0 || Tw % 32) return fail(FSN_EINVAL, "Tw = %d: the window must be 0 or a positive multiple of 32 frames", Tw);
+    if (Tw && !runs_layerwise(c, m->env_impl)) return fail(FSN_EINVAL, "time windows of the sub-band stage need the layer-wise LSTM path");
+    const int32_t* fr = nullptr;
+    int rc = check_frames(m, h_frames, B, T, &fr);
+    if (rc) return rc;
+    if ((rc = check_length(c, B, T))) return rc;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    for (auto& ln : m->lane)                                             // batches still in flight in the pipeline share the scratch buffers
+        if (ln.used) CK(cudaStreamWaitEvent(s, ln.ev_lstm, 0));
+    Lane& ln = m->lane[0];
+    if ((rc = ensure_ws(m, ln, B, T, Tw, 0, s, s))) return rc;
+    const int* tl = nullptr;
+    if (fr) {
+        if ((rc = stage_lengths(m, ln, fr, B, s))) return rc;
+        tl = static_cast<const int*>(ln.tlen.p);
+    }
+    m->launches = 0;
+    m->last_lane = 0;
+    SbPackLaunch sp{};
+    sp.raw = d_x;
+    sp.B = B; sp.F = c.num_freqs; sp.Tp = T + c.look_ahead; sp.Ns = c.sb_num_neighbors; sp.Nf = c.fb_num_neighbors;
+    sp.nfb = c.model_kind == FSN_KIND_PLUS ? 3 : 1;
+    sp.ximg = static_cast<__half*>(ln.ximg.p);
+    sp.t0 = 0; sp.Tw = sp.Tp;
+    sp.tlen = tl;
+    if (!Tw) {                                                          // windowed: run_sb_lstm packs each window
+        launch_sb_pack(sp, s);
+        m->launches++;
+    }
+    if ((rc = run_sb_lstm(m, ln, B, T, Tw, sp, d_out, d_real, d_imag, d_enh, tl, s))) return rc;
+    CK(cudaGetLastError());
+    return FSN_OK;
+}
+
 extern "C" int fsn_model_submit(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
                                 float* d_out, void* stream) {
     if (!d_out) return fail(FSN_EINVAL, "null argument");

@@ -85,6 +85,9 @@ struct SbPackLaunch {
     // xtm only: the bins f0 .. f0 + Fc - 1 of every sample (a chunk of the sub-band TCN; f0 = 0, Fc = F: all of them).  Sequence
     // (b, f) is row b * Fc + (f - f0) of xtm and amax; neighbours are still read from the absolute bins, reflected over the whole F
     int f0, Fc;
+    // test hook (fsn_model_sb_forward): the sub-band input itself, [B*F, I, Tp] fp32; launch_sb_pack then writes it into the images
+    // unnormalised (frames t0 .. t0 + Tw - 1 of every row of the padded tile pairs; rows >= B*F, columns >= I and frames past tlen zero)
+    const float* raw;
 };
 void launch_sb_stats(const SbPackLaunch& a, cudaStream_t s);
 void launch_sb_pack(const SbPackLaunch& a, cudaStream_t s);

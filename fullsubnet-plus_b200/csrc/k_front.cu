@@ -617,7 +617,27 @@ static void sb_pack_go(const SbPackLaunch& a, cudaStream_t s) {
         sb_pack_kernel<Store><<<dim3((a.Tw + SBP_T - 1) / SBP_T, (Fn + SBP_F - 1) / SBP_F, a.B), 256, smem, s>>>(a);
     }
 }
-void launch_sb_pack(const SbPackLaunch& a, cudaStream_t s) { sb_pack_go<Fp16Img>(a, s); }
+// The raw form (SbPackLaunch::raw): one thread per (row, frame, 8 channels), 8 consecutive threads write one row of a step's image
+__global__ void __launch_bounds__(256) sb_pack_raw_kernel(SbPackLaunch a) {
+    const int I = 2 * a.Ns + 1 + a.nfb * (2 * a.Nf + 1), rows = a.B * a.F;
+    const long long n = (long long)((rows + 255) / 256 * 2) * a.Tw * 128 * 8;     // every row of the padded tile pairs
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(i & 7), r = (int)((i >> 3) & 127);
+        const long long q = i >> 10;
+        const int row = (int)(q / a.Tw) * 128 + r, t = a.t0 + (int)(q % a.Tw);
+        float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        if (row < rows && t < (a.tlen ? a.tlen[row / a.F] : a.Tp))
+#pragma unroll
+            for (int e = 0; e < 8; ++e)
+                if (c * 8 + e < I) v[e] = a.raw[((size_t)row * I + c * 8 + e) * a.Tp + t];
+        Fp16Img::store(a, row, t, c * 8, v);
+    }
+}
+
+void launch_sb_pack(const SbPackLaunch& a, cudaStream_t s) {
+    if (a.raw) { sb_pack_raw_kernel<<<1024, 256, 0, s>>>(a); return; }
+    sb_pack_go<Fp16Img>(a, s);
+}
 void launch_sb_pack_tm(const SbPackLaunch& a, cudaStream_t s) {
     cudaMemsetAsync(a.amax, 0, (size_t)a.B * a.Fc * sizeof(float), s);
     sb_pack_go<Fp32Tm>(a, s);

@@ -202,3 +202,7 @@ int launch_lstm_mma(const LstmMmaLaunch& a, cudaStream_t s) {
 }
 
 }  // namespace fsn
+
+extern "C" int32_t fsn_lstm_mma_rows(int32_t L, int32_t H, int32_t Ipad, int32_t O) {
+    return (H % 16 || H < 16 || Ipad % 16 || L < 1 || L > 4 || O < 0) ? FSN_EINVAL : fsn::pick_rows(L, H, Ipad, O);
+}

@@ -404,3 +404,18 @@ extern "C" int fsn_tc5r_pack_layer(int32_t H, int32_t Kin, int32_t Kpad, const f
     std::memcpy(h_bias, bp.data(), bp.size() * 4);
     return FSN_OK;
 }
+
+extern "C" int fsn_tc5r_gin_weights(int32_t H, int32_t Kin, int32_t Kpad, const float* w_ih, uint16_t* h_wih) {
+    if (H % 64 || H < 64 || H > 512 || Kin < 1 || Kin > Kpad || !w_ih || !h_wih) return FSN_EINVAL;
+    const std::vector<float> zero((size_t)4 * H * H, 0.f);             // W_hh and the biases do not enter the input-projection matrix
+    std::vector<uint16_t> st, wp;
+    std::vector<float> bp;
+    fsn::lstm_tc5r_pack_layer(H, Kin, Kpad, w_ih, zero.data(), zero.data(), zero.data(), false, st, wp, bp);
+    fsn::lstm_tc5r_gin_order(H, Kpad, wp);
+    std::memcpy(h_wih, wp.data(), wp.size() * 2);
+    return FSN_OK;
+}
+
+extern "C" int32_t fsn_tc5r_ring_stages(int32_t H, int32_t first, int32_t last) {
+    return (H % 64 || H < 64 || H > 512) ? FSN_EINVAL : fsn::r5_plan(H, first != 0, last != 0).nstage;
+}

@@ -21,6 +21,7 @@ SYMBOLS = [
     "fsn_plan_forward_bins", "fsn_model_plan_bins", "fsn_model_last_plan_bins",
     "fsn_sw128_offset", "fsn_tc5_weight_stream_bytes", "fsn_tc5_pack_weights", "fsn_tc5_gate_row", "fsn_tc5r_weight_stream_bytes", "fsn_tc5r_pack_layer",
     "fsn_gemm_f16", "fsn_gemm_f16_tile_n",
+    "fsn_tc5r_gin_weights", "fsn_tc5r_ring_stages", "fsn_lstm_mma_rows", "fsn_model_sb_forward",
 ]
 
 
@@ -109,6 +110,12 @@ def load_library():
     lib.fsn_gemm_f16.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp]
     lib.fsn_gemm_f16_tile_n.argtypes = [i64, i32, i32, i32]
     lib.fsn_gemm_f16_tile_n.restype = i32
+    lib.fsn_tc5r_gin_weights.argtypes = [i32, i32, i32, vp, vp]
+    lib.fsn_tc5r_ring_stages.argtypes = [i32, i32, i32]
+    lib.fsn_tc5r_ring_stages.restype = i32
+    lib.fsn_lstm_mma_rows.argtypes = [i32, i32, i32, i32]
+    lib.fsn_lstm_mma_rows.restype = i32
+    lib.fsn_model_sb_forward.argtypes = [vp, vp, i32, i32, i32, C.POINTER(i32), vp, vp, vp, vp, vp]
     _LIB = lib
     return lib
 

@@ -266,6 +266,25 @@ int fsn_tc5_pack_weights(int32_t input_size, int32_t hidden, const float* w_ih0,
 int64_t fsn_tc5r_weight_stream_bytes(int32_t hidden);
 int fsn_tc5r_pack_layer(int32_t hidden, int32_t k_in, int32_t k_pad, const float* w_ih, const float* w_hh, const float* b_ih,
                         const float* b_hh, int32_t gru, uint16_t* h_stream, uint16_t* h_wih, float* h_bias);
+/* The input-projection matrix of a deeper layer exactly as fsn_model_finalize uploads it: [4 hidden, k_pad] fp16 whose row c gives
+ * Gin column c, in the order the recurrent kernel reads (column j*128 + p*32 + cg*8 + q*2 + e = gate q of unit 32 j + 8 cg + 2 p + e). */
+int fsn_tc5r_gin_weights(int32_t hidden, int32_t k_in, int32_t k_pad, const float* w_ih, uint16_t* h_wih);
+/* Weight-ring slots (shared-memory plan) of the layer-wise kernel for one layer role: first = input projection in the recurrence,
+ * last = fused output Linear.  FSN_EINVAL for a hidden size it does not take. */
+int32_t fsn_tc5r_ring_stages(int32_t hidden, int32_t first, int32_t last);
+/* Sequences per CTA (64, 32 or 16) the generic mma.sync kernel runs a stack of `layers` layers with (0: none fits). */
+int32_t fsn_lstm_mma_rows(int32_t layers, int32_t hidden, int32_t input_pad, int32_t output_size);
+
+/* Test hook: the sub-band LSTM / GRU stage of a finalized model alone, on a given sub-band input, through the forward's own layer and
+ * window loop (GEMM dispatch, per-layer cell / hidden state, fused epilogues); only the packer differs.
+ * d_x: [B, F, Isb, T + look_ahead] float32, device -- the normalised input sb_model receives (same layout as get_stage "sb_in");
+ * rounded to fp16 (nearest) like the forward's packed input.
+ * Tw: 0 = one launch per layer over all frames; else windows of Tw frames (positive multiple of 32; layer-wise path only).
+ * h_frames: NULL or B host frame counts, as fsn_model_forward_ragged.  Output: d_out [B, 2, F, T] (mask), or, when d_enh != NULL,
+ * the enhanced spectrum [B, F, T] complex64 from d_real / d_imag [B, F, T], as fsn_model_forward_enhance.
+ * FSN_EINVAL for a sub-band TCN model, a bad window or frame count; FSN_ESTATE before fsn_model_finalize. */
+int fsn_model_sb_forward(fsn_model* m, const float* d_x, int32_t B, int32_t T, int32_t Tw, const int32_t* h_frames,
+                         float* d_out, const float* d_real, const float* d_imag, float* d_enh, void* stream);
 
 /* The layer-wise path's input-projection GEMM alone (test / bench hook): d_c[M, N] = d_a[M, K] d_b[N, K]^T, fp16 row-major device
  * buffers, fp32 accumulation, enqueued on `stream`.  M % 128 == 0, N % 128 == 0, K % 64 == 0.  tile_n: 0 (or 256) = 128 x 256 tiles

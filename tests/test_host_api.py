@@ -228,6 +228,27 @@ def test_tc5r_layer_packing(built_lib):
     assert built_lib.fsn_tc5r_pack_layer(100, Kin, Kpad, vp(w_ih), vp(w_hh), vp(b_ih), vp(b_hh), 0, vp(stream), vp(wih), vp(bias)) != 0
 
 
+@pytest.mark.parametrize("H", [64, 384, 512])
+def test_tc5r_gin_column_order(built_lib, H):
+    """The deeper layers' input-projection matrix as finalize uploads it (lstm_tc5r_gin_order): Gin column
+    j * 128 + p * 32 + cg * 8 + q * 2 + e holds gate q of unit 32 j + 8 cg + 2 p + e -- the words the recurrent kernel's thread of
+    lane quad p reads for its units.  W_ih row r is tagged with r itself (exact in fp16 below 2048)."""
+    Kin, Kpad = H, H
+    w_ih = np.zeros((4 * H, Kin), np.float32)
+    w_ih[:, 0] = np.arange(4 * H)
+    w_ih[:, 1] = 1.0
+    out = np.zeros(4 * H * Kpad, np.uint16)
+    assert built_lib.fsn_tc5r_gin_weights(H, Kin, Kpad, C.c_void_p(w_ih.ctypes.data), C.c_void_p(out.ctypes.data)) == 0
+    wp = out.view(np.float16).reshape(4 * H, Kpad).astype(np.float32)
+    c = np.arange(4 * H)
+    j, p, cg, q, e = c // 128, (c // 32) % 4, (c // 8) % 4, (c // 2) % 4, c % 2
+    unit = 32 * j + 8 * cg + 2 * p + e
+    assert np.array_equal(wp[:, 0], q * H + unit)                       # nn.LSTM row of gate q, unit u: q * H + u
+    assert np.array_equal(wp[:, 1], np.ones(4 * H)) and not wp[:, 2:].any()
+    assert sorted(set((q * H + unit).tolist())) == list(range(4 * H))   # a permutation of the gate rows
+    assert built_lib.fsn_tc5r_gin_weights(96, Kin, Kpad, C.c_void_p(w_ih.ctypes.data), C.c_void_p(out.ctypes.data)) != 0
+
+
 def test_oracle_is_test_infrastructure_only():
     """Only tests/, __graft_entry__.smoke() and bench.py's CPU-baseline legs may import oracle/ (the product path has no CPU route)."""
     import os

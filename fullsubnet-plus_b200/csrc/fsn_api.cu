@@ -1645,10 +1645,19 @@ extern "C" int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst,
 // ---------------------------------------------------------------------------------------------
 struct fsn_stream {
     fsn_model* m;
-    int B, n = 0;
+    int B, n = 0;                                      // n: ticks of the handle (the weight-stationary exchange-buffer parity)
     DevBuf cum_in, cum_sb, fbin, fbx, hseq, fbout, ximg, c_fb, c_sb, h_fb, h_sb, ws_h, ws_c, ws_bar;
     bool use_ws = false;
     int ra_fb = 0, ra_sb = 0, rows_pad = 0, Ipad = 0;
+    // slot call (fsn_stream_step_slots): once used, every step runs per slot.  nb: frames each slot has consumed since its START
+    // (seeded with n at the first slot call); d_slot: this tick's per-slot counts for the kernels, -1 = held.  The counts reach the
+    // device through pinned staging slots, each refilled only after the event behind its last H2D copy has fired.
+    bool slots = false;
+    std::vector<int32_t> nb, all_step, valid;
+    DevBuf d_slot;
+    static const int NSTAGE = 4;
+    struct Stage { int32_t* h = nullptr; cudaEvent_t ev = nullptr; bool used = false; } stage[NSTAGE];
+    int64_t nstage = 0;
 };
 
 extern "C" int fsn_stream_create(fsn_model* m, int32_t B, fsn_stream** out) {
@@ -1689,16 +1698,39 @@ extern "C" void fsn_stream_destroy(fsn_stream* st) {
     if (!st) return;
     DevBuf* all[] = {&st->cum_in, &st->cum_sb, &st->fbin, &st->fbx, &st->hseq, &st->fbout, &st->ximg, &st->c_fb, &st->c_sb, &st->h_fb, &st->h_sb, &st->ws_h, &st->ws_c, &st->ws_bar};
     for (auto* b : all) b->release();
+    for (auto& g : st->stage) {
+        if (g.h) cudaFreeHost(g.h);
+        if (g.ev) cudaEventDestroy(g.ev);
+    }
+    st->d_slot.release();
     delete st;
 }
 
-extern "C" int fsn_stream_step(fsn_stream* st, const float* d_mag, float* d_mask, int32_t* h_valid, void* stream) {
-    if (!st || !d_mag || !d_mask) return fail(FSN_EINVAL, "null argument");
+// One tick of the handle.  slot: null (the lockstep step: every slot at frame n) or the device per-slot counts of the slot call;
+// reset: this tick has a START, so the slots at count 0 get their recurrent state zeroed first.
+static int stream_tick(fsn_stream* st, const float* d_mag, float* d_mask, const int* slot, bool reset, cudaStream_t s) {
     fsn_model* m = st->m;
     const fsn_config& c = m->cfg;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    const int B = st->B, F = c.num_freqs, n = st->n, resume = n > 0;
-    StreamNormLaunch na{d_mag, static_cast<float*>(st->fbin.p), static_cast<double*>(st->cum_in.p), B, F, 4, n, c.norm_type};
+    const int B = st->B, F = c.num_freqs, n = st->n, resume = slot ? 1 : n > 0;    // slot call: a START zeroes instead of resume = 0
+    if (reset) {
+        StreamResetLaunch r{};
+        auto add = [&](void* p, size_t layer_bytes, size_t row_bytes, int rows_per_slot) {
+            r.buf[r.nbuf++] = StreamResetBuf{p, layer_bytes, row_bytes, c.num_layers, rows_per_slot};
+        };
+        const size_t Hf = c.fb_hidden, Hs = c.sb_hidden;
+        if (st->use_ws) {                                // ws_h [L][2][64][Hf]: the parity this tick's step reads; ws_c [L][64][Hf]
+            add(static_cast<char*>(st->ws_h.p) + ((n ^ 1) & 1) * 64 * Hf * 2, 2 * 64 * Hf * 2, Hf * 2, 1);
+            add(st->ws_c.p, 64 * Hf * 4, Hf * 4, 1);
+        } else {                                         // generic full-band step: [L][ra_fb][Hf]
+            add(st->h_fb.p, st->ra_fb * Hf * 2, Hf * 2, 1);
+            add(st->c_fb.p, st->ra_fb * Hf * 4, Hf * 4, 1);
+        }
+        add(st->h_sb.p, st->ra_sb * Hs * 2, Hs * 2, F);  // sub-band: [L][ra_sb][Hs], slot b = rows b F .. b F + F - 1
+        add(st->c_sb.p, st->ra_sb * Hs * 4, Hs * 4, F);
+        r.B = B; r.slot = slot;
+        launch_stream_reset(r, s);
+    }
+    StreamNormLaunch na{d_mag, static_cast<float*>(st->fbin.p), static_cast<double*>(st->cum_in.p), B, F, 4, n, c.norm_type, slot};
     launch_stream_norm(na, s);
     launch_fb_pack(static_cast<const float*>(st->fbin.p), static_cast<__half*>(st->fbx.p), B, F, 1, 4, st->rows_pad, st->Ipad, s);
     int e = 0;
@@ -1708,7 +1740,7 @@ extern "C" int fsn_stream_step(fsn_stream* st, const float* d_mag, float* d_mask
         w.rows = B; w.rows_pad = st->rows_pad; w.Tp = 1;
         w.x = static_cast<const __half*>(st->fbx.p); w.hbuf = static_cast<__half*>(st->ws_h.p); w.cbuf = static_cast<float*>(st->ws_c.p);
         w.barrier = static_cast<unsigned int*>(st->ws_bar.p);
-        w.hseq = static_cast<float*>(st->hseq.p); w.P = 4; w.resume = resume; w.t0 = n;
+        w.hseq = static_cast<float*>(st->hseq.p); w.P = 4; w.resume = resume; w.t0 = n; w.slot = slot;
         e = launch_lstm_ws(w, s);
     } else {
         LstmMmaLaunch a{};
@@ -1717,7 +1749,7 @@ extern "C" int fsn_stream_step(fsn_stream* st, const float* d_mag, float* d_mask
         a.xplain = static_cast<const __half*>(st->fbx.p); a.rows_pad = st->rows_pad;
         a.cstate = static_cast<float*>(st->c_fb.p); a.rows_alloc = st->ra_fb;
         a.hseq = static_cast<float*>(st->hseq.p); a.P = 4; a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU;
-        a.hstate = static_cast<__half*>(st->h_fb.p); a.resume = resume;
+        a.hstate = static_cast<__half*>(st->h_fb.p); a.resume = resume; a.slot = slot; a.slot_rows = 1;
         e = launch_lstm_mma(a, s);
     }
     if (e) return fail(FSN_ECUDA, "full-band LSTM step failed: %s", cudaGetErrorString((cudaError_t)e));
@@ -1727,7 +1759,7 @@ extern "C" int fsn_stream_step(fsn_stream* st, const float* d_mag, float* d_mask
     cf.W = P(m, "fb_model.fc_output_layer.weight"); cf.bias = P(m, "fb_model.fc_output_layer.bias");
     launch_conv1x1(cf, s);
     StreamPackLaunch pa{d_mag, static_cast<const float*>(st->fbout.p), 4, static_cast<double*>(st->cum_sb.p), static_cast<__half*>(st->ximg.p),
-                        B, F, c.sb_num_neighbors, c.fb_num_neighbors, n, c.norm_type};
+                        B, F, c.sb_num_neighbors, c.fb_num_neighbors, n, c.norm_type, slot};
     launch_stream_pack(pa, s);
     LstmMmaLaunch b{};
     for (int l = 0; l < c.num_layers; ++l) { b.w.wfrag[l] = static_cast<const uint4*>(m->sb_frag[l].p); b.w.bias[l] = static_cast<const float*>(m->sb_bias[l].p); }
@@ -1736,12 +1768,67 @@ extern "C" int fsn_stream_step(fsn_stream* st, const float* d_mag, float* d_mask
     b.img = static_cast<const __half*>(st->ximg.p); b.ntiles = (B * F + 127) / 128;
     b.cstate = static_cast<float*>(st->c_sb.p); b.rows_alloc = st->ra_sb;
     b.out = d_mask; b.O = c.output_size; b.F = F; b.la = 0; b.act = c.sb_act; b.fast = c.fast_math; b.gru = c.rnn_type == FSN_RNN_GRU;
-    b.hstate = static_cast<__half*>(st->h_sb.p); b.resume = resume;
+    b.hstate = static_cast<__half*>(st->h_sb.p); b.resume = resume; b.slot = slot; b.slot_rows = F; b.slot_la = c.look_ahead;
     e = launch_lstm_mma(b, s);
     if (e) return fail(FSN_ECUDA, "sub-band LSTM step failed: %s", cudaGetErrorString((cudaError_t)e));
     CK(cudaGetLastError());
-    if (h_valid) *h_valid = (n >= c.look_ahead) ? 1 : 0;
     st->n++;
+    return FSN_OK;
+}
+
+extern "C" int fsn_stream_step_slots(fsn_stream* st, const float* d_mag, float* d_mask, const int32_t* h_flags, int32_t* h_valid,
+                                     void* stream) {
+    if (!st || !d_mag || !d_mask) return fail(FSN_EINVAL, "null argument");
+    if (!h_flags) return fail(FSN_EINVAL, "h_flags is null (one flag per slot, slots 0..%d)", st->B - 1);
+    if (!h_valid) return fail(FSN_EINVAL, "h_valid is null (one result per slot, slots 0..%d)", st->B - 1);
+    const int B = st->B, la = st->m->cfg.look_ahead;
+    bool reset = false;
+    for (int b = 0; b < B; ++b) {
+        const int f = h_flags[b];
+        if (f != FSN_SLOT_HOLD && f != FSN_SLOT_STEP && f != FSN_SLOT_START)
+            return fail(FSN_EINVAL, "slot %d: flag %d is not FSN_SLOT_HOLD (0), FSN_SLOT_STEP (1) or FSN_SLOT_START (2)", b, f);
+        reset = reset || f == FSN_SLOT_START;
+    }
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (!st->slots) {                                                   // until now every slot stepped with the handle
+        if (st->d_slot.ensure((size_t)B * sizeof(int32_t), false)) return fail(FSN_ECUDA, "slot-count buffer allocation failed");
+        st->nb.assign(B, st->n);
+        st->slots = true;
+    }
+    fsn_stream::Stage& g = st->stage[st->nstage++ % fsn_stream::NSTAGE];
+    if (!g.ev) CK(cudaEventCreateWithFlags(&g.ev, cudaEventDisableTiming));
+    if (g.used) CK(cudaEventSynchronize(g.ev));                         // the copy that last read this slot has completed
+    if (!g.h) CK(cudaHostAlloc(reinterpret_cast<void**>(&g.h), (size_t)B * sizeof(int32_t), cudaHostAllocDefault));
+    for (int b = 0; b < B; ++b)
+        g.h[b] = h_flags[b] == FSN_SLOT_HOLD ? -1 : h_flags[b] == FSN_SLOT_START ? 0 : st->nb[b];
+    CK(cudaMemcpyAsync(st->d_slot.p, g.h, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CK(cudaEventRecord(g.ev, s));
+    g.used = true;
+    const int rc = stream_tick(st, d_mag, d_mask, static_cast<const int*>(st->d_slot.p), reset, s);
+    if (rc) return rc;
+    for (int b = 0; b < B; ++b) {
+        if (g.h[b] >= 0) st->nb[b] = g.h[b] + 1;
+        h_valid[b] = g.h[b] >= 0 && st->nb[b] > la ? 1 : 0;
+    }
+    return FSN_OK;
+}
+
+extern "C" int fsn_stream_step(fsn_stream* st, const float* d_mag, float* d_mask, int32_t* h_valid, void* stream) {
+    if (!st || !d_mag || !d_mask) return fail(FSN_EINVAL, "null argument");
+    if (st->slots) {                                                    // the slot call with every slot stepping
+        st->all_step.assign(st->B, FSN_SLOT_STEP);
+        st->valid.resize(st->B);
+        const int rc = fsn_stream_step_slots(st, d_mag, d_mask, st->all_step.data(), st->valid.data(), stream);
+        if (rc) return rc;
+        bool all = true;
+        for (int v : st->valid) all = all && v;
+        if (h_valid) *h_valid = all ? 1 : 0;
+        return FSN_OK;
+    }
+    const int n = st->n;
+    const int rc = stream_tick(st, d_mag, d_mask, nullptr, false, static_cast<cudaStream_t>(stream));
+    if (rc) return rc;
+    if (h_valid) *h_valid = (n >= st->m->cfg.look_ahead) ? 1 : 0;
     return FSN_OK;
 }
 

@@ -106,11 +106,18 @@ void launch_apply_cirm(const float* crm, const float2* noisy, float2* enh, int B
 void launch_apply_cirm_planar(const float* crm, const float* nreal, const float* nimag, float2* enh, int B, int F, int T, const int* tlen,
                               int la, cudaStream_t s);
 
-// streaming step kernels (k_front.cu): one frame of the cumulative norms with running sums carried in global memory
-struct StreamNormLaunch { const float* x; float* y; double* cum; int B, F, P, n, type; };       // x [B,F] -> y [B,F,P] (t = 0)
+// streaming step kernels (k_front.cu): one frame of the cumulative norms with running sums carried in global memory.
+// slot: null (every slot is at frame n), or [B] per-slot frame counts of the slot call (fsn_stream_step_slots), -1 = held: a held
+// slot's frame is not read, its sums are untouched and its outputs are zero
+struct StreamNormLaunch { const float* x; float* y; double* cum; int B, F, P, n, type; const int* slot; };       // x [B,F] -> y [B,F,P] (t = 0)
 void launch_stream_norm(const StreamNormLaunch& a, cudaStream_t s);
-struct StreamPackLaunch { const float* mag; const float* fb; int Pfb; double* cum; __half* ximg; int B, F, Ns, Nf, n, type; };
+struct StreamPackLaunch { const float* mag; const float* fb; int Pfb; double* cum; __half* ximg; int B, F, Ns, Nf, n, type; const int* slot; };
 void launch_stream_pack(const StreamPackLaunch& a, cudaStream_t s);
+// zero the carried recurrent state of every slot whose count slot[b] is 0 (the slots a START resets): per buffer, L layers of
+// `rows_per_slot` rows of `row_bytes` each, layer l at p + l * layer_bytes, slot b's rows from b * rows_per_slot
+struct StreamResetBuf { void* p; size_t layer_bytes, row_bytes; int L, rows_per_slot; };
+struct StreamResetLaunch { StreamResetBuf buf[4]; int nbuf, B; const int* slot; };
+void launch_stream_reset(const StreamResetLaunch& a, cudaStream_t s);
 
 // ---- k_lstm_mma.cu ---------------------------------------------------------------------------
 struct LstmMmaWeights {       // device, produced by pack (fsn_api.cu)
@@ -137,6 +144,10 @@ struct LstmMmaLaunch {
     // streaming: hidden state carried across launches ([L, rows_alloc, H] fp16); resume = 1 continues from it
     __half* hstate; int resume;
     const int* tlen;          // optional [B] per-sample extent in frames of Tp: output frames t - la >= tlen[b] - la are written as zero
+    // optional (streaming slot call, Tp = 1): per-slot frame counts, -1 = held; row r belongs to slot r / slot_rows.  A held row
+    // writes neither cstate nor hstate.  The fused-FC output of a slot whose count is below slot_la (held, or still filling its
+    // look-ahead) is zero
+    const int* slot; int slot_rows, slot_la;
 };
 size_t lstm_mma_cstate_bytes(int L, int rows, int H, int* rows_alloc);
 int launch_lstm_mma(const LstmMmaLaunch& a, cudaStream_t s);   // returns 0 or cudaError
@@ -152,6 +163,8 @@ struct LstmWsLaunch {
     float* hseq; int P;       // top-layer h as fp32 [rows, H, P]
     int fast, resume, t0;     // t0: absolute index of the first step (exchange-buffer parity)
     int gru;                  // 1: pseudo-gate GRU cell, cbuf / cst carry h in fp32
+    const int* slot;          // optional (streaming slot call, Tp = 1): [rows] per-slot frame counts, -1 = held: the row keeps its
+                              // cell state and carries its previous h into this step's exchange-buffer parity
 };
 bool lstm_ws_supported(int L, int H, int Ipad, int rows, int num_sms);
 int launch_lstm_ws(const LstmWsLaunch& a, cudaStream_t s);

@@ -664,6 +664,11 @@ __global__ void __launch_bounds__(256) stream_norm_kernel(StreamNormLaunch a) {
     __shared__ double red[16];
     __shared__ float s_a, s_b;
     const int b = blockIdx.x, F = a.F;
+    const int n = a.slot ? a.slot[b] : a.n;                         // this slot's frame count (block-uniform)
+    if (n < 0) {                                                    // held: frame unread, sums untouched
+        for (int f = threadIdx.x; f < F; f += blockDim.x) a.y[((size_t)b * F + f) * a.P] = 0.f;
+        return;
+    }
     const float* x = a.x + (size_t)b * F;
     double s = 0, q = 0;
     for (int f = threadIdx.x; f < F; f += blockDim.x) { const double v = x[f]; s += v; q += v * v; }
@@ -675,9 +680,9 @@ __global__ void __launch_bounds__(256) stream_norm_kernel(StreamNormLaunch a) {
         double ts = 0, tq = 0;
         for (int i = 0; i < 8; ++i) { ts += red[i]; tq += red[8 + i]; }
         const double EPS = 1.1920928955078125e-07;
-        const double cs = (a.n == 0 ? 0.0 : a.cum[2 * b]) + ts, cq = (a.n == 0 ? 0.0 : a.cum[2 * b + 1]) + tq;
+        const double cs = (n == 0 ? 0.0 : a.cum[2 * b]) + ts, cq = (n == 0 ? 0.0 : a.cum[2 * b + 1]) + tq;
         a.cum[2 * b] = cs; a.cum[2 * b + 1] = cq;
-        const double cnt = (double)F * (a.n + 1), cm = cs / cnt;
+        const double cnt = (double)F * (n + 1), cm = cs / cnt;
         if (a.type == FSN_NORM_CUMULATIVE_LAPLACE) { s_a = (float)(1.0 / (cm + EPS)); s_b = 0.f; }
         else { const double cv = (cq - 2.0 * cm * cs) / cnt + cm * cm, inv = 1.0 / sqrt(cv + EPS); s_a = (float)inv; s_b = (float)(-cm * inv); }
     }
@@ -692,6 +697,13 @@ __global__ void __launch_bounds__(128) stream_pack_kernel(StreamPackLaunch a) {
     if (row >= a.B * F) return;
     const int b = row / F, f = row % F, tile = row >> 7, r = row & 127;
     const int nw = 2 * a.Ns + 1, nf = 2 * a.Nf + 1, I = nw + nf;
+    char* img = reinterpret_cast<char*>(a.ximg) + (size_t)tile * (128 * 128);
+    const int n = a.slot ? a.slot[b] : a.n;                         // the frame count of this row's slot
+    if (n < 0) {                                                    // held: frame unread, sums untouched, zero input row
+#pragma unroll
+        for (int c = 0; c < 8; ++c) *reinterpret_cast<uint4*>(img + sw128_offset(r, c * 8)) = make_uint4(0u, 0u, 0u, 0u);
+        return;
+    }
     float v[64];
     double s = 0, q = 0;
 #pragma unroll
@@ -702,13 +714,12 @@ __global__ void __launch_bounds__(128) stream_pack_kernel(StreamPackLaunch a) {
         v[k] = x; s += x; q += (double)x * x;
     }
     const double EPS = 1.1920928955078125e-07;
-    const double cs = (a.n == 0 ? 0.0 : a.cum[2 * row]) + s, cq = (a.n == 0 ? 0.0 : a.cum[2 * row + 1]) + q;
+    const double cs = (n == 0 ? 0.0 : a.cum[2 * row]) + s, cq = (n == 0 ? 0.0 : a.cum[2 * row + 1]) + q;
     a.cum[2 * row] = cs; a.cum[2 * row + 1] = cq;
-    const double cnt = (double)I * (a.n + 1), cm = cs / cnt;
+    const double cnt = (double)I * (n + 1), cm = cs / cnt;
     float sc, sh;
     if (a.type == FSN_NORM_CUMULATIVE_LAPLACE) { sc = (float)(1.0 / (cm + EPS)); sh = 0.f; }
     else { const double cv = (cq - 2.0 * cm * cs) / cnt + cm * cm, inv = 1.0 / sqrt(cv + EPS); sc = (float)inv; sh = (float)(-cm * inv); }
-    char* img = reinterpret_cast<char*>(a.ximg) + (size_t)tile * (128 * 128);
 #pragma unroll
     for (int c = 0; c < 8; ++c) {
         float w[8];
@@ -719,6 +730,22 @@ __global__ void __launch_bounds__(128) stream_pack_kernel(StreamPackLaunch a) {
     }
 }
 void launch_stream_pack(const StreamPackLaunch& a, cudaStream_t s) { stream_pack_kernel<<<(a.B * a.F + 127) / 128, 128, 0, s>>>(a); }
+
+// START of the slot call: zero the recurrent state rows of the slots whose count is 0.  Those are the started slots, plus slots that
+// have never stepped, whose rows are still zero from creation.  grid (B, nbuf, L): one block per (slot, buffer, layer).
+__global__ void __launch_bounds__(256) stream_reset_kernel(StreamResetLaunch a) {
+    const int b = blockIdx.x, l = blockIdx.z;
+    const StreamResetBuf& d = a.buf[blockIdx.y];
+    if (a.slot[b] != 0 || l >= d.L) return;
+    const size_t bytes = d.row_bytes * d.rows_per_slot;                   // rows are whole 16-byte chunks (H % 16 == 0)
+    uint4* p = reinterpret_cast<uint4*>(static_cast<char*>(d.p) + l * d.layer_bytes + b * bytes);
+    for (size_t i = threadIdx.x; i < bytes / 16; i += blockDim.x) p[i] = make_uint4(0u, 0u, 0u, 0u);
+}
+void launch_stream_reset(const StreamResetLaunch& a, cudaStream_t s) {
+    int L = 1;
+    for (int i = 0; i < a.nbuf; ++i) L = a.buf[i].L > L ? a.buf[i].L : L;
+    stream_reset_kernel<<<dim3(a.B, a.nbuf, L), 256, 0, s>>>(a);
+}
 
 // decompress_cIRM + complex multiply (inferencer.py:152-157, mask.py:60-63) in one pass.
 __global__ void apply_cirm_kernel(const float* crm, const float2* noisy, float2* enh, int FT, size_t n) {

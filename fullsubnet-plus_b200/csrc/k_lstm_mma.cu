@@ -27,7 +27,8 @@ static inline MmaSmemPlan mma_plan(int L, int H, int Ipad, int R, int O) {
     return p;
 }
 
-template <int R, bool FAST>
+// SLOTS: the streaming slot call (a.slot != null); the other instantiations compile without its per-row tests
+template <int R, bool FAST, bool SLOTS>
 __global__ void __launch_bounds__(256, 1) lstm_mma_kernel(LstmMmaLaunch a) {
     constexpr int MT = R / 16;
     extern __shared__ __align__(16) unsigned char smraw[];
@@ -50,6 +51,14 @@ __global__ void __launch_bounds__(256, 1) lstm_mma_kernel(LstmMmaLaunch a) {
         }
     }
     if (a.out) for (int i = tid; i < a.O * H; i += blockDim.x) fcw[i] = a.w.fc_w[i];
+    // streaming slot call: bit 2 mt + half = the row this thread updates in row tile mt (lane / 4, + 8 for half 1) is held
+    unsigned held = 0;
+    if (SLOTS)
+#pragma unroll
+        for (int i = 0; i < 2 * MT; ++i) {
+            const int grow = row0 + (i >> 1) * 16 + (lane >> 2) + (i & 1) * 8;
+            if (grow < a.rows && a.slot[grow / a.slot_rows] < 0) held |= 1u << i;
+        }
     __syncthreads();
 
     for (int t = 0; t < Tp; ++t) {
@@ -121,7 +130,7 @@ __global__ void __launch_bounds__(256, 1) lstm_mma_kernel(LstmMmaLaunch a) {
                         float c, h;
                         if (a.gru) { h = gru_cell_plain<FAST>(gi, gf, gg, go, cprev); c = h; }
                         else { c = sigm<FAST>(gf) * cprev + sigm<FAST>(gi) * tanh_<FAST>(gg); h = sigm<FAST>(go) * tanh_<FAST>(c); }
-                        cst[ci] = c;
+                        if (!SLOTS || !((held >> (2 * mt + (q >> 1))) & 1u)) cst[ci] = c;
                         hout[(size_t)r * HS + u] = __float2half_rn(h);
                         if (top && a.hseq && row0 + r < a.rows) a.hseq[((size_t)(row0 + r) * H + u) * a.P + t] = h;
                     }
@@ -135,7 +144,10 @@ __global__ void __launch_bounds__(256, 1) lstm_mma_kernel(LstmMmaLaunch a) {
                 const int r = e / a.O, o = e % a.O, grow = row0 + r;
                 if (grow >= a.rows) continue;
                 const int b = grow / a.F, f = grow % a.F;
-                if (a.tlen && t >= a.tlen[b]) { a.out[(((size_t)b * a.O + o) * a.F + f) * (Tp - a.la) + (t - a.la)] = 0.f; continue; }   // past the clip's end
+                if ((a.tlen && t >= a.tlen[b]) || (SLOTS && a.slot[grow / a.slot_rows] < a.slot_la)) {   // past the clip's end; no valid mask
+                    a.out[(((size_t)b * a.O + o) * a.F + f) * (Tp - a.la) + (t - a.la)] = 0.f;
+                    continue;
+                }
                 float acc = a.w.fc_b[o];
                 const __half2* hr = reinterpret_cast<const __half2*>(htop + (size_t)r * HS);
                 const float* w = fcw + (size_t)o * H;
@@ -157,6 +169,7 @@ __global__ void __launch_bounds__(256, 1) lstm_mma_kernel(LstmMmaLaunch a) {
         const int pl = (Tp - 1) & 1;
         for (int e = tid; e < L * R * (H / 2); e += blockDim.x) {
             const int l = e / (R * (H / 2)), r = (e / (H / 2)) % R, u2 = e % (H / 2);
+            if (SLOTS && row0 + r < a.rows && a.slot[(row0 + r) / a.slot_rows] < 0) continue;   // held: h stays
             reinterpret_cast<uint32_t*>(a.hstate + ((size_t)l * a.rows_alloc + row0 + r) * H)[u2] =
                 reinterpret_cast<const uint32_t*>(hb + ((size_t)l * 2 + pl) * R * HS + (size_t)r * HS)[u2];
         }
@@ -175,21 +188,19 @@ size_t lstm_mma_cstate_bytes(int L, int rows, int H, int* rows_alloc) {
     return (size_t)L * ra * H * sizeof(float);
 }
 
+template <int R, bool FAST, bool SLOTS>
+static int launch_k(const LstmMmaLaunch& a, cudaStream_t s) {
+    const MmaSmemPlan p = mma_plan(a.L, a.H, a.Ipad, R, a.out ? a.O : 0);
+    const cudaError_t e = cudaFuncSetAttribute(lstm_mma_kernel<R, FAST, SLOTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.total);
+    if (e != cudaSuccess) return (int)e;
+    lstm_mma_kernel<R, FAST, SLOTS><<<dim3((a.rows + R - 1) / R), 256, p.total, s>>>(a);
+    return (int)cudaGetLastError();
+}
+
 template <int R>
 static int launch_r(const LstmMmaLaunch& a, cudaStream_t s) {
-    MmaSmemPlan p = mma_plan(a.L, a.H, a.Ipad, R, a.out ? a.O : 0);
-    dim3 grid((a.rows + R - 1) / R);
-    cudaError_t e;
-    if (a.fast) {
-        e = cudaFuncSetAttribute(lstm_mma_kernel<R, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.total);
-        if (e != cudaSuccess) return (int)e;
-        lstm_mma_kernel<R, true><<<grid, 256, p.total, s>>>(a);
-    } else {
-        e = cudaFuncSetAttribute(lstm_mma_kernel<R, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.total);
-        if (e != cudaSuccess) return (int)e;
-        lstm_mma_kernel<R, false><<<grid, 256, p.total, s>>>(a);
-    }
-    return (int)cudaGetLastError();
+    if (a.fast) return a.slot ? launch_k<R, true, true>(a, s) : launch_k<R, true, false>(a, s);
+    return a.slot ? launch_k<R, false, true>(a, s) : launch_k<R, false, false>(a, s);
 }
 
 int launch_lstm_mma(const LstmMmaLaunch& a, cudaStream_t s) {

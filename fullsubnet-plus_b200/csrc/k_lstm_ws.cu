@@ -40,7 +40,8 @@ __device__ __forceinline__ void grid_barrier(unsigned int* counter, unsigned int
     __syncthreads();
 }
 
-template <bool FAST>
+// SLOTS: the streaming slot call (a.slot != null); the other instantiations compile without its per-row tests
+template <bool FAST, bool SLOTS>
 __global__ void __launch_bounds__(WS_THREADS, 1) lstm_ws_kernel(LstmWsLaunch a) {
     extern __shared__ __align__(16) unsigned char smraw[];
     const int L = a.L, H = a.H, Ipad = a.Ipad, Tp = a.Tp;
@@ -84,6 +85,11 @@ __global__ void __launch_bounds__(WS_THREADS, 1) lstm_ws_kernel(LstmWsLaunch a) 
             cst[l][1] = (a.resume && a.cbuf) ? a.cbuf[((size_t)l * WS_ROWS + r0 + 8) * H + unit] : 0.f;
         }
     }
+    // streaming slot call: rows r0 / r0 + 8 held (they keep cst and carry their previous h forward)
+    bool held[2] = {false, false};
+    if (SLOTS)
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) held[rr] = r0 + rr * 8 < a.rows && a.slot[r0 + rr * 8] < 0;
     __syncthreads();
 
     unsigned int bar_target = 0;
@@ -125,6 +131,11 @@ __global__ void __launch_bounds__(WS_THREADS, 1) lstm_ws_kernel(LstmWsLaunch a) 
                 __half* hout = a.hbuf + ((size_t)l * 2 + par) * WS_ROWS * H;
 #pragma unroll
                 for (int rr = 0; rr < 2; ++rr) {
+                    if (SLOTS && held[rr]) {                                  // h_prev (A tile column K0 + unit) into this step's parity
+                        const int row = r0 + rr * 8;
+                        hout[(size_t)row * H + unit] = asm_[(size_t)row * KA + K0 + unit];
+                        continue;
+                    }
                     const float gi = (rr ? acc[2] : acc[0]) + bias[l][0], gf = (rr ? acc[3] : acc[1]) + bias[l][1];
                     const float gg = (rr ? o2 : o0) + bias[l][2], go = (rr ? o3 : o1) + bias[l][3];
                     float c, h;
@@ -168,15 +179,11 @@ int launch_lstm_ws(const LstmWsLaunch& a, cudaStream_t s) {
     if (e != cudaSuccess) return (int)e;
     LstmWsLaunch arg = a;
     void* params[] = {&arg};
-    if (a.fast) {
-        e = cudaFuncSetAttribute(lstm_ws_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return (int)e;
-        e = cudaLaunchCooperativeKernel(reinterpret_cast<void*>(lstm_ws_kernel<true>), dim3(grid), dim3(WS_THREADS), params, smem, s);
-    } else {
-        e = cudaFuncSetAttribute(lstm_ws_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return (int)e;
-        e = cudaLaunchCooperativeKernel(reinterpret_cast<void*>(lstm_ws_kernel<false>), dim3(grid), dim3(WS_THREADS), params, smem, s);
-    }
+    void (*k)(LstmWsLaunch) = a.fast ? (a.slot ? lstm_ws_kernel<true, true> : lstm_ws_kernel<true, false>)
+                                     : (a.slot ? lstm_ws_kernel<false, true> : lstm_ws_kernel<false, false>);
+    e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return (int)e;
+    e = cudaLaunchCooperativeKernel(reinterpret_cast<void*>(k), dim3(grid), dim3(WS_THREADS), params, smem, s);
     return (int)e;
 }
 

@@ -177,6 +177,22 @@ int fsn_stream_create(fsn_model* m, int32_t B, fsn_stream** out);
 int fsn_stream_step(fsn_stream* st, const float* d_mag_frame, float* d_mask, int32_t* h_valid, void* stream);
 void fsn_stream_destroy(fsn_stream* st);
 
+/* Independent sessions on one handle (DESIGN.md §3.9): each of the B slots serves its own session, which starts, pauses and ends on
+ * its own schedule and gets exactly the masks it would get streamed alone.  h_flags: HOST array of B flags for this tick. */
+#define FSN_SLOT_HOLD 0   /* no frame this tick: the slot's state is unchanged, its frame is never read, its mask row is zero */
+#define FSN_SLOT_STEP 1   /* consume the slot's frame, advance its state by one frame                                         */
+#define FSN_SLOT_START 2  /* reset the slot's state (norm sums, frame count, h and c of every layer of both LSTMs), then STEP  */
+/* h_valid (HOST, [B]): h_valid[b] = 1 when slot b stepped at this tick and has consumed more than look_ahead frames since its last
+ * START; d_mask[b] is then the mask of the slot's frame n_b - look_ahead (n_b: frames consumed, this one included).  Otherwise
+ * h_valid[b] = 0 and d_mask[b] is zero.  To end a session feed look_ahead zero frames with STEP (the reference's right padding), then
+ * HOLD the slot until a START reuses it.  A slot that has never been started behaves as if it had just been reset.
+ * FSN_EINVAL, naming the slot, for a flag outside {0, 1, 2}; FSN_EINVAL for a null h_flags or h_valid.  The flags are staged through
+ * pinned buffers, so both arrays are free when the call returns; the call does not synchronise the stream.
+ * fsn_stream_step on a handle that has never used the slot call runs exactly as before.  Once the handle has used it,
+ * fsn_stream_step is the slot call with every flag FSN_SLOT_STEP, and *h_valid is 1 when every slot's mask is valid. */
+int fsn_stream_step_slots(fsn_stream* st, const float* d_mag_frame, float* d_mask, const int32_t* h_flags, int32_t* h_valid,
+                          void* stream);
+
 /* Fused post-processing of the inferencer method (fullsubnet_plus/inferencer/inferencer.py:152-157 and
  * audio_zen/acoustics/mask.py:60-63): decompress_cIRM (K = 10, limit = 9.9) + complex multiply with the noisy spectrum.
  * d_crm [B, 2, F, T] float32 (model output), d_noisy / d_enh [B, F, T] complex64 (interleaved re, im). */

@@ -1656,8 +1656,16 @@ struct fsn_stream {
     std::vector<int32_t> nb, all_step, valid;
     DevBuf d_slot;
     static const int NSTAGE = 4;
-    struct Stage { int32_t* h = nullptr; cudaEvent_t ev = nullptr; bool used = false; } stage[NSTAGE];
+    struct Stage { int32_t* h = nullptr; cudaEvent_t ev = nullptr; bool used = false; size_t cap = 0; } stage[NSTAGE];
     int64_t nstage = 0;
+    // A handle serves either the mask calls (fsn_stream_step, fsn_stream_step_slots) or the audio call, whichever it meets first
+    enum { MODE_NONE, MODE_MASK, MODE_AUDIO } mode = MODE_NONE;
+    // audio call (fsn_stream_step_audio_slots), allocated at its first use.  Per slot on the host: a_tick = ticks of the session so
+    // far, HOLD excluded (-1: no session); a_hops = its hops K, known from its first FLUSH (0 before).  On the device: the history
+    // ring, the noisy-spectrum ring, the overlap tail, the model's input row, the mask rows when the caller passes none, and the tables
+    std::vector<int32_t> a_tick, a_hops;
+    std::vector<float> a_tables;
+    DevBuf a_hist, a_spec, a_tail, a_mag, a_mask, a_tab;
 };
 
 extern "C" int fsn_stream_create(fsn_model* m, int32_t B, fsn_stream** out) {
@@ -1703,7 +1711,34 @@ extern "C" void fsn_stream_destroy(fsn_stream* st) {
         if (g.ev) cudaEventDestroy(g.ev);
     }
     st->d_slot.release();
+    DevBuf* audio[] = {&st->a_hist, &st->a_spec, &st->a_tail, &st->a_mag, &st->a_mask, &st->a_tab};
+    for (auto* b : audio) b->release();
     delete st;
+}
+
+static int claim_mode(fsn_stream* st, int mode) {
+    if (st->mode != fsn_stream::MODE_NONE && st->mode != mode)
+        return fail(FSN_ESTATE, mode == fsn_stream::MODE_AUDIO
+                                    ? "this handle serves the mask calls (fsn_stream_step, fsn_stream_step_slots): create another for audio"
+                                    : "this handle serves the audio call (fsn_stream_step_audio_slots): create another for masks");
+    st->mode = static_cast<decltype(st->mode)>(mode);
+    return FSN_OK;
+}
+
+// The next pinned staging slot for the per-slot values of one tick, holding at least n int32.  A slot is refilled only after the
+// event behind its last H2D copy has fired.
+static int stage_next(fsn_stream* st, size_t n, fsn_stream::Stage** out) {
+    fsn_stream::Stage& g = st->stage[st->nstage++ % fsn_stream::NSTAGE];
+    if (!g.ev) CK(cudaEventCreateWithFlags(&g.ev, cudaEventDisableTiming));
+    if (g.used) CK(cudaEventSynchronize(g.ev));                         // the copy that last read this slot has completed
+    if (g.cap < n) {
+        if (g.h) CK(cudaFreeHost(g.h));
+        g.h = nullptr; g.cap = 0;
+        CK(cudaHostAlloc(reinterpret_cast<void**>(&g.h), n * sizeof(int32_t), cudaHostAllocDefault));
+        g.cap = n;
+    }
+    *out = &g;
+    return FSN_OK;
 }
 
 // One tick of the handle.  slot: null (the lockstep step: every slot at frame n) or the device per-slot counts of the slot call;
@@ -1789,16 +1824,16 @@ extern "C" int fsn_stream_step_slots(fsn_stream* st, const float* d_mag, float* 
             return fail(FSN_EINVAL, "slot %d: flag %d is not FSN_SLOT_HOLD (0), FSN_SLOT_STEP (1) or FSN_SLOT_START (2)", b, f);
         reset = reset || f == FSN_SLOT_START;
     }
+    if (int rc = claim_mode(st, fsn_stream::MODE_MASK)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     if (!st->slots) {                                                   // until now every slot stepped with the handle
         if (st->d_slot.ensure((size_t)B * sizeof(int32_t), false)) return fail(FSN_ECUDA, "slot-count buffer allocation failed");
         st->nb.assign(B, st->n);
         st->slots = true;
     }
-    fsn_stream::Stage& g = st->stage[st->nstage++ % fsn_stream::NSTAGE];
-    if (!g.ev) CK(cudaEventCreateWithFlags(&g.ev, cudaEventDisableTiming));
-    if (g.used) CK(cudaEventSynchronize(g.ev));                         // the copy that last read this slot has completed
-    if (!g.h) CK(cudaHostAlloc(reinterpret_cast<void**>(&g.h), (size_t)B * sizeof(int32_t), cudaHostAllocDefault));
+    fsn_stream::Stage* gp = nullptr;
+    if (int rc = stage_next(st, B, &gp)) return rc;
+    fsn_stream::Stage& g = *gp;
     for (int b = 0; b < B; ++b)
         g.h[b] = h_flags[b] == FSN_SLOT_HOLD ? -1 : h_flags[b] == FSN_SLOT_START ? 0 : st->nb[b];
     CK(cudaMemcpyAsync(st->d_slot.p, g.h, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
@@ -1815,6 +1850,7 @@ extern "C" int fsn_stream_step_slots(fsn_stream* st, const float* d_mag, float* 
 
 extern "C" int fsn_stream_step(fsn_stream* st, const float* d_mag, float* d_mask, int32_t* h_valid, void* stream) {
     if (!st || !d_mag || !d_mask) return fail(FSN_EINVAL, "null argument");
+    if (int rc = claim_mode(st, fsn_stream::MODE_MASK)) return rc;
     if (st->slots) {                                                    // the slot call with every slot stepping
         st->all_step.assign(st->B, FSN_SLOT_STEP);
         st->valid.resize(st->B);
@@ -1829,6 +1865,111 @@ extern "C" int fsn_stream_step(fsn_stream* st, const float* d_mag, float* d_mask
     const int rc = stream_tick(st, d_mag, d_mask, nullptr, false, static_cast<cudaStream_t>(stream));
     if (rc) return rc;
     if (h_valid) *h_valid = (n >= st->m->cfg.look_ahead) ? 1 : 0;
+    return FSN_OK;
+}
+
+// Audio state of the handle, zero-filled on the call's stream, and the tables of its n_fft (computed in double).
+static int audio_alloc(fsn_stream* st, int N, cudaStream_t s) {
+    const fsn_config& c = st->m->cfg;
+    const size_t B = st->B, H = N / 2, F = H + 1, la = c.look_ahead;
+    int e = 0;
+    e |= st->a_hist.ensure(B * 3 * H * sizeof(float), true, s);
+    e |= st->a_spec.ensure(B * (la + 1) * F * sizeof(float2), true, s);
+    e |= st->a_tail.ensure(B * H * sizeof(float), true, s);
+    e |= st->a_mag.ensure(B * F * sizeof(float), true, s);
+    e |= st->a_mask.ensure(B * 2 * F * sizeof(float), true, s);
+    std::vector<float> w, tw, inv;
+    stream_audio_tables(N, w, tw, inv);
+    st->a_tables = w;
+    st->a_tables.insert(st->a_tables.end(), tw.begin(), tw.end());
+    st->a_tables.insert(st->a_tables.end(), inv.begin(), inv.end());
+    e |= st->a_tab.ensure(st->a_tables.size() * sizeof(float), false, s);
+    if (e) return fail(FSN_ECUDA, "audio stream state allocation failed");
+    CK(cudaMemcpyAsync(st->a_tab.p, st->a_tables.data(), st->a_tables.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+    st->a_tick.assign(B, -1);
+    st->a_hops.assign(B, 0);
+    return FSN_OK;
+}
+
+extern "C" int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_samples, float* d_out, const int32_t* h_flags,
+                                           int32_t* h_valid, float* d_mask, void* stream) {
+    if (!st) return fail(FSN_EINVAL, "st is null");
+    if (!d_samples) return fail(FSN_EINVAL, "d_samples is null (one hop of samples per slot, [B, hop] float32 on the device)");
+    if (!d_out) return fail(FSN_EINVAL, "d_out is null (one hop of output per slot, [B, hop] float32 on the device)");
+    if (!h_flags) return fail(FSN_EINVAL, "h_flags is null (one flag per slot, slots 0..%d)", st->B - 1);
+    if (!h_valid) return fail(FSN_EINVAL, "h_valid is null (one result per slot, slots 0..%d)", st->B - 1);
+    const fsn_config& c = st->m->cfg;
+    const int B = st->B, F = c.num_freqs, la = c.look_ahead, N = 2 * (F - 1);
+    if (N < 64 || N > 1024 || (N & (N - 1)))
+        return fail(FSN_EINVAL, "num_freqs %d: the audio call needs n_fft = 2 (num_freqs - 1) to be a power of two from 64 to 1024 "
+                                "(num_freqs 33, 65, 129, 257 or 513)", F);
+    for (int b = 0; b < B; ++b) {                                       // every flag is checked before any state changes
+        const int f = h_flags[b], t = st->a_tick.empty() ? -1 : st->a_tick[b], K = st->a_hops.empty() ? 0 : st->a_hops[b];
+        if (f < FSN_SLOT_HOLD || f > FSN_SLOT_FLUSH)
+            return fail(FSN_EINVAL, "slot %d: flag %d is not FSN_SLOT_HOLD (0), FSN_SLOT_STEP (1), FSN_SLOT_START (2) or FSN_SLOT_FLUSH (3)", b, f);
+        if ((f == FSN_SLOT_STEP || f == FSN_SLOT_FLUSH) && t < 0)
+            return fail(FSN_EINVAL, "slot %d: %s on a slot without a session (START one first)", b, f == FSN_SLOT_STEP ? "STEP" : "FLUSH");
+        if (f == FSN_SLOT_STEP && K)
+            return fail(FSN_EINVAL, "slot %d: STEP after the session's FLUSH (its input has ended: START a new session)", b);
+        if (f == FSN_SLOT_FLUSH && !K && t < 2)
+            return fail(FSN_EINVAL, "slot %d: FLUSH after %d hop: a session needs at least 2 hops (the STFT's reflect padding reads "
+                                    "n_fft / 2 + 1 samples)", b, t);
+    }
+    if (int rc = claim_mode(st, fsn_stream::MODE_AUDIO)) return rc;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (st->a_tick.empty()) {
+        if (int rc = audio_alloc(st, N, s)) return rc;
+        if (st->d_slot.ensure((size_t)4 * B * sizeof(int32_t), false)) return fail(FSN_ECUDA, "slot-count buffer allocation failed");
+    }
+    // One staging slot carries the tick's four per-slot planes: the model's frame counts (-1 = the model row holds), the AUDIO_* ops,
+    // the slot ticks and the hop counts.  The schedule (DESIGN.md §3.10) for a session of K hops, slot tick k:
+    //   k = 0 (START): store hop 0, the model row holds;  1 <= k <= K + 1: analyse frame k - 1, the model steps frame k - 1 (count
+    //   k - 1, a START at k = 1);  k > K + 1: a zero frame;  k - 1 - la >= 0: synthesise that frame, emitting hop k - 2 - la from 1.
+    fsn_stream::Stage* gp = nullptr;
+    if (int rc = stage_next(st, (size_t)4 * B, &gp)) return rc;
+    fsn_stream::Stage& g = *gp;
+    int32_t *cnt = g.h, *op = g.h + B, *tick = g.h + 2 * B, *hops = g.h + 3 * B;
+    bool reset = false;
+    for (int b = 0; b < B; ++b) {
+        const int f = h_flags[b];
+        int k = st->a_tick[b], K = st->a_hops[b];
+        cnt[b] = -1; op[b] = 0;
+        if (f == FSN_SLOT_START) {
+            k = 0; K = 0; op[b] = AUDIO_STORE;
+        } else if (f == FSN_SLOT_STEP || f == FSN_SLOT_FLUSH) {
+            if (f == FSN_SLOT_FLUSH && !K) K = k;
+            if (k <= K + la + 1 || !K) {                                // past that, a FLUSH is a HOLD
+                const int j = k - 1, m = k - 1 - la;
+                cnt[b] = j;
+                op[b] = (f == FSN_SLOT_STEP ? AUDIO_STORE : 0) | (!K || j <= K ? AUDIO_FRAME : AUDIO_ZERO) |
+                        (m >= 0 ? AUDIO_SYNTH : 0) | (m >= 1 ? AUDIO_EMIT : 0);
+            }
+        }
+        tick[b] = k; hops[b] = K;
+        reset = reset || cnt[b] == 0;
+    }
+    int32_t* d = static_cast<int32_t*>(st->d_slot.p);
+    CK(cudaMemcpyAsync(d, g.h, (size_t)4 * B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CK(cudaEventRecord(g.ev, s));
+    g.used = true;
+    float* mask = d_mask ? d_mask : static_cast<float*>(st->a_mask.p);
+    StreamAudioLaunch a{};
+    a.op = d + B; a.tick = d + 2 * B; a.hops = d + 3 * B;
+    a.samples = d_samples; a.out = d_out;
+    a.hist = static_cast<float*>(st->a_hist.p); a.spec = static_cast<float2*>(st->a_spec.p); a.tail = static_cast<float*>(st->a_tail.p);
+    a.mag = static_cast<float*>(st->a_mag.p); a.mask = mask;
+    const float* tab = static_cast<const float*>(st->a_tab.p);
+    a.window = tab; a.twiddle = reinterpret_cast<const float2*>(tab + N); a.inv_env = tab + N + 2 * (N / 2 + 1);
+    a.B = B; a.n_fft = N; a.la = la;
+    launch_stream_stft(a, s);
+    const int rc = stream_tick(st, a.mag, mask, d, reset, s);
+    if (rc) return rc;
+    launch_stream_istft(a, s);
+    CK(cudaGetLastError());
+    for (int b = 0; b < B; ++b) {
+        if (h_flags[b] == FSN_SLOT_START || cnt[b] >= 0) { st->a_tick[b] = tick[b] + 1; st->a_hops[b] = hops[b]; }
+        h_valid[b] = (op[b] & AUDIO_EMIT) ? 1 : 0;
+    }
     return FSN_OK;
 }
 

@@ -119,6 +119,31 @@ struct StreamResetBuf { void* p; size_t layer_bytes, row_bytes; int L, rows_per_
 struct StreamResetLaunch { StreamResetBuf buf[4]; int nbuf, B; const int* slot; };
 void launch_stream_reset(const StreamResetLaunch& a, cudaStream_t s);
 
+// ---- k_stream_audio.cu: audio in and out of the streaming slot call (fsn_stream_step_audio_slots) ---------------------------
+// Per-slot ops of one tick, derived on the host from the slot's flag, tick count and hop count (fsn_api.cu, audio_plan)
+enum { AUDIO_STORE = 1,       // the slot's hop of samples goes to its history ring
+       AUDIO_FRAME = 2,       // analyse frame tick - 1: spectrum to the ring, magnitude to the model's input row
+       AUDIO_ZERO = 4,        // frame tick - 1 is a look-ahead zero frame: zero spectrum and magnitude rows
+       AUDIO_SYNTH = 8,       // synthesise frame tick - 1 - la from this tick's mask row
+       AUDIO_EMIT = 16 };     // ... and write hop tick - 2 - la of the session to the output row (else the row is zero)
+struct StreamAudioLaunch {
+    const int* op; const int* tick; const int* hops;   // [B] each: AUDIO_* bits, slot tick (HOLD excluded), hops K (0 = not flushed)
+    const float* samples;     // [B, hop] this tick's hops (read for AUDIO_STORE only)
+    float* out;               // [B, hop] output hops
+    float* hist;              // [B, 3, hop] history ring: hop q at q % 3
+    float2* spec;             // [B, la + 1, F] noisy spectrum ring: frame j at j % (la + 1)
+    float* tail;              // [B, hop] second half of the last synthesised windowed frame
+    float* mag;               // [B, F] the model step's input row
+    const float* mask;        // [B, 2, F] the model step's output
+    const float* window;      // [n_fft] periodic Hann
+    const float2* twiddle;    // [n_fft / 2 + 1] exp(-2 pi i k / n_fft)
+    const float* inv_env;     // [hop] 1 / (w^2(i) + w^2(i + hop))
+    int B, n_fft, la;         // n_fft: power of two, 64 .. 1024
+};
+void launch_stream_stft(const StreamAudioLaunch& a, cudaStream_t s);
+void launch_stream_istft(const StreamAudioLaunch& a, cudaStream_t s);
+void stream_audio_tables(int n_fft, std::vector<float>& window, std::vector<float>& twiddle, std::vector<float>& inv_env);
+
 // ---- k_lstm_mma.cu ---------------------------------------------------------------------------
 struct LstmMmaWeights {       // device, produced by pack (fsn_api.cu)
     const uint4* wfrag[4];    // per layer: [H/8 groups][K/16][32 lanes][2 x uint4]

@@ -22,7 +22,7 @@ SYMBOLS = [
     "fsn_sw128_offset", "fsn_tc5_weight_stream_bytes", "fsn_tc5_pack_weights", "fsn_tc5_gate_row", "fsn_tc5r_weight_stream_bytes", "fsn_tc5r_pack_layer",
     "fsn_gemm_f16", "fsn_gemm_f16_tile_n",
     "fsn_tc5r_gin_weights", "fsn_tc5r_ring_stages", "fsn_lstm_mma_rows", "fsn_model_sb_forward",
-    "fsn_stream_step_slots",
+    "fsn_stream_step_slots", "fsn_stream_step_audio_slots",
 ]
 
 
@@ -78,6 +78,7 @@ def load_library():
     lib.fsn_stream_create.argtypes = [vp, i32, C.POINTER(vp)]
     lib.fsn_stream_step.argtypes = [vp, vp, vp, C.POINTER(i32), vp]
     lib.fsn_stream_step_slots.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.fsn_stream_step_audio_slots.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.fsn_stream_destroy.argtypes = [vp]
     lib.fsn_stream_destroy.restype = None
     lib.fsn_apply_cirm.argtypes = [vp, vp, vp, i32, i32, i32, vp]

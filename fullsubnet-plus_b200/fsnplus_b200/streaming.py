@@ -8,6 +8,10 @@ produced when frame n arrives, exactly as the reference's right zero-padding + o
 
 Independent sessions share one handle through ``step_slots``: each of the B slots serves its own session, which starts, pauses
 and ends on its own schedule (flags HOLD / STEP / START per slot and tick, DESIGN.md §3.9).
+
+``step_audio`` serves the same sessions with audio in and out: one hop of samples per slot and tick goes in, one hop of enhanced
+audio comes out, with the STFT, the cIRM and the overlap-add iSTFT on the device (flag FLUSH ends a session, DESIGN.md §3.10).
+A handle serves either the mask calls or the audio call.
 """
 import ctypes as C
 
@@ -15,7 +19,7 @@ import torch
 
 from . import _lib
 
-HOLD, STEP, START = 0, 1, 2            # FSN_SLOT_* of include/fsnplus_b200.h
+HOLD, STEP, START, FLUSH = 0, 1, 2, 3  # FSN_SLOT_* of include/fsnplus_b200.h (FLUSH: audio call only)
 
 
 class StreamingFullSubNet:
@@ -57,6 +61,32 @@ class StreamingFullSubNet:
             _lib.check(self.lib.fsn_stream_step_slots(self._st, C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()),
                                                       C.c_void_p(f.data_ptr()), C.c_void_p(valid.data_ptr()), stream))
         return out, valid.bool()
+
+    @property
+    def hop(self):
+        """Samples per hop of the audio call: n_fft / 2 = num_freqs - 1."""
+        return self.F - 1
+
+    def step_audio(self, samples, flags, return_mask=False):
+        """One tick of independent audio sessions.  samples [B, hop] float32 CUDA: one hop per slot (rows of HOLD and FLUSH slots are
+        never read); flags: B values of HOLD / STEP / START / FLUSH.  Returns (audio [B, hop], valid bool CPU tensor [B]), plus the
+        masks [B, 2, F] with return_mask: valid[b] when audio[b] is hop q of the slot's session, which comes out at the slot's tick
+        q + look_ahead + 2 (HOLD ticks not counted); every other row is zero.  A session of K >= 2 hops ends with look_ahead + 2
+        FLUSH ticks; at slot tick k the mask row is that of frame k - look_ahead - 1 (zero before frame 0)."""
+        assert samples.shape == (self.B, self.hop) and samples.is_cuda
+        f = torch.as_tensor(flags, dtype=torch.int32)
+        assert f.device.type == "cpu" and f.shape == (self.B,), "flags: B host values"
+        f = f.contiguous()
+        x = samples.contiguous().float()
+        out = torch.empty((self.B, self.hop), dtype=torch.float32, device=self.device)
+        mask = torch.empty((self.B, 2, self.F), dtype=torch.float32, device=self.device) if return_mask else None
+        valid = torch.zeros(self.B, dtype=torch.int32)
+        with torch.cuda.device(self.device):
+            stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+            _lib.check(self.lib.fsn_stream_step_audio_slots(self._st, C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()),
+                                                            C.c_void_p(f.data_ptr()), C.c_void_p(valid.data_ptr()),
+                                                            C.c_void_p(mask.data_ptr() if return_mask else None), stream))
+        return (out, valid.bool(), mask) if return_mask else (out, valid.bool())
 
     def flush(self):
         """Feed look_ahead zero frames (the reference's right padding) and return the remaining masks."""

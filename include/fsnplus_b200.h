@@ -193,6 +193,30 @@ void fsn_stream_destroy(fsn_stream* st);
 int fsn_stream_step_slots(fsn_stream* st, const float* d_mag_frame, float* d_mask, const int32_t* h_flags, int32_t* h_valid,
                           void* stream);
 
+/* Audio in, audio out (DESIGN.md §3.10): the slot call with the STFT before the model step and decompress_cIRM x noisy spectrum,
+ * inverse FFT and overlap-add after it, on the device.  Each slot's waveform equals the offline enhancement of its session's audio
+ * (torch.stft(center=True, reflect) -> model -> decompress_cIRM x spectrum -> torch.istft(length = L)).
+ * Geometry from the model: n_fft = 2 (num_freqs - 1), a power of two from 64 to 1024; hop = n_fft / 2; periodic Hann window of n_fft.
+ * Any other num_freqs is FSN_EINVAL, naming it.
+ * d_samples [B, hop] float32 device: one hop of new samples per slot (rows of HOLD and FLUSH slots are never read).
+ * d_out [B, hop] float32 device: one hop of enhanced audio per slot.  h_flags: HOST, B flags of FSN_SLOT_HOLD / STEP / START and: */
+#define FSN_SLOT_FLUSH 3  /* audio call only: no samples this tick; the session's input has ended, advance its tail                   */
+/* A START resets the slot's audio and model state and consumes the session's first hop; STEP consumes the next hop; HOLD is no tick
+ * (state unchanged, output row zero).  A session of K >= 2 hops (L = K hop samples; pad a partial last hop with zeros and trim the
+ * output) ends with exactly look_ahead + 2 FLUSH ticks; further FLUSH ticks act as HOLD until a START reuses the slot.
+ * h_valid (HOST, [B]): h_valid[b] = 1 when d_out[b] holds hop q of the slot's session; hop q comes out at the slot's tick
+ * q + look_ahead + 2 (ticks counted from 0 at the START, HOLD ticks excluded): the algorithmic latency is look_ahead + 2 hops.
+ * Every other output row is zero.  d_mask: null, or [B, 2, F] float32 device, which receives at slot tick k the cIRM of the slot's
+ * frame k - look_ahead - 1 when that index is >= 0, and zero otherwise.
+ * FSN_EINVAL, naming the slot, for a flag outside {0, 1, 2, 3}, a STEP after the session's first FLUSH, a STEP or FLUSH on a slot
+ * that has no session, and a FLUSH after fewer than 2 hops; FSN_EINVAL, naming the argument, for a null array.  A handle serves
+ * either the mask calls (fsn_stream_step, fsn_stream_step_slots) or this call: mixing them is FSN_ESTATE.  The audio state
+ * (history, spectrum ring, overlap tail) is allocated at the first call.  Per tick: one H2D copy and 8 kernels (+ the reset kernel on
+ * ticks where a session's model row starts, + the grid-barrier memset of the full-band step at B <= 64).  The call does not
+ * synchronise the stream. */
+int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_samples, float* d_out, const int32_t* h_flags, int32_t* h_valid,
+                                float* d_mask, void* stream);
+
 /* Fused post-processing of the inferencer method (fullsubnet_plus/inferencer/inferencer.py:152-157 and
  * audio_zen/acoustics/mask.py:60-63): decompress_cIRM (K = 10, limit = 9.9) + complex multiply with the noisy spectrum.
  * d_crm [B, 2, F, T] float32 (model output), d_noisy / d_enh [B, F, T] complex64 (interleaved re, im). */

@@ -5,6 +5,7 @@
 #include "fsn_kernels.h"
 
 #include <cstdarg>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -46,6 +47,19 @@ struct DevBuf {
     void release() { if (p) cudaFree(p); p = nullptr; bytes = 0; }
 };
 
+// weights_id: folds n bytes into h 8 bytes at a time (the last word zero-padded).  Each step is a bijection of h (xor, odd multiply,
+// xorshift), so two byte strings of the same length that differ in any word give different results.
+static uint64_t hash_words(uint64_t h, const void* p, size_t n) {
+    const unsigned char* b = static_cast<const unsigned char*>(p);
+    for (size_t i = 0; i < n; i += 8) {
+        uint64_t w = 0;
+        memcpy(&w, b + i, n - i < 8 ? n - i : 8);
+        h = (h ^ w) * 0x100000001b3ull;
+        h ^= h >> 29;
+    }
+    return h;
+}
+
 struct ParamSpec { std::string key; int64_t numel; };
 
 // The packed block weights of one TCN (pack_tcn_blocks): nbr branches (key prefixes pre[b] = "<module>.sequence_model.") of C channels
@@ -86,6 +100,8 @@ struct fsn_model {
     std::vector<ParamSpec> specs;
     std::map<std::string, std::vector<float>> host;   // raw fp32 parameters (reference layout)
     std::map<std::string, float*> dev;                // same, on device
+    std::map<std::string, uint64_t> param_hash;       // per key: hash of the key and its fp32 bytes as set (fsn_model_set_param)
+    uint64_t weights_id = 0;                          // the per-key hashes combined in key order at fsn_model_finalize; 0 before
     DevBuf arena;
     bool finalized = false;
     int Isb = 0;                                      // sub-band LSTM input size
@@ -433,7 +449,7 @@ static int pack_sb_tcn(fsn_model* m) {
 // ---------------------------------------------------------------------------------------------
 // C ABI
 // ---------------------------------------------------------------------------------------------
-extern "C" int fsn_version(void) { return 100; }
+extern "C" int fsn_version(void) { return 101; }
 extern "C" const char* fsn_last_error(void) { return g_err; }
 
 extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
@@ -550,7 +566,11 @@ extern "C" int fsn_model_set_param(fsn_model* m, const char* key, const float* h
         if (s.key == key) {
             if (s.numel != numel) return fail(FSN_EINVAL, "size mismatch for %s: expected %lld, got %lld", key, (long long)s.numel, (long long)numel);
             m->host[key].assign(h, h + numel);
+            uint64_t x = hash_words(0xcbf29ce484222325ull, key, strlen(key));
+            x = hash_words(x, &numel, sizeof(numel));
+            m->param_hash[key] = hash_words(x, h, (size_t)numel * sizeof(float));
             m->finalized = false;
+            m->weights_id = 0;
             return FSN_OK;
         }
     return fail(FSN_EINVAL, "unexpected key %s", key);
@@ -609,6 +629,10 @@ extern "C" int fsn_model_finalize(fsn_model* m) {
         int rc = pack_sb_tcn(m);
         if (rc) return rc;
     }
+    uint64_t id = 0xcbf29ce484222325ull;
+    for (const auto& kv : m->param_hash) id = hash_words(id, &kv.second, sizeof(kv.second));   // std::map: key order
+    id ^= id >> 33; id *= 0xff51afd7ed558ccdull; id ^= id >> 33;                              // final avalanche
+    m->weights_id = id ? id : 1;                                                               // 0 means "not finalized"
     m->finalized = true;
     return FSN_OK;
 }
@@ -1666,6 +1690,8 @@ struct fsn_stream {
     std::vector<int32_t> a_tick, a_hops;
     std::vector<float> a_tables;
     DevBuf a_hist, a_spec, a_tail, a_mag, a_mask, a_tab;
+    // save / load (fsn_stream_save_slots, fsn_stream_load_slots): the slot list of the last call on the device
+    DevBuf x_slot;
 };
 
 extern "C" int fsn_stream_create(fsn_model* m, int32_t B, fsn_stream** out) {
@@ -1711,6 +1737,7 @@ extern "C" void fsn_stream_destroy(fsn_stream* st) {
         if (g.ev) cudaEventDestroy(g.ev);
     }
     st->d_slot.release();
+    st->x_slot.release();
     DevBuf* audio[] = {&st->a_hist, &st->a_spec, &st->a_tail, &st->a_mag, &st->a_mask, &st->a_tab};
     for (auto* b : audio) b->release();
     delete st;
@@ -1969,6 +1996,264 @@ extern "C" int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_sample
     for (int b = 0; b < B; ++b) {
         if (h_flags[b] == FSN_SLOT_START || cnt[b] >= 0) { st->a_tick[b] = tick[b] + 1; st->a_hops[b] = hops[b]; }
         h_valid[b] = (op[b] & AUDIO_EMIT) ? 1 : 0;
+    }
+    return FSN_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// park, resume and move sessions (DESIGN.md §3.11)
+// ---------------------------------------------------------------------------------------------
+// The payload's segments in payload order; per segment the bytes of one slot's rows of one layer and the layer count
+enum { SEG_CUM_IN, SEG_CUM_SB, SEG_FB_H, SEG_FB_C, SEG_SB_H, SEG_SB_C, SEG_HIST, SEG_SPEC, SEG_TAIL };
+struct StateSegSpec { size_t slot_bytes; int L; };
+
+static int state_layout(const fsn_config& c, int mode, StateSegSpec* seg, size_t* off, int* nseg, int64_t* stride) {
+    if (c.model_kind != FSN_KIND_FSN)
+        return fail(FSN_EINVAL, "model_kind %d: only fullsubnet.Model streams (FullSubNet+ is not causal: TSSE pools over all time)", c.model_kind);
+    if (c.norm_type != FSN_NORM_CUMULATIVE_LAPLACE && c.norm_type != FSN_NORM_CUMULATIVE_LAYER)
+        return fail(FSN_EINVAL, "norm_type %d: streaming needs a cumulative norm_type", c.norm_type);
+    if (mode != FSN_STATE_MODE_MASK && mode != FSN_STATE_MODE_AUDIO)
+        return fail(FSN_EINVAL, "mode %d is not FSN_STATE_MODE_MASK (1) or FSN_STATE_MODE_AUDIO (2)", mode);
+    if (c.num_freqs < 4 || c.num_freqs > 2048 || c.look_ahead < 0 || c.num_layers < 1 || c.num_layers > 4 || c.fb_hidden < 16 ||
+        c.fb_hidden % 16 || c.sb_hidden < 16 || c.sb_hidden % 16)
+        return fail(FSN_EINVAL, "bad configuration: num_freqs %d, look_ahead %d, num_layers %d, fb_hidden %d, sb_hidden %d", c.num_freqs,
+                    c.look_ahead, c.num_layers, c.fb_hidden, c.sb_hidden);
+    const size_t F = c.num_freqs, H = F - 1, N = 2 * H, la = c.look_ahead, Hf = c.fb_hidden, Hs = c.sb_hidden;
+    const int L = c.num_layers;
+    if (mode == FSN_STATE_MODE_AUDIO && (N < 64 || N > 1024 || (N & (N - 1))))
+        return fail(FSN_EINVAL, "num_freqs %d: the audio call needs n_fft = 2 (num_freqs - 1) to be a power of two from 64 to 1024", c.num_freqs);
+    const StateSegSpec s[9] = {{16, 1}, {F * 16, 1}, {Hf * 2, L}, {Hf * 4, L}, {F * Hs * 2, L}, {F * Hs * 4, L},
+                               {3 * H * 4, 1}, {(la + 1) * F * 8, 1}, {H * 4, 1}};
+    const int ns = mode == FSN_STATE_MODE_AUDIO ? 9 : 6;
+    size_t o = 0;
+    for (int i = 0; i < ns; ++i) {
+        if (seg) seg[i] = s[i];
+        if (off) off[i] = o;
+        o += (s[i].slot_bytes * s[i].L + 15) & ~(size_t)15;
+    }
+    if (nseg) *nseg = ns;
+    *stride = (int64_t)((o + 255) & ~(size_t)255);
+    return FSN_OK;
+}
+
+extern "C" int fsn_stream_state_layout(const fsn_config* cfg, int32_t mode, int64_t* payload_bytes, int32_t* meta_bytes) {
+    if (!cfg) return fail(FSN_EINVAL, "cfg is null");
+    int64_t stride = 0;
+    if (int rc = state_layout(*cfg, mode, nullptr, nullptr, nullptr, &stride)) return rc;
+    if (payload_bytes) *payload_bytes = stride;
+    if (meta_bytes) *meta_bytes = (int32_t)sizeof(fsn_slot_meta);
+    return FSN_OK;
+}
+
+extern "C" uint64_t fsn_model_weights_id(const fsn_model* m) { return m && m->finalized ? m->weights_id : 0; }
+
+static int state_mode(const fsn_stream* st) {
+    return st->mode == fsn_stream::MODE_MASK ? FSN_STATE_MODE_MASK : st->mode == fsn_stream::MODE_AUDIO ? FSN_STATE_MODE_AUDIO : 0;
+}
+
+extern "C" int64_t fsn_stream_state_bytes(const fsn_stream* st) {
+    if (!st) return fail(FSN_EINVAL, "st is null");
+    const int mode = state_mode(st);
+    if (!mode) return fail(FSN_ESTATE, "the handle has served no call and no load yet: its mode (masks or audio) is not known");
+    int64_t stride = 0;
+    if (int rc = state_layout(st->m->cfg, mode, nullptr, nullptr, nullptr, &stride)) return rc;
+    return stride;
+}
+
+// The first configuration field in which a and b differ, lstm_impl excepted (streaming always runs the mma kernels); null if none
+static const char* cfg_diff(const fsn_config& a, const fsn_config& b, int* va, int* vb) {
+    static const struct { const char* name; size_t off; } f[] = {
+        {"model_kind", offsetof(fsn_config, model_kind)}, {"num_freqs", offsetof(fsn_config, num_freqs)},
+        {"look_ahead", offsetof(fsn_config, look_ahead)}, {"sb_num_neighbors", offsetof(fsn_config, sb_num_neighbors)},
+        {"fb_num_neighbors", offsetof(fsn_config, fb_num_neighbors)}, {"fb_hidden", offsetof(fsn_config, fb_hidden)},
+        {"sb_hidden", offsetof(fsn_config, sb_hidden)}, {"num_layers", offsetof(fsn_config, num_layers)},
+        {"output_size", offsetof(fsn_config, output_size)}, {"fb_act", offsetof(fsn_config, fb_act)}, {"sb_act", offsetof(fsn_config, sb_act)},
+        {"norm_type", offsetof(fsn_config, norm_type)}, {"kersize[0]", offsetof(fsn_config, kersize)},
+        {"kersize[1]", offsetof(fsn_config, kersize) + 4}, {"kersize[2]", offsetof(fsn_config, kersize) + 8},
+        {"fast_math", offsetof(fsn_config, fast_math)}, {"channel_attention", offsetof(fsn_config, channel_attention)},
+        {"rnn_type", offsetof(fsn_config, rnn_type)}, {"subband_num", offsetof(fsn_config, subband_num)},
+        {"tcn_causal", offsetof(fsn_config, tcn_causal)}, {"sb_tcn", offsetof(fsn_config, sb_tcn)}};
+    static_assert(sizeof(fsn_config) == (sizeof(f) / sizeof(f[0]) + 1) * sizeof(int32_t), "every fsn_config field but lstm_impl is compared");
+    for (const auto& e : f) {
+        memcpy(va, reinterpret_cast<const char*>(&a) + e.off, 4);
+        memcpy(vb, reinterpret_cast<const char*>(&b) + e.off, 4);
+        if (*va != *vb) return e.name;
+    }
+    return nullptr;
+}
+
+static int state_slots_ok(const fsn_stream* st, int n, const int32_t* h_slots, bool unique) {
+    if (n < 1) return fail(FSN_EINVAL, "n = %d: at least one slot", n);
+    if (!h_slots) return fail(FSN_EINVAL, "h_slots is null (n = %d slot indices)", n);
+    std::vector<int> seen(unique ? st->B : 0, -1);
+    for (int i = 0; i < n; ++i) {
+        const int b = h_slots[i];
+        if (b < 0 || b >= st->B) return fail(FSN_EINVAL, "h_slots[%d] = %d is out of range (slots 0..%d)", i, b, st->B - 1);
+        if (unique && seen[b] >= 0) return fail(FSN_EINVAL, "h_slots[%d] = %d: slot %d is loaded twice (also h_slots[%d])", i, b, b, seen[b]);
+        if (unique) seen[b] = i;
+    }
+    return FSN_OK;
+}
+
+static int state_buffer_ok(const fsn_stream* st, const void* d_state) {
+    if (!d_state) return fail(FSN_EINVAL, "d_state is null");
+    cudaPointerAttributes pa{}, ph{};
+    const cudaError_t e = cudaPointerGetAttributes(&pa, d_state);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return fail(FSN_EINVAL, "d_state is not device memory (%s)", cudaGetErrorString(e));
+    }
+    if (pa.type != cudaMemoryTypeDevice && pa.type != cudaMemoryTypeManaged)
+        return fail(FSN_EINVAL, "d_state is not device memory (memory type %d: a host pointer)", (int)pa.type);
+    CK(cudaPointerGetAttributes(&ph, st->cum_in.p));
+    if (pa.device != ph.device) return fail(FSN_EINVAL, "d_state is memory of device %d, the handle lives on device %d", pa.device, ph.device);
+    if (reinterpret_cast<uintptr_t>(d_state) % 256) return fail(FSN_EINVAL, "d_state is not 256-byte aligned");
+    return FSN_OK;
+}
+
+// A handle that has only used fsn_stream_step takes per-slot counts, as at its first slot call
+static int use_slot_counts(fsn_stream* st) {
+    if (st->slots) return FSN_OK;
+    if (st->d_slot.ensure((size_t)st->B * sizeof(int32_t), false)) return fail(FSN_ECUDA, "slot-count buffer allocation failed");
+    st->nb.assign(st->B, st->n);
+    st->slots = true;
+    return FSN_OK;
+}
+
+// One launch of stream_state_copy_kernel for n sessions: the segments at their handle rows, cut into items of at most `chunk` bytes
+// (32 KB, doubled until the items fit the launch's table).  Weight-stationary handles read and write the exchange-buffer parity the
+// next tick reads.
+static int state_copy(fsn_stream* st, int n, const int32_t* h_slots, void* d_state, int mode, bool save, cudaStream_t s) {
+    const fsn_config& c = st->m->cfg;
+    StateSegSpec sp[STREAM_STATE_MAX_SEG];
+    size_t off[STREAM_STATE_MAX_SEG];
+    int ns = 0;
+    int64_t stride = 0;
+    if (int rc = state_layout(c, mode, sp, off, &ns, &stride)) return rc;
+    const size_t Hf = c.fb_hidden, Hs = c.sb_hidden;
+    const int par = (st->n ^ 1) & 1;
+    char* base[STREAM_STATE_MAX_SEG] = {};
+    size_t lstride[STREAM_STATE_MAX_SEG] = {};
+    base[SEG_CUM_IN] = static_cast<char*>(st->cum_in.p);
+    base[SEG_CUM_SB] = static_cast<char*>(st->cum_sb.p);
+    if (st->use_ws) {                                    // ws_h [L][2][64][Hf], ws_c [L][64][Hf]
+        base[SEG_FB_H] = static_cast<char*>(st->ws_h.p) + par * 64 * Hf * 2; lstride[SEG_FB_H] = 2 * 64 * Hf * 2;
+        base[SEG_FB_C] = static_cast<char*>(st->ws_c.p); lstride[SEG_FB_C] = 64 * Hf * 4;
+    } else {                                             // h_fb / c_fb [L][ra_fb][Hf]
+        base[SEG_FB_H] = static_cast<char*>(st->h_fb.p); lstride[SEG_FB_H] = st->ra_fb * Hf * 2;
+        base[SEG_FB_C] = static_cast<char*>(st->c_fb.p); lstride[SEG_FB_C] = st->ra_fb * Hf * 4;
+    }
+    base[SEG_SB_H] = static_cast<char*>(st->h_sb.p); lstride[SEG_SB_H] = st->ra_sb * Hs * 2;
+    base[SEG_SB_C] = static_cast<char*>(st->c_sb.p); lstride[SEG_SB_C] = st->ra_sb * Hs * 4;
+    if (mode == FSN_STATE_MODE_AUDIO) {
+        base[SEG_HIST] = static_cast<char*>(st->a_hist.p);
+        base[SEG_SPEC] = static_cast<char*>(st->a_spec.p);
+        base[SEG_TAIL] = static_cast<char*>(st->a_tail.p);
+    }
+    StreamStateLaunch a{};
+    a.nseg = ns;
+    for (int i = 0; i < ns; ++i)
+        a.seg[i] = StreamStateSeg{base[i], lstride[i], sp[i].slot_bytes, off[i], sp[i].L, (sp[i].slot_bytes % 16 || lstride[i] % 16) ? 8 : 16};
+    auto cut = [&](size_t chunk) {
+        int k = 0;
+        for (int i = 0; i < ns; ++i)
+            for (int l = 0; l < sp[i].L; ++l)
+                for (size_t b = 0; b < sp[i].slot_bytes; b += chunk) {
+                    if (k == STREAM_STATE_MAX_ITEMS) return false;
+                    a.item[k++] = StreamStateItem{i, l, (uint32_t)b, (uint32_t)(b + chunk < sp[i].slot_bytes ? b + chunk : sp[i].slot_bytes)};
+                }
+        a.nitem = k;
+        return true;
+    };
+    for (size_t chunk = 32768; !cut(chunk); chunk *= 2) {}
+    if (st->x_slot.ensure((size_t)(n > st->B ? n : st->B) * sizeof(int32_t), false)) return fail(FSN_ECUDA, "slot-list buffer allocation failed");
+    fsn_stream::Stage* gp = nullptr;
+    if (int rc = stage_next(st, n, &gp)) return rc;
+    memcpy(gp->h, h_slots, (size_t)n * sizeof(int32_t));
+    CK(cudaMemcpyAsync(st->x_slot.p, gp->h, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    CK(cudaEventRecord(gp->ev, s));
+    gp->used = true;
+    a.slots = static_cast<const int*>(st->x_slot.p); a.n = n;
+    a.payload = static_cast<char*>(d_state); a.stride = (size_t)stride; a.save = save ? 1 : 0;
+    const int e = launch_stream_state(a, s);
+    if (e) return fail(FSN_ECUDA, "session state copy failed: %s", cudaGetErrorString((cudaError_t)e));
+    return FSN_OK;
+}
+
+extern "C" int fsn_stream_save_slots(fsn_stream* st, int32_t n, const int32_t* h_slots, void* d_state, fsn_slot_meta* h_meta, void* stream) {
+    if (!st) return fail(FSN_EINVAL, "st is null");
+    if (int rc = state_slots_ok(st, n, h_slots, false)) return rc;
+    if (!h_meta) return fail(FSN_EINVAL, "h_meta is null (n = %d metas)", n);
+    const int mode = state_mode(st);
+    if (!mode || (mode == FSN_STATE_MODE_AUDIO && st->a_tick.empty()))
+        return fail(FSN_ESTATE, "the handle has served no call and no load: it holds no session to save");
+    if (int rc = state_buffer_ok(st, d_state)) return rc;
+    int64_t stride = 0;
+    if (int rc = state_layout(st->m->cfg, mode, nullptr, nullptr, nullptr, &stride)) return rc;
+    if (mode == FSN_STATE_MODE_MASK)
+        if (int rc = use_slot_counts(st)) return rc;
+    if (int rc = state_copy(st, n, h_slots, d_state, mode, true, static_cast<cudaStream_t>(stream))) return rc;
+    for (int i = 0; i < n; ++i) {
+        const int b = h_slots[i];
+        fsn_slot_meta& q = h_meta[i];
+        memset(&q, 0, sizeof(q));
+        q.magic = FSN_SLOT_STATE_MAGIC; q.version = FSN_SLOT_STATE_VERSION;
+        q.cfg = st->m->cfg; q.weights_id = st->m->weights_id; q.mode = mode;
+        if (mode == FSN_STATE_MODE_MASK) q.frames = st->nb[b];
+        else { q.tick = st->a_tick[b]; q.hops = st->a_hops[b]; }
+        q.payload_bytes = stride;
+    }
+    return FSN_OK;
+}
+
+extern "C" int fsn_stream_load_slots(fsn_stream* st, int32_t n, const int32_t* h_slots, const void* d_state, const fsn_slot_meta* h_meta,
+                                     void* stream) {
+    if (!st) return fail(FSN_EINVAL, "st is null");
+    if (int rc = state_slots_ok(st, n, h_slots, true)) return rc;
+    if (!h_meta) return fail(FSN_EINVAL, "h_meta is null (n = %d metas)", n);
+    const fsn_model* m = st->m;
+    const int hmode = state_mode(st);
+    static const char* kModeName[3] = {"", "mask", "audio"};
+    for (int i = 0; i < n; ++i) {                                       // every meta is checked before any state changes
+        const fsn_slot_meta& q = h_meta[i];
+        if (q.magic != FSN_SLOT_STATE_MAGIC) return fail(FSN_EINVAL, "h_meta[%d]: bad magic 0x%08x (not a saved session)", i, q.magic);
+        if (q.version != FSN_SLOT_STATE_VERSION)
+            return fail(FSN_EINVAL, "h_meta[%d]: version %u, this library reads version %d", i, q.version, FSN_SLOT_STATE_VERSION);
+        if (q.mode != FSN_STATE_MODE_MASK && q.mode != FSN_STATE_MODE_AUDIO)
+            return fail(FSN_EINVAL, "h_meta[%d]: mode %d is not FSN_STATE_MODE_MASK (1) or FSN_STATE_MODE_AUDIO (2)", i, q.mode);
+        const int want = hmode ? hmode : h_meta[0].mode;
+        if (q.mode != want)
+            return fail(FSN_ESTATE, "h_meta[%d]: a session of the %s call, this handle serves the %s call%s", i, kModeName[q.mode],
+                        kModeName[want], hmode ? "" : " (the mode of h_meta[0])");
+        int va = 0, vb = 0;
+        if (const char* f = cfg_diff(q.cfg, m->cfg, &va, &vb))
+            return fail(FSN_EINVAL, "h_meta[%d]: cfg.%s = %d, this handle's model has %d", i, f, va, vb);
+        if (q.weights_id != m->weights_id)
+            return fail(FSN_EINVAL, "h_meta[%d]: weights_id %016llx, this handle's model has %016llx (other weights)", i,
+                        (unsigned long long)q.weights_id, (unsigned long long)m->weights_id);
+        int64_t stride = 0;
+        if (int rc = state_layout(m->cfg, q.mode, nullptr, nullptr, nullptr, &stride)) return rc;
+        if (q.payload_bytes != stride)
+            return fail(FSN_EINVAL, "h_meta[%d]: payload_bytes %lld, this handle's payload is %lld bytes", i, (long long)q.payload_bytes,
+                        (long long)stride);
+        if (q.mode == FSN_STATE_MODE_MASK ? q.frames < 0 : (q.tick < -1 || q.hops < 0))
+            return fail(FSN_EINVAL, "h_meta[%d]: bad counters (frames %d, tick %d, hops %d)", i, q.frames, q.tick, q.hops);
+    }
+    if (int rc = state_buffer_ok(st, d_state)) return rc;
+    const int mode = h_meta[0].mode;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = claim_mode(st, mode == FSN_STATE_MODE_AUDIO ? fsn_stream::MODE_AUDIO : fsn_stream::MODE_MASK)) return rc;
+    if (mode == FSN_STATE_MODE_AUDIO && st->a_tick.empty()) {
+        if (int rc = audio_alloc(st, 2 * (m->cfg.num_freqs - 1), s)) return rc;
+        if (st->d_slot.ensure((size_t)4 * st->B * sizeof(int32_t), false)) return fail(FSN_ECUDA, "slot-count buffer allocation failed");
+    }
+    if (mode == FSN_STATE_MODE_MASK)
+        if (int rc = use_slot_counts(st)) return rc;
+    if (int rc = state_copy(st, n, h_slots, const_cast<void*>(d_state), mode, false, s)) return rc;
+    for (int i = 0; i < n; ++i) {
+        const int b = h_slots[i];
+        if (mode == FSN_STATE_MODE_MASK) st->nb[b] = h_meta[i].frames;
+        else { st->a_tick[b] = h_meta[i].tick; st->a_hops[b] = h_meta[i].hops; }
     }
     return FSN_OK;
 }

@@ -119,6 +119,23 @@ struct StreamResetBuf { void* p; size_t layer_bytes, row_bytes; int L, rows_per_
 struct StreamResetLaunch { StreamResetBuf buf[4]; int nbuf, B; const int* slot; };
 void launch_stream_reset(const StreamResetLaunch& a, cudaStream_t s);
 
+// ---- k_stream_state.cu: save / load of streaming sessions (fsn_stream_save_slots, fsn_stream_load_slots) ------------------------
+// One segment of the payload: the handle's rows of one state buffer.  Slot b's rows of layer l start at base + l layer_stride +
+// b slot_bytes; in the payload of session i they lie at i stride + pay_off + l slot_bytes.  vec: 16 or 8, the access width every
+// handle-side offset is a multiple of.
+struct StreamStateSeg { char* base; size_t layer_stride, slot_bytes, pay_off; int L, vec; };
+// A work item: bytes [begin, end) of one layer's rows of one segment (multiples of 16, except at the end of an 8-byte segment)
+struct StreamStateItem { int seg, layer; uint32_t begin, end; };
+constexpr int STREAM_STATE_MAX_SEG = 9, STREAM_STATE_MAX_ITEMS = 96;
+struct StreamStateLaunch {
+    StreamStateSeg seg[STREAM_STATE_MAX_SEG]; int nseg;
+    StreamStateItem item[STREAM_STATE_MAX_ITEMS]; int nitem;
+    const int* slots; int n;  // [n] device: the handle slot of session i
+    char* payload; size_t stride;
+    int save;                 // 1: handle -> payload (gather); 0: payload -> handle (scatter)
+};
+int launch_stream_state(const StreamStateLaunch& a, cudaStream_t s);   // returns 0 or cudaError
+
 // ---- k_stream_audio.cu: audio in and out of the streaming slot call (fsn_stream_step_audio_slots) ---------------------------
 // Per-slot ops of one tick, derived on the host from the slot's flag, tick count and hop count (fsn_api.cu, audio_plan)
 enum { AUDIO_STORE = 1,       // the slot's hop of samples goes to its history ring

@@ -23,6 +23,7 @@ SYMBOLS = [
     "fsn_gemm_f16", "fsn_gemm_f16_tile_n",
     "fsn_tc5r_gin_weights", "fsn_tc5r_ring_stages", "fsn_lstm_mma_rows", "fsn_model_sb_forward",
     "fsn_stream_step_slots", "fsn_stream_step_audio_slots",
+    "fsn_stream_state_bytes", "fsn_stream_state_layout", "fsn_model_weights_id", "fsn_stream_save_slots", "fsn_stream_load_slots",
 ]
 
 
@@ -36,6 +37,25 @@ class FsnConfig(C.Structure):
                                           "norm_type")] + [("kersize", C.c_int32 * 3), ("lstm_impl", C.c_int32),
                                                            ("fast_math", C.c_int32), ("channel_attention", C.c_int32), ("rnn_type", C.c_int32), ("subband_num", C.c_int32), ("tcn_causal", C.c_int32),
                                                            ("sb_tcn", C.c_int32)]
+
+
+STATE_MODE_MASK, STATE_MODE_AUDIO = 1, 2                    # FSN_STATE_MODE_*
+SLOT_STATE_MAGIC, SLOT_STATE_VERSION = 0x534E5346, 1        # FSN_SLOT_STATE_MAGIC ('F' 'S' 'N' 'S'), FSN_SLOT_STATE_VERSION
+
+
+class FsnSlotMeta(C.Structure):
+    """fsn_slot_meta: the host-side description of one saved streaming session (include/fsnplus_b200.h)."""
+    _fields_ = [("magic", C.c_uint32), ("version", C.c_uint32), ("cfg", FsnConfig), ("weights_id", C.c_uint64), ("mode", C.c_int32),
+                ("frames", C.c_int32), ("tick", C.c_int32), ("hops", C.c_int32), ("payload_bytes", C.c_int64)]
+
+
+def state_layout(cfg, mode):
+    """fsn_stream_state_layout: (payload bytes per session, sizeof(fsn_slot_meta)) of a configuration in mode STATE_MODE_MASK or
+    STATE_MODE_AUDIO.  Host only; needs no GPU."""
+    lib = load_library()
+    nb, mb = C.c_int64(), C.c_int32()
+    check(lib.fsn_stream_state_layout(C.byref(cfg), int(mode), C.byref(nb), C.byref(mb)))
+    return nb.value, mb.value
 
 
 def lib_path():
@@ -81,6 +101,13 @@ def load_library():
     lib.fsn_stream_step_audio_slots.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.fsn_stream_destroy.argtypes = [vp]
     lib.fsn_stream_destroy.restype = None
+    lib.fsn_stream_state_bytes.argtypes = [vp]
+    lib.fsn_stream_state_bytes.restype = i64
+    lib.fsn_stream_state_layout.argtypes = [C.POINTER(FsnConfig), i32, C.POINTER(i64), C.POINTER(i32)]
+    lib.fsn_model_weights_id.argtypes = [vp]
+    lib.fsn_model_weights_id.restype = C.c_uint64
+    lib.fsn_stream_save_slots.argtypes = [vp, i32, vp, vp, vp, vp]
+    lib.fsn_stream_load_slots.argtypes = [vp, i32, vp, vp, vp, vp]
     lib.fsn_apply_cirm.argtypes = [vp, vp, vp, i32, i32, i32, vp]
     lib.fsn_model_get_stage.argtypes = [vp, C.c_char_p, vp, i64, vp]
     lib.fsn_model_last_launch_count.argtypes = [vp]

@@ -332,6 +332,10 @@ class _B200Model(nn.Module):
     def last_launch_count(self):
         return int(_lib.load_library().fsn_model_last_launch_count(self._handle)) if self._handle else 0
 
+    def weights_id(self):
+        """fsn_model_weights_id: 64-bit hash of the parameters last pushed to the handle (0 before the first forward / stream)."""
+        return int(_lib.load_library().fsn_model_weights_id(self._handle)) if self._handle else 0
+
     def workspace_bytes(self):
         """Bytes this model currently holds in forward workspaces (both lanes and the sub-band scratch; parameters excluded)."""
         return int(_lib.load_library().fsn_model_workspace_bytes(self._handle)) if self._handle else 0

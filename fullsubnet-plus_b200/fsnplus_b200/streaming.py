@@ -12,6 +12,10 @@ and ends on its own schedule (flags HOLD / STEP / START per slot and tick, DESIG
 ``step_audio`` serves the same sessions with audio in and out: one hop of samples per slot and tick goes in, one hop of enhanced
 audio comes out, with the STFT, the cIRM and the overlap-add iSTFT on the device (flag FLUSH ends a session, DESIGN.md §3.10).
 A handle serves either the mask calls or the audio call.
+
+``save_slots`` / ``load_slots`` park, resume and move sessions (DESIGN.md §3.11): a ``SessionState`` holds the saved state of some
+slots, and loading it into any slot of a handle of the same model -- this one, one with another B, or one on another GPU -- continues
+each session where it was saved.
 """
 import ctypes as C
 
@@ -20,6 +24,56 @@ import torch
 from . import _lib
 
 HOLD, STEP, START, FLUSH = 0, 1, 2, 3  # FSN_SLOT_* of include/fsnplus_b200.h (FLUSH: audio call only)
+
+
+class SessionState:
+    """Saved streaming sessions: ``payload`` [n, stride] uint8 (a CUDA tensor, or pinned host memory after ``.to("cpu")``) and
+    ``meta``, a ctypes array of n ``fsn_slot_meta``.  ``len()``, indexing / selection (``state[2]``, ``state[[0, 3]]``, slices) and
+    ``.to(device)`` return new SessionState objects; the payload format is that of this library version only."""
+
+    def __init__(self, payload, meta):
+        assert payload.dtype == torch.uint8 and payload.dim() == 2 and payload.shape[0] == len(meta)
+        self.payload, self.meta = payload, meta
+
+    def __len__(self):
+        return self.payload.shape[0]
+
+    @property
+    def device(self):
+        return self.payload.device
+
+    def __getitem__(self, idx):
+        if isinstance(idx, slice):
+            ids = list(range(len(self)))[idx]
+        elif torch.is_tensor(idx):
+            ids = [int(i) for i in idx.reshape(-1).tolist()]
+        elif isinstance(idx, int):
+            ids = [idx]
+        else:
+            ids = [int(i) for i in idx]
+        ids = [i + len(self) if i < 0 else i for i in ids]
+        if any(i < 0 or i >= len(self) for i in ids):
+            raise IndexError(f"session index out of range (0..{len(self) - 1})")
+        meta = (_lib.FsnSlotMeta * len(ids))(*[self.meta[i] for i in ids])
+        sel = torch.tensor(ids, dtype=torch.long, device=self.payload.device)
+        payload = self.payload.index_select(0, sel)
+        if payload.device.type == "cpu" and self.payload.is_pinned():
+            payload = payload.pin_memory()
+        return SessionState(payload, meta)
+
+    def to(self, device):
+        """A copy on `device`: "cpu" gives pinned host memory, a CUDA device a plain copy (this object itself if it is there already)."""
+        device = torch.device(device)
+        if device.type == "cuda" and device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        if device == self.payload.device:
+            return self
+        if device.type == "cpu":
+            payload = torch.empty(self.payload.shape, dtype=torch.uint8).pin_memory()
+            payload.copy_(self.payload)
+        else:
+            payload = self.payload.to(device)
+        return SessionState(payload, (_lib.FsnSlotMeta * len(self))(*self.meta))
 
 
 class StreamingFullSubNet:
@@ -32,6 +86,9 @@ class StreamingFullSubNet:
             _lib.check(self.lib.fsn_stream_create(model._handle, batch_size, C.byref(h)))
         self._st = h
         self.F = model._cfg.num_freqs
+        _, meta_bytes = _lib.state_layout(model._cfg, _lib.STATE_MODE_MASK)
+        if meta_bytes != C.sizeof(_lib.FsnSlotMeta):
+            raise _lib.FsnError(f"fsn_slot_meta is {meta_bytes} bytes in the library, {C.sizeof(_lib.FsnSlotMeta)} in the ctypes mirror")
 
     def step(self, mag_frame):
         """mag_frame [B, F] float32 CUDA -> mask [B, 2, F] of frame (n - look_ahead), or None while the look-ahead fills."""
@@ -87,6 +144,39 @@ class StreamingFullSubNet:
                                                             C.c_void_p(f.data_ptr()), C.c_void_p(valid.data_ptr()),
                                                             C.c_void_p(mask.data_ptr() if return_mask else None), stream))
         return (out, valid.bool(), mask) if return_mask else (out, valid.bool())
+
+    def _slot_array(self, slots):
+        s = torch.as_tensor(slots, dtype=torch.int32).reshape(-1).contiguous()
+        assert s.device.type == "cpu" and s.numel() >= 1, "slots: host slot indices"
+        return s
+
+    def save_slots(self, slots):
+        """Snapshot the sessions of `slots` (a sequence or a CPU integer tensor) into a SessionState on this handle's device.  The slots
+        are unchanged: they may keep stepping (a fork) or START other sessions.  Ordered on the current stream like the step calls."""
+        s = self._slot_array(slots)
+        n = s.numel()
+        with torch.cuda.device(self.device):
+            stride = int(self.lib.fsn_stream_state_bytes(self._st))
+            _lib.check(stride if stride < 0 else 0)
+            payload = torch.empty((n, stride), dtype=torch.uint8, device=self.device)
+            meta = (_lib.FsnSlotMeta * n)()
+            stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+            _lib.check(self.lib.fsn_stream_save_slots(self._st, n, C.c_void_p(s.data_ptr()), C.c_void_p(payload.data_ptr()), meta, stream))
+        return SessionState(payload, meta)
+
+    def load_slots(self, slots, state):
+        """Load session i of `state` into slot slots[i] (distinct slots), replacing a START: the slot's next tick continues the session
+        where it was saved.  The state is copied to this handle's device first if it lives elsewhere."""
+        s = self._slot_array(slots)
+        assert s.numel() == len(state), f"{s.numel()} slots for {len(state)} sessions"
+        state = state.to(self.device)
+        payload = state.payload.contiguous()
+        if payload.data_ptr() % 256:
+            payload = payload.clone()
+        with torch.cuda.device(self.device):
+            stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+            _lib.check(self.lib.fsn_stream_load_slots(self._st, s.numel(), C.c_void_p(s.data_ptr()), C.c_void_p(payload.data_ptr()),
+                                                      state.meta, stream))
 
     def flush(self):
         """Feed look_ahead zero frames (the reference's right padding) and return the remaining masks."""

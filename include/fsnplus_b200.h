@@ -217,6 +217,53 @@ int fsn_stream_step_slots(fsn_stream* st, const float* d_mag_frame, float* d_mas
 int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_samples, float* d_out, const int32_t* h_flags, int32_t* h_valid,
                                 float* d_mask, void* stream);
 
+/* Park, resume and move sessions (DESIGN.md §3.11): save the state of some slots to a device buffer and load it into any slot of a
+ * compatible handle -- the same one, another with a different B or full-band kernel, or one on another device after the caller has
+ * copied the payload there.
+ *
+ * A saved session is a payload row of payload_bytes (d_state [n, payload_bytes], device) plus a host fsn_slot_meta.  The payload is
+ * canonical: one layout per (configuration, mode), independent of B, of the slot, of the full-band kernel (weight-stationary at B <= 64,
+ * generic above) and of the handle's tick parity.  Segments in this order, each at a 16-byte aligned offset: cum_in (2 fp64), cum_sb
+ * (num_freqs x 2 fp64), full-band h (fp16, every layer) and c (fp32, every layer; the GRU keeps its fp32 h there), sub-band h and c
+ * (num_freqs rows per layer each), then in audio mode the history ring, the spectrum ring and the overlap tail.  payload_bytes is a
+ * multiple of 256.
+ *
+ * fsn_stream_save_slots is a snapshot: the slots are unchanged and may keep stepping (a fork) or START other sessions.  h_meta[i]
+ * describes session i, saved from slot h_slots[i].
+ * fsn_stream_load_slots replaces a START: it overwrites the whole state of slot h_slots[i] with session i, host counters included, and
+ * the slot's next tick is a STEP (or FLUSH).  A START after a load discards the loaded state like any other.
+ * Both calls are ordered on `stream` like the step calls: h_meta is filled (save) or validated (load) on the host before the call
+ * returns, the payload copy (one kernel) is enqueued and the stream is not synchronised; h_slots and h_meta are free on return.
+ * A handle that has served no call yet takes the meta's mode at a load (and allocates its audio state in audio mode); a handle that
+ * has only used fsn_stream_step switches to per-slot counts at a save or load, as at its first slot call.
+ * Errors change no state.  FSN_EINVAL, naming the index or field: a null array, n < 1, a slot out of range, a slot twice in one load, a
+ * bad magic or version, a payload_bytes other than this handle's, a configuration field that differs (lstm_impl excepted: streaming
+ * always runs the mma kernels), a weights_id that differs, a d_state that is not 256-byte aligned device memory of the handle's
+ * device.  FSN_ESTATE: a meta whose mode is not the handle's, a save on a handle that has served no call. */
+#define FSN_SLOT_STATE_VERSION 1
+#define FSN_SLOT_STATE_MAGIC 0x534E5346u   /* the bytes 'F' 'S' 'N' 'S' */
+#define FSN_STATE_MODE_MASK 1              /* saved from a handle serving fsn_stream_step / fsn_stream_step_slots */
+#define FSN_STATE_MODE_AUDIO 2             /* saved from a handle serving fsn_stream_step_audio_slots             */
+typedef struct fsn_slot_meta {      /* host-side description of one saved session                                  */
+    uint32_t magic, version;        /* FSN_SLOT_STATE_MAGIC, FSN_SLOT_STATE_VERSION                                 */
+    fsn_config cfg;                 /* the saving model's configuration                                             */
+    uint64_t weights_id;            /* fsn_model_weights_id of the saving model                                     */
+    int32_t mode;                   /* FSN_STATE_MODE_MASK or FSN_STATE_MODE_AUDIO                                  */
+    int32_t frames;                 /* mask mode: frames the slot consumed since its START (0 in audio mode)        */
+    int32_t tick, hops;             /* audio mode: the slot's tick count (-1 = no session) and hops K (0 before its first FLUSH); 0 in mask mode */
+    int64_t payload_bytes;          /* stride of one session in d_state                                             */
+} fsn_slot_meta;
+/* Payload stride of this handle's mode; FSN_ESTATE before the handle has served a call or a load. */
+int64_t fsn_stream_state_bytes(const fsn_stream* st);
+/* Payload stride of a (configuration, mode) and sizeof(fsn_slot_meta).  Host only, no GPU.  FSN_EINVAL for a configuration that cannot
+ * stream (FullSubNet+, a non-cumulative norm), a mode other than 1 or 2, or an audio mode whose num_freqs the audio call rejects. */
+int fsn_stream_state_layout(const fsn_config* cfg, int32_t mode, int64_t* payload_bytes, int32_t* meta_bytes);
+/* 64-bit hash of every parameter (key and fp32 bytes) of a finalized model: equal weights give equal ids.  0 before fsn_model_finalize. */
+uint64_t fsn_model_weights_id(const fsn_model* m);
+int fsn_stream_save_slots(fsn_stream* st, int32_t n, const int32_t* h_slots, void* d_state, fsn_slot_meta* h_meta, void* stream);
+int fsn_stream_load_slots(fsn_stream* st, int32_t n, const int32_t* h_slots, const void* d_state, const fsn_slot_meta* h_meta,
+                          void* stream);
+
 /* Fused post-processing of the inferencer method (fullsubnet_plus/inferencer/inferencer.py:152-157 and
  * audio_zen/acoustics/mask.py:60-63): decompress_cIRM (K = 10, limit = 9.9) + complex multiply with the noisy spectrum.
  * d_crm [B, 2, F, T] float32 (model output), d_noisy / d_enh [B, F, T] complex64 (interleaved re, im). */

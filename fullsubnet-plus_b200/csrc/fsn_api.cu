@@ -47,6 +47,42 @@ struct DevBuf {
     void release() { if (p) cudaFree(p); p = nullptr; bytes = 0; }
 };
 
+// Pinned host staging of small int32 arrays on their way to the device: a ring of slots, each refilled only after the event recorded
+// behind its last H2D copy has fired.  So the caller's host array is free when a call returns and no stream has to be synchronised.
+struct PinnedStage {
+    static const int NSLOT = 4;
+    struct Slot { int32_t* h = nullptr; size_t cap = 0; cudaEvent_t ev = nullptr; bool used = false; } slot[NSLOT];
+    int64_t next = 0;
+    Slot* cur = nullptr;
+    // The next slot, holding at least n int32, once the copy that last read it has completed
+    int take(size_t n, int32_t** h) {
+        Slot& g = *(cur = &slot[next++ % NSLOT]);
+        if (!g.ev) CK(cudaEventCreateWithFlags(&g.ev, cudaEventDisableTiming));
+        if (g.used) CK(cudaEventSynchronize(g.ev));
+        if (g.cap < n) {
+            if (g.h) CK(cudaFreeHost(g.h));
+            g.h = nullptr; g.cap = 0;
+            CK(cudaHostAlloc(reinterpret_cast<void**>(&g.h), n * sizeof(int32_t), cudaHostAllocDefault));
+            g.cap = n;
+        }
+        *h = g.h;
+        return FSN_OK;
+    }
+    // Copy the first n int32 of the slot last taken to d on stream s
+    int send(void* d, size_t n, cudaStream_t s) {
+        CK(cudaMemcpyAsync(d, cur->h, n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+        CK(cudaEventRecord(cur->ev, s));
+        cur->used = true;
+        return FSN_OK;
+    }
+    ~PinnedStage() {
+        for (Slot& g : slot) {
+            if (g.h) cudaFreeHost(g.h);
+            if (g.ev) cudaEventDestroy(g.ev);
+        }
+    }
+};
+
 // weights_id: folds n bytes into h 8 bytes at a time (the last word zero-padded).  Each step is a bijection of h (xor, odd multiply,
 // xorshift), so two byte strings of the same length that differ in any word give different results.
 static uint64_t hash_words(uint64_t h, const void* p, size_t n) {
@@ -168,11 +204,7 @@ struct fsn_model {
     cudaEvent_t ev0[NEV] = {}, ev1[NEV] = {};               // sub-band LSTM start / end
     cudaEvent_t evf0[NEV] = {}, evf1[NEV] = {};             // front end start / end (same ring index)
     int64_t nfwd = 0;                                 // forwards whose LSTM events were recorded
-    // ragged forwards: pinned staging slots of the per-sample extents.  A slot is refilled only after the event recorded behind its
-    // H2D copy has fired, so the caller's frames array is free when the call returns and no stream has to be synchronised.
-    static const int NLEN = 4;
-    struct LenSlot { int32_t* h = nullptr; size_t cap = 0; cudaEvent_t ev = nullptr; bool used = false; } len_slot[NLEN];
-    int64_t nlen = 0;
+    PinnedStage len_stage;                            // ragged forwards: the per-sample extents
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -545,10 +577,6 @@ extern "C" void fsn_model_destroy(fsn_model* m) {
         if (m->evf1[i]) cudaEventDestroy(m->evf1[i]);
     }
     for (int i = 0; i < 4; ++i) { m->sb_frag[i].release(); m->sb_bias[i].release(); m->fb_frag[i].release(); m->fb_bias[i].release(); }
-    for (auto& ls : m->len_slot) {
-        if (ls.h) cudaFreeHost(ls.h);
-        if (ls.ev) cudaEventDestroy(ls.ev);
-    }
     delete m;
 }
 
@@ -1041,25 +1069,15 @@ static int run_sb_tcn(fsn_model* m, Lane& ln, int B, int T, int Fc, SbPackLaunch
 // the sub-band LSTM on stream `sl` (== s for the plain entry point; the pipelined entry points pass the LSTM stream, ordered
 // after the front end by the lane's ev_front).
 // Copy the per-sample extents frames[b] + look_ahead of a ragged forward into the lane's device buffer ln.tlen ([3][B]: one row per
-// full-band branch, so a full-band gLN group z = branch * B + b indexes it directly) through the next pinned staging slot.
+// full-band branch, so a full-band gLN group z = branch * B + b indexes it directly) through the model's pinned staging.
 static int stage_lengths(fsn_model* m, Lane& ln, const int32_t* h_frames, int B, cudaStream_t s) {
-    fsn_model::LenSlot& ls = m->len_slot[m->nlen++ % fsn_model::NLEN];
     const size_t n = (size_t)3 * B;
-    if (!ls.ev) CK(cudaEventCreateWithFlags(&ls.ev, cudaEventDisableTiming));
-    if (ls.used) CK(cudaEventSynchronize(ls.ev));                        // the copy that last read this slot has completed
-    if (ls.cap < n) {
-        if (ls.h) CK(cudaFreeHost(ls.h));
-        ls.h = nullptr; ls.cap = 0;
-        CK(cudaHostAlloc(reinterpret_cast<void**>(&ls.h), n * sizeof(int32_t), cudaHostAllocDefault));
-        ls.cap = n;
-    }
+    int32_t* h = nullptr;
+    if (int rc = m->len_stage.take(n, &h)) return rc;
     for (int br = 0; br < 3; ++br)
-        for (int b = 0; b < B; ++b) ls.h[(size_t)br * B + b] = h_frames[b] + m->cfg.look_ahead;
+        for (int b = 0; b < B; ++b) h[(size_t)br * B + b] = h_frames[b] + m->cfg.look_ahead;
     if (ln.tlen.ensure(n * sizeof(int32_t), false, s)) return fail(FSN_ECUDA, "workspace allocation failed for the clip lengths");
-    CK(cudaMemcpyAsync(ln.tlen.p, ls.h, n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    CK(cudaEventRecord(ls.ev, s));
-    ls.used = true;
-    return FSN_OK;
+    return m->len_stage.send(ln.tlen.p, n, s);
 }
 
 // h_frames: the frame count of every sample of a ragged batch (validated by the caller), or null when every sample spans T frames
@@ -1670,20 +1688,20 @@ extern "C" int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst,
 struct fsn_stream {
     fsn_model* m;
     int B, n = 0;                                      // n: ticks of the handle (the weight-stationary exchange-buffer parity)
-    DevBuf cum_in, cum_sb, fbin, fbx, hseq, fbout, ximg, c_fb, c_sb, h_fb, h_sb, ws_h, ws_c, ws_bar;
+    DevBuf cum_in, cum_sb, h_fb, c_fb, h_sb, c_sb, ws_h, ws_c;   // session state (the table STATE)
+    DevBuf fbin, fbx, hseq, fbout, ximg, ws_bar;       // per-tick scratch of the step
     bool use_ws = false;
     int ra_fb = 0, ra_sb = 0, rows_pad = 0, Ipad = 0;
     // slot call (fsn_stream_step_slots): once used, every step runs per slot.  nb: frames each slot has consumed since its START
-    // (seeded with n at the first slot call); d_slot: this tick's per-slot counts for the kernels, -1 = held.  The counts reach the
-    // device through pinned staging slots, each refilled only after the event behind its last H2D copy has fired.
+    // (seeded with n at the first slot call); d_slot [5 B]: this tick's per-slot values for the kernels -- the counts (-1 = held),
+    // then the audio call's three planes, then the slots a START zeroes.  They reach the device through `stage`.
     bool slots = false;
     std::vector<int32_t> nb, all_step, valid;
     DevBuf d_slot;
-    static const int NSTAGE = 4;
-    struct Stage { int32_t* h = nullptr; cudaEvent_t ev = nullptr; bool used = false; size_t cap = 0; } stage[NSTAGE];
-    int64_t nstage = 0;
-    // A handle serves either the mask calls (fsn_stream_step, fsn_stream_step_slots) or the audio call, whichever it meets first
-    enum { MODE_NONE, MODE_MASK, MODE_AUDIO } mode = MODE_NONE;
+    PinnedStage stage;                                 // every tick's d_slot values, and the slot lists of save / load
+    // A handle serves either the mask calls (fsn_stream_step, fsn_stream_step_slots) or the audio call, whichever it meets first:
+    // FSN_STATE_MODE_MASK or FSN_STATE_MODE_AUDIO, 0 before
+    int mode = 0;
     // audio call (fsn_stream_step_audio_slots), allocated at its first use.  Per slot on the host: a_tick = ticks of the session so
     // far, HOLD excluded (-1: no session); a_hops = its hops K, known from its first FLUSH (0 before).  On the device: the history
     // ring, the noisy-spectrum ring, the overlap tail, the model's input row, the mask rows when the caller passes none, and the tables
@@ -1694,103 +1712,175 @@ struct fsn_stream {
     DevBuf x_slot;
 };
 
+// The state of a session: one entry per buffer, in payload order (DESIGN.md §3.11).  The handle's allocation (fsn_stream_create,
+// audio_alloc), its release, the payload layout (state_layout), the save / load copy and the START reset all read this table.
+enum { SEG_CUM_IN, SEG_CUM_SB, SEG_FB_H, SEG_FB_C, SEG_SB_H, SEG_SB_C, SEG_HIST, SEG_SPEC, SEG_TAIL, NSEG };
+static_assert(NSEG <= STREAM_STATE_MAX_SEG, "every segment fits the copy kernel's table");
+enum : unsigned {
+    ST_LAYERS = 1,      // one set of rows per LSTM layer (else one set)
+    ST_BINS = 2,        // F rows per slot, one per bin (else one row)
+    ST_START = 4,       // a START zeroes it: the recurrent state (the norm sums restart at count 0, the audio state at slot tick 0)
+    ST_AUDIO = 8,       // audio mode only, after every segment of both modes
+    ST_PARITY = 16,     // the weight-stationary variant holds two parities of rows per layer
+};
+struct StateBuf {
+    DevBuf fsn_stream::*buf;
+    DevBuf fsn_stream::*ws;                            // the weight-stationary full-band step's buffer in its place (64 rows), or null
+    size_t (*row_bytes)(const fsn_config&);
+    unsigned flags;
+};
+static const StateBuf STATE[NSEG] = {
+    {&fsn_stream::cum_in, nullptr, [](const fsn_config&) -> size_t { return 2 * sizeof(double); }, 0},   // running sum, sum of squares
+    {&fsn_stream::cum_sb, nullptr, [](const fsn_config&) -> size_t { return 2 * sizeof(double); }, ST_BINS},
+    {&fsn_stream::h_fb, &fsn_stream::ws_h, [](const fsn_config& c) -> size_t { return c.fb_hidden * sizeof(__half); }, ST_LAYERS | ST_START | ST_PARITY},
+    {&fsn_stream::c_fb, &fsn_stream::ws_c, [](const fsn_config& c) -> size_t { return c.fb_hidden * sizeof(float); }, ST_LAYERS | ST_START},
+    {&fsn_stream::h_sb, nullptr, [](const fsn_config& c) -> size_t { return c.sb_hidden * sizeof(__half); }, ST_LAYERS | ST_BINS | ST_START},
+    {&fsn_stream::c_sb, nullptr, [](const fsn_config& c) -> size_t { return c.sb_hidden * sizeof(float); }, ST_LAYERS | ST_BINS | ST_START},
+    {&fsn_stream::a_hist, nullptr, [](const fsn_config& c) -> size_t { return 3 * (c.num_freqs - 1) * sizeof(float); }, ST_AUDIO},   // 3 hops
+    {&fsn_stream::a_spec, nullptr, [](const fsn_config& c) -> size_t { return (c.look_ahead + 1) * c.num_freqs * sizeof(float2); }, ST_AUDIO},
+    {&fsn_stream::a_tail, nullptr, [](const fsn_config& c) -> size_t { return (c.num_freqs - 1) * sizeof(float); }, ST_AUDIO},      // 1 hop
+};
+static size_t seg_slot_bytes(const fsn_config& c, int i) { return (STATE[i].flags & ST_BINS ? c.num_freqs : 1) * STATE[i].row_bytes(c); }
+static int seg_layers(const fsn_config& c, int i) { return STATE[i].flags & ST_LAYERS ? c.num_layers : 1; }
+
+// Where handle st keeps segment i: slot b's rows of layer l at buf + offset + l * layer + b * seg_slot_bytes.  Layers of the generic
+// step's buffers are its rows_alloc rows apart.  The weight-stationary step's h is double-buffered by tick parity (tick n reads
+// (n - 1) & 1, writes n & 1): the state is the parity the handle's next tick reads.
+struct SegPlace { DevBuf* buf; size_t offset, layer; };
+static SegPlace seg_place(fsn_stream* st, int i) {
+    const StateBuf& e = STATE[i];
+    const fsn_config& c = st->m->cfg;
+    const size_t row = e.row_bytes(c);
+    SegPlace p{&(st->*e.buf), 0, (size_t)st->B * seg_slot_bytes(c, i)};
+    if (st->use_ws && e.ws) {
+        p.buf = &(st->*e.ws);
+        p.layer = (e.flags & ST_PARITY ? 2 : 1) * 64 * row;
+        if (e.flags & ST_PARITY) p.offset = ((st->n ^ 1) & 1) * 64 * row;
+    } else if (e.flags & ST_LAYERS) {
+        p.layer = (size_t)(e.flags & ST_BINS ? st->ra_sb : st->ra_fb) * row;
+    }
+    return p;
+}
+
+// Allocate, zero-filled on stream s, the state segments of both modes (audio = 0) or of the audio mode only (audio = ST_AUDIO)
+static int state_alloc(fsn_stream* st, unsigned audio, cudaStream_t s) {
+    int e = 0;
+    for (int i = 0; i < NSEG; ++i)
+        if ((STATE[i].flags & ST_AUDIO) == audio) {
+            const SegPlace p = seg_place(st, i);
+            e |= p.buf->ensure(seg_layers(st->m->cfg, i) * p.layer, true, s);
+        }
+    return e;
+}
+
+// stream_state_copy_kernel's tables for the segments i < ns whose flags include `need`: each at its handle place and payload offset
+// off[i] (off null: zeroing, no payload), each layer cut into items of at most `chunk` bytes (32 KB, doubled until the items fit)
+static void state_launch(fsn_stream* st, int ns, unsigned need, const size_t* off, StreamStateLaunch& a) {
+    const fsn_config& c = st->m->cfg;
+    a.nseg = ns;
+    for (int i = 0; i < ns; ++i) {
+        if ((STATE[i].flags & need) != need) continue;
+        const SegPlace p = seg_place(st, i);
+        const size_t n = seg_slot_bytes(c, i);
+        a.seg[i] = StreamStateSeg{static_cast<char*>(p.buf->p) + p.offset, p.layer, n, off ? off[i] : 0, seg_layers(c, i),
+                                  (n % 16 || p.layer % 16) ? 8 : 16};
+    }
+    auto cut = [&](size_t chunk) {
+        int k = 0;
+        for (int i = 0; i < ns; ++i)                   // segments left out have L = 0
+            for (int l = 0; l < a.seg[i].L; ++l)
+                for (size_t b = 0, n = a.seg[i].slot_bytes; b < n; b += chunk) {
+                    if (k == STREAM_STATE_MAX_ITEMS) return false;
+                    a.item[k++] = StreamStateItem{i, l, (uint32_t)b, (uint32_t)(b + chunk < n ? b + chunk : n)};
+                }
+        a.nitem = k;
+        return true;
+    };
+    for (size_t chunk = 32768; !cut(chunk); chunk *= 2) {}
+}
+
+// The configurations that stream: fullsubnet.Model with a cumulative norm
+static int streams_ok(const fsn_config& c) {
+    if (c.model_kind != FSN_KIND_FSN)
+        return fail(FSN_EINVAL, "model_kind %d: streaming needs fullsubnet.Model (FullSubNet+ is not causal: TSSE pools over all time)", c.model_kind);
+    if (c.norm_type != FSN_NORM_CUMULATIVE_LAPLACE && c.norm_type != FSN_NORM_CUMULATIVE_LAYER)
+        return fail(FSN_EINVAL, "norm_type %d: streaming needs a cumulative norm_type", c.norm_type);
+    return FSN_OK;
+}
+
+// The audio call's geometry: n_fft = 2 (num_freqs - 1) a power of two from 64 to 1024
+static int audio_fft_ok(const fsn_config& c) {
+    const int N = 2 * (c.num_freqs - 1);
+    if (N < 64 || N > 1024 || (N & (N - 1)))
+        return fail(FSN_EINVAL, "num_freqs %d: the audio call needs n_fft = 2 (num_freqs - 1) to be a power of two from 64 to 1024 "
+                                "(num_freqs 33, 65, 129, 257 or 513)", c.num_freqs);
+    return FSN_OK;
+}
+
 extern "C" int fsn_stream_create(fsn_model* m, int32_t B, fsn_stream** out) {
     if (!m || !out || B < 1) return fail(FSN_EINVAL, "bad argument");
     if (!m->finalized) return fail(FSN_ESTATE, "fsn_model_finalize has not been called");
     const fsn_config& c = m->cfg;
-    if (c.model_kind != FSN_KIND_FSN) return fail(FSN_EINVAL, "streaming needs fullsubnet.Model (FullSubNet+ is not causal: TSSE pools over all time)");
-    if (c.norm_type != FSN_NORM_CUMULATIVE_LAPLACE && c.norm_type != FSN_NORM_CUMULATIVE_LAYER)
-        return fail(FSN_EINVAL, "streaming needs a cumulative norm_type");
+    if (int rc = streams_ok(c)) return rc;
     fsn_stream* st = new fsn_stream();
     st->m = m; st->B = B;
     const int F = c.num_freqs, rows = B * F, ntiles = (rows + 127) / 128;
     st->Ipad = (F + 15) / 16 * 16; st->rows_pad = (B + 63) / 64 * 64;
-    int e = 0;
-    e |= st->cum_in.ensure((size_t)B * 2 * sizeof(double), true);
-    e |= st->cum_sb.ensure((size_t)rows * 2 * sizeof(double), true);
-    e |= st->fbin.ensure((size_t)B * F * 4 * 4, true);
+    lstm_mma_cstate_bytes(1, B, 1, &st->ra_fb);
+    lstm_mma_cstate_bytes(1, rows, 1, &st->ra_sb);
+    st->use_ws = lstm_ws_supported(c.num_layers, c.fb_hidden, st->Ipad, B, m->num_sms) && !m->env_no_ws;
+    // scratch, then state, then the barrier: with the state allocated first, steps at 16-64 slots measured ~0.03 ms slower per tick
+    int e = st->fbin.ensure((size_t)B * F * 4 * 4, true);
     e |= st->fbx.ensure((size_t)st->rows_pad * st->Ipad * 2, true);
     e |= st->hseq.ensure((size_t)B * c.fb_hidden * 4 * 4, true);
     e |= st->fbout.ensure((size_t)B * F * 4 * 4, true);
     e |= st->ximg.ensure((size_t)ntiles * 16384, true);
-    e |= st->c_fb.ensure(lstm_mma_cstate_bytes(c.num_layers, B, c.fb_hidden, &st->ra_fb), true);
-    e |= st->c_sb.ensure(lstm_mma_cstate_bytes(c.num_layers, rows, c.sb_hidden, &st->ra_sb), true);
-    e |= st->h_fb.ensure((size_t)c.num_layers * st->ra_fb * c.fb_hidden * 2, true);
-    e |= st->h_sb.ensure((size_t)c.num_layers * st->ra_sb * c.sb_hidden * 2, true);
-    st->use_ws = lstm_ws_supported(c.num_layers, c.fb_hidden, st->Ipad, B, m->num_sms) && !m->env_no_ws;
-    if (st->use_ws) {
-        e |= st->ws_h.ensure((size_t)c.num_layers * 2 * 64 * c.fb_hidden * 2, true);
-        e |= st->ws_c.ensure((size_t)c.num_layers * 64 * c.fb_hidden * 4, true);
-        e |= st->ws_bar.ensure(64, true);
-    }
-    if (e) { delete st; return fail(FSN_ECUDA, "stream state allocation failed"); }
+    e |= state_alloc(st, 0, nullptr);
+    if (st->use_ws) e |= st->ws_bar.ensure(64, true);
+    e |= st->d_slot.ensure((size_t)5 * B * sizeof(int32_t), false);
+    if (e) { fsn_stream_destroy(st); return fail(FSN_ECUDA, "stream state allocation failed"); }
     *out = st;
     return FSN_OK;
 }
 
 extern "C" void fsn_stream_destroy(fsn_stream* st) {
     if (!st) return;
-    DevBuf* all[] = {&st->cum_in, &st->cum_sb, &st->fbin, &st->fbx, &st->hseq, &st->fbout, &st->ximg, &st->c_fb, &st->c_sb, &st->h_fb, &st->h_sb, &st->ws_h, &st->ws_c, &st->ws_bar};
-    for (auto* b : all) b->release();
-    for (auto& g : st->stage) {
-        if (g.h) cudaFreeHost(g.h);
-        if (g.ev) cudaEventDestroy(g.ev);
+    for (const StateBuf& e : STATE) {
+        (st->*e.buf).release();
+        if (e.ws) (st->*e.ws).release();
     }
-    st->d_slot.release();
-    st->x_slot.release();
-    DevBuf* audio[] = {&st->a_hist, &st->a_spec, &st->a_tail, &st->a_mag, &st->a_mask, &st->a_tab};
-    for (auto* b : audio) b->release();
+    DevBuf* scratch[] = {&st->fbin, &st->fbx, &st->hseq, &st->fbout, &st->ximg, &st->ws_bar, &st->a_mag, &st->a_mask, &st->a_tab,
+                         &st->d_slot, &st->x_slot};
+    for (auto* b : scratch) b->release();
     delete st;
 }
 
 static int claim_mode(fsn_stream* st, int mode) {
-    if (st->mode != fsn_stream::MODE_NONE && st->mode != mode)
-        return fail(FSN_ESTATE, mode == fsn_stream::MODE_AUDIO
+    if (st->mode && st->mode != mode)
+        return fail(FSN_ESTATE, mode == FSN_STATE_MODE_AUDIO
                                     ? "this handle serves the mask calls (fsn_stream_step, fsn_stream_step_slots): create another for audio"
                                     : "this handle serves the audio call (fsn_stream_step_audio_slots): create another for masks");
-    st->mode = static_cast<decltype(st->mode)>(mode);
+    st->mode = mode;
     return FSN_OK;
 }
 
-// The next pinned staging slot for the per-slot values of one tick, holding at least n int32.  A slot is refilled only after the
-// event behind its last H2D copy has fired.
-static int stage_next(fsn_stream* st, size_t n, fsn_stream::Stage** out) {
-    fsn_stream::Stage& g = st->stage[st->nstage++ % fsn_stream::NSTAGE];
-    if (!g.ev) CK(cudaEventCreateWithFlags(&g.ev, cudaEventDisableTiming));
-    if (g.used) CK(cudaEventSynchronize(g.ev));                         // the copy that last read this slot has completed
-    if (g.cap < n) {
-        if (g.h) CK(cudaFreeHost(g.h));
-        g.h = nullptr; g.cap = 0;
-        CK(cudaHostAlloc(reinterpret_cast<void**>(&g.h), n * sizeof(int32_t), cudaHostAllocDefault));
-        g.cap = n;
-    }
-    *out = &g;
-    return FSN_OK;
+// A handle that has only used fsn_stream_step takes per-slot counts, each slot at the handle's frame count
+static void use_slot_counts(fsn_stream* st) {
+    if (!st->slots) st->nb.assign(st->B, st->n);
+    st->slots = true;
 }
 
 // One tick of the handle.  slot: null (the lockstep step: every slot at frame n) or the device per-slot counts of the slot call;
-// reset: this tick has a START, so the slots at count 0 get their recurrent state zeroed first.
-static int stream_tick(fsn_stream* st, const float* d_mag, float* d_mask, const int* slot, bool reset, cudaStream_t s) {
+// zero[nzero]: device list of the slots whose recurrent state is zeroed first (a START's).
+static int stream_tick(fsn_stream* st, const float* d_mag, float* d_mask, const int* slot, const int* zero, int nzero, cudaStream_t s) {
     fsn_model* m = st->m;
     const fsn_config& c = m->cfg;
     const int B = st->B, F = c.num_freqs, n = st->n, resume = slot ? 1 : n > 0;    // slot call: a START zeroes instead of resume = 0
-    if (reset) {
-        StreamResetLaunch r{};
-        auto add = [&](void* p, size_t layer_bytes, size_t row_bytes, int rows_per_slot) {
-            r.buf[r.nbuf++] = StreamResetBuf{p, layer_bytes, row_bytes, c.num_layers, rows_per_slot};
-        };
-        const size_t Hf = c.fb_hidden, Hs = c.sb_hidden;
-        if (st->use_ws) {                                // ws_h [L][2][64][Hf]: the parity this tick's step reads; ws_c [L][64][Hf]
-            add(static_cast<char*>(st->ws_h.p) + ((n ^ 1) & 1) * 64 * Hf * 2, 2 * 64 * Hf * 2, Hf * 2, 1);
-            add(st->ws_c.p, 64 * Hf * 4, Hf * 4, 1);
-        } else {                                         // generic full-band step: [L][ra_fb][Hf]
-            add(st->h_fb.p, st->ra_fb * Hf * 2, Hf * 2, 1);
-            add(st->c_fb.p, st->ra_fb * Hf * 4, Hf * 4, 1);
-        }
-        add(st->h_sb.p, st->ra_sb * Hs * 2, Hs * 2, F);  // sub-band: [L][ra_sb][Hs], slot b = rows b F .. b F + F - 1
-        add(st->c_sb.p, st->ra_sb * Hs * 4, Hs * 4, F);
-        r.B = B; r.slot = slot;
-        launch_stream_reset(r, s);
+    if (nzero) {
+        StreamStateLaunch z{};
+        state_launch(st, NSEG, ST_START, nullptr, z);
+        z.slots = zero; z.n = nzero; z.dir = STREAM_STATE_ZERO;
+        if (int e = launch_stream_state(z, s)) return fail(FSN_ECUDA, "session state reset failed: %s", cudaGetErrorString((cudaError_t)e));
     }
     StreamNormLaunch na{d_mag, static_cast<float*>(st->fbin.p), static_cast<double*>(st->cum_in.p), B, F, 4, n, c.norm_type, slot};
     launch_stream_norm(na, s);
@@ -1851,33 +1941,29 @@ extern "C" int fsn_stream_step_slots(fsn_stream* st, const float* d_mag, float* 
             return fail(FSN_EINVAL, "slot %d: flag %d is not FSN_SLOT_HOLD (0), FSN_SLOT_STEP (1) or FSN_SLOT_START (2)", b, f);
         reset = reset || f == FSN_SLOT_START;
     }
-    if (int rc = claim_mode(st, fsn_stream::MODE_MASK)) return rc;
+    if (int rc = claim_mode(st, FSN_STATE_MODE_MASK)) return rc;
+    use_slot_counts(st);
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (!st->slots) {                                                   // until now every slot stepped with the handle
-        if (st->d_slot.ensure((size_t)B * sizeof(int32_t), false)) return fail(FSN_ECUDA, "slot-count buffer allocation failed");
-        st->nb.assign(B, st->n);
-        st->slots = true;
-    }
-    fsn_stream::Stage* gp = nullptr;
-    if (int rc = stage_next(st, B, &gp)) return rc;
-    fsn_stream::Stage& g = *gp;
-    for (int b = 0; b < B; ++b)
-        g.h[b] = h_flags[b] == FSN_SLOT_HOLD ? -1 : h_flags[b] == FSN_SLOT_START ? 0 : st->nb[b];
-    CK(cudaMemcpyAsync(st->d_slot.p, g.h, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    CK(cudaEventRecord(g.ev, s));
-    g.used = true;
-    const int rc = stream_tick(st, d_mag, d_mask, static_cast<const int*>(st->d_slot.p), reset, s);
-    if (rc) return rc;
+    int32_t* cnt = nullptr;                                             // [B] counts, then the slots this tick's START zeroes
+    if (int rc = st->stage.take((size_t)2 * B, &cnt)) return rc;
+    int nzero = 0;
     for (int b = 0; b < B; ++b) {
-        if (g.h[b] >= 0) st->nb[b] = g.h[b] + 1;
-        h_valid[b] = g.h[b] >= 0 && st->nb[b] > la ? 1 : 0;
+        cnt[b] = h_flags[b] == FSN_SLOT_HOLD ? -1 : h_flags[b] == FSN_SLOT_START ? 0 : st->nb[b];
+        if (reset && cnt[b] == 0) cnt[B + nzero++] = b;                 // started, or never stepped
+    }
+    const int* d = static_cast<const int*>(st->d_slot.p);
+    if (int rc = st->stage.send(st->d_slot.p, (size_t)B + nzero, s)) return rc;
+    if (int rc = stream_tick(st, d_mag, d_mask, d, d + B, nzero, s)) return rc;
+    for (int b = 0; b < B; ++b) {
+        if (cnt[b] >= 0) st->nb[b] = cnt[b] + 1;
+        h_valid[b] = cnt[b] >= 0 && st->nb[b] > la ? 1 : 0;
     }
     return FSN_OK;
 }
 
 extern "C" int fsn_stream_step(fsn_stream* st, const float* d_mag, float* d_mask, int32_t* h_valid, void* stream) {
     if (!st || !d_mag || !d_mask) return fail(FSN_EINVAL, "null argument");
-    if (int rc = claim_mode(st, fsn_stream::MODE_MASK)) return rc;
+    if (int rc = claim_mode(st, FSN_STATE_MODE_MASK)) return rc;
     if (st->slots) {                                                    // the slot call with every slot stepping
         st->all_step.assign(st->B, FSN_SLOT_STEP);
         st->valid.resize(st->B);
@@ -1889,24 +1975,20 @@ extern "C" int fsn_stream_step(fsn_stream* st, const float* d_mag, float* d_mask
         return FSN_OK;
     }
     const int n = st->n;
-    const int rc = stream_tick(st, d_mag, d_mask, nullptr, false, static_cast<cudaStream_t>(stream));
+    const int rc = stream_tick(st, d_mag, d_mask, nullptr, nullptr, 0, static_cast<cudaStream_t>(stream));
     if (rc) return rc;
     if (h_valid) *h_valid = (n >= st->m->cfg.look_ahead) ? 1 : 0;
     return FSN_OK;
 }
 
-// Audio state of the handle, zero-filled on the call's stream, and the tables of its n_fft (computed in double).
-static int audio_alloc(fsn_stream* st, int N, cudaStream_t s) {
-    const fsn_config& c = st->m->cfg;
-    const size_t B = st->B, H = N / 2, F = H + 1, la = c.look_ahead;
-    int e = 0;
-    e |= st->a_hist.ensure(B * 3 * H * sizeof(float), true, s);
-    e |= st->a_spec.ensure(B * (la + 1) * F * sizeof(float2), true, s);
-    e |= st->a_tail.ensure(B * H * sizeof(float), true, s);
+// Audio state of the handle and its scratch, zero-filled on the call's stream, and the tables of its n_fft (computed in double).
+static int audio_alloc(fsn_stream* st, cudaStream_t s) {
+    const size_t B = st->B, F = st->m->cfg.num_freqs;
+    int e = state_alloc(st, ST_AUDIO, s);
     e |= st->a_mag.ensure(B * F * sizeof(float), true, s);
     e |= st->a_mask.ensure(B * 2 * F * sizeof(float), true, s);
     std::vector<float> w, tw, inv;
-    stream_audio_tables(N, w, tw, inv);
+    stream_audio_tables((int)(2 * (F - 1)), w, tw, inv);
     st->a_tables = w;
     st->a_tables.insert(st->a_tables.end(), tw.begin(), tw.end());
     st->a_tables.insert(st->a_tables.end(), inv.begin(), inv.end());
@@ -1926,10 +2008,8 @@ extern "C" int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_sample
     if (!h_flags) return fail(FSN_EINVAL, "h_flags is null (one flag per slot, slots 0..%d)", st->B - 1);
     if (!h_valid) return fail(FSN_EINVAL, "h_valid is null (one result per slot, slots 0..%d)", st->B - 1);
     const fsn_config& c = st->m->cfg;
-    const int B = st->B, F = c.num_freqs, la = c.look_ahead, N = 2 * (F - 1);
-    if (N < 64 || N > 1024 || (N & (N - 1)))
-        return fail(FSN_EINVAL, "num_freqs %d: the audio call needs n_fft = 2 (num_freqs - 1) to be a power of two from 64 to 1024 "
-                                "(num_freqs 33, 65, 129, 257 or 513)", F);
+    const int B = st->B, la = c.look_ahead, N = 2 * (c.num_freqs - 1);
+    if (int rc = audio_fft_ok(c)) return rc;
     for (int b = 0; b < B; ++b) {                                       // every flag is checked before any state changes
         const int f = h_flags[b], t = st->a_tick.empty() ? -1 : st->a_tick[b], K = st->a_hops.empty() ? 0 : st->a_hops[b];
         if (f < FSN_SLOT_HOLD || f > FSN_SLOT_FLUSH)
@@ -1942,21 +2022,19 @@ extern "C" int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_sample
             return fail(FSN_EINVAL, "slot %d: FLUSH after %d hop: a session needs at least 2 hops (the STFT's reflect padding reads "
                                     "n_fft / 2 + 1 samples)", b, t);
     }
-    if (int rc = claim_mode(st, fsn_stream::MODE_AUDIO)) return rc;
+    if (int rc = claim_mode(st, FSN_STATE_MODE_AUDIO)) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (st->a_tick.empty()) {
-        if (int rc = audio_alloc(st, N, s)) return rc;
-        if (st->d_slot.ensure((size_t)4 * B * sizeof(int32_t), false)) return fail(FSN_ECUDA, "slot-count buffer allocation failed");
-    }
+    if (st->a_tick.empty())
+        if (int rc = audio_alloc(st, s)) return rc;
     // One staging slot carries the tick's four per-slot planes: the model's frame counts (-1 = the model row holds), the AUDIO_* ops,
-    // the slot ticks and the hop counts.  The schedule (DESIGN.md §3.10) for a session of K hops, slot tick k:
+    // the slot ticks and the hop counts; then the slots whose model row starts.  The schedule (DESIGN.md §3.10) for a session of K
+    // hops, slot tick k:
     //   k = 0 (START): store hop 0, the model row holds;  1 <= k <= K + 1: analyse frame k - 1, the model steps frame k - 1 (count
     //   k - 1, a START at k = 1);  k > K + 1: a zero frame;  k - 1 - la >= 0: synthesise that frame, emitting hop k - 2 - la from 1.
-    fsn_stream::Stage* gp = nullptr;
-    if (int rc = stage_next(st, (size_t)4 * B, &gp)) return rc;
-    fsn_stream::Stage& g = *gp;
-    int32_t *cnt = g.h, *op = g.h + B, *tick = g.h + 2 * B, *hops = g.h + 3 * B;
-    bool reset = false;
+    int32_t* cnt = nullptr;
+    if (int rc = st->stage.take((size_t)5 * B, &cnt)) return rc;
+    int32_t *op = cnt + B, *tick = cnt + 2 * B, *hops = cnt + 3 * B;
+    int nzero = 0;
     for (int b = 0; b < B; ++b) {
         const int f = h_flags[b];
         int k = st->a_tick[b], K = st->a_hops[b];
@@ -1973,12 +2051,10 @@ extern "C" int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_sample
             }
         }
         tick[b] = k; hops[b] = K;
-        reset = reset || cnt[b] == 0;
+        if (cnt[b] == 0) cnt[4 * B + nzero++] = b;
     }
     int32_t* d = static_cast<int32_t*>(st->d_slot.p);
-    CK(cudaMemcpyAsync(d, g.h, (size_t)4 * B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    CK(cudaEventRecord(g.ev, s));
-    g.used = true;
+    if (int rc = st->stage.send(d, (size_t)4 * B + nzero, s)) return rc;
     float* mask = d_mask ? d_mask : static_cast<float*>(st->a_mask.p);
     StreamAudioLaunch a{};
     a.op = d + B; a.tick = d + 2 * B; a.hops = d + 3 * B;
@@ -1989,7 +2065,7 @@ extern "C" int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_sample
     a.window = tab; a.twiddle = reinterpret_cast<const float2*>(tab + N); a.inv_env = tab + N + 2 * (N / 2 + 1);
     a.B = B; a.n_fft = N; a.la = la;
     launch_stream_stft(a, s);
-    const int rc = stream_tick(st, a.mag, mask, d, reset, s);
+    const int rc = stream_tick(st, a.mag, mask, d, d + 4 * B, nzero, s);
     if (rc) return rc;
     launch_stream_istft(a, s);
     CK(cudaGetLastError());
@@ -2003,35 +2079,25 @@ extern "C" int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_sample
 // ---------------------------------------------------------------------------------------------
 // park, resume and move sessions (DESIGN.md §3.11)
 // ---------------------------------------------------------------------------------------------
-// The payload's segments in payload order; per segment the bytes of one slot's rows of one layer and the layer count
-enum { SEG_CUM_IN, SEG_CUM_SB, SEG_FB_H, SEG_FB_C, SEG_SB_H, SEG_SB_C, SEG_HIST, SEG_SPEC, SEG_TAIL };
-struct StateSegSpec { size_t slot_bytes; int L; };
-
-static int state_layout(const fsn_config& c, int mode, StateSegSpec* seg, size_t* off, int* nseg, int64_t* stride) {
-    if (c.model_kind != FSN_KIND_FSN)
-        return fail(FSN_EINVAL, "model_kind %d: only fullsubnet.Model streams (FullSubNet+ is not causal: TSSE pools over all time)", c.model_kind);
-    if (c.norm_type != FSN_NORM_CUMULATIVE_LAPLACE && c.norm_type != FSN_NORM_CUMULATIVE_LAYER)
-        return fail(FSN_EINVAL, "norm_type %d: streaming needs a cumulative norm_type", c.norm_type);
+// The payload: the mode's segments of the table STATE in order, each at a 16-byte aligned offset off[i]; ns of them, the stride
+// rounded up to 256 bytes
+static int state_layout(const fsn_config& c, int mode, size_t* off, int* ns, int64_t* stride) {
+    if (int rc = streams_ok(c)) return rc;
     if (mode != FSN_STATE_MODE_MASK && mode != FSN_STATE_MODE_AUDIO)
         return fail(FSN_EINVAL, "mode %d is not FSN_STATE_MODE_MASK (1) or FSN_STATE_MODE_AUDIO (2)", mode);
     if (c.num_freqs < 4 || c.num_freqs > 2048 || c.look_ahead < 0 || c.num_layers < 1 || c.num_layers > 4 || c.fb_hidden < 16 ||
         c.fb_hidden % 16 || c.sb_hidden < 16 || c.sb_hidden % 16)
         return fail(FSN_EINVAL, "bad configuration: num_freqs %d, look_ahead %d, num_layers %d, fb_hidden %d, sb_hidden %d", c.num_freqs,
                     c.look_ahead, c.num_layers, c.fb_hidden, c.sb_hidden);
-    const size_t F = c.num_freqs, H = F - 1, N = 2 * H, la = c.look_ahead, Hf = c.fb_hidden, Hs = c.sb_hidden;
-    const int L = c.num_layers;
-    if (mode == FSN_STATE_MODE_AUDIO && (N < 64 || N > 1024 || (N & (N - 1))))
-        return fail(FSN_EINVAL, "num_freqs %d: the audio call needs n_fft = 2 (num_freqs - 1) to be a power of two from 64 to 1024", c.num_freqs);
-    const StateSegSpec s[9] = {{16, 1}, {F * 16, 1}, {Hf * 2, L}, {Hf * 4, L}, {F * Hs * 2, L}, {F * Hs * 4, L},
-                               {3 * H * 4, 1}, {(la + 1) * F * 8, 1}, {H * 4, 1}};
-    const int ns = mode == FSN_STATE_MODE_AUDIO ? 9 : 6;
+    if (mode == FSN_STATE_MODE_AUDIO)
+        if (int rc = audio_fft_ok(c)) return rc;
     size_t o = 0;
-    for (int i = 0; i < ns; ++i) {
-        if (seg) seg[i] = s[i];
-        if (off) off[i] = o;
-        o += (s[i].slot_bytes * s[i].L + 15) & ~(size_t)15;
+    int k = 0;
+    for (; k < NSEG && (mode == FSN_STATE_MODE_AUDIO || !(STATE[k].flags & ST_AUDIO)); ++k) {
+        if (off) off[k] = o;
+        o += (seg_slot_bytes(c, k) * seg_layers(c, k) + 15) & ~(size_t)15;
     }
-    if (nseg) *nseg = ns;
+    if (ns) *ns = k;
     *stride = (int64_t)((o + 255) & ~(size_t)255);
     return FSN_OK;
 }
@@ -2039,7 +2105,7 @@ static int state_layout(const fsn_config& c, int mode, StateSegSpec* seg, size_t
 extern "C" int fsn_stream_state_layout(const fsn_config* cfg, int32_t mode, int64_t* payload_bytes, int32_t* meta_bytes) {
     if (!cfg) return fail(FSN_EINVAL, "cfg is null");
     int64_t stride = 0;
-    if (int rc = state_layout(*cfg, mode, nullptr, nullptr, nullptr, &stride)) return rc;
+    if (int rc = state_layout(*cfg, mode, nullptr, nullptr, &stride)) return rc;
     if (payload_bytes) *payload_bytes = stride;
     if (meta_bytes) *meta_bytes = (int32_t)sizeof(fsn_slot_meta);
     return FSN_OK;
@@ -2047,16 +2113,11 @@ extern "C" int fsn_stream_state_layout(const fsn_config* cfg, int32_t mode, int6
 
 extern "C" uint64_t fsn_model_weights_id(const fsn_model* m) { return m && m->finalized ? m->weights_id : 0; }
 
-static int state_mode(const fsn_stream* st) {
-    return st->mode == fsn_stream::MODE_MASK ? FSN_STATE_MODE_MASK : st->mode == fsn_stream::MODE_AUDIO ? FSN_STATE_MODE_AUDIO : 0;
-}
-
 extern "C" int64_t fsn_stream_state_bytes(const fsn_stream* st) {
     if (!st) return fail(FSN_EINVAL, "st is null");
-    const int mode = state_mode(st);
-    if (!mode) return fail(FSN_ESTATE, "the handle has served no call and no load yet: its mode (masks or audio) is not known");
+    if (!st->mode) return fail(FSN_ESTATE, "the handle has served no call and no load yet: its mode (masks or audio) is not known");
     int64_t stride = 0;
-    if (int rc = state_layout(st->m->cfg, mode, nullptr, nullptr, nullptr, &stride)) return rc;
+    if (int rc = state_layout(st->m->cfg, st->mode, nullptr, nullptr, &stride)) return rc;
     return stride;
 }
 
@@ -2111,70 +2172,23 @@ static int state_buffer_ok(const fsn_stream* st, const void* d_state) {
     return FSN_OK;
 }
 
-// A handle that has only used fsn_stream_step takes per-slot counts, as at its first slot call
-static int use_slot_counts(fsn_stream* st) {
-    if (st->slots) return FSN_OK;
-    if (st->d_slot.ensure((size_t)st->B * sizeof(int32_t), false)) return fail(FSN_ECUDA, "slot-count buffer allocation failed");
-    st->nb.assign(st->B, st->n);
-    st->slots = true;
-    return FSN_OK;
-}
-
-// One launch of stream_state_copy_kernel for n sessions: the segments at their handle rows, cut into items of at most `chunk` bytes
-// (32 KB, doubled until the items fit the launch's table).  Weight-stationary handles read and write the exchange-buffer parity the
-// next tick reads.
-static int state_copy(fsn_stream* st, int n, const int32_t* h_slots, void* d_state, int mode, bool save, cudaStream_t s) {
-    const fsn_config& c = st->m->cfg;
-    StateSegSpec sp[STREAM_STATE_MAX_SEG];
-    size_t off[STREAM_STATE_MAX_SEG];
+// One launch of stream_state_copy_kernel for n sessions: the mode's segments between their handle slots h_slots and the payload.
+// A lockstep handle switches to per-slot counts first, as at its first slot call.
+static int state_copy(fsn_stream* st, int n, const int32_t* h_slots, void* d_state, int mode, int dir, cudaStream_t s) {
+    size_t off[NSEG] = {};
     int ns = 0;
     int64_t stride = 0;
-    if (int rc = state_layout(c, mode, sp, off, &ns, &stride)) return rc;
-    const size_t Hf = c.fb_hidden, Hs = c.sb_hidden;
-    const int par = (st->n ^ 1) & 1;
-    char* base[STREAM_STATE_MAX_SEG] = {};
-    size_t lstride[STREAM_STATE_MAX_SEG] = {};
-    base[SEG_CUM_IN] = static_cast<char*>(st->cum_in.p);
-    base[SEG_CUM_SB] = static_cast<char*>(st->cum_sb.p);
-    if (st->use_ws) {                                    // ws_h [L][2][64][Hf], ws_c [L][64][Hf]
-        base[SEG_FB_H] = static_cast<char*>(st->ws_h.p) + par * 64 * Hf * 2; lstride[SEG_FB_H] = 2 * 64 * Hf * 2;
-        base[SEG_FB_C] = static_cast<char*>(st->ws_c.p); lstride[SEG_FB_C] = 64 * Hf * 4;
-    } else {                                             // h_fb / c_fb [L][ra_fb][Hf]
-        base[SEG_FB_H] = static_cast<char*>(st->h_fb.p); lstride[SEG_FB_H] = st->ra_fb * Hf * 2;
-        base[SEG_FB_C] = static_cast<char*>(st->c_fb.p); lstride[SEG_FB_C] = st->ra_fb * Hf * 4;
-    }
-    base[SEG_SB_H] = static_cast<char*>(st->h_sb.p); lstride[SEG_SB_H] = st->ra_sb * Hs * 2;
-    base[SEG_SB_C] = static_cast<char*>(st->c_sb.p); lstride[SEG_SB_C] = st->ra_sb * Hs * 4;
-    if (mode == FSN_STATE_MODE_AUDIO) {
-        base[SEG_HIST] = static_cast<char*>(st->a_hist.p);
-        base[SEG_SPEC] = static_cast<char*>(st->a_spec.p);
-        base[SEG_TAIL] = static_cast<char*>(st->a_tail.p);
-    }
+    if (int rc = state_layout(st->m->cfg, mode, off, &ns, &stride)) return rc;
+    if (mode == FSN_STATE_MODE_MASK) use_slot_counts(st);
     StreamStateLaunch a{};
-    a.nseg = ns;
-    for (int i = 0; i < ns; ++i)
-        a.seg[i] = StreamStateSeg{base[i], lstride[i], sp[i].slot_bytes, off[i], sp[i].L, (sp[i].slot_bytes % 16 || lstride[i] % 16) ? 8 : 16};
-    auto cut = [&](size_t chunk) {
-        int k = 0;
-        for (int i = 0; i < ns; ++i)
-            for (int l = 0; l < sp[i].L; ++l)
-                for (size_t b = 0; b < sp[i].slot_bytes; b += chunk) {
-                    if (k == STREAM_STATE_MAX_ITEMS) return false;
-                    a.item[k++] = StreamStateItem{i, l, (uint32_t)b, (uint32_t)(b + chunk < sp[i].slot_bytes ? b + chunk : sp[i].slot_bytes)};
-                }
-        a.nitem = k;
-        return true;
-    };
-    for (size_t chunk = 32768; !cut(chunk); chunk *= 2) {}
+    state_launch(st, ns, 0, off, a);
     if (st->x_slot.ensure((size_t)(n > st->B ? n : st->B) * sizeof(int32_t), false)) return fail(FSN_ECUDA, "slot-list buffer allocation failed");
-    fsn_stream::Stage* gp = nullptr;
-    if (int rc = stage_next(st, n, &gp)) return rc;
-    memcpy(gp->h, h_slots, (size_t)n * sizeof(int32_t));
-    CK(cudaMemcpyAsync(st->x_slot.p, gp->h, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    CK(cudaEventRecord(gp->ev, s));
-    gp->used = true;
+    int32_t* h = nullptr;
+    if (int rc = st->stage.take(n, &h)) return rc;
+    memcpy(h, h_slots, (size_t)n * sizeof(int32_t));
+    if (int rc = st->stage.send(st->x_slot.p, n, s)) return rc;
     a.slots = static_cast<const int*>(st->x_slot.p); a.n = n;
-    a.payload = static_cast<char*>(d_state); a.stride = (size_t)stride; a.save = save ? 1 : 0;
+    a.payload = static_cast<char*>(d_state); a.stride = (size_t)stride; a.dir = dir;
     const int e = launch_stream_state(a, s);
     if (e) return fail(FSN_ECUDA, "session state copy failed: %s", cudaGetErrorString((cudaError_t)e));
     return FSN_OK;
@@ -2184,15 +2198,13 @@ extern "C" int fsn_stream_save_slots(fsn_stream* st, int32_t n, const int32_t* h
     if (!st) return fail(FSN_EINVAL, "st is null");
     if (int rc = state_slots_ok(st, n, h_slots, false)) return rc;
     if (!h_meta) return fail(FSN_EINVAL, "h_meta is null (n = %d metas)", n);
-    const int mode = state_mode(st);
+    const int mode = st->mode;
     if (!mode || (mode == FSN_STATE_MODE_AUDIO && st->a_tick.empty()))
         return fail(FSN_ESTATE, "the handle has served no call and no load: it holds no session to save");
     if (int rc = state_buffer_ok(st, d_state)) return rc;
     int64_t stride = 0;
-    if (int rc = state_layout(st->m->cfg, mode, nullptr, nullptr, nullptr, &stride)) return rc;
-    if (mode == FSN_STATE_MODE_MASK)
-        if (int rc = use_slot_counts(st)) return rc;
-    if (int rc = state_copy(st, n, h_slots, d_state, mode, true, static_cast<cudaStream_t>(stream))) return rc;
+    if (int rc = state_layout(st->m->cfg, mode, nullptr, nullptr, &stride)) return rc;
+    if (int rc = state_copy(st, n, h_slots, d_state, mode, STREAM_STATE_SAVE, static_cast<cudaStream_t>(stream))) return rc;
     for (int i = 0; i < n; ++i) {
         const int b = h_slots[i];
         fsn_slot_meta& q = h_meta[i];
@@ -2212,7 +2224,7 @@ extern "C" int fsn_stream_load_slots(fsn_stream* st, int32_t n, const int32_t* h
     if (int rc = state_slots_ok(st, n, h_slots, true)) return rc;
     if (!h_meta) return fail(FSN_EINVAL, "h_meta is null (n = %d metas)", n);
     const fsn_model* m = st->m;
-    const int hmode = state_mode(st);
+    const int hmode = st->mode;
     static const char* kModeName[3] = {"", "mask", "audio"};
     for (int i = 0; i < n; ++i) {                                       // every meta is checked before any state changes
         const fsn_slot_meta& q = h_meta[i];
@@ -2232,7 +2244,7 @@ extern "C" int fsn_stream_load_slots(fsn_stream* st, int32_t n, const int32_t* h
             return fail(FSN_EINVAL, "h_meta[%d]: weights_id %016llx, this handle's model has %016llx (other weights)", i,
                         (unsigned long long)q.weights_id, (unsigned long long)m->weights_id);
         int64_t stride = 0;
-        if (int rc = state_layout(m->cfg, q.mode, nullptr, nullptr, nullptr, &stride)) return rc;
+        if (int rc = state_layout(m->cfg, q.mode, nullptr, nullptr, &stride)) return rc;
         if (q.payload_bytes != stride)
             return fail(FSN_EINVAL, "h_meta[%d]: payload_bytes %lld, this handle's payload is %lld bytes", i, (long long)q.payload_bytes,
                         (long long)stride);
@@ -2242,14 +2254,10 @@ extern "C" int fsn_stream_load_slots(fsn_stream* st, int32_t n, const int32_t* h
     if (int rc = state_buffer_ok(st, d_state)) return rc;
     const int mode = h_meta[0].mode;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (int rc = claim_mode(st, mode == FSN_STATE_MODE_AUDIO ? fsn_stream::MODE_AUDIO : fsn_stream::MODE_MASK)) return rc;
-    if (mode == FSN_STATE_MODE_AUDIO && st->a_tick.empty()) {
-        if (int rc = audio_alloc(st, 2 * (m->cfg.num_freqs - 1), s)) return rc;
-        if (st->d_slot.ensure((size_t)4 * st->B * sizeof(int32_t), false)) return fail(FSN_ECUDA, "slot-count buffer allocation failed");
-    }
-    if (mode == FSN_STATE_MODE_MASK)
-        if (int rc = use_slot_counts(st)) return rc;
-    if (int rc = state_copy(st, n, h_slots, const_cast<void*>(d_state), mode, false, s)) return rc;
+    if (int rc = claim_mode(st, mode)) return rc;
+    if (mode == FSN_STATE_MODE_AUDIO && st->a_tick.empty())
+        if (int rc = audio_alloc(st, s)) return rc;
+    if (int rc = state_copy(st, n, h_slots, const_cast<void*>(d_state), mode, STREAM_STATE_LOAD, s)) return rc;
     for (int i = 0; i < n; ++i) {
         const int b = h_slots[i];
         if (mode == FSN_STATE_MODE_MASK) st->nb[b] = h_meta[i].frames;

@@ -113,13 +113,8 @@ struct StreamNormLaunch { const float* x; float* y; double* cum; int B, F, P, n,
 void launch_stream_norm(const StreamNormLaunch& a, cudaStream_t s);
 struct StreamPackLaunch { const float* mag; const float* fb; int Pfb; double* cum; __half* ximg; int B, F, Ns, Nf, n, type; const int* slot; };
 void launch_stream_pack(const StreamPackLaunch& a, cudaStream_t s);
-// zero the carried recurrent state of every slot whose count slot[b] is 0 (the slots a START resets): per buffer, L layers of
-// `rows_per_slot` rows of `row_bytes` each, layer l at p + l * layer_bytes, slot b's rows from b * rows_per_slot
-struct StreamResetBuf { void* p; size_t layer_bytes, row_bytes; int L, rows_per_slot; };
-struct StreamResetLaunch { StreamResetBuf buf[4]; int nbuf, B; const int* slot; };
-void launch_stream_reset(const StreamResetLaunch& a, cudaStream_t s);
 
-// ---- k_stream_state.cu: save / load of streaming sessions (fsn_stream_save_slots, fsn_stream_load_slots) ------------------------
+// ---- k_stream_state.cu: save / load of streaming sessions (fsn_stream_save_slots, fsn_stream_load_slots), START reset ----------
 // One segment of the payload: the handle's rows of one state buffer.  Slot b's rows of layer l start at base + l layer_stride +
 // b slot_bytes; in the payload of session i they lie at i stride + pay_off + l slot_bytes.  vec: 16 or 8, the access width every
 // handle-side offset is a multiple of.
@@ -127,12 +122,13 @@ struct StreamStateSeg { char* base; size_t layer_stride, slot_bytes, pay_off; in
 // A work item: bytes [begin, end) of one layer's rows of one segment (multiples of 16, except at the end of an 8-byte segment)
 struct StreamStateItem { int seg, layer; uint32_t begin, end; };
 constexpr int STREAM_STATE_MAX_SEG = 9, STREAM_STATE_MAX_ITEMS = 96;
+enum { STREAM_STATE_LOAD, STREAM_STATE_SAVE, STREAM_STATE_ZERO };
 struct StreamStateLaunch {
     StreamStateSeg seg[STREAM_STATE_MAX_SEG]; int nseg;
     StreamStateItem item[STREAM_STATE_MAX_ITEMS]; int nitem;
     const int* slots; int n;  // [n] device: the handle slot of session i
     char* payload; size_t stride;
-    int save;                 // 1: handle -> payload (gather); 0: payload -> handle (scatter)
+    int dir;                  // LOAD: payload -> handle (scatter); SAVE: handle -> payload (gather); ZERO: zeros -> handle, no payload
 };
 int launch_stream_state(const StreamStateLaunch& a, cudaStream_t s);   // returns 0 or cudaError
 

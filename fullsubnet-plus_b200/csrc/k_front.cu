@@ -731,22 +731,6 @@ __global__ void __launch_bounds__(128) stream_pack_kernel(StreamPackLaunch a) {
 }
 void launch_stream_pack(const StreamPackLaunch& a, cudaStream_t s) { stream_pack_kernel<<<(a.B * a.F + 127) / 128, 128, 0, s>>>(a); }
 
-// START of the slot call: zero the recurrent state rows of the slots whose count is 0.  Those are the started slots, plus slots that
-// have never stepped, whose rows are still zero from creation.  grid (B, nbuf, L): one block per (slot, buffer, layer).
-__global__ void __launch_bounds__(256) stream_reset_kernel(StreamResetLaunch a) {
-    const int b = blockIdx.x, l = blockIdx.z;
-    const StreamResetBuf& d = a.buf[blockIdx.y];
-    if (a.slot[b] != 0 || l >= d.L) return;
-    const size_t bytes = d.row_bytes * d.rows_per_slot;                   // rows are whole 16-byte chunks (H % 16 == 0)
-    uint4* p = reinterpret_cast<uint4*>(static_cast<char*>(d.p) + l * d.layer_bytes + b * bytes);
-    for (size_t i = threadIdx.x; i < bytes / 16; i += blockDim.x) p[i] = make_uint4(0u, 0u, 0u, 0u);
-}
-void launch_stream_reset(const StreamResetLaunch& a, cudaStream_t s) {
-    int L = 1;
-    for (int i = 0; i < a.nbuf; ++i) L = a.buf[i].L > L ? a.buf[i].L : L;
-    stream_reset_kernel<<<dim3(a.B, a.nbuf, L), 256, 0, s>>>(a);
-}
-
 // decompress_cIRM + complex multiply (inferencer.py:152-157, mask.py:60-63) in one pass.
 __global__ void apply_cirm_kernel(const float* crm, const float2* noisy, float2* enh, int FT, size_t n) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;

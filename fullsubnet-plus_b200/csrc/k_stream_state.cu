@@ -1,6 +1,6 @@
-// Save and load of streaming sessions (fsn_stream_save_slots / fsn_stream_load_slots, DESIGN.md §3.11): one launch moves the state of
-// n slots between the handle's per-slot rows and the canonical payload, [n, stride] bytes.  grid (n, items): block (i, j) copies work
-// item j of session i -- a piece of at most `chunk` bytes of one layer of one segment (StreamStateLaunch).  Memory-bound by design: each
+// Save, load and START reset of streaming sessions (DESIGN.md §3.11): one launch moves the state of n slots between the handle's
+// per-slot rows and the canonical payload, [n, stride] bytes, or zeroes those rows.  grid (n, items): block (i, j) handles work item j
+// of session i -- a piece of at most `chunk` bytes of one layer of one segment (StreamStateLaunch).  Memory-bound by design: each
 // thread keeps four 16-byte loads in flight before it stores them.
 #include "fsn_common.cuh"
 #include "fsn_kernels.h"
@@ -20,15 +20,26 @@ __device__ __forceinline__ void copy_vec(const char* __restrict__ src, char* __r
     for (; i < n; i += step) d[i] = s[i];
 }
 
+template <typename V>
+__device__ __forceinline__ void zero_vec(char* __restrict__ dst, uint32_t bytes) {
+    V* d = reinterpret_cast<V*>(dst);
+    for (uint32_t i = threadIdx.x; i < bytes / sizeof(V); i += blockDim.x) d[i] = V{};
+}
+
 __global__ void __launch_bounds__(256) stream_state_copy_kernel(StreamStateLaunch a) {
     const int i = blockIdx.x;
     const StreamStateItem it = a.item[blockIdx.y];
     const StreamStateSeg& g = a.seg[it.seg];
     const int slot = a.slots[i];
     char* h = g.base + it.layer * g.layer_stride + (size_t)slot * g.slot_bytes + it.begin;
+    if (a.dir == STREAM_STATE_ZERO) {
+        if (g.vec == 16) zero_vec<uint4>(h, it.end - it.begin);
+        else zero_vec<uint2>(h, it.end - it.begin);
+        return;
+    }
     char* p = a.payload + (size_t)i * a.stride + g.pay_off + (size_t)it.layer * g.slot_bytes + it.begin;
-    const char* src = a.save ? h : p;
-    char* dst = a.save ? p : h;
+    const char* src = a.dir == STREAM_STATE_SAVE ? h : p;
+    char* dst = a.dir == STREAM_STATE_SAVE ? p : h;
     if (g.vec == 16) copy_vec<uint4>(src, dst, it.end - it.begin);
     else copy_vec<uint2>(src, dst, it.end - it.begin);
 }

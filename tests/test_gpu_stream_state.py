@@ -189,6 +189,31 @@ def test_fork_park_resume(built_lib, kind, B, wait):
         assert e < MASK_TOL
 
 
+@pytest.mark.parametrize("B,slots", [(3, [0, 1, 2]), (80, [0, 37, 64, 79])])
+def test_start_after_random_load(built_lib, B, slots):
+    """A START zeroes every byte of recurrent state a load can write, in the exchange-buffer parity its tick reads: payloads of seeded
+    random bytes with valid metas are loaded into slots, then sessions START there, one per tick (both tick parities), at 3 slots
+    (weight-stationary full band) and 80 slots (generic full band).  Every session is bit-identical to its lone run."""
+    from fsnplus_b200.streaming import StreamingFullSubNet
+    cfg, _, m = _model("default")
+    la = cfg["look_ahead"]
+    clips = _clips("default", [9 + i for i in range(len(slots))], 41)
+    st = StreamingFullSubNet(m, batch_size=B, device=DEV)
+    d = Driver({"h": st}, la)
+    d.run(1)                                    # an all-held tick: the handle serves masks
+    state = st.save_slots(slots)
+    g = torch.Generator().manual_seed(B)
+    state.payload.copy_(torch.randint(0, 256, tuple(state.payload.shape), dtype=torch.uint8, generator=g))
+    st.load_slots(slots, state)
+    for i, slot in enumerate(slots):
+        d.start(i, "h", slot, clips[i])
+        d.run(1)
+    d.finish()
+    st.close()
+    for i, slot in enumerate(slots):
+        assert _same(d.result(i), _lone_of(m, d, i)), f"session {i} (slot {slot}) differs from its lone run"
+
+
 def test_neighbours_untouched(built_lib):
     """Every slot that is not loaded into gives, tick by tick, exactly the rows of the same schedule without the save and load calls
     (failed calls included)."""

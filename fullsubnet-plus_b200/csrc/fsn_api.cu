@@ -205,6 +205,10 @@ struct fsn_model {
     cudaEvent_t evf0[NEV] = {}, evf1[NEV] = {};             // front end start / end (same ring index)
     int64_t nfwd = 0;                                 // forwards whose LSTM events were recorded
     PinnedStage len_stage;                            // ragged forwards: the per-sample extents
+    // audio call (fsn_model_enhance_audio): its workspace (the analysis planes, the enhanced spectrum) is in the table WS; the tables of
+    // its n_fft are built at its first call.  au_valid: the workspace holds the whole batch of the last forward, an audio call
+    DevBuf au_planes, au_enh, au_tab;
+    bool au_valid = false;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -558,7 +562,7 @@ extern "C" void fsn_model_destroy(fsn_model* m) {
     if (!m) return;
     cudaDeviceSynchronize();
     release_ws(*m);
-    DevBuf* all[] = {&m->arena, &m->stage_in[0], &m->stage_in[1], &m->stage_in[2], &m->stage_out, &m->fb_fc, &m->fb_fc_b, &m->sb_fc};
+    DevBuf* all[] = {&m->arena, &m->stage_in[0], &m->stage_in[1], &m->stage_in[2], &m->stage_out, &m->fb_fc, &m->fb_fc_b, &m->sb_fc, &m->au_tab};
     for (auto* b : all) b->release();
     m->tcn_fb.release(); m->tcn_sb.release();
     for (auto& ln : m->lane) {
@@ -693,8 +697,9 @@ static int map_tcn_scratch(TcnScratch& sc, const TcnWeights& w, long long rows) 
 }
 
 // Bytes of every forward workspace buffer for a batch of B clips of T frames, the sub-band images and the layer-wise path's Gin / layer
-// output sized by the window Tw (0: the whole clip), the sub-band TCN's input and scratch by the bin chunk Fc (0: all bins).  One field
-// per entry of the table WS; ensure_ws allocates exactly these sizes, so the plan's count is what a forward holds.
+// output sized by the window Tw (0: the whole clip), the sub-band TCN's input and scratch by the bin chunk Fc (0: all bins); with
+// audio (fsn_model_enhance_audio) also its analysis planes and enhanced spectrum, and the clips' sample counts.  One field per entry of
+// the table WS; ensure_ws allocates exactly these sizes, so the plan's count is what a forward holds.
 struct WsSizes {
     size_t fbin = 0, fbout = 0, mu = 0, sigma = 0, tsse_scale = 0, sb_rowsum = 0, xn = 0, tlen = 0;       // lane: front end, ragged extents
     size_t sbx = 0, ximg = 0;                                                   // lane: sub-band TCN input, or the sub-band images
@@ -704,9 +709,10 @@ struct WsSizes {
     size_t sb_xa = 0, sb_xb = 0, sb_y1 = 0, sb_y2 = 0, sb_stats = 0;            // sub-band TCN scratch
     size_t ws_h = 0, ws_bar = 0;                                                // fullsubnet.Model's weight-stationary h exchange, barrier
     size_t mask_tmp = 0;                                                        // the generic kernel's scratch mask: not counted
+    size_t au_planes = 0, au_enh = 0;                                           // audio call: mag / real / imag planes, enhanced spectrum
     size_t total() const;
 };
-static WsSizes ws_sizes(const fsn_config& c, bool layerwise, int B, int T, int Tw, int Fc = 0) {
+static WsSizes ws_sizes(const fsn_config& c, bool layerwise, int B, int T, int Tw, int Fc = 0, bool audio = false) {
     WsSizes z;
     const int F = c.num_freqs, Tp = T + c.look_ahead, Pp = (Tp + 3) & ~3, Ts = Tw ? Tw : Tp;
     const int nbr = (c.model_kind == FSN_KIND_PLUS) ? 3 : 1;
@@ -715,7 +721,8 @@ static WsSizes ws_sizes(const fsn_config& c, bool layerwise, int B, int T, int T
     z.mu = z.sigma = (size_t)B * 4;
     z.tsse_scale = (size_t)nbr * B * F * 4 * (1 + tsse_row_floats());          // per-row scale | row statistics
     z.sb_rowsum = (size_t)B * 4 * F * 2 * 4;
-    z.tlen = (size_t)3 * B * sizeof(int32_t);                                   // counted whether the forward is ragged or not
+    z.tlen = (size_t)(audio ? 4 : 3) * B * sizeof(int32_t);                     // counted whether the forward is ragged or not
+    if (audio) { z.au_planes = (size_t)3 * B * F * T * 4; z.au_enh = (size_t)B * F * T * 8; }
     if (c.norm_type != FSN_NORM_OFFLINE_LAPLACE) z.xn = (size_t)nbr * B * F * Tp * 4;
     if (c.sb_tcn) {
         const size_t seqs = (size_t)B * (Fc ? Fc : F), srows = seqs * Tp;      // the sequences of one chunk run
@@ -809,6 +816,8 @@ static const WsBuf WS[] = {
     {MODEL_BUF(ws_h), &WsSizes::ws_h, WS_ON_USE},                                  // forward_impl
     {MODEL_BUF(ws_bar), &WsSizes::ws_bar, WS_ON_USE},
     {MODEL_BUF(mask_tmp), &WsSizes::mask_tmp, WS_ON_USE},                          // run_sb_lstm
+    {MODEL_BUF(au_planes), &WsSizes::au_planes, 0},                                // written whole by the analysis kernel
+    {MODEL_BUF(au_enh), &WsSizes::au_enh, 0},                                      // written whole by the sub-band stage's epilogue
 };
 
 size_t WsSizes::total() const {
@@ -822,6 +831,7 @@ static void release_lane(fsn_model& m, Lane& ln) {
     ln.geo = WsGeo{};
 }
 static void release_ws(fsn_model& m) {
+    m.au_valid = false;
     for (Lane& ln : m.lane) release_lane(m, ln);
     for (const WsBuf& e : WS) if (!(e.flags & WS_LANE)) e.buf(m, m.lane[0]).release();
 }
@@ -846,17 +856,18 @@ static int check_length(const fsn_config& c, int B, int T) {
     return FSN_OK;
 }
 
-// Size lane ln and the model's buffers for a forward of B clips of T frames with window Tw and bin chunk Fc (ws_sizes), each fresh
-// allocation zero-filled on its own stream (s: front end, sl: sub-band stage), and encode their tensor maps.
-static int ensure_ws(fsn_model* m, Lane& ln, int B, int T, int Tw, int Fc, cudaStream_t s, cudaStream_t sl) {
+// Size lane ln and the model's buffers for a forward of B clips of T frames with window Tw and bin chunk Fc (ws_sizes; audio: the audio
+// call's), each fresh allocation zero-filled on its own stream (s: front end, sl: sub-band stage), and encode their tensor maps.
+static int ensure_ws(fsn_model* m, Lane& ln, int B, int T, int Tw, int Fc, cudaStream_t s, cudaStream_t sl, bool audio = false) {
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs, Tp = T + c.look_ahead;
     const long long srows = (long long)B * (Fc ? Fc : F) * Tp;          // sub-band TCN: the rows of one chunk run
     if (c.sb_tcn && srows > SB_MAX_ROWS)
         return fail(FSN_EINVAL, "B * %s * (T + look_ahead) = %lld rows exceeds the sub-band TCN's 2^31 limit", Fc ? "bins per chunk" : "num_freqs", srows);
     if (c.model_kind == FSN_KIND_PLUS && !m->tcn5) return fail(FSN_ESTATE, "the TCN weights were not packed");
-    const WsSizes z = ws_sizes(c, runs_layerwise(c, m->env_impl), B, T, Tw, Fc);
+    const WsSizes z = ws_sizes(c, runs_layerwise(c, m->env_impl), B, T, Tw, Fc, audio);
     const WsGeo geo{B, T, Tw, Fc};
+    m->au_valid = false;
     const bool regeo = ln.geo != geo;
     if (Tw || Fc) {
         // A windowed or bin-chunked forward exists to bound the workspace: first give back every buffer earlier forwards left larger than
@@ -1069,29 +1080,40 @@ static int run_sb_tcn(fsn_model* m, Lane& ln, int B, int T, int Fc, SbPackLaunch
 // the sub-band LSTM on stream `sl` (== s for the plain entry point; the pipelined entry points pass the LSTM stream, ordered
 // after the front end by the lane's ev_front).
 // Copy the per-sample extents frames[b] + look_ahead of a ragged forward into the lane's device buffer ln.tlen ([3][B]: one row per
-// full-band branch, so a full-band gLN group z = branch * B + b indexes it directly) through the model's pinned staging.
-static int stage_lengths(fsn_model* m, Lane& ln, const int32_t* h_frames, int B, cudaStream_t s) {
-    const size_t n = (size_t)3 * B;
+// full-band branch, so a full-band gLN group z = branch * B + b indexes it directly) through the model's pinned staging.  h_samples:
+// the audio call's sample counts, appended as a fourth row in the same copy, or null.  h_frames may be null when h_samples is not
+// (clips of one frame count but different sample counts): the three rows are then zero and unread.
+static int stage_lengths(fsn_model* m, Lane& ln, const int32_t* h_frames, int B, cudaStream_t s, const int32_t* h_samples = nullptr) {
+    const size_t n = (size_t)(h_samples ? 4 : 3) * B;
     int32_t* h = nullptr;
     if (int rc = m->len_stage.take(n, &h)) return rc;
     for (int br = 0; br < 3; ++br)
-        for (int b = 0; b < B; ++b) h[(size_t)br * B + b] = h_frames[b] + m->cfg.look_ahead;
+        for (int b = 0; b < B; ++b) h[(size_t)br * B + b] = h_frames ? h_frames[b] + m->cfg.look_ahead : 0;
+    if (h_samples) memcpy(h + (size_t)3 * B, h_samples, (size_t)B * sizeof(int32_t));
     if (ln.tlen.ensure(n * sizeof(int32_t), false, s)) return fail(FSN_ECUDA, "workspace allocation failed for the clip lengths");
     return m->len_stage.send(ln.tlen.p, n, s);
 }
 
+// The waveform ends of one sub-batch of the audio call (fsn_model_enhance_audio): rows [B, L] in and out, and the clips' sample counts
+// (host; null when every clip is Lall samples; validated by the caller).  The forward then reads its spectra from, and writes the
+// enhanced spectrum to, the audio workspace.
+struct AudioIO { const float* wave; float* out; long long L; int Lall; const int32_t* h_samples; };
+
 // h_frames: the frame count of every sample of a ragged batch (validated by the caller), or null when every sample spans T frames
 // Tw: time window of the sub-band stage (0: the whole clip; > 0 needs s == sl, the plain entry points)
 // Fc: bin chunk of the sub-band TCN (0: all bins at once; > 0 needs s == sl, the plain entry points)
+// au: the audio call (s == sl): d_mag, d_real, d_imag, d_out and d_enh are ignored; one analysis launch runs before the forward and
+// one synthesis launch after it
 static int forward_impl(fsn_model* m, Lane& ln, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
-                        const int32_t* h_frames, float* d_out, float* d_enh, cudaStream_t s, cudaStream_t sl, int Tw = 0, int Fc = 0) {
-    if (!m || !d_mag || (!d_out && !d_enh)) return fail(FSN_EINVAL, "null argument");
-    if (d_enh && (!d_real || !d_imag)) return fail(FSN_EINVAL, "the enhanced-spectrum output needs the noisy real and imaginary planes");
-    if (d_enh && m->cfg.output_size != 2) return fail(FSN_EINVAL, "the enhanced-spectrum output needs output_size 2 (a complex mask)");
+                        const int32_t* h_frames, float* d_out, float* d_enh, cudaStream_t s, cudaStream_t sl, int Tw = 0, int Fc = 0,
+                        const AudioIO* au = nullptr) {
+    if (!m || (!au && (!d_mag || (!d_out && !d_enh)))) return fail(FSN_EINVAL, "null argument");
+    if (!au && d_enh && (!d_real || !d_imag)) return fail(FSN_EINVAL, "the enhanced-spectrum output needs the noisy real and imaginary planes");
+    if ((d_enh || au) && m->cfg.output_size != 2) return fail(FSN_EINVAL, "the enhanced-spectrum output needs output_size 2 (a complex mask)");
     if (!m->finalized) return fail(FSN_ESTATE, "fsn_model_finalize has not been called");
     const fsn_config& c = m->cfg;
     if (B < 1 || T < 1) return fail(FSN_EINVAL, "bad batch/frames");
-    if (c.model_kind == FSN_KIND_PLUS && (!d_real || !d_imag)) return fail(FSN_EINVAL, "FullSubNet_Plus.forward needs mag, real and imag");
+    if (c.model_kind == FSN_KIND_PLUS && !au && (!d_real || !d_imag)) return fail(FSN_EINVAL, "FullSubNet_Plus.forward needs mag, real and imag");
     const int F = c.num_freqs, Tp = T + c.look_ahead, Pp = (Tp + 3) & ~3;
     // chained (programmatic dependent) launches of this thread's front-end kernels: see env_pdl; "small" = at most 16 row-tile pairs,
     // where the forward is launch-latency-bound
@@ -1101,18 +1123,33 @@ static int forward_impl(fsn_model* m, Lane& ln, const float* d_mag, const float*
             if (Tp < c.kersize[i]) return fail(FSN_EINVAL, "sequence shorter than the TSSE kernel size");
     int rc = check_length(c, B, T);
     if (rc) return rc;
-    rc = ensure_ws(m, ln, B, T, Tw, Fc, s, sl);
+    rc = ensure_ws(m, ln, B, T, Tw, Fc, s, sl, au != nullptr);
     if (rc) return rc;
     const int* tl = nullptr;                                            // per-sample extents on the device (null: all Tp)
-    if (h_frames) {
-        rc = stage_lengths(m, ln, h_frames, B, s);
+    const int32_t* h_samples = au ? au->h_samples : nullptr;
+    if (h_frames || h_samples) {
+        rc = stage_lengths(m, ln, h_frames, B, s, h_samples);
         if (rc) return rc;
-        tl = static_cast<const int*>(ln.tlen.p);
+        if (h_frames) tl = static_cast<const int*>(ln.tlen.p);
     }
     m->launches = 0;
     m->last_lane = (int)(&ln - m->lane);
     const int evi = (int)(m->nfwd % fsn_model::NEV);
     cudaEventRecord(m->evf0[evi], s);
+    AudioLaunch al{};
+    if (au) {                                                           // the STFT of every clip into the planes the forward reads
+        const int N = 2 * (F - 1);
+        const AudioTables tab = audio_table_ptrs(static_cast<const float*>(m->au_tab.p), N);
+        al.wave = au->wave; al.out = au->out; al.L = au->L;
+        al.len = h_samples ? static_cast<const int*>(ln.tlen.p) + 3 * B : nullptr; al.Lall = au->Lall;
+        al.B = B; al.T = T; al.n_fft = N;
+        al.planes = static_cast<float*>(m->au_planes.p); al.enh = static_cast<const float2*>(m->au_enh.p);
+        al.window = tab.window; al.twiddle = tab.twiddle; al.inv_env = tab.inv_env; al.inv_last = tab.inv_last;
+        launch_audio_stft(al, s); m->launches++;
+        const size_t plane = (size_t)B * F * T;
+        d_mag = al.planes; d_real = al.planes + plane; d_imag = al.planes + 2 * plane;
+        d_out = nullptr; d_enh = static_cast<float*>(m->au_enh.p);
+    }
 
     SbPackLaunch sp{};
     sp.B = B; sp.F = F; sp.Tp = Tp; sp.Ns = c.sb_num_neighbors; sp.Nf = c.fb_num_neighbors; sp.P = Pp;
@@ -1261,6 +1298,7 @@ static int forward_impl(fsn_model* m, Lane& ln, const float* d_mag, const float*
                   : run_sb_lstm(m, ln, B, T, Tw, sp, d_out, d_real, d_imag, d_enh, tl, sl);
     cudaEventRecord(m->ev1[evi], sl);
     if (rc) return rc;
+    if (au) { launch_audio_istft(al, sl); m->launches++; }             // the iSTFT of every clip over its own frames
     m->nfwd++;
     CK(cudaGetLastError());
     return FSN_OK;
@@ -1310,9 +1348,9 @@ static int submit_impl(fsn_model* m, cudaEvent_t ready, const float* d_mag, cons
 // layer-wise path dominates: its time-batched input projection Gin takes 257 x T' x 4H x 2 bytes per sample (0.2 GB at config #5).
 // This estimate picks the sub-batch of a batch that fits unwindowed (plan_forward); it counts F rows per sample where the layer-wise
 // buffers hold whole pairs of 128-row tiles, so plan_forward checks its choice against the exact count of ws_sizes.
-static double ws_bytes_per_sample(const fsn_config& c, bool layerwise, int T) {
+static double ws_bytes_per_sample(const fsn_config& c, bool layerwise, int T, bool audio) {
     const double F = c.num_freqs, Tp = T + c.look_ahead, rows = F;              // sequences per sample
-    double b = 0;
+    double b = audio ? 20 * F * T : 0;                                           // the audio call's planes and enhanced spectrum
     if (c.model_kind == FSN_KIND_PLUS) b += 3 * F * Tp * 4 * 2 + 3 * Tp * (4.0 * ((c.num_freqs + 31) / 32 * 32) + 512) * 4;   // fb_in/out, X0/Xa/Xb/Xr (fp32), Y1/Y2 (fp16)
     else b += F * Tp * 4 * 4 + Tp * (F + c.fb_hidden) * 4;
     if (c.sb_tcn) {                                                             // input + two fp32 streams of 64 channels, two fp16 hidden
@@ -1344,20 +1382,20 @@ template <class Ok> static int largest(int lo, int hi, Ok ok) {
 //     chunk runs ceil(B / Bs) * ceil(F / Fc) wins, ties to the larger Bs (Fc = F, unchunked, is a candidate);
 //   * nothing fits: one clip at a time in one-bin chunks, allocated anyway.
 // Every chunk run keeps Bs * Fc * T' <= SB_MAX_ROWS.  force_bins > 0 (FSN_SB_CHUNK) chunks every TCN forward with exactly that many bins
-// (>= F: unchunked) and the largest equal split that fits with them.
-static Plan plan_forward(const fsn_config& c, bool layerwise, int B, int T, double cap, int force, int force_bins) {
+// (>= F: unchunked) and the largest equal split that fits with them.  audio: the audio call's plan, its workspace counted (ws_sizes).
+static Plan plan_forward(const fsn_config& c, bool layerwise, int B, int T, double cap, int force, int force_bins, bool audio = false) {
     const int Tp = T + c.look_ahead, wmax = (Tp + 31) / 32 * 32;
     const long long blim = max_clips_for_rows(c, T);             // sub-batches never exceed the full-band TCN's row limit
     auto split = [&](int bmax) { if (bmax > blim) bmax = (int)blim; if (bmax < 1) bmax = 1; if (B <= bmax) return B; const int n = (B + bmax - 1) / bmax; return (B + n - 1) / n; };
-    auto bytes = [&](int bs, int tw) { return (double)ws_sizes(c, layerwise, bs, T, tw).total(); };
+    auto bytes = [&](int bs, int tw) { return (double)ws_sizes(c, layerwise, bs, T, tw, 0, audio).total(); };
     // largest equal split bs with fits(bs) (0 if even one clip does not fit)
     auto max_split = [&](auto fits) { const int b = largest(0, B, [&](int v) { return fits(split(v)); }); return b ? split(b) : 0; };
-    const double per = ws_bytes_per_sample(c, layerwise, T);
+    const double per = ws_bytes_per_sample(c, layerwise, T, audio);
     const double bmax = cap / (per > 1 ? per : 1);
     Plan p{split(bmax < B ? (int)bmax : B)};
     if (c.sb_tcn) {
         const int F = c.num_freqs;
-        auto fits = [&](int bs, int fc) { return (long long)bs * fc * Tp <= SB_MAX_ROWS && ws_sizes(c, false, bs, T, 0, fc < F ? fc : 0).total() <= cap; };
+        auto fits = [&](int bs, int fc) { return (long long)bs * fc * Tp <= SB_MAX_ROWS && ws_sizes(c, false, bs, T, 0, fc < F ? fc : 0, audio).total() <= cap; };
         const int fforce = force_bins > 0 ? (force_bins < F ? force_bins : F) : 0;
         if (fforce) {                                                   // chunks of fforce bins (F: unchunked), the largest equal split that fits
             if (fforce < F || !fits(p.Bs, F)) {
@@ -1401,7 +1439,7 @@ static Plan plan_forward(const fsn_config& c, bool layerwise, int B, int T, doub
             p.Tw = ((Tp + nwin - 1) / nwin + 31) / 32 * 32;
         }
     }
-    p.bytes = (int64_t)ws_sizes(c, layerwise, p.Bs, T, p.Tw, p.Fc).total();
+    p.bytes = (int64_t)ws_sizes(c, layerwise, p.Bs, T, p.Tw, p.Fc, audio).total();
     return p;
 }
 
@@ -1500,6 +1538,99 @@ extern "C" int fsn_model_forward_enhance_ragged(fsn_model* m, const float* d_mag
     int rc = check_frames(m, h_frames, B, T, &fr);
     return rc ? rc : forward_plain(m, d_mag, d_real, d_imag, B, T, fr, nullptr, d_enh, stream);
 }
+// The audio call's geometry: n_fft = 2 (num_freqs - 1) a power of two from 64 to 1024
+static int audio_fft_ok(const fsn_config& c) {
+    const int N = 2 * (c.num_freqs - 1);
+    if (N < 64 || N > 1024 || (N & (N - 1)))
+        return fail(FSN_EINVAL, "num_freqs %d: the audio call needs n_fft = 2 (num_freqs - 1) to be a power of two from 64 to 1024 "
+                                "(num_freqs 33, 65, 129, 257 or 513)", c.num_freqs);
+    return FSN_OK;
+}
+
+// The audio call's geometry and clips (fsn_model_enhance_audio, fsn_plan_audio): n_fft = 2 (num_freqs - 1), every clip longer than
+// n_fft / 2 (torch.stft's reflect padding) and no longer than L, with enough frames for the TSSE kernels (check_frames, in samples),
+// and the forward's length limits on T = max_b L_b / hop + 1.  *Lmax: the longest clip; *all: every clip is Lmax samples long.
+static int audio_check(const fsn_config& c, int32_t B, int64_t L, const int64_t* h_lengths, int* T, int* Lmax, bool* all) {
+    if (int rc = audio_fft_ok(c)) return rc;
+    if (B < 1) return fail(FSN_EINVAL, "B = %d: the batch needs at least one clip", B);
+    if (L < 1 || L > 0x7fffffffLL) return fail(FSN_EINVAL, "L = %lld: the row length must be 1 .. 2^31 - 1 samples", (long long)L);
+    const int H = c.num_freqs - 1;                                      // hop = n_fft / 2
+    int kmax = 1;
+    if (c.model_kind == FSN_KIND_PLUS && c.channel_attention == FSN_ATTN_TSSE)
+        for (int i = 0; i < 3; ++i) kmax = c.kersize[i] > kmax ? c.kersize[i] : kmax;
+    long long mx = 0;
+    *all = true;
+    for (int b = 0; b < (h_lengths ? B : 1); ++b) {
+        const long long n = h_lengths ? h_lengths[b] : L;
+        char nm[40];
+        if (h_lengths) snprintf(nm, sizeof(nm), "clip %d: h_lengths[%d]", b, b);
+        else snprintf(nm, sizeof(nm), "L");
+        if (n <= H)
+            return fail(FSN_EINVAL, "%s = %lld: a clip needs more than n_fft / 2 = %d samples (torch.stft's reflect padding)", nm, n, H);
+        if (n > L) return fail(FSN_EINVAL, "%s = %lld exceeds the row length L = %lld", nm, n, (long long)L);
+        if (n / H + 1 + c.look_ahead < kmax)
+            return fail(FSN_EINVAL, "%s = %lld samples give %lld frames: frames + look_ahead = %lld is shorter than the TSSE kernel size %d "
+                                    "(a clip needs at least %lld samples)", nm, n, n / H + 1, n / H + 1 + c.look_ahead, kmax,
+                        (long long)(kmax - c.look_ahead - 1) * H);
+        if (b && n != mx) *all = false;
+        if (n > mx) mx = n;
+    }
+    *Lmax = (int)mx;
+    *T = (int)(mx / H + 1);
+    return check_length(c, 1, *T);
+}
+
+extern "C" int fsn_model_enhance_audio(fsn_model* m, const float* d_wave, int32_t B, int64_t L, const int64_t* h_lengths, float* d_out,
+                                       void* stream) {
+    if (!m) return fail(FSN_EINVAL, "m is null");
+    if (!d_wave) return fail(FSN_EINVAL, "d_wave is null ([B, L] float32 samples on the device)");
+    if (!d_out) return fail(FSN_EINVAL, "d_out is null ([B, L] float32 on the device)");
+    if (!m->finalized) return fail(FSN_ESTATE, "fsn_model_finalize has not been called");
+    const fsn_config& c = m->cfg;
+    int T = 0, Lmax = 0;
+    bool all = true;
+    if (int rc = audio_check(c, B, L, h_lengths, &T, &Lmax, &all)) return rc;
+    if (c.output_size != 2) return fail(FSN_EINVAL, "the audio call needs output_size 2 (a complex mask)");
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    for (auto& ln : m->lane)                                             // batches still in flight in the pipeline share the scratch buffers
+        if (ln.used) CK(cudaStreamWaitEvent(s, ln.ev_lstm, 0));
+    const int N = 2 * (c.num_freqs - 1), H = N / 2;
+    if (!m->au_tab.bytes) {                                              // the tables of this model's n_fft, once
+        std::vector<float> tab;
+        audio_tables(N, tab);
+        if (m->au_tab.ensure(tab.size() * sizeof(float), false)) return fail(FSN_ECUDA, "allocation of the audio tables failed");
+        CK(cudaMemcpy(m->au_tab.p, tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice));
+    }
+    // ragged: every clip's sample count, and its frame count unless every clip has T frames (check_frames)
+    std::vector<int32_t> samples, frames;
+    bool ragged_frames = false;
+    if (!all) {
+        samples.resize(B); frames.resize(B);
+        for (int b = 0; b < B; ++b) {
+            samples[b] = (int32_t)h_lengths[b];
+            frames[b] = samples[b] / H + 1;
+            ragged_frames = ragged_frames || frames[b] != T;
+        }
+    }
+    m->plan = plan_forward(c, runs_layerwise(c, m->env_impl), B, T, m->ws_cap_bytes, m->env_sb_window, m->env_sb_chunk, true);
+    const int Bs = m->plan.Bs;
+    int64_t launches = 0;
+    for (int b0 = 0; b0 < B; b0 += Bs) {
+        const int nb = (B - b0 < Bs) ? B - b0 : Bs;
+        const AudioIO io{d_wave + b0 * L, d_out + b0 * L, L, Lmax, all ? nullptr : samples.data() + b0};
+        if (int rc = forward_impl(m, m->lane[0], nullptr, nullptr, nullptr, nb, T, ragged_frames ? frames.data() + b0 : nullptr, nullptr,
+                                  nullptr, s, s, m->plan.Tw, m->plan.Fc, &io))
+            return rc;
+        launches += m->launches;
+    }
+    m->launches = launches;
+    m->au_valid = Bs >= B;
+    if (!m->ev_plain) CK(cudaEventCreateWithFlags(&m->ev_plain, cudaEventDisableTiming));
+    CK(cudaEventRecord(m->ev_plain, s));
+    m->plain_pending = true;
+    return FSN_OK;
+}
+
 // Test hook: the sub-band stage alone on a given input, through the forward's own run_sb_lstm (its GEMM dispatch, per-layer state,
 // windows and epilogues); only the packer differs (SbPackLaunch::raw: the input as given instead of the normalised unfold)
 extern "C" int fsn_model_sb_forward(fsn_model* m, const float* d_x, int32_t B, int32_t T, int32_t Tw, const int32_t* h_frames,
@@ -1673,6 +1804,14 @@ extern "C" int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst,
         CK(cudaGetLastError());
         return FSN_OK;
     }
+    if (n == "stft" || n == "enh") {
+        if (!m->au_valid)
+            return fail(FSN_ESTATE, "%s is kept only by an audio call (fsn_model_enhance_audio) that ran as one sub-batch, and the last forward was not one", name);
+        const int64_t cnt = (int64_t)(n == "stft" ? 3 : 2) * B * F * ln.geo.T;
+        if (numel != cnt) return fail(FSN_EINVAL, "%s needs %lld elements", name, (long long)cnt);
+        CK(cudaMemcpyAsync(d_dst, n == "stft" ? m->au_planes.p : m->au_enh.p, (size_t)cnt * 4, cudaMemcpyDeviceToDevice, s));
+        return FSN_OK;
+    }
     if (n == "sb_mu") {
         if (numel != B) return fail(FSN_EINVAL, "sb_mu needs %d elements", B);
         CK(cudaMemcpyAsync(d_dst, ln.mu.p, (size_t)B * 4, cudaMemcpyDeviceToDevice, s));
@@ -1805,15 +1944,6 @@ static int streams_ok(const fsn_config& c) {
         return fail(FSN_EINVAL, "model_kind %d: streaming needs fullsubnet.Model (FullSubNet+ is not causal: TSSE pools over all time)", c.model_kind);
     if (c.norm_type != FSN_NORM_CUMULATIVE_LAPLACE && c.norm_type != FSN_NORM_CUMULATIVE_LAYER)
         return fail(FSN_EINVAL, "norm_type %d: streaming needs a cumulative norm_type", c.norm_type);
-    return FSN_OK;
-}
-
-// The audio call's geometry: n_fft = 2 (num_freqs - 1) a power of two from 64 to 1024
-static int audio_fft_ok(const fsn_config& c) {
-    const int N = 2 * (c.num_freqs - 1);
-    if (N < 64 || N > 1024 || (N & (N - 1)))
-        return fail(FSN_EINVAL, "num_freqs %d: the audio call needs n_fft = 2 (num_freqs - 1) to be a power of two from 64 to 1024 "
-                                "(num_freqs 33, 65, 129, 257 or 513)", c.num_freqs);
     return FSN_OK;
 }
 
@@ -1987,11 +2117,7 @@ static int audio_alloc(fsn_stream* st, cudaStream_t s) {
     int e = state_alloc(st, ST_AUDIO, s);
     e |= st->a_mag.ensure(B * F * sizeof(float), true, s);
     e |= st->a_mask.ensure(B * 2 * F * sizeof(float), true, s);
-    std::vector<float> w, tw, inv;
-    stream_audio_tables((int)(2 * (F - 1)), w, tw, inv);
-    st->a_tables = w;
-    st->a_tables.insert(st->a_tables.end(), tw.begin(), tw.end());
-    st->a_tables.insert(st->a_tables.end(), inv.begin(), inv.end());
+    audio_tables((int)(2 * (F - 1)), st->a_tables);
     e |= st->a_tab.ensure(st->a_tables.size() * sizeof(float), false, s);
     if (e) return fail(FSN_ECUDA, "audio stream state allocation failed");
     CK(cudaMemcpyAsync(st->a_tab.p, st->a_tables.data(), st->a_tables.size() * sizeof(float), cudaMemcpyHostToDevice, s));
@@ -2061,8 +2187,8 @@ extern "C" int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_sample
     a.samples = d_samples; a.out = d_out;
     a.hist = static_cast<float*>(st->a_hist.p); a.spec = static_cast<float2*>(st->a_spec.p); a.tail = static_cast<float*>(st->a_tail.p);
     a.mag = static_cast<float*>(st->a_mag.p); a.mask = mask;
-    const float* tab = static_cast<const float*>(st->a_tab.p);
-    a.window = tab; a.twiddle = reinterpret_cast<const float2*>(tab + N); a.inv_env = tab + N + 2 * (N / 2 + 1);
+    const AudioTables tab = audio_table_ptrs(static_cast<const float*>(st->a_tab.p), N);
+    a.window = tab.window; a.twiddle = tab.twiddle; a.inv_env = tab.inv_env;
     a.B = B; a.n_fft = N; a.la = la;
     launch_stream_stft(a, s);
     const int rc = stream_tick(st, a.mag, mask, d, d + 4 * B, nzero, s);
@@ -2342,6 +2468,18 @@ extern "C" int fsn_plan_forward_bins(const fsn_config* cfg, int32_t B, int32_t T
     if (cfg->num_freqs < 4 || cfg->num_layers < 1 || cfg->num_layers > 4 || cfg->look_ahead < 0) return fail(FSN_EINVAL, "bad configuration");
     if (int rc = check_length(*cfg, 1, T)) return rc;
     return put_plan(plan_forward(*cfg, runs_layerwise(*cfg, 0), B, T, cap_bytes, force_window, force_bins), Bs, Tw, Fc, bytes);
+}
+
+extern "C" int fsn_plan_audio(const fsn_config* cfg, int32_t B, int64_t L, const int64_t* h_lengths, double cap_bytes, int32_t force_window,
+                              int32_t force_bins, int32_t* Bs, int32_t* Tw, int32_t* Fc, int64_t* bytes) {
+    if (!cfg || !Bs || !Tw || !Fc || !(cap_bytes > 0)) return fail(FSN_EINVAL, "bad argument");
+    if (force_window < 0 || force_window % 32) return fail(FSN_EINVAL, "force_window must be 0 or a positive multiple of 32");
+    if (force_bins < 0) return fail(FSN_EINVAL, "force_bins must be 0 or a positive number of bins");
+    if (cfg->num_layers < 1 || cfg->num_layers > 4 || cfg->look_ahead < 0) return fail(FSN_EINVAL, "bad configuration");
+    int T = 0, Lmax = 0;
+    bool all = true;
+    if (int rc = audio_check(*cfg, B, L, h_lengths, &T, &Lmax, &all)) return rc;
+    return put_plan(plan_forward(*cfg, runs_layerwise(*cfg, 0), B, T, cap_bytes, force_window, force_bins, true), Bs, Tw, Fc, bytes);
 }
 
 extern "C" int fsn_plan_forward(const fsn_config* cfg, int32_t B, int32_t T, double cap_bytes, int32_t force_window, int32_t* Bs, int32_t* Tw,

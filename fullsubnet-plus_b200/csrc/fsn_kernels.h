@@ -155,7 +155,30 @@ struct StreamAudioLaunch {
 };
 void launch_stream_stft(const StreamAudioLaunch& a, cudaStream_t s);
 void launch_stream_istft(const StreamAudioLaunch& a, cudaStream_t s);
-void stream_audio_tables(int n_fft, std::vector<float>& window, std::vector<float>& twiddle, std::vector<float>& inv_env);
+
+// ---- k_audio.cu: audio in and out of the offline forward (fsn_model_enhance_audio), and the tables of both audio paths -------
+struct AudioLaunch {
+    const float* wave;        // [B, L] input rows (analysis; samples past a clip's length are never read)
+    float* out;               // [B, L] output rows (synthesis; samples past a clip's length are written as zero)
+    long long L;              // row stride of wave and out
+    const int* len;           // [B] samples per clip (device), or null: every clip is Lall samples
+    int Lall;
+    int B, T, n_fft;          // T: frames of the planes (the batch's longest clip); n_fft: power of two, 64 .. 1024
+    float* planes;            // [3][B][F][T] mag, real, imag: analysis output, the forward's input
+    const float2* enh;        // [B, F, T] enhanced spectrum: synthesis input, the forward's output
+    const float* window; const float2* twiddle; const float* inv_env; const float* inv_last;   // audio_tables
+};
+void launch_audio_stft(const AudioLaunch& a, cudaStream_t s);
+void launch_audio_istft(const AudioLaunch& a, cudaStream_t s);
+// Tables of one n_fft, computed in double, in one array: periodic Hann window w [n_fft] | twiddles exp(-2 pi i k / n_fft) for
+// k = 0 .. hop (hop + 1 float2) | 1 / (w^2(i) + w^2(i + hop)) for i < hop | 1 / w^2(i + hop) for i < hop (the last L mod hop samples of a
+// clip, which one frame covers)
+void audio_tables(int n_fft, std::vector<float>& tab);
+struct AudioTables { const float* window; const float2* twiddle; const float* inv_env; const float* inv_last; };
+inline AudioTables audio_table_ptrs(const float* tab, int n_fft) {
+    const int H = n_fft / 2;
+    return {tab, reinterpret_cast<const float2*>(tab + n_fft), tab + n_fft + 2 * (H + 1), tab + n_fft + 2 * (H + 1) + H};
+}
 
 // ---- k_lstm_mma.cu ---------------------------------------------------------------------------
 struct LstmMmaWeights {       // device, produced by pack (fsn_api.cu)

@@ -2,39 +2,16 @@
 // turns one hop of samples into one frame of torch.stft(center=True, reflect, periodic Hann), and the synthesis kernel turns the mask
 // the model step produced into one hop of torch.istft output (decompress_cIRM x noisy spectrum, inverse real FFT, window, overlap-add,
 // division by the window envelope).  One CTA per slot; the real FFTs of n_fft points run as complex FFTs of n_fft / 2 points
-// (radix 2, fp32, in shared memory) with the even / odd split folded in.  The tables (window, twiddles, 1 / envelope) are computed in
-// double on the host once per handle.
-#include <cmath>
-
+// (radix 2, fp32, in shared memory, fsn_fft.cuh) with the even / odd split folded in.  The tables (window, twiddles, 1 / envelope) are
+// computed in double on the host once per handle (audio_tables).
 #include "fsn_common.cuh"
+#include "fsn_fft.cuh"
 #include "fsn_kernels.h"
 
 namespace fsn {
 
 constexpr int AUDIO_THREADS = 128;
 constexpr int AUDIO_MAX_HOP = 512;                              // n_fft <= 1024
-
-__device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
-__device__ __forceinline__ float2 cmul_conj(float2 a, float2 b) { return make_float2(a.x * b.x + a.y * b.y, a.y * b.x - a.x * b.y); }   // a conj(b)
-
-// In-place radix-2 decimation-in-time FFT of H points (input in bit-reversed order, output in natural order).  tw[k] = exp(-2 pi i k / N),
-// N = 2 H; INV: exp(+...), unscaled.
-template <bool INV>
-__device__ __forceinline__ void fft_dit(float2* z, const float2* __restrict__ tw, int H) {
-    for (int h = 1; h < H; h <<= 1) {
-        const int step = H / h;                                  // W_{2h}^p = W_N^{p N / (2h)} = tw[p * H / h]
-        for (int t = threadIdx.x; t < H / 2; t += blockDim.x) {
-            const int p = t & (h - 1), i0 = ((t - p) << 1) + p, i1 = i0 + h;
-            const float2 w = __ldg(tw + p * step);
-            const float2 u = z[i0], v = INV ? cmul_conj(z[i1], w) : cmul(z[i1], w);
-            z[i0] = make_float2(u.x + v.x, u.y + v.y);
-            z[i1] = make_float2(u.x - v.x, u.y - v.y);
-        }
-        __syncthreads();
-    }
-}
-
-__device__ __forceinline__ int bitrev(int n, int lg) { return (int)(__brev((unsigned)n) >> (32 - lg)); }
 
 // grid B: analysis of one tick.  STORE: the slot's hop goes to its history ring (hop q at q % 3).  FRAME: frame j = tick - 1 of the
 // session, original samples [hop (j - 1), hop (j + 1)) reflected at 0 and, once the session's length is known, at L - 1; its spectrum
@@ -73,13 +50,8 @@ __global__ void __launch_bounds__(AUDIO_THREADS) stream_stft_kernel(StreamAudioL
     }
     __syncthreads();
     fft_dit<false>(z, a.twiddle, H);
-    // X[f] = Xe[f] + W_N^f Xo[f], Xe = (Z[f] + conj Z[H - f]) / 2, Xo = (Z[f] - conj Z[H - f]) / 2i  (indices mod H)
     for (int f = threadIdx.x; f < F; f += blockDim.x) {
-        const float2 p = z[f & (H - 1)], q = z[(H - f) & (H - 1)];
-        const float2 xe = make_float2(0.5f * (p.x + q.x), 0.5f * (p.y - q.y));
-        const float2 xo = make_float2(0.5f * (p.y + q.y), -0.5f * (p.x - q.x));
-        const float2 t = cmul(__ldg(a.twiddle + f), xo);
-        const float2 X = make_float2(xe.x + t.x, xe.y + t.y);
+        const float2 X = rfft_split(z[f & (H - 1)], z[(H - f) & (H - 1)], __ldg(a.twiddle + f));
         spec[f] = X;
         mag[f] = hypotf(X.x, X.y);
     }
@@ -109,14 +81,7 @@ __global__ void __launch_bounds__(AUDIO_THREADS) stream_istft_kernel(StreamAudio
         e[f] = E;
     }
     __syncthreads();
-    // Z[k] = Xe[k] + i Xo[k], Xe = (E[k] + conj E[H - k]) / 2, Xo = (E[k] - conj E[H - k]) conj(W_N^k) / 2; z = IFFT_H(Z) / H
-    // interleaves the inverse real transform: y[2n] = Re z[n], y[2n + 1] = Im z[n]
-    for (int k = threadIdx.x; k < H; k += blockDim.x) {
-        const float2 p = e[k], q = e[H - k];
-        const float2 xe = make_float2(0.5f * (p.x + q.x), 0.5f * (p.y - q.y));
-        const float2 xo = cmul_conj(make_float2(0.5f * (p.x - q.x), 0.5f * (p.y + q.y)), __ldg(a.twiddle + k));
-        z[bitrev(k, lg)] = make_float2(xe.x - xo.y, xe.y + xo.x);
-    }
+    for (int k = threadIdx.x; k < H; k += blockDim.x) z[bitrev(k, lg)] = irfft_split(e[k], e[H - k], __ldg(a.twiddle + k));
     __syncthreads();
     fft_dit<true>(z, a.twiddle, H);
     const float* y = reinterpret_cast<const float*>(z);
@@ -133,22 +98,5 @@ __global__ void __launch_bounds__(AUDIO_THREADS) stream_istft_kernel(StreamAudio
 
 void launch_stream_stft(const StreamAudioLaunch& a, cudaStream_t s) { stream_stft_kernel<<<a.B, AUDIO_THREADS, 0, s>>>(a); }
 void launch_stream_istft(const StreamAudioLaunch& a, cudaStream_t s) { stream_istft_kernel<<<a.B, AUDIO_THREADS, 0, s>>>(a); }
-
-// Tables of one n_fft, computed in double: periodic Hann window [n_fft], twiddles exp(-2 pi i k / n_fft) for k = 0 .. n_fft / 2
-// (n_fft / 2 + 1 of them), 1 / (w^2(i) + w^2(i + hop)) for i < hop.
-void stream_audio_tables(int n_fft, std::vector<float>& window, std::vector<float>& twiddle, std::vector<float>& inv_env) {
-    const int H = n_fft / 2;
-    const double PI = 3.14159265358979323846;
-    std::vector<double> w(n_fft);
-    for (int i = 0; i < n_fft; ++i) w[i] = 0.5 - 0.5 * cos(2.0 * PI * i / n_fft);
-    window.assign(w.begin(), w.end());
-    twiddle.resize(2 * (H + 1));
-    for (int k = 0; k <= H; ++k) {
-        twiddle[2 * k] = (float)cos(2.0 * PI * k / n_fft);
-        twiddle[2 * k + 1] = (float)-sin(2.0 * PI * k / n_fft);
-    }
-    inv_env.resize(H);
-    for (int i = 0; i < H; ++i) inv_env[i] = (float)(1.0 / (w[i] * w[i] + w[i + H] * w[i + H]));
-}
 
 }  // namespace fsn

@@ -24,6 +24,7 @@ SYMBOLS = [
     "fsn_tc5r_gin_weights", "fsn_tc5r_ring_stages", "fsn_lstm_mma_rows", "fsn_model_sb_forward",
     "fsn_stream_step_slots", "fsn_stream_step_audio_slots",
     "fsn_stream_state_bytes", "fsn_stream_state_layout", "fsn_model_weights_id", "fsn_stream_save_slots", "fsn_stream_load_slots",
+    "fsn_model_enhance_audio", "fsn_plan_audio",
 ]
 
 
@@ -146,6 +147,9 @@ def load_library():
     lib.fsn_lstm_mma_rows.argtypes = [i32, i32, i32, i32]
     lib.fsn_lstm_mma_rows.restype = i32
     lib.fsn_model_sb_forward.argtypes = [vp, vp, i32, i32, i32, C.POINTER(i32), vp, vp, vp, vp, vp]
+    lib.fsn_model_enhance_audio.argtypes = [vp, vp, i32, i64, C.POINTER(i64), vp, vp]
+    lib.fsn_plan_audio.argtypes = [C.POINTER(FsnConfig), i32, i64, C.POINTER(i64), C.c_double, i32, i32, C.POINTER(i32), C.POINTER(i32),
+                                   C.POINTER(i32), C.POINTER(i64)]
     _LIB = lib
     return lib
 
@@ -185,4 +189,29 @@ def plan_forward_bins(cfg, B, T, cap_bytes=None, force_window=0, force_bins=0):
     cap = ws_cap_bytes() if cap_bytes is None else float(cap_bytes)
     check(lib.fsn_plan_forward_bins(C.byref(cfg), int(B), int(T), cap, int(force_window), int(force_bins), C.byref(bs), C.byref(tw),
                                     C.byref(fc), C.byref(nb)))
+    return bs.value, tw.value, fc.value, nb.value
+
+
+def lengths_arg(lengths, B):
+    """``lengths`` (None, a sequence of ints or a 1-D CPU integer tensor of length B) as a C int64 array, or None."""
+    if lengths is None:
+        return None
+    if hasattr(lengths, "is_cuda"):
+        if lengths.is_cuda or lengths.is_floating_point() or lengths.is_complex() or lengths.dim() != 1:
+            raise ValueError("lengths must be a 1-D CPU integer tensor or a sequence of ints")
+        lengths = lengths.tolist()
+    lengths = [int(n) for n in lengths]
+    if len(lengths) != B:
+        raise ValueError(f"lengths has {len(lengths)} entries for a batch of {B}")
+    return (C.c_int64 * B)(*lengths)
+
+
+def plan_audio(cfg, B, L, lengths=None, cap_bytes=None, force_window=0, force_bins=0):
+    """fsn_plan_audio: the (Bs, Tw, Fc, bytes) plan of the audio call (fsn_model_enhance_audio) for B clips in rows of L samples, each
+    ``lengths[b]`` long (None: L), after the call's own checks (FsnError with its message).  Needs no GPU."""
+    lib = load_library()
+    bs, tw, fc, nb = C.c_int32(), C.c_int32(), C.c_int32(), C.c_int64()
+    cap = ws_cap_bytes() if cap_bytes is None else float(cap_bytes)
+    check(lib.fsn_plan_audio(C.byref(cfg), int(B), int(L), lengths_arg(lengths, B), cap, int(force_window), int(force_bins),
+                             C.byref(bs), C.byref(tw), C.byref(fc), C.byref(nb)))
     return bs.value, tw.value, fc.value, nb.value

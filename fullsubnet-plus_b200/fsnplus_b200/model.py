@@ -193,6 +193,30 @@ class _B200Model(nn.Module):
         ``pipelined=True``: like ``submit()`` -- valid after ``wait()`` / ``wait_lane()``.  ``frames``: as in ``forward()``."""
         return self._run(noisy_mag, noisy_real, noisy_imag, enhance=True, pipelined=pipelined, out=out, hold=hold, frames=frames)
 
+    def enhance_audio(self, wave, lengths=None):
+        """Waveforms in, enhanced waveforms out in ONE call (C ABI: fsn_model_enhance_audio): torch.stft -> model -> decompress_cIRM x
+        spectrum -> torch.istft(length = L_b) per clip, with both transforms on the device (what ``inference.enhance_batch`` /
+        ``enhance_ragged`` compute).  ``wave``: [B, L] float32 CUDA; ``lengths``: None (every clip is L samples) or B sample counts (a
+        sequence or a 1-D CPU integer tensor), clip b being the first lengths[b] samples of its row.  Returns [B, L], zero past each
+        clip's length.  n_fft = 2 (num_freqs - 1), hop = n_fft / 2, periodic Hann window."""
+        if wave.dim() != 2:
+            raise ValueError(f"enhance_audio: wave must be [B, L], got {tuple(wave.shape)}")
+        if self.training:
+            raise NotImplementedError("fsnplus_b200 implements the inference (eval) forward only; call .eval()")
+        if not wave.is_cuda:
+            raise RuntimeError("fsnplus_b200 has no CPU fallback: move the model and its inputs to a CUDA (H100) device")
+        if self._kind == _lib.KIND_PLUS and not self._subband_runs:
+            raise RuntimeError(f"subband_num={self.subband_num}: only channel_attention_model='ECA' runs with subband_num > 1")
+        B, L = wave.shape
+        hl = _lib.lengths_arg(lengths, B)
+        x = wave.detach().to(dtype=torch.float32).contiguous()
+        with torch.cuda.device(x.device):
+            lib = self._ensure_handle(x.device)
+            out = torch.empty((B, L), dtype=torch.float32, device=x.device)
+            stream = C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
+            _lib.check(lib.fsn_model_enhance_audio(self._handle, C.c_void_p(x.data_ptr()), B, L, hl, C.c_void_p(out.data_ptr()), stream))
+        return out
+
     @staticmethod
     def _frames_arg(frames, B):
         """``frames`` (a sequence of ints or a CPU integer tensor of length B) as a C int32 array."""

@@ -135,6 +135,29 @@ int fsn_model_forward_ragged(fsn_model* m, const float* d_mag, const float* d_re
                              const int32_t* h_frames, float* d_out, void* stream);
 int fsn_model_forward_enhance_ragged(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
                                      const int32_t* h_frames, float* d_enh, void* stream);
+/* Waveforms in, waveforms out (DESIGN.md §3.12): the inferencer's whole method -- STFT, model, decompress_cIRM x noisy spectrum,
+ * iSTFT -- for a batch of clips, with both transforms on the device (no FFT library, no torch).  Clip b's output is
+ *   torch.istft(decompress_cIRM(model(|X|, Re X, Im X)) * X, n_fft, hop, n_fft, hann, length = L_b)
+ *   X = torch.stft(x_b, n_fft, hop, n_fft, window = torch.hann_window(n_fft) (periodic), center = True, pad_mode = "reflect")
+ * of that clip alone, T_b = L_b / hop + 1 frames (fullsubnet.Model: model(|X|)), up to fp32 rounding.  Every clip is reflected at its
+ * own end and synthesised over its own frames only; the window envelope of its last L_b mod hop samples is the one frame that covers
+ * them, as in torch.istft.
+ * Geometry from the model: n_fft = 2 (num_freqs - 1), a power of two from 64 to 1024; hop = n_fft / 2; win_length = n_fft.
+ * d_wave, d_out: [B, L] float32 device.  Clip b is the first h_lengths[b] samples of its row (h_lengths: HOST array of B counts, free
+ * when the call returns; NULL: every clip is L samples).  Samples past a clip's length are never read (NaN there does not matter);
+ * its output samples there are exact zeros.
+ * FSN_EINVAL, naming the clip: h_lengths[b] <= n_fft / 2 (the reflect padding needs more), h_lengths[b] > L, or too few frames for the
+ * TSSE kernels (the clip needs (max kersize - look_ahead - 1) hop samples).  FSN_EINVAL for another num_freqs (naming it), null
+ * pointers, B < 1, L outside 1 .. 2^31 - 1, and the length limits below on T = max_b L_b / hop + 1.
+ * The call is a plain forward: it plans sub-batches, sub-band time windows and bin chunks under FSN_WS_CAP_GB (fsn_plan_audio) with
+ * its own workspace counted (20 bytes per bin and frame of each clip: the mag / real / imag planes and the enhanced spectrum).  Per
+ * sub-batch: one analysis launch, the forward (unmasked when every clip has the longest clip's length, as fsn_model_forward_ragged),
+ * one synthesis launch.  The call does not synchronise the stream. */
+int fsn_model_enhance_audio(fsn_model* m, const float* d_wave, int32_t B, int64_t L, const int64_t* h_lengths, float* d_out, void* stream);
+/* The plan of fsn_model_enhance_audio for these clips (fsn_plan_forward_bins with the audio workspace counted), after the same checks
+ * of the configuration and lengths, with the same FSN_EINVAL messages.  Host only, no GPU. */
+int fsn_plan_audio(const fsn_config* cfg, int32_t B, int64_t L, const int64_t* h_lengths, double cap_bytes, int32_t force_window,
+                   int32_t force_bins, int32_t* Bs, int32_t* Tw, int32_t* Fc, int64_t* bytes);
 /* Same call with HOST buffers (pinned or pageable): H2D copies, the forward and the D2H copy of the
  * mask are all enqueued on `stream` and the call returns after the result is in h_out. */
 int fsn_model_forward_host(fsn_model* m, const float* h_mag, const float* h_real, const float* h_imag, int32_t B, int32_t T,
@@ -273,7 +296,10 @@ int fsn_apply_cirm(const float* d_crm, const float* d_noisy, float* d_enh, int32
  *   "fb_in"  [nbranch, B, F, T+look_ahead]  post-norm (and post-attention) full-band inputs
  *   "fb_out" [nbranch, B, F, T+look_ahead]  full-band model outputs
  *   "sb_mu"  [B]                            utterance mean of the (un-normalised) sub-band input
- *   "sb_in"  [B, F, Isb, T+look_ahead]       normalised sub-band input (sub-band TCN only) */
+ *   "sb_in"  [B, F, Isb, T+look_ahead]       normalised sub-band input (sub-band TCN only)
+ *   "stft"   [3, B, 1, F, T]                 the mag / real / imag planes the audio call's forward read
+ *   "enh"    [B, F, T] complex64 (2 floats)  the enhanced spectrum the audio call synthesised
+ * "stft" and "enh" are kept only when the last forward was an audio call that ran as one sub-batch; FSN_ESTATE otherwise. */
 int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst, int64_t numel, void* stream);
 /* Kernels launched by the last forward (bench.py reports it as gpu_launches). */
 int64_t fsn_model_last_launch_count(const fsn_model* m);

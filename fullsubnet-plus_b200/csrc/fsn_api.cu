@@ -1849,6 +1849,12 @@ struct fsn_stream {
     DevBuf a_hist, a_spec, a_tail, a_mag, a_mask, a_tab;
     // save / load (fsn_stream_save_slots, fsn_stream_load_slots): the slot list of the last call on the device
     DevBuf x_slot;
+    // chunk call (fsn_stream_step_chunk, DESIGN.md §3.13): its scratch, allocated at its first use, grow-only, apart from the model's
+    // workspace (the model may forward offline on another stream meanwhile).  Full band over all B slots: the normalised input
+    // [B, F, P], its fp16 form [K, rows_pad, Ipad], the top layer's h [B, H, P], the output [B, F, P]; sub band: the images, and on the
+    // layer-wise path the Gin / layer output, the per-layer h / c carry and the compact masks of one sub-batch; c_slot: the slot's
+    // counts, the START list, each slot's active-session index and the active slots
+    DevBuf c_fbin, c_fbx, c_hseq, c_fbout, c_ximg, c_gin, c_hsb, c_h, c_c, c_mask, c_slot;
 };
 
 // The state of a session: one entry per buffer, in payload order (DESIGN.md §3.11).  The handle's allocation (fsn_stream_create,
@@ -1980,7 +1986,8 @@ extern "C" void fsn_stream_destroy(fsn_stream* st) {
         if (e.ws) (st->*e.ws).release();
     }
     DevBuf* scratch[] = {&st->fbin, &st->fbx, &st->hseq, &st->fbout, &st->ximg, &st->ws_bar, &st->a_mag, &st->a_mask, &st->a_tab,
-                         &st->d_slot, &st->x_slot};
+                         &st->d_slot, &st->x_slot, &st->c_fbin, &st->c_fbx, &st->c_hseq, &st->c_fbout, &st->c_ximg, &st->c_gin,
+                         &st->c_hsb, &st->c_h, &st->c_c, &st->c_mask, &st->c_slot};
     for (auto* b : scratch) b->release();
     delete st;
 }
@@ -2108,6 +2115,244 @@ extern "C" int fsn_stream_step(fsn_stream* st, const float* d_mag, float* d_mask
     const int rc = stream_tick(st, d_mag, d_mask, nullptr, nullptr, 0, static_cast<cudaStream_t>(stream));
     if (rc) return rc;
     if (h_valid) *h_valid = (n >= st->m->cfg.look_ahead) ? 1 : 0;
+    return FSN_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// chunk call: K frames per slot and call (DESIGN.md §3.13)
+// ---------------------------------------------------------------------------------------------
+// The layer-wise sub-band scratch of a chunk call for a sub-batch of bs sessions, K frames, windows of tw frames (tw = K: one window):
+// the images, Gin and the layer output (ws_sizes: the offline forward's windowed buffers), the per-layer h carry (r_hstate's size),
+// the per-layer c carry and the compact masks [bs, 2, F, K]
+static size_t chunk_sb_bytes(const fsn_config& c, int bs, int K, int tw) {
+    const WsSizes z = ws_sizes(c, true, bs, K, tw);
+    const int ntiles = (int)(((size_t)bs * c.num_freqs + 127) / 128);
+    return z.ximg + z.r_gin + z.r_hseq + z.r_hstate + (size_t)c.num_layers * lstm_tc5r_cstate_bytes(ntiles, c.sb_hidden) +
+           (size_t)bs * 2 * c.num_freqs * K * sizeof(float);
+}
+
+// Length limits of a chunk: the layer-wise recurrence runs K + 4 steps (t0 = 4, see fsn_stream_step_chunk), within a forward's frame
+// limit; a session's K frames of one bin plane are indexed with an int
+static int chunk_check(const fsn_config& c, int K) {
+    if (K < 1) return fail(FSN_EINVAL, "K = %d: a chunk has at least 1 frame", K);
+    if ((long long)K + 4 > FSN_MAX_TP)
+        return fail(FSN_EINVAL, "K = %d exceeds the chunk limit of %lld frames (65535 x 256 - 4, the frame limit of a forward)", K, FSN_MAX_TP - 4);
+    if ((long long)c.num_freqs * K > 0x7fffffffLL)
+        return fail(FSN_EINVAL, "num_freqs x K = %lld exceeds 2^31 - 1, the per-session plane index limit", (long long)c.num_freqs * K);
+    return FSN_OK;
+}
+
+// The plan of a chunk call with n stepping sessions: on the layer-wise path the sessions run in equal sub-batches of Bs so that
+// chunk_sb_bytes stays within cap (the largest that fits, evened out); if even one session's K frames do not fit, one session at a
+// time in windows of Tw frames (a multiple of 4, the longest that fits, evened out; 4 if none does).  Tw = 0: one window.  The generic
+// path runs in place over the handle's slots in one piece (bytes: its images).
+static int chunk_plan(const fsn_config& c, bool layerwise, int n, int K, double cap, Plan* p) {
+    if (int rc = streams_ok(c)) return rc;
+    if (n < 1) return fail(FSN_EINVAL, "n_active = %d: a plan needs at least 1 stepping session", n);
+    if (int rc = chunk_check(c, K)) return rc;
+    *p = Plan{n};
+    if (!layerwise) {
+        p->bytes = (int64_t)(((size_t)n * c.num_freqs + 127) / 128) * K * 16384;
+        return FSN_OK;
+    }
+    auto fits = [&](int bs, int tw) { return (double)chunk_sb_bytes(c, bs, K, tw) <= cap; };
+    if (!fits(n, K)) {
+        if (const int b = largest(0, n, [&](int v) { return fits(v, K); })) {
+            const int nsub = (n + b - 1) / b;
+            p->Bs = (n + nsub - 1) / nsub;
+        } else {
+            p->Bs = 1;
+            const int u = largest(1, K / 4, [&](int v) { return fits(1, 4 * v); });
+            const int nwin = (K + 4 * u - 1) / (4 * u);
+            p->Tw = ((K + nwin - 1) / nwin + 3) / 4 * 4;
+            if (p->Tw >= K) p->Tw = 0;
+        }
+    }
+    p->bytes = (int64_t)chunk_sb_bytes(c, p->Bs, K, p->Tw ? p->Tw : K);
+    return FSN_OK;
+}
+
+extern "C" int fsn_stream_chunk_plan(const fsn_config* cfg, int32_t n_active, int32_t K, double cap_bytes, int32_t* Bs, int32_t* Tw,
+                                     int64_t* bytes) {
+    if (!cfg) return fail(FSN_EINVAL, "cfg is null");
+    if (!(cap_bytes > 0)) return fail(FSN_EINVAL, "cap_bytes = %g: the cap must be > 0", cap_bytes);
+    Plan p;
+    if (int rc = chunk_plan(*cfg, runs_layerwise(*cfg, 0), n_active, K, cap_bytes, &p)) return rc;
+    if (Bs) *Bs = p.Bs;
+    if (Tw) *Tw = p.Tw;
+    if (bytes) *bytes = p.bytes;
+    return FSN_OK;
+}
+
+extern "C" int fsn_stream_step_chunk(fsn_stream* st, const float* d_mag, int32_t K, float* d_mask, const int32_t* h_flags,
+                                     int32_t* h_valid, void* stream) {
+    if (!st) return fail(FSN_EINVAL, "st is null");
+    if (!d_mag) return fail(FSN_EINVAL, "d_mag is null (K magnitude frames per slot, [B, F, K] float32 on the device)");
+    if (!d_mask) return fail(FSN_EINVAL, "d_mask is null (K mask columns per slot, [B, 2, F, K] float32 on the device)");
+    if (!h_flags) return fail(FSN_EINVAL, "h_flags is null (one flag per slot, slots 0..%d)", st->B - 1);
+    if (!h_valid) return fail(FSN_EINVAL, "h_valid is null (one result per slot, slots 0..%d)", st->B - 1);
+    fsn_model* m = st->m;
+    const fsn_config& c = m->cfg;
+    const int B = st->B, F = c.num_freqs, la = c.look_ahead, H = c.sb_hidden, L = c.num_layers;
+    if (int rc = chunk_check(c, K)) return rc;
+    int nact = 0;
+    bool reset = false;
+    for (int b = 0; b < B; ++b) {
+        const int f = h_flags[b];
+        if (f != FSN_SLOT_HOLD && f != FSN_SLOT_STEP && f != FSN_SLOT_START)
+            return fail(FSN_EINVAL, "slot %d: flag %d is not FSN_SLOT_HOLD (0), FSN_SLOT_STEP (1) or FSN_SLOT_START (2)", b, f);
+        nact += f != FSN_SLOT_HOLD;
+        reset = reset || f == FSN_SLOT_START;
+    }
+    if (st->mode == FSN_STATE_MODE_AUDIO) return claim_mode(st, FSN_STATE_MODE_MASK);
+    const bool lw = runs_layerwise(c, m->env_impl);
+    Plan p{nact};
+    if (lw && nact)
+        if (int rc = chunk_plan(c, true, nact, K, m->ws_cap_bytes, &p)) return rc;
+    // the scratch, before any state changes (DevBuf::ensure only grows)
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const int Pk = (K + 3) & ~3, ntiles = (B * F + 127) / 128;
+    int e = st->c_fbin.ensure((size_t)B * F * Pk * 4, false, s);
+    e |= st->c_fbout.ensure((size_t)B * F * Pk * 4, false, s);
+    e |= st->c_fbx.ensure((size_t)K * st->rows_pad * st->Ipad * 2, false, s);
+    e |= st->c_hseq.ensure((size_t)B * c.fb_hidden * Pk * 4, false, s);
+    e |= st->c_slot.ensure((size_t)4 * B * sizeof(int32_t), false, s);
+    if (!lw) {
+        e |= st->c_ximg.ensure((size_t)ntiles * K * 16384, true, s);
+    } else if (nact) {
+        const int tw = p.Tw ? p.Tw : K, nt = (p.Bs * F + 127) / 128;
+        const WsSizes z = ws_sizes(c, true, p.Bs, K, tw);
+        e |= st->c_ximg.ensure(z.ximg, true, s);
+        e |= st->c_gin.ensure(z.r_gin, false, s);
+        e |= st->c_hsb.ensure(z.r_hseq, false, s);
+        e |= st->c_h.ensure(z.r_hstate, true, s);
+        e |= st->c_c.ensure((size_t)L * lstm_tc5r_cstate_bytes(nt, H), true, s);
+        e |= st->c_mask.ensure((size_t)p.Bs * 2 * F * K * sizeof(float), false, s);
+    }
+    if (e) return fail(FSN_ECUDA, "chunk scratch allocation failed (B = %d, K = %d)", B, K);
+    if (int rc = claim_mode(st, FSN_STATE_MODE_MASK)) return rc;
+    use_slot_counts(st);
+    // staged per-slot values: counts [B] (-1 = held), active-session index [B] (-1 = held), the active slots [nact], the START list
+    int32_t* h = nullptr;
+    if (int rc = st->stage.take((size_t)4 * B, &h)) return rc;
+    int32_t *cnt = h, *idx = h + B, *sess = h + 2 * B, *zero = sess + nact;
+    int nzero = 0;
+    for (int b = 0, j = 0; b < B; ++b) {
+        cnt[b] = h_flags[b] == FSN_SLOT_HOLD ? -1 : h_flags[b] == FSN_SLOT_START ? 0 : st->nb[b];
+        idx[b] = cnt[b] >= 0 ? j : -1;
+        if (cnt[b] >= 0) sess[j++] = b;
+        if (reset && cnt[b] == 0) zero[nzero++] = b;                    // started, or never stepped
+    }
+    const int* d = static_cast<const int*>(st->c_slot.p);
+    const int *d_cnt = d, *d_idx = d + B, *d_sess = d + 2 * B, *d_zero = d + 2 * B + nact;
+    if (int rc = st->stage.send(st->c_slot.p, (size_t)2 * B + nact + nzero, s)) return rc;
+    if (nzero) {
+        StreamStateLaunch z{};
+        state_launch(st, NSEG, ST_START, nullptr, z);
+        z.slots = d_zero; z.n = nzero; z.dir = STREAM_STATE_ZERO;
+        if (int e2 = launch_stream_state(z, s)) return fail(FSN_ECUDA, "session state reset failed: %s", cudaGetErrorString((cudaError_t)e2));
+    }
+    // full band: every slot, K frames per launch (held slots keep their state)
+    StreamNormChunkLaunch na{d_mag, static_cast<float*>(st->c_fbin.p), static_cast<double*>(st->cum_in.p), B, F, K, Pk, c.norm_type, d_cnt};
+    launch_stream_norm_chunk(na, s);
+    launch_fb_pack(static_cast<const float*>(st->c_fbin.p), static_cast<__half*>(st->c_fbx.p), B, F, K, Pk, st->rows_pad, st->Ipad, s);
+    if (st->use_ws) {
+        LstmWsLaunch w{};
+        fill_ws(m, w);
+        w.rows = B; w.rows_pad = st->rows_pad; w.Tp = K;
+        w.x = static_cast<const __half*>(st->c_fbx.p); w.hbuf = static_cast<__half*>(st->ws_h.p); w.cbuf = static_cast<float*>(st->ws_c.p);
+        w.barrier = static_cast<unsigned int*>(st->ws_bar.p);
+        w.hseq = static_cast<float*>(st->c_hseq.p); w.P = Pk; w.resume = 1; w.t0 = st->n; w.slot = d_cnt;
+        e = launch_lstm_ws(w, s);
+    } else {
+        LstmMmaLaunch a{};
+        for (int l = 0; l < L; ++l) { a.w.wfrag[l] = static_cast<const uint4*>(m->fb_frag[l].p); a.w.bias[l] = static_cast<const float*>(m->fb_bias[l].p); }
+        a.L = L; a.H = c.fb_hidden; a.I = F; a.Ipad = st->Ipad; a.rows = B; a.Tp = K;
+        a.xplain = static_cast<const __half*>(st->c_fbx.p); a.rows_pad = st->rows_pad;
+        a.cstate = static_cast<float*>(st->c_fb.p); a.rows_alloc = st->ra_fb;
+        a.hseq = static_cast<float*>(st->c_hseq.p); a.P = Pk; a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU;
+        a.hstate = static_cast<__half*>(st->h_fb.p); a.resume = 1; a.slot = d_cnt; a.slot_rows = 1;
+        e = launch_lstm_mma(a, s);
+    }
+    if (e) return fail(FSN_ECUDA, "full-band LSTM chunk failed: %s", cudaGetErrorString((cudaError_t)e));
+    ConvLaunch cf{};
+    cf.X = static_cast<const float*>(st->c_hseq.p); cf.Y = static_cast<float*>(st->c_fbout.p);
+    cf.Z = B; cf.M = F; cf.K = c.fb_hidden; cf.Tp = K; cf.P = Pk; cf.act = c.fb_act;
+    cf.W = P(m, "fb_model.fc_output_layer.weight"); cf.bias = P(m, "fb_model.fc_output_layer.bias");
+    launch_conv1x1(cf, s);
+    StreamPackChunkLaunch pa{d_mag, static_cast<const float*>(st->c_fbout.p), Pk, static_cast<double*>(st->cum_sb.p),
+                             static_cast<__half*>(st->c_ximg.p), B, F, K, c.sb_num_neighbors, c.fb_num_neighbors, c.norm_type, 0, K, d_cnt,
+                             nullptr, 0, 0};
+    if (!lw) {
+        // generic sub band: the per-frame step's kernel and state, in place over every slot, K steps
+        launch_stream_pack_chunk(pa, s);
+        LstmMmaLaunch b{};
+        for (int l = 0; l < L; ++l) { b.w.wfrag[l] = static_cast<const uint4*>(m->sb_frag[l].p); b.w.bias[l] = static_cast<const float*>(m->sb_bias[l].p); }
+        b.w.fc_w = P(m, "sb_model.fc_output_layer.weight"); b.w.fc_b = P(m, "sb_model.fc_output_layer.bias");
+        b.L = L; b.H = H; b.I = m->Isb; b.Ipad = 64; b.rows = B * F; b.Tp = K;
+        b.img = static_cast<const __half*>(st->c_ximg.p); b.ntiles = ntiles;
+        b.cstate = static_cast<float*>(st->c_sb.p); b.rows_alloc = st->ra_sb;
+        b.out = d_mask; b.O = c.output_size; b.F = F; b.la = 0; b.act = c.sb_act; b.fast = c.fast_math; b.gru = c.rnn_type == FSN_RNN_GRU;
+        b.hstate = static_cast<__half*>(st->h_sb.p); b.resume = 1; b.slot = d_cnt; b.slot_rows = F; b.slot_la = la;
+        e = launch_lstm_mma(b, s);
+        if (e) return fail(FSN_ECUDA, "sub-band LSTM chunk failed: %s", cudaGetErrorString((cudaError_t)e));
+    } else if (!nact) {
+        StreamChunkScatterLaunch sc{nullptr, d_mask, d_cnt, d_idx, 0, 0, B, F, K, la, 1};
+        launch_stream_chunk_scatter(sc, s);
+    } else {
+        // layer-wise sub band: the stepping sessions only, compacted to rows j F + f, in sub-batches of p.Bs sessions and windows of
+        // p.Tw frames.  The recurrence runs as window t0 = 4 + w0 of a 4 + K step sequence with la = 4: it loads h / c from the carry
+        // (t0 > 0), its parities are those of a launch from 0 (t0 % 4 == 0), and local frame k is output column k of [bs, 2, F, K]
+        const int tw_max = p.Tw ? p.Tw : K;
+        for (int j0 = 0; j0 < nact; j0 += p.Bs) {
+            const int bs = nact - j0 < p.Bs ? nact - j0 : p.Bs, srows = bs * F, nt = (srows + 127) / 128, ntp = (nt + 1) / 2 * 2;
+            const size_t cs_layer = lstm_tc5r_cstate_bytes(nt, H) / sizeof(float), hs_layer = (size_t)ntp * 128 * H;
+            StreamSbCarryLaunch cy{static_cast<__half*>(st->h_sb.p), static_cast<float*>(st->c_sb.p), st->ra_sb,
+                                   static_cast<__half*>(st->c_h.p), hs_layer, static_cast<float*>(st->c_c.p), cs_layer, d_sess + j0, bs, F, H, L, 0};
+            launch_stream_sb_carry(cy, s);
+            for (int w0 = 0; w0 < K; w0 += tw_max) {
+                const int tw = K - w0 < tw_max ? K - w0 : tw_max;
+                pa.k0 = w0; pa.Kw = tw; pa.idx = d_idx; pa.j0 = j0; pa.nsess = bs;
+                launch_stream_pack_chunk(pa, s);
+                for (int l = 0; l < L; ++l) {
+                    if (l > 0) {
+                        GemmF16Launch g{(long long)ntp * tw * 128, 4 * H, H, static_cast<__half*>(st->c_gin.p), 4LL * H, m->env_gin_tile_n};
+                        const int ge = launch_gemm_f16(st->c_hsb.p, m->r_wih[l].p, g, m->num_sms, s);
+                        if (ge) return fail(FSN_ECUDA, "input-projection GEMM launch failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)ge));
+                    }
+                    LstmTc5rLaunch a{};
+                    a.wstream = static_cast<const __half*>(m->r_stream[l].p);
+                    a.bias = static_cast<const float*>(m->r_bias[l].p);
+                    a.fc_w = P(m, "sb_model.fc_output_layer.weight");
+                    a.fc_b = P(m, "sb_model.fc_output_layer.bias");
+                    a.H = H; a.rows = srows; a.Tp = 4 + K; a.ntiles = nt;
+                    a.t0 = 4 + w0; a.Tw = tw;
+                    if (l == 0) a.ximg = static_cast<const __half*>(st->c_ximg.p);
+                    else a.gin = static_cast<const __half*>(st->c_gin.p);
+                    a.hseq = static_cast<__half*>(st->c_hsb.p);
+                    a.cstate = static_cast<float*>(st->c_c.p) + l * cs_layer;
+                    a.hstate = static_cast<__half*>(st->c_h.p) + l * hs_layer;
+                    a.out = static_cast<float*>(st->c_mask.p); a.F = F; a.la = 4;
+                    a.act = c.sb_act; a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU; a.last = (l == L - 1);
+                    const int le = launch_lstm_tc5r(a, s);
+                    if (le) return fail(FSN_ECUDA, "layer-wise LSTM chunk failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)le));
+                }
+            }
+            cy.out = 1;
+            launch_stream_sb_carry(cy, s);
+            StreamChunkScatterLaunch sc{static_cast<const float*>(st->c_mask.p), d_mask, d_cnt, d_idx, j0, bs, B, F, K, la, j0 == 0};
+            launch_stream_chunk_scatter(sc, s);
+        }
+    }
+    CK(cudaGetLastError());
+    st->n += K;
+    for (int b = 0; b < B; ++b) {
+        h_valid[b] = 0;
+        if (cnt[b] < 0) continue;
+        st->nb[b] = cnt[b] + K;
+        const int v = cnt[b] + K - la;
+        h_valid[b] = v < 0 ? 0 : v > K ? K : v;
+    }
     return FSN_OK;
 }
 

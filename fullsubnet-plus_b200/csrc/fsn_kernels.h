@@ -113,6 +113,21 @@ struct StreamNormLaunch { const float* x; float* y; double* cum; int B, F, P, n,
 void launch_stream_norm(const StreamNormLaunch& a, cudaStream_t s);
 struct StreamPackLaunch { const float* mag; const float* fb; int Pfb; double* cum; __half* ximg; int B, F, Ns, Nf, n, type; const int* slot; };
 void launch_stream_pack(const StreamPackLaunch& a, cudaStream_t s);
+// K-frame forms (fsn_stream_step_chunk): the one-frame arithmetic frame after frame; slot [B] per-slot counts (-1 = held) is required.
+// x [B, F, K] -> y [B, F, P] (frames at columns 0 .. K - 1)
+struct StreamNormChunkLaunch { const float* x; float* y; double* cum; int B, F, K, P, type; const int* slot; };
+void launch_stream_norm_chunk(const StreamNormChunkLaunch& a, cudaStream_t s);
+// frames k0 .. k0 + Kw - 1 of mag [B, F, K] and fb [B, F, Pfb] -> images [tile, Kw, 128 rows, 64 halves].  idx null: row b F + f,
+// held rows zero.  idx [B]: row (idx[b] - j0) F + f for the sessions j0 .. j0 + nsess - 1 of a sub-batch, nothing for any other slot
+struct StreamPackChunkLaunch {
+    const float* mag; const float* fb; int Pfb; double* cum; __half* ximg; int B, F, K, Ns, Nf, type, k0, Kw; const int* slot;
+    const int* idx; int j0, nsess;
+};
+void launch_stream_pack_chunk(const StreamPackChunkLaunch& a, cudaStream_t s);
+// compact masks src [nsess, 2, F, K] of the sessions j0 .. j0 + nsess - 1 -> dst [B, 2, F, K] at their slots (idx[b] - j0), leading
+// columns with slot[b] + k < la zero; zero_held: also zero the rows of held slots
+struct StreamChunkScatterLaunch { const float* src; float* dst; const int* slot; const int* idx; int j0, nsess, B, F, K, la, zero_held; };
+void launch_stream_chunk_scatter(const StreamChunkScatterLaunch& a, cudaStream_t s);
 
 // ---- k_stream_state.cu: save / load of streaming sessions (fsn_stream_save_slots, fsn_stream_load_slots), START reset ----------
 // One segment of the payload: the handle's rows of one state buffer.  Slot b's rows of layer l start at base + l layer_stride +
@@ -131,6 +146,15 @@ struct StreamStateLaunch {
     int dir;                  // LOAD: payload -> handle (scatter); SAVE: handle -> payload (gather); ZERO: zeros -> handle, no payload
 };
 int launch_stream_state(const StreamStateLaunch& a, cudaStream_t s);   // returns 0 or cudaError
+// The sub-band h / c of n sessions (slots sess[0 .. n - 1]) between the handle ([L, rows_alloc, H] rows b F + f, fp16 h, fp32 c) and
+// the layer-wise recurrence's carry (LstmTc5rLaunch::hstate rows j F + f, h_layer halves per layer; cstate in its CTA-private
+// order, c_layer floats per layer).  out = 0: handle -> carry; 1: carry -> handle
+struct StreamSbCarryLaunch {
+    __half* h_handle; float* c_handle; int rows_alloc;
+    __half* h_carry; size_t h_layer; float* c_carry; size_t c_layer;
+    const int* sess; int n, F, H, L, out;
+};
+void launch_stream_sb_carry(const StreamSbCarryLaunch& a, cudaStream_t s);
 
 // ---- k_stream_audio.cu: audio in and out of the streaming slot call (fsn_stream_step_audio_slots) ---------------------------
 // Per-slot ops of one tick, derived on the host from the slot's flag, tick count and hop count (fsn_api.cu, audio_plan)
@@ -205,9 +229,9 @@ struct LstmMmaLaunch {
     // streaming: hidden state carried across launches ([L, rows_alloc, H] fp16); resume = 1 continues from it
     __half* hstate; int resume;
     const int* tlen;          // optional [B] per-sample extent in frames of Tp: output frames t - la >= tlen[b] - la are written as zero
-    // optional (streaming slot call, Tp = 1): per-slot frame counts, -1 = held; row r belongs to slot r / slot_rows.  A held row
-    // writes neither cstate nor hstate.  The fused-FC output of a slot whose count is below slot_la (held, or still filling its
-    // look-ahead) is zero
+    // optional (streaming slot and chunk calls): per-slot frame counts, -1 = held; row r belongs to slot r / slot_rows.  A held row
+    // writes neither cstate nor hstate.  The fused-FC output at step t of a held slot, or of a slot whose frame count + t is below
+    // slot_la (still filling its look-ahead), is zero
     const int* slot; int slot_rows, slot_la;
 };
 size_t lstm_mma_cstate_bytes(int L, int rows, int H, int* rows_alloc);

@@ -731,6 +731,126 @@ __global__ void __launch_bounds__(128) stream_pack_kernel(StreamPackLaunch a) {
 }
 void launch_stream_pack(const StreamPackLaunch& a, cudaStream_t s) { stream_pack_kernel<<<(a.B * a.F + 127) / 128, 128, 0, s>>>(a); }
 
+// K-frame forms of the two kernels above (fsn_stream_step_chunk, DESIGN.md §3.13).  Every frame runs exactly the one-frame kernel's
+// arithmetic -- the same reduction order and the same fp64 running sums, frame after frame -- so one launch over K frames writes the
+// bits K one-frame launches write.  Frame k of slot b is its frame slot[b] + k.
+__global__ void __launch_bounds__(256) stream_norm_chunk_kernel(StreamNormChunkLaunch a) {
+    __shared__ double red[16];
+    __shared__ float s_a, s_b;
+    const int b = blockIdx.x, F = a.F, n0 = a.slot[b];
+    if (n0 < 0) {                                                   // held: frames unread, sums untouched, zero rows
+        for (int i = threadIdx.x; i < F * a.K; i += blockDim.x) a.y[((size_t)b * F + i / a.K) * a.P + i % a.K] = 0.f;
+        return;
+    }
+    const float* x = a.x + (size_t)b * F * a.K;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    double cs = n0 == 0 ? 0.0 : a.cum[2 * b], cq = n0 == 0 ? 0.0 : a.cum[2 * b + 1];   // thread 0's running sums
+#pragma unroll 1
+    for (int k = 0; k < a.K; ++k) {
+        const int n = n0 + k;
+        double s = 0, q = 0;
+        for (int f = threadIdx.x; f < F; f += blockDim.x) { const double v = x[(size_t)f * a.K + k]; s += v; q += v * v; }
+        s = warp_sum_d(s); q = warp_sum_d(q);
+        if (lane == 0) { red[warp] = s; red[8 + warp] = q; }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            double ts = 0, tq = 0;
+            for (int i = 0; i < 8; ++i) { ts += red[i]; tq += red[8 + i]; }
+            const double EPS = 1.1920928955078125e-07;
+            cs += ts; cq += tq;
+            const double cnt = (double)F * (n + 1), cm = cs / cnt;
+            if (a.type == FSN_NORM_CUMULATIVE_LAPLACE) { s_a = (float)(1.0 / (cm + EPS)); s_b = 0.f; }
+            else { const double cv = (cq - 2.0 * cm * cs) / cnt + cm * cm, inv = 1.0 / sqrt(cv + EPS); s_a = (float)inv; s_b = (float)(-cm * inv); }
+        }
+        __syncthreads();
+        for (int f = threadIdx.x; f < F; f += blockDim.x) a.y[((size_t)b * F + f) * a.P + k] = fmaf(x[(size_t)f * a.K + k], s_a, s_b);
+        __syncthreads();                                            // red, s_a and s_b are reused by the next frame
+    }
+    if (threadIdx.x == 0) { a.cum[2 * b] = cs; a.cum[2 * b + 1] = cq; }
+}
+void launch_stream_norm_chunk(const StreamNormChunkLaunch& a, cudaStream_t s) { stream_norm_chunk_kernel<<<a.B, 256, 0, s>>>(a); }
+
+// thread = sequence (b, f); frames k0 .. k0 + Kw - 1 of the chunk into the window-local images [tile, Kw, 128, 64]
+__global__ void __launch_bounds__(128) stream_pack_chunk_kernel(StreamPackChunkLaunch a) {
+    const int row = blockIdx.x * blockDim.x + threadIdx.x, F = a.F;
+    if (row >= a.B * F) return;
+    const int b = row / F, f = row % F;
+    const int nw = 2 * a.Ns + 1, nf = 2 * a.Nf + 1, I = nw + nf;
+    const int n0 = a.slot[b];
+    int crow = row;                                                 // the row of the images
+    if (a.idx) {                                                    // compact rows: session idx[b] - j0 of this sub-batch, or not packed
+        const int j = n0 < 0 ? -1 : a.idx[b] - a.j0;
+        if (j < 0 || j >= a.nsess) return;
+        crow = j * F + f;
+    }
+    const int tile = crow >> 7, r = crow & 127;
+    char* img = reinterpret_cast<char*>(a.ximg) + (size_t)tile * a.Kw * (128 * 128);
+    if (n0 < 0) {                                                   // held: frames unread, sums untouched, zero input rows
+        for (int k = 0; k < a.Kw; ++k)
+#pragma unroll
+            for (int c = 0; c < 8; ++c) *reinterpret_cast<uint4*>(img + (size_t)k * (128 * 128) + sw128_offset(r, c * 8)) = make_uint4(0u, 0u, 0u, 0u);
+        return;
+    }
+    const float* mag = a.mag + (size_t)b * F * a.K;
+    const float* fb = a.fb + (size_t)b * F * a.Pfb;
+    double cs = n0 + a.k0 == 0 ? 0.0 : a.cum[2 * row], cq = n0 + a.k0 == 0 ? 0.0 : a.cum[2 * row + 1];
+#pragma unroll 1
+    for (int kk = 0; kk < a.Kw; ++kk) {
+        const int k = a.k0 + kk, n = n0 + k;
+        int fo = f;                                                 // opaque per frame: the 64 neighbour offsets are recomputed, not
+        asm volatile("" : "+r"(fo));                                // hoisted out of the frame loop (which spills them)
+        float v[64];
+        double s = 0, q = 0;
+#pragma unroll
+        for (int i = 0; i < 64; ++i) {
+            float x = 0.f;
+            if (i < nw) x = mag[(size_t)reflect_idx(fo + i - a.Ns, F) * a.K + k];
+            else if (i < I) x = fb[(size_t)reflect_idx(fo + (i - nw) - a.Nf, F) * a.Pfb + k];
+            v[i] = x; s += x; q += (double)x * x;
+        }
+        const double EPS = 1.1920928955078125e-07;
+        cs += s; cq += q;
+        const double cnt = (double)I * (n + 1), cm = cs / cnt;
+        float sc, sh;
+        if (a.type == FSN_NORM_CUMULATIVE_LAPLACE) { sc = (float)(1.0 / (cm + EPS)); sh = 0.f; }
+        else { const double cv = (cq - 2.0 * cm * cs) / cnt + cm * cm, inv = 1.0 / sqrt(cv + EPS); sc = (float)inv; sh = (float)(-cm * inv); }
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+            float w[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) w[i] = (c * 8 + i < I) ? fminf(fmaxf(fmaf(v[c * 8 + i], sc, sh), -65504.f), 65504.f) : 0.f;
+            *reinterpret_cast<uint4*>(img + (size_t)kk * (128 * 128) + sw128_offset(r, c * 8)) =
+                make_uint4(pack_half2(w[0], w[1]), pack_half2(w[2], w[3]), pack_half2(w[4], w[5]), pack_half2(w[6], w[7]));
+        }
+    }
+    a.cum[2 * row] = cs; a.cum[2 * row + 1] = cq;
+}
+void launch_stream_pack_chunk(const StreamPackChunkLaunch& a, cudaStream_t s) {
+    stream_pack_chunk_kernel<<<(a.B * a.F + 127) / 128, 128, 0, s>>>(a);
+}
+
+// The compact masks of one sub-batch [nsess, 2, F, K] into the slots' rows of d_mask [B, 2, F, K]: column k of slot b is the mask of
+// its frame slot[b] + k - la, zero while that index is negative.  zero_held: also write the rows of held slots as zeros.
+__global__ void stream_chunk_scatter_kernel(StreamChunkScatterLaunch a) {
+    const size_t plane = (size_t)2 * a.F * a.K, n = (size_t)a.B * plane;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const int b = (int)(i / plane), k = (int)(i % a.K), n0 = a.slot[b];
+        if (n0 < 0) {
+            if (a.zero_held) a.dst[i] = 0.f;
+            continue;
+        }
+        const int j = a.idx[b] - a.j0;
+        if (j < 0 || j >= a.nsess) continue;
+        a.dst[i] = n0 + k < a.la ? 0.f : a.src[(size_t)j * plane + i % plane];
+    }
+}
+void launch_stream_chunk_scatter(const StreamChunkScatterLaunch& a, cudaStream_t s) {
+    const size_t n = (size_t)a.B * 2 * a.F * a.K;
+    size_t blocks = (n + 255) / 256;
+    if (blocks > 4096) blocks = 4096;
+    stream_chunk_scatter_kernel<<<(unsigned)blocks, 256, 0, s>>>(a);
+}
+
 // decompress_cIRM + complex multiply (inferencer.py:152-157, mask.py:60-63) in one pass.
 __global__ void apply_cirm_kernel(const float* crm, const float2* noisy, float2* enh, int FT, size_t n) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;

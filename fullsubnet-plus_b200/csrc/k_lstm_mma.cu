@@ -144,7 +144,8 @@ __global__ void __launch_bounds__(256, 1) lstm_mma_kernel(LstmMmaLaunch a) {
                 const int r = e / a.O, o = e % a.O, grow = row0 + r;
                 if (grow >= a.rows) continue;
                 const int b = grow / a.F, f = grow % a.F;
-                if ((a.tlen && t >= a.tlen[b]) || (SLOTS && a.slot[grow / a.slot_rows] < a.slot_la)) {   // past the clip's end; no valid mask
+                const int sn = SLOTS ? a.slot[grow / a.slot_rows] : 0;  // the slot's count: frame t is its frame sn + t
+                if ((a.tlen && t >= a.tlen[b]) || (SLOTS && (sn < 0 || sn + t < a.slot_la))) {   // past the clip's end; held; no valid mask
                     a.out[(((size_t)b * a.O + o) * a.F + f) * (Tp - a.la) + (t - a.la)] = 0.f;
                     continue;
                 }

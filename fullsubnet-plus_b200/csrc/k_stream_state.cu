@@ -49,4 +49,41 @@ int launch_stream_state(const StreamStateLaunch& a, cudaStream_t s) {
     return (int)cudaGetLastError();
 }
 
+// The sub-band h and c of the sessions of a chunk's sub-batch between the handle and the layer-wise recurrence's carry
+// (fsn_stream_step_chunk, DESIGN.md §3.13).  Thread = (layer, compact row j F + f, 8 hidden units).  h: fp16 rows, 16 bytes at a time.
+// c (GRU: its fp32 h): the handle's row-major [rows_alloc, H] against lstm_tc5r_kernel's CTA-private order -- CTA cta = row / 64,
+// chunk j = u / 32, thread wt and fragment element v of the float4 at cstate + (cta NCH + j) 2048 + (v / 4 * 128 + wt) * 4 + v % 4.
+__global__ void __launch_bounds__(256) stream_sb_carry_kernel(StreamSbCarryLaunch a) {
+    const int H = a.H, NCH = H / 32, F = a.F;
+    const size_t per_layer = (size_t)a.n * F * (H / 8), n = per_layer * a.L;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const int l = (int)(i / per_layer);
+        const size_t e = i % per_layer;
+        const int jr = (int)(e / (H / 8)), u0 = (int)(e % (H / 8)) * 8;
+        const int hrow = a.sess[jr / F] * F + jr % F;              // the handle's row of this sequence
+        uint4* hh = reinterpret_cast<uint4*>(a.h_handle + (l * (size_t)a.rows_alloc + hrow) * H + u0);
+        uint4* hc = reinterpret_cast<uint4*>(a.h_carry + l * a.h_layer + (size_t)jr * H + u0);
+        float* ch = a.c_handle + (l * (size_t)a.rows_alloc + hrow) * H + u0;
+        float* cc = a.c_carry + l * a.c_layer + (size_t)(jr / 64) * NCH * 2048;
+        const int rl = jr % 64, wi = rl / 16, hr = (rl % 16) / 8, lr = rl % 8;
+#pragma unroll
+        for (int w = 0; w < 8; ++w) {
+            const int u = u0 + w, j = u / 32, cg = (u % 32) / 8, q = (u % 8) / 2, ev = u % 2;
+            const int wt = wi * 32 + lr * 4 + q, v = hr * 8 + cg * 2 + ev;
+            float* c = cc + (size_t)j * 2048 + ((v / 4) * 128 + wt) * 4 + v % 4;
+            if (a.out) ch[w] = *c;
+            else *c = ch[w];
+        }
+        if (a.out) *hh = *hc;
+        else *hc = *hh;
+    }
+}
+
+void launch_stream_sb_carry(const StreamSbCarryLaunch& a, cudaStream_t s) {
+    const size_t n = (size_t)a.L * a.n * a.F * (a.H / 8);
+    size_t blocks = (n + 255) / 256;
+    if (blocks > 4096) blocks = 4096;
+    stream_sb_carry_kernel<<<(unsigned)blocks, 256, 0, s>>>(a);
+}
+
 }  // namespace fsn

@@ -25,6 +25,7 @@ SYMBOLS = [
     "fsn_stream_step_slots", "fsn_stream_step_audio_slots",
     "fsn_stream_state_bytes", "fsn_stream_state_layout", "fsn_model_weights_id", "fsn_stream_save_slots", "fsn_stream_load_slots",
     "fsn_model_enhance_audio", "fsn_plan_audio",
+    "fsn_stream_step_chunk", "fsn_stream_chunk_plan",
 ]
 
 
@@ -100,6 +101,8 @@ def load_library():
     lib.fsn_stream_step.argtypes = [vp, vp, vp, C.POINTER(i32), vp]
     lib.fsn_stream_step_slots.argtypes = [vp, vp, vp, vp, vp, vp]
     lib.fsn_stream_step_audio_slots.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+    lib.fsn_stream_step_chunk.argtypes = [vp, vp, i32, vp, vp, vp, vp]
+    lib.fsn_stream_chunk_plan.argtypes = [C.POINTER(FsnConfig), i32, i32, C.c_double, C.POINTER(i32), C.POINTER(i32), C.POINTER(i64)]
     lib.fsn_stream_destroy.argtypes = [vp]
     lib.fsn_stream_destroy.restype = None
     lib.fsn_stream_state_bytes.argtypes = [vp]
@@ -190,6 +193,16 @@ def plan_forward_bins(cfg, B, T, cap_bytes=None, force_window=0, force_bins=0):
     check(lib.fsn_plan_forward_bins(C.byref(cfg), int(B), int(T), cap, int(force_window), int(force_bins), C.byref(bs), C.byref(tw),
                                     C.byref(fc), C.byref(nb)))
     return bs.value, tw.value, fc.value, nb.value
+
+
+def stream_chunk_plan(cfg, n_active, K, cap_bytes=None):
+    """fsn_stream_chunk_plan: (sessions per sub-batch, window in frames or 0, scratch bytes of one sub-batch) of a streaming chunk call
+    with n_active stepping sessions of K frames under the cap (default: ws_cap_bytes()).  Needs no GPU."""
+    lib = load_library()
+    bs, tw, nb = C.c_int32(), C.c_int32(), C.c_int64()
+    cap = ws_cap_bytes() if cap_bytes is None else float(cap_bytes)
+    check(lib.fsn_stream_chunk_plan(C.byref(cfg), int(n_active), int(K), cap, C.byref(bs), C.byref(tw), C.byref(nb)))
+    return bs.value, tw.value, nb.value
 
 
 def lengths_arg(lengths, B):

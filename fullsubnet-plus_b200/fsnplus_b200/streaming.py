@@ -9,6 +9,9 @@ produced when frame n arrives, exactly as the reference's right zero-padding + o
 Independent sessions share one handle through ``step_slots``: each of the B slots serves its own session, which starts, pauses
 and ends on its own schedule (flags HOLD / STEP / START per slot and tick, DESIGN.md §3.9).
 
+``step_chunk`` advances the same sessions K frames per call, with the sub-band LSTM on the offline forward's tensor-core kernels
+where the configuration takes them (DESIGN.md §3.13); it mixes freely with ``step_slots`` on one handle.
+
 ``step_audio`` serves the same sessions with audio in and out: one hop of samples per slot and tick goes in, one hop of enhanced
 audio comes out, with the STFT, the cIRM and the overlap-add iSTFT on the device (flag FLUSH ends a session, DESIGN.md §3.10).
 A handle serves either the mask calls or the audio call.
@@ -118,6 +121,26 @@ class StreamingFullSubNet:
             _lib.check(self.lib.fsn_stream_step_slots(self._st, C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()),
                                                       C.c_void_p(f.data_ptr()), C.c_void_p(valid.data_ptr()), stream))
         return out, valid.bool()
+
+    def step_chunk(self, mag, flags):
+        """K ticks of independent sessions in one call (DESIGN.md §3.13).  mag [B, F, K] float32 CUDA: each slot's next K frames
+        (rows of held slots are never read); flags: B values of HOLD / STEP / START, which STEP or START K frames.  Returns (mask
+        [B, 2, F, K], nvalid int32 CPU tensor [B]): column k of slot b is the mask of its frame n_b + k - look_ahead (n_b: frames
+        consumed since its START before this call), and the nvalid[b] valid columns are the trailing ones; every other column and
+        every held row is zero."""
+        assert mag.dim() == 3 and mag.shape[:2] == (self.B, self.F) and mag.is_cuda
+        K = mag.shape[2]
+        f = torch.as_tensor(flags, dtype=torch.int32)
+        assert f.device.type == "cpu" and f.shape == (self.B,), "flags: B host values"
+        f = f.contiguous()
+        x = mag.contiguous().float()
+        out = torch.empty((self.B, 2, self.F, K), dtype=torch.float32, device=self.device)
+        nvalid = torch.zeros(self.B, dtype=torch.int32)
+        with torch.cuda.device(self.device):
+            stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+            _lib.check(self.lib.fsn_stream_step_chunk(self._st, C.c_void_p(x.data_ptr()), K, C.c_void_p(out.data_ptr()),
+                                                      C.c_void_p(f.data_ptr()), C.c_void_p(nvalid.data_ptr()), stream))
+        return out, nvalid
 
     @property
     def hop(self):

@@ -216,6 +216,30 @@ void fsn_stream_destroy(fsn_stream* st);
 int fsn_stream_step_slots(fsn_stream* st, const float* d_mag_frame, float* d_mask, const int32_t* h_flags, int32_t* h_valid,
                           void* stream);
 
+/* Many frames per call (DESIGN.md §3.13): K fsn_stream_step_slots ticks in one call, for callers that take 8-64 frames at a time or
+ * catch a session up on a backlog.  d_mag [B, F, K] float32 device: slot b's next K magnitude frames along the last axis (rows of
+ * HOLD slots are never read).  h_flags: HOST, B flags as in fsn_stream_step_slots; STEP and START consume K frames, HOLD leaves the
+ * slot's state (frame count and norm sums included) unchanged.  d_mask [B, 2, F, K] float32 device: with n_b the frames slot b had
+ * consumed since its START before this call (0 on START), column k is the mask of frame n_b + k - look_ahead when that index is >= 0,
+ * else zero; rows of held slots are zero.  h_valid (HOST, [B]): the number of valid columns, always the trailing ones:
+ * clamp(n_b + K - look_ahead, 0, K) for a stepping slot, 0 for a held one.  The call may be mixed freely with fsn_stream_step /
+ * fsn_stream_step_slots and save / load on the same handle; the session state and its payload are the per-frame step's.
+ * The sub-band stage runs on the offline forward's path: the layer-wise tensor-core kernels when the configuration takes them
+ * (then only the stepping sessions run, in sub-batches and time windows under FSN_WS_CAP_GB, fsn_stream_chunk_plan; the result does
+ * not depend on the split, but it is not the per-frame step's bits: both meet the same accuracy), else the per-frame step's kernel
+ * over K steps, bit-identical to K fsn_stream_step_slots calls.  The scratch belongs to the handle: allocated at the first call,
+ * grow-only, freed by fsn_stream_destroy.
+ * FSN_EINVAL naming the slot for a flag outside {0, 1, 2}; naming the argument for K < 1 or a null array; naming the limit for K past
+ * 65535 x 256 - 4 frames or num_freqs x K past 2^31 - 1.  FSN_ESTATE on a handle that serves the audio call.  A failed call changes no
+ * state.  Both host arrays are free when the call returns; the call does not synchronise the stream. */
+int fsn_stream_step_chunk(fsn_stream* st, const float* d_mag, int32_t K, float* d_mask, const int32_t* h_flags, int32_t* h_valid,
+                          void* stream);
+/* The chunk call's sub-band plan for n_active stepping sessions of K frames under cap_bytes: sessions per sub-batch *Bs, window *Tw
+ * (0: the whole chunk) and the scratch *bytes of one sub-batch (layer-wise path: images, Gin, layer output, h / c carry, compact
+ * masks; generic path: one piece, the images).  Same FSN_EINVAL messages as the call, plus a non-streaming configuration and
+ * n_active < 1.  Host only, no GPU. */
+int fsn_stream_chunk_plan(const fsn_config* cfg, int32_t n_active, int32_t K, double cap_bytes, int32_t* Bs, int32_t* Tw, int64_t* bytes);
+
 /* Audio in, audio out (DESIGN.md §3.10): the slot call with the STFT before the model step and decompress_cIRM x noisy spectrum,
  * inverse FFT and overlap-add after it, on the device.  Each slot's waveform equals the offline enhancement of its session's audio
  * (torch.stft(center=True, reflect) -> model -> decompress_cIRM x spectrum -> torch.istft(length = L)).

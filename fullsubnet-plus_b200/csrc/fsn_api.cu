@@ -896,6 +896,38 @@ static int ensure_ws(fsn_model* m, Lane& ln, int B, int T, int Tw, int Fc, cudaS
     return FSN_OK;
 }
 
+// One window of the layer-wise sub-band recurrence, layer after layer: for l > 0 the input-projection GEMM of every row and frame of
+// the window into gin (k_gemm_tc5.cu), then lstm_tc5r_kernel; layer 0 projects its input (the packed images) itself.  a: the
+// window's launch (rows, ntiles, Tp, t0, Tw, ximg, hseq, out, la and the epilogue) with layer 0's cstate and hstate (null: none);
+// layer l's lie cs_layer floats and hs_layer halves further.  Returns the number of launches, or the error code.
+static int sb_layers(fsn_model* m, const LstmTc5rLaunch& a, __half* gin, size_t cs_layer, size_t hs_layer, cudaStream_t s) {
+    const fsn_config& c = m->cfg;
+    const int H = c.sb_hidden;
+    int launches = 0;
+    for (int l = 0; l < c.num_layers; ++l) {
+        LstmTc5rLaunch al = a;
+        if (l > 0) {
+            // row-major Gin[M, 4H] = X[M, H] * Wp[4H, H]^T, both operands K-major
+            GemmF16Launch g{(long long)(a.ntiles + 1) / 2 * 2 * a.Tw * 128, 4 * H, H, gin, 4LL * H, m->env_gin_tile_n};
+            const int ge = launch_gemm_f16(a.hseq, m->r_wih[l].p, g, m->num_sms, s);
+            if (ge) return fail(FSN_ECUDA, "input-projection GEMM launch failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)ge));
+            launches++;
+            al.ximg = nullptr; al.gin = gin;
+        }
+        al.wstream = static_cast<const __half*>(m->r_stream[l].p);
+        al.bias = static_cast<const float*>(m->r_bias[l].p);
+        al.fc_w = P(m, "sb_model.fc_output_layer.weight");
+        al.fc_b = P(m, "sb_model.fc_output_layer.bias");
+        al.H = H; al.F = c.num_freqs; al.act = c.sb_act; al.fast = c.fast_math; al.gru = c.rnn_type == FSN_RNN_GRU; al.last = (l == c.num_layers - 1);
+        al.cstate = a.cstate + l * cs_layer;
+        if (a.hstate) al.hstate = a.hstate + l * hs_layer;
+        const int e = launch_lstm_tc5r(al, s);
+        if (e) return fail(FSN_ECUDA, "layer-wise LSTM launch failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)e));
+        launches++;
+    }
+    return launches;
+}
+
 // d_enh != null: write the enhanced spectrum (decompress_cIRM x noisy) instead of the mask -- fused into the epilogue of the
 // layer-wise kernel's last layer, a separate pass over a scratch mask for the generic kernel
 // Tw > 0: the sub-band stage runs in time windows of Tw frames (the last one shorter); for each window the images are packed (`sp`, the
@@ -909,9 +941,9 @@ static int run_sb_lstm(fsn_model* m, Lane& ln, int B, int T, int Tw, SbPackLaunc
     m->last_impl = impl;
     if (runs_layerwise(c, m->env_impl)) {
         // one recurrent launch per layer; the first one also projects its input (the packed images), each deeper one is preceded by
-        // one GEMM: the input projection of every row and time step of the window (k_gemm_tc5.cu)
-        const int H = c.sb_hidden, ntp = (ntiles + 1) / 2 * 2;
-        const size_t cs_layer = lstm_tc5r_cstate_bytes(ntiles, H) / sizeof(float), hs_layer = (size_t)ntp * 128 * H;
+        // one GEMM: the input projection of every row and time step of the window (sb_layers)
+        const size_t cs_layer = lstm_tc5r_cstate_bytes(ntiles, c.sb_hidden) / sizeof(float);
+        const size_t hs_layer = (size_t)(ntiles + 1) / 2 * 2 * 128 * c.sb_hidden;
         for (int w0 = 0; w0 < Tp; w0 += (Tw ? Tw : Tp)) {
             const int tw = Tw ? (Tp - w0 < Tw ? Tp - w0 : Tw) : Tp;
             if (Tw) {
@@ -919,34 +951,17 @@ static int run_sb_lstm(fsn_model* m, Lane& ln, int B, int T, int Tw, SbPackLaunc
                 launch_sb_pack(sp, s);
                 m->launches++;
             }
-            const long long M = (long long)ntp * tw * 128;
-            for (int l = 0; l < c.num_layers; ++l) {
-                if (l > 0) {
-                    // row-major Gin[M, 4H] = X[M, H] * Wp[4H, H]^T, both operands K-major
-                    GemmF16Launch g{M, 4 * H, H, static_cast<__half*>(m->r_gin.p), 4LL * H, m->env_gin_tile_n};
-                    int ge = launch_gemm_f16(m->r_hseq.p, m->r_wih[l].p, g, m->num_sms, s);
-                    if (ge) return fail(FSN_ECUDA, "input-projection GEMM launch failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)ge));
-                    m->launches++;
-                }
-                LstmTc5rLaunch a{};
-                a.wstream = static_cast<const __half*>(m->r_stream[l].p);
-                a.bias = static_cast<const float*>(m->r_bias[l].p);
-                a.fc_w = P(m, "sb_model.fc_output_layer.weight");
-                a.fc_b = P(m, "sb_model.fc_output_layer.bias");
-                a.H = H; a.rows = rows; a.Tp = Tp; a.ntiles = ntiles;
-                a.t0 = w0; a.Tw = tw;
-                if (l == 0) a.ximg = static_cast<const __half*>(ln.ximg.p);
-                else a.gin = static_cast<const __half*>(m->r_gin.p);
-                a.hseq = static_cast<__half*>(m->r_hseq.p);
-                a.cstate = static_cast<float*>(m->cstate.p) + (Tw ? l * cs_layer : 0);
-                if (Tw) a.hstate = static_cast<__half*>(m->r_hstate.p) + l * hs_layer;
-                a.out = d_out; a.F = F; a.la = c.look_ahead;
-                a.act = c.sb_act; a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU; a.last = (l == c.num_layers - 1);
-                a.nreal = d_real; a.nimag = d_imag; a.enh = reinterpret_cast<float2*>(d_enh); a.tlen = tlen;
-                int e = launch_lstm_tc5r(a, s);
-                if (e) return fail(FSN_ECUDA, "layer-wise LSTM launch failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)e));
-                m->launches++;
-            }
+            LstmTc5rLaunch a{};
+            a.rows = rows; a.Tp = Tp; a.ntiles = ntiles; a.t0 = w0; a.Tw = tw;
+            a.ximg = static_cast<const __half*>(ln.ximg.p);
+            a.hseq = static_cast<__half*>(m->r_hseq.p);
+            a.cstate = static_cast<float*>(m->cstate.p);
+            if (Tw) a.hstate = static_cast<__half*>(m->r_hstate.p);
+            a.out = d_out; a.la = c.look_ahead;
+            a.nreal = d_real; a.nimag = d_imag; a.enh = reinterpret_cast<float2*>(d_enh); a.tlen = tlen;
+            const int nl = sb_layers(m, a, static_cast<__half*>(m->r_gin.p), Tw ? cs_layer : 0, hs_layer, s);
+            if (nl < 0) return nl;
+            m->launches += nl;
         }
     } else if (Tw) {
         return fail(FSN_EINVAL, "time windows of the sub-band stage need the layer-wise LSTM path");
@@ -1824,16 +1839,29 @@ extern "C" int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst,
 // ---------------------------------------------------------------------------------------------
 // streaming step API (causal fullsubnet.Model)
 // ---------------------------------------------------------------------------------------------
+// The scratch of a step of K frames over all B slots (step_frames), P = K rounded up to 4: the normalised input [B, F, P], its fp16
+// form [K, rows_pad, Ipad], the top layer's h [B, H, P], the full-band output [B, F, P] and the sub-band images (img bytes, zeroed)
+struct fsn_stream;
+struct StepScratch {
+    DevBuf fbin, fbx, hseq, fbout, ximg;
+    int ensure(const fsn_stream& st, int K, size_t img, bool zero, cudaStream_t s);
+    void release() { for (DevBuf* b : {&fbin, &fbx, &hseq, &fbout, &ximg}) b->release(); }
+};
+// the generic sub-band step's images of `rows` rows over K frames
+static size_t step_img_bytes(long long rows, int K) { return (size_t)((rows + 127) / 128) * K * 16384; }
+
 struct fsn_stream {
     fsn_model* m;
     int B, n = 0;                                      // n: ticks of the handle (the weight-stationary exchange-buffer parity)
     DevBuf cum_in, cum_sb, h_fb, c_fb, h_sb, c_sb, ws_h, ws_c;   // session state (the table STATE)
-    DevBuf fbin, fbx, hseq, fbout, ximg, ws_bar;       // per-tick scratch of the step
+    StepScratch tick;                                  // the per-frame calls' scratch (K = 1)
+    DevBuf ws_bar;
     bool use_ws = false;
     int ra_fb = 0, ra_sb = 0, rows_pad = 0, Ipad = 0;
-    // slot call (fsn_stream_step_slots): once used, every step runs per slot.  nb: frames each slot has consumed since its START
-    // (seeded with n at the first slot call); d_slot [5 B]: this tick's per-slot values for the kernels -- the counts (-1 = held),
-    // then the audio call's three planes, then the slots a START zeroes.  They reach the device through `stage`.
+    // slot calls (fsn_stream_step_slots, the chunk call): once used, every step runs per slot.  nb: frames each slot has consumed since
+    // its START (seeded with n at the first slot call); d_slot [5 B]: this call's per-slot values for the kernels -- the counts (-1 =
+    // held), then the audio call's three planes or the chunk call's layer-wise session lists, then the slots a START zeroes.  They reach
+    // the device through `stage`.
     bool slots = false;
     std::vector<int32_t> nb, all_step, valid;
     DevBuf d_slot;
@@ -1850,12 +1878,21 @@ struct fsn_stream {
     // save / load (fsn_stream_save_slots, fsn_stream_load_slots): the slot list of the last call on the device
     DevBuf x_slot;
     // chunk call (fsn_stream_step_chunk, DESIGN.md §3.13): its scratch, allocated at its first use, grow-only, apart from the model's
-    // workspace (the model may forward offline on another stream meanwhile).  Full band over all B slots: the normalised input
-    // [B, F, P], its fp16 form [K, rows_pad, Ipad], the top layer's h [B, H, P], the output [B, F, P]; sub band: the images, and on the
-    // layer-wise path the Gin / layer output, the per-layer h / c carry and the compact masks of one sub-batch; c_slot: the slot's
-    // counts, the START list, each slot's active-session index and the active slots
-    DevBuf c_fbin, c_fbx, c_hseq, c_fbout, c_ximg, c_gin, c_hsb, c_h, c_c, c_mask, c_slot;
+    // workspace (the model may forward offline on another stream meanwhile).  On the layer-wise path the images are those of one
+    // sub-batch, and c_*: its Gin / layer output, the per-layer h / c carry and the compact masks
+    StepScratch chunk;
+    DevBuf c_gin, c_hsb, c_h, c_c, c_mask;
 };
+
+int StepScratch::ensure(const fsn_stream& st, int K, size_t img, bool zero, cudaStream_t s) {
+    const size_t B = st.B, F = st.m->cfg.num_freqs, P = (K + 3) & ~3;
+    int e = fbin.ensure(B * F * P * 4, zero, s);
+    e |= fbx.ensure((size_t)K * st.rows_pad * st.Ipad * 2, zero, s);
+    e |= hseq.ensure(B * st.m->cfg.fb_hidden * P * 4, zero, s);
+    e |= fbout.ensure(B * F * P * 4, zero, s);
+    e |= ximg.ensure(img, true, s);
+    return e;
+}
 
 // The state of a session: one entry per buffer, in payload order (DESIGN.md §3.11).  The handle's allocation (fsn_stream_create,
 // audio_alloc), its release, the payload layout (state_layout), the save / load copy and the START reset all read this table.
@@ -1960,17 +1997,13 @@ extern "C" int fsn_stream_create(fsn_model* m, int32_t B, fsn_stream** out) {
     if (int rc = streams_ok(c)) return rc;
     fsn_stream* st = new fsn_stream();
     st->m = m; st->B = B;
-    const int F = c.num_freqs, rows = B * F, ntiles = (rows + 127) / 128;
+    const int F = c.num_freqs, rows = B * F;
     st->Ipad = (F + 15) / 16 * 16; st->rows_pad = (B + 63) / 64 * 64;
     lstm_mma_cstate_bytes(1, B, 1, &st->ra_fb);
     lstm_mma_cstate_bytes(1, rows, 1, &st->ra_sb);
     st->use_ws = lstm_ws_supported(c.num_layers, c.fb_hidden, st->Ipad, B, m->num_sms) && !m->env_no_ws;
     // scratch, then state, then the barrier: with the state allocated first, steps at 16-64 slots measured ~0.03 ms slower per tick
-    int e = st->fbin.ensure((size_t)B * F * 4 * 4, true);
-    e |= st->fbx.ensure((size_t)st->rows_pad * st->Ipad * 2, true);
-    e |= st->hseq.ensure((size_t)B * c.fb_hidden * 4 * 4, true);
-    e |= st->fbout.ensure((size_t)B * F * 4 * 4, true);
-    e |= st->ximg.ensure((size_t)ntiles * 16384, true);
+    int e = st->tick.ensure(*st, 1, step_img_bytes(rows, 1), true, nullptr);
     e |= state_alloc(st, 0, nullptr);
     if (st->use_ws) e |= st->ws_bar.ensure(64, true);
     e |= st->d_slot.ensure((size_t)5 * B * sizeof(int32_t), false);
@@ -1985,10 +2018,11 @@ extern "C" void fsn_stream_destroy(fsn_stream* st) {
         (st->*e.buf).release();
         if (e.ws) (st->*e.ws).release();
     }
-    DevBuf* scratch[] = {&st->fbin, &st->fbx, &st->hseq, &st->fbout, &st->ximg, &st->ws_bar, &st->a_mag, &st->a_mask, &st->a_tab,
-                         &st->d_slot, &st->x_slot, &st->c_fbin, &st->c_fbx, &st->c_hseq, &st->c_fbout, &st->c_ximg, &st->c_gin,
-                         &st->c_hsb, &st->c_h, &st->c_c, &st->c_mask, &st->c_slot};
-    for (auto* b : scratch) b->release();
+    st->tick.release();
+    st->chunk.release();
+    for (DevBuf* b : {&st->ws_bar, &st->d_slot, &st->x_slot, &st->a_mag, &st->a_mask, &st->a_tab, &st->c_gin, &st->c_hsb, &st->c_h,
+                      &st->c_c, &st->c_mask})
+        b->release();
     delete st;
 }
 
@@ -2007,94 +2041,101 @@ static void use_slot_counts(fsn_stream* st) {
     st->slots = true;
 }
 
-// One tick of the handle.  slot: null (the lockstep step: every slot at frame n) or the device per-slot counts of the slot call;
-// zero[nzero]: device list of the slots whose recurrent state is zeroed first (a START's).
-static int stream_tick(fsn_stream* st, const float* d_mag, float* d_mask, const int* slot, const int* zero, int nzero, cudaStream_t s) {
+// The layer-wise sub band of a chunk call (DESIGN.md §3.13): the plan of its nact stepping sessions, and on the device each slot's
+// session index (-1 = held) and the stepping slots
+struct LwSessions { Plan p; int nact; const int *idx, *sess; };
+
+// K frames of every slot on scratch x (DESIGN.md §3.9, §3.13): d_mag [B, F, K] -> d_mask [B, 2, F, K].  slot: null (the lockstep step:
+// every slot at frame n) or the device per-slot counts (-1 = held); zero[nzero]: device list of the slots whose recurrent state is
+// zeroed first (a START's).  The full band runs in place over every slot; the sub band too (lw null: the per-frame step's kernel and
+// state), or on the layer-wise kernels over the stepping sessions only.
+static int step_frames(fsn_stream* st, StepScratch& x, const float* d_mag, int K, const int* slot, const int* zero, int nzero,
+                       float* d_mask, const LwSessions* lw, cudaStream_t s) {
     fsn_model* m = st->m;
     const fsn_config& c = m->cfg;
-    const int B = st->B, F = c.num_freqs, n = st->n, resume = slot ? 1 : n > 0;    // slot call: a START zeroes instead of resume = 0
+    const int B = st->B, F = c.num_freqs, L = c.num_layers, n = st->n, Pk = (K + 3) & ~3;
+    const int resume = slot ? 1 : n > 0;                                // slot calls: a START zeroes instead of resume = 0
     if (nzero) {
         StreamStateLaunch z{};
         state_launch(st, NSEG, ST_START, nullptr, z);
         z.slots = zero; z.n = nzero; z.dir = STREAM_STATE_ZERO;
         if (int e = launch_stream_state(z, s)) return fail(FSN_ECUDA, "session state reset failed: %s", cudaGetErrorString((cudaError_t)e));
     }
-    StreamNormLaunch na{d_mag, static_cast<float*>(st->fbin.p), static_cast<double*>(st->cum_in.p), B, F, 4, n, c.norm_type, slot};
+    StreamNormLaunch na{d_mag, static_cast<float*>(x.fbin.p), static_cast<double*>(st->cum_in.p), B, F, K, Pk, n, c.norm_type, slot};
     launch_stream_norm(na, s);
-    launch_fb_pack(static_cast<const float*>(st->fbin.p), static_cast<__half*>(st->fbx.p), B, F, 1, 4, st->rows_pad, st->Ipad, s);
+    launch_fb_pack(static_cast<const float*>(x.fbin.p), static_cast<__half*>(x.fbx.p), B, F, K, Pk, st->rows_pad, st->Ipad, s);
     int e = 0;
     if (st->use_ws) {
         LstmWsLaunch w{};
         fill_ws(m, w);
-        w.rows = B; w.rows_pad = st->rows_pad; w.Tp = 1;
-        w.x = static_cast<const __half*>(st->fbx.p); w.hbuf = static_cast<__half*>(st->ws_h.p); w.cbuf = static_cast<float*>(st->ws_c.p);
+        w.rows = B; w.rows_pad = st->rows_pad; w.Tp = K;
+        w.x = static_cast<const __half*>(x.fbx.p); w.hbuf = static_cast<__half*>(st->ws_h.p); w.cbuf = static_cast<float*>(st->ws_c.p);
         w.barrier = static_cast<unsigned int*>(st->ws_bar.p);
-        w.hseq = static_cast<float*>(st->hseq.p); w.P = 4; w.resume = resume; w.t0 = n; w.slot = slot;
+        w.hseq = static_cast<float*>(x.hseq.p); w.P = Pk; w.resume = resume; w.t0 = n; w.slot = slot;
         e = launch_lstm_ws(w, s);
     } else {
         LstmMmaLaunch a{};
-        for (int l = 0; l < c.num_layers; ++l) { a.w.wfrag[l] = static_cast<const uint4*>(m->fb_frag[l].p); a.w.bias[l] = static_cast<const float*>(m->fb_bias[l].p); }
-        a.L = c.num_layers; a.H = c.fb_hidden; a.I = F; a.Ipad = st->Ipad; a.rows = B; a.Tp = 1;
-        a.xplain = static_cast<const __half*>(st->fbx.p); a.rows_pad = st->rows_pad;
+        for (int l = 0; l < L; ++l) { a.w.wfrag[l] = static_cast<const uint4*>(m->fb_frag[l].p); a.w.bias[l] = static_cast<const float*>(m->fb_bias[l].p); }
+        a.L = L; a.H = c.fb_hidden; a.I = F; a.Ipad = st->Ipad; a.rows = B; a.Tp = K;
+        a.xplain = static_cast<const __half*>(x.fbx.p); a.rows_pad = st->rows_pad;
         a.cstate = static_cast<float*>(st->c_fb.p); a.rows_alloc = st->ra_fb;
-        a.hseq = static_cast<float*>(st->hseq.p); a.P = 4; a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU;
+        a.hseq = static_cast<float*>(x.hseq.p); a.P = Pk; a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU;
         a.hstate = static_cast<__half*>(st->h_fb.p); a.resume = resume; a.slot = slot; a.slot_rows = 1;
         e = launch_lstm_mma(a, s);
     }
     if (e) return fail(FSN_ECUDA, "full-band LSTM step failed: %s", cudaGetErrorString((cudaError_t)e));
     ConvLaunch cf{};
-    cf.X = static_cast<const float*>(st->hseq.p); cf.Y = static_cast<float*>(st->fbout.p);
-    cf.Z = B; cf.M = F; cf.K = c.fb_hidden; cf.Tp = 1; cf.P = 4; cf.act = c.fb_act;
+    cf.X = static_cast<const float*>(x.hseq.p); cf.Y = static_cast<float*>(x.fbout.p);
+    cf.Z = B; cf.M = F; cf.K = c.fb_hidden; cf.Tp = K; cf.P = Pk; cf.act = c.fb_act;
     cf.W = P(m, "fb_model.fc_output_layer.weight"); cf.bias = P(m, "fb_model.fc_output_layer.bias");
     launch_conv1x1(cf, s);
-    StreamPackLaunch pa{d_mag, static_cast<const float*>(st->fbout.p), 4, static_cast<double*>(st->cum_sb.p), static_cast<__half*>(st->ximg.p),
-                        B, F, c.sb_num_neighbors, c.fb_num_neighbors, n, c.norm_type, slot};
-    launch_stream_pack(pa, s);
-    LstmMmaLaunch b{};
-    for (int l = 0; l < c.num_layers; ++l) { b.w.wfrag[l] = static_cast<const uint4*>(m->sb_frag[l].p); b.w.bias[l] = static_cast<const float*>(m->sb_bias[l].p); }
-    b.w.fc_w = P(m, "sb_model.fc_output_layer.weight"); b.w.fc_b = P(m, "sb_model.fc_output_layer.bias");
-    b.L = c.num_layers; b.H = c.sb_hidden; b.I = m->Isb; b.Ipad = 64; b.rows = B * F; b.Tp = 1;
-    b.img = static_cast<const __half*>(st->ximg.p); b.ntiles = (B * F + 127) / 128;
-    b.cstate = static_cast<float*>(st->c_sb.p); b.rows_alloc = st->ra_sb;
-    b.out = d_mask; b.O = c.output_size; b.F = F; b.la = 0; b.act = c.sb_act; b.fast = c.fast_math; b.gru = c.rnn_type == FSN_RNN_GRU;
-    b.hstate = static_cast<__half*>(st->h_sb.p); b.resume = resume; b.slot = slot; b.slot_rows = F; b.slot_la = c.look_ahead;
-    e = launch_lstm_mma(b, s);
-    if (e) return fail(FSN_ECUDA, "sub-band LSTM step failed: %s", cudaGetErrorString((cudaError_t)e));
+    StreamPackLaunch pa{d_mag, static_cast<const float*>(x.fbout.p), Pk, static_cast<double*>(st->cum_sb.p), static_cast<__half*>(x.ximg.p),
+                        B, F, K, c.sb_num_neighbors, c.fb_num_neighbors, n, c.norm_type, 0, K, slot, nullptr, 0, 0};
+    if (!lw) {
+        launch_stream_pack(pa, s);
+        LstmMmaLaunch b{};
+        for (int l = 0; l < L; ++l) { b.w.wfrag[l] = static_cast<const uint4*>(m->sb_frag[l].p); b.w.bias[l] = static_cast<const float*>(m->sb_bias[l].p); }
+        b.w.fc_w = P(m, "sb_model.fc_output_layer.weight"); b.w.fc_b = P(m, "sb_model.fc_output_layer.bias");
+        b.L = L; b.H = c.sb_hidden; b.I = m->Isb; b.Ipad = 64; b.rows = B * F; b.Tp = K;
+        b.img = static_cast<const __half*>(x.ximg.p); b.ntiles = (B * F + 127) / 128;
+        b.cstate = static_cast<float*>(st->c_sb.p); b.rows_alloc = st->ra_sb;
+        b.out = d_mask; b.O = c.output_size; b.F = F; b.la = 0; b.act = c.sb_act; b.fast = c.fast_math; b.gru = c.rnn_type == FSN_RNN_GRU;
+        b.hstate = static_cast<__half*>(st->h_sb.p); b.resume = resume; b.slot = slot; b.slot_rows = F; b.slot_la = c.look_ahead;
+        e = launch_lstm_mma(b, s);
+        if (e) return fail(FSN_ECUDA, "sub-band LSTM step failed: %s", cudaGetErrorString((cudaError_t)e));
+    } else if (!lw->nact) {
+        StreamChunkScatterLaunch sc{nullptr, d_mask, slot, lw->idx, 0, 0, B, F, K, c.look_ahead, 1};
+        launch_stream_chunk_scatter(sc, s);
+    } else {
+        // layer-wise sub band: the stepping sessions only, compacted to rows j F + f, in sub-batches of p.Bs sessions and windows of
+        // p.Tw frames.  The recurrence runs as window t0 = 4 + w0 of a 4 + K step sequence with la = 4: it loads h / c from the carry
+        // (t0 > 0), its parities are those of a launch from 0 (t0 % 4 == 0), and local frame k is output column k of [bs, 2, F, K]
+        const int H = c.sb_hidden, bs_max = lw->p.Bs, tw_max = lw->p.Tw ? lw->p.Tw : K;
+        for (int j0 = 0; j0 < lw->nact; j0 += bs_max) {
+            const int bs = lw->nact - j0 < bs_max ? lw->nact - j0 : bs_max, nt = (bs * F + 127) / 128;
+            const size_t cs_layer = lstm_tc5r_cstate_bytes(nt, H) / sizeof(float), hs_layer = (size_t)(nt + 1) / 2 * 2 * 128 * H;
+            StreamSbCarryLaunch cy{static_cast<__half*>(st->h_sb.p), static_cast<float*>(st->c_sb.p), st->ra_sb,
+                                   static_cast<__half*>(st->c_h.p), hs_layer, static_cast<float*>(st->c_c.p), cs_layer, lw->sess + j0, bs, F, H, L, 0};
+            launch_stream_sb_carry(cy, s);
+            for (int w0 = 0; w0 < K; w0 += tw_max) {
+                const int tw = K - w0 < tw_max ? K - w0 : tw_max;
+                pa.k0 = w0; pa.Kw = tw; pa.idx = lw->idx; pa.j0 = j0; pa.nsess = bs;
+                launch_stream_pack(pa, s);
+                LstmTc5rLaunch a{};
+                a.rows = bs * F; a.Tp = 4 + K; a.ntiles = nt; a.t0 = 4 + w0; a.Tw = tw;
+                a.ximg = static_cast<const __half*>(x.ximg.p); a.hseq = static_cast<__half*>(st->c_hsb.p);
+                a.cstate = static_cast<float*>(st->c_c.p); a.hstate = static_cast<__half*>(st->c_h.p);
+                a.out = static_cast<float*>(st->c_mask.p); a.la = 4;
+                if (int nl = sb_layers(m, a, static_cast<__half*>(st->c_gin.p), cs_layer, hs_layer, s); nl < 0) return nl;
+            }
+            cy.out = 1;
+            launch_stream_sb_carry(cy, s);
+            StreamChunkScatterLaunch sc{static_cast<const float*>(st->c_mask.p), d_mask, slot, lw->idx, j0, bs, B, F, K, c.look_ahead, j0 == 0};
+            launch_stream_chunk_scatter(sc, s);
+        }
+    }
     CK(cudaGetLastError());
-    st->n++;
-    return FSN_OK;
-}
-
-extern "C" int fsn_stream_step_slots(fsn_stream* st, const float* d_mag, float* d_mask, const int32_t* h_flags, int32_t* h_valid,
-                                     void* stream) {
-    if (!st || !d_mag || !d_mask) return fail(FSN_EINVAL, "null argument");
-    if (!h_flags) return fail(FSN_EINVAL, "h_flags is null (one flag per slot, slots 0..%d)", st->B - 1);
-    if (!h_valid) return fail(FSN_EINVAL, "h_valid is null (one result per slot, slots 0..%d)", st->B - 1);
-    const int B = st->B, la = st->m->cfg.look_ahead;
-    bool reset = false;
-    for (int b = 0; b < B; ++b) {
-        const int f = h_flags[b];
-        if (f != FSN_SLOT_HOLD && f != FSN_SLOT_STEP && f != FSN_SLOT_START)
-            return fail(FSN_EINVAL, "slot %d: flag %d is not FSN_SLOT_HOLD (0), FSN_SLOT_STEP (1) or FSN_SLOT_START (2)", b, f);
-        reset = reset || f == FSN_SLOT_START;
-    }
-    if (int rc = claim_mode(st, FSN_STATE_MODE_MASK)) return rc;
-    use_slot_counts(st);
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    int32_t* cnt = nullptr;                                             // [B] counts, then the slots this tick's START zeroes
-    if (int rc = st->stage.take((size_t)2 * B, &cnt)) return rc;
-    int nzero = 0;
-    for (int b = 0; b < B; ++b) {
-        cnt[b] = h_flags[b] == FSN_SLOT_HOLD ? -1 : h_flags[b] == FSN_SLOT_START ? 0 : st->nb[b];
-        if (reset && cnt[b] == 0) cnt[B + nzero++] = b;                 // started, or never stepped
-    }
-    const int* d = static_cast<const int*>(st->d_slot.p);
-    if (int rc = st->stage.send(st->d_slot.p, (size_t)B + nzero, s)) return rc;
-    if (int rc = stream_tick(st, d_mag, d_mask, d, d + B, nzero, s)) return rc;
-    for (int b = 0; b < B; ++b) {
-        if (cnt[b] >= 0) st->nb[b] = cnt[b] + 1;
-        h_valid[b] = cnt[b] >= 0 && st->nb[b] > la ? 1 : 0;
-    }
+    st->n += K;
     return FSN_OK;
 }
 
@@ -2112,7 +2153,7 @@ extern "C" int fsn_stream_step(fsn_stream* st, const float* d_mag, float* d_mask
         return FSN_OK;
     }
     const int n = st->n;
-    const int rc = stream_tick(st, d_mag, d_mask, nullptr, nullptr, 0, static_cast<cudaStream_t>(stream));
+    const int rc = step_frames(st, st->tick, d_mag, 1, nullptr, nullptr, 0, d_mask, nullptr, static_cast<cudaStream_t>(stream));
     if (rc) return rc;
     if (h_valid) *h_valid = (n >= st->m->cfg.look_ahead) ? 1 : 0;
     return FSN_OK;
@@ -2184,16 +2225,13 @@ extern "C" int fsn_stream_chunk_plan(const fsn_config* cfg, int32_t n_active, in
     return FSN_OK;
 }
 
-extern "C" int fsn_stream_step_chunk(fsn_stream* st, const float* d_mag, int32_t K, float* d_mask, const int32_t* h_flags,
-                                     int32_t* h_valid, void* stream) {
-    if (!st) return fail(FSN_EINVAL, "st is null");
-    if (!d_mag) return fail(FSN_EINVAL, "d_mag is null (K magnitude frames per slot, [B, F, K] float32 on the device)");
-    if (!d_mask) return fail(FSN_EINVAL, "d_mask is null (K mask columns per slot, [B, 2, F, K] float32 on the device)");
-    if (!h_flags) return fail(FSN_EINVAL, "h_flags is null (one flag per slot, slots 0..%d)", st->B - 1);
-    if (!h_valid) return fail(FSN_EINVAL, "h_valid is null (one result per slot, slots 0..%d)", st->B - 1);
+// The slot calls after their argument checks: every slot advances K frames by its flag (fsn_stream_step_slots: K = 1 on the per-tick
+// scratch; the chunk call: on its own scratch, with the layer-wise sub band where the offline forward runs it).  Errors change no state.
+static int step_slots(fsn_stream* st, const float* d_mag, int K, float* d_mask, const int32_t* h_flags, int32_t* h_valid, bool chunk,
+                      cudaStream_t s) {
     fsn_model* m = st->m;
     const fsn_config& c = m->cfg;
-    const int B = st->B, F = c.num_freqs, la = c.look_ahead, H = c.sb_hidden, L = c.num_layers;
+    const int B = st->B, F = c.num_freqs, la = c.look_ahead;
     if (int rc = chunk_check(c, K)) return rc;
     int nact = 0;
     bool reset = false;
@@ -2205,147 +2243,47 @@ extern "C" int fsn_stream_step_chunk(fsn_stream* st, const float* d_mag, int32_t
         reset = reset || f == FSN_SLOT_START;
     }
     if (st->mode == FSN_STATE_MODE_AUDIO) return claim_mode(st, FSN_STATE_MODE_MASK);
-    const bool lw = runs_layerwise(c, m->env_impl);
-    Plan p{nact};
-    if (lw && nact)
-        if (int rc = chunk_plan(c, true, nact, K, m->ws_cap_bytes, &p)) return rc;
+    const bool layerwise = chunk && runs_layerwise(c, m->env_impl);
+    LwSessions lw{Plan{nact}, nact};
+    if (layerwise && nact)
+        if (int rc = chunk_plan(c, true, nact, K, m->ws_cap_bytes, &lw.p)) return rc;
     // the scratch, before any state changes (DevBuf::ensure only grows)
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    const int Pk = (K + 3) & ~3, ntiles = (B * F + 127) / 128;
-    int e = st->c_fbin.ensure((size_t)B * F * Pk * 4, false, s);
-    e |= st->c_fbout.ensure((size_t)B * F * Pk * 4, false, s);
-    e |= st->c_fbx.ensure((size_t)K * st->rows_pad * st->Ipad * 2, false, s);
-    e |= st->c_hseq.ensure((size_t)B * c.fb_hidden * Pk * 4, false, s);
-    e |= st->c_slot.ensure((size_t)4 * B * sizeof(int32_t), false, s);
-    if (!lw) {
-        e |= st->c_ximg.ensure((size_t)ntiles * K * 16384, true, s);
-    } else if (nact) {
-        const int tw = p.Tw ? p.Tw : K, nt = (p.Bs * F + 127) / 128;
-        const WsSizes z = ws_sizes(c, true, p.Bs, K, tw);
-        e |= st->c_ximg.ensure(z.ximg, true, s);
+    StepScratch& x = chunk ? st->chunk : st->tick;
+    int e = 0;
+    if (!layerwise || !nact) {
+        e = x.ensure(*st, K, layerwise ? 0 : step_img_bytes((long long)B * F, K), false, s);
+    } else {
+        const int nt = (lw.p.Bs * F + 127) / 128;
+        const WsSizes z = ws_sizes(c, true, lw.p.Bs, K, lw.p.Tw ? lw.p.Tw : K);
+        e = x.ensure(*st, K, z.ximg, false, s);
         e |= st->c_gin.ensure(z.r_gin, false, s);
         e |= st->c_hsb.ensure(z.r_hseq, false, s);
         e |= st->c_h.ensure(z.r_hstate, true, s);
-        e |= st->c_c.ensure((size_t)L * lstm_tc5r_cstate_bytes(nt, H), true, s);
-        e |= st->c_mask.ensure((size_t)p.Bs * 2 * F * K * sizeof(float), false, s);
+        e |= st->c_c.ensure((size_t)c.num_layers * lstm_tc5r_cstate_bytes(nt, c.sb_hidden), true, s);
+        e |= st->c_mask.ensure((size_t)lw.p.Bs * 2 * F * K * sizeof(float), false, s);
     }
     if (e) return fail(FSN_ECUDA, "chunk scratch allocation failed (B = %d, K = %d)", B, K);
     if (int rc = claim_mode(st, FSN_STATE_MODE_MASK)) return rc;
     use_slot_counts(st);
-    // staged per-slot values: counts [B] (-1 = held), active-session index [B] (-1 = held), the active slots [nact], the START list
+    // staged per-slot values: counts [B] (-1 = held); on the layer-wise path each slot's session index [B] (-1 = held) and the
+    // stepping slots [nact]; then the START list
     int32_t* h = nullptr;
     if (int rc = st->stage.take((size_t)4 * B, &h)) return rc;
-    int32_t *cnt = h, *idx = h + B, *sess = h + 2 * B, *zero = sess + nact;
+    const int nlw = layerwise ? B + nact : 0;
+    int32_t *cnt = h, *idx = h + B, *sess = h + 2 * B, *zero = h + B + nlw;
     int nzero = 0;
     for (int b = 0, j = 0; b < B; ++b) {
         cnt[b] = h_flags[b] == FSN_SLOT_HOLD ? -1 : h_flags[b] == FSN_SLOT_START ? 0 : st->nb[b];
-        idx[b] = cnt[b] >= 0 ? j : -1;
-        if (cnt[b] >= 0) sess[j++] = b;
+        if (layerwise) {
+            idx[b] = cnt[b] >= 0 ? j : -1;
+            if (cnt[b] >= 0) sess[j++] = b;
+        }
         if (reset && cnt[b] == 0) zero[nzero++] = b;                    // started, or never stepped
     }
-    const int* d = static_cast<const int*>(st->c_slot.p);
-    const int *d_cnt = d, *d_idx = d + B, *d_sess = d + 2 * B, *d_zero = d + 2 * B + nact;
-    if (int rc = st->stage.send(st->c_slot.p, (size_t)2 * B + nact + nzero, s)) return rc;
-    if (nzero) {
-        StreamStateLaunch z{};
-        state_launch(st, NSEG, ST_START, nullptr, z);
-        z.slots = d_zero; z.n = nzero; z.dir = STREAM_STATE_ZERO;
-        if (int e2 = launch_stream_state(z, s)) return fail(FSN_ECUDA, "session state reset failed: %s", cudaGetErrorString((cudaError_t)e2));
-    }
-    // full band: every slot, K frames per launch (held slots keep their state)
-    StreamNormChunkLaunch na{d_mag, static_cast<float*>(st->c_fbin.p), static_cast<double*>(st->cum_in.p), B, F, K, Pk, c.norm_type, d_cnt};
-    launch_stream_norm_chunk(na, s);
-    launch_fb_pack(static_cast<const float*>(st->c_fbin.p), static_cast<__half*>(st->c_fbx.p), B, F, K, Pk, st->rows_pad, st->Ipad, s);
-    if (st->use_ws) {
-        LstmWsLaunch w{};
-        fill_ws(m, w);
-        w.rows = B; w.rows_pad = st->rows_pad; w.Tp = K;
-        w.x = static_cast<const __half*>(st->c_fbx.p); w.hbuf = static_cast<__half*>(st->ws_h.p); w.cbuf = static_cast<float*>(st->ws_c.p);
-        w.barrier = static_cast<unsigned int*>(st->ws_bar.p);
-        w.hseq = static_cast<float*>(st->c_hseq.p); w.P = Pk; w.resume = 1; w.t0 = st->n; w.slot = d_cnt;
-        e = launch_lstm_ws(w, s);
-    } else {
-        LstmMmaLaunch a{};
-        for (int l = 0; l < L; ++l) { a.w.wfrag[l] = static_cast<const uint4*>(m->fb_frag[l].p); a.w.bias[l] = static_cast<const float*>(m->fb_bias[l].p); }
-        a.L = L; a.H = c.fb_hidden; a.I = F; a.Ipad = st->Ipad; a.rows = B; a.Tp = K;
-        a.xplain = static_cast<const __half*>(st->c_fbx.p); a.rows_pad = st->rows_pad;
-        a.cstate = static_cast<float*>(st->c_fb.p); a.rows_alloc = st->ra_fb;
-        a.hseq = static_cast<float*>(st->c_hseq.p); a.P = Pk; a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU;
-        a.hstate = static_cast<__half*>(st->h_fb.p); a.resume = 1; a.slot = d_cnt; a.slot_rows = 1;
-        e = launch_lstm_mma(a, s);
-    }
-    if (e) return fail(FSN_ECUDA, "full-band LSTM chunk failed: %s", cudaGetErrorString((cudaError_t)e));
-    ConvLaunch cf{};
-    cf.X = static_cast<const float*>(st->c_hseq.p); cf.Y = static_cast<float*>(st->c_fbout.p);
-    cf.Z = B; cf.M = F; cf.K = c.fb_hidden; cf.Tp = K; cf.P = Pk; cf.act = c.fb_act;
-    cf.W = P(m, "fb_model.fc_output_layer.weight"); cf.bias = P(m, "fb_model.fc_output_layer.bias");
-    launch_conv1x1(cf, s);
-    StreamPackChunkLaunch pa{d_mag, static_cast<const float*>(st->c_fbout.p), Pk, static_cast<double*>(st->cum_sb.p),
-                             static_cast<__half*>(st->c_ximg.p), B, F, K, c.sb_num_neighbors, c.fb_num_neighbors, c.norm_type, 0, K, d_cnt,
-                             nullptr, 0, 0};
-    if (!lw) {
-        // generic sub band: the per-frame step's kernel and state, in place over every slot, K steps
-        launch_stream_pack_chunk(pa, s);
-        LstmMmaLaunch b{};
-        for (int l = 0; l < L; ++l) { b.w.wfrag[l] = static_cast<const uint4*>(m->sb_frag[l].p); b.w.bias[l] = static_cast<const float*>(m->sb_bias[l].p); }
-        b.w.fc_w = P(m, "sb_model.fc_output_layer.weight"); b.w.fc_b = P(m, "sb_model.fc_output_layer.bias");
-        b.L = L; b.H = H; b.I = m->Isb; b.Ipad = 64; b.rows = B * F; b.Tp = K;
-        b.img = static_cast<const __half*>(st->c_ximg.p); b.ntiles = ntiles;
-        b.cstate = static_cast<float*>(st->c_sb.p); b.rows_alloc = st->ra_sb;
-        b.out = d_mask; b.O = c.output_size; b.F = F; b.la = 0; b.act = c.sb_act; b.fast = c.fast_math; b.gru = c.rnn_type == FSN_RNN_GRU;
-        b.hstate = static_cast<__half*>(st->h_sb.p); b.resume = 1; b.slot = d_cnt; b.slot_rows = F; b.slot_la = la;
-        e = launch_lstm_mma(b, s);
-        if (e) return fail(FSN_ECUDA, "sub-band LSTM chunk failed: %s", cudaGetErrorString((cudaError_t)e));
-    } else if (!nact) {
-        StreamChunkScatterLaunch sc{nullptr, d_mask, d_cnt, d_idx, 0, 0, B, F, K, la, 1};
-        launch_stream_chunk_scatter(sc, s);
-    } else {
-        // layer-wise sub band: the stepping sessions only, compacted to rows j F + f, in sub-batches of p.Bs sessions and windows of
-        // p.Tw frames.  The recurrence runs as window t0 = 4 + w0 of a 4 + K step sequence with la = 4: it loads h / c from the carry
-        // (t0 > 0), its parities are those of a launch from 0 (t0 % 4 == 0), and local frame k is output column k of [bs, 2, F, K]
-        const int tw_max = p.Tw ? p.Tw : K;
-        for (int j0 = 0; j0 < nact; j0 += p.Bs) {
-            const int bs = nact - j0 < p.Bs ? nact - j0 : p.Bs, srows = bs * F, nt = (srows + 127) / 128, ntp = (nt + 1) / 2 * 2;
-            const size_t cs_layer = lstm_tc5r_cstate_bytes(nt, H) / sizeof(float), hs_layer = (size_t)ntp * 128 * H;
-            StreamSbCarryLaunch cy{static_cast<__half*>(st->h_sb.p), static_cast<float*>(st->c_sb.p), st->ra_sb,
-                                   static_cast<__half*>(st->c_h.p), hs_layer, static_cast<float*>(st->c_c.p), cs_layer, d_sess + j0, bs, F, H, L, 0};
-            launch_stream_sb_carry(cy, s);
-            for (int w0 = 0; w0 < K; w0 += tw_max) {
-                const int tw = K - w0 < tw_max ? K - w0 : tw_max;
-                pa.k0 = w0; pa.Kw = tw; pa.idx = d_idx; pa.j0 = j0; pa.nsess = bs;
-                launch_stream_pack_chunk(pa, s);
-                for (int l = 0; l < L; ++l) {
-                    if (l > 0) {
-                        GemmF16Launch g{(long long)ntp * tw * 128, 4 * H, H, static_cast<__half*>(st->c_gin.p), 4LL * H, m->env_gin_tile_n};
-                        const int ge = launch_gemm_f16(st->c_hsb.p, m->r_wih[l].p, g, m->num_sms, s);
-                        if (ge) return fail(FSN_ECUDA, "input-projection GEMM launch failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)ge));
-                    }
-                    LstmTc5rLaunch a{};
-                    a.wstream = static_cast<const __half*>(m->r_stream[l].p);
-                    a.bias = static_cast<const float*>(m->r_bias[l].p);
-                    a.fc_w = P(m, "sb_model.fc_output_layer.weight");
-                    a.fc_b = P(m, "sb_model.fc_output_layer.bias");
-                    a.H = H; a.rows = srows; a.Tp = 4 + K; a.ntiles = nt;
-                    a.t0 = 4 + w0; a.Tw = tw;
-                    if (l == 0) a.ximg = static_cast<const __half*>(st->c_ximg.p);
-                    else a.gin = static_cast<const __half*>(st->c_gin.p);
-                    a.hseq = static_cast<__half*>(st->c_hsb.p);
-                    a.cstate = static_cast<float*>(st->c_c.p) + l * cs_layer;
-                    a.hstate = static_cast<__half*>(st->c_h.p) + l * hs_layer;
-                    a.out = static_cast<float*>(st->c_mask.p); a.F = F; a.la = 4;
-                    a.act = c.sb_act; a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU; a.last = (l == L - 1);
-                    const int le = launch_lstm_tc5r(a, s);
-                    if (le) return fail(FSN_ECUDA, "layer-wise LSTM chunk failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)le));
-                }
-            }
-            cy.out = 1;
-            launch_stream_sb_carry(cy, s);
-            StreamChunkScatterLaunch sc{static_cast<const float*>(st->c_mask.p), d_mask, d_cnt, d_idx, j0, bs, B, F, K, la, j0 == 0};
-            launch_stream_chunk_scatter(sc, s);
-        }
-    }
-    CK(cudaGetLastError());
-    st->n += K;
+    const int* d = static_cast<const int*>(st->d_slot.p);
+    if (int rc = st->stage.send(st->d_slot.p, (size_t)B + nlw + nzero, s)) return rc;
+    lw.idx = d + B; lw.sess = d + 2 * B;
+    if (int rc = step_frames(st, x, d_mag, K, d, d + B + nlw, nzero, d_mask, layerwise ? &lw : nullptr, s)) return rc;
     for (int b = 0; b < B; ++b) {
         h_valid[b] = 0;
         if (cnt[b] < 0) continue;
@@ -2354,6 +2292,24 @@ extern "C" int fsn_stream_step_chunk(fsn_stream* st, const float* d_mag, int32_t
         h_valid[b] = v < 0 ? 0 : v > K ? K : v;
     }
     return FSN_OK;
+}
+
+extern "C" int fsn_stream_step_slots(fsn_stream* st, const float* d_mag, float* d_mask, const int32_t* h_flags, int32_t* h_valid,
+                                     void* stream) {
+    if (!st || !d_mag || !d_mask) return fail(FSN_EINVAL, "null argument");
+    if (!h_flags) return fail(FSN_EINVAL, "h_flags is null (one flag per slot, slots 0..%d)", st->B - 1);
+    if (!h_valid) return fail(FSN_EINVAL, "h_valid is null (one result per slot, slots 0..%d)", st->B - 1);
+    return step_slots(st, d_mag, 1, d_mask, h_flags, h_valid, false, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int fsn_stream_step_chunk(fsn_stream* st, const float* d_mag, int32_t K, float* d_mask, const int32_t* h_flags,
+                                     int32_t* h_valid, void* stream) {
+    if (!st) return fail(FSN_EINVAL, "st is null");
+    if (!d_mag) return fail(FSN_EINVAL, "d_mag is null (K magnitude frames per slot, [B, F, K] float32 on the device)");
+    if (!d_mask) return fail(FSN_EINVAL, "d_mask is null (K mask columns per slot, [B, 2, F, K] float32 on the device)");
+    if (!h_flags) return fail(FSN_EINVAL, "h_flags is null (one flag per slot, slots 0..%d)", st->B - 1);
+    if (!h_valid) return fail(FSN_EINVAL, "h_valid is null (one result per slot, slots 0..%d)", st->B - 1);
+    return step_slots(st, d_mag, K, d_mask, h_flags, h_valid, true, static_cast<cudaStream_t>(stream));
 }
 
 // Audio state of the handle and its scratch, zero-filled on the call's stream, and the tables of its n_fft (computed in double).
@@ -2436,7 +2392,7 @@ extern "C" int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_sample
     a.window = tab.window; a.twiddle = tab.twiddle; a.inv_env = tab.inv_env;
     a.B = B; a.n_fft = N; a.la = la;
     launch_stream_stft(a, s);
-    const int rc = stream_tick(st, a.mag, mask, d, d + 4 * B, nzero, s);
+    const int rc = step_frames(st, st->tick, a.mag, 1, d, d + 4 * B, nzero, mask, nullptr, s);
     if (rc) return rc;
     launch_stream_istft(a, s);
     CK(cudaGetLastError());

@@ -106,24 +106,19 @@ void launch_apply_cirm(const float* crm, const float2* noisy, float2* enh, int B
 void launch_apply_cirm_planar(const float* crm, const float* nreal, const float* nimag, float2* enh, int B, int F, int T, const int* tlen,
                               int la, cudaStream_t s);
 
-// streaming step kernels (k_front.cu): one frame of the cumulative norms with running sums carried in global memory.
-// slot: null (every slot is at frame n), or [B] per-slot frame counts of the slot call (fsn_stream_step_slots), -1 = held: a held
-// slot's frame is not read, its sums are untouched and its outputs are zero
-struct StreamNormLaunch { const float* x; float* y; double* cum; int B, F, P, n, type; const int* slot; };       // x [B,F] -> y [B,F,P] (t = 0)
+// streaming step kernels (k_front.cu): K frames of the cumulative norms with running sums carried in global memory, frame after
+// frame.  slot: null (every slot is at frame n), or [B] per-slot frame counts of the slot calls, -1 = held: a held slot's frames are
+// not read, its sums are untouched and its outputs are zero.  x [B, F, K] -> y [B, F, P] (frames at columns 0 .. K - 1)
+struct StreamNormLaunch { const float* x; float* y; double* cum; int B, F, K, P, n, type; const int* slot; };
 void launch_stream_norm(const StreamNormLaunch& a, cudaStream_t s);
-struct StreamPackLaunch { const float* mag; const float* fb; int Pfb; double* cum; __half* ximg; int B, F, Ns, Nf, n, type; const int* slot; };
-void launch_stream_pack(const StreamPackLaunch& a, cudaStream_t s);
-// K-frame forms (fsn_stream_step_chunk): the one-frame arithmetic frame after frame; slot [B] per-slot counts (-1 = held) is required.
-// x [B, F, K] -> y [B, F, P] (frames at columns 0 .. K - 1)
-struct StreamNormChunkLaunch { const float* x; float* y; double* cum; int B, F, K, P, type; const int* slot; };
-void launch_stream_norm_chunk(const StreamNormChunkLaunch& a, cudaStream_t s);
 // frames k0 .. k0 + Kw - 1 of mag [B, F, K] and fb [B, F, Pfb] -> images [tile, Kw, 128 rows, 64 halves].  idx null: row b F + f,
-// held rows zero.  idx [B]: row (idx[b] - j0) F + f for the sessions j0 .. j0 + nsess - 1 of a sub-batch, nothing for any other slot
-struct StreamPackChunkLaunch {
-    const float* mag; const float* fb; int Pfb; double* cum; __half* ximg; int B, F, K, Ns, Nf, type, k0, Kw; const int* slot;
+// held rows zero.  idx [B]: row (idx[b] - j0) F + f for the sessions j0 .. j0 + nsess - 1 of a sub-batch, nothing for any other slot.
+// K = 1 with idx null runs a one-frame kernel with the same arithmetic in fewer registers (faster at 1024 slots)
+struct StreamPackLaunch {
+    const float* mag; const float* fb; int Pfb; double* cum; __half* ximg; int B, F, K, Ns, Nf, n, type, k0, Kw; const int* slot;
     const int* idx; int j0, nsess;
 };
-void launch_stream_pack_chunk(const StreamPackChunkLaunch& a, cudaStream_t s);
+void launch_stream_pack(const StreamPackLaunch& a, cudaStream_t s);
 // compact masks src [nsess, 2, F, K] of the sessions j0 .. j0 + nsess - 1 -> dst [B, 2, F, K] at their slots (idx[b] - j0), leading
 // columns with slot[b] + k < la zero; zero_held: also zero the rows of held slots
 struct StreamChunkScatterLaunch { const float* src; float* dst; const int* slot; const int* idx; int j0, nsess, B, F, K, la, zero_held; };

@@ -657,87 +657,15 @@ void launch_tm_to_fm(const float* x, int ld, float* y, int Z, int C, int Tp, cud
 
 
 // =============================================================================================
-// Streaming (frame-by-frame) forms of the cumulative norms: the running sums live in global memory (fp64) and one
-// launch handles frame n.  reference: base_model.py:227-258 / :277-316 evaluated one column at a time.
+// Streaming forms of the cumulative norms: the running sums live in global memory (fp64) and one launch handles K frames of every
+// slot, frame after frame, with the same reduction order and running sums for each frame -- so one launch over K frames writes the
+// bits K launches of one frame write.  reference: base_model.py:227-258 / :277-316 evaluated one column at a time.
+// Frame k of slot b is its frame n0 + k, n0 = slot[b] (or n when slot is null).
 // =============================================================================================
 __global__ void __launch_bounds__(256) stream_norm_kernel(StreamNormLaunch a) {
     __shared__ double red[16];
     __shared__ float s_a, s_b;
-    const int b = blockIdx.x, F = a.F;
-    const int n = a.slot ? a.slot[b] : a.n;                         // this slot's frame count (block-uniform)
-    if (n < 0) {                                                    // held: frame unread, sums untouched
-        for (int f = threadIdx.x; f < F; f += blockDim.x) a.y[((size_t)b * F + f) * a.P] = 0.f;
-        return;
-    }
-    const float* x = a.x + (size_t)b * F;
-    double s = 0, q = 0;
-    for (int f = threadIdx.x; f < F; f += blockDim.x) { const double v = x[f]; s += v; q += v * v; }
-    s = warp_sum_d(s); q = warp_sum_d(q);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (lane == 0) { red[warp] = s; red[8 + warp] = q; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double ts = 0, tq = 0;
-        for (int i = 0; i < 8; ++i) { ts += red[i]; tq += red[8 + i]; }
-        const double EPS = 1.1920928955078125e-07;
-        const double cs = (n == 0 ? 0.0 : a.cum[2 * b]) + ts, cq = (n == 0 ? 0.0 : a.cum[2 * b + 1]) + tq;
-        a.cum[2 * b] = cs; a.cum[2 * b + 1] = cq;
-        const double cnt = (double)F * (n + 1), cm = cs / cnt;
-        if (a.type == FSN_NORM_CUMULATIVE_LAPLACE) { s_a = (float)(1.0 / (cm + EPS)); s_b = 0.f; }
-        else { const double cv = (cq - 2.0 * cm * cs) / cnt + cm * cm, inv = 1.0 / sqrt(cv + EPS); s_a = (float)inv; s_b = (float)(-cm * inv); }
-    }
-    __syncthreads();
-    for (int f = threadIdx.x; f < F; f += blockDim.x) a.y[((size_t)b * F + f) * a.P] = fmaf(x[f], s_a, s_b);
-}
-void launch_stream_norm(const StreamNormLaunch& a, cudaStream_t s) { stream_norm_kernel<<<a.B, 256, 0, s>>>(a); }
-
-// one frame of the sub-band input with the per-sequence cumulative norm; thread = sequence (b, f)
-__global__ void __launch_bounds__(128) stream_pack_kernel(StreamPackLaunch a) {
-    const int row = blockIdx.x * blockDim.x + threadIdx.x, F = a.F;
-    if (row >= a.B * F) return;
-    const int b = row / F, f = row % F, tile = row >> 7, r = row & 127;
-    const int nw = 2 * a.Ns + 1, nf = 2 * a.Nf + 1, I = nw + nf;
-    char* img = reinterpret_cast<char*>(a.ximg) + (size_t)tile * (128 * 128);
-    const int n = a.slot ? a.slot[b] : a.n;                         // the frame count of this row's slot
-    if (n < 0) {                                                    // held: frame unread, sums untouched, zero input row
-#pragma unroll
-        for (int c = 0; c < 8; ++c) *reinterpret_cast<uint4*>(img + sw128_offset(r, c * 8)) = make_uint4(0u, 0u, 0u, 0u);
-        return;
-    }
-    float v[64];
-    double s = 0, q = 0;
-#pragma unroll
-    for (int k = 0; k < 64; ++k) {
-        float x = 0.f;
-        if (k < nw) x = a.mag[(size_t)b * F + reflect_idx(f + k - a.Ns, F)];
-        else if (k < I) x = a.fb[((size_t)b * F + reflect_idx(f + (k - nw) - a.Nf, F)) * a.Pfb];
-        v[k] = x; s += x; q += (double)x * x;
-    }
-    const double EPS = 1.1920928955078125e-07;
-    const double cs = (n == 0 ? 0.0 : a.cum[2 * row]) + s, cq = (n == 0 ? 0.0 : a.cum[2 * row + 1]) + q;
-    a.cum[2 * row] = cs; a.cum[2 * row + 1] = cq;
-    const double cnt = (double)I * (n + 1), cm = cs / cnt;
-    float sc, sh;
-    if (a.type == FSN_NORM_CUMULATIVE_LAPLACE) { sc = (float)(1.0 / (cm + EPS)); sh = 0.f; }
-    else { const double cv = (cq - 2.0 * cm * cs) / cnt + cm * cm, inv = 1.0 / sqrt(cv + EPS); sc = (float)inv; sh = (float)(-cm * inv); }
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-        float w[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) w[i] = (c * 8 + i < I) ? fminf(fmaxf(fmaf(v[c * 8 + i], sc, sh), -65504.f), 65504.f) : 0.f;
-        *reinterpret_cast<uint4*>(img + sw128_offset(r, c * 8)) =
-            make_uint4(pack_half2(w[0], w[1]), pack_half2(w[2], w[3]), pack_half2(w[4], w[5]), pack_half2(w[6], w[7]));
-    }
-}
-void launch_stream_pack(const StreamPackLaunch& a, cudaStream_t s) { stream_pack_kernel<<<(a.B * a.F + 127) / 128, 128, 0, s>>>(a); }
-
-// K-frame forms of the two kernels above (fsn_stream_step_chunk, DESIGN.md §3.13).  Every frame runs exactly the one-frame kernel's
-// arithmetic -- the same reduction order and the same fp64 running sums, frame after frame -- so one launch over K frames writes the
-// bits K one-frame launches write.  Frame k of slot b is its frame slot[b] + k.
-__global__ void __launch_bounds__(256) stream_norm_chunk_kernel(StreamNormChunkLaunch a) {
-    __shared__ double red[16];
-    __shared__ float s_a, s_b;
-    const int b = blockIdx.x, F = a.F, n0 = a.slot[b];
+    const int b = blockIdx.x, F = a.F, n0 = a.slot ? a.slot[b] : a.n;
     if (n0 < 0) {                                                   // held: frames unread, sums untouched, zero rows
         for (int i = threadIdx.x; i < F * a.K; i += blockDim.x) a.y[((size_t)b * F + i / a.K) * a.P + i % a.K] = 0.f;
         return;
@@ -768,15 +696,15 @@ __global__ void __launch_bounds__(256) stream_norm_chunk_kernel(StreamNormChunkL
     }
     if (threadIdx.x == 0) { a.cum[2 * b] = cs; a.cum[2 * b + 1] = cq; }
 }
-void launch_stream_norm_chunk(const StreamNormChunkLaunch& a, cudaStream_t s) { stream_norm_chunk_kernel<<<a.B, 256, 0, s>>>(a); }
+void launch_stream_norm(const StreamNormLaunch& a, cudaStream_t s) { stream_norm_kernel<<<a.B, 256, 0, s>>>(a); }
 
 // thread = sequence (b, f); frames k0 .. k0 + Kw - 1 of the chunk into the window-local images [tile, Kw, 128, 64]
-__global__ void __launch_bounds__(128) stream_pack_chunk_kernel(StreamPackChunkLaunch a) {
+__global__ void __launch_bounds__(128) stream_pack_kernel(StreamPackLaunch a) {
     const int row = blockIdx.x * blockDim.x + threadIdx.x, F = a.F;
     if (row >= a.B * F) return;
     const int b = row / F, f = row % F;
     const int nw = 2 * a.Ns + 1, nf = 2 * a.Nf + 1, I = nw + nf;
-    const int n0 = a.slot[b];
+    const int n0 = a.slot ? a.slot[b] : a.n;
     int crow = row;                                                 // the row of the images
     if (a.idx) {                                                    // compact rows: session idx[b] - j0 of this sub-batch, or not packed
         const int j = n0 < 0 ? -1 : a.idx[b] - a.j0;
@@ -825,8 +753,49 @@ __global__ void __launch_bounds__(128) stream_pack_chunk_kernel(StreamPackChunkL
     }
     a.cum[2 * row] = cs; a.cum[2 * row + 1] = cq;
 }
-void launch_stream_pack_chunk(const StreamPackChunkLaunch& a, cudaStream_t s) {
-    stream_pack_chunk_kernel<<<(a.B * a.F + 127) / 128, 128, 0, s>>>(a);
+// The same for one frame (K = 1, no compact rows): the arithmetic above without the frame loop, in 96 registers instead of 120; at
+// 1024 slots it runs 49 us per tick where the K-frame kernel at K = 1 takes 55 us (H100 80GB HBM3, 700 W; DESIGN.md §4)
+__global__ void __launch_bounds__(128) stream_pack_frame_kernel(StreamPackLaunch a) {
+    const int row = blockIdx.x * blockDim.x + threadIdx.x, F = a.F;
+    if (row >= a.B * F) return;
+    const int b = row / F, f = row % F, tile = row >> 7, r = row & 127;
+    const int nw = 2 * a.Ns + 1, nf = 2 * a.Nf + 1, I = nw + nf;
+    char* img = reinterpret_cast<char*>(a.ximg) + (size_t)tile * (128 * 128);
+    const int n = a.slot ? a.slot[b] : a.n;                         // the frame count of this row's slot
+    if (n < 0) {                                                    // held: frame unread, sums untouched, zero input row
+#pragma unroll
+        for (int c = 0; c < 8; ++c) *reinterpret_cast<uint4*>(img + sw128_offset(r, c * 8)) = make_uint4(0u, 0u, 0u, 0u);
+        return;
+    }
+    float v[64];
+    double s = 0, q = 0;
+#pragma unroll
+    for (int k = 0; k < 64; ++k) {
+        float x = 0.f;
+        if (k < nw) x = a.mag[(size_t)b * F + reflect_idx(f + k - a.Ns, F)];
+        else if (k < I) x = a.fb[((size_t)b * F + reflect_idx(f + (k - nw) - a.Nf, F)) * a.Pfb];
+        v[k] = x; s += x; q += (double)x * x;
+    }
+    const double EPS = 1.1920928955078125e-07;
+    const double cs = (n == 0 ? 0.0 : a.cum[2 * row]) + s, cq = (n == 0 ? 0.0 : a.cum[2 * row + 1]) + q;
+    a.cum[2 * row] = cs; a.cum[2 * row + 1] = cq;
+    const double cnt = (double)I * (n + 1), cm = cs / cnt;
+    float sc, sh;
+    if (a.type == FSN_NORM_CUMULATIVE_LAPLACE) { sc = (float)(1.0 / (cm + EPS)); sh = 0.f; }
+    else { const double cv = (cq - 2.0 * cm * cs) / cnt + cm * cm, inv = 1.0 / sqrt(cv + EPS); sc = (float)inv; sh = (float)(-cm * inv); }
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+        float w[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) w[i] = (c * 8 + i < I) ? fminf(fmaxf(fmaf(v[c * 8 + i], sc, sh), -65504.f), 65504.f) : 0.f;
+        *reinterpret_cast<uint4*>(img + sw128_offset(r, c * 8)) =
+            make_uint4(pack_half2(w[0], w[1]), pack_half2(w[2], w[3]), pack_half2(w[4], w[5]), pack_half2(w[6], w[7]));
+    }
+}
+
+void launch_stream_pack(const StreamPackLaunch& a, cudaStream_t s) {
+    if (a.K == 1 && !a.idx) stream_pack_frame_kernel<<<(a.B * a.F + 127) / 128, 128, 0, s>>>(a);
+    else stream_pack_kernel<<<(a.B * a.F + 127) / 128, 128, 0, s>>>(a);
 }
 
 // The compact masks of one sub-batch [nsess, 2, F, K] into the slots' rows of d_mask [B, 2, F, K]: column k of slot b is the mask of

@@ -4,6 +4,7 @@
 #include "fsn_common.cuh"
 #include "fsn_kernels.h"
 
+#include <algorithm>
 #include <cstdarg>
 #include <cstddef>
 #include <cstdio>
@@ -1882,6 +1883,10 @@ struct fsn_stream {
     // sub-batch, and c_*: its Gin / layer output, the per-layer h / c carry and the compact masks
     StepScratch chunk;
     DevBuf c_gin, c_hsb, c_h, c_c, c_mask;
+    // audio chunk call (fsn_stream_step_audio_chunk, DESIGN.md §3.14): its scratch, allocated at its first use, grow-only: the spectra
+    // of the call's frames [B, K, F], the model's input and output planes (runs of columns, see StreamAudioChunkLaunch) and the
+    // staged per-slot plan
+    DevBuf x_spec, x_mag, x_mask, x_plan;
 };
 
 int StepScratch::ensure(const fsn_stream& st, int K, size_t img, bool zero, cudaStream_t s) {
@@ -2021,7 +2026,7 @@ extern "C" void fsn_stream_destroy(fsn_stream* st) {
     st->tick.release();
     st->chunk.release();
     for (DevBuf* b : {&st->ws_bar, &st->d_slot, &st->x_slot, &st->a_mag, &st->a_mask, &st->a_tab, &st->c_gin, &st->c_hsb, &st->c_h,
-                      &st->c_c, &st->c_mask})
+                      &st->c_c, &st->c_mask, &st->x_spec, &st->x_mag, &st->x_mask, &st->x_plan})
         b->release();
     delete st;
 }
@@ -2041,16 +2046,17 @@ static void use_slot_counts(fsn_stream* st) {
     st->slots = true;
 }
 
-// The layer-wise sub band of a chunk call (DESIGN.md §3.13): the plan of its nact stepping sessions, and on the device each slot's
-// session index (-1 = held) and the stepping slots
-struct LwSessions { Plan p; int nact; const int *idx, *sess; };
+// The layer-wise sub band of a chunk step (DESIGN.md §3.13, §3.14): its stepping sessions in groups of one frame count kf each.  Per
+// group: the plan of its nact sessions, and on the device each slot's session index in the group (-1 = not in it) and its slots
+struct LwGroup { Plan p; int nact, kf; const int *idx, *sess; };
 
-// K frames of every slot on scratch x (DESIGN.md §3.9, §3.13): d_mag [B, F, K] -> d_mask [B, 2, F, K].  slot: null (the lockstep step:
-// every slot at frame n) or the device per-slot counts (-1 = held); zero[nzero]: device list of the slots whose recurrent state is
-// zeroed first (a START's).  The full band runs in place over every slot; the sub band too (lw null: the per-frame step's kernel and
-// state), or on the layer-wise kernels over the stepping sessions only.
-static int step_frames(fsn_stream* st, StepScratch& x, const float* d_mag, int K, const int* slot, const int* zero, int nzero,
-                       float* d_mask, const LwSessions* lw, cudaStream_t s) {
+// K frames of every slot on scratch x (DESIGN.md §3.9, §3.13, §3.14): d_mag [B, F, K] -> d_mask [B, 2, F, K].  slot: null (the
+// lockstep step: every slot at frame n) or the device per-slot counts (-1 = held); kf: null (every stepping slot runs K frames) or the
+// device per-slot frame counts (a stepping slot runs frames 0 .. kf - 1 and holds after them); zero[nzero]: device list of the slots
+// whose recurrent state is zeroed first (a START's).  The full band runs in place over every slot; the sub band too (lw null: the
+// per-frame step's kernel and state), or on the layer-wise kernels over the stepping sessions only, one pass per frame-count group.
+static int step_frames(fsn_stream* st, StepScratch& x, const float* d_mag, int K, const int* slot, const int* kf, const int* zero,
+                       int nzero, float* d_mask, const std::vector<LwGroup>* lw, cudaStream_t s) {
     fsn_model* m = st->m;
     const fsn_config& c = m->cfg;
     const int B = st->B, F = c.num_freqs, L = c.num_layers, n = st->n, Pk = (K + 3) & ~3;
@@ -2061,7 +2067,7 @@ static int step_frames(fsn_stream* st, StepScratch& x, const float* d_mag, int K
         z.slots = zero; z.n = nzero; z.dir = STREAM_STATE_ZERO;
         if (int e = launch_stream_state(z, s)) return fail(FSN_ECUDA, "session state reset failed: %s", cudaGetErrorString((cudaError_t)e));
     }
-    StreamNormLaunch na{d_mag, static_cast<float*>(x.fbin.p), static_cast<double*>(st->cum_in.p), B, F, K, Pk, n, c.norm_type, slot};
+    StreamNormLaunch na{d_mag, static_cast<float*>(x.fbin.p), static_cast<double*>(st->cum_in.p), B, F, K, Pk, n, c.norm_type, slot, kf};
     launch_stream_norm(na, s);
     launch_fb_pack(static_cast<const float*>(x.fbin.p), static_cast<__half*>(x.fbx.p), B, F, K, Pk, st->rows_pad, st->Ipad, s);
     int e = 0;
@@ -2071,7 +2077,7 @@ static int step_frames(fsn_stream* st, StepScratch& x, const float* d_mag, int K
         w.rows = B; w.rows_pad = st->rows_pad; w.Tp = K;
         w.x = static_cast<const __half*>(x.fbx.p); w.hbuf = static_cast<__half*>(st->ws_h.p); w.cbuf = static_cast<float*>(st->ws_c.p);
         w.barrier = static_cast<unsigned int*>(st->ws_bar.p);
-        w.hseq = static_cast<float*>(x.hseq.p); w.P = Pk; w.resume = resume; w.t0 = n; w.slot = slot;
+        w.hseq = static_cast<float*>(x.hseq.p); w.P = Pk; w.resume = resume; w.t0 = n; w.slot = slot; w.kf = kf;
         e = launch_lstm_ws(w, s);
     } else {
         LstmMmaLaunch a{};
@@ -2080,7 +2086,7 @@ static int step_frames(fsn_stream* st, StepScratch& x, const float* d_mag, int K
         a.xplain = static_cast<const __half*>(x.fbx.p); a.rows_pad = st->rows_pad;
         a.cstate = static_cast<float*>(st->c_fb.p); a.rows_alloc = st->ra_fb;
         a.hseq = static_cast<float*>(x.hseq.p); a.P = Pk; a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU;
-        a.hstate = static_cast<__half*>(st->h_fb.p); a.resume = resume; a.slot = slot; a.slot_rows = 1;
+        a.hstate = static_cast<__half*>(st->h_fb.p); a.resume = resume; a.slot = slot; a.slot_rows = 1; a.kf = kf;
         e = launch_lstm_mma(a, s);
     }
     if (e) return fail(FSN_ECUDA, "full-band LSTM step failed: %s", cudaGetErrorString((cudaError_t)e));
@@ -2090,7 +2096,7 @@ static int step_frames(fsn_stream* st, StepScratch& x, const float* d_mag, int K
     cf.W = P(m, "fb_model.fc_output_layer.weight"); cf.bias = P(m, "fb_model.fc_output_layer.bias");
     launch_conv1x1(cf, s);
     StreamPackLaunch pa{d_mag, static_cast<const float*>(x.fbout.p), Pk, static_cast<double*>(st->cum_sb.p), static_cast<__half*>(x.ximg.p),
-                        B, F, K, c.sb_num_neighbors, c.fb_num_neighbors, n, c.norm_type, 0, K, slot, nullptr, 0, 0};
+                        B, F, K, c.sb_num_neighbors, c.fb_num_neighbors, n, c.norm_type, 0, K, slot, nullptr, 0, 0, kf};
     if (!lw) {
         launch_stream_pack(pa, s);
         LstmMmaLaunch b{};
@@ -2100,37 +2106,45 @@ static int step_frames(fsn_stream* st, StepScratch& x, const float* d_mag, int K
         b.img = static_cast<const __half*>(x.ximg.p); b.ntiles = (B * F + 127) / 128;
         b.cstate = static_cast<float*>(st->c_sb.p); b.rows_alloc = st->ra_sb;
         b.out = d_mask; b.O = c.output_size; b.F = F; b.la = 0; b.act = c.sb_act; b.fast = c.fast_math; b.gru = c.rnn_type == FSN_RNN_GRU;
-        b.hstate = static_cast<__half*>(st->h_sb.p); b.resume = resume; b.slot = slot; b.slot_rows = F; b.slot_la = c.look_ahead;
+        b.hstate = static_cast<__half*>(st->h_sb.p); b.resume = resume; b.slot = slot; b.slot_rows = F; b.slot_la = c.look_ahead; b.kf = kf;
         e = launch_lstm_mma(b, s);
         if (e) return fail(FSN_ECUDA, "sub-band LSTM step failed: %s", cudaGetErrorString((cudaError_t)e));
-    } else if (!lw->nact) {
-        StreamChunkScatterLaunch sc{nullptr, d_mask, slot, lw->idx, 0, 0, B, F, K, c.look_ahead, 1};
-        launch_stream_chunk_scatter(sc, s);
     } else {
-        // layer-wise sub band: the stepping sessions only, compacted to rows j F + f, in sub-batches of p.Bs sessions and windows of
-        // p.Tw frames.  The recurrence runs as window t0 = 4 + w0 of a 4 + K step sequence with la = 4: it loads h / c from the carry
-        // (t0 > 0), its parities are those of a launch from 0 (t0 % 4 == 0), and local frame k is output column k of [bs, 2, F, K]
-        const int H = c.sb_hidden, bs_max = lw->p.Bs, tw_max = lw->p.Tw ? lw->p.Tw : K;
-        for (int j0 = 0; j0 < lw->nact; j0 += bs_max) {
-            const int bs = lw->nact - j0 < bs_max ? lw->nact - j0 : bs_max, nt = (bs * F + 127) / 128;
-            const size_t cs_layer = lstm_tc5r_cstate_bytes(nt, H) / sizeof(float), hs_layer = (size_t)(nt + 1) / 2 * 2 * 128 * H;
-            StreamSbCarryLaunch cy{static_cast<__half*>(st->h_sb.p), static_cast<float*>(st->c_sb.p), st->ra_sb,
-                                   static_cast<__half*>(st->c_h.p), hs_layer, static_cast<float*>(st->c_c.p), cs_layer, lw->sess + j0, bs, F, H, L, 0};
-            launch_stream_sb_carry(cy, s);
-            for (int w0 = 0; w0 < K; w0 += tw_max) {
-                const int tw = K - w0 < tw_max ? K - w0 : tw_max;
-                pa.k0 = w0; pa.Kw = tw; pa.idx = lw->idx; pa.j0 = j0; pa.nsess = bs;
-                launch_stream_pack(pa, s);
-                LstmTc5rLaunch a{};
-                a.rows = bs * F; a.Tp = 4 + K; a.ntiles = nt; a.t0 = 4 + w0; a.Tw = tw;
-                a.ximg = static_cast<const __half*>(x.ximg.p); a.hseq = static_cast<__half*>(st->c_hsb.p);
-                a.cstate = static_cast<float*>(st->c_c.p); a.hstate = static_cast<__half*>(st->c_h.p);
-                a.out = static_cast<float*>(st->c_mask.p); a.la = 4;
-                if (int nl = sb_layers(m, a, static_cast<__half*>(st->c_gin.p), cs_layer, hs_layer, s); nl < 0) return nl;
+        // layer-wise sub band, per group of kf frames: its sessions compacted to rows j F + f, in sub-batches of p.Bs sessions and
+        // windows of p.Tw frames.  The recurrence runs as window t0 = 4 + w0 of a 4 + kf step sequence with la = 4: it loads h / c from
+        // the carry (t0 > 0), its parities are those of a launch from 0 (t0 % 4 == 0), and local frame k is output column k of
+        // [bs, 2, F, kf]; the scatter zeroes the slots' columns from kf on
+        const int H = c.sb_hidden;
+        int zero_held = 1;
+        for (const LwGroup& g : *lw) {
+            const int Kg = g.kf, bs_max = g.p.Bs, tw_max = g.p.Tw ? g.p.Tw : Kg;
+            for (int j0 = 0; j0 < g.nact; j0 += bs_max) {
+                const int bs = g.nact - j0 < bs_max ? g.nact - j0 : bs_max, nt = (bs * F + 127) / 128;
+                const size_t cs_layer = lstm_tc5r_cstate_bytes(nt, H) / sizeof(float), hs_layer = (size_t)(nt + 1) / 2 * 2 * 128 * H;
+                StreamSbCarryLaunch cy{static_cast<__half*>(st->h_sb.p), static_cast<float*>(st->c_sb.p), st->ra_sb,
+                                       static_cast<__half*>(st->c_h.p), hs_layer, static_cast<float*>(st->c_c.p), cs_layer, g.sess + j0, bs, F, H, L, 0};
+                launch_stream_sb_carry(cy, s);
+                for (int w0 = 0; w0 < Kg; w0 += tw_max) {
+                    const int tw = Kg - w0 < tw_max ? Kg - w0 : tw_max;
+                    pa.k0 = w0; pa.Kw = tw; pa.idx = g.idx; pa.j0 = j0; pa.nsess = bs;
+                    launch_stream_pack(pa, s);
+                    LstmTc5rLaunch a{};
+                    a.rows = bs * F; a.Tp = 4 + Kg; a.ntiles = nt; a.t0 = 4 + w0; a.Tw = tw;
+                    a.ximg = static_cast<const __half*>(x.ximg.p); a.hseq = static_cast<__half*>(st->c_hsb.p);
+                    a.cstate = static_cast<float*>(st->c_c.p); a.hstate = static_cast<__half*>(st->c_h.p);
+                    a.out = static_cast<float*>(st->c_mask.p); a.la = 4;
+                    if (int nl = sb_layers(m, a, static_cast<__half*>(st->c_gin.p), cs_layer, hs_layer, s); nl < 0) return nl;
+                }
+                cy.out = 1;
+                launch_stream_sb_carry(cy, s);
+                StreamChunkScatterLaunch sc{static_cast<const float*>(st->c_mask.p), d_mask, slot, g.idx, j0, bs, B, F, K, Kg, c.look_ahead,
+                                            zero_held};
+                launch_stream_chunk_scatter(sc, s);
+                zero_held = 0;
             }
-            cy.out = 1;
-            launch_stream_sb_carry(cy, s);
-            StreamChunkScatterLaunch sc{static_cast<const float*>(st->c_mask.p), d_mask, slot, lw->idx, j0, bs, B, F, K, c.look_ahead, j0 == 0};
+        }
+        if (zero_held) {                                                // no stepping session: every row is held
+            StreamChunkScatterLaunch sc{nullptr, d_mask, slot, nullptr, 0, 0, B, F, K, K, c.look_ahead, 1};
             launch_stream_chunk_scatter(sc, s);
         }
     }
@@ -2153,7 +2167,7 @@ extern "C" int fsn_stream_step(fsn_stream* st, const float* d_mag, float* d_mask
         return FSN_OK;
     }
     const int n = st->n;
-    const int rc = step_frames(st, st->tick, d_mag, 1, nullptr, nullptr, 0, d_mask, nullptr, static_cast<cudaStream_t>(stream));
+    const int rc = step_frames(st, st->tick, d_mag, 1, nullptr, nullptr, nullptr, 0, d_mask, nullptr, static_cast<cudaStream_t>(stream));
     if (rc) return rc;
     if (h_valid) *h_valid = (n >= st->m->cfg.look_ahead) ? 1 : 0;
     return FSN_OK;
@@ -2225,6 +2239,20 @@ extern "C" int fsn_stream_chunk_plan(const fsn_config* cfg, int32_t n_active, in
     return FSN_OK;
 }
 
+// The chunk scratch of a layer-wise sub-band step of K frames under plan p: images, Gin, layer output, h / c carry and compact masks
+static int chunk_lw_ensure(fsn_stream* st, const Plan& p, int K, cudaStream_t s) {
+    const fsn_config& c = st->m->cfg;
+    const int F = c.num_freqs, nt = (p.Bs * F + 127) / 128;
+    const WsSizes z = ws_sizes(c, true, p.Bs, K, p.Tw ? p.Tw : K);
+    int e = st->chunk.ensure(*st, K, z.ximg, false, s);
+    e |= st->c_gin.ensure(z.r_gin, false, s);
+    e |= st->c_hsb.ensure(z.r_hseq, false, s);
+    e |= st->c_h.ensure(z.r_hstate, true, s);
+    e |= st->c_c.ensure((size_t)c.num_layers * lstm_tc5r_cstate_bytes(nt, c.sb_hidden), true, s);
+    e |= st->c_mask.ensure((size_t)p.Bs * 2 * F * K * sizeof(float), false, s);
+    return e;
+}
+
 // The slot calls after their argument checks: every slot advances K frames by its flag (fsn_stream_step_slots: K = 1 on the per-tick
 // scratch; the chunk call: on its own scratch, with the layer-wise sub band where the offline forward runs it).  Errors change no state.
 static int step_slots(fsn_stream* st, const float* d_mag, int K, float* d_mask, const int32_t* h_flags, int32_t* h_valid, bool chunk,
@@ -2244,23 +2272,18 @@ static int step_slots(fsn_stream* st, const float* d_mag, int K, float* d_mask, 
     }
     if (st->mode == FSN_STATE_MODE_AUDIO) return claim_mode(st, FSN_STATE_MODE_MASK);
     const bool layerwise = chunk && runs_layerwise(c, m->env_impl);
-    LwSessions lw{Plan{nact}, nact};
-    if (layerwise && nact)
-        if (int rc = chunk_plan(c, true, nact, K, m->ws_cap_bytes, &lw.p)) return rc;
+    std::vector<LwGroup> lw;                                            // every stepping session runs K frames: one group
+    if (layerwise && nact) {
+        lw.push_back(LwGroup{Plan{nact}, nact, K, nullptr, nullptr});
+        if (int rc = chunk_plan(c, true, nact, K, m->ws_cap_bytes, &lw[0].p)) return rc;
+    }
     // the scratch, before any state changes (DevBuf::ensure only grows)
     StepScratch& x = chunk ? st->chunk : st->tick;
     int e = 0;
     if (!layerwise || !nact) {
         e = x.ensure(*st, K, layerwise ? 0 : step_img_bytes((long long)B * F, K), false, s);
     } else {
-        const int nt = (lw.p.Bs * F + 127) / 128;
-        const WsSizes z = ws_sizes(c, true, lw.p.Bs, K, lw.p.Tw ? lw.p.Tw : K);
-        e = x.ensure(*st, K, z.ximg, false, s);
-        e |= st->c_gin.ensure(z.r_gin, false, s);
-        e |= st->c_hsb.ensure(z.r_hseq, false, s);
-        e |= st->c_h.ensure(z.r_hstate, true, s);
-        e |= st->c_c.ensure((size_t)c.num_layers * lstm_tc5r_cstate_bytes(nt, c.sb_hidden), true, s);
-        e |= st->c_mask.ensure((size_t)lw.p.Bs * 2 * F * K * sizeof(float), false, s);
+        e = chunk_lw_ensure(st, lw[0].p, K, s);
     }
     if (e) return fail(FSN_ECUDA, "chunk scratch allocation failed (B = %d, K = %d)", B, K);
     if (int rc = claim_mode(st, FSN_STATE_MODE_MASK)) return rc;
@@ -2282,8 +2305,8 @@ static int step_slots(fsn_stream* st, const float* d_mag, int K, float* d_mask, 
     }
     const int* d = static_cast<const int*>(st->d_slot.p);
     if (int rc = st->stage.send(st->d_slot.p, (size_t)B + nlw + nzero, s)) return rc;
-    lw.idx = d + B; lw.sess = d + 2 * B;
-    if (int rc = step_frames(st, x, d_mag, K, d, d + B + nlw, nzero, d_mask, layerwise ? &lw : nullptr, s)) return rc;
+    if (!lw.empty()) { lw[0].idx = d + B; lw[0].sess = d + 2 * B; }
+    if (int rc = step_frames(st, x, d_mag, K, d, nullptr, d + B + nlw, nzero, d_mask, layerwise ? &lw : nullptr, s)) return rc;
     for (int b = 0; b < B; ++b) {
         h_valid[b] = 0;
         if (cnt[b] < 0) continue;
@@ -2327,6 +2350,192 @@ static int audio_alloc(fsn_stream* st, cudaStream_t s) {
     return FSN_OK;
 }
 
+// One slot's ticks in an audio call of K hops (DESIGN.md §3.10, §3.14).  Flag f with n hops stands for K per-hop ticks: START,
+// STEP x (n - 1) / STEP x n / STEP x n then FLUSH, the rest HOLD.  The active ones -- every tick but the HOLDs and the FLUSH ticks past
+// the session's end -- come first: na of them, at slot ticks k0 .. k0 + na - 1 (a START's k0 is 0).  The first nstore store the row's
+// hops, and every active tick but a START's is a model frame.  hops: the session's K after the call (0 before its FLUSH); nout: the
+// hops the call emits (those of slot ticks k >= la + 2).  Checks the flag and hop count against the slot's session.
+struct AudioSlotPlan { int k0, na, start, nstore, hops, nout; };
+static int audio_slot_plan(const fsn_stream* st, int b, int f, int n, int K, AudioSlotPlan* p) {
+    const int la = st->m->cfg.look_ahead;
+    const int t = st->a_tick.empty() ? -1 : st->a_tick[b], Kh = st->a_hops.empty() ? 0 : st->a_hops[b];
+    *p = AudioSlotPlan{t, 0, 0, 0, Kh, 0};
+    if (f < FSN_SLOT_HOLD || f > FSN_SLOT_FLUSH)
+        return fail(FSN_EINVAL, "slot %d: flag %d is not FSN_SLOT_HOLD (0), FSN_SLOT_STEP (1), FSN_SLOT_START (2) or FSN_SLOT_FLUSH (3)", b, f);
+    if (f == FSN_SLOT_HOLD) return FSN_OK;
+    const int lo = f == FSN_SLOT_FLUSH ? 0 : 1;
+    const char* name = f == FSN_SLOT_START ? "START" : f == FSN_SLOT_STEP ? "STEP" : "FLUSH";
+    if (n < lo || n > K) return fail(FSN_EINVAL, "slot %d: h_hops = %d: a %s consumes %d to K = %d hops", b, n, name, lo, K);
+    if (f == FSN_SLOT_START) {
+        *p = AudioSlotPlan{0, n, 1, n, 0, 0};
+    } else {
+        if (t < 0) return fail(FSN_EINVAL, "slot %d: %s on a slot without a session (START one first)", b, name);
+        if (f == FSN_SLOT_STEP && Kh)
+            return fail(FSN_EINVAL, "slot %d: STEP after the session's FLUSH (its input has ended: START a new session)", b);
+        if (f == FSN_SLOT_FLUSH && Kh && n)
+            return fail(FSN_EINVAL, "slot %d: FLUSH with h_hops = %d after the session's FLUSH (its input has ended: pass 0 hops)", b, n);
+        if (f == FSN_SLOT_FLUSH && !Kh && t + n < 2)
+            return fail(FSN_EINVAL, "slot %d: FLUSH after %d hop: a session needs at least 2 hops (the STFT's reflect padding reads "
+                                    "n_fft / 2 + 1 samples)", b, t + n);
+        p->k0 = t; p->nstore = n;
+        if (f == FSN_SLOT_STEP) {
+            p->na = n;
+        } else {                                                        // active up to slot tick K + la + 1, then a FLUSH is a HOLD
+            p->hops = Kh ? Kh : n < K ? t + n : 0;                      // n = K: no FLUSH tick yet, the end is not known
+            const int left = p->hops ? p->hops + la + 2 - t : n;
+            p->na = left < 0 ? 0 : left < K ? left : K;
+        }
+    }
+    const int e0 = p->k0 > la + 2 ? p->k0 : la + 2, e1 = p->k0 + p->na;
+    p->nout = e1 > e0 ? e1 - e0 : 0;
+    return FSN_OK;
+}
+
+// The audio calls after their argument checks: every slot advances by its flag and hop count (fsn_stream_step_audio_slots: K = 1,
+// h_hops null, one hop per START / STEP).  The per-hop call runs the per-hop kernels around the per-frame step; the chunk call, at any
+// K, the K-hop kernels around the chunk call's K-frame step.  Errors change no state.
+static int step_audio(fsn_stream* st, const float* d_samples, int K, const int32_t* h_flags, const int32_t* h_hops, float* d_out,
+                      int32_t* h_nout, float* d_mask, cudaStream_t s) {
+    fsn_model* m = st->m;
+    const fsn_config& c = m->cfg;
+    const int B = st->B, F = c.num_freqs, H = F - 1, la = c.look_ahead, N = 2 * H;
+    if (int rc = audio_fft_ok(c)) return rc;
+    if (int rc = chunk_check(c, K)) return rc;                         // num_freqs x K < 2^31 bounds the rows' K x hop too
+    std::vector<AudioSlotPlan> plan(B);
+    for (int b = 0; b < B; ++b) {                                       // every slot is checked before any state changes
+        const int n = h_hops ? h_hops[b] : h_flags[b] == FSN_SLOT_FLUSH ? 0 : 1;
+        if (int rc = audio_slot_plan(st, b, h_flags[b], n, K, &plan[b])) return rc;
+    }
+    if (st->mode == FSN_STATE_MODE_MASK) return claim_mode(st, FSN_STATE_MODE_AUDIO);
+    int32_t* h = nullptr;
+    if (!h_hops) {
+        if (int rc = claim_mode(st, FSN_STATE_MODE_AUDIO)) return rc;
+        if (st->a_tick.empty())
+            if (int rc = audio_alloc(st, s)) return rc;
+        // One staging slot carries the tick's four per-slot planes: the model's frame counts (-1 = the model row holds), the AUDIO_*
+        // ops, the slot ticks and the hop counts; then the slots whose model row starts.  The schedule (DESIGN.md §3.10) for a session
+        // of K hops, slot tick k:
+        //   k = 0 (START): store hop 0, the model row holds;  1 <= k <= K + 1: analyse frame k - 1, the model steps frame k - 1 (count
+        //   k - 1, a START at k = 1);  k > K + 1: a zero frame;  k - 1 - la >= 0: synthesise that frame, emitting hop k - 2 - la from 1.
+        if (int rc = st->stage.take((size_t)5 * B, &h)) return rc;
+        int32_t *cnt = h, *op = h + B, *tick = h + 2 * B, *hops = h + 3 * B;
+        int nzero = 0;
+        for (int b = 0; b < B; ++b) {
+            const AudioSlotPlan& p = plan[b];
+            const int j = p.k0 - 1, mm = j - la;
+            cnt[b] = -1; op[b] = 0;
+            tick[b] = p.k0; hops[b] = p.hops;
+            if (p.na && p.start) {
+                op[b] = AUDIO_STORE;
+            } else if (p.na) {
+                cnt[b] = j;
+                op[b] = (p.nstore ? AUDIO_STORE : 0) | (!p.hops || j <= p.hops ? AUDIO_FRAME : AUDIO_ZERO) | (mm >= 0 ? AUDIO_SYNTH : 0) |
+                        (mm >= 1 ? AUDIO_EMIT : 0);
+            }
+            if (cnt[b] == 0) h[4 * B + nzero++] = b;
+        }
+        int32_t* d = static_cast<int32_t*>(st->d_slot.p);
+        if (int rc = st->stage.send(d, (size_t)4 * B + nzero, s)) return rc;
+        float* mask = d_mask ? d_mask : static_cast<float*>(st->a_mask.p);
+        StreamAudioLaunch a{};
+        a.op = d + B; a.tick = d + 2 * B; a.hops = d + 3 * B;
+        a.samples = d_samples; a.out = d_out;
+        a.hist = static_cast<float*>(st->a_hist.p); a.spec = static_cast<float2*>(st->a_spec.p); a.tail = static_cast<float*>(st->a_tail.p);
+        a.mag = static_cast<float*>(st->a_mag.p); a.mask = mask;
+        const AudioTables tab = audio_table_ptrs(static_cast<const float*>(st->a_tab.p), N);
+        a.window = tab.window; a.twiddle = tab.twiddle; a.inv_env = tab.inv_env;
+        a.B = B; a.n_fft = N; a.la = la;
+        launch_stream_stft(a, s);
+        if (int rc = step_frames(st, st->tick, a.mag, 1, d, nullptr, d + 4 * B, nzero, mask, nullptr, s)) return rc;
+        launch_stream_istft(a, s);
+    } else {
+        // The model's frames: slot b's kf of them, left-aligned in columns 0 .. kf - 1 of [B, F, Km], Km the largest kf.  One K-frame
+        // step runs them all, each slot holding after its kf frames; on the layer-wise path its sub band runs one pass per group of
+        // sessions with one kf (in steady state a single group).
+        std::vector<int> kf(B);
+        int Km = 0, nzero = 0;
+        for (int b = 0; b < B; ++b) {
+            kf[b] = plan[b].na > plan[b].start ? plan[b].na - plan[b].start : 0;
+            Km = kf[b] > Km ? kf[b] : Km;
+            nzero += kf[b] && plan[b].k0 + plan[b].start == 1;          // model frame 0 in column 0: a START's reset
+        }
+        const bool layerwise = runs_layerwise(c, m->env_impl);
+        std::vector<LwGroup> lw;
+        if (layerwise) {
+            std::vector<int> ks;
+            for (int v : kf) if (v) ks.push_back(v);
+            std::sort(ks.begin(), ks.end());
+            for (size_t i = 0; i < ks.size();) {
+                size_t e = i;
+                while (e < ks.size() && ks[e] == ks[i]) ++e;
+                lw.push_back(LwGroup{Plan{(int)(e - i)}, (int)(e - i), ks[i], nullptr, nullptr});
+                i = e;
+            }
+        }
+        size_t nstage = (size_t)7 * B + nzero;
+        int e = 0;
+        for (LwGroup& g : lw) {
+            nstage += B + g.nact;
+            if (int rc = chunk_plan(c, true, g.nact, g.kf, m->ws_cap_bytes, &g.p)) return rc;
+            e |= chunk_lw_ensure(st, g.p, g.kf, s);
+        }
+        if (Km) e |= st->chunk.ensure(*st, Km, layerwise ? 0 : step_img_bytes((long long)B * F, Km), false, s);
+        e |= st->x_spec.ensure((size_t)B * K * F * sizeof(float2), false, s);
+        e |= st->x_mag.ensure((size_t)B * F * Km * sizeof(float), false, s);
+        e |= st->x_mask.ensure((size_t)B * 2 * F * Km * sizeof(float), false, s);
+        e |= st->x_plan.ensure(nstage * sizeof(int32_t), false, s);
+        if (e) return fail(FSN_ECUDA, "audio chunk scratch allocation failed (B = %d, K = %d)", B, K);
+        if (int rc = claim_mode(st, FSN_STATE_MODE_AUDIO)) return rc;
+        if (st->a_tick.empty())
+            if (int rc = audio_alloc(st, s)) return rc;
+        // staged: the five per-slot planes of the kernels, the model's frame counts at column 0 (-1 = held) and frame counts, the
+        // slots whose model frame 0 is in this call, then per layer-wise group each slot's session index and the group's slots
+        if (int rc = st->stage.take(nstage, &h)) return rc;
+        const int32_t* d = static_cast<const int32_t*>(st->x_plan.p);
+        int32_t *cnt = h + 5 * B, *kfp = h + 6 * B, *zero = h + 7 * B;
+        for (int b = 0, z = 0; b < B; ++b) {
+            const AudioSlotPlan& p = plan[b];
+            h[b] = p.k0; h[B + b] = p.na; h[2 * B + b] = p.start; h[3 * B + b] = p.nstore; h[4 * B + b] = p.hops;
+            cnt[b] = kf[b] ? p.k0 + p.start - 1 : -1;
+            kfp[b] = kf[b];
+            if (kf[b] && cnt[b] == 0) zero[z++] = b;
+        }
+        size_t at = (size_t)7 * B + nzero;
+        for (LwGroup& g : lw) {
+            int32_t *idx = h + at, *sess = idx + B;
+            g.idx = d + at; g.sess = d + at + B;
+            for (int b = 0, j = 0; b < B; ++b) {
+                idx[b] = kf[b] == g.kf ? j : -1;
+                if (kf[b] == g.kf) sess[j++] = b;
+            }
+            at += B + g.nact;
+        }
+        if (int rc = st->stage.send(st->x_plan.p, nstage, s)) return rc;
+        StreamAudioChunkLaunch a{};
+        a.k0 = d; a.na = d + B; a.start = d + 2 * B; a.nstore = d + 3 * B; a.hops = d + 4 * B;
+        a.samples = d_samples; a.out = d_out;
+        a.hist = static_cast<float*>(st->a_hist.p); a.spec = static_cast<float2*>(st->a_spec.p); a.tail = static_cast<float*>(st->a_tail.p);
+        a.sspec = static_cast<float2*>(st->x_spec.p); a.mag = static_cast<float*>(st->x_mag.p); a.mask = static_cast<float*>(st->x_mask.p);
+        a.umask = d_mask;
+        const AudioTables tab = audio_table_ptrs(static_cast<const float*>(st->a_tab.p), N);
+        a.window = tab.window; a.twiddle = tab.twiddle; a.inv_env = tab.inv_env;
+        a.B = B; a.K = K; a.Km = Km; a.n_fft = N; a.la = la;
+        launch_stream_stft_chunk(a, s);
+        if (Km)
+            if (int rc = step_frames(st, st->chunk, a.mag, Km, d + 5 * B, d + 6 * B, d + 7 * B, nzero, static_cast<float*>(st->x_mask.p),
+                                     layerwise ? &lw : nullptr, s))
+                return rc;
+        launch_stream_istft_chunk(a, s);
+    }
+    CK(cudaGetLastError());
+    for (int b = 0; b < B; ++b) {
+        const AudioSlotPlan& p = plan[b];
+        if (h_flags[b] != FSN_SLOT_HOLD) { st->a_tick[b] = p.k0 + p.na; st->a_hops[b] = p.hops; }
+        h_nout[b] = p.nout;
+    }
+    return FSN_OK;
+}
+
 extern "C" int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_samples, float* d_out, const int32_t* h_flags,
                                            int32_t* h_valid, float* d_mask, void* stream) {
     if (!st) return fail(FSN_EINVAL, "st is null");
@@ -2334,73 +2543,18 @@ extern "C" int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_sample
     if (!d_out) return fail(FSN_EINVAL, "d_out is null (one hop of output per slot, [B, hop] float32 on the device)");
     if (!h_flags) return fail(FSN_EINVAL, "h_flags is null (one flag per slot, slots 0..%d)", st->B - 1);
     if (!h_valid) return fail(FSN_EINVAL, "h_valid is null (one result per slot, slots 0..%d)", st->B - 1);
-    const fsn_config& c = st->m->cfg;
-    const int B = st->B, la = c.look_ahead, N = 2 * (c.num_freqs - 1);
-    if (int rc = audio_fft_ok(c)) return rc;
-    for (int b = 0; b < B; ++b) {                                       // every flag is checked before any state changes
-        const int f = h_flags[b], t = st->a_tick.empty() ? -1 : st->a_tick[b], K = st->a_hops.empty() ? 0 : st->a_hops[b];
-        if (f < FSN_SLOT_HOLD || f > FSN_SLOT_FLUSH)
-            return fail(FSN_EINVAL, "slot %d: flag %d is not FSN_SLOT_HOLD (0), FSN_SLOT_STEP (1), FSN_SLOT_START (2) or FSN_SLOT_FLUSH (3)", b, f);
-        if ((f == FSN_SLOT_STEP || f == FSN_SLOT_FLUSH) && t < 0)
-            return fail(FSN_EINVAL, "slot %d: %s on a slot without a session (START one first)", b, f == FSN_SLOT_STEP ? "STEP" : "FLUSH");
-        if (f == FSN_SLOT_STEP && K)
-            return fail(FSN_EINVAL, "slot %d: STEP after the session's FLUSH (its input has ended: START a new session)", b);
-        if (f == FSN_SLOT_FLUSH && !K && t < 2)
-            return fail(FSN_EINVAL, "slot %d: FLUSH after %d hop: a session needs at least 2 hops (the STFT's reflect padding reads "
-                                    "n_fft / 2 + 1 samples)", b, t);
-    }
-    if (int rc = claim_mode(st, FSN_STATE_MODE_AUDIO)) return rc;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (st->a_tick.empty())
-        if (int rc = audio_alloc(st, s)) return rc;
-    // One staging slot carries the tick's four per-slot planes: the model's frame counts (-1 = the model row holds), the AUDIO_* ops,
-    // the slot ticks and the hop counts; then the slots whose model row starts.  The schedule (DESIGN.md §3.10) for a session of K
-    // hops, slot tick k:
-    //   k = 0 (START): store hop 0, the model row holds;  1 <= k <= K + 1: analyse frame k - 1, the model steps frame k - 1 (count
-    //   k - 1, a START at k = 1);  k > K + 1: a zero frame;  k - 1 - la >= 0: synthesise that frame, emitting hop k - 2 - la from 1.
-    int32_t* cnt = nullptr;
-    if (int rc = st->stage.take((size_t)5 * B, &cnt)) return rc;
-    int32_t *op = cnt + B, *tick = cnt + 2 * B, *hops = cnt + 3 * B;
-    int nzero = 0;
-    for (int b = 0; b < B; ++b) {
-        const int f = h_flags[b];
-        int k = st->a_tick[b], K = st->a_hops[b];
-        cnt[b] = -1; op[b] = 0;
-        if (f == FSN_SLOT_START) {
-            k = 0; K = 0; op[b] = AUDIO_STORE;
-        } else if (f == FSN_SLOT_STEP || f == FSN_SLOT_FLUSH) {
-            if (f == FSN_SLOT_FLUSH && !K) K = k;
-            if (k <= K + la + 1 || !K) {                                // past that, a FLUSH is a HOLD
-                const int j = k - 1, m = k - 1 - la;
-                cnt[b] = j;
-                op[b] = (f == FSN_SLOT_STEP ? AUDIO_STORE : 0) | (!K || j <= K ? AUDIO_FRAME : AUDIO_ZERO) |
-                        (m >= 0 ? AUDIO_SYNTH : 0) | (m >= 1 ? AUDIO_EMIT : 0);
-            }
-        }
-        tick[b] = k; hops[b] = K;
-        if (cnt[b] == 0) cnt[4 * B + nzero++] = b;
-    }
-    int32_t* d = static_cast<int32_t*>(st->d_slot.p);
-    if (int rc = st->stage.send(d, (size_t)4 * B + nzero, s)) return rc;
-    float* mask = d_mask ? d_mask : static_cast<float*>(st->a_mask.p);
-    StreamAudioLaunch a{};
-    a.op = d + B; a.tick = d + 2 * B; a.hops = d + 3 * B;
-    a.samples = d_samples; a.out = d_out;
-    a.hist = static_cast<float*>(st->a_hist.p); a.spec = static_cast<float2*>(st->a_spec.p); a.tail = static_cast<float*>(st->a_tail.p);
-    a.mag = static_cast<float*>(st->a_mag.p); a.mask = mask;
-    const AudioTables tab = audio_table_ptrs(static_cast<const float*>(st->a_tab.p), N);
-    a.window = tab.window; a.twiddle = tab.twiddle; a.inv_env = tab.inv_env;
-    a.B = B; a.n_fft = N; a.la = la;
-    launch_stream_stft(a, s);
-    const int rc = step_frames(st, st->tick, a.mag, 1, d, d + 4 * B, nzero, mask, nullptr, s);
-    if (rc) return rc;
-    launch_stream_istft(a, s);
-    CK(cudaGetLastError());
-    for (int b = 0; b < B; ++b) {
-        if (h_flags[b] == FSN_SLOT_START || cnt[b] >= 0) { st->a_tick[b] = tick[b] + 1; st->a_hops[b] = hops[b]; }
-        h_valid[b] = (op[b] & AUDIO_EMIT) ? 1 : 0;
-    }
-    return FSN_OK;
+    return step_audio(st, d_samples, 1, h_flags, nullptr, d_out, h_valid, d_mask, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int fsn_stream_step_audio_chunk(fsn_stream* st, const float* d_samples, int32_t K, const int32_t* h_flags,
+                                           const int32_t* h_hops, float* d_out, int32_t* h_nout, float* d_mask, void* stream) {
+    if (!st) return fail(FSN_EINVAL, "st is null");
+    if (!d_samples) return fail(FSN_EINVAL, "d_samples is null (K hops of samples per slot, [B, K x hop] float32 on the device)");
+    if (!d_out) return fail(FSN_EINVAL, "d_out is null (K hops of output per slot, [B, K x hop] float32 on the device)");
+    if (!h_flags) return fail(FSN_EINVAL, "h_flags is null (one flag per slot, slots 0..%d)", st->B - 1);
+    if (!h_hops) return fail(FSN_EINVAL, "h_hops is null (one hop count per slot, slots 0..%d)", st->B - 1);
+    if (!h_nout) return fail(FSN_EINVAL, "h_nout is null (one result per slot, slots 0..%d)", st->B - 1);
+    return step_audio(st, d_samples, K, h_flags, h_hops, d_out, h_nout, d_mask, static_cast<cudaStream_t>(stream));
 }
 
 // ---------------------------------------------------------------------------------------------

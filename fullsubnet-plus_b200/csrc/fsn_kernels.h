@@ -109,7 +109,8 @@ void launch_apply_cirm_planar(const float* crm, const float* nreal, const float*
 // streaming step kernels (k_front.cu): K frames of the cumulative norms with running sums carried in global memory, frame after
 // frame.  slot: null (every slot is at frame n), or [B] per-slot frame counts of the slot calls, -1 = held: a held slot's frames are
 // not read, its sums are untouched and its outputs are zero.  x [B, F, K] -> y [B, F, P] (frames at columns 0 .. K - 1)
-struct StreamNormLaunch { const float* x; float* y; double* cum; int B, F, K, P, n, type; const int* slot; };
+// kf: null, or [B] per-slot frame counts (slot calls): a stepping slot runs frames 0 .. kf - 1 only, the rest of its row is zero
+struct StreamNormLaunch { const float* x; float* y; double* cum; int B, F, K, P, n, type; const int* slot; const int* kf; };
 void launch_stream_norm(const StreamNormLaunch& a, cudaStream_t s);
 // frames k0 .. k0 + Kw - 1 of mag [B, F, K] and fb [B, F, Pfb] -> images [tile, Kw, 128 rows, 64 halves].  idx null: row b F + f,
 // held rows zero.  idx [B]: row (idx[b] - j0) F + f for the sessions j0 .. j0 + nsess - 1 of a sub-batch, nothing for any other slot.
@@ -117,11 +118,13 @@ void launch_stream_norm(const StreamNormLaunch& a, cudaStream_t s);
 struct StreamPackLaunch {
     const float* mag; const float* fb; int Pfb; double* cum; __half* ximg; int B, F, K, Ns, Nf, n, type, k0, Kw; const int* slot;
     const int* idx; int j0, nsess;
+    const int* kf;            // null, or [B]: frames k >= kf[b] of a stepping slot are zero images and leave its sums untouched
 };
 void launch_stream_pack(const StreamPackLaunch& a, cudaStream_t s);
 // compact masks src [nsess, 2, F, K] of the sessions j0 .. j0 + nsess - 1 -> dst [B, 2, F, K] at their slots (idx[b] - j0), leading
 // columns with slot[b] + k < la zero; zero_held: also zero the rows of held slots
-struct StreamChunkScatterLaunch { const float* src; float* dst; const int* slot; const int* idx; int j0, nsess, B, F, K, la, zero_held; };
+// src has Ks <= K columns; dst columns k >= Ks of the sub-batch's slots are zero
+struct StreamChunkScatterLaunch { const float* src; float* dst; const int* slot; const int* idx; int j0, nsess, B, F, K, Ks, la, zero_held; };
 void launch_stream_chunk_scatter(const StreamChunkScatterLaunch& a, cudaStream_t s);
 
 // ---- k_stream_state.cu: save / load of streaming sessions (fsn_stream_save_slots, fsn_stream_load_slots), START reset ----------
@@ -174,6 +177,24 @@ struct StreamAudioLaunch {
 };
 void launch_stream_stft(const StreamAudioLaunch& a, cudaStream_t s);
 void launch_stream_istft(const StreamAudioLaunch& a, cudaStream_t s);
+// K hops per slot (fsn_stream_step_audio_chunk, DESIGN.md §3.14): slot b's active ticks are the first na[b] of the call, at slot ticks
+// k0[b] + i; with start[b] its tick 0 is a START (store hop 0, no model frame).  Its first nstore[b] active ticks store the row's hops
+// 0 .. nstore - 1.  Every other active tick is a model frame: model column c = i - start, frame j = k0 + start - 1 + c, its
+// magnitude and mask at column c of the model's planes [B, F, Km] and [B, 2, F, Km].
+struct StreamAudioChunkLaunch {
+    const int *k0, *na, *start, *nstore, *hops;   // [B] each; hops: the session's K after this call (0 = not flushed)
+    const float* samples;     // [B, K hop] this call's hops at the front of each row
+    float* out;               // [B, K hop] output hops at the front of each row, zero after them
+    float* hist; float2* spec; float* tail;       // the slot state of StreamAudioLaunch
+    float2* sspec;            // [B, K, F] scratch: the spectrum of each model column's frame
+    float* mag;               // model input [B, F, Km]
+    const float* mask;        // model output [B, 2, F, Km]
+    float* umask;             // [B, 2, F, K] the caller's masks by tick, or null
+    const float* window; const float2* twiddle; const float* inv_env;
+    int B, K, Km, n_fft, la;  // Km: model columns, the largest frame count of the call
+};
+void launch_stream_stft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s);
+void launch_stream_istft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s);
 
 // ---- k_audio.cu: audio in and out of the offline forward (fsn_model_enhance_audio), and the tables of both audio paths -------
 struct AudioLaunch {
@@ -228,6 +249,9 @@ struct LstmMmaLaunch {
     // writes neither cstate nor hstate.  The fused-FC output at step t of a held slot, or of a slot whose frame count + t is below
     // slot_la (still filling its look-ahead), is zero
     const int* slot; int slot_rows, slot_la;
+    // optional with slot: [B] per-slot frame counts; a stepping row holds at every step t >= kf (keeps c, carries its h forward,
+    // output zero)
+    const int* kf;
 };
 size_t lstm_mma_cstate_bytes(int L, int rows, int H, int* rows_alloc);
 int launch_lstm_mma(const LstmMmaLaunch& a, cudaStream_t s);   // returns 0 or cudaError
@@ -245,6 +269,7 @@ struct LstmWsLaunch {
     int gru;                  // 1: pseudo-gate GRU cell, cbuf / cst carry h in fp32
     const int* slot;          // optional (streaming slot call, Tp = 1): [rows] per-slot frame counts, -1 = held: the row keeps its
                               // cell state and carries its previous h into this step's exchange-buffer parity
+    const int* kf;            // optional with slot: [rows] per-slot frame counts; a stepping row holds as above at steps t >= kf
 };
 bool lstm_ws_supported(int L, int H, int Ipad, int rows, int num_sms);
 int launch_lstm_ws(const LstmWsLaunch& a, cudaStream_t s);

@@ -671,10 +671,12 @@ __global__ void __launch_bounds__(256) stream_norm_kernel(StreamNormLaunch a) {
         return;
     }
     const float* x = a.x + (size_t)b * F * a.K;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, kb = a.kf ? a.kf[b] : a.K;
+    for (int i = threadIdx.x; i < F * (a.K - kb); i += blockDim.x)  // frames past the slot's count: zero
+        a.y[((size_t)b * F + i / (a.K - kb)) * a.P + kb + i % (a.K - kb)] = 0.f;
     double cs = n0 == 0 ? 0.0 : a.cum[2 * b], cq = n0 == 0 ? 0.0 : a.cum[2 * b + 1];   // thread 0's running sums
 #pragma unroll 1
-    for (int k = 0; k < a.K; ++k) {
+    for (int k = 0; k < kb; ++k) {
         const int n = n0 + k;
         double s = 0, q = 0;
         for (int f = threadIdx.x; f < F; f += blockDim.x) { const double v = x[(size_t)f * a.K + k]; s += v; q += v * v; }
@@ -722,9 +724,15 @@ __global__ void __launch_bounds__(128) stream_pack_kernel(StreamPackLaunch a) {
     const float* mag = a.mag + (size_t)b * F * a.K;
     const float* fb = a.fb + (size_t)b * F * a.Pfb;
     double cs = n0 + a.k0 == 0 ? 0.0 : a.cum[2 * row], cq = n0 + a.k0 == 0 ? 0.0 : a.cum[2 * row + 1];
+    const int kb = a.kf ? a.kf[b] : a.K;
 #pragma unroll 1
     for (int kk = 0; kk < a.Kw; ++kk) {
         const int k = a.k0 + kk, n = n0 + k;
+        if (k >= kb) {                                              // past the slot's frames: zero input rows, sums untouched
+#pragma unroll
+            for (int c = 0; c < 8; ++c) *reinterpret_cast<uint4*>(img + (size_t)kk * (128 * 128) + sw128_offset(r, c * 8)) = make_uint4(0u, 0u, 0u, 0u);
+            continue;
+        }
         int fo = f;                                                 // opaque per frame: the 64 neighbour offsets are recomputed, not
         asm volatile("" : "+r"(fo));                                // hoisted out of the frame loop (which spills them)
         float v[64];
@@ -810,7 +818,8 @@ __global__ void stream_chunk_scatter_kernel(StreamChunkScatterLaunch a) {
         }
         const int j = a.idx[b] - a.j0;
         if (j < 0 || j >= a.nsess) continue;
-        a.dst[i] = n0 + k < a.la ? 0.f : a.src[(size_t)j * plane + i % plane];
+        const size_t e = i % plane;                                 // (o, f, k) of the dst plane
+        a.dst[i] = (n0 + k < a.la || k >= a.Ks) ? 0.f : a.src[(size_t)j * 2 * a.F * a.Ks + e / a.K * a.Ks + k];
     }
 }
 void launch_stream_chunk_scatter(const StreamChunkScatterLaunch& a, cudaStream_t s) {

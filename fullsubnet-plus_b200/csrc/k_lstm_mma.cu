@@ -52,17 +52,25 @@ __global__ void __launch_bounds__(256, 1) lstm_mma_kernel(LstmMmaLaunch a) {
     }
     if (a.out) for (int i = tid; i < a.O * H; i += blockDim.x) fcw[i] = a.w.fc_w[i];
     // streaming slot call: bit 2 mt + half = the row this thread updates in row tile mt (lane / 4, + 8 for half 1) is held
+    // (and kf: from step hf[i] on it holds too)
     unsigned held = 0;
+    int hf[2 * MT];
     if (SLOTS)
 #pragma unroll
         for (int i = 0; i < 2 * MT; ++i) {
             const int grow = row0 + (i >> 1) * 16 + (lane >> 2) + (i & 1) * 8;
             if (grow < a.rows && a.slot[grow / a.slot_rows] < 0) held |= 1u << i;
+            hf[i] = (grow < a.rows && a.kf) ? a.kf[grow / a.slot_rows] : Tp;
         }
     __syncthreads();
 
     for (int t = 0; t < Tp; ++t) {
         const int p = t & 1;
+        unsigned hold = held;                                            // the rows held at this step
+        if (SLOTS)
+#pragma unroll
+            for (int i = 0; i < 2 * MT; ++i)
+                if (t >= hf[i]) hold |= 1u << i;
         // ---- stage x_t rows ------------------------------------------------------------------
         {
             const int cpr = Ipad / 8;                                    // 16-byte chunks per row
@@ -130,8 +138,12 @@ __global__ void __launch_bounds__(256, 1) lstm_mma_kernel(LstmMmaLaunch a) {
                         float c, h;
                         if (a.gru) { h = gru_cell_plain<FAST>(gi, gf, gg, go, cprev); c = h; }
                         else { c = sigm<FAST>(gf) * cprev + sigm<FAST>(gi) * tanh_<FAST>(gg); h = sigm<FAST>(go) * tanh_<FAST>(c); }
-                        if (!SLOTS || !((held >> (2 * mt + (q >> 1))) & 1u)) cst[ci] = c;
-                        hout[(size_t)r * HS + u] = __float2half_rn(h);
+                        if (!SLOTS || !((hold >> (2 * mt + (q >> 1))) & 1u)) {
+                            cst[ci] = c;
+                            hout[(size_t)r * HS + u] = __float2half_rn(h);
+                        } else {
+                            hout[(size_t)r * HS + u] = seg1[(size_t)r * HS + u];   // held: its h carries into this step's parity
+                        }
                         if (top && a.hseq && row0 + r < a.rows) a.hseq[((size_t)(row0 + r) * H + u) * a.P + t] = h;
                     }
             }
@@ -145,7 +157,8 @@ __global__ void __launch_bounds__(256, 1) lstm_mma_kernel(LstmMmaLaunch a) {
                 if (grow >= a.rows) continue;
                 const int b = grow / a.F, f = grow % a.F;
                 const int sn = SLOTS ? a.slot[grow / a.slot_rows] : 0;  // the slot's count: frame t is its frame sn + t
-                if ((a.tlen && t >= a.tlen[b]) || (SLOTS && (sn < 0 || sn + t < a.slot_la))) {   // past the clip's end; held; no valid mask
+                if ((a.tlen && t >= a.tlen[b]) || (SLOTS && (sn < 0 || sn + t < a.slot_la || (a.kf && t >= a.kf[grow / a.slot_rows])))) {
+                    // past the clip's end; held; no valid mask
                     a.out[(((size_t)b * a.O + o) * a.F + f) * (Tp - a.la) + (t - a.la)] = 0.f;
                     continue;
                 }

@@ -86,10 +86,15 @@ __global__ void __launch_bounds__(WS_THREADS, 1) lstm_ws_kernel(LstmWsLaunch a) 
         }
     }
     // streaming slot call: rows r0 / r0 + 8 held (they keep cst and carry their previous h forward)
+    // (and kf: from step hf[rr] on)
     bool held[2] = {false, false};
+    int hf[2] = {Tp, Tp};
     if (SLOTS)
 #pragma unroll
-        for (int rr = 0; rr < 2; ++rr) held[rr] = r0 + rr * 8 < a.rows && a.slot[r0 + rr * 8] < 0;
+        for (int rr = 0; rr < 2; ++rr) {
+            held[rr] = r0 + rr * 8 < a.rows && a.slot[r0 + rr * 8] < 0;
+            if (a.kf && r0 + rr * 8 < a.rows) hf[rr] = a.kf[r0 + rr * 8];
+        }
     __syncthreads();
 
     unsigned int bar_target = 0;
@@ -131,7 +136,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) lstm_ws_kernel(LstmWsLaunch a) 
                 __half* hout = a.hbuf + ((size_t)l * 2 + par) * WS_ROWS * H;
 #pragma unroll
                 for (int rr = 0; rr < 2; ++rr) {
-                    if (SLOTS && held[rr]) {                                  // h_prev (A tile column K0 + unit) into this step's parity
+                    if (SLOTS && (held[rr] || t >= hf[rr])) {                                  // h_prev (A tile column K0 + unit) into this step's parity
                         const int row = r0 + rr * 8;
                         hout[(size_t)row * H + unit] = asm_[(size_t)row * KA + K0 + unit];
                         continue;

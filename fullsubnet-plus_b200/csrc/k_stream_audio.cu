@@ -1,9 +1,11 @@
-// Audio in and out of the streaming slot call (fsn_stream_step_audio_slots, DESIGN.md §3.10): per slot and tick, the analysis kernel
-// turns one hop of samples into one frame of torch.stft(center=True, reflect, periodic Hann), and the synthesis kernel turns the mask
-// the model step produced into one hop of torch.istft output (decompress_cIRM x noisy spectrum, inverse real FFT, window, overlap-add,
-// division by the window envelope).  One CTA per slot; the real FFTs of n_fft points run as complex FFTs of n_fft / 2 points
-// (radix 2, fp32, in shared memory, fsn_fft.cuh) with the even / odd split folded in.  The tables (window, twiddles, 1 / envelope) are
-// computed in double on the host once per handle (audio_tables).
+// Audio in and out of the streaming slot calls (DESIGN.md §3.10, §3.14): per slot and tick, the analysis turns one hop of samples into
+// one frame of torch.stft(center=True, reflect, periodic Hann), and the synthesis turns the mask the model step produced into one hop
+// of torch.istft output (decompress_cIRM x noisy spectrum, inverse real FFT, window, overlap-add, division by the window envelope).
+// One CTA per slot; the real FFTs of n_fft points run as complex FFTs of n_fft / 2 points (radix 2, fp32, in shared memory,
+// fsn_fft.cuh) with the even / odd split folded in.  The tables (window, twiddles, 1 / envelope) are computed in double on the host
+// once per handle (audio_tables).  The per-hop call (fsn_stream_step_audio_slots) runs one tick per launch; the chunk call
+// (fsn_stream_step_audio_chunk) runs each slot's ticks of the call in order inside its CTA, through the same frame helpers, so both
+// give the same bits.
 #include "fsn_common.cuh"
 #include "fsn_fft.cuh"
 #include "fsn_kernels.h"
@@ -13,10 +15,61 @@ namespace fsn {
 constexpr int AUDIO_THREADS = 128;
 constexpr int AUDIO_MAX_HOP = 512;                              // n_fft <= 1024
 
+// Frame j of a session from its history ring hist [3, H] (hop q at q % 3): original samples [H (j - 1), H (j + 1)) reflected at 0 and,
+// with L > 0 (the session's length), at L - 1.  Spectrum to spec[f], magnitude to mag[f ms].  z: shared scratch of H points.
+__device__ __forceinline__ void analyse_frame(const float* hist, int j, int L, int H, int lg, const float* __restrict__ window,
+                                              const float2* __restrict__ twiddle, float2* z, float2* spec, float* mag, int ms) {
+    for (int n = threadIdx.x; n < H; n += blockDim.x) {          // z[n] = x[2n] + i x[2n + 1], windowed, stored bit-reversed
+        float v[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            int p = H * (j - 1) + 2 * n + e;
+            if (p < 0) p = -p;
+            if (L && p >= L) p = 2 * (L - 1) - p;
+            v[e] = hist[((p / H) % 3) * H + p % H] * __ldg(window + 2 * n + e);
+        }
+        z[bitrev(n, lg)] = make_float2(v[0], v[1]);
+    }
+    __syncthreads();
+    fft_dit<false>(z, twiddle, H);
+    for (int f = threadIdx.x; f <= H; f += blockDim.x) {
+        const float2 X = rfft_split(z[f & (H - 1)], z[(H - f) & (H - 1)], __ldg(twiddle + f));
+        spec[f] = X;
+        mag[f * ms] = hypotf(X.x, X.y);
+    }
+}
+
+// Synthesis of one frame from its mask rows mask[f ms], mask[(F + f) ms] and noisy spectrum spec: the second half of the windowed
+// inverse transform becomes the tail; with emit, out[i] = (tail + first half) / env (the session's next hop), else out[i] = 0.
+// z, e: shared scratch of H and H + 1 points.
+__device__ __forceinline__ void synth_frame(const float* mask, int ms, const float2* spec, float* tail, float* out, bool emit, int H,
+                                            int lg, const float* __restrict__ window, const float2* __restrict__ twiddle,
+                                            const float* __restrict__ inv_env, float2* z, float2* e) {
+    const int F = H + 1;
+    for (int f = threadIdx.x; f < F; f += blockDim.x) {          // decompress_cIRM x noisy spectrum (inferencer.py:152-157)
+        const float m0 = decompress_cirm(mask[f * ms]), m1 = decompress_cirm(mask[(F + f) * ms]);
+        const float2 x = spec[f];
+        float2 E = make_float2(m0 * x.x - m1 * x.y, m1 * x.x + m0 * x.y);
+        if (f == 0 || f == H) E.y = 0.f;                         // a real inverse transform ignores the DC and Nyquist imaginary parts
+        e[f] = E;
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < H; k += blockDim.x) z[bitrev(k, lg)] = irfft_split(e[k], e[H - k], __ldg(twiddle + k));
+    __syncthreads();
+    fft_dit<true>(z, twiddle, H);
+    const float* y = reinterpret_cast<const float*>(z);
+    const float s = 1.0f / (float)H;
+    for (int i = threadIdx.x; i < H; i += blockDim.x) {
+        const float lo = y[i] * s * __ldg(window + i), hi = y[H + i] * s * __ldg(window + H + i);
+        if (emit) out[i] = (tail[i] + lo) * __ldg(inv_env + i);
+        else out[i] = 0.f;
+        tail[i] = hi;
+    }
+}
+
 // grid B: analysis of one tick.  STORE: the slot's hop goes to its history ring (hop q at q % 3).  FRAME: frame j = tick - 1 of the
-// session, original samples [hop (j - 1), hop (j + 1)) reflected at 0 and, once the session's length is known, at L - 1; its spectrum
-// goes to the ring (frame j at j % (la + 1)) and its magnitude to the model's input row.  ZERO: the same two rows are zero (the
-// right padding of the look-ahead).  A slot without an op touches nothing.
+// session; its spectrum goes to the ring (frame j at j % (la + 1)) and its magnitude to the model's input row.  ZERO: the same two
+// rows are zero (the right padding of the look-ahead).  A slot without an op touches nothing.
 __global__ void __launch_bounds__(AUDIO_THREADS) stream_stft_kernel(StreamAudioLaunch a) {
     __shared__ float2 z[AUDIO_MAX_HOP];
     const int b = blockIdx.x, op = a.op[b];
@@ -36,25 +89,7 @@ __global__ void __launch_bounds__(AUDIO_THREADS) stream_stft_kernel(StreamAudioL
         for (int f = threadIdx.x; f < F; f += blockDim.x) { spec[f] = make_float2(0.f, 0.f); mag[f] = 0.f; }
         return;
     }
-    const int L = a.hops[b] * H;                                 // 0 while the session's length is unknown
-    for (int n = threadIdx.x; n < H; n += blockDim.x) {          // z[n] = x[2n] + i x[2n + 1], windowed, stored bit-reversed
-        float v[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-            int p = H * (j - 1) + 2 * n + e;
-            if (p < 0) p = -p;
-            if (L && p >= L) p = 2 * (L - 1) - p;
-            v[e] = hist[((p / H) % 3) * H + p % H] * __ldg(a.window + 2 * n + e);
-        }
-        z[bitrev(n, lg)] = make_float2(v[0], v[1]);
-    }
-    __syncthreads();
-    fft_dit<false>(z, a.twiddle, H);
-    for (int f = threadIdx.x; f < F; f += blockDim.x) {
-        const float2 X = rfft_split(z[f & (H - 1)], z[(H - f) & (H - 1)], __ldg(a.twiddle + f));
-        spec[f] = X;
-        mag[f] = hypotf(X.x, X.y);
-    }
+    analyse_frame(hist, j, a.hops[b] * H, H, lg, a.window, a.twiddle, z, spec, mag, 1);
 }
 
 // grid B: synthesis of one tick.  SYNTH: frame m = tick - 1 - la from the mask row the model step wrote this tick and the spectrum
@@ -72,31 +107,86 @@ __global__ void __launch_bounds__(AUDIO_THREADS) stream_istft_kernel(StreamAudio
     }
     const int m = a.tick[b] - 1 - a.la;
     const float2* spec = a.spec + ((size_t)b * (a.la + 1) + m % (a.la + 1)) * F;
-    const float* mask = a.mask + (size_t)b * 2 * F;
-    for (int f = threadIdx.x; f < F; f += blockDim.x) {          // decompress_cIRM x noisy spectrum (inferencer.py:152-157)
-        const float m0 = decompress_cirm(mask[f]), m1 = decompress_cirm(mask[F + f]);
-        const float2 x = spec[f];
-        float2 E = make_float2(m0 * x.x - m1 * x.y, m1 * x.x + m0 * x.y);
-        if (f == 0 || f == H) E.y = 0.f;                         // a real inverse transform ignores the DC and Nyquist imaginary parts
-        e[f] = E;
+    synth_frame(a.mask + (size_t)b * 2 * F, 1, spec, a.tail + (size_t)b * H, out, op & AUDIO_EMIT, H, lg, a.window, a.twiddle, a.inv_env,
+                z, e);
+}
+
+// The model planes' address of slot b's column c (row 0 of its rows rows): [B, rows, Km]
+__device__ __forceinline__ size_t chunk_col(const StreamAudioChunkLaunch& a, int b, int c, int rows) {
+    return ((size_t)b * rows) * a.Km + c;
+}
+
+// grid B: the analysis of a slot's active ticks, in order.  Stored hops go to the history ring as the per-hop kernel stores them; the
+// spectrum of model column c goes to the scratch sspec (the ring still holds the frames the synthesis of this call reads), its
+// magnitude to the model's input.  Frames past the session's end (j > K) are zero.
+__global__ void __launch_bounds__(AUDIO_THREADS) stream_stft_chunk_kernel(StreamAudioChunkLaunch a) {
+    __shared__ float2 z[AUDIO_MAX_HOP];
+    const int b = blockIdx.x, na = a.na[b];
+    const int H = a.n_fft >> 1, F = H + 1, lg = 31 - __clz(H), k0 = a.k0[b], st = a.start[b], ns = a.nstore[b], K = a.hops[b];
+    float* hist = a.hist + (size_t)b * 3 * H;
+    const float* x = a.samples + (size_t)b * a.K * H;
+    for (int i = 0; i < na; ++i) {
+        const int k = k0 + i;
+        __syncthreads();                                         // the last tick's reads of hist and z are done
+        if (i < ns) {
+            for (int t = threadIdx.x; t < H; t += blockDim.x) hist[(k % 3) * H + t] = x[(size_t)i * H + t];
+            __syncthreads();
+        }
+        if (i < st) continue;                                    // a START stores hop 0 and analyses no frame
+        const int c = i - st, j = k - 1;
+        float2* spec = a.sspec + ((size_t)b * a.K + c) * F;
+        float* mag = a.mag + chunk_col(a, b, c, F);
+        const int ms = a.Km;
+        if (K && j > K) {
+            for (int f = threadIdx.x; f < F; f += blockDim.x) { spec[f] = make_float2(0.f, 0.f); mag[f * ms] = 0.f; }
+        } else {
+            analyse_frame(hist, j, K * H, H, lg, a.window, a.twiddle, z, spec, mag, ms);
+        }
     }
-    __syncthreads();
-    for (int k = threadIdx.x; k < H; k += blockDim.x) z[bitrev(k, lg)] = irfft_split(e[k], e[H - k], __ldg(a.twiddle + k));
-    __syncthreads();
-    fft_dit<true>(z, a.twiddle, H);
-    const float* y = reinterpret_cast<const float*>(z);
-    const float s = 1.0f / (float)H;
+}
+
+// grid B: the synthesis of a slot's model columns, in order.  Column c synthesises frame m = j - la (if m >= 0) from its mask and the
+// spectrum of frame m: from the scratch if this call analysed it, else from the ring.  Emitted hops fill the front of the output row
+// and the rest is zero.  Then the caller's masks by tick (zero on the START tick and past the active ticks) and the ring's last la + 1
+// frames, written only after every read of the ring.
+__global__ void __launch_bounds__(AUDIO_THREADS) stream_istft_chunk_kernel(StreamAudioChunkLaunch a) {
+    __shared__ float2 z[AUDIO_MAX_HOP];
+    __shared__ float2 e[AUDIO_MAX_HOP + 1];
+    const int b = blockIdx.x, na = a.na[b], st = a.start[b], K = a.K, R = a.la + 1;
+    const int H = a.n_fft >> 1, F = H + 1, lg = 31 - __clz(H);
+    const int kf = na > st ? na - st : 0, j0 = a.k0[b] + st - 1;  // model columns, the frame of column 0
+    float* out = a.out + (size_t)b * K * H;
     float* tail = a.tail + (size_t)b * H;
-    const bool emit = op & AUDIO_EMIT;
-    for (int i = threadIdx.x; i < H; i += blockDim.x) {
-        const float lo = y[i] * s * __ldg(a.window + i), hi = y[H + i] * s * __ldg(a.window + H + i);
-        if (emit) out[i] = (tail[i] + lo) * __ldg(a.inv_env + i);
-        else out[i] = 0.f;
-        tail[i] = hi;
+    float2* ring = a.spec + (size_t)b * R * F;
+    const float2* sspec = a.sspec + (size_t)b * K * F;
+    int nout = 0;
+    for (int c = 0; c < kf; ++c) {
+        const int m = j0 + c - a.la;
+        if (m < 0) continue;
+        __syncthreads();                                         // the last frame's reads of z and e are done
+        const float2* spec = m >= j0 ? sspec + (size_t)(m - j0) * F : ring + (m % R) * F;
+        synth_frame(a.mask + chunk_col(a, b, c, 2 * F), a.Km, spec, tail, out + (size_t)nout * H, m >= 1, H, lg, a.window,
+                    a.twiddle, a.inv_env, z, e);
+        nout += m >= 1;
+    }
+    for (size_t t = (size_t)nout * H + threadIdx.x; t < (size_t)K * H; t += blockDim.x) out[t] = 0.f;
+    if (a.umask) {
+        float* um = a.umask + (size_t)b * 2 * F * K;
+        for (size_t t = threadIdx.x; t < (size_t)2 * F * K; t += blockDim.x) {
+            const int r = (int)(t / K), i = (int)(t % K), c = i - st;
+            um[t] = (i >= st && i < na) ? a.mask[chunk_col(a, b, c, 2 * F) + (size_t)r * a.Km] : 0.f;
+        }
+    }
+    __syncthreads();                                             // every read of the ring is done
+    for (int t = threadIdx.x; t < R * F; t += blockDim.x) {
+        const int c = kf - R + t / F, f = t % F;
+        if (c >= 0) ring[((j0 + c) % R) * F + f] = sspec[(size_t)c * F + f];
     }
 }
 
 void launch_stream_stft(const StreamAudioLaunch& a, cudaStream_t s) { stream_stft_kernel<<<a.B, AUDIO_THREADS, 0, s>>>(a); }
 void launch_stream_istft(const StreamAudioLaunch& a, cudaStream_t s) { stream_istft_kernel<<<a.B, AUDIO_THREADS, 0, s>>>(a); }
+void launch_stream_stft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s) { stream_stft_chunk_kernel<<<a.B, AUDIO_THREADS, 0, s>>>(a); }
+void launch_stream_istft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s) { stream_istft_chunk_kernel<<<a.B, AUDIO_THREADS, 0, s>>>(a); }
 
 }  // namespace fsn

@@ -25,7 +25,7 @@ SYMBOLS = [
     "fsn_stream_step_slots", "fsn_stream_step_audio_slots",
     "fsn_stream_state_bytes", "fsn_stream_state_layout", "fsn_model_weights_id", "fsn_stream_save_slots", "fsn_stream_load_slots",
     "fsn_model_enhance_audio", "fsn_plan_audio",
-    "fsn_stream_step_chunk", "fsn_stream_chunk_plan",
+    "fsn_stream_step_chunk", "fsn_stream_chunk_plan", "fsn_stream_step_audio_chunk",
 ]
 
 
@@ -102,6 +102,7 @@ def load_library():
     lib.fsn_stream_step_slots.argtypes = [vp, vp, vp, vp, vp, vp]
     lib.fsn_stream_step_audio_slots.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.fsn_stream_step_chunk.argtypes = [vp, vp, i32, vp, vp, vp, vp]
+    lib.fsn_stream_step_audio_chunk.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp, vp]
     lib.fsn_stream_chunk_plan.argtypes = [C.POINTER(FsnConfig), i32, i32, C.c_double, C.POINTER(i32), C.POINTER(i32), C.POINTER(i64)]
     lib.fsn_stream_destroy.argtypes = [vp]
     lib.fsn_stream_destroy.restype = None

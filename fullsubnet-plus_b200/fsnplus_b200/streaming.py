@@ -14,7 +14,8 @@ where the configuration takes them (DESIGN.md §3.13); it mixes freely with ``st
 
 ``step_audio`` serves the same sessions with audio in and out: one hop of samples per slot and tick goes in, one hop of enhanced
 audio comes out, with the STFT, the cIRM and the overlap-add iSTFT on the device (flag FLUSH ends a session, DESIGN.md §3.10).
-A handle serves either the mask calls or the audio call.
+``step_audio_chunk`` advances audio sessions many hops per call: each slot brings its own number of hops, and the call equals that
+many ``step_audio`` ticks on the slot (DESIGN.md §3.14).  A handle serves either the mask calls or the audio calls.
 
 ``save_slots`` / ``load_slots`` park, resume and move sessions (DESIGN.md §3.11): a ``SessionState`` holds the saved state of some
 slots, and loading it into any slot of a handle of the same model -- this one, one with another B, or one on another GPU -- continues
@@ -167,6 +168,31 @@ class StreamingFullSubNet:
                                                             C.c_void_p(f.data_ptr()), C.c_void_p(valid.data_ptr()),
                                                             C.c_void_p(mask.data_ptr() if return_mask else None), stream))
         return (out, valid.bool(), mask) if return_mask else (out, valid.bool())
+
+    def step_audio_chunk(self, samples, flags, hops, return_mask=False):
+        """Up to K hops per slot in one call (DESIGN.md §3.14).  samples [B, K hop] float32 CUDA: slot b's hops[b] new hops at the front
+        of its row (nothing else is read); flags, hops: B values each (sequences or CPU integer tensors).  For slot b the call is K
+        ``step_audio`` ticks: HOLD x K; START, STEP x (n - 1), HOLD...; STEP x n, HOLD...; or STEP x n, FLUSH... (n = hops[b], 1..K,
+        or 0..K for FLUSH).  Returns (audio [B, K hop], nout int32 CPU tensor [B]): the nout[b] hops the ticks emitted at the front of
+        row b, zero after them; plus the masks [B, 2, F, K] with return_mask, column i being tick i's mask row."""
+        assert samples.dim() == 2 and samples.shape[0] == self.B and samples.shape[1] % self.hop == 0 and samples.is_cuda
+        K = samples.shape[1] // self.hop
+        f = torch.as_tensor(flags, dtype=torch.int32)
+        n = torch.as_tensor(hops, dtype=torch.int32)
+        assert f.device.type == "cpu" and f.shape == (self.B,), "flags: B host values"
+        assert n.device.type == "cpu" and n.shape == (self.B,), "hops: B host values"
+        f, n = f.contiguous(), n.contiguous()
+        x = samples.contiguous().float()
+        out = torch.empty((self.B, K * self.hop), dtype=torch.float32, device=self.device)
+        mask = torch.empty((self.B, 2, self.F, K), dtype=torch.float32, device=self.device) if return_mask else None
+        nout = torch.zeros(self.B, dtype=torch.int32)
+        with torch.cuda.device(self.device):
+            stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+            _lib.check(self.lib.fsn_stream_step_audio_chunk(self._st, C.c_void_p(x.data_ptr()), K, C.c_void_p(f.data_ptr()),
+                                                            C.c_void_p(n.data_ptr()), C.c_void_p(out.data_ptr()),
+                                                            C.c_void_p(nout.data_ptr()),
+                                                            C.c_void_p(mask.data_ptr() if return_mask else None), stream))
+        return (out, nout, mask) if return_mask else (out, nout)
 
     def _slot_array(self, slots):
         s = torch.as_tensor(slots, dtype=torch.int32).reshape(-1).contiguous()

@@ -264,6 +264,28 @@ int fsn_stream_chunk_plan(const fsn_config* cfg, int32_t n_active, int32_t K, do
 int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_samples, float* d_out, const int32_t* h_flags, int32_t* h_valid,
                                 float* d_mask, void* stream);
 
+/* Many hops per call (DESIGN.md §3.14): audio in and out, K hops per slot, for callers that hold audio buffers of 8-64 hops or catch
+ * a session up after a stall.  For slot b the call is exactly K fsn_stream_step_audio_slots ticks on that slot, by h_flags[b] and
+ * n = h_hops[b] (HOST arrays of B values):
+ *   HOLD: HOLD x K (h_hops ignored);  START (1 <= n <= K): START, STEP x (n - 1), HOLD x (K - n);  STEP (1 <= n <= K): STEP x n,
+ *   HOLD x (K - n);  FLUSH (0 <= n <= K): STEP x n, FLUSH x (K - n) -- the input ends after these n hops.
+ * A session ends within a FLUSH call when n + look_ahead + 2 <= K; otherwise further FLUSH calls with n = 0 complete it.  A session
+ * that STARTs and FLUSHes takes two calls.
+ * d_samples [B, K hop] float32 device: slot b's n new hops at the front of its row; no other sample is read.  d_out [B, K hop] float32
+ * device: the hops those ticks emit, in order, at the front of the row, zero after them; h_nout (HOST, [B]) their count.  d_mask: null,
+ * or [B, 2, F, K] float32 device, whose column i is the mask row of tick i (zero on HOLD ticks, the START tick and before frame 0).
+ * The slot's state and counters afterwards are those the K ticks leave, so this call, fsn_stream_step_audio_slots and save / load mix
+ * freely on one handle.  The model steps each session's frames of the call on the chunk call's path (fsn_stream_step_chunk: the
+ * layer-wise sub band where the configuration takes it, else bit-identical to the per-hop call).  The scratch belongs to the handle:
+ * allocated at the first call, grow-only, freed by fsn_stream_destroy.
+ * FSN_EINVAL naming the slot for a flag outside {0, 1, 2, 3}, h_hops outside the range above, a STEP or FLUSH on a slot that has no
+ * session, a STEP or a FLUSH with n > 0 after the session's FLUSH, and a FLUSH that would end a session of fewer than 2 hops; naming the
+ * argument for a null array and K < 1; naming the limit for K past fsn_stream_step_chunk's limits or K x hop past 2^31 - 1.  FSN_ESTATE
+ * on a handle that serves the mask calls.  A failed call changes no state.  The host arrays are free when the call returns; the call
+ * does not synchronise the stream. */
+int fsn_stream_step_audio_chunk(fsn_stream* st, const float* d_samples, int32_t K, const int32_t* h_flags, const int32_t* h_hops,
+                                float* d_out, int32_t* h_nout, float* d_mask, void* stream);
+
 /* Park, resume and move sessions (DESIGN.md §3.11): save the state of some slots to a device buffer and load it into any slot of a
  * compatible handle -- the same one, another with a different B or full-band kernel, or one on another device after the caller has
  * copied the payload there.

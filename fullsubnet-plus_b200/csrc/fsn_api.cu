@@ -180,6 +180,7 @@ struct fsn_model {
     TcnScratch sb_scratch;
     int64_t launches = 0;
     int last_impl = 0;
+    int last_fb_ws = 0;                 // the last forward's full-band LSTM ran on the weight-stationary kernel (fsn_model_last_fb_ws)
     // tuning knobs, read ONCE at fsn_model_create (never on the forward path): FSN_LSTM_IMPL overrides cfg.lstm_impl,
     // FSN_NO_WS=1 keeps the full-band LSTM of fullsubnet.Model off the weight-stationary kernel
     int env_impl = 0;
@@ -1213,6 +1214,7 @@ static int forward_impl(fsn_model* m, Lane& ln, const float* d_mag, const float*
             for (int b = 0; b < 3; ++b) ta.x[b] = static_cast<const float*>(ln.xn.p) + (size_t)b * B * F * Tp;
             ta.T = Tp; ta.prenorm = 1;                                  // padded frames are part of the normalised signal
         }
+        m->last_fb_ws = 0;
         const TcnWeights& w = m->tcn_fb;
         CK(cudaMemsetAsync(ln.tcn.stats.p, 0, tcn_stats_bytes(3 * B), s));
         ta.amax = tcn_amax(ln.tcn.stats.p, 3 * B, 0);                  // block 0: written by the gate kernel
@@ -1254,7 +1256,8 @@ static int forward_impl(fsn_model* m, Lane& ln, const float* d_mag, const float*
         // sub-band stages
         const int Ipad = (F + 15) / 16 * 16, rows_pad = (B + 63) / 64 * 64;
         launch_fb_pack(static_cast<const float*>(ln.fbin.p), static_cast<__half*>(ln.fbx.p), B, F, Tp, Pp, rows_pad, Ipad, s); m->launches++;
-        if (lstm_ws_supported(c.num_layers, c.fb_hidden, Ipad, B, m->num_sms) && !m->env_no_ws) {
+        m->last_fb_ws = lstm_ws_supported(c.num_layers, c.fb_hidden, Ipad, B, m->num_sms) && !m->env_no_ws;
+        if (m->last_fb_ws) {
             const size_t hb = (size_t)c.num_layers * 2 * 64 * c.fb_hidden * 2;
             if (m->ws_h.ensure(hb, false, s) || m->ws_bar.ensure(64, true, s)) return fail(FSN_ECUDA, "allocation failed");
             CK(cudaMemsetAsync(m->ws_h.p, 0, hb, s));
@@ -2808,6 +2811,7 @@ extern "C" float fsn_model_last_lstm_ms(fsn_model* m) {
     return fsn_model_lstm_ms_history(m, &ms, 1) == 1 ? ms : -1.f;
 }
 extern "C" int fsn_model_last_lstm_impl(const fsn_model* m) { return m ? m->last_impl : 0; }
+extern "C" int fsn_model_last_fb_ws(const fsn_model* m) { return m ? m->last_fb_ws : 0; }
 
 static int put_plan(const Plan& p, int32_t* Bs, int32_t* Tw, int32_t* Fc, int64_t* bytes) {
     *Bs = p.Bs; *Tw = p.Tw; *Fc = p.Fc;

@@ -16,7 +16,7 @@ ATTENTION = {"TSSE": 0, "SE": 1, "CBAM": 2, "ECA": 3}     # FSN_ATTN_* (referenc
 SYMBOLS = [
     "fsn_version", "fsn_last_error", "fsn_model_create", "fsn_model_destroy", "fsn_model_set_param",
     "fsn_model_num_params", "fsn_model_param_info", "fsn_model_finalize", "fsn_model_forward",
-    "fsn_model_forward_host", "fsn_model_forward_host_async", "fsn_model_sync_host", "fsn_model_submit", "fsn_model_wait", "fsn_model_forward_enhance", "fsn_model_submit_enhance", "fsn_model_forward_ragged", "fsn_model_forward_enhance_ragged", "fsn_model_last_lane", "fsn_model_wait_lane", "fsn_apply_cirm", "fsn_stream_create", "fsn_stream_step", "fsn_stream_destroy", "fsn_model_get_stage", "fsn_model_last_launch_count", "fsn_model_last_lstm_impl", "fsn_model_last_lstm_ms", "fsn_model_lstm_ms_history", "fsn_model_timeline",
+    "fsn_model_forward_host", "fsn_model_forward_host_async", "fsn_model_sync_host", "fsn_model_submit", "fsn_model_wait", "fsn_model_forward_enhance", "fsn_model_submit_enhance", "fsn_model_forward_ragged", "fsn_model_forward_enhance_ragged", "fsn_model_last_lane", "fsn_model_wait_lane", "fsn_apply_cirm", "fsn_stream_create", "fsn_stream_step", "fsn_stream_destroy", "fsn_model_get_stage", "fsn_model_last_launch_count", "fsn_model_last_lstm_impl", "fsn_model_last_fb_ws", "fsn_model_last_lstm_ms", "fsn_model_lstm_ms_history", "fsn_model_timeline",
     "fsn_plan_forward", "fsn_model_workspace_bytes", "fsn_model_last_plan", "fsn_model_plan", "fsn_model_release_workspace",
     "fsn_plan_forward_bins", "fsn_model_plan_bins", "fsn_model_last_plan_bins",
     "fsn_sw128_offset", "fsn_tc5_weight_stream_bytes", "fsn_tc5_pack_weights", "fsn_tc5_gate_row", "fsn_tc5r_weight_stream_bytes", "fsn_tc5r_pack_layer",
@@ -118,6 +118,7 @@ def load_library():
     lib.fsn_model_last_launch_count.argtypes = [vp]
     lib.fsn_model_last_launch_count.restype = i64
     lib.fsn_model_last_lstm_impl.argtypes = [vp]
+    lib.fsn_model_last_fb_ws.argtypes = [vp]
     lib.fsn_model_last_lstm_ms.argtypes = [vp]
     lib.fsn_model_last_lstm_ms.restype = C.c_float
     lib.fsn_model_lstm_ms_history.argtypes = [vp, fp, i32]

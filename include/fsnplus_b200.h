@@ -360,6 +360,10 @@ int fsn_model_lstm_ms_history(fsn_model* m, float* h_ms, int32_t n);
 int fsn_model_timeline(fsn_model* m, float* h_ms4, int32_t n);
 /* Which implementation the last forward used for the sub-band model (FSN_LSTM_MMA / _TCGEN05 / _TCN). */
 int fsn_model_last_lstm_impl(const fsn_model* m);
+/* Test-only: 1 if the last forward of a fullsubnet.Model ran its full-band LSTM on the weight-stationary kernel (k_lstm_ws.cu), 0 if
+ * on the generic mma kernel, for a FullSubNet_Plus (whose full band is the TCN) or before any forward.  Lets the element-wise tests
+ * assert which kernel they checked. */
+int fsn_model_last_fb_ws(const fsn_model* m);
 
 /* Long clips (DESIGN.md §3.7).  The plain entry points (fsn_model_forward, _enhance, both _ragged ones, fsn_model_forward_host) plan
  * every call so that its forward workspace stays within FSN_WS_CAP_GB (default 24): a batch that fits runs whole or as equal

@@ -2,12 +2,17 @@
 
 The stage is sb_model of the reference: nn.LSTM / nn.GRU (batch_first) -> Linear(H -> 2) -> output activation, the first
 look_ahead frames dropped (sequence_model.py:113-122, fullsubnet_plus.py:200-208).  Both references read the model's own
-state_dict (sb_model.sequence_model.*, sb_model.fc_output_layer.*), so the parameter packing is under test as well.
+state_dict (<prefix>.sequence_model.*, <prefix>.fc_output_layer.*), so the parameter packing is under test as well.  With
+prefix="fb_model", head="fb" they check the full-band LSTM / GRU of fullsubnet.Model instead (fullsubnet.py:86-87): Linear(H -> F) +
+fb_output_activate_function on every frame (conv1x1_tf32_kernel, k_front.cu), no look-ahead drop.
 
 * truth():   torch.nn.LSTM / torch.nn.GRU in float64.
 * emulate(): the same recurrence in float64, rounded where the kernels round: W_ih and W_hh to fp16, h to fp16 after every step,
              the input projection Gin of layers >= 1 to fp16 (the GEMM's fp16 output), the carried c (GRU: h) to fp32.  Its distance
-             from truth() on the same elements is the error the kernels' number formats make unavoidable.  ``fault`` plants one of
+             from truth() on the same elements is the error the kernels' number formats make unavoidable.  Full band: fb_pack
+             (k_front.cu) rounds the fp32 input to fp16 first, Gin of the deeper layers stays in fp32 (k_lstm_ws.cu and lstm_mma_kernel
+             accumulate it with the recurrent product), and the head reads the top layer's fp32 h (hseq), both operands rounded to
+             tf32 (cvt.rna) by conv1x1_tf32_kernel.  ``fault`` plants one of
              the bugs the rule must catch (test_sb_recurrence_cpu.py).
 
 Rule (compare()): err = |kernel - truth| per element; max err <= factor * (3 max |emulation - truth| + 1e-6 RMS), factor = 1 for
@@ -15,6 +20,8 @@ accurate gate math, FAST_FACTOR for fast math (tanh.approx, which the emulation 
 """
 import numpy as np
 import torch
+
+import tcn_ref
 
 # Fast-math gates (tanh.approx, max rel. error 2^-11) on top of the fp16 rounding the emulation models: the accurate bound is
 # multiplied by this factor.  Measured once on one H100 80GB HBM3 SXM (700 W power limit): the kernels' max err reached at most 1.15x
@@ -44,25 +51,34 @@ def _sd(sd, key, device):
     return v.to(device=device, dtype=torch.float64)
 
 
-def num_layers(sd):
-    return sum(1 for k in sd if k.startswith("sb_model.sequence_model.weight_ih_l"))
+def num_layers(sd, prefix="sb_model"):
+    return sum(1 for k in sd if k.startswith(f"{prefix}.sequence_model.weight_ih_l"))
 
 
-def layers(sd, device="cpu"):
+def layers(sd, device="cpu", prefix="sb_model"):
     """[(w_ih, w_hh, b_ih, b_hh)] per layer, float64, reference (nn.LSTM / nn.GRU) layout."""
-    p = "sb_model.sequence_model."
-    return [tuple(_sd(sd, f"{p}{n}_l{l}", device) for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh")) for l in range(num_layers(sd))]
+    p = f"{prefix}.sequence_model."
+    return [tuple(_sd(sd, f"{p}{n}_l{l}", device) for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"))
+            for l in range(num_layers(sd, prefix))]
 
 
-def _head(sd, y, look_ahead, act, device):
-    """y: [N, Tp, H] -> act(Linear(y)) without the first look_ahead frames, as [N, 2, Tp - look_ahead]."""
-    w, b = _sd(sd, "sb_model.fc_output_layer.weight", device), _sd(sd, "sb_model.fc_output_layer.bias", device)
-    return _act(y[:, look_ahead:] @ w.T + b, act).permute(0, 2, 1).contiguous()
+def _head(sd, y, look_ahead, act, device, prefix="sb_model", head="sb", tf32=False):
+    """y: [N, Tp, H] -> act(Linear(y)), as [N, O, Tp - look_ahead] (head "sb": the first look_ahead frames dropped) or [N, O, Tp]
+    (head "fb").  tf32: both operands rounded as cvt.rna.tf32 does (the full band's conv1x1_tf32_kernel)."""
+    w, b = _sd(sd, f"{prefix}.fc_output_layer.weight", device), _sd(sd, f"{prefix}.fc_output_layer.bias", device)
+    if head == "fb":
+        look_ahead = 0
+    elif head != "sb":
+        raise ValueError(head)
+    y = y[:, look_ahead:]
+    if tf32:
+        y, w = tcn_ref.round_tf32_away(y), tcn_ref.round_tf32_away(w)
+    return _act(y @ w.T + b, act).permute(0, 2, 1).contiguous()
 
 
-def truth(sd, kind, x, look_ahead, act, device="cpu"):
-    """x: [N, I, Tp] (any float type; the values are taken as they are) -> [N, 2, Tp - look_ahead] float64."""
-    ls = layers(sd, device)
+def truth(sd, kind, x, look_ahead, act, device="cpu", prefix="sb_model", head="sb"):
+    """x: [N, I, Tp] (any float type; the values are taken as they are) -> [N, O, Tp - look_ahead] float64 (head "fb": [N, O, Tp])."""
+    ls = layers(sd, device, prefix)
     I, H = ls[0][0].shape[1], ls[0][1].shape[1]
     rnn = getattr(torch.nn, kind)(I, H, len(ls), batch_first=True).to(device=device, dtype=torch.float64)
     with torch.no_grad():
@@ -70,10 +86,11 @@ def truth(sd, kind, x, look_ahead, act, device="cpu"):
             for n, v in (("weight_ih", wi), ("weight_hh", wh), ("bias_ih", bi), ("bias_hh", bh)):
                 getattr(rnn, f"{n}_l{l}").copy_(v)
         y, _ = rnn(torch.as_tensor(x).to(device=device, dtype=torch.float64).permute(0, 2, 1).contiguous())
-    return _head(sd, y, look_ahead, act, device)
+    return _head(sd, y, look_ahead, act, device, prefix, head)
 
 
-def emulate(sd, kind, x, look_ahead, act, device="cpu", dtype=torch.float64, fault=None, fault_t=32, fault_row=0):
+def emulate(sd, kind, x, look_ahead, act, device="cpu", dtype=torch.float64, fault=None, fault_t=32, fault_row=0, prefix="sb_model",
+            head="sb"):
     """The kernels' rounding in `dtype` arithmetic (see the module docstring); x as in truth().  fault: None or one of FAULTS
       swap_units:    hidden units 3 and 5 (one 32-unit chunk) of layer 0 trade places after every step;
       c_reset:       c (GRU: the carried h) restarts from zero at step fault_t, as if a window boundary dropped it;
@@ -84,17 +101,20 @@ def emulate(sd, kind, x, look_ahead, act, device="cpu", dtype=torch.float64, fau
     f32 = lambda t: t.to(torch.float32).to(dtype)
     gru = kind == "GRU"
     inp = torch.as_tensor(x).to(device=device, dtype=dtype).permute(2, 0, 1)          # [Tp, N, I]
+    if head == "fb":
+        inp = f16(inp)                                                                 # fb_pack: the fp32 input to fp16
     Tp, N = inp.shape[0], inp.shape[1]
-    for l, (wi, wh, bi, bh) in enumerate(layers(sd, device)):
+    ls = layers(sd, device, prefix)
+    for l, (wi, wh, bi, bh) in enumerate(ls):
         H = wh.shape[1]
         wi16, wh16, bi, bh = f16(wi.to(dtype)), f16(wh.to(dtype)), bi.to(dtype), bh.to(dtype)
         gin = inp @ wi16.T                                                             # [Tp, N, G H]
-        if l > 0:
+        if l > 0 and head != "fb":                                                     # the full band's kernels keep Gin in fp32
             gin = f16(gin)
         h16 = torch.zeros(N, H, dtype=dtype, device=device)
         hold = h16                                                                     # h(t - 2) for h_lag
         c = torch.zeros(N, H, dtype=dtype, device=device)                              # LSTM: c; GRU: h in fp32
-        out = []
+        out, top = [], []
         for t in range(Tp):
             if fault == "c_reset" and t == fault_t:
                 c = torch.zeros_like(c)
@@ -120,8 +140,11 @@ def emulate(sd, kind, x, look_ahead, act, device="cpu", dtype=torch.float64, fau
             if fault == "swap_units" and l == 0:
                 h16 = h16[:, [*range(3), 5, 4, 3, *range(6, H)]]
             out.append(h16)
+            top.append(f32(h))
         inp = torch.stack(out)
-    return _head(sd, inp.permute(1, 0, 2).to(torch.float64), look_ahead, act, device)
+    if head == "fb":                                                                   # the head reads the top layer's fp32 h
+        inp = torch.stack(top)
+    return _head(sd, inp.permute(1, 0, 2).to(torch.float64), look_ahead, act, device, prefix, head, tf32=head == "fb")
 
 
 def sample_rows(nrows, seed=0, full_below=512):

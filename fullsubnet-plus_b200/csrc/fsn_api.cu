@@ -1858,14 +1858,13 @@ struct fsn_stream {
     fsn_model* m;
     int B, n = 0;                                      // n: ticks of the handle (the weight-stationary exchange-buffer parity)
     DevBuf cum_in, cum_sb, h_fb, c_fb, h_sb, c_sb, ws_h, ws_c;   // session state (the table STATE)
-    StepScratch tick;                                  // the per-frame calls' scratch (K = 1)
+    StepScratch tick;                                  // the per-frame and per-hop calls' scratch (K = 1)
     DevBuf ws_bar;
     bool use_ws = false;
     int ra_fb = 0, ra_sb = 0, rows_pad = 0, Ipad = 0;
     // slot calls (fsn_stream_step_slots, the chunk call): once used, every step runs per slot.  nb: frames each slot has consumed since
-    // its START (seeded with n at the first slot call); d_slot [5 B]: this call's per-slot values for the kernels -- the counts (-1 =
-    // held), then the audio call's three planes or the chunk call's layer-wise session lists, then the slots a START zeroes.  They reach
-    // the device through `stage`.
+    // its START (seeded with n at the first slot call); d_slot [4 B]: this call's per-slot values for the kernels -- the counts (-1 =
+    // held), then the chunk call's layer-wise session lists, then the slots a START zeroes.  They reach the device through `stage`.
     bool slots = false;
     std::vector<int32_t> nb, all_step, valid;
     DevBuf d_slot;
@@ -1873,12 +1872,12 @@ struct fsn_stream {
     // A handle serves either the mask calls (fsn_stream_step, fsn_stream_step_slots) or the audio call, whichever it meets first:
     // FSN_STATE_MODE_MASK or FSN_STATE_MODE_AUDIO, 0 before
     int mode = 0;
-    // audio call (fsn_stream_step_audio_slots), allocated at its first use.  Per slot on the host: a_tick = ticks of the session so
-    // far, HOLD excluded (-1: no session); a_hops = its hops K, known from its first FLUSH (0 before).  On the device: the history
-    // ring, the noisy-spectrum ring, the overlap tail, the model's input row, the mask rows when the caller passes none, and the tables
+    // audio calls (fsn_stream_step_audio_slots, fsn_stream_step_audio_chunk), allocated at their first use.  Per slot on the host:
+    // a_tick = ticks of the session so far, HOLD excluded (-1: no session); a_hops = its hops K, known from its first FLUSH (0 before).
+    // On the device: the history ring, the noisy-spectrum ring, the overlap tail and the tables
     std::vector<int32_t> a_tick, a_hops;
     std::vector<float> a_tables;
-    DevBuf a_hist, a_spec, a_tail, a_mag, a_mask, a_tab;
+    DevBuf a_hist, a_spec, a_tail, a_tab;
     // save / load (fsn_stream_save_slots, fsn_stream_load_slots): the slot list of the last call on the device
     DevBuf x_slot;
     // chunk call (fsn_stream_step_chunk, DESIGN.md §3.13): its scratch, allocated at its first use, grow-only, apart from the model's
@@ -1886,9 +1885,8 @@ struct fsn_stream {
     // sub-batch, and c_*: its Gin / layer output, the per-layer h / c carry and the compact masks
     StepScratch chunk;
     DevBuf c_gin, c_hsb, c_h, c_c, c_mask;
-    // audio chunk call (fsn_stream_step_audio_chunk, DESIGN.md §3.14): its scratch, allocated at its first use, grow-only: the spectra
-    // of the call's frames [B, K, F], the model's input and output planes (runs of columns, see StreamAudioChunkLaunch) and the
-    // staged per-slot plan
+    // audio calls (DESIGN.md §3.10, §3.14): their scratch, allocated at their first use, grow-only: the spectra of the call's frames
+    // [B, K, F], the model's input and output planes (runs of columns, see StreamAudioChunkLaunch) and the staged per-slot plan
     DevBuf x_spec, x_mag, x_mask, x_plan;
 };
 
@@ -2014,7 +2012,7 @@ extern "C" int fsn_stream_create(fsn_model* m, int32_t B, fsn_stream** out) {
     int e = st->tick.ensure(*st, 1, step_img_bytes(rows, 1), true, nullptr);
     e |= state_alloc(st, 0, nullptr);
     if (st->use_ws) e |= st->ws_bar.ensure(64, true);
-    e |= st->d_slot.ensure((size_t)5 * B * sizeof(int32_t), false);
+    e |= st->d_slot.ensure((size_t)4 * B * sizeof(int32_t), false);
     if (e) { fsn_stream_destroy(st); return fail(FSN_ECUDA, "stream state allocation failed"); }
     *out = st;
     return FSN_OK;
@@ -2028,8 +2026,8 @@ extern "C" void fsn_stream_destroy(fsn_stream* st) {
     }
     st->tick.release();
     st->chunk.release();
-    for (DevBuf* b : {&st->ws_bar, &st->d_slot, &st->x_slot, &st->a_mag, &st->a_mask, &st->a_tab, &st->c_gin, &st->c_hsb, &st->c_h,
-                      &st->c_c, &st->c_mask, &st->x_spec, &st->x_mag, &st->x_mask, &st->x_plan})
+    for (DevBuf* b : {&st->ws_bar, &st->d_slot, &st->x_slot, &st->a_tab, &st->c_gin, &st->c_hsb, &st->c_h, &st->c_c, &st->c_mask,
+                      &st->x_spec, &st->x_mag, &st->x_mask, &st->x_plan})
         b->release();
     delete st;
 }
@@ -2256,6 +2254,40 @@ static int chunk_lw_ensure(fsn_stream* st, const Plan& p, int K, cudaStream_t s)
     return e;
 }
 
+// The layer-wise sub band's session groups of a chunk step whose slot b runs kf[b] frames (0: not stepping), one per distinct
+// count in increasing order: each planned under the model's cap and the chunk scratch grown to fit it, before any state changes
+// (allocation failures go to *e)
+static int lw_groups(fsn_stream* st, const std::vector<int>& kf, std::vector<LwGroup>* lw, int* e, cudaStream_t s) {
+    std::vector<int> ks;
+    for (int v : kf) if (v) ks.push_back(v);
+    std::sort(ks.begin(), ks.end());
+    for (size_t i = 0, j; i < ks.size(); i = j) {
+        for (j = i; j < ks.size() && ks[j] == ks[i]; ++j) {}
+        LwGroup g{Plan{}, (int)(j - i), ks[i], nullptr, nullptr};
+        if (int rc = chunk_plan(st->m->cfg, true, g.nact, g.kf, st->m->ws_cap_bytes, &g.p)) return rc;
+        *e |= chunk_lw_ensure(st, g.p, g.kf, s);
+        lw->push_back(g);
+    }
+    return FSN_OK;
+}
+
+// The groups' slot lists, staged at h on their way to d: per group each slot's session index [B] (-1: not in it), then its slots
+// [nact].  Returns the number of values.
+static size_t lw_stage(const std::vector<int>& kf, std::vector<LwGroup>& lw, int32_t* h, const int32_t* d) {
+    const int B = (int)kf.size();
+    size_t at = 0;
+    for (LwGroup& g : lw) {
+        int32_t *idx = h + at, *sess = idx + B;
+        g.idx = d + at; g.sess = d + at + B;
+        for (int b = 0, j = 0; b < B; ++b) {
+            idx[b] = kf[b] == g.kf ? j : -1;
+            if (kf[b] == g.kf) sess[j++] = b;
+        }
+        at += B + g.nact;
+    }
+    return at;
+}
+
 // The slot calls after their argument checks: every slot advances K frames by its flag (fsn_stream_step_slots: K = 1 on the per-tick
 // scratch; the chunk call: on its own scratch, with the layer-wise sub band where the offline forward runs it).  Errors change no state.
 static int step_slots(fsn_stream* st, const float* d_mag, int K, float* d_mask, const int32_t* h_flags, int32_t* h_valid, bool chunk,
@@ -2264,51 +2296,41 @@ static int step_slots(fsn_stream* st, const float* d_mag, int K, float* d_mask, 
     const fsn_config& c = m->cfg;
     const int B = st->B, F = c.num_freqs, la = c.look_ahead;
     if (int rc = chunk_check(c, K)) return rc;
-    int nact = 0;
     bool reset = false;
     for (int b = 0; b < B; ++b) {
         const int f = h_flags[b];
         if (f != FSN_SLOT_HOLD && f != FSN_SLOT_STEP && f != FSN_SLOT_START)
             return fail(FSN_EINVAL, "slot %d: flag %d is not FSN_SLOT_HOLD (0), FSN_SLOT_STEP (1) or FSN_SLOT_START (2)", b, f);
-        nact += f != FSN_SLOT_HOLD;
         reset = reset || f == FSN_SLOT_START;
     }
     if (st->mode == FSN_STATE_MODE_AUDIO) return claim_mode(st, FSN_STATE_MODE_MASK);
+    // the scratch, before any state changes (DevBuf::ensure only grows); on the layer-wise path every stepping session runs K
+    // frames: one group
     const bool layerwise = chunk && runs_layerwise(c, m->env_impl);
-    std::vector<LwGroup> lw;                                            // every stepping session runs K frames: one group
-    if (layerwise && nact) {
-        lw.push_back(LwGroup{Plan{nact}, nact, K, nullptr, nullptr});
-        if (int rc = chunk_plan(c, true, nact, K, m->ws_cap_bytes, &lw[0].p)) return rc;
-    }
-    // the scratch, before any state changes (DevBuf::ensure only grows)
     StepScratch& x = chunk ? st->chunk : st->tick;
+    std::vector<int> kf;
+    std::vector<LwGroup> lw;
     int e = 0;
-    if (!layerwise || !nact) {
-        e = x.ensure(*st, K, layerwise ? 0 : step_img_bytes((long long)B * F, K), false, s);
-    } else {
-        e = chunk_lw_ensure(st, lw[0].p, K, s);
+    if (layerwise) {
+        for (int b = 0; b < B; ++b) kf.push_back(h_flags[b] == FSN_SLOT_HOLD ? 0 : K);
+        if (int rc = lw_groups(st, kf, &lw, &e, s)) return rc;
     }
+    if (lw.empty()) e |= x.ensure(*st, K, layerwise ? 0 : step_img_bytes((long long)B * F, K), false, s);
     if (e) return fail(FSN_ECUDA, "chunk scratch allocation failed (B = %d, K = %d)", B, K);
     if (int rc = claim_mode(st, FSN_STATE_MODE_MASK)) return rc;
     use_slot_counts(st);
-    // staged per-slot values: counts [B] (-1 = held); on the layer-wise path each slot's session index [B] (-1 = held) and the
-    // stepping slots [nact]; then the START list
+    // staged per-slot values: counts [B] (-1 = held), the layer-wise group's lists, then the START list
     int32_t* h = nullptr;
     if (int rc = st->stage.take((size_t)4 * B, &h)) return rc;
-    const int nlw = layerwise ? B + nact : 0;
-    int32_t *cnt = h, *idx = h + B, *sess = h + 2 * B, *zero = h + B + nlw;
+    const int* d = static_cast<const int*>(st->d_slot.p);
+    const size_t nlw = lw_stage(kf, lw, h + B, d + B);
+    int32_t *cnt = h, *zero = h + B + nlw;
     int nzero = 0;
-    for (int b = 0, j = 0; b < B; ++b) {
+    for (int b = 0; b < B; ++b) {
         cnt[b] = h_flags[b] == FSN_SLOT_HOLD ? -1 : h_flags[b] == FSN_SLOT_START ? 0 : st->nb[b];
-        if (layerwise) {
-            idx[b] = cnt[b] >= 0 ? j : -1;
-            if (cnt[b] >= 0) sess[j++] = b;
-        }
         if (reset && cnt[b] == 0) zero[nzero++] = b;                    // started, or never stepped
     }
-    const int* d = static_cast<const int*>(st->d_slot.p);
-    if (int rc = st->stage.send(st->d_slot.p, (size_t)B + nlw + nzero, s)) return rc;
-    if (!lw.empty()) { lw[0].idx = d + B; lw[0].sess = d + 2 * B; }
+    if (int rc = st->stage.send(st->d_slot.p, B + nlw + nzero, s)) return rc;
     if (int rc = step_frames(st, x, d_mag, K, d, nullptr, d + B + nlw, nzero, d_mask, layerwise ? &lw : nullptr, s)) return rc;
     for (int b = 0; b < B; ++b) {
         h_valid[b] = 0;
@@ -2338,12 +2360,10 @@ extern "C" int fsn_stream_step_chunk(fsn_stream* st, const float* d_mag, int32_t
     return step_slots(st, d_mag, K, d_mask, h_flags, h_valid, true, static_cast<cudaStream_t>(stream));
 }
 
-// Audio state of the handle and its scratch, zero-filled on the call's stream, and the tables of its n_fft (computed in double).
+// Audio state of the handle, zero-filled on the call's stream, and the tables of its n_fft (computed in double).
 static int audio_alloc(fsn_stream* st, cudaStream_t s) {
     const size_t B = st->B, F = st->m->cfg.num_freqs;
     int e = state_alloc(st, ST_AUDIO, s);
-    e |= st->a_mag.ensure(B * F * sizeof(float), true, s);
-    e |= st->a_mask.ensure(B * 2 * F * sizeof(float), true, s);
     audio_tables((int)(2 * (F - 1)), st->a_tables);
     e |= st->a_tab.ensure(st->a_tables.size() * sizeof(float), false, s);
     if (e) return fail(FSN_ECUDA, "audio stream state allocation failed");
@@ -2395,8 +2415,9 @@ static int audio_slot_plan(const fsn_stream* st, int b, int f, int n, int K, Aud
 }
 
 // The audio calls after their argument checks: every slot advances by its flag and hop count (fsn_stream_step_audio_slots: K = 1,
-// h_hops null, one hop per START / STEP).  The per-hop call runs the per-hop kernels around the per-frame step; the chunk call, at any
-// K, the K-hop kernels around the chunk call's K-frame step.  Errors change no state.
+// h_hops null, one hop per START / STEP) through the K-hop kernels around one K-frame model step.  The per-hop call steps the model
+// on the per-tick scratch with the generic sub band; the chunk call on its own scratch, with the layer-wise sub band where the
+// offline forward runs it.  Errors change no state.
 static int step_audio(fsn_stream* st, const float* d_samples, int K, const int32_t* h_flags, const int32_t* h_hops, float* d_out,
                       int32_t* h_nout, float* d_mask, cudaStream_t s) {
     fsn_model* m = st->m;
@@ -2410,126 +2431,64 @@ static int step_audio(fsn_stream* st, const float* d_samples, int K, const int32
         if (int rc = audio_slot_plan(st, b, h_flags[b], n, K, &plan[b])) return rc;
     }
     if (st->mode == FSN_STATE_MODE_MASK) return claim_mode(st, FSN_STATE_MODE_AUDIO);
-    int32_t* h = nullptr;
-    if (!h_hops) {
-        if (int rc = claim_mode(st, FSN_STATE_MODE_AUDIO)) return rc;
-        if (st->a_tick.empty())
-            if (int rc = audio_alloc(st, s)) return rc;
-        // One staging slot carries the tick's four per-slot planes: the model's frame counts (-1 = the model row holds), the AUDIO_*
-        // ops, the slot ticks and the hop counts; then the slots whose model row starts.  The schedule (DESIGN.md §3.10) for a session
-        // of K hops, slot tick k:
-        //   k = 0 (START): store hop 0, the model row holds;  1 <= k <= K + 1: analyse frame k - 1, the model steps frame k - 1 (count
-        //   k - 1, a START at k = 1);  k > K + 1: a zero frame;  k - 1 - la >= 0: synthesise that frame, emitting hop k - 2 - la from 1.
-        if (int rc = st->stage.take((size_t)5 * B, &h)) return rc;
-        int32_t *cnt = h, *op = h + B, *tick = h + 2 * B, *hops = h + 3 * B;
-        int nzero = 0;
-        for (int b = 0; b < B; ++b) {
-            const AudioSlotPlan& p = plan[b];
-            const int j = p.k0 - 1, mm = j - la;
-            cnt[b] = -1; op[b] = 0;
-            tick[b] = p.k0; hops[b] = p.hops;
-            if (p.na && p.start) {
-                op[b] = AUDIO_STORE;
-            } else if (p.na) {
-                cnt[b] = j;
-                op[b] = (p.nstore ? AUDIO_STORE : 0) | (!p.hops || j <= p.hops ? AUDIO_FRAME : AUDIO_ZERO) | (mm >= 0 ? AUDIO_SYNTH : 0) |
-                        (mm >= 1 ? AUDIO_EMIT : 0);
-            }
-            if (cnt[b] == 0) h[4 * B + nzero++] = b;
-        }
-        int32_t* d = static_cast<int32_t*>(st->d_slot.p);
-        if (int rc = st->stage.send(d, (size_t)4 * B + nzero, s)) return rc;
-        float* mask = d_mask ? d_mask : static_cast<float*>(st->a_mask.p);
-        StreamAudioLaunch a{};
-        a.op = d + B; a.tick = d + 2 * B; a.hops = d + 3 * B;
-        a.samples = d_samples; a.out = d_out;
-        a.hist = static_cast<float*>(st->a_hist.p); a.spec = static_cast<float2*>(st->a_spec.p); a.tail = static_cast<float*>(st->a_tail.p);
-        a.mag = static_cast<float*>(st->a_mag.p); a.mask = mask;
-        const AudioTables tab = audio_table_ptrs(static_cast<const float*>(st->a_tab.p), N);
-        a.window = tab.window; a.twiddle = tab.twiddle; a.inv_env = tab.inv_env;
-        a.B = B; a.n_fft = N; a.la = la;
-        launch_stream_stft(a, s);
-        if (int rc = step_frames(st, st->tick, a.mag, 1, d, nullptr, d + 4 * B, nzero, mask, nullptr, s)) return rc;
-        launch_stream_istft(a, s);
-    } else {
-        // The model's frames: slot b's kf of them, left-aligned in columns 0 .. kf - 1 of [B, F, Km], Km the largest kf.  One K-frame
-        // step runs them all, each slot holding after its kf frames; on the layer-wise path its sub band runs one pass per group of
-        // sessions with one kf (in steady state a single group).
-        std::vector<int> kf(B);
-        int Km = 0, nzero = 0;
-        for (int b = 0; b < B; ++b) {
-            kf[b] = plan[b].na > plan[b].start ? plan[b].na - plan[b].start : 0;
-            Km = kf[b] > Km ? kf[b] : Km;
-            nzero += kf[b] && plan[b].k0 + plan[b].start == 1;          // model frame 0 in column 0: a START's reset
-        }
-        const bool layerwise = runs_layerwise(c, m->env_impl);
-        std::vector<LwGroup> lw;
-        if (layerwise) {
-            std::vector<int> ks;
-            for (int v : kf) if (v) ks.push_back(v);
-            std::sort(ks.begin(), ks.end());
-            for (size_t i = 0; i < ks.size();) {
-                size_t e = i;
-                while (e < ks.size() && ks[e] == ks[i]) ++e;
-                lw.push_back(LwGroup{Plan{(int)(e - i)}, (int)(e - i), ks[i], nullptr, nullptr});
-                i = e;
-            }
-        }
-        size_t nstage = (size_t)7 * B + nzero;
-        int e = 0;
-        for (LwGroup& g : lw) {
-            nstage += B + g.nact;
-            if (int rc = chunk_plan(c, true, g.nact, g.kf, m->ws_cap_bytes, &g.p)) return rc;
-            e |= chunk_lw_ensure(st, g.p, g.kf, s);
-        }
-        if (Km) e |= st->chunk.ensure(*st, Km, layerwise ? 0 : step_img_bytes((long long)B * F, Km), false, s);
-        e |= st->x_spec.ensure((size_t)B * K * F * sizeof(float2), false, s);
-        e |= st->x_mag.ensure((size_t)B * F * Km * sizeof(float), false, s);
-        e |= st->x_mask.ensure((size_t)B * 2 * F * Km * sizeof(float), false, s);
-        e |= st->x_plan.ensure(nstage * sizeof(int32_t), false, s);
-        if (e) return fail(FSN_ECUDA, "audio chunk scratch allocation failed (B = %d, K = %d)", B, K);
-        if (int rc = claim_mode(st, FSN_STATE_MODE_AUDIO)) return rc;
-        if (st->a_tick.empty())
-            if (int rc = audio_alloc(st, s)) return rc;
-        // staged: the five per-slot planes of the kernels, the model's frame counts at column 0 (-1 = held) and frame counts, the
-        // slots whose model frame 0 is in this call, then per layer-wise group each slot's session index and the group's slots
-        if (int rc = st->stage.take(nstage, &h)) return rc;
-        const int32_t* d = static_cast<const int32_t*>(st->x_plan.p);
-        int32_t *cnt = h + 5 * B, *kfp = h + 6 * B, *zero = h + 7 * B;
-        for (int b = 0, z = 0; b < B; ++b) {
-            const AudioSlotPlan& p = plan[b];
-            h[b] = p.k0; h[B + b] = p.na; h[2 * B + b] = p.start; h[3 * B + b] = p.nstore; h[4 * B + b] = p.hops;
-            cnt[b] = kf[b] ? p.k0 + p.start - 1 : -1;
-            kfp[b] = kf[b];
-            if (kf[b] && cnt[b] == 0) zero[z++] = b;
-        }
-        size_t at = (size_t)7 * B + nzero;
-        for (LwGroup& g : lw) {
-            int32_t *idx = h + at, *sess = idx + B;
-            g.idx = d + at; g.sess = d + at + B;
-            for (int b = 0, j = 0; b < B; ++b) {
-                idx[b] = kf[b] == g.kf ? j : -1;
-                if (kf[b] == g.kf) sess[j++] = b;
-            }
-            at += B + g.nact;
-        }
-        if (int rc = st->stage.send(st->x_plan.p, nstage, s)) return rc;
-        StreamAudioChunkLaunch a{};
-        a.k0 = d; a.na = d + B; a.start = d + 2 * B; a.nstore = d + 3 * B; a.hops = d + 4 * B;
-        a.samples = d_samples; a.out = d_out;
-        a.hist = static_cast<float*>(st->a_hist.p); a.spec = static_cast<float2*>(st->a_spec.p); a.tail = static_cast<float*>(st->a_tail.p);
-        a.sspec = static_cast<float2*>(st->x_spec.p); a.mag = static_cast<float*>(st->x_mag.p); a.mask = static_cast<float*>(st->x_mask.p);
-        a.umask = d_mask;
-        const AudioTables tab = audio_table_ptrs(static_cast<const float*>(st->a_tab.p), N);
-        a.window = tab.window; a.twiddle = tab.twiddle; a.inv_env = tab.inv_env;
-        a.B = B; a.K = K; a.Km = Km; a.n_fft = N; a.la = la;
-        launch_stream_stft_chunk(a, s);
-        if (Km)
-            if (int rc = step_frames(st, st->chunk, a.mag, Km, d + 5 * B, d + 6 * B, d + 7 * B, nzero, static_cast<float*>(st->x_mask.p),
-                                     layerwise ? &lw : nullptr, s))
-                return rc;
-        launch_stream_istft_chunk(a, s);
+    // The model's frames: slot b's kf of them, left-aligned in columns 0 .. kf - 1 of [B, F, Km], Km the largest kf.  One K-frame
+    // step runs them all, each slot holding after its kf frames; on the layer-wise path its sub band runs one pass per group of
+    // sessions with one kf (in steady state a single group).  Km = 0 (every slot holds): no model step.
+    std::vector<int> kf(B);
+    int Km = 0, nzero = 0;
+    for (int b = 0; b < B; ++b) {
+        kf[b] = plan[b].na > plan[b].start ? plan[b].na - plan[b].start : 0;
+        Km = kf[b] > Km ? kf[b] : Km;
+        nzero += kf[b] && plan[b].k0 + plan[b].start == 1;          // model frame 0 in column 0: a START's reset
     }
+    const bool chunk = h_hops != nullptr, layerwise = chunk && runs_layerwise(c, m->env_impl);
+    StepScratch& x = chunk ? st->chunk : st->tick;
+    std::vector<LwGroup> lw;
+    int e = 0;
+    if (layerwise)
+        if (int rc = lw_groups(st, kf, &lw, &e, s)) return rc;
+    size_t nstage = (size_t)7 * B + nzero;
+    for (const LwGroup& g : lw) nstage += B + g.nact;
+    if (Km) e |= x.ensure(*st, Km, layerwise ? 0 : step_img_bytes((long long)B * F, Km), false, s);
+    e |= st->x_spec.ensure((size_t)B * K * F * sizeof(float2), false, s);
+    e |= st->x_mag.ensure((size_t)B * F * Km * sizeof(float), false, s);
+    e |= st->x_mask.ensure((size_t)B * 2 * F * Km * sizeof(float), false, s);
+    e |= st->x_plan.ensure(nstage * sizeof(int32_t), false, s);
+    if (e) return fail(FSN_ECUDA, "audio chunk scratch allocation failed (B = %d, K = %d)", B, K);
+    if (int rc = claim_mode(st, FSN_STATE_MODE_AUDIO)) return rc;
+    if (st->a_tick.empty())
+        if (int rc = audio_alloc(st, s)) return rc;
+    // staged: the five per-slot planes of the kernels, the model's frame counts at column 0 (-1 = held) and frame counts, the
+    // slots whose model frame 0 is in this call, then the layer-wise groups' lists
+    int32_t* h = nullptr;
+    if (int rc = st->stage.take(nstage, &h)) return rc;
+    const int32_t* d = static_cast<const int32_t*>(st->x_plan.p);
+    int32_t *cnt = h + 5 * B, *kfp = h + 6 * B, *zero = h + 7 * B;
+    for (int b = 0, z = 0; b < B; ++b) {
+        const AudioSlotPlan& p = plan[b];
+        h[b] = p.k0; h[B + b] = p.na; h[2 * B + b] = p.start; h[3 * B + b] = p.nstore; h[4 * B + b] = p.hops;
+        cnt[b] = kf[b] ? p.k0 + p.start - 1 : -1;
+        kfp[b] = kf[b];
+        if (kf[b] && cnt[b] == 0) zero[z++] = b;
+    }
+    lw_stage(kf, lw, zero + nzero, d + 7 * B + nzero);
+    if (int rc = st->stage.send(st->x_plan.p, nstage, s)) return rc;
+    StreamAudioChunkLaunch a{};
+    a.k0 = d; a.na = d + B; a.start = d + 2 * B; a.nstore = d + 3 * B; a.hops = d + 4 * B;
+    a.samples = d_samples; a.out = d_out;
+    a.hist = static_cast<float*>(st->a_hist.p); a.spec = static_cast<float2*>(st->a_spec.p); a.tail = static_cast<float*>(st->a_tail.p);
+    a.sspec = static_cast<float2*>(st->x_spec.p); a.mag = static_cast<float*>(st->x_mag.p); a.mask = static_cast<float*>(st->x_mask.p);
+    a.umask = d_mask;
+    const AudioTables tab = audio_table_ptrs(static_cast<const float*>(st->a_tab.p), N);
+    a.window = tab.window; a.twiddle = tab.twiddle; a.inv_env = tab.inv_env;
+    a.B = B; a.K = K; a.Km = Km; a.n_fft = N; a.la = la;
+    launch_stream_stft_chunk(a, s);
+    // at Km = 1 the counts alone say which slots step a frame: no frame counts, so the per-frame step's kernels and arguments
+    if (Km)
+        if (int rc = step_frames(st, x, a.mag, Km, d + 5 * B, Km > 1 ? d + 6 * B : nullptr, d + 7 * B, nzero,
+                                 static_cast<float*>(st->x_mask.p), layerwise ? &lw : nullptr, s))
+            return rc;
+    launch_stream_istft_chunk(a, s);
     CK(cudaGetLastError());
     for (int b = 0; b < B; ++b) {
         const AudioSlotPlan& p = plan[b];

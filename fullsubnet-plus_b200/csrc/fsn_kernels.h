@@ -154,44 +154,26 @@ struct StreamSbCarryLaunch {
 };
 void launch_stream_sb_carry(const StreamSbCarryLaunch& a, cudaStream_t s);
 
-// ---- k_stream_audio.cu: audio in and out of the streaming slot call (fsn_stream_step_audio_slots) ---------------------------
-// Per-slot ops of one tick, derived on the host from the slot's flag, tick count and hop count (fsn_api.cu, audio_plan)
-enum { AUDIO_STORE = 1,       // the slot's hop of samples goes to its history ring
-       AUDIO_FRAME = 2,       // analyse frame tick - 1: spectrum to the ring, magnitude to the model's input row
-       AUDIO_ZERO = 4,        // frame tick - 1 is a look-ahead zero frame: zero spectrum and magnitude rows
-       AUDIO_SYNTH = 8,       // synthesise frame tick - 1 - la from this tick's mask row
-       AUDIO_EMIT = 16 };     // ... and write hop tick - 2 - la of the session to the output row (else the row is zero)
-struct StreamAudioLaunch {
-    const int* op; const int* tick; const int* hops;   // [B] each: AUDIO_* bits, slot tick (HOLD excluded), hops K (0 = not flushed)
-    const float* samples;     // [B, hop] this tick's hops (read for AUDIO_STORE only)
-    float* out;               // [B, hop] output hops
-    float* hist;              // [B, 3, hop] history ring: hop q at q % 3
-    float2* spec;             // [B, la + 1, F] noisy spectrum ring: frame j at j % (la + 1)
-    float* tail;              // [B, hop] second half of the last synthesised windowed frame
-    float* mag;               // [B, F] the model step's input row
-    const float* mask;        // [B, 2, F] the model step's output
-    const float* window;      // [n_fft] periodic Hann
-    const float2* twiddle;    // [n_fft / 2 + 1] exp(-2 pi i k / n_fft)
-    const float* inv_env;     // [hop] 1 / (w^2(i) + w^2(i + hop))
-    int B, n_fft, la;         // n_fft: power of two, 64 .. 1024
-};
-void launch_stream_stft(const StreamAudioLaunch& a, cudaStream_t s);
-void launch_stream_istft(const StreamAudioLaunch& a, cudaStream_t s);
-// K hops per slot (fsn_stream_step_audio_chunk, DESIGN.md §3.14): slot b's active ticks are the first na[b] of the call, at slot ticks
-// k0[b] + i; with start[b] its tick 0 is a START (store hop 0, no model frame).  Its first nstore[b] active ticks store the row's hops
-// 0 .. nstore - 1.  Every other active tick is a model frame: model column c = i - start, frame j = k0 + start - 1 + c, its
-// magnitude and mask at column c of the model's planes [B, F, Km] and [B, 2, F, Km].
+// ---- k_stream_audio.cu: audio in and out of the streaming audio calls (fsn_stream_step_audio_slots, _chunk) ------------------
+// K hops per slot (DESIGN.md §3.10, §3.14; the per-hop call is K = 1): slot b's active ticks are the first na[b] of the call, at
+// slot ticks k0[b] + i; with start[b] its tick 0 is a START (store hop 0, no model frame).  Its first nstore[b] active ticks store
+// the row's hops 0 .. nstore - 1.  Every other active tick is a model frame: model column c = i - start, frame j = k0 + start - 1 + c,
+// its magnitude and mask at column c of the model's planes [B, F, Km] and [B, 2, F, Km].
 struct StreamAudioChunkLaunch {
     const int *k0, *na, *start, *nstore, *hops;   // [B] each; hops: the session's K after this call (0 = not flushed)
     const float* samples;     // [B, K hop] this call's hops at the front of each row
     float* out;               // [B, K hop] output hops at the front of each row, zero after them
-    float* hist; float2* spec; float* tail;       // the slot state of StreamAudioLaunch
+    float* hist;              // [B, 3, hop] history ring: hop q at q % 3
+    float2* spec;             // [B, la + 1, F] noisy spectrum ring: frame j at j % (la + 1)
+    float* tail;              // [B, hop] second half of the last synthesised windowed frame
     float2* sspec;            // [B, K, F] scratch: the spectrum of each model column's frame
     float* mag;               // model input [B, F, Km]
     const float* mask;        // model output [B, 2, F, Km]
     float* umask;             // [B, 2, F, K] the caller's masks by tick, or null
-    const float* window; const float2* twiddle; const float* inv_env;
-    int B, K, Km, n_fft, la;  // Km: model columns, the largest frame count of the call
+    const float* window;      // [n_fft] periodic Hann
+    const float2* twiddle;    // [n_fft / 2 + 1] exp(-2 pi i k / n_fft)
+    const float* inv_env;     // [hop] 1 / (w^2(i) + w^2(i + hop))
+    int B, K, Km, n_fft, la;  // Km: model columns, the largest frame count of the call; n_fft: power of two, 64 .. 1024
 };
 void launch_stream_stft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s);
 void launch_stream_istft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s);

@@ -3,9 +3,8 @@
 // of torch.istft output (decompress_cIRM x noisy spectrum, inverse real FFT, window, overlap-add, division by the window envelope).
 // One CTA per slot; the real FFTs of n_fft points run as complex FFTs of n_fft / 2 points (radix 2, fp32, in shared memory,
 // fsn_fft.cuh) with the even / odd split folded in.  The tables (window, twiddles, 1 / envelope) are computed in double on the host
-// once per handle (audio_tables).  The per-hop call (fsn_stream_step_audio_slots) runs one tick per launch; the chunk call
-// (fsn_stream_step_audio_chunk) runs each slot's ticks of the call in order inside its CTA, through the same frame helpers, so both
-// give the same bits.
+// once per handle (audio_tables).  Both audio calls run these kernels: each slot's ticks of the call run in order inside its CTA, K
+// of them for the chunk call (fsn_stream_step_audio_chunk), one for the per-hop call (fsn_stream_step_audio_slots).
 #include "fsn_common.cuh"
 #include "fsn_fft.cuh"
 #include "fsn_kernels.h"
@@ -67,58 +66,14 @@ __device__ __forceinline__ void synth_frame(const float* mask, int ms, const flo
     }
 }
 
-// grid B: analysis of one tick.  STORE: the slot's hop goes to its history ring (hop q at q % 3).  FRAME: frame j = tick - 1 of the
-// session; its spectrum goes to the ring (frame j at j % (la + 1)) and its magnitude to the model's input row.  ZERO: the same two
-// rows are zero (the right padding of the look-ahead).  A slot without an op touches nothing.
-__global__ void __launch_bounds__(AUDIO_THREADS) stream_stft_kernel(StreamAudioLaunch a) {
-    __shared__ float2 z[AUDIO_MAX_HOP];
-    const int b = blockIdx.x, op = a.op[b];
-    if (!(op & (AUDIO_STORE | AUDIO_FRAME | AUDIO_ZERO))) return;
-    const int H = a.n_fft >> 1, F = H + 1, k = a.tick[b], lg = 31 - __clz(H);
-    float* hist = a.hist + (size_t)b * 3 * H;
-    if (op & AUDIO_STORE) {
-        const float* x = a.samples + (size_t)b * H;
-        for (int i = threadIdx.x; i < H; i += blockDim.x) hist[(k % 3) * H + i] = x[i];
-        __syncthreads();                                         // frame 0 reads the first sample of the hop stored now
-    }
-    if (!(op & (AUDIO_FRAME | AUDIO_ZERO))) return;
-    const int j = k - 1;
-    float2* spec = a.spec + ((size_t)b * (a.la + 1) + j % (a.la + 1)) * F;
-    float* mag = a.mag + (size_t)b * F;
-    if (op & AUDIO_ZERO) {
-        for (int f = threadIdx.x; f < F; f += blockDim.x) { spec[f] = make_float2(0.f, 0.f); mag[f] = 0.f; }
-        return;
-    }
-    analyse_frame(hist, j, a.hops[b] * H, H, lg, a.window, a.twiddle, z, spec, mag, 1);
-}
-
-// grid B: synthesis of one tick.  SYNTH: frame m = tick - 1 - la from the mask row the model step wrote this tick and the spectrum
-// ring; the second half of the windowed frame becomes the slot's tail.  EMIT (m >= 1): out = (tail of frame m - 1 + first half) / env,
-// which is hop m - 1 of the session.  Every row without EMIT is written as zero.
-__global__ void __launch_bounds__(AUDIO_THREADS) stream_istft_kernel(StreamAudioLaunch a) {
-    __shared__ float2 z[AUDIO_MAX_HOP];
-    __shared__ float2 e[AUDIO_MAX_HOP + 1];
-    const int b = blockIdx.x, op = a.op[b];
-    const int H = a.n_fft >> 1, F = H + 1, lg = 31 - __clz(H);
-    float* out = a.out + (size_t)b * H;
-    if (!(op & AUDIO_SYNTH)) {
-        for (int i = threadIdx.x; i < H; i += blockDim.x) out[i] = 0.f;
-        return;
-    }
-    const int m = a.tick[b] - 1 - a.la;
-    const float2* spec = a.spec + ((size_t)b * (a.la + 1) + m % (a.la + 1)) * F;
-    synth_frame(a.mask + (size_t)b * 2 * F, 1, spec, a.tail + (size_t)b * H, out, op & AUDIO_EMIT, H, lg, a.window, a.twiddle, a.inv_env,
-                z, e);
-}
-
 // The model planes' address of slot b's column c (row 0 of its rows rows): [B, rows, Km]
 __device__ __forceinline__ size_t chunk_col(const StreamAudioChunkLaunch& a, int b, int c, int rows) {
     return ((size_t)b * rows) * a.Km + c;
 }
 
-// grid B: the analysis of a slot's active ticks, in order.  Stored hops go to the history ring as the per-hop kernel stores them; the
-// spectrum of model column c goes to the scratch sspec (the ring still holds the frames the synthesis of this call reads), its
-// magnitude to the model's input.  Frames past the session's end (j > K) are zero.
+// grid B: the analysis of a slot's active ticks, in order.  Stored hops go to the history ring (hop q at q % 3); the spectrum of model
+// column c goes to the scratch sspec (the ring still holds the frames the synthesis of this call reads), its magnitude to the model's
+// input.  Frames past the session's end (j > K) are zero.
 __global__ void __launch_bounds__(AUDIO_THREADS) stream_stft_chunk_kernel(StreamAudioChunkLaunch a) {
     __shared__ float2 z[AUDIO_MAX_HOP];
     const int b = blockIdx.x, na = a.na[b];
@@ -184,8 +139,6 @@ __global__ void __launch_bounds__(AUDIO_THREADS) stream_istft_chunk_kernel(Strea
     }
 }
 
-void launch_stream_stft(const StreamAudioLaunch& a, cudaStream_t s) { stream_stft_kernel<<<a.B, AUDIO_THREADS, 0, s>>>(a); }
-void launch_stream_istft(const StreamAudioLaunch& a, cudaStream_t s) { stream_istft_kernel<<<a.B, AUDIO_THREADS, 0, s>>>(a); }
 void launch_stream_stft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s) { stream_stft_chunk_kernel<<<a.B, AUDIO_THREADS, 0, s>>>(a); }
 void launch_stream_istft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s) { stream_istft_chunk_kernel<<<a.B, AUDIO_THREADS, 0, s>>>(a); }
 

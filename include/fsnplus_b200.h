@@ -258,9 +258,9 @@ int fsn_stream_chunk_plan(const fsn_config* cfg, int32_t n_active, int32_t K, do
  * FSN_EINVAL, naming the slot, for a flag outside {0, 1, 2, 3}, a STEP after the session's first FLUSH, a STEP or FLUSH on a slot
  * that has no session, and a FLUSH after fewer than 2 hops; FSN_EINVAL, naming the argument, for a null array.  A handle serves
  * either the mask calls (fsn_stream_step, fsn_stream_step_slots) or this call: mixing them is FSN_ESTATE.  The audio state
- * (history, spectrum ring, overlap tail) is allocated at the first call.  Per tick: one H2D copy and 8 kernels (+ the reset kernel on
- * ticks where a session's model row starts, + the grid-barrier memset of the full-band step at B <= 64).  The call does not
- * synchronise the stream. */
+ * (history, spectrum ring, overlap tail) and the scratch shared with fsn_stream_step_audio_chunk are allocated at the first call.
+ * Per tick: one H2D copy and 8 kernels (+ the reset kernel on ticks where a session's model row starts, + the grid-barrier memset of
+ * the full-band step at B <= 64; 2 kernels when no slot has a model frame).  The call does not synchronise the stream. */
 int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_samples, float* d_out, const int32_t* h_flags, int32_t* h_valid,
                                 float* d_mask, void* stream);
 

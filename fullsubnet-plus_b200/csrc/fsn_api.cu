@@ -99,13 +99,13 @@ static uint64_t hash_words(uint64_t h, const void* p, size_t n) {
 
 struct ParamSpec { std::string key; int64_t numel; };
 
-// The packed block weights of one TCN (pack_tcn_blocks): nbr branches (key prefixes pre[b] = "<module>.sequence_model.") of C channels
-// padded to Cp, gLN2 folded into the second 1x1 convolution; NT / ntiles = N tile and N tiles of its Cp-wide GEMMs.
+// The packed block weights of one TCN (pack_tcn_blocks): nbr branches of C channels padded to Cp, gLN2 folded into the second 1x1
+// convolution; NT / ntiles = N tile and N tiles of its Cp-wide GEMMs.
 struct TcnWeights {
     const char* name = "";                             // in error messages
-    std::vector<std::string> pre;
     int nbr = 0, C = 0, Cp = 0, NT = 0, ntiles = 0;
     DevBuf W1, W2, S1, S2b;                            // [8][nbr][512][Cp] tf32, [8][nbr][Cp][512] fp16, [8][nbr][Cp] x2
+    struct Block { const float *conv1x1_b, *prelu1, *norm1_w, *norm1_b, *dw_w, *dw_b, *prelu2; } p[8][3];   // [block][branch], unpacked
     alignas(64) unsigned char mapW1[8][128], mapW2[8][128];
     void release() { W1.release(); W2.release(); S1.release(); S2b.release(); }
 };
@@ -135,8 +135,7 @@ static float* tcn_amax(void* stats, size_t Z, int blk) { return reinterpret_cast
 struct fsn_model {
     fsn_config cfg;
     std::vector<ParamSpec> specs;
-    std::map<std::string, std::vector<float>> host;   // raw fp32 parameters (reference layout)
-    std::map<std::string, float*> dev;                // same, on device
+    std::map<std::string, std::vector<float>> host;   // raw fp32 parameters (reference layout), copied to `arena` at finalize
     std::map<std::string, uint64_t> param_hash;       // per key: hash of the key and its fp32 bytes as set (fsn_model_set_param)
     uint64_t weights_id = 0;                          // the per-key hashes combined in key order at fsn_model_finalize; 0 before
     DevBuf arena;
@@ -145,6 +144,14 @@ struct fsn_model {
     // packed LSTM weights
     DevBuf sb_frag[4], sb_bias[4];
     DevBuf fb_frag[4], fb_bias[4];
+    // launch templates, bound at every fsn_model_finalize (bind_weights): weights and model constants only; each launch adds its geometry,
+    // buffers and state, so none names a state_dict key.  The offline forward and the streaming step share them.
+    TsseParams tsse[3] = {};                          // FullSubNet+: the channel attention of each branch
+    LstmWsLaunch fb_ws{};                             // fullsubnet.Model: the full-band LSTM, weight-stationary kernel
+    LstmMmaLaunch fb_mma{};                           // fullsubnet.Model: the full-band LSTM, generic kernel
+    ConvLaunch fb_out{};                              // fullsubnet.Model: the full band's output Linear
+    LstmMmaLaunch sb_mma{};                           // the sub-band LSTM, generic kernel
+    const float *sb_fc_w = nullptr, *sb_fc_b = nullptr;   // the sub band's output Linear: layer-wise kernels, TCN head (bias only)
     // layer-wise wgmma path (k_lstm_tc5r.cu): per-layer recurrent streams, permuted input-projection matrices, biases
     DevBuf r_stream[4], r_wih[4], r_bias[4], r_gin, r_hseq;    // r_wih: input-projection matrices of the layers > 0
     DevBuf r_hstate, sb_cum;                           // windowed forwards: per-layer h at the window's end, the packer's cumulative sums
@@ -303,6 +310,7 @@ static void build_specs(fsn_model* m) {
 // ---------------------------------------------------------------------------------------------
 // packing
 // ---------------------------------------------------------------------------------------------
+using DevPtrs = std::map<std::string, const float*>;   // every parameter's copy in the arena, by key (fsn_model_finalize)
 static uint16_t h_bits(float f) { __half h = __float2half_rn(f); uint16_t b; std::memcpy(&b, &h, 2); return b; }
 
 // mma.sync fragment order (k_lstm_mma.cu): [group of 8 units][k16 step][lane][i.b0 i.b1 f.b0 f.b1 | g.b0 g.b1 o.b0 o.b1]
@@ -399,10 +407,11 @@ static float to_tf32(float x) {
 // pre[b] = "<module>.sequence_model.") stacked, gLN2 folded into the second 1x1 convolution:
 //   conv(W2, gLN(y)) = rstd * (W2 diag(gamma2)) y - mean * rstd * s1 + s2,  s1[n] = sum_c W2'[n,c],  s2[n] = sum_c W2[n,c] beta2[c]
 // W1 [8][nbr][512][Cp] tf32, W2' [8][nbr][Cp][512] fp16, s1 / s2 + conv bias [8][nbr][Cp]; tensor maps per block: W1 in 128-row
-// boxes, W2' in NT-row boxes.
-static int pack_tcn_blocks(fsn_model* m, TcnWeights& w, const char* name, const std::vector<std::string>& pre, int C, int Cp) {
+// boxes, W2' in NT-row boxes.  The parameters the kernels read unpacked are bound from dev into w.p.
+static int pack_tcn_blocks(fsn_model* m, const DevPtrs& dev, TcnWeights& w, const char* name, const std::vector<std::string>& pre, int C,
+                           int Cp) {
     const int nbr = (int)pre.size(), Hd = 512;
-    w.name = name; w.pre = pre; w.nbr = nbr; w.C = C; w.Cp = Cp;
+    w.name = name; w.nbr = nbr; w.C = C; w.Cp = Cp;
     // N tile of the Cp-wide GEMMs: 64 or 128 columns (the last tile of a branch may overhang; those columns are not stored)
     w.NT = Cp <= 64 ? 64 : 128;
     w.ntiles = (Cp + w.NT - 1) / w.NT;
@@ -417,6 +426,8 @@ static int pack_tcn_blocks(fsn_model* m, TcnWeights& w, const char* name, const 
             const auto& b2 = m->host[q + "sconv.bias"];
             const auto& g2 = m->host[q + "norm2.weight"];
             const auto& be2 = m->host[q + "norm2.bias"];
+            w.p[blk][b] = {dev.at(q + "conv1x1.bias"), dev.at(q + "prelu1.weight"), dev.at(q + "norm1.weight"), dev.at(q + "norm1.bias"),
+                           dev.at(q + "depthwise_conv.weight"), dev.at(q + "depthwise_conv.bias"), dev.at(q + "prelu2.weight")};
             float* d1 = &W1[((size_t)blk * nbr + b) * Hd * Cp];
             for (int o = 0; o < Hd; ++o)
                 for (int k = 0; k < C; ++k) d1[(size_t)o * Cp + k] = to_tf32(w1[(size_t)o * C + k]);
@@ -446,13 +457,13 @@ static int pack_tcn_blocks(fsn_model* m, TcnWeights& w, const char* name, const 
 }
 
 // the three full-band TCNs of FullSubNet+ (F channels each) and their output Linear
-static int pack_tcn5(fsn_model* m) {
+static int pack_tcn5(fsn_model* m, const DevPtrs& dev) {
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs, Cp = (F + 31) / 32 * 32;
     const char* sfx[3] = {"", "_real", "_imag"};
     std::vector<std::string> pre;
     for (int b = 0; b < 3; ++b) pre.push_back(std::string("fb_model") + sfx[b] + ".sequence_model.");
-    int rc = pack_tcn_blocks(m, m->tcn_fb, "full-band TCN", pre, F, Cp);
+    int rc = pack_tcn_blocks(m, dev, m->tcn_fb, "full-band TCN", pre, F, Cp);
     if (rc) return rc;
     std::vector<float> Wfc((size_t)3 * Cp * Cp, 0.f), Bfc((size_t)3 * Cp, 0.f);
     for (int b = 0; b < 3; ++b) {
@@ -472,9 +483,9 @@ static int pack_tcn5(fsn_model* m) {
 
 // the sub-band TCN (sequence_model = "TCN"): one branch of Isb <= 64 channels padded to 64 -- the GLN_HEAD epilogue needs a row's
 // channels in one 64-column N tile -- and its Linear(Isb -> O) as [O][64] fp32 (read by that epilogue)
-static int pack_sb_tcn(fsn_model* m) {
+static int pack_sb_tcn(fsn_model* m, const DevPtrs& dev) {
     const int I = m->Isb, O = m->cfg.output_size;
-    int rc = pack_tcn_blocks(m, m->tcn_sb, "sub-band TCN", {"sb_model.sequence_model."}, I, 64);
+    int rc = pack_tcn_blocks(m, dev, m->tcn_sb, "sub-band TCN", {"sb_model.sequence_model."}, I, 64);
     if (rc) return rc;
     std::vector<float> fc((size_t)O * 64, 0.f);
     const auto& w = m->host["sb_model.fc_output_layer.weight"];
@@ -482,6 +493,59 @@ static int pack_sb_tcn(fsn_model* m) {
         for (int k = 0; k < I; ++k) fc[(size_t)o * 64 + k] = w[(size_t)o * I + k];
     if (upload(m->sb_fc, fc.data(), fc.size() * 4)) return fail(FSN_ECUDA, "upload of the sub-band TCN head failed");
     return FSN_OK;
+}
+
+// The launch templates of fsn_model (after the packers), each where its model part exists: the attention for FullSubNet+, the full band
+// for fullsubnet.Model, the generic sub-band LSTM unless the sub band is a TCN
+static void bind_weights(fsn_model* m, const DevPtrs& dev) {
+    const fsn_config& c = m->cfg;
+    const int L = c.num_layers, gru = c.rnn_type == FSN_RNN_GRU;
+    if (c.model_kind == FSN_KIND_PLUS) {
+        const char* sfx[3] = {"", "_real", "_imag"};
+        const char* cn[3] = {"smallConv1d", "middleConv1d", "largeConv1d"};
+        for (int b = 0; b < 3; ++b) {
+            TsseParams& t = m->tsse[b];
+            const std::string p = std::string("channel_attention") + sfx[b];
+            if (c.channel_attention == FSN_ATTN_ECA) { t.eca_w = dev.at(p + ".conv.weight"); continue; }
+            if (c.channel_attention == FSN_ATTN_TSSE) {
+                for (int i = 0; i < 3; ++i) {
+                    t.conv_w[i] = dev.at(p + "." + cn[i] + ".0.weight");
+                    t.conv_b[i] = dev.at(p + "." + cn[i] + ".0.bias");
+                }
+                t.cat_w = dev.at(p + ".feature_concate_fc.weight"); t.cat_b = dev.at(p + ".feature_concate_fc.bias");
+            }
+            t.fc1_w = dev.at(p + ".fc1.weight"); t.fc1_b = dev.at(p + ".fc1.bias");
+            t.fc2_w = dev.at(p + ".fc2.weight"); t.fc2_b = dev.at(p + ".fc2.bias");
+        }
+    } else {
+        const int F = c.num_freqs, Ipad = (F + 15) / 16 * 16;
+        LstmWsLaunch& w = m->fb_ws;
+        LstmMmaLaunch& a = m->fb_mma;
+        for (int l = 0; l < L; ++l) {
+            const std::string q = "fb_model.sequence_model.", s = std::to_string(l);
+            w.w_ih[l] = dev.at(q + "weight_ih_l" + s); w.w_hh[l] = dev.at(q + "weight_hh_l" + s);
+            w.b_ih[l] = dev.at(q + "bias_ih_l" + s); w.b_hh[l] = dev.at(q + "bias_hh_l" + s);
+            a.w.wfrag[l] = static_cast<const uint4*>(m->fb_frag[l].p);
+            a.w.bias[l] = static_cast<const float*>(m->fb_bias[l].p);
+        }
+        w.L = L; w.H = c.fb_hidden; w.I = F; w.Ipad = Ipad; w.fast = c.fast_math; w.gru = gru;
+        a.L = L; a.H = c.fb_hidden; a.I = F; a.Ipad = Ipad; a.fast = c.fast_math; a.gru = gru;
+        ConvLaunch& cf = m->fb_out;
+        cf.W = dev.at("fb_model.fc_output_layer.weight"); cf.bias = dev.at("fb_model.fc_output_layer.bias");
+        cf.M = F; cf.K = c.fb_hidden; cf.act = c.fb_act;
+    }
+    m->sb_fc_b = dev.at("sb_model.fc_output_layer.bias");
+    if (!c.sb_tcn) {
+        m->sb_fc_w = dev.at("sb_model.fc_output_layer.weight");
+        LstmMmaLaunch& a = m->sb_mma;
+        for (int l = 0; l < L; ++l) {
+            a.w.wfrag[l] = static_cast<const uint4*>(m->sb_frag[l].p);
+            a.w.bias[l] = static_cast<const float*>(m->sb_bias[l].p);
+        }
+        a.w.fc_w = m->sb_fc_w; a.w.fc_b = m->sb_fc_b;
+        a.L = L; a.H = c.sb_hidden; a.I = m->Isb; a.Ipad = 64;
+        a.O = c.output_size; a.F = c.num_freqs; a.act = c.sb_act; a.fast = c.fast_math; a.gru = gru;
+    }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -623,11 +687,12 @@ extern "C" int fsn_model_finalize(fsn_model* m) {
     for (const auto& s : m->specs) total += (m->host[s.key].size() * 4 + 255) & ~(size_t)255;
     if (m->arena.ensure(total, false)) return fail(FSN_ECUDA, "cudaMalloc of %zu bytes failed", total);
     size_t off = 0;
+    DevPtrs dev;
     for (const auto& s : m->specs) {
         const auto& hv = m->host[s.key];
         float* d = reinterpret_cast<float*>(static_cast<char*>(m->arena.p) + off);
         CK(cudaMemcpy(d, hv.data(), hv.size() * 4, cudaMemcpyHostToDevice));
-        m->dev[s.key] = d;
+        dev[s.key] = d;
         off += (hv.size() * 4 + 255) & ~(size_t)255;
     }
     if (!c.sb_tcn && pack_lstm(m, "sb_model", m->Isb, 64, c.sb_hidden, c.num_layers, m->sb_frag, m->sb_bias)) return fail(FSN_ECUDA, "packing sb_model failed");
@@ -656,32 +721,20 @@ extern "C" int fsn_model_finalize(fsn_model* m) {
         }
     }
     if (c.model_kind == FSN_KIND_PLUS) {
-        int rc = pack_tcn5(m);
+        int rc = pack_tcn5(m, dev);
         if (rc) return rc;
     }
     if (c.sb_tcn) {
-        int rc = pack_sb_tcn(m);
+        int rc = pack_sb_tcn(m, dev);
         if (rc) return rc;
     }
+    bind_weights(m, dev);
     uint64_t id = 0xcbf29ce484222325ull;
     for (const auto& kv : m->param_hash) id = hash_words(id, &kv.second, sizeof(kv.second));   // std::map: key order
     id ^= id >> 33; id *= 0xff51afd7ed558ccdull; id ^= id >> 33;                              // final avalanche
     m->weights_id = id ? id : 1;                                                               // 0 means "not finalized"
     m->finalized = true;
     return FSN_OK;
-}
-
-static const float* P(fsn_model* m, const std::string& k) { return m->dev.at(k); }
-
-
-static void fill_ws(fsn_model* m, LstmWsLaunch& w) {
-    const fsn_config& c = m->cfg;
-    for (int l = 0; l < c.num_layers; ++l) {
-        const std::string s = std::to_string(l);
-        w.w_ih[l] = P(m, "fb_model.sequence_model.weight_ih_l" + s); w.w_hh[l] = P(m, "fb_model.sequence_model.weight_hh_l" + s);
-        w.b_ih[l] = P(m, "fb_model.sequence_model.bias_ih_l" + s); w.b_hh[l] = P(m, "fb_model.sequence_model.bias_hh_l" + s);
-    }
-    w.L = c.num_layers; w.H = c.fb_hidden; w.I = c.num_freqs; w.Ipad = (c.num_freqs + 15) / 16 * 16; w.fast = c.fast_math; w.gru = c.rnn_type == FSN_RNN_GRU;
 }
 
 // The implementation the sub-band LSTM reports (last_impl), and the one a forced lstm_impl names in its error
@@ -918,8 +971,8 @@ static int sb_layers(fsn_model* m, const LstmTc5rLaunch& a, __half* gin, size_t 
         }
         al.wstream = static_cast<const __half*>(m->r_stream[l].p);
         al.bias = static_cast<const float*>(m->r_bias[l].p);
-        al.fc_w = P(m, "sb_model.fc_output_layer.weight");
-        al.fc_b = P(m, "sb_model.fc_output_layer.bias");
+        al.fc_w = m->sb_fc_w;
+        al.fc_b = m->sb_fc_b;
         al.H = H; al.F = c.num_freqs; al.act = c.sb_act; al.fast = c.fast_math; al.gru = c.rnn_type == FSN_RNN_GRU; al.last = (l == c.num_layers - 1);
         al.cstate = a.cstate + l * cs_layer;
         if (a.hstate) al.hstate = a.hstate + l * hs_layer;
@@ -970,20 +1023,12 @@ static int run_sb_lstm(fsn_model* m, Lane& ln, int B, int T, int Tw, SbPackLaunc
     } else if (impl == FSN_LSTM_TCGEN05) {
         return fail(FSN_EINVAL, "the tensor-core LSTM needs hidden %% 64 == 0 and <= 512, input <= 64, output_size 2");
     } else {
-        LstmMmaLaunch a{};
-        for (int l = 0; l < c.num_layers; ++l) {
-            a.w.wfrag[l] = static_cast<const uint4*>(m->sb_frag[l].p);
-            a.w.bias[l] = static_cast<const float*>(m->sb_bias[l].p);
-        }
-        a.w.fc_w = P(m, "sb_model.fc_output_layer.weight");
-        a.w.fc_b = P(m, "sb_model.fc_output_layer.bias");
-        a.L = c.num_layers; a.H = c.sb_hidden; a.I = m->Isb; a.Ipad = 64;
+        LstmMmaLaunch a = m->sb_mma;
         a.rows = rows; a.Tp = Tp;
         a.img = static_cast<const __half*>(ln.ximg.p); a.ntiles = ntiles;
         a.cstate = static_cast<float*>(m->cstate.p);
         lstm_mma_cstate_bytes(c.num_layers, rows, c.sb_hidden, &a.rows_alloc);
-        a.out = d_out; a.O = c.output_size; a.F = F; a.la = c.look_ahead; a.act = c.sb_act;
-        a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU; a.tlen = tlen;
+        a.out = d_out; a.la = c.look_ahead; a.tlen = tlen;
         if (d_enh) {                                                    // generic kernel: mask into a scratch buffer, then one fused post-processing pass
             if (m->mask_tmp.ensure((size_t)B * 2 * F * T * 4, false, s)) return fail(FSN_ECUDA, "allocation failed");
             a.out = static_cast<float*>(m->mask_tmp.p);
@@ -1016,11 +1061,11 @@ static int run_tcn_blocks(fsn_model* m, const TcnWeights& w, TcnScratch& sc, con
         double* st1 = tcn_gln_sums(sc.stats.p, Z, blk, 0);
         double* st2 = tcn_gln_sums(sc.stats.p, Z, blk, 1);
         const float* amax_in = blk ? tcn_amax(sc.stats.p, Z, blk) : amax0;
-        auto key = [&](int b, const char* leaf) { return w.pre[b] + std::to_string(blk) + "." + leaf; };
+        const TcnWeights::Block* p = w.p[blk];
         GemmTc5Launch g1{};
         set_tcn_rows(g1, w, G, Tp);
         g1.epi = EPI5_PRELU_STATS; g1.Kp = w.Cp; g1.NT = 128; g1.ntiles_n = 4; g1.Npad = 512;
-        for (int b = 0; b < w.nbr; ++b) { g1.bias[b] = P(m, key(b, "conv1x1.bias")); g1.prelu[b] = P(m, key(b, "prelu1.weight")); }
+        for (int b = 0; b < w.nbr; ++b) { g1.bias[b] = p[b].conv1x1_b; g1.prelu[b] = p[b].prelu1; }
         g1.stats_out = st1; g1.Y16 = static_cast<__half*>(sc.y1.p); g1.ldY = 512; g1.amax_in = amax_in; g1.tlen = tlen; g1.zdiv = zdiv;
         int e = launch_gemm_tc5(curmap, w.mapW1[blk], g1, m->num_sms, s);
         if (e) return fail(FSN_ECUDA, "%s GEMM1 launch failed: %s", w.name, cudaGetErrorString((cudaError_t)e));
@@ -1031,9 +1076,7 @@ static int run_tcn_blocks(fsn_model* m, const TcnWeights& w, TcnScratch& sc, con
         dw.Z = (int)Z; dw.B = G; dw.C = 512; dw.Tp = Tp; dw.dilation = dil[blk]; dw.causal = causal ? 1 : 0;
         dw.stats_in = st1; dw.stats_out = st2; dw.amax = amax_in; dw.tlen = tlen; dw.zdiv = zdiv;
         for (int b = 0; b < w.nbr; ++b) {
-            dw.gamma[b] = P(m, key(b, "norm1.weight")); dw.beta[b] = P(m, key(b, "norm1.bias"));
-            dw.w[b] = P(m, key(b, "depthwise_conv.weight")); dw.b[b] = P(m, key(b, "depthwise_conv.bias"));
-            dw.prelu[b] = P(m, key(b, "prelu2.weight"));
+            dw.gamma[b] = p[b].norm1_w; dw.beta[b] = p[b].norm1_b; dw.w[b] = p[b].dw_w; dw.b[b] = p[b].dw_b; dw.prelu[b] = p[b].prelu2;
         }
         e = launch_dwconv_tm(dw, s);
         if (e) return fail(FSN_ECUDA, "%s depth-wise conv launch failed: %s", w.name, cudaGetErrorString((cudaError_t)e));
@@ -1073,7 +1116,7 @@ static int run_sb_tcn(fsn_model* m, Lane& ln, int B, int T, int Fc, SbPackLaunch
     m->last_impl = FSN_LSTM_TCN;
     GemmTc5Launch head{};
     head.epi = EPI5_GLN_HEAD;
-    head.fc_w = static_cast<const float*>(m->sb_fc.p); head.fc_b = P(m, "sb_model.fc_output_layer.bias");
+    head.fc_w = static_cast<const float*>(m->sb_fc.p); head.fc_b = m->sb_fc_b;
     head.O = c.output_size; head.la = c.look_ahead; head.F = F; head.act = c.sb_act;
     head.out = d_out; head.nreal = d_real; head.nimag = d_imag; head.enh = reinterpret_cast<float2*>(d_enh);
     float* x = static_cast<float*>(ln.sbx.p);
@@ -1091,6 +1134,35 @@ static int run_sb_tcn(fsn_model* m, Lane& ln, int B, int T, int Fc, SbPackLaunch
         if (rc) return rc;
     }
     return FSN_OK;
+}
+
+// The state of the full-band LSTM of fullsubnet.Model (run_fb), as LstmWsLaunch / LstmMmaLaunch name it; cbuf and hstate are null in
+// the offline forward, which keeps no state.  slot, kf: the streaming slot calls' per-slot counts and frame counts, or null.
+struct FbState {
+    __half* hbuf; float* cbuf; unsigned int* barrier;  // weight-stationary kernel
+    float* cstate; int rows_alloc; __half* hstate;     // generic kernel
+    int resume, t0;
+    const int *slot, *kf;
+};
+
+// The full band of fullsubnet.Model over `rows` clips (or slots) of Tp frames at row pitch P: fb_pack of fbin [rows, F, P] into fbx
+// [Tp, rows_pad, Ipad], the LSTM into hseq [rows, H, P] (the weight-stationary kernel if use_ws, else the generic one), then the output
+// Linear into fbout [rows, F, P].  Returns the number of launches, or minus the LSTM's launch error (each caller words its report).
+static int run_fb(fsn_model* m, const float* fbin, __half* fbx, float* hseq, float* fbout, int rows, int rows_pad, int Tp, int P,
+                  bool use_ws, const FbState& fs, cudaStream_t s) {
+    launch_fb_pack(fbin, fbx, rows, m->cfg.num_freqs, Tp, P, rows_pad, m->fb_mma.Ipad, s);
+    LstmWsLaunch w = m->fb_ws;
+    LstmMmaLaunch a = m->fb_mma;
+    w.rows = rows; w.rows_pad = rows_pad; w.Tp = Tp; w.x = fbx; w.hseq = hseq; w.P = P;
+    w.hbuf = fs.hbuf; w.cbuf = fs.cbuf; w.barrier = fs.barrier; w.resume = fs.resume; w.t0 = fs.t0; w.slot = fs.slot; w.kf = fs.kf;
+    a.rows = rows; a.rows_pad = rows_pad; a.Tp = Tp; a.xplain = fbx; a.hseq = hseq; a.P = P;
+    a.cstate = fs.cstate; a.rows_alloc = fs.rows_alloc; a.hstate = fs.hstate; a.resume = fs.resume; a.slot = fs.slot; a.kf = fs.kf;
+    a.slot_rows = fs.hstate ? 1 : 0;                                    // streaming: row r is slot r
+    if (int e = use_ws ? launch_lstm_ws(w, s) : launch_lstm_mma(a, s)) return -e;
+    ConvLaunch cf = m->fb_out;
+    cf.X = hseq; cf.Y = fbout; cf.Z = rows; cf.Tp = Tp; cf.P = P;
+    launch_conv1x1(cf, s);
+    return 3;
 }
 
 // The whole forward.  Front end (norm, attention, full-band model, sub-band statistics + packing) on stream `s` into lane `ln`;
@@ -1181,45 +1253,34 @@ static int forward_impl(fsn_model* m, Lane& ln, const float* d_mag, const float*
     sp.tlen = tl;
     sp.f0 = 0; sp.Fc = F;
 
-    if (c.model_kind == FSN_KIND_PLUS) {
-        const char* sfx[3] = {"", "_real", "_imag"};
-        const char* cn[3] = {"smallConv1d", "middleConv1d", "largeConv1d"};
-        TsseLaunch ta{};
-        ta.x[0] = d_mag; ta.x[1] = d_real; ta.x[2] = d_imag;
-        ta.nbranch = 3; ta.B = B; ta.F = F; ta.T = T; ta.Tp = Tp; ta.P = Pp; ta.attention = 1 + c.channel_attention; ta.sub = c.subband_num;
+    // the input norm of every branch (3 in FullSubNet+, 1 in fullsubnet.Model), and FullSubNet+'s channel attention
+    const bool plus = c.model_kind == FSN_KIND_PLUS;
+    const int nbr = plus ? 3 : 1;
+    TsseLaunch ta{{d_mag, plus ? d_real : nullptr, plus ? d_imag : nullptr}};
+    ta.nbranch = nbr; ta.B = B; ta.F = F; ta.T = T; ta.Tp = Tp; ta.P = Pp;
+    ta.out = static_cast<float*>(ln.fbin.p);
+    ta.scale = static_cast<float*>(ln.tsse_scale.p);
+    ta.rows = ta.scale + (size_t)nbr * B * F;
+    ta.tlen = tl;
+    if (c.norm_type != FSN_NORM_OFFLINE_LAPLACE) {
+        const NormLaunch na{{ta.x[0], ta.x[1], ta.x[2]}, static_cast<float*>(ln.xn.p), nbr, B, F, T, Tp, c.norm_type, tl};
+        launch_input_norm(na, s); m->launches++;
+        for (int b = 0; b < nbr; ++b) ta.x[b] = static_cast<const float*>(ln.xn.p) + (size_t)b * B * F * Tp;
+        ta.T = Tp; ta.prenorm = 1;                                      // padded frames are part of the normalised signal
+    }
+    if (plus) {
+        ta.attention = 1 + c.channel_attention; ta.sub = c.subband_num;
         for (int i = 0; i < 3; ++i) ta.ksz[i] = c.kersize[i];
-        for (int b = 0; b < 3; ++b) {
-            const std::string p = std::string("channel_attention") + sfx[b];
-            if (c.channel_attention == FSN_ATTN_ECA) { ta.p[b].eca_w = P(m, p + ".conv.weight"); continue; }
-            if (c.channel_attention == FSN_ATTN_TSSE) {
-                for (int i = 0; i < 3; ++i) {
-                    ta.p[b].conv_w[i] = P(m, p + "." + cn[i] + ".0.weight");
-                    ta.p[b].conv_b[i] = P(m, p + "." + cn[i] + ".0.bias");
-                }
-                ta.p[b].cat_w = P(m, p + ".feature_concate_fc.weight"); ta.p[b].cat_b = P(m, p + ".feature_concate_fc.bias");
-            }
-            ta.p[b].fc1_w = P(m, p + ".fc1.weight"); ta.p[b].fc1_b = P(m, p + ".fc1.bias");
-            ta.p[b].fc2_w = P(m, p + ".fc2.weight"); ta.p[b].fc2_b = P(m, p + ".fc2.bias");
-        }
-        ta.out = static_cast<float*>(ln.fbin.p);
-        ta.scale = static_cast<float*>(ln.tsse_scale.p);
-        ta.rows = ta.scale + (size_t)ta.nbranch * B * F;
+        for (int b = 0; b < 3; ++b) ta.p[b] = m->tsse[b];
         ta.out_tm = static_cast<float*>(ln.x0.p); ta.Cp = m->tcn_fb.Cp;
-        ta.tlen = tl;
-        if (c.norm_type != FSN_NORM_OFFLINE_LAPLACE) {
-            NormLaunch na{};
-            na.x[0] = d_mag; na.x[1] = d_real; na.x[2] = d_imag; na.y = static_cast<float*>(ln.xn.p);
-            na.nbranch = 3; na.B = B; na.F = F; na.T = T; na.Tp = Tp; na.type = c.norm_type; na.tlen = tl;
-            launch_input_norm(na, s); m->launches++;
-            for (int b = 0; b < 3; ++b) ta.x[b] = static_cast<const float*>(ln.xn.p) + (size_t)b * B * F * Tp;
-            ta.T = Tp; ta.prenorm = 1;                                  // padded frames are part of the normalised signal
-        }
         m->last_fb_ws = 0;
-        const TcnWeights& w = m->tcn_fb;
         CK(cudaMemsetAsync(ln.tcn.stats.p, 0, tcn_stats_bytes(3 * B), s));
         ta.amax = tcn_amax(ln.tcn.stats.p, 3 * B, 0);                  // block 0: written by the gate kernel
-        launch_tsse_norm(ta, s); m->launches += 3;
+    }
+    launch_tsse_norm(ta, s); m->launches += 3;
 
+    if (plus) {
+        const TcnWeights& w = m->tcn_fb;
         GemmTc5Launch last{};                                           // the last block also writes relu(x) for the output Linear
         last.epi = EPI5_GLN_RES; last.Xrelu = static_cast<float*>(ln.xr.p);
         rc = run_tcn_blocks(m, w, ln.tcn, static_cast<const float*>(ln.x0.p), ln.mapX0, ta.amax, B, Tp, c.tcn_causal, last, tl, 1, s);
@@ -1237,59 +1298,22 @@ static int forward_impl(fsn_model* m, Lane& ln, const float* d_mag, const float*
         sp.nfb = 3;
         for (int b = 0; b < 3; ++b) sp.fb[b] = static_cast<const float*>(ln.fbout.p) + (size_t)b * B * F * Pp;
     } else {
-        TsseLaunch ta{};
-        ta.x[0] = d_mag; ta.nbranch = 1; ta.B = B; ta.F = F; ta.T = T; ta.Tp = Tp; ta.P = Pp; ta.attention = 0;
-        ta.out = static_cast<float*>(ln.fbin.p);
-        ta.scale = static_cast<float*>(ln.tsse_scale.p);
-        ta.rows = ta.scale + (size_t)ta.nbranch * B * F;
-        ta.tlen = tl;
-        if (c.norm_type != FSN_NORM_OFFLINE_LAPLACE) {
-            NormLaunch na{};
-            na.x[0] = d_mag; na.y = static_cast<float*>(ln.xn.p);
-            na.nbranch = 1; na.B = B; na.F = F; na.T = T; na.Tp = Tp; na.type = c.norm_type; na.tlen = tl;
-            launch_input_norm(na, s); m->launches++;
-            ta.x[0] = static_cast<const float*>(ln.xn.p); ta.T = Tp; ta.prenorm = 1;
-        }
-        launch_tsse_norm(ta, s); m->launches += 3;
         launch_pad_copy(d_mag, static_cast<float*>(ln.magpad.p), B, F, T, Pp, tl, c.look_ahead, s); m->launches++;
         // the full-band LSTM is causal, and its input (fb_in) is already zero past each clip's end: its outputs there are masked by the
         // sub-band stages
-        const int Ipad = (F + 15) / 16 * 16, rows_pad = (B + 63) / 64 * 64;
-        launch_fb_pack(static_cast<const float*>(ln.fbin.p), static_cast<__half*>(ln.fbx.p), B, F, Tp, Pp, rows_pad, Ipad, s); m->launches++;
-        m->last_fb_ws = lstm_ws_supported(c.num_layers, c.fb_hidden, Ipad, B, m->num_sms) && !m->env_no_ws;
+        m->last_fb_ws = lstm_ws_supported(c.num_layers, c.fb_hidden, m->fb_ws.Ipad, B, m->num_sms) && !m->env_no_ws;
         if (m->last_fb_ws) {
             const size_t hb = (size_t)c.num_layers * 2 * 64 * c.fb_hidden * 2;
             if (m->ws_h.ensure(hb, false, s) || m->ws_bar.ensure(64, true, s)) return fail(FSN_ECUDA, "allocation failed");
             CK(cudaMemsetAsync(m->ws_h.p, 0, hb, s));
-            LstmWsLaunch w{};
-            fill_ws(m, w);
-            w.rows = B; w.rows_pad = rows_pad; w.Tp = Tp;
-            w.x = static_cast<const __half*>(ln.fbx.p); w.hbuf = static_cast<__half*>(m->ws_h.p); w.cbuf = nullptr;
-            w.barrier = static_cast<unsigned int*>(m->ws_bar.p);
-            w.hseq = static_cast<float*>(ln.hseq.p); w.P = Pp; w.resume = 0; w.t0 = 0;
-            int e = launch_lstm_ws(w, s);
-            if (e) return fail(FSN_ECUDA, "weight-stationary full-band LSTM launch failed: %s", cudaGetErrorString((cudaError_t)e));
-            m->launches++;
-        } else {
-        LstmMmaLaunch a{};
-        for (int l = 0; l < c.num_layers; ++l) {
-            a.w.wfrag[l] = static_cast<const uint4*>(m->fb_frag[l].p);
-            a.w.bias[l] = static_cast<const float*>(m->fb_bias[l].p);
         }
-        a.L = c.num_layers; a.H = c.fb_hidden; a.I = F; a.Ipad = Ipad; a.rows = B; a.Tp = Tp;
-        a.xplain = static_cast<const __half*>(ln.fbx.p); a.rows_pad = rows_pad;
-        a.cstate = static_cast<float*>(m->cstate.p);
-        lstm_mma_cstate_bytes(c.num_layers, B, c.fb_hidden, &a.rows_alloc);
-        a.hseq = static_cast<float*>(ln.hseq.p); a.P = Pp; a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU;
-        int e = launch_lstm_mma(a, s);
-        if (e) return fail(FSN_ECUDA, "full-band LSTM launch failed: %s", cudaGetErrorString((cudaError_t)e));
-        m->launches++;
-        }
-        ConvLaunch cf{};
-        cf.X = static_cast<const float*>(ln.hseq.p); cf.Y = static_cast<float*>(ln.fbout.p);
-        cf.Z = B; cf.M = F; cf.K = c.fb_hidden; cf.Tp = Tp; cf.P = Pp; cf.act = c.fb_act;
-        cf.W = P(m, "fb_model.fc_output_layer.weight"); cf.bias = P(m, "fb_model.fc_output_layer.bias");
-        launch_conv1x1(cf, s); m->launches++;
+        FbState fs{static_cast<__half*>(m->ws_h.p), nullptr, static_cast<unsigned int*>(m->ws_bar.p), static_cast<float*>(m->cstate.p)};
+        lstm_mma_cstate_bytes(c.num_layers, B, c.fb_hidden, &fs.rows_alloc);
+        const int nl = run_fb(m, static_cast<const float*>(ln.fbin.p), static_cast<__half*>(ln.fbx.p), static_cast<float*>(ln.hseq.p),
+                              static_cast<float*>(ln.fbout.p), B, (B + 63) / 64 * 64, Tp, Pp, m->last_fb_ws, fs, s);
+        if (nl < 0)
+            return fail(FSN_ECUDA, "%sfull-band LSTM launch failed: %s", m->last_fb_ws ? "weight-stationary " : "", cudaGetErrorString((cudaError_t)-nl));
+        m->launches += nl;
 
         sp.win = static_cast<const float*>(ln.magpad.p); sp.Pw = Pp;    // raw padded magnitude (fullsubnet.py:94)
         sp.nfb = 1;
@@ -2070,46 +2094,21 @@ static int step_frames(fsn_stream* st, StepScratch& x, const float* d_mag, int K
     }
     StreamNormLaunch na{d_mag, static_cast<float*>(x.fbin.p), static_cast<double*>(st->cum_in.p), B, F, K, Pk, n, c.norm_type, slot, kf};
     launch_stream_norm(na, s);
-    launch_fb_pack(static_cast<const float*>(x.fbin.p), static_cast<__half*>(x.fbx.p), B, F, K, Pk, st->rows_pad, st->Ipad, s);
-    int e = 0;
-    if (st->use_ws) {
-        LstmWsLaunch w{};
-        fill_ws(m, w);
-        w.rows = B; w.rows_pad = st->rows_pad; w.Tp = K;
-        w.x = static_cast<const __half*>(x.fbx.p); w.hbuf = static_cast<__half*>(st->ws_h.p); w.cbuf = static_cast<float*>(st->ws_c.p);
-        w.barrier = static_cast<unsigned int*>(st->ws_bar.p);
-        w.hseq = static_cast<float*>(x.hseq.p); w.P = Pk; w.resume = resume; w.t0 = n; w.slot = slot; w.kf = kf;
-        e = launch_lstm_ws(w, s);
-    } else {
-        LstmMmaLaunch a{};
-        for (int l = 0; l < L; ++l) { a.w.wfrag[l] = static_cast<const uint4*>(m->fb_frag[l].p); a.w.bias[l] = static_cast<const float*>(m->fb_bias[l].p); }
-        a.L = L; a.H = c.fb_hidden; a.I = F; a.Ipad = st->Ipad; a.rows = B; a.Tp = K;
-        a.xplain = static_cast<const __half*>(x.fbx.p); a.rows_pad = st->rows_pad;
-        a.cstate = static_cast<float*>(st->c_fb.p); a.rows_alloc = st->ra_fb;
-        a.hseq = static_cast<float*>(x.hseq.p); a.P = Pk; a.fast = c.fast_math; a.gru = c.rnn_type == FSN_RNN_GRU;
-        a.hstate = static_cast<__half*>(st->h_fb.p); a.resume = resume; a.slot = slot; a.slot_rows = 1; a.kf = kf;
-        e = launch_lstm_mma(a, s);
-    }
-    if (e) return fail(FSN_ECUDA, "full-band LSTM step failed: %s", cudaGetErrorString((cudaError_t)e));
-    ConvLaunch cf{};
-    cf.X = static_cast<const float*>(x.hseq.p); cf.Y = static_cast<float*>(x.fbout.p);
-    cf.Z = B; cf.M = F; cf.K = c.fb_hidden; cf.Tp = K; cf.P = Pk; cf.act = c.fb_act;
-    cf.W = P(m, "fb_model.fc_output_layer.weight"); cf.bias = P(m, "fb_model.fc_output_layer.bias");
-    launch_conv1x1(cf, s);
+    const FbState fs{static_cast<__half*>(st->ws_h.p), static_cast<float*>(st->ws_c.p), static_cast<unsigned int*>(st->ws_bar.p),
+                     static_cast<float*>(st->c_fb.p), st->ra_fb, static_cast<__half*>(st->h_fb.p), resume, n, slot, kf};
+    const int nl = run_fb(m, static_cast<const float*>(x.fbin.p), static_cast<__half*>(x.fbx.p), static_cast<float*>(x.hseq.p),
+                          static_cast<float*>(x.fbout.p), B, st->rows_pad, K, Pk, st->use_ws, fs, s);
+    if (nl < 0) return fail(FSN_ECUDA, "full-band LSTM step failed: %s", cudaGetErrorString((cudaError_t)-nl));
     StreamPackLaunch pa{d_mag, static_cast<const float*>(x.fbout.p), Pk, static_cast<double*>(st->cum_sb.p), static_cast<__half*>(x.ximg.p),
                         B, F, K, c.sb_num_neighbors, c.fb_num_neighbors, n, c.norm_type, 0, K, slot, nullptr, 0, 0, kf};
     if (!lw) {
         launch_stream_pack(pa, s);
-        LstmMmaLaunch b{};
-        for (int l = 0; l < L; ++l) { b.w.wfrag[l] = static_cast<const uint4*>(m->sb_frag[l].p); b.w.bias[l] = static_cast<const float*>(m->sb_bias[l].p); }
-        b.w.fc_w = P(m, "sb_model.fc_output_layer.weight"); b.w.fc_b = P(m, "sb_model.fc_output_layer.bias");
-        b.L = L; b.H = c.sb_hidden; b.I = m->Isb; b.Ipad = 64; b.rows = B * F; b.Tp = K;
+        LstmMmaLaunch b = m->sb_mma;
+        b.rows = B * F; b.Tp = K; b.out = d_mask; b.la = 0;
         b.img = static_cast<const __half*>(x.ximg.p); b.ntiles = (B * F + 127) / 128;
         b.cstate = static_cast<float*>(st->c_sb.p); b.rows_alloc = st->ra_sb;
-        b.out = d_mask; b.O = c.output_size; b.F = F; b.la = 0; b.act = c.sb_act; b.fast = c.fast_math; b.gru = c.rnn_type == FSN_RNN_GRU;
         b.hstate = static_cast<__half*>(st->h_sb.p); b.resume = resume; b.slot = slot; b.slot_rows = F; b.slot_la = c.look_ahead; b.kf = kf;
-        e = launch_lstm_mma(b, s);
-        if (e) return fail(FSN_ECUDA, "sub-band LSTM step failed: %s", cudaGetErrorString((cudaError_t)e));
+        if (int e = launch_lstm_mma(b, s)) return fail(FSN_ECUDA, "sub-band LSTM step failed: %s", cudaGetErrorString((cudaError_t)e));
     } else {
         // layer-wise sub band, per group of kf frames: its sessions compacted to rows j F + f, in sub-batches of p.Bs sessions and
         // windows of p.Tw frames.  The recurrence runs as window t0 = 4 + w0 of a 4 + kf step sequence with la = 4: it loads h / c from

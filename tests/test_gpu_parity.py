@@ -543,3 +543,38 @@ def test_layerwise_tcgen05_vs_oracle(built_lib, L, H, rnn):
     print(f"\n[layer-wise L={L} H={H} {rnn}] cIRM {err:.3e}")
     assert torch.equal(out, out2)
     assert err < MASK_TOL
+
+
+@pytest.mark.parametrize("case", ["plus_lstm", "plus_sbtcn", "fsn_ws", "fsn_no_ws"])
+def test_weights_changed_after_forward(built_lib, monkeypatch, case):
+    """Parameters changed in place after a forward are pushed again at the next call, and that forward reads them everywhere: the
+    attention, the full-band TCN and the layer-wise sub-band LSTM's head (H = 64), the sub-band TCN, and fullsubnet.Model's full band on
+    the weight-stationary and the generic kernel with its generic sub-band LSTM.  It must match a model built with the new weights."""
+    from fsnplus_b200 import _lib
+    if case == "fsn_no_ws":
+        monkeypatch.setenv("FSN_NO_WS", "1")
+    mag, real, imag = small_inputs(2, 33, 20, 7)
+    if case.startswith("plus"):
+        from sbtcn_oracle import make_params
+        cfg = dict(small_cfg(64), sequence_model="TCN" if case == "plus_sbtcn" else "LSTM")
+        params = make_params(cfg, seed=3) if case == "plus_sbtcn" else O.make_params_plus(cfg, seed=3)
+        build, x = build_plus, (mag, real, imag)
+    else:
+        cfg = O.default_fsn_config()
+        cfg.update(num_freqs=33, sb_num_neighbors=3, sb_model_hidden_size=32, fb_model_hidden_size=48)
+        params, build, x = O.make_params_fsn(cfg, seed=4), build_fsn, (mag,)
+    m = build(cfg, params)
+    with torch.no_grad():
+        before = m(*map(_t, x)).cpu().numpy()
+        for p in m.parameters():
+            p.mul_(1.25)
+        after = m(*map(_t, x)).cpu().numpy()
+    if case.startswith("fsn"):
+        assert _lib.load_library().fsn_model_last_fb_ws(m._handle) == (case == "fsn_ws")
+    fresh = build(cfg, {k: v * np.float32(1.25) for k, v in params.items()})
+    with torch.no_grad():
+        want = fresh(*map(_t, x)).cpu().numpy()
+    changed, err = O.rel_l2(after, before), O.rel_l2(after, want)
+    print(f"\n[{case}] changed {changed:.3e}, vs fresh model {err:.3e}")
+    assert changed > 1e-3
+    assert err < 1e-6

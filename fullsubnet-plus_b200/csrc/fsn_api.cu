@@ -263,9 +263,15 @@ static int sb_input_size(const fsn_config& c) {
     return (2 * c.sb_num_neighbors + 1) + (c.model_kind == FSN_KIND_PLUS ? 3 : 1) * (2 * c.fb_num_neighbors + 1);
 }
 
-// The layer-wise kernels (k_lstm_tc5r.cu) take this geometry (hidden % 64 == 0 and <= 512, output_size 2, input <= 64): their weights are packed
+// A wide sub-band input (64 < Isb <= 128, DESIGN.md §3.3): packed as plain fp16 rows of 128 halves (the fused first-layer tile and the
+// swizzled images hold 64); the layer-wise path projects it with one GEMM per window, the generic kernel reads it with Ipad = 128
+static bool sb_wide(const fsn_config& c) { return sb_input_size(c) > 64; }
+// bytes of one packed sub-band input row (one sequence, one frame)
+static size_t sb_row_bytes(const fsn_config& c) { return sb_wide(c) ? 256 : 128; }
+
+// The layer-wise kernels (k_lstm_tc5r.cu) take this geometry (hidden % 64 == 0 and <= 512, output_size 2, input <= 128): their weights are packed
 static bool tc5r_ok(const fsn_config& c) {
-    return !c.sb_tcn && lstm_tc5r_supported(c.sb_hidden, c.output_size) && sb_input_size(c) <= 64;
+    return !c.sb_tcn && lstm_tc5r_supported(c.sb_hidden, c.output_size) && sb_input_size(c) <= 128;
 }
 
 // The sub-band LSTM runs layer-wise (else on the generic mma.sync kernel): lstm_impl = auto or tcgen05 (FSN_LSTM_TCGEN05, the historical
@@ -543,7 +549,7 @@ static void bind_weights(fsn_model* m, const DevPtrs& dev) {
             a.w.bias[l] = static_cast<const float*>(m->sb_bias[l].p);
         }
         a.w.fc_w = m->sb_fc_w; a.w.fc_b = m->sb_fc_b;
-        a.L = L; a.H = c.sb_hidden; a.I = m->Isb; a.Ipad = 64;
+        a.L = L; a.H = c.sb_hidden; a.I = m->Isb; a.Ipad = sb_wide(c) ? 128 : 64;
         a.O = c.output_size; a.F = c.num_freqs; a.act = c.sb_act; a.fast = c.fast_math; a.gru = gru;
     }
 }
@@ -578,7 +584,9 @@ extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
             if (c.channel_attention == FSN_ATTN_TSSE && (c.kersize[i] < 1 || c.kersize[i] > 16)) return fail(FSN_EINVAL, "kersize must be in 1..16");
     }
     const int isb = sb_input_size(c);
-    if (isb > 64) return fail(FSN_EINVAL, "sub-band input size %d > 64 not supported", isb);
+    if (c.sb_tcn && isb > 64)
+        return fail(FSN_EINVAL, "sub-band input size %d > 64 not supported by the sub-band TCN (its output head holds a row's channels in one 64-column tile)", isb);
+    if (isb > 128) return fail(FSN_EINVAL, "sub-band input size %d > 128 not supported", isb);
     int sb_window = 0;
     if (const char* e = getenv("FSN_SB_WINDOW"); e && *e) {
         char* end = nullptr;
@@ -695,7 +703,8 @@ extern "C" int fsn_model_finalize(fsn_model* m) {
         dev[s.key] = d;
         off += (hv.size() * 4 + 255) & ~(size_t)255;
     }
-    if (!c.sb_tcn && pack_lstm(m, "sb_model", m->Isb, 64, c.sb_hidden, c.num_layers, m->sb_frag, m->sb_bias)) return fail(FSN_ECUDA, "packing sb_model failed");
+    if (!c.sb_tcn && pack_lstm(m, "sb_model", m->Isb, sb_wide(c) ? 128 : 64, c.sb_hidden, c.num_layers, m->sb_frag, m->sb_bias))
+        return fail(FSN_ECUDA, "packing sb_model failed");
     if (c.model_kind == FSN_KIND_FSN) {
         const int Ipad = (c.num_freqs + 15) / 16 * 16;
         if (pack_lstm(m, "fb_model", c.num_freqs, Ipad, c.fb_hidden, c.num_layers, m->fb_frag, m->fb_bias)) return fail(FSN_ECUDA, "packing fb_model failed");
@@ -704,15 +713,16 @@ extern "C" int fsn_model_finalize(fsn_model* m) {
         const int H = c.sb_hidden;
         for (int l = 0; l < c.num_layers; ++l) {
             const std::string q = "sb_model.sequence_model.", sl = std::to_string(l);
-            const int Kin = (l == 0) ? m->Isb : H, Kpad = (l == 0) ? 64 : H;
+            const bool fused = l == 0 && !sb_wide(c);                       // the input projection is part of the recurrence
+            const int Kin = (l == 0) ? m->Isb : H, Kpad = (l == 0) ? (fused ? 64 : 128) : H;
             std::vector<uint16_t> st, wp;
             std::vector<float> bp;
             lstm_tc5r_pack_layer(H, Kin, Kpad, m->host[q + "weight_ih_l" + sl].data(), m->host[q + "weight_hh_l" + sl].data(),
                                  m->host[q + "bias_ih_l" + sl].data(), m->host[q + "bias_hh_l" + sl].data(), c.rnn_type == FSN_RNN_GRU, st, wp, bp);
-            if (l == 0) {                                                   // first layer: [W_ih | W_hh] blocks, the input projection is in the recurrence
+            if (fused) {                                                    // first layer: [W_ih | W_hh] blocks, the input projection is in the recurrence
                 st.assign((size_t)(H / 32) * (1 + H / 64) * 8192, 0);
                 lstm_tc5_pack_first_layer(Kin, H, m->host[q + "weight_ih_l0"].data(), m->host[q + "weight_hh_l0"].data(), st.data());
-            } else {                                                        // deeper layers: W_hh blocks + the input-projection GEMM's matrix
+            } else {                                                        // deeper layers, and a wide first layer: W_hh blocks + the input-projection GEMM's matrix
                 lstm_tc5r_gin_order(H, Kpad, wp);
                 if (upload(m->r_wih[l], wp.data(), wp.size() * 2)) return fail(FSN_ECUDA, "upload of the layer-wise LSTM weights failed");
             }
@@ -784,14 +794,15 @@ static WsSizes ws_sizes(const fsn_config& c, bool layerwise, int B, int T, int T
         z.sbx = srows * 64 * 4 + seqs * 4;                                      // input | block 0's stream maxima
         z.sb_xa = z.sb_xb = srows * 64 * 4; z.sb_y1 = z.sb_y2 = srows * 512 * sizeof(__half); z.sb_stats = tcn_stats_bytes(seqs);
     } else {
-        z.ximg = ntiles * Ts * 16384;
+        z.ximg = ntiles * Ts * 128 * sb_row_bytes(c);                          // wide: GEMM rows / time-major rows of 128 halves
     }
     int ra = 0;
     size_t cs = c.sb_tcn ? 0 : lstm_mma_cstate_bytes(c.num_layers, (int)rows, c.sb_hidden, &ra), cs5 = 0;
     if (layerwise) {
         const size_t M = ntiles * Ts * 128;
         cs5 = lstm_tc5r_cstate_bytes((int)ntiles, c.sb_hidden);
-        if (c.num_layers > 1) { z.r_gin = M * 4 * c.sb_hidden * 2; z.r_hseq = M * c.sb_hidden * 2; }
+        if (c.num_layers > 1 || sb_wide(c)) z.r_gin = M * 4 * c.sb_hidden * 2;   // a wide layer 0 is projected by the GEMM too
+        if (c.num_layers > 1) z.r_hseq = M * c.sb_hidden * 2;
         if (Tw) {                                                               // windowed: c / h of every layer carried to the next window
             cs5 *= c.num_layers;
             z.r_hstate = (size_t)c.num_layers * ntiles * 128 * c.sb_hidden * 2;
@@ -952,19 +963,21 @@ static int ensure_ws(fsn_model* m, Lane& ln, int B, int T, int Tw, int Fc, cudaS
 }
 
 // One window of the layer-wise sub-band recurrence, layer after layer: for l > 0 the input-projection GEMM of every row and frame of
-// the window into gin (k_gemm_tc5.cu), then lstm_tc5r_kernel; layer 0 projects its input (the packed images) itself.  a: the
-// window's launch (rows, ntiles, Tp, t0, Tw, ximg, hseq, out, la and the epilogue) with layer 0's cstate and hstate (null: none);
-// layer l's lie cs_layer floats and hs_layer halves further.  Returns the number of launches, or the error code.
+// the window into gin (k_gemm_tc5.cu), then lstm_tc5r_kernel; layer 0 projects its input (the packed images) itself, or, with a wide
+// input, through the same GEMM from a.ximg's rows of 128 halves (K = 128).  a: the window's launch (rows, ntiles, Tp, t0, Tw, ximg, hseq,
+// out, la and the epilogue) with layer 0's cstate and hstate (null: none); layer l's lie cs_layer floats and hs_layer halves further.
+// Returns the number of launches, or the error code.
 static int sb_layers(fsn_model* m, const LstmTc5rLaunch& a, __half* gin, size_t cs_layer, size_t hs_layer, cudaStream_t s) {
     const fsn_config& c = m->cfg;
     const int H = c.sb_hidden;
     int launches = 0;
     for (int l = 0; l < c.num_layers; ++l) {
         LstmTc5rLaunch al = a;
-        if (l > 0) {
-            // row-major Gin[M, 4H] = X[M, H] * Wp[4H, H]^T, both operands K-major
-            GemmF16Launch g{(long long)(a.ntiles + 1) / 2 * 2 * a.Tw * 128, 4 * H, H, gin, 4LL * H, m->env_gin_tile_n};
-            const int ge = launch_gemm_f16(a.hseq, m->r_wih[l].p, g, m->num_sms, s);
+        if (l > 0 || sb_wide(c)) {
+            // row-major Gin[M, 4H] = X[M, K] * Wp[4H, K]^T, both operands K-major (K = H; a wide layer 0: 128)
+            const int K = l > 0 ? H : 128;
+            GemmF16Launch g{(long long)(a.ntiles + 1) / 2 * 2 * a.Tw * 128, 4 * H, K, gin, 4LL * H, m->env_gin_tile_n};
+            const int ge = launch_gemm_f16(l > 0 ? static_cast<const void*>(a.hseq) : static_cast<const void*>(a.ximg), m->r_wih[l].p, g, m->num_sms, s);
             if (ge) return fail(FSN_ECUDA, "input-projection GEMM launch failed (layer %d): %s", l, cudaGetErrorString((cudaError_t)ge));
             launches++;
             al.ximg = nullptr; al.gin = gin;
@@ -1003,7 +1016,8 @@ static int run_sb_lstm(fsn_model* m, Lane& ln, int B, int T, int Tw, SbPackLaunc
             const int tw = Tw ? (Tp - w0 < Tw ? Tp - w0 : Tw) : Tp;
             if (Tw) {
                 sp.t0 = w0; sp.Tw = tw;
-                launch_sb_pack(sp, s);
+                if (sb_wide(c)) launch_sb_pack_wide(sp, false, s);
+                else launch_sb_pack(sp, s);
                 m->launches++;
             }
             LstmTc5rLaunch a{};
@@ -1021,11 +1035,13 @@ static int run_sb_lstm(fsn_model* m, Lane& ln, int B, int T, int Tw, SbPackLaunc
     } else if (Tw) {
         return fail(FSN_EINVAL, "time windows of the sub-band stage need the layer-wise LSTM path");
     } else if (impl == FSN_LSTM_TCGEN05) {
-        return fail(FSN_EINVAL, "the tensor-core LSTM needs hidden %% 64 == 0 and <= 512, input <= 64, output_size 2");
+        return fail(FSN_EINVAL, "the tensor-core LSTM needs hidden %% 64 == 0 and <= 512, input <= 128, output_size 2");
     } else {
         LstmMmaLaunch a = m->sb_mma;
         a.rows = rows; a.Tp = Tp;
-        a.img = static_cast<const __half*>(ln.ximg.p); a.ntiles = ntiles;
+        if (sb_wide(c)) { a.xplain = static_cast<const __half*>(ln.ximg.p); a.rows_pad = ntiles * 128; }   // time-major rows of 128 halves
+        else a.img = static_cast<const __half*>(ln.ximg.p);
+        a.ntiles = ntiles;
         a.cstate = static_cast<float*>(m->cstate.p);
         lstm_mma_cstate_bytes(c.num_layers, rows, c.sb_hidden, &a.rows_alloc);
         a.out = d_out; a.la = c.look_ahead; a.tlen = tlen;
@@ -1328,7 +1344,8 @@ static int forward_impl(fsn_model* m, Lane& ln, const float* d_mag, const float*
             m->launches++;
         }
     } else if (!Tw) {                                                   // windowed: run_sb_lstm packs each window
-        launch_sb_pack(sp, s);
+        if (sb_wide(c)) launch_sb_pack_wide(sp, !runs_layerwise(c, m->env_impl), s);
+        else launch_sb_pack(sp, s);
         m->launches++;
     }
     cudaEventRecord(m->evf1[evi], s);
@@ -1400,9 +1417,10 @@ static double ws_bytes_per_sample(const fsn_config& c, bool layerwise, int T, bo
         b += rows * Tp * (3 * 64 * 4 + 2 * 512 * 2) + rows * (tcn_stats_bytes(1) + 4);   // buffers of 512; statistics, the input's max |x|
         return b;
     }
-    b += rows * Tp * 128;                                                       // packed sub-band images (when used)
+    b += rows * Tp * sb_row_bytes(c);                                           // packed sub-band images (when used)
     b += rows * c.num_layers * c.sb_hidden * 4;                                  // cell state
     if (layerwise && c.num_layers > 1) b += rows * Tp * (4.0 * c.sb_hidden + c.sb_hidden) * 2;   // Gin + layer output sequence
+    else if (layerwise && sb_wide(c)) b += rows * Tp * 4.0 * c.sb_hidden * 2;     // a wide layer 0's Gin
     return b;
 }
 
@@ -1708,10 +1726,12 @@ extern "C" int fsn_model_sb_forward(fsn_model* m, const float* d_x, int32_t B, i
     sp.B = B; sp.F = c.num_freqs; sp.Tp = T + c.look_ahead; sp.Ns = c.sb_num_neighbors; sp.Nf = c.fb_num_neighbors;
     sp.nfb = c.model_kind == FSN_KIND_PLUS ? 3 : 1;
     sp.ximg = static_cast<__half*>(ln.ximg.p);
+    sp.ntiles = (B * sp.F + 127) / 128;
     sp.t0 = 0; sp.Tw = sp.Tp;
     sp.tlen = tl;
     if (!Tw) {                                                          // windowed: run_sb_lstm packs each window
-        launch_sb_pack(sp, s);
+        if (sb_wide(c)) launch_sb_pack_wide(sp, !runs_layerwise(c, m->env_impl), s);
+        else launch_sb_pack(sp, s);
         m->launches++;
     }
     if ((rc = run_sb_lstm(m, ln, B, T, Tw, sp, d_out, d_real, d_imag, d_enh, tl, s))) return rc;
@@ -1875,8 +1895,8 @@ struct StepScratch {
     int ensure(const fsn_stream& st, int K, size_t img, bool zero, cudaStream_t s);
     void release() { for (DevBuf* b : {&fbin, &fbx, &hseq, &fbout, &ximg}) b->release(); }
 };
-// the generic sub-band step's images of `rows` rows over K frames
-static size_t step_img_bytes(long long rows, int K) { return (size_t)((rows + 127) / 128) * K * 16384; }
+// the generic sub-band step's images of `rows` rows over K frames (wide: time-major rows of 128 halves)
+static size_t step_img_bytes(const fsn_config& c, long long rows, int K) { return (size_t)((rows + 127) / 128) * K * 128 * sb_row_bytes(c); }
 
 struct fsn_stream {
     fsn_model* m;
@@ -2033,7 +2053,7 @@ extern "C" int fsn_stream_create(fsn_model* m, int32_t B, fsn_stream** out) {
     lstm_mma_cstate_bytes(1, rows, 1, &st->ra_sb);
     st->use_ws = lstm_ws_supported(c.num_layers, c.fb_hidden, st->Ipad, B, m->num_sms) && !m->env_no_ws;
     // scratch, then state, then the barrier: with the state allocated first, steps at 16-64 slots measured ~0.03 ms slower per tick
-    int e = st->tick.ensure(*st, 1, step_img_bytes(rows, 1), true, nullptr);
+    int e = st->tick.ensure(*st, 1, step_img_bytes(c, rows, 1), true, nullptr);
     e |= state_alloc(st, 0, nullptr);
     if (st->use_ws) e |= st->ws_bar.ensure(64, true);
     e |= st->d_slot.ensure((size_t)4 * B * sizeof(int32_t), false);
@@ -2101,11 +2121,15 @@ static int step_frames(fsn_stream* st, StepScratch& x, const float* d_mag, int K
     if (nl < 0) return fail(FSN_ECUDA, "full-band LSTM step failed: %s", cudaGetErrorString((cudaError_t)-nl));
     StreamPackLaunch pa{d_mag, static_cast<const float*>(x.fbout.p), Pk, static_cast<double*>(st->cum_sb.p), static_cast<__half*>(x.ximg.p),
                         B, F, K, c.sb_num_neighbors, c.fb_num_neighbors, n, c.norm_type, 0, K, slot, nullptr, 0, 0, kf};
+    const bool wide = sb_wide(c);
     if (!lw) {
-        launch_stream_pack(pa, s);
+        if (wide) launch_stream_pack_wide(pa, s);
+        else launch_stream_pack(pa, s);
         LstmMmaLaunch b = m->sb_mma;
         b.rows = B * F; b.Tp = K; b.out = d_mask; b.la = 0;
-        b.img = static_cast<const __half*>(x.ximg.p); b.ntiles = (B * F + 127) / 128;
+        b.ntiles = (B * F + 127) / 128;
+        if (wide) { b.xplain = static_cast<const __half*>(x.ximg.p); b.rows_pad = b.ntiles * 128; }   // time-major rows of 128 halves
+        else b.img = static_cast<const __half*>(x.ximg.p);
         b.cstate = static_cast<float*>(st->c_sb.p); b.rows_alloc = st->ra_sb;
         b.hstate = static_cast<__half*>(st->h_sb.p); b.resume = resume; b.slot = slot; b.slot_rows = F; b.slot_la = c.look_ahead; b.kf = kf;
         if (int e = launch_lstm_mma(b, s)) return fail(FSN_ECUDA, "sub-band LSTM step failed: %s", cudaGetErrorString((cudaError_t)e));
@@ -2127,7 +2151,8 @@ static int step_frames(fsn_stream* st, StepScratch& x, const float* d_mag, int K
                 for (int w0 = 0; w0 < Kg; w0 += tw_max) {
                     const int tw = Kg - w0 < tw_max ? Kg - w0 : tw_max;
                     pa.k0 = w0; pa.Kw = tw; pa.idx = g.idx; pa.j0 = j0; pa.nsess = bs;
-                    launch_stream_pack(pa, s);
+                    if (wide) launch_stream_pack_wide(pa, s);
+                    else launch_stream_pack(pa, s);
                     LstmTc5rLaunch a{};
                     a.rows = bs * F; a.Tp = 4 + Kg; a.ntiles = nt; a.t0 = 4 + w0; a.Tw = tw;
                     a.ximg = static_cast<const __half*>(x.ximg.p); a.hseq = static_cast<__half*>(st->c_hsb.p);
@@ -2207,7 +2232,7 @@ static int chunk_plan(const fsn_config& c, bool layerwise, int n, int K, double 
     if (int rc = chunk_check(c, K)) return rc;
     *p = Plan{n};
     if (!layerwise) {
-        p->bytes = (int64_t)(((size_t)n * c.num_freqs + 127) / 128) * K * 16384;
+        p->bytes = (int64_t)step_img_bytes(c, (long long)n * c.num_freqs, K);
         return FSN_OK;
     }
     auto fits = [&](int bs, int tw) { return (double)chunk_sb_bytes(c, bs, K, tw) <= cap; };
@@ -2314,7 +2339,7 @@ static int step_slots(fsn_stream* st, const float* d_mag, int K, float* d_mask, 
         for (int b = 0; b < B; ++b) kf.push_back(h_flags[b] == FSN_SLOT_HOLD ? 0 : K);
         if (int rc = lw_groups(st, kf, &lw, &e, s)) return rc;
     }
-    if (lw.empty()) e |= x.ensure(*st, K, layerwise ? 0 : step_img_bytes((long long)B * F, K), false, s);
+    if (lw.empty()) e |= x.ensure(*st, K, layerwise ? 0 : step_img_bytes(c, (long long)B * F, K), false, s);
     if (e) return fail(FSN_ECUDA, "chunk scratch allocation failed (B = %d, K = %d)", B, K);
     if (int rc = claim_mode(st, FSN_STATE_MODE_MASK)) return rc;
     use_slot_counts(st);
@@ -2448,7 +2473,7 @@ static int step_audio(fsn_stream* st, const float* d_samples, int K, const int32
         if (int rc = lw_groups(st, kf, &lw, &e, s)) return rc;
     size_t nstage = (size_t)7 * B + nzero;
     for (const LwGroup& g : lw) nstage += B + g.nact;
-    if (Km) e |= x.ensure(*st, Km, layerwise ? 0 : step_img_bytes((long long)B * F, Km), false, s);
+    if (Km) e |= x.ensure(*st, Km, layerwise ? 0 : step_img_bytes(c, (long long)B * F, Km), false, s);
     e |= st->x_spec.ensure((size_t)B * K * F * sizeof(float2), false, s);
     e |= st->x_mag.ensure((size_t)B * F * Km * sizeof(float), false, s);
     e |= st->x_mask.ensure((size_t)B * 2 * F * Km * sizeof(float), false, s);

@@ -91,6 +91,10 @@ struct SbPackLaunch {
 };
 void launch_sb_stats(const SbPackLaunch& a, cudaStream_t s);
 void launch_sb_pack(const SbPackLaunch& a, cudaStream_t s);
+// a wide sub-band input (64 < I <= 128): the same values as plain fp16 rows of 128 halves, columns >= I zero.  time_major = false:
+// the A operand of layer 0's input-projection GEMM, row (tile * Tw + t - t0) * 128 + r (LstmTc5rLaunch::hseq's order); true: the
+// generic kernel's plain input [Tw, ntiles * 128, 128] (LstmMmaLaunch::xplain, rows_pad = ntiles * 128)
+void launch_sb_pack_wide(const SbPackLaunch& a, bool time_major, cudaStream_t s);
 // the same normalised values as launch_sb_pack, written to a.xtm / a.amax instead of the fp16 images
 void launch_sb_pack_tm(const SbPackLaunch& a, cudaStream_t s);
 // time-major [Z*Tp, ld] -> [Z, C, Tp] (test hook of the sub-band TCN input)
@@ -121,6 +125,9 @@ struct StreamPackLaunch {
     const int* kf;            // null, or [B]: frames k >= kf[b] of a stepping slot are zero images and leave its sums untouched
 };
 void launch_stream_pack(const StreamPackLaunch& a, cudaStream_t s);
+// a wide input (64 < I <= 128) as plain fp16 rows of 128 halves: with idx, row (tile * Kw + k - k0) * 128 + r of the compact rows (layer
+// 0's input-projection GEMM); without, time-major [K, ntiles * 128, 128] for the generic kernel (ntiles = ceil(B F / 128))
+void launch_stream_pack_wide(const StreamPackLaunch& a, cudaStream_t s);
 // compact masks src [nsess, 2, F, K] of the sessions j0 .. j0 + nsess - 1 -> dst [B, 2, F, K] at their slots (idx[b] - j0), leading
 // columns with slot[b] + k < la zero; zero_held: also zero the rows of held slots
 // src has Ks <= K columns; dst columns k >= Ks of the sub-batch's slots are zero
@@ -268,7 +275,9 @@ struct LstmTc5rLaunch {
     int t0, Tw;
     const __half* gin;        // [ntiles_pad * Tw * 128, 4H] fp16 input projection X_l W_ih^T (lstm_tc5r_gin_order), or null with ximg
     const __half* ximg;       // first layer: [ntiles_pad, Tw, 128 rows, 64 halves] SW128 input images; the input projection is then part
-                              // of the recurrence, with W_ih as one extra k-block in front of every chunk of the stream
+                              // of the recurrence, with W_ih as one extra k-block in front of every chunk of the stream.  A wide input
+                              // (64 < Isb <= 128) is rows of 128 halves in hseq's order instead: the host projects it with the GEMM
+                              // (fsn_api.cu, sb_layers) and the kernel gets ximg = null
     __half* hseq;             // [ntiles_pad * Tw * 128, H] fp16 output sequence (not the last layer)
     float* cstate;            // [2 ntiles_pad CTAs][H/32 chunks][4][128 threads] float4: c (GRU: h in fp32), read back at t0 > 0
     __half* hstate;           // windowed forwards: this layer's fp16 h [ntiles_pad * 128, H], loaded at entry when t0 > 0 (instead

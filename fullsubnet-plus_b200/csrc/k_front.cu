@@ -401,7 +401,9 @@ void launch_conv1x1(const ConvLaunch& a, cudaStream_t s) {
 // The [B, F, I, T'] unfolded tensor is never materialised in fp32: its utterance mean follows from
 // row sums (each reflected row counted as often as it appears in some window), and the normalised
 // values are written once, in fp16, directly in the per-step 128-row tile images the LSTM kernels
-// stream (K-major, SWIZZLE_128B, 64 halves per row; columns >= I and rows >= B*F are zero).
+// stream (K-major, SWIZZLE_128B, 64 halves per row; columns >= I and rows >= B*F are zero).  A wide input (64 < I <= 128, DESIGN.md
+// §3.3) is written as plain fp16 rows of 128 halves instead (Fp16Wide): the A operand of layer 0's input-projection GEMM, or the
+// generic kernel's time-major input.
 // =============================================================================================
 // row sums (and sums of squares) of the window source and the full-band outputs: one warp per row, the whole GPU
 __global__ void __launch_bounds__(256) sb_rowsum_kernel(SbPackLaunch a) {
@@ -462,6 +464,8 @@ void launch_sb_stats(const SbPackLaunch& a, cudaStream_t s) {
 // kChunk: the store takes the bin range a.f0 .. a.f0 + a.Fc - 1 (rows b * Fc + f - f0); without it every bin, rows b * F + f.
 struct Fp16Img {
     static constexpr bool kChunk = false;
+    static constexpr int kWidth = 64;                  // channels per row
+    static constexpr bool kTimeMajor = false;
     static __device__ __forceinline__ void store(const SbPackLaunch& a, int row, int t, int k0, const float (&v)[8]) {
         float w[8];
 #pragma unroll
@@ -474,6 +478,7 @@ struct Fp16Img {
 };
 struct Fp32Tm {
     static constexpr bool kChunk = true;
+    static constexpr int kWidth = 64;
     static __device__ __forceinline__ void store(const SbPackLaunch& a, int row, int t, int k0, const float (&v)[8]) {
         float4* dst = reinterpret_cast<float4*>(a.xtm + ((size_t)row * a.Tp + t) * 64 + k0);
         dst[0] = make_float4(v[0], v[1], v[2], v[3]);
@@ -485,6 +490,28 @@ struct Fp32Tm {
         if ((threadIdx.x & (width - 1)) == 0 && row >= 0) atomicMax(reinterpret_cast<int*>(a.amax + row), __float_as_int(m));
     }
 };
+// Fp16Wide: rows of 128 halves, unswizzled (values clamped like Fp16Img).  TM = false: the rows of layer 0's input-projection GEMM,
+// (tile * Tw + t - t0) * 128 + r in the order of the recurrence's hseq; TM = true: the generic kernel's time-major input
+// [Tw, ntiles * 128, 128], row (t - t0) * ntiles * 128 + row.
+__device__ __forceinline__ size_t wide_row(bool tm, int row, int t, int t0, int Tw, int ntiles) {
+    return tm ? (size_t)(t - t0) * ntiles * 128 + row : ((size_t)(row >> 7) * Tw + (t - t0)) * 128 + (row & 127);
+}
+__device__ __forceinline__ uint4 pack_half8(const float (&v)[8]) {
+    float w[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) w[i] = fminf(fmaxf(v[i], -65504.f), 65504.f);
+    return make_uint4(pack_half2(w[0], w[1]), pack_half2(w[2], w[3]), pack_half2(w[4], w[5]), pack_half2(w[6], w[7]));
+}
+template <bool TM>
+struct Fp16Wide {
+    static constexpr bool kChunk = false;
+    static constexpr int kWidth = 128;
+    static constexpr bool kTimeMajor = TM;
+    static __device__ __forceinline__ void store(const SbPackLaunch& a, int row, int t, int k0, const float (&v)[8]) {
+        *reinterpret_cast<uint4*>(a.ximg + wide_row(TM, row, t, a.t0, a.Tw, a.ntiles) * 128 + k0) = pack_half8(v);
+    }
+    static __device__ __forceinline__ void finish(const SbPackLaunch&, int, float, unsigned) {}
+};
 __device__ __forceinline__ float vmax8(float m, const float (&v)[8]) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) m = fmaxf(m, fabsf(v[i]));
@@ -493,7 +520,8 @@ __device__ __forceinline__ float vmax8(float m, const float (&v)[8]) {
 
 // One CTA = (sample, 32 consecutive bins of the range, 32 frames).  The window source rows [f0 - Ns, f0 + 31 + Ns] (reflected) and the
 // full-band rows of the 32 bins are staged once in shared memory; work item = (bin, frame, 8 channels), so 8 consecutive lanes
-// write one whole row of 64 channels (one 128-byte line of the SWIZZLE_128B image).
+// write one whole row of 64 channels (one 128-byte line of the SWIZZLE_128B image).  Rows of 128 channels (Fp16Wide): 16 lanes per
+// row, the CTA's bins in two passes of 16.
 constexpr int SBP_F = 32, SBP_T = 32;
 template <class Store>
 __global__ void __launch_bounds__(256) sb_pack_kernel(SbPackLaunch a) {
@@ -522,30 +550,39 @@ __global__ void __launch_bounds__(256) sb_pack_kernel(SbPackLaunch a) {
         }
     }
     __syncthreads();
-    const int c = threadIdx.x & 7, fr = threadIdx.x >> 3;          // chunk, bin inside the tile
-    const int f = f0 + fr;
-    const bool live = f < fb + Fn;
-    const int row = b * Fn + (f - fb);
-    auto val = [&](int k, int tt) -> float {
-        float v = 0.f;
-        if (k < nw) v = wsm[(fr + k) * (SBP_T + 1) + tt];
-        else if (k < I) { const int kk = k - nw, q = kk / nf, j = kk % nf; v = fsm[(q * frows + fr + j) * (SBP_T + 1) + tt]; }
-        return (k < I && t0 + tt < Tpe) ? (v - sub) * inv : 0.f;
-    };
-    float m = 0.f;
-    for (int tt = 0; live && tt < SBP_T && t0 + tt < Tp; ++tt) {
-        float v[8];
+    // work item (bin fr of the tile, chunk c of 8 channels)
+    auto pack_bin = [&](int fr, int c) {
+        const int f = f0 + fr;
+        const bool live = f < fb + Fn;
+        const int row = b * Fn + (f - fb);
+        auto val = [&](int k, int tt) -> float {
+            float v = 0.f;
+            if (k < nw) v = wsm[(fr + k) * (SBP_T + 1) + tt];
+            else if (k < I) { const int kk = k - nw, q = kk / nf, j = kk % nf; v = fsm[(q * frows + fr + j) * (SBP_T + 1) + tt]; }
+            return (k < I && t0 + tt < Tpe) ? (v - sub) * inv : 0.f;
+        };
+        float m = 0.f;
+        for (int tt = 0; live && tt < SBP_T && t0 + tt < Tp; ++tt) {
+            float v[8];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = val(c * 8 + i, tt);
-        m = vmax8(m, v);
-        Store::store(a, row, t0 + tt, c * 8, v);
+            for (int i = 0; i < 8; ++i) v[i] = val(c * 8 + i, tt);
+            m = vmax8(m, v);
+            Store::store(a, row, t0 + tt, c * 8, v);
+        }
+        Store::finish(a, live ? row : -1, m, 8);
+    };
+    if (Store::kWidth == 64) {
+        pack_bin(threadIdx.x >> 3, threadIdx.x & 7);
+    } else {                                                        // 16 chunks per row: two passes of 16 bins
+        pack_bin(threadIdx.x >> 4, threadIdx.x & 15);
+        pack_bin((threadIdx.x >> 4) + 16, threadIdx.x & 15);
     }
-    Store::finish(a, live ? row : -1, m, 8);
 }
 
 // Cumulative norms of the 4-D sub-band input (base_model.py:227-258 / :277-316 with dim 1 = F folded into the batch): every
 // sequence (b, f) is normalised by the running mean (and std) over its I channels.  One warp per sequence, lanes over
-// frames, warp scan with carry.
+// frames, warp scan with carry.  Rows of 128 channels (Fp16Wide) hold 64 values per thread as the 64-wide rows do: the first half's
+// values enter the sums, the second half's are kept, and the first half is read again for its stores.
 template <class Store>
 __global__ void __launch_bounds__(128) sb_pack_cum_kernel(SbPackLaunch a) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -561,12 +598,10 @@ __global__ void __launch_bounds__(128) sb_pack_cum_kernel(SbPackLaunch a) {
     double cs = 0.0, cq = 0.0;                                   // running sums carried across 32-frame chunks (and windows: a.cum)
     if (a.cum && a.t0 > 0) { cs = a.cum[2 * (size_t)row]; cq = a.cum[2 * (size_t)row + 1]; }
     float mx = 0.f;
+    constexpr int K0 = Store::kWidth - 64;                        // the first channel held in v
     for (int t0 = a.t0; t0 < Tp; t0 += 32) {
         const int t = t0 + lane;
-        float v[64];
-        float s = 0.f, q = 0.f;
-#pragma unroll
-        for (int k = 0; k < 64; ++k) {
+        auto load = [&](int k) -> float {                         // channel k of (sequence, frame t)
             float x = 0.f;
             if (t < Tpe && k < I) {
                 if (k < nw) x = a.win[((size_t)b * F + reflect_idx(f + k - a.Ns, F)) * a.Pw + t];
@@ -576,6 +611,17 @@ __global__ void __launch_bounds__(128) sb_pack_cum_kernel(SbPackLaunch a) {
                     x = src[((size_t)b * F + reflect_idx(f + j - a.Nf, F)) * a.P + t];
                 }
             }
+            return x;
+        };
+        float v[64];
+        float s = 0.f, q = 0.f;
+        if (K0) {
+#pragma unroll
+            for (int k = 0; k < K0; ++k) { const float x = load(k); s += x; q = fmaf(x, x, q); }
+        }
+#pragma unroll
+        for (int k = 0; k < 64; ++k) {
+            const float x = load(K0 + k);
             v[k] = x; s += x; q = fmaf(x, x, q);
         }
         double ds = s, dq = q;                                   // inclusive scan over the 32 frames of this chunk
@@ -591,13 +637,23 @@ __global__ void __launch_bounds__(128) sb_pack_cum_kernel(SbPackLaunch a) {
         else { const double cv = (dq - 2.0 * cm * ds) / cnt + cm * cm; const double inv = 1.0 / sqrt(cv + EPS); sc = (float)inv; sh = (float)(-cm * inv); }
         cs = __shfl_sync(0xffffffffu, ds, 31); cq = __shfl_sync(0xffffffffu, dq, 31);
         if (t < Tp) {
+            if (K0) {
+#pragma unroll 1
+                for (int c = 0; c < K0 / 8; ++c) {
+                    float w[8];
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) w[i] = (c * 8 + i < I && t < Tpe) ? fmaf(load(c * 8 + i), sc, sh) : 0.f;
+                    mx = vmax8(mx, w);
+                    Store::store(a, row, t, c * 8, w);
+                }
+            }
 #pragma unroll
             for (int c = 0; c < 8; ++c) {
                 float w[8];
 #pragma unroll
-                for (int i = 0; i < 8; ++i) w[i] = (c * 8 + i < I && t < Tpe) ? fmaf(v[c * 8 + i], sc, sh) : 0.f;
+                for (int i = 0; i < 8; ++i) w[i] = (K0 + c * 8 + i < I && t < Tpe) ? fmaf(v[c * 8 + i], sc, sh) : 0.f;
                 mx = vmax8(mx, w);
-                Store::store(a, row, t, c * 8, w);
+                Store::store(a, row, t, K0 + c * 8, w);
             }
         }
     }
@@ -618,25 +674,35 @@ static void sb_pack_go(const SbPackLaunch& a, cudaStream_t s) {
     }
 }
 // The raw form (SbPackLaunch::raw): one thread per (row, frame, 8 channels), 8 consecutive threads write one row of a step's image
+// (Store = Fp16Img; 16 threads per row of Fp16Wide)
+template <class Store>
 __global__ void __launch_bounds__(256) sb_pack_raw_kernel(SbPackLaunch a) {
+    constexpr int NC = Store::kWidth / 8, LNC = NC == 8 ? 3 : 4;
     const int I = 2 * a.Ns + 1 + a.nfb * (2 * a.Nf + 1), rows = a.B * a.F;
-    const long long n = (long long)((rows + 255) / 256 * 2) * a.Tw * 128 * 8;     // every row of the padded tile pairs
+    const long long n = (long long)((rows + 255) / 256 * 2) * a.Tw * 128 * NC;    // every row of the padded tile pairs
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-        const int c = (int)(i & 7), r = (int)((i >> 3) & 127);
-        const long long q = i >> 10;
+        const int c = (int)(i & (NC - 1)), r = (int)((i >> LNC) & 127);
+        const long long q = i >> (LNC + 7);
         const int row = (int)(q / a.Tw) * 128 + r, t = a.t0 + (int)(q % a.Tw);
         float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
         if (row < rows && t < (a.tlen ? a.tlen[row / a.F] : a.Tp))
 #pragma unroll
             for (int e = 0; e < 8; ++e)
                 if (c * 8 + e < I) v[e] = a.raw[((size_t)row * I + c * 8 + e) * a.Tp + t];
-        Fp16Img::store(a, row, t, c * 8, v);
+        // the time-major rows stop at ntiles * 128: the pad tile of a pair is not part of the generic kernel's input
+        if (!Store::kTimeMajor || row < a.ntiles * 128) Store::store(a, row, t, c * 8, v);
     }
 }
 
-void launch_sb_pack(const SbPackLaunch& a, cudaStream_t s) {
-    if (a.raw) { sb_pack_raw_kernel<<<1024, 256, 0, s>>>(a); return; }
-    sb_pack_go<Fp16Img>(a, s);
+template <class Store>
+static void sb_pack_any(const SbPackLaunch& a, cudaStream_t s) {
+    if (a.raw) sb_pack_raw_kernel<Store><<<1024, 256, 0, s>>>(a);
+    else sb_pack_go<Store>(a, s);
+}
+void launch_sb_pack(const SbPackLaunch& a, cudaStream_t s) { sb_pack_any<Fp16Img>(a, s); }
+void launch_sb_pack_wide(const SbPackLaunch& a, bool time_major, cudaStream_t s) {
+    if (time_major) sb_pack_any<Fp16Wide<true>>(a, s);
+    else sb_pack_any<Fp16Wide<false>>(a, s);
 }
 void launch_sb_pack_tm(const SbPackLaunch& a, cudaStream_t s) {
     cudaMemsetAsync(a.amax, 0, (size_t)a.B * a.Fc * sizeof(float), s);
@@ -801,9 +867,86 @@ __global__ void __launch_bounds__(128) stream_pack_frame_kernel(StreamPackLaunch
     }
 }
 
+// The wide form (64 < I <= 128) of both kernels above, one launch for K frames: plain rows of 128 halves, in the order of layer 0's
+// input-projection GEMM with compact rows (idx: row (tile * Kw + kk) * 128 + r), else time-major [Kw, ntiles * 128, 128] for the
+// generic kernel.  A thread holds 64 values at a time: the first half's enter the sums, the second half's are kept, and the first
+// half is read again for its stores (same sums, same order as one pass over 128).
+__global__ void __launch_bounds__(128) stream_pack_wide_kernel(StreamPackLaunch a) {
+    const int row = blockIdx.x * blockDim.x + threadIdx.x, F = a.F;
+    if (row >= a.B * F) return;
+    const int b = row / F, f = row % F;
+    const int nw = 2 * a.Ns + 1, nf = 2 * a.Nf + 1, I = nw + nf;
+    const int n0 = a.slot ? a.slot[b] : a.n;
+    int crow = row;                                                 // the row of the images
+    if (a.idx) {                                                    // compact rows: session idx[b] - j0 of this sub-batch, or not packed
+        const int j = n0 < 0 ? -1 : a.idx[b] - a.j0;
+        if (j < 0 || j >= a.nsess) return;
+        crow = j * F + f;
+    }
+    const int ntiles = (a.B * F + 127) / 128;
+    auto dst = [&](int kk) { return a.ximg + wide_row(a.idx == nullptr, crow, kk, 0, a.Kw, ntiles) * 128; };
+    auto zero_row = [&](int kk) {
+        uint4* d = reinterpret_cast<uint4*>(dst(kk));
+#pragma unroll
+        for (int c = 0; c < 16; ++c) d[c] = make_uint4(0u, 0u, 0u, 0u);
+    };
+    if (n0 < 0) {                                                   // held: frames unread, sums untouched, zero input rows
+        for (int k = 0; k < a.Kw; ++k) zero_row(k);
+        return;
+    }
+    const float* mag = a.mag + (size_t)b * F * a.K;
+    const float* fb = a.fb + (size_t)b * F * a.Pfb;
+    double cs = n0 + a.k0 == 0 ? 0.0 : a.cum[2 * row], cq = n0 + a.k0 == 0 ? 0.0 : a.cum[2 * row + 1];
+    const int kb = a.kf ? a.kf[b] : a.K;
+#pragma unroll 1
+    for (int kk = 0; kk < a.Kw; ++kk) {
+        const int k = a.k0 + kk, n = n0 + k;
+        if (k >= kb) { zero_row(kk); continue; }                    // past the slot's frames: zero input rows, sums untouched
+        int fo = f;                                                 // opaque per frame: the neighbour offsets are recomputed, not
+        asm volatile("" : "+r"(fo));                                // hoisted out of the frame loop
+        auto load = [&](int i) -> float {
+            float x = 0.f;
+            if (i < nw) x = mag[(size_t)reflect_idx(fo + i - a.Ns, F) * a.K + k];
+            else if (i < I) x = fb[(size_t)reflect_idx(fo + (i - nw) - a.Nf, F) * a.Pfb + k];
+            return x;
+        };
+        float v[64];
+        double s = 0, q = 0;
+#pragma unroll
+        for (int i = 0; i < 64; ++i) { const float x = load(i); s += x; q += (double)x * x; }
+#pragma unroll
+        for (int i = 0; i < 64; ++i) { const float x = load(64 + i); v[i] = x; s += x; q += (double)x * x; }
+        const double EPS = 1.1920928955078125e-07;
+        cs += s; cq += q;
+        const double cnt = (double)I * (n + 1), cm = cs / cnt;
+        float sc, sh;
+        if (a.type == FSN_NORM_CUMULATIVE_LAPLACE) { sc = (float)(1.0 / (cm + EPS)); sh = 0.f; }
+        else { const double cv = (cq - 2.0 * cm * cs) / cnt + cm * cm, inv = 1.0 / sqrt(cv + EPS); sc = (float)inv; sh = (float)(-cm * inv); }
+        uint4* d = reinterpret_cast<uint4*>(dst(kk));
+        auto store64 = [&](int k0) {                                // channels k0 .. k0 + 63 from v
+#pragma unroll
+            for (int c = 0; c < 8; ++c) {
+                float w[8];
+#pragma unroll
+                for (int i = 0; i < 8; ++i) w[i] = (k0 + c * 8 + i < I) ? fmaf(v[c * 8 + i], sc, sh) : 0.f;
+                d[k0 / 8 + c] = pack_half8(w);
+            }
+        };
+        store64(64);
+        asm volatile("" : "+r"(fo));
+#pragma unroll
+        for (int i = 0; i < 64; ++i) v[i] = load(i);
+        store64(0);
+    }
+    a.cum[2 * row] = cs; a.cum[2 * row + 1] = cq;
+}
+
 void launch_stream_pack(const StreamPackLaunch& a, cudaStream_t s) {
     if (a.K == 1 && !a.idx) stream_pack_frame_kernel<<<(a.B * a.F + 127) / 128, 128, 0, s>>>(a);
     else stream_pack_kernel<<<(a.B * a.F + 127) / 128, 128, 0, s>>>(a);
+}
+void launch_stream_pack_wide(const StreamPackLaunch& a, cudaStream_t s) {
+    stream_pack_wide_kernel<<<(a.B * a.F + 127) / 128, 128, 0, s>>>(a);
 }
 
 // The compact masks of one sub-batch [nsess, 2, F, K] into the slots' rows of d_mask [B, 2, F, K]: column k of slot b is the mask of

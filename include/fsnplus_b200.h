@@ -95,7 +95,9 @@ int fsn_version(void);
 const char* fsn_last_error(void);
 
 /* Replaces FullSubNet_Plus.__init__ / Model.__init__ (fullsubnet_plus.py:17-120, fullsubnet.py:13-66):
- * validates the configuration and creates an empty parameter store on the current CUDA device. */
+ * validates the configuration and creates an empty parameter store on the current CUDA device.  The sub-band input size
+ * Isb = (2 sb_num_neighbors + 1) + k (2 fb_num_neighbors + 1) (k = 3 for FSN_KIND_PLUS, 1 for FSN_KIND_FSN) must be <= 128 for an LSTM /
+ * GRU sub band and <= 64 for the sub-band TCN, else FSN_EINVAL naming the limit (DESIGN.md §3.3). */
 int fsn_model_create(const fsn_config* cfg, fsn_model** out);
 void fsn_model_destroy(fsn_model* m);
 
@@ -440,7 +442,8 @@ int32_t fsn_lstm_mma_rows(int32_t layers, int32_t hidden, int32_t input_pad, int
 
 /* Test hook: the sub-band LSTM / GRU stage of a finalized model alone, on a given sub-band input, through the forward's own layer and
  * window loop (GEMM dispatch, per-layer cell / hidden state, fused epilogues); only the packer differs.
- * d_x: [B, F, Isb, T + look_ahead] float32, device -- the normalised input sb_model receives (same layout as get_stage "sb_in");
+ * d_x: [B, F, Isb, T + look_ahead] float32, device -- the normalised input sb_model receives (same layout as get_stage "sb_in"; any
+ * Isb the model takes, up to 128);
  * rounded to fp16 (nearest) like the forward's packed input.
  * Tw: 0 = one launch per layer over all frames; else windows of Tw frames (positive multiple of 32; layer-wise path only).
  * h_frames: NULL or B host frame counts, as fsn_model_forward_ragged.  Output: d_out [B, 2, F, T] (mask), or, when d_enh != NULL,

@@ -191,6 +191,7 @@ struct fsn_model {
     // tuning knobs, read ONCE at fsn_model_create (never on the forward path): FSN_LSTM_IMPL overrides cfg.lstm_impl,
     // FSN_NO_WS=1 keeps the full-band LSTM of fullsubnet.Model off the weight-stationary kernel
     int env_impl = 0;
+    bool layerwise = false;                            // the sub-band route, fixed with config and knobs at create: runs_layerwise
     // FSN_FRONT_OVERLAP=1: the pipelined entry points run the front end of batch i+1 concurrently with the sub-band LSTM of batch i
     // (two lanes, two streams).  Off by default: no gain at the flagship size on the H100 (DESIGN.md §4), the LSTM occupies every SM.
     bool env_front_overlap = false;
@@ -616,6 +617,7 @@ extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
     m->env_sb_window = sb_window;
     m->env_sb_chunk = sb_chunk;
     { const char* e = getenv("FSN_LSTM_IMPL"); if (e && *e) m->env_impl = atoi(e); }
+    m->layerwise = runs_layerwise(c, m->env_impl);
     { const char* e = getenv("FSN_NO_WS"); m->env_no_ws = e && atoi(e) != 0; }
     { const char* e = getenv("FSN_FRONT_OVERLAP"); m->env_front_overlap = e && atoi(e) != 0; }
     // FSN_PDL: programmatic dependent launch of the ~30 kernels of the front-end chain.  0 = never, 1 = always, unset = only for small
@@ -750,7 +752,7 @@ extern "C" int fsn_model_finalize(fsn_model* m) {
 // The implementation the sub-band LSTM reports (last_impl), and the one a forced lstm_impl names in its error
 static int pick_impl(const fsn_model* m) {
     const int impl = m->env_impl ? m->env_impl : m->cfg.lstm_impl;
-    return runs_layerwise(m->cfg, m->env_impl) ? FSN_LSTM_TCGEN05 : impl == FSN_LSTM_AUTO ? FSN_LSTM_MMA : impl;
+    return m->layerwise ? FSN_LSTM_TCGEN05 : impl == FSN_LSTM_AUTO ? FSN_LSTM_MMA : impl;
 }
 
 // Encode the tensor maps of TCN w's scratch over `rows` rows
@@ -922,6 +924,122 @@ static int check_length(const fsn_config& c, int B, int T) {
     return FSN_OK;
 }
 
+// One offline call, as every offline entry point fills it, checks it once (check_batch) and runs it (run_plain, submit_impl, the test
+// hook): B clips of T frames (the audio call: T of its longest clip), their inputs and one output.  The kind of entry point (call)
+// decides the checks and the way the batch runs.
+enum Call { CALL_FORWARD, CALL_PIPELINED, CALL_AUDIO, CALL_HOOK };
+struct Batch {
+    Call call = CALL_FORWARD;
+    const float *mag = nullptr, *real = nullptr, *imag = nullptr;   // noisy spectra [B, F, T] (the audio call: its STFT planes)
+    int B = 0, T = 0;
+    const int32_t* frames = nullptr;           // frame count of every clip of a ragged batch; null: every clip spans T frames
+    float *mask = nullptr, *enh = nullptr;     // output: the mask [B, O, F, T] or the enhanced spectrum [B, F, T] complex
+    // the audio call: waveform rows [B, L] in and out and the clips' sample counts (null: every clip is L samples); once checked, the
+    // longest clip Lall and the counts as int32 (null: every clip is Lall samples)
+    const float* wave = nullptr; float* wave_out = nullptr; long long L = 0; const int64_t* lengths = nullptr;
+    int Lall = 0; const int32_t* samples = nullptr;
+    const float* raw = nullptr; int Tw = 0;    // the test hook: the sub-band input [B*F, Isb, T'] and its time window
+};
+
+// The longest TSSE kernel (1 without the TSSE attention): every clip needs frames + look_ahead >= it
+static int tsse_kmax(const fsn_config& c) {
+    int k = 1;
+    if (c.model_kind == FSN_KIND_PLUS && c.channel_attention == FSN_ATTN_TSSE)
+        for (int i = 0; i < 3; ++i) k = c.kersize[i] > k ? c.kersize[i] : k;
+    return k;
+}
+
+// The frame counts of a ragged batch: each in 1..T, and long enough for the TSSE convolutions.  Drops them (b.frames = null) when every
+// clip spans all T frames, so that case runs exactly the unmasked forward.
+static int check_frames(const fsn_config& c, Batch& b) {
+    if (!b.frames) return FSN_OK;
+    const int kmax = tsse_kmax(c);
+    bool all = true;
+    for (int i = 0; i < b.B; ++i) {
+        const int n = b.frames[i];
+        if (n < 1 || n > b.T) return fail(FSN_EINVAL, "frames[%d] = %d is outside 1..T = %d", i, n, b.T);
+        if (n + c.look_ahead < kmax)
+            return fail(FSN_EINVAL, "frames[%d] = %d: frames + look_ahead = %d is shorter than the TSSE kernel size %d", i, n, n + c.look_ahead, kmax);
+        all = all && n == b.T;
+    }
+    if (all) b.frames = nullptr;
+    return FSN_OK;
+}
+
+// The audio call's geometry: n_fft = 2 (num_freqs - 1) a power of two from 64 to 1024
+static int audio_fft_ok(const fsn_config& c) {
+    const int N = 2 * (c.num_freqs - 1);
+    if (N < 64 || N > 1024 || (N & (N - 1)))
+        return fail(FSN_EINVAL, "num_freqs %d: the audio call needs n_fft = 2 (num_freqs - 1) to be a power of two from 64 to 1024 "
+                                "(num_freqs 33, 65, 129, 257 or 513)", c.num_freqs);
+    return FSN_OK;
+}
+
+// The audio call's geometry and clips (check_batch, fsn_plan_audio): n_fft = 2 (num_freqs - 1), every clip longer than n_fft / 2
+// (torch.stft's reflect padding) and no longer than L, with enough frames for the TSSE kernels (check_frames, in samples), and the
+// forward's length limits on T = max_b L_b / hop + 1.  *Lmax: the longest clip; *all: every clip is Lmax samples long.
+static int audio_check(const fsn_config& c, int32_t B, int64_t L, const int64_t* h_lengths, int* T, int* Lmax, bool* all) {
+    if (int rc = audio_fft_ok(c)) return rc;
+    if (B < 1) return fail(FSN_EINVAL, "B = %d: the batch needs at least one clip", B);
+    if (L < 1 || L > 0x7fffffffLL) return fail(FSN_EINVAL, "L = %lld: the row length must be 1 .. 2^31 - 1 samples", (long long)L);
+    const int H = c.num_freqs - 1, kmax = tsse_kmax(c);                 // hop = n_fft / 2
+    long long mx = 0;
+    *all = true;
+    for (int b = 0; b < (h_lengths ? B : 1); ++b) {
+        const long long n = h_lengths ? h_lengths[b] : L;
+        char nm[40];
+        if (h_lengths) snprintf(nm, sizeof(nm), "clip %d: h_lengths[%d]", b, b);
+        else snprintf(nm, sizeof(nm), "L");
+        if (n <= H)
+            return fail(FSN_EINVAL, "%s = %lld: a clip needs more than n_fft / 2 = %d samples (torch.stft's reflect padding)", nm, n, H);
+        if (n > L) return fail(FSN_EINVAL, "%s = %lld exceeds the row length L = %lld", nm, n, (long long)L);
+        if (n / H + 1 + c.look_ahead < kmax)
+            return fail(FSN_EINVAL, "%s = %lld samples give %lld frames: frames + look_ahead = %lld is shorter than the TSSE kernel size %d "
+                                    "(a clip needs at least %lld samples)", nm, n, n / H + 1, n / H + 1 + c.look_ahead, kmax,
+                        (long long)(kmax - c.look_ahead - 1) * H);
+        if (b && n != mx) *all = false;
+        if (n > mx) mx = n;
+    }
+    *Lmax = (int)mx;
+    *T = (int)(mx / H + 1);
+    return check_length(c, 1, *T);
+}
+
+// Every check of an offline call, before it allocates, copies, records or waits on anything.  The audio call also sets b.T and
+// b.Lall and, for a ragged batch, b.samples and b.frames (unless every clip has T frames) into lens.  A plain forward is checked for
+// the length limits of one clip: plan_forward keeps every sub-batch within them.
+static int check_batch(const fsn_model* m, Batch& b, std::vector<int32_t>* lens = nullptr) {
+    if (b.call == CALL_AUDIO) {
+        if (!m) return fail(FSN_EINVAL, "m is null");
+        if (!b.wave) return fail(FSN_EINVAL, "d_wave is null ([B, L] float32 samples on the device)");
+        if (!b.wave_out) return fail(FSN_EINVAL, "d_out is null ([B, L] float32 on the device)");
+        if (!m->finalized) return fail(FSN_ESTATE, "fsn_model_finalize has not been called");
+        bool all = true;
+        if (int rc = audio_check(m->cfg, b.B, b.L, b.lengths, &b.T, &b.Lall, &all)) return rc;
+        if (m->cfg.output_size != 2) return fail(FSN_EINVAL, "the audio call needs output_size 2 (a complex mask)");
+        if (!all) {                                                     // ragged: every clip's sample count, then its frame count
+            lens->resize(2 * (size_t)b.B);
+            for (int i = 0; i < b.B; ++i) (*lens)[b.B + i] = ((*lens)[i] = (int32_t)b.lengths[i]) / (m->cfg.num_freqs - 1) + 1;
+            b.samples = lens->data(); b.frames = lens->data() + b.B;
+        }
+        return check_frames(m->cfg, b);                                 // drops the frame counts when every clip has T frames
+    }
+    const bool hook = b.call == CALL_HOOK;
+    if (!m || !(hook ? b.raw : b.mag) || (!b.mask && !b.enh)) return fail(FSN_EINVAL, "null argument");
+    if (!m->finalized) return fail(FSN_ESTATE, "fsn_model_finalize has not been called");
+    const fsn_config& c = m->cfg;
+    if (hook && c.sb_tcn) return fail(FSN_EINVAL, "fsn_model_sb_forward runs the sub-band LSTM / GRU; this model's sub-band model is the TCN");
+    if (b.enh && (!b.real || !b.imag)) return fail(FSN_EINVAL, "the enhanced-spectrum output needs the noisy real and imaginary planes");
+    if (b.enh && c.output_size != 2) return fail(FSN_EINVAL, "the enhanced-spectrum output needs output_size 2 (a complex mask)");
+    if (b.B < 1 || b.T < 1) return fail(FSN_EINVAL, "bad batch/frames");
+    if (!hook && c.model_kind == FSN_KIND_PLUS && (!b.real || !b.imag)) return fail(FSN_EINVAL, "FullSubNet_Plus.forward needs mag, real and imag");
+    if (hook && (b.Tw < 0 || b.Tw % 32)) return fail(FSN_EINVAL, "Tw = %d: the window must be 0 or a positive multiple of 32 frames", b.Tw);
+    if (hook && b.Tw && !m->layerwise) return fail(FSN_EINVAL, "time windows of the sub-band stage need the layer-wise LSTM path");
+    if (int rc = check_frames(c, b)) return rc;
+    if (!hook && b.T + c.look_ahead < tsse_kmax(c)) return fail(FSN_EINVAL, "sequence shorter than the TSSE kernel size");
+    return check_length(c, b.call == CALL_FORWARD ? 1 : b.B, b.T);
+}
+
 // Size lane ln and the model's buffers for a forward of B clips of T frames with window Tw and bin chunk Fc (ws_sizes; audio: the audio
 // call's), each fresh allocation zero-filled on its own stream (s: front end, sl: sub-band stage), and encode their tensor maps.
 static int ensure_ws(fsn_model* m, Lane& ln, int B, int T, int Tw, int Fc, cudaStream_t s, cudaStream_t sl, bool audio = false) {
@@ -931,7 +1049,7 @@ static int ensure_ws(fsn_model* m, Lane& ln, int B, int T, int Tw, int Fc, cudaS
     if (c.sb_tcn && srows > SB_MAX_ROWS)
         return fail(FSN_EINVAL, "B * %s * (T + look_ahead) = %lld rows exceeds the sub-band TCN's 2^31 limit", Fc ? "bins per chunk" : "num_freqs", srows);
     if (c.model_kind == FSN_KIND_PLUS && !m->tcn5) return fail(FSN_ESTATE, "the TCN weights were not packed");
-    const WsSizes z = ws_sizes(c, runs_layerwise(c, m->env_impl), B, T, Tw, Fc, audio);
+    const WsSizes z = ws_sizes(c, m->layerwise, B, T, Tw, Fc, audio);
     const WsGeo geo{B, T, Tw, Fc};
     m->au_valid = false;
     const bool regeo = ln.geo != geo;
@@ -996,18 +1114,25 @@ static int sb_layers(fsn_model* m, const LstmTc5rLaunch& a, __half* gin, size_t 
     return launches;
 }
 
-// d_enh != null: write the enhanced spectrum (decompress_cIRM x noisy) instead of the mask -- fused into the epilogue of the
+// The sub-band LSTM / GRU's input images of the frames sp names (a wide input: plain rows of 128 halves, time-major for the generic
+// kernel): the whole clip's, a window's, or the test hook's raw input
+static void pack_images(fsn_model* m, const SbPackLaunch& sp, cudaStream_t s) {
+    if (sb_wide(m->cfg)) launch_sb_pack_wide(sp, !m->layerwise, s);
+    else launch_sb_pack(sp, s);
+    m->launches++;
+}
+
+// b.enh != null: write the enhanced spectrum (decompress_cIRM x noisy) instead of the mask -- fused into the epilogue of the
 // layer-wise kernel's last layer, a separate pass over a scratch mask for the generic kernel
 // Tw > 0: the sub-band stage runs in time windows of Tw frames (the last one shorter); for each window the images are packed (`sp`, the
 // front end's packer arguments) and every layer resumes from the h / c its previous window left (DESIGN.md §3.7).  Tw = 0: the images of
 // the whole clip are already packed and every layer runs once over all frames.
-static int run_sb_lstm(fsn_model* m, Lane& ln, int B, int T, int Tw, SbPackLaunch sp, float* d_out, const float* d_real,
-                       const float* d_imag, float* d_enh, const int* tlen, cudaStream_t s) {
+static int run_sb_lstm(fsn_model* m, Lane& ln, const Batch& b, int Tw, SbPackLaunch sp, const int* tlen, cudaStream_t s) {
     const fsn_config& c = m->cfg;
-    const int F = c.num_freqs, Tp = T + c.look_ahead, rows = B * F, ntiles = (rows + 127) / 128;
+    const int B = b.B, T = b.T, F = c.num_freqs, Tp = T + c.look_ahead, rows = B * F, ntiles = (rows + 127) / 128;
     const int impl = pick_impl(m);
     m->last_impl = impl;
-    if (runs_layerwise(c, m->env_impl)) {
+    if (m->layerwise) {
         // one recurrent launch per layer; the first one also projects its input (the packed images), each deeper one is preceded by
         // one GEMM: the input projection of every row and time step of the window (sb_layers)
         const size_t cs_layer = lstm_tc5r_cstate_bytes(ntiles, c.sb_hidden) / sizeof(float);
@@ -1016,9 +1141,7 @@ static int run_sb_lstm(fsn_model* m, Lane& ln, int B, int T, int Tw, SbPackLaunc
             const int tw = Tw ? (Tp - w0 < Tw ? Tp - w0 : Tw) : Tp;
             if (Tw) {
                 sp.t0 = w0; sp.Tw = tw;
-                if (sb_wide(c)) launch_sb_pack_wide(sp, false, s);
-                else launch_sb_pack(sp, s);
-                m->launches++;
+                pack_images(m, sp, s);
             }
             LstmTc5rLaunch a{};
             a.rows = rows; a.Tp = Tp; a.ntiles = ntiles; a.t0 = w0; a.Tw = tw;
@@ -1026,8 +1149,8 @@ static int run_sb_lstm(fsn_model* m, Lane& ln, int B, int T, int Tw, SbPackLaunc
             a.hseq = static_cast<__half*>(m->r_hseq.p);
             a.cstate = static_cast<float*>(m->cstate.p);
             if (Tw) a.hstate = static_cast<__half*>(m->r_hstate.p);
-            a.out = d_out; a.la = c.look_ahead;
-            a.nreal = d_real; a.nimag = d_imag; a.enh = reinterpret_cast<float2*>(d_enh); a.tlen = tlen;
+            a.out = b.mask; a.la = c.look_ahead;
+            a.nreal = b.real; a.nimag = b.imag; a.enh = reinterpret_cast<float2*>(b.enh); a.tlen = tlen;
             const int nl = sb_layers(m, a, static_cast<__half*>(m->r_gin.p), Tw ? cs_layer : 0, hs_layer, s);
             if (nl < 0) return nl;
             m->launches += nl;
@@ -1044,14 +1167,14 @@ static int run_sb_lstm(fsn_model* m, Lane& ln, int B, int T, int Tw, SbPackLaunc
         a.ntiles = ntiles;
         a.cstate = static_cast<float*>(m->cstate.p);
         lstm_mma_cstate_bytes(c.num_layers, rows, c.sb_hidden, &a.rows_alloc);
-        a.out = d_out; a.la = c.look_ahead; a.tlen = tlen;
-        if (d_enh) {                                                    // generic kernel: mask into a scratch buffer, then one fused post-processing pass
+        a.out = b.mask; a.la = c.look_ahead; a.tlen = tlen;
+        if (b.enh) {                                                    // generic kernel: mask into a scratch buffer, then one fused post-processing pass
             if (m->mask_tmp.ensure((size_t)B * 2 * F * T * 4, false, s)) return fail(FSN_ECUDA, "allocation failed");
             a.out = static_cast<float*>(m->mask_tmp.p);
         }
         int e = launch_lstm_mma(a, s);
         if (e) return fail(FSN_ECUDA, "mma LSTM launch failed: %s", cudaGetErrorString((cudaError_t)e));
-        if (d_enh) { launch_apply_cirm_planar(a.out, d_real, d_imag, reinterpret_cast<float2*>(d_enh), B, F, T, tlen, c.look_ahead, s); m->launches++; }
+        if (b.enh) { launch_apply_cirm_planar(a.out, b.real, b.imag, reinterpret_cast<float2*>(b.enh), B, F, T, tlen, c.look_ahead, s); m->launches++; }
     }
     m->launches++;
     return FSN_OK;
@@ -1125,16 +1248,15 @@ static int run_tcn_blocks(fsn_model* m, const TcnWeights& w, TcnScratch& sc, con
 // Fc > 0: the sequences run in chunks of Fc bins (the last one narrower), each packed here from the front end's whole-clip outputs (`sp`,
 // the front end's packer arguments) into the same buffers; every sequence is its own gLN group, so nothing carries from one chunk to the
 // next (DESIGN.md §3.8).  Fc = 0: the input of all bins is already packed and the blocks run once.
-static int run_sb_tcn(fsn_model* m, Lane& ln, int B, int T, int Fc, SbPackLaunch sp, float* d_out, const float* d_real,
-                      const float* d_imag, float* d_enh, const int* tlen, cudaStream_t s) {
+static int run_sb_tcn(fsn_model* m, Lane& ln, const Batch& b, int Fc, SbPackLaunch sp, const int* tlen, cudaStream_t s) {
     const fsn_config& c = m->cfg;
-    const int F = c.num_freqs, Tp = T + c.look_ahead, W = Fc ? Fc : F;
+    const int B = b.B, F = c.num_freqs, Tp = b.T + c.look_ahead, W = Fc ? Fc : F;
     m->last_impl = FSN_LSTM_TCN;
     GemmTc5Launch head{};
     head.epi = EPI5_GLN_HEAD;
     head.fc_w = static_cast<const float*>(m->sb_fc.p); head.fc_b = m->sb_fc_b;
     head.O = c.output_size; head.la = c.look_ahead; head.F = F; head.act = c.sb_act;
-    head.out = d_out; head.nreal = d_real; head.nimag = d_imag; head.enh = reinterpret_cast<float2*>(d_enh);
+    head.out = b.mask; head.nreal = b.real; head.nimag = b.imag; head.enh = reinterpret_cast<float2*>(b.enh);
     float* x = static_cast<float*>(ln.sbx.p);
     float* amax0 = x + (size_t)B * W * Tp * 64;
     for (int f0 = 0; f0 < F; f0 += W) {
@@ -1181,9 +1303,6 @@ static int run_fb(fsn_model* m, const float* fbin, __half* fbx, float* hseq, flo
     return 3;
 }
 
-// The whole forward.  Front end (norm, attention, full-band model, sub-band statistics + packing) on stream `s` into lane `ln`;
-// the sub-band LSTM on stream `sl` (== s for the plain entry point; the pipelined entry points pass the LSTM stream, ordered
-// after the front end by the lane's ev_front).
 // Copy the per-sample extents frames[b] + look_ahead of a ragged forward into the lane's device buffer ln.tlen ([3][B]: one row per
 // full-band branch, so a full-band gLN group z = branch * B + b indexes it directly) through the model's pinned staging.  h_samples:
 // the audio call's sample counts, appended as a fourth row in the same copy, or null.  h_frames may be null when h_samples is not
@@ -1199,80 +1318,63 @@ static int stage_lengths(fsn_model* m, Lane& ln, const int32_t* h_frames, int B,
     return m->len_stage.send(ln.tlen.p, n, s);
 }
 
-// The waveform ends of one sub-batch of the audio call (fsn_model_enhance_audio): rows [B, L] in and out, and the clips' sample counts
-// (host; null when every clip is Lall samples; validated by the caller).  The forward then reads its spectra from, and writes the
-// enhanced spectrum to, the audio workspace.
-struct AudioIO { const float* wave; float* out; long long L; int Lall; const int32_t* h_samples; };
-
-// h_frames: the frame count of every sample of a ragged batch (validated by the caller), or null when every sample spans T frames
-// Tw: time window of the sub-band stage (0: the whole clip; > 0 needs s == sl, the plain entry points)
-// Fc: bin chunk of the sub-band TCN (0: all bins at once; > 0 needs s == sl, the plain entry points)
-// au: the audio call (s == sl): d_mag, d_real, d_imag, d_out and d_enh are ignored; one analysis launch runs before the forward and
-// one synthesis launch after it
-static int forward_impl(fsn_model* m, Lane& ln, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
-                        const int32_t* h_frames, float* d_out, float* d_enh, cudaStream_t s, cudaStream_t sl, int Tw = 0, int Fc = 0,
-                        const AudioIO* au = nullptr) {
-    if (!m || (!au && (!d_mag || (!d_out && !d_enh)))) return fail(FSN_EINVAL, "null argument");
-    if (!au && d_enh && (!d_real || !d_imag)) return fail(FSN_EINVAL, "the enhanced-spectrum output needs the noisy real and imaginary planes");
-    if ((d_enh || au) && m->cfg.output_size != 2) return fail(FSN_EINVAL, "the enhanced-spectrum output needs output_size 2 (a complex mask)");
-    if (!m->finalized) return fail(FSN_ESTATE, "fsn_model_finalize has not been called");
-    const fsn_config& c = m->cfg;
-    if (B < 1 || T < 1) return fail(FSN_EINVAL, "bad batch/frames");
-    if (c.model_kind == FSN_KIND_PLUS && !au && (!d_real || !d_imag)) return fail(FSN_EINVAL, "FullSubNet_Plus.forward needs mag, real and imag");
-    const int F = c.num_freqs, Tp = T + c.look_ahead, Pp = (Tp + 3) & ~3;
-    // chained (programmatic dependent) launches of this thread's front-end kernels: see env_pdl; "small" = at most 16 row-tile pairs,
-    // where the forward is launch-latency-bound
-    fsn_chain_launch_set(m->env_pdl == 1 || (m->env_pdl < 0 && ((long long)B * F + 255) / 256 <= 16));
-    if (c.model_kind == FSN_KIND_PLUS && c.channel_attention == FSN_ATTN_TSSE)
-        for (int i = 0; i < 3; ++i)
-            if (Tp < c.kersize[i]) return fail(FSN_EINVAL, "sequence shorter than the TSSE kernel size");
-    int rc = check_length(c, B, T);
-    if (rc) return rc;
-    rc = ensure_ws(m, ln, B, T, Tw, Fc, s, sl, au != nullptr);
-    if (rc) return rc;
-    const int* tl = nullptr;                                            // per-sample extents on the device (null: all Tp)
-    const int32_t* h_samples = au ? au->h_samples : nullptr;
-    if (h_frames || h_samples) {
-        rc = stage_lengths(m, ln, h_frames, B, s, h_samples);
-        if (rc) return rc;
-        if (h_frames) tl = static_cast<const int*>(ln.tlen.p);
+// Set lane ln up for checked batch b (every forward and the test hook): this thread's chained (programmatic dependent) launches, see
+// env_pdl -- "small" = at most 16 row-tile pairs, where the forward is launch-latency-bound; the workspace for window Tw and bin
+// chunk Fc (ensure_ws); the clips' lengths on the device, *tl (null on entry): their frame extents, unless every clip spans T'.  Resets the launch count.
+static int prepare(fsn_model* m, Lane& ln, const Batch& b, int Tw, int Fc, cudaStream_t s, cudaStream_t sl, const int** tl) {
+    fsn_chain_launch_set(m->env_pdl == 1 || (m->env_pdl < 0 && ((long long)b.B * m->cfg.num_freqs + 255) / 256 <= 16));
+    if (int rc = ensure_ws(m, ln, b.B, b.T, Tw, Fc, s, sl, b.wave != nullptr)) return rc;
+    if (b.frames || b.samples) {
+        if (int rc = stage_lengths(m, ln, b.frames, b.B, s, b.samples)) return rc;
+        if (b.frames) *tl = static_cast<const int*>(ln.tlen.p);
     }
     m->launches = 0;
     m->last_lane = (int)(&ln - m->lane);
-    const int evi = (int)(m->nfwd % fsn_model::NEV);
-    cudaEventRecord(m->evf0[evi], s);
-    AudioLaunch al{};
-    if (au) {                                                           // the STFT of every clip into the planes the forward reads
-        const int N = 2 * (F - 1);
-        const AudioTables tab = audio_table_ptrs(static_cast<const float*>(m->au_tab.p), N);
-        al.wave = au->wave; al.out = au->out; al.L = au->L;
-        al.len = h_samples ? static_cast<const int*>(ln.tlen.p) + 3 * B : nullptr; al.Lall = au->Lall;
-        al.B = B; al.T = T; al.n_fft = N;
-        al.planes = static_cast<float*>(m->au_planes.p); al.enh = static_cast<const float2*>(m->au_enh.p);
-        al.window = tab.window; al.twiddle = tab.twiddle; al.inv_env = tab.inv_env; al.inv_last = tab.inv_last;
-        launch_audio_stft(al, s); m->launches++;
-        const size_t plane = (size_t)B * F * T;
-        d_mag = al.planes; d_real = al.planes + plane; d_imag = al.planes + 2 * plane;
-        d_out = nullptr; d_enh = static_cast<float*>(m->au_enh.p);
-    }
+    return FSN_OK;
+}
 
+// Audio analysis: the STFT of every clip of b into the audio workspace, whose planes then are b's inputs and whose enhanced spectrum
+// its output.  al: the launch, kept for the synthesis after the sub-band stage.
+static void audio_analysis(fsn_model* m, Lane& ln, Batch& b, AudioLaunch& al, cudaStream_t s) {
+    const int F = m->cfg.num_freqs, N = 2 * (F - 1);
+    const AudioTables tab = audio_table_ptrs(static_cast<const float*>(m->au_tab.p), N);
+    al.wave = b.wave; al.out = b.wave_out; al.L = b.L;
+    al.len = b.samples ? static_cast<const int*>(ln.tlen.p) + 3 * b.B : nullptr; al.Lall = b.Lall;
+    al.B = b.B; al.T = b.T; al.n_fft = N;
+    al.planes = static_cast<float*>(m->au_planes.p); al.enh = static_cast<const float2*>(m->au_enh.p);
+    al.window = tab.window; al.twiddle = tab.twiddle; al.inv_env = tab.inv_env; al.inv_last = tab.inv_last;
+    launch_audio_stft(al, s); m->launches++;
+    const size_t plane = (size_t)b.B * F * b.T;
+    b.mag = al.planes; b.real = al.planes + plane; b.imag = al.planes + 2 * plane;
+    b.mask = nullptr; b.enh = static_cast<float*>(m->au_enh.p);
+}
+
+// The sub-band packer's arguments for a batch of B clips of T frames in lane ln, window Tw, extents tl; the front end adds its sources,
+// the test hook its raw input (SbPackLaunch::raw)
+static SbPackLaunch pack_args(const fsn_model* m, Lane& ln, int B, int T, int Tw, const int* tl) {
+    const fsn_config& c = m->cfg;
     SbPackLaunch sp{};
-    sp.B = B; sp.F = F; sp.Tp = Tp; sp.Ns = c.sb_num_neighbors; sp.Nf = c.fb_num_neighbors; sp.P = Pp;
-    sp.mu = static_cast<float*>(ln.mu.p);
-    sp.sigma = static_cast<float*>(ln.sigma.p);
-    sp.rowsum = static_cast<float*>(ln.sb_rowsum.p);
+    sp.B = B; sp.F = c.num_freqs; sp.Tp = T + c.look_ahead; sp.Ns = c.sb_num_neighbors; sp.Nf = c.fb_num_neighbors; sp.P = (sp.Tp + 3) & ~3;
+    sp.nfb = c.model_kind == FSN_KIND_PLUS ? 3 : 1;
+    sp.mu = static_cast<float*>(ln.mu.p); sp.sigma = static_cast<float*>(ln.sigma.p); sp.rowsum = static_cast<float*>(ln.sb_rowsum.p);
     sp.norm_type = c.norm_type;
     sp.ximg = static_cast<__half*>(ln.ximg.p);
-    sp.ntiles = (B * F + 127) / 128;
-    sp.t0 = 0; sp.Tw = Tp;
+    sp.ntiles = (B * sp.F + 127) / 128;
+    sp.t0 = 0; sp.Tw = sp.Tp;
     sp.cum = Tw ? static_cast<double*>(m->sb_cum.p) : nullptr;
     sp.tlen = tl;
-    sp.f0 = 0; sp.Fc = F;
+    sp.f0 = 0; sp.Fc = sp.F;
+    return sp;
+}
 
-    // the input norm of every branch (3 in FullSubNet+, 1 in fullsubnet.Model), and FullSubNet+'s channel attention
+// The front end on stream s into lane ln: the input norm of every branch (3 in FullSubNet+, 1 in fullsubnet.Model), FullSubNet+'s
+// channel attention, the full-band model and the sub-band statistics; adds the full-band outputs to the packer's arguments sp
+static int front_end(fsn_model* m, Lane& ln, const Batch& bt, const int* tl, SbPackLaunch& sp, cudaStream_t s) {
+    const fsn_config& c = m->cfg;
+    const int B = bt.B, T = bt.T, F = c.num_freqs, Tp = T + c.look_ahead, Pp = sp.P;
     const bool plus = c.model_kind == FSN_KIND_PLUS;
     const int nbr = plus ? 3 : 1;
-    TsseLaunch ta{{d_mag, plus ? d_real : nullptr, plus ? d_imag : nullptr}};
+    TsseLaunch ta{{bt.mag, plus ? bt.real : nullptr, plus ? bt.imag : nullptr}};
     ta.nbranch = nbr; ta.B = B; ta.F = F; ta.T = T; ta.Tp = Tp; ta.P = Pp;
     ta.out = static_cast<float*>(ln.fbin.p);
     ta.scale = static_cast<float*>(ln.tsse_scale.p);
@@ -1299,7 +1401,7 @@ static int forward_impl(fsn_model* m, Lane& ln, const float* d_mag, const float*
         const TcnWeights& w = m->tcn_fb;
         GemmTc5Launch last{};                                           // the last block also writes relu(x) for the output Linear
         last.epi = EPI5_GLN_RES; last.Xrelu = static_cast<float*>(ln.xr.p);
-        rc = run_tcn_blocks(m, w, ln.tcn, static_cast<const float*>(ln.x0.p), ln.mapX0, ta.amax, B, Tp, c.tcn_causal, last, tl, 1, s);
+        int rc = run_tcn_blocks(m, w, ln.tcn, static_cast<const float*>(ln.x0.p), ln.mapX0, ta.amax, B, Tp, c.tcn_causal, last, tl, 1, s);
         if (rc) return rc;
         GemmTc5Launch g3{};
         set_tcn_rows(g3, w, B, Tp);
@@ -1311,10 +1413,9 @@ static int forward_impl(fsn_model* m, Lane& ln, const float* d_mag, const float*
         m->launches++;
 
         sp.win = static_cast<const float*>(ln.fbin.p); sp.Pw = Pp;      // post-attention mag branch (fullsubnet_plus.py:182)
-        sp.nfb = 3;
         for (int b = 0; b < 3; ++b) sp.fb[b] = static_cast<const float*>(ln.fbout.p) + (size_t)b * B * F * Pp;
     } else {
-        launch_pad_copy(d_mag, static_cast<float*>(ln.magpad.p), B, F, T, Pp, tl, c.look_ahead, s); m->launches++;
+        launch_pad_copy(bt.mag, static_cast<float*>(ln.magpad.p), B, F, T, Pp, tl, c.look_ahead, s); m->launches++;
         // the full-band LSTM is causal, and its input (fb_in) is already zero past each clip's end: its outputs there are masked by the
         // sub-band stages
         m->last_fb_ws = lstm_ws_supported(c.num_layers, c.fb_hidden, m->fb_ws.Ipad, B, m->num_sms) && !m->env_no_ws;
@@ -1332,33 +1433,58 @@ static int forward_impl(fsn_model* m, Lane& ln, const float* d_mag, const float*
         m->launches += nl;
 
         sp.win = static_cast<const float*>(ln.magpad.p); sp.Pw = Pp;    // raw padded magnitude (fullsubnet.py:94)
-        sp.nfb = 1;
         sp.fb[0] = static_cast<const float*>(ln.fbout.p);
     }
     launch_sb_stats(sp, s); m->launches += 2;
-    if (c.sb_tcn) {
-        if (!Fc) {                                                      // chunked: run_sb_tcn packs each chunk
-            sp.xtm = static_cast<float*>(ln.sbx.p);
-            sp.amax = sp.xtm + (size_t)B * F * Tp * 64;
-            launch_sb_pack_tm(sp, s);
-            m->launches++;
-        }
-    } else if (!Tw) {                                                   // windowed: run_sb_lstm packs each window
-        if (sb_wide(c)) launch_sb_pack_wide(sp, !runs_layerwise(c, m->env_impl), s);
-        else launch_sb_pack(sp, s);
+    return FSN_OK;
+}
+
+// The whole clip's sub-band input on stream s, unless the sub-band stage packs it itself: window by window (Tw, run_sb_lstm) or chunk
+// by chunk (Fc, run_sb_tcn)
+static void pack_clip(fsn_model* m, Lane& ln, SbPackLaunch sp, int Tw, int Fc, cudaStream_t s) {
+    if (m->cfg.sb_tcn) {
+        if (Fc) return;
+        sp.xtm = static_cast<float*>(ln.sbx.p);
+        sp.amax = sp.xtm + (size_t)sp.B * sp.F * sp.Tp * 64;
+        launch_sb_pack_tm(sp, s);
         m->launches++;
+    } else if (!Tw) {
+        pack_images(m, sp, s);
     }
+}
+
+// The sub-band stage on stream sl: the LSTM / GRU or the TCN over the packed input (sp: the packer's arguments, for windows and chunks)
+static int sub_band(fsn_model* m, Lane& ln, const Batch& b, int Tw, int Fc, const SbPackLaunch& sp, const int* tl, cudaStream_t sl) {
+    return m->cfg.sb_tcn ? run_sb_tcn(m, ln, b, Fc, sp, tl, sl) : run_sb_lstm(m, ln, b, Tw, sp, tl, sl);
+}
+
+// The forward of checked batch b in lane ln, its stages in order: audio analysis (the audio call), the front end and the whole clip's
+// sub-band packing on stream `s`, the sub-band stage and audio synthesis on stream `sl` (== s for the plain driver; the pipeline passes
+// the LSTM stream, ordered after the front end by the lane's ev_front).
+// Tw: time window of the sub-band stage (0: the whole clip; > 0 needs s == sl, the plain driver)
+// Fc: bin chunk of the sub-band TCN (0: all bins at once; > 0 needs s == sl, the plain driver)
+static int forward_impl(fsn_model* m, Lane& ln, const Batch& in, cudaStream_t s, cudaStream_t sl, int Tw = 0, int Fc = 0) {
+    const int* tl = nullptr;                                            // per-sample extents on the device (null: all Tp)
+    int rc = prepare(m, ln, in, Tw, Fc, s, sl, &tl);
+    if (rc) return rc;
+    const int evi = (int)(m->nfwd % fsn_model::NEV);
+    cudaEventRecord(m->evf0[evi], s);
+    Batch b = in;
+    AudioLaunch al{};
+    if (in.wave) audio_analysis(m, ln, b, al, s);
+    SbPackLaunch sp = pack_args(m, ln, b.B, b.T, Tw, tl);
+    if ((rc = front_end(m, ln, b, tl, sp, s))) return rc;
+    pack_clip(m, ln, sp, Tw, Fc, s);
     cudaEventRecord(m->evf1[evi], s);
     if (sl != s) {                                                      // pipelined: the LSTM stream picks the lane up when the front end is done
         CK(cudaEventRecord(ln.ev_front, s));
         CK(cudaStreamWaitEvent(sl, ln.ev_front, 0));
     }
     cudaEventRecord(m->ev0[evi], sl);
-    rc = c.sb_tcn ? run_sb_tcn(m, ln, B, T, Fc, sp, d_out, d_real, d_imag, d_enh, tl, sl)
-                  : run_sb_lstm(m, ln, B, T, Tw, sp, d_out, d_real, d_imag, d_enh, tl, sl);
+    rc = sub_band(m, ln, b, Tw, Fc, sp, tl, sl);
     cudaEventRecord(m->ev1[evi], sl);
     if (rc) return rc;
-    if (au) { launch_audio_istft(al, sl); m->launches++; }             // the iSTFT of every clip over its own frames
+    if (in.wave) { launch_audio_istft(al, sl); m->launches++; }        // the iSTFT of every clip over its own frames
     m->nfwd++;
     CK(cudaGetLastError());
     return FSN_OK;
@@ -1381,11 +1507,8 @@ static int ensure_pipeline(fsn_model* m) {
     return FSN_OK;
 }
 
-// one pipelined batch: inputs are ready once `ready` (an event, may be null) has fired; returns the lane used
-static int submit_impl(fsn_model* m, cudaEvent_t ready, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
-                       float* d_out, float* d_enh, int* lane_out) {
-    int rc = ensure_pipeline(m);
-    if (rc) return rc;
+// one checked pipelined batch (after ensure_pipeline): inputs are ready once `ready` (an event, may be null) has fired; returns the lane used
+static int submit_impl(fsn_model* m, cudaEvent_t ready, const Batch& b, int* lane_out) {
     // overlap needs the opt-in (see env_front_overlap) and FullSubNet+ (fullsubnet.Model's full-band LSTM is a cooperative launch and
     // shares the LSTM scratch): otherwise one lane, one stream -- the pipeline still overlaps copies and the caller's post-processing
     const bool overlap = m->env_front_overlap && (m->cfg.model_kind == FSN_KIND_PLUS);
@@ -1395,8 +1518,7 @@ static int submit_impl(fsn_model* m, cudaEvent_t ready, const float* d_mag, cons
     if (ready) CK(cudaStreamWaitEvent(sf, ready, 0));
     if (m->plain_pending) { CK(cudaStreamWaitEvent(sf, m->ev_plain, 0)); CK(cudaStreamWaitEvent(m->s_lstm, m->ev_plain, 0)); }
     if (ln.used) CK(cudaStreamWaitEvent(sf, ln.ev_lstm, 0));              // the LSTM that read this lane has finished
-    rc = forward_impl(m, ln, d_mag, d_real, d_imag, B, T, nullptr, d_out, d_enh, sf, m->s_lstm);
-    if (rc) return rc;
+    if (int rc = forward_impl(m, ln, b, sf, m->s_lstm)) return rc;
     CK(cudaEventRecord(ln.ev_lstm, m->s_lstm));
     ln.used = true;
     m->nsub++;
@@ -1504,250 +1626,118 @@ static Plan plan_forward(const fsn_config& c, bool layerwise, int B, int T, doub
     return p;
 }
 
-static int forward_plain(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
-                         const int32_t* h_frames, float* d_out, float* d_enh, void* stream) {
-    if (!m) return fail(FSN_EINVAL, "null argument");
-    if (!m->finalized) return fail(FSN_ESTATE, "fsn_model_finalize has not been called");
-    if (B < 1 || T < 1) return fail(FSN_EINVAL, "bad batch/frames");
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    for (auto& ln : m->lane)                                             // batches still in flight in the pipeline share the scratch buffers
+// Make stream s wait for the pipelined batches still in flight: they share the scratch buffers
+static int wait_lanes(fsn_model* m, cudaStream_t s) {
+    for (auto& ln : m->lane)
         if (ln.used) CK(cudaStreamWaitEvent(s, ln.ev_lstm, 0));
-    // Samples are independent, so a batch whose workspace would exceed the cap (FSN_WS_CAP_GB, default 24 of the 80 GB) is run as
-    // equal sub-batches one after the other on the same stream -- same results, bounded memory (e.g. 256 clips on the layer-wise path);
-    // a clip too long for the cap runs its sub-band stage in time windows (plan_forward) -- same bits, O(window) sub-band memory --
-    // or, with the sub-band TCN, in bin chunks -- O(chunk) sub-band memory.
-    if (int rc = check_length(m->cfg, 1, T)) return rc;
-    m->plan = plan_forward(m->cfg, runs_layerwise(m->cfg, m->env_impl), B, T, m->ws_cap_bytes, m->env_sb_window, m->env_sb_chunk);
-    const int Bs = m->plan.Bs, Tw = m->plan.Tw, Fc = m->plan.Fc;
-    int rc = FSN_OK;
-    if (Bs >= B) {
-        rc = forward_impl(m, m->lane[0], d_mag, d_real, d_imag, B, T, h_frames, d_out, d_enh, s, s, Tw, Fc);
-    } else {
-        const size_t in_stride = (size_t)m->cfg.num_freqs * T, out_stride = (size_t)m->cfg.output_size * m->cfg.num_freqs * T;
-        int64_t launches = 0;
-        for (int b0 = 0; b0 < B && rc == FSN_OK; b0 += Bs) {
-            const int nb = (B - b0 < Bs) ? B - b0 : Bs;
-            rc = forward_impl(m, m->lane[0], d_mag + b0 * in_stride, d_real ? d_real + b0 * in_stride : nullptr, d_imag ? d_imag + b0 * in_stride : nullptr,
-                              nb, T, h_frames ? h_frames + b0 : nullptr, d_out ? d_out + b0 * out_stride : nullptr,
-                              d_enh ? d_enh + b0 * in_stride * 2 : nullptr, s, s, Tw, Fc);
-            launches += m->launches;
-        }
-        m->launches = launches;
-    }
+    return FSN_OK;
+}
+
+// Clips b0 .. b0 + nb - 1 of batch b (fewer at its end): every pointer advanced by its per-clip stride
+static Batch slice(const fsn_config& c, const Batch& b, int b0, int nb) {
+    const size_t plane = (size_t)c.num_freqs * b.T;
+    auto at = [b0](auto* p, size_t stride) { return p ? p + b0 * stride : p; };
+    Batch s = b;
+    s.B = b.B - b0 < nb ? b.B - b0 : nb;
+    s.mag = at(b.mag, plane); s.real = at(b.real, plane); s.imag = at(b.imag, plane); s.frames = at(b.frames, 1);
+    s.mask = at(b.mask, c.output_size * plane); s.enh = at(b.enh, 2 * plane);
+    s.wave = at(b.wave, b.L); s.wave_out = at(b.wave_out, b.L); s.samples = at(b.samples, 1);
+    return s;
+}
+
+// The plain forward of checked batch b on stream s, after the pipelined batches in flight.  Samples are independent, so a batch whose
+// workspace would exceed the cap (FSN_WS_CAP_GB, default 24 of the 80 GB) is run as equal sub-batches one after the other on the same
+// stream -- same results, bounded memory (e.g. 256 clips on the layer-wise path); a clip too long for the cap runs its sub-band stage
+// in time windows (plan_forward) -- same bits, O(window) sub-band memory -- or, with the sub-band TCN, in bin chunks -- O(chunk)
+// sub-band memory.
+static int run_plain(fsn_model* m, const Batch& b, cudaStream_t s) {
+    int rc = wait_lanes(m, s);
     if (rc) return rc;
+    const bool audio = b.call == CALL_AUDIO;
+    if (audio && !m->au_tab.bytes) {                                    // the tables of this model's n_fft, once
+        std::vector<float> tab;
+        audio_tables(2 * (m->cfg.num_freqs - 1), tab);
+        if (m->au_tab.ensure(tab.size() * sizeof(float), false)) return fail(FSN_ECUDA, "allocation of the audio tables failed");
+        CK(cudaMemcpy(m->au_tab.p, tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice));
+    }
+    m->plan = plan_forward(m->cfg, m->layerwise, b.B, b.T, m->ws_cap_bytes, m->env_sb_window, m->env_sb_chunk, audio);
+    const int Bs = m->plan.Bs;
+    int64_t launches = 0;
+    for (int b0 = 0; b0 < b.B && rc == FSN_OK; b0 += Bs) {
+        rc = forward_impl(m, m->lane[0], slice(m->cfg, b, b0, Bs), s, s, m->plan.Tw, m->plan.Fc);
+        launches += m->launches;
+    }
+    m->launches = launches;
+    if (rc) return rc;
+    m->au_valid = audio && Bs >= b.B;
     if (!m->ev_plain) CK(cudaEventCreateWithFlags(&m->ev_plain, cudaEventDisableTiming));
     CK(cudaEventRecord(m->ev_plain, s));
     m->plain_pending = true;
     return FSN_OK;
 }
 
-static int submit_plain(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
-                        float* d_out, float* d_enh, void* stream) {
-    if (!m) return fail(FSN_EINVAL, "null argument");
-    int rc = ensure_pipeline(m);
-    if (rc) return rc;
-    CK(cudaEventRecord(m->ev_in, static_cast<cudaStream_t>(stream)));    // everything enqueued on the caller's stream so far (the inputs)
-    return submit_impl(m, m->ev_in, d_mag, d_real, d_imag, B, T, d_out, d_enh, nullptr);
+// A device-buffer spectral call: check batch b, then run it plain or pipelined
+static int run_spectra(fsn_model* m, Batch b, void* stream) {
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = check_batch(m, b)) return rc;
+    if (b.call == CALL_FORWARD) return run_plain(m, b, s);
+    if (int rc = ensure_pipeline(m)) return rc;
+    CK(cudaEventRecord(m->ev_in, s));                                   // everything enqueued on the caller's stream so far (the inputs)
+    return submit_impl(m, m->ev_in, b, nullptr);
 }
 
 extern "C" int fsn_model_forward(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
                                  float* d_out, void* stream) {
-    if (!d_out) return fail(FSN_EINVAL, "null argument");
-    return forward_plain(m, d_mag, d_real, d_imag, B, T, nullptr, d_out, nullptr, stream);
+    return run_spectra(m, Batch{CALL_FORWARD, d_mag, d_real, d_imag, B, T, nullptr, d_out}, stream);
 }
 extern "C" int fsn_model_forward_enhance(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
                                          float* d_enh, void* stream) {
-    if (!d_enh) return fail(FSN_EINVAL, "null argument");
-    return forward_plain(m, d_mag, d_real, d_imag, B, T, nullptr, nullptr, d_enh, stream);
-}
-
-// The frame counts of a ragged batch: each in 1..T, and long enough for the TSSE convolutions.  Returns the array to pass on: null
-// when every clip spans all T frames, so that case runs exactly the unmasked forward.
-static int check_frames(const fsn_model* m, const int32_t* h_frames, int32_t B, int32_t T, const int32_t** use) {
-    *use = nullptr;
-    if (!h_frames) return FSN_OK;
-    if (!m) return fail(FSN_EINVAL, "null argument");
-    const fsn_config& c = m->cfg;
-    int kmax = 1;
-    if (c.model_kind == FSN_KIND_PLUS && c.channel_attention == FSN_ATTN_TSSE)
-        for (int i = 0; i < 3; ++i) kmax = c.kersize[i] > kmax ? c.kersize[i] : kmax;
-    bool all = true;
-    for (int b = 0; b < B; ++b) {
-        const int n = h_frames[b];
-        if (n < 1 || n > T) return fail(FSN_EINVAL, "frames[%d] = %d is outside 1..T = %d", b, n, T);
-        if (n + c.look_ahead < kmax)
-            return fail(FSN_EINVAL, "frames[%d] = %d: frames + look_ahead = %d is shorter than the TSSE kernel size %d", b, n, n + c.look_ahead, kmax);
-        all = all && n == T;
-    }
-    if (!all) *use = h_frames;
-    return FSN_OK;
+    return run_spectra(m, Batch{CALL_FORWARD, d_mag, d_real, d_imag, B, T, nullptr, nullptr, d_enh}, stream);
 }
 
 extern "C" int fsn_model_forward_ragged(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
                                         const int32_t* h_frames, float* d_out, void* stream) {
-    if (!d_out) return fail(FSN_EINVAL, "null argument");
-    if (B < 1 || T < 1) return fail(FSN_EINVAL, "bad batch/frames");
-    const int32_t* fr = nullptr;
-    int rc = check_frames(m, h_frames, B, T, &fr);
-    return rc ? rc : forward_plain(m, d_mag, d_real, d_imag, B, T, fr, d_out, nullptr, stream);
+    return run_spectra(m, Batch{CALL_FORWARD, d_mag, d_real, d_imag, B, T, h_frames, d_out}, stream);
 }
 extern "C" int fsn_model_forward_enhance_ragged(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
                                                 const int32_t* h_frames, float* d_enh, void* stream) {
-    if (!d_enh) return fail(FSN_EINVAL, "null argument");
-    if (B < 1 || T < 1) return fail(FSN_EINVAL, "bad batch/frames");
-    const int32_t* fr = nullptr;
-    int rc = check_frames(m, h_frames, B, T, &fr);
-    return rc ? rc : forward_plain(m, d_mag, d_real, d_imag, B, T, fr, nullptr, d_enh, stream);
-}
-// The audio call's geometry: n_fft = 2 (num_freqs - 1) a power of two from 64 to 1024
-static int audio_fft_ok(const fsn_config& c) {
-    const int N = 2 * (c.num_freqs - 1);
-    if (N < 64 || N > 1024 || (N & (N - 1)))
-        return fail(FSN_EINVAL, "num_freqs %d: the audio call needs n_fft = 2 (num_freqs - 1) to be a power of two from 64 to 1024 "
-                                "(num_freqs 33, 65, 129, 257 or 513)", c.num_freqs);
-    return FSN_OK;
-}
-
-// The audio call's geometry and clips (fsn_model_enhance_audio, fsn_plan_audio): n_fft = 2 (num_freqs - 1), every clip longer than
-// n_fft / 2 (torch.stft's reflect padding) and no longer than L, with enough frames for the TSSE kernels (check_frames, in samples),
-// and the forward's length limits on T = max_b L_b / hop + 1.  *Lmax: the longest clip; *all: every clip is Lmax samples long.
-static int audio_check(const fsn_config& c, int32_t B, int64_t L, const int64_t* h_lengths, int* T, int* Lmax, bool* all) {
-    if (int rc = audio_fft_ok(c)) return rc;
-    if (B < 1) return fail(FSN_EINVAL, "B = %d: the batch needs at least one clip", B);
-    if (L < 1 || L > 0x7fffffffLL) return fail(FSN_EINVAL, "L = %lld: the row length must be 1 .. 2^31 - 1 samples", (long long)L);
-    const int H = c.num_freqs - 1;                                      // hop = n_fft / 2
-    int kmax = 1;
-    if (c.model_kind == FSN_KIND_PLUS && c.channel_attention == FSN_ATTN_TSSE)
-        for (int i = 0; i < 3; ++i) kmax = c.kersize[i] > kmax ? c.kersize[i] : kmax;
-    long long mx = 0;
-    *all = true;
-    for (int b = 0; b < (h_lengths ? B : 1); ++b) {
-        const long long n = h_lengths ? h_lengths[b] : L;
-        char nm[40];
-        if (h_lengths) snprintf(nm, sizeof(nm), "clip %d: h_lengths[%d]", b, b);
-        else snprintf(nm, sizeof(nm), "L");
-        if (n <= H)
-            return fail(FSN_EINVAL, "%s = %lld: a clip needs more than n_fft / 2 = %d samples (torch.stft's reflect padding)", nm, n, H);
-        if (n > L) return fail(FSN_EINVAL, "%s = %lld exceeds the row length L = %lld", nm, n, (long long)L);
-        if (n / H + 1 + c.look_ahead < kmax)
-            return fail(FSN_EINVAL, "%s = %lld samples give %lld frames: frames + look_ahead = %lld is shorter than the TSSE kernel size %d "
-                                    "(a clip needs at least %lld samples)", nm, n, n / H + 1, n / H + 1 + c.look_ahead, kmax,
-                        (long long)(kmax - c.look_ahead - 1) * H);
-        if (b && n != mx) *all = false;
-        if (n > mx) mx = n;
-    }
-    *Lmax = (int)mx;
-    *T = (int)(mx / H + 1);
-    return check_length(c, 1, *T);
+    return run_spectra(m, Batch{CALL_FORWARD, d_mag, d_real, d_imag, B, T, h_frames, nullptr, d_enh}, stream);
 }
 
 extern "C" int fsn_model_enhance_audio(fsn_model* m, const float* d_wave, int32_t B, int64_t L, const int64_t* h_lengths, float* d_out,
                                        void* stream) {
-    if (!m) return fail(FSN_EINVAL, "m is null");
-    if (!d_wave) return fail(FSN_EINVAL, "d_wave is null ([B, L] float32 samples on the device)");
-    if (!d_out) return fail(FSN_EINVAL, "d_out is null ([B, L] float32 on the device)");
-    if (!m->finalized) return fail(FSN_ESTATE, "fsn_model_finalize has not been called");
-    const fsn_config& c = m->cfg;
-    int T = 0, Lmax = 0;
-    bool all = true;
-    if (int rc = audio_check(c, B, L, h_lengths, &T, &Lmax, &all)) return rc;
-    if (c.output_size != 2) return fail(FSN_EINVAL, "the audio call needs output_size 2 (a complex mask)");
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    for (auto& ln : m->lane)                                             // batches still in flight in the pipeline share the scratch buffers
-        if (ln.used) CK(cudaStreamWaitEvent(s, ln.ev_lstm, 0));
-    const int N = 2 * (c.num_freqs - 1), H = N / 2;
-    if (!m->au_tab.bytes) {                                              // the tables of this model's n_fft, once
-        std::vector<float> tab;
-        audio_tables(N, tab);
-        if (m->au_tab.ensure(tab.size() * sizeof(float), false)) return fail(FSN_ECUDA, "allocation of the audio tables failed");
-        CK(cudaMemcpy(m->au_tab.p, tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice));
-    }
-    // ragged: every clip's sample count, and its frame count unless every clip has T frames (check_frames)
-    std::vector<int32_t> samples, frames;
-    bool ragged_frames = false;
-    if (!all) {
-        samples.resize(B); frames.resize(B);
-        for (int b = 0; b < B; ++b) {
-            samples[b] = (int32_t)h_lengths[b];
-            frames[b] = samples[b] / H + 1;
-            ragged_frames = ragged_frames || frames[b] != T;
-        }
-    }
-    m->plan = plan_forward(c, runs_layerwise(c, m->env_impl), B, T, m->ws_cap_bytes, m->env_sb_window, m->env_sb_chunk, true);
-    const int Bs = m->plan.Bs;
-    int64_t launches = 0;
-    for (int b0 = 0; b0 < B; b0 += Bs) {
-        const int nb = (B - b0 < Bs) ? B - b0 : Bs;
-        const AudioIO io{d_wave + b0 * L, d_out + b0 * L, L, Lmax, all ? nullptr : samples.data() + b0};
-        if (int rc = forward_impl(m, m->lane[0], nullptr, nullptr, nullptr, nb, T, ragged_frames ? frames.data() + b0 : nullptr, nullptr,
-                                  nullptr, s, s, m->plan.Tw, m->plan.Fc, &io))
-            return rc;
-        launches += m->launches;
-    }
-    m->launches = launches;
-    m->au_valid = Bs >= B;
-    if (!m->ev_plain) CK(cudaEventCreateWithFlags(&m->ev_plain, cudaEventDisableTiming));
-    CK(cudaEventRecord(m->ev_plain, s));
-    m->plain_pending = true;
-    return FSN_OK;
+    Batch b{CALL_AUDIO, nullptr, nullptr, nullptr, B, 0, nullptr, nullptr, nullptr, d_wave, d_out, L, h_lengths};
+    std::vector<int32_t> lens;
+    if (int rc = check_batch(m, b, &lens)) return rc;
+    return run_plain(m, b, static_cast<cudaStream_t>(stream));
 }
 
-// Test hook: the sub-band stage alone on a given input, through the forward's own run_sb_lstm (its GEMM dispatch, per-layer state,
-// windows and epilogues); only the packer differs (SbPackLaunch::raw: the input as given instead of the normalised unfold)
+// Test hook: the sub-band stage alone on a given input, through the forward's own setup (prepare) and sub-band stage (its GEMM dispatch,
+// per-layer state, windows and epilogues); only the packer's arguments differ (SbPackLaunch::raw: the input as given instead of the
+// normalised unfold).  Outside the timing-event ring and the plan of the last plain forward.
 extern "C" int fsn_model_sb_forward(fsn_model* m, const float* d_x, int32_t B, int32_t T, int32_t Tw, const int32_t* h_frames,
                                     float* d_out, const float* d_real, const float* d_imag, float* d_enh, void* stream) {
-    if (!m || !d_x || (!d_out && !d_enh)) return fail(FSN_EINVAL, "null argument");
-    if (!m->finalized) return fail(FSN_ESTATE, "fsn_model_finalize has not been called");
-    const fsn_config& c = m->cfg;
-    if (c.sb_tcn) return fail(FSN_EINVAL, "fsn_model_sb_forward runs the sub-band LSTM / GRU; this model's sub-band model is the TCN");
-    if (d_enh && (!d_real || !d_imag)) return fail(FSN_EINVAL, "the enhanced-spectrum output needs the noisy real and imaginary planes");
-    if (d_enh && c.output_size != 2) return fail(FSN_EINVAL, "the enhanced-spectrum output needs output_size 2 (a complex mask)");
-    if (B < 1 || T < 1) return fail(FSN_EINVAL, "bad batch/frames");
-    if (Tw < 0 || Tw % 32) return fail(FSN_EINVAL, "Tw = %d: the window must be 0 or a positive multiple of 32 frames", Tw);
-    if (Tw && !runs_layerwise(c, m->env_impl)) return fail(FSN_EINVAL, "time windows of the sub-band stage need the layer-wise LSTM path");
-    const int32_t* fr = nullptr;
-    int rc = check_frames(m, h_frames, B, T, &fr);
-    if (rc) return rc;
-    if ((rc = check_length(c, B, T))) return rc;
+    Batch b{CALL_HOOK, nullptr, d_real, d_imag, B, T, h_frames, d_out, d_enh, nullptr, nullptr, 0, nullptr, 0, nullptr, d_x, Tw};
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    for (auto& ln : m->lane)                                             // batches still in flight in the pipeline share the scratch buffers
-        if (ln.used) CK(cudaStreamWaitEvent(s, ln.ev_lstm, 0));
-    Lane& ln = m->lane[0];
-    if ((rc = ensure_ws(m, ln, B, T, Tw, 0, s, s))) return rc;
     const int* tl = nullptr;
-    if (fr) {
-        if ((rc = stage_lengths(m, ln, fr, B, s))) return rc;
-        tl = static_cast<const int*>(ln.tlen.p);
-    }
-    m->launches = 0;
-    m->last_lane = 0;
-    SbPackLaunch sp{};
+    int rc = check_batch(m, b);
+    if (rc || (rc = wait_lanes(m, s)) || (rc = prepare(m, m->lane[0], b, Tw, 0, s, s, &tl))) return rc;
+    Lane& ln = m->lane[0];
+    SbPackLaunch sp = pack_args(m, ln, B, T, Tw, tl);
     sp.raw = d_x;
-    sp.B = B; sp.F = c.num_freqs; sp.Tp = T + c.look_ahead; sp.Ns = c.sb_num_neighbors; sp.Nf = c.fb_num_neighbors;
-    sp.nfb = c.model_kind == FSN_KIND_PLUS ? 3 : 1;
-    sp.ximg = static_cast<__half*>(ln.ximg.p);
-    sp.ntiles = (B * sp.F + 127) / 128;
-    sp.t0 = 0; sp.Tw = sp.Tp;
-    sp.tlen = tl;
-    if (!Tw) {                                                          // windowed: run_sb_lstm packs each window
-        if (sb_wide(c)) launch_sb_pack_wide(sp, !runs_layerwise(c, m->env_impl), s);
-        else launch_sb_pack(sp, s);
-        m->launches++;
-    }
-    if ((rc = run_sb_lstm(m, ln, B, T, Tw, sp, d_out, d_real, d_imag, d_enh, tl, s))) return rc;
+    pack_clip(m, ln, sp, Tw, 0, s);
+    if ((rc = sub_band(m, ln, b, Tw, 0, sp, tl, s))) return rc;
     CK(cudaGetLastError());
     return FSN_OK;
 }
 
 extern "C" int fsn_model_submit(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
                                 float* d_out, void* stream) {
-    if (!d_out) return fail(FSN_EINVAL, "null argument");
-    return submit_plain(m, d_mag, d_real, d_imag, B, T, d_out, nullptr, stream);
+    return run_spectra(m, Batch{CALL_PIPELINED, d_mag, d_real, d_imag, B, T, nullptr, d_out}, stream);
 }
 extern "C" int fsn_model_submit_enhance(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
                                         float* d_enh, void* stream) {
-    if (!d_enh) return fail(FSN_EINVAL, "null argument");
-    return submit_plain(m, d_mag, d_real, d_imag, B, T, nullptr, d_enh, stream);
+    return run_spectra(m, Batch{CALL_PIPELINED, d_mag, d_real, d_imag, B, T, nullptr, nullptr, d_enh}, stream);
 }
 
 extern "C" int fsn_model_last_lane(const fsn_model* m) { return m ? m->last_lane : 0; }
@@ -1760,29 +1750,36 @@ extern "C" int fsn_model_wait_lane(fsn_model* m, int32_t lane, void* stream) {
 
 extern "C" int fsn_model_wait(fsn_model* m, void* stream) {
     if (!m) return fail(FSN_EINVAL, "null model");
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    for (auto& ln : m->lane)
-        if (ln.used) CK(cudaStreamWaitEvent(s, ln.ev_lstm, 0));
-    return FSN_OK;
+    return wait_lanes(m, static_cast<cudaStream_t>(stream));
+}
+
+// The host-buffer calls' batch, checked before any staging: the inputs the model reads (mag; FullSubNet+: real and imag too) and the
+// output [B, O, F, T] in host memory
+static int host_batch(fsn_model* m, Call call, const float* const (&hin)[3], int32_t B, int32_t T, float* h_out, Batch* b) {
+    if (!m || !hin[0] || !h_out) return fail(FSN_EINVAL, "null argument");
+    for (int i = 1; i < (m->cfg.model_kind == FSN_KIND_PLUS ? 3 : 1); ++i)
+        if (!hin[i]) return fail(FSN_EINVAL, "missing input %d", i);
+    *b = Batch{call, hin[0], hin[1], hin[2], B, T, nullptr, h_out};
+    return check_batch(m, *b);
 }
 
 extern "C" int fsn_model_forward_host(fsn_model* m, const float* h_mag, const float* h_real, const float* h_imag, int32_t B, int32_t T,
                                       float* h_out, void* stream) {
-    if (!m || !h_mag || !h_out) return fail(FSN_EINVAL, "null argument");
+    const float* const hin[3] = {h_mag, h_real, h_imag};
+    Batch b;
+    if (int rc = host_batch(m, CALL_FORWARD, hin, B, T, h_out, &b)) return rc;
     const fsn_config& c = m->cfg;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const size_t in_bytes = (size_t)B * c.num_freqs * T * 4, out_bytes = (size_t)B * c.output_size * c.num_freqs * T * 4;
-    const float* hin[3] = {h_mag, h_real, h_imag};
     const int nin = (c.model_kind == FSN_KIND_PLUS) ? 3 : 1;
     for (int i = 0; i < nin; ++i) {
-        if (!hin[i]) return fail(FSN_EINVAL, "missing input %d", i);
         if (m->stage_in[i].ensure(in_bytes, false)) return fail(FSN_ECUDA, "staging allocation failed");
         CK(cudaMemcpyAsync(m->stage_in[i].p, hin[i], in_bytes, cudaMemcpyHostToDevice, s));
     }
     if (m->stage_out.ensure(out_bytes, false)) return fail(FSN_ECUDA, "staging allocation failed");
-    int rc = fsn_model_forward(m, static_cast<const float*>(m->stage_in[0].p), static_cast<const float*>(m->stage_in[1].p),
-                               static_cast<const float*>(m->stage_in[2].p), B, T, static_cast<float*>(m->stage_out.p), stream);
-    if (rc) return rc;
+    b.mag = static_cast<const float*>(m->stage_in[0].p); b.real = static_cast<const float*>(m->stage_in[1].p);
+    b.imag = static_cast<const float*>(m->stage_in[2].p); b.mask = static_cast<float*>(m->stage_out.p);
+    if (int rc = run_plain(m, b, s)) return rc;
     CK(cudaMemcpyAsync(h_out, m->stage_out.p, out_bytes, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     return FSN_OK;
@@ -1790,8 +1787,10 @@ extern "C" int fsn_model_forward_host(fsn_model* m, const float* h_mag, const fl
 
 extern "C" int fsn_model_forward_host_async(fsn_model* m, const float* h_mag, const float* h_real, const float* h_imag, int32_t B, int32_t T,
                                             float* h_out, void* stream) {
-    if (!m || !h_mag || !h_out) return fail(FSN_EINVAL, "null argument");
     (void)stream;                                                        // host buffers carry no stream order; the work runs on internal streams
+    const float* const hin[3] = {h_mag, h_real, h_imag};
+    Batch b;
+    if (int rc = host_batch(m, CALL_PIPELINED, hin, B, T, h_out, &b)) return rc;
     const fsn_config& c = m->cfg;
     int rc = ensure_pipeline(m);
     if (rc) return rc;
@@ -1806,12 +1805,10 @@ extern "C" int fsn_model_forward_host_async(fsn_model* m, const float* h_mag, co
     }
     const int slot = (int)(m->nsub & 1);                                 // staging slot (the workspace lane is chosen by submit_impl)
     const size_t in_bytes = (size_t)B * c.num_freqs * T * 4, out_bytes = (size_t)B * c.output_size * c.num_freqs * T * 4;
-    const float* hin[3] = {h_mag, h_real, h_imag};
     const int nin = (c.model_kind == FSN_KIND_PLUS) ? 3 : 1;
     // the forward that read this input slot (front end: mag / real / imag; fused epilogue: real / imag) has finished
     if (m->d2h_used[slot]) CK(cudaStreamWaitEvent(m->s_in, m->ev_done[slot], 0));
     for (int i = 0; i < nin; ++i) {
-        if (!hin[i]) return fail(FSN_EINVAL, "missing input %d", i);
         if (m->a_in[slot][i].bytes < in_bytes) {
             CK(cudaDeviceSynchronize());                                       // (re)allocation only on the first calls / size changes
             if (m->a_in[slot][i].ensure(in_bytes, false)) return fail(FSN_ECUDA, "staging allocation failed");
@@ -1824,10 +1821,9 @@ extern "C" int fsn_model_forward_host_async(fsn_model* m, const float* h_mag, co
         if (m->a_out[slot].ensure(out_bytes, false)) return fail(FSN_ECUDA, "staging allocation failed");
     }
     if (m->d2h_used[slot]) CK(cudaStreamWaitEvent(m->s_lstm, m->ev_d2h[slot], 0));   // the copy-out that read this output slot is done
-    int used = 0;
-    rc = submit_impl(m, m->ev_h2d[slot], static_cast<const float*>(m->a_in[slot][0].p), static_cast<const float*>(m->a_in[slot][1].p),
-                     static_cast<const float*>(m->a_in[slot][2].p), B, T, static_cast<float*>(m->a_out[slot].p), nullptr, &used);
-    if (rc) return rc;
+    b.mag = static_cast<const float*>(m->a_in[slot][0].p); b.real = static_cast<const float*>(m->a_in[slot][1].p);
+    b.imag = static_cast<const float*>(m->a_in[slot][2].p); b.mask = static_cast<float*>(m->a_out[slot].p);
+    if ((rc = submit_impl(m, m->ev_h2d[slot], b, nullptr))) return rc;
     CK(cudaEventRecord(m->ev_done[slot], m->s_lstm));
     CK(cudaStreamWaitEvent(m->s_out, m->ev_done[slot], 0));
     CK(cudaMemcpyAsync(h_out, m->a_out[slot].p, out_bytes, cudaMemcpyDeviceToHost, m->s_out));
@@ -2330,7 +2326,7 @@ static int step_slots(fsn_stream* st, const float* d_mag, int K, float* d_mask, 
     if (st->mode == FSN_STATE_MODE_AUDIO) return claim_mode(st, FSN_STATE_MODE_MASK);
     // the scratch, before any state changes (DevBuf::ensure only grows); on the layer-wise path every stepping session runs K
     // frames: one group
-    const bool layerwise = chunk && runs_layerwise(c, m->env_impl);
+    const bool layerwise = chunk && m->layerwise;
     StepScratch& x = chunk ? st->chunk : st->tick;
     std::vector<int> kf;
     std::vector<LwGroup> lw;
@@ -2465,7 +2461,7 @@ static int step_audio(fsn_stream* st, const float* d_samples, int K, const int32
         Km = kf[b] > Km ? kf[b] : Km;
         nzero += kf[b] && plan[b].k0 + plan[b].start == 1;          // model frame 0 in column 0: a START's reset
     }
-    const bool chunk = h_hops != nullptr, layerwise = chunk && runs_layerwise(c, m->env_impl);
+    const bool chunk = h_hops != nullptr, layerwise = chunk && m->layerwise;
     StepScratch& x = chunk ? st->chunk : st->tick;
     std::vector<LwGroup> lw;
     int e = 0;
@@ -2833,7 +2829,7 @@ extern "C" int fsn_plan_forward(const fsn_config* cfg, int32_t B, int32_t T, dou
 extern "C" int fsn_model_plan_bins(const fsn_model* m, int32_t B, int32_t T, int32_t* Bs, int32_t* Tw, int32_t* Fc, int64_t* bytes) {
     if (!m || !Bs || !Tw || !Fc || B < 1 || T < 1) return fail(FSN_EINVAL, "bad argument");
     if (int rc = check_length(m->cfg, 1, T)) return rc;
-    return put_plan(plan_forward(m->cfg, runs_layerwise(m->cfg, m->env_impl), B, T, m->ws_cap_bytes, m->env_sb_window, m->env_sb_chunk),
+    return put_plan(plan_forward(m->cfg, m->layerwise, B, T, m->ws_cap_bytes, m->env_sb_window, m->env_sb_chunk),
                     Bs, Tw, Fc, bytes);
 }
 

@@ -115,6 +115,7 @@ class _B200Model(nn.Module):
     """Shared machinery: C-ABI handle, lazy parameter push, forward dispatch."""
 
     _kind = None
+    _subband_runs = True
 
     def _setup(self, num_freqs, look_ahead, sb_num_neighbors, fb_num_neighbors, fb_hidden, sb_hidden, num_layers,
                output_size, fb_act, sb_act, norm_type, kersize, lstm_impl, fast_math, channel_attention="TSSE",
@@ -186,6 +187,18 @@ class _B200Model(nn.Module):
             pass
 
     # -- forward -------------------------------------------------------------------------------
+    def _check_call(self, x=None):
+        """What every entry point needs before it creates a handle: a subband_num the reference forward runs (FullSubNet_Plus), eval
+        mode and, for ``x`` (the input tensor; None for the host-buffer call), a CUDA device."""
+        if not self._subband_runs:
+            raise RuntimeError(f"subband_num={self.subband_num}: the attention was built for {self.num_channels} channels but the "
+                               "real/imag branches have num_freqs channels (the reference forward raises here too, "
+                               "fullsubnet_plus.py:157-163); only channel_attention_model='ECA' runs with subband_num > 1")
+        if self.training:
+            raise NotImplementedError("fsnplus_b200 implements the inference (eval) forward only; call .eval()")
+        if x is not None and not x.is_cuda:
+            raise RuntimeError("fsnplus_b200 has no CPU fallback: move the model and its inputs to a CUDA (H100) device")
+
     def enhance_spectrum(self, noisy_mag, noisy_real, noisy_imag, pipelined=False, out=None, hold=True, frames=None):
         """Model forward + decompress_cIRM + complex multiply with the noisy spectrum in ONE call (C ABI: fsn_model_forward_enhance /
         fsn_model_submit_enhance; reference inferencer.py:149-157): [B, 1, F, T] x3 -> enhanced spectrum complex64 [B, F, T], the
@@ -201,12 +214,7 @@ class _B200Model(nn.Module):
         clip's length.  n_fft = 2 (num_freqs - 1), hop = n_fft / 2, periodic Hann window."""
         if wave.dim() != 2:
             raise ValueError(f"enhance_audio: wave must be [B, L], got {tuple(wave.shape)}")
-        if self.training:
-            raise NotImplementedError("fsnplus_b200 implements the inference (eval) forward only; call .eval()")
-        if not wave.is_cuda:
-            raise RuntimeError("fsnplus_b200 has no CPU fallback: move the model and its inputs to a CUDA (H100) device")
-        if self._kind == _lib.KIND_PLUS and not self._subband_runs:
-            raise RuntimeError(f"subband_num={self.subband_num}: only channel_attention_model='ECA' runs with subband_num > 1")
+        self._check_call(wave)
         B, L = wave.shape
         hl = _lib.lengths_arg(lengths, B)
         x = wave.detach().to(dtype=torch.float32).contiguous()
@@ -236,10 +244,7 @@ class _B200Model(nn.Module):
             raise ValueError("frames (ragged batches) is not supported with pipelined=True / submit()")
         hframes = self._frames_arg(frames, B) if frames is not None else None
         assert Cn == 1, f"{self.__class__.__name__} takes the mag feature as inputs."      # :141
-        if self.training:
-            raise NotImplementedError("fsnplus_b200 implements the inference (eval) forward only; call .eval()")
-        if not mag.is_cuda:
-            raise RuntimeError("fsnplus_b200 has no CPU fallback: move the model and its inputs to a CUDA (H100) device")
+        self._check_call(mag)
         if F != self._cfg.num_freqs:
             raise ValueError(f"expected {self._cfg.num_freqs} frequency bins, got {F}")
         ins = [x.detach().to(dtype=torch.float32).contiguous() if x is not None else None for x in (mag, real, imag)]
@@ -302,6 +307,7 @@ class _B200Model(nn.Module):
         ``pipelined=True`` uses the double-buffered async entry point (copies and the front end of the next batch overlap the
         sub-band LSTM of the previous one); it needs PINNED buffers, the returned tensor is valid after ``sync_host()`` and the
         inputs/outputs are kept referenced until then."""
+        self._check_call()
         if mag.dim() != 4:
             raise ValueError("forward_host: mag must be [B, 1, F, T]")
         B, _, F, T = mag.shape
@@ -439,7 +445,8 @@ class FullSubNet_Plus(_B200Model):
             raise NotImplementedError(f"Not implemented channel attention model {channel_attention_model}")
         # fullsubnet_plus.py:47-50.  With subband_num > 1 the reference builds all three attentions for F // subband_num + 1
         # channels but applies the real / imag ones to F channels (:157-163), so its forward only runs with the
-        # channel-agnostic ECA; the containers keep the reference's shapes and forward() raises like the reference otherwise.
+        # channel-agnostic ECA; the containers keep the reference's shapes and every entry point raises like the reference
+        # forward otherwise (_check_call).
         self.num_channels = num_freqs if subband_num == 1 else num_freqs // subband_num + 1
         self._subband_runs = subband_num == 1 or channel_attention_model == "ECA"
         for sfx in ("", "_real", "_imag"):
@@ -471,10 +478,6 @@ class FullSubNet_Plus(_B200Model):
         ``frames`` (additive, keyword-only): the frame count of every clip of a ragged batch, 1 <= frames[b] <= T.  Clip b is then
         its first frames[b] frames; its output equals that clip's own forward there and is zero after (C ABI:
         fsn_model_forward_ragged)."""
-        if not self._subband_runs:
-            raise RuntimeError(f"subband_num={self.subband_num}: the attention was built for {self.num_channels} channels but the "
-                               "real/imag branches have num_freqs channels (the reference forward raises here too, "
-                               "fullsubnet_plus.py:157-163); only channel_attention_model='ECA' runs with subband_num > 1")
         return self._run(noisy_mag, noisy_real, noisy_imag, frames=frames)
 
 

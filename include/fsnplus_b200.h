@@ -161,7 +161,8 @@ int fsn_model_enhance_audio(fsn_model* m, const float* d_wave, int32_t B, int64_
 int fsn_plan_audio(const fsn_config* cfg, int32_t B, int64_t L, const int64_t* h_lengths, double cap_bytes, int32_t force_window,
                    int32_t force_bins, int32_t* Bs, int32_t* Tw, int32_t* Fc, int64_t* bytes);
 /* Same call with HOST buffers (pinned or pageable): H2D copies, the forward and the D2H copy of the
- * mask are all enqueued on `stream` and the call returns after the result is in h_out. */
+ * mask are all enqueued on `stream` and the call returns after the result is in h_out.  Its arguments are checked as
+ * fsn_model_forward checks them, before anything is staged, copied or synchronised. */
 int fsn_model_forward_host(fsn_model* m, const float* h_mag, const float* h_real, const float* h_imag, int32_t B, int32_t T,
                            float* h_out, void* stream);
 
@@ -178,7 +179,8 @@ int fsn_model_forward_host(fsn_model* m, const float* h_mag, const float* h_real
  *
  * fsn_model_forward_host_async: pinned host buffers; additionally the H2D copy of batch i+1 and the D2H copy of batch i-1
  * overlap on two copy streams.  `stream` is ignored (host memory carries no stream order).  The host buffers must stay
- * untouched (h_out unread) until fsn_model_sync_host() returns. */
+ * untouched (h_out unread) until fsn_model_sync_host() returns.  Both pipelined calls check their arguments as fsn_model_forward
+ * does (with the length limits of the whole batch) before they record, wait on, allocate or copy anything. */
 int fsn_model_submit(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
                      float* d_out, void* stream);
 int fsn_model_submit_enhance(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,

@@ -5,6 +5,7 @@
 #include "fsn_kernels.h"
 
 #include <algorithm>
+#include <cerrno>
 #include <cstdarg>
 #include <cstddef>
 #include <cstdio>
@@ -98,6 +99,22 @@ static uint64_t hash_words(uint64_t h, const void* p, size_t n) {
 }
 
 struct ParamSpec { std::string key; int64_t numel; };
+
+// Every fsn_config field by name, in declaration order: the saved-session check (cfg_diff) and the model file's config section
+// (fsn_model_file_write, read_model_file) name the fields from this one list
+static const struct CfgField { const char* name; size_t off; } kCfgFields[] = {
+    {"model_kind", offsetof(fsn_config, model_kind)}, {"num_freqs", offsetof(fsn_config, num_freqs)},
+    {"look_ahead", offsetof(fsn_config, look_ahead)}, {"sb_num_neighbors", offsetof(fsn_config, sb_num_neighbors)},
+    {"fb_num_neighbors", offsetof(fsn_config, fb_num_neighbors)}, {"fb_hidden", offsetof(fsn_config, fb_hidden)},
+    {"sb_hidden", offsetof(fsn_config, sb_hidden)}, {"num_layers", offsetof(fsn_config, num_layers)},
+    {"output_size", offsetof(fsn_config, output_size)}, {"fb_act", offsetof(fsn_config, fb_act)}, {"sb_act", offsetof(fsn_config, sb_act)},
+    {"norm_type", offsetof(fsn_config, norm_type)}, {"kersize[0]", offsetof(fsn_config, kersize)},
+    {"kersize[1]", offsetof(fsn_config, kersize) + 4}, {"kersize[2]", offsetof(fsn_config, kersize) + 8},
+    {"lstm_impl", offsetof(fsn_config, lstm_impl)},
+    {"fast_math", offsetof(fsn_config, fast_math)}, {"channel_attention", offsetof(fsn_config, channel_attention)},
+    {"rnn_type", offsetof(fsn_config, rnn_type)}, {"subband_num", offsetof(fsn_config, subband_num)},
+    {"tcn_causal", offsetof(fsn_config, tcn_causal)}, {"sb_tcn", offsetof(fsn_config, sb_tcn)}};
+static_assert(sizeof(fsn_config) == sizeof(kCfgFields) / sizeof(kCfgFields[0]) * sizeof(int32_t), "kCfgFields names every fsn_config field");
 
 // The packed block weights of one TCN (pack_tcn_blocks): nbr branches of C channels padded to Cp, gLN2 folded into the second 1x1
 // convolution; NT / ntiles = N tile and N tiles of its Cp-wide GEMMs.
@@ -282,11 +299,10 @@ static bool runs_layerwise(const fsn_config& c, int env_impl) {
     return tc5r_ok(c) && (impl == FSN_LSTM_AUTO || impl == FSN_LSTM_TCGEN05);
 }
 
-static void build_specs(fsn_model* m) {
-    const fsn_config& c = m->cfg;
+// The state_dict keys and sizes a valid configuration expects, in the reference's order (fsn_model_param_info, the model file)
+static std::vector<ParamSpec> param_specs(const fsn_config& c) {
     const int F = c.num_freqs;
-    auto& v = m->specs;
-    m->Isb = sb_input_size(c);
+    std::vector<ParamSpec> v;
     if (c.model_kind == FSN_KIND_PLUS) {
         const char* sfx[3] = {"", "_real", "_imag"};
         const char* cn[3] = {"smallConv1d", "middleConv1d", "largeConv1d"};
@@ -310,8 +326,10 @@ static void build_specs(fsn_model* m) {
     } else {
         lstm_specs(v, "fb_model", F, c.fb_hidden, c.num_layers, F, c.rnn_type == FSN_RNN_GRU ? 3 : 4);
     }
-    if (c.sb_tcn) tcn_specs(v, "sb_model", m->Isb, c.output_size);       // hidden width 512: sb_hidden and num_layers are unused
-    else lstm_specs(v, "sb_model", m->Isb, c.sb_hidden, c.num_layers, c.output_size, c.rnn_type == FSN_RNN_GRU ? 3 : 4);
+    const int isb = sb_input_size(c);
+    if (c.sb_tcn) tcn_specs(v, "sb_model", isb, c.output_size);           // hidden width 512: sb_hidden and num_layers are unused
+    else lstm_specs(v, "sb_model", isb, c.sb_hidden, c.num_layers, c.output_size, c.rnn_type == FSN_RNN_GRU ? 3 : 4);
+    return v;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -561,9 +579,9 @@ static void bind_weights(fsn_model* m, const DevPtrs& dev) {
 extern "C" int fsn_version(void) { return 101; }
 extern "C" const char* fsn_last_error(void) { return g_err; }
 
-extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
-    if (!cfg || !out) return fail(FSN_EINVAL, "null argument");
-    const fsn_config& c = *cfg;
+// The configuration checks of fsn_model_create, host only: fsn_model_file_write and the model file reader refuse what create refuses,
+// with the same code and message
+static int config_check(const fsn_config& c) {
     if (c.model_kind != FSN_KIND_PLUS && c.model_kind != FSN_KIND_FSN) return fail(FSN_EINVAL, "unknown model_kind %d", c.model_kind);
     if (c.num_freqs > 2048) return fail(FSN_EINVAL, "num_freqs > 2048 is not supported");
     if (c.num_freqs < 4 || c.look_ahead < 0 || c.sb_num_neighbors < 0 || c.fb_num_neighbors < 0) return fail(FSN_EINVAL, "bad geometry");
@@ -588,6 +606,13 @@ extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
     if (c.sb_tcn && isb > 64)
         return fail(FSN_EINVAL, "sub-band input size %d > 64 not supported by the sub-band TCN (its output head holds a row's channels in one 64-column tile)", isb);
     if (isb > 128) return fail(FSN_EINVAL, "sub-band input size %d > 128 not supported", isb);
+    return FSN_OK;
+}
+
+extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
+    if (!cfg || !out) return fail(FSN_EINVAL, "null argument");
+    const fsn_config& c = *cfg;
+    if (int rc = config_check(c)) return rc;
     int sb_window = 0;
     if (const char* e = getenv("FSN_SB_WINDOW"); e && *e) {
         char* end = nullptr;
@@ -625,7 +650,8 @@ extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
     // iSTFT kernels of the pipelined entry points.
     { const char* e = getenv("FSN_PDL"); m->env_pdl = e ? (atoi(e) != 0 ? 1 : 0) : -1; }
     { const char* e = getenv("FSN_WS_CAP_GB"); if (e && atof(e) > 0) m->ws_cap_bytes = atof(e) * 1e9; }
-    build_specs(m);
+    m->Isb = sb_input_size(c);
+    m->specs = param_specs(c);
     for (int i = 0; i < fsn_model::NEV; ++i) { cudaEventCreate(&m->ev0[i]); cudaEventCreate(&m->ev1[i]); cudaEventCreate(&m->evf0[i]); cudaEventCreate(&m->evf1[i]); }
     { cudaDeviceProp prop; int dev = 0; cudaGetDevice(&dev); if (cudaGetDeviceProperties(&prop, dev) == cudaSuccess) m->num_sms = prop.multiProcessorCount; }
     *out = m;
@@ -746,6 +772,235 @@ extern "C" int fsn_model_finalize(fsn_model* m) {
     id ^= id >> 33; id *= 0xff51afd7ed558ccdull; id ^= id >> 33;                              // final avalanche
     m->weights_id = id ? id : 1;                                                               // 0 means "not finalized"
     m->finalized = true;
+    return FSN_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// model file (DESIGN.md §3.15): the configuration by field name and the reference state_dict in one little-endian, versioned,
+// checksummed file.  Host only.
+// ---------------------------------------------------------------------------------------------
+static_assert(__BYTE_ORDER__ == __ORDER_LITTLE_ENDIAN__, "the model file's integers and floats are copied in host byte order");
+static const char kFileMagic[8] = {'F', 'S', 'N', 'M', 'O', 'D', 'E', 'L'};
+static const uint32_t kFileVersion = 1;
+static const uint64_t kFileHashBasis = 0xcbf29ce484222325ull;   // hash_words over every byte before the checksum, from the FNV-1a basis
+
+static void put_bytes(std::vector<unsigned char>& b, const void* p, size_t n) {
+    const unsigned char* c = static_cast<const unsigned char*>(p);
+    b.insert(b.end(), c, c + n);
+}
+template <class T> static void put(std::vector<unsigned char>& b, T v) { put_bytes(b, &v, sizeof(T)); }
+
+// Matches records (keys[i], numel[i]) with the configuration's spec list: (*rec)[s] is the record of spec s.  FSN_EINVAL with the
+// messages of fsn_model_set_param (an unexpected key, a size mismatch) and fsn_model_finalize (a missing parameter), or a duplicate key.
+static int match_params(const std::vector<ParamSpec>& specs, const std::vector<std::string>& keys, const std::vector<int64_t>& numel,
+                        std::vector<int>* rec) {
+    std::map<std::string, int> idx;
+    for (size_t s = 0; s < specs.size(); ++s) idx[specs[s].key] = (int)s;
+    rec->assign(specs.size(), -1);
+    for (size_t i = 0; i < keys.size(); ++i) {
+        const auto it = idx.find(keys[i]);
+        if (it == idx.end()) return fail(FSN_EINVAL, "unexpected key %s", keys[i].c_str());
+        const ParamSpec& s = specs[it->second];
+        if (numel[i] != s.numel)
+            return fail(FSN_EINVAL, "size mismatch for %s: expected %lld, got %lld", s.key.c_str(), (long long)s.numel, (long long)numel[i]);
+        int& r = (*rec)[it->second];
+        if (r >= 0) return fail(FSN_EINVAL, "duplicate key %s", s.key.c_str());
+        r = (int)i;
+    }
+    for (size_t s = 0; s < specs.size(); ++s)
+        if ((*rec)[s] < 0) return fail(FSN_EINVAL, "missing parameter %s", specs[s].key.c_str());
+    return FSN_OK;
+}
+
+// Writes b to path through path + ".tmp" and a rename: a failed write leaves no file at path and removes its temporary
+static int write_file(const char* path, const std::vector<unsigned char>& b) {
+    const std::string tmp = std::string(path) + ".tmp";
+    FILE* f = fopen(tmp.c_str(), "wb");
+    if (!f) return fail(FSN_EINVAL, "cannot create %s: %s", tmp.c_str(), strerror(errno));
+    int err = 0;
+    if (fwrite(b.data(), 1, b.size(), f) != b.size()) err = errno ? errno : EIO;
+    if (fflush(f) && !err) err = errno;
+    if (fclose(f) && !err) err = errno;
+    if (err) {
+        remove(tmp.c_str());
+        return fail(FSN_EINVAL, "writing %s failed: %s", tmp.c_str(), strerror(err));
+    }
+    if (rename(tmp.c_str(), path)) {
+        err = errno;
+        remove(tmp.c_str());
+        return fail(FSN_EINVAL, "cannot rename %s to %s: %s", tmp.c_str(), path, strerror(err));
+    }
+    return FSN_OK;
+}
+
+extern "C" int fsn_model_file_write(const char* path, const fsn_config* cfg, int32_t n, const char* const* keys, const float* const* h_data,
+                                    const int64_t* numel) {
+    if (!path || !cfg) return fail(FSN_EINVAL, "null argument");
+    if (n < 0) return fail(FSN_EINVAL, "n = %d: the parameter count is negative", n);
+    if (n > 0 && (!keys || !h_data || !numel)) return fail(FSN_EINVAL, "null argument");
+    if (int rc = config_check(*cfg)) return rc;
+    std::vector<std::string> k(n);
+    for (int i = 0; i < n; ++i) {
+        if (!keys[i] || !h_data[i]) return fail(FSN_EINVAL, "null argument: keys[%d] or h_data[%d]", i, i);
+        k[i] = keys[i];
+    }
+    const std::vector<ParamSpec> specs = param_specs(*cfg);
+    std::vector<int> rec;
+    if (int rc = match_params(specs, k, std::vector<int64_t>(numel, numel + n), &rec)) return rc;
+    size_t bytes = sizeof(kFileMagic) + 4 + 4 + 4 + 8;
+    for (const auto& f : kCfgFields) bytes += 2 + strlen(f.name) + 4;
+    for (const auto& s : specs) bytes += 2 + s.key.size() + 8 + (size_t)s.numel * 4;
+    std::vector<unsigned char> b;
+    b.reserve(bytes);
+    put_bytes(b, kFileMagic, sizeof(kFileMagic));
+    put<uint32_t>(b, kFileVersion);
+    put<uint32_t>(b, (uint32_t)(sizeof(kCfgFields) / sizeof(kCfgFields[0])));
+    for (const auto& f : kCfgFields) {
+        int32_t v;
+        memcpy(&v, reinterpret_cast<const char*>(cfg) + f.off, 4);
+        put<uint16_t>(b, (uint16_t)strlen(f.name));
+        put_bytes(b, f.name, strlen(f.name));
+        put<int32_t>(b, v);
+    }
+    put<uint32_t>(b, (uint32_t)specs.size());
+    for (size_t s = 0; s < specs.size(); ++s) {
+        put<uint16_t>(b, (uint16_t)specs[s].key.size());
+        put_bytes(b, specs[s].key.data(), specs[s].key.size());
+        put<int64_t>(b, specs[s].numel);
+        put_bytes(b, h_data[rec[s]], (size_t)specs[s].numel * 4);
+    }
+    put<uint64_t>(b, hash_words(kFileHashBasis, b.data(), b.size()));
+    return write_file(path, b);
+}
+
+// One parameter record of a model file: its key, size and the byte offset of its float32 data
+struct FileRecord { std::string key; int64_t numel; size_t off; };
+
+// Reads and verifies a whole model file: magic, version, bounds, trailing bytes, checksum, config field names, the configuration
+// (config_check) and the key set (match_params).  On success *cfg is the configuration, *bytes the file and *recs its records in
+// spec order.  Every error is FSN_EINVAL; a structural one names the file and, for a truncation, the byte offset.
+static int read_model_file(const char* path, fsn_config* cfg, std::vector<unsigned char>* bytes, std::vector<FileRecord>* recs) {
+    FILE* f = fopen(path, "rb");
+    if (!f) return fail(FSN_EINVAL, "cannot open %s: %s", path, strerror(errno));
+    std::vector<unsigned char>& b = *bytes;
+    size_t n = 0;
+    b.resize(1 << 20);
+    for (;;) {
+        n += fread(b.data() + n, 1, b.size() - n, f);
+        if (n < b.size()) break;
+        b.resize(2 * b.size());
+    }
+    b.resize(n);
+    const bool rerr = ferror(f);
+    fclose(f);
+    if (rerr) return fail(FSN_EINVAL, "reading %s failed", path);
+
+    size_t pos = 0;
+    auto get = [&](void* dst, uint64_t k, const std::string& what) -> int {
+        if (n - pos < k)
+            return fail(FSN_EINVAL, "model file %s: truncated: %s at byte %zu needs %llu bytes, the file ends at byte %zu", path, what.c_str(),
+                        pos, (unsigned long long)k, n);
+        if (dst) memcpy(dst, b.data() + pos, k);
+        pos += k;
+        return FSN_OK;
+    };
+    char magic[8];
+    if (int rc = get(magic, 8, "the magic")) return rc;
+    if (memcmp(magic, kFileMagic, 8)) return fail(FSN_EINVAL, "model file %s: bad magic (not an FSNMODEL file)", path);
+    uint32_t version = 0, nfield = 0, nparam = 0;
+    if (int rc = get(&version, 4, "the format version")) return rc;
+    if (version != kFileVersion) return fail(FSN_EINVAL, "model file %s: format version %u, this library reads version %u", path, version, kFileVersion);
+    if (int rc = get(&nfield, 4, "the config field count")) return rc;
+    std::vector<std::pair<std::string, int32_t>> fields;
+    for (uint32_t i = 0; i < nfield; ++i) {
+        const std::string at = "config field " + std::to_string(i);
+        uint16_t len = 0;
+        int32_t v = 0;
+        if (int rc = get(&len, 2, "the name length of " + at)) return rc;
+        std::string name(len, '\0');
+        if (int rc = get(&name[0], len, "the name of " + at)) return rc;
+        if (int rc = get(&v, 4, "the value of config field " + name)) return rc;
+        fields.emplace_back(name, v);
+    }
+    if (int rc = get(&nparam, 4, "the parameter count")) return rc;
+    std::vector<FileRecord> r;
+    for (uint32_t i = 0; i < nparam; ++i) {
+        const std::string at = "parameter " + std::to_string(i);
+        uint16_t len = 0;
+        if (int rc = get(&len, 2, "the key length of " + at)) return rc;
+        if (len == 0 || len > 255)
+            return fail(FSN_EINVAL, "model file %s: %s: key length %u at byte %zu (a key is 1..255 bytes)", path, at.c_str(), len, pos - 2);
+        FileRecord q;
+        q.key.assign(len, '\0');
+        if (int rc = get(&q.key[0], len, "the key of " + at)) return rc;
+        if (int rc = get(&q.numel, 8, "the size of parameter " + q.key)) return rc;
+        if (q.numel < 0) return fail(FSN_EINVAL, "model file %s: parameter %s: negative size %lld at byte %zu", path, q.key.c_str(), (long long)q.numel, pos - 8);
+        q.off = pos;
+        const uint64_t data = (uint64_t)q.numel <= UINT64_MAX / 4 ? (uint64_t)q.numel * 4 : UINT64_MAX;
+        if (int rc = get(nullptr, data, "the data of parameter " + q.key)) return rc;
+        r.push_back(std::move(q));
+    }
+    if (n - pos < 8) return get(nullptr, 8, "the checksum");
+    if (n - pos > 8) return fail(FSN_EINVAL, "model file %s: %zu trailing bytes after the checksum at byte %zu", path, n - pos - 8, pos);
+    uint64_t stored;
+    memcpy(&stored, b.data() + pos, 8);
+    const uint64_t sum = hash_words(kFileHashBasis, b.data(), pos);
+    if (stored != sum)
+        return fail(FSN_EINVAL, "model file %s: checksum mismatch (stored %016llx, computed %016llx): the file is corrupt", path,
+                    (unsigned long long)stored, (unsigned long long)sum);
+
+    fsn_config c;
+    memset(&c, 0, sizeof(c));                                         // a field the file does not name takes 0, the documented default
+    std::vector<bool> seen(sizeof(kCfgFields) / sizeof(kCfgFields[0]), false);
+    for (const auto& fv : fields) {
+        size_t j = 0;
+        while (j < seen.size() && fv.first != kCfgFields[j].name) ++j;
+        if (j == seen.size()) return fail(FSN_EINVAL, "model file %s: unknown config field \"%s\"", path, fv.first.c_str());
+        if (seen[j]) return fail(FSN_EINVAL, "model file %s: config field %s appears twice", path, kCfgFields[j].name);
+        seen[j] = true;
+        memcpy(reinterpret_cast<char*>(&c) + kCfgFields[j].off, &fv.second, 4);
+    }
+    if (int rc = config_check(c)) return rc;
+    std::vector<std::string> keys;
+    std::vector<int64_t> numel;
+    for (const auto& q : r) { keys.push_back(q.key); numel.push_back(q.numel); }
+    std::vector<int> rec;
+    const std::vector<ParamSpec> specs = param_specs(c);
+    if (int rc = match_params(specs, keys, numel, &rec)) return rc;
+    recs->clear();
+    for (int i : rec) recs->push_back(r[i]);
+    *cfg = c;
+    return FSN_OK;
+}
+
+extern "C" int fsn_model_file_config(const char* path, fsn_config* cfg) {
+    if (!path || !cfg) return fail(FSN_EINVAL, "null argument");
+    fsn_config c;
+    std::vector<unsigned char> b;
+    std::vector<FileRecord> recs;
+    if (int rc = read_model_file(path, &c, &b, &recs)) return rc;
+    *cfg = c;
+    return FSN_OK;
+}
+
+extern "C" int fsn_model_load(const char* path, fsn_model** out) {
+    if (!out) return fail(FSN_EINVAL, "null argument");
+    *out = nullptr;
+    if (!path) return fail(FSN_EINVAL, "null argument");
+    fsn_config c;
+    std::vector<unsigned char> b;
+    std::vector<FileRecord> recs;
+    if (int rc = read_model_file(path, &c, &b, &recs)) return rc;
+    fsn_model* m = nullptr;
+    if (int rc = fsn_model_create(&c, &m)) return rc;
+    std::vector<float> v;                                             // the records' data is not 4-byte aligned in the file
+    for (const auto& q : recs) {
+        v.resize((size_t)q.numel);
+        memcpy(v.data(), b.data() + q.off, (size_t)q.numel * 4);
+        if (int rc = fsn_model_set_param(m, q.key.c_str(), v.data(), q.numel)) { fsn_model_destroy(m); return rc; }
+    }
+    if (int rc = fsn_model_finalize(m)) { fsn_model_destroy(m); return rc; }
+    *out = m;
     return FSN_OK;
 }
 
@@ -2586,19 +2841,8 @@ extern "C" int64_t fsn_stream_state_bytes(const fsn_stream* st) {
 
 // The first configuration field in which a and b differ, lstm_impl excepted (streaming always runs the mma kernels); null if none
 static const char* cfg_diff(const fsn_config& a, const fsn_config& b, int* va, int* vb) {
-    static const struct { const char* name; size_t off; } f[] = {
-        {"model_kind", offsetof(fsn_config, model_kind)}, {"num_freqs", offsetof(fsn_config, num_freqs)},
-        {"look_ahead", offsetof(fsn_config, look_ahead)}, {"sb_num_neighbors", offsetof(fsn_config, sb_num_neighbors)},
-        {"fb_num_neighbors", offsetof(fsn_config, fb_num_neighbors)}, {"fb_hidden", offsetof(fsn_config, fb_hidden)},
-        {"sb_hidden", offsetof(fsn_config, sb_hidden)}, {"num_layers", offsetof(fsn_config, num_layers)},
-        {"output_size", offsetof(fsn_config, output_size)}, {"fb_act", offsetof(fsn_config, fb_act)}, {"sb_act", offsetof(fsn_config, sb_act)},
-        {"norm_type", offsetof(fsn_config, norm_type)}, {"kersize[0]", offsetof(fsn_config, kersize)},
-        {"kersize[1]", offsetof(fsn_config, kersize) + 4}, {"kersize[2]", offsetof(fsn_config, kersize) + 8},
-        {"fast_math", offsetof(fsn_config, fast_math)}, {"channel_attention", offsetof(fsn_config, channel_attention)},
-        {"rnn_type", offsetof(fsn_config, rnn_type)}, {"subband_num", offsetof(fsn_config, subband_num)},
-        {"tcn_causal", offsetof(fsn_config, tcn_causal)}, {"sb_tcn", offsetof(fsn_config, sb_tcn)}};
-    static_assert(sizeof(fsn_config) == (sizeof(f) / sizeof(f[0]) + 1) * sizeof(int32_t), "every fsn_config field but lstm_impl is compared");
-    for (const auto& e : f) {
+    for (const auto& e : kCfgFields) {
+        if (e.off == offsetof(fsn_config, lstm_impl)) continue;
         memcpy(va, reinterpret_cast<const char*>(&a) + e.off, 4);
         memcpy(vb, reinterpret_cast<const char*>(&b) + e.off, 4);
         if (*va != *vb) return e.name;

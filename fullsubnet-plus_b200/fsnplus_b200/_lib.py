@@ -26,6 +26,7 @@ SYMBOLS = [
     "fsn_stream_state_bytes", "fsn_stream_state_layout", "fsn_model_weights_id", "fsn_stream_save_slots", "fsn_stream_load_slots",
     "fsn_model_enhance_audio", "fsn_plan_audio",
     "fsn_stream_step_chunk", "fsn_stream_chunk_plan", "fsn_stream_step_audio_chunk",
+    "fsn_model_file_write", "fsn_model_file_config", "fsn_model_load",
 ]
 
 
@@ -58,6 +59,24 @@ def state_layout(cfg, mode):
     nb, mb = C.c_int64(), C.c_int32()
     check(lib.fsn_stream_state_layout(C.byref(cfg), int(mode), C.byref(nb), C.byref(mb)))
     return nb.value, mb.value
+
+
+def write_model_file(path, cfg, params):
+    """fsn_model_file_write: ``cfg`` and ``params`` ({state_dict key: contiguous float32 CPU tensor}) to the model file ``path``.  Host
+    only; needs no GPU."""
+    keys = list(params)
+    n = len(keys)
+    ckeys = (C.c_char_p * n)(*[k.encode() for k in keys])
+    data = (C.c_void_p * n)(*[params[k].data_ptr() for k in keys])
+    numel = (C.c_int64 * n)(*[params[k].numel() for k in keys])
+    check(load_library().fsn_model_file_write(os.fsencode(path), C.byref(cfg), n, ckeys, data, numel))
+
+
+def model_file_config(path):
+    """fsn_model_file_config: the FsnConfig of the model file ``path``, after verifying the whole file.  Host only; needs no GPU."""
+    cfg = FsnConfig()
+    check(load_library().fsn_model_file_config(os.fsencode(path), C.byref(cfg)))
+    return cfg
 
 
 def lib_path():
@@ -155,6 +174,9 @@ def load_library():
     lib.fsn_model_enhance_audio.argtypes = [vp, vp, i32, i64, C.POINTER(i64), vp, vp]
     lib.fsn_plan_audio.argtypes = [C.POINTER(FsnConfig), i32, i64, C.POINTER(i64), C.c_double, i32, i32, C.POINTER(i32), C.POINTER(i32),
                                    C.POINTER(i32), C.POINTER(i64)]
+    lib.fsn_model_file_write.argtypes = [C.c_char_p, C.POINTER(FsnConfig), i32, C.POINTER(C.c_char_p), C.POINTER(vp), C.POINTER(i64)]
+    lib.fsn_model_file_config.argtypes = [C.c_char_p, C.POINTER(FsnConfig)]
+    lib.fsn_model_load.argtypes = [C.c_char_p, C.POINTER(vp)]
     _LIB = lib
     return lib
 

@@ -167,13 +167,25 @@ class _B200Model(nn.Module):
                 k = key.value.decode()
                 if k not in sd:
                     raise _lib.FsnError(f"state_dict has no entry {k}")
-                t = sd[k].detach().to(device="cpu", dtype=torch.float32).contiguous()
+                t = self._host_param(sd[k])
                 if t.numel() != numel.value:
                     raise _lib.FsnError(f"size mismatch for {k}: {tuple(t.shape)} vs {numel.value} elements")
                 _lib.check(lib.fsn_model_set_param(self._handle, key.value, C.c_void_p(t.data_ptr()), t.numel()))
             _lib.check(lib.fsn_model_finalize(self._handle))
             self._pushed_version = ver
         return lib
+
+    @staticmethod
+    def _host_param(t):
+        """A state_dict tensor as the library takes it: contiguous float32 on the host."""
+        return t.detach().to(device="cpu", dtype=torch.float32).contiguous()
+
+    def save_model_file(self, path):
+        """Write the configuration and parameters to the model file ``path`` (C ABI: fsn_model_file_write; format in
+        include/fsnplus_b200.h), which ``fsn_model_load`` turns into a ready handle in a C or C++ program.  Host only: the model may
+        live on any device and no GPU is needed.  A handle loaded from the file has this model's ``weights_id()``."""
+        sd = self.state_dict()
+        _lib.write_model_file(path, self._cfg, {k: self._host_param(v) for k, v in sd.items()})
 
     def _release(self):
         if getattr(self, "_handle", None) is not None:

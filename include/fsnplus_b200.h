@@ -110,6 +110,33 @@ int fsn_model_param_info(const fsn_model* m, int index, const char** key, int64_
 /* Re-orders / converts the parameters into the kernel layouts (fp16 gate-interleaved LSTM images, ...). */
 int fsn_model_finalize(fsn_model* m);
 
+/* Model files (DESIGN.md §3.15, INTEGRATION.md): a configuration and its reference state_dict in one file, so a C or C++ program gets a
+ * ready handle without Python.  Little-endian, all integers unsigned unless noted:
+ *   magic       8 bytes "FSNMODEL"
+ *   version     u32 = 1
+ *   config      u32 count, then per field: u16 name length, the name (an fsn_config member: "num_freqs", "kersize[0]", ...), i32 value
+ *   parameters  u32 count, then per key: u16 key length (1..255), the key, i64 numel, numel float32 values in the reference's shape
+ *               order.  The keys are exactly those fsn_model_param_info lists for the configuration, in that order.
+ *   checksum    u64: h = 0xcbf29ce484222325 (the FNV-1a basis); for each 8-byte little-endian word w of every preceding byte (the
+ *               last word zero-padded): h = (h ^ w) * 0x100000001b3 mod 2^64, h ^= h >> 29.
+ * A config field the file does not name takes 0 (the zero-initialised default); a field name this library does not know is refused.
+ *
+ * fsn_model_file_write: writes cfg and the n parameters (keys[i], h_data[i]: numel[i] float32 host values in the reference's shape) to
+ * path.  Host only, no GPU.  cfg is checked as fsn_model_create checks it, with the same codes and messages; the keys must be exactly the
+ * configuration's, in any order, each with its size (FSN_EINVAL naming the unexpected, duplicate, mis-sized or missing key).  The file is
+ * written to path + ".tmp" and renamed over path: a failed write (FSN_EINVAL naming the file and the cause) leaves no file at path. */
+int fsn_model_file_write(const char* path, const fsn_config* cfg, int32_t n, const char* const* keys, const float* const* h_data,
+                         const int64_t* numel);
+/* Reads and verifies the whole file -- magic, version, bounds, trailing bytes, checksum, config fields, the configuration as
+ * fsn_model_create checks it, the key set and every size -- and returns its configuration, e.g. for fsn_plan_audio or
+ * fsn_stream_state_layout before a GPU is touched.  Host only.  A malformed file is FSN_EINVAL with a message naming the file and what
+ * is wrong (for a truncation, the byte offset); a configuration create refuses gives create's code and message. */
+int fsn_model_file_config(const char* path, fsn_config* cfg);
+/* The same verification, then fsn_model_create, fsn_model_set_param for every record and fsn_model_finalize: a finalized handle whose
+ * fsn_model_weights_id equals that of any handle built from the same configuration and parameters (so sessions saved from a handle
+ * built in Python load into it).  *out is set to NULL first and stays NULL on any error; no handle leaks. */
+int fsn_model_load(const char* path, fsn_model** out);
+
 /* Replaces FullSubNet_Plus.forward(noisy_mag, noisy_real, noisy_imag) (fullsubnet_plus.py:122-209) and
  * Model.forward(noisy_mag) (fullsubnet.py:68-118; pass d_real = d_imag = NULL).
  * Inputs: [B, 1, F, T] float32, contiguous, device.  Output: [B, output_size, F, T] float32, contiguous,

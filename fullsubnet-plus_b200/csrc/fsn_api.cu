@@ -6,6 +6,7 @@
 
 #include <algorithm>
 #include <cerrno>
+#include <cmath>
 #include <cstdarg>
 #include <cstddef>
 #include <cstdio>
@@ -2792,6 +2793,155 @@ extern "C" int fsn_stream_step_audio_chunk(fsn_stream* st, const float* d_sample
     if (!h_hops) return fail(FSN_EINVAL, "h_hops is null (one hop count per slot, slots 0..%d)", st->B - 1);
     if (!h_nout) return fail(FSN_EINVAL, "h_nout is null (one result per slot, slots 0..%d)", st->B - 1);
     return step_audio(st, d_samples, K, h_flags, h_hops, d_out, h_nout, d_mask, static_cast<cudaStream_t>(stream));
+}
+
+// ---------------------------------------------------------------------------------------------
+// overlapped-chunk sessions (DESIGN.md §3.16): the reference's overlapped_chunk inferencer (inferencer.py:191-250) per slot, every
+// chunk completed in a call enhanced in one offline audio forward
+// ---------------------------------------------------------------------------------------------
+static const int CHUNK_PRE = 256;                      // P: the reference's pre-context, in samples at every geometry
+
+// Per slot on the host: n = samples of the session so far (-1: no session) and k = its chunks enhanced; chunk k covers session samples
+// [k H - P, k H + C), and y[0, k H) has been emitted (all of y[0, L) once the session has ended).  On the device: the sample ring
+// [B, C + P], the overlap tail [B, H] and the window [C]; the plan and the batch's rows are per call, grow-only.
+struct fsn_chunk_stream {
+    fsn_model* m;
+    int B, C;
+    std::vector<int64_t> n, k;
+    DevBuf ring, tail, window, plan, rows, enh;
+    PinnedStage stage;
+};
+
+// The plan of slot b for flag f and count c (CP_* fields into p), and its n and k after the call.  Checks the flag and the count.
+static int chunk_slot_plan(const fsn_chunk_stream* cs, int b, int f, int c, int S, int row0, int32_t* p, int64_t* n1, int64_t* k1) {
+    const int H = cs->C / 2;
+    if (f < FSN_SLOT_HOLD || f > FSN_SLOT_FLUSH)
+        return fail(FSN_EINVAL, "slot %d: flag %d is not FSN_SLOT_HOLD (0), FSN_SLOT_STEP (1), FSN_SLOT_START (2) or FSN_SLOT_FLUSH (3)", b, f);
+    for (int i = 0; i < CHUNK_PLAN_FIELDS; ++i) p[i] = 0;
+    p[CP_ROW0] = row0;
+    *n1 = cs->n[b]; *k1 = cs->k[b];
+    if (f == FSN_SLOT_HOLD) return FSN_OK;
+    const char* name = f == FSN_SLOT_START ? "START" : f == FSN_SLOT_STEP ? "STEP" : "FLUSH";
+    if (c < 0 || c > S) return fail(FSN_EINVAL, "slot %d: h_counts = %d: a %s consumes 0 to S = %d samples", b, c, name, S);
+    if (f != FSN_SLOT_START && cs->n[b] < 0) return fail(FSN_EINVAL, "slot %d: %s on a slot without a session (START one first)", b, name);
+    const int64_t n0 = f == FSN_SLOT_START ? 0 : cs->n[b], k0 = f == FSN_SLOT_START ? 0 : cs->k[b], a0 = k0 * H, n = n0 + c;
+    // chunk k is complete once the input reaches k H + C; at FLUSH every chunk that starts before the end is, zero-padded
+    const int64_t kend = f == FSN_SLOT_FLUSH ? (n + H - 1) / H : std::max(k0, n / H - 1);
+    p[CP_NC] = (int32_t)(kend - k0);
+    p[CP_REL0] = (int32_t)(n0 - a0);
+    p[CP_REL1] = (int32_t)(n - a0);
+    p[CP_LO] = k0 ? -CHUNK_PRE : 0;
+    p[CP_PHASE] = (int32_t)(a0 % (cs->C + CHUNK_PRE));
+    p[CP_NOUT] = (int32_t)(f == FSN_SLOT_FLUSH ? n - a0 : (kend - k0) * H);
+    *n1 = f == FSN_SLOT_FLUSH ? -1 : n;
+    *k1 = f == FSN_SLOT_FLUSH ? 0 : kend;
+    return FSN_OK;
+}
+
+extern "C" int fsn_chunk_stream_create(fsn_model* m, int32_t B, int32_t chunk_samples, fsn_chunk_stream** out) {
+    if (!m) return fail(FSN_EINVAL, "m is null");
+    if (!out) return fail(FSN_EINVAL, "out is null");
+    if (B < 1) return fail(FSN_EINVAL, "B = %d: the handle needs at least one slot", B);
+    if (!m->finalized) return fail(FSN_ESTATE, "fsn_model_finalize has not been called");
+    const int C = chunk_samples;
+    if (C < 2 || C % 2) return fail(FSN_EINVAL, "chunk_samples = %d: the chunk length must be even (two halves of 50 %% overlap)", C);
+    if (C / 2 < CHUNK_PRE)
+        return fail(FSN_EINVAL, "chunk_samples = %d: the half-chunk %d is shorter than the %d-sample pre-context (chunk_samples >= %d)", C,
+                    C / 2, CHUNK_PRE, 2 * CHUNK_PRE);
+    if ((long long)C > 0x3fffffffLL - CHUNK_PRE)
+        return fail(FSN_EINVAL, "chunk_samples = %d exceeds 2^30 - 1 - %d samples", C, CHUNK_PRE);
+    // every batch of the step is fsn_model_enhance_audio on rows of P + C samples: refused here with that call's message
+    int T = 0, Lmax = 0;
+    bool all = true;
+    int rc = audio_check(m->cfg, 1, (int64_t)CHUNK_PRE + C, nullptr, &T, &Lmax, &all);
+    if (!rc && m->cfg.output_size != 2) rc = fail(FSN_EINVAL, "the audio call needs output_size 2 (a complex mask)");
+    if (rc) {
+        char why[512];
+        snprintf(why, sizeof(why), "%s", g_err);
+        return fail(rc, "chunk_samples = %d: fsn_model_enhance_audio refuses rows of %d + %d samples: %s", C, CHUNK_PRE, C, why);
+    }
+    fsn_chunk_stream* cs = new fsn_chunk_stream();
+    cs->m = m; cs->B = B; cs->C = C;
+    cs->n.assign(B, -1);
+    cs->k.assign(B, 0);
+    std::vector<float> w(C);
+    const double pi = std::acos(-1.0);
+    for (int i = 0; i < C; ++i) w[i] = (float)(0.5 - 0.5 * std::cos(2.0 * pi * i / C));   // torch.hann_window(C), periodic
+    int e = cs->ring.ensure((size_t)B * (C + CHUNK_PRE) * sizeof(float), true);
+    e |= cs->tail.ensure((size_t)B * (C / 2) * sizeof(float), true);
+    e |= cs->window.ensure((size_t)C * sizeof(float), false);
+    e |= cs->plan.ensure((size_t)B * CHUNK_PLAN_FIELDS * sizeof(int32_t), false);
+    if (e || cudaMemcpy(cs->window.p, w.data(), (size_t)C * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) {
+        fsn_chunk_stream_destroy(cs);
+        return fail(FSN_ECUDA, "chunk stream state allocation failed (B = %d, chunk_samples = %d)", B, C);
+    }
+    *out = cs;
+    return FSN_OK;
+}
+
+extern "C" void fsn_chunk_stream_destroy(fsn_chunk_stream* cs) {
+    if (!cs) return;
+    for (DevBuf* b : {&cs->ring, &cs->tail, &cs->window, &cs->plan, &cs->rows, &cs->enh}) b->release();
+    delete cs;
+}
+
+// Every slot's plan is made and checked, then the batch of the completed chunks is checked as the offline audio call, before anything
+// is allocated, staged or launched.  Then: the gather, the forward (run_plain: it waits for pipelined batches and plans sub-batches
+// under the cap as fsn_model_enhance_audio does; none when no chunk completes), the cross-fade, and the host counters.
+extern "C" int fsn_chunk_stream_step(fsn_chunk_stream* cs, const float* d_samples, int32_t S, const int32_t* h_flags,
+                                     const int32_t* h_counts, float* d_out, int32_t* h_nout, void* stream) {
+    if (!cs) return fail(FSN_EINVAL, "cs is null");
+    const int B = cs->B, C = cs->C, W = C + CHUNK_PRE;
+    if (!d_samples) return fail(FSN_EINVAL, "d_samples is null ([B, S] float32 on the device)");
+    if (!d_out) return fail(FSN_EINVAL, "d_out is null ([B, S + chunk_samples] float32 on the device)");
+    if (!h_flags) return fail(FSN_EINVAL, "h_flags is null (one flag per slot, slots 0..%d)", B - 1);
+    if (!h_counts) return fail(FSN_EINVAL, "h_counts is null (one sample count per slot, slots 0..%d)", B - 1);
+    if (!h_nout) return fail(FSN_EINVAL, "h_nout is null (one result per slot, slots 0..%d)", B - 1);
+    if (S < 1) return fail(FSN_EINVAL, "S = %d: a row needs at least one sample", S);
+    if ((long long)S + 2LL * W > 0x7fffffffLL)
+        return fail(FSN_EINVAL, "S = %d: S + 2 (chunk_samples + %d) exceeds 2^31 - 1", S, CHUNK_PRE);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    std::vector<int32_t> plan((size_t)B * CHUNK_PLAN_FIELDS);
+    std::vector<int64_t> n1(B), k1(B);
+    int nrows = 0;
+    for (int b = 0; b < B; ++b) {
+        int32_t* p = plan.data() + (size_t)b * CHUNK_PLAN_FIELDS;
+        if (int rc = chunk_slot_plan(cs, b, h_flags[b], h_counts[b], S, nrows, p, &n1[b], &k1[b])) return rc;
+        if ((long long)nrows + p[CP_NC] > 0x7fffffffLL / W) return fail(FSN_EINVAL, "more than 2^31 - 1 samples of chunk rows in one call");
+        nrows += p[CP_NC];
+    }
+    // the batch of every completed chunk: rows [nrows, P + C]; the caller's buffers stand in for the rows until they are allocated
+    Batch fwd{CALL_AUDIO, nullptr, nullptr, nullptr, nrows, 0, nullptr, nullptr, nullptr, d_samples, d_out, W, nullptr};
+    std::vector<int32_t> lens;
+    if (nrows)
+        if (int rc = check_batch(cs->m, fwd, &lens)) return rc;
+    const size_t rb = (size_t)nrows * W * sizeof(float);
+    int e = nrows ? cs->rows.ensure(rb, false, s) | cs->enh.ensure(rb, false, s) : 0;
+    if (e) return fail(FSN_ECUDA, "chunk row allocation failed (%d rows of %d samples)", nrows, W);
+    int32_t* h = nullptr;
+    if (int rc = cs->stage.take(plan.size(), &h)) return rc;
+    memcpy(h, plan.data(), plan.size() * sizeof(int32_t));
+    if (int rc = cs->stage.send(cs->plan.p, plan.size(), s)) return rc;
+    ChunkStreamLaunch a{};
+    a.plan = static_cast<const int*>(cs->plan.p);
+    a.samples = d_samples; a.out = d_out;
+    a.ring = static_cast<float*>(cs->ring.p); a.tail = static_cast<float*>(cs->tail.p);
+    a.rows = static_cast<float*>(cs->rows.p); a.enh = static_cast<const float*>(cs->enh.p);
+    a.window = static_cast<const float*>(cs->window.p);
+    a.B = B; a.S = S; a.C = C; a.P = CHUNK_PRE;
+    launch_chunk_gather(a, s);
+    CK(cudaGetLastError());
+    if (nrows) {
+        fwd.wave = a.rows; fwd.wave_out = static_cast<float*>(cs->enh.p);
+        if (int rc = run_plain(cs->m, fwd, s)) return rc;
+    }
+    launch_chunk_crossfade(a, s);
+    CK(cudaGetLastError());
+    for (int b = 0; b < B; ++b) {
+        cs->n[b] = n1[b]; cs->k[b] = k1[b];
+        h_nout[b] = plan[(size_t)b * CHUNK_PLAN_FIELDS + CP_NOUT];
+    }
+    return FSN_OK;
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -209,6 +209,25 @@ inline AudioTables audio_table_ptrs(const float* tab, int n_fft) {
     return {tab, reinterpret_cast<const float2*>(tab + n_fft), tab + n_fft + 2 * (H + 1), tab + n_fft + 2 * (H + 1) + H};
 }
 
+// ---- k_chunk_stream.cu: overlapped-chunk sessions around the offline audio forward (fsn_chunk_stream_step, DESIGN.md §3.16) -------
+// The per-slot plan, CHUNK_PLAN_FIELDS int32 per slot: the chunks this call completes (nc, at batch rows row0 .. row0 + nc - 1), the
+// slot's samples relative to its next chunk's start a0 = k0 H (ring below rel0, the call's row in [rel0, rel1), zero below lo and
+// from rel1 on), the ring position of a0 (phase) and the samples emitted (nout).  lo = 0 exactly when that next chunk is chunk 0.
+enum { CP_NC, CP_ROW0, CP_REL0, CP_REL1, CP_LO, CP_PHASE, CP_NOUT, CHUNK_PLAN_FIELDS };
+struct ChunkStreamLaunch {
+    const int* plan;          // [B, CHUNK_PLAN_FIELDS] device
+    const float* samples;     // [B, S] this call's samples at the front of each row
+    float* ring;              // [B, C + P] the slot's last C + P samples, sample p at p mod (C + P)
+    float* rows;              // [n, P + C] the completed chunks' input rows (gather output, the forward's input)
+    const float* enh;         // [n, P + C] the forward's output rows
+    float* tail;              // [B, C / 2] the windowed second half of the slot's last enhanced chunk
+    const float* window;      // [C] periodic Hann window
+    float* out;               // [B, S + C] emitted samples at the front of each row, zero after them
+    int B, S, C, P;
+};
+void launch_chunk_gather(const ChunkStreamLaunch& a, cudaStream_t s);
+void launch_chunk_crossfade(const ChunkStreamLaunch& a, cudaStream_t s);
+
 // ---- k_lstm_mma.cu ---------------------------------------------------------------------------
 struct LstmMmaWeights {       // device, produced by pack (fsn_api.cu)
     const uint4* wfrag[4];    // per layer: [H/8 groups][K/16][32 lanes][2 x uint4]

@@ -27,6 +27,7 @@ SYMBOLS = [
     "fsn_model_enhance_audio", "fsn_plan_audio",
     "fsn_stream_step_chunk", "fsn_stream_chunk_plan", "fsn_stream_step_audio_chunk",
     "fsn_model_file_write", "fsn_model_file_config", "fsn_model_load",
+    "fsn_chunk_stream_create", "fsn_chunk_stream_step", "fsn_chunk_stream_destroy",
 ]
 
 
@@ -177,6 +178,10 @@ def load_library():
     lib.fsn_model_file_write.argtypes = [C.c_char_p, C.POINTER(FsnConfig), i32, C.POINTER(C.c_char_p), C.POINTER(vp), C.POINTER(i64)]
     lib.fsn_model_file_config.argtypes = [C.c_char_p, C.POINTER(FsnConfig)]
     lib.fsn_model_load.argtypes = [C.c_char_p, C.POINTER(vp)]
+    lib.fsn_chunk_stream_create.argtypes = [vp, i32, i32, C.POINTER(vp)]
+    lib.fsn_chunk_stream_step.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp]
+    lib.fsn_chunk_stream_destroy.argtypes = [vp]
+    lib.fsn_chunk_stream_destroy.restype = None
     _LIB = lib
     return lib
 

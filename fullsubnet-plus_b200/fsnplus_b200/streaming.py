@@ -20,6 +20,10 @@ many ``step_audio`` ticks on the slot (DESIGN.md §3.14).  A handle serves eithe
 ``save_slots`` / ``load_slots`` park, resume and move sessions (DESIGN.md §3.11): a ``SessionState`` holds the saved state of some
 slots, and loading it into any slot of a handle of the same model -- this one, one with another B, or one on another GPU -- continues
 each session where it was saved.
+
+``ChunkStream`` serves live audio to the models that cannot stream frame by frame -- FullSubNet+ and ``Model`` with an offline norm --
+by the reference's overlapped-chunk inferencer: chunks of C samples with 50 % overlap, each enhanced by the offline audio call, the
+halves cross-faded with a Hann window; the latency is C / 2 to C samples (DESIGN.md §3.16).
 """
 import ctypes as C
 
@@ -236,6 +240,56 @@ class StreamingFullSubNet:
         if self._st is not None:
             self.lib.fsn_stream_destroy(self._st)
             self._st = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class ChunkStream:
+    """Live audio for any model ``enhance_audio`` runs -- FullSubNet+ (any attention, norm or sub-band model) and ``Model`` with any
+    norm -- by the reference's overlapped-chunk inferencer (DESIGN.md §3.16; C: ``fsn_chunk_stream_*``).  Each of the B slots serves
+    its own session: its input is cut into chunks of ``chunk_samples`` (C, even) with 50 % overlap and 256 samples of pre-context,
+    each chunk is enhanced by the offline audio call, and the halves are cross-faded with a periodic Hann window of C.  Every chunk
+    completed by every slot in one ``step`` runs as one batch.  The output lags the input by C / 2 to C samples."""
+
+    def __init__(self, model, batch_size=1, chunk_samples=16000, device="cuda:0"):
+        self.model, self.B, self.C, self.device = model, batch_size, chunk_samples, torch.device(device)
+        model._check_call()
+        with torch.cuda.device(self.device):
+            self.lib = model._ensure_handle(self.device)
+            h = C.c_void_p()
+            _lib.check(self.lib.fsn_chunk_stream_create(model._handle, batch_size, chunk_samples, C.byref(h)))
+        self._cs = h
+
+    def step(self, samples, counts, flags):
+        """One call.  samples [B, S] float32 CUDA: slot b's counts[b] new samples at the front of its row (nothing else is read);
+        counts, flags: B values each (sequences or CPU integer tensors), flags HOLD / STEP / START / FLUSH (FLUSH consumes, then ends
+        the session).  Returns (out [B, S + C], nout int32 CPU tensor [B]): slot b's nout[b] newly final output samples at the front
+        of its row, zero after them.  A session's outputs concatenated over its calls are its enhanced audio, as long as its input."""
+        assert samples.dim() == 2 and samples.shape[0] == self.B and samples.is_cuda
+        S = samples.shape[1]
+        f = torch.as_tensor(flags, dtype=torch.int32)
+        n = torch.as_tensor(counts, dtype=torch.int32)
+        assert f.device.type == "cpu" and f.shape == (self.B,), "flags: B host values"
+        assert n.device.type == "cpu" and n.shape == (self.B,), "counts: B host values"
+        f, n = f.contiguous(), n.contiguous()
+        x = samples.contiguous().float()
+        out = torch.empty((self.B, S + self.C), dtype=torch.float32, device=self.device)
+        nout = torch.zeros(self.B, dtype=torch.int32)
+        with torch.cuda.device(self.device):
+            stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+            _lib.check(self.lib.fsn_chunk_stream_step(self._cs, C.c_void_p(x.data_ptr()), S, C.c_void_p(f.data_ptr()),
+                                                      C.c_void_p(n.data_ptr()), C.c_void_p(out.data_ptr()),
+                                                      C.c_void_p(nout.data_ptr()), stream))
+        return out, nout
+
+    def close(self):
+        if self._cs is not None:
+            self.lib.fsn_chunk_stream_destroy(self._cs)
+            self._cs = None
 
     def __del__(self):
         try:

@@ -317,6 +317,34 @@ int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_samples, float* d
 int fsn_stream_step_audio_chunk(fsn_stream* st, const float* d_samples, int32_t K, const int32_t* h_flags, const int32_t* h_hops,
                                 float* d_out, int32_t* h_nout, float* d_mask, void* stream);
 
+/* Overlapped-chunk sessions (DESIGN.md §3.16): live audio for any model fsn_model_enhance_audio runs -- FullSubNet+ with any attention
+ * and norm, the sub-band TCN, fullsubnet.Model with any norm -- by the reference's overlapped_chunk inferencer
+ * (fullsubnet_plus/inferencer/inferencer.py:191-250).  With C = chunk_samples (even), H = C / 2, P = 256 samples of pre-context and
+ * w = torch.hann_window(C) (periodic), a session's input x[0, L) is cut into chunks k = 0 .. ceil(L / H) - 1 of rows
+ * x[k H - P, k H + C) (zero before 0 and past L), each enhanced by fsn_model_enhance_audio, its first P output samples dropped: e_k.
+ * Output region y[k H, (k + 1) H) is e_0[0, H) for k = 0 and e_k[0, H) w[0, H) + e_{k-1}[H, C) w[H, C) after it; the output is y[0, L).
+ * Chunk k completes once the input reaches k H + C (at FLUSH: every chunk, zero-padded), and region k is emitted with it, so the
+ * output lags the input by H to 2H samples.  Every chunk completed by every slot in one call runs as ONE batch of rows of P + C
+ * samples through the offline audio call (sub-batches under FSN_WS_CAP_GB, fsn_plan_audio; no forward when none completes).
+ * fsn_chunk_stream_create: FSN_EINVAL naming the argument for a null m or out and B < 1; naming the limit for an odd C, H < P, and
+ * rows of P + C samples that fsn_model_enhance_audio refuses for this model (its message); FSN_ESTATE before fsn_model_finalize.  The
+ * handle keeps per slot a ring of C + P samples and a tail of H samples, and the window, allocated here; the staged plan and the
+ * batch's rows are allocated at first use, grow-only.  fsn_chunk_stream_destroy frees them all.
+ * fsn_chunk_stream_step: d_samples [B, S] float32 device, slot b reading its first h_counts[b] samples (0 <= h_counts[b] <= S; no other
+ * sample is read).  h_flags (HOST, B values of FSN_SLOT_*): HOLD no samples, no change (h_counts ignored); START resets the slot,
+ * then consumes; STEP consumes; FLUSH consumes, then ends the session (the remaining chunks are enhanced and y through L is emitted),
+ * leaving the slot without a session.  d_out [B, S + C] float32 device: each slot's newly final samples at the front of its row,
+ * zero after them; h_nout (HOST, [B]) their count.  A session's outputs concatenated over its calls are y[0, L).
+ * FSN_EINVAL naming the slot for a flag outside {0, 1, 2, 3}, a count outside [0, S], a STEP or FLUSH on a slot without a session;
+ * naming the argument for a null array and S < 1; naming the limit for S + 2 (C + P) past 2^31 - 1 and for chunk rows of more than
+ * 2^31 - 1 samples in one call.  A failed call changes no state.
+ * The host arrays are free when the call returns; the call does not synchronise the stream. */
+typedef struct fsn_chunk_stream fsn_chunk_stream;
+int fsn_chunk_stream_create(fsn_model* m, int32_t B, int32_t chunk_samples, fsn_chunk_stream** out);
+int fsn_chunk_stream_step(fsn_chunk_stream* cs, const float* d_samples, int32_t S, const int32_t* h_flags, const int32_t* h_counts,
+                          float* d_out, int32_t* h_nout, void* stream);
+void fsn_chunk_stream_destroy(fsn_chunk_stream* cs);
+
 /* Park, resume and move sessions (DESIGN.md §3.11): save the state of some slots to a device buffer and load it into any slot of a
  * compatible handle -- the same one, another with a different B or full-band kernel, or one on another device after the caller has
  * copied the payload there.

@@ -1041,6 +1041,9 @@ static WsSizes ws_sizes(const fsn_config& c, bool layerwise, int B, int T, int T
     const int nbr = (c.model_kind == FSN_KIND_PLUS) ? 3 : 1;
     const size_t rows = (size_t)B * F, ntiles = ((rows + 127) / 128 + 1) / 2 * 2;   // whole pairs of 128-row tiles (clusters of k_lstm_tc5r.cu)
     z.fbin = z.fbout = (size_t)nbr * B * F * Pp * 4;
+    // fbout is also input_norm_kernel's per-frame scratch: it runs before anything writes or reads the full-band outputs (front_end).
+    // num_freqs >= 4 makes the scratch (16 bytes per frame) fit within fbout's F * Pp * 4 bytes; the max keeps that explicit.
+    if (c.norm_type != FSN_NORM_OFFLINE_LAPLACE) z.fbout = std::max(z.fbout, input_norm_frames_bytes(nbr, B, Tp));
     z.mu = z.sigma = (size_t)B * 4;
     z.tsse_scale = (size_t)nbr * B * F * 4 * (1 + tsse_row_floats());          // per-row scale | row statistics
     z.sb_rowsum = (size_t)B * 4 * F * 2 * 4;
@@ -1107,7 +1110,7 @@ struct WsBuf {
 #define MODEL_BUF(f) [](fsn_model& m, Lane&) -> DevBuf& { return m.f; }
 static const WsBuf WS[] = {
     {LANE_BUF(fbin), &WsSizes::fbin, WS_LANE | WS_ZERO},
-    {LANE_BUF(fbout), &WsSizes::fbout, WS_LANE | WS_ZERO},
+    {LANE_BUF(fbout), &WsSizes::fbout, WS_LANE | WS_ZERO},                         // first input_norm_kernel's scratch (ws_sizes)
     {LANE_BUF(mu), &WsSizes::mu, WS_LANE | WS_ZERO},
     {LANE_BUF(sigma), &WsSizes::sigma, WS_LANE | WS_ZERO},
     {LANE_BUF(tsse_scale), &WsSizes::tsse_scale, WS_LANE | WS_ZERO},
@@ -1372,10 +1375,12 @@ static int sb_layers(fsn_model* m, const LstmTc5rLaunch& a, __half* gin, size_t 
 
 // The sub-band LSTM / GRU's input images of the frames sp names (a wide input: plain rows of 128 halves, time-major for the generic
 // kernel): the whole clip's, a window's, or the test hook's raw input
-static void pack_images(fsn_model* m, const SbPackLaunch& sp, cudaStream_t s) {
-    if (sb_wide(m->cfg)) launch_sb_pack_wide(sp, !m->layerwise, s);
-    else launch_sb_pack(sp, s);
+static int pack_images(fsn_model* m, const SbPackLaunch& sp, cudaStream_t s) {
+    cudaError_t e = cudaSuccess;
+    const char* k = sb_wide(m->cfg) ? launch_sb_pack_wide(sp, !m->layerwise, s, &e) : launch_sb_pack(sp, s, &e);
+    if (k) return fail(FSN_ECUDA, "%s launch failed: %s", k, cudaGetErrorString(e));
     m->launches++;
+    return FSN_OK;
 }
 
 // b.enh != null: write the enhanced spectrum (decompress_cIRM x noisy) instead of the mask -- fused into the epilogue of the
@@ -1397,7 +1402,7 @@ static int run_sb_lstm(fsn_model* m, Lane& ln, const Batch& b, int Tw, SbPackLau
             const int tw = Tw ? (Tp - w0 < Tw ? Tp - w0 : Tw) : Tp;
             if (Tw) {
                 sp.t0 = w0; sp.Tw = tw;
-                pack_images(m, sp, s);
+                if (int rc = pack_images(m, sp, s)) return rc;
             }
             LstmTc5rLaunch a{};
             a.rows = rows; a.Tp = Tp; a.ntiles = ntiles; a.t0 = w0; a.Tw = tw;
@@ -1519,7 +1524,8 @@ static int run_sb_tcn(fsn_model* m, Lane& ln, const Batch& b, int Fc, SbPackLaun
         const int fc = F - f0 < W ? F - f0 : W, Z = B * fc;
         if (Fc) {
             sp.xtm = x; sp.amax = amax0; sp.f0 = f0; sp.Fc = fc;
-            launch_sb_pack_tm(sp, s);
+            cudaError_t e = cudaSuccess;
+            if (const char* k = launch_sb_pack_tm(sp, s, &e)) return fail(FSN_ECUDA, "%s launch failed: %s", k, cudaGetErrorString(e));
             m->launches++;
         }
         CK(cudaMemsetAsync(m->sb_scratch.stats.p, 0, tcn_stats_bytes(Z), s));
@@ -1637,8 +1643,10 @@ static int front_end(fsn_model* m, Lane& ln, const Batch& bt, const int* tl, SbP
     ta.rows = ta.scale + (size_t)nbr * B * F;
     ta.tlen = tl;
     if (c.norm_type != FSN_NORM_OFFLINE_LAPLACE) {
-        const NormLaunch na{{ta.x[0], ta.x[1], ta.x[2]}, static_cast<float*>(ln.xn.p), nbr, B, F, T, Tp, c.norm_type, tl};
-        launch_input_norm(na, s); m->launches++;
+        const NormLaunch na{{ta.x[0], ta.x[1], ta.x[2]}, static_cast<float*>(ln.xn.p), nbr, B, F, T, Tp, c.norm_type, tl,
+                            static_cast<float*>(ln.fbout.p)};            // scratch: the full-band outputs are written later
+        if (cudaError_t e = launch_input_norm(na, s)) return fail(FSN_ECUDA, "input_norm_kernel launch failed: %s", cudaGetErrorString(e));
+        m->launches++;
         for (int b = 0; b < nbr; ++b) ta.x[b] = static_cast<const float*>(ln.xn.p) + (size_t)b * B * F * Tp;
         ta.T = Tp; ta.prenorm = 1;                                      // padded frames are part of the normalised signal
     }
@@ -1651,7 +1659,9 @@ static int front_end(fsn_model* m, Lane& ln, const Batch& bt, const int* tl, SbP
         CK(cudaMemsetAsync(ln.tcn.stats.p, 0, tcn_stats_bytes(3 * B), s));
         ta.amax = tcn_amax(ln.tcn.stats.p, 3 * B, 0);                  // block 0: written by the gate kernel
     }
-    launch_tsse_norm(ta, s); m->launches += 3;
+    cudaError_t e = cudaSuccess;
+    if (const char* k = launch_tsse_norm(ta, s, &e)) return fail(FSN_ECUDA, "%s launch failed: %s", k, cudaGetErrorString(e));
+    m->launches += 3;
 
     if (plus) {
         const TcnWeights& w = m->tcn_fb;
@@ -1664,8 +1674,8 @@ static int front_end(fsn_model* m, Lane& ln, const Batch& bt, const int* tl, SbP
         g3.epi = EPI5_OUT; g3.Kp = w.Cp; g3.NT = w.NT; g3.ntiles_n = w.ntiles; g3.Npad = w.Cp;
         for (int b = 0; b < 3; ++b) g3.bias[b] = static_cast<const float*>(m->fb_fc_b.p) + (size_t)b * w.Cp;
         g3.out = static_cast<float*>(ln.fbout.p); g3.F = F; g3.P = Pp; g3.act = c.fb_act;    // finite past each clip's end; the sub-band stages mask it
-        int e = launch_gemm_tc5(ln.mapXr, m->map_fb_fc, g3, m->num_sms, s);
-        if (e) return fail(FSN_ECUDA, "TCN output GEMM launch failed: %s", cudaGetErrorString((cudaError_t)e));
+        const int eo = launch_gemm_tc5(ln.mapXr, m->map_fb_fc, g3, m->num_sms, s);
+        if (eo) return fail(FSN_ECUDA, "TCN output GEMM launch failed: %s", cudaGetErrorString((cudaError_t)eo));
         m->launches++;
 
         sp.win = static_cast<const float*>(ln.fbin.p); sp.Pw = Pp;      // post-attention mag branch (fullsubnet_plus.py:182)
@@ -1691,22 +1701,25 @@ static int front_end(fsn_model* m, Lane& ln, const Batch& bt, const int* tl, SbP
         sp.win = static_cast<const float*>(ln.magpad.p); sp.Pw = Pp;    // raw padded magnitude (fullsubnet.py:94)
         sp.fb[0] = static_cast<const float*>(ln.fbout.p);
     }
-    launch_sb_stats(sp, s); m->launches += 2;
+    if (const char* k = launch_sb_stats(sp, s, &e)) return fail(FSN_ECUDA, "%s launch failed: %s", k, cudaGetErrorString(e));
+    m->launches += 2;
     return FSN_OK;
 }
 
 // The whole clip's sub-band input on stream s, unless the sub-band stage packs it itself: window by window (Tw, run_sb_lstm) or chunk
 // by chunk (Fc, run_sb_tcn)
-static void pack_clip(fsn_model* m, Lane& ln, SbPackLaunch sp, int Tw, int Fc, cudaStream_t s) {
+static int pack_clip(fsn_model* m, Lane& ln, SbPackLaunch sp, int Tw, int Fc, cudaStream_t s) {
     if (m->cfg.sb_tcn) {
-        if (Fc) return;
+        if (Fc) return FSN_OK;
         sp.xtm = static_cast<float*>(ln.sbx.p);
         sp.amax = sp.xtm + (size_t)sp.B * sp.F * sp.Tp * 64;
-        launch_sb_pack_tm(sp, s);
+        cudaError_t e = cudaSuccess;
+        if (const char* k = launch_sb_pack_tm(sp, s, &e)) return fail(FSN_ECUDA, "%s launch failed: %s", k, cudaGetErrorString(e));
         m->launches++;
     } else if (!Tw) {
-        pack_images(m, sp, s);
+        return pack_images(m, sp, s);
     }
+    return FSN_OK;
 }
 
 // The sub-band stage on stream sl: the LSTM / GRU or the TCN over the packed input (sp: the packer's arguments, for windows and chunks)
@@ -1729,8 +1742,7 @@ static int forward_impl(fsn_model* m, Lane& ln, const Batch& in, cudaStream_t s,
     AudioLaunch al{};
     if (in.wave) audio_analysis(m, ln, b, al, s);
     SbPackLaunch sp = pack_args(m, ln, b.B, b.T, Tw, tl);
-    if ((rc = front_end(m, ln, b, tl, sp, s))) return rc;
-    pack_clip(m, ln, sp, Tw, Fc, s);
+    if ((rc = front_end(m, ln, b, tl, sp, s)) || (rc = pack_clip(m, ln, sp, Tw, Fc, s))) return rc;
     cudaEventRecord(m->evf1[evi], s);
     if (sl != s) {                                                      // pipelined: the LSTM stream picks the lane up when the front end is done
         CK(cudaEventRecord(ln.ev_front, s));
@@ -1981,8 +1993,7 @@ extern "C" int fsn_model_sb_forward(fsn_model* m, const float* d_x, int32_t B, i
     Lane& ln = m->lane[0];
     SbPackLaunch sp = pack_args(m, ln, B, T, Tw, tl);
     sp.raw = d_x;
-    pack_clip(m, ln, sp, Tw, 0, s);
-    if ((rc = sub_band(m, ln, b, Tw, 0, sp, tl, s))) return rc;
+    if ((rc = pack_clip(m, ln, sp, Tw, 0, s)) || (rc = sub_band(m, ln, b, Tw, 0, sp, tl, s))) return rc;
     CK(cudaGetLastError());
     return FSN_OK;
 }
@@ -2117,6 +2128,14 @@ extern "C" int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst,
         if (numel != (int64_t)B * F * m->Isb * Tp) return fail(FSN_EINVAL, "sb_in needs %lld elements", (long long)B * F * m->Isb * Tp);
         launch_tm_to_fm(static_cast<const float*>(ln.sbx.p), 64, d_dst, B * F, m->Isb, Tp, s);
         CK(cudaGetLastError());
+        return FSN_OK;
+    }
+    if (n == "sb_img") {
+        if (c.sb_tcn) return fail(FSN_EINVAL, "sb_img is the LSTM / GRU's input: the sub-band TCN keeps sb_in instead");
+        if (ln.geo.Tw) return fail(FSN_ESTATE, "sb_img is not kept: the last forward packed the images in windows (%d frames each), its buffer holds the last window only", ln.geo.Tw);
+        const size_t bytes = ws_sizes(c, m->layerwise, B, ln.geo.T, 0).ximg;
+        if (numel * 4 != (int64_t)bytes) return fail(FSN_EINVAL, "sb_img needs %lld elements", (long long)(bytes / 4));
+        CK(cudaMemcpyAsync(d_dst, ln.ximg.p, bytes, cudaMemcpyDeviceToDevice, s));
         return FSN_OK;
     }
     if (n == "stft" || n == "enh") {

@@ -50,10 +50,16 @@ struct TsseLaunch {
     const int* tlen;           // optional [nbranch, B] per-sample extent frames[b] + look_ahead (clip_len); null: every sample spans Tp
 };
 inline size_t tsse_row_floats() { return 3 + 2 * 16; }
-void launch_tsse_norm(const TsseLaunch& a, cudaStream_t s);
-// norm types other than offline_laplace_norm (reference base_model.py:227-316): y[nbranch, B, F, Tp] = norm(pad(x))
-struct NormLaunch { const float* x[3]; float* y; int nbranch, B, F, T, Tp, type; const int* tlen; };   // tlen: as TsseLaunch
-void launch_input_norm(const NormLaunch& a, cudaStream_t s);
+// dynamic shared memory of tsse_norm_kernel in bytes at F bins: 5 F + F / 2 + 8 floats (46 KB at F = 2048)
+size_t tsse_norm_smem(int F);
+// The front end's launchers return null, or the name of the kernel whose launch (or cudaFuncSetAttribute) failed with *err
+const char* launch_tsse_norm(const TsseLaunch& a, cudaStream_t s, cudaError_t* err);
+// norm types other than offline_laplace_norm (reference base_model.py:227-316): y[nbranch, B, F, Tp] = norm(pad(x)).  frames: scratch
+// [nbranch, B, 4, Tp] floats (per-frame sums, sums of squares, scale and shift), input_norm_frames_bytes; the forward lends it the
+// lane's full-band output buffer, which is written only after the input norm has run
+struct NormLaunch { const float* x[3]; float* y; int nbranch, B, F, T, Tp, type; const int* tlen; float* frames; };   // tlen: as TsseLaunch
+inline size_t input_norm_frames_bytes(int nbranch, int B, int Tp) { return (size_t)nbranch * B * 4 * Tp * sizeof(float); }
+cudaError_t launch_input_norm(const NormLaunch& a, cudaStream_t s);
 
 struct ConvLaunch {          // Y[z] = act(W X[z] + b): output Linear of the full-band LSTM (fullsubnet.Model)
     const float* X;          // [Z, K, P]
@@ -89,14 +95,14 @@ struct SbPackLaunch {
     // unnormalised (frames t0 .. t0 + Tw - 1 of every row of the padded tile pairs; rows >= B*F, columns >= I and frames past tlen zero)
     const float* raw;
 };
-void launch_sb_stats(const SbPackLaunch& a, cudaStream_t s);
-void launch_sb_pack(const SbPackLaunch& a, cudaStream_t s);
+const char* launch_sb_stats(const SbPackLaunch& a, cudaStream_t s, cudaError_t* err);
+const char* launch_sb_pack(const SbPackLaunch& a, cudaStream_t s, cudaError_t* err);
 // a wide sub-band input (64 < I <= 128): the same values as plain fp16 rows of 128 halves, columns >= I zero.  time_major = false:
 // the A operand of layer 0's input-projection GEMM, row (tile * Tw + t - t0) * 128 + r (LstmTc5rLaunch::hseq's order); true: the
 // generic kernel's plain input [Tw, ntiles * 128, 128] (LstmMmaLaunch::xplain, rows_pad = ntiles * 128)
-void launch_sb_pack_wide(const SbPackLaunch& a, bool time_major, cudaStream_t s);
+const char* launch_sb_pack_wide(const SbPackLaunch& a, bool time_major, cudaStream_t s, cudaError_t* err);
 // the same normalised values as launch_sb_pack, written to a.xtm / a.amax instead of the fp16 images
-void launch_sb_pack_tm(const SbPackLaunch& a, cudaStream_t s);
+const char* launch_sb_pack_tm(const SbPackLaunch& a, cudaStream_t s, cudaError_t* err);
 // time-major [Z*Tp, ld] -> [Z, C, Tp] (test hook of the sub-band TCN input)
 void launch_tm_to_fm(const float* x, int ld, float* y, int Z, int C, int Tp, cudaStream_t s);
 // [B, F, T] fp32 (+ zero look-ahead pad) -> zero-padded copy [B, F, P]; with tlen [B], sample b's input ends at tlen[b] - la

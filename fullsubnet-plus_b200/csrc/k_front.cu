@@ -69,10 +69,10 @@ __global__ void __launch_bounds__(1024) tsse_norm_kernel(TsseLaunch a) {
     pdl_wait();
     const int b = blockIdx.x, br = blockIdx.y;
     const int F = a.F, Tp = a.tlen ? a.tlen[br * a.B + b] : a.Tp, T = Tp - (a.Tp - a.T);   // this sample's extent
+    // shared memory: 5 F + F / 2 + 1 floats (tsse_norm_smem).  The exclusive prefix / suffix sums of the first / last KMAX samples stay in
+    // the row statistics (global memory, just written by tsse_rowstats_kernel), read only by the thread of their channel.
     float* S = sm;                                  // [F] row sums
-    float* Pfx = S + F;                             // [F][KMAX]   Pfx[f][j] = sum_{t<j} x[f][t]
-    float* Sfx = Pfx + F * TSSE_KMAX;               // [F][KMAX]   Sfx[f][m] = sum_{t>=Tp-m} x[f][t]
-    float* sq = Sfx + F * TSSE_KMAX;                // [F]
+    float* sq = S + F;                              // [F]
     float* gate = sq + F;                           // [F]
     float* f1 = gate + F;                           // [F/2]
     float* Mx = f1 + (F / 2 + 1);                   // [F] row max / [F] row min (CBAM squeeze)
@@ -80,17 +80,11 @@ __global__ void __launch_bounds__(1024) tsse_norm_kernel(TsseLaunch a) {
     __shared__ float s_inv;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarp = blockDim.x >> 5;
-    {
-        const float* rows = a.rows + ((size_t)br * a.B + b) * F * TSSE_ROWW;
-        for (int e = threadIdx.x; e < F * TSSE_ROWW; e += blockDim.x) {
-            const int f = e / TSSE_ROWW, j = e % TSSE_ROWW;
-            const float v = rows[e];
-            if (j == 0) S[f] = v;
-            else if (j == 1) Mx[f] = v;
-            else if (j == 2) Mn[f] = v;
-            else if (j < 3 + TSSE_KMAX) Pfx[f * TSSE_KMAX + j - 3] = v;
-            else Sfx[f * TSSE_KMAX + j - 3 - TSSE_KMAX] = v;
-        }
+    const float* rows = a.rows + ((size_t)br * a.B + b) * F * TSSE_ROWW;   // [F][TSSE_ROWW]: sum, max, min, prefix sums, suffix sums
+    for (int f = threadIdx.x; f < F; f += blockDim.x) {
+        S[f] = rows[(size_t)f * TSSE_ROWW];
+        Mx[f] = rows[(size_t)f * TSSE_ROWW + 1];
+        Mn[f] = rows[(size_t)f * TSSE_ROWW + 2];
     }
     __syncthreads();
     if (warp == 0) {
@@ -108,6 +102,8 @@ __global__ void __launch_bounds__(1024) tsse_norm_kernel(TsseLaunch a) {
         const float rT = 1.0f / (float)Tp;
         if (kind == FSN_ATTN_TSSE) {                 // attention_model.py:78-104: three depthwise convs, time-averaged, mixed by a 3 -> 1 linear
             for (int c = threadIdx.x; c < F; c += blockDim.x) {
+                const float* Pfx = rows + (size_t)c * TSSE_ROWW + 3;              // Pfx[j] = sum_{t<j} x[c][t]
+                const float* Sfx = Pfx + TSSE_KMAX;                               // Sfx[m] = sum_{t>=Tp-m} x[c][t]
                 float s = p.cat_b[0];
 #pragma unroll
                 for (int i = 0; i < 3; ++i) {
@@ -115,7 +111,7 @@ __global__ void __launch_bounds__(1024) tsse_norm_kernel(TsseLaunch a) {
                     const float rlen = 1.0f / (float)(Tp - k + 1);
                     float acc = 0.f;
                     for (int j = 0; j < k; ++j) {
-                        float wsum = S[c] - Pfx[c * TSSE_KMAX + j] - Sfx[c * TSSE_KMAX + (k - 1 - j)];
+                        float wsum = S[c] - Pfx[j] - Sfx[k - 1 - j];
                         acc = fmaf(p.conv_w[i][c * k + j], wsum, acc);
                     }
                     float feat = fmaxf(fmaf(acc, inv * rlen, p.conv_b[i][c]), 0.f);
@@ -248,12 +244,16 @@ __global__ void __launch_bounds__(256) tsse_apply_kernel(TsseLaunch a) {
         }
 }
 
-void launch_tsse_norm(const TsseLaunch& a, cudaStream_t s) {
-    size_t smem = sizeof(float) * ((size_t)a.F * (5 + 2 * TSSE_KMAX) + a.F / 2 + 8);
-    cudaFuncSetAttribute(tsse_norm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    launch_chain(tsse_rowstats_kernel, dim3((a.nbranch * a.B * a.F + 7) / 8), dim3(256), 0, s, a);
-    launch_chain(tsse_norm_kernel, dim3(a.B, a.nbranch), dim3(1024), smem, s, a);
-    launch_chain(tsse_apply_kernel, dim3((a.P + 31) / 32, (a.F + 31) / 32, a.B * a.nbranch), dim3(256), 0, s, a);
+size_t tsse_norm_smem(int F) { return sizeof(float) * ((size_t)F * 5 + F / 2 + 8); }
+
+const char* launch_tsse_norm(const TsseLaunch& a, cudaStream_t s, cudaError_t* err) {
+    const size_t smem = tsse_norm_smem(a.F);
+    if ((*err = cudaFuncSetAttribute(tsse_norm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem))) return "tsse_norm_kernel";
+    if ((*err = launch_chain(tsse_rowstats_kernel, dim3((a.nbranch * a.B * a.F + 7) / 8), dim3(256), 0, s, a))) return "tsse_rowstats_kernel";
+    if ((*err = launch_chain(tsse_norm_kernel, dim3(a.B, a.nbranch), dim3(1024), smem, s, a))) return "tsse_norm_kernel";
+    if ((*err = launch_chain(tsse_apply_kernel, dim3((a.P + 31) / 32, (a.F + 31) / 32, a.B * a.nbranch), dim3(256), 0, s, a)))
+        return "tsse_apply_kernel";
+    return nullptr;
 }
 
 
@@ -264,10 +264,9 @@ void launch_tsse_norm(const TsseLaunch& a, cudaStream_t s) {
 // One CTA per (sample, branch): per-frame sums over F, a serial fp64 scan over the frames, y = x * a[t] + b[t].
 // =============================================================================================
 __global__ void __launch_bounds__(256) input_norm_kernel(NormLaunch a) {
-    extern __shared__ float sm[];
     const int b = blockIdx.x, br = blockIdx.y, F = a.F, T = a.T, Tp = a.Tp;
     const int Tpe = a.tlen ? a.tlen[br * a.B + b] : Tp, Te = Tpe - (Tp - T);   // this sample's extent: padded, input
-    float* cs = sm;             // [Tp] column sums
+    float* cs = a.frames + ((size_t)br * a.B + b) * 4 * Tp;   // [Tp] column sums (global scratch: any clip length fits)
     float* cq = cs + Tp;        // [Tp] column sums of squares
     float* sa = cq + Tp;        // [Tp] scale
     float* sb = sa + Tp;        // [Tp] shift
@@ -312,10 +311,9 @@ __global__ void __launch_bounds__(256) input_norm_kernel(NormLaunch a) {
     }
 }
 
-void launch_input_norm(const NormLaunch& a, cudaStream_t s) {
-    const size_t smem = sizeof(float) * 4 * a.Tp;
-    cudaFuncSetAttribute(input_norm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    input_norm_kernel<<<dim3(a.B, a.nbranch), 256, smem, s>>>(a);
+cudaError_t launch_input_norm(const NormLaunch& a, cudaStream_t s) {
+    input_norm_kernel<<<dim3(a.B, a.nbranch), 256, 0, s>>>(a);
+    return cudaGetLastError();
 }
 
 // =============================================================================================
@@ -453,9 +451,10 @@ __global__ void __launch_bounds__(256) sb_stats_kernel(SbPackLaunch a) {
     }
 }
 
-void launch_sb_stats(const SbPackLaunch& a, cudaStream_t s) {
-    launch_chain(sb_rowsum_kernel, dim3((a.B * (1 + a.nfb) * a.F + 7) / 8), dim3(256), 0, s, a);
-    launch_chain(sb_stats_kernel, dim3(a.B), dim3(256), 0, s, a);
+const char* launch_sb_stats(const SbPackLaunch& a, cudaStream_t s, cudaError_t* err) {
+    if ((*err = launch_chain(sb_rowsum_kernel, dim3((a.B * (1 + a.nfb) * a.F + 7) / 8), dim3(256), 0, s, a))) return "sb_rowsum_kernel";
+    if ((*err = launch_chain(sb_stats_kernel, dim3(a.B), dim3(256), 0, s, a))) return "sb_stats_kernel";
+    return nullptr;
 }
 
 // Stores of the normalised sub-band input.  Fp16Img: the SWIZZLE_128B images of the LSTM kernels (values clamped to the fp16
@@ -661,17 +660,18 @@ __global__ void __launch_bounds__(128) sb_pack_cum_kernel(SbPackLaunch a) {
     Store::finish(a, row, mx, 32);
 }
 
+// The launchers of the packers return the name of the kernel whose launch failed (and its error in *err), or null
 template <class Store>
-static void sb_pack_go(const SbPackLaunch& a, cudaStream_t s) {
+static const char* sb_pack_go(const SbPackLaunch& a, cudaStream_t s, cudaError_t* err) {
     const int Fn = Store::kChunk ? a.Fc : a.F;
-    if (a.norm_type == FSN_NORM_CUMULATIVE_LAPLACE || a.norm_type == FSN_NORM_CUMULATIVE_LAYER)
+    if (a.norm_type == FSN_NORM_CUMULATIVE_LAPLACE || a.norm_type == FSN_NORM_CUMULATIVE_LAYER) {
         sb_pack_cum_kernel<Store><<<(a.B * Fn + 3) / 4, 128, 0, s>>>(a);
-    else
-    {
-        const size_t smem = sizeof(float) * (SBP_T + 1) * ((SBP_F + 2 * a.Ns) + a.nfb * (SBP_F + 2 * a.Nf));
-        cudaFuncSetAttribute(sb_pack_kernel<Store>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        sb_pack_kernel<Store><<<dim3((a.Tw + SBP_T - 1) / SBP_T, (Fn + SBP_F - 1) / SBP_F, a.B), 256, smem, s>>>(a);
+        return (*err = cudaGetLastError()) ? "sb_pack_cum_kernel" : nullptr;
     }
+    const size_t smem = sizeof(float) * (SBP_T + 1) * ((SBP_F + 2 * a.Ns) + a.nfb * (SBP_F + 2 * a.Nf));
+    if ((*err = cudaFuncSetAttribute(sb_pack_kernel<Store>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem))) return "sb_pack_kernel";
+    sb_pack_kernel<Store><<<dim3((a.Tw + SBP_T - 1) / SBP_T, (Fn + SBP_F - 1) / SBP_F, a.B), 256, smem, s>>>(a);
+    return (*err = cudaGetLastError()) ? "sb_pack_kernel" : nullptr;
 }
 // The raw form (SbPackLaunch::raw): one thread per (row, frame, 8 channels), 8 consecutive threads write one row of a step's image
 // (Store = Fp16Img; 16 threads per row of Fp16Wide)
@@ -695,18 +695,18 @@ __global__ void __launch_bounds__(256) sb_pack_raw_kernel(SbPackLaunch a) {
 }
 
 template <class Store>
-static void sb_pack_any(const SbPackLaunch& a, cudaStream_t s) {
-    if (a.raw) sb_pack_raw_kernel<Store><<<1024, 256, 0, s>>>(a);
-    else sb_pack_go<Store>(a, s);
+static const char* sb_pack_any(const SbPackLaunch& a, cudaStream_t s, cudaError_t* err) {
+    if (!a.raw) return sb_pack_go<Store>(a, s, err);
+    sb_pack_raw_kernel<Store><<<1024, 256, 0, s>>>(a);
+    return (*err = cudaGetLastError()) ? "sb_pack_raw_kernel" : nullptr;
 }
-void launch_sb_pack(const SbPackLaunch& a, cudaStream_t s) { sb_pack_any<Fp16Img>(a, s); }
-void launch_sb_pack_wide(const SbPackLaunch& a, bool time_major, cudaStream_t s) {
-    if (time_major) sb_pack_any<Fp16Wide<true>>(a, s);
-    else sb_pack_any<Fp16Wide<false>>(a, s);
+const char* launch_sb_pack(const SbPackLaunch& a, cudaStream_t s, cudaError_t* err) { return sb_pack_any<Fp16Img>(a, s, err); }
+const char* launch_sb_pack_wide(const SbPackLaunch& a, bool time_major, cudaStream_t s, cudaError_t* err) {
+    return time_major ? sb_pack_any<Fp16Wide<true>>(a, s, err) : sb_pack_any<Fp16Wide<false>>(a, s, err);
 }
-void launch_sb_pack_tm(const SbPackLaunch& a, cudaStream_t s) {
-    cudaMemsetAsync(a.amax, 0, (size_t)a.B * a.Fc * sizeof(float), s);
-    sb_pack_go<Fp32Tm>(a, s);
+const char* launch_sb_pack_tm(const SbPackLaunch& a, cudaStream_t s, cudaError_t* err) {
+    if ((*err = cudaMemsetAsync(a.amax, 0, (size_t)a.B * a.Fc * sizeof(float), s))) return "cudaMemsetAsync of the sub-band TCN's maxima";
+    return sb_pack_go<Fp32Tm>(a, s, err);
 }
 
 __global__ void tm_to_fm_kernel(const float* x, int ld, float* y, int Z, int C, int Tp) {

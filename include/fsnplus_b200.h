@@ -404,6 +404,14 @@ int fsn_apply_cirm(const float* d_crm, const float* d_noisy, float* d_enh, int32
  *   "sb_in"  [B, F, Isb, T+look_ahead]       normalised sub-band input (sub-band TCN only)
  *   "stft"   [3, B, 1, F, T]                 the mag / real / imag planes the audio call's forward read
  *   "enh"    [B, F, T] complex64 (2 floats)  the enhanced spectrum the audio call synthesised
+ *   "sb_img" raw bytes, numel = bytes / 4    the fp16 sub-band input of the LSTM / GRU (not the TCN: FSN_EINVAL) as the last
+ *            forward packed it, with np = ceil(B*F / 128) rounded up to even tiles and T' = T + look_ahead:
+ *              Isb <= 64:                 SWIZZLE_128B images [np, T', 128 rows, 64 halves]: row r's 16-byte chunk k / 8 sits
+ *                                         at chunk (k / 8) ^ (r % 8) of its 128-byte line
+ *              Isb > 64, layer-wise path: rows of 128 halves, sequence `row` at frame t is row ((row / 128) * T' + t) * 128 + row % 128
+ *              Isb > 64, generic kernel:  time-major rows of 128 halves [T', ceil(B*F / 128) * 128, 128] (the rest of the buffer unused)
+ *            (fsn_model_last_lstm_impl tells the path); bytes = np * T' * 128 * (128 or 256).  Rows >= B*F, channels >= Isb and
+ *            frames past a clip's extent are zero.  FSN_ESTATE after a forward that packed the images in time windows.
  * "stft" and "enh" are kept only when the last forward was an audio call that ran as one sub-batch; FSN_ESTATE otherwise. */
 int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst, int64_t numel, void* stream);
 /* Kernels launched by the last forward (bench.py reports it as gpu_launches). */

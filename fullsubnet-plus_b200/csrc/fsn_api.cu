@@ -2276,8 +2276,25 @@ static int state_alloc(fsn_stream* st, unsigned audio, cudaStream_t s) {
     return e;
 }
 
+// stream_state_copy_kernel's work items for the a.nseg segments of a: each layer cut into items of at most `chunk` bytes (32 KB, doubled
+// until the items fit)
+static void state_items(StreamStateLaunch& a) {
+    auto cut = [&](size_t chunk) {
+        int k = 0;
+        for (int i = 0; i < a.nseg; ++i)               // segments left out have L = 0
+            for (int l = 0; l < a.seg[i].L; ++l)
+                for (size_t b = 0, n = a.seg[i].slot_bytes; b < n; b += chunk) {
+                    if (k == STREAM_STATE_MAX_ITEMS) return false;
+                    a.item[k++] = StreamStateItem{i, l, (uint32_t)b, (uint32_t)(b + chunk < n ? b + chunk : n)};
+                }
+        a.nitem = k;
+        return true;
+    };
+    for (size_t chunk = 32768; !cut(chunk); chunk *= 2) {}
+}
+
 // stream_state_copy_kernel's tables for the segments i < ns whose flags include `need`: each at its handle place and payload offset
-// off[i] (off null: zeroing, no payload), each layer cut into items of at most `chunk` bytes (32 KB, doubled until the items fit)
+// off[i] (off null: zeroing, no payload), cut into items by state_items
 static void state_launch(fsn_stream* st, int ns, unsigned need, const size_t* off, StreamStateLaunch& a) {
     const fsn_config& c = st->m->cfg;
     a.nseg = ns;
@@ -2288,18 +2305,7 @@ static void state_launch(fsn_stream* st, int ns, unsigned need, const size_t* of
         a.seg[i] = StreamStateSeg{static_cast<char*>(p.buf->p) + p.offset, p.layer, n, off ? off[i] : 0, seg_layers(c, i),
                                   (n % 16 || p.layer % 16) ? 8 : 16};
     }
-    auto cut = [&](size_t chunk) {
-        int k = 0;
-        for (int i = 0; i < ns; ++i)                   // segments left out have L = 0
-            for (int l = 0; l < a.seg[i].L; ++l)
-                for (size_t b = 0, n = a.seg[i].slot_bytes; b < n; b += chunk) {
-                    if (k == STREAM_STATE_MAX_ITEMS) return false;
-                    a.item[k++] = StreamStateItem{i, l, (uint32_t)b, (uint32_t)(b + chunk < n ? b + chunk : n)};
-                }
-        a.nitem = k;
-        return true;
-    };
-    for (size_t chunk = 32768; !cut(chunk); chunk *= 2) {}
+    state_items(a);
 }
 
 // The configurations that stream: fullsubnet.Model with a cumulative norm
@@ -2822,14 +2828,26 @@ static const int CHUNK_PRE = 256;                      // P: the reference's pre
 
 // Per slot on the host: n = samples of the session so far (-1: no session) and k = its chunks enhanced; chunk k covers session samples
 // [k H - P, k H + C), and y[0, k H) has been emitted (all of y[0, L) once the session has ended).  On the device: the sample ring
-// [B, C + P], the overlap tail [B, H] and the window [C]; the plan and the batch's rows are per call, grow-only.
+// [B, C + P], the overlap tail [B, chunk_tail_stride(C)] and the window [C]; the plan and the batch's rows are per call, grow-only;
+// x_slot: the slot list of the last save / load (DESIGN.md §3.17), grow-only.
 struct fsn_chunk_stream {
     fsn_model* m;
     int B, C;
     std::vector<int64_t> n, k;
-    DevBuf ring, tail, window, plan, rows, enh;
+    DevBuf ring, tail, window, plan, rows, enh, x_slot;
     PinnedStage stage;
 };
+
+// The chunk lengths a handle can take on its own, whatever the model: even, H >= P, C + P < 2^30
+static int chunk_length_ok(int C) {
+    if (C < 2 || C % 2) return fail(FSN_EINVAL, "chunk_samples = %d: the chunk length must be even (two halves of 50 %% overlap)", C);
+    if (C / 2 < CHUNK_PRE)
+        return fail(FSN_EINVAL, "chunk_samples = %d: the half-chunk %d is shorter than the %d-sample pre-context (chunk_samples >= %d)", C,
+                    C / 2, CHUNK_PRE, 2 * CHUNK_PRE);
+    if ((long long)C > 0x3fffffffLL - CHUNK_PRE)
+        return fail(FSN_EINVAL, "chunk_samples = %d exceeds 2^30 - 1 - %d samples", C, CHUNK_PRE);
+    return FSN_OK;
+}
 
 // The plan of slot b for flag f and count c (CP_* fields into p), and its n and k after the call.  Checks the flag and the count.
 static int chunk_slot_plan(const fsn_chunk_stream* cs, int b, int f, int c, int S, int row0, int32_t* p, int64_t* n1, int64_t* k1) {
@@ -2863,12 +2881,7 @@ extern "C" int fsn_chunk_stream_create(fsn_model* m, int32_t B, int32_t chunk_sa
     if (B < 1) return fail(FSN_EINVAL, "B = %d: the handle needs at least one slot", B);
     if (!m->finalized) return fail(FSN_ESTATE, "fsn_model_finalize has not been called");
     const int C = chunk_samples;
-    if (C < 2 || C % 2) return fail(FSN_EINVAL, "chunk_samples = %d: the chunk length must be even (two halves of 50 %% overlap)", C);
-    if (C / 2 < CHUNK_PRE)
-        return fail(FSN_EINVAL, "chunk_samples = %d: the half-chunk %d is shorter than the %d-sample pre-context (chunk_samples >= %d)", C,
-                    C / 2, CHUNK_PRE, 2 * CHUNK_PRE);
-    if ((long long)C > 0x3fffffffLL - CHUNK_PRE)
-        return fail(FSN_EINVAL, "chunk_samples = %d exceeds 2^30 - 1 - %d samples", C, CHUNK_PRE);
+    if (int rc = chunk_length_ok(C)) return rc;
     // every batch of the step is fsn_model_enhance_audio on rows of P + C samples: refused here with that call's message
     int T = 0, Lmax = 0;
     bool all = true;
@@ -2887,7 +2900,7 @@ extern "C" int fsn_chunk_stream_create(fsn_model* m, int32_t B, int32_t chunk_sa
     const double pi = std::acos(-1.0);
     for (int i = 0; i < C; ++i) w[i] = (float)(0.5 - 0.5 * std::cos(2.0 * pi * i / C));   // torch.hann_window(C), periodic
     int e = cs->ring.ensure((size_t)B * (C + CHUNK_PRE) * sizeof(float), true);
-    e |= cs->tail.ensure((size_t)B * (C / 2) * sizeof(float), true);
+    e |= cs->tail.ensure((size_t)B * chunk_tail_stride(C) * sizeof(float), true);
     e |= cs->window.ensure((size_t)C * sizeof(float), false);
     e |= cs->plan.ensure((size_t)B * CHUNK_PLAN_FIELDS * sizeof(int32_t), false);
     if (e || cudaMemcpy(cs->window.p, w.data(), (size_t)C * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) {
@@ -2900,7 +2913,7 @@ extern "C" int fsn_chunk_stream_create(fsn_model* m, int32_t B, int32_t chunk_sa
 
 extern "C" void fsn_chunk_stream_destroy(fsn_chunk_stream* cs) {
     if (!cs) return;
-    for (DevBuf* b : {&cs->ring, &cs->tail, &cs->window, &cs->plan, &cs->rows, &cs->enh}) b->release();
+    for (DevBuf* b : {&cs->ring, &cs->tail, &cs->window, &cs->plan, &cs->rows, &cs->enh, &cs->x_slot}) b->release();
     delete cs;
 }
 
@@ -3019,20 +3032,22 @@ static const char* cfg_diff(const fsn_config& a, const fsn_config& b, int* va, i
     return nullptr;
 }
 
-static int state_slots_ok(const fsn_stream* st, int n, const int32_t* h_slots, bool unique) {
+// n slot indices of a handle of B slots, distinct when `unique`
+static int state_slots_ok(int B, int n, const int32_t* h_slots, bool unique) {
     if (n < 1) return fail(FSN_EINVAL, "n = %d: at least one slot", n);
     if (!h_slots) return fail(FSN_EINVAL, "h_slots is null (n = %d slot indices)", n);
-    std::vector<int> seen(unique ? st->B : 0, -1);
+    std::vector<int> seen(unique ? B : 0, -1);
     for (int i = 0; i < n; ++i) {
         const int b = h_slots[i];
-        if (b < 0 || b >= st->B) return fail(FSN_EINVAL, "h_slots[%d] = %d is out of range (slots 0..%d)", i, b, st->B - 1);
+        if (b < 0 || b >= B) return fail(FSN_EINVAL, "h_slots[%d] = %d is out of range (slots 0..%d)", i, b, B - 1);
         if (unique && seen[b] >= 0) return fail(FSN_EINVAL, "h_slots[%d] = %d: slot %d is loaded twice (also h_slots[%d])", i, b, b, seen[b]);
         if (unique) seen[b] = i;
     }
     return FSN_OK;
 }
 
-static int state_buffer_ok(const fsn_stream* st, const void* d_state) {
+// d_state: 256-byte aligned device memory of the device that holds handle_mem, the handle's state
+static int state_buffer_ok(const void* handle_mem, const void* d_state) {
     if (!d_state) return fail(FSN_EINVAL, "d_state is null");
     cudaPointerAttributes pa{}, ph{};
     const cudaError_t e = cudaPointerGetAttributes(&pa, d_state);
@@ -3042,7 +3057,7 @@ static int state_buffer_ok(const fsn_stream* st, const void* d_state) {
     }
     if (pa.type != cudaMemoryTypeDevice && pa.type != cudaMemoryTypeManaged)
         return fail(FSN_EINVAL, "d_state is not device memory (memory type %d: a host pointer)", (int)pa.type);
-    CK(cudaPointerGetAttributes(&ph, st->cum_in.p));
+    CK(cudaPointerGetAttributes(&ph, handle_mem));
     if (pa.device != ph.device) return fail(FSN_EINVAL, "d_state is memory of device %d, the handle lives on device %d", pa.device, ph.device);
     if (reinterpret_cast<uintptr_t>(d_state) % 256) return fail(FSN_EINVAL, "d_state is not 256-byte aligned");
     return FSN_OK;
@@ -3072,12 +3087,12 @@ static int state_copy(fsn_stream* st, int n, const int32_t* h_slots, void* d_sta
 
 extern "C" int fsn_stream_save_slots(fsn_stream* st, int32_t n, const int32_t* h_slots, void* d_state, fsn_slot_meta* h_meta, void* stream) {
     if (!st) return fail(FSN_EINVAL, "st is null");
-    if (int rc = state_slots_ok(st, n, h_slots, false)) return rc;
+    if (int rc = state_slots_ok(st->B, n, h_slots, false)) return rc;
     if (!h_meta) return fail(FSN_EINVAL, "h_meta is null (n = %d metas)", n);
     const int mode = st->mode;
     if (!mode || (mode == FSN_STATE_MODE_AUDIO && st->a_tick.empty()))
         return fail(FSN_ESTATE, "the handle has served no call and no load: it holds no session to save");
-    if (int rc = state_buffer_ok(st, d_state)) return rc;
+    if (int rc = state_buffer_ok(st->cum_in.p, d_state)) return rc;
     int64_t stride = 0;
     if (int rc = state_layout(st->m->cfg, mode, nullptr, nullptr, &stride)) return rc;
     if (int rc = state_copy(st, n, h_slots, d_state, mode, STREAM_STATE_SAVE, static_cast<cudaStream_t>(stream))) return rc;
@@ -3097,7 +3112,7 @@ extern "C" int fsn_stream_save_slots(fsn_stream* st, int32_t n, const int32_t* h
 extern "C" int fsn_stream_load_slots(fsn_stream* st, int32_t n, const int32_t* h_slots, const void* d_state, const fsn_slot_meta* h_meta,
                                      void* stream) {
     if (!st) return fail(FSN_EINVAL, "st is null");
-    if (int rc = state_slots_ok(st, n, h_slots, true)) return rc;
+    if (int rc = state_slots_ok(st->B, n, h_slots, true)) return rc;
     if (!h_meta) return fail(FSN_EINVAL, "h_meta is null (n = %d metas)", n);
     const fsn_model* m = st->m;
     const int hmode = st->mode;
@@ -3127,7 +3142,7 @@ extern "C" int fsn_stream_load_slots(fsn_stream* st, int32_t n, const int32_t* h
         if (q.mode == FSN_STATE_MODE_MASK ? q.frames < 0 : (q.tick < -1 || q.hops < 0))
             return fail(FSN_EINVAL, "h_meta[%d]: bad counters (frames %d, tick %d, hops %d)", i, q.frames, q.tick, q.hops);
     }
-    if (int rc = state_buffer_ok(st, d_state)) return rc;
+    if (int rc = state_buffer_ok(st->cum_in.p, d_state)) return rc;
     const int mode = h_meta[0].mode;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     if (int rc = claim_mode(st, mode)) return rc;
@@ -3138,6 +3153,110 @@ extern "C" int fsn_stream_load_slots(fsn_stream* st, int32_t n, const int32_t* h
         const int b = h_slots[i];
         if (mode == FSN_STATE_MODE_MASK) st->nb[b] = h_meta[i].frames;
         else { st->a_tick[b] = h_meta[i].tick; st->a_hops[b] = h_meta[i].hops; }
+    }
+    return FSN_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// park, resume and move overlapped-chunk sessions (DESIGN.md §3.17)
+// ---------------------------------------------------------------------------------------------
+// The payload of C: the ring row at 0, the tail row at the next 16-byte boundary, the stride rounded up to 256 bytes.  The copy moves
+// the tail's handle row, chunk_tail_stride(C) floats: H floats and the padding up to the payload's next 16-byte boundary.
+struct ChunkLayout { size_t ring, tail_off, tail_copy, stride; };
+static int chunk_layout(int C, ChunkLayout* l) {
+    if (int rc = chunk_length_ok(C)) return rc;
+    l->ring = (size_t)(C + CHUNK_PRE) * sizeof(float);
+    l->tail_off = (l->ring + 15) & ~(size_t)15;
+    l->tail_copy = (size_t)chunk_tail_stride(C) * sizeof(float);
+    l->stride = (l->tail_off + (size_t)(C / 2) * sizeof(float) + 255) & ~(size_t)255;
+    return FSN_OK;
+}
+
+extern "C" int fsn_chunk_stream_state_layout(int32_t chunk_samples, int64_t* payload_bytes, int32_t* meta_bytes) {
+    ChunkLayout l{};
+    if (int rc = chunk_layout(chunk_samples, &l)) return rc;
+    if (payload_bytes) *payload_bytes = (int64_t)l.stride;
+    if (meta_bytes) *meta_bytes = (int32_t)sizeof(fsn_chunk_slot_meta);
+    return FSN_OK;
+}
+
+// One launch of stream_state_copy_kernel for n sessions: the ring and the tail as two segments of one layer each, between the handle
+// slots h_slots and the payload.  Ring rows are (C + P) 4 bytes (8-byte multiples when C = 2 mod 4), tail rows 16-byte multiples.
+static int chunk_state_copy(fsn_chunk_stream* cs, int n, const int32_t* h_slots, void* d_state, int dir, cudaStream_t s) {
+    ChunkLayout l{};
+    if (int rc = chunk_layout(cs->C, &l)) return rc;
+    StreamStateLaunch a{};
+    a.nseg = 2;
+    a.seg[0] = StreamStateSeg{static_cast<char*>(cs->ring.p), 0, l.ring, 0, 1, l.ring % 16 ? 8 : 16};
+    a.seg[1] = StreamStateSeg{static_cast<char*>(cs->tail.p), 0, l.tail_copy, l.tail_off, 1, 16};
+    state_items(a);
+    if (cs->x_slot.ensure((size_t)(n > cs->B ? n : cs->B) * sizeof(int32_t), false)) return fail(FSN_ECUDA, "slot-list buffer allocation failed");
+    int32_t* h = nullptr;
+    if (int rc = cs->stage.take(n, &h)) return rc;
+    memcpy(h, h_slots, (size_t)n * sizeof(int32_t));
+    if (int rc = cs->stage.send(cs->x_slot.p, n, s)) return rc;
+    a.slots = static_cast<const int*>(cs->x_slot.p); a.n = n;
+    a.payload = static_cast<char*>(d_state); a.stride = l.stride; a.dir = dir;
+    const int e = launch_stream_state(a, s);
+    if (e) return fail(FSN_ECUDA, "chunk session state copy failed: %s", cudaGetErrorString((cudaError_t)e));
+    return FSN_OK;
+}
+
+extern "C" int fsn_chunk_stream_save_slots(fsn_chunk_stream* cs, int32_t n, const int32_t* h_slots, void* d_state, fsn_chunk_slot_meta* h_meta,
+                                           void* stream) {
+    if (!cs) return fail(FSN_EINVAL, "cs is null");
+    if (int rc = state_slots_ok(cs->B, n, h_slots, false)) return rc;
+    if (!h_meta) return fail(FSN_EINVAL, "h_meta is null (n = %d metas)", n);
+    if (int rc = state_buffer_ok(cs->ring.p, d_state)) return rc;
+    ChunkLayout l{};
+    if (int rc = chunk_layout(cs->C, &l)) return rc;
+    if (int rc = chunk_state_copy(cs, n, h_slots, d_state, STREAM_STATE_SAVE, static_cast<cudaStream_t>(stream))) return rc;
+    const fsn_model* m = cs->m;
+    for (int i = 0; i < n; ++i) {
+        const int b = h_slots[i];
+        fsn_chunk_slot_meta& q = h_meta[i];
+        memset(&q, 0, sizeof(q));
+        q.magic = FSN_CHUNK_STATE_MAGIC; q.version = FSN_CHUNK_STATE_VERSION;
+        q.chunk_samples = cs->C; q.pre_context = CHUNK_PRE;
+        q.num_freqs = m->cfg.num_freqs; q.model_kind = m->cfg.model_kind; q.weights_id = m->weights_id;
+        q.samples = cs->n[b]; q.chunks = cs->k[b];
+        q.payload_bytes = (int64_t)l.stride;
+    }
+    return FSN_OK;
+}
+
+extern "C" int fsn_chunk_stream_load_slots(fsn_chunk_stream* cs, int32_t n, const int32_t* h_slots, const void* d_state,
+                                           const fsn_chunk_slot_meta* h_meta, void* stream) {
+    if (!cs) return fail(FSN_EINVAL, "cs is null");
+    if (int rc = state_slots_ok(cs->B, n, h_slots, true)) return rc;
+    if (!h_meta) return fail(FSN_EINVAL, "h_meta is null (n = %d metas)", n);
+    ChunkLayout l{};
+    if (int rc = chunk_layout(cs->C, &l)) return rc;
+    const int64_t H = cs->C / 2;
+    for (int i = 0; i < n; ++i) {                                       // every meta is checked before any state changes
+        const fsn_chunk_slot_meta& q = h_meta[i];
+        if (q.magic != FSN_CHUNK_STATE_MAGIC) return fail(FSN_EINVAL, "h_meta[%d]: bad magic 0x%08x (not a saved chunk session)", i, q.magic);
+        if (q.version != FSN_CHUNK_STATE_VERSION)
+            return fail(FSN_EINVAL, "h_meta[%d]: version %u, this library reads version %d", i, q.version, FSN_CHUNK_STATE_VERSION);
+        if (q.chunk_samples != cs->C)
+            return fail(FSN_EINVAL, "h_meta[%d]: chunk_samples %d, this handle's chunks are %d samples", i, q.chunk_samples, cs->C);
+        if (q.pre_context != CHUNK_PRE)
+            return fail(FSN_EINVAL, "h_meta[%d]: pre_context %d, this handle's pre-context is %d samples", i, q.pre_context, CHUNK_PRE);
+        if (q.payload_bytes != (int64_t)l.stride)
+            return fail(FSN_EINVAL, "h_meta[%d]: payload_bytes %lld, this handle's payload is %lld bytes", i, (long long)q.payload_bytes,
+                        (long long)l.stride);
+        if (q.samples < -1 || q.samples > (1LL << 62))
+            return fail(FSN_EINVAL, "h_meta[%d]: samples %lld is outside -1 .. 2^62", i, (long long)q.samples);
+        const int64_t k = q.samples < 0 ? 0 : std::max<int64_t>(0, q.samples / H - 1);
+        if (q.chunks != k)
+            return fail(FSN_EINVAL, "h_meta[%d]: chunks %lld, a session of %lld samples has enhanced %lld (max(0, floor(samples / %lld) - 1))",
+                        i, (long long)q.chunks, (long long)q.samples, (long long)k, (long long)H);
+    }
+    if (int rc = state_buffer_ok(cs->ring.p, d_state)) return rc;
+    if (int rc = chunk_state_copy(cs, n, h_slots, const_cast<void*>(d_state), STREAM_STATE_LOAD, static_cast<cudaStream_t>(stream))) return rc;
+    for (int i = 0; i < n; ++i) {
+        const int b = h_slots[i];
+        cs->n[b] = h_meta[i].samples; cs->k[b] = h_meta[i].chunks;
     }
     return FSN_OK;
 }

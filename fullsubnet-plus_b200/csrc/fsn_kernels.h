@@ -220,13 +220,16 @@ inline AudioTables audio_table_ptrs(const float* tab, int n_fft) {
 // slot's samples relative to its next chunk's start a0 = k0 H (ring below rel0, the call's row in [rel0, rel1), zero below lo and
 // from rel1 on), the ring position of a0 (phase) and the samples emitted (nout).  lo = 0 exactly when that next chunk is chunk 0.
 enum { CP_NC, CP_ROW0, CP_REL0, CP_REL1, CP_LO, CP_PHASE, CP_NOUT, CHUNK_PLAN_FIELDS };
+// Floats between two slots' tails: C / 2 rounded up to a multiple of 4, so that every slot's tail starts 16-byte aligned and the save /
+// load copy (stream_state_copy_kernel) moves it in 16-byte or 8-byte accesses whatever the parity of C / 2 (DESIGN.md §3.17)
+__host__ __device__ inline int chunk_tail_stride(int C) { return ((C >> 1) + 3) & ~3; }
 struct ChunkStreamLaunch {
     const int* plan;          // [B, CHUNK_PLAN_FIELDS] device
     const float* samples;     // [B, S] this call's samples at the front of each row
     float* ring;              // [B, C + P] the slot's last C + P samples, sample p at p mod (C + P)
     float* rows;              // [n, P + C] the completed chunks' input rows (gather output, the forward's input)
     const float* enh;         // [n, P + C] the forward's output rows
-    float* tail;              // [B, C / 2] the windowed second half of the slot's last enhanced chunk
+    float* tail;              // [B, chunk_tail_stride(C)] the windowed second half of the slot's last enhanced chunk (C / 2 floats)
     const float* window;      // [C] periodic Hann window
     float* out;               // [B, S + C] emitted samples at the front of each row, zero after them
     int B, S, C, P;

@@ -46,7 +46,7 @@ __global__ void __launch_bounds__(CHUNK_THREADS) chunk_crossfade_kernel(ChunkStr
     const int H = a.C >> 1, W = a.C + a.P;
     const size_t ow = (size_t)a.S + a.C;
     float* out = a.out + (size_t)b * ow;
-    float* tail = a.tail + (size_t)b * H;
+    float* tail = a.tail + (size_t)b * chunk_tail_stride(a.C);
     for (int t = threadIdx.x; t < H; t += blockDim.x) {
         const float w0 = __ldg(a.window + t), w1 = __ldg(a.window + H + t);
         float tl = tail[t];

@@ -28,6 +28,7 @@ SYMBOLS = [
     "fsn_stream_step_chunk", "fsn_stream_chunk_plan", "fsn_stream_step_audio_chunk",
     "fsn_model_file_write", "fsn_model_file_config", "fsn_model_load",
     "fsn_chunk_stream_create", "fsn_chunk_stream_step", "fsn_chunk_stream_destroy",
+    "fsn_chunk_stream_state_layout", "fsn_chunk_stream_save_slots", "fsn_chunk_stream_load_slots",
 ]
 
 
@@ -51,6 +52,25 @@ class FsnSlotMeta(C.Structure):
     """fsn_slot_meta: the host-side description of one saved streaming session (include/fsnplus_b200.h)."""
     _fields_ = [("magic", C.c_uint32), ("version", C.c_uint32), ("cfg", FsnConfig), ("weights_id", C.c_uint64), ("mode", C.c_int32),
                 ("frames", C.c_int32), ("tick", C.c_int32), ("hops", C.c_int32), ("payload_bytes", C.c_int64)]
+
+
+CHUNK_STATE_MAGIC, CHUNK_STATE_VERSION = 0x434E5346, 1      # FSN_CHUNK_STATE_MAGIC ('F' 'S' 'N' 'C'), FSN_CHUNK_STATE_VERSION
+
+
+class FsnChunkSlotMeta(C.Structure):
+    """fsn_chunk_slot_meta: the host-side description of one saved overlapped-chunk session (include/fsnplus_b200.h)."""
+    _fields_ = [("magic", C.c_uint32), ("version", C.c_uint32), ("chunk_samples", C.c_int32), ("pre_context", C.c_int32),
+                ("num_freqs", C.c_int32), ("model_kind", C.c_int32), ("weights_id", C.c_uint64), ("samples", C.c_int64),
+                ("chunks", C.c_int64), ("payload_bytes", C.c_int64)]
+
+
+def chunk_state_layout(chunk_samples):
+    """fsn_chunk_stream_state_layout: (payload bytes per session, sizeof(fsn_chunk_slot_meta)) of chunk sessions of chunk_samples.
+    Host only; needs no GPU."""
+    lib = load_library()
+    nb, mb = C.c_int64(), C.c_int32()
+    check(lib.fsn_chunk_stream_state_layout(int(chunk_samples), C.byref(nb), C.byref(mb)))
+    return nb.value, mb.value
 
 
 def state_layout(cfg, mode):
@@ -182,6 +202,9 @@ def load_library():
     lib.fsn_chunk_stream_step.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp]
     lib.fsn_chunk_stream_destroy.argtypes = [vp]
     lib.fsn_chunk_stream_destroy.restype = None
+    lib.fsn_chunk_stream_state_layout.argtypes = [i32, C.POINTER(i64), C.POINTER(i32)]
+    lib.fsn_chunk_stream_save_slots.argtypes = [vp, i32, vp, vp, vp, vp]
+    lib.fsn_chunk_stream_load_slots.argtypes = [vp, i32, vp, vp, vp, vp]
     _LIB = lib
     return lib
 

@@ -23,7 +23,8 @@ each session where it was saved.
 
 ``ChunkStream`` serves live audio to the models that cannot stream frame by frame -- FullSubNet+ and ``Model`` with an offline norm --
 by the reference's overlapped-chunk inferencer: chunks of C samples with 50 % overlap, each enhanced by the offline audio call, the
-halves cross-faded with a Hann window; the latency is C / 2 to C samples (DESIGN.md §3.16).
+halves cross-faded with a Hann window; the latency is C / 2 to C samples (DESIGN.md §3.16).  Its ``save_slots`` / ``load_slots`` park,
+resume and move those sessions between chunk handles of the same C, whatever their model (DESIGN.md §3.17).
 """
 import ctypes as C
 
@@ -34,9 +35,16 @@ from . import _lib
 HOLD, STEP, START, FLUSH = 0, 1, 2, 3  # FSN_SLOT_* of include/fsnplus_b200.h (FLUSH: audio call only)
 
 
+def _slot_array(slots):
+    s = torch.as_tensor(slots, dtype=torch.int32).reshape(-1).contiguous()
+    assert s.device.type == "cpu" and s.numel() >= 1, "slots: host slot indices"
+    return s
+
+
 class SessionState:
     """Saved streaming sessions: ``payload`` [n, stride] uint8 (a CUDA tensor, or pinned host memory after ``.to("cpu")``) and
-    ``meta``, a ctypes array of n ``fsn_slot_meta``.  ``len()``, indexing / selection (``state[2]``, ``state[[0, 3]]``, slices) and
+    ``meta``, a ctypes array of n ``fsn_slot_meta`` (StreamingFullSubNet) or ``fsn_chunk_slot_meta`` (ChunkStream), whose element
+    type the selections and copies keep.  ``len()``, indexing / selection (``state[2]``, ``state[[0, 3]]``, slices) and
     ``.to(device)`` return new SessionState objects; the payload format is that of this library version only."""
 
     def __init__(self, payload, meta):
@@ -50,6 +58,10 @@ class SessionState:
     def device(self):
         return self.payload.device
 
+    @property
+    def _meta_type(self):
+        return self.meta._type_
+
     def __getitem__(self, idx):
         if isinstance(idx, slice):
             ids = list(range(len(self)))[idx]
@@ -62,7 +74,7 @@ class SessionState:
         ids = [i + len(self) if i < 0 else i for i in ids]
         if any(i < 0 or i >= len(self) for i in ids):
             raise IndexError(f"session index out of range (0..{len(self) - 1})")
-        meta = (_lib.FsnSlotMeta * len(ids))(*[self.meta[i] for i in ids])
+        meta = (self._meta_type * len(ids))(*[self.meta[i] for i in ids])
         sel = torch.tensor(ids, dtype=torch.long, device=self.payload.device)
         payload = self.payload.index_select(0, sel)
         if payload.device.type == "cpu" and self.payload.is_pinned():
@@ -81,7 +93,7 @@ class SessionState:
             payload.copy_(self.payload)
         else:
             payload = self.payload.to(device)
-        return SessionState(payload, (_lib.FsnSlotMeta * len(self))(*self.meta))
+        return SessionState(payload, (self._meta_type * len(self))(*self.meta))
 
 
 class StreamingFullSubNet:
@@ -199,9 +211,7 @@ class StreamingFullSubNet:
         return (out, nout, mask) if return_mask else (out, nout)
 
     def _slot_array(self, slots):
-        s = torch.as_tensor(slots, dtype=torch.int32).reshape(-1).contiguous()
-        assert s.device.type == "cpu" and s.numel() >= 1, "slots: host slot indices"
-        return s
+        return _slot_array(slots)
 
     def save_slots(self, slots):
         """Snapshot the sessions of `slots` (a sequence or a CPU integer tensor) into a SessionState on this handle's device.  The slots
@@ -285,6 +295,38 @@ class ChunkStream:
                                                       C.c_void_p(n.data_ptr()), C.c_void_p(out.data_ptr()),
                                                       C.c_void_p(nout.data_ptr()), stream))
         return out, nout
+
+    def save_slots(self, slots):
+        """Snapshot the sessions of `slots` (a sequence or a CPU integer tensor) into a SessionState on this handle's device (DESIGN.md
+        §3.17).  The slots are unchanged: they may keep stepping (a fork) or START other sessions; a slot without a session saves as
+        samples = -1.  Ordered on the current stream like ``step``."""
+        s = _slot_array(slots)
+        n = s.numel()
+        stride, _ = _lib.chunk_state_layout(self.C)
+        payload = torch.empty((n, stride), dtype=torch.uint8, device=self.device)
+        meta = (_lib.FsnChunkSlotMeta * n)()
+        with torch.cuda.device(self.device):
+            stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+            _lib.check(self.lib.fsn_chunk_stream_save_slots(self._cs, n, C.c_void_p(s.data_ptr()), C.c_void_p(payload.data_ptr()), meta,
+                                                            stream))
+        return SessionState(payload, meta)
+
+    def load_slots(self, slots, state):
+        """Load session i of `state` into slot slots[i] (distinct slots), replacing a START: the slot's next STEP or FLUSH continues the
+        session where it was saved, with this handle's model for the chunks still to come.  The state may come from any chunk handle of
+        the same C -- another B, another device (it is copied to this handle's device first), another model."""
+        s = _slot_array(slots)
+        assert s.numel() == len(state), f"{s.numel()} slots for {len(state)} sessions"
+        if state._meta_type is not _lib.FsnChunkSlotMeta:
+            raise TypeError("state holds frame-by-frame sessions (StreamingFullSubNet.save_slots), not chunk sessions")
+        state = state.to(self.device)
+        payload = state.payload.contiguous()
+        if payload.data_ptr() % 256:
+            payload = payload.clone()
+        with torch.cuda.device(self.device):
+            stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+            _lib.check(self.lib.fsn_chunk_stream_load_slots(self._cs, s.numel(), C.c_void_p(s.data_ptr()), C.c_void_p(payload.data_ptr()),
+                                                            state.meta, stream))
 
     def close(self):
         if self._cs is not None:

@@ -345,6 +345,56 @@ int fsn_chunk_stream_step(fsn_chunk_stream* cs, const float* d_samples, int32_t 
                           float* d_out, int32_t* h_nout, void* stream);
 void fsn_chunk_stream_destroy(fsn_chunk_stream* cs);
 
+/* Park, resume and move overlapped-chunk sessions (DESIGN.md §3.17): save the state of some slots of a chunk handle to a device buffer
+ * and load it into any slot of any chunk handle with the same chunk_samples -- the same one, one with another B, one on another device
+ * after the caller has copied the payload there, or one of ANOTHER MODEL.
+ *
+ * A session's state holds no model state: the sample ring, the overlap tail and two host counters.  A saved session is a payload row
+ * of payload_bytes (d_state [n, payload_bytes], device) plus a host fsn_chunk_slot_meta.  The payload, one layout per C:
+ *   bytes [0, (C + P) 4)            the ring, float32: session sample p at float p mod (C + P) (the last C + P samples the slot read)
+ *   bytes [t, t + H 4)              the tail, float32 (H = C / 2), t = (C + P) 4 rounded up to 16: the windowed second half of the
+ *                                   session's last enhanced chunk
+ *   payload_bytes = t + H 4 rounded up to 256.
+ * The bytes between the ring and the tail and after the tail are padding: a save writes them with unspecified values, a load never
+ * reads what lies between the ring and the tail and writes what follows the tail only to the handle's own padding, which nothing
+ * reads.  The ring is indexed by absolute session position, so a raw copy of the rows is canonical: independent of B, of the slot and
+ * of the device.
+ *
+ * Model identity is NOT checked: a session saved from one model continues on another (other weights, the sub-band TCN, fullsubnet.Model)
+ * -- the chunks enhanced before the load come from the saving model, the rest from the loading one, cross-faded by the usual rule.
+ * num_freqs, model_kind and weights_id are in the meta for the caller to enforce its own policy.
+ *
+ * fsn_chunk_stream_save_slots is a snapshot: the slots are unchanged and may keep stepping (a fork) or START other sessions.  h_meta[i]
+ * describes session i, saved from slot h_slots[i]; a slot without a session saves as samples = -1, chunks = 0.
+ * fsn_chunk_stream_load_slots replaces a START: it overwrites the state of slot h_slots[i] with session i, host counters included, and
+ * the slot's next call is a STEP or FLUSH that continues the session.  Loading a meta with samples = -1 leaves the slot without a
+ * session.
+ * Both calls are ordered on `stream` like the step: h_meta is filled (save) or validated (load) on the host before the call returns,
+ * the payload copy (one kernel for the n sessions) is enqueued and the stream is not synchronised; h_slots and h_meta are free on
+ * return.
+ * Every check runs before any state changes or launch: a failed call changes nothing.  FSN_EINVAL, naming the index or field: a null
+ * array, n < 1, a slot out of range, a slot twice in one load, a bad magic or version, a chunk_samples, pre_context or payload_bytes
+ * other than this handle's, samples outside -1 .. 2^62, chunks other than max(0, floor(samples / H) - 1) (0 when samples = -1), a
+ * d_state that is not 256-byte aligned device memory of the handle's device. */
+#define FSN_CHUNK_STATE_VERSION 1
+#define FSN_CHUNK_STATE_MAGIC 0x434E5346u  /* the bytes 'F' 'S' 'N' 'C' */
+typedef struct fsn_chunk_slot_meta { /* host-side description of one saved overlapped-chunk session                   */
+    uint32_t magic, version;         /* FSN_CHUNK_STATE_MAGIC, FSN_CHUNK_STATE_VERSION                                */
+    int32_t chunk_samples, pre_context; /* C and P (256) of the saving handle                                         */
+    int32_t num_freqs, model_kind;   /* the saving model: for the caller, not checked at a load                       */
+    uint64_t weights_id;             /* fsn_model_weights_id of the saving model: for the caller, not checked         */
+    int64_t samples;                 /* n: samples since START, -1 = the slot had no session                          */
+    int64_t chunks;                  /* k: chunks enhanced (max(0, floor(n / H) - 1) for a live session)              */
+    int64_t payload_bytes;           /* stride of one session in d_state                                              */
+} fsn_chunk_slot_meta;
+/* Payload stride for chunk_samples and sizeof(fsn_chunk_slot_meta).  Host only, no GPU.  FSN_EINVAL naming the limit for a
+ * chunk_samples that fsn_chunk_stream_create refuses on its own (odd, H < P, past 2^30 - 1 - P). */
+int fsn_chunk_stream_state_layout(int32_t chunk_samples, int64_t* payload_bytes, int32_t* meta_bytes);
+int fsn_chunk_stream_save_slots(fsn_chunk_stream* cs, int32_t n, const int32_t* h_slots, void* d_state, fsn_chunk_slot_meta* h_meta,
+                                void* stream);
+int fsn_chunk_stream_load_slots(fsn_chunk_stream* cs, int32_t n, const int32_t* h_slots, const void* d_state,
+                                const fsn_chunk_slot_meta* h_meta, void* stream);
+
 /* Park, resume and move sessions (DESIGN.md §3.11): save the state of some slots to a device buffer and load it into any slot of a
  * compatible handle -- the same one, another with a different B or full-band kernel, or one on another device after the caller has
  * copied the payload there.

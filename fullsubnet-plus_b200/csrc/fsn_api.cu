@@ -1035,7 +1035,7 @@ struct WsSizes {
     size_t au_planes = 0, au_enh = 0;                                           // audio call: mag / real / imag planes, enhanced spectrum
     size_t total() const;
 };
-static WsSizes ws_sizes(const fsn_config& c, bool layerwise, int B, int T, int Tw, int Fc = 0, bool audio = false) {
+static WsSizes ws_sizes(const fsn_config& c, bool layerwise, int B, int T, int Tw, int Fc = 0, bool audio = false, bool lim = false) {
     WsSizes z;
     const int F = c.num_freqs, Tp = T + c.look_ahead, Pp = (Tp + 3) & ~3, Ts = Tw ? Tw : Tp;
     const int nbr = (c.model_kind == FSN_KIND_PLUS) ? 3 : 1;
@@ -1047,7 +1047,8 @@ static WsSizes ws_sizes(const fsn_config& c, bool layerwise, int B, int T, int T
     z.mu = z.sigma = (size_t)B * 4;
     z.tsse_scale = (size_t)nbr * B * F * 4 * (1 + tsse_row_floats());          // per-row scale | row statistics
     z.sb_rowsum = (size_t)B * 4 * F * 2 * 4;
-    z.tlen = (size_t)(audio ? 4 : 3) * B * sizeof(int32_t);                     // counted whether the forward is ragged or not
+    z.tlen = (size_t)(3 + audio + lim) * B * sizeof(int32_t);                   // counted whether the forward is ragged or not; lim: the
+                                                                                // clips' attenuation floors (stage_lengths)
     if (audio) { z.au_planes = (size_t)3 * B * F * T * 4; z.au_enh = (size_t)B * F * T * 8; }
     if (c.norm_type != FSN_NORM_OFFLINE_LAPLACE) z.xn = (size_t)nbr * B * F * Tp * 4;
     if (c.sb_tcn) {
@@ -1198,6 +1199,9 @@ struct Batch {
     const float* wave = nullptr; float* wave_out = nullptr; long long L = 0; const int64_t* lengths = nullptr;
     int Lall = 0; const int32_t* samples = nullptr;
     const float* raw = nullptr; int Tw = 0;    // the test hook: the sub-band input [B*F, Isb, T'] and its time window
+    // the _lim calls: every clip's attenuation limit in dB (host, null: none); once checked, its floor lam = 10^(-dB / 20) per clip (host,
+    // null when every floor is 0: the batch then runs exactly the unlimited forward) and, in the forward, the floors on the device
+    const float* atten_db = nullptr; const float* lam = nullptr; const float* dlam = nullptr;
 };
 
 // The longest TSSE kernel (1 without the TSSE attention): every clip needs frames + look_ahead >= it
@@ -1264,10 +1268,33 @@ static int audio_check(const fsn_config& c, int32_t B, int64_t L, const int64_t*
     return check_length(c, 1, *T);
 }
 
+// An attenuation limit of L dB (DESIGN.md §3.18), entry i of h_atten_db: L >= 0 or +inf, else FSN_EINVAL naming what it limits (the clip
+// or slot `id`) and the value.  Its floor lam = 10^(-L / 20), computed in double and rounded to float (+inf: 0, no limit).
+static int atten_floor(double db, const char* what, int id, int i, float* lam) {
+    if (!(db >= 0.0))
+        return fail(FSN_EINVAL, "%s %d: h_atten_db[%d] = %g: an attenuation limit is a number of dB >= 0 (+inf: no limit)", what, id, i, db);
+    *lam = (float)std::pow(10.0, -db / 20.0);
+    return FSN_OK;
+}
+
+// The floors of b's clips into lam from b.atten_db; b.lam stays null when there is no array or every floor is 0 (no limit on any clip)
+static int check_atten(Batch& b, std::vector<float>* lam) {
+    if (!b.atten_db) return FSN_OK;
+    lam->resize((size_t)b.B);
+    bool any = false;
+    for (int i = 0; i < b.B; ++i) {
+        if (int rc = atten_floor(b.atten_db[i], "clip", i, i, &(*lam)[i])) return rc;
+        any = any || (*lam)[i] > 0.f;
+    }
+    if (any) b.lam = lam->data();
+    return FSN_OK;
+}
+
 // Every check of an offline call, before it allocates, copies, records or waits on anything.  The audio call also sets b.T and
 // b.Lall and, for a ragged batch, b.samples and b.frames (unless every clip has T frames) into lens.  A plain forward is checked for
 // the length limits of one clip: plan_forward keeps every sub-batch within them.
-static int check_batch(const fsn_model* m, Batch& b, std::vector<int32_t>* lens = nullptr) {
+static int check_batch(const fsn_model* m, Batch& b, std::vector<int32_t>* lens = nullptr, std::vector<float>* lam = nullptr) {
+    if (b.atten_db && (!lam || b.call == CALL_PIPELINED || b.call == CALL_HOOK)) return fail(FSN_EINVAL, "this call takes no attenuation limit");
     if (b.call == CALL_AUDIO) {
         if (!m) return fail(FSN_EINVAL, "m is null");
         if (!b.wave) return fail(FSN_EINVAL, "d_wave is null ([B, L] float32 samples on the device)");
@@ -1281,7 +1308,8 @@ static int check_batch(const fsn_model* m, Batch& b, std::vector<int32_t>* lens 
             for (int i = 0; i < b.B; ++i) (*lens)[b.B + i] = ((*lens)[i] = (int32_t)b.lengths[i]) / (m->cfg.num_freqs - 1) + 1;
             b.samples = lens->data(); b.frames = lens->data() + b.B;
         }
-        return check_frames(m->cfg, b);                                 // drops the frame counts when every clip has T frames
+        if (int rc = check_frames(m->cfg, b)) return rc;                // drops the frame counts when every clip has T frames
+        return check_atten(b, lam);
     }
     const bool hook = b.call == CALL_HOOK;
     if (!m || !(hook ? b.raw : b.mag) || (!b.mask && !b.enh)) return fail(FSN_EINVAL, "null argument");
@@ -1296,19 +1324,22 @@ static int check_batch(const fsn_model* m, Batch& b, std::vector<int32_t>* lens 
     if (hook && b.Tw && !m->layerwise) return fail(FSN_EINVAL, "time windows of the sub-band stage need the layer-wise LSTM path");
     if (int rc = check_frames(c, b)) return rc;
     if (!hook && b.T + c.look_ahead < tsse_kmax(c)) return fail(FSN_EINVAL, "sequence shorter than the TSSE kernel size");
-    return check_length(c, b.call == CALL_FORWARD ? 1 : b.B, b.T);
+    if (b.atten_db && !b.enh) return fail(FSN_EINVAL, "an attenuation limit applies to the enhanced spectrum, not to the mask");
+    if (int rc = check_length(c, b.call == CALL_FORWARD ? 1 : b.B, b.T)) return rc;
+    return check_atten(b, lam);
 }
 
 // Size lane ln and the model's buffers for a forward of B clips of T frames with window Tw and bin chunk Fc (ws_sizes; audio: the audio
 // call's), each fresh allocation zero-filled on its own stream (s: front end, sl: sub-band stage), and encode their tensor maps.
-static int ensure_ws(fsn_model* m, Lane& ln, int B, int T, int Tw, int Fc, cudaStream_t s, cudaStream_t sl, bool audio = false) {
+static int ensure_ws(fsn_model* m, Lane& ln, int B, int T, int Tw, int Fc, cudaStream_t s, cudaStream_t sl, bool audio = false,
+                     bool lim = false) {
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs, Tp = T + c.look_ahead;
     const long long srows = (long long)B * (Fc ? Fc : F) * Tp;          // sub-band TCN: the rows of one chunk run
     if (c.sb_tcn && srows > SB_MAX_ROWS)
         return fail(FSN_EINVAL, "B * %s * (T + look_ahead) = %lld rows exceeds the sub-band TCN's 2^31 limit", Fc ? "bins per chunk" : "num_freqs", srows);
     if (c.model_kind == FSN_KIND_PLUS && !m->tcn5) return fail(FSN_ESTATE, "the TCN weights were not packed");
-    const WsSizes z = ws_sizes(c, m->layerwise, B, T, Tw, Fc, audio);
+    const WsSizes z = ws_sizes(c, m->layerwise, B, T, Tw, Fc, audio, lim);
     const WsGeo geo{B, T, Tw, Fc};
     m->au_valid = false;
     const bool regeo = ln.geo != geo;
@@ -1411,7 +1442,7 @@ static int run_sb_lstm(fsn_model* m, Lane& ln, const Batch& b, int Tw, SbPackLau
             a.cstate = static_cast<float*>(m->cstate.p);
             if (Tw) a.hstate = static_cast<__half*>(m->r_hstate.p);
             a.out = b.mask; a.la = c.look_ahead;
-            a.nreal = b.real; a.nimag = b.imag; a.enh = reinterpret_cast<float2*>(b.enh); a.tlen = tlen;
+            a.nreal = b.real; a.nimag = b.imag; a.enh = reinterpret_cast<float2*>(b.enh); a.tlen = tlen; a.lam = b.dlam;
             const int nl = sb_layers(m, a, static_cast<__half*>(m->r_gin.p), Tw ? cs_layer : 0, hs_layer, s);
             if (nl < 0) return nl;
             m->launches += nl;
@@ -1435,7 +1466,7 @@ static int run_sb_lstm(fsn_model* m, Lane& ln, const Batch& b, int Tw, SbPackLau
         }
         int e = launch_lstm_mma(a, s);
         if (e) return fail(FSN_ECUDA, "mma LSTM launch failed: %s", cudaGetErrorString((cudaError_t)e));
-        if (b.enh) { launch_apply_cirm_planar(a.out, b.real, b.imag, reinterpret_cast<float2*>(b.enh), B, F, T, tlen, c.look_ahead, s); m->launches++; }
+        if (b.enh) { launch_apply_cirm_planar(a.out, b.real, b.imag, reinterpret_cast<float2*>(b.enh), B, F, T, tlen, c.look_ahead, s, b.dlam); m->launches++; }
     }
     m->launches++;
     return FSN_OK;
@@ -1514,10 +1545,10 @@ static int run_sb_tcn(fsn_model* m, Lane& ln, const Batch& b, int Fc, SbPackLaun
     const int B = b.B, F = c.num_freqs, Tp = b.T + c.look_ahead, W = Fc ? Fc : F;
     m->last_impl = FSN_LSTM_TCN;
     GemmTc5Launch head{};
-    head.epi = EPI5_GLN_HEAD;
+    head.epi = b.dlam ? EPI5_GLN_HEAD_LIM : EPI5_GLN_HEAD;
     head.fc_w = static_cast<const float*>(m->sb_fc.p); head.fc_b = m->sb_fc_b;
     head.O = c.output_size; head.la = c.look_ahead; head.F = F; head.act = c.sb_act;
-    head.out = b.mask; head.nreal = b.real; head.nimag = b.imag; head.enh = reinterpret_cast<float2*>(b.enh);
+    head.out = b.mask; head.nreal = b.real; head.nimag = b.imag; head.enh = reinterpret_cast<float2*>(b.enh); head.lam = b.dlam;
     float* x = static_cast<float*>(ln.sbx.p);
     float* amax0 = x + (size_t)B * W * Tp * 64;
     for (int f0 = 0; f0 < F; f0 += W) {
@@ -1568,26 +1599,32 @@ static int run_fb(fsn_model* m, const float* fbin, __half* fbx, float* hseq, flo
 // Copy the per-sample extents frames[b] + look_ahead of a ragged forward into the lane's device buffer ln.tlen ([3][B]: one row per
 // full-band branch, so a full-band gLN group z = branch * B + b indexes it directly) through the model's pinned staging.  h_samples:
 // the audio call's sample counts, appended as a fourth row in the same copy, or null.  h_frames may be null when h_samples is not
-// (clips of one frame count but different sample counts): the three rows are then zero and unread.
-static int stage_lengths(fsn_model* m, Lane& ln, const int32_t* h_frames, int B, cudaStream_t s, const int32_t* h_samples = nullptr) {
-    const size_t n = (size_t)(h_samples ? 4 : 3) * B;
+// (clips of one frame count but different sample counts): the three rows are then zero and unread.  h_lam: the clips' attenuation
+// floors (float), appended as the last row of the same copy, or null; *d_lam: that row on the device.
+static int stage_lengths(fsn_model* m, Lane& ln, const int32_t* h_frames, int B, cudaStream_t s, const int32_t* h_samples = nullptr,
+                         const float* h_lam = nullptr, const float** d_lam = nullptr) {
+    const size_t rows = 3 + (h_samples ? 1 : 0), n = (rows + (h_lam ? 1 : 0)) * B;
     int32_t* h = nullptr;
     if (int rc = m->len_stage.take(n, &h)) return rc;
     for (int br = 0; br < 3; ++br)
         for (int b = 0; b < B; ++b) h[(size_t)br * B + b] = h_frames ? h_frames[b] + m->cfg.look_ahead : 0;
     if (h_samples) memcpy(h + (size_t)3 * B, h_samples, (size_t)B * sizeof(int32_t));
+    if (h_lam) memcpy(h + rows * B, h_lam, (size_t)B * sizeof(float));
     if (ln.tlen.ensure(n * sizeof(int32_t), false, s)) return fail(FSN_ECUDA, "workspace allocation failed for the clip lengths");
+    if (h_lam) *d_lam = reinterpret_cast<const float*>(static_cast<const int32_t*>(ln.tlen.p) + rows * B);
     return m->len_stage.send(ln.tlen.p, n, s);
 }
 
 // Set lane ln up for checked batch b (every forward and the test hook): this thread's chained (programmatic dependent) launches, see
 // env_pdl -- "small" = at most 16 row-tile pairs, where the forward is launch-latency-bound; the workspace for window Tw and bin
-// chunk Fc (ensure_ws); the clips' lengths on the device, *tl (null on entry): their frame extents, unless every clip spans T'.  Resets the launch count.
-static int prepare(fsn_model* m, Lane& ln, const Batch& b, int Tw, int Fc, cudaStream_t s, cudaStream_t sl, const int** tl) {
+// chunk Fc (ensure_ws); the clips' lengths on the device, *tl (null on entry): their frame extents, unless every clip spans T', and with
+// them the clips' attenuation floors, *dlam (null on entry; stays null without b.lam).  Resets the launch count.
+static int prepare(fsn_model* m, Lane& ln, const Batch& b, int Tw, int Fc, cudaStream_t s, cudaStream_t sl, const int** tl,
+                   const float** dlam = nullptr) {
     fsn_chain_launch_set(m->env_pdl == 1 || (m->env_pdl < 0 && ((long long)b.B * m->cfg.num_freqs + 255) / 256 <= 16));
-    if (int rc = ensure_ws(m, ln, b.B, b.T, Tw, Fc, s, sl, b.wave != nullptr)) return rc;
-    if (b.frames || b.samples) {
-        if (int rc = stage_lengths(m, ln, b.frames, b.B, s, b.samples)) return rc;
+    if (int rc = ensure_ws(m, ln, b.B, b.T, Tw, Fc, s, sl, b.wave != nullptr, b.lam != nullptr)) return rc;
+    if (b.frames || b.samples || b.lam) {
+        if (int rc = stage_lengths(m, ln, b.frames, b.B, s, b.samples, b.lam, dlam)) return rc;
         if (b.frames) *tl = static_cast<const int*>(ln.tlen.p);
     }
     m->launches = 0;
@@ -1734,11 +1771,13 @@ static int sub_band(fsn_model* m, Lane& ln, const Batch& b, int Tw, int Fc, cons
 // Fc: bin chunk of the sub-band TCN (0: all bins at once; > 0 needs s == sl, the plain driver)
 static int forward_impl(fsn_model* m, Lane& ln, const Batch& in, cudaStream_t s, cudaStream_t sl, int Tw = 0, int Fc = 0) {
     const int* tl = nullptr;                                            // per-sample extents on the device (null: all Tp)
-    int rc = prepare(m, ln, in, Tw, Fc, s, sl, &tl);
+    const float* dlam = nullptr;                                        // attenuation floors on the device (null: no limit)
+    int rc = prepare(m, ln, in, Tw, Fc, s, sl, &tl, &dlam);
     if (rc) return rc;
     const int evi = (int)(m->nfwd % fsn_model::NEV);
     cudaEventRecord(m->evf0[evi], s);
     Batch b = in;
+    b.dlam = dlam;
     AudioLaunch al{};
     if (in.wave) audio_analysis(m, ln, b, al, s);
     SbPackLaunch sp = pack_args(m, ln, b.B, b.T, Tw, tl);
@@ -1834,11 +1873,12 @@ template <class Ok> static int largest(int lo, int hi, Ok ok) {
 //   * nothing fits: one clip at a time in one-bin chunks, allocated anyway.
 // Every chunk run keeps Bs * Fc * T' <= SB_MAX_ROWS.  force_bins > 0 (FSN_SB_CHUNK) chunks every TCN forward with exactly that many bins
 // (>= F: unchunked) and the largest equal split that fits with them.  audio: the audio call's plan, its workspace counted (ws_sizes).
-static Plan plan_forward(const fsn_config& c, bool layerwise, int B, int T, double cap, int force, int force_bins, bool audio = false) {
+static Plan plan_forward(const fsn_config& c, bool layerwise, int B, int T, double cap, int force, int force_bins, bool audio = false,
+                         bool lim = false) {
     const int Tp = T + c.look_ahead, wmax = (Tp + 31) / 32 * 32;
     const long long blim = max_clips_for_rows(c, T);             // sub-batches never exceed the full-band TCN's row limit
     auto split = [&](int bmax) { if (bmax > blim) bmax = (int)blim; if (bmax < 1) bmax = 1; if (B <= bmax) return B; const int n = (B + bmax - 1) / bmax; return (B + n - 1) / n; };
-    auto bytes = [&](int bs, int tw) { return (double)ws_sizes(c, layerwise, bs, T, tw, 0, audio).total(); };
+    auto bytes = [&](int bs, int tw) { return (double)ws_sizes(c, layerwise, bs, T, tw, 0, audio, lim).total(); };
     // largest equal split bs with fits(bs) (0 if even one clip does not fit)
     auto max_split = [&](auto fits) { const int b = largest(0, B, [&](int v) { return fits(split(v)); }); return b ? split(b) : 0; };
     const double per = ws_bytes_per_sample(c, layerwise, T, audio);
@@ -1846,7 +1886,7 @@ static Plan plan_forward(const fsn_config& c, bool layerwise, int B, int T, doub
     Plan p{split(bmax < B ? (int)bmax : B)};
     if (c.sb_tcn) {
         const int F = c.num_freqs;
-        auto fits = [&](int bs, int fc) { return (long long)bs * fc * Tp <= SB_MAX_ROWS && ws_sizes(c, false, bs, T, 0, fc < F ? fc : 0, audio).total() <= cap; };
+        auto fits = [&](int bs, int fc) { return (long long)bs * fc * Tp <= SB_MAX_ROWS && ws_sizes(c, false, bs, T, 0, fc < F ? fc : 0, audio, lim).total() <= cap; };
         const int fforce = force_bins > 0 ? (force_bins < F ? force_bins : F) : 0;
         if (fforce) {                                                   // chunks of fforce bins (F: unchunked), the largest equal split that fits
             if (fforce < F || !fits(p.Bs, F)) {
@@ -1890,7 +1930,7 @@ static Plan plan_forward(const fsn_config& c, bool layerwise, int B, int T, doub
             p.Tw = ((Tp + nwin - 1) / nwin + 31) / 32 * 32;
         }
     }
-    p.bytes = (int64_t)ws_sizes(c, layerwise, p.Bs, T, p.Tw, p.Fc, audio).total();
+    p.bytes = (int64_t)ws_sizes(c, layerwise, p.Bs, T, p.Tw, p.Fc, audio, lim).total();
     return p;
 }
 
@@ -1909,7 +1949,7 @@ static Batch slice(const fsn_config& c, const Batch& b, int b0, int nb) {
     s.B = b.B - b0 < nb ? b.B - b0 : nb;
     s.mag = at(b.mag, plane); s.real = at(b.real, plane); s.imag = at(b.imag, plane); s.frames = at(b.frames, 1);
     s.mask = at(b.mask, c.output_size * plane); s.enh = at(b.enh, 2 * plane);
-    s.wave = at(b.wave, b.L); s.wave_out = at(b.wave_out, b.L); s.samples = at(b.samples, 1);
+    s.wave = at(b.wave, b.L); s.wave_out = at(b.wave_out, b.L); s.samples = at(b.samples, 1); s.lam = at(b.lam, 1);
     return s;
 }
 
@@ -1928,7 +1968,7 @@ static int run_plain(fsn_model* m, const Batch& b, cudaStream_t s) {
         if (m->au_tab.ensure(tab.size() * sizeof(float), false)) return fail(FSN_ECUDA, "allocation of the audio tables failed");
         CK(cudaMemcpy(m->au_tab.p, tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice));
     }
-    m->plan = plan_forward(m->cfg, m->layerwise, b.B, b.T, m->ws_cap_bytes, m->env_sb_window, m->env_sb_chunk, audio);
+    m->plan = plan_forward(m->cfg, m->layerwise, b.B, b.T, m->ws_cap_bytes, m->env_sb_window, m->env_sb_chunk, audio, b.lam != nullptr);
     const int Bs = m->plan.Bs;
     int64_t launches = 0;
     for (int b0 = 0; b0 < b.B && rc == FSN_OK; b0 += Bs) {
@@ -1947,7 +1987,8 @@ static int run_plain(fsn_model* m, const Batch& b, cudaStream_t s) {
 // A device-buffer spectral call: check batch b, then run it plain or pipelined
 static int run_spectra(fsn_model* m, Batch b, void* stream) {
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (int rc = check_batch(m, b)) return rc;
+    std::vector<float> lam;
+    if (int rc = check_batch(m, b, nullptr, &lam)) return rc;
     if (b.call == CALL_FORWARD) return run_plain(m, b, s);
     if (int rc = ensure_pipeline(m)) return rc;
     CK(cudaEventRecord(m->ev_in, s));                                   // everything enqueued on the caller's stream so far (the inputs)
@@ -1960,7 +2001,7 @@ extern "C" int fsn_model_forward(fsn_model* m, const float* d_mag, const float* 
 }
 extern "C" int fsn_model_forward_enhance(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
                                          float* d_enh, void* stream) {
-    return run_spectra(m, Batch{CALL_FORWARD, d_mag, d_real, d_imag, B, T, nullptr, nullptr, d_enh}, stream);
+    return fsn_model_forward_enhance_lim(m, d_mag, d_real, d_imag, B, T, nullptr, nullptr, d_enh, stream);
 }
 
 extern "C" int fsn_model_forward_ragged(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
@@ -1969,14 +2010,26 @@ extern "C" int fsn_model_forward_ragged(fsn_model* m, const float* d_mag, const 
 }
 extern "C" int fsn_model_forward_enhance_ragged(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
                                                 const int32_t* h_frames, float* d_enh, void* stream) {
-    return run_spectra(m, Batch{CALL_FORWARD, d_mag, d_real, d_imag, B, T, h_frames, nullptr, d_enh}, stream);
+    return fsn_model_forward_enhance_lim(m, d_mag, d_real, d_imag, B, T, h_frames, nullptr, d_enh, stream);
+}
+extern "C" int fsn_model_forward_enhance_lim(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
+                                             const int32_t* h_frames, const float* h_atten_db, float* d_enh, void* stream) {
+    Batch b{CALL_FORWARD, d_mag, d_real, d_imag, B, T, h_frames, nullptr, d_enh};
+    b.atten_db = h_atten_db;
+    return run_spectra(m, b, stream);
 }
 
 extern "C" int fsn_model_enhance_audio(fsn_model* m, const float* d_wave, int32_t B, int64_t L, const int64_t* h_lengths, float* d_out,
                                        void* stream) {
+    return fsn_model_enhance_audio_lim(m, d_wave, B, L, h_lengths, nullptr, d_out, stream);
+}
+extern "C" int fsn_model_enhance_audio_lim(fsn_model* m, const float* d_wave, int32_t B, int64_t L, const int64_t* h_lengths,
+                                           const float* h_atten_db, float* d_out, void* stream) {
     Batch b{CALL_AUDIO, nullptr, nullptr, nullptr, B, 0, nullptr, nullptr, nullptr, d_wave, d_out, L, h_lengths};
+    b.atten_db = h_atten_db;
     std::vector<int32_t> lens;
-    if (int rc = check_batch(m, b, &lens)) return rc;
+    std::vector<float> lam;
+    if (int rc = check_batch(m, b, &lens, &lam)) return rc;
     return run_plain(m, b, static_cast<cudaStream_t>(stream));
 }
 
@@ -2203,6 +2256,9 @@ struct fsn_stream {
     // audio calls (DESIGN.md §3.10, §3.14): their scratch, allocated at their first use, grow-only: the spectra of the call's frames
     // [B, K, F], the model's input and output planes (runs of columns, see StreamAudioChunkLaunch) and the staged per-slot plan
     DevBuf x_spec, x_mag, x_mask, x_plan;
+    // attenuation floors of the audio calls (fsn_stream_set_atten_lim, DESIGN.md §3.18): [B] on the host, empty until first set; staged
+    // with each audio call's plan when any is > 0.  A handle setting, not session state
+    std::vector<float> lam;
 };
 
 int StepScratch::ensure(const fsn_stream& st, int K, size_t img, bool zero, cudaStream_t s) {
@@ -2750,6 +2806,9 @@ static int step_audio(fsn_stream* st, const float* d_samples, int K, const int32
         if (int rc = lw_groups(st, kf, &lw, &e, s)) return rc;
     size_t nstage = (size_t)7 * B + nzero;
     for (const LwGroup& g : lw) nstage += B + g.nact;
+    const bool lim = std::any_of(st->lam.begin(), st->lam.end(), [](float v) { return v > 0.f; });
+    const size_t lam_at = nstage;                                       // the slots' attenuation floors, last (when any is set)
+    if (lim) nstage += B;
     if (Km) e |= x.ensure(*st, Km, layerwise ? 0 : step_img_bytes(c, (long long)B * F, Km), false, s);
     e |= st->x_spec.ensure((size_t)B * K * F * sizeof(float2), false, s);
     e |= st->x_mag.ensure((size_t)B * F * Km * sizeof(float), false, s);
@@ -2773,6 +2832,7 @@ static int step_audio(fsn_stream* st, const float* d_samples, int K, const int32
         if (kf[b] && cnt[b] == 0) zero[z++] = b;
     }
     lw_stage(kf, lw, zero + nzero, d + 7 * B + nzero);
+    if (lim) memcpy(h + lam_at, st->lam.data(), (size_t)B * sizeof(float));
     if (int rc = st->stage.send(st->x_plan.p, nstage, s)) return rc;
     StreamAudioChunkLaunch a{};
     a.k0 = d; a.na = d + B; a.start = d + 2 * B; a.nstore = d + 3 * B; a.hops = d + 4 * B;
@@ -2783,6 +2843,7 @@ static int step_audio(fsn_stream* st, const float* d_samples, int K, const int32
     const AudioTables tab = audio_table_ptrs(static_cast<const float*>(st->a_tab.p), N);
     a.window = tab.window; a.twiddle = tab.twiddle; a.inv_env = tab.inv_env;
     a.B = B; a.K = K; a.Km = Km; a.n_fft = N; a.la = la;
+    a.lam = lim ? reinterpret_cast<const float*>(d + lam_at) : nullptr;
     launch_stream_stft_chunk(a, s);
     // at Km = 1 the counts alone say which slots step a frame: no frame counts, so the per-frame step's kernels and arguments
     if (Km)
@@ -2836,6 +2897,7 @@ struct fsn_chunk_stream {
     std::vector<int64_t> n, k;
     DevBuf ring, tail, window, plan, rows, enh, x_slot;
     PinnedStage stage;
+    std::vector<float> lam_db;                         // attenuation limits in dB (fsn_chunk_stream_set_atten_lim): [B], empty until first set
 };
 
 // The chunk lengths a handle can take on its own, whatever the model: even, H >= P, C + P < 2^30
@@ -2945,8 +3007,15 @@ extern "C" int fsn_chunk_stream_step(fsn_chunk_stream* cs, const float* d_sample
     // the batch of every completed chunk: rows [nrows, P + C]; the caller's buffers stand in for the rows until they are allocated
     Batch fwd{CALL_AUDIO, nullptr, nullptr, nullptr, nrows, 0, nullptr, nullptr, nullptr, d_samples, d_out, W, nullptr};
     std::vector<int32_t> lens;
+    std::vector<float> row_db, row_lam;                                 // each row enhanced with its slot's limit (check_batch drops
+    if (nrows && !cs->lam_db.empty()) {                                 // them when none is finite)
+        row_db.reserve((size_t)nrows);
+        for (int b = 0; b < B; ++b)
+            row_db.insert(row_db.end(), (size_t)plan[(size_t)b * CHUNK_PLAN_FIELDS + CP_NC], cs->lam_db[b]);
+        fwd.atten_db = row_db.data();
+    }
     if (nrows)
-        if (int rc = check_batch(cs->m, fwd, &lens)) return rc;
+        if (int rc = check_batch(cs->m, fwd, &lens, &row_lam)) return rc;
     const size_t rb = (size_t)nrows * W * sizeof(float);
     int e = nrows ? cs->rows.ensure(rb, false, s) | cs->enh.ensure(rb, false, s) : 0;
     if (e) return fail(FSN_ECUDA, "chunk row allocation failed (%d rows of %d samples)", nrows, W);
@@ -2973,6 +3042,42 @@ extern "C" int fsn_chunk_stream_step(fsn_chunk_stream* cs, const float* d_sample
         cs->n[b] = n1[b]; cs->k[b] = k1[b];
         h_nout[b] = plan[(size_t)b * CHUNK_PLAN_FIELDS + CP_NOUT];
     }
+    return FSN_OK;
+}
+
+// The checks of a set_atten_lim call on a handle of B slots (fsn_stream_set_atten_lim, fsn_chunk_stream_set_atten_lim): the arrays, n,
+// every slot in range and named once, every limit valid (atten_floor); *lam: the n floors.  Nothing is changed here.
+static int slot_limits_ok(int B, int32_t n, const int32_t* h_slots, const float* h_atten_db, std::vector<float>* lam) {
+    if (n < 1) return fail(FSN_EINVAL, "n = %d: at least one slot", n);
+    if (!h_slots) return fail(FSN_EINVAL, "h_slots is null (n = %d slot indices)", n);
+    if (!h_atten_db) return fail(FSN_EINVAL, "h_atten_db is null (n = %d limits in dB)", n);
+    std::vector<int> seen(B, -1);
+    lam->resize((size_t)n);
+    for (int i = 0; i < n; ++i) {
+        const int b = h_slots[i];
+        if (b < 0 || b >= B) return fail(FSN_EINVAL, "h_slots[%d] = %d is out of range (slots 0..%d)", i, b, B - 1);
+        if (seen[b] >= 0) return fail(FSN_EINVAL, "h_slots[%d] = %d: slot %d is named twice (also h_slots[%d])", i, b, b, seen[b]);
+        seen[b] = i;
+        if (int rc = atten_floor(h_atten_db[i], "slot", b, i, &(*lam)[i])) return rc;
+    }
+    return FSN_OK;
+}
+
+extern "C" int fsn_stream_set_atten_lim(fsn_stream* st, int32_t n, const int32_t* h_slots, const float* h_atten_db) {
+    if (!st) return fail(FSN_EINVAL, "st is null");
+    std::vector<float> lam;
+    if (int rc = slot_limits_ok(st->B, n, h_slots, h_atten_db, &lam)) return rc;
+    if (st->lam.empty()) st->lam.assign((size_t)st->B, 0.f);
+    for (int i = 0; i < n; ++i) st->lam[h_slots[i]] = lam[i];
+    return FSN_OK;
+}
+
+extern "C" int fsn_chunk_stream_set_atten_lim(fsn_chunk_stream* cs, int32_t n, const int32_t* h_slots, const float* h_atten_db) {
+    if (!cs) return fail(FSN_EINVAL, "cs is null");
+    std::vector<float> lam;
+    if (int rc = slot_limits_ok(cs->B, n, h_slots, h_atten_db, &lam)) return rc;
+    if (cs->lam_db.empty()) cs->lam_db.assign((size_t)cs->B, INFINITY);
+    for (int i = 0; i < n; ++i) cs->lam_db[h_slots[i]] = h_atten_db[i];
     return FSN_OK;
 }
 

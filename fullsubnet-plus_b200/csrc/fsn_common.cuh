@@ -50,6 +50,16 @@ __device__ __forceinline__ float decompress_cirm(float v) {
     return -10.f * logf((10.f - v) / (10.f + v));
 }
 
+// Attenuation limit (DESIGN.md §3.18) on a decompressed complex mask (m0, m1): a magnitude below lam = 10^(-L / 20) is raised to lam,
+// keeping the mask's phase; a zero mask becomes (lam, 0).  lam = 0 (L = +inf) leaves every mask as it is.  So |M' X| >= lam |X|.
+__device__ __forceinline__ void limit_mask(float& m0, float& m1, float lam) {
+    const float a2 = m0 * m0 + m1 * m1;
+    if (a2 < lam * lam) {
+        if (a2 > 0.f) { const float s = lam / sqrtf(a2); m0 *= s; m1 *= s; }
+        else { m0 = lam; m1 = 0.f; }
+    }
+}
+
 __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
     __half2 h = __floats2half2_rn(lo, hi);
     return *reinterpret_cast<uint32_t*>(&h);

@@ -112,9 +112,10 @@ void launch_fb_pack(const float* x, __half* y, int B, int F, int Tp, int P, int 
 
 void launch_apply_cirm(const float* crm, const float2* noisy, float2* enh, int B, int F, int T, cudaStream_t s);
 // same with the noisy spectrum as two planes [B, F, T] (the model's own real / imag inputs); with tlen [B], frames
-// t >= tlen[b] - la are written as zero without reading the planes
+// t >= tlen[b] - la are written as zero without reading the planes; with lam [B] (device, or null: no limit) each clip's mask gets
+// its attenuation floor (limit_mask, DESIGN.md §3.18)
 void launch_apply_cirm_planar(const float* crm, const float* nreal, const float* nimag, float2* enh, int B, int F, int T, const int* tlen,
-                              int la, cudaStream_t s);
+                              int la, cudaStream_t s, const float* lam = nullptr);
 
 // streaming step kernels (k_front.cu): K frames of the cumulative norms with running sums carried in global memory, frame after
 // frame.  slot: null (every slot is at frame n), or [B] per-slot frame counts of the slot calls, -1 = held: a held slot's frames are
@@ -187,6 +188,7 @@ struct StreamAudioChunkLaunch {
     const float2* twiddle;    // [n_fft / 2 + 1] exp(-2 pi i k / n_fft)
     const float* inv_env;     // [hop] 1 / (w^2(i) + w^2(i + hop))
     int B, K, Km, n_fft, la;  // Km: model columns, the largest frame count of the call; n_fft: power of two, 64 .. 1024
+    const float* lam;         // optional [B] attenuation floor of each slot (limit_mask, DESIGN.md §3.18); null: the unlimited synthesis
 };
 void launch_stream_stft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s);
 void launch_stream_istft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s);
@@ -317,6 +319,8 @@ struct LstmTc5rLaunch {
     // noisy spectrum (planes [B, F, T]) instead of writing the mask: enh [B, F, T] complex64 (interleaved re, im)
     const float* nreal; const float* nimag; float2* enh;
     const int* tlen;          // optional [B] per-sample extent in frames of Tp: output frames t - la >= tlen[b] - la are written as zero
+    const float* lam;         // with enh: optional [B] attenuation floor of each clip (limit_mask, DESIGN.md §3.18); null: no limit, and
+                              // the launch runs the kernel instantiated without it
 };
 bool lstm_tc5r_supported(int H, int O);
 size_t lstm_tc5r_cstate_bytes(int ntiles, int H);
@@ -336,7 +340,9 @@ bool gemm_f16_pair_tiles(const GemmF16Launch& g);
 int launch_gemm_f16(const void* A, const void* B, const GemmF16Launch& a, int num_sms, cudaStream_t s);
 int make_tmap_f16_2d(void* out_map /*128 B, 64 B aligned*/, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows);   // box = 64 halves x box_rows, SWIZZLE_128B
 
-enum { EPI5_PRELU_STATS = 1, EPI5_GLN_RES = 2, EPI5_OUT = 3, EPI5_F16OUT = 4, EPI5_GLN_HEAD = 5 };
+// EPI5_GLN_HEAD_LIM: EPI5_GLN_HEAD writing the enhanced spectrum with each clip's attenuation floor lam[z / Fg] (a sibling instantiation,
+// so the unlimited head is unchanged)
+enum { EPI5_PRELU_STATS = 1, EPI5_GLN_RES = 2, EPI5_OUT = 3, EPI5_F16OUT = 4, EPI5_GLN_HEAD = 5, EPI5_GLN_HEAD_LIM = 6 };
 struct GemmTc5Launch {
     int Kp, NT, nstage, ntiles_n, Npad;        // K (multiple of 32; GLN_RES: fp16 operands, multiple of 64), N tile (64 or 128), ring depth, N tiles and padded N per branch
     int rows_per_branch, tiles_m, nbranch, Tp, B;
@@ -363,6 +369,7 @@ struct GemmTc5Launch {
     // GLN_HEAD: group z is bin f0 + z % Fg of clip z / Fg (a chunk of Fg bins from f0; Fg = F, f0 = 0: every bin).  F still sets the
     // layout of the mask, the enhanced spectrum and the noisy planes
     int Fg, f0;
+    const float* lam;                          // GLN_HEAD_LIM: [B] attenuation floor of each clip (limit_mask, DESIGN.md §3.18)
 };
 int make_tmap_f32_2d(void* out_map /*128 B, 64 B aligned*/, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows);
 int launch_gemm_tc5(const void* mapA, const void* mapB, GemmTc5Launch a, int num_sms, cudaStream_t s);

@@ -987,20 +987,24 @@ __global__ void apply_cirm_kernel(const float* crm, const float2* noisy, float2*
     const float2 x = noisy[i];
     enh[i] = make_float2(m[0] * x.x - m[1] * x.y, m[1] * x.x + m[0] * x.y);
 }
+// LIM: each clip's attenuation floor lam[b] (limit_mask); the instantiation without it is the pass as it was before limits existed
+template <bool LIM>
 __global__ void apply_cirm_planar_kernel(const float* crm, const float* nreal, const float* nimag, float2* enh, int T, int FT, size_t n,
-                                         const int* tlen, int la) {
+                                         const int* tlen, int la, const float* lam) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const size_t b = i / FT, e = i % FT;
     if (tlen && (int)(e % T) >= tlen[b] - la) { enh[i] = make_float2(0.f, 0.f); return; }   // past the clip: the planes are not read
-    const float m0 = decompress_cirm(crm[(b * 2 + 0) * FT + e]), m1 = decompress_cirm(crm[(b * 2 + 1) * FT + e]);
+    float m0 = decompress_cirm(crm[(b * 2 + 0) * FT + e]), m1 = decompress_cirm(crm[(b * 2 + 1) * FT + e]);
+    if (LIM) limit_mask(m0, m1, __ldg(lam + b));
     const float xr = nreal[i], xi = nimag[i];
     enh[i] = make_float2(m0 * xr - m1 * xi, m1 * xr + m0 * xi);
 }
 void launch_apply_cirm_planar(const float* crm, const float* nreal, const float* nimag, float2* enh, int B, int F, int T, const int* tlen,
-                              int la, cudaStream_t s) {
+                              int la, cudaStream_t s, const float* lam) {
     const size_t n = (size_t)B * F * T;
-    apply_cirm_planar_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(crm, nreal, nimag, enh, T, F * T, n, tlen, la);
+    if (lam) apply_cirm_planar_kernel<true><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(crm, nreal, nimag, enh, T, F * T, n, tlen, la, lam);
+    else apply_cirm_planar_kernel<false><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(crm, nreal, nimag, enh, T, F * T, n, tlen, la, lam);
 }
 void launch_apply_cirm(const float* crm, const float2* noisy, float2* enh, int B, int F, int T, cudaStream_t s) {
     const size_t n = (size_t)B * F * T;

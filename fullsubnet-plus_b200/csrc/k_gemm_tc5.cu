@@ -143,7 +143,8 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     // reads is overwritten) before this point
     pdl_trigger();
     pdl_wait();
-    constexpr bool AH = (EPI == EPI5_GLN_RES || EPI == EPI5_F16OUT || EPI == EPI5_GLN_HEAD);   // fp16 operands: a 128-byte swizzle atom holds 64 k-elements instead of 32
+    constexpr bool HEAD = (EPI == EPI5_GLN_HEAD || EPI == EPI5_GLN_HEAD_LIM);
+    constexpr bool AH = (EPI == EPI5_GLN_RES || EPI == EPI5_F16OUT || HEAD);   // fp16 operands: a 128-byte swizzle atom holds 64 k-elements instead of 32
     constexpr int KBW = AH ? 64 : 32;
     const int nkb = a.Kp / KBW;
     const int tiles_per_branch = a.tiles_m * a.ntiles_n;
@@ -281,7 +282,7 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
 #pragma unroll
                 for (int h = 0; h < 2; ++h) g5_max_add(valid[h] ? z[h] : -1, rowmax[h], a.amax_out);
             }
-        } else if constexpr (EPI == EPI5_GLN_HEAD) {
+        } else if constexpr (HEAD) {
             static_assert(NT == 64, "the head needs all channels of a row in one lane quad");
             const float* bias = a.bias[br];
             const float* s1 = a.s1[br];
@@ -327,8 +328,9 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                     else
                         for (int q = 0; q < a.O; ++q) a.out[(((size_t)ob * a.O + q) * a.F + of) * Tout + (tt[h] - a.la)] = 0.f;
                 } else if (a.enh) {                            // fused decompress_cIRM x noisy spectrum (inferencer.py:152-157), O = 2
-                    const float m0 = decompress_cirm(apply_act(fc[h][0] + __ldg(a.fc_b), a.act));
-                    const float m1 = decompress_cirm(apply_act(fc[h][1] + __ldg(a.fc_b + 1), a.act));
+                    float m0 = decompress_cirm(apply_act(fc[h][0] + __ldg(a.fc_b), a.act));
+                    float m1 = decompress_cirm(apply_act(fc[h][1] + __ldg(a.fc_b + 1), a.act));
+                    if constexpr (EPI == EPI5_GLN_HEAD_LIM) limit_mask(m0, m1, __ldg(a.lam + ob));   // the clip's attenuation floor
                     const float nr = __ldg(a.nreal + ni), nim = __ldg(a.nimag + ni);
                     a.enh[ni] = make_float2(m0 * nr - m1 * nim, m1 * nr + m0 * nim);
                 } else {
@@ -403,14 +405,17 @@ static int g5_launch(const CUtensorMap& mA, const CUtensorMap& mB, GemmTc5Launch
 }
 
 int launch_gemm_tc5(const void* mapA, const void* mapB, GemmTc5Launch a, int num_sms, cudaStream_t s) {
-    const bool f16k = a.epi == EPI5_GLN_RES || a.epi == EPI5_GLN_HEAD;
+    const bool head = a.epi == EPI5_GLN_HEAD || a.epi == EPI5_GLN_HEAD_LIM;
+    const bool f16k = a.epi == EPI5_GLN_RES || head;
     if ((a.NT != 64 && a.NT != 128) || a.Kp % (f16k ? 64 : 32) || a.Npad % 2) return (int)cudaErrorInvalidValue;
-    if (a.epi == EPI5_GLN_HEAD && (a.NT != 64 || a.Npad != 64 || a.ntiles_n != 1 || a.nbranch != 1 || a.O < 1 || a.O > 8 || (a.enh && a.O != 2)))
+    if (head && (a.NT != 64 || a.Npad != 64 || a.ntiles_n != 1 || a.nbranch != 1 || a.O < 1 || a.O > 8 || (a.enh && a.O != 2)))
         return (int)cudaErrorInvalidValue;
+    if (a.epi == EPI5_GLN_HEAD_LIM && (!a.enh || !a.lam)) return (int)cudaErrorInvalidValue;
     const CUtensorMap& mA = *reinterpret_cast<const CUtensorMap*>(mapA);
     const CUtensorMap& mB = *reinterpret_cast<const CUtensorMap*>(mapB);
     if (a.NT == 64) {
         if (a.epi == EPI5_GLN_HEAD) return g5_launch<EPI5_GLN_HEAD, 64>(mA, mB, a, num_sms, s);
+        if (a.epi == EPI5_GLN_HEAD_LIM) return g5_launch<EPI5_GLN_HEAD_LIM, 64>(mA, mB, a, num_sms, s);
         if (a.epi == EPI5_PRELU_STATS) return g5_launch<EPI5_PRELU_STATS, 64>(mA, mB, a, num_sms, s);
         if (a.epi == EPI5_GLN_RES) return g5_launch<EPI5_GLN_RES, 64>(mA, mB, a, num_sms, s);
         return g5_launch<EPI5_OUT, 64>(mA, mB, a, num_sms, s);

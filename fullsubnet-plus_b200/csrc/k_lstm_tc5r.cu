@@ -61,7 +61,9 @@ bool lstm_tc5r_supported(int H, int O) { return H % 64 == 0 && H >= 64 && H <= 5
 size_t lstm_tc5r_cstate_bytes(int ntiles, int H) { return (size_t)((ntiles + 1) / 2 * 2) * H * 128 * sizeof(float); }
 int64_t lstm_tc5r_weight_stream_bytes(int H) { return (int64_t)(H / 32) * (H / 64) * R5_STAGE; }
 
-template <int H, bool FAST, bool GRU, bool LAST>
+// LIM (last layer with enh only): each clip's mask gets its attenuation floor a.lam[clip] before the product (limit_mask); a sibling
+// instantiation, so the kernels without a limit are the same code as before it existed
+template <int H, bool FAST, bool GRU, bool LAST, bool LIM = false>
 __global__ void __cluster_dims__(R5_CL, 1, 1) __launch_bounds__(R5_THREADS, 1) lstm_tc5r_kernel(LstmTc5rLaunch a, int nstage) {
     extern __shared__ uint8_t smem_raw[];
     constexpr int NCH = H / 32, KBH = H / 64, HBUF = KBH * R5_ROWS * 128;
@@ -281,7 +283,8 @@ __global__ void __cluster_dims__(R5_CL, 1, 1) __launch_bounds__(R5_THREADS, 1) l
                     const float o1 = apply_act(fc1[h] + fcpart[((t & 1) * R5_ROWS + rl[h]) * 2 + 1] + __ldg(a.fc_b + 1), a.act);
                     const size_t ni = ((size_t)ob * a.F + of) * Tout + (t - a.la);
                     if (a.enh) {                                       // fused decompress_cIRM x noisy spectrum (inferencer.py:152-157)
-                        const float m0 = decompress_cirm(o0), m1 = decompress_cirm(o1);
+                        float m0 = decompress_cirm(o0), m1 = decompress_cirm(o1);
+                        if (LIM) limit_mask(m0, m1, __ldg(a.lam + ob));
                         const float nr = __ldg(a.nreal + ni), nim = __ldg(a.nimag + ni);
                         a.enh[ni] = make_float2(m0 * nr - m1 * nim, m1 * nr + m0 * nim);
                     } else {
@@ -304,16 +307,24 @@ __global__ void __cluster_dims__(R5_CL, 1, 1) __launch_bounds__(R5_THREADS, 1) l
     cluster_sync_all();                                            // no CTA leaves while its peer may still arrive on its barriers
 }
 
-template <int HH, bool FF, bool GG, bool LL>
+template <int HH, bool FF, bool GG, bool LL, bool LIM = false>
 static int r5_go(const LstmTc5rLaunch& a, int grid, const R5Plan& p, cudaStream_t s) {
-    cudaError_t e = cudaFuncSetAttribute(lstm_tc5r_kernel<HH, FF, GG, LL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.total);
+    cudaError_t e = cudaFuncSetAttribute(lstm_tc5r_kernel<HH, FF, GG, LL, LIM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.total);
     if (e != cudaSuccess) return (int)e;
-    lstm_tc5r_kernel<HH, FF, GG, LL><<<grid, R5_THREADS, p.total, s>>>(a, p.nstage);
+    lstm_tc5r_kernel<HH, FF, GG, LL, LIM><<<grid, R5_THREADS, p.total, s>>>(a, p.nstage);
     return (int)cudaGetLastError();
 }
 template <int HH>
 static int r5_dispatch(const LstmTc5rLaunch& a, int grid, const R5Plan& p, cudaStream_t s) {
     const int key = (a.fast ? 4 : 0) | (a.gru ? 2 : 0) | (a.last ? 1 : 0);
+    if (a.last && a.enh && a.lam) {                                 // the last layer with an attenuation limit
+        switch (key) {
+            case 1: return r5_go<HH, false, false, true, true>(a, grid, p, s);
+            case 3: return r5_go<HH, false, true, true, true>(a, grid, p, s);
+            case 5: return r5_go<HH, true, false, true, true>(a, grid, p, s);
+            default: return r5_go<HH, true, true, true, true>(a, grid, p, s);
+        }
+    }
     switch (key) {
         case 0: return r5_go<HH, false, false, false>(a, grid, p, s);
         case 1: return r5_go<HH, false, false, true>(a, grid, p, s);

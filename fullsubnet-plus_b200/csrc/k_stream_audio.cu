@@ -40,13 +40,15 @@ __device__ __forceinline__ void analyse_frame(const float* hist, int j, int L, i
 
 // Synthesis of one frame from its mask rows mask[f ms], mask[(F + f) ms] and noisy spectrum spec: the second half of the windowed
 // inverse transform becomes the tail; with emit, out[i] = (tail + first half) / env (the session's next hop), else out[i] = 0.
-// z, e: shared scratch of H and H + 1 points.
+// z, e: shared scratch of H and H + 1 points.  LIM: the mask gets the slot's attenuation floor lam (limit_mask, DESIGN.md §3.18).
+template <bool LIM>
 __device__ __forceinline__ void synth_frame(const float* mask, int ms, const float2* spec, float* tail, float* out, bool emit, int H,
                                             int lg, const float* __restrict__ window, const float2* __restrict__ twiddle,
-                                            const float* __restrict__ inv_env, float2* z, float2* e) {
+                                            const float* __restrict__ inv_env, float2* z, float2* e, float lam) {
     const int F = H + 1;
     for (int f = threadIdx.x; f < F; f += blockDim.x) {          // decompress_cIRM x noisy spectrum (inferencer.py:152-157)
-        const float m0 = decompress_cirm(mask[f * ms]), m1 = decompress_cirm(mask[(F + f) * ms]);
+        float m0 = decompress_cirm(mask[f * ms]), m1 = decompress_cirm(mask[(F + f) * ms]);
+        if (LIM) limit_mask(m0, m1, lam);
         const float2 x = spec[f];
         float2 E = make_float2(m0 * x.x - m1 * x.y, m1 * x.x + m0 * x.y);
         if (f == 0 || f == H) E.y = 0.f;                         // a real inverse transform ignores the DC and Nyquist imaginary parts
@@ -103,7 +105,9 @@ __global__ void __launch_bounds__(AUDIO_THREADS) stream_stft_chunk_kernel(Stream
 // grid B: the synthesis of a slot's model columns, in order.  Column c synthesises frame m = j - la (if m >= 0) from its mask and the
 // spectrum of frame m: from the scratch if this call analysed it, else from the ring.  Emitted hops fill the front of the output row
 // and the rest is zero.  Then the caller's masks by tick (zero on the START tick and past the active ticks) and the ring's last la + 1
-// frames, written only after every read of the ring.
+// frames, written only after every read of the ring.  LIM: with the slots' attenuation floors a.lam (the instantiation without them is
+// the synthesis as it was before limits existed).
+template <bool LIM>
 __global__ void __launch_bounds__(AUDIO_THREADS) stream_istft_chunk_kernel(StreamAudioChunkLaunch a) {
     __shared__ float2 z[AUDIO_MAX_HOP];
     __shared__ float2 e[AUDIO_MAX_HOP + 1];
@@ -114,14 +118,15 @@ __global__ void __launch_bounds__(AUDIO_THREADS) stream_istft_chunk_kernel(Strea
     float* tail = a.tail + (size_t)b * H;
     float2* ring = a.spec + (size_t)b * R * F;
     const float2* sspec = a.sspec + (size_t)b * K * F;
+    const float lam = LIM ? __ldg(a.lam + b) : 0.f;
     int nout = 0;
     for (int c = 0; c < kf; ++c) {
         const int m = j0 + c - a.la;
         if (m < 0) continue;
         __syncthreads();                                         // the last frame's reads of z and e are done
         const float2* spec = m >= j0 ? sspec + (size_t)(m - j0) * F : ring + (m % R) * F;
-        synth_frame(a.mask + chunk_col(a, b, c, 2 * F), a.Km, spec, tail, out + (size_t)nout * H, m >= 1, H, lg, a.window,
-                    a.twiddle, a.inv_env, z, e);
+        synth_frame<LIM>(a.mask + chunk_col(a, b, c, 2 * F), a.Km, spec, tail, out + (size_t)nout * H, m >= 1, H, lg, a.window,
+                         a.twiddle, a.inv_env, z, e, lam);
         nout += m >= 1;
     }
     for (size_t t = (size_t)nout * H + threadIdx.x; t < (size_t)K * H; t += blockDim.x) out[t] = 0.f;
@@ -140,6 +145,9 @@ __global__ void __launch_bounds__(AUDIO_THREADS) stream_istft_chunk_kernel(Strea
 }
 
 void launch_stream_stft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s) { stream_stft_chunk_kernel<<<a.B, AUDIO_THREADS, 0, s>>>(a); }
-void launch_stream_istft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s) { stream_istft_chunk_kernel<<<a.B, AUDIO_THREADS, 0, s>>>(a); }
+void launch_stream_istft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s) {
+    if (a.lam) stream_istft_chunk_kernel<true><<<a.B, AUDIO_THREADS, 0, s>>>(a);
+    else stream_istft_chunk_kernel<false><<<a.B, AUDIO_THREADS, 0, s>>>(a);
+}
 
 }  // namespace fsn

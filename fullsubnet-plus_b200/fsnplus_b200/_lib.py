@@ -29,6 +29,7 @@ SYMBOLS = [
     "fsn_model_file_write", "fsn_model_file_config", "fsn_model_load",
     "fsn_chunk_stream_create", "fsn_chunk_stream_step", "fsn_chunk_stream_destroy",
     "fsn_chunk_stream_state_layout", "fsn_chunk_stream_save_slots", "fsn_chunk_stream_load_slots",
+    "fsn_model_forward_enhance_lim", "fsn_model_enhance_audio_lim", "fsn_stream_set_atten_lim", "fsn_chunk_stream_set_atten_lim",
 ]
 
 
@@ -205,6 +206,10 @@ def load_library():
     lib.fsn_chunk_stream_state_layout.argtypes = [i32, C.POINTER(i64), C.POINTER(i32)]
     lib.fsn_chunk_stream_save_slots.argtypes = [vp, i32, vp, vp, vp, vp]
     lib.fsn_chunk_stream_load_slots.argtypes = [vp, i32, vp, vp, vp, vp]
+    lib.fsn_model_forward_enhance_lim.argtypes = [vp, vp, vp, vp, i32, i32, C.POINTER(i32), fp, vp, vp]
+    lib.fsn_model_enhance_audio_lim.argtypes = [vp, vp, i32, i64, C.POINTER(i64), fp, vp, vp]
+    lib.fsn_stream_set_atten_lim.argtypes = [vp, i32, C.POINTER(i32), fp]
+    lib.fsn_chunk_stream_set_atten_lim.argtypes = [vp, i32, C.POINTER(i32), fp]
     _LIB = lib
     return lib
 
@@ -269,6 +274,32 @@ def lengths_arg(lengths, B):
     if len(lengths) != B:
         raise ValueError(f"lengths has {len(lengths)} entries for a batch of {B}")
     return (C.c_int64 * B)(*lengths)
+
+
+def atten_arg(atten_lim_db, B):
+    """An attenuation limit in dB (DESIGN.md §3.18) as a C float array of B values, or None: ``atten_lim_db`` is None (no limit), one
+    number (every clip or slot) or B numbers (a sequence or a 1-D CPU tensor).  float('inf') is no limit; the library refuses a negative
+    or NaN value, naming the clip or slot."""
+    if atten_lim_db is None:
+        return None
+    if hasattr(atten_lim_db, "is_cuda"):
+        if atten_lim_db.is_cuda or atten_lim_db.is_complex() or atten_lim_db.dim() > 1:
+            raise ValueError("atten_lim_db must be a number, a sequence of numbers or a 0-/1-D CPU tensor")
+        atten_lim_db = atten_lim_db.tolist()
+    if isinstance(atten_lim_db, (int, float)):
+        vals = [float(atten_lim_db)] * B
+    else:
+        vals = [float(v) for v in atten_lim_db]
+        if len(vals) != B:
+            raise ValueError(f"atten_lim_db has {len(vals)} entries for {B} clips / slots")
+    return (C.c_float * B)(*vals)
+
+
+def atten_floor(db):
+    """The floor lam = 10^(-db / 20) of an attenuation limit of ``db`` dB, computed in double and rounded to float32 as the library
+    does (float('inf'): 0.0, no limit)."""
+    import numpy as np
+    return float(np.float32(10.0 ** (-float(db) / 20.0)))
 
 
 def plan_audio(cfg, B, L, lengths=None, cap_bytes=None, force_window=0, force_bins=0):

@@ -86,13 +86,21 @@ def apply_cirm(crm, X):
 
 
 @torch.no_grad()
-def enhance_batch(model, noisy, n_fft=512, hop_length=256, win_length=512, complex_inputs=True):
+def _atten_ok(model, X, atten_lim_db):
+    if atten_lim_db is not None and not (hasattr(model, "enhance_spectrum") and X.is_cuda):
+        raise ValueError("atten_lim_db needs an fsnplus_b200 model on a CUDA device (the limit is applied inside its enhance call)")
+
+
+@torch.no_grad()
+def enhance_batch(model, noisy, n_fft=512, hop_length=256, win_length=512, complex_inputs=True, atten_lim_db=None):
     """noisy [B, L] float32 on the model's device -> enhanced [B, L].
-    complex_inputs=True mirrors mag_complex_full_band_crm_mask (FullSubNet_Plus), False full_band_crm_mask (Model)."""
+    complex_inputs=True mirrors mag_complex_full_band_crm_mask (FullSubNet_Plus), False full_band_crm_mask (Model).
+    atten_lim_db: None, or a limit in dB for every clip or one per clip (``enhance_spectrum``, DESIGN.md §3.18)."""
     X = stft(noisy, n_fft, hop_length, win_length)
     mag = X.abs().unsqueeze(1)
+    _atten_ok(model, X, atten_lim_db)
     if hasattr(model, "enhance_spectrum") and X.is_cuda:          # model + decompress + complex multiply in one call (fused epilogue)
-        enh = model.enhance_spectrum(mag, X.real.unsqueeze(1).contiguous(), X.imag.unsqueeze(1).contiguous())
+        enh = model.enhance_spectrum(mag, X.real.unsqueeze(1).contiguous(), X.imag.unsqueeze(1).contiguous(), atten_lim_db=atten_lim_db)
         return istft(enh, n_fft, hop_length, win_length, length=noisy.size(-1))
     if complex_inputs:
         crm = model(mag, X.real.unsqueeze(1).contiguous(), X.imag.unsqueeze(1).contiguous())
@@ -102,7 +110,7 @@ def enhance_batch(model, noisy, n_fft=512, hop_length=256, win_length=512, compl
 
 
 @torch.no_grad()
-def enhance_ragged(model, clips, n_fft=512, hop_length=256, win_length=512, complex_inputs=True):
+def enhance_ragged(model, clips, n_fft=512, hop_length=256, win_length=512, complex_inputs=True, atten_lim_db=None):
     """Clips of different lengths in ONE model call: ``clips`` is a list of 1-D waveforms on one device; returns the list of
     enhanced waveforms, each as long as its input and equal to what ``enhance_batch`` gives for that clip alone.
 
@@ -110,7 +118,7 @@ def enhance_ragged(model, clips, n_fft=512, hop_length=256, win_length=512, comp
     frames, whose windows reach past its end.  The spectra are scattered into a zero [B, F, T_max] batch and the model runs once with
     ``frames`` = every clip's own frame count (the forward masks each clip at its own end).  The iSTFT runs per clip over the clip's
     own frames only: a batched iSTFT over the padded spectra would put the padded frames into the window envelope
-    of the last hop."""
+    of the last hop.  atten_lim_db: as in ``enhance_batch``."""
     if len(clips) == 0:
         return []
     lengths = [int(c.numel()) for c in clips]
@@ -127,8 +135,10 @@ def enhance_ragged(model, clips, n_fft=512, hop_length=256, win_length=512, comp
     for n, idx in groups.items():
         X[idx, :, :specs[n].size(-1)] = specs[n]
     mag = X.abs().unsqueeze(1)
+    _atten_ok(model, X, atten_lim_db)
     if hasattr(model, "enhance_spectrum") and X.is_cuda:
-        enh = model.enhance_spectrum(mag, X.real.unsqueeze(1).contiguous(), X.imag.unsqueeze(1).contiguous(), frames=frames)
+        enh = model.enhance_spectrum(mag, X.real.unsqueeze(1).contiguous(), X.imag.unsqueeze(1).contiguous(), frames=frames,
+                                     atten_lim_db=atten_lim_db)
     else:
         crm = (model(mag, X.real.unsqueeze(1).contiguous(), X.imag.unsqueeze(1).contiguous(), frames=frames) if complex_inputs
                else model(mag, frames=frames))

@@ -211,30 +211,42 @@ class _B200Model(nn.Module):
         if x is not None and not x.is_cuda:
             raise RuntimeError("fsnplus_b200 has no CPU fallback: move the model and its inputs to a CUDA (H100) device")
 
-    def enhance_spectrum(self, noisy_mag, noisy_real, noisy_imag, pipelined=False, out=None, hold=True, frames=None):
+    def enhance_spectrum(self, noisy_mag, noisy_real, noisy_imag, pipelined=False, out=None, hold=True, frames=None, atten_lim_db=None):
         """Model forward + decompress_cIRM + complex multiply with the noisy spectrum in ONE call (C ABI: fsn_model_forward_enhance /
         fsn_model_submit_enhance; reference inferencer.py:149-157): [B, 1, F, T] x3 -> enhanced spectrum complex64 [B, F, T], the
         argument of the inferencer's iSTFT.  The cIRM never goes to memory (fused into the sub-band LSTM's epilogue).
-        ``pipelined=True``: like ``submit()`` -- valid after ``wait()`` / ``wait_lane()``.  ``frames``: as in ``forward()``."""
-        return self._run(noisy_mag, noisy_real, noisy_imag, enhance=True, pipelined=pipelined, out=out, hold=hold, frames=frames)
+        ``pipelined=True``: like ``submit()`` -- valid after ``wait()`` / ``wait_lane()``.  ``frames``: as in ``forward()``.
+        ``atten_lim_db``: None, one number or B numbers -- no bin of clip b loses more than atten_lim_db[b] dB (C ABI:
+        fsn_model_forward_enhance_lim, DESIGN.md §3.18; float('inf'): no limit).  The pipelined call takes no limit (ValueError)."""
+        if atten_lim_db is not None and pipelined:
+            raise ValueError("atten_lim_db is not supported with pipelined=True (the pipelined entry points take no limit)")
+        return self._run(noisy_mag, noisy_real, noisy_imag, enhance=True, pipelined=pipelined, out=out, hold=hold, frames=frames,
+                         atten_lim_db=atten_lim_db)
 
-    def enhance_audio(self, wave, lengths=None):
+    def enhance_audio(self, wave, lengths=None, atten_lim_db=None):
         """Waveforms in, enhanced waveforms out in ONE call (C ABI: fsn_model_enhance_audio): torch.stft -> model -> decompress_cIRM x
         spectrum -> torch.istft(length = L_b) per clip, with both transforms on the device (what ``inference.enhance_batch`` /
         ``enhance_ragged`` compute).  ``wave``: [B, L] float32 CUDA; ``lengths``: None (every clip is L samples) or B sample counts (a
         sequence or a 1-D CPU integer tensor), clip b being the first lengths[b] samples of its row.  Returns [B, L], zero past each
-        clip's length.  n_fft = 2 (num_freqs - 1), hop = n_fft / 2, periodic Hann window."""
+        clip's length.  n_fft = 2 (num_freqs - 1), hop = n_fft / 2, periodic Hann window.  ``atten_lim_db``: None, one number or B
+        numbers -- no bin of clip b loses more than atten_lim_db[b] dB (C ABI: fsn_model_enhance_audio_lim, DESIGN.md §3.18;
+        float('inf'): no limit)."""
         if wave.dim() != 2:
             raise ValueError(f"enhance_audio: wave must be [B, L], got {tuple(wave.shape)}")
         self._check_call(wave)
         B, L = wave.shape
         hl = _lib.lengths_arg(lengths, B)
+        ha = _lib.atten_arg(atten_lim_db, B)
         x = wave.detach().to(dtype=torch.float32).contiguous()
         with torch.cuda.device(x.device):
             lib = self._ensure_handle(x.device)
             out = torch.empty((B, L), dtype=torch.float32, device=x.device)
             stream = C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
-            _lib.check(lib.fsn_model_enhance_audio(self._handle, C.c_void_p(x.data_ptr()), B, L, hl, C.c_void_p(out.data_ptr()), stream))
+            if ha is None:
+                _lib.check(lib.fsn_model_enhance_audio(self._handle, C.c_void_p(x.data_ptr()), B, L, hl, C.c_void_p(out.data_ptr()), stream))
+            else:
+                _lib.check(lib.fsn_model_enhance_audio_lim(self._handle, C.c_void_p(x.data_ptr()), B, L, hl, ha, C.c_void_p(out.data_ptr()),
+                                                           stream))
         return out
 
     @staticmethod
@@ -249,12 +261,13 @@ class _B200Model(nn.Module):
             raise ValueError(f"frames has {len(frames)} entries for a batch of {B}")
         return (C.c_int32 * B)(*frames)
 
-    def _run(self, mag, real, imag, enhance=False, pipelined=False, out=None, hold=True, frames=None):
+    def _run(self, mag, real, imag, enhance=False, pipelined=False, out=None, hold=True, frames=None, atten_lim_db=None):
         assert mag.dim() == 4                                            # fullsubnet_plus.py:136
         B, Cn, F, T = mag.shape
         if frames is not None and pipelined:
             raise ValueError("frames (ragged batches) is not supported with pipelined=True / submit()")
         hframes = self._frames_arg(frames, B) if frames is not None else None
+        hatten = _lib.atten_arg(atten_lim_db, B)
         assert Cn == 1, f"{self.__class__.__name__} takes the mag feature as inputs."      # :141
         self._check_call(mag)
         if F != self._cfg.num_freqs:
@@ -267,6 +280,10 @@ class _B200Model(nn.Module):
                        torch.empty((B, self._cfg.output_size, F, T), dtype=torch.float32, device=mag.device))
             ptr = lambda x: C.c_void_p(x.data_ptr()) if x is not None else C.c_void_p()
             stream = C.c_void_p(torch.cuda.current_stream(mag.device).cuda_stream)
+            if hatten is not None:                                          # enhance only (enhance_spectrum)
+                _lib.check(lib.fsn_model_forward_enhance_lim(self._handle, ptr(ins[0]), ptr(ins[1]), ptr(ins[2]), B, T, hframes, hatten,
+                                                             ptr(out), stream))
+                return out
             if hframes is not None:
                 fn = lib.fsn_model_forward_enhance_ragged if enhance else lib.fsn_model_forward_ragged
                 _lib.check(fn(self._handle, ptr(ins[0]), ptr(ins[1]), ptr(ins[2]), B, T, hframes, ptr(out), stream))

@@ -241,6 +241,15 @@ class StreamingFullSubNet:
             _lib.check(self.lib.fsn_stream_load_slots(self._st, s.numel(), C.c_void_p(s.data_ptr()), C.c_void_p(payload.data_ptr()),
                                                       state.meta, stream))
 
+    def set_atten_lim(self, slots, db):
+        """Attenuation limit of `slots` (a sequence or a CPU integer tensor) in dB -- one number for all of them or one per slot,
+        float('inf') = no limit (DESIGN.md §3.18; C: fsn_stream_set_atten_lim).  ``step_audio`` / ``step_audio_chunk`` apply it to every
+        frame they synthesise from now on; the masks are unchanged.  The limit belongs to the slot, not to the session: START and
+        ``load_slots`` keep it, and ``save_slots`` does not carry it."""
+        s = self._slot_array(slots)
+        _lib.check(self.lib.fsn_stream_set_atten_lim(self._st, s.numel(), C.cast(s.data_ptr(), C.POINTER(C.c_int32)),
+                                                     _lib.atten_arg(db, s.numel())))
+
     def flush(self):
         """Feed look_ahead zero frames (the reference's right padding) and return the remaining masks."""
         z = torch.zeros((self.B, self.F), dtype=torch.float32, device=self.device)
@@ -327,6 +336,13 @@ class ChunkStream:
             stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
             _lib.check(self.lib.fsn_chunk_stream_load_slots(self._cs, s.numel(), C.c_void_p(s.data_ptr()), C.c_void_p(payload.data_ptr()),
                                                             state.meta, stream))
+
+    def set_atten_lim(self, slots, db):
+        """Attenuation limit of `slots` in dB, as ``StreamingFullSubNet.set_atten_lim`` (C: fsn_chunk_stream_set_atten_lim): every chunk a
+        slot completes from now on is enhanced with its limit (``enhance_audio(..., atten_lim_db)``)."""
+        s = _slot_array(slots)
+        _lib.check(self.lib.fsn_chunk_stream_set_atten_lim(self._cs, s.numel(), C.cast(s.data_ptr(), C.POINTER(C.c_int32)),
+                                                           _lib.atten_arg(db, s.numel())))
 
     def close(self):
         if self._cs is not None:

@@ -184,7 +184,7 @@ def _rank_world():
 
 @torch.no_grad()
 def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=print, model_and_epoch=None, trust_checkpoint=False, streams=4,
-        ragged=False, max_batch_seconds=None, replicas=None):
+        ragged=False, max_batch_seconds=None, replicas=None, atten_lim_db=None):
     """Enhance every file of config["dataset"]["args"]["dataset_dir_list"].  Under torchrun each rank takes every
     world-size-th batch (files are independent: no collective).  Returns {name: path} of the files this rank wrote.
     ``model_and_epoch`` (tests of the host logic) replaces the checkpoint load with a ready ``(callable, epoch)``.
@@ -193,7 +193,9 @@ def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=pri
     A batch whose forward the model plans in time windows or bin chunks (a long clip: it uses the model's whole workspace cap) runs alone on the
     first replica: every batch in flight is finished and every replica's workspaces are released first, and the first replica's
     after it, so only one capped workspace exists at a time.
-    ``replicas`` (tests of the host logic, with ``model_and_epoch``): ready models for the replicas after the first."""
+    ``replicas`` (tests of the host logic, with ``model_and_epoch``): ready models for the replicas after the first.
+    ``atten_lim_db``: None (no limit: the output of every release before limits existed), or the most any bin of any clip may be
+    attenuated, in dB (DESIGN.md §3.18); every batch then runs through the model's non-pipelined limited call."""
     rank, world, local_rank = _rank_world()
     if device is None:
         device = f"cuda:{local_rank}"
@@ -262,7 +264,7 @@ def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=pri
             if on_gpu:
                 with torch.cuda.stream(cuda_streams[k]):
                     enh = H.enhance_ragged(models[k], [c.pin_memory().to(device, non_blocking=True) for c in clips], n_fft, hop, win,
-                                           complex_inputs=INFERENCE_TYPES[itype])
+                                           complex_inputs=INFERENCE_TYPES[itype], atten_lim_db=atten_lim_db)
                     host = [torch.empty(tuple(e.shape), dtype=e.dtype).pin_memory() for e in enh]
                     for h, e in zip(host, enh):
                         h.copy_(e, non_blocking=True)
@@ -270,7 +272,7 @@ def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=pri
                     ev.record(cuda_streams[k])
                 inflight.append((bi, idx, host, ev, desc))
             else:
-                enh = H.enhance_ragged(models[k], clips, n_fft, hop, win, complex_inputs=INFERENCE_TYPES[itype])
+                enh = H.enhance_ragged(models[k], clips, n_fft, hop, win, complex_inputs=INFERENCE_TYPES[itype], atten_lim_db=atten_lim_db)
                 inflight.append((bi, idx, [e.cpu() for e in enh], None, desc))
             if alone:
                 finish(inflight.pop(0))
@@ -281,14 +283,15 @@ def run(config, checkpoint_path, output_dir, batch_size=64, device=None, log=pri
         if on_gpu:
             with torch.cuda.stream(cuda_streams[k]):
                 dev_noisy = noisy.pin_memory().to(device, non_blocking=True)
-                enh = H.enhance_batch(models[k], dev_noisy, n_fft, hop, win, complex_inputs=INFERENCE_TYPES[itype])
+                enh = H.enhance_batch(models[k], dev_noisy, n_fft, hop, win, complex_inputs=INFERENCE_TYPES[itype], atten_lim_db=atten_lim_db)
                 host = torch.empty(tuple(enh.shape), dtype=enh.dtype).pin_memory()
                 host.copy_(enh, non_blocking=True)
                 ev = torch.cuda.Event()
                 ev.record(cuda_streams[k])
             inflight.append((bi, idx, host, ev, noisy.size(1)))
         else:
-            inflight.append((bi, idx, H.enhance_batch(models[k], noisy, n_fft, hop, win, complex_inputs=INFERENCE_TYPES[itype]).cpu(), None, noisy.size(1)))
+            inflight.append((bi, idx, H.enhance_batch(models[k], noisy, n_fft, hop, win, complex_inputs=INFERENCE_TYPES[itype],
+                                                      atten_lim_db=atten_lim_db).cpu(), None, noisy.size(1)))
         if alone:
             finish(inflight.pop(0))                                        # nothing starts while the windowed batch holds its workspace
             release_all(models[:1])
@@ -313,13 +316,17 @@ def main(argv=None):
                         help="batch clips of different lengths (sorted by length, --batch_size per batch) in one ragged model call (additive)")
     parser.add_argument("--max_batch_seconds", type=float, default=None,
                         help="also cut a batch before its total audio exceeds this many seconds; a longer clip goes alone (additive)")
+    parser.add_argument("--atten_lim_db", type=float, default=None,
+                        help="attenuation limit: no time-frequency bin loses more than this many dB (>= 0; default: no limit) (additive)")
     args = parser.parse_args(argv)
+    if args.atten_lim_db is not None and not args.atten_lim_db >= 0:
+        parser.error(f"--atten_lim_db {args.atten_lim_db}: an attenuation limit is a number of dB >= 0")
     configuration = load_toml(args.configuration)
     if len(args.dataset_dir_list) > 0:
         print(f"use specified dataset_dir_list: {args.dataset_dir_list}, instead of in config")
         configuration["dataset"]["args"]["dataset_dir_list"] = args.dataset_dir_list
     run(configuration, args.model_checkpoint_path, args.output_dir, batch_size=args.batch_size, trust_checkpoint=args.trust_checkpoint, streams=args.streams,
-        ragged=args.ragged, max_batch_seconds=args.max_batch_seconds)
+        ragged=args.ragged, max_batch_seconds=args.max_batch_seconds, atten_lim_db=args.atten_lim_db)
 
 
 if __name__ == "__main__":

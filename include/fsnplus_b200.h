@@ -183,6 +183,25 @@ int fsn_model_forward_enhance_ragged(fsn_model* m, const float* d_mag, const flo
  * sub-batch: one analysis launch, the forward (unmasked when every clip has the longest clip's length, as fsn_model_forward_ragged),
  * one synthesis launch.  The call does not synchronise the stream. */
 int fsn_model_enhance_audio(fsn_model* m, const float* d_wave, int32_t B, int64_t L, const int64_t* h_lengths, float* d_out, void* stream);
+
+/* Attenuation limits (DESIGN.md §3.18): how much noise suppression may take away, per clip or per live session.  A limit of L dB
+ * (L >= 0, or +inf) has the floor lam = 10^(-L / 20), computed in double and rounded to float.  After decompress_cIRM the complex mask
+ * M of every bin and frame becomes M' = M where |M| >= lam (always at lam = 0, i.e. L = +inf: no limit), lam M / |M| where
+ * 0 < |M| < lam (the mask's phase, its magnitude raised to lam), (lam, 0) where M = 0; then Y = M' X as without a limit.  So
+ * |Y| >= lam |X| in every bin: no bin loses more than L dB.  A mask that amplifies is never touched; L = 0 attenuates no bin.
+ * The limit acts only where the library forms the enhanced spectrum or audio: every mask output (fsn_model_forward*, the streaming
+ * d_mask) stays the model's raw cIRM.  A negative or NaN limit is FSN_EINVAL naming the clip or slot and the value.  A call whose
+ * limits are all +inf runs exactly the unlimited call: the same kernels, bits and launch counts.
+ *
+ * Offline: h_atten_db is a HOST array of B floats, one per clip (NULL: no limit), free when the call returns; it reaches the device
+ * with the clips' lengths (one copy per sub-batch).  fsn_model_forward_enhance_lim is fsn_model_forward_enhance (h_frames NULL) or
+ * fsn_model_forward_enhance_ragged with limits; fsn_model_enhance_audio_lim is fsn_model_enhance_audio with limits.  Both plan, check
+ * and run exactly as those calls; with h_atten_db NULL they are those calls.  The pipelined entry points and fsn_apply_cirm take no
+ * limit. */
+int fsn_model_forward_enhance_lim(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
+                                  const int32_t* h_frames, const float* h_atten_db, float* d_enh, void* stream);
+int fsn_model_enhance_audio_lim(fsn_model* m, const float* d_wave, int32_t B, int64_t L, const int64_t* h_lengths, const float* h_atten_db,
+                                float* d_out, void* stream);
 /* The plan of fsn_model_enhance_audio for these clips (fsn_plan_forward_bins with the audio workspace counted), after the same checks
  * of the configuration and lengths, with the same FSN_EINVAL messages.  Host only, no GPU. */
 int fsn_plan_audio(const fsn_config* cfg, int32_t B, int64_t L, const int64_t* h_lengths, double cap_bytes, int32_t force_window,
@@ -317,6 +336,16 @@ int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_samples, float* d
 int fsn_stream_step_audio_chunk(fsn_stream* st, const float* d_samples, int32_t K, const int32_t* h_flags, const int32_t* h_hops,
                                 float* d_out, int32_t* h_nout, float* d_mask, void* stream);
 
+/* Per-slot attenuation limits of the streaming audio calls (semantics: fsn_model_enhance_audio_lim above): slot h_slots[i] gets
+ * h_atten_db[i] dB (+inf: no limit), kept until it is set again.  fsn_stream_step_audio_slots and fsn_stream_step_audio_chunk apply it
+ * to every frame they synthesise after this call; the mask calls and every d_mask ignore it.  A fresh handle has no limit on any slot;
+ * START and fsn_stream_load_slots leave a slot's limit as it is, and the limit is not part of a saved session (payload and meta are
+ * unchanged): a caller who moves a session sets the limit of the slot it loads into.  Host only: it enqueues nothing, the next step
+ * stages the limits with its plan.  Errors, checked before anything changes: FSN_EINVAL for a null array, n < 1, a slot out of range, a
+ * slot twice in one call (naming the index) and a negative or NaN limit (naming the slot and the value).  Both arrays are free when
+ * the call returns. */
+int fsn_stream_set_atten_lim(fsn_stream* st, int32_t n, const int32_t* h_slots, const float* h_atten_db);
+
 /* Overlapped-chunk sessions (DESIGN.md §3.16): live audio for any model fsn_model_enhance_audio runs -- FullSubNet+ with any attention
  * and norm, the sub-band TCN, fullsubnet.Model with any norm -- by the reference's overlapped_chunk inferencer
  * (fullsubnet_plus/inferencer/inferencer.py:191-250).  With C = chunk_samples (even), H = C / 2, P = 256 samples of pre-context and
@@ -344,6 +373,10 @@ int fsn_chunk_stream_create(fsn_model* m, int32_t B, int32_t chunk_samples, fsn_
 int fsn_chunk_stream_step(fsn_chunk_stream* cs, const float* d_samples, int32_t S, const int32_t* h_flags, const int32_t* h_counts,
                           float* d_out, int32_t* h_nout, void* stream);
 void fsn_chunk_stream_destroy(fsn_chunk_stream* cs);
+/* Per-slot attenuation limits of overlapped-chunk sessions, with fsn_stream_set_atten_lim's rules: every chunk row a slot completes in a
+ * later fsn_chunk_stream_step is enhanced with that slot's limit in the call's one audio batch (fsn_model_enhance_audio_lim).  The
+ * cross-fade is linear, so a session whose limit never changes gets exactly the overlapped-chunk output of the limited enhancement. */
+int fsn_chunk_stream_set_atten_lim(fsn_chunk_stream* cs, int32_t n, const int32_t* h_slots, const float* h_atten_db);
 
 /* Park, resume and move overlapped-chunk sessions (DESIGN.md §3.17): save the state of some slots of a chunk handle to a device buffer
  * and load it into any slot of any chunk handle with the same chunk_samples -- the same one, one with another B, one on another device

@@ -2259,6 +2259,11 @@ struct fsn_stream {
     // attenuation floors of the audio calls (fsn_stream_set_atten_lim, DESIGN.md §3.18): [B] on the host, empty until first set; staged
     // with each audio call's plan when any is > 0.  A handle setting, not session state
     std::vector<float> lam;
+    // the last call that stepped the model, for fsn_stream_get_stage: its scratch (null before any step and after an audio call that
+    // stepped none), its K, whether its sub band ran layer-wise and whether it was an audio call (x_mag then holds its input)
+    const StepScratch* last = nullptr;
+    int last_K = 0;
+    bool last_lw = false, last_audio = false;
 };
 
 int StepScratch::ensure(const fsn_stream& st, int K, size_t img, bool zero, cudaStream_t s) {
@@ -2439,6 +2444,7 @@ static int step_frames(fsn_stream* st, StepScratch& x, const float* d_mag, int K
     const fsn_config& c = m->cfg;
     const int B = st->B, F = c.num_freqs, L = c.num_layers, n = st->n, Pk = (K + 3) & ~3;
     const int resume = slot ? 1 : n > 0;                                // slot calls: a START zeroes instead of resume = 0
+    st->last = nullptr;                                                 // until this step completes, fsn_stream_get_stage refuses
     if (nzero) {
         StreamStateLaunch z{};
         state_launch(st, NSEG, ST_START, nullptr, z);
@@ -2508,6 +2514,7 @@ static int step_frames(fsn_stream* st, StepScratch& x, const float* d_mag, int K
     }
     CK(cudaGetLastError());
     st->n += K;
+    st->last = &x; st->last_K = K; st->last_lw = lw != nullptr; st->last_audio = false;
     return FSN_OK;
 }
 
@@ -2665,6 +2672,7 @@ static int step_slots(fsn_stream* st, const float* d_mag, int K, float* d_mask, 
     // frames: one group
     const bool layerwise = chunk && m->layerwise;
     StepScratch& x = chunk ? st->chunk : st->tick;
+    st->last = nullptr;                                                 // the scratch may be reallocated below
     std::vector<int> kf;
     std::vector<LwGroup> lw;
     int e = 0;
@@ -2800,6 +2808,7 @@ static int step_audio(fsn_stream* st, const float* d_samples, int K, const int32
     }
     const bool chunk = h_hops != nullptr, layerwise = chunk && m->layerwise;
     StepScratch& x = chunk ? st->chunk : st->tick;
+    st->last = nullptr;                                                 // the scratch may be reallocated below
     std::vector<LwGroup> lw;
     int e = 0;
     if (layerwise)
@@ -2850,6 +2859,8 @@ static int step_audio(fsn_stream* st, const float* d_samples, int K, const int32
         if (int rc = step_frames(st, x, a.mag, Km, d + 5 * B, Km > 1 ? d + 6 * B : nullptr, d + 7 * B, nzero,
                                  static_cast<float*>(st->x_mask.p), layerwise ? &lw : nullptr, s))
             return rc;
+    if (Km) st->last_audio = true;
+    else st->last = nullptr;
     launch_stream_istft_chunk(a, s);
     CK(cudaGetLastError());
     for (int b = 0; b < B; ++b) {
@@ -2879,6 +2890,36 @@ extern "C" int fsn_stream_step_audio_chunk(fsn_stream* st, const float* d_sample
     if (!h_hops) return fail(FSN_EINVAL, "h_hops is null (one hop count per slot, slots 0..%d)", st->B - 1);
     if (!h_nout) return fail(FSN_EINVAL, "h_nout is null (one result per slot, slots 0..%d)", st->B - 1);
     return step_audio(st, d_samples, K, h_flags, h_hops, d_out, h_nout, d_mask, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int fsn_stream_fb_ws(const fsn_stream* st) { return st && st->use_ws ? 1 : 0; }
+
+extern "C" int fsn_stream_get_stage(fsn_stream* st, const char* name, float* d_dst, int64_t numel, void* stream) {
+    if (!st || !name || !d_dst) return fail(FSN_EINVAL, "null argument");
+    const std::string n(name);
+    if (n != "fb_in" && n != "fb_out" && n != "sb_img" && n != "mag") return fail(FSN_EINVAL, "unknown stage %s", name);
+    if (!st->last) return fail(FSN_ESTATE, "no step call has stepped the model yet, or the last one failed or stepped no frame");
+    const fsn_config& c = st->m->cfg;
+    const int B = st->B, F = c.num_freqs, K = st->last_K, Pk = (K + 3) & ~3;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (n == "fb_in" || n == "fb_out") {
+        if (numel != (int64_t)B * F * K) return fail(FSN_EINVAL, "%s needs %lld elements", name, (long long)B * F * K);
+        const void* src = (n == "fb_in") ? st->last->fbin.p : st->last->fbout.p;
+        CK(cudaMemcpy2DAsync(d_dst, (size_t)K * 4, src, (size_t)Pk * 4, (size_t)K * 4, (size_t)B * F, cudaMemcpyDeviceToDevice, s));
+        return FSN_OK;
+    }
+    if (n == "sb_img") {
+        if (st->last_lw)
+            return fail(FSN_ESTATE, "sb_img is not kept: the last step ran the sub band layer-wise, its images are compact rows per group, sub-batch and window");
+        const size_t bytes = step_img_bytes(c, (long long)B * F, K);
+        if (numel * 4 != (int64_t)bytes) return fail(FSN_EINVAL, "sb_img needs %lld elements", (long long)(bytes / 4));
+        CK(cudaMemcpyAsync(d_dst, st->last->ximg.p, bytes, cudaMemcpyDeviceToDevice, s));
+        return FSN_OK;
+    }
+    if (!st->last_audio) return fail(FSN_ESTATE, "mag is kept only by the audio calls, and the last step was a mask call");
+    if (numel != (int64_t)B * F * K) return fail(FSN_EINVAL, "mag needs %lld elements", (long long)B * F * K);
+    CK(cudaMemcpyAsync(d_dst, st->x_mag.p, (size_t)B * F * K * 4, cudaMemcpyDeviceToDevice, s));
+    return FSN_OK;
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -30,6 +30,7 @@ SYMBOLS = [
     "fsn_chunk_stream_create", "fsn_chunk_stream_step", "fsn_chunk_stream_destroy",
     "fsn_chunk_stream_state_layout", "fsn_chunk_stream_save_slots", "fsn_chunk_stream_load_slots",
     "fsn_model_forward_enhance_lim", "fsn_model_enhance_audio_lim", "fsn_stream_set_atten_lim", "fsn_chunk_stream_set_atten_lim",
+    "fsn_stream_get_stage", "fsn_stream_fb_ws",
 ]
 
 
@@ -156,6 +157,8 @@ def load_library():
     lib.fsn_stream_load_slots.argtypes = [vp, i32, vp, vp, vp, vp]
     lib.fsn_apply_cirm.argtypes = [vp, vp, vp, i32, i32, i32, vp]
     lib.fsn_model_get_stage.argtypes = [vp, C.c_char_p, vp, i64, vp]
+    lib.fsn_stream_get_stage.argtypes = [vp, C.c_char_p, vp, i64, vp]
+    lib.fsn_stream_fb_ws.argtypes = [vp]
     lib.fsn_model_last_launch_count.argtypes = [vp]
     lib.fsn_model_last_launch_count.restype = i64
     lib.fsn_model_last_lstm_impl.argtypes = [vp]

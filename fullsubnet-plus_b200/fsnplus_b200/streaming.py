@@ -250,6 +250,15 @@ class StreamingFullSubNet:
         _lib.check(self.lib.fsn_stream_set_atten_lim(self._st, s.numel(), C.cast(s.data_ptr(), C.POINTER(C.c_int32)),
                                                      _lib.atten_arg(db, s.numel())))
 
+    def get_stage(self, name, shape):
+        """Test hook (C: fsn_stream_get_stage): a float32 CUDA tensor of `shape` with the intermediate `name` ("fb_in", "fb_out",
+        "sb_img", "mag") of the last call that stepped the model, ordered on the current stream like the step calls."""
+        t = torch.empty(shape, dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+            _lib.check(self.lib.fsn_stream_get_stage(self._st, name.encode(), C.c_void_p(t.data_ptr()), t.numel(), stream))
+        return t
+
     def flush(self):
         """Feed look_ahead zero frames (the reference's right padding) and return the remaining masks."""
         z = torch.zeros((self.B, self.F), dtype=torch.float32, device=self.device)

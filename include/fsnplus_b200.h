@@ -497,6 +497,21 @@ int fsn_apply_cirm(const float* d_crm, const float* d_noisy, float* d_enh, int32
  *            frames past a clip's extent are zero.  FSN_ESTATE after a forward that packed the images in time windows.
  * "stft" and "enh" are kept only when the last forward was an audio call that ran as one sub-batch; FSN_ESTATE otherwise. */
 int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst, int64_t numel, void* stream);
+/* Test hook of the streaming handle: copy an intermediate of the LAST step call that stepped the model (fsn_stream_step, _step_slots,
+ * _step_chunk, _step_audio_slots, _step_audio_chunk) to a device buffer.  K: that call's frames (the audio calls: its largest model
+ * frame count per slot); every slot's row, held ones included.
+ *   "fb_in"  [B, F, K]                 the cumulative-norm output, the full band's input
+ *   "fb_out" [B, F, K]                 the full band's output
+ *   "sb_img" raw bytes, numel = bytes / 4  the fp16 sub-band input of the generic kernel: SWIZZLE_128B images [nt, K, 128, 64] (Isb <= 64)
+ *            or time-major rows of 128 halves [K, nt * 128, 128] (Isb > 64), nt = ceil(B*F / 128), bytes = nt * K * 128 * (128 or 256)
+ *   "mag"    [B, F, K]                 the audio calls only: the magnitude frames the model stepped
+ * FSN_ESTATE before any step, after a step call that failed, after an audio call that stepped no frame, for "sb_img" after a step whose sub band ran layer-wise
+ * (its images are compact rows per group, sub-batch and window) and for "mag" after a mask call.  FSN_EINVAL for a null argument,
+ * an unknown name or a numel other than the one the message names.  Reading it changes nothing on any step path. */
+int fsn_stream_get_stage(fsn_stream* st, const char* name, float* d_dst, int64_t numel, void* stream);
+/* Test-only: 1 if the handle's full-band step runs on the weight-stationary kernel (k_lstm_ws.cu), 0 if on the generic mma kernel
+ * (fixed at fsn_stream_create: B <= 64 slots on a shape lstm_ws_supported takes, and FSN_NO_WS unset) or for a null handle. */
+int fsn_stream_fb_ws(const fsn_stream* st);
 /* Kernels launched by the last forward (bench.py reports it as gpu_launches). */
 int64_t fsn_model_last_launch_count(const fsn_model* m);
 /* Device time (ms, CUDA events on the forward's stream) of the sub-band model (LSTM kernels or the TCN) of the last forward;

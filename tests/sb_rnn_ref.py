@@ -76,8 +76,10 @@ def _head(sd, y, look_ahead, act, device, prefix="sb_model", head="sb", tf32=Fal
     return _act(y @ w.T + b, act).permute(0, 2, 1).contiguous()
 
 
-def truth(sd, kind, x, look_ahead, act, device="cpu", prefix="sb_model", head="sb"):
-    """x: [N, I, Tp] (any float type; the values are taken as they are) -> [N, O, Tp - look_ahead] float64 (head "fb": [N, O, Tp])."""
+def truth(sd, kind, x, look_ahead, act, device="cpu", prefix="sb_model", head="sb", state=None, return_state=False):
+    """x: [N, I, Tp] (any float type; the values are taken as they are) -> [N, O, Tp - look_ahead] float64 (head "fb": [N, O, Tp]).
+    state: None (zero) or the initial (h, c) [L, N, H] of a carried session (GRU: c is the fp32 h, which the recurrence starts from);
+    return_state: also return the final (h, c) [L, N, H] (GRU: both the final h)."""
     ls = layers(sd, device, prefix)
     I, H = ls[0][0].shape[1], ls[0][1].shape[1]
     rnn = getattr(torch.nn, kind)(I, H, len(ls), batch_first=True).to(device=device, dtype=torch.float64)
@@ -85,13 +87,23 @@ def truth(sd, kind, x, look_ahead, act, device="cpu", prefix="sb_model", head="s
         for l, (wi, wh, bi, bh) in enumerate(ls):
             for n, v in (("weight_ih", wi), ("weight_hh", wh), ("bias_ih", bi), ("bias_hh", bh)):
                 getattr(rnn, f"{n}_l{l}").copy_(v)
-        y, _ = rnn(torch.as_tensor(x).to(device=device, dtype=torch.float64).permute(0, 2, 1).contiguous())
-    return _head(sd, y, look_ahead, act, device, prefix, head)
+        xin = torch.as_tensor(x).to(device=device, dtype=torch.float64).permute(0, 2, 1).contiguous()
+        if state is None:
+            y, hc = rnn(xin)
+        else:
+            h0, c0 = (torch.as_tensor(v).to(device=device, dtype=torch.float64).contiguous() for v in state[:2])
+            y, hc = rnn(xin, c0 if kind == "GRU" else (h0, c0))
+    out = _head(sd, y, look_ahead, act, device, prefix, head)
+    if not return_state:
+        return out
+    return out, ((hc, hc) if kind == "GRU" else hc)
 
 
 def emulate(sd, kind, x, look_ahead, act, device="cpu", dtype=torch.float64, fault=None, fault_t=32, fault_row=0, prefix="sb_model",
-            head="sb"):
-    """The kernels' rounding in `dtype` arithmetic (see the module docstring); x as in truth().  fault: None or one of FAULTS
+            head="sb", state=None, return_state=False):
+    """The kernels' rounding in `dtype` arithmetic (see the module docstring); x, state and return_state as in truth(): state's h is
+    the carried fp16 h, its c the carried fp32 c (GRU: fp32 h); an optional third entry [L, N, H] is h(t - 2) of the first frame
+    (h_lag at fault_t = 0).  The final state is (fp16 h, fp32 c) per layer.  fault: None or one of FAULTS
       swap_units:    hidden units 3 and 5 (one 32-unit chunk) of layer 0 trade places after every step;
       c_reset:       c (GRU: the carried h) restarts from zero at step fault_t, as if a window boundary dropped it;
       h_lag:         step fault_t reads h(t - 2) instead of h(t - 1);
@@ -105,6 +117,7 @@ def emulate(sd, kind, x, look_ahead, act, device="cpu", dtype=torch.float64, fau
         inp = f16(inp)                                                                 # fb_pack: the fp32 input to fp16
     Tp, N = inp.shape[0], inp.shape[1]
     ls = layers(sd, device, prefix)
+    hs, cs = [], []
     for l, (wi, wh, bi, bh) in enumerate(ls):
         H = wh.shape[1]
         wi16, wh16, bi, bh = f16(wi.to(dtype)), f16(wh.to(dtype)), bi.to(dtype), bh.to(dtype)
@@ -112,8 +125,10 @@ def emulate(sd, kind, x, look_ahead, act, device="cpu", dtype=torch.float64, fau
         if l > 0 and head != "fb":                                                     # the full band's kernels keep Gin in fp32
             gin = f16(gin)
         h16 = torch.zeros(N, H, dtype=dtype, device=device)
-        hold = h16                                                                     # h(t - 2) for h_lag
         c = torch.zeros(N, H, dtype=dtype, device=device)                              # LSTM: c; GRU: h in fp32
+        if state is not None:
+            h16, c = (torch.as_tensor(v[l]).to(device=device, dtype=dtype).clone() for v in state[:2])
+        hold = h16 if state is None or len(state) < 3 else torch.as_tensor(state[2][l]).to(device=device, dtype=dtype)   # h(t - 2)
         out, top = [], []
         for t in range(Tp):
             if fault == "c_reset" and t == fault_t:
@@ -141,10 +156,13 @@ def emulate(sd, kind, x, look_ahead, act, device="cpu", dtype=torch.float64, fau
                 h16 = h16[:, [*range(3), 5, 4, 3, *range(6, H)]]
             out.append(h16)
             top.append(f32(h))
+        hs.append(h16)
+        cs.append(c)
         inp = torch.stack(out)
     if head == "fb":                                                                   # the head reads the top layer's fp32 h
         inp = torch.stack(top)
-    return _head(sd, inp.permute(1, 0, 2).to(torch.float64), look_ahead, act, device, prefix, head, tf32=head == "fb")
+    y = _head(sd, inp.permute(1, 0, 2).to(torch.float64), look_ahead, act, device, prefix, head, tf32=head == "fb")
+    return (y, (torch.stack(hs).to(torch.float64), torch.stack(cs).to(torch.float64))) if return_state else y
 
 
 def sample_rows(nrows, seed=0, full_below=512):

@@ -2241,9 +2241,10 @@ struct fsn_stream {
     // FSN_STATE_MODE_MASK or FSN_STATE_MODE_AUDIO, 0 before
     int mode = 0;
     // audio calls (fsn_stream_step_audio_slots, fsn_stream_step_audio_chunk), allocated at their first use.  Per slot on the host:
-    // a_tick = ticks of the session so far, HOLD excluded (-1: no session); a_hops = its hops K, known from its first FLUSH (0 before).
+    // a_tick = ticks of the session so far, HOLD excluded (-1: no session); a_hops = its hops K, known from its first FLUSH (0 before);
+    // a_pend = samples of its partial next hop (fsn_stream_step_audio_samples, 0 .. hop - 1; held in ring slot a_tick % 3).
     // On the device: the history ring, the noisy-spectrum ring, the overlap tail and the tables
-    std::vector<int32_t> a_tick, a_hops;
+    std::vector<int32_t> a_tick, a_hops, a_pend;
     std::vector<float> a_tables;
     DevBuf a_hist, a_spec, a_tail, a_tab;
     // save / load (fsn_stream_save_slots, fsn_stream_load_slots): the slot list of the last call on the device
@@ -2735,6 +2736,7 @@ static int audio_alloc(fsn_stream* st, cudaStream_t s) {
     CK(cudaMemcpyAsync(st->a_tab.p, st->a_tables.data(), st->a_tables.size() * sizeof(float), cudaMemcpyHostToDevice, s));
     st->a_tick.assign(B, -1);
     st->a_hops.assign(B, 0);
+    st->a_pend.assign(B, 0);
     return FSN_OK;
 }
 
@@ -2742,9 +2744,11 @@ static int audio_alloc(fsn_stream* st, cudaStream_t s) {
 // STEP x (n - 1) / STEP x n / STEP x n then FLUSH, the rest HOLD.  The active ones -- every tick but the HOLDs and the FLUSH ticks past
 // the session's end -- come first: na of them, at slot ticks k0 .. k0 + na - 1 (a START's k0 is 0).  The first nstore store the row's
 // hops, and every active tick but a START's is a model frame.  hops: the session's K after the call (0 before its FLUSH); nout: the
-// hops the call emits (those of slot ticks k >= la + 2).  Checks the flag and hop count against the slot's session.
+// hops the call emits (those of slot ticks k >= la + 2).  Checks the flag and hop count against the slot's session.  A session at
+// tick 0 (started by the sample call with less than a hop) runs its START tick with its first hop, whatever the flag.  r: the samples
+// past the last whole hop of a session the sample call ends (L = (t + n) hop + r), 0 for the hop calls.
 struct AudioSlotPlan { int k0, na, start, nstore, hops, nout; };
-static int audio_slot_plan(const fsn_stream* st, int b, int f, int n, int K, AudioSlotPlan* p) {
+static int audio_slot_plan(const fsn_stream* st, int b, int f, int n, int K, AudioSlotPlan* p, int r = 0) {
     const int la = st->m->cfg.look_ahead;
     const int t = st->a_tick.empty() ? -1 : st->a_tick[b], Kh = st->a_hops.empty() ? 0 : st->a_hops[b];
     *p = AudioSlotPlan{t, 0, 0, 0, Kh, 0};
@@ -2762,10 +2766,10 @@ static int audio_slot_plan(const fsn_stream* st, int b, int f, int n, int K, Aud
             return fail(FSN_EINVAL, "slot %d: STEP after the session's FLUSH (its input has ended: START a new session)", b);
         if (f == FSN_SLOT_FLUSH && Kh && n)
             return fail(FSN_EINVAL, "slot %d: FLUSH with h_hops = %d after the session's FLUSH (its input has ended: pass 0 hops)", b, n);
-        if (f == FSN_SLOT_FLUSH && !Kh && t + n < 2)
+        if (f == FSN_SLOT_FLUSH && !Kh && t + n < 2 && !(t + n == 1 && r))
             return fail(FSN_EINVAL, "slot %d: FLUSH after %d hop: a session needs at least 2 hops (the STFT's reflect padding reads "
                                     "n_fft / 2 + 1 samples)", b, t + n);
-        p->k0 = t; p->nstore = n;
+        p->k0 = t; p->nstore = n; p->start = t == 0;
         if (f == FSN_SLOT_STEP) {
             p->na = n;
         } else {                                                        // active up to slot tick K + la + 1, then a FLUSH is a HOLD
@@ -2779,23 +2783,20 @@ static int audio_slot_plan(const fsn_stream* st, int b, int f, int n, int K, Aud
     return FSN_OK;
 }
 
-// The audio calls after their argument checks: every slot advances by its flag and hop count (fsn_stream_step_audio_slots: K = 1,
-// h_hops null, one hop per START / STEP) through the K-hop kernels around one K-frame model step.  The per-hop call steps the model
-// on the per-tick scratch with the generic sub band; the chunk call on its own scratch, with the layer-wise sub band where the
-// offline forward runs it.  Errors change no state.
-static int step_audio(fsn_stream* st, const float* d_samples, int K, const int32_t* h_flags, const int32_t* h_hops, float* d_out,
-                      int32_t* h_nout, float* d_mask, cudaStream_t s) {
+// The sample call's part of an audio call (fsn_stream_step_audio_samples, DESIGN.md §3.19): per slot the samples pending before the
+// call and the trailing partial hop after it (StreamAudioSamples), the rows' strides, and whether any slot ticks (else only the
+// analysis kernel runs: it stores the partial hops and zeroes the output rows)
+struct SampleRows { const int32_t *r0, *r; int S, So; bool tick; };
+
+// The audio calls after their argument checks: every slot advances by its plan (fsn_stream_step_audio_slots: K = 1, one hop per
+// START / STEP) through the K-hop kernels around one K-frame model step.  The per-hop call (chunk = false) steps the model on the
+// per-tick scratch with the generic sub band; the chunk call on its own scratch, with the layer-wise sub band where the offline
+// forward runs it.  smp: the sample call's rows and planes (null for the hop calls).  Errors change no state.
+static int run_audio(fsn_stream* st, const std::vector<AudioSlotPlan>& plan, const float* d_samples, int K, bool chunk, float* d_out,
+                     float* d_mask, const SampleRows* smp, cudaStream_t s) {
     fsn_model* m = st->m;
     const fsn_config& c = m->cfg;
-    const int B = st->B, F = c.num_freqs, H = F - 1, la = c.look_ahead, N = 2 * H;
-    if (int rc = audio_fft_ok(c)) return rc;
-    if (int rc = chunk_check(c, K)) return rc;                         // num_freqs x K < 2^31 bounds the rows' K x hop too
-    std::vector<AudioSlotPlan> plan(B);
-    for (int b = 0; b < B; ++b) {                                       // every slot is checked before any state changes
-        const int n = h_hops ? h_hops[b] : h_flags[b] == FSN_SLOT_FLUSH ? 0 : 1;
-        if (int rc = audio_slot_plan(st, b, h_flags[b], n, K, &plan[b])) return rc;
-    }
-    if (st->mode == FSN_STATE_MODE_MASK) return claim_mode(st, FSN_STATE_MODE_AUDIO);
+    const int B = st->B, F = c.num_freqs, la = c.look_ahead, N = 2 * (F - 1);
     // The model's frames: slot b's kf of them, left-aligned in columns 0 .. kf - 1 of [B, F, Km], Km the largest kf.  One K-frame
     // step runs them all, each slot holding after its kf frames; on the layer-wise path its sub band runs one pass per group of
     // sessions with one kf (in steady state a single group).  Km = 0 (every slot holds): no model step.
@@ -2806,7 +2807,7 @@ static int step_audio(fsn_stream* st, const float* d_samples, int K, const int32
         Km = kf[b] > Km ? kf[b] : Km;
         nzero += kf[b] && plan[b].k0 + plan[b].start == 1;          // model frame 0 in column 0: a START's reset
     }
-    const bool chunk = h_hops != nullptr, layerwise = chunk && m->layerwise;
+    const bool layerwise = chunk && m->layerwise;
     StepScratch& x = chunk ? st->chunk : st->tick;
     st->last = nullptr;                                                 // the scratch may be reallocated below
     std::vector<LwGroup> lw;
@@ -2818,6 +2819,8 @@ static int step_audio(fsn_stream* st, const float* d_samples, int K, const int32
     const bool lim = std::any_of(st->lam.begin(), st->lam.end(), [](float v) { return v > 0.f; });
     const size_t lam_at = nstage;                                       // the slots' attenuation floors, last (when any is set)
     if (lim) nstage += B;
+    const size_t smp_at = nstage;                                       // the sample call's two planes after everything else
+    if (smp) nstage += 2 * (size_t)B;
     if (Km) e |= x.ensure(*st, Km, layerwise ? 0 : step_img_bytes(c, (long long)B * F, Km), false, s);
     e |= st->x_spec.ensure((size_t)B * K * F * sizeof(float2), false, s);
     e |= st->x_mag.ensure((size_t)B * F * Km * sizeof(float), false, s);
@@ -2842,6 +2845,10 @@ static int step_audio(fsn_stream* st, const float* d_samples, int K, const int32
     }
     lw_stage(kf, lw, zero + nzero, d + 7 * B + nzero);
     if (lim) memcpy(h + lam_at, st->lam.data(), (size_t)B * sizeof(float));
+    if (smp) {
+        memcpy(h + smp_at, smp->r0, (size_t)B * sizeof(int32_t));
+        memcpy(h + smp_at + B, smp->r, (size_t)B * sizeof(int32_t));
+    }
     if (int rc = st->stage.send(st->x_plan.p, nstage, s)) return rc;
     StreamAudioChunkLaunch a{};
     a.k0 = d; a.na = d + B; a.start = d + 2 * B; a.nstore = d + 3 * B; a.hops = d + 4 * B;
@@ -2853,7 +2860,19 @@ static int step_audio(fsn_stream* st, const float* d_samples, int K, const int32
     a.window = tab.window; a.twiddle = tab.twiddle; a.inv_env = tab.inv_env;
     a.B = B; a.K = K; a.Km = Km; a.n_fft = N; a.la = la;
     a.lam = lim ? reinterpret_cast<const float*>(d + lam_at) : nullptr;
-    launch_stream_stft_chunk(a, s);
+    StreamAudioSamplesLaunch sa{};
+    if (smp) {
+        sa.a = a;
+        sa.x = StreamAudioSamples{d + smp_at, d + smp_at + B, smp->S, smp->So, !smp->tick, tab.inv_last};
+        launch_stream_stft_samples(sa, s);
+        if (!smp->tick) {                                               // no tick: no model step and no synthesis
+            st->last = nullptr;
+            CK(cudaGetLastError());
+            return FSN_OK;
+        }
+    } else {
+        launch_stream_stft_chunk(a, s);
+    }
     // at Km = 1 the counts alone say which slots step a frame: no frame counts, so the per-frame step's kernels and arguments
     if (Km)
         if (int rc = step_frames(st, x, a.mag, Km, d + 5 * B, Km > 1 ? d + 6 * B : nullptr, d + 7 * B, nzero,
@@ -2861,11 +2880,32 @@ static int step_audio(fsn_stream* st, const float* d_samples, int K, const int32
             return rc;
     if (Km) st->last_audio = true;
     else st->last = nullptr;
-    launch_stream_istft_chunk(a, s);
+    if (smp) launch_stream_istft_samples(sa, s);
+    else launch_stream_istft_chunk(a, s);
     CK(cudaGetLastError());
+    return FSN_OK;
+}
+
+// The hop calls (fsn_stream_step_audio_slots: K = 1, h_hops null; fsn_stream_step_audio_chunk): their plans, then run_audio
+static int step_audio(fsn_stream* st, const float* d_samples, int K, const int32_t* h_flags, const int32_t* h_hops, float* d_out,
+                      int32_t* h_nout, float* d_mask, cudaStream_t s) {
+    const fsn_config& c = st->m->cfg;
+    const int B = st->B;
+    if (int rc = audio_fft_ok(c)) return rc;
+    if (int rc = chunk_check(c, K)) return rc;                         // num_freqs x K < 2^31 bounds the rows' K x hop too
+    std::vector<AudioSlotPlan> plan(B);
+    for (int b = 0; b < B; ++b) {                                       // every slot is checked before any state changes
+        const int n = h_hops ? h_hops[b] : h_flags[b] == FSN_SLOT_FLUSH ? 0 : 1;
+        if (int rc = audio_slot_plan(st, b, h_flags[b], n, K, &plan[b])) return rc;
+        if ((h_flags[b] == FSN_SLOT_STEP || h_flags[b] == FSN_SLOT_FLUSH) && !st->a_pend.empty() && st->a_pend[b])
+            return fail(FSN_EINVAL, "slot %d: %s on a session holding a partial hop of %d samples (continue it with "
+                                    "fsn_stream_step_audio_samples)", b, h_flags[b] == FSN_SLOT_STEP ? "STEP" : "FLUSH", st->a_pend[b]);
+    }
+    if (st->mode == FSN_STATE_MODE_MASK) return claim_mode(st, FSN_STATE_MODE_AUDIO);
+    if (int rc = run_audio(st, plan, d_samples, K, h_hops != nullptr, d_out, d_mask, nullptr, s)) return rc;
     for (int b = 0; b < B; ++b) {
         const AudioSlotPlan& p = plan[b];
-        if (h_flags[b] != FSN_SLOT_HOLD) { st->a_tick[b] = p.k0 + p.na; st->a_hops[b] = p.hops; }
+        if (h_flags[b] != FSN_SLOT_HOLD) { st->a_tick[b] = p.k0 + p.na; st->a_hops[b] = p.hops; st->a_pend[b] = 0; }
         h_nout[b] = p.nout;
     }
     return FSN_OK;
@@ -2890,6 +2930,101 @@ extern "C" int fsn_stream_step_audio_chunk(fsn_stream* st, const float* d_sample
     if (!h_hops) return fail(FSN_EINVAL, "h_hops is null (one hop count per slot, slots 0..%d)", st->B - 1);
     if (!h_nout) return fail(FSN_EINVAL, "h_nout is null (one result per slot, slots 0..%d)", st->B - 1);
     return step_audio(st, d_samples, K, h_flags, h_hops, d_out, h_nout, d_mask, static_cast<cudaStream_t>(stream));
+}
+
+// Any number of samples per slot and call (DESIGN.md §3.19).  Each slot's completed hops become the ticks of a hop call: START with n
+// hops (a START, or any first hop of a session at tick 0), STEP with n, or FLUSH with n and then the ticks that end the session.  A
+// call of at most one hop per slot and no FLUSH runs the per-hop call's path; any other the K-hop path, K the most ticks of a slot.
+// The partial hops are the kernels' r0 / r planes.  Every check runs before any state changes.
+extern "C" int fsn_stream_step_audio_samples(fsn_stream* st, const float* d_samples, int32_t S, const int32_t* h_flags,
+                                             const int32_t* h_counts, float* d_out, int32_t* h_nout, void* stream) {
+    if (!st) return fail(FSN_EINVAL, "st is null");
+    if (!d_samples) return fail(FSN_EINVAL, "d_samples is null (S samples per slot, [B, S] float32 on the device)");
+    if (!d_out) return fail(FSN_EINVAL, "d_out is null ([B, S + (look_ahead + 3) hop] float32 on the device)");
+    if (!h_flags) return fail(FSN_EINVAL, "h_flags is null (one flag per slot, slots 0..%d)", st->B - 1);
+    if (!h_counts) return fail(FSN_EINVAL, "h_counts is null (one sample count per slot, slots 0..%d)", st->B - 1);
+    if (!h_nout) return fail(FSN_EINVAL, "h_nout is null (one result per slot, slots 0..%d)", st->B - 1);
+    if (S < 1) return fail(FSN_EINVAL, "S = %d: the rows hold at least one sample", S);
+    const fsn_config& c = st->m->cfg;
+    if (int rc = audio_fft_ok(c)) return rc;
+    const int B = st->B, H = c.num_freqs - 1, la = c.look_ahead;
+    const long long So = (long long)S + (long long)(la + 3) * H;
+    if (So > 0x7fffffffLL) return fail(FSN_EINVAL, "S + (look_ahead + 3) hop = %lld output samples per row: past 2^31 - 1", So);
+    const bool fresh = st->a_tick.empty();
+    std::vector<int32_t> n(B, 0), need(B, 0), r0(B, 0), r(B, 0);
+    int K = 0;
+    bool flush = false, consume = false;
+    for (int b = 0; b < B; ++b) {                                       // every slot is checked before any state changes
+        const int f = h_flags[b], cnt = h_counts[b];
+        if (f < FSN_SLOT_HOLD || f > FSN_SLOT_FLUSH)
+            return fail(FSN_EINVAL, "slot %d: flag %d is not FSN_SLOT_HOLD (0), FSN_SLOT_STEP (1), FSN_SLOT_START (2) or FSN_SLOT_FLUSH (3)", b, f);
+        const int t = fresh ? -1 : st->a_tick[b], Kh = fresh ? 0 : st->a_hops[b], p0 = fresh ? 0 : st->a_pend[b];
+        r0[b] = r[b] = p0;
+        if (f == FSN_SLOT_HOLD) continue;
+        if (cnt < 0 || cnt > S) return fail(FSN_EINVAL, "slot %d: h_counts = %d is outside [0, S = %d]", b, cnt, S);
+        const char* name = f == FSN_SLOT_START ? "START" : f == FSN_SLOT_STEP ? "STEP" : "FLUSH";
+        if (f != FSN_SLOT_START && t < 0) return fail(FSN_EINVAL, "slot %d: %s on a slot without a session (START one first)", b, name);
+        if (f == FSN_SLOT_STEP && Kh)
+            return fail(FSN_EINVAL, "slot %d: STEP after the session's FLUSH (its input has ended: START a new session)", b);
+        if (f == FSN_SLOT_FLUSH && Kh && cnt)
+            return fail(FSN_EINVAL, "slot %d: FLUSH with h_counts = %d after the session's FLUSH (its input has ended: pass 0 samples)", b, cnt);
+        consume = consume || cnt > 0;
+        if (f == FSN_SLOT_START) r0[b] = 0;
+        const long long tot = (long long)r0[b] + cnt;
+        n[b] = (int)(tot / H);
+        r[b] = (int)(tot % H);
+        need[b] = n[b];
+        if (f == FSN_SLOT_FLUSH) {
+            if (Kh) {
+                need[b] = Kh + la + 2 - t > 0 ? Kh + la + 2 - t : 0;
+            } else {
+                const long long L = (long long)(t + n[b]) * H + r[b];
+                if (L <= H)
+                    return fail(FSN_EINVAL, "slot %d: FLUSH would end a session of %lld samples: a session needs more than n_fft / 2 = %d "
+                                            "(the STFT's reflect padding reads n_fft / 2 + 1 samples)", b, L, H);
+                need[b] = n[b] + la + 2;
+            }
+            flush = flush || need[b] > 0;
+        }
+        K = need[b] > K ? need[b] : K;
+    }
+    const bool chunk = flush || K > 1;                                  // else the per-hop call's path
+    const int Kc = K ? K : 1;
+    if (chunk)
+        if (int rc = chunk_check(c, Kc)) return rc;
+    std::vector<AudioSlotPlan> plan(B);
+    for (int b = 0; b < B; ++b) {
+        const int f = h_flags[b];
+        AudioSlotPlan& p = plan[b];
+        if (f == FSN_SLOT_HOLD || (f != FSN_SLOT_FLUSH && !n[b])) {     // no tick; a START of less than a hop starts at tick 0
+            if (int rc = audio_slot_plan(st, b, FSN_SLOT_HOLD, 0, Kc, &p)) return rc;
+            if (f == FSN_SLOT_START) { p.k0 = 0; p.hops = 0; }
+        } else if (int rc = audio_slot_plan(st, b, f, n[b], Kc, &p, f == FSN_SLOT_FLUSH ? r[b] : 0)) {
+            return rc;
+        }
+    }
+    if (st->mode == FSN_STATE_MODE_MASK) return claim_mode(st, FSN_STATE_MODE_AUDIO);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (K == 0 && !consume) {                                           // nothing to store or synthesise: the rows are zero
+        if (int rc = claim_mode(st, FSN_STATE_MODE_AUDIO)) return rc;
+        if (st->a_tick.empty())
+            if (int rc = audio_alloc(st, s)) return rc;
+        CK(cudaMemsetAsync(d_out, 0, (size_t)B * So * sizeof(float), s));
+    } else {
+        const SampleRows rows{r0.data(), r.data(), S, (int)So, K > 0};
+        if (int rc = run_audio(st, plan, d_samples, Kc, chunk, d_out, nullptr, &rows, s)) return rc;
+    }
+    for (int b = 0; b < B; ++b) {
+        const int f = h_flags[b];
+        const AudioSlotPlan& p = plan[b];
+        h_nout[b] = p.nout * H;
+        if (f == FSN_SLOT_HOLD) continue;
+        st->a_tick[b] = p.k0 + p.na;
+        st->a_hops[b] = p.hops;
+        st->a_pend[b] = f == FSN_SLOT_FLUSH ? 0 : r[b];
+        if (f == FSN_SLOT_FLUSH) h_nout[b] += r[b];                     // the partial end (0 for a session a hop call ended)
+    }
+    return FSN_OK;
 }
 
 extern "C" int fsn_stream_fb_ws(const fsn_stream* st) { return st && st->use_ws ? 1 : 0; }
@@ -3249,7 +3384,7 @@ extern "C" int fsn_stream_save_slots(fsn_stream* st, int32_t n, const int32_t* h
         q.magic = FSN_SLOT_STATE_MAGIC; q.version = FSN_SLOT_STATE_VERSION;
         q.cfg = st->m->cfg; q.weights_id = st->m->weights_id; q.mode = mode;
         if (mode == FSN_STATE_MODE_MASK) q.frames = st->nb[b];
-        else { q.tick = st->a_tick[b]; q.hops = st->a_hops[b]; }
+        else { q.tick = st->a_tick[b]; q.hops = st->a_hops[b]; q.frames = st->a_pend[b]; }
         q.payload_bytes = stride;
     }
     return FSN_OK;
@@ -3287,6 +3422,13 @@ extern "C" int fsn_stream_load_slots(fsn_stream* st, int32_t n, const int32_t* h
                         (long long)stride);
         if (q.mode == FSN_STATE_MODE_MASK ? q.frames < 0 : (q.tick < -1 || q.hops < 0))
             return fail(FSN_EINVAL, "h_meta[%d]: bad counters (frames %d, tick %d, hops %d)", i, q.frames, q.tick, q.hops);
+        if (q.mode == FSN_STATE_MODE_AUDIO && q.frames) {               // the samples of a partial hop (fsn_stream_step_audio_samples)
+            const int H = m->cfg.num_freqs - 1;
+            if (q.frames < 0 || q.frames >= H)
+                return fail(FSN_EINVAL, "h_meta[%d]: frames = %d pending samples, outside [0, hop = %d)", i, q.frames, H);
+            if (q.tick < 0) return fail(FSN_EINVAL, "h_meta[%d]: frames = %d pending samples on a meta without a session (tick -1)", i, q.frames);
+            if (q.hops) return fail(FSN_EINVAL, "h_meta[%d]: frames = %d pending samples after the session's FLUSH (hops %d)", i, q.frames, q.hops);
+        }
     }
     if (int rc = state_buffer_ok(st->cum_in.p, d_state)) return rc;
     const int mode = h_meta[0].mode;
@@ -3298,7 +3440,7 @@ extern "C" int fsn_stream_load_slots(fsn_stream* st, int32_t n, const int32_t* h
     for (int i = 0; i < n; ++i) {
         const int b = h_slots[i];
         if (mode == FSN_STATE_MODE_MASK) st->nb[b] = h_meta[i].frames;
-        else { st->a_tick[b] = h_meta[i].tick; st->a_hops[b] = h_meta[i].hops; }
+        else { st->a_tick[b] = h_meta[i].tick; st->a_hops[b] = h_meta[i].hops; st->a_pend[b] = h_meta[i].frames; }
     }
     return FSN_OK;
 }

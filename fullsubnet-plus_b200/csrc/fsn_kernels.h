@@ -192,6 +192,17 @@ struct StreamAudioChunkLaunch {
 };
 void launch_stream_stft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s);
 void launch_stream_istft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s);
+// The sample call's additions (fsn_stream_step_audio_samples, DESIGN.md §3.19): the same kernels' SMP instantiations
+struct StreamAudioSamples {
+    const int *r0, *r;        // [B] each: samples pending before the call; the trailing partial hop after it (the next pending count,
+                              // or at a FLUSH the partial end: L = K hop + r)
+    int S, So;                // row strides of samples [B, S] and out [B, So], So = S + (la + 3) hop
+    int zero_out;             // the analysis zeroes the output rows (a call with no tick runs no synthesis)
+    const float* inv_last;    // [hop] 1 / w^2(i + hop)
+};
+struct StreamAudioSamplesLaunch { StreamAudioChunkLaunch a; StreamAudioSamples x; };
+void launch_stream_stft_samples(const StreamAudioSamplesLaunch& a, cudaStream_t s);
+void launch_stream_istft_samples(const StreamAudioSamplesLaunch& a, cudaStream_t s);
 
 // ---- k_audio.cu: audio in and out of the offline forward (fsn_model_enhance_audio), and the tables of both audio paths -------
 struct AudioLaunch {

@@ -30,7 +30,7 @@ SYMBOLS = [
     "fsn_chunk_stream_create", "fsn_chunk_stream_step", "fsn_chunk_stream_destroy",
     "fsn_chunk_stream_state_layout", "fsn_chunk_stream_save_slots", "fsn_chunk_stream_load_slots",
     "fsn_model_forward_enhance_lim", "fsn_model_enhance_audio_lim", "fsn_stream_set_atten_lim", "fsn_chunk_stream_set_atten_lim",
-    "fsn_stream_get_stage", "fsn_stream_fb_ws",
+    "fsn_stream_get_stage", "fsn_stream_fb_ws", "fsn_stream_step_audio_samples",
 ]
 
 
@@ -145,6 +145,7 @@ def load_library():
     lib.fsn_stream_step_audio_slots.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.fsn_stream_step_chunk.argtypes = [vp, vp, i32, vp, vp, vp, vp]
     lib.fsn_stream_step_audio_chunk.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp, vp]
+    lib.fsn_stream_step_audio_samples.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp]
     lib.fsn_stream_chunk_plan.argtypes = [C.POINTER(FsnConfig), i32, i32, C.c_double, C.POINTER(i32), C.POINTER(i32), C.POINTER(i64)]
     lib.fsn_stream_destroy.argtypes = [vp]
     lib.fsn_stream_destroy.restype = None

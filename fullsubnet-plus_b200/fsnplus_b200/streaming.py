@@ -15,7 +15,9 @@ where the configuration takes them (DESIGN.md §3.13); it mixes freely with ``st
 ``step_audio`` serves the same sessions with audio in and out: one hop of samples per slot and tick goes in, one hop of enhanced
 audio comes out, with the STFT, the cIRM and the overlap-add iSTFT on the device (flag FLUSH ends a session, DESIGN.md §3.10).
 ``step_audio_chunk`` advances audio sessions many hops per call: each slot brings its own number of hops, and the call equals that
-many ``step_audio`` ticks on the slot (DESIGN.md §3.14).  A handle serves either the mask calls or the audio calls.
+many ``step_audio`` ticks on the slot (DESIGN.md §3.14).  ``step_audio_samples`` takes any number of samples per slot and call and
+ends a session at any length, with ``ChunkStream.step``'s arguments (DESIGN.md §3.19).  A handle serves either the mask calls or the
+audio calls.
 
 ``save_slots`` / ``load_slots`` park, resume and move sessions (DESIGN.md §3.11): a ``SessionState`` holds the saved state of some
 slots, and loading it into any slot of a handle of the same model -- this one, one with another B, or one on another GPU -- continues
@@ -169,7 +171,7 @@ class StreamingFullSubNet:
         never read); flags: B values of HOLD / STEP / START / FLUSH.  Returns (audio [B, hop], valid bool CPU tensor [B]), plus the
         masks [B, 2, F] with return_mask: valid[b] when audio[b] is hop q of the slot's session, which comes out at the slot's tick
         q + look_ahead + 2 (HOLD ticks not counted); every other row is zero.  A session of K >= 2 hops ends with look_ahead + 2
-        FLUSH ticks; at slot tick k the mask row is that of frame k - look_ahead - 1 (zero before frame 0)."""
+        FLUSH ticks (other lengths: ``step_audio_samples``); at slot tick k the mask row is that of frame k - look_ahead - 1 (zero before frame 0)."""
         assert samples.shape == (self.B, self.hop) and samples.is_cuda
         f = torch.as_tensor(flags, dtype=torch.int32)
         assert f.device.type == "cpu" and f.shape == (self.B,), "flags: B host values"
@@ -209,6 +211,29 @@ class StreamingFullSubNet:
                                                             C.c_void_p(nout.data_ptr()),
                                                             C.c_void_p(mask.data_ptr() if return_mask else None), stream))
         return (out, nout, mask) if return_mask else (out, nout)
+
+    def step_audio_samples(self, samples, counts, flags):
+        """Any number of samples per slot (DESIGN.md §3.19; C: fsn_stream_step_audio_samples).  samples [B, S] float32 CUDA: slot b's
+        counts[b] new samples at the front of its row (nothing else is read); counts, flags: B values each (sequences or CPU integer
+        tensors), flags HOLD / STEP / START / FLUSH (FLUSH consumes, then ends the session).  Returns (out [B, S + (look_ahead + 3)
+        hop], nout int32 CPU tensor [B]): slot b's nout[b] newly final samples at the front of its row, zero after them.  A session's
+        outputs concatenated over its calls are its offline enhancement (``enhance_audio``), as long as its input."""
+        assert samples.dim() == 2 and samples.shape[0] == self.B and samples.is_cuda
+        S = samples.shape[1]
+        f = torch.as_tensor(flags, dtype=torch.int32)
+        n = torch.as_tensor(counts, dtype=torch.int32)
+        assert f.device.type == "cpu" and f.shape == (self.B,), "flags: B host values"
+        assert n.device.type == "cpu" and n.shape == (self.B,), "counts: B host values"
+        f, n = f.contiguous(), n.contiguous()
+        x = samples.contiguous().float()
+        out = torch.empty((self.B, S + (self.look_ahead + 3) * self.hop), dtype=torch.float32, device=self.device)
+        nout = torch.zeros(self.B, dtype=torch.int32)
+        with torch.cuda.device(self.device):
+            stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+            _lib.check(self.lib.fsn_stream_step_audio_samples(self._st, C.c_void_p(x.data_ptr()), S, C.c_void_p(f.data_ptr()),
+                                                              C.c_void_p(n.data_ptr()), C.c_void_p(out.data_ptr()),
+                                                              C.c_void_p(nout.data_ptr()), stream))
+        return out, nout
 
     def _slot_array(self, slots):
         return _slot_array(slots)

@@ -299,8 +299,9 @@ int fsn_stream_chunk_plan(const fsn_config* cfg, int32_t n_active, int32_t K, do
  * d_out [B, hop] float32 device: one hop of enhanced audio per slot.  h_flags: HOST, B flags of FSN_SLOT_HOLD / STEP / START and: */
 #define FSN_SLOT_FLUSH 3  /* audio call only: no samples this tick; the session's input has ended, advance its tail                   */
 /* A START resets the slot's audio and model state and consumes the session's first hop; STEP consumes the next hop; HOLD is no tick
- * (state unchanged, output row zero).  A session of K >= 2 hops (L = K hop samples; pad a partial last hop with zeros and trim the
- * output) ends with exactly look_ahead + 2 FLUSH ticks; further FLUSH ticks act as HOLD until a START reuses the slot.
+ * (state unchanged, output row zero).  A session of K >= 2 hops (L = K hop samples; a session of any other length runs through
+ * fsn_stream_step_audio_samples below) ends with exactly look_ahead + 2 FLUSH ticks; further FLUSH ticks act as HOLD until a START
+ * reuses the slot.
  * h_valid (HOST, [B]): h_valid[b] = 1 when d_out[b] holds hop q of the slot's session; hop q comes out at the slot's tick
  * q + look_ahead + 2 (ticks counted from 0 at the START, HOLD ticks excluded): the algorithmic latency is look_ahead + 2 hops.
  * Every other output row is zero.  d_mask: null, or [B, 2, F] float32 device, which receives at slot tick k the cIRM of the slot's
@@ -335,6 +336,40 @@ int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_samples, float* d
  * does not synchronise the stream. */
 int fsn_stream_step_audio_chunk(fsn_stream* st, const float* d_samples, int32_t K, const int32_t* h_flags, const int32_t* h_hops,
                                 float* d_out, int32_t* h_nout, float* d_mask, void* stream);
+
+/* Any number of samples per slot and call (DESIGN.md §3.19), with fsn_chunk_stream_step's call shape: packets of 10 ms, 20 ms or
+ * whatever a transport delivers, and sessions of any length.  hop = n_fft / 2, la = look_ahead.
+ * d_samples [B, S] float32 device: slot b reads its first h_counts[b] samples (0 <= h_counts[b] <= S); no other sample is read.
+ * h_flags (HOST, B values): HOLD no change (h_counts ignored); START resets the slot, then consumes its samples; STEP consumes; FLUSH
+ * consumes, then ends the session: every remaining output sample through L comes out in this call and the slot has no live session
+ * after it (a later FLUSH of 0 samples acts as HOLD, a START reuses the slot).
+ * d_out [B, S + (la + 3) hop] float32 device: each slot's newly final samples at the front of its row, zero after them; h_nout (HOST,
+ * [B]) their count.  The bound: before a call a session has read t hop + r0 samples (t whole hops, r0 < hop) and emitted
+ * max(0, t - la - 2) hops, so it lags by at most (la + 2) hop + r0 < (la + 3) hop; a call adds at most S.
+ * Result: a session's outputs concatenated over its calls are fsn_model_enhance_audio of its input x[0, L), up to fp32 rounding, for
+ * every L > n_fft / 2 (the offline call's minimum) and any schedule of counts, holds and calls.
+ * Timing: output sample n is final in the call where the session's input reaches (floor(n / hop) + la + 3) hop samples, or at its FLUSH
+ * -- the hop calls' latency of la + 2 hops, counted from the end of the hop the sample is in.
+ * Equivalence: completed hops drive exactly the ticks of the hop calls.  A call that completes at most one hop per slot and FLUSHes
+ * no live session runs fsn_stream_step_audio_slots' path; any other call runs fsn_stream_step_audio_chunk's path with each slot's hop
+ * count and K = the most ticks of any slot, bit-identical to that hop call.  So a session fed whole hops and ended on a hop boundary
+ * gives the hop calls' bits.  A session ending at L = K hop + r, 0 < r < hop, has K + 1 frames: frame K is analysed from its r real
+ * samples reflected at L - 1, and after it is synthesised the last r samples are its tail times 1 / w^2(i + hop), as offline.
+ * Between calls the r < hop samples of a partial hop wait in the history-ring slot the next hop takes (the payload layout does not
+ * change); a session started with fewer than hop samples exists at tick 0 and its first whole hop runs the START tick.
+ * Mixing: the hop calls and this call mix freely on one audio handle, except that a hop call's STEP or FLUSH on a slot holding a
+ * partial hop is FSN_EINVAL naming the slot (a START discards the partial hop); a FLUSH of 0 samples from this call completes a
+ * session a hop call left mid-flush.  fsn_stream_set_atten_lim applies to every frame this call synthesises.  No mask output: the
+ * hop calls provide it.
+ * Launches: a call in which no slot completes a hop or FLUSHes launches one kernel (the partial-hop store, which also zeroes d_out),
+ * and a call in which no slot consumes a sample launches none (d_out is cleared by a memset).  Otherwise as the hop call it runs.
+ * Errors, all checked before any state changes (a failed call changes nothing): FSN_EINVAL naming the slot for a flag outside
+ * {0, 1, 2, 3}, a count outside [0, S], a STEP or FLUSH on a slot without a session, a STEP or a FLUSH with a count > 0 after the
+ * session's FLUSH, and a FLUSH that would end a session of L <= n_fft / 2 samples; naming the argument for a null array and S < 1;
+ * naming the limit for a derived K past fsn_stream_step_audio_chunk's limits and for S + (la + 3) hop past 2^31 - 1.  FSN_ESTATE on a
+ * handle that serves the mask calls.  The host arrays are free when the call returns; the call does not synchronise the stream. */
+int fsn_stream_step_audio_samples(fsn_stream* st, const float* d_samples, int32_t S, const int32_t* h_flags, const int32_t* h_counts,
+                                  float* d_out, int32_t* h_nout, void* stream);
 
 /* Per-slot attenuation limits of the streaming audio calls (semantics: fsn_model_enhance_audio_lim above): slot h_slots[i] gets
  * h_atten_db[i] dB (+inf: no limit), kept until it is set again.  fsn_stream_step_audio_slots and fsn_stream_step_audio_chunk apply it
@@ -448,7 +483,8 @@ int fsn_chunk_stream_load_slots(fsn_chunk_stream* cs, int32_t n, const int32_t* 
  * A handle that has served no call yet takes the meta's mode at a load (and allocates its audio state in audio mode); a handle that
  * has only used fsn_stream_step switches to per-slot counts at a save or load, as at its first slot call.
  * Errors change no state.  FSN_EINVAL, naming the index or field: a null array, n < 1, a slot out of range, a slot twice in one load, a
- * bad magic or version, a payload_bytes other than this handle's, a configuration field that differs (lstm_impl excepted: streaming
+ * bad magic or version, an audio meta's frames outside [0, hop) or > 0 with tick -1 or hops > 0, a payload_bytes other than this
+ * handle's, a configuration field that differs (lstm_impl excepted: streaming
  * always runs the mma kernels), a weights_id that differs, a d_state that is not 256-byte aligned device memory of the handle's
  * device.  FSN_ESTATE: a meta whose mode is not the handle's, a save on a handle that has served no call. */
 #define FSN_SLOT_STATE_VERSION 1
@@ -460,7 +496,8 @@ typedef struct fsn_slot_meta {      /* host-side description of one saved sessio
     fsn_config cfg;                 /* the saving model's configuration                                             */
     uint64_t weights_id;            /* fsn_model_weights_id of the saving model                                     */
     int32_t mode;                   /* FSN_STATE_MODE_MASK or FSN_STATE_MODE_AUDIO                                  */
-    int32_t frames;                 /* mask mode: frames the slot consumed since its START (0 in audio mode)        */
+    int32_t frames;                 /* mask mode: frames the slot consumed since its START; audio mode: the samples r of a
+                                       partial hop (fsn_stream_step_audio_samples), 0 <= r < hop, 0 without a session or after its FLUSH */
     int32_t tick, hops;             /* audio mode: the slot's tick count (-1 = no session) and hops K (0 before its first FLUSH); 0 in mask mode */
     int64_t payload_bytes;          /* stride of one session in d_state                                             */
 } fsn_slot_meta;

@@ -1174,13 +1174,22 @@ static const long long FSN_MAX_TP = 65535LL * 256;
 static long long max_clips_for_rows(const fsn_config& c, int T) {
     return c.model_kind == FSN_KIND_PLUS ? (0x7fffffffLL - 128) / (3LL * (T + c.look_ahead)) : 0x7fffffffLL;
 }
-static int check_length(const fsn_config& c, int B, int T) {
+// Clips of one forward that the launch grids hold: gridDim.y and gridDim.z take at most 65535 blocks, and the front end's
+// tsse_apply_kernel puts its (branch, clip) planes on gridDim.z (3 B in FullSubNet+); the sub-band packer, fullsubnet.Model's
+// full-band output convolution and the audio transforms put the clips on gridDim.y or z.
+static const long long FSN_MAX_GRID_YZ = 65535;
+static long long max_clips_for_grid(const fsn_config& c) { return FSN_MAX_GRID_YZ / (c.model_kind == FSN_KIND_PLUS ? 3 : 1); }
+static int check_length(const fsn_config& c, int B, int T, bool front = true) {
     const long long Tp = (long long)T + c.look_ahead;
     if (Tp > FSN_MAX_TP) return fail(FSN_EINVAL, "T + look_ahead = %lld frames exceeds the limit of %lld (65535 x 256, the TCN convolution grid)", Tp, FSN_MAX_TP);
     if ((long long)c.num_freqs * Tp > 0x7fffffffLL)
         return fail(FSN_EINVAL, "num_freqs x (T + look_ahead) = %lld exceeds 2^31 - 1, the per-clip plane index limit", (long long)c.num_freqs * Tp);
     if (B > max_clips_for_rows(c, T))
         return fail(FSN_EINVAL, "3 x B x (T + look_ahead) = %lld rows exceeds the full-band TCN's 2^31 row limit", 3LL * B * Tp);
+    const long long glim = front ? max_clips_for_grid(c) : FSN_MAX_GRID_YZ;   // the sub-band hook runs no front end (no TSSE planes)
+    if (B > glim)
+        return fail(FSN_EINVAL, "B = %d clips exceeds the launch-grid limit of %lld clips per forward (65535 blocks on gridDim.y / z%s)", B,
+                    glim, front && c.model_kind == FSN_KIND_PLUS ? ", 3 B for the TSSE planes" : "");
     return FSN_OK;
 }
 
@@ -1325,7 +1334,7 @@ static int check_batch(const fsn_model* m, Batch& b, std::vector<int32_t>* lens 
     if (int rc = check_frames(c, b)) return rc;
     if (!hook && b.T + c.look_ahead < tsse_kmax(c)) return fail(FSN_EINVAL, "sequence shorter than the TSSE kernel size");
     if (b.atten_db && !b.enh) return fail(FSN_EINVAL, "an attenuation limit applies to the enhanced spectrum, not to the mask");
-    if (int rc = check_length(c, b.call == CALL_FORWARD ? 1 : b.B, b.T)) return rc;
+    if (int rc = check_length(c, b.call == CALL_FORWARD ? 1 : b.B, b.T, !hook)) return rc;
     return check_atten(b, lam);
 }
 
@@ -1634,7 +1643,7 @@ static int prepare(fsn_model* m, Lane& ln, const Batch& b, int Tw, int Fc, cudaS
 
 // Audio analysis: the STFT of every clip of b into the audio workspace, whose planes then are b's inputs and whose enhanced spectrum
 // its output.  al: the launch, kept for the synthesis after the sub-band stage.
-static void audio_analysis(fsn_model* m, Lane& ln, Batch& b, AudioLaunch& al, cudaStream_t s) {
+static int audio_analysis(fsn_model* m, Lane& ln, Batch& b, AudioLaunch& al, cudaStream_t s) {
     const int F = m->cfg.num_freqs, N = 2 * (F - 1);
     const AudioTables tab = audio_table_ptrs(static_cast<const float*>(m->au_tab.p), N);
     al.wave = b.wave; al.out = b.wave_out; al.L = b.L;
@@ -1642,10 +1651,12 @@ static void audio_analysis(fsn_model* m, Lane& ln, Batch& b, AudioLaunch& al, cu
     al.B = b.B; al.T = b.T; al.n_fft = N;
     al.planes = static_cast<float*>(m->au_planes.p); al.enh = static_cast<const float2*>(m->au_enh.p);
     al.window = tab.window; al.twiddle = tab.twiddle; al.inv_env = tab.inv_env; al.inv_last = tab.inv_last;
-    launch_audio_stft(al, s); m->launches++;
+    if (cudaError_t e = launch_audio_stft(al, s)) return fail(FSN_ECUDA, "audio_stft_kernel launch failed: %s", cudaGetErrorString(e));
+    m->launches++;
     const size_t plane = (size_t)b.B * F * b.T;
     b.mag = al.planes; b.real = al.planes + plane; b.imag = al.planes + 2 * plane;
     b.mask = nullptr; b.enh = static_cast<float*>(m->au_enh.p);
+    return FSN_OK;
 }
 
 // The sub-band packer's arguments for a batch of B clips of T frames in lane ln, window Tw, extents tl; the front end adds its sources,
@@ -1779,7 +1790,7 @@ static int forward_impl(fsn_model* m, Lane& ln, const Batch& in, cudaStream_t s,
     Batch b = in;
     b.dlam = dlam;
     AudioLaunch al{};
-    if (in.wave) audio_analysis(m, ln, b, al, s);
+    if (in.wave && (rc = audio_analysis(m, ln, b, al, s))) return rc;
     SbPackLaunch sp = pack_args(m, ln, b.B, b.T, Tw, tl);
     if ((rc = front_end(m, ln, b, tl, sp, s)) || (rc = pack_clip(m, ln, sp, Tw, Fc, s))) return rc;
     cudaEventRecord(m->evf1[evi], s);
@@ -1791,7 +1802,10 @@ static int forward_impl(fsn_model* m, Lane& ln, const Batch& in, cudaStream_t s,
     rc = sub_band(m, ln, b, Tw, Fc, sp, tl, sl);
     cudaEventRecord(m->ev1[evi], sl);
     if (rc) return rc;
-    if (in.wave) { launch_audio_istft(al, sl); m->launches++; }        // the iSTFT of every clip over its own frames
+    if (in.wave) {                                                      // the iSTFT of every clip over its own frames
+        if (cudaError_t e = launch_audio_istft(al, sl)) return fail(FSN_ECUDA, "audio_istft_kernel launch failed: %s", cudaGetErrorString(e));
+        m->launches++;
+    }
     m->nfwd++;
     CK(cudaGetLastError());
     return FSN_OK;
@@ -1876,7 +1890,8 @@ template <class Ok> static int largest(int lo, int hi, Ok ok) {
 static Plan plan_forward(const fsn_config& c, bool layerwise, int B, int T, double cap, int force, int force_bins, bool audio = false,
                          bool lim = false) {
     const int Tp = T + c.look_ahead, wmax = (Tp + 31) / 32 * 32;
-    const long long blim = max_clips_for_rows(c, T);             // sub-batches never exceed the full-band TCN's row limit
+    // sub-batches never exceed the full-band TCN's row limit or the launch grids
+    const long long blim = std::min(max_clips_for_rows(c, T), max_clips_for_grid(c));
     auto split = [&](int bmax) { if (bmax > blim) bmax = (int)blim; if (bmax < 1) bmax = 1; if (B <= bmax) return B; const int n = (B + bmax - 1) / bmax; return (B + n - 1) / n; };
     auto bytes = [&](int bs, int tw) { return (double)ws_sizes(c, layerwise, bs, T, tw, 0, audio, lim).total(); };
     // largest equal split bs with fits(bs) (0 if even one clip does not fit)
@@ -2265,6 +2280,7 @@ struct fsn_stream {
     const StepScratch* last = nullptr;
     int last_K = 0;
     bool last_lw = false, last_audio = false;
+    int last_spec_K = 0;                // the last audio call's K: the slot stride (in frames) of its spectrum scratch x_spec
 };
 
 int StepScratch::ensure(const fsn_stream& st, int K, size_t img, bool zero, cudaStream_t s) {
@@ -2878,7 +2894,7 @@ static int run_audio(fsn_stream* st, const std::vector<AudioSlotPlan>& plan, con
         if (int rc = step_frames(st, x, a.mag, Km, d + 5 * B, Km > 1 ? d + 6 * B : nullptr, d + 7 * B, nzero,
                                  static_cast<float*>(st->x_mask.p), layerwise ? &lw : nullptr, s))
             return rc;
-    if (Km) st->last_audio = true;
+    if (Km) { st->last_audio = true; st->last_spec_K = K; }
     else st->last = nullptr;
     if (smp) launch_stream_istft_samples(sa, s);
     else launch_stream_istft_chunk(a, s);
@@ -3032,7 +3048,8 @@ extern "C" int fsn_stream_fb_ws(const fsn_stream* st) { return st && st->use_ws 
 extern "C" int fsn_stream_get_stage(fsn_stream* st, const char* name, float* d_dst, int64_t numel, void* stream) {
     if (!st || !name || !d_dst) return fail(FSN_EINVAL, "null argument");
     const std::string n(name);
-    if (n != "fb_in" && n != "fb_out" && n != "sb_img" && n != "mag") return fail(FSN_EINVAL, "unknown stage %s", name);
+    if (n != "fb_in" && n != "fb_out" && n != "sb_img" && n != "mag" && n != "mask" && n != "spec")
+        return fail(FSN_EINVAL, "unknown stage %s", name);
     if (!st->last) return fail(FSN_ESTATE, "no step call has stepped the model yet, or the last one failed or stepped no frame");
     const fsn_config& c = st->m->cfg;
     const int B = st->B, F = c.num_freqs, K = st->last_K, Pk = (K + 3) & ~3;
@@ -3051,9 +3068,16 @@ extern "C" int fsn_stream_get_stage(fsn_stream* st, const char* name, float* d_d
         CK(cudaMemcpyAsync(d_dst, st->last->ximg.p, bytes, cudaMemcpyDeviceToDevice, s));
         return FSN_OK;
     }
-    if (!st->last_audio) return fail(FSN_ESTATE, "mag is kept only by the audio calls, and the last step was a mask call");
-    if (numel != (int64_t)B * F * K) return fail(FSN_EINVAL, "mag needs %lld elements", (long long)B * F * K);
-    CK(cudaMemcpyAsync(d_dst, st->x_mag.p, (size_t)B * F * K * 4, cudaMemcpyDeviceToDevice, s));
+    if (!st->last_audio) return fail(FSN_ESTATE, "%s is kept only by the audio calls, and the last step was a mask call", name);
+    if (n == "spec") {                                                  // [B, K, F] complex of the call's scratch [B, K_call, F]
+        if (numel != (int64_t)2 * B * K * F) return fail(FSN_EINVAL, "spec needs %lld elements", (long long)2 * B * K * F);
+        const size_t row = (size_t)K * F * sizeof(float2);
+        CK(cudaMemcpy2DAsync(d_dst, row, st->x_spec.p, (size_t)st->last_spec_K * F * sizeof(float2), row, (size_t)B, cudaMemcpyDeviceToDevice, s));
+        return FSN_OK;
+    }
+    const int rows = n == "mask" ? 2 * F : F;
+    if (numel != (int64_t)B * rows * K) return fail(FSN_EINVAL, "%s needs %lld elements", name, (long long)B * rows * K);
+    CK(cudaMemcpyAsync(d_dst, n == "mask" ? st->x_mask.p : st->x_mag.p, (size_t)B * rows * K * 4, cudaMemcpyDeviceToDevice, s));
     return FSN_OK;
 }
 

@@ -216,8 +216,9 @@ struct AudioLaunch {
     const float2* enh;        // [B, F, T] enhanced spectrum: synthesis input, the forward's output
     const float* window; const float2* twiddle; const float* inv_env; const float* inv_last;   // audio_tables
 };
-void launch_audio_stft(const AudioLaunch& a, cudaStream_t s);
-void launch_audio_istft(const AudioLaunch& a, cudaStream_t s);
+// Both put the batch on gridDim.y (B <= 65535, kept by plan_forward); they return the launch's error
+cudaError_t launch_audio_stft(const AudioLaunch& a, cudaStream_t s);
+cudaError_t launch_audio_istft(const AudioLaunch& a, cudaStream_t s);
 // Tables of one n_fft, computed in double, in one array: periodic Hann window w [n_fft] | twiddles exp(-2 pi i k / n_fft) for
 // k = 0 .. hop (hop + 1 float2) | 1 / (w^2(i) + w^2(i + hop)) for i < hop | 1 / w^2(i + hop) for i < hop (the last L mod hop samples of a
 // clip, which one frame covers)

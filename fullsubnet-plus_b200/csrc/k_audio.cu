@@ -112,13 +112,15 @@ __global__ void __launch_bounds__(AUDIO_OFF_THREADS) audio_istft_kernel(AudioLau
 
 static int run_tiles(long long n, int R) { return (int)((n + R - 1) / R); }
 
-void launch_audio_stft(const AudioLaunch& a, cudaStream_t s) {
+cudaError_t launch_audio_stft(const AudioLaunch& a, cudaStream_t s) {
     const int R = AUDIO_RUN_POINTS / (a.n_fft / 2);
     audio_stft_kernel<<<dim3(run_tiles(a.T, R), a.B), AUDIO_OFF_THREADS, 0, s>>>(a);
+    return cudaGetLastError();
 }
-void launch_audio_istft(const AudioLaunch& a, cudaStream_t s) {
+cudaError_t launch_audio_istft(const AudioLaunch& a, cudaStream_t s) {
     const int H = a.n_fft / 2, R = AUDIO_RUN_POINTS / H;
     audio_istft_kernel<<<dim3(run_tiles((a.L + H - 1) / H, R), a.B), AUDIO_OFF_THREADS, 0, s>>>(a);
+    return cudaGetLastError();
 }
 
 void audio_tables(int n_fft, std::vector<float>& tab) {

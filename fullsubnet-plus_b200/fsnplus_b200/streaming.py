@@ -277,11 +277,15 @@ class StreamingFullSubNet:
 
     def get_stage(self, name, shape):
         """Test hook (C: fsn_stream_get_stage): a float32 CUDA tensor of `shape` with the intermediate `name` ("fb_in", "fb_out",
-        "sb_img", "mag") of the last call that stepped the model, ordered on the current stream like the step calls."""
-        t = torch.empty(shape, dtype=torch.float32, device=self.device)
+        "sb_img", "mag", "mask", "spec") of the last call that stepped the model, ordered on the current stream like the step calls.
+        "spec" is complex: `shape` is its [B, K, F] and the tensor complex64."""
+        cplx = name == "spec"
+        t = torch.empty(tuple(shape) + ((2,) if cplx else ()), dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
             stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
             _lib.check(self.lib.fsn_stream_get_stage(self._st, name.encode(), C.c_void_p(t.data_ptr()), t.numel(), stream))
+        if cplx:
+            return torch.view_as_complex(t)
         return t
 
     def flush(self):

@@ -535,15 +535,19 @@ int fsn_apply_cirm(const float* d_crm, const float* d_noisy, float* d_enh, int32
  * "stft" and "enh" are kept only when the last forward was an audio call that ran as one sub-batch; FSN_ESTATE otherwise. */
 int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst, int64_t numel, void* stream);
 /* Test hook of the streaming handle: copy an intermediate of the LAST step call that stepped the model (fsn_stream_step, _step_slots,
- * _step_chunk, _step_audio_slots, _step_audio_chunk) to a device buffer.  K: that call's frames (the audio calls: its largest model
- * frame count per slot); every slot's row, held ones included.
+ * _step_chunk, _step_audio_slots, _step_audio_chunk, _step_audio_samples) to a device buffer.  K: that call's frames (the audio calls:
+ * its largest model frame count per slot); every slot's row, held ones included.  In the audio calls slot b's frames are columns
+ * 0 .. k_b - 1 (k_b: the frames it stepped in the call); its columns past k_b hold no frame of the call.
  *   "fb_in"  [B, F, K]                 the cumulative-norm output, the full band's input
  *   "fb_out" [B, F, K]                 the full band's output
  *   "sb_img" raw bytes, numel = bytes / 4  the fp16 sub-band input of the generic kernel: SWIZZLE_128B images [nt, K, 128, 64] (Isb <= 64)
  *            or time-major rows of 128 halves [K, nt * 128, 128] (Isb > 64), nt = ceil(B*F / 128), bytes = nt * K * 128 * (128 or 256)
  *   "mag"    [B, F, K]                 the audio calls only: the magnitude frames the model stepped
+ *   "mask"   [B, 2, F, K]              the audio calls only: the model's cIRM columns (the mask each column's synthesis reads; the
+ *                                      sample call returns no masks)
+ *   "spec"   [B, K, F] complex64       the audio calls only: the noisy spectra of the frames the call analysed (numel = 2 B K F floats)
  * FSN_ESTATE before any step, after a step call that failed, after an audio call that stepped no frame, for "sb_img" after a step whose sub band ran layer-wise
- * (its images are compact rows per group, sub-batch and window) and for "mag" after a mask call.  FSN_EINVAL for a null argument,
+ * (its images are compact rows per group, sub-batch and window) and for "mag", "mask" and "spec" after a mask call.  FSN_EINVAL for a null argument,
  * an unknown name or a numel other than the one the message names.  Reading it changes nothing on any step path. */
 int fsn_stream_get_stage(fsn_stream* st, const char* name, float* d_dst, int64_t numel, void* stream);
 /* Test-only: 1 if the handle's full-band step runs on the weight-stationary kernel (k_lstm_ws.cu), 0 if on the generic mma kernel

@@ -3708,3 +3708,96 @@ extern "C" int fsn_model_last_plan_bins(const fsn_model* m, int32_t* Bs, int32_t
     if (!m || !Bs || !Tw || !Fc) return fail(FSN_EINVAL, "null argument");
     return put_plan(m->plan, Bs, Tw, Fc, nullptr);
 }
+
+// ---- speech metrics (DESIGN.md §3.20): model-free, one score per clip ----------------------------------------------------------
+
+static int metric_check(const char* fn, int32_t B, int64_t L, const int64_t* h_lengths, long long* Lmax) {
+    if (B < 1 || B > 65535) return fail(FSN_EINVAL, "%s: B = %d: a batch holds 1 .. 65535 clips", fn, B);
+    if (L < 1 || L > 0x7fffffffLL) return fail(FSN_EINVAL, "%s: L = %lld: the row length must be 1 .. 2^31 - 1 samples", fn, (long long)L);
+    long long mx = 0;
+    for (int b = 0; b < (h_lengths ? B : 1); ++b) {
+        const long long n = h_lengths ? h_lengths[b] : L;
+        if (n < 1 || n > L)
+            return fail(FSN_EINVAL, "%s: clip %d: h_lengths[%d] = %lld is outside 1 .. L = %lld", fn, b, b, n, (long long)L);
+        if (n > mx) mx = n;
+    }
+    *Lmax = mx;
+    return FSN_OK;
+}
+
+static int metric_sr_check(const char* fn, int32_t sr) {
+    if (sr < 8000 || sr > 48000) return fail(FSN_EINVAL, "%s: sr = %d: the sample rate must be 8000 .. 48000 Hz", fn, sr);
+    return FSN_OK;
+}
+
+static int metric_work_check(const char* fn, const void* d_ref, const void* d_est, const void* d_work, const void* d_out, int64_t work_bytes,
+                             size_t need) {
+    if (!d_ref || !d_est || !d_out || !d_work) return fail(FSN_EINVAL, "%s: null device pointer", fn);
+    if (work_bytes < 0 || (size_t)work_bytes < need)
+        return fail(FSN_EINVAL, "%s: work_bytes = %lld, the call needs %zu", fn, (long long)work_bytes, need);
+    return FSN_OK;
+}
+
+static std::vector<long long> metric_lengths(int32_t B, int64_t L, const int64_t* h_lengths) {
+    std::vector<long long> len(B, (long long)L);
+    if (h_lengths) for (int b = 0; b < B; ++b) len[b] = h_lengths[b];
+    return len;
+}
+
+extern "C" int fsn_metric_si_sdr_workspace(int32_t B, int64_t L, const int64_t* h_lengths, int64_t* bytes) {
+    long long Lmax = 0;
+    if (!bytes) return fail(FSN_EINVAL, "fsn_metric_si_sdr_workspace: null bytes");
+    if (int rc = metric_check("fsn_metric_si_sdr_workspace", B, L, h_lengths, &Lmax)) return rc;
+    SiSdrLaunch a{};
+    *bytes = (int64_t)si_sdr_layout(a, nullptr, B, Lmax);
+    return FSN_OK;
+}
+
+extern "C" int fsn_metric_si_sdr(const float* d_ref, const float* d_est, int32_t B, int64_t L, const int64_t* h_lengths, void* d_work,
+                                 int64_t work_bytes, double* d_out, void* stream) {
+    const char* fn = "fsn_metric_si_sdr";
+    long long Lmax = 0;
+    if (int rc = metric_check(fn, B, L, h_lengths, &Lmax)) return rc;
+    SiSdrLaunch a{};
+    if (int rc = metric_work_check(fn, d_ref, d_est, d_work, d_out, work_bytes, si_sdr_layout(a, nullptr, B, Lmax))) return rc;
+    si_sdr_layout(a, d_work, B, Lmax);
+    a.ref = d_ref; a.est = d_est; a.L = L; a.out = d_out;
+    const cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const std::vector<long long> len = metric_lengths(B, L, h_lengths);
+    CK(cudaMemcpyAsync(const_cast<long long*>(a.len), len.data(), len.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+    CK(launch_si_sdr(a, s));
+    return FSN_OK;
+}
+
+extern "C" int fsn_metric_stoi_workspace(int32_t B, int64_t L, const int64_t* h_lengths, int32_t sr, int64_t* bytes) {
+    const char* fn = "fsn_metric_stoi_workspace";
+    long long Lmax = 0;
+    if (!bytes) return fail(FSN_EINVAL, "%s: null bytes", fn);
+    if (int rc = metric_check(fn, B, L, h_lengths, &Lmax)) return rc;
+    if (int rc = metric_sr_check(fn, sr)) return rc;
+    StoiLaunch a{};
+    stoi_geometry(sr, a);
+    *bytes = (int64_t)stoi_layout(a, nullptr, B, Lmax);
+    return FSN_OK;
+}
+
+extern "C" int fsn_metric_stoi(const float* d_ref, const float* d_est, int32_t B, int64_t L, const int64_t* h_lengths, int32_t sr,
+                               void* d_work, int64_t work_bytes, double* d_out, void* stream) {
+    const char* fn = "fsn_metric_stoi";
+    long long Lmax = 0;
+    if (int rc = metric_check(fn, B, L, h_lengths, &Lmax)) return rc;
+    if (int rc = metric_sr_check(fn, sr)) return rc;
+    StoiLaunch a{};
+    stoi_geometry(sr, a);
+    if (int rc = metric_work_check(fn, d_ref, d_est, d_work, d_out, work_bytes, stoi_layout(a, nullptr, B, Lmax))) return rc;
+    stoi_layout(a, d_work, B, Lmax);
+    a.x = d_ref; a.y = d_est; a.L = L; a.out = d_out;
+    const cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const std::vector<long long> len = metric_lengths(B, L, h_lengths);
+    std::vector<float> tab;
+    stoi_tables(a, tab);
+    CK(cudaMemcpyAsync(const_cast<long long*>(a.len), len.data(), len.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(const_cast<float2*>(a.tw), tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+    CK(launch_stoi(a, s));
+    return FSN_OK;
+}

@@ -396,4 +396,28 @@ struct DwTmLaunch {
 };
 int launch_dwconv_tm(const DwTmLaunch& a, cudaStream_t s);
 
+// ---- k_metrics.cu (fsn_metric_si_sdr, fsn_metric_stoi) -----------------------------------------------------------------------
+struct SiSdrLaunch {
+    const float* ref; const float* est; long long L; int B;    // [B, L] rows, clip b = the first len[b] samples of its row
+    const long long* len;                                      // [B], on the device
+    int nchunk; double2* part; double* alpha; double* out;     // partials [B, nchunk], alpha [B], scores [B]
+};
+// Sets a's workspace pointers (ws = nullptr: offsets from 0) for B clips of at most Lmax samples; returns the bytes.
+size_t si_sdr_layout(SiSdrLaunch& a, void* ws, int B, long long Lmax);
+cudaError_t launch_si_sdr(const SiSdrLaunch& a, cudaStream_t s);
+
+struct StoiLaunch {
+    const float* x; const float* y; long long L; int B;        // reference and estimate rows
+    const long long* len;                                      // [B], on the device
+    int up, down, half, ntap;                                  // 10 kHz = sr up / down; filter taps 2 half + 1, ntap per phase
+    const float* poly; const float* win; const float2* tw;     // stoi_tables, in the workspace
+    long long F; long long P;                                  // frame stride (the longest clip's frames), partial stride
+    double* energy; int* kept; int* nkept; double* env; double* part; double* out;
+};
+void stoi_geometry(int sr, StoiLaunch& a);                         // up, down, half, ntap of sr
+size_t stoi_table_floats(const StoiLaunch& a);
+void stoi_tables(const StoiLaunch& a, std::vector<float>& tab);   // what the workspace's table segment holds
+size_t stoi_layout(StoiLaunch& a, void* ws, int B, long long Lmax);  // as si_sdr_layout, after stoi_geometry
+cudaError_t launch_stoi(const StoiLaunch& a, cudaStream_t s);
+
 }  // namespace fsn

@@ -31,6 +31,7 @@ SYMBOLS = [
     "fsn_chunk_stream_state_layout", "fsn_chunk_stream_save_slots", "fsn_chunk_stream_load_slots",
     "fsn_model_forward_enhance_lim", "fsn_model_enhance_audio_lim", "fsn_stream_set_atten_lim", "fsn_chunk_stream_set_atten_lim",
     "fsn_stream_get_stage", "fsn_stream_fb_ws", "fsn_stream_step_audio_samples",
+    "fsn_metric_si_sdr_workspace", "fsn_metric_si_sdr", "fsn_metric_stoi_workspace", "fsn_metric_stoi",
 ]
 
 
@@ -214,6 +215,10 @@ def load_library():
     lib.fsn_model_enhance_audio_lim.argtypes = [vp, vp, i32, i64, C.POINTER(i64), fp, vp, vp]
     lib.fsn_stream_set_atten_lim.argtypes = [vp, i32, C.POINTER(i32), fp]
     lib.fsn_chunk_stream_set_atten_lim.argtypes = [vp, i32, C.POINTER(i32), fp]
+    lib.fsn_metric_si_sdr_workspace.argtypes = [i32, i64, C.POINTER(i64), C.POINTER(i64)]
+    lib.fsn_metric_si_sdr.argtypes = [vp, vp, i32, i64, C.POINTER(i64), vp, i64, vp, vp]
+    lib.fsn_metric_stoi_workspace.argtypes = [i32, i64, C.POINTER(i64), i32, C.POINTER(i64)]
+    lib.fsn_metric_stoi.argtypes = [vp, vp, i32, i64, C.POINTER(i64), i32, vp, i64, vp, vp]
     _LIB = lib
     return lib
 

@@ -67,9 +67,10 @@ def find_files(dirs):
     return files
 
 
-def read_wav(path, sr):
+def read_wav(path, sr, first_channel=False):
     """float32 mono in [-1, 1) like librosa.load(path, sr=sr)[0] (dataset_inference.py:36-37): integer PCM is divided by
-    its full scale, channels are averaged; a different sample rate is converted with a polyphase resampler."""
+    its full scale, channels are averaged (``first_channel``: the first channel is taken instead, like
+    librosa.load(path, sr=sr, mono=False)[0][0]); a different sample rate is converted with a polyphase resampler."""
     from scipy.io import wavfile
     rate, x = wavfile.read(str(path))
     if x.dtype == np.uint8:
@@ -79,7 +80,7 @@ def read_wav(path, sr):
     else:
         y = x.astype(np.float32)
     if y.ndim == 2:
-        y = y.mean(axis=1)
+        y = y[:, 0] if first_channel else y.mean(axis=1)
     if rate != sr:
         from math import gcd
         from scipy.signal import resample_poly

@@ -663,6 +663,29 @@ int fsn_gemm_f16(const void* d_a, const void* d_b, void* d_c, int64_t M, int32_t
 /* The N tile (128 or 256) fsn_gemm_f16 runs that shape with, or FSN_EINVAL for a shape it rejects; host only. */
 int32_t fsn_gemm_f16_tile_n(int64_t M, int32_t N, int32_t K, int32_t tile_n);
 
+/* ---- Speech metrics (DESIGN.md §3.20): no model, no weights ----------------------------------------------------------------
+ * Objective scores of an estimate against its clean reference, one float64 score per clip.  d_ref and d_est are [B, L] float32 device
+ * rows; clip b is the first h_lengths[b] samples of its rows (h_lengths == NULL: every clip is L samples).  No reduction crosses clips:
+ * a clip's score is bit-identical whatever else is in the batch.  d_work is a device buffer of at least the bytes the matching
+ * *_workspace call reports for the same B, L, h_lengths (and sr); the call enqueues on `stream` and returns before the scores exist.
+ * Every argument is checked before any device work: FSN_EINVAL, naming the argument, for B outside 1 .. 65535, L outside
+ * 1 .. 2^31 - 1, a clip length outside 1 .. L (naming the clip), sr outside 8000 .. 48000, a null pointer or too small a workspace. */
+
+/* SI-SDR in dB: 10 log10(|a r|^2 / |e - a r|^2), a = <r, e> / <r, r>, accumulated in fp64 over two passes.  A silent reference
+ * gives NaN, an estimate equal to the reference +inf (as the float64 formula does).  Workspace: B (16 ceil(max L_b / 16384) + 16)
+ * bytes, rounded up. */
+int fsn_metric_si_sdr_workspace(int32_t B, int64_t L, const int64_t* h_lengths, int64_t* bytes);
+int fsn_metric_si_sdr(const float* d_ref, const float* d_est, int32_t B, int64_t L, const int64_t* h_lengths, void* d_work,
+                      int64_t work_bytes, double* d_out, void* stream);
+
+/* Classic STOI (Taal et al. 2011) as pystoi 0.3.3's stoi(ref, est, sr, extended=False) computes it: resampling to 10 kHz, removal of
+ * the frames more than 40 dB below the reference's loudest, 15 one-third-octave band envelopes, 30-frame segments.  A clip with fewer
+ * than 30 envelope frames after silent-frame removal, or with no frame at all, scores 1e-5.  Workspace: about 270 bytes per 128
+ * samples at 10 kHz of the longest clip, per clip, plus the resampling filter. */
+int fsn_metric_stoi_workspace(int32_t B, int64_t L, const int64_t* h_lengths, int32_t sr, int64_t* bytes);
+int fsn_metric_stoi(const float* d_ref, const float* d_est, int32_t B, int64_t L, const int64_t* h_lengths, int32_t sr, void* d_work,
+                    int64_t work_bytes, double* d_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

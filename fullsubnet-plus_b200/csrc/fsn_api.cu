@@ -36,16 +36,20 @@ struct DevBuf {
     void* p = nullptr;
     size_t bytes = 0;
     // grow-only; a fresh allocation is zero-filled ON THE STREAM THAT WILL USE IT (a legacy-stream cudaMemset is not ordered
-    // against kernels on a non-blocking stream)
-    int ensure(size_t n, bool zero, cudaStream_t s = nullptr) {
-        if (n <= bytes) return 0;
-        if (p) cudaFree(p);
-        p = nullptr; bytes = 0;
-        cudaError_t e = cudaMalloc(&p, n);
-        if (e != cudaSuccess) return (int)e;
-        bytes = n;
-        if (zero) e = cudaMemsetAsync(p, 0, n, s);
-        return (int)e;
+    // against kernels on a non-blocking stream).  poison (FSN_POISON, fsn_model::env_poison): a buffer not promised zero is filled
+    // whole with 0xFF bytes on the same stream at every call that ensures it -- NaN in fp16 / fp32 / fp64, -1 in int32 -- so that
+    // a read of anything the call did not write shows in its outputs.  Without it nothing is enqueued unless the buffer grows.
+    int ensure(size_t n, bool zero, cudaStream_t s = nullptr, bool poison = false) {
+        if (n > bytes) {
+            if (p) cudaFree(p);
+            p = nullptr; bytes = 0;
+            cudaError_t e = cudaMalloc(&p, n);
+            if (e != cudaSuccess) return (int)e;
+            bytes = n;
+            if (zero && (e = cudaMemsetAsync(p, 0, n, s)) != cudaSuccess) return (int)e;
+        }
+        if (poison && !zero && p) return (int)cudaMemsetAsync(p, 0xFF, bytes, s);
+        return 0;
     }
     void release() { if (p) cudaFree(p); p = nullptr; bytes = 0; }
 };
@@ -219,6 +223,10 @@ struct fsn_model {
     int env_sb_chunk = 0;                              // FSN_SB_CHUNK: run the sub-band TCN in chunks of this many bins (>= num_freqs: unchunked)
     Plan plan;                                         // plan of the last plain forward
     bool env_no_ws = false;
+    // FSN_POISON=1 (tests): every call fills the scratch it uses that is not promised zero with NaN first (DevBuf::ensure's poison):
+    // the forward workspace entries of WS without WS_ZERO, and the streaming and chunk-session scratch; handles made from the model
+    // take it from here.  State, weights, tables and staging are never filled.
+    bool env_poison = false;
     int env_gin_tile_n = 0;                            // FSN_GIN_GEMM=128: the input-projection GEMM on 128 x 128 tiles (GemmF16Launch::tile_n)
     // pipelined execution: front-end stream, LSTM stream (higher priority), copy-in / copy-out streams, per-slot events
     cudaStream_t s_front = nullptr, s_lstm = nullptr, s_in = nullptr, s_out = nullptr;
@@ -645,6 +653,7 @@ extern "C" int fsn_model_create(const fsn_config* cfg, fsn_model** out) {
     { const char* e = getenv("FSN_LSTM_IMPL"); if (e && *e) m->env_impl = atoi(e); }
     m->layerwise = runs_layerwise(c, m->env_impl);
     { const char* e = getenv("FSN_NO_WS"); m->env_no_ws = e && atoi(e) != 0; }
+    { const char* e = getenv("FSN_POISON"); m->env_poison = e && atoi(e) != 0; }
     { const char* e = getenv("FSN_FRONT_OVERLAP"); m->env_front_overlap = e && atoi(e) != 0; }
     // FSN_PDL: programmatic dependent launch of the ~30 kernels of the front-end chain.  0 = never, 1 = always, unset = only for small
     // batches, where the forward is launch-latency-bound; for large batches a denser front end leaves no gaps for the side stream's
@@ -1097,7 +1106,7 @@ static WsSizes ws_sizes(const fsn_config& c, bool layerwise, int B, int T, int T
 using Lane = fsn_model::Lane;
 enum : unsigned {
     WS_LANE = 1,        // one per lane (else one for the model, shared by both lanes: the sub-band stage runs one batch at a time)
-    WS_ZERO = 2,        // a fresh allocation is zero-filled, on the buffer's stream
+    WS_ZERO = 2,        // a fresh allocation is zero-filled, on the buffer's stream; without it, FSN_POISON fills it with NaN at every call
     WS_SL = 4,          // ordered on the sub-band stream sl (else the front stream s)
     WS_REGEO = 8,       // a new geometry frees it first: the fresh zero-filled allocation keeps pad rows and columns zero
     WS_ON_USE = 16,     // allocated where it is used, not by ensure_ws: ragged extents, weight-stationary LSTM, the scratch mask
@@ -1141,7 +1150,7 @@ static const WsBuf WS[] = {
     {LANE_BUF(fbx), &WsSizes::fbx, WS_LANE | WS_ZERO},
     {LANE_BUF(hseq), &WsSizes::hseq, WS_LANE | WS_ZERO},
     {LANE_BUF(tlen), &WsSizes::tlen, WS_LANE | WS_ON_USE},                         // stage_lengths
-    {MODEL_BUF(ws_h), &WsSizes::ws_h, WS_ON_USE},                                  // forward_impl
+    {MODEL_BUF(ws_h), &WsSizes::ws_h, WS_ON_USE},                                  // front_end: zeroed by every forward that uses it
     {MODEL_BUF(ws_bar), &WsSizes::ws_bar, WS_ON_USE},
     {MODEL_BUF(mask_tmp), &WsSizes::mask_tmp, WS_ON_USE},                          // run_sb_lstm
     {MODEL_BUF(au_planes), &WsSizes::au_planes, 0},                                // written whole by the analysis kernel
@@ -1362,7 +1371,7 @@ static int ensure_ws(fsn_model* m, Lane& ln, int B, int T, int Tw, int Fc, cudaS
         DevBuf& b = e.buf(*m, ln);
         if (e.flags & WS_ON_USE) continue;
         if (regeo && (e.flags & WS_REGEO)) b.release();
-        if (b.ensure(z.*e.need, e.flags & WS_ZERO, (e.flags & WS_SL) ? sl : s)) return fail(FSN_ECUDA, "workspace allocation failed for B=%d T=%d", B, T);
+        if (b.ensure(z.*e.need, e.flags & WS_ZERO, (e.flags & WS_SL) ? sl : s, m->env_poison)) return fail(FSN_ECUDA, "workspace allocation failed for B=%d T=%d", B, T);
     }
     // every forward encodes the tensor maps on the buffers as they now are: none outlives the allocation it was encoded for
     if (c.sb_tcn) {
@@ -1470,7 +1479,7 @@ static int run_sb_lstm(fsn_model* m, Lane& ln, const Batch& b, int Tw, SbPackLau
         lstm_mma_cstate_bytes(c.num_layers, rows, c.sb_hidden, &a.rows_alloc);
         a.out = b.mask; a.la = c.look_ahead; a.tlen = tlen;
         if (b.enh) {                                                    // generic kernel: mask into a scratch buffer, then one fused post-processing pass
-            if (m->mask_tmp.ensure((size_t)B * 2 * F * T * 4, false, s)) return fail(FSN_ECUDA, "allocation failed");
+            if (m->mask_tmp.ensure((size_t)B * 2 * F * T * 4, false, s, m->env_poison)) return fail(FSN_ECUDA, "allocation failed");
             a.out = static_cast<float*>(m->mask_tmp.p);
         }
         int e = launch_lstm_mma(a, s);
@@ -1619,7 +1628,7 @@ static int stage_lengths(fsn_model* m, Lane& ln, const int32_t* h_frames, int B,
         for (int b = 0; b < B; ++b) h[(size_t)br * B + b] = h_frames ? h_frames[b] + m->cfg.look_ahead : 0;
     if (h_samples) memcpy(h + (size_t)3 * B, h_samples, (size_t)B * sizeof(int32_t));
     if (h_lam) memcpy(h + rows * B, h_lam, (size_t)B * sizeof(float));
-    if (ln.tlen.ensure(n * sizeof(int32_t), false, s)) return fail(FSN_ECUDA, "workspace allocation failed for the clip lengths");
+    if (ln.tlen.ensure(n * sizeof(int32_t), false, s, m->env_poison)) return fail(FSN_ECUDA, "workspace allocation failed for the clip lengths");
     if (h_lam) *d_lam = reinterpret_cast<const float*>(static_cast<const int32_t*>(ln.tlen.p) + rows * B);
     return m->len_stage.send(ln.tlen.p, n, s);
 }
@@ -2285,10 +2294,11 @@ struct fsn_stream {
 
 int StepScratch::ensure(const fsn_stream& st, int K, size_t img, bool zero, cudaStream_t s) {
     const size_t B = st.B, F = st.m->cfg.num_freqs, P = (K + 3) & ~3;
-    int e = fbin.ensure(B * F * P * 4, zero, s);
-    e |= fbx.ensure((size_t)K * st.rows_pad * st.Ipad * 2, zero, s);
-    e |= hseq.ensure(B * st.m->cfg.fb_hidden * P * 4, zero, s);
-    e |= fbout.ensure(B * F * P * 4, zero, s);
+    const bool poison = st.m->env_poison;                               // the images' pad rows stay zero: never poisoned
+    int e = fbin.ensure(B * F * P * 4, zero, s, poison);
+    e |= fbx.ensure((size_t)K * st.rows_pad * st.Ipad * 2, zero, s, poison);
+    e |= hseq.ensure(B * st.m->cfg.fb_hidden * P * 4, zero, s, poison);
+    e |= fbout.ensure(B * F * P * 4, zero, s, poison);
     e |= ximg.ensure(img, true, s);
     return e;
 }
@@ -2549,6 +2559,10 @@ extern "C" int fsn_stream_step(fsn_stream* st, const float* d_mag, float* d_mask
         return FSN_OK;
     }
     const int n = st->n;
+    const fsn_config& c = st->m->cfg;
+    // sized at create: grows nothing, and enqueues only FSN_POISON's fill
+    if (st->tick.ensure(*st, 1, step_img_bytes(c, (long long)st->B * c.num_freqs, 1), false, static_cast<cudaStream_t>(stream)))
+        return fail(FSN_ECUDA, "step scratch allocation failed");
     const int rc = step_frames(st, st->tick, d_mag, 1, nullptr, nullptr, nullptr, 0, d_mask, nullptr, static_cast<cudaStream_t>(stream));
     if (rc) return rc;
     if (h_valid) *h_valid = (n >= st->m->cfg.look_ahead) ? 1 : 0;
@@ -2626,12 +2640,13 @@ static int chunk_lw_ensure(fsn_stream* st, const Plan& p, int K, cudaStream_t s)
     const fsn_config& c = st->m->cfg;
     const int F = c.num_freqs, nt = (p.Bs * F + 127) / 128;
     const WsSizes z = ws_sizes(c, true, p.Bs, K, p.Tw ? p.Tw : K);
+    const bool poison = st->m->env_poison;
     int e = st->chunk.ensure(*st, K, z.ximg, false, s);
-    e |= st->c_gin.ensure(z.r_gin, false, s);
-    e |= st->c_hsb.ensure(z.r_hseq, false, s);
+    e |= st->c_gin.ensure(z.r_gin, false, s, poison);
+    e |= st->c_hsb.ensure(z.r_hseq, false, s, poison);
     e |= st->c_h.ensure(z.r_hstate, true, s);
     e |= st->c_c.ensure((size_t)c.num_layers * lstm_tc5r_cstate_bytes(nt, c.sb_hidden), true, s);
-    e |= st->c_mask.ensure((size_t)p.Bs * 2 * F * K * sizeof(float), false, s);
+    e |= st->c_mask.ensure((size_t)p.Bs * 2 * F * K * sizeof(float), false, s, poison);
     return e;
 }
 
@@ -2838,9 +2853,9 @@ static int run_audio(fsn_stream* st, const std::vector<AudioSlotPlan>& plan, con
     const size_t smp_at = nstage;                                       // the sample call's two planes after everything else
     if (smp) nstage += 2 * (size_t)B;
     if (Km) e |= x.ensure(*st, Km, layerwise ? 0 : step_img_bytes(c, (long long)B * F, Km), false, s);
-    e |= st->x_spec.ensure((size_t)B * K * F * sizeof(float2), false, s);
-    e |= st->x_mag.ensure((size_t)B * F * Km * sizeof(float), false, s);
-    e |= st->x_mask.ensure((size_t)B * 2 * F * Km * sizeof(float), false, s);
+    e |= st->x_spec.ensure((size_t)B * K * F * sizeof(float2), false, s, m->env_poison);
+    e |= st->x_mag.ensure((size_t)B * F * Km * sizeof(float), false, s, m->env_poison);
+    e |= st->x_mask.ensure((size_t)B * 2 * F * Km * sizeof(float), false, s, m->env_poison);
     e |= st->x_plan.ensure(nstage * sizeof(int32_t), false, s);
     if (e) return fail(FSN_ECUDA, "audio chunk scratch allocation failed (B = %d, K = %d)", B, K);
     if (int rc = claim_mode(st, FSN_STATE_MODE_AUDIO)) return rc;
@@ -3217,7 +3232,7 @@ extern "C" int fsn_chunk_stream_step(fsn_chunk_stream* cs, const float* d_sample
     if (nrows)
         if (int rc = check_batch(cs->m, fwd, &lens, &row_lam)) return rc;
     const size_t rb = (size_t)nrows * W * sizeof(float);
-    int e = nrows ? cs->rows.ensure(rb, false, s) | cs->enh.ensure(rb, false, s) : 0;
+    int e = nrows ? cs->rows.ensure(rb, false, s, cs->m->env_poison) | cs->enh.ensure(rb, false, s, cs->m->env_poison) : 0;
     if (e) return fail(FSN_ECUDA, "chunk row allocation failed (%d rows of %d samples)", nrows, W);
     int32_t* h = nullptr;
     if (int rc = cs->stage.take(plan.size(), &h)) return rc;

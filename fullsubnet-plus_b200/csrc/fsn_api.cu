@@ -3816,3 +3816,29 @@ extern "C" int fsn_metric_stoi(const float* d_ref, const float* d_est, int32_t B
     CK(launch_stoi(a, s));
     return FSN_OK;
 }
+
+extern "C" int fsn_metric_sdr_workspace(int32_t B, int64_t L, const int64_t* h_lengths, int64_t* bytes) {
+    const char* fn = "fsn_metric_sdr_workspace";
+    long long Lmax = 0;
+    if (!bytes) return fail(FSN_EINVAL, "%s: null bytes", fn);
+    if (int rc = metric_check(fn, B, L, h_lengths, &Lmax)) return rc;
+    SdrLaunch a{};
+    *bytes = (int64_t)sdr_layout(a, nullptr, B, Lmax);
+    return FSN_OK;
+}
+
+extern "C" int fsn_metric_sdr(const float* d_ref, const float* d_est, int32_t B, int64_t L, const int64_t* h_lengths, void* d_work,
+                              int64_t work_bytes, double* d_out, void* stream) {
+    const char* fn = "fsn_metric_sdr";
+    long long Lmax = 0;
+    if (int rc = metric_check(fn, B, L, h_lengths, &Lmax)) return rc;
+    SdrLaunch a{};
+    if (int rc = metric_work_check(fn, d_ref, d_est, d_work, d_out, work_bytes, sdr_layout(a, nullptr, B, Lmax))) return rc;
+    sdr_layout(a, d_work, B, Lmax);
+    a.ref = d_ref; a.est = d_est; a.L = L; a.out = d_out;
+    const cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const std::vector<long long> len = metric_lengths(B, L, h_lengths);
+    CK(cudaMemcpyAsync(const_cast<long long*>(a.len), len.data(), len.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+    CK(launch_sdr(a, s));
+    return FSN_OK;
+}

@@ -396,7 +396,7 @@ struct DwTmLaunch {
 };
 int launch_dwconv_tm(const DwTmLaunch& a, cudaStream_t s);
 
-// ---- k_metrics.cu (fsn_metric_si_sdr, fsn_metric_stoi) -----------------------------------------------------------------------
+// ---- k_metrics.cu (fsn_metric_si_sdr, fsn_metric_stoi, fsn_metric_sdr) -----------------------------------------------------------------------
 struct SiSdrLaunch {
     const float* ref; const float* est; long long L; int B;    // [B, L] rows, clip b = the first len[b] samples of its row
     const long long* len;                                      // [B], on the device
@@ -419,5 +419,17 @@ size_t stoi_table_floats(const StoiLaunch& a);
 void stoi_tables(const StoiLaunch& a, std::vector<float>& tab);   // what the workspace's table segment holds
 size_t stoi_layout(StoiLaunch& a, void* ws, int B, long long Lmax);  // as si_sdr_layout, after stoi_geometry
 cudaError_t launch_stoi(const StoiLaunch& a, cudaStream_t s);
+
+struct SdrLaunch {
+    const float* ref; const float* est; long long L; int B;    // as SiSdrLaunch
+    const long long* len;                                      // [B], on the device
+    long long nct, npt;                                        // correlation / projection tiles of the longest clip (partial strides)
+    double* corr;                                              // per-tile partials [B, nct, 1024]: R[0 .. 511], D[0 .. 511]
+    double* rd;                                                // their per-clip sums [B, 1024]
+    double* coef;                                              // distortion filter c [B, 512] (NaN where the solve stopped)
+    double2* part; double* out;                                // projection partials [B, npt] (sum P^2, sum (e' - P)^2), scores [B]
+};
+size_t sdr_layout(SdrLaunch& a, void* ws, int B, long long Lmax);  // as si_sdr_layout
+cudaError_t launch_sdr(const SdrLaunch& a, cudaStream_t s);
 
 }  // namespace fsn

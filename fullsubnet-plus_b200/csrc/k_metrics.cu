@@ -1,6 +1,7 @@
-// Objective scores of enhanced speech against its clean reference (fsn_metric_si_sdr, fsn_metric_stoi; DESIGN.md §3.20), one
-// score per clip of a ragged [B, L] batch.  Every reduction that feeds a decision or a score is fp64, over a fixed per-clip tiling
-// and in a fixed order, with no atomics: a clip's score depends on its own samples only, bit for bit, whatever else is in the batch.
+// Objective scores of enhanced speech against its clean reference (fsn_metric_si_sdr, fsn_metric_stoi, DESIGN.md §3.20;
+// fsn_metric_sdr, §3.21), one score per clip of a ragged [B, L] batch.  Every reduction that feeds a decision or a score is fp64,
+// over a fixed per-clip tiling and in a fixed order, with no atomics: a clip's score depends on its own samples only, bit for bit,
+// whatever else is in the batch.
 //
 // SI-SDR: two passes over the samples (the noise energy |e - a r|^2 is summed directly: the closed form |e|^2 - 2 a <r, e> + a^2 |r|^2
 // cancels catastrophically at high SI-SDR), each a per-chunk partial kernel and a per-clip finalize kernel.
@@ -9,6 +10,10 @@
 // recomputed wherever a 10 kHz sample is needed, never stored.  Four kernels: frame energies of x; a per-clip max and keep-mask
 // compaction; the band envelopes of the compacted x and y, gathered straight from the kept frames' original positions; the
 // per-segment correlations with per-CTA partials; and the per-clip mean.
+//
+// SDR (BSS Eval v3 for one source, mir_eval's 512-tap distortion filter), fp64 throughout: the 512-lag auto- and cross-correlations
+// as per-tile partials and their per-clip sum; a Levinson solve of the 512 x 512 Toeplitz system per clip; the projection P = c * r
+// computed explicitly with per-tile sums of P^2 and (e' - P)^2 (the closed form |e|^2 - c.D cancels at high SDR); the per-clip score.
 #include <cmath>
 #include <vector>
 
@@ -27,6 +32,11 @@ constexpr int STOI_SEGS = 16;                // segments per CTA of the correlat
 constexpr int STOI_SCAN_THREADS = 1024;
 constexpr double STOI_EPS = 2.220446049250313e-16;   // float64 machine epsilon
 constexpr double STOI_SHORT = 1e-5;                  // fewer than 30 envelope frames
+constexpr int SDR_F = 512;                   // distortion filter taps = correlation lags
+constexpr int SDR_KB = 16;                   // lags per register block of the correlation kernel (x 2: R and D)
+constexpr int SDR_RUN = 112;                 // samples per lane of the correlation kernel
+constexpr int SDR_CORR_TILE = 32 * SDR_RUN;  // 3584 samples per correlation CTA
+constexpr int SDR_PROJ_TILE = 4096;          // outputs per projection CTA: 16 per thread
 
 __constant__ int c_band_lo[STOI_BANDS] = {7, 9, 11, 14, 17, 22, 27, 34, 43, 55, 69, 87, 109, 138, 174};
 __constant__ int c_band_hi[STOI_BANDS] = {9, 11, 14, 17, 22, 27, 34, 43, 55, 69, 87, 109, 138, 174, 219};
@@ -355,6 +365,215 @@ cudaError_t launch_stoi(const StoiLaunch& a, cudaStream_t s) {
     stoi_envelope_kernel<<<dim3(grid_x(a.F - 1, STOI_ENV_FRAMES), a.B), MET_THREADS, 0, s>>>(a);
     stoi_segment_kernel<<<dim3(grid_x(a.F - STOI_SEG, STOI_SEGS), a.B), MET_THREADS, 0, s>>>(a);
     stoi_final_kernel<<<a.B, MET_THREADS, 0, s>>>(a);
+    return cudaGetLastError();
+}
+
+// ---- SDR (BSS Eval v3, one source, 512-tap distortion filter) --------------------------------------------------------------------
+
+// Shared-memory index of staged sample m: one pad double per 16, so runs that start 16 q samples apart (q odd, or q = 1 plus its pad)
+// sit an odd number of doubles apart and a half-warp's 64-bit loads hit 16 different bank pairs.
+__device__ __forceinline__ int sdr_pad(int m) { return m + (m >> 4); }
+
+constexpr int SDR_CS = SDR_CORR_TILE + SDR_F + (SDR_CORR_TILE + SDR_F) / 16;   // padded staged length per signal, correlations
+constexpr int SDR_PS = SDR_PROJ_TILE + SDR_F + (SDR_PROJ_TILE + SDR_F) / 16;   // the same, projection
+static_assert(SDR_RUN % SDR_KB == 0 && (SDR_RUN / 16) % 2 == 1 && SDR_PROJ_TILE == MET_THREADS * 16, "sdr tiling");
+
+// Sums each of the 2 H accumulators over the warp and leaves the sum of accumulator l in lane l's acc[0]: at each halving step the
+// lanes with bit h set keep the upper half of the live accumulators and their partners the lower half (fixed pairs, fixed order).
+template <int H>
+__device__ __forceinline__ void reduce_scatter(double* acc, int lane) {
+    const bool up = lane & H;
+#pragma unroll
+    for (int j = 0; j < H; ++j) {
+        const double send = up ? acc[j] : acc[j + H], keep = up ? acc[j + H] : acc[j];
+        acc[j] = keep + __shfl_xor_sync(0xffffffffu, send, H);
+    }
+    if constexpr (H > 1) reduce_scatter<H / 2>(acc, lane);
+}
+
+// grid (ceil(max L_b / 3584), B): samples n0 .. n0 + 3583 of clip b.  r and e are staged as fp64 with a 512-sample halo (zero past
+// L_b); an fp32 x fp32 product is exact in fp64, so only the sums round.  Warp w takes lag blocks k0 = 16 kb, kb = w, w + 8, ..; lane l
+// sums its 112-sample run n0 + 112 l + s for all 16 lags of R and of D, with the 16 values r[n + k0 + j] and e[n + k0 + j] in a
+// circular register window that takes one new sample per step.  A reduce-scatter over the lanes (fixed pairs, so fixed order) leaves
+// lane l with the warp's sum of accumulator l: R[k0 + l] for l < 16, D[k0 + l - 16] above.  Partial [b][tile][R 0..511, D 0..511].
+__global__ void __launch_bounds__(MET_THREADS) sdr_corr_kernel(SdrLaunch a) {
+    extern __shared__ __align__(8) double sdr_sm[];
+    double* rs = sdr_sm;
+    double* es = sdr_sm + SDR_CS;
+    const int b = blockIdx.y;
+    const long long Lb = a.len[b], n0 = (long long)blockIdx.x * SDR_CORR_TILE;
+    if (n0 >= Lb) return;                                         // block-uniform
+    const float* r = a.ref + (size_t)b * a.L;
+    const float* e = a.est + (size_t)b * a.L;
+    for (int m = threadIdx.x; m < SDR_CORR_TILE + SDR_F; m += MET_THREADS) {
+        const long long n = n0 + m;
+        rs[sdr_pad(m)] = n < Lb ? (double)__ldg(r + n) : 0.0;
+        es[sdr_pad(m)] = n < Lb ? (double)__ldg(e + n) : 0.0;
+    }
+    __syncthreads();
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31, m0 = lane * SDR_RUN;
+    double* out = a.corr + ((size_t)b * a.nct + blockIdx.x) * (2 * SDR_F);
+    for (int kb = w; kb < SDR_F / SDR_KB; kb += MET_THREADS / 32) {
+        const int k0 = kb * SDR_KB;
+        double acc[2 * SDR_KB], wr[SDR_KB], we[SDR_KB];
+#pragma unroll
+        for (int j = 0; j < SDR_KB; ++j) {
+            acc[j] = 0.0; acc[SDR_KB + j] = 0.0;
+            wr[j] = rs[sdr_pad(m0 + k0 + j)]; we[j] = es[sdr_pad(m0 + k0 + j)];
+        }
+        for (int s = 0; s < SDR_RUN; s += SDR_KB) {                  // m0 + s and m0 + s + k0 + 16 are multiples of 16
+            const double* xr = rs + sdr_pad(m0 + s);
+            const double* nr = rs + sdr_pad(m0 + s + k0 + SDR_KB);
+            const double* ne = es + sdr_pad(m0 + s + k0 + SDR_KB);
+#pragma unroll
+            for (int u = 0; u < SDR_KB; ++u) {                       // slot (u + j) % 16 holds sample m0 + s + u + k0 + j
+                const double x = xr[u];
+#pragma unroll
+                for (int j = 0; j < SDR_KB; ++j) {
+                    acc[j] = fma(x, wr[(u + j) % SDR_KB], acc[j]);
+                    acc[SDR_KB + j] = fma(x, we[(u + j) % SDR_KB], acc[SDR_KB + j]);
+                }
+                wr[u] = nr[u];
+                we[u] = ne[u];
+            }
+        }
+        reduce_scatter<16>(acc, lane);
+        out[lane < SDR_KB ? k0 + lane : SDR_F + k0 + lane - SDR_KB] = acc[0];
+    }
+}
+
+// grid (32, B): correlations 32 x .. 32 x + 31 of clip b summed over its tiles.  Warp g sums tiles g, g + 8, .. in order; lane 0 .. 31
+// of warp 0 then adds the eight warp sums in warp order.
+__global__ void __launch_bounds__(MET_THREADS) sdr_corr_sum_kernel(SdrLaunch a) {
+    __shared__ double sh[MET_THREADS / 32][32];
+    const int b = blockIdx.y, w = threadIdx.x >> 5, lane = threadIdx.x & 31, i = blockIdx.x * 32 + lane;
+    const long long nt = (a.len[b] + SDR_CORR_TILE - 1) / SDR_CORR_TILE;
+    const double* p = a.corr + (size_t)b * a.nct * (2 * SDR_F) + i;
+    double s = 0.0;
+    for (long long t = w; t < nt; t += MET_THREADS / 32) s += p[t * (2 * SDR_F)];
+    sh[w][lane] = s;
+    __syncthreads();
+    if (w == 0) {
+        s = sh[0][lane];
+        for (int k = 1; k < MET_THREADS / 32; ++k) s += sh[k][lane];
+        a.rd[(size_t)b * 2 * SDR_F + i] = s;
+    }
+}
+
+// grid B, one warp: G c = D by Levinson's recursion (Durbin's prediction-error filter f, G_m f = E_m e_0, grown one order per step,
+// and the solution x of the leading m x m system corrected by (D_m - <x, R[m - .]>) / E_{m+1} times the reversed new filter), fp64.
+// R[0] = 0 (a silent reference) or a prediction error that is not a positive finite number stops it, and c is NaN.
+__global__ void __launch_bounds__(32) sdr_solve_kernel(SdrLaunch a) {
+    __shared__ double R[SDR_F], D[SDR_F], f[2][SDR_F], x[SDR_F];
+    const int b = blockIdx.x, lane = threadIdx.x;
+    const double* rd = a.rd + (size_t)b * 2 * SDR_F;
+    for (int i = lane; i < SDR_F; i += 32) { R[i] = rd[i]; D[i] = rd[SDR_F + i]; f[0][i] = f[1][i] = x[i] = 0.0; }
+    __syncwarp();
+    double E = R[0];
+    bool ok = E > 0.0;
+    if (lane == 0) { f[0][0] = 1.0; x[0] = D[0] / E; }
+    __syncwarp();
+    for (int m = 1, cur = 0; m < SDR_F && ok; ++m, cur ^= 1) {      // f[cur] holds the order-m filter, zero from index m on
+        const double* A = f[cur];
+        double* An = f[cur ^ 1];
+        double dl = 0.0, ep = 0.0;
+        for (int j = lane; j < m; j += 32) { const double rr = R[m - j]; dl = fma(A[j], rr, dl); ep = fma(x[j], rr, ep); }
+        for (int o = 16; o; o >>= 1) { dl += __shfl_xor_sync(0xffffffffu, dl, o); ep += __shfl_xor_sync(0xffffffffu, ep, o); }
+        const double kappa = -dl / E;
+        E = fma(kappa, dl, E);                                        // E_m (1 - kappa^2)
+        ok = E > 0.0 && isfinite(E);                                  // the same on every lane: the butterfly sums are
+        for (int j = lane; j <= m; j += 32) An[j] = fma(kappa, A[m - j], A[j]);
+        __syncwarp();
+        const double g = (D[m] - ep) / E;
+        for (int j = lane; j <= m; j += 32) x[j] = fma(g, An[m - j], x[j]);
+        __syncwarp();
+    }
+    for (int i = lane; i < SDR_F; i += 32) a.coef[(size_t)b * SDR_F + i] = ok ? x[i] : __longlong_as_double(0x7ff8000000000000LL);
+}
+
+// grid (ceil((max L_b + 511) / 4096), B): outputs p0 .. p0 + 4095 of clip b.  r[p0 - 512 ..] is staged as fp64 (zero outside the clip);
+// thread t computes P[n] = sum_k c[k] r[n - k] for its 16 outputs q0 = 16 t .., the values r[n - k] in a circular window that takes one
+// new sample per lag, then sums P^2 and (e' - P)^2 in output order; the CTA's sums (block_sum) are partial blockIdx.x.  Past
+// n = L_b + 510 both P and e' are zero, so a tile's tail adds nothing.
+__global__ void __launch_bounds__(MET_THREADS) sdr_proj_kernel(SdrLaunch a) {
+    __shared__ double rs[SDR_PS];
+    __shared__ double cs[SDR_F];
+    __shared__ double sh[33];
+    const int b = blockIdx.y;
+    const long long Lb = a.len[b], p0 = (long long)blockIdx.x * SDR_PROJ_TILE;
+    if (p0 >= Lb + SDR_F - 1) return;                             // block-uniform
+    const float* r = a.ref + (size_t)b * a.L;
+    const float* e = a.est + (size_t)b * a.L;
+    for (int m = threadIdx.x; m < SDR_PROJ_TILE + SDR_F; m += MET_THREADS) {
+        const long long n = p0 - SDR_F + m;
+        rs[sdr_pad(m)] = n >= 0 && n < Lb ? (double)__ldg(r + n) : 0.0;
+    }
+    for (int k = threadIdx.x; k < SDR_F; k += MET_THREADS) cs[k] = a.coef[(size_t)b * SDR_F + k];
+    __syncthreads();
+    const int q0 = threadIdx.x * 16;
+    double acc[16], win[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) { acc[j] = 0.0; win[j] = rs[sdr_pad(q0 + SDR_F + j)]; }   // lag 0: slot j holds r[p0 + q0 + j]
+    for (int k0 = 0; k0 < SDR_F; k0 += 16) {
+        const double* nr = rs + sdr_pad(q0 + SDR_F - 16 - k0);       // next sample at lag k0 + u: nr[15 - u] (r[p0 + q0 - k0 - u - 1])
+#pragma unroll
+        for (int u = 0; u < 16; ++u) {                               // slot (j - u) % 16 holds r[p0 + q0 + j - k0 - u]
+            const double c = cs[k0 + u];
+#pragma unroll
+            for (int j = 0; j < 16; ++j) acc[j] = fma(c, win[(j - u + 16) % 16], acc[j]);
+            win[15 - u] = nr[15 - u];
+        }
+    }
+    double sp = 0.0, sn = 0.0;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+        const long long n = p0 + q0 + j;
+        const double ev = n < Lb ? (double)__ldg(e + n) : 0.0, d = ev - acc[j];
+        sp = fma(acc[j], acc[j], sp);
+        sn = fma(d, d, sn);
+    }
+    sp = block_sum(sp, sh);
+    sn = block_sum(sn, sh);
+    if (threadIdx.x == 0) a.part[(size_t)b * a.npt + blockIdx.x] = make_double2(sp, sn);
+}
+
+// grid B: clip b's projection partials in tile order, then 10 log10(sum P^2 / sum (e' - P)^2).
+__global__ void __launch_bounds__(MET_THREADS) sdr_final_kernel(SdrLaunch a) {
+    __shared__ double sh[33];
+    const int b = blockIdx.x;
+    const int n = (int)((a.len[b] + SDR_F - 1 + SDR_PROJ_TILE - 1) / SDR_PROJ_TILE);
+    const double2* p = a.part + (size_t)b * a.npt;
+    double s0 = 0.0, s1 = 0.0;
+    for (int i = threadIdx.x; i < n; i += MET_THREADS) { s0 += p[i].x; s1 += p[i].y; }
+    s0 = block_sum(s0, sh);
+    s1 = block_sum(s1, sh);
+    if (threadIdx.x == 0) a.out[b] = 10.0 * log10(s0 / s1);
+}
+
+// [lengths: B int64][correlation partials: B x nct x 1024 double][R, D: B x 1024 double][c: B x 512 double][projection partials:
+// B x npt double2], nct = ceil(max L_b / 3584), npt = ceil((max L_b + 511) / 4096).
+size_t sdr_layout(SdrLaunch& a, void* ws, int B, long long Lmax) {
+    size_t off = 0;
+    a.B = B;
+    a.nct = (Lmax + SDR_CORR_TILE - 1) / SDR_CORR_TILE;
+    a.npt = (Lmax + SDR_F - 1 + SDR_PROJ_TILE - 1) / SDR_PROJ_TILE;
+    a.len = at<long long>(ws, carve(off, (size_t)B * sizeof(long long)));
+    a.corr = at<double>(ws, carve(off, (size_t)B * a.nct * 2 * SDR_F * sizeof(double)));
+    a.rd = at<double>(ws, carve(off, (size_t)B * 2 * SDR_F * sizeof(double)));
+    a.coef = at<double>(ws, carve(off, (size_t)B * SDR_F * sizeof(double)));
+    a.part = at<double2>(ws, carve(off, (size_t)B * a.npt * sizeof(double2)));
+    return off;
+}
+
+cudaError_t launch_sdr(const SdrLaunch& a, cudaStream_t s) {
+    const size_t smem = 2 * SDR_CS * sizeof(double);
+    cudaError_t e = cudaFuncSetAttribute(sdr_corr_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    sdr_corr_kernel<<<dim3((unsigned)a.nct, a.B), MET_THREADS, smem, s>>>(a);
+    sdr_corr_sum_kernel<<<dim3(2 * SDR_F / 32, a.B), MET_THREADS, 0, s>>>(a);
+    sdr_solve_kernel<<<a.B, 32, 0, s>>>(a);
+    sdr_proj_kernel<<<dim3((unsigned)a.npt, a.B), MET_THREADS, 0, s>>>(a);
+    sdr_final_kernel<<<a.B, MET_THREADS, 0, s>>>(a);
     return cudaGetLastError();
 }
 

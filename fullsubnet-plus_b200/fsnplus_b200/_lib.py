@@ -32,6 +32,7 @@ SYMBOLS = [
     "fsn_model_forward_enhance_lim", "fsn_model_enhance_audio_lim", "fsn_stream_set_atten_lim", "fsn_chunk_stream_set_atten_lim",
     "fsn_stream_get_stage", "fsn_stream_fb_ws", "fsn_stream_step_audio_samples",
     "fsn_metric_si_sdr_workspace", "fsn_metric_si_sdr", "fsn_metric_stoi_workspace", "fsn_metric_stoi",
+    "fsn_metric_sdr_workspace", "fsn_metric_sdr",
 ]
 
 
@@ -219,6 +220,8 @@ def load_library():
     lib.fsn_metric_si_sdr.argtypes = [vp, vp, i32, i64, C.POINTER(i64), vp, i64, vp, vp]
     lib.fsn_metric_stoi_workspace.argtypes = [i32, i64, C.POINTER(i64), i32, C.POINTER(i64)]
     lib.fsn_metric_stoi.argtypes = [vp, vp, i32, i64, C.POINTER(i64), i32, vp, i64, vp, vp]
+    lib.fsn_metric_sdr_workspace.argtypes = [i32, i64, C.POINTER(i64), C.POINTER(i64)]
+    lib.fsn_metric_sdr.argtypes = [vp, vp, i32, i64, C.POINTER(i64), vp, i64, vp, vp]
     _LIB = lib
     return lib
 

@@ -1,10 +1,11 @@
-"""Objective scores of enhanced speech on the device, one per clip (C ABI: fsn_metric_si_sdr / fsn_metric_stoi, DESIGN.md §3.20).
+"""Objective scores of enhanced speech on the device, one per clip (C ABI: fsn_metric_si_sdr / fsn_metric_stoi, DESIGN.md §3.20;
+fsn_metric_sdr, §3.21).
 
     from fsnplus_b200 import metrics
     enhanced = model.enhance_audio(noisy, lengths)
     scores = metrics.stoi(clean, enhanced, sr=16000, lengths=lengths)     # float64 [B] on the same device
 
-Both take the reference and the estimate as CUDA float32 ``[B, L]`` tensors with optional per-clip ``lengths`` (clip b is the first
+Each takes the reference and the estimate as CUDA float32 ``[B, L]`` tensors with optional per-clip ``lengths`` (clip b is the first
 lengths[b] samples of its row, as ``model.enhance_audio`` takes them), or as two lists of 1-D CUDA tensors, packed here into that
 form.  A clip's score does not depend on the rest of the batch.  The workspace is allocated by torch on the tensors' device, and the
 call runs on its current stream.
@@ -80,3 +81,12 @@ def stoi(ref, est, sr=16000, lengths=None):
     sr = int(sr)
     return _run(ref, est, lengths, lambda lib, B, L, hl, nb: lib.fsn_metric_stoi_workspace(B, L, hl, sr, nb),
                 lambda lib, r, e, B, L, hl, w, nw, o, s: lib.fsn_metric_stoi(r, e, B, L, hl, sr, w, nw, o, s))
+
+
+def sdr(ref, est, lengths=None):
+    """BSS Eval v3 SDR in dB of each clip of ``est`` against ``ref``, as mir_eval's bss_eval_sources scores one source: the
+    projection P of ``est`` onto the 512 delayed copies of ``ref`` (a 512-tap distortion filter, one Toeplitz solve per clip) and
+    10 log10(|P|^2 / |e' - P|^2), all in float64.  No sample rate: SDR does not depend on it.  A silent reference or estimate gives
+    NaN; scores above 100 dB measure rounding noise.  Returns a float64 CUDA tensor [B]."""
+    return _run(ref, est, lengths, lambda lib, B, L, hl, nb: lib.fsn_metric_sdr_workspace(B, L, hl, nb),
+                lambda lib, r, e, B, L, hl, w, nw, o, s: lib.fsn_metric_sdr(r, e, B, L, hl, w, nw, o, s))

@@ -686,6 +686,17 @@ int fsn_metric_stoi_workspace(int32_t B, int64_t L, const int64_t* h_lengths, in
 int fsn_metric_stoi(const float* d_ref, const float* d_est, int32_t B, int64_t L, const int64_t* h_lengths, int32_t sr, void* d_work,
                     int64_t work_bytes, double* d_out, void* stream);
 
+/* SDR in dB as BSS Eval v3 computes it for one source with a 512-tap distortion filter (mir_eval's bss_eval_sources; DESIGN.md
+ * §3.21): with r, e zero-extended, R[k] = sum r[n] r[n + k], D[k] = sum r[n] e[n + k] (k < 512), G c = D for G[i][j] = R[|i - j|],
+ * P = c * r over n < L_b + 511 and SDR = 10 log10(sum P^2 / sum (e' - P)^2), e' = e followed by 511 zeros.  fp64 throughout (a
+ * Levinson solve per clip); no sample rate.  A silent reference or a silent estimate gives NaN, and so does a reference whose
+ * Levinson recursion meets a prediction error that is not a positive finite number (numerically singular); a zero denominator gives
+ * +inf.  Scores above 100 dB (est = ref, clips of a few samples) measure rounding noise.  Workspace: B (8192 ceil(max L_b / 3584)
+ * + 16 ceil((max L_b + 511) / 4096) + 12296) bytes, each of its five segments rounded up to 256 bytes. */
+int fsn_metric_sdr_workspace(int32_t B, int64_t L, const int64_t* h_lengths, int64_t* bytes);
+int fsn_metric_sdr(const float* d_ref, const float* d_est, int32_t B, int64_t L, const int64_t* h_lengths, void* d_work,
+                   int64_t work_bytes, double* d_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -2771,6 +2771,26 @@ static int audio_alloc(fsn_stream* st, cudaStream_t s) {
     return FSN_OK;
 }
 
+// The rules of slot b's flag f against its session that every audio call checks, in the order they are reported: the flag's range;
+// for a START, STEP or FLUSH the call's own count check count(name of the flag); then a STEP or FLUSH needs a session, a STEP one
+// whose input has not ended, and a FLUSH after the session's FLUSH a count n of 0.  arg, unit: the count's argument and unit.
+template <class CountCheck>
+static int audio_session_check(const fsn_stream* st, int b, int f, int n, const char* arg, const char* unit, CountCheck count) {
+    if (f < FSN_SLOT_HOLD || f > FSN_SLOT_FLUSH)
+        return fail(FSN_EINVAL, "slot %d: flag %d is not FSN_SLOT_HOLD (0), FSN_SLOT_STEP (1), FSN_SLOT_START (2) or FSN_SLOT_FLUSH (3)", b, f);
+    if (f == FSN_SLOT_HOLD) return FSN_OK;
+    const char* name = f == FSN_SLOT_START ? "START" : f == FSN_SLOT_STEP ? "STEP" : "FLUSH";
+    if (int rc = count(name)) return rc;
+    if (f == FSN_SLOT_START) return FSN_OK;
+    const int t = st->a_tick.empty() ? -1 : st->a_tick[b], Kh = st->a_hops.empty() ? 0 : st->a_hops[b];
+    if (t < 0) return fail(FSN_EINVAL, "slot %d: %s on a slot without a session (START one first)", b, name);
+    if (f == FSN_SLOT_STEP && Kh)
+        return fail(FSN_EINVAL, "slot %d: STEP after the session's FLUSH (its input has ended: START a new session)", b);
+    if (f == FSN_SLOT_FLUSH && Kh && n)
+        return fail(FSN_EINVAL, "slot %d: FLUSH with %s = %d after the session's FLUSH (its input has ended: pass 0 %s)", b, arg, n, unit);
+    return FSN_OK;
+}
+
 // One slot's ticks in an audio call of K hops (DESIGN.md §3.10, §3.14).  Flag f with n hops stands for K per-hop ticks: START,
 // STEP x (n - 1) / STEP x n / STEP x n then FLUSH, the rest HOLD.  The active ones -- every tick but the HOLDs and the FLUSH ticks past
 // the session's end -- come first: na of them, at slot ticks k0 .. k0 + na - 1 (a START's k0 is 0).  The first nstore store the row's
@@ -2783,20 +2803,15 @@ static int audio_slot_plan(const fsn_stream* st, int b, int f, int n, int K, Aud
     const int la = st->m->cfg.look_ahead;
     const int t = st->a_tick.empty() ? -1 : st->a_tick[b], Kh = st->a_hops.empty() ? 0 : st->a_hops[b];
     *p = AudioSlotPlan{t, 0, 0, 0, Kh, 0};
-    if (f < FSN_SLOT_HOLD || f > FSN_SLOT_FLUSH)
-        return fail(FSN_EINVAL, "slot %d: flag %d is not FSN_SLOT_HOLD (0), FSN_SLOT_STEP (1), FSN_SLOT_START (2) or FSN_SLOT_FLUSH (3)", b, f);
-    if (f == FSN_SLOT_HOLD) return FSN_OK;
     const int lo = f == FSN_SLOT_FLUSH ? 0 : 1;
-    const char* name = f == FSN_SLOT_START ? "START" : f == FSN_SLOT_STEP ? "STEP" : "FLUSH";
-    if (n < lo || n > K) return fail(FSN_EINVAL, "slot %d: h_hops = %d: a %s consumes %d to K = %d hops", b, n, name, lo, K);
+    if (int rc = audio_session_check(st, b, f, n, "h_hops", "hops", [&](const char* name) {
+            return n < lo || n > K ? fail(FSN_EINVAL, "slot %d: h_hops = %d: a %s consumes %d to K = %d hops", b, n, name, lo, K) : FSN_OK;
+        }))
+        return rc;
+    if (f == FSN_SLOT_HOLD) return FSN_OK;
     if (f == FSN_SLOT_START) {
         *p = AudioSlotPlan{0, n, 1, n, 0, 0};
     } else {
-        if (t < 0) return fail(FSN_EINVAL, "slot %d: %s on a slot without a session (START one first)", b, name);
-        if (f == FSN_SLOT_STEP && Kh)
-            return fail(FSN_EINVAL, "slot %d: STEP after the session's FLUSH (its input has ended: START a new session)", b);
-        if (f == FSN_SLOT_FLUSH && Kh && n)
-            return fail(FSN_EINVAL, "slot %d: FLUSH with h_hops = %d after the session's FLUSH (its input has ended: pass 0 hops)", b, n);
         if (f == FSN_SLOT_FLUSH && !Kh && t + n < 2 && !(t + n == 1 && r))
             return fail(FSN_EINVAL, "slot %d: FLUSH after %d hop: a session needs at least 2 hops (the STFT's reflect padding reads "
                                     "n_fft / 2 + 1 samples)", b, t + n);
@@ -2815,14 +2830,15 @@ static int audio_slot_plan(const fsn_stream* st, int b, int f, int n, int K, Aud
 }
 
 // The sample call's part of an audio call (fsn_stream_step_audio_samples, DESIGN.md §3.19): per slot the samples pending before the
-// call and the trailing partial hop after it (StreamAudioSamples), the rows' strides, and whether any slot ticks (else only the
-// analysis kernel runs: it stores the partial hops and zeroes the output rows)
+// call and the trailing partial hop after it (StreamAudioLaunch::r0, r), the rows' strides, and whether any slot ticks (else only
+// the analysis kernel runs: it stores the partial hops and zeroes the output rows)
 struct SampleRows { const int32_t *r0, *r; int S, So; bool tick; };
 
 // The audio calls after their argument checks: every slot advances by its plan (fsn_stream_step_audio_slots: K = 1, one hop per
 // START / STEP) through the K-hop kernels around one K-frame model step.  The per-hop call (chunk = false) steps the model on the
 // per-tick scratch with the generic sub band; the chunk call on its own scratch, with the layer-wise sub band where the offline
-// forward runs it.  smp: the sample call's rows and planes (null for the hop calls).  Errors change no state.
+// forward runs it.  smp: the sample call's rows and planes (null for the hop calls: rows of K hops, no partial hops).  Errors
+// change no state.
 static int run_audio(fsn_stream* st, const std::vector<AudioSlotPlan>& plan, const float* d_samples, int K, bool chunk, float* d_out,
                      float* d_mask, const SampleRows* smp, cudaStream_t s) {
     fsn_model* m = st->m;
@@ -2881,28 +2897,23 @@ static int run_audio(fsn_stream* st, const std::vector<AudioSlotPlan>& plan, con
         memcpy(h + smp_at + B, smp->r, (size_t)B * sizeof(int32_t));
     }
     if (int rc = st->stage.send(st->x_plan.p, nstage, s)) return rc;
-    StreamAudioChunkLaunch a{};
+    StreamAudioLaunch a{};
     a.k0 = d; a.na = d + B; a.start = d + 2 * B; a.nstore = d + 3 * B; a.hops = d + 4 * B;
     a.samples = d_samples; a.out = d_out;
+    a.S = a.So = K * (F - 1);
+    if (smp) { a.r0 = d + smp_at; a.r = d + smp_at + B; a.S = smp->S; a.So = smp->So; a.zero_out = !smp->tick; }
     a.hist = static_cast<float*>(st->a_hist.p); a.spec = static_cast<float2*>(st->a_spec.p); a.tail = static_cast<float*>(st->a_tail.p);
     a.sspec = static_cast<float2*>(st->x_spec.p); a.mag = static_cast<float*>(st->x_mag.p); a.mask = static_cast<float*>(st->x_mask.p);
     a.umask = d_mask;
     const AudioTables tab = audio_table_ptrs(static_cast<const float*>(st->a_tab.p), N);
-    a.window = tab.window; a.twiddle = tab.twiddle; a.inv_env = tab.inv_env;
+    a.window = tab.window; a.twiddle = tab.twiddle; a.inv_env = tab.inv_env; a.inv_last = tab.inv_last;
     a.B = B; a.K = K; a.Km = Km; a.n_fft = N; a.la = la;
     a.lam = lim ? reinterpret_cast<const float*>(d + lam_at) : nullptr;
-    StreamAudioSamplesLaunch sa{};
-    if (smp) {
-        sa.a = a;
-        sa.x = StreamAudioSamples{d + smp_at, d + smp_at + B, smp->S, smp->So, !smp->tick, tab.inv_last};
-        launch_stream_stft_samples(sa, s);
-        if (!smp->tick) {                                               // no tick: no model step and no synthesis
-            st->last = nullptr;
-            CK(cudaGetLastError());
-            return FSN_OK;
-        }
-    } else {
-        launch_stream_stft_chunk(a, s);
+    launch_stream_stft(a, s);
+    if (a.zero_out) {                                                   // no tick: no model step and no synthesis
+        st->last = nullptr;
+        CK(cudaGetLastError());
+        return FSN_OK;
     }
     // at Km = 1 the counts alone say which slots step a frame: no frame counts, so the per-frame step's kernels and arguments
     if (Km)
@@ -2911,8 +2922,7 @@ static int run_audio(fsn_stream* st, const std::vector<AudioSlotPlan>& plan, con
             return rc;
     if (Km) { st->last_audio = true; st->last_spec_K = K; }
     else st->last = nullptr;
-    if (smp) launch_stream_istft_samples(sa, s);
-    else launch_stream_istft_chunk(a, s);
+    launch_stream_istft(a, s);
     CK(cudaGetLastError());
     return FSN_OK;
 }
@@ -2987,18 +2997,13 @@ extern "C" int fsn_stream_step_audio_samples(fsn_stream* st, const float* d_samp
     bool flush = false, consume = false;
     for (int b = 0; b < B; ++b) {                                       // every slot is checked before any state changes
         const int f = h_flags[b], cnt = h_counts[b];
-        if (f < FSN_SLOT_HOLD || f > FSN_SLOT_FLUSH)
-            return fail(FSN_EINVAL, "slot %d: flag %d is not FSN_SLOT_HOLD (0), FSN_SLOT_STEP (1), FSN_SLOT_START (2) or FSN_SLOT_FLUSH (3)", b, f);
+        if (int rc = audio_session_check(st, b, f, cnt, "h_counts", "samples", [&](const char*) {
+                return cnt < 0 || cnt > S ? fail(FSN_EINVAL, "slot %d: h_counts = %d is outside [0, S = %d]", b, cnt, S) : FSN_OK;
+            }))
+            return rc;
         const int t = fresh ? -1 : st->a_tick[b], Kh = fresh ? 0 : st->a_hops[b], p0 = fresh ? 0 : st->a_pend[b];
         r0[b] = r[b] = p0;
         if (f == FSN_SLOT_HOLD) continue;
-        if (cnt < 0 || cnt > S) return fail(FSN_EINVAL, "slot %d: h_counts = %d is outside [0, S = %d]", b, cnt, S);
-        const char* name = f == FSN_SLOT_START ? "START" : f == FSN_SLOT_STEP ? "STEP" : "FLUSH";
-        if (f != FSN_SLOT_START && t < 0) return fail(FSN_EINVAL, "slot %d: %s on a slot without a session (START one first)", b, name);
-        if (f == FSN_SLOT_STEP && Kh)
-            return fail(FSN_EINVAL, "slot %d: STEP after the session's FLUSH (its input has ended: START a new session)", b);
-        if (f == FSN_SLOT_FLUSH && Kh && cnt)
-            return fail(FSN_EINVAL, "slot %d: FLUSH with h_counts = %d after the session's FLUSH (its input has ended: pass 0 samples)", b, cnt);
         consume = consume || cnt > 0;
         if (f == FSN_SLOT_START) r0[b] = 0;
         const long long tot = (long long)r0[b] + cnt;

@@ -168,15 +168,19 @@ struct StreamSbCarryLaunch {
 };
 void launch_stream_sb_carry(const StreamSbCarryLaunch& a, cudaStream_t s);
 
-// ---- k_stream_audio.cu: audio in and out of the streaming audio calls (fsn_stream_step_audio_slots, _chunk) ------------------
-// K hops per slot (DESIGN.md §3.10, §3.14; the per-hop call is K = 1): slot b's active ticks are the first na[b] of the call, at
-// slot ticks k0[b] + i; with start[b] its tick 0 is a START (store hop 0, no model frame).  Its first nstore[b] active ticks store
-// the row's hops 0 .. nstore - 1.  Every other active tick is a model frame: model column c = i - start, frame j = k0 + start - 1 + c,
-// its magnitude and mask at column c of the model's planes [B, F, Km] and [B, 2, F, Km].
-struct StreamAudioChunkLaunch {
+// ---- k_stream_audio.cu: audio in and out of the streaming audio calls (fsn_stream_step_audio_slots, _chunk, _samples) ---------
+// Up to K hops per slot (DESIGN.md §3.10, §3.14, §3.19; the per-hop call is K = 1): slot b's active ticks are the first na[b] of the
+// call, at slot ticks k0[b] + i; with start[b] its tick 0 is a START (store hop 0, no model frame).  Its first nstore[b] active ticks
+// store the row's hops 0 .. nstore - 1.  Every other active tick is a model frame: model column c = i - start, frame
+// j = k0 + start - 1 + c, its magnitude and mask at column c of the model's planes [B, F, Km] and [B, 2, F, Km].
+struct StreamAudioLaunch {
     const int *k0, *na, *start, *nstore, *hops;   // [B] each; hops: the session's K after this call (0 = not flushed)
-    const float* samples;     // [B, K hop] this call's hops at the front of each row
-    float* out;               // [B, K hop] output hops at the front of each row, zero after them
+    const int *r0, *r;        // [B] each, or null (no partial hops: both 0): samples pending before the call; the trailing partial
+                              // hop after it (the next pending count, or at a FLUSH the partial end: L = K hop + r)
+    const float* samples;     // [B, S] this call's samples of each row (the hop calls: S = K hop)
+    float* out;               // [B, So] output hops, then a FLUSH's last r samples, at the front of each row, zero after them
+    int S, So;                // row strides of samples and out (the hop calls: K hop; the sample call: So = S + (la + 3) hop)
+    int zero_out;             // the analysis zeroes the output rows (a call with no tick runs no synthesis)
     float* hist;              // [B, 3, hop] history ring: hop q at q % 3
     float2* spec;             // [B, la + 1, F] noisy spectrum ring: frame j at j % (la + 1)
     float* tail;              // [B, hop] second half of the last synthesised windowed frame
@@ -187,22 +191,12 @@ struct StreamAudioChunkLaunch {
     const float* window;      // [n_fft] periodic Hann
     const float2* twiddle;    // [n_fft / 2 + 1] exp(-2 pi i k / n_fft)
     const float* inv_env;     // [hop] 1 / (w^2(i) + w^2(i + hop))
+    const float* inv_last;    // [hop] 1 / w^2(i + hop)
     int B, K, Km, n_fft, la;  // Km: model columns, the largest frame count of the call; n_fft: power of two, 64 .. 1024
     const float* lam;         // optional [B] attenuation floor of each slot (limit_mask, DESIGN.md §3.18); null: the unlimited synthesis
 };
-void launch_stream_stft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s);
-void launch_stream_istft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s);
-// The sample call's additions (fsn_stream_step_audio_samples, DESIGN.md §3.19): the same kernels' SMP instantiations
-struct StreamAudioSamples {
-    const int *r0, *r;        // [B] each: samples pending before the call; the trailing partial hop after it (the next pending count,
-                              // or at a FLUSH the partial end: L = K hop + r)
-    int S, So;                // row strides of samples [B, S] and out [B, So], So = S + (la + 3) hop
-    int zero_out;             // the analysis zeroes the output rows (a call with no tick runs no synthesis)
-    const float* inv_last;    // [hop] 1 / w^2(i + hop)
-};
-struct StreamAudioSamplesLaunch { StreamAudioChunkLaunch a; StreamAudioSamples x; };
-void launch_stream_stft_samples(const StreamAudioSamplesLaunch& a, cudaStream_t s);
-void launch_stream_istft_samples(const StreamAudioSamplesLaunch& a, cudaStream_t s);
+void launch_stream_stft(const StreamAudioLaunch& a, cudaStream_t s);
+void launch_stream_istft(const StreamAudioLaunch& a, cudaStream_t s);
 
 // ---- k_audio.cu: audio in and out of the offline forward (fsn_model_enhance_audio), and the tables of both audio paths -------
 struct AudioLaunch {

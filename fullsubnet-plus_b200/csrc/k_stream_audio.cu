@@ -3,9 +3,9 @@
 // of torch.istft output (decompress_cIRM x noisy spectrum, inverse real FFT, window, overlap-add, division by the window envelope).
 // One CTA per slot; the real FFTs of n_fft points run as complex FFTs of n_fft / 2 points (radix 2, fp32, in shared memory,
 // fsn_fft.cuh) with the even / odd split folded in.  The tables (window, twiddles, 1 / envelope) are computed in double on the host
-// once per handle (audio_tables).  Both audio calls run these kernels: each slot's ticks of the call run in order inside its CTA, K
-// of them for the chunk call (fsn_stream_step_audio_chunk), one for the per-hop call (fsn_stream_step_audio_slots).  The sample call
-// (fsn_stream_step_audio_samples) runs its own pair, the same per-tick work with sample-granular stores and the exact end.
+// once per handle (audio_tables).  Every audio call runs this one pair: each slot's ticks of the call run in order inside its CTA, one
+// for the per-hop call (fsn_stream_step_audio_slots), up to K for the chunk call (fsn_stream_step_audio_chunk) and the sample call
+// (fsn_stream_step_audio_samples).  The sample call adds sample-granular rows, partial hops and the exact end; the hop calls pass none.
 #include "fsn_common.cuh"
 #include "fsn_fft.cuh"
 #include "fsn_kernels.h"
@@ -70,92 +70,12 @@ __device__ __forceinline__ void synth_frame(const float* mask, int ms, const flo
 }
 
 // The model planes' address of slot b's column c (row 0 of its rows rows): [B, rows, Km]
-__device__ __forceinline__ size_t chunk_col(const StreamAudioChunkLaunch& a, int b, int c, int rows) {
+__device__ __forceinline__ size_t chunk_col(const StreamAudioLaunch& a, int b, int c, int rows) {
     return ((size_t)b * rows) * a.Km + c;
 }
 
-// grid B: the analysis of a slot's active ticks, in order.  Stored hops go to the history ring (hop q at q % 3); the spectrum of model
-// column c goes to the scratch sspec (the ring still holds the frames the synthesis of this call reads), its magnitude to the model's
-// input.  Frames past the session's end (j > K) are zero.
-__global__ void __launch_bounds__(AUDIO_THREADS) stream_stft_chunk_kernel(StreamAudioChunkLaunch a) {
-    __shared__ float2 z[AUDIO_MAX_HOP];
-    const int b = blockIdx.x, na = a.na[b];
-    const int H = a.n_fft >> 1, F = H + 1, lg = 31 - __clz(H), k0 = a.k0[b], st = a.start[b], ns = a.nstore[b], K = a.hops[b];
-    float* hist = a.hist + (size_t)b * 3 * H;
-    const float* x = a.samples + (size_t)b * a.K * H;
-    for (int i = 0; i < na; ++i) {
-        const int k = k0 + i;
-        __syncthreads();                                         // the last tick's reads of hist and z are done
-        if (i < ns) {
-            for (int t = threadIdx.x; t < H; t += blockDim.x) hist[(k % 3) * H + t] = x[(size_t)i * H + t];
-            __syncthreads();
-        }
-        if (i < st) continue;                                    // a START stores hop 0 and analyses no frame
-        const int c = i - st, j = k - 1;
-        float2* spec = a.sspec + ((size_t)b * a.K + c) * F;
-        float* mag = a.mag + chunk_col(a, b, c, F);
-        const int ms = a.Km;
-        if (K && j > K) {
-            for (int f = threadIdx.x; f < F; f += blockDim.x) { spec[f] = make_float2(0.f, 0.f); mag[f * ms] = 0.f; }
-        } else {
-            analyse_frame(hist, j, K * H, H, lg, a.window, a.twiddle, z, spec, mag, ms);
-        }
-    }
-}
-
-// grid B: the synthesis of a slot's model columns, in order.  Column c synthesises frame m = j - la (if m >= 0) from its mask and the
-// spectrum of frame m: from the scratch if this call analysed it, else from the ring.  Emitted hops fill the front of the output row
-// and the rest is zero.  Then the caller's masks by tick (zero on the START tick and past the active ticks) and the ring's last la + 1
-// frames, written only after every read of the ring.  LIM: with the slots' attenuation floors a.lam (the instantiation without them is
-// the synthesis as it was before limits existed).
-template <bool LIM>
-__global__ void __launch_bounds__(AUDIO_THREADS) stream_istft_chunk_kernel(StreamAudioChunkLaunch a) {
-    __shared__ float2 z[AUDIO_MAX_HOP];
-    __shared__ float2 e[AUDIO_MAX_HOP + 1];
-    const int b = blockIdx.x, na = a.na[b], st = a.start[b], K = a.K, R = a.la + 1;
-    const int H = a.n_fft >> 1, F = H + 1, lg = 31 - __clz(H);
-    const int kf = na > st ? na - st : 0, j0 = a.k0[b] + st - 1;  // model columns, the frame of column 0
-    float* out = a.out + (size_t)b * K * H;
-    float* tail = a.tail + (size_t)b * H;
-    float2* ring = a.spec + (size_t)b * R * F;
-    const float2* sspec = a.sspec + (size_t)b * K * F;
-    const float lam = LIM ? __ldg(a.lam + b) : 0.f;
-    int nout = 0;
-    for (int c = 0; c < kf; ++c) {
-        const int m = j0 + c - a.la;
-        if (m < 0) continue;
-        __syncthreads();                                         // the last frame's reads of z and e are done
-        const float2* spec = m >= j0 ? sspec + (size_t)(m - j0) * F : ring + (m % R) * F;
-        synth_frame<LIM>(a.mask + chunk_col(a, b, c, 2 * F), a.Km, spec, tail, out + (size_t)nout * H, m >= 1, H, lg, a.window,
-                         a.twiddle, a.inv_env, z, e, lam);
-        nout += m >= 1;
-    }
-    for (size_t t = (size_t)nout * H + threadIdx.x; t < (size_t)K * H; t += blockDim.x) out[t] = 0.f;
-    if (a.umask) {
-        float* um = a.umask + (size_t)b * 2 * F * K;
-        for (size_t t = threadIdx.x; t < (size_t)2 * F * K; t += blockDim.x) {
-            const int r = (int)(t / K), i = (int)(t % K), c = i - st;
-            um[t] = (i >= st && i < na) ? a.mask[chunk_col(a, b, c, 2 * F) + (size_t)r * a.Km] : 0.f;
-        }
-    }
-    __syncthreads();                                             // every read of the ring is done
-    for (int t = threadIdx.x; t < R * F; t += blockDim.x) {
-        const int c = kf - R + t / F, f = t % F;
-        if (c >= 0) ring[((j0 + c) % R) * F + f] = sspec[(size_t)c * F + f];
-    }
-}
-
-void launch_stream_stft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s) { stream_stft_chunk_kernel<<<a.B, AUDIO_THREADS, 0, s>>>(a); }
-void launch_stream_istft_chunk(const StreamAudioChunkLaunch& a, cudaStream_t s) {
-    if (a.lam) stream_istft_chunk_kernel<true><<<a.B, AUDIO_THREADS, 0, s>>>(a);
-    else stream_istft_chunk_kernel<false><<<a.B, AUDIO_THREADS, 0, s>>>(a);
-}
-
-// ---- the sample call (fsn_stream_step_audio_samples, DESIGN.md §3.19) ---------------------------------------------------------
-// The chunk kernels above with the sample call's additions.  They are separate kernels so that the hop calls' code stays as it is.
-
-// Hop-chunk i of a slot's sample call into the history ring (hop k at k % 3): session samples P = i hop + t (t < n) counted from the
-// start of the slot's first pending hop; those at P >= r0 come from the call's row, x[P - r0] (the r0 below are already in the ring)
+// Hop-chunk i of a slot's call into the history ring (hop k at k % 3): session samples P = i hop + t (t < n) counted from the start
+// of the slot's first pending hop; those at P >= r0 come from the call's row, x[P - r0] (the r0 below are already in the ring)
 __device__ __forceinline__ void store_samples(float* hist, int k, const float* x, int i, int n, int r0, int H) {
     for (int t = threadIdx.x; t < n; t += blockDim.x) {
         const int P = i * H + t;
@@ -163,18 +83,20 @@ __device__ __forceinline__ void store_samples(float* hist, int k, const float* x
     }
 }
 
-// grid B: stream_stft_chunk_kernel on rows of S samples whose first hop completes the r0 pending ones.  The trailing r samples (the
-// next pending hop, or at a FLUSH the partial end) go to ring slot (k0 + nstore) % 3 at iteration nstore: after the analysis of frame
-// k0 + nstore - 2, the last reader of the hop that slot held, and before that of frame k0 + nstore, the first reader of the new one.
-// A session that has ended is reflected at L = K hop + r.  With zero_out the output rows are zeroed (no synthesis runs in the call).
-__global__ void __launch_bounds__(AUDIO_THREADS) stream_stft_samples_kernel(StreamAudioSamplesLaunch s) {
+// grid B: the analysis of a slot's active ticks, in order, from its row of S samples, whose first hop completes the r0 pending ones.
+// Stored hops go to the history ring (hop q at q % 3); the spectrum of model column c goes to the scratch sspec (the ring still holds
+// the frames the synthesis of this call reads), its magnitude to the model's input.  The trailing r samples (the next pending hop, or
+// at a FLUSH the partial end) go to ring slot (k0 + nstore) % 3 at iteration nstore: after the analysis of frame k0 + nstore - 2, the
+// last reader of the hop that slot held, and before that of frame k0 + nstore, the first reader of the new one.  A session that has
+// ended is reflected at L = K hop + r, and its frames past the end (j > K) are zero.  With zero_out the output rows are zeroed (no
+// synthesis runs in the call).
+__global__ void __launch_bounds__(AUDIO_THREADS) stream_stft_kernel(StreamAudioLaunch a) {
     __shared__ float2 z[AUDIO_MAX_HOP];
-    const StreamAudioChunkLaunch& a = s.a;
     const int b = blockIdx.x, na = a.na[b];
     const int H = a.n_fft >> 1, F = H + 1, lg = 31 - __clz(H), k0 = a.k0[b], st = a.start[b], ns = a.nstore[b], K = a.hops[b];
-    const int r0 = s.x.r0[b], r = s.x.r[b];
+    const int r0 = a.r0 ? a.r0[b] : 0, r = a.r ? a.r[b] : 0;
     float* hist = a.hist + (size_t)b * 3 * H;
-    const float* x = a.samples + (size_t)b * s.x.S;
+    const float* x = a.samples + (size_t)b * a.S;
     for (int i = 0; i < na; ++i) {
         const int k = k0 + i;
         __syncthreads();                                         // the last tick's reads of hist and z are done
@@ -197,24 +119,28 @@ __global__ void __launch_bounds__(AUDIO_THREADS) stream_stft_samples_kernel(Stre
         __syncthreads();
         store_samples(hist, k0 + ns, x, ns, r, r0, H);
     }
-    if (s.x.zero_out) {
-        float* out = a.out + (size_t)b * s.x.So;
-        for (int t = threadIdx.x; t < s.x.So; t += blockDim.x) out[t] = 0.f;
+    if (a.zero_out) {
+        float* out = a.out + (size_t)b * a.So;
+        for (int t = threadIdx.x; t < a.So; t += blockDim.x) out[t] = 0.f;
     }
 }
 
-// grid B: stream_istft_chunk_kernel on output rows of So samples, without the caller's masks.  A session that ends at L = K hop + r
-// with r > 0 emits, after frame K, its last r samples: frame K's tail times 1 / w^2(i + hop), as the offline synthesis does.
+// grid B: the synthesis of a slot's model columns, in order, into its output row of So samples.  Column c synthesises frame
+// m = j - la (if m >= 0) from its mask and the spectrum of frame m: from the scratch if this call analysed it, else from the ring.
+// Emitted hops fill the front of the output row.  A session that ends at L = K hop + r with r > 0 emits, after frame K, its last r
+// samples: frame K's tail times 1 / w^2(i + hop), as the offline synthesis does.  The rest of the row is zero.  Then the caller's
+// masks by tick (zero on the START tick and past the active ticks) and the ring's last la + 1 frames, written only after every read
+// of the ring.  LIM: with the slots' attenuation floors a.lam (the instantiation without them is the synthesis as it was before
+// limits existed).
 template <bool LIM>
-__global__ void __launch_bounds__(AUDIO_THREADS) stream_istft_samples_kernel(StreamAudioSamplesLaunch s) {
+__global__ void __launch_bounds__(AUDIO_THREADS) stream_istft_kernel(StreamAudioLaunch a) {
     __shared__ float2 z[AUDIO_MAX_HOP];
     __shared__ float2 e[AUDIO_MAX_HOP + 1];
-    const StreamAudioChunkLaunch& a = s.a;
     const int b = blockIdx.x, na = a.na[b], st = a.start[b], K = a.K, R = a.la + 1;
     const int H = a.n_fft >> 1, F = H + 1, lg = 31 - __clz(H);
     const int kf = na > st ? na - st : 0, j0 = a.k0[b] + st - 1;  // model columns, the frame of column 0
-    const int Kend = a.hops[b], rend = Kend ? s.x.r[b] : 0;
-    float* out = a.out + (size_t)b * s.x.So;
+    const int Kend = a.hops[b], rend = Kend && a.r ? a.r[b] : 0;
+    float* out = a.out + (size_t)b * a.So;
     float* tail = a.tail + (size_t)b * H;
     float2* ring = a.spec + (size_t)b * R * F;
     const float2* sspec = a.sspec + (size_t)b * K * F;
@@ -229,12 +155,19 @@ __global__ void __launch_bounds__(AUDIO_THREADS) stream_istft_samples_kernel(Str
                          a.twiddle, a.inv_env, z, e, lam);
         nout += m >= 1;
         if (m == Kend && rend) {                                 // each thread reads the tail entries it has just written
-            for (int i = threadIdx.x; i < rend; i += blockDim.x) out[(size_t)nout * H + i] = tail[i] * __ldg(s.x.inv_last + i);
+            for (int i = threadIdx.x; i < rend; i += blockDim.x) out[(size_t)nout * H + i] = tail[i] * __ldg(a.inv_last + i);
             nlast = rend;
         }
     }
     const int n = nout * H + nlast;
-    for (int t = n + threadIdx.x; t < s.x.So; t += blockDim.x) out[t] = 0.f;
+    for (int t = n + threadIdx.x; t < a.So; t += blockDim.x) out[t] = 0.f;
+    if (a.umask) {
+        float* um = a.umask + (size_t)b * 2 * F * K;
+        for (size_t t = threadIdx.x; t < (size_t)2 * F * K; t += blockDim.x) {
+            const int r = (int)(t / K), i = (int)(t % K), c = i - st;
+            um[t] = (i >= st && i < na) ? a.mask[chunk_col(a, b, c, 2 * F) + (size_t)r * a.Km] : 0.f;
+        }
+    }
     __syncthreads();                                             // every read of the ring is done
     for (int t = threadIdx.x; t < R * F; t += blockDim.x) {
         const int c = kf - R + t / F, f = t % F;
@@ -242,12 +175,10 @@ __global__ void __launch_bounds__(AUDIO_THREADS) stream_istft_samples_kernel(Str
     }
 }
 
-void launch_stream_stft_samples(const StreamAudioSamplesLaunch& a, cudaStream_t s) {
-    stream_stft_samples_kernel<<<a.a.B, AUDIO_THREADS, 0, s>>>(a);
-}
-void launch_stream_istft_samples(const StreamAudioSamplesLaunch& a, cudaStream_t s) {
-    if (a.a.lam) stream_istft_samples_kernel<true><<<a.a.B, AUDIO_THREADS, 0, s>>>(a);
-    else stream_istft_samples_kernel<false><<<a.a.B, AUDIO_THREADS, 0, s>>>(a);
+void launch_stream_stft(const StreamAudioLaunch& a, cudaStream_t s) { stream_stft_kernel<<<a.B, AUDIO_THREADS, 0, s>>>(a); }
+void launch_stream_istft(const StreamAudioLaunch& a, cudaStream_t s) {
+    if (a.lam) stream_istft_kernel<true><<<a.B, AUDIO_THREADS, 0, s>>>(a);
+    else stream_istft_kernel<false><<<a.B, AUDIO_THREADS, 0, s>>>(a);
 }
 
 }  // namespace fsn

@@ -67,10 +67,15 @@ struct PinnedStage {
         if (!g.ev) CK(cudaEventCreateWithFlags(&g.ev, cudaEventDisableTiming));
         if (g.used) CK(cudaEventSynchronize(g.ev));
         if (g.cap < n) {
-            if (g.h) CK(cudaFreeHost(g.h));
-            g.h = nullptr; g.cap = 0;
-            CK(cudaHostAlloc(reinterpret_cast<void**>(&g.h), n * sizeof(int32_t), cudaHostAllocDefault));
-            g.cap = n;
+            // every slot grows at once: cudaFreeHost synchronises the device, so a call that stages more values than any before it
+            // synchronises once, and the calls after it up to that size never do
+            for (Slot& o : slot) {
+                if (o.used) CK(cudaEventSynchronize(o.ev));
+                if (o.h) CK(cudaFreeHost(o.h));
+                o.h = nullptr; o.cap = 0;
+                CK(cudaHostAlloc(reinterpret_cast<void**>(&o.h), n * sizeof(int32_t), cudaHostAllocDefault));
+                o.cap = n;
+            }
         }
         *h = g.h;
         return FSN_OK;
@@ -88,6 +93,31 @@ struct PinnedStage {
             if (g.ev) cudaEventDestroy(g.ev);
         }
     }
+};
+
+// The calls of one handle run in call order whatever streams they are issued on: each waits for the event recorded behind the
+// previous one, then records its own.  The handle's state and scratch are shared by all its calls.
+struct CallOrder {
+    cudaEvent_t ev = nullptr;
+    bool used = false;
+    int wait(cudaStream_t s) {
+        if (used) CK(cudaStreamWaitEvent(s, ev, 0));
+        return FSN_OK;
+    }
+    int record(cudaStream_t s) {
+        if (!ev) CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        CK(cudaEventRecord(ev, s));
+        used = true;
+        return FSN_OK;
+    }
+    // call f() between the two; the event is recorded even when f fails part-way, behind whatever it enqueued
+    template <class Fn> int run(void* stream, Fn f) {
+        cudaStream_t s = static_cast<cudaStream_t>(stream);
+        if (int rc = wait(s)) return rc;
+        const int rc = f(), rr = record(s);
+        return rc ? rc : rr;
+    }
+    ~CallOrder() { if (ev) cudaEventDestroy(ev); }
 };
 
 // weights_id: folds n bytes into h 8 bytes at a time (the last word zero-padded).  Each step is a bijection of h (xor, odd multiply,
@@ -242,7 +272,7 @@ struct fsn_model {
     int64_t nfwd = 0;                                 // forwards whose LSTM events were recorded
     PinnedStage len_stage;                            // ragged forwards: the per-sample extents
     // audio call (fsn_model_enhance_audio): its workspace (the analysis planes, the enhanced spectrum) is in the table WS; the tables of
-    // its n_fft are built at its first call.  au_valid: the workspace holds the whole batch of the last forward, an audio call
+    // its n_fft are uploaded at finalize.  au_valid: the workspace holds the whole batch of the last forward, an audio call
     DevBuf au_planes, au_enh, au_tab;
     bool au_valid = false;
 };
@@ -777,6 +807,15 @@ extern "C" int fsn_model_finalize(fsn_model* m) {
         if (rc) return rc;
     }
     bind_weights(m, dev);
+    const int nfft = 2 * (c.num_freqs - 1);
+    if (nfft >= 64 && nfft <= 1024 && !(nfft & (nfft - 1))) {             // the audio call's tables, for the n_fft it takes (audio_fft_ok)
+        std::vector<float> tab;
+        audio_tables(nfft, tab);
+        if (upload(m->au_tab, tab.data(), tab.size() * sizeof(float))) return fail(FSN_ECUDA, "upload of the audio tables failed");
+    }
+    // The uploads above are legacy-stream copies from pageable memory, which may return before their DMA lands, and the packers may
+    // launch there: a forward on a non-blocking stream is not ordered after them, so the weights are in place when finalize returns
+    CK(cudaDeviceSynchronize());
     uint64_t id = 0xcbf29ce484222325ull;
     for (const auto& kv : m->param_hash) id = hash_words(id, &kv.second, sizeof(kv.second));   // std::map: key order
     id ^= id >> 33; id *= 0xff51afd7ed558ccdull; id ^= id >> 33;                              // final avalanche
@@ -1965,6 +2004,19 @@ static int wait_lanes(fsn_model* m, cudaStream_t s) {
     return FSN_OK;
 }
 
+// A plain call (forward, audio, test hooks) on stream s runs after the pipelined batches and after the last plain call, on whichever
+// stream that ran: they all use lane 0's workspace.  mark_plain records the call's end for the next one.
+static int wait_plain(fsn_model* m, cudaStream_t s) {
+    if (m->plain_pending) CK(cudaStreamWaitEvent(s, m->ev_plain, 0));
+    return wait_lanes(m, s);
+}
+static int mark_plain(fsn_model* m, cudaStream_t s) {
+    if (!m->ev_plain) CK(cudaEventCreateWithFlags(&m->ev_plain, cudaEventDisableTiming));
+    CK(cudaEventRecord(m->ev_plain, s));
+    m->plain_pending = true;
+    return FSN_OK;
+}
+
 // Clips b0 .. b0 + nb - 1 of batch b (fewer at its end): every pointer advanced by its per-clip stride
 static Batch slice(const fsn_config& c, const Batch& b, int b0, int nb) {
     const size_t plane = (size_t)c.num_freqs * b.T;
@@ -1983,15 +2035,9 @@ static Batch slice(const fsn_config& c, const Batch& b, int b0, int nb) {
 // in time windows (plan_forward) -- same bits, O(window) sub-band memory -- or, with the sub-band TCN, in bin chunks -- O(chunk)
 // sub-band memory.
 static int run_plain(fsn_model* m, const Batch& b, cudaStream_t s) {
-    int rc = wait_lanes(m, s);
+    int rc = wait_plain(m, s);
     if (rc) return rc;
     const bool audio = b.call == CALL_AUDIO;
-    if (audio && !m->au_tab.bytes) {                                    // the tables of this model's n_fft, once
-        std::vector<float> tab;
-        audio_tables(2 * (m->cfg.num_freqs - 1), tab);
-        if (m->au_tab.ensure(tab.size() * sizeof(float), false)) return fail(FSN_ECUDA, "allocation of the audio tables failed");
-        CK(cudaMemcpy(m->au_tab.p, tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice));
-    }
     m->plan = plan_forward(m->cfg, m->layerwise, b.B, b.T, m->ws_cap_bytes, m->env_sb_window, m->env_sb_chunk, audio, b.lam != nullptr);
     const int Bs = m->plan.Bs;
     int64_t launches = 0;
@@ -2000,12 +2046,10 @@ static int run_plain(fsn_model* m, const Batch& b, cudaStream_t s) {
         launches += m->launches;
     }
     m->launches = launches;
+    const int rr = mark_plain(m, s);                                    // also behind a sub-batch that failed part-way
     if (rc) return rc;
     m->au_valid = audio && Bs >= b.B;
-    if (!m->ev_plain) CK(cudaEventCreateWithFlags(&m->ev_plain, cudaEventDisableTiming));
-    CK(cudaEventRecord(m->ev_plain, s));
-    m->plain_pending = true;
-    return FSN_OK;
+    return rr;
 }
 
 // A device-buffer spectral call: check batch b, then run it plain or pipelined
@@ -2066,13 +2110,16 @@ extern "C" int fsn_model_sb_forward(fsn_model* m, const float* d_x, int32_t B, i
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const int* tl = nullptr;
     int rc = check_batch(m, b);
-    if (rc || (rc = wait_lanes(m, s)) || (rc = prepare(m, m->lane[0], b, Tw, 0, s, s, &tl))) return rc;
-    Lane& ln = m->lane[0];
-    SbPackLaunch sp = pack_args(m, ln, B, T, Tw, tl);
-    sp.raw = d_x;
-    if ((rc = pack_clip(m, ln, sp, Tw, 0, s)) || (rc = sub_band(m, ln, b, Tw, 0, sp, tl, s))) return rc;
-    CK(cudaGetLastError());
-    return FSN_OK;
+    if (rc || (rc = wait_plain(m, s))) return rc;
+    if (!(rc = prepare(m, m->lane[0], b, Tw, 0, s, s, &tl))) {
+        Lane& ln = m->lane[0];
+        SbPackLaunch sp = pack_args(m, ln, B, T, Tw, tl);
+        sp.raw = d_x;
+        if (!(rc = pack_clip(m, ln, sp, Tw, 0, s)) && !(rc = sub_band(m, ln, b, Tw, 0, sp, tl, s)))
+            if (cudaError_t e = cudaGetLastError()) rc = fail(FSN_ECUDA, "fsn_model_sb_forward: %s", cudaGetErrorString(e));
+    }
+    const int rr = mark_plain(m, s);                                    // also behind a call that failed part-way
+    return rc ? rc : rr;
 }
 
 extern "C" int fsn_model_submit(fsn_model* m, const float* d_mag, const float* d_real, const float* d_imag, int32_t B, int32_t T,
@@ -2184,14 +2231,11 @@ extern "C" int fsn_model_sync_host(fsn_model* m) {
     return FSN_OK;
 }
 
-extern "C" int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst, int64_t numel, void* stream) {
-    if (!m || !name || !d_dst) return fail(FSN_EINVAL, "null argument");
+static int get_stage(fsn_model* m, const char* name, float* d_dst, int64_t numel, cudaStream_t s) {
     Lane& ln = m->lane[m->last_lane];
-    if (!ln.geo.B) return fail(FSN_ESTATE, "no forward has run yet");
     const fsn_config& c = m->cfg;
     const int F = c.num_freqs, Tp = ln.geo.T + c.look_ahead, Pp = (Tp + 3) & ~3, B = ln.geo.B;
     const int nbr = (c.model_kind == FSN_KIND_PLUS) ? 3 : 1;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
     const std::string n(name);
     if (n == "fb_in" || n == "fb_out") {
         if (numel != (int64_t)nbr * B * F * Tp) return fail(FSN_EINVAL, "%s needs %lld elements", name, (long long)nbr * B * F * Tp);
@@ -2231,6 +2275,16 @@ extern "C" int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst,
     return fail(FSN_EINVAL, "unknown stage %s", name);
 }
 
+// Ordered like a plain call: after the forward it reads, whatever stream that ran on, and before the next call rewrites the workspace
+extern "C" int fsn_model_get_stage(fsn_model* m, const char* name, float* d_dst, int64_t numel, void* stream) {
+    if (!m || !name || !d_dst) return fail(FSN_EINVAL, "null argument");
+    if (!m->lane[m->last_lane].geo.B) return fail(FSN_ESTATE, "no forward has run yet");
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (int rc = wait_plain(m, s)) return rc;
+    const int rc = get_stage(m, name, d_dst, numel, s), rr = mark_plain(m, s);
+    return rc ? rc : rr;
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // streaming step API (causal fullsubnet.Model)
@@ -2261,6 +2315,7 @@ struct fsn_stream {
     std::vector<int32_t> nb, all_step, valid;
     DevBuf d_slot;
     PinnedStage stage;                                 // every tick's d_slot values, and the slot lists of save / load
+    CallOrder order;                                   // every call that takes a stream runs after the handle's previous one
     // A handle serves either the mask calls (fsn_stream_step, fsn_stream_step_slots) or the audio call, whichever it meets first:
     // FSN_STATE_MODE_MASK or FSN_STATE_MODE_AUDIO, 0 before
     int mode = 0;
@@ -2422,13 +2477,15 @@ extern "C" int fsn_stream_create(fsn_model* m, int32_t B, fsn_stream** out) {
     e |= state_alloc(st, 0, nullptr);
     if (st->use_ws) e |= st->ws_bar.ensure(64, true);
     e |= st->d_slot.ensure((size_t)4 * B * sizeof(int32_t), false);
-    if (e) { fsn_stream_destroy(st); return fail(FSN_ECUDA, "stream state allocation failed"); }
+    // the zero-fills above ran on the legacy stream, which a first step on a non-blocking stream is not ordered after
+    if (e || cudaDeviceSynchronize() != cudaSuccess) { fsn_stream_destroy(st); return fail(FSN_ECUDA, "stream state allocation failed"); }
     *out = st;
     return FSN_OK;
 }
 
 extern "C" void fsn_stream_destroy(fsn_stream* st) {
     if (!st) return;
+    cudaDeviceSynchronize();                                             // nothing in flight may still use the buffers
     for (const StateBuf& e : STATE) {
         (st->*e.buf).release();
         if (e.ws) (st->*e.ws).release();
@@ -2561,9 +2618,11 @@ extern "C" int fsn_stream_step(fsn_stream* st, const float* d_mag, float* d_mask
     const int n = st->n;
     const fsn_config& c = st->m->cfg;
     // sized at create: grows nothing, and enqueues only FSN_POISON's fill
-    if (st->tick.ensure(*st, 1, step_img_bytes(c, (long long)st->B * c.num_freqs, 1), false, static_cast<cudaStream_t>(stream)))
-        return fail(FSN_ECUDA, "step scratch allocation failed");
-    const int rc = step_frames(st, st->tick, d_mag, 1, nullptr, nullptr, nullptr, 0, d_mask, nullptr, static_cast<cudaStream_t>(stream));
+    const int rc = st->order.run(stream, [&] {
+        if (st->tick.ensure(*st, 1, step_img_bytes(c, (long long)st->B * c.num_freqs, 1), false, static_cast<cudaStream_t>(stream)))
+            return fail(FSN_ECUDA, "step scratch allocation failed");
+        return step_frames(st, st->tick, d_mag, 1, nullptr, nullptr, nullptr, 0, d_mask, nullptr, static_cast<cudaStream_t>(stream));
+    });
     if (rc) return rc;
     if (h_valid) *h_valid = (n >= st->m->cfg.look_ahead) ? 1 : 0;
     return FSN_OK;
@@ -2744,7 +2803,7 @@ extern "C" int fsn_stream_step_slots(fsn_stream* st, const float* d_mag, float* 
     if (!st || !d_mag || !d_mask) return fail(FSN_EINVAL, "null argument");
     if (!h_flags) return fail(FSN_EINVAL, "h_flags is null (one flag per slot, slots 0..%d)", st->B - 1);
     if (!h_valid) return fail(FSN_EINVAL, "h_valid is null (one result per slot, slots 0..%d)", st->B - 1);
-    return step_slots(st, d_mag, 1, d_mask, h_flags, h_valid, false, static_cast<cudaStream_t>(stream));
+    return st->order.run(stream, [&] { return step_slots(st, d_mag, 1, d_mask, h_flags, h_valid, false, static_cast<cudaStream_t>(stream)); });
 }
 
 extern "C" int fsn_stream_step_chunk(fsn_stream* st, const float* d_mag, int32_t K, float* d_mask, const int32_t* h_flags,
@@ -2754,7 +2813,7 @@ extern "C" int fsn_stream_step_chunk(fsn_stream* st, const float* d_mag, int32_t
     if (!d_mask) return fail(FSN_EINVAL, "d_mask is null (K mask columns per slot, [B, 2, F, K] float32 on the device)");
     if (!h_flags) return fail(FSN_EINVAL, "h_flags is null (one flag per slot, slots 0..%d)", st->B - 1);
     if (!h_valid) return fail(FSN_EINVAL, "h_valid is null (one result per slot, slots 0..%d)", st->B - 1);
-    return step_slots(st, d_mag, K, d_mask, h_flags, h_valid, true, static_cast<cudaStream_t>(stream));
+    return st->order.run(stream, [&] { return step_slots(st, d_mag, K, d_mask, h_flags, h_valid, true, static_cast<cudaStream_t>(stream)); });
 }
 
 // Audio state of the handle, zero-filled on the call's stream, and the tables of its n_fft (computed in double).
@@ -2959,7 +3018,9 @@ extern "C" int fsn_stream_step_audio_slots(fsn_stream* st, const float* d_sample
     if (!d_out) return fail(FSN_EINVAL, "d_out is null (one hop of output per slot, [B, hop] float32 on the device)");
     if (!h_flags) return fail(FSN_EINVAL, "h_flags is null (one flag per slot, slots 0..%d)", st->B - 1);
     if (!h_valid) return fail(FSN_EINVAL, "h_valid is null (one result per slot, slots 0..%d)", st->B - 1);
-    return step_audio(st, d_samples, 1, h_flags, nullptr, d_out, h_valid, d_mask, static_cast<cudaStream_t>(stream));
+    return st->order.run(stream, [&] {
+        return step_audio(st, d_samples, 1, h_flags, nullptr, d_out, h_valid, d_mask, static_cast<cudaStream_t>(stream));
+    });
 }
 
 extern "C" int fsn_stream_step_audio_chunk(fsn_stream* st, const float* d_samples, int32_t K, const int32_t* h_flags,
@@ -2970,7 +3031,9 @@ extern "C" int fsn_stream_step_audio_chunk(fsn_stream* st, const float* d_sample
     if (!h_flags) return fail(FSN_EINVAL, "h_flags is null (one flag per slot, slots 0..%d)", st->B - 1);
     if (!h_hops) return fail(FSN_EINVAL, "h_hops is null (one hop count per slot, slots 0..%d)", st->B - 1);
     if (!h_nout) return fail(FSN_EINVAL, "h_nout is null (one result per slot, slots 0..%d)", st->B - 1);
-    return step_audio(st, d_samples, K, h_flags, h_hops, d_out, h_nout, d_mask, static_cast<cudaStream_t>(stream));
+    return st->order.run(stream, [&] {
+        return step_audio(st, d_samples, K, h_flags, h_hops, d_out, h_nout, d_mask, static_cast<cudaStream_t>(stream));
+    });
 }
 
 // Any number of samples per slot and call (DESIGN.md §3.19).  Each slot's completed hops become the ticks of a hop call: START with n
@@ -3041,15 +3104,18 @@ extern "C" int fsn_stream_step_audio_samples(fsn_stream* st, const float* d_samp
     }
     if (st->mode == FSN_STATE_MODE_MASK) return claim_mode(st, FSN_STATE_MODE_AUDIO);
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (K == 0 && !consume) {                                           // nothing to store or synthesise: the rows are zero
-        if (int rc = claim_mode(st, FSN_STATE_MODE_AUDIO)) return rc;
-        if (st->a_tick.empty())
-            if (int rc = audio_alloc(st, s)) return rc;
-        CK(cudaMemsetAsync(d_out, 0, (size_t)B * So * sizeof(float), s));
-    } else {
+    const int rc = st->order.run(stream, [&] {
+        if (K == 0 && !consume) {                                       // nothing to store or synthesise: the rows are zero
+            if (int rc = claim_mode(st, FSN_STATE_MODE_AUDIO)) return rc;
+            if (st->a_tick.empty())
+                if (int rc = audio_alloc(st, s)) return rc;
+            CK(cudaMemsetAsync(d_out, 0, (size_t)B * So * sizeof(float), s));
+            return FSN_OK;
+        }
         const SampleRows rows{r0.data(), r.data(), S, (int)So, K > 0};
-        if (int rc = run_audio(st, plan, d_samples, Kc, chunk, d_out, nullptr, &rows, s)) return rc;
-    }
+        return run_audio(st, plan, d_samples, Kc, chunk, d_out, nullptr, &rows, s);
+    });
+    if (rc) return rc;
     for (int b = 0; b < B; ++b) {
         const int f = h_flags[b];
         const AudioSlotPlan& p = plan[b];
@@ -3065,8 +3131,7 @@ extern "C" int fsn_stream_step_audio_samples(fsn_stream* st, const float* d_samp
 
 extern "C" int fsn_stream_fb_ws(const fsn_stream* st) { return st && st->use_ws ? 1 : 0; }
 
-extern "C" int fsn_stream_get_stage(fsn_stream* st, const char* name, float* d_dst, int64_t numel, void* stream) {
-    if (!st || !name || !d_dst) return fail(FSN_EINVAL, "null argument");
+static int stream_get_stage(fsn_stream* st, const char* name, float* d_dst, int64_t numel, void* stream) {
     const std::string n(name);
     if (n != "fb_in" && n != "fb_out" && n != "sb_img" && n != "mag" && n != "mask" && n != "spec")
         return fail(FSN_EINVAL, "unknown stage %s", name);
@@ -3101,6 +3166,11 @@ extern "C" int fsn_stream_get_stage(fsn_stream* st, const char* name, float* d_d
     return FSN_OK;
 }
 
+extern "C" int fsn_stream_get_stage(fsn_stream* st, const char* name, float* d_dst, int64_t numel, void* stream) {
+    if (!st || !name || !d_dst) return fail(FSN_EINVAL, "null argument");
+    return st->order.run(stream, [&] { return stream_get_stage(st, name, d_dst, numel, stream); });
+}
+
 // ---------------------------------------------------------------------------------------------
 // overlapped-chunk sessions (DESIGN.md §3.16): the reference's overlapped_chunk inferencer (inferencer.py:191-250) per slot, every
 // chunk completed in a call enhanced in one offline audio forward
@@ -3117,6 +3187,7 @@ struct fsn_chunk_stream {
     std::vector<int64_t> n, k;
     DevBuf ring, tail, window, plan, rows, enh, x_slot;
     PinnedStage stage;
+    CallOrder order;                                   // step, save and load run in call order whatever their streams
     std::vector<float> lam_db;                         // attenuation limits in dB (fsn_chunk_stream_set_atten_lim): [B], empty until first set
 };
 
@@ -3185,7 +3256,9 @@ extern "C" int fsn_chunk_stream_create(fsn_model* m, int32_t B, int32_t chunk_sa
     e |= cs->tail.ensure((size_t)B * chunk_tail_stride(C) * sizeof(float), true);
     e |= cs->window.ensure((size_t)C * sizeof(float), false);
     e |= cs->plan.ensure((size_t)B * CHUNK_PLAN_FIELDS * sizeof(int32_t), false);
-    if (e || cudaMemcpy(cs->window.p, w.data(), (size_t)C * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) {
+    // the zero-fills and the pageable copy ran on the legacy stream, which a non-blocking stream's first step is not ordered after
+    if (e || cudaMemcpy(cs->window.p, w.data(), (size_t)C * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess ||
+        cudaDeviceSynchronize() != cudaSuccess) {
         fsn_chunk_stream_destroy(cs);
         return fail(FSN_ECUDA, "chunk stream state allocation failed (B = %d, chunk_samples = %d)", B, C);
     }
@@ -3195,6 +3268,7 @@ extern "C" int fsn_chunk_stream_create(fsn_model* m, int32_t B, int32_t chunk_sa
 
 extern "C" void fsn_chunk_stream_destroy(fsn_chunk_stream* cs) {
     if (!cs) return;
+    cudaDeviceSynchronize();                                             // nothing in flight may still use the buffers
     for (DevBuf* b : {&cs->ring, &cs->tail, &cs->window, &cs->plan, &cs->rows, &cs->enh, &cs->x_slot}) b->release();
     delete cs;
 }
@@ -3237,27 +3311,31 @@ extern "C" int fsn_chunk_stream_step(fsn_chunk_stream* cs, const float* d_sample
     if (nrows)
         if (int rc = check_batch(cs->m, fwd, &lens, &row_lam)) return rc;
     const size_t rb = (size_t)nrows * W * sizeof(float);
-    int e = nrows ? cs->rows.ensure(rb, false, s, cs->m->env_poison) | cs->enh.ensure(rb, false, s, cs->m->env_poison) : 0;
-    if (e) return fail(FSN_ECUDA, "chunk row allocation failed (%d rows of %d samples)", nrows, W);
-    int32_t* h = nullptr;
-    if (int rc = cs->stage.take(plan.size(), &h)) return rc;
-    memcpy(h, plan.data(), plan.size() * sizeof(int32_t));
-    if (int rc = cs->stage.send(cs->plan.p, plan.size(), s)) return rc;
-    ChunkStreamLaunch a{};
-    a.plan = static_cast<const int*>(cs->plan.p);
-    a.samples = d_samples; a.out = d_out;
-    a.ring = static_cast<float*>(cs->ring.p); a.tail = static_cast<float*>(cs->tail.p);
-    a.rows = static_cast<float*>(cs->rows.p); a.enh = static_cast<const float*>(cs->enh.p);
-    a.window = static_cast<const float*>(cs->window.p);
-    a.B = B; a.S = S; a.C = C; a.P = CHUNK_PRE;
-    launch_chunk_gather(a, s);
-    CK(cudaGetLastError());
-    if (nrows) {
-        fwd.wave = a.rows; fwd.wave_out = static_cast<float*>(cs->enh.p);
-        if (int rc = run_plain(cs->m, fwd, s)) return rc;
-    }
-    launch_chunk_crossfade(a, s);
-    CK(cudaGetLastError());
+    const int rc = cs->order.run(stream, [&] {
+        int e = nrows ? cs->rows.ensure(rb, false, s, cs->m->env_poison) | cs->enh.ensure(rb, false, s, cs->m->env_poison) : 0;
+        if (e) return fail(FSN_ECUDA, "chunk row allocation failed (%d rows of %d samples)", nrows, W);
+        int32_t* h = nullptr;
+        if (int rc = cs->stage.take(plan.size(), &h)) return rc;
+        memcpy(h, plan.data(), plan.size() * sizeof(int32_t));
+        if (int rc = cs->stage.send(cs->plan.p, plan.size(), s)) return rc;
+        ChunkStreamLaunch a{};
+        a.plan = static_cast<const int*>(cs->plan.p);
+        a.samples = d_samples; a.out = d_out;
+        a.ring = static_cast<float*>(cs->ring.p); a.tail = static_cast<float*>(cs->tail.p);
+        a.rows = static_cast<float*>(cs->rows.p); a.enh = static_cast<const float*>(cs->enh.p);
+        a.window = static_cast<const float*>(cs->window.p);
+        a.B = B; a.S = S; a.C = C; a.P = CHUNK_PRE;
+        launch_chunk_gather(a, s);
+        CK(cudaGetLastError());
+        if (nrows) {
+            fwd.wave = a.rows; fwd.wave_out = static_cast<float*>(cs->enh.p);
+            if (int rc = run_plain(cs->m, fwd, s)) return rc;
+        }
+        launch_chunk_crossfade(a, s);
+        CK(cudaGetLastError());
+        return FSN_OK;
+    });
+    if (rc) return rc;
     for (int b = 0; b < B; ++b) {
         cs->n[b] = n1[b]; cs->k[b] = k1[b];
         h_nout[b] = plan[(size_t)b * CHUNK_PLAN_FIELDS + CP_NOUT];
@@ -3420,7 +3498,8 @@ extern "C" int fsn_stream_save_slots(fsn_stream* st, int32_t n, const int32_t* h
     if (int rc = state_buffer_ok(st->cum_in.p, d_state)) return rc;
     int64_t stride = 0;
     if (int rc = state_layout(st->m->cfg, mode, nullptr, nullptr, &stride)) return rc;
-    if (int rc = state_copy(st, n, h_slots, d_state, mode, STREAM_STATE_SAVE, static_cast<cudaStream_t>(stream))) return rc;
+    if (int rc = st->order.run(stream, [&] { return state_copy(st, n, h_slots, d_state, mode, STREAM_STATE_SAVE, static_cast<cudaStream_t>(stream)); }))
+        return rc;
     for (int i = 0; i < n; ++i) {
         const int b = h_slots[i];
         fsn_slot_meta& q = h_meta[i];
@@ -3478,9 +3557,12 @@ extern "C" int fsn_stream_load_slots(fsn_stream* st, int32_t n, const int32_t* h
     const int mode = h_meta[0].mode;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     if (int rc = claim_mode(st, mode)) return rc;
-    if (mode == FSN_STATE_MODE_AUDIO && st->a_tick.empty())
-        if (int rc = audio_alloc(st, s)) return rc;
-    if (int rc = state_copy(st, n, h_slots, const_cast<void*>(d_state), mode, STREAM_STATE_LOAD, s)) return rc;
+    if (int rc = st->order.run(stream, [&] {
+            if (mode == FSN_STATE_MODE_AUDIO && st->a_tick.empty())
+                if (int rc = audio_alloc(st, s)) return rc;
+            return state_copy(st, n, h_slots, const_cast<void*>(d_state), mode, STREAM_STATE_LOAD, s);
+        }))
+        return rc;
     for (int i = 0; i < n; ++i) {
         const int b = h_slots[i];
         if (mode == FSN_STATE_MODE_MASK) st->nb[b] = h_meta[i].frames;
@@ -3542,7 +3624,8 @@ extern "C" int fsn_chunk_stream_save_slots(fsn_chunk_stream* cs, int32_t n, cons
     if (int rc = state_buffer_ok(cs->ring.p, d_state)) return rc;
     ChunkLayout l{};
     if (int rc = chunk_layout(cs->C, &l)) return rc;
-    if (int rc = chunk_state_copy(cs, n, h_slots, d_state, STREAM_STATE_SAVE, static_cast<cudaStream_t>(stream))) return rc;
+    if (int rc = cs->order.run(stream, [&] { return chunk_state_copy(cs, n, h_slots, d_state, STREAM_STATE_SAVE, static_cast<cudaStream_t>(stream)); }))
+        return rc;
     const fsn_model* m = cs->m;
     for (int i = 0; i < n; ++i) {
         const int b = h_slots[i];
@@ -3585,7 +3668,10 @@ extern "C" int fsn_chunk_stream_load_slots(fsn_chunk_stream* cs, int32_t n, cons
                         i, (long long)q.chunks, (long long)q.samples, (long long)k, (long long)H);
     }
     if (int rc = state_buffer_ok(cs->ring.p, d_state)) return rc;
-    if (int rc = chunk_state_copy(cs, n, h_slots, const_cast<void*>(d_state), STREAM_STATE_LOAD, static_cast<cudaStream_t>(stream))) return rc;
+    if (int rc = cs->order.run(stream, [&] {
+            return chunk_state_copy(cs, n, h_slots, const_cast<void*>(d_state), STREAM_STATE_LOAD, static_cast<cudaStream_t>(stream));
+        }))
+        return rc;
     for (int i = 0; i < n; ++i) {
         const int b = h_slots[i];
         cs->n[b] = h_meta[i].samples; cs->k[b] = h_meta[i].chunks;

@@ -14,6 +14,23 @@
  * pointer; `stream` is a cudaStream_t passed as void* (NULL = legacy default stream); all entry points
  * return 0 on success or a negative FSN_E* code, with a message available from fsn_last_error().
  * There is no CPU fallback: without a CUDA device every compute entry point fails with FSN_ECUDA.
+ *
+ * Stream order.  A call that takes `stream` reads its device inputs and writes its device outputs in `stream` order, and returns
+ * without synchronising it, unless its comment says otherwise (fsn_model_forward_host, which returns with the result).  The calls of
+ * one handle (a model, a streaming handle, a chunk handle) run in the order they are made whatever streams they are issued on: each
+ * call waits on the device for the handle's previous call, so one handle may be driven from several streams (from one host thread at
+ * a time).  The calls without a stream -- fsn_model_finalize, fsn_model_load, fsn_stream_create, fsn_chunk_stream_create and the
+ * destroys -- synchronise the device before they return, so a handle is ready for a first call on any stream and freed only once
+ * nothing in flight uses it.
+ * Queue depth: host arrays (h_frames, h_lengths, h_atten_db, h_flags, h_hops, h_counts, slot lists) go to the device through a ring of
+ * 4 pinned staging slots per handle, and are free when the call returns.  Every streaming slot call (all but fsn_stream_step before
+ * the handle's first slot call), chunk step, save and load takes one slot of its handle; an offline call with host arrays takes one of
+ * the model's per sub-batch (a chunk step whose chunks complete also takes the model's, one per sub-batch).  So 4 such calls may be
+ * queued ahead of the GPU; the 5th waits on the host until the GPU has read the slot it reuses, i.e. reached the first of them.
+ * A call that stages more values than any call before it on the handle grows the 4 slots, a call that grows a workspace frees the
+ * old one, and a forward at another batch geometry (clips, frames, window, bin chunk) than the model's previous one frees part of
+ * it: each synchronises the device.  So a first call, a call at a larger shape, and a chunk step whose completed-row count differs
+ * from the model's previous forward may wait.
  */
 #ifndef FSNPLUS_B200_H_
 #define FSNPLUS_B200_H_
@@ -221,7 +238,8 @@ int fsn_model_forward_host(fsn_model* m, const float* h_mag, const float* h_real
  *
  * fsn_model_submit: device buffers.  The inputs must be complete in `stream` order at the time of the call and stay untouched,
  * d_out unread, until fsn_model_wait(m, stream) has been called (it makes `stream` wait for every submitted batch; it does not
- * block the host) or fsn_model_sync_host(m) has returned.  A plain fsn_model_forward on any stream first waits for the pipeline.
+ * block the host) or fsn_model_sync_host(m) has returned.  A plain fsn_model_forward on any stream first waits for the pipeline, and
+ * a submit waits for the last plain call (the model's calls run in call order on the device; "Stream order" above).
  *
  * fsn_model_forward_host_async: pinned host buffers; additionally the H2D copy of batch i+1 and the D2H copy of batch i-1
  * overlap on two copy streams.  `stream` is ignored (host memory carries no stream order).  The host buffers must stay
